@@ -1,11 +1,11 @@
-# Builds the product in-tree (the .so / binary travel to the GPU box with the snapshot):
-#   roc_b200/lib/libroc_b200.so  — sm_100a kernels + C ABI (include/roc_b200.h) + C++ host (include/roc_gnn.h, roc_host.h)
+# Builds the product in-tree:
+#   roc_b200/lib/libroc_b200.so  — sm_90a kernels + C ABI (include/roc_b200.h) + C++ host (include/roc_gnn.h, roc_host.h)
 #   roc_b200/bin/roc_gnn         — stand-alone driver with the reference's CLI
 # and the test infrastructure (oracle/Makefile): oracle/libroc_oracle.so, oracle/_ref/libroc_ref.so
 CUDA   ?= /usr/local/cuda
 NVCC   ?= $(CUDA)/bin/nvcc
 CXX    := g++
-ARCH   := -gencode arch=compute_100a,code=sm_100a
+ARCH   := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS := $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Iinclude -Iroc_b200/csrc
 CXXFLAGS := -O2 -std=c++17 -fPIC -Iinclude -Iroc_b200/csrc -Iroc_b200/csrc/host -I$(CUDA)/include -Wall -Wno-unused-function
 
@@ -41,10 +41,6 @@ oracle:
 # compute-sanitizer (memcheck + racecheck) over the tiny configuration; needs a GPU
 sanitize: $(LIB)
 	tools/sanitize.sh
-
-# the gather-ceiling measurement tool (what can a B200 deliver for random row gathers?)
-tools/gather_ceiling: tools/gather_ceiling.cu
-	$(NVCC) $(ARCH) -O3 -o $@ $<
 
 clean:
 	rm -rf $(BUILD) $(LIB) $(BIN)

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — GCN training edges/sec on synthetic graphs (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config 1..5]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config 1..5] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Workloads (BASELINE.json `configs`, --config; the default, 2, is the one the metric is quoted on):
@@ -23,6 +23,8 @@ DRAM traffic ncu measured for that (config, N) when profiles/sg_traffic.json has
 `--impl reference` time the CPU oracle (OpenMP, all host cores, thread count set explicitly) on a bounded sample
 of the same workload — ROC ships no CPU kernels (SURVEY §8c/d).  For N > 1 a `parity_check` (outside the timed
 region) trains a bounded graph on the N-rank engine and on a 1-rank engine and compares logits / loss / dW.
+`--dump-outputs DIR` writes what the last timed step computed (see dump_outputs) as DIR/<name>.npy, so two builds
+can be compared output for output: the inputs depend only on the arguments.
 """
 import argparse
 import importlib.util
@@ -79,11 +81,11 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -303,6 +305,31 @@ def parity_check(rank, local_rank, world, dist, dev):
             "max_rel_err": max(errs.values()), "errs": errs, "tolerance": 1e-4, "ok": bool(ok)}
 
 
+DUMP_ROWS = 1 << 17          # logits rows kept by --dump-outputs (a fixed, seeded sample)
+
+
+def dump_outputs(outdir, m, hnd, rank, world):
+    """The arrays a caller of the timed step receives, after the last timed step: the logits of its forward pass
+    (a fixed, seeded sample of DUMP_ROWS rows; `logits_rows` lists them), every parameter after its Adam update
+    and the gradient the step computed for it, and the loss metrics.  float32 / float64, well under 64 MB."""
+    os.makedirs(outdir, exist_ok=True)
+    sfx = "" if world == 1 else "_rank%d" % rank
+    logits = m.get_tensor(hnd["logits"])
+    rows = np.arange(logits.shape[0])
+    if logits.shape[0] > DUMP_ROWS:
+        rows = np.sort(np.random.RandomState(0).choice(logits.shape[0], DUMP_ROWS, replace=False))
+    out = {"logits": logits[rows], "logits_rows": rows.astype(np.float64)}
+    for p in range(m.num_parameters()):
+        out["W%d" % p] = m.get_parameter(p)
+        out["dW%d" % p] = m.get_parameter(p, "grad")
+    perf = m.metrics()
+    out["metrics"] = np.array([perf[k] for k in ("trainLoss", "trainAll", "testAll", "valAll", "trainCorrect",
+                                                 "testCorrect", "valCorrect")], dtype=np.float64)
+    for name, a in out.items():
+        np.save(os.path.join(outdir, name + sfx + ".npy"), a)
+    log("[bench] wrote %d arrays (%.1f MB) to %s" % (len(out), sum(a.nbytes for a in out.values()) / 1e6, outdir))
+
+
 def run_ours(args, rank, local_rank, world):
     import torch
     import torch.distributed as dist
@@ -364,7 +391,7 @@ def run_ours(args, rank, local_rank, world):
     d2h = 28   # sizeof(PerfMetrics)
 
     stream = torch.cuda.ExternalStream(host.stream, device=dev)
-    # configs whose working set fits in the 126 MB L2 (config 1) get an L2 flush between timed steps
+    # configs whose working set fits in the 50 MB L2 (config 1) get an L2 flush between timed steps
     small = (nloc * (layers[0] + 2 * max(layers[1:])) * 4 + e * 4) < (256 << 20)
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev) if small else None
 
@@ -414,6 +441,8 @@ def run_ours(args, rank, local_rank, world):
     sg_times = m.profile_sg_read()
     m.profile_sg(False)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, m, hnd, rank, world)
     perf = m.metrics()
     value = e * args.steps / (ms_total * 1e-3)
 
@@ -539,7 +568,7 @@ def reference_kernel_column(row_end_h, col_h, dev, h=64, iters=5):
     e1.record()
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / iters
-    return {"kernel": "aggre_coop_kernel (reference, sm_100a build)", "H": h, "launch_ms": ms,
+    return {"kernel": "aggre_coop_kernel (reference, sm_90a build)", "H": h, "launch_ms": ms,
             "algorithmic_GBps": sg_bytes(n, e, h) / (ms * 1e-3) / 1e9, "edges_per_s": e / (ms * 1e-3)}
 
 
@@ -554,6 +583,8 @@ def main():
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--no-e2e", action="store_true", help="skip the host-buffer leg (profiling runs)")
     ap.add_argument("--no-parity", action="store_true", help="skip the N-rank vs 1-rank parity check (N > 1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's outputs to DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))

@@ -1,5 +1,5 @@
 /*
- * roc_b200.h — C ABI of the B200-native kernel layer for ROC's GCN-training path.
+ * roc_b200.h — C ABI of the H100-native kernel layer for ROC's GCN-training path.
  *
  * This is the drop-in boundary (SURVEY.md §8b).  The reference has no FFI: its
  * device code is reached through Legion task variants
@@ -79,7 +79,7 @@ int roc_device_count(void);
 uint64_t roc_launch_count(void);
 /* Persistent / grid-stride kernels launched by the CALLING THREAD from now on size their grids for
  * (SMs - numSMs), leaving SMs to work running beside them on another stream (the peer-write halo exchange:
- * a tcgen05 GEMM CTA holds a whole SM, nothing co-resides with it).  0 restores full-chip grids.  Returns the
+ * a tensor-core GEMM CTA holds a whole SM, nothing co-resides with it).  0 restores full-chip grids.  Returns the
  * previous reserve. */
 int roc_set_sm_reserve(int numSMs);
 
@@ -132,7 +132,7 @@ int roc_sg_plan_info(const roc_sg_plan* plan, uint64_t* numChunks,
  * `in` is indexed by whatever ids colSrc holds (global ids over the whole
  * [N][ldIn] matrix as in scattergather.cc:69-73, or local+halo ids).
  * Deterministic: the per-row summation order is fixed by the plan — and is the same in every kernel variant the
- * library may pick for a width (registers / cp.async / TMA gather4 rings; ROC_SG_VARIANT forces one), so results
+ * library may pick for a width (registers / cp.async / TMA bulk-copy rings; ROC_SG_VARIANT forces one), so results
  * do not depend on the variant either. */
 int roc_sg_forward_planned(const roc_sg_plan* plan, int H, const float* in,
                            int64_t ldIn, float* out, int64_t ldOut, int epilogue,

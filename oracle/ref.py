@@ -1,7 +1,7 @@
 """ref.py — ctypes front end of oracle/_ref/libroc_ref.so: the REFERENCE's own CUDA
-kernels (cut from /root/reference by oracle/Makefile) launched with the
+kernels (cut from the reference sources by oracle/Makefile) launched with the
 reference's grid shapes on torch CUDA tensors.  TEST INFRASTRUCTURE ONLY: the
-second parity witness and the "reference kernel on the same B200" timing column.
+second parity witness and the "reference kernel on the same H100" timing column.
 """
 import ctypes as C
 import os

@@ -2,7 +2,7 @@
  * ref_harness.cu — launch harness for the REFERENCE's own CUDA kernels.
  *
  * TEST INFRASTRUCTURE (second parity witness + "reference kernel on the same
- * B200" timing column).  Nothing under roc_b200/ uses it.
+ * H100" timing column).  Nothing under roc_b200/ uses it.
  *
  * The reference cannot be built whole (every TU includes legion.h; the Legion
  * submodule is absent), but its __global__ kernel bodies have no Legion

@@ -9,7 +9,7 @@
  * the reference checkout, jiazhihao/ROC @ 1f58108).  The reference ships no CPU
  * kernels and no tests; this restatement is pinned against the reference's own
  * CUDA kernels (compiled from /root/reference by oracle/Makefile into
- * oracle/_ref/ and run on a B200; outputs committed under tests/golden/).
+ * oracle/_ref/ and run on the GPU; outputs committed under tests/golden/).
  *
  * Conventions (types.h:5-15, load_task.cu:283-292):
  *   V_ID = uint32, E_ID = uint64, DATATYPE = float.

@@ -1,4 +1,4 @@
-"""roc_b200 — B200-native (sm_100a) engine for ROC's GCN-training hot path.
+"""roc_b200 — H100-native (sm_90a) engine for ROC's GCN-training hot path.
 
 The compute lives in roc_b200/lib/libroc_b200.so (CUDA kernels + C ABI + C++ host);
 this package is the ctypes mirror of the reference's Model/op-builder API plus

@@ -176,4 +176,4 @@ def device_count():
 
 def require_device():
     if device_count() <= 0:
-        raise RocError("roc_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+        raise RocError("roc_b200 needs a CUDA device (sm_90a); there is no CPU fallback")

@@ -1,4 +1,4 @@
-// elementwise.cu — the HBM-bound pointwise ops of the GCN path for sm_100a:
+// elementwise.cu — the HBM-bound pointwise ops of the GCN path for sm_90a:
 // indegree_norm (+fused relu-mask backward), activation, add, dropout (Philox),
 // softmax-cross-entropy backward + metrics (one kernel), Adam, scale, fill,
 // device CSR build.  Each replaces a reference kernel or cuDNN call; see
@@ -6,7 +6,7 @@
 //
 // All are grid-stride kernels over [rows][H] windows of [rows][ld] tensors,
 // 16-byte vectorised when H, ld and the base pointers allow, launched with a
-// grid that is a multiple of the SM count (148 on B200).
+// grid that is a multiple of the SM count (132 on H100).
 #include <initializer_list>
 #include "common.cuh"
 
@@ -16,16 +16,16 @@ std::atomic<uint64_t> g_launches{0};
 
 // SMs a persistent / grid-stride launch sizes itself for: the device's count minus what the calling thread
 // reserved with roc_set_sm_reserve (so that a peer-write exchange running on another stream finds free SMs:
-// the tcgen05 GEMMs hold a whole SM's registers and shared memory per CTA, nothing can co-reside with them).
+// the tensor-core GEMMs hold a whole SM's registers and shared memory per CTA, nothing can co-reside with them).
 static thread_local int t_smReserve = 0;
 int sm_count() {
   static int n = 0;
   if (n == 0) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
     cudaDeviceProp p;
-    if (cudaGetDeviceProperties(&p, dev) != cudaSuccess) return 148;
-    n = p.multiProcessorCount > 0 ? p.multiProcessorCount : 148;
+    if (cudaGetDeviceProperties(&p, dev) != cudaSuccess) return 132;
+    n = p.multiProcessorCount > 0 ? p.multiProcessorCount : 132;
   }
   const int avail = n - t_smReserve;
   return avail > 8 ? avail : 8;
@@ -538,7 +538,7 @@ static inline bool vec_ok(int H, std::initializer_list<int64_t> lds, std::initia
 
 using namespace roc;
 
-extern "C" const char* roc_version(void) { return "roc_b200 0.1 (sm_100a)"; }
+extern "C" const char* roc_version(void) { return "roc_b200 0.1 (sm_90a)"; }
 
 extern "C" int roc_device_count(void) {
   int n = 0;

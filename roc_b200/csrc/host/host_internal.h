@@ -79,8 +79,7 @@ struct RuntimeImpl {
   std::vector<cudaEvent_t> peerDone;       // last copy of the current exchange on that stream
   cudaEvent_t evPacked = nullptr;
   bool exchInFlight = false;           // copies of the previous exchange may still read the send buffer
-  int pushSMs = 0;                     // SMs a pipelined producer leaves free for the push kernel (0: none — reserving
-                                       // 16 or 32 measured no better at 2 and 4 GPUs, r2 runs m5 / m6)
+  int pushSMs = 0;                     // SMs a pipelined producer leaves free for the push kernel (0: none)
   int pushGridSMs = 0;                 // SMs the pipelined push kernel's grid is sized for (-1: pushSMs, 0: whole chip)
   int* d_barrier = nullptr;
   std::vector<TensorImpl> tensors;

@@ -213,10 +213,8 @@ bool Model::init(const Config& config) {
       // CUDA IPC is not available between the devices).
       const char* he = getenv("ROC_B200_HALO");
       rt->p2p = !(he && he[0] == 'n') && rt->numParts <= ROC_MAX_PEERS;
-      // Two ways to fill the peers' slabs, chosen by measurement (r2 runs m5-m8, ms/step at 2 / 4 / 8 GPUs):
-      // pack + one DMA copy per peer 20.8 / - / 33.1 (the copy engines do not keep 7 peer copies busy), the SM
-      // kernel roc_push_rows 21.2 / 24.8 / 29.0, staged rows + NCCL 21.8 / 26.0 / 30.7.
-      // ROC_B200_HALO=push | ce forces one.
+      // Two ways to fill the peers' slabs: pack + one DMA copy per peer at 2 GPUs (the copy engines do not keep
+      // many peer copies busy), the SM kernel roc_push_rows beyond.  ROC_B200_HALO=push | ce forces one.
       rt->p2pCopyEngines = (he && he[0] == 'c') ? true : (he && he[0] == 'p') ? false : rt->numParts == 2;
       for (size_t l = 0; l < layers.size() && rt->p2p; l++) {
         if (!as<ScatterGather>(layers[l])) continue;
@@ -403,7 +401,7 @@ void Model::set_tensor(const Tensor& t, const void* host, bool grad) {
   } else {
     // Dense host rows -> padded device rows.  A strided cudaMemcpy2D of 2.4 KB rows runs at
     // ~17 GB/s; contiguous chunks into a staging buffer run at PCIe speed and the re-pitch
-    // is a device copy at HBM speed (r1 run 4: 10.1 GB upload 600 ms -> ~190 ms).
+    // is a device copy at HBM speed.
     const int64_t chunkRows = std::max<int64_t>(1, (int64_t)(64u << 20) / x.H);   // ~256 MB of floats
     rt->ensure_staging((size_t)std::min<int64_t>(chunkRows, x.rows) * x.H * sizeof(float));
     const float* h = static_cast<const float*>(host);

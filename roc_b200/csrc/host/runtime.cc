@@ -351,7 +351,7 @@ Runtime::Runtime(int device, int myPart, int numParts) {
     // The compute stream outranks the exchange stream: when a producer block and the push of the previous block
     // become runnable together, the producer's CTAs (a whole SM each) are placed first and the push kernel takes
     // the SMs the producer left free — the other way round its small CTAs would sit on every SM and keep the
-    // producer out (r2 run m2: 29.0 ms/step at 8 GPUs although only 2.0 ms of the exchange were exposed).
+    // producer out.
     int lo = 0, hi = 0;   // numerically lower = higher priority
     ROC_CHECK(cudaDeviceGetStreamPriorityRange(&lo, &hi));
     const char* pe = getenv("ROC_B200_PUSH_PRIO");          // experiments: 0 = equal priorities
@@ -377,7 +377,7 @@ Runtime::Runtime(int device, int myPart, int numParts) {
   {
     // The stream-ordered allocations of the kernel layer (the GEMMs' split-weight scratch) come from the device's
     // default pool; by default it hands unused memory back at every synchronisation and the next step pays the
-    // driver allocation again (one 35 ms step among ten 18.7 ms ones, r2 session 1).  Keep it.
+    // driver allocation again (one slow step in every few).  Keep it.
     cudaMemPool_t pool = nullptr;
     if (cudaDeviceGetDefaultMemPool(&pool, device) == cudaSuccess && pool) {
       uint64_t keep = UINT64_MAX;

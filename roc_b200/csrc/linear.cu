@@ -15,8 +15,8 @@ int simt_linear_dw(int64_t rows, int inDim, int outDim, const float* X, int64_t 
                    float* dW, float* workspace, size_t wsBytes, const DropMask* dm, cudaStream_t st);
 int relu_bwd_inplace(int64_t rows, int H, const float* Y, int64_t ldY, float* dY, int64_t ldDY, cudaStream_t st);
 
-// tensor-core path (linear_tc.cu); each returns ROC_ERR_UNSUPPORTED when the
-// shape / alignment is outside what the tcgen05 kernels take.
+// tensor-core path (linear_tc.cu, linear_tc_dw.cu); each returns ROC_ERR_UNSUPPORTED when the
+// shape / alignment is outside what the wgmma kernels take.
 int tc_linear_fwd(int64_t rows, int inDim, int outDim, const float* X, int64_t ldX, const float* W, float* Y,
                   int64_t ldY, int relu, const uint64_t* rowEnd, uint64_t colLeft, const DropMask* dm,
                   cudaStream_t st);
@@ -36,8 +36,8 @@ static bool force_simt() {
 }
 // which kernel family served the calling thread's last Linear GEMM of each kind (test hook: the tensor-core path
 // returns ROC_ERR_UNSUPPORTED for shapes it does not take and the dispatcher then uses SIMT — a test that means to
-// check tcgen05 must be able to see that it did)
-static thread_local int t_lastPath[3] = {0, 0, 0};   // fwd, dW, dX: 0 none, 1 tcgen05, 2 SIMT
+// check the tensor cores must be able to see that it did)
+static thread_local int t_lastPath[3] = {0, 0, 0};   // fwd, dW, dX: 0 none, 1 tensor cores (wgmma), 2 SIMT
 }  // namespace roc
 
 using namespace roc;

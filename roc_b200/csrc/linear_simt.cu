@@ -2,7 +2,7 @@
 //
 // Replaces the three cublasSgemm calls of the reference Linear op
 // (linear_kernel.cu:76-80 fwd, :220-224 dW, :227-231 dX).  This file is the
-// exact-fp32 register-tiled version; linear_tc.cu holds the tcgen05/TMEM
+// exact-fp32 register-tiled version; linear_tc.cu holds the wgmma
 // tensor-core version that the dispatcher in linear.cu prefers for large shapes.
 //
 //   FWD : Y[v][o]  = sum_i X[v][i]  * W[o*in+i]       (A K-contig, B K-contig)

@@ -1,4 +1,4 @@
-// linear_tc.cu — tcgen05 / TMEM tensor-core GEMMs for the Linear op, fed by TMA.
+// linear_tc.cu — wgmma tensor-core GEMMs for the Linear op, fed by TMA (sm_90a).
 //
 // Replaces cublasSgemm of Linear::forward_task (linear_kernel.cu:76-80) and the dX sgemm of
 // Linear::backward_task (linear_kernel.cu:227-231):
@@ -6,24 +6,22 @@
 //     dX : dX[v][i] = sum_o dY[v][o] * W[o*in + i]      M = rows, N = inDim,  K = outDim
 // fp32 in, fp32 out, within 1e-4 of sgemm: the tensor cores have no fp32 MMA, so
 // each operand is split hi + lo (hi = fp32 truncated to TF32's 10-bit mantissa,
-// lo = exact remainder) and three kind::tf32 MMAs accumulate hi*hi + lo*hi + hi*lo
-// in fp32 TMEM (3xTF32: error ~2^-20 relative per product).
+// lo = exact remainder) and three tf32 MMAs accumulate lo*hi + hi*lo + hi*hi
+// in fp32 registers (3xTF32: error ~2^-20 relative per product).
 //
 // One kernel serves both: a row-major [rows][K] streaming operand A (X or dY) times a
 // small K-major weight operand prepared by k_split_w ([N][K] hi / lo; dX passes W
-// transposed).  The streaming operand reaches the tensor core through TMEM: moving it
-// through shared memory as hi + lo costs ~136 KB of smem traffic per k-block (~1100 smem
-// cycles against ~700 cycles of HBM time); here the split warps read the TMA tile once
-// and tcgen05.st hi / lo straight into TMEM (A operand, K-major: lane = row, column = k).
-// One persistent CTA per SM (x N-tiles of <= 128 columns in grid.y), 12 or 16 warps:
-//   warp 0     TMA producer (A tile [128 rows][32 k] + W_hi + W_lo tile per stage), elect.sync
-//   warp 1     MMA issuer: 12 x tcgen05.mma [D], [A_tmem], B_smem per stage, elect.sync
-//   warp 2     TMEM allocator (512 columns: 2 accumulators + `stages` A slots of 64)
-//   warps 4-11 split (1 or 2 groups of 4 alternate k-blocks): smem (128B-swizzled) -> regs
-//              [-> dropout mask] -> hi/lo -> tcgen05.st
-//   last 4     epilogue of tile i (relu / dropout-backward mask / relu mask / row norm /
-//              accumulate) overlaps the main loop of tile i+1 (two accumulators)
-// HBM-bound on A (rows*K*4 bytes read once); W (tens of KB) stays in L2.  Roofline: DESIGN.md.
+// transposed).  The streaming operand is split where it is consumed: each consumer thread
+// reads its wgmma A fragment from the TMA tile (128-byte swizzle, conflict-free), applies the
+// fused dropout mask, splits it hi / lo in registers and issues wgmma with A from registers,
+// so the tile crosses shared memory once.  W_hi / W_lo come from shared memory (K-major,
+// 128-byte swizzle).  One persistent CTA per SM (x N-tiles of <= 128 columns in grid.y):
+//   warps 0-7  two consumer warpgroups, 64 rows of the 128-row tile each: fragment load,
+//              [dropout mask ->] hi/lo split, 3 x wgmma m64n32k8 per 32-column chunk and k8
+//              step, then the epilogue (relu / dropout-backward mask / relu mask / row norm /
+//              accumulate) straight from the accumulator registers
+//   warp 8     TMA producer (A tile [128 rows][32 k] + W_hi + W_lo tile per stage)
+// HBM-bound on A (rows*K*4 bytes read once); W (tens of KB) stays in L2.
 #include <cstdio>
 #include <cstdlib>
 #include "common.cuh"
@@ -33,11 +31,10 @@ namespace roc {
 
 using namespace tc;
 
-constexpr int TC_BM = 128;       // rows per tile (UMMA M)
-constexpr int TC_BK = 32;        // fp32 per k-block = one 128-byte swizzle row
-constexpr int TC_UK = 8;         // UMMA K for tf32
-constexpr int TS_THREADS = 512;  // 4 control warps + 4 x splitGroups split warps + epiWarps epilogue warps
-constexpr int TS_MAX_STAGES = 6;
+constexpr int TC_BM = 128;        // rows per tile: two consumer warpgroups of 64
+constexpr int TC_BK = 32;         // fp32 per k-block = one 128-byte swizzle row
+constexpr int TC_THREADS = 288;   // 8 consumer warps + 1 producer warp
+constexpr int TC_MAX_STAGES = 8;
 
 // Whi/Wlo[n][k] (n < Npad, k < Kpad, zero padded) = split of B(n, k), where
 //   transposed == 0: B(n, k) = W[n * ldW + k]   (fwd: n = output o, k = input i, ldW = inDim)
@@ -55,12 +52,9 @@ __global__ void k_split_w(int N, int K, int Npad, int Kpad, int ldW, int transpo
   }
 }
 
-struct TcTsParams {
+struct TcParams {
   float* Y; int64_t ldY;
-  int64_t rows; int outDim; int BN; int numKb; int stages;
-  uint32_t tmemCols, dStride, aCol0;
-  int splitGroups;      // 1 or 2 warpgroups of split warps (alternate k-blocks)
-  int epiWarps;         // 4 or 8 epilogue warps (8: two warps per TMEM lane quarter alternate 32-column chunks)
+  int64_t rows; int outDim; int numKb; int stages;
   const uint32_t* mask; int64_t ldm; float mscale;      // dropout of A fused into the operand load (NULL = none)
   // epilogue, applied in this order to acc(row, col):
   int relu;                                             //   relu (Linear's activation, linear_kernel.cu:83-104)
@@ -68,13 +62,10 @@ struct TcTsParams {
   const float* reluOf; int64_t ldR;                     //   relu backward: reluOf(row, col) > 0 ? x : 0
   const uint64_t* rowEnd; uint64_t colLeft;             //   indegree norm: x / sqrtf(deg(row))
   int accumulate;                                       //   Y += x instead of Y = x
-  int epiStaged;        // transpose the accumulator through smem for row-coalesced global accesses
 };
 
 // Epilogue stage switches: compile-time when the kernel is instantiated for a fixed combination
-// (EPI >= 0, a bit mask), read from the parameters for the generic instantiation (EPI < 0).  With all
-// five stages dynamic the unrolled epilogue was ~2000 SASS instructions and the epilogue warps stalled
-// on instruction fetch (r1 run 29).
+// (EPI >= 0, a bit mask), read from the parameters for the generic instantiation (EPI < 0).
 enum { EPI_RELU = 1, EPI_OMASK = 2, EPI_RELUOF = 4, EPI_NORM = 8, EPI_ACC = 16 };
 #define EPI_FLAGS(EPI, p)                                                        \
   const bool fRelu = (EPI) < 0 ? (p).relu != 0 : ((EPI) & EPI_RELU) != 0;         \
@@ -83,201 +74,72 @@ enum { EPI_RELU = 1, EPI_OMASK = 2, EPI_RELUOF = 4, EPI_NORM = 8, EPI_ACC = 16 }
   const bool fNorm = (EPI) < 0 ? (p).rowEnd != nullptr : ((EPI) & EPI_NORM) != 0;  \
   const bool fAcc = (EPI) < 0 ? (p).accumulate != 0 : ((EPI) & EPI_ACC) != 0;
 
-// Direct epilogue: each lane writes its own row (32 rows x 16 B per store instruction).
-template <int EPI>
-__device__ __forceinline__ void tc_epilogue_rows(uint32_t taddr, int n0, int64_t row, const TcTsParams& p, float d) {
-  EPI_FLAGS(EPI, p)
-  const RowDiv rd = rowdiv_make(d);
-  for (int c0 = 0; c0 < p.BN; c0 += 16) {
-    uint32_t r[16];
-    tmem_ld16(taddr + (uint32_t)c0, r);
-    tmem_ld_wait();
-    const int col0 = n0 + c0;
-    if (row < p.rows && col0 < p.outDim) {
-      float* y = p.Y + row * p.ldY + col0;
-      uint32_t mw = 0xFFFFFFFFu;      // the 16 columns of this chunk lie in one mask word (col0 % 16 == 0)
-      if (fOmask) mw = __ldg(p.omask + row * p.oldm + (col0 >> 5)) >> (col0 & 31);
-#pragma unroll
-      for (int q = 0; q < 4; q++) {
-        const int c = col0 + q * 4;
-        const bool full = c + 4 <= p.outDim;
-        float v[4], old[4] = {0.f, 0.f, 0.f, 0.f}, ro[4] = {1.f, 1.f, 1.f, 1.f};
-        if (fAcc) {
-          if (full) *reinterpret_cast<float4*>(old) = *reinterpret_cast<const float4*>(y + q * 4);
-          else
-#pragma unroll
-            for (int k = 0; k < 4; k++) if (c + k < p.outDim) old[k] = y[q * 4 + k];
-        }
-        if (fReluOf) {
-          const float* rp = p.reluOf + row * p.ldR + c;
-          if (full) *reinterpret_cast<float4*>(ro) = __ldg(reinterpret_cast<const float4*>(rp));
-          else
-#pragma unroll
-            for (int k = 0; k < 4; k++) if (c + k < p.outDim) ro[k] = rp[k];
-        }
-#pragma unroll
-        for (int k = 0; k < 4; k++) {
-          float x = __uint_as_float(r[q * 4 + k]);
-          if (fRelu) x = relu_nanprop(x);
-          if (fOmask) x = ((mw >> (q * 4 + k)) & 1u) ? x * p.oscale : 0.f;
-          if (fReluOf) x = (ro[k] > 0.f) ? x : 0.f;
-          if (fNorm) x = rowdiv(x, rd);   // == x / d bit for bit (common.cuh)
-          if (fAcc) x = old[k] + x;
-          v[k] = x;
-        }
-        if (full) *reinterpret_cast<float4*>(y + q * 4) = make_float4(v[0], v[1], v[2], v[3]);
-        else
-#pragma unroll
-          for (int k = 0; k < 4; k++) if (c + k < p.outDim) y[q * 4 + k] = v[k];
-      }
-    }
-  }
+__device__ __forceinline__ float row_norm_divisor(const TcParams& p, int64_t row) {
+  if (!p.rowEnd || row >= p.rows) return 1.0f;
+  const uint64_t st = (row == 0) ? p.colLeft : p.rowEnd[row - 1];
+  return sqrtf((float)(uint32_t)(p.rowEnd[row] - st));
 }
 
-// Epilogue of one warp's 32 rows of a tile.  tcgen05.ld hands each lane ITS row (lane = TMEM
-// lane); written straight to global that is 32 rows x 16 B per instruction.  So each 32-column
-// chunk is transposed through a padded shared tile ([32][36] floats per warp) and then handled
-// with 8 lanes per row: every global access (Y, the accumulate read, reluOf) is a 128-byte row
-// segment, and the per-row scalars (norm divisor, dropout-mask word) are shared by the row's lanes.
-constexpr int EPI_LD = 36;                        // padded row of the transposition tile: 16-byte aligned, conflict-free
-constexpr int EPI_STG_FLOATS = 32 * EPI_LD + 32; // per warp: transposition tile + per-row divisors
-
+// Epilogue of two adjacent columns (col even) of one row: the accumulator pair a thread holds.
 template <int EPI>
-__device__ __forceinline__ void tc_epilogue_warp(uint32_t taddr, int n0, int64_t row0, const TcTsParams& p,
-                                                 float* stg, int lane, float myD, int chunk0, int chunkStep) {
+__device__ __forceinline__ void tc_store_pair(const TcParams& p, int64_t row, int col, float x0, float x1,
+                                              const RowDiv& rd) {
   EPI_FLAGS(EPI, p)
-  float* sd = stg + 32 * EPI_LD;
-  sd[lane] = myD;     // this lane's row divisor (computed by the caller before the accumulator wait)
-  const int rq = lane >> 3, cq = (lane & 7) * 4;
-  for (int c0 = chunk0 * 32; c0 < p.BN; c0 += chunkStep * 32) {
-    const int cw = min(32, p.BN - c0);     // 32, or 16 for the last chunk of BN % 32 == 16
-    uint32_t r[32];
-    tmem_ld16(taddr + (uint32_t)c0, *reinterpret_cast<uint32_t(*)[16]>(&r[0]));
-    if (cw == 32) tmem_ld16(taddr + (uint32_t)c0 + 16u, *reinterpret_cast<uint32_t(*)[16]>(&r[16]));
-    tmem_ld_wait();
-    __syncwarp();                           // the previous chunk's readers are done with the tile
-#pragma unroll
-    for (int k = 0; k < 32; k += 4)
-      if (k < cw)
-        *reinterpret_cast<uint4*>(stg + lane * EPI_LD + k) = make_uint4(r[k], r[k + 1], r[k + 2], r[k + 3]);
-    __syncwarp();
-    const int c = n0 + c0 + cq;             // global column of this lane's 4 values
-    if (cq < cw && c < p.outDim) {
-      const bool full = c + 4 <= p.outDim;
-      // two batches of 4 rows: every load of a batch is issued before its arithmetic
-#pragma unroll
-      for (int hb = 0; hb < 2; hb++) {
-        float acc[4][4], old[4][4], ro[4][4], dd[4];
-        uint32_t mw[4];
-#pragma unroll
-        for (int i = 0; i < 4; i++) {
-          const int rl = (hb * 4 + i) * 4 + rq;
-          const int64_t row = row0 + rl;
-          const bool ok = row < p.rows;
-          *reinterpret_cast<float4*>(acc[i]) = *reinterpret_cast<const float4*>(stg + rl * EPI_LD + cq);
-          dd[i] = fNorm ? sd[rl] : 1.0f;
-          mw[i] = 0xFu;                   // c % 4 == 0: the 4 mask bits sit in one word
-          if (fOmask && ok) mw[i] = __ldg(p.omask + row * p.oldm + (c >> 5)) >> (c & 31);
-#pragma unroll
-          for (int k = 0; k < 4; k++) { old[i][k] = 0.f; ro[i][k] = 1.f; }
-          if (fAcc && ok) {
-            const float* y = p.Y + row * p.ldY + c;
-            if (full) *reinterpret_cast<float4*>(old[i]) = *reinterpret_cast<const float4*>(y);
-            else
-#pragma unroll
-              for (int k = 0; k < 4; k++) if (c + k < p.outDim) old[i][k] = y[k];
-          }
-          if (fReluOf && ok) {
-            const float* rp = p.reluOf + row * p.ldR + c;
-            if (full) *reinterpret_cast<float4*>(ro[i]) = __ldg(reinterpret_cast<const float4*>(rp));
-            else
-#pragma unroll
-              for (int k = 0; k < 4; k++) if (c + k < p.outDim) ro[i][k] = rp[k];
-          }
-        }
-#pragma unroll
-        for (int i = 0; i < 4; i++) {
-          const int rl = (hb * 4 + i) * 4 + rq;
-          const int64_t row = row0 + rl;
-          if (row >= p.rows) continue;
-          float v[4];
-#pragma unroll
-          for (int k = 0; k < 4; k++) {
-            float x = acc[i][k];
-            if (fRelu) x = relu_nanprop(x);
-            if (fOmask) x = x * p.oscale;       // the kept value; dropped ones are zeroed after the divide
-            v[k] = x;
-          }
-          // x / d first, masks after: (m ? x : 0) / d == m ? x / d : 0 bit for bit for a finite d > 0, and
-          // the divide then never sees the masked-out zeros.  Degenerate divisors (deg 0 -> 0 / 0 = NaN must
-          // survive) keep the literal order.
-          const RowDiv rd = rowdiv_make(dd[i]);
-          const bool maskFirst = fNorm && rd.plain;
-#pragma unroll
-          for (int pass = 0; pass < 2; pass++) {
-            if (pass == (maskFirst ? 0 : 1)) {
-#pragma unroll
-              for (int k = 0; k < 4; k++) {
-                float x = v[k];
-                if (fOmask) x = ((mw[i] >> k) & 1u) ? x : 0.f;
-                if (fReluOf) x = (ro[i][k] > 0.f) ? x : 0.f;
-                v[k] = x;
-              }
-            } else if (fNorm) {
-              rowdiv4(v, rd, full ? 4 : p.outDim - c);
-            }
-          }
-          if (fAcc) {
-#pragma unroll
-            for (int k = 0; k < 4; k++) v[k] = old[i][k] + v[k];
-          }
-          float* y = p.Y + row * p.ldY + c;
-          if (full) *reinterpret_cast<float4*>(y) = make_float4(v[0], v[1], v[2], v[3]);
-          else
-#pragma unroll
-            for (int k = 0; k < 4; k++) if (c + k < p.outDim) y[k] = v[k];
-        }
-      }
-    }
+  if (row >= p.rows || col >= p.outDim) return;
+  const bool two = col + 1 < p.outDim;
+  float* y = p.Y + row * p.ldY + col;
+  uint32_t mw = 3u;                 // col is even: col and col + 1 sit in one mask word
+  if (fOmask) mw = __ldg(p.omask + row * p.oldm + (col >> 5)) >> (col & 31);
+  float old[2] = {0.f, 0.f}, ro[2] = {1.f, 1.f};
+  if (fAcc) {
+    if (two) { const float2 o = *reinterpret_cast<const float2*>(y); old[0] = o.x; old[1] = o.y; }
+    else old[0] = y[0];
   }
-  __syncwarp();
+  if (fReluOf) {
+    const float* rp = p.reluOf + row * p.ldR + col;
+    if (two) { const float2 o = __ldg(reinterpret_cast<const float2*>(rp)); ro[0] = o.x; ro[1] = o.y; }
+    else ro[0] = rp[0];
+  }
+  float v[2] = {x0, x1};
+#pragma unroll
+  for (int k = 0; k < 2; k++) {
+    float x = v[k];
+    if (fRelu) x = relu_nanprop(x);
+    if (fOmask) x = ((mw >> k) & 1u) ? x * p.oscale : 0.f;
+    if (fReluOf) x = (ro[k] > 0.f) ? x : 0.f;
+    if (fNorm) x = rowdiv(x, rd);   // == x / d bit for bit (common.cuh)
+    if (fAcc) x = old[k] + x;
+    v[k] = x;
+  }
+  if (two) *reinterpret_cast<float2*>(y) = make_float2(v[0], v[1]);
+  else y[0] = v[0];
 }
 
-template <int EPI>
-__global__ void __launch_bounds__(TS_THREADS, 1)
-k_tc_linear_ts(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CUtensorMap mapWhi,
-                   const __grid_constant__ CUtensorMap mapWlo, const TcTsParams p) {
+template <int NC, int EPI>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+k_tc_linear(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapWhi,
+            const __grid_constant__ CUtensorMap mapWlo, const TcParams p) {
+  constexpr int BN = 32 * NC;
+  constexpr uint32_t aBytes = TC_BM * TC_BK * 4;       // 16 KB of A per stage
+  constexpr uint32_t bBytes = BN * TC_BK * 4;
+  constexpr uint32_t stageBytes = aBytes + 2 * bBytes;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const uint32_t aBytes = TC_BM * TC_BK * 4;                 // 16 KB of X per stage
-  const uint32_t bBytes = (uint32_t)p.BN * TC_BK * 4;
-  const uint32_t stageBytes = aBytes + 2 * bBytes;
-  uint8_t* barBase = smem + (size_t)p.stages * stageBytes;
-  uint64_t* full = reinterpret_cast<uint64_t*>(barBase);    // [stages] TMA landed (X, W_hi, W_lo)
-  uint64_t* aFull = full + TS_MAX_STAGES;                   // [stages] hi/lo of X are in TMEM slot s
-  uint64_t* empty = aFull + TS_MAX_STAGES;                  // [stages] MMAs done with smem stage + TMEM slot
-  uint64_t* dFull = empty + TS_MAX_STAGES;                  // [2] accumulator complete
-  uint64_t* dEmpty = dFull + 2;                             // [2] accumulator drained by the epilogue
-  uint32_t* tmemAddr = reinterpret_cast<uint32_t*>(dEmpty + 2);
-  float* epiStg = reinterpret_cast<float*>(barBase + 256);   // 4 warps x EPI_STG_FLOATS
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * stageBytes);   // [stages] TMA landed
+  uint64_t* empty = full + TC_MAX_STAGES;                                                // [stages] consumers done
 
-  const int warp = uniform_warp_idx(), lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t numTiles = (p.rows + TC_BM - 1) / TC_BM;
-  const int n0 = blockIdx.y * p.BN;          // this CTA's slice of the N (output column) dimension
+  const int n0 = blockIdx.y * BN;          // this CTA's slice of the N (output column) dimension
 
   if (threadIdx.x == 0) {
-    tma_prefetch_desc(&mapX); tma_prefetch_desc(&mapWhi); tma_prefetch_desc(&mapWlo);
-    for (int s = 0; s < p.stages; s++) { mbar_init(&full[s], 1); mbar_init(&aFull[s], 4); mbar_init(&empty[s], 1); }
-    for (int b = 0; b < 2; b++) { mbar_init(&dFull[b], 1); mbar_init(&dEmpty[b], (uint32_t)p.epiWarps); }
+    tma_prefetch_desc(&mapA); tma_prefetch_desc(&mapWhi); tma_prefetch_desc(&mapWlo);
+    for (int s = 0; s < p.stages; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(tmemAddr, p.tmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmemBase = *tmemAddr;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ================================ TMA producer ================================
     int s = 0; uint32_t ph = 0;
     for (int64_t tile = blockIdx.x; tile < numTiles; tile += gridDim.x) {
@@ -285,8 +147,8 @@ k_tc_linear_ts(const __grid_constant__ CUtensorMap mapX, const __grid_constant__
         mbar_wait(&empty[s], ph ^ 1);
         uint8_t* st = smem + (size_t)s * stageBytes;
         if (elect_one()) {
-          mbar_arrive_expect_tx(&full[s], aBytes + 2 * bBytes);
-          tma_load_2d(st, &mapX, kb * TC_BK, (int)(tile * TC_BM), &full[s]);
+          mbar_arrive_expect_tx(&full[s], stageBytes);
+          tma_load_2d(st, &mapA, kb * TC_BK, (int)(tile * TC_BM), &full[s]);
           tma_load_2d(st + aBytes, &mapWhi, kb * TC_BK, n0, &full[s]);
           tma_load_2d(st + aBytes + bBytes, &mapWlo, kb * TC_BK, n0, &full[s]);
         }
@@ -294,149 +156,80 @@ k_tc_linear_ts(const __grid_constant__ CUtensorMap mapX, const __grid_constant__
         if (++s == p.stages) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    // ================================= MMA issuer =================================
-    // the whole warp runs the loop converged; one elected lane issues (see elect_one)
-    const uint32_t idesc = make_idesc_tf32(TC_BM, p.BN, 0, 0);
-    int s = 0; uint32_t ph = 0; uint32_t tl = 0;
-    for (int64_t tile = blockIdx.x; tile < numTiles; tile += gridDim.x, tl++) {
-      const uint32_t b = tl & 1u;
-      mbar_wait(&dEmpty[b], ((tl >> 1) & 1u) ^ 1u);   // the epilogue has drained accumulator b
-      tc_fence_after();
-      const uint32_t dAddr = tmemBase + b * p.dStride;
-      for (int kb = 0; kb < p.numKb; kb++) {
-        mbar_wait(&full[s], ph);                      // W tiles landed
-        mbar_wait(&aFull[s], ph);                     // X hi/lo stored to TMEM slot s
-        tc_fence_after();
-        const uint32_t aHi = tmemBase + p.aCol0 + (uint32_t)s * 64u;
-        const uint32_t aLo = aHi + 32u;
-        const uint32_t bHi = smem_u32(smem + (size_t)s * stageBytes) + aBytes;
-        const uint32_t bLo = bHi + bBytes;
-        if (elect_one()) {
+    return;
+  }
+
+  // ================================== consumers ===================================
+  const bool fNorm = (EPI) < 0 ? p.rowEnd != nullptr : ((EPI) & EPI_NORM) != 0;
+  const int g = lane >> 2, t = lane & 3;
+  const int rl = (warp >> 2) * 64 + (warp & 3) * 16 + g;    // tile rows of this thread: rl and rl + 8 (both == g mod 8)
+  const bool masked = p.mask != nullptr;
+  int s = 0; uint32_t ph = 0;
+  for (int64_t tile = blockIdx.x; tile < numTiles; tile += gridDim.x) {
+    const int64_t row0 = tile * TC_BM + rl, row1 = row0 + 8;
+    // the rows' norm divisors are fetched before the main loop so their DRAM latency overlaps it
+    const float d0 = fNorm ? row_norm_divisor(p, row0) : 1.0f;
+    const float d1 = fNorm ? row_norm_divisor(p, row1) : 1.0f;
+    float acc[NC][16];
 #pragma unroll
-          for (int k = 0; k < TC_BK / TC_UK; k++) {
-            const uint32_t off = k * TC_UK * 4;   // bytes along K inside the swizzled row
-            const uint64_t dBh = make_sdesc_sw128(bHi + off, 16, 1024), dBl = make_sdesc_sw128(bLo + off, 16, 1024);
-            umma_tf32_ts(dAddr, aLo + k * TC_UK, dBh, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-            umma_tf32_ts(dAddr, aHi + k * TC_UK, dBl, idesc, 1u);
-            umma_tf32_ts(dAddr, aHi + k * TC_UK, dBh, idesc, 1u);
-          }
-          umma_commit(&empty[s]);                           // smem stage + TMEM slot reusable
-          if (kb == p.numKb - 1) umma_commit(&dFull[b]);   // accumulator of this tile complete
-        }
-        __syncwarp();
-        if (++s == p.stages) { s = 0; ph ^= 1; }
-      }
-    }
-  } else if (warp >= 4 && warp < 4 + 4 * p.splitGroups) {
-    // ============== operand split: smem X tile -> hi / lo in TMEM slot s ==============
-    // group g of the split warps takes every splitGroups-th k-block, so one group's
-    // tcgen05.st / wait::st latency overlaps the other group's loads
-    const int g = (warp - 4) >> 2;
-    const int t = (threadIdx.x - 128) & 127;    // row of the tile == TMEM lane
-    const uint32_t laneBase = (uint32_t)((warp & 3) * 32) << 16;
-    const int64_t myTiles = (numTiles - blockIdx.x + gridDim.x - 1) / gridDim.x;
-    const int64_t iters = myTiles * p.numKb;
-    const bool masked = p.mask != nullptr;
-    int s = g % p.stages; uint32_t ph = (uint32_t)(g / p.stages) & 1u;
-    int kb = g % p.numKb; int64_t tile = blockIdx.x + (int64_t)(g / p.numKb) * gridDim.x;
-    // dropout fused into the operand load: bit c of mask[row][kb] keeps column 32 kb + c.  The word
-    // for this group's NEXT k-block is fetched one iteration ahead so its latency hides behind the split.
-    uint32_t mwNext = 0xFFFFFFFFu;
-    if (masked && g < iters) {
-      const int64_t row = tile * TC_BM + t;
-      mwNext = (row < p.rows) ? __ldg(p.mask + row * p.ldm + kb) : 0u;
-    }
-    for (int64_t it = g; it < iters; it += p.splitGroups) {
-      const uint32_t mw = mwNext;
-      if (masked && it + p.splitGroups < iters) {
-        int kbN = kb + p.splitGroups; int64_t tileN = tile;
-        while (kbN >= p.numKb) { kbN -= p.numKb; tileN += gridDim.x; }
-        const int64_t rowN = tileN * TC_BM + t;
-        mwNext = (rowN < p.rows) ? __ldg(p.mask + rowN * p.ldm + kbN) : 0u;
+    for (int c = 0; c < NC; c++)
+#pragma unroll
+      for (int i = 0; i < 16; i++) acc[c][i] = 0.f;
+    for (int kb = 0; kb < p.numKb; kb++) {
+      // dropout fused into the operand load: bit c of mask[row][kb] keeps column 32 kb + c
+      uint32_t mw0 = 0xFFFFFFFFu, mw1 = 0xFFFFFFFFu;
+      if (masked) {
+        mw0 = (row0 < p.rows) ? __ldg(p.mask + row0 * p.ldm + kb) : 0u;
+        mw1 = (row1 < p.rows) ? __ldg(p.mask + row1 * p.ldm + kb) : 0u;
       }
       mbar_wait(&full[s], ph);
-      // 128B swizzle: 16-byte chunk j of row t sits at chunk j ^ (t & 7)
-      const float4* xr = reinterpret_cast<const float4*>(smem + (size_t)s * stageBytes) + t * 8;
-      const uint32_t taddr = tmemBase + laneBase + p.aCol0 + (uint32_t)s * 64u;
+      const float* as = reinterpret_cast<const float*>(smem + (size_t)s * stageBytes);
+      const uint32_t bHi = smem_u32(smem + (size_t)s * stageBytes + aBytes), bLo = bHi + bBytes;
+      uint32_t fr[TC_BK / 8][2][4];    // A fragments (hi, lo) of every k8 step: live until the MMAs are retired
 #pragma unroll
-      for (int half = 0; half < 2; half++) {
-        uint32_t hi[16], lo[16];
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-          const float4 v = xr[(half * 4 + j) ^ (t & 7)];
-          const float e[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-          for (int k = 0; k < 4; k++) {
-            float x = e[k];
-            if (masked) x = ((mw >> (half * 16 + j * 4 + k)) & 1u) ? x * p.mscale : 0.f;   // == k_dropout
-            const uint32_t h = __float_as_uint(x) & 0xFFFFE000u;
-            hi[j * 4 + k] = h;
-            lo[j * 4 + k] = __float_as_uint(x - __uint_as_float(h));
-          }
+      for (int kk = 0; kk < TC_BK / 8; kk++) {
+        // 128B swizzle: 16-byte chunk j of row r sits at chunk j ^ (r & 7); columns 8 kk + t and 8 kk + t + 4
+        const int o0 = (((2 * kk) ^ g) << 2) + t, o1 = (((2 * kk + 1) ^ g) << 2) + t;
+        float x[4] = {as[rl * TC_BK + o0], as[(rl + 8) * TC_BK + o0], as[rl * TC_BK + o1], as[(rl + 8) * TC_BK + o1]};
+        if (masked) {
+          const int b0 = 8 * kk + t, b1 = b0 + 4;
+          x[0] = ((mw0 >> b0) & 1u) ? x[0] * p.mscale : 0.f;   // == k_dropout
+          x[1] = ((mw1 >> b0) & 1u) ? x[1] * p.mscale : 0.f;
+          x[2] = ((mw0 >> b1) & 1u) ? x[2] * p.mscale : 0.f;
+          x[3] = ((mw1 >> b1) & 1u) ? x[3] * p.mscale : 0.f;
         }
-        tmem_st16(taddr + half * 16, hi);
-        tmem_st16(taddr + 32 + half * 16, lo);
-      }
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&aFull[s]);
-      s += p.splitGroups; if (s >= p.stages) { s -= p.stages; ph ^= 1u; }
-      kb += p.splitGroups; while (kb >= p.numKb) { kb -= p.numKb; tile += gridDim.x; }
-    }
-  } else if (warp >= 4 + 4 * p.splitGroups) {
-    // ===== epilogue: TMEM lane = row of the tile; this warp owns lanes 32*(warp%4)..+31 =====
-    uint32_t tl = 0;
-    for (int64_t tile = blockIdx.x; tile < numTiles; tile += gridDim.x, tl++) {
-      const uint32_t b = tl & 1u;
-      // the row's norm divisor is fetched BEFORE waiting for the accumulator: its DRAM latency
-      // (rowEnd streams, always cold) then overlaps the main loop instead of adding to every tile
-      const int64_t row0 = tile * TC_BM + (warp & 3) * 32;
-      float myD = 1.0f;
-      if (p.rowEnd && row0 + lane < p.rows) {
-        const int64_t myRow = row0 + lane;
-        const uint64_t st = (myRow == 0) ? p.colLeft : p.rowEnd[myRow - 1];
-        myD = sqrtf((float)(uint32_t)(p.rowEnd[myRow] - st));
-      }
-      const int e = warp - 4 - 4 * p.splitGroups;      // epilogue warp index; warps e and e + 4 share a lane quarter
-      if (p.epiStaged && p.rowEnd && (lane & 15) == 0) {   // next tile's degrees (32 x u64 per warp = 2 lines)
-        const int64_t nrow = (tile + gridDim.x) * TC_BM + (warp & 3) * 32 + lane;
-        if (nrow < p.rows) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.rowEnd + nrow));
-      }
-      if (p.epiStaged && (p.reluOf || p.accumulate || p.omask)) {
-        // pull this warp's first chunk of the NEXT tile's epilogue operands into L2 (and, for the first
-        // tile, this one's): they stream (always cold); fetched on demand each batch exposes a DRAM latency.
-        // The epilogue paces short-K GEMMs, so the accumulator is usually ready: one tile ahead is needed.
-        const int c = n0 + (e >> 2) * 32 + (lane & 7) * 4;
-        if (c < p.outDim) {
-#pragma unroll 1
-          for (int64_t pt = (tl == 0) ? tile : tile + gridDim.x; pt <= tile + gridDim.x && pt < numTiles; pt += gridDim.x) {
-            const int64_t prow0 = pt * TC_BM + (warp & 3) * 32;
 #pragma unroll
-            for (int i = 0; i < 8; i++) {
-              const int64_t row = prow0 + i * 4 + (lane >> 3);
-              if (row < p.rows) {
-                if (p.reluOf) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.reluOf + row * p.ldR + c));
-                if (p.accumulate) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.Y + row * p.ldY + c));
-                if (p.omask && (lane & 7) == 0) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.omask + row * p.oldm + (c >> 5)));
-              }
-            }
-          }
+        for (int i = 0; i < 4; i++) split_tf32(x[i], fr[kk][0][i], fr[kk][1][i]);
+        wgmma_fence();
+#pragma unroll
+        for (int c = 0; c < NC; c++) {
+          const uint32_t off = (uint32_t)c * 32u * 128u + (uint32_t)kk * 32u;
+          const uint64_t dBh = make_sdesc_sw128(bHi + off), dBl = make_sdesc_sw128(bLo + off);
+          wgmma_m64n32k8_tf32(acc[c], fr[kk][1], dBh);
+          wgmma_m64n32k8_tf32(acc[c], fr[kk][0], dBl);
+          wgmma_m64n32k8_tf32(acc[c], fr[kk][0], dBh);
         }
       }
-      mbar_wait(&dFull[b], (tl >> 1) & 1u);
-      tc_fence_after();
-      const uint32_t taddr = tmemBase + ((uint32_t)((warp & 3) * 32) << 16) + b * p.dStride;
-      if (p.epiStaged) tc_epilogue_warp<EPI>(taddr, n0, row0, p, epiStg + e * EPI_STG_FLOATS, lane, myD, e >> 2, p.epiWarps >> 2);
-      else if (e < 4) tc_epilogue_rows<EPI>(taddr, n0, row0 + lane, p, myD);
-      tc_fence_before();
+      wgmma_commit();
+      wgmma_wait_all();
+      keep_live(fr);
+#pragma unroll
+      for (int c = 0; c < NC; c++) wgmma_fence_acc(acc[c]);
       __syncwarp();
-      if (lane == 0) mbar_arrive(&dEmpty[b]);
+      if (lane == 0) mbar_arrive(&empty[s]);
+      if (++s == p.stages) { s = 0; ph ^= 1; }
     }
+    // epilogue: acc[c][4j + {0,1}] = (row0, col, col + 1), acc[c][4j + {2,3}] = (row1, ...), col = n0 + 32c + 8j + 2t
+    const RowDiv rd0 = rowdiv_make(d0), rd1 = rowdiv_make(d1);
+#pragma unroll
+    for (int c = 0; c < NC; c++)
+#pragma unroll
+      for (int j = 0; j < 4; j++) {
+        const int col = n0 + c * 32 + j * 8 + 2 * t;
+        tc_store_pair<EPI>(p, row0, col, acc[c][4 * j], acc[c][4 * j + 1], rd0);
+        tc_store_pair<EPI>(p, row1, col, acc[c][4 * j + 2], acc[c][4 * j + 3], rd1);
+      }
   }
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmemBase, p.tmemCols);
 }
 
 // The split weights (W_hi / W_lo, padded) live in a stream-ordered allocation made for this call
@@ -451,6 +244,27 @@ struct TsEpilogue {
   int accumulate = 0;
 };
 
+template <int NC>
+static int tc_launch(dim3 grid, size_t smemBytes, int epi, const CUtensorMap& mapA, const CUtensorMap& mapWhi,
+                     const CUtensorMap& mapWlo, const TcParams& q, cudaStream_t st) {
+#define ROC_TC_LAUNCH(E)                                                                                          \
+  do {                                                                                                            \
+    static DynSmemCache configured;                                                                               \
+    ROC_CUDA(ensure_dyn_smem(k_tc_linear<NC, E>, smemBytes, configured));                                         \
+    k_tc_linear<NC, E><<<grid, TC_THREADS, smemBytes, st>>>(mapA, mapWhi, mapWlo, q);                             \
+  } while (0)
+  switch (epi) {   // the combinations the GCN path produces; anything else takes the generic kernel
+    case 0: ROC_TC_LAUNCH(0); break;
+    case EPI_NORM: ROC_TC_LAUNCH(EPI_NORM); break;
+    case EPI_OMASK: ROC_TC_LAUNCH(EPI_OMASK); break;
+    case EPI_OMASK | EPI_RELUOF | EPI_NORM: ROC_TC_LAUNCH(EPI_OMASK | EPI_RELUOF | EPI_NORM); break;
+    default: ROC_TC_LAUNCH(-1); break;
+  }
+#undef ROC_TC_LAUNCH
+  ROC_LAUNCH_CHECK();
+  return ROC_OK;
+}
+
 // Y[rows][N] (op)= A[rows][K] * B^T with B(n, k) taken from W as k_split_w describes
 static int ts_gemm(int64_t rows, int K, int N, const float* A, int64_t ldA, const float* W, int ldW, int transposed,
                    float* Y, int64_t ldY, const DropMask* inMask, const TsEpilogue& e, cudaStream_t st) {
@@ -460,13 +274,9 @@ static int ts_gemm(int64_t rows, int K, int N, const float* A, int64_t ldA, cons
   if (rows > 0x7FFFFF00ll) return ROC_ERR_UNSUPPORTED;   // TMA coordinates are int32
   if (!encode_tiled_fn()) return ROC_ERR_UNSUPPORTED;
   { const char* g = getenv("ROC_B200_GEMM"); if (g && g[0] == 'n' && g[1] == 'o') return ROC_ERR_UNSUPPORTED; }   // "notc"
-  int BN = (N + 15) / 16 * 16;
-  if (BN > 128) BN = 128;
-  // (128-column tiles hung sporadically in r2 sessions 1 / 3 / 6 — every time on the 4.2 M-row 602 -> 128 product of
-  // configs[3]: the ring had 3 stages and the two split groups met a stage's barrier only every other phase; fixed
-  // below by keeping the stage count even.  Validated on configs 2-4 and the GEMM / model tests in sessions 8 / 9;
-  // ROC_TS_BN128=0 goes back to 64-column tiles, which stream A once per 64 output columns.)
-  { const char* e = getenv("ROC_TS_BN128"); if (BN > 64 && e && e[0] == '0') BN = 64; }
+  // N-tile of 32, 64 or 128 columns (wgmma chunks of 32): the widest tile streams A once per 128 output columns
+  const int NC = (N <= 32) ? 1 : (N <= 64) ? 2 : 4;
+  const int BN = 32 * NC;
   const int nTiles = (N + BN - 1) / BN;
   const int Npad = nTiles * BN;
   const int Kpad = (K + TC_BK - 1) / TC_BK * TC_BK;
@@ -487,42 +297,15 @@ static int ts_gemm(int64_t rows, int K, int N, const float* A, int64_t ldA, cons
   if (!make_tmap_f32_2d(&mapWhi, Whi, (uint64_t)Npad, (uint64_t)Kpad, (uint64_t)Kpad, (uint32_t)BN, TC_BK)) return ROC_ERR_UNSUPPORTED;
   if (!make_tmap_f32_2d(&mapWlo, Wlo, (uint64_t)Npad, (uint64_t)Kpad, (uint64_t)Kpad, (uint32_t)BN, TC_BK)) return ROC_ERR_UNSUPPORTED;
 
-  // 2 accumulators of dStride columns + `stages` A slots of 64 columns in the 512 TMEM columns
-  const uint32_t dStride = (uint32_t)((BN + 31) / 32 * 32);
+  // as many stages as fit in the 227 KB an H100 block may use (beside the alignment slack and the barriers)
   const size_t stageBytes = (size_t)TC_BM * TC_BK * 4 + (size_t)2 * BN * TC_BK * 4;
-  // Warp roles first (they size the epilogue staging), then the stage count.
-  // Few k-blocks per tile (K <= 128): the epilogue, not the main loop, paces the kernel -> 8 epilogue warps and one
-  // split group; otherwise two split groups (alternate k-blocks) and 4 epilogue warps.  512 threads either way.
-  int epiStaged = 1;
-  { const char* ee = getenv("ROC_TS_EPI"); if (ee) epiStaged = (ee[0] == 's'); }
-  int splitGroups = (Kpad / TC_BK <= 4 && epiStaged) ? 1 : 2;
-  { const char* s2 = getenv("ROC_TS_SPLIT"); if (s2) splitGroups = (s2[0] == '1') ? 1 : 2; }
-  if (!epiStaged) splitGroups = 2;
-  int stages = 0;
-  size_t fixedBytes = 0;
-  for (;;) {
-    const int epiWarps = 12 - 4 * splitGroups;
-    fixedBytes = 1024 /*align*/ + 256 /*barriers*/ + (size_t)epiWarps * EPI_STG_FLOATS * sizeof(float);
-    stages = (int)((512 - 2 * dStride) / 64);
-    if (stages > TS_MAX_STAGES) stages = TS_MAX_STAGES;
-    while (stages > 0 && (size_t)stages * stageBytes + fixedBytes > (size_t)224 * 1024) stages--;
-    // Two split groups take alternate k-blocks, i.e. alternate stages: with an EVEN stage count each group owns its
-    // stages and meets every phase of their barriers.  With an odd count a group would meet a stage's `full` barrier
-    // only every other phase, and an mbarrier parity wait that skipped a phase takes the stale completion for its
-    // own (3 stages: sporadic hangs of the 128-column tiles, r2 sessions 1 / 3 / 6; 5 stages — what the 64-column
-    // tiles ran with before the staging was sized by the warp roles — left two loads of slack and never tripped).
-    if (splitGroups == 2 && (stages & 1)) stages--;
-    if (stages >= 3 || splitGroups == 1) break;
-    splitGroups = 1;                       // not enough room for an even ring of >= 4: one group, any stage count
-  }
-  if (stages < 3) return ROC_ERR_UNSUPPORTED;
-  TcTsParams q{};
-  q.Y = Y; q.ldY = ldY; q.rows = rows; q.outDim = N; q.BN = BN; q.numKb = Kpad / TC_BK;
-  q.stages = stages; q.tmemCols = 512; q.dStride = dStride; q.aCol0 = 2 * dStride;
+  const size_t fixedBytes = 1024 /*align*/ + 256 /*barriers*/;
+  int stages = (int)(((size_t)227 * 1024 - fixedBytes) / stageBytes);
+  if (stages > TC_MAX_STAGES) stages = TC_MAX_STAGES;
+  if (stages < 2) return ROC_ERR_UNSUPPORTED;
+  TcParams q{};
+  q.Y = Y; q.ldY = ldY; q.rows = rows; q.outDim = N; q.numKb = Kpad / TC_BK; q.stages = stages;
   q.accumulate = e.accumulate;
-  q.epiStaged = epiStaged;
-  q.splitGroups = splitGroups;
-  q.epiWarps = 12 - 4 * q.splitGroups;
   if (inMask) { q.mask = inMask->bits; q.ldm = inMask->ld; q.mscale = inMask->scale; }
   q.relu = e.relu;
   if (e.outMask) { q.omask = e.outMask->bits; q.oldm = e.outMask->ld; q.oscale = e.outMask->scale; }
@@ -536,23 +319,11 @@ static int ts_gemm(int64_t rows, int K, int N, const float* A, int64_t ldA, cons
   dim3 grid((unsigned)gx, (unsigned)nTiles, 1);
   const int epi = (q.relu ? EPI_RELU : 0) | (q.omask ? EPI_OMASK : 0) | (q.reluOf ? EPI_RELUOF : 0) |
                   (q.rowEnd ? EPI_NORM : 0) | (q.accumulate ? EPI_ACC : 0);
-  const unsigned threads = TS_THREADS;
-#define ROC_TS_LAUNCH(E)                                                                                          \
-  do {                                                                                                            \
-    static DynSmemCache configured;                                                                               \
-    ROC_CUDA(ensure_dyn_smem(k_tc_linear_ts<E>, smemBytes, configured));                                          \
-    k_tc_linear_ts<E><<<grid, threads, smemBytes, st>>>(mapA, mapWhi, mapWlo, q);                                 \
-  } while (0)
-  switch (epi) {   // the combinations the GCN path produces; anything else takes the generic kernel
-    case 0: ROC_TS_LAUNCH(0); break;
-    case EPI_NORM: ROC_TS_LAUNCH(EPI_NORM); break;
-    case EPI_OMASK: ROC_TS_LAUNCH(EPI_OMASK); break;
-    case EPI_OMASK | EPI_RELUOF | EPI_NORM: ROC_TS_LAUNCH(EPI_OMASK | EPI_RELUOF | EPI_NORM); break;
-    default: ROC_TS_LAUNCH(-1); break;
+  switch (NC) {
+    case 1: return tc_launch<1>(grid, smemBytes, epi, mapA, mapWhi, mapWlo, q, st);
+    case 2: return tc_launch<2>(grid, smemBytes, epi, mapA, mapWhi, mapWlo, q, st);
+    default: return tc_launch<4>(grid, smemBytes, epi, mapA, mapWhi, mapWlo, q, st);
   }
-#undef ROC_TS_LAUNCH
-  ROC_LAUNCH_CHECK();
-  return ROC_OK;
 }
 
 int tc_linear_fwd(int64_t rows, int inDim, int outDim, const float* X, int64_t ldX, const float* W, float* Y,

@@ -1,11 +1,21 @@
-// linear_tc_dw.cu — dW of the Linear op on tcgen05 / TMEM, fed by TMA (3xTF32).
+// linear_tc_dw.cu — dW of the Linear op on wgmma (sm_90a), fed by TMA (3xTF32).
 //
 // Replaces cublasSgemm(OP_N, OP_T) of Linear::backward_task (linear_kernel.cu:220-224):
 //     dW[o][i] += sum_v dY[v][o] * X[v][i]
-//   M = i (X columns, tiles of 128), N = o, K = v (vertices).  A CTA owns a vertex range
-//   (split-K) and up to 5 M-tiles at once, so X and dY stream through HBM once; the
-//   accumulators [128 x BN] sit side by side in TMEM.  Partials go to a workspace
-//   [splits][out][in]; a reduce kernel adds them into dW in split order (deterministic).
+//   M = i (X columns, tiles of 128), N = o (<= 256), K = v (vertices).  A CTA owns one M-tile and a
+//   vertex range (split-K), so X streams through HBM once; the accumulator [128 x N] sits in the
+//   registers of two consumer warpgroups.  Partials go to a workspace [splits][out][in]; a reduce
+//   kernel adds them into dW in split order (deterministic).
+//
+// wgmma takes tf32 operands from shared memory only K-major, and both X and dY are vertex-major
+// (MN-major for this product), so:
+//   A = X^T comes from registers: each consumer thread reads its fragment straight from the TMA tile
+//       [KS][128] (column i = row of A), applies the fused dropout mask and splits it hi / lo;
+//   B = dY^T is transposed and split once per stage by the consumers into two K-major tiles
+//       [N][KS] (hi, lo; 128-byte swizzle) that the MMAs of both warpgroups read.
+// Two warpgroups of 64 X columns each and nothing else: with the accumulator of up to 256 columns in
+// registers a third (producer) warp would cap them at 168 registers and serialise the MMAs.  Thread 0
+// refills a stage with TMA (X box + dY box) once both warpgroups are past it.
 #include <cstdlib>
 #include "common.cuh"
 #include "tc_common.cuh"
@@ -14,221 +24,143 @@ namespace roc {
 
 using namespace tc;
 
-constexpr int DW_BM = 128;
+constexpr int DW_BM = 128;         // X columns per CTA
+constexpr int DW_KS = 32;          // vertices per stage = one 128-byte swizzle row of dY^T
+constexpr int DW_THREADS = 256;    // two consumer warpgroups
+constexpr int DW_MAX_STAGES = 4;
 
-// X^T reaches the tensor core through TMEM (A operand, K-major: lane =
-// X column i, TMEM column = vertex), so the X tile crosses shared memory once (TMA in,
-// one transposing read by the split warps) instead of five times.  Only the small
-// dY tile is split hi/lo in shared memory (B operand, MN-major, as above).
-//   stage  = KS vertices: G boxes [KS x 128] of X (no swizzle) + dY atoms (+ the dropout-mask box)
-//   A slot = one M-tile of one stage: KS hi + KS lo TMEM columns, ring of up to 6 slots
-//   TMEM   = G accumulators [128 x BN] + the A slots behind them
-// KS = 16 when several M-tiles share the TMEM (inDim > 128); KS = 64 for a single M-tile, where the
-// per-stage fixed costs (barrier round trips, tcgen05.st / wait::st) otherwise dominate a 7 KB stage.
-constexpr int DWT_SLOTS = 6;
-constexpr int DWT_MAX_STAGES = 4;
-
-struct TcDwTsParams {
-  float* ws; int64_t rows; int inDim, outDim, BN, nbAtoms, G, MT;
-  int64_t vPerSplit;       // multiple of KS
-  uint32_t tmemCols, aCol0;
-  int stages, slots;
-  int splitGroups;         // 1 or 2 warpgroups of split warps (alternate A slots)
+struct TcDwParams {
+  float* ws; int64_t rows; int inDim, outDim;
+  int64_t vPerSplit;       // multiple of DW_KS
+  int stages;
   const uint32_t* mask; int64_t ldm; float mscale;   // fused dropout of X (NULL = none)
 };
 
-template <int KS>
-__global__ void __launch_bounds__(384, 1)
-k_tc_linear_dw_ts(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CUtensorMap mapDY,
-                  const __grid_constant__ CUtensorMap mapM, const TcDwTsParams p) {
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
+template <int NC>
+__global__ void __launch_bounds__(DW_THREADS, 1)
+k_tc_linear_dw(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CUtensorMap mapDY,
+               const TcDwParams p) {
+  constexpr int BN = 32 * NC;
+  constexpr uint32_t xBytes = DW_KS * DW_BM * 4;      // [KS][128] of X
+  constexpr uint32_t yBytes = DW_KS * BN * 4;         // [KS][BN] of dY
+  constexpr uint32_t stageBytes = xBytes + yBytes;
+  constexpr uint32_t bBytes = BN * DW_KS * 4;         // dY^T hi; lo beside it
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int g0 = blockIdx.y * p.G;
-  const int nt = min(p.G, p.MT - g0);
-  const uint32_t xTile = KS * DW_BM * 4;                         // 8 KB per M-tile
-  const uint32_t xBytes = (uint32_t)p.G * xTile;
-  const uint32_t bBytes = (uint32_t)p.nbAtoms * 1024u * (KS / 8);  // raw dY (later hi), lo beside it
-  const uint32_t mBox = (uint32_t)KS * (uint32_t)p.G * 4u * 4u;   // mask box: KS rows x (4 words per M-tile)
-  const uint32_t mBytes = p.mask ? (mBox + 1023u) / 1024u * 1024u : 0u;
-  const uint32_t stageBytes = xBytes + 2 * bBytes + mBytes;
-  uint8_t* barBase = smem + (size_t)p.stages * stageBytes;
-  uint64_t* fullTma = reinterpret_cast<uint64_t*>(barBase);          // [stages]
-  uint64_t* bFull = fullTma + DWT_MAX_STAGES;                        // [stages] dY hi/lo ready in smem
-  uint64_t* empty = bFull + DWT_MAX_STAGES;                          // [stages] stage's MMAs retired
-  uint64_t* aFull = empty + DWT_MAX_STAGES;                          // [slots] X^T hi/lo stored to TMEM
-  uint64_t* aEmpty = aFull + DWT_SLOTS;                              // [slots] MMAs done with the slot
-  uint64_t* tmemFull = aEmpty + DWT_SLOTS;
-  uint32_t* tmemAddr = reinterpret_cast<uint32_t*>(tmemFull + 1);
+  float* bHi = reinterpret_cast<float*>(smem);
+  float* bLo = reinterpret_cast<float*>(smem + bBytes);
+  uint8_t* stages = smem + 2 * bBytes;
+  uint64_t* full = reinterpret_cast<uint64_t*>(stages + (size_t)p.stages * stageBytes);   // [stages] TMA landed
 
-  const int warp = uniform_warp_idx(), lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int i0 = blockIdx.y * DW_BM;
   const int64_t v0 = (int64_t)blockIdx.x * p.vPerSplit;
   const int64_t v1 = min(p.rows, v0 + p.vPerSplit);
-  const int numSteps = (v1 > v0) ? (int)((v1 - v0 + KS - 1) / KS) : 0;
+  const int numSteps = (v1 > v0) ? (int)((v1 - v0 + DW_KS - 1) / DW_KS) : 0;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&mapX); tma_prefetch_desc(&mapDY);
-    if (p.mask) tma_prefetch_desc(&mapM);
-    for (int s = 0; s < p.stages; s++) { mbar_init(&fullTma[s], 1); mbar_init(&bFull[s], 4); mbar_init(&empty[s], 1); }
-    for (int a = 0; a < p.slots; a++) { mbar_init(&aFull[a], 4); mbar_init(&aEmpty[a], 1); }
-    mbar_init(tmemFull, 1);
+    for (int s = 0; s < p.stages; s++) mbar_init(&full[s], 1);
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(tmemAddr, p.tmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmemBase = *tmemAddr;
+  auto load = [&](int step) {     // TMA of vertex block `step` into stage step % stages (thread 0)
+    uint8_t* st = stages + (size_t)(step % p.stages) * stageBytes;
+    uint64_t* bar = &full[step % p.stages];
+    const int v = (int)(v0 + (int64_t)step * DW_KS);
+    mbar_arrive_expect_tx(bar, stageBytes);
+    tma_load_2d(st, &mapX, i0, v, bar);
+    tma_load_2d(st + xBytes, &mapDY, 0, v, bar);
+  };
+  if (threadIdx.x == 0)
+    for (int step = 0; step < p.stages && step < numSteps; step++) load(step);
 
-  if (warp == 0) {
-    // ================================ TMA producer ================================
-    int s = 0; uint32_t ph = 0;
-    const uint32_t tx = (uint32_t)nt * xTile + bBytes + (p.mask ? mBox : 0u);
-    for (int step = 0; step < numSteps; step++) {
-      mbar_wait(&empty[s], ph ^ 1);
-      uint8_t* st = smem + (size_t)s * stageBytes;
-      const int v = (int)(v0 + (int64_t)step * KS);
-      if (elect_one()) {
-        mbar_arrive_expect_tx(&fullTma[s], tx);
-        for (int j = 0; j < nt; j++) tma_load_2d(st + (size_t)j * xTile, &mapX, (g0 + j) * DW_BM, v, &fullTma[s]);
-        for (int ks = 0; ks < KS / 8; ks++)
-          for (int b = 0; b < p.nbAtoms; b++)
-            tma_load_2d(st + xBytes + (size_t)(ks * p.nbAtoms + b) * 1024, &mapDY, b * 32, v + ks * 8, &fullTma[s]);
-        if (p.mask) tma_load_2d(st + xBytes + 2 * bBytes, &mapM, g0 * 4, v, &fullTma[s]);
-      }
-      __syncwarp();
-      if (++s == p.stages) { s = 0; ph ^= 1; }
+  // ================================== consumers ===================================
+  const int g = lane >> 2, t = lane & 3;
+  const int il = (warp >> 2) * 64 + (warp & 3) * 16 + g;   // X columns of this thread: i0 + il and i0 + il + 8
+  const bool masked = p.mask != nullptr && i0 + il < p.inDim;   // (columns past inDim are zero-filled by TMA)
+  const int mcol = (i0 + il) >> 5, mb0 = (i0 + il) & 31, mb1 = mb0 + 8;   // both columns sit in one mask word
+  float acc[NC][16];
+#pragma unroll
+  for (int c = 0; c < NC; c++)
+#pragma unroll
+    for (int i = 0; i < 16; i++) acc[c][i] = 0.f;
+  int s = 0; uint32_t ph = 0;
+  for (int step = 0; step < numSteps; step++) {
+    const int64_t v = v0 + (int64_t)step * DW_KS;
+    // dropout fused into the operand load: this thread's mask words of vertices v + 8 kk + t (+ 4)
+    uint32_t mw[8];
+#pragma unroll
+    for (int q = 0; q < 8; q++) {
+      const int64_t row = v + 4 * q + t;                    // q = 2 kk + h: vertex 8 kk + 4 h + t
+      mw[q] = masked ? ((row < p.rows) ? __ldg(p.mask + row * p.ldm + mcol) : 0u) : 0xFFFFFFFFu;
     }
-  } else if (warp == 1) {
-    // ================================= MMA issuer =================================
-    // the whole warp runs the loop converged; one elected lane issues (see elect_one)
-    const uint32_t idesc = make_idesc_tf32(DW_BM, p.BN, 0, 1);    // A K-major (TMEM), B MN-major
-    int s = 0; uint32_t ph = 0; int a = 0; uint32_t aph = 0;
-    for (int step = 0; step < numSteps; step++) {
-      mbar_wait(&bFull[s], ph);
-      const uint32_t bHi = smem_u32(smem + (size_t)s * stageBytes) + xBytes;
-      const uint32_t bLo = bHi + bBytes;
-      for (int j = 0; j < nt; j++) {
-        mbar_wait(&aFull[a], aph);
-        tc_fence_after();
-        const uint32_t aHi = tmemBase + p.aCol0 + (uint32_t)a * (2u * KS);
-        const uint32_t aLo = aHi + (uint32_t)KS;
-        const uint32_t d = tmemBase + (uint32_t)(j * p.BN);
-        if (elect_one()) {
-#pragma unroll
-          for (int ks = 0; ks < KS / 8; ks++) {
-            const uint32_t off = (uint32_t)(ks * p.nbAtoms) * 1024u;
-            const uint64_t dBh = make_sdesc(bHi + off, 1024u, 512u, 1u), dBl = make_sdesc(bLo + off, 1024u, 512u, 1u);
-            umma_tf32_ts(d, aLo + ks * 8, dBh, idesc, (step > 0 || ks > 0) ? 1u : 0u);
-            umma_tf32_ts(d, aHi + ks * 8, dBl, idesc, 1u);
-            umma_tf32_ts(d, aHi + ks * 8, dBh, idesc, 1u);
-          }
-          umma_commit(&aEmpty[a]);
-          if (j == nt - 1) {
-            umma_commit(&empty[s]);
-            if (step == numSteps - 1) umma_commit(tmemFull);
-          }
-        }
-        __syncwarp();
-        if (++a == p.slots) { a = 0; aph ^= 1; }
-      }
-      if (++s == p.stages) { s = 0; ph ^= 1; }
+    mbar_wait(&full[s], ph);
+    const float* xs = reinterpret_cast<const float*>(stages + (size_t)s * stageBytes);
+    const float* ys = xs + DW_KS * DW_BM;
+    consumer_sync();              // both warpgroups are done with the previous stage (and its MMAs have completed)
+    if (threadIdx.x == 0 && step > 0 && step - 1 + p.stages < numSteps) load(step - 1 + p.stages);
+    // dY [KS][BN] -> dY^T hi / lo [BN][KS]; 128-byte swizzle: element (o, k) at o*32 + ((k/4 ^ o%8) * 4) + k%4
+    for (int idx = threadIdx.x; idx < DW_KS * BN; idx += 256) {
+      const int k = idx / BN, o = idx - k * BN;
+      uint32_t h, l;
+      split_tf32(ys[idx], h, l);
+      const int d = o * DW_KS + ((((k >> 2) ^ (o & 7))) << 2) + (k & 3);
+      bHi[d] = __uint_as_float(h);
+      bLo[d] = __uint_as_float(l);
     }
-  } else if (warp >= 4) {
-    // ============ dY split (smem), X^T split (TMEM), then the epilogue ============
-    // split group g takes every splitGroups-th A slot (flattened over steps x M-tiles); the
-    // group that owns a step's first slot also splits that step's dY tile
-    const int g = (warp - 4) >> 2;
-    const int t = (threadIdx.x - 128) & 127;   // X column inside the M-tile == TMEM lane
-    const uint32_t laneBase = (uint32_t)((warp & 3) * 32) << 16;
-    const int nB4 = (int)(bBytes / 16);
-    const int64_t iters = (int64_t)numSteps * nt;
-    int lastStep = -1;
-    const bool masked = p.mask != nullptr;
-    int step = g / nt, j = g % nt;
-    int s = step % p.stages; uint32_t sph = (uint32_t)(step / p.stages) & 1u;
-    int a = g % p.slots; uint32_t aph = (uint32_t)(g / p.slots) & 1u;
-    for (int64_t it = g; it < iters; it += p.splitGroups) {
-      uint8_t* st = smem + (size_t)s * stageBytes;
-      if (step != lastStep) {
-        lastStep = step;
-        mbar_wait(&fullTma[s], sph);
-        if (j < p.splitGroups && (it - j) % p.splitGroups == g) {   // owner of the step's slot 0
-          float4* b = reinterpret_cast<float4*>(st + xBytes);
-          float4* bl = reinterpret_cast<float4*>(st + xBytes + bBytes);
-          for (int i = t; i < nB4; i += 128) {
-            float4 v = b[i], h, l;
-            h.x = __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u); l.x = v.x - h.x;
-            h.y = __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u); l.y = v.y - h.y;
-            h.z = __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u); l.z = v.z - h.z;
-            h.w = __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u); l.w = v.w - h.w;
-            b[i] = h; bl[i] = l;
-          }
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&bFull[s]);
-        }
+    fence_proxy_async_smem();
+    consumer_sync();
+    const uint32_t dHi = smem_u32(bHi), dLo = smem_u32(bLo);
+    uint32_t fr[DW_KS / 8][2][4];      // A fragments (hi, lo) of every k8 step: live until the MMAs are retired
+#pragma unroll
+    for (int kk = 0; kk < DW_KS / 8; kk++) {
+      const int k0 = 8 * kk + t, k1 = k0 + 4;
+      float x[4] = {xs[k0 * DW_BM + il], xs[k0 * DW_BM + il + 8], xs[k1 * DW_BM + il], xs[k1 * DW_BM + il + 8]};
+      if (p.mask) {
+        const uint32_t m0 = mw[2 * kk], m1 = mw[2 * kk + 1];
+        x[0] = ((m0 >> mb0) & 1u) ? x[0] * p.mscale : 0.f;   // == k_dropout
+        x[1] = ((m0 >> mb1) & 1u) ? x[1] * p.mscale : 0.f;
+        x[2] = ((m1 >> mb0) & 1u) ? x[2] * p.mscale : 0.f;
+        x[3] = ((m1 >> mb1) & 1u) ? x[3] * p.mscale : 0.f;
       }
-      const float* x = reinterpret_cast<const float*>(st + (size_t)j * xTile) + t;   // [KS][128]: column t
-      // dropout fused into the operand load: this warp's 32 X columns are one mask word per vertex,
-      // TMA'd beside the X tile as [KS][4 G] words
-      const uint32_t* mk = reinterpret_cast<const uint32_t*>(st + xBytes + 2 * bBytes) + j * 4 + (warp & 3);
-      const uint32_t taddr = tmemBase + laneBase + p.aCol0 + (uint32_t)a * (2u * KS);
-      bool waited = false;
 #pragma unroll
-      for (int sb = 0; sb < KS / 16; sb++) {
-        uint32_t hi[16], lo[16];
+      for (int i = 0; i < 4; i++) split_tf32(x[i], fr[kk][0][i], fr[kk][1][i]);
+      wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 16; k++) {
-          const int kk = sb * 16 + k;
-          float e = x[kk * DW_BM];
-          if (masked) e = ((mk[kk * p.G * 4] >> lane) & 1u) ? e * p.mscale : 0.f;   // == k_dropout
-          const uint32_t h = __float_as_uint(e) & 0xFFFFE000u;
-          hi[k] = h;
-          lo[k] = __float_as_uint(e - __uint_as_float(h));
-        }
-        if (!waited) { mbar_wait(&aEmpty[a], aph ^ 1); tc_fence_after(); waited = true; }
-        tmem_st16(taddr + sb * 16, hi);
-        tmem_st16(taddr + KS + sb * 16, lo);
-      }
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&aFull[a]);
-      a += p.splitGroups; if (a >= p.slots) { a -= p.slots; aph ^= 1u; }
-      j += p.splitGroups;
-      while (j >= nt) { j -= nt; step++; if (++s == p.stages) { s = 0; sph ^= 1u; } }
-    }
-    if (g == 0) {
-    // ---- epilogue: D_j[i_local][o] -> ws[split][o*inDim + i]  (lane = i_local: coalesced along i)
-    float* ws = p.ws + (size_t)blockIdx.x * ((size_t)p.inDim * p.outDim);
-    if (numSteps > 0) {
-      mbar_wait(tmemFull, 0);
-      tc_fence_after();
-    }
-    for (int j = 0; j < nt; j++) {
-      const int i = (g0 + j) * DW_BM + (warp - 4) * 32 + lane;
-      const uint32_t taddr = tmemBase + laneBase + (uint32_t)(j * p.BN);
-      for (int c0 = 0; c0 < p.BN; c0 += 16) {
-        uint32_t r[16];
-        if (numSteps > 0) { tmem_ld16(taddr + (uint32_t)c0, r); tmem_ld_wait(); }
-        else {
-#pragma unroll
-          for (int k = 0; k < 16; k++) r[k] = 0u;
-        }
-        if (i < p.inDim) {
-#pragma unroll
-          for (int k = 0; k < 16; k++) {
-            const int o = c0 + k;
-            if (o < p.outDim) ws[(size_t)o * p.inDim + i] = __uint_as_float(r[k]);
-          }
-        }
+      for (int c = 0; c < NC; c++) {
+        const uint32_t off = (uint32_t)c * 32u * 128u + (uint32_t)kk * 32u;
+        const uint64_t bh = make_sdesc_sw128(dHi + off), bl = make_sdesc_sw128(dLo + off);
+        wgmma_m64n32k8_tf32(acc[c], fr[kk][1], bh);
+        wgmma_m64n32k8_tf32(acc[c], fr[kk][0], bl);
+        wgmma_m64n32k8_tf32(acc[c], fr[kk][0], bh);
       }
     }
-    tc_fence_before();
-    }
+    wgmma_commit();
+    wgmma_wait_all();
+    keep_live(fr);
+#pragma unroll
+    for (int c = 0; c < NC; c++) wgmma_fence_acc(acc[c]);
+    if (++s == p.stages) { s = 0; ph ^= 1; }
   }
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmemBase, p.tmemCols);
+  // ---- epilogue: acc[c][4j + {0,1}] = (i0 + il, o, o + 1), [4j + {2,3}] = (i0 + il + 8, ...), o = 32c + 8j + 2t
+  float* ws = p.ws + (size_t)blockIdx.x * ((size_t)p.inDim * p.outDim);
+  const int ia = i0 + il, ib = ia + 8;
+#pragma unroll
+  for (int c = 0; c < NC; c++)
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      const int o = c * 32 + j * 8 + 2 * t;
+#pragma unroll
+      for (int h = 0; h < 2; h++) {
+        if (o + h >= p.outDim) continue;
+        float* col = ws + (size_t)(o + h) * p.inDim;
+        if (ia < p.inDim) col[ia] = acc[c][4 * j + h];
+        if (ib < p.inDim) col[ib] = acc[c][4 * j + 2 + h];
+      }
+    }
 }
 
 __global__ void __launch_bounds__(256)
@@ -240,43 +172,44 @@ k_tc_splitk_reduce(int64_t count, int splits, const float* __restrict__ part, fl
   }
 }
 
-struct DwPlan { int BN, nb, G, MT, groups, splits, stages, KS, slots, aCol0; size_t stageBytes; };
+struct DwPlan { int NC, MT, splits, stages; size_t smemBytes; };
 
 static int tc_dw_plan(int64_t rows, int inDim, int outDim, DwPlan* q) {
   if (outDim > 256 || outDim < 1 || inDim < 4 || rows < 8) return ROC_ERR_UNSUPPORTED;
-  q->BN = (outDim + 15) / 16 * 16;
-  q->nb = (outDim + 31) / 32;
-  q->MT = (inDim + DW_BM - 1) / DW_BM;
   { const char* e = getenv("ROC_B200_GEMM"); if (e && e[0] == 'n' && e[1] == 'o') return ROC_ERR_UNSUPPORTED; }   // "notc"
-  // several M-tiles: accumulators in <= 320 TMEM columns + 6 A slots of 32; a single M-tile: KS = 64
-  int g = 320 / q->BN;
-  if (g > q->MT) g = q->MT;
-  if (g < 1) return ROC_ERR_UNSUPPORTED;
-  q->G = g;
-  q->groups = (q->MT + g - 1) / g;
-  q->KS = (q->MT == 1) ? 64 : 16;
-  { const char* e = getenv("ROC_DW_KS"); if (e && atoi(e) == 16) q->KS = 16; }
-  q->aCol0 = (q->KS == 16) ? 320 : (g * q->BN + 31) / 32 * 32;
-  q->slots = (512 - q->aCol0) / (2 * q->KS);
-  if (q->slots > DWT_SLOTS) q->slots = DWT_SLOTS;
-  if (q->slots < 2) return ROC_ERR_UNSUPPORTED;
-  q->stageBytes = (size_t)g * q->KS * DW_BM * 4 + (size_t)2 * q->nb * 1024 * (q->KS / 8) + 2048 /* mask box */;
-  int st = (int)((200 * 1024) / q->stageBytes);
-  if (st > DWT_MAX_STAGES) st = DWT_MAX_STAGES;
+  const int nc = (outDim + 31) / 32;
+  q->NC = nc <= 1 ? 1 : nc <= 2 ? 2 : nc <= 4 ? 4 : 8;
+  q->MT = (inDim + DW_BM - 1) / DW_BM;
+  const size_t bn = (size_t)32 * q->NC;
+  const size_t stageBytes = (size_t)DW_KS * DW_BM * 4 + (size_t)DW_KS * bn * 4;
+  const size_t fixedBytes = 1024 /*align*/ + 64 /*barriers*/ + 2 * bn * DW_KS * 4 /*dY^T hi / lo*/;
+  int st = (int)(((size_t)227 * 1024 - fixedBytes) / stageBytes);
+  if (st > DW_MAX_STAGES) st = DW_MAX_STAGES;
+  if (st < 2) return ROC_ERR_UNSUPPORTED;
   q->stages = st;
-  int sp = sm_count() / q->groups;
+  q->smemBytes = (size_t)st * stageBytes + fixedBytes;
+  int sp = sm_count() / q->MT;
   if (sp < 1) sp = 1;
   int64_t maxSp = (rows + 63) / 64;
   if (sp > maxSp) sp = (int)maxSp;
   q->splits = sp;
-  if (st >= 2) return ROC_OK;
-  return ROC_ERR_UNSUPPORTED;
+  return ROC_OK;
 }
 
 size_t tc_dw_workspace_bytes(int64_t rows, int inDim, int outDim) {
   DwPlan q;
   if (tc_dw_plan(rows, inDim, outDim, &q) != ROC_OK) return 0;
   return (size_t)q.splits * (size_t)inDim * (size_t)outDim * sizeof(float);
+}
+
+template <int NC>
+static int dw_launch(const DwPlan& q, const CUtensorMap& mapX, const CUtensorMap& mapDY, const TcDwParams& t,
+                     cudaStream_t st) {
+  static DynSmemCache configured;
+  ROC_CUDA(ensure_dyn_smem(k_tc_linear_dw<NC>, q.smemBytes, configured));
+  k_tc_linear_dw<NC><<<dim3((unsigned)q.splits, (unsigned)q.MT, 1), DW_THREADS, q.smemBytes, st>>>(mapX, mapDY, t);
+  ROC_LAUNCH_CHECK();
+  return ROC_OK;
 }
 
 int tc_linear_dw(int64_t rows, int inDim, int outDim, const float* X, int64_t ldX, const float* dY, int64_t ldDY,
@@ -288,48 +221,28 @@ int tc_linear_dw(int64_t rows, int inDim, int outDim, const float* X, int64_t ld
   const size_t count = (size_t)inDim * outDim;
   if (wsBytes < (size_t)q.splits * count * sizeof(float)) return ROC_ERR_INVALID;
   CUtensorMap mapX, mapDY;
-  {
-    if (!make_tmap_f32_2d(&mapX, X, (uint64_t)rows, (uint64_t)inDim, (uint64_t)ldX, (uint32_t)q.KS, DW_BM, CU_TENSOR_MAP_SWIZZLE_NONE)) return ROC_ERR_UNSUPPORTED;
-    if (!make_tmap_f32_2d(&mapDY, dY, (uint64_t)rows, (uint64_t)outDim, (uint64_t)ldDY, 8, 32, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B)) return ROC_ERR_UNSUPPORTED;
-    TcDwTsParams t{};
-    t.ws = workspace; t.rows = rows; t.inDim = inDim; t.outDim = outDim; t.BN = q.BN; t.nbAtoms = q.nb; t.G = q.G;
-    t.MT = q.MT; t.stages = q.stages; t.slots = q.slots;
-    t.vPerSplit = ((rows + q.splits - 1) / q.splits + q.KS - 1) / q.KS * q.KS;
-    t.tmemCols = 512; t.aCol0 = (uint32_t)q.aCol0;
-    { const char* e = getenv("ROC_TS_SPLIT"); t.splitGroups = (e && e[0] == '1') ? 1 : 2; }
-    // Two split groups take alternate A slots (and, with a single M-tile, alternate stages).  With an ODD number of
-    // slots or stages a group then meets the same barrier only every other phase — and an mbarrier parity wait is
-    // only meaningful one phase ahead (a waiter that skipped a phase takes the stale completion for its own).  One
-    // group sees every phase of every barrier.  (Found through the forward kernel's 128-column tiles, which run
-    // with 3 stages: sporadic hangs, r2 sessions 1 / 3 / 6.)
-    if (t.splitGroups == 2 && ((q.stages & 1) || (q.slots & 1))) t.splitGroups = 1;
-    CUtensorMap mapM = mapDY;   // placeholder when there is no mask (never dereferenced)
-    if (dm) {
-      t.mask = dm->bits; t.ldm = dm->ld; t.mscale = dm->scale;
-      if ((size_t)q.KS * q.G * 16 > 2048) return ROC_ERR_UNSUPPORTED;
-      if (!make_tmap_u32_2d(&mapM, dm->bits, (uint64_t)rows, (uint64_t)dm->ld, (uint64_t)dm->ld, (uint32_t)q.KS, (uint32_t)q.G * 4))
-        return ROC_ERR_UNSUPPORTED;
-    }
-    const size_t smemTs = (size_t)q.stages * q.stageBytes + 1024 + 256;
-    dim3 gridTs((unsigned)q.splits, (unsigned)q.groups, 1);
-    const unsigned threadsTs = 128 + 128 * t.splitGroups;
-    if (q.KS == 64) {
-      static DynSmemCache configured64;
-      ROC_CUDA(ensure_dyn_smem(k_tc_linear_dw_ts<64>, smemTs, configured64));
-      k_tc_linear_dw_ts<64><<<gridTs, threadsTs, smemTs, st>>>(mapX, mapDY, mapM, t);
-    } else {
-      static DynSmemCache configured16;
-      ROC_CUDA(ensure_dyn_smem(k_tc_linear_dw_ts<16>, smemTs, configured16));
-      k_tc_linear_dw_ts<16><<<gridTs, threadsTs, smemTs, st>>>(mapX, mapDY, mapM, t);
-    }
-    ROC_LAUNCH_CHECK();
-    int64_t blocksTs = ((int64_t)count + 255) / 256;
-    if (blocksTs > sm_count() * 8) blocksTs = sm_count() * 8;
-    k_tc_splitk_reduce<<<(unsigned)blocksTs, 256, 0, st>>>((int64_t)count, q.splits, workspace, dW);
-    ROC_LAUNCH_CHECK();
-    return ROC_OK;
+  if (!make_tmap_f32_2d(&mapX, X, (uint64_t)rows, (uint64_t)inDim, (uint64_t)ldX, DW_KS, DW_BM, CU_TENSOR_MAP_SWIZZLE_NONE))
+    return ROC_ERR_UNSUPPORTED;
+  if (!make_tmap_f32_2d(&mapDY, dY, (uint64_t)rows, (uint64_t)outDim, (uint64_t)ldDY, DW_KS, (uint32_t)(32 * q.NC),
+                        CU_TENSOR_MAP_SWIZZLE_NONE))
+    return ROC_ERR_UNSUPPORTED;
+  TcDwParams t{};
+  t.ws = workspace; t.rows = rows; t.inDim = inDim; t.outDim = outDim; t.stages = q.stages;
+  t.vPerSplit = ((rows + q.splits - 1) / q.splits + DW_KS - 1) / DW_KS * DW_KS;
+  if (dm) { t.mask = dm->bits; t.ldm = dm->ld; t.mscale = dm->scale; }
+  int rc;
+  switch (q.NC) {
+    case 1: rc = dw_launch<1>(q, mapX, mapDY, t, st); break;
+    case 2: rc = dw_launch<2>(q, mapX, mapDY, t, st); break;
+    case 4: rc = dw_launch<4>(q, mapX, mapDY, t, st); break;
+    default: rc = dw_launch<8>(q, mapX, mapDY, t, st); break;
   }
-  return ROC_ERR_UNSUPPORTED;
+  if (rc != ROC_OK) return rc;
+  int64_t blocks = ((int64_t)count + 255) / 256;
+  if (blocks > sm_count() * 8) blocks = sm_count() * 8;
+  k_tc_splitk_reduce<<<(unsigned)blocks, 256, 0, st>>>((int64_t)count, q.splits, workspace, dW);
+  ROC_LAUNCH_CHECK();
+  return ROC_OK;
 }
 
 }  // namespace roc

@@ -1,4 +1,4 @@
-// sg.cu — ScatterGather (CSR row-parallel SpMM, sum aggregation) for sm_100a.
+// sg.cu — ScatterGather (CSR row-parallel SpMM, sum aggregation) for sm_90a.
 //
 // Replaces aggre_coop_kernel + ScatterGather::{forward,backward}_task
 // (reference scattergather_kernel.cu:20-76, 78-170).  The reference walks one
@@ -22,11 +22,11 @@
 //      A  sg_chunk_kernel      registers: L = min(32, H/4) lanes per worker, one LDG.128 per lane and row,
 //                              8 rows in flight per lane (default up to 64 floats per row)
 //      C  sg_chunk_kernel_c2   cp.async (LDGSTS) ring per worker (rows wider than 256 floats)
-//      T  sg_chunk_kernel_t    TMA: one cp.async.bulk.tensor ... tile::gather4 per 4 edges into a shared-memory
+//      T  sg_chunk_kernel_t    TMA: cp.async.bulk row copies, four per 4-edge unit, into a shared-memory
 //                              ring per worker, mbarrier completion (default for 129..256 floats)
 //      U  (T, MODE 2)          the same with the source ids held by the lanes that issue them (65..128 floats)
 //      b  (T, MODE 1)          one plain cp.async.bulk per row (measurement only)
-//      R  sg_ring_kernel       producer / consumer ring: producer warps issue gather4s for whole chunks into a
+//      R  sg_ring_kernel       producer / consumer ring: producer warps issue the row copies for whole chunks into a
 //                              two-slot ring, two worker warps consume (the structure the measured gather ceilings
 //                              ask for; not yet faster — DESIGN.md §3.1)
 //    The choice per width is by measurement (pick_variant); ROC_SG_VARIANT forces one.
@@ -57,7 +57,6 @@ struct roc_sg_plan {
   const uint32_t* col = nullptr;  // caller's colSrc
   float* carry = nullptr;         // [numCarries][carryLd]
   size_t carryLd = 0;
-  uint64_t inRows = 1;            // 1 + largest source id in col: the rows a TMA tensor map of the input spans
   uint32_t* desc = nullptr;       // [numChunks][8] per-chunk start state of the ring kernel (k_chunk_desc)
   int device = 0;
 };
@@ -166,7 +165,7 @@ template <> struct V<4> {
   static __device__ __forceinline__ void add(T& a, const T& b) { a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w; }
   // IEEE divide.  A zero numerator sends nvcc's div.rn sequence down its slow path (FCHK flags
   // zero operands) and one such lane drags the whole warp along: gradients and pad columns are
-  // full of zeros (+28 % instructions in the backward launches, r1 run 12).  0/d == 0 (same
+  // full of zeros.  0/d == 0 (same
   // sign) for d != 0, so those lanes skip the divide; d == 0 (degree 0) still yields NaN/Inf.
   static __device__ __forceinline__ float div1(float a, float d) { return (a != 0.0f || d == 0.0f) ? a / d : a; }
   static __device__ __forceinline__ T div(const T& a, float d) {
@@ -215,8 +214,8 @@ struct SgParams {
 // out[v] = relu?(acc / sqrtf(deg)) — what the model applies right after
 // scatter_gather (gnn.cc:84-85), IEEE sqrt and divide like graphnorm_kernel.cu:49-51.
 // The divisor is uniform over the row, so the divide is the row-uniform form of common.cuh
-// (one refined reciprocal, 3 FMAs per element, bit-identical to div.rn): the plain `/` here
-// cost +0.7 ms (H=64) .. +1.8 ms (H=41, zero pad lanes on the slow path) per launch (r1 run 14).
+// (one refined reciprocal, 3 FMAs per element, bit-identical to div.rn), cheaper than the plain `/`
+// (zero pad lanes take its slow path).
 template <int VEC>
 __device__ __forceinline__ void epi_store(typename V<VEC>::T v, typename V<VEC>::T* dst, uint32_t deg, int epi) {
   if (epi & ROC_SG_EPI_NORM) {
@@ -255,7 +254,7 @@ sg_chunk_kernel(const SgParams p) {
 
   // The worker's start state comes from the plan's 32-byte chunk record (k_chunk_desc) — one load instead of
   // the dependent walk firstRow[w] -> rs[r0], rs[r0 - 1] -> ... that cost every worker three round trips
-  // before its first gather (r2: ~7 % of a warp's lifetime).
+  // before its first gather.
   const uint4 dA = __ldg(reinterpret_cast<const uint4*>(p.desc) + 2 * (size_t)w);
   const uint4 dB = __ldg(reinterpret_cast<const uint4*>(p.desc) + 2 * (size_t)w + 1);
   if (dB.z & 2u) return;           // nothing owned, nothing carried
@@ -274,7 +273,7 @@ sg_chunk_kernel(const SgParams p) {
 
   // Row store.  The epilogue (IEEE sqrt + divides) lives in ONE out-of-line copy:
   // inlining it at every edge position made the kernel 4096 SASS instructions and
-  // instruction-fetch bound (ncu: stalled_no_instruction 22.9 per issue, r1 run 2).
+  // instruction-fetch bound.
   auto flush = [&]() {
     char* dstb = (kind == 0)
         ? reinterpret_cast<char*>(reinterpret_cast<T*>(p.carry) + lane) + (uint64_t)carrySlot * ((uint32_t)p.ldC * (uint32_t)sizeof(T))
@@ -303,7 +302,7 @@ sg_chunk_kernel(const SgParams p) {
   // Gathers are unpredicated: a group that runs past the worker's last edge re-reads that edge's
   // source (index clamped; an L1 hit) and the tail values are simply never added.  With the tail
   // predicates (16 ISETP + 20 zero-inits per group) and a 64 x 64-bit address multiply the group
-  // preamble was 146 SASS instructions for 8 gathers (r1 run 39); now one VIMNMX + LDG + IMAD.WIDE
+  // preamble was 146 SASS instructions for 8 gathers; now one VIMNMX + LDG + IMAD.WIDE
   // + LDG.128 per edge.
   // lanes beyond the row's last column gather that last column instead (same sector, no extra
   // traffic): their sums are never stored (flush tests act[]), and no load needs a predicate
@@ -336,9 +335,9 @@ sg_chunk_kernel(const SgParams p) {
       // One rolled loop over the row segments of the group (predicated adds of the edges [pos, lim)
       // of the current segment, then ONE copy of the row store).  A separate branch-free path for
       // groups inside one row did not pay: the two 16-lane workers of a warp rarely agree, so the
-      // warp ran both paths in most iterations (r1 run 45).  The
+      // warp ran both paths in most iterations.  The
       // unrolled per-edge `while (edge == segEnd) { flush; advance; }` had 8 inlined copies of the
-      // store and cost ~180 SASS instructions per row (42 % of all instructions, r1 run 39).
+      // store and cost ~180 SASS instructions per row.
       uint32_t pos = 0;
       for (;;) {
         const uint32_t lim = min(cnt, segEnd - base);
@@ -378,7 +377,7 @@ template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
 // ------------------------------------------- main kernel, variant C (lean) ---
-// Variant C with the instruction stream trimmed (r1 run 10: the first version issued
+// Variant C with the instruction stream trimmed (a first version issued
 // 34 instructions per edge — generic-address arithmetic and per-edge predicates —
 // and was issue-bound once the latency was hidden): 32-bit shared addresses with
 // immediate slot offsets, whole-group fast paths when the group is complete and no
@@ -475,7 +474,7 @@ sg_chunk_kernel_c2(const SgParams p) {
   // issue group gi into the ring slots at byte offset slotOff (= (gi % P) * GRPB).
   // Every lane of the worker reads the source id itself (same address: one broadcast
   // transaction, L1-resident): a sub-warp __shfl_sync with a runtime mask costs a
-  // MATCH.ANY sequence, ~11 instructions per edge (ncu source page, r1 run 11).
+  // MATCH.ANY sequence of ~11 instructions per edge.
   (void)wmask;
   auto issue = [&](uint32_t gi, uint32_t slotOff) {
     if (gi < nG) {
@@ -551,20 +550,19 @@ sg_chunk_kernel_c2(const SgParams p) {
 
 // ------------------------------------------------- main kernel, variant T ---
 // Same schedule and the same per-row summation order again, but the neighbour rows are fetched by
-// the TMA unit: one `cp.async.bulk.tensor ... tile::gather4` per four edges (four row indices in
-// one instruction, sm_100 only) lands 4 x rowBytes in the worker's shared-memory ring and
+// the TMA unit: four `cp.async.bulk` row copies per four edges (one unit) land 4 x rowBytes in the
+// worker's shared-memory ring and
 // completes on an mbarrier; the lanes then add with LDS.128 + FADD.  What this buys over the
-// register variant A: (1) bytes in flight are bounded by the ring (P stages x S gather4s per
+// register variant A: (1) bytes in flight are bounded by the ring (P stages x S units per
 // worker, ~100 KB per SM) instead of by the register file — variant A holds 8 rows per lane in
 // registers, issues them as a burst, waits for all of them and only then adds, so its *average*
-// bytes in flight are well under half of its peak (ncu r1 run 45: latency-bound at 0.52 of the
-// DRAM peak, 47 % issue utilisation, nothing saturated); the ring is refilled stage by stage,
-// so it stays full.  (2) one TMA instruction per 4 edges replaces 4 x (index load + IMAD.WIDE +
-// LDG.128) per lane group.  MODE 1 issues one plain `cp.async.bulk` per row instead (no tensor
-// map; kept for measurement).
-// The tensor map's box is L*NCH*4 floats wide (the worker's whole lane span) over a tensor
-// that is Q*4 floats wide: columns past the row's end are zero-filled by the TMA unit, which
-// makes the shared-memory row pitch a compile-time constant and the adds unpredicated.
+// bytes in flight are well under half of its peak; the ring is refilled stage by stage, so it
+// stays full.  (2) the copies are issued by one lane instead of an index load + IMAD.WIDE +
+// LDG.128 per lane group.  MODE 1 issues the copies of a stage one row at a time (kept for
+// measurement).
+// A row slot is L*NCH*16 bytes (the worker's whole lane span), so the shared-memory row pitch is a
+// compile-time constant and the adds are unpredicated; lanes past the row's end add stale slot
+// contents they never store.
 __device__ __forceinline__ void mbar_init_a(uint32_t bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
 }
@@ -582,29 +580,29 @@ __device__ __forceinline__ void mbar_wait_a(uint32_t bar, uint32_t parity) {
       ::"r"(bar), "r"(parity)
       : "memory");
 }
-__device__ __forceinline__ void tma_gather4(uint32_t dst, const CUtensorMap* m, int c0, uint32_t r0, uint32_t r1,
-                                            uint32_t r2, uint32_t r3, uint32_t bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile::gather4.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%2, %3, %4, %5, %6}], [%7];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(r0), "r"(r1), "r"(r2), "r"(r3), "r"(bar)
-      : "memory");
-}
 __device__ __forceinline__ void bulk_row(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(dst), "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
+// four rows (source ids r0..r3) into consecutive slots of slotB bytes: one bulk copy of rowB bytes per row
+__device__ __forceinline__ void bulk_rows4(uint32_t dst, const char* inB, uint32_t strideB, uint32_t rowB, uint32_t slotB,
+                                           uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3, uint32_t bar) {
+  bulk_row(dst, inB + (size_t)r0 * strideB, rowB, bar);
+  bulk_row(dst + slotB, inB + (size_t)r1 * strideB, rowB, bar);
+  bulk_row(dst + 2 * slotB, inB + (size_t)r2 * strideB, rowB, bar);
+  bulk_row(dst + 3 * slotB, inB + (size_t)r3 * strideB, rowB, bar);
+}
 
 template <int L, int NCH, int S, int P, int NT, int MINB, int MODE>
 __global__ void __launch_bounds__(NT, MINB)
-sg_chunk_kernel_t(const SgParams p, const __grid_constant__ CUtensorMap tmap) {
+sg_chunk_kernel_t(const SgParams p) {
   typedef float4 T;
   constexpr int WPB = NT / L;
   constexpr uint32_t CH = SG_CH;
   constexpr int G = 4 * S;                       // edges per stage
   constexpr uint32_t SLOTB = NCH * L * 16;       // shared-memory bytes per gathered row
-  constexpr uint32_t G4B = 4 * SLOTB;            // one gather4
+  constexpr uint32_t G4B = 4 * SLOTB;            // one four-row unit
   constexpr uint32_t STAGEB = S * G4B;
   constexpr uint32_t RINGB = P * STAGEB;
   extern __shared__ __align__(128) unsigned char sg_smem_t[];
@@ -692,9 +690,9 @@ sg_chunk_kernel_t(const SgParams p, const __grid_constant__ CUtensorMap tmap) {
   const uint32_t strideB = (uint32_t)p.ldIn * 16u;
   const uint32_t rowB = p.Q * 16u;
   // MODE 2: the source ids never sit in front of the issue.  Lane j of the worker loads, once and up front, the
-  // ids of gather4 units j, j + L, ... of the worker's edge range (a worker has at most 127 edges = 32 units) and
-  // issues those units itself when their ring slot frees (ncu on MODE 0: 21 % of the stall samples waited for the
-  // id load of the stage about to be issued).
+  // ids of units j, j + L, ... of the worker's edge range (a worker has at most 127 edges = 32 units) and
+  // issues those units itself when their ring slot frees (on MODE 0 the id load of the stage about to be issued
+  // is a large share of the stalls).
   constexpr int NU = (MODE == 2) ? (32 / L) : 1;
   uint4 ids[NU];
   if (MODE == 2 && nE) {
@@ -715,15 +713,15 @@ sg_chunk_kernel_t(const SgParams p, const __grid_constant__ CUtensorMap tmap) {
         const uint32_t dst = ring + slot * STAGEB;
         const uint32_t nv = min((uint32_t)G, nE - off);
         const uint32_t n4 = (nv + 3u) >> 2;
-        if ((uint32_t)lane == (k * S) % (uint32_t)L) mbar_expect_tx_a(bar, n4 * G4B);
+        if ((uint32_t)lane == (k * S) % (uint32_t)L) mbar_expect_tx_a(bar, n4 * 4u * rowB);
 #pragma unroll
         for (int s = 0; s < S; s++) {
-          const uint32_t g = k * S + (uint32_t)s;              // gather4 unit within the worker's range
+          const uint32_t g = k * S + (uint32_t)s;              // unit within the worker's range
           if ((uint32_t)s < n4 && (uint32_t)lane == g % (uint32_t)L) {
             uint4 id = ids[0];
 #pragma unroll
             for (int n = 1; n < NU; n++) if (g / (uint32_t)L == (uint32_t)n) id = ids[n];
-            tma_gather4(dst + s * G4B, &tmap, 0, id.x, id.y, id.z, id.w, bar);
+            bulk_rows4(dst + s * G4B, inB, strideB, rowB, SLOTB, id.x, id.y, id.z, id.w, bar);
           }
         }
       }
@@ -737,7 +735,7 @@ sg_chunk_kernel_t(const SgParams p, const __grid_constant__ CUtensorMap tmap) {
       const uint32_t nv = min((uint32_t)G, nE - off);
       if (MODE == 0) {
         const uint32_t n4 = (nv + 3u) >> 2;
-        mbar_expect_tx_a(bar, n4 * G4B);
+        mbar_expect_tx_a(bar, n4 * 4u * rowB);
 #pragma unroll
         for (int s = 0; s < S; s++) {
           if ((uint32_t)s < n4) {
@@ -749,7 +747,7 @@ sg_chunk_kernel_t(const SgParams p, const __grid_constant__ CUtensorMap tmap) {
               i0 = __ldg(cp + min((uint32_t)(4 * s), last)); i1 = __ldg(cp + min((uint32_t)(4 * s + 1), last));
               i2 = __ldg(cp + min((uint32_t)(4 * s + 2), last)); i3 = __ldg(cp + min((uint32_t)(4 * s + 3), last));
             }
-            tma_gather4(dst + s * G4B, &tmap, 0, i0, i1, i2, i3, bar);
+            bulk_rows4(dst + s * G4B, inB, strideB, rowB, SLOTB, i0, i1, i2, i3, bar);
           }
         }
       } else {
@@ -813,18 +811,14 @@ sg_chunk_kernel_t(const SgParams p, const __grid_constant__ CUtensorMap tmap) {
 }
 
 // ------------------------------------------------- main kernel, variant R ---
-// Producer / consumer ring.  What the measurements of r2 asked for (tools/gather_ceiling.cu, B200):
-//  * the gather of this graph's row mix (69 % of the row fetches hit L2) is latency-bound: the pure
-//    LDG.128 gather reaches 38 B/clk/SM with variant A's 8 rows x 32 warps in flight and 58 with twice
-//    the warps — more requests outstanding than the register file can hold;
-//  * a shared-memory ring filled by `cp.async.bulk.tensor ... tile::gather4` sustains 55-60 B/clk/SM at
-//    that mix when (a) ~190 KB per SM are in flight, (b) the index loads never sit on the issue path
-//    and (c) several warps per SM issue: one UTMALDG costs its warp ~68 cycles (an ELECT / R2UR loop per
-//    lane), 15 B/clk per issuing warp at 1 KB per instruction.
+// Producer / consumer ring.  The gather of an R-MAT row mix (most row fetches hit L2) is latency-bound:
+// the register-held gather of variant A is limited by the requests the register file can back, while a
+// shared-memory ring filled by the TMA unit keeps more bytes in flight when (a) the ring is large, (b) the
+// index loads never sit on the issue path and (c) several warps per SM issue copies.
 // So: a CTA is ONE producer warp and TWO worker warps that share a two-slot ring; six CTAs per SM for rows
 // of up to 256 bytes.  A slot holds one 64-edge chunk of gathered rows (64 x SLOTB bytes) and completes on
 // one `full` mbarrier.  The CTA walks a contiguous range of chunk pairs; worker h owns the chunks of parity
-// h and slot h holds them.  The producer's lane j (of half-warp h) holds the four source ids of gather4 #j
+// h and slot h holds them.  The producer's lane j (of half-warp h) holds the four source ids of unit #j
 // of its chunk in registers — one coalesced LDG.128 per lane, loaded one pair ahead — and issues it as soon
 // as the slot's `empty` barrier says both readers are done.
 // Readers of a slot: the chunk's own worker, and the worker of the PREVIOUS chunk, whose last rows may run
@@ -867,7 +861,7 @@ template <> struct RV<4> {
 
 template <int VW, int NCH, int NPW, int MINB>
 __global__ void __launch_bounds__(32 * (NPW + 2), MINB)
-sg_ring_kernel(const SgParams p, const __grid_constant__ CUtensorMap tmap, uint32_t pairsPerCta) {
+sg_ring_kernel(const SgParams p, uint32_t pairsPerCta) {
   typedef typename RV<VW>::T T;
   constexpr uint32_t CH = SG_CH;
   constexpr uint32_t LANEB = VW * 4;                // bytes per lane per column block
@@ -894,15 +888,16 @@ sg_ring_kernel(const SgParams p, const __grid_constant__ CUtensorMap tmap, uint3
 
   if (warp < NPW) {
     // ----------------------------------------------------------- producers ---
-    // NPW warps share the 32 gather4s of a chunk pair: 32 / NPW lanes of each are active, lanes of one warp
-    // always serve the same slot (so the warp sees every phase of that slot's `empty` barrier).  One UTMALDG
-    // costs the issuing warp ~68 cycles (ELECT / R2UR loop), so a single warp needs ~2200 cycles per pair.
-    constexpr int PERW = 32 / NPW;                        // gather4s per producer warp and pair
-    const int g = warp * PERW + lane;                     // gather4 index within the pair: 0..15 slot 0, 16..31 slot 1
+    // NPW warps share the 32 units of a chunk pair: 32 / NPW lanes of each are active, lanes of one warp
+    // always serve the same slot (so the warp sees every phase of that slot's `empty` barrier).
+    constexpr int PERW = 32 / NPW;                        // units per producer warp and pair
+    const int g = warp * PERW + lane;                     // unit index within the pair: 0..15 slot 0, 16..31 slot 1
     const int h = g >> 4, j = g & 15;
     const bool mine = lane < PERW;
     const uint32_t* __restrict__ col = p.col;
-    auto load_ids = [&](uint32_t c, uint4& v) {           // the four sources of gather4 #j of chunk c
+    const char* inB = reinterpret_cast<const char*>(p.in);
+    const uint32_t strideB = (uint32_t)p.ldIn * 16u, rowB = p.Q * 16u;
+    auto load_ids = [&](uint32_t c, uint4& v) {           // the four sources of unit #j of chunk c
       const uint32_t e = c * CH + 4u * (uint32_t)j;
       if (e + 4u <= p.E) {
         v = __ldg(reinterpret_cast<const uint4*>(col + e));
@@ -927,8 +922,10 @@ sg_ring_kernel(const SgParams p, const __grid_constant__ CUtensorMap tmap, uint3
         const uint32_t nv = min(CH, p.E - c * CH);
         const uint32_t n4 = (nv + 3u) >> 2;
         mbar_wait_a(emptyB + 8u * h, (it & 1u) ^ 1u);
-        if (j == 0) mbar_expect_tx_a(fullB + 8u * h, n4 * G4B);
-        if ((uint32_t)j < n4) tma_gather4(ring + (uint32_t)h * CHUNKB + (uint32_t)j * G4B, &tmap, 0, ids.x, ids.y, ids.z, ids.w, fullB + 8u * h);
+        if (j == 0) mbar_expect_tx_a(fullB + 8u * h, n4 * 4u * rowB);
+        if ((uint32_t)j < n4)
+          bulk_rows4(ring + (uint32_t)h * CHUNKB + (uint32_t)j * G4B, inB, strideB, rowB, SLOTB, ids.x, ids.y, ids.z, ids.w,
+                     fullB + 8u * h);
       }
     }
     return;
@@ -1107,7 +1104,7 @@ sg_fixup_kernel(const SgParams p) {
 // Rows with more than SG_BIG carries (hubs: R-MAT-22's largest row spans 1 524 chunks) get a
 // whole CTA: each of the 256/L lane groups sums a contiguous block of the carries, the blocks
 // are combined in order through shared memory.  With one worker per row the hubs' serial
-// chains set the kernel's duration (0.56 ms for 250 MB of traffic, r1 run 15).
+// chains set the kernel's duration.
 constexpr uint32_t SG_BIG = 32;
 
 template <int VEC, int L, int NCH, int U>
@@ -1164,7 +1161,7 @@ sg_fixup_big_kernel(const SgParams p) {
 // Variant A keeps the gathers in registers, variant C stages them in shared memory with
 // cp.async; C wins once a row needs two or more float4 per lane at L = 32 (H > 128).
 // ROC_SG_VARIANT=a|c forces one (experiments / cross-checks).
-static int sg_variant_env() {   // -1 default, 0 = A, 2 = C, 3 = T (TMA gather4), 4 = T with per-row bulk copies, 5 = R (ring)
+static int sg_variant_env() {   // -1 default, 0 = A, 2 = C, 3 = T (bulk-copy ring), 4 = T with per-stage ids and one copy per row, 5 = R (ring)
   const char* e = getenv("ROC_SG_VARIANT");   // re-read per call: the kernel bench switches it in-process
   if (!e) return -1;
   switch (e[0]) { case 'a': return 0; case 'c': return 2; case 't': return 3; case 'b': return 4; case 'r': return 5; case 'u': return 6; default: return -1; }
@@ -1191,9 +1188,9 @@ static cudaError_t launch_c(const SgParams& p, unsigned grid, cudaStream_t st) {
   return cudaGetLastError();
 }
 
-// ---- variant T launchers: ring = P stages x S gather4s per worker, NT threads per CTA
+// ---- variant T launchers: ring = P stages x S four-row units per worker, NT threads per CTA
 template <int L, int NCH, int S, int P, int NT, int MINB, int MODE>
-static cudaError_t launch_t(const SgParams& p, const CUtensorMap& tm, cudaStream_t st) {
+static cudaError_t launch_t(const SgParams& p, cudaStream_t st) {
   constexpr int WPB = NT / L;
   constexpr size_t smem = (size_t)WPB * P * S * 4 * NCH * L * 16 + (size_t)WPB * P * 8;
   static_assert(smem <= 227 * 1024, "ring too large");
@@ -1203,13 +1200,13 @@ static cudaError_t launch_t(const SgParams& p, const CUtensorMap& tm, cudaStream
   });
   if (e != cudaSuccess) return e;
   const unsigned grid = (p.numChunks + WPB - 1) / WPB;
-  sg_chunk_kernel_t<L, NCH, S, P, NT, MINB, MODE><<<grid, NT, smem, st>>>(p, tm);
+  sg_chunk_kernel_t<L, NCH, S, P, NT, MINB, MODE><<<grid, NT, smem, st>>>(p);
   return cudaGetLastError();
 }
 
 // ---- variant R launcher: NPW producer warps + two worker warps per CTA, MINB CTAs per SM
 template <int VW, int NCH, int NPW, int MINB>
-static cudaError_t launch_r(const SgParams& p, const CUtensorMap& tm, cudaStream_t st) {
+static cudaError_t launch_r(const SgParams& p, cudaStream_t st) {
   constexpr size_t smem = (size_t)2 * SG_CH * NCH * 32 * VW * 4 + 64;
   static_assert(smem * MINB <= 227 * 1024, "ring too large");
   static std::atomic<uint64_t> configured{0};
@@ -1222,60 +1219,60 @@ static cudaError_t launch_r(const SgParams& p, const CUtensorMap& tm, cudaStream
   if (grid > numPairs) grid = numPairs;
   const uint32_t per = (numPairs + grid - 1) / grid;
   grid = (numPairs + per - 1) / per;
-  sg_ring_kernel<VW, NCH, NPW, MINB><<<grid, 32 * (NPW + 2), smem, st>>>(p, tm, per);
+  sg_ring_kernel<VW, NCH, NPW, MINB><<<grid, 32 * (NPW + 2), smem, st>>>(p, per);
   return cudaGetLastError();
 }
 // rows of up to 256 / 512 / 1024 bytes: 32 / 64 / 128 KB of ring per CTA.  cfg = producer warps (experiments)
-static cudaError_t launch_r_cfg(const SgParams& p, const CUtensorMap& tm, int cfg, cudaStream_t st) {
+static cudaError_t launch_r_cfg(const SgParams& p, int cfg, cudaStream_t st) {
   if (p.Q <= 16) {
     switch (cfg) {
-      case 1: return launch_r<2, 1, 1, 6>(p, tm, st);
-      case 4: return launch_r<2, 1, 4, 6>(p, tm, st);
-      default: return launch_r<2, 1, 2, 6>(p, tm, st);
+      case 1: return launch_r<2, 1, 1, 6>(p, st);
+      case 4: return launch_r<2, 1, 4, 6>(p, st);
+      default: return launch_r<2, 1, 2, 6>(p, st);
     }
   }
   if (p.Q <= 32) {
     switch (cfg) {
-      case 1: return launch_r<4, 1, 1, 3>(p, tm, st);
-      case 4: return launch_r<4, 1, 4, 3>(p, tm, st);
-      default: return launch_r<4, 1, 2, 3>(p, tm, st);
+      case 1: return launch_r<4, 1, 1, 3>(p, st);
+      case 4: return launch_r<4, 1, 4, 3>(p, st);
+      default: return launch_r<4, 1, 2, 3>(p, st);
     }
   }
   switch (cfg) {
-    case 1: return launch_r<4, 2, 1, 1>(p, tm, st);
-    case 4: return launch_r<4, 2, 4, 1>(p, tm, st);
-    default: return launch_r<4, 2, 2, 1>(p, tm, st);
+    case 1: return launch_r<4, 2, 1, 1>(p, st);
+    case 4: return launch_r<4, 2, 4, 1>(p, st);
+    default: return launch_r<4, 2, 2, 1>(p, st);
   }
 }
 
 // Ring shapes.  cfg < 0: the default for this width (chosen by measurement, DESIGN.md §3.1).
 template <int L, int NCH, int MODE>
-static cudaError_t launch_t_cfg(const SgParams& p, const CUtensorMap& tm, int cfg, cudaStream_t st) {
+static cudaError_t launch_t_cfg(const SgParams& p, int cfg, cudaStream_t st) {
   // bytes per row slot = NCH*L*16; per worker ring = P*S*4 slots
   if constexpr (NCH * L <= 16) {          // rows <= 256 B: 2+ workers per warp
     switch (cfg) {
-      case 1: return launch_t<L, NCH, 2, 2, 128, 4, MODE>(p, tm, st);
-      case 2: return launch_t<L, NCH, 1, 8, 128, 3, MODE>(p, tm, st);
-      case 3: return launch_t<L, NCH, 2, 4, 128, 3, MODE>(p, tm, st);
-      case 4: return launch_t<L, NCH, 1, 4, 256, 3, MODE>(p, tm, st);
-      case 5: return launch_t<L, NCH, 1, 3, 128, 8, MODE>(p, tm, st);
-      case 6: return launch_t<L, NCH, 1, 6, 128, 4, MODE>(p, tm, st);
-      default: return launch_t<L, NCH, 1, 4, 128, 6, MODE>(p, tm, st);
+      case 1: return launch_t<L, NCH, 2, 2, 128, 4, MODE>(p, st);
+      case 2: return launch_t<L, NCH, 1, 8, 128, 3, MODE>(p, st);
+      case 3: return launch_t<L, NCH, 2, 4, 128, 3, MODE>(p, st);
+      case 4: return launch_t<L, NCH, 1, 4, 256, 3, MODE>(p, st);
+      case 5: return launch_t<L, NCH, 1, 3, 128, 8, MODE>(p, st);
+      case 6: return launch_t<L, NCH, 1, 6, 128, 4, MODE>(p, st);
+      default: return launch_t<L, NCH, 1, 4, 128, 6, MODE>(p, st);
     }
   } else if constexpr (NCH == 1) {        // 512 B rows, one worker per warp
-    if (cfg < 0 && MODE == 2) cfg = 1;     // ids held by the lanes: two 8-edge stages (3.18 ms vs 5.45 with four 4-edge ones)
+    if (cfg < 0 && MODE == 2) cfg = 1;     // ids held by the lanes: two 8-edge stages
     switch (cfg) {
-      case 1: return launch_t<L, NCH, 2, 2, 128, 4, MODE>(p, tm, st);
-      case 2: return launch_t<L, NCH, 1, 8, 128, 3, MODE>(p, tm, st);
-      case 3: return launch_t<L, NCH, 1, 3, 128, 8, MODE>(p, tm, st);
-      default: return launch_t<L, NCH, 1, 4, 128, 6, MODE>(p, tm, st);
+      case 1: return launch_t<L, NCH, 2, 2, 128, 4, MODE>(p, st);
+      case 2: return launch_t<L, NCH, 1, 8, 128, 3, MODE>(p, st);
+      case 3: return launch_t<L, NCH, 1, 3, 128, 8, MODE>(p, st);
+      default: return launch_t<L, NCH, 1, 4, 128, 6, MODE>(p, st);
     }
-  } else {                                 // 1 KB rows: two 4 KB stages per warp, 6 CTAs (7.08 ms vs 8.34 with 4 stages x 3 CTAs)
+  } else {                                 // 1 KB rows: two 4 KB stages per warp, 6 CTAs
     switch (cfg) {
-      case 1: return launch_t<L, NCH, 1, 4, 128, 3, MODE>(p, tm, st);
-      case 2: return launch_t<L, NCH, 1, 6, 128, 2, MODE>(p, tm, st);
-      case 3: return launch_t<L, NCH, 1, 3, 128, 4, MODE>(p, tm, st);
-      default: return launch_t<L, NCH, 1, 2, 128, 6, MODE>(p, tm, st);
+      case 1: return launch_t<L, NCH, 1, 4, 128, 3, MODE>(p, st);
+      case 2: return launch_t<L, NCH, 1, 6, 128, 2, MODE>(p, st);
+      case 3: return launch_t<L, NCH, 1, 3, 128, 4, MODE>(p, st);
+      default: return launch_t<L, NCH, 1, 2, 128, 6, MODE>(p, st);
     }
   }
 }
@@ -1291,9 +1288,8 @@ static cudaError_t launch_c_cfg(const SgParams& p, unsigned grid, cudaStream_t s
 }
 
 struct SgLaunch {
-  int variant;               // 0 = A, 2 = C, 3 = T (gather4), 4 = T (bulk rows)
+  int variant;               // 0 = A, 2 = C, 3 = T (bulk-copy ring), 4 = T (one copy per row)
   int tcfg;                  // ring shape of variant T (-1 = default)
-  const CUtensorMap* tmap;   // variant T (gather4) only
 };
 
 template <int VEC, int L, int NCH, int U, int MINB>
@@ -1305,7 +1301,7 @@ static int launch_cfg(const SgParams& p, const SgLaunch& how, cudaStream_t st) {
     bool done = false;
     if constexpr (VEC == 4 && NCH <= 2 && L >= 16) {
       if (variant == 5) {
-        cudaError_t e = launch_r_cfg(p, *how.tmap, how.tcfg, st);
+        cudaError_t e = launch_r_cfg(p, how.tcfg, st);
         if (e != cudaSuccess) return (int)e;
         count_launch();
         done = true;
@@ -1313,7 +1309,7 @@ static int launch_cfg(const SgParams& p, const SgLaunch& how, cudaStream_t st) {
     }
     if constexpr (VEC == 4 && NCH <= 2 && L >= 16) {
       if (variant == 6) {
-        cudaError_t e = launch_t_cfg<L, NCH, 2>(p, *how.tmap, how.tcfg, st);
+        cudaError_t e = launch_t_cfg<L, NCH, 2>(p, how.tcfg, st);
         if (e != cudaSuccess) return (int)e;
         count_launch();
         done = true;
@@ -1321,8 +1317,8 @@ static int launch_cfg(const SgParams& p, const SgLaunch& how, cudaStream_t st) {
     }
     if constexpr (VEC == 4 && NCH <= 2) {
       if (variant == 3 || variant == 4) {
-        cudaError_t e = (variant == 3) ? launch_t_cfg<L, NCH, 0>(p, *how.tmap, how.tcfg, st)
-                                       : launch_t_cfg<L, NCH, 1>(p, *how.tmap, how.tcfg, st);
+        cudaError_t e = (variant == 3) ? launch_t_cfg<L, NCH, 0>(p, how.tcfg, st)
+                                       : launch_t_cfg<L, NCH, 1>(p, how.tcfg, st);
         if (e != cudaSuccess) return (int)e;
         count_launch();
         done = true;
@@ -1371,11 +1367,12 @@ static int dispatch(const SgParams& p, const SgLaunch& how, cudaStream_t st) {
 static int pick_variant(uint32_t Q, bool vec) {
   int v = sg_variant_env();
   if (!vec) return 0;
-  // measured on R-MAT-22 (r2 runs 2 / 6 / 8 and session 5, ms at H = 64 / 128 / 256): A 1.91 / 3.55 / 7.9,
-  // C 2.65 / 4.40 / 7.8, T 2.11 / 3.42 / 7.08, T with lane-held ids (U) 2.20 / 3.18 / 6.77, R 2.43 / 4.5 / 15.3
-  // -> registers up to 64 floats, the TMA gather4 ring with lane-held ids for 65..128, with per-stage ids for 129..256
-  if (v < 0) v = (Q > 64) ? 2 : (Q > 32 ? 3 : (Q > 16 ? 6 : 0));   // 129..256: U's 4 % over T not worth a less exercised path
-  if ((v == 3 || v == 4 || v == 5 || v == 6) && Q > 64) v = 2;     // TMA boxes are at most 256 elements wide
+  // measured on R-MAT-22 (H100, ms at H = 41 / 64 / 128 / 256): A 3.23 / 3.56 / 8.26 / 19.04, C 3.94 / 3.89 / 8.27 /
+  // 19.03, T 4.14 / 4.09 / 8.28 / 19.07, T with lane-held ids (U) 3.88 / 3.78 / 8.23 / 18.95, R 4.03 / 4.02 / 8.59 / 24.0
+  // -> registers up to 64 floats; beyond, every kernel but R is within 1 %: the ring with lane-held ids for 65..128,
+  // with per-stage ids for 129..256
+  if (v < 0) v = (Q > 64) ? 2 : (Q > 32 ? 3 : (Q > 16 ? 6 : 0));
+  if ((v == 3 || v == 4 || v == 5 || v == 6) && Q > 64) v = 2;     // the ring kernels take rows of at most 256 floats
   if ((v == 5 || v == 6) && Q <= 8) v = 0;                // these want rows of 9+ float4
   return v;
 }
@@ -1466,18 +1463,6 @@ extern "C" int roc_sg_plan_create(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid
     count_launch();
     PL_CUDA(cudaGetLastError());
     PL_CUDA(cudaStreamSynchronize(st));
-    if (pl->E) {
-      // rows the input matrix must have (1 + largest source id): the extent of the TMA tensor map
-      size_t tb3 = 0;
-      uint32_t maxSrc = 0;
-      cub::DeviceReduce::Max(nullptr, tb3, colSrc, dcount, (int64_t)pl->E, st);
-      if (tb3 > tb) { cudaFree(tmp); tmp = nullptr; PL_CUDA(cudaMalloc(&tmp, tb3)); }
-      PL_CUDA(cub::DeviceReduce::Max(tmp, tb3, colSrc, dcount, (int64_t)pl->E, st));
-      count_launch(2);
-      PL_CUDA(cudaMemcpyAsync(&maxSrc, dcount, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-      PL_CUDA(cudaStreamSynchronize(st));
-      pl->inRows = (uint64_t)maxSrc + 1;
-    }
   }
 done:
 #undef PL_CUDA
@@ -1514,7 +1499,7 @@ extern "C" int roc_sg_forward_planned(const roc_sg_plan* plc, int H, const float
   cudaStream_t st = as_stream(stream);
   const bool vec = (ldIn % 4 == 0) && (ldOut % 4 == 0) && aligned16(in) && aligned16(out);
   // column blocks: the widest kernel covers 256 T-columns (1024 floats vectorised, 256 scalar);
-  // the TMA variants take 64 T-columns (a tensor-map box is at most 256 elements wide)
+  // the ring variants take 64 T-columns (they are instantiated for rows of at most 256 floats)
   int variant = pick_variant(vec ? ((uint32_t)H + 3) / 4 : (uint32_t)H, vec);
   if ((variant == 3 || variant == 4 || variant == 5 || variant == 6) && H > 256 && sg_variant_env() < 0) variant = 2;
   const int blockCols = !vec ? 256 : ((variant == 3 || variant == 4 || variant == 5 || variant == 6) ? 256 : 1024);
@@ -1532,28 +1517,12 @@ extern "C" int roc_sg_forward_planned(const roc_sg_plan* plc, int H, const float
     p.dense = (pl->nloc > 0 && pl->E / pl->nloc >= (uint32_t)SG_CH) ? 1 : 0;
     p.desc = pl->desc; p.nloc = pl->nloc;
     SgLaunch how;
-    how.variant = variant; how.tcfg = sg_tcfg_env(); how.tmap = nullptr;
-    CUtensorMap tm;
-    memset(&tm, 0, sizeof(tm));     // only the gather4 kernels read it
-    how.tmap = &tm;
+    how.variant = variant; how.tcfg = sg_tcfg_env();
     int rc;
     if (vec) {
       p.ldIn = (size_t)ldIn / 4; p.ldOut = (size_t)ldOut / 4; p.ldC = pl->carryLd / 4;
       p.Q = ((uint32_t)hb + 3) / 4;
       if (variant == 5 && (!aligned16(pl->col) || p.Q <= 8)) how.variant = 0;   // producer reads col as uint4
-      if (variant == 3 || variant == 6 || how.variant == 5) {
-        // tensor map of the input: [inRows][Q*4] floats, rows ldIn floats apart; the box is the worker's
-        // whole lane span (columns past Q*4 are zero-filled), one row per box — gather4 fetches four
-        const uint32_t span = p.Q <= 4 ? 4u : p.Q <= 8 ? 8u : p.Q <= 16 ? 16u : p.Q <= 32 ? 32u : 64u;
-        const uint64_t rowBytes = (uint64_t)p.Q * 16u;
-        const CUtensorMapL2promotion promo = rowBytes >= 256 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B
-                                            : rowBytes >= 128 ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B
-                                                              : CU_TENSOR_MAP_L2_PROMOTION_L2_64B;
-        if (!tc::make_tmap_32b_2d(&tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, in + c0, pl->inRows, (uint64_t)p.Q * 4u,
-                                  (uint64_t)ldIn, 1u, span * 4u, CU_TENSOR_MAP_SWIZZLE_NONE, promo))
-          return ROC_ERR_UNSUPPORTED;
-        how.tmap = &tm;
-      }
       rc = dispatch<4>(p, how, st);
     } else {
       p.ldIn = (size_t)ldIn; p.ldOut = (size_t)ldOut; p.ldC = pl->carryLd;

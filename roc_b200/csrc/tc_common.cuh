@@ -1,7 +1,6 @@
-// tc_common.cuh — sm_100a building blocks written as inline PTX: mbarrier, TMA
-// (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld) and the UMMA
-// shared-memory + instruction descriptors.  Formats follow the PTX ISA as mirrored
-// in CUTLASS' cute/arch/mma_sm100_desc.hpp (InstrDescriptor, SmemDescriptor).
+// tc_common.cuh — sm_90a building blocks written as inline PTX: mbarrier, TMA
+// (cp.async.bulk.tensor), warpgroup MMA (wgmma) and its shared-memory descriptor.
+// Formats follow the PTX ISA (wgmma matrix descriptor, register fragment layouts).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -14,10 +13,8 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
-// One lane of a converged warp (elect.sync).  The MMA / TMA issuing loops run warp-converged and
-// branch on this only around the issue itself: under `if (lane == 0) { loop }` ptxas cannot prove
-// the tcgen05 operands warp-uniform and wraps every UTCHMMA in an ELECT / BRA.U.ANY serialisation
-// loop (~60 cycles per MMA, r1 run 21: the issuing thread, not the tensor pipe, paced the GEMM).
+// One lane of a converged warp (elect.sync).  The TMA issuing loops run warp-converged and branch on
+// this only around the issue itself, so ptxas knows the operands are warp-uniform.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred = 0;
   asm volatile(
@@ -55,7 +52,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         : "memory");
   } while (!ok);
 }
-// make generic-proxy smem writes visible to the async proxy (TMA / tcgen05 reads)
+// make generic-proxy smem writes visible to the async proxy (TMA / wgmma reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -72,91 +69,65 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
-// ------------------------------------------------------------------ tcgen05 ---
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// -------------------------------------------------------------------- wgmma ---
+// Warpgroup MMA (sm_90a): the 128 threads of a warpgroup issue together; the accumulator lives in
+// their registers (m64nNk8 f32: warp w of the group holds rows 16w..16w+15, thread lane l holds rows
+// 16w + l/4 and 16w + l/4 + 8, columns 8j + 2(l%4) and +1 for each n8 block j).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// An MMA reads its register A fragment asynchronously, after the instruction has issued.  A fake use of the
+// fragments placed after the wgmma_wait_all that retires their MMAs keeps the compiler from handing those
+// registers to other values (the next k-step's fragments, say) while the MMAs may still read them.
+template <int A, int B, int C>
+__device__ __forceinline__ void keep_live(const uint32_t (&r)[A][B][C]) {
+#pragma unroll
+  for (int i = 0; i < A; i++)
+#pragma unroll
+    for (int j = 0; j < B; j++)
+#pragma unroll
+      for (int k = 0; k < C; k++) asm volatile("" ::"r"(r[i][j][k]) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
+// keeps the compiler from moving accumulator accesses across the asynchronous MMAs
+__device__ __forceinline__ void wgmma_fence_acc(float (&d)[16]) {
+#pragma unroll
+  for (int i = 0; i < 16; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem] * B[smem], kind::tf32 (fp32 containers, fp32 accumulate)
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
+// D[64 x 32] += A[64 x 8] * B[32 x 8]^T, kind tf32 with fp32 accumulate.  A comes from registers
+// (thread lane l of warp w: a0 = (16w + l/4, l%4), a1 = row + 8, a2 = col + 4, a3 = both), B from
+// shared memory through a descriptor (K-major, 128-byte swizzle).
+__device__ __forceinline__ void wgmma_m64n32k8_tf32(float (&d)[16], const uint32_t (&a)[4], uint64_t bdesc) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc)
       : "memory");
 }
-// D[tmem] (+)= A[tmem] * B[smem]: A is K-major in TMEM (lane = row, one 32-bit column per k)
-__device__ __forceinline__ void umma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier once every previously issued tcgen05.mma has completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 16 consecutive 32-bit columns: thread t of the warp gets row (lane base + t)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-// registers -> TMEM: thread t of the warp writes 16 consecutive 32-bit columns of lane (base + t)
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // -------------------------------------------------------------- descriptors ---
-// Instruction descriptor, kind::tf32, fp32 accumulate (InstrDescriptor bit layout):
-//  [4,6) c_format = 1 (F32)  [7,10) a_format = 2 (TF32)  [10,13) b_format = 2
-//  [15] a_major  [16] b_major (0 = K-major, 1 = MN-major)  [17,23) N>>3  [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// Shared-memory matrix descriptor (SmemDescriptor): start>>4 [0,14), LBO>>4 [16,30),
-// SBO>>4 [32,46), version = 1 at [46,48), layout type [61,64) (2 = SWIZZLE_128B).
-// layout_type: 2 = SWIZZLE_128B (16-byte chunks; K-major operands), 1 = SWIZZLE_128B_BASE32B
-// (32-byte chunks, 4-row atoms) — the only swizzled layout tcgen05 accepts for MN-major
-// 32-bit (tf32) operands (CUTLASS sm100_common.inl: "for mn-major tf32 operands, SW128_32B is
-// the only available smem layout"); plain SWIZZLE_128B there silently yields zeros (r1 run 6).
-__device__ __forceinline__ uint64_t make_sdesc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                               uint32_t layout_type) {
+// wgmma shared-memory matrix descriptor: start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46),
+// base offset [49,52) (0: every tile here starts 1024-byte aligned), layout [62,64) (1 = SWIZZLE_128B).
+// A K-major tf32 operand written by TMA with CU_TENSOR_MAP_SWIZZLE_128B: rows of 32 floats (128 bytes),
+// 8-row atoms of 1024 bytes (SBO); LBO is unused for swizzled K-major layouts.  The k8 step inside the
+// 128-byte row advances the start address by 32 bytes (the hardware applies the swizzle to the
+// absolute address).
+__device__ __forceinline__ uint64_t make_sdesc_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= 1ull << 46;
-  d |= (uint64_t)layout_type << 61;
+  d |= (uint64_t)1u << 16;
+  d |= (uint64_t)(1024u >> 4) << 32;
+  d |= 1ull << 62;
   return d;
 }
-__device__ __forceinline__ uint64_t make_sdesc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  return make_sdesc(smem_addr, lbo_bytes, sbo_bytes, 2u);
+
+// split of an fp32 value into a TF32 head (10-bit mantissa, truncated) and the exact remainder
+__device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
+  hi = __float_as_uint(x) & 0xFFFFE000u;
+  lo = __float_as_uint(x - __uint_as_float(hi));
 }
 
 // ------------------------------------------------------ host: tensor maps -----

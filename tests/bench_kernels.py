@@ -64,7 +64,7 @@ def main():
     plan = K.SgPlan(0, n - 1, 0, re, col)
     info = plan.info()
     print(json.dumps({"graph": a.graph, "N": n, "E": e, "max_deg": int(deg.max()), "plan": info}), flush=True)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)     # 256 MB > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)     # 256 MB > 50 MB L2
     use_ref = ref.available() and not a.no_ref
     if use_ref:
         rp, es = ref.edge_structs(col, re, 0, 0)

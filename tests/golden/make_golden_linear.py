@@ -1,11 +1,12 @@
-"""make_golden_linear.py — Linear golden vectors at the headline shapes, minted on a GPU box from the REFERENCE's
+"""make_golden_linear.py — Linear golden vectors at the headline shapes, minted on the GPU from the REFERENCE's
 own cublasSgemm calls (oracle/_ref: linear_kernel.cu:76-80 forward, :220-231 backward, the reference's arguments).
 
     python tests/golden/make_golden_linear.py [out.npz]        # needs a GPU and oracle/_ref/libroc_ref.so
 
 1000 x 602 . 64 x 602 and 1000 x 64 . 41 x 64: the shapes of BASELINE.json configs[1].  The GPU tests feed them
-row-padded (ld % 4 == 0), so the tcgen05 kernels — not the SIMT fallback the small unpadded golden case reaches —
-are what meets the reference library's outputs.  Inputs are regenerated from the seed by the test."""
+row-padded (ld % 4 == 0), so the tensor-core kernels — not the SIMT fallback the small unpadded golden case reaches —
+are what meets the reference library's outputs.  Inputs are regenerated from the seed by the test; Y and dX are
+stored for a fixed sample of 128 rows (rows_<shape>), dW whole, which keeps the file under 1 MB."""
 import os
 import sys
 
@@ -37,7 +38,9 @@ def main():
         ref.linear_bwd(x, w, y, gy.clone(), gw, gx, relu=False)
         torch.cuda.synchronize()
         k = "%dx%dx%d" % (n, i, o)
-        G["Y_" + k], G["dW_" + k], G["dX_" + k] = y.cpu().numpy(), gw.cpu().numpy(), gx.cpu().numpy()
+        rows = np.sort(np.random.RandomState(11).choice(n, 128, replace=False))
+        G["rows_" + k] = rows
+        G["Y_" + k], G["dW_" + k], G["dX_" + k] = y.cpu().numpy()[rows], gw.cpu().numpy(), gx.cpu().numpy()[rows]
     np.savez_compressed(out, **G)
     print("wrote", out, {k: v.shape for k, v in G.items()})
 

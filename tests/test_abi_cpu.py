@@ -54,10 +54,10 @@ def test_struct_layouts_match_the_header(tmp_path):
     assert out[-1] == C.sizeof(_lib.PerfMetrics)
 
 
-def test_library_is_sm100a_only():
+def test_library_is_sm90a_only():
     out = subprocess.run(["cuobjdump", "--list-elf", _lib.LIB_PATH], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_\d+a?", out))
-    assert archs == {"sm_100a"}, archs
+    assert archs == {"sm_90a"}, archs
 
 
 def test_partition_matches_oracle_bit_for_bit():

@@ -4,6 +4,7 @@ oracle/_ref is present) against the reference kernels run side by side.
 Bit-exact for indices / masks / partition bounds; 1e-4 relative for fp32 tensors."""
 import ctypes as C
 import os
+import sys
 
 import numpy as np
 import pytest
@@ -66,7 +67,7 @@ def test_sg_planned_vs_oracle(kind, h):
 @pytest.mark.parametrize("kind", ["uniform", "rmat", "dense", "ragged", "single"])
 @pytest.mark.parametrize("h", [4, 16, 41, 64, 100, 128, 200, 256, 602])
 def test_sg_variants_are_bitwise_identical(kind, h, monkeypatch):
-    """The register (A), cp.async (C), TMA gather4 / bulk-copy (T) and producer/consumer ring (R) kernels share
+    """The register (A), cp.async (C), TMA bulk-copy (T) and producer/consumer ring (R) kernels share
     the chunk plan and the per-row summation order, so they must agree bit for bit — with every ring shape of
     variant T, every CTA-range split of variant R and with the fused epilogue — and the TMA paths must meet
     the oracle exactly like the others."""
@@ -463,9 +464,10 @@ def test_kernels_vs_reference_golden(golden):
     plan = K.SgPlan(0, n - 1, 0, d_re, d_col)
     for h in (16, 41, 64):
         x = torch.from_numpy(g["A_sg_in_%d" % h]).to(DEV)
-        rel_close(plan.forward(x, out=torch.empty((n, h), device=DEV)).cpu().numpy(), g["A_sg_out_%d" % h],
+        rows = g["A_rows_%d" % h]
+        rel_close(plan.forward(x, out=torch.empty((n, h), device=DEV)).cpu().numpy()[rows], g["A_sg_out_%d" % h],
                   what="vs aggre_coop_kernel H=%d" % h)
-        assert np.array_equal(K.indegree_norm(0, n - 1, 0, d_re, x).cpu().numpy(), g["A_norm_out_%d" % h])
+        assert np.array_equal(K.indegree_norm(0, n - 1, 0, d_re, x).cpu().numpy()[rows], g["A_norm_out_%d" % h])
     rp, es, _ = K.build_csr(0, n - 1, 0, d_re, d_col)
     assert np.array_equal(es.cpu().numpy().astype(np.uint32), g["A_edgestructs"])
     x, w, dy = (torch.from_numpy(g[k]).to(DEV) for k in ("lin_X", "lin_W", "lin_dY"))
@@ -487,23 +489,32 @@ def test_kernels_vs_reference_golden(golden):
     rel_close(dw.cpu().numpy(), g["adam_w_out"], rtol=1e-6, what="vs adam_update")
 
 
-@pytest.mark.skipif(not ref.available(), reason="oracle/_ref/libroc_ref.so not built (no /root/reference here)")
+SG_GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_golden_sg.npz")
+
+
 def test_side_by_side_with_reference_kernel():
-    re_t, col_t = datasets.rmat_graph(14, 150000, seed=8)
-    row_end, col = re_t.numpy().astype(np.uint64), col_t.numpy().astype(np.uint32)
+    """R-MAT scale 14 at the widths the variants split on, against the reference's aggre_coop_kernel: the stored
+    rows of tests/golden/make_golden_sg.py always, and the whole output live when oracle/_ref is built."""
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
+    from make_golden_sg import graph, features
+    row_end, col = graph()
     n = row_end.shape[0]
     d_re, d_col = to_dev(row_end, col)
-    rp, es = ref.edge_structs(d_col, d_re, 0, 0)
     plan = K.SgPlan(0, n - 1, 0, d_re, d_col)
+    g = np.load(SG_GOLDEN)
+    if ref.available():
+        rp, es = ref.edge_structs(d_col, d_re, 0, 0)
     for h in (16, 64, 128, 256):
-        x = torch.rand((n, h), device=DEV) - 0.5
-        want = ref.scatter_gather(0, n - 1, 0, rp, es, x)
-        got = plan.forward(x)
-        torch.cuda.synchronize()
-        rel_close(got.cpu().numpy(), want.cpu().numpy(), what="vs live aggre_coop_kernel H=%d" % h)
+        x = torch.from_numpy(features(n, h)).to(DEV)
+        got = plan.forward(x).cpu().numpy()
+        rel_close(got[g["rows"]], g["out_%d" % h], what="vs stored aggre_coop_kernel rows H=%d" % h)
+        if ref.available():
+            want = ref.scatter_gather(0, n - 1, 0, rp, es, x)
+            torch.cuda.synchronize()
+            rel_close(got, want.cpu().numpy(), what="vs live aggre_coop_kernel H=%d" % h)
 
 
-# ---------------------------------------- tcgen05 Linear vs the reference library at the headline shapes ---
+# ---------------------------------- tensor-core Linear vs the reference library at the headline shapes ---
 LIN_GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_golden_linear.npz")
 
 
@@ -514,39 +525,37 @@ def _lin_inputs(n, i, o):
 
 
 @pytest.mark.parametrize("n,i,o", [(1000, 602, 64), (1000, 64, 41)])
-def test_tcgen05_linear_meets_the_reference_cublas(n, i, o):
-    """BASELINE.json configs[1]'s two Linear shapes, fed row-padded so the tcgen05 / TMEM kernels run (asserted
-    through roc_last_gemm_path) — against outputs of the REFERENCE's cublasSgemm calls (linear_kernel.cu:76-80,
-    220-231) minted on a B200 by tests/golden/make_golden_linear.py, and live against oracle/_ref when it is there."""
+def test_tensor_core_linear_meets_the_reference_cublas(n, i, o):
+    """BASELINE.json configs[1]'s two Linear shapes, fed row-padded so the wgmma kernels run (asserted through
+    roc_last_gemm_path) — against outputs of the REFERENCE's cublasSgemm calls (linear_kernel.cu:76-80, 220-231)
+    minted on the GPU by tests/golden/make_golden_linear.py (Y and dX on a stored sample of rows), and live against
+    oracle/_ref when it is there."""
     X, W, dY = _lin_inputs(n, i, o)
     xp = K.padded(n, i, DEV, fill=torch.from_numpy(X).to(DEV))
     w = torch.from_numpy(W).to(DEV)
     gyp = K.padded(n, o, DEV, fill=torch.from_numpy(dY).to(DEV))
     y = K.linear_fwd(xp, w)
-    assert _lib.lib.roc_last_gemm_path(0) == 1, "forward did not take the tcgen05 path"
+    assert _lib.lib.roc_last_gemm_path(0) == 1, "forward did not take the tensor-core path"
     dw = torch.zeros_like(w)
     dx = K.padded(n, i, DEV)
     K.linear_bwd(xp, w, None, gyp, dw, dx, activation=0)
-    assert _lib.lib.roc_last_gemm_path(1) == 1 and _lib.lib.roc_last_gemm_path(2) == 1, "dW / dX not on tcgen05"
+    assert _lib.lib.roc_last_gemm_path(1) == 1 and _lib.lib.roc_last_gemm_path(2) == 1, "dW / dX not on tensor cores"
     torch.cuda.synchronize()
     k = "%dx%dx%d" % (n, i, o)
-    wants = []
-    if os.path.exists(LIN_GOLDEN):
-        g = np.load(LIN_GOLDEN)
-        wants.append(("golden", g["Y_" + k], g["dW_" + k], g["dX_" + k]))
+    g = np.load(LIN_GOLDEN)
+    rows = g["rows_" + k]
+    wants = [("golden", rows, g["Y_" + k], g["dW_" + k], g["dX_" + k])]
     if ref.available():
         xd, gyd = torch.from_numpy(X).to(DEV), torch.from_numpy(dY).to(DEV)
         ry = ref.linear_fwd(xd, w, relu=False)
         rw, rx = torch.zeros_like(w), torch.zeros_like(xd)
         ref.linear_bwd(xd, w, ry, gyd.clone(), rw, rx, relu=False)
         torch.cuda.synchronize()
-        wants.append(("live reference", ry.cpu().numpy(), rw.cpu().numpy(), rx.cpu().numpy()))
-    if not wants:
-        pytest.skip("neither tests/golden/ref_golden_linear.npz nor oracle/_ref is present")
-    for name, wy, wdw, wdx in wants:
-        rel_close(y.cpu().numpy(), wy, what="Y vs %s" % name)
+        wants.append(("live reference", slice(None), ry.cpu().numpy(), rw.cpu().numpy(), rx.cpu().numpy()))
+    for name, r, wy, wdw, wdx in wants:
+        rel_close(y.cpu().numpy()[r], wy, what="Y vs %s" % name)
         rel_close(dw.cpu().numpy(), wdw, what="dW vs %s" % name)
-        rel_close(dx.cpu().numpy(), wdx, what="dX vs %s" % name)
+        rel_close(dx.cpu().numpy()[r], wdx, what="dX vs %s" % name)
 
 
 def test_unpadded_linear_reports_the_simt_fallback():

@@ -1,12 +1,12 @@
 #!/bin/bash
 # compute-sanitizer over the tiny configuration (SURVEY §5): memcheck, then racecheck, on
-#   (a) __graft_entry__.smoke()  — one GCN training step through the Model API (SG, tcgen05 GEMMs, softmax, Adam)
-#   (b) every ScatterGather variant (registers / cp.async / TMA gather4 / bulk / producer-consumer ring) on the
+#   (a) __graft_entry__.smoke()  — one GCN training step through the Model API (SG, wgmma GEMMs, softmax, Adam)
+#   (b) every ScatterGather variant (registers / cp.async / TMA bulk-copy rings / producer-consumer ring) on the
 #       ragged test graph.
 # Usage: tools/sanitize.sh [logdir]   (needs a GPU; `make sanitize`)
 set -u
 ROOT="$(cd "$(dirname "$0")/.." && pwd)"
-LOG="${1:-$ROOT/gpurun_out/sanitize}"
+LOG="${1:-$ROOT/sanitize_logs}"
 mkdir -p "$LOG"
 cd "$ROOT"
 cat > "$LOG/sg_variants.py" <<'PY'

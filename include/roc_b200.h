@@ -66,6 +66,10 @@ typedef void*    roc_stream_t; /* cudaStream_t */
 #define ROC_SG_EPI_NORM 1
 #define ROC_SG_EPI_RELU 2
 
+/* aggregation of roc_sg_minmax_forward_planned (the values of AGGR_MAX / AGGR_MIN, gnn.h:75-80) */
+#define ROC_SG_AGGR_MAX 1
+#define ROC_SG_AGGR_MIN 2
+
 /* PerfMetrics, softmax_kernel.cu:35-39 (same field order) */
 typedef struct {
   float trainLoss;
@@ -125,6 +129,9 @@ void roc_sg_plan_destroy(roc_sg_plan* plan);
 /* Introspection for tests / DESIGN.md numbers. */
 int roc_sg_plan_info(const roc_sg_plan* plan, uint64_t* numChunks,
                      uint64_t* numCarries, uint64_t* numHeavyRows);
+/* *sorted = 1 if every row's sources are strictly increasing (so no row has a duplicate edge), else 0.  One device
+ * pass; synchronises the stream. */
+int roc_sg_plan_rows_sorted(const roc_sg_plan* plan, int* sorted, roc_stream_t stream);
 
 /* Replaces aggre_coop_kernel + ScatterGather::forward_task,
  * scattergather_kernel.cu:20-76, 78-158:
@@ -137,6 +144,26 @@ int roc_sg_plan_info(const roc_sg_plan* plan, uint64_t* numChunks,
 int roc_sg_forward_planned(const roc_sg_plan* plan, int H, const float* in,
                            int64_t ldIn, float* out, int64_t ldOut, int epilogue,
                            roc_stream_t stream);
+
+/* Max / min aggregation (GraphSAGE-pool).  The reference declares AGGR_MAX / AGGR_MIN but never implements them;
+ * these semantics are this library's own.  For a row v with in-edges e in CSR order:
+ *   out[v-rowLeft][h] = max (aggr = ROC_SG_AGGR_MAX) or min (ROC_SG_AGGR_MIN) of in[colSrc[e]][h]
+ *   arg[v-rowLeft][h] = colSrc[e] of the FIRST edge in CSR order that holds that value
+ * A row starts with its first edge's value and id; a later value replaces them only if it is strictly greater
+ * (smaller) or it is NaN and the current value is not, so NaN propagates as in torch.amax.  A row of degree 0 gets
+ * out = 0 and arg = 0xFFFFFFFF.  Exact (no rounding) and independent of how the plan cuts rows into chunks.
+ * `in` is indexed like roc_sg_forward_planned's.  Kernel A (registers) only: ROC_SG_VARIANT does not apply.
+ * ROC_ERR_INVALID for an aggr other than MAX / MIN, a NULL pointer or a leading dimension < H. */
+int roc_sg_minmax_forward_planned(const roc_sg_plan* plan, int aggr, int H, const float* in, int64_t ldIn,
+                                  float* out, int64_t ldOut, roc_vid_t* arg, int64_t ldArg, roc_stream_t stream);
+/* Its backward, as a gather over the same CSR (like the sum's, quirk Q1), in the plan's fixed order, no atomics:
+ *   inGrad[u][h] = sum_{e in row u, v = colSrc[e]} (arg[v][h] == selfBase + u ? outGrad[v][h] : 0)
+ * outGrad and arg are indexed by colSrc's ids; selfBase + u is local row u's id in that space (0 for a whole graph,
+ * rowLeft for a slice with global ids).  This is the true adjoint only when the graph is symmetric and has no
+ * duplicate edges. */
+int roc_sg_minmax_backward_planned(const roc_sg_plan* plan, int H, roc_vid_t selfBase,
+                                   const float* outGrad, int64_t ldG, const roc_vid_t* arg, int64_t ldArg,
+                                   float* inGrad, int64_t ldIn, roc_stream_t stream);
 
 /* Plan-less form with exactly the reference kernel's argument list
  * (scattergather_kernel.cu:21-28, EdgeStruct.dst dropped), dense ld == H.

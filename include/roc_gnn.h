@@ -182,6 +182,13 @@ public:
   Tensor add(const Tensor& _input1, const Tensor& _input2);
   Tensor dropout(const Tensor& _input, float rate, int seed = 0);
   Tensor scatter_gather(const Tensor& _input);
+  /* With an aggregator (not in gnn.h, which declares AggrType but only sums).  AGGR_SUM is the one-argument form.
+   * AGGR_AVG appends scatter_gather -> indegree_norm -> indegree_norm (x / sqrt(deg) / sqrt(deg): the mean to within
+   * one fp32 rounding, the wiring of GraphSAGE-mean).  AGGR_MAX / AGGR_MIN: per feature, the max / min over the
+   * in-neighbours (roc_sg_minmax_forward_planned); the backward sends each output gradient to the first source that
+   * held the extreme.  That is the true gradient only on a symmetric graph without duplicate edges: init() refuses
+   * a graph whose rows do not have strictly increasing sources.  Single partition only (exit(1) otherwise). */
+  Tensor scatter_gather(const Tensor& _input, AggrType aggr);
   void softmax_cross_entropy(const Tensor& logits, const Tensor& labels, const Tensor& mask);
   Tensor indegree_norm(const Tensor& _input);
   Tensor linear(const Tensor& _input, int outDim, ActiMode activation, Initializer* initializer = NULL);
@@ -208,6 +215,8 @@ public:
   void set_labels(const Tensor& label, const int* host_class_idx);
   roc_perf_metrics last_metrics(void) const;   /* PerfMetrics of the latest softmax pass */
   void set_fusion(bool on) { fuse = on; }
+  /* the source ids a max / min scatter_gather chose (its `arg`), [rows_local][H] u32; `out` is its output tensor */
+  void get_aggr_index(const Tensor& out, uint32_t* host) const;
   int64_t local_rows(void) const { return (int64_t)myGraph.rowRight - myGraph.rowLeft + 1; }
 
 public:
@@ -244,10 +253,13 @@ public:
 
 class ScatterGather : public GnnOp {  /* gnn.h:225-242, scattergather.cc */
 public:
-  ScatterGather(const Model& model, const Tensor& input);
+  ScatterGather(const Model& model, const Tensor& input, AggrType aggr = AGGR_SUM);
   virtual void init(const Model& model);
   virtual void forward(const Model& model);
   virtual void backward(const Model& model);
+  AggrType aggr;     /* AGGR_SUM, or AGGR_MAX / AGGR_MIN (never fused with neighbouring ops) */
+  uint32_t* arg;     /* max / min: [Nloc][argLd] source id behind each output value (first forward; Runtime arena) */
+  int64_t argLd;
   int epilogue;      /* ROC_SG_EPI_* the forward store applies (set by Model::init fusion) */
   int bwdEpilogue;   /* same for the backward launch */
   int fwdOut, bwdOut;/* region the fused forward / backward writes (-1: own output / input grad) */

@@ -40,6 +40,8 @@ int roc_host_dropout(roc_host* h, int t, float rate, int seed);
 int roc_host_linear(roc_host* h, int t, int outDim, int activation);
 int roc_host_indegree_norm(roc_host* h, int t);
 int roc_host_scatter_gather(roc_host* h, int t);
+/* Model::scatter_gather(t, aggr); aggr = AggrType (0 AVG, 1 MAX, 2 MIN, 3 SUM) */
+int roc_host_scatter_gather_aggr(roc_host* h, int t, int aggr);
 int roc_host_relu(roc_host* h, int t);
 int roc_host_sigmoid(roc_host* h, int t);
 int roc_host_add(roc_host* h, int a, int b);
@@ -59,6 +61,8 @@ int roc_host_load_train_mask(roc_host* h, int t, const char* prefix);
 int roc_host_set_tensor(roc_host* h, int t, const void* host, int grad);
 int roc_host_get_tensor(roc_host* h, int t, void* host, int grad);
 int roc_host_set_labels(roc_host* h, int t, const int32_t* host_class_idx);
+/* the source ids a max / min scatter_gather output t was taken from, [rows][hidden] u32 (Model::get_aggr_index) */
+int roc_host_get_aggr_index(roc_host* h, int t, uint32_t* host);
 int roc_host_tensor_shape(roc_host* h, int t, int64_t out[3]);   /* rows, hidden, ld */
 void* roc_host_tensor_ptr(roc_host* h, int t, int grad);          /* device pointer */
 int roc_host_num_parameters(roc_host* h);

@@ -15,6 +15,8 @@ ROC_ERR_INVALID, ROC_ERR_UNSUPPORTED, ROC_ERR_NOMEM, ROC_ERR_NO_DEVICE, ROC_ERR_
 AC_MODE_NONE, AC_MODE_RELU, AC_MODE_SIGMOID = 0, 1, 2
 MASK_TRAIN, MASK_VAL, MASK_TEST, MASK_NONE = 0, 1, 2, 3
 SG_EPI_NONE, SG_EPI_NORM, SG_EPI_RELU = 0, 1, 2
+AGGR_AVG, AGGR_MAX, AGGR_MIN, AGGR_SUM = 0, 1, 2, 3        # AggrType (gnn.h:75-80); ROC_SG_AGGR_MAX / _MIN = 1 / 2
+SG_NOARG = 0xFFFFFFFF                                      # arg of a row with no in-edge
 LINEAR_NORM_EPILOGUE = 1
 
 
@@ -70,7 +72,10 @@ PROTOTYPES = {
     "roc_sg_plan_reserve": (i32, [vp, i32]),
     "roc_sg_plan_destroy": (None, [vp]),
     "roc_sg_plan_info": (i32, [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]),
+    "roc_sg_plan_rows_sorted": (i32, [vp, C.POINTER(i32), vp]),
     "roc_sg_forward_planned": (i32, [vp, i32, vp, i64, vp, i64, i32, vp]),
+    "roc_sg_minmax_forward_planned": (i32, [vp, i32, i32, vp, i64, vp, i64, vp, i64, vp]),
+    "roc_sg_minmax_backward_planned": (i32, [vp, i32, u32, vp, i64, vp, i64, vp, i64, vp]),
     "roc_sg_forward": (i32, [u32, u32, u64, i32, vp, vp, vp, vp, vp]),
     "roc_sg_backward": (i32, [u32, u32, u64, i32, vp, vp, vp, vp, vp]),
     "roc_halo_create": (i32, [u32, u32, u64, vp, vp, C.POINTER(vp)]),
@@ -123,6 +128,8 @@ PROTOTYPES = {
     "roc_host_linear": (i32, [vp, i32, i32, i32]),
     "roc_host_indegree_norm": (i32, [vp, i32]),
     "roc_host_scatter_gather": (i32, [vp, i32]),
+    "roc_host_scatter_gather_aggr": (i32, [vp, i32, i32]),
+    "roc_host_get_aggr_index": (i32, [vp, i32, vp]),
     "roc_host_relu": (i32, [vp, i32]),
     "roc_host_sigmoid": (i32, [vp, i32]),
     "roc_host_add": (i32, [vp, i32, i32]),

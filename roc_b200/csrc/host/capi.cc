@@ -87,6 +87,11 @@ int roc_host_linear(roc_host* h, int t, int outDim, int activation) {
 }
 int roc_host_indegree_norm(roc_host* h, int t) { return h->push(h->m().indegree_norm(h->at(t))); }
 int roc_host_scatter_gather(roc_host* h, int t) { return h->push(h->m().scatter_gather(h->at(t))); }
+int roc_host_scatter_gather_aggr(roc_host* h, int t, int aggr) {
+  if (aggr < AGGR_AVG || aggr > AGGR_SUM) ROC_FATAL("roc_host_scatter_gather_aggr: bad AggrType");
+  return h->push(h->m().scatter_gather(h->at(t), (AggrType)aggr));
+}
+int roc_host_get_aggr_index(roc_host* h, int t, uint32_t* host) { h->m().get_aggr_index(h->at(t), host); return 0; }
 int roc_host_relu(roc_host* h, int t) { return h->push(h->m().relu(h->at(t))); }
 int roc_host_sigmoid(roc_host* h, int t) { return h->push(h->m().sigmoid(h->at(t))); }
 int roc_host_add(roc_host* h, int a, int b) { return h->push(h->m().add(h->at(a), h->at(b))); }

@@ -93,6 +93,36 @@ Tensor Model::scatter_gather(const Tensor& _input) {
   layers.push_back(op);
   return op->outputs[0];
 }
+Tensor Model::scatter_gather(const Tensor& _input, AggrType aggr) {
+  switch (aggr) {
+    case AGGR_SUM: return scatter_gather(_input);
+    case AGGR_AVG: return indegree_norm(indegree_norm(scatter_gather(_input)));   // the fusions of init() apply
+    case AGGR_MAX:
+    case AGGR_MIN: {
+      if (ctx->numParts > 1)
+        ROC_FATAL("scatter_gather: max / min aggregation runs on one partition only (numParts > 1 is not supported)");
+      GnnOp* op = new ScatterGather(*this, _input, aggr);
+      layers.push_back(op);
+      return op->outputs[0];
+    }
+  }
+  ROC_FATAL("scatter_gather: unknown AggrType");
+  return Tensor();
+}
+void Model::get_aggr_index(const Tensor& out, uint32_t* host) const {
+  for (GnnOp* op : layers) {
+    ScatterGather* sg = dynamic_cast<ScatterGather*>(op);
+    if (!sg || sg->outputs[0].region != out.region) continue;
+    if (sg->aggr != AGGR_MAX && sg->aggr != AGGR_MIN) ROC_FATAL("get_aggr_index: not a max / min scatter_gather");
+    if (!sg->arg) ROC_FATAL("get_aggr_index: run forward() first");
+    const int64_t H = (int64_t)sg->outputs[0].dims[0];
+    ROC_CHECK(cudaMemcpy2DAsync(host, (size_t)H * sizeof(uint32_t), sg->arg, (size_t)sg->argLd * sizeof(uint32_t),
+                                (size_t)H * sizeof(uint32_t), (size_t)local_rows(), cudaMemcpyDeviceToHost, ctx->stream));
+    ROC_CHECK(cudaStreamSynchronize(ctx->stream));
+    return;
+  }
+  ROC_FATAL("get_aggr_index: no scatter_gather produces this tensor");
+}
 void Model::softmax_cross_entropy(const Tensor& logits, const Tensor& labels, const Tensor& mask) {
   layers.push_back(new SoftmaxCrossEntropy(*this, logits, labels, mask));
 }
@@ -142,6 +172,11 @@ Wiring wire(const std::vector<GnnOp*>& layers) {
 }
 template <typename T>
 T* as(GnnOp* op) { return dynamic_cast<T*>(op); }
+// a ScatterGather that sums: the only kind the epilogue fusions apply to (a max / min op keeps its own output)
+ScatterGather* as_sum_sg(GnnOp* op) {
+  ScatterGather* sg = dynamic_cast<ScatterGather*>(op);
+  return (sg && sg->aggr == AGGR_SUM) ? sg : nullptr;
+}
 }  // namespace
 
 // gnn.cc:625-673.  No graph loading / ResourceManager creation left to do here
@@ -192,6 +227,16 @@ bool Model::init(const Config& config) {
     if (as<ScatterGather>(layers[l])) maxSg = std::max(maxSg, (int)layers[l]->inputs[0].dims[0]);
   }
   rt->ensure_lin_ws(ws);
+  // max / min aggregation sends each gradient to one source per (row, feature): a duplicate edge would receive it
+  // twice.  Strictly increasing sources per row rule duplicates out.
+  for (size_t l = 0; l < layers.size(); l++) {
+    ScatterGather* sg = as<ScatterGather>(layers[l]);
+    if (!sg || (sg->aggr != AGGR_MAX && sg->aggr != AGGR_MIN)) continue;
+    int sorted = 0;
+    ROC_CHECK(roc_sg_plan_rows_sorted(myGraph.plan, &sorted, rt->stream));
+    if (!sorted) ROC_FATAL("scatter_gather(max / min): every row's sources must be strictly increasing (no duplicate edges)");
+    break;
+  }
   if (maxSg > 0) {
     ROC_CHECK(roc_sg_plan_reserve(myGraph.plan, maxSg));
     if (rt->numParts > 1 && !myGraph.halo) rt->ensure_gather((size_t)myGraph.numNodes * (size_t)round_up4(maxSg));
@@ -237,7 +282,7 @@ bool Model::init(const Config& config) {
   if (fuse) {
     Wiring w = wire(layers);
     for (size_t l = 0; l < layers.size(); l++) {
-      ScatterGather* sg = as<ScatterGather>(layers[l]);
+      ScatterGather* sg = as_sum_sg(layers[l]);
       if (!sg) continue;
       // upstream: Linear(NONE) -> InDegreeNorm -> SG, each feeding only the next
       int rin = sg->inputs[0].region;
@@ -332,7 +377,10 @@ bool Model::init(const Config& config) {
   for (size_t l = 0; l < layers.size(); l++) layers[l]->init(*this);
   rt->opNames.clear();
   for (size_t l = 0; l < layers.size(); l++) {
-    const char* nm = as<ScatterGather>(layers[l]) ? "scatter_gather" : as<Linear>(layers[l]) ? "linear" :
+    const ScatterGather* sgl = as<ScatterGather>(layers[l]);
+    const char* nm = sgl ? (sgl->aggr == AGGR_MAX ? "scatter_gather(max)" : sgl->aggr == AGGR_MIN ? "scatter_gather(min)"
+                                                                                                  : "scatter_gather") :
+                     as<Linear>(layers[l]) ? "linear" :
                      as<InDegreeNorm>(layers[l]) ? "indegree_norm" : as<Activation>(layers[l]) ? "activation" :
                      as<Dropout>(layers[l]) ? "dropout" : as<Element>(layers[l]) ? "add" :
                      as<SoftmaxCrossEntropy>(layers[l]) ? "softmax_cross_entropy" : "op";
@@ -608,8 +656,8 @@ struct PushPipe {
 }  // namespace
 
 // -------------------------------------------------------- ScatterGather -----
-ScatterGather::ScatterGather(const Model& model, const Tensor& _input)
-    : GnnOp(_input), epilogue(0), bwdEpilogue(0), fwdOut(-1), bwdOut(-1) {
+ScatterGather::ScatterGather(const Model& model, const Tensor& _input, AggrType _aggr)
+    : GnnOp(_input), aggr(_aggr), arg(nullptr), argLd(0), epilogue(0), bwdEpilogue(0), fwdOut(-1), bwdOut(-1) {
   // scattergather.cc:33-37
   ROC_ASSERT(inputs[0].type == Tensor::NODE_TENSOR);
   ROC_ASSERT(inputs[0].numDim == 2);
@@ -668,6 +716,19 @@ void ScatterGather::forward(const Model& model) {
   RuntimeImpl* rt = model.ctx;
   const int H = (int)inputs[0].dims[0];
   const int64_t ldIn = rt->t(inputs[0].region).ld;
+  if (aggr == AGGR_MAX || aggr == AGGR_MIN) {   // one partition (Model::scatter_gather): no exchange, no fusion
+    const int64_t ldOut = rt->t(outputs[0].region).ld;
+    if (!arg) {
+      argLd = ldOut;
+      arg = (uint32_t*)rt->dmalloc((size_t)model.local_rows() * (size_t)argLd * sizeof(uint32_t));
+    }
+    rt->sg_begin(H);
+    ROC_CHECK(roc_sg_minmax_forward_planned(model.myGraph.plan, aggr == AGGR_MAX ? ROC_SG_AGGR_MAX : ROC_SG_AGGR_MIN, H,
+                                            rt->data(inputs[0].region), ldIn, rt->data(outputs[0].region), ldOut, arg,
+                                            argLd, rt->stream));
+    rt->sg_end();
+    return;
+  }
   const int outRegion = fwdOut >= 0 ? fwdOut : outputs[0].region;
   rt->sg_begin(-H);          // negative width = the exposed part of the halo exchange (profile mode only)
   const float* src = gathered(model, rt->data(inputs[0].region), ldIn, H, &rt->t(inputs[0].region), false);
@@ -684,6 +745,15 @@ void ScatterGather::backward(const Model& model) {
   if (!rt->t(inputs[0].region).requiresGrad) return;
   const int H = (int)inputs[0].dims[0];
   const int64_t ld = rt->t(outputs[0].region).ld;
+  if (aggr == AGGR_MAX || aggr == AGGR_MIN) {
+    // each output gradient goes to the source its forward chose; a gather over the same CSR (no atomics)
+    const int src = inputs[0].region;
+    rt->sg_begin(H);
+    ROC_CHECK(roc_sg_minmax_backward_planned(model.myGraph.plan, H, model.myGraph.rowLeft, rt->grad(outputs[0].region),
+                                             ld, arg, argLd, rt->grad(src), rt->t(src).ld, rt->stream));
+    rt->sg_end();
+    return;
+  }
   const int dstRegion = bwdOut >= 0 ? bwdOut : inputs[0].region;
   // Forward and backward do exactly the same thing, on gradients (scattergather_kernel.cu:168-169)
   rt->sg_begin(-H);

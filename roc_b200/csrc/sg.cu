@@ -30,8 +30,11 @@
 //                              two-slot ring, two worker warps consume (the structure the measured gather ceilings
 //                              ask for; not yet faster — DESIGN.md §3.1)
 //    The choice per width is by measurement (pick_variant); ROC_SG_VARIANT forces one.
+//  * min / max aggregation (roc_sg_minmax_*) runs kernel A templated on the reduction, with its own fix-ups
+//    for the forward; its backward is the sum schedule with a second gathered row and a predicated add.
 //
-// Algorithmic bytes per launch (DESIGN.md): E*(4H+4) + Nloc*(4H+8).
+// Algorithmic bytes per launch (DESIGN.md): E*(4H+4) + Nloc*(4H+8); min / max forward E*(4H+4) + Nloc*(8H+8),
+// backward E*(8H+4) + Nloc*(4H+8).
 #include <cub/cub.cuh>
 #include <thrust/iterator/counting_iterator.h>
 #include <cstdlib>
@@ -57,6 +60,8 @@ struct roc_sg_plan {
   const uint32_t* col = nullptr;  // caller's colSrc
   float* carry = nullptr;         // [numCarries][carryLd]
   size_t carryLd = 0;
+  uint32_t* carryArg = nullptr;   // [numCarries][carryLd] indices of the min / max carries (first use)
+  size_t carryArgLd = 0;
   uint32_t* desc = nullptr;       // [numChunks][8] per-chunk start state of the ring kernel (k_chunk_desc)
   int device = 0;
 };
@@ -153,11 +158,22 @@ __global__ void k_chunk_desc(uint32_t numChunks, uint32_t E, const uint32_t* __r
   d[1] = make_uint4(curT, r1, flags, carryIdx[w]);
 }
 
+// bad = 1 if some row's sources are not strictly increasing (one thread per row; an init-time check)
+__global__ void k_rows_sorted(uint32_t nloc, const uint32_t* __restrict__ rs, const uint32_t* __restrict__ col,
+                              uint32_t* __restrict__ bad) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= nloc) return;
+  const uint32_t t = rs[r + 1];
+  for (uint32_t e = rs[r] + 1; e < t; e++)
+    if (col[e] <= col[e - 1]) { *bad = 1u; return; }
+}
+
 // ----------------------------------------------------------- vector helper ---
 
 template <int VEC> struct V;
 template <> struct V<4> {
   typedef float4 T;
+  typedef uint4 I;           // the index of each float (min / max aggregation)
   static __device__ __forceinline__ T zero() { return make_float4(0.f, 0.f, 0.f, 0.f); }
   static __device__ __forceinline__ T ld(const T* p) { return __ldg(p); }
   static __device__ __forceinline__ T ld_plain(const T* p) { return *p; }
@@ -182,6 +198,7 @@ template <> struct V<4> {
 };
 template <> struct V<1> {
   typedef float T;
+  typedef uint32_t I;
   static __device__ __forceinline__ T zero() { return 0.f; }
   static __device__ __forceinline__ T ld(const T* p) { return __ldg(p); }
   static __device__ __forceinline__ T ld_plain(const T* p) { return *p; }
@@ -191,6 +208,57 @@ template <> struct V<1> {
   static __device__ __forceinline__ T rdiv(const T& a, const RowDiv& r) { return rowdiv(a, r); }
   static __device__ __forceinline__ T relu(const T& a) { return relu_nanprop(a); }
 };
+
+// ------------------------------------------------------- min / max reduction ---
+// What a kernel does with each gathered row.  SUM adds it; MAX / MIN keep, per float, the value and the source id of
+// the first edge in CSR order that holds the extreme (roc_sg_minmax_forward_planned); MASK is the backward of those:
+// it adds the gathered gradient only where the gathered index names the row being computed.
+enum { SG_RED_SUM = 0, SG_RED_MAX = ROC_SG_AGGR_MAX, SG_RED_MIN = ROC_SG_AGGR_MIN, SG_RED_MASK = 3 };
+constexpr uint32_t SG_NOARG = 0xFFFFFFFFu;   // index of a row that has no edge yet
+
+// The ordering rule: the candidate v replaces the current a iff it is strictly greater (smaller) or it is NaN and a
+// is not.  `!(v <= a || a != a)` is exactly that for max.  A current index of SG_NOARG means "no edge yet": the
+// first edge always wins.  Taking the partials of consecutive edge ranges in order with the same rule gives the
+// result of one sequential pass (the rule picks the leftmost maximal element of a total preorder).
+template <int RED>
+__device__ __forceinline__ void mm_take(float& a, uint32_t& ai, float v, uint32_t vi) {
+  const bool better = (RED == SG_RED_MAX) ? !(v <= a || a != a) : !(v >= a || a != a);
+  if (ai == SG_NOARG || better) { a = v; ai = vi; }
+}
+// one edge: every float of the row has the same source id
+template <int RED>
+__device__ __forceinline__ void mm_add(float4& a, uint4& ai, const float4& v, uint32_t src) {
+  mm_take<RED>(a.x, ai.x, v.x, src); mm_take<RED>(a.y, ai.y, v.y, src);
+  mm_take<RED>(a.z, ai.z, v.z, src); mm_take<RED>(a.w, ai.w, v.w, src);
+}
+template <int RED>
+__device__ __forceinline__ void mm_add(float& a, uint32_t& ai, float v, uint32_t src) { mm_take<RED>(a, ai, v, src); }
+// a partial of a later edge range (fix-ups): one with no edge is skipped
+template <int RED>
+__device__ __forceinline__ void mm_combine1(float& a, uint32_t& ai, float v, uint32_t vi) {
+  if (vi != SG_NOARG) mm_take<RED>(a, ai, v, vi);
+}
+template <int RED>
+__device__ __forceinline__ void mm_combine(float4& a, uint4& ai, const float4& v, const uint4& vi) {
+  mm_combine1<RED>(a.x, ai.x, v.x, vi.x); mm_combine1<RED>(a.y, ai.y, v.y, vi.y);
+  mm_combine1<RED>(a.z, ai.z, v.z, vi.z); mm_combine1<RED>(a.w, ai.w, v.w, vi.w);
+}
+template <int RED>
+__device__ __forceinline__ void mm_combine(float& a, uint32_t& ai, float v, uint32_t vi) { mm_combine1<RED>(a, ai, v, vi); }
+// a row with no edge stores 0 (its index stays SG_NOARG)
+__device__ __forceinline__ float mm_value1(float a, uint32_t ai) { return ai == SG_NOARG ? 0.f : a; }
+__device__ __forceinline__ float4 mm_value(const float4& a, const uint4& ai) {
+  return make_float4(mm_value1(a.x, ai.x), mm_value1(a.y, ai.y), mm_value1(a.z, ai.z), mm_value1(a.w, ai.w));
+}
+__device__ __forceinline__ float mm_value(float a, uint32_t ai) { return mm_value1(a, ai); }
+__device__ __forceinline__ uint4 mm_noarg(uint4*) { return make_uint4(SG_NOARG, SG_NOARG, SG_NOARG, SG_NOARG); }
+__device__ __forceinline__ uint32_t mm_noarg(uint32_t*) { return SG_NOARG; }
+// backward: acc += (arg == me) ? g : 0
+__device__ __forceinline__ void mask_add(float4& acc, const float4& g, const uint4& a, uint32_t me) {
+  acc.x += (a.x == me) ? g.x : 0.f; acc.y += (a.y == me) ? g.y : 0.f;
+  acc.z += (a.z == me) ? g.z : 0.f; acc.w += (a.w == me) ? g.w : 0.f;
+}
+__device__ __forceinline__ void mask_add(float& acc, float g, uint32_t a, uint32_t me) { acc += (a == me) ? g : 0.f; }
 
 struct SgParams {
   const uint32_t* rs;
@@ -209,6 +277,11 @@ struct SgParams {
   int dense;           // mean degree >= chunk size: nearly every row is cut at chunk boundaries
   const uint32_t* desc; // [numChunks][8] chunk start records (ring kernel)
   uint32_t nloc;        // rows of the partition (rs has nloc + 1 entries)
+  // min / max aggregation (kernel A only)
+  void* arg;            // MAX / MIN: [nloc][ldArg] indices written; MASK: [*][ldArg] indices gathered like `in`
+  void* carryArg;       // MAX / MIN: [numCarries][ldC] indices of the carry partials
+  size_t ldArg;         // in units of T
+  uint32_t selfBase;    // MASK: id of local row 0 in the id space of col
 };
 
 // out[v] = relu?(acc / sqrtf(deg)) — what the model applies right after
@@ -228,10 +301,14 @@ __device__ __forceinline__ void epi_store(typename V<VEC>::T v, typename V<VEC>:
 
 // ------------------------------------------------------------- main kernel ---
 // One worker (L lanes) per chunk.  Lane `lane` owns T-columns lane + ch*L.
-template <int VEC, int L, int NCH, int U, int MINB>
+// RED (SG_RED_*) changes only what is done with a gathered row and what the row store writes; the schedule, the
+// gathers and the single store site are the same for every reduction.
+template <int VEC, int L, int NCH, int U, int MINB, int RED = SG_RED_SUM>
 __global__ void __launch_bounds__(SG_THREADS, MINB)
 sg_chunk_kernel(const SgParams p) {
   typedef typename V<VEC>::T T;
+  typedef typename V<VEC>::I I;
+  constexpr bool MM = RED == SG_RED_MAX || RED == SG_RED_MIN;
   constexpr int WPB = SG_THREADS / L;
   constexpr uint32_t CH = SG_CH;
   const int lane = threadIdx.x % L;
@@ -268,8 +345,12 @@ sg_chunk_kernel(const SgParams p) {
   uint32_t segEnd = (kind == 1) ? curT : min(curT, ce);        // where this worker stops accumulating into it
 
   T acc[NCH];
+  I aidx[NCH];          // MAX / MIN: source id behind each float of acc
 #pragma unroll
-  for (int ch = 0; ch < NCH; ch++) acc[ch] = V<VEC>::zero();
+  for (int ch = 0; ch < NCH; ch++) {
+    acc[ch] = V<VEC>::zero();
+    if constexpr (MM) aidx[ch] = mm_noarg((I*)nullptr);
+  }
 
   // Row store.  The epilogue (IEEE sqrt + divides) lives in ONE out-of-line copy:
   // inlining it at every edge position made the kernel 4096 SASS instructions and
@@ -279,6 +360,23 @@ sg_chunk_kernel(const SgParams p) {
         ? reinterpret_cast<char*>(reinterpret_cast<T*>(p.carry) + lane) + (uint64_t)carrySlot * ((uint32_t)p.ldC * (uint32_t)sizeof(T))
         : reinterpret_cast<char*>(out + lane) + (uint64_t)cur * ((uint32_t)p.ldOut * (uint32_t)sizeof(T));
     T* dst = reinterpret_cast<T*>(dstb);
+    if constexpr (MM) {
+      // the owner of a cut row stores its partial to out / arg, a later chunk to its carry slot
+      char* ib = (kind == 0)
+          ? reinterpret_cast<char*>(reinterpret_cast<I*>(p.carryArg) + lane) + (uint64_t)carrySlot * ((uint32_t)p.ldC * (uint32_t)sizeof(I))
+          : reinterpret_cast<char*>(reinterpret_cast<I*>(p.arg) + lane) + (uint64_t)cur * ((uint32_t)p.ldArg * (uint32_t)sizeof(I));
+      I* idst = reinterpret_cast<I*>(ib);
+#pragma unroll
+      for (int ch = 0; ch < NCH; ch++) {
+        if (act[ch]) {
+          V<VEC>::st(dst + ch * L, mm_value(acc[ch], aidx[ch]));
+          idst[ch * L] = aidx[ch];
+        }
+        acc[ch] = V<VEC>::zero();
+        aidx[ch] = mm_noarg((I*)nullptr);
+      }
+      return;
+    }
     const int epi = (kind == 1) ? p.epi : 0;
 #pragma unroll
     for (int ch = 0; ch < NCH; ch++) {
@@ -311,6 +409,15 @@ sg_chunk_kernel(const SgParams p) {
   for (int ch = 0; ch < NCH; ch++)
     inl[ch] = reinterpret_cast<const char*>(in + min((uint32_t)(lane + ch * L), p.Q - 1u));
   const uint32_t rowBytes = (uint32_t)p.ldIn * (uint32_t)sizeof(T);
+  // MASK: the index row of each edge's source is gathered next to its gradient row
+  const char* argl[RED == SG_RED_MASK ? NCH : 1];
+  uint32_t argRowBytes = 0;
+  if constexpr (RED == SG_RED_MASK) {
+#pragma unroll
+    for (int ch = 0; ch < NCH; ch++)
+      argl[ch] = reinterpret_cast<const char*>(reinterpret_cast<const I*>(p.arg) + min((uint32_t)(lane + ch * L), p.Q - 1u));
+    argRowBytes = (uint32_t)p.ldArg * (uint32_t)sizeof(I);
+  }
   const uint32_t eLast = ee - 1u;
 #pragma unroll 1
   for (uint32_t base = e; base < ee; base += U) {
@@ -325,11 +432,17 @@ sg_chunk_kernel(const SgParams p) {
       for (int u = 0; u < U; u++) srcs[u] = __ldg(col + min(base + (uint32_t)u, eLast));
     }
     T v[U][NCH];
+    I av[RED == SG_RED_MASK ? U : 1][RED == SG_RED_MASK ? NCH : 1];
 #pragma unroll
     for (int u = 0; u < U; u++) {
       const uint64_t off = (uint64_t)srcs[u] * rowBytes;
 #pragma unroll
       for (int ch = 0; ch < NCH; ch++) v[u][ch] = V<VEC>::ld(reinterpret_cast<const T*>(inl[ch] + off));
+      if constexpr (RED == SG_RED_MASK) {
+        const uint64_t aoff = (uint64_t)srcs[u] * argRowBytes;
+#pragma unroll
+        for (int ch = 0; ch < NCH; ch++) av[u][ch] = __ldg(reinterpret_cast<const I*>(argl[ch] + aoff));
+      }
     }
     {
       // One rolled loop over the row segments of the group (predicated adds of the edges [pos, lim)
@@ -345,7 +458,11 @@ sg_chunk_kernel(const SgParams p) {
         for (int u = 0; u < U; u++) {
           if ((uint32_t)u >= pos && (uint32_t)u < lim) {
 #pragma unroll
-            for (int ch = 0; ch < NCH; ch++) V<VEC>::add(acc[ch], v[u][ch]);
+            for (int ch = 0; ch < NCH; ch++) {
+              if constexpr (RED == SG_RED_SUM) V<VEC>::add(acc[ch], v[u][ch]);
+              else if constexpr (RED == SG_RED_MASK) mask_add(acc[ch], v[u][ch], av[u][ch], p.selfBase + cur);
+              else mm_add<RED>(acc[ch], aidx[ch], v[u][ch], srcs[u]);
+            }
           }
         }
         pos = lim;
@@ -1158,6 +1275,123 @@ sg_fixup_big_kernel(const SgParams p) {
   }
 }
 
+// Min / max: one worker per heavy row takes the owner's partial (out[R], arg[R]), then the carries, k ascending,
+// with the same ordering rule.
+template <int VEC, int L, int NCH, int U, int RED>
+__global__ void __launch_bounds__(SG_THREADS)
+sg_fixup_minmax_kernel(const SgParams p) {
+  typedef typename V<VEC>::T T;
+  typedef typename V<VEC>::I I;
+  constexpr int WPB = SG_THREADS / L;
+  constexpr uint32_t CH = SG_CH;
+  const int lane = threadIdx.x % L;
+  const uint32_t w = blockIdx.x * WPB + threadIdx.x / L;
+  if (w >= p.numHeavy) return;
+  const uint32_t R = p.heavyRows[w];
+  const uint32_t s = p.rs[R], t = p.rs[R + 1];
+  const uint32_t c0 = s / CH, cLast = (t - 1) / CH;
+  const uint32_t n = cLast - c0;
+  const uint32_t slot0 = p.carryIdx[c0 + 1];
+  T* dst = reinterpret_cast<T*>(p.out) + (size_t)R * p.ldOut;
+  const T* cbase = reinterpret_cast<const T*>(p.carry) + (size_t)slot0 * p.ldC;
+  bool act[NCH];
+  T acc[NCH];
+  I* adst = reinterpret_cast<I*>(p.arg) + (size_t)R * p.ldArg;
+  const I* abase = reinterpret_cast<const I*>(p.carryArg) + (size_t)slot0 * p.ldC;
+  I ai[NCH];
+#pragma unroll
+  for (int ch = 0; ch < NCH; ch++) {
+    act[ch] = (uint32_t)(lane + ch * L) < p.Q;
+    acc[ch] = act[ch] ? V<VEC>::ld_plain(dst + lane + ch * L) : V<VEC>::zero();
+    ai[ch] = act[ch] ? adst[lane + ch * L] : mm_noarg((I*)nullptr);
+  }
+  for (uint32_t k = 0; k < n; k += U) {
+    T v[U][NCH];
+    I vi[U][NCH];
+#pragma unroll
+    for (int u = 0; u < U; u++)
+#pragma unroll
+      for (int ch = 0; ch < NCH; ch++) {
+        const bool ok = k + u < n && act[ch];
+        v[u][ch] = ok ? V<VEC>::ld_plain(cbase + (size_t)(k + u) * p.ldC + lane + ch * L) : V<VEC>::zero();
+        vi[u][ch] = ok ? abase[(size_t)(k + u) * p.ldC + lane + ch * L] : mm_noarg((I*)nullptr);
+      }
+#pragma unroll
+    for (int u = 0; u < U; u++)
+#pragma unroll
+      for (int ch = 0; ch < NCH; ch++) mm_combine<RED>(acc[ch], ai[ch], v[u][ch], vi[u][ch]);
+  }
+#pragma unroll
+  for (int ch = 0; ch < NCH; ch++)
+    if (act[ch]) { V<VEC>::st(dst + lane + ch * L, acc[ch]); adst[lane + ch * L] = ai[ch]; }
+}
+
+// Min / max rows with more than SG_BIG carries: each lane group reduces its block of carries in order, then group 0
+// takes the owner's partial and the groups' results in group order — chunk order again.
+template <int VEC, int L, int NCH, int U, int RED>
+__global__ void __launch_bounds__(SG_THREADS)
+sg_fixup_big_minmax_kernel(const SgParams p) {
+  typedef typename V<VEC>::T T;
+  typedef typename V<VEC>::I I;
+  constexpr int WPB = SG_THREADS / L;
+  constexpr uint32_t CH = SG_CH;
+  __shared__ __align__(16) float part[WPB * NCH * L * VEC];
+  __shared__ __align__(16) uint32_t parti[WPB * NCH * L * VEC];
+  const int lane = threadIdx.x % L;
+  const int g = threadIdx.x / L;
+  const uint32_t R = p.bigRows[blockIdx.x];
+  const uint32_t s = p.rs[R], t = p.rs[R + 1];
+  const uint32_t c0 = s / CH, cLast = (t - 1) / CH;
+  const uint32_t n = cLast - c0;
+  const uint32_t slot0 = p.carryIdx[c0 + 1];
+  const T* cbase = reinterpret_cast<const T*>(p.carry) + (size_t)slot0 * p.ldC;
+  const I* abase = reinterpret_cast<const I*>(p.carryArg) + (size_t)slot0 * p.ldC;
+  const uint32_t per = (n + WPB - 1) / WPB;
+  const uint32_t k0 = min(n, (uint32_t)g * per), k1 = min(n, k0 + per);
+  bool act[NCH];
+  T acc[NCH];
+  I ai[NCH];
+#pragma unroll
+  for (int ch = 0; ch < NCH; ch++) {
+    act[ch] = (uint32_t)(lane + ch * L) < p.Q; acc[ch] = V<VEC>::zero(); ai[ch] = mm_noarg((I*)nullptr);
+  }
+  for (uint32_t k = k0; k < k1; k += U) {
+    T v[U][NCH];
+    I vi[U][NCH];
+#pragma unroll
+    for (int u = 0; u < U; u++)
+#pragma unroll
+      for (int ch = 0; ch < NCH; ch++) {
+        const bool ok = k + u < k1 && act[ch];
+        v[u][ch] = ok ? V<VEC>::ld_plain(cbase + (size_t)(k + u) * p.ldC + lane + ch * L) : V<VEC>::zero();
+        vi[u][ch] = ok ? abase[(size_t)(k + u) * p.ldC + lane + ch * L] : mm_noarg((I*)nullptr);
+      }
+#pragma unroll
+    for (int u = 0; u < U; u++)
+#pragma unroll
+      for (int ch = 0; ch < NCH; ch++) mm_combine<RED>(acc[ch], ai[ch], v[u][ch], vi[u][ch]);
+  }
+  T* sp = reinterpret_cast<T*>(part);
+  I* spi = reinterpret_cast<I*>(parti);
+#pragma unroll
+  for (int ch = 0; ch < NCH; ch++) { sp[(g * NCH + ch) * L + lane] = acc[ch]; spi[(g * NCH + ch) * L + lane] = ai[ch]; }
+  __syncthreads();
+  if (g == 0) {
+    T* dst = reinterpret_cast<T*>(p.out) + (size_t)R * p.ldOut;
+    I* adst = reinterpret_cast<I*>(p.arg) + (size_t)R * p.ldArg;
+#pragma unroll
+    for (int ch = 0; ch < NCH; ch++) {
+      if (act[ch]) {
+        T a = V<VEC>::ld_plain(dst + lane + ch * L);      // the owner chunk's partial
+        I ia = adst[lane + ch * L];
+        for (int gg = 0; gg < WPB; gg++) mm_combine<RED>(a, ia, sp[(gg * NCH + ch) * L + lane], spi[(gg * NCH + ch) * L + lane]);
+        V<VEC>::st(dst + lane + ch * L, a);
+        adst[lane + ch * L] = ia;
+      }
+    }
+  }
+}
+
 // Variant A keeps the gathers in registers, variant C stages them in shared memory with
 // cp.async; C wins once a row needs two or more float4 per lane at L = 32 (H > 128).
 // ROC_SG_VARIANT=a|c forces one (experiments / cross-checks).
@@ -1292,6 +1526,47 @@ struct SgLaunch {
   int tcfg;                  // ring shape of variant T (-1 = default)
 };
 
+// Min / max forward (MAX, MIN) and its backward (MASK): kernel A and its fix-ups only.  The backward's partials are
+// sums, so it uses the sum fix-ups.
+template <int VEC, int L, int NCH, int U, int MINB, int RED>
+static int launch_red(const SgParams& p, cudaStream_t st) {
+  constexpr int WPB = SG_THREADS / L;
+  if (p.numChunks) {
+    sg_chunk_kernel<VEC, L, NCH, U, MINB, RED><<<(p.numChunks + WPB - 1) / WPB, SG_THREADS, 0, st>>>(p);
+    ROC_LAUNCH_CHECK();
+  }
+  if (p.numHeavy) {
+    if constexpr (RED == SG_RED_MASK) sg_fixup_kernel<VEC, L, NCH, U><<<(p.numHeavy + WPB - 1) / WPB, SG_THREADS, 0, st>>>(p);
+    else sg_fixup_minmax_kernel<VEC, L, NCH, U, RED><<<(p.numHeavy + WPB - 1) / WPB, SG_THREADS, 0, st>>>(p);
+    ROC_LAUNCH_CHECK();
+  }
+  if (p.numBig) {
+    if constexpr (RED == SG_RED_MASK) sg_fixup_big_kernel<VEC, L, NCH, U><<<p.numBig, SG_THREADS, 0, st>>>(p);
+    else sg_fixup_big_minmax_kernel<VEC, L, NCH, U, RED><<<p.numBig, SG_THREADS, 0, st>>>(p);
+    ROC_LAUNCH_CHECK();
+  }
+  return ROC_OK;
+}
+
+// Column blocks of the min / max entry points: 128 T-columns vectorised (512 floats: the big-row fix-up keeps values
+// and indices of every lane group in static shared memory), 256 scalar.  Gathers in flight (U) are lowered where the
+// index per float (forward) or the second gathered row (backward) would otherwise spill under kernel A's occupancy.
+template <int VEC, int RED>
+static int dispatch_red(const SgParams& p, cudaStream_t st) {
+  constexpr bool B = RED == SG_RED_MASK;
+  const uint32_t Q = p.Q;
+  if (Q <= 4) return launch_red<VEC, 4, 1, 4, 4, RED>(p, st);
+  if (Q <= 8) return launch_red<VEC, 8, 1, 4, 4, RED>(p, st);
+  if (Q <= 16) return launch_red<VEC, 16, 1, 4, 4, RED>(p, st);
+  if (Q <= 32) return launch_red<VEC, 32, 1, 4, 4, RED>(p, st);
+  if (Q <= 64) return launch_red<VEC, 32, 2, B ? 2 : 4, 3, RED>(p, st);
+  if (Q <= 128) return launch_red<VEC, 32, 4, 1, 3, RED>(p, st);
+  if constexpr (VEC == 1) {
+    if (Q <= 256) return launch_red<VEC, 32, 8, 1, 2, RED>(p, st);
+  }
+  return ROC_ERR_UNSUPPORTED;
+}
+
 template <int VEC, int L, int NCH, int U, int MINB>
 static int launch_cfg(const SgParams& p, const SgLaunch& how, cudaStream_t st) {
   constexpr int WPB = SG_THREADS / L;
@@ -1395,6 +1670,21 @@ static int ensure_carry(roc_sg_plan* plan, size_t ldFloats, cudaStream_t st, boo
   return ROC_OK;
 }
 
+// The index carries of the min / max forward: u32 [numCarries][carryLd], the shape of the float carries (the kernels
+// address both with one leading dimension), grown the same way.
+static int ensure_carry_arg(roc_sg_plan* plan, cudaStream_t st) {
+  if (plan->numCarries == 0 || plan->carryArgLd == plan->carryLd) return ROC_OK;
+  if (plan->carryArg) {
+    ROC_CUDA(cudaFreeAsync(plan->carryArg, st));
+    plan->carryArg = nullptr; plan->carryArgLd = 0;
+  }
+  const size_t bytes = (size_t)plan->numCarries * plan->carryLd * sizeof(uint32_t);
+  cudaError_t e = cudaMallocAsync((void**)&plan->carryArg, bytes, st);
+  if (e != cudaSuccess) { plan->carryArg = nullptr; plan->carryArgLd = 0; return (int)e; }
+  plan->carryArgLd = plan->carryLd;
+  return ROC_OK;
+}
+
 }  // namespace roc
 
 using namespace roc;
@@ -1475,6 +1765,7 @@ done:
 extern "C" void roc_sg_plan_destroy(roc_sg_plan* pl) {
   if (!pl) return;
   cudaFree(pl->rs); cudaFree(pl->firstRow); cudaFree(pl->carryIdx); cudaFree(pl->heavyRows); cudaFree(pl->bigRows); cudaFree(pl->carry); cudaFree(pl->desc);
+  cudaFree(pl->carryArg);
   delete pl;
 }
 
@@ -1528,6 +1819,108 @@ extern "C" int roc_sg_forward_planned(const roc_sg_plan* plc, int H, const float
       p.ldIn = (size_t)ldIn; p.ldOut = (size_t)ldOut; p.ldC = pl->carryLd;
       p.Q = (uint32_t)hb;
       rc = dispatch<1>(p, how, st);
+    }
+    if (rc != ROC_OK) return rc;
+  }
+  return ROC_OK;
+}
+
+extern "C" int roc_sg_plan_rows_sorted(const roc_sg_plan* pl, int* sorted, roc_stream_t stream) {
+  if (!pl || !sorted) return ROC_ERR_INVALID;
+  cudaStream_t st = as_stream(stream);
+  uint32_t* bad = nullptr;
+  uint32_t h = 0;
+  ROC_CUDA(cudaMallocAsync((void**)&bad, sizeof(uint32_t), st));
+  cudaError_t e = cudaMemsetAsync(bad, 0, sizeof(uint32_t), st);
+  if (e == cudaSuccess && pl->nloc && pl->E) {
+    k_rows_sorted<<<(pl->nloc + 255) / 256, 256, 0, st>>>(pl->nloc, pl->rs, pl->col, bad);
+    count_launch();
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&h, bad, sizeof(uint32_t), cudaMemcpyDeviceToHost, st);
+  cudaError_t f = cudaFreeAsync(bad, st);
+  if (e == cudaSuccess) e = f;
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return (int)e;
+  *sorted = h ? 0 : 1;
+  return ROC_OK;
+}
+
+// The plan parameters shared by every launch of column block c0 (units of T applied by the caller).
+static SgParams plan_params(const roc_sg_plan* pl) {
+  SgParams p;
+  memset(&p, 0, sizeof(p));
+  p.rs = pl->rs; p.firstRow = pl->firstRow; p.carryIdx = pl->carryIdx; p.heavyRows = pl->heavyRows; p.bigRows = pl->bigRows;
+  p.col = pl->col; p.carry = pl->carry; p.carryArg = pl->carryArg;
+  p.E = pl->E; p.numChunks = pl->numChunks; p.numHeavy = pl->numHeavy; p.numBig = pl->numBig; p.epi = 0;
+  p.desc = pl->desc; p.nloc = pl->nloc;
+  return p;
+}
+
+extern "C" int roc_sg_minmax_forward_planned(const roc_sg_plan* plc, int aggr, int H, const float* in, int64_t ldIn,
+                                             float* out, int64_t ldOut, roc_vid_t* arg, int64_t ldArg,
+                                             roc_stream_t stream) {
+  roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  if (!pl || (aggr != ROC_SG_AGGR_MAX && aggr != ROC_SG_AGGR_MIN) || H <= 0 || !in || !out || !arg || ldIn < H ||
+      ldOut < H || ldArg < H)
+    return ROC_ERR_INVALID;
+  cudaStream_t st = as_stream(stream);
+  const bool vec = (ldIn % 4 == 0) && (ldOut % 4 == 0) && (ldArg % 4 == 0) && aligned16(in) && aligned16(out) &&
+                   aligned16(arg);
+  const int blockCols = vec ? 512 : 256;
+  {
+    int need = H < blockCols ? H : blockCols;
+    int rc = ensure_carry(pl, ((size_t)need + 3) / 4 * 4, st, true);
+    if (rc != ROC_OK) return rc;
+    rc = ensure_carry_arg(pl, st);
+    if (rc != ROC_OK) return rc;
+  }
+  for (int c0 = 0; c0 < H; c0 += blockCols) {
+    const int hb = (H - c0 < blockCols) ? H - c0 : blockCols;
+    SgParams p = plan_params(pl);
+    p.in = in + c0; p.out = out + c0; p.arg = arg + c0;
+    int rc;
+    if (vec) {
+      p.ldIn = (size_t)ldIn / 4; p.ldOut = (size_t)ldOut / 4; p.ldArg = (size_t)ldArg / 4; p.ldC = pl->carryLd / 4;
+      p.Q = ((uint32_t)hb + 3) / 4;
+      rc = aggr == ROC_SG_AGGR_MAX ? dispatch_red<4, SG_RED_MAX>(p, st) : dispatch_red<4, SG_RED_MIN>(p, st);
+    } else {
+      p.ldIn = (size_t)ldIn; p.ldOut = (size_t)ldOut; p.ldArg = (size_t)ldArg; p.ldC = pl->carryLd;
+      p.Q = (uint32_t)hb;
+      rc = aggr == ROC_SG_AGGR_MAX ? dispatch_red<1, SG_RED_MAX>(p, st) : dispatch_red<1, SG_RED_MIN>(p, st);
+    }
+    if (rc != ROC_OK) return rc;
+  }
+  return ROC_OK;
+}
+
+extern "C" int roc_sg_minmax_backward_planned(const roc_sg_plan* plc, int H, roc_vid_t selfBase, const float* outGrad,
+                                              int64_t ldG, const roc_vid_t* arg, int64_t ldArg, float* inGrad,
+                                              int64_t ldIn, roc_stream_t stream) {
+  roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  if (!pl || H <= 0 || !outGrad || !arg || !inGrad || ldG < H || ldArg < H || ldIn < H) return ROC_ERR_INVALID;
+  cudaStream_t st = as_stream(stream);
+  const bool vec = (ldG % 4 == 0) && (ldArg % 4 == 0) && (ldIn % 4 == 0) && aligned16(outGrad) && aligned16(arg) &&
+                   aligned16(inGrad);
+  const int blockCols = vec ? 512 : 256;
+  {
+    int need = H < blockCols ? H : blockCols;
+    int rc = ensure_carry(pl, ((size_t)need + 3) / 4 * 4, st, true);
+    if (rc != ROC_OK) return rc;
+  }
+  for (int c0 = 0; c0 < H; c0 += blockCols) {
+    const int hb = (H - c0 < blockCols) ? H - c0 : blockCols;
+    SgParams p = plan_params(pl);
+    p.in = outGrad + c0; p.out = inGrad + c0; p.arg = const_cast<roc_vid_t*>(arg) + c0; p.selfBase = selfBase;
+    int rc;
+    if (vec) {
+      p.ldIn = (size_t)ldG / 4; p.ldOut = (size_t)ldIn / 4; p.ldArg = (size_t)ldArg / 4; p.ldC = pl->carryLd / 4;
+      p.Q = ((uint32_t)hb + 3) / 4;
+      rc = dispatch_red<4, SG_RED_MASK>(p, st);
+    } else {
+      p.ldIn = (size_t)ldG; p.ldOut = (size_t)ldIn; p.ldArg = (size_t)ldArg; p.ldC = pl->carryLd;
+      p.Q = (uint32_t)hb;
+      rc = dispatch_red<1, SG_RED_MASK>(p, st);
     }
     if (rc != ROC_OK) return rc;
   }

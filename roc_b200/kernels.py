@@ -66,6 +66,40 @@ class SgPlan:
                                          _stream()), "roc_sg_forward_planned")
         return out
 
+    def rows_sorted(self):
+        """True if every row's sources are strictly increasing (no duplicate edges)."""
+        ok = C.c_int()
+        check(lib.roc_sg_plan_rows_sorted(self.handle, C.byref(ok), _stream()), "roc_sg_plan_rows_sorted")
+        return bool(ok.value)
+
+    def minmax_forward(self, x, aggr, out=None, arg=None):
+        """Max (aggr = AGGR_MAX) or min (AGGR_MIN) aggregation -> (out [Nloc][H] fp32, arg [Nloc][H]): arg holds the
+        source id of the first edge in CSR order with the extreme value (uint32 bits in int32 storage; SG_NOARG,
+        i.e. -1, for a row with no edge)."""
+        nloc = self.row_right - self.row_left + 1
+        h = x.shape[1]
+        vec = _ld(x) % 4 == 0
+        if out is None:
+            out = padded(nloc, h, x.device) if vec else torch.empty((nloc, h), device=x.device)
+        if arg is None:
+            arg = padded(nloc, h, x.device, dtype=torch.int32) if vec else \
+                torch.empty((nloc, h), device=x.device, dtype=torch.int32)
+        check(lib.roc_sg_minmax_forward_planned(self.handle, int(aggr), h, _ptr(x), _ld(x), _ptr(out), _ld(out),
+                                                _ptr(arg), _ld(arg), _stream()), "roc_sg_minmax_forward_planned")
+        return out, arg
+
+    def minmax_backward(self, gy, arg, self_base=0, out=None):
+        """Gradient of minmax_forward's input: out[u] = sum over row u's edges e (v = col[e]) of gy[v] where
+        arg[v] == self_base + u.  gy and arg are indexed like the forward's input."""
+        nloc = self.row_right - self.row_left + 1
+        h = gy.shape[1]
+        if out is None:
+            out = padded(nloc, h, gy.device) if _ld(gy) % 4 == 0 else torch.empty((nloc, h), device=gy.device)
+        check(lib.roc_sg_minmax_backward_planned(self.handle, h, int(self_base), _ptr(gy), _ld(gy), _ptr(arg),
+                                                 _ld(arg), _ptr(out), _ld(out), _stream()),
+              "roc_sg_minmax_backward_planned")
+        return out
+
     def close(self):
         if self.handle:
             lib.roc_sg_plan_destroy(self.handle)

@@ -92,8 +92,12 @@ class Model:
     def indegree_norm(self, t):
         return lib.roc_host_indegree_norm(self.h, t)
 
-    def scatter_gather(self, t):
-        return lib.roc_host_scatter_gather(self.h, t)
+    def scatter_gather(self, t, aggr=_lib.AGGR_SUM):
+        """aggr: AGGR_SUM (the reference's op), AGGR_AVG (sum -> indegree_norm -> indegree_norm), AGGR_MAX / AGGR_MIN
+        (per feature over the in-neighbours; one partition only)."""
+        if aggr == _lib.AGGR_SUM:
+            return lib.roc_host_scatter_gather(self.h, t)
+        return lib.roc_host_scatter_gather_aggr(self.h, t, int(aggr))
 
     def relu(self, t):
         return lib.roc_host_relu(self.h, t)
@@ -156,6 +160,13 @@ class Model:
         rows, hidden, _ = self.tensor_shape(t)
         out = np.empty((rows, hidden), dtype=dtype)
         check(lib.roc_host_get_tensor(self.h, t, out.ctypes.data, int(grad)))
+        return out
+
+    def get_aggr_index(self, t):
+        """The source ids a max / min scatter_gather output t was taken from, [rows][hidden] uint32 (after forward)."""
+        rows, hidden, _ = self.tensor_shape(t)
+        out = np.empty((rows, hidden), dtype=np.uint32)
+        check(lib.roc_host_get_aggr_index(self.h, t, out.ctypes.data))
         return out
 
     def set_labels(self, t, class_idx):
@@ -279,3 +290,38 @@ def build_sage_mean(model, layers, dropout_rate, lr=0.01, weight_decay=0.05):
     model.adam(lr, weight_decay)
     model.init()
     return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs}
+
+
+def build_sage_pool(model, layers, dropout_rate, aggr=_lib.AGGR_MAX, lr=0.01, weight_decay=0.05):
+    """GraphSAGE with the pooling aggregator (Hamilton et al., 2017) composed from the reference's ops plus the max
+    (or min) ScatterGather.  The reference's Linear has no bias, so neither has this.  Per layer:
+
+        d  = dropout(t)
+        p  = relu(linear(d, d_i))                      # the pooling network
+        nb = scatter_gather(p, aggr)                   # per feature, max (min) over N(v) + v (self loops are in A)
+        t  = add(linear(nb, d_i), linear(d, d_i))      # neighbour weight + root / self weight
+        t  = relu(t)                                   # all but the last layer
+
+    Single partition; init refuses a graph with a duplicate edge in a row.  Returns the handles, with `pools`
+    (the scatter_gather outputs, for get_aggr_index) and `pool_ins` (their inputs)."""
+    L = len(layers)
+    x = model.create_node_tensor(layers[0])
+    label = model.create_node_tensor(layers[-1])
+    mask = model.create_node_tensor(1, is_int=True)
+    t = x
+    relu_outs, pools, pool_ins = [], [], []
+    for i in range(1, L):
+        d = model.dropout(t, dropout_rate)
+        p = model.relu(model.linear(d, layers[i], _lib.AC_MODE_NONE))
+        nb = model.scatter_gather(p, aggr)
+        pool_ins.append(p)
+        pools.append(nb)
+        t = model.add(model.linear(nb, layers[i], _lib.AC_MODE_NONE), model.linear(d, layers[i], _lib.AC_MODE_NONE))
+        if i != L - 1:
+            t = model.relu(t)
+            relu_outs.append(t)
+    model.softmax_cross_entropy(t, label, mask)
+    model.adam(lr, weight_decay)
+    model.init()
+    return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs, "pools": pools,
+            "pool_ins": pool_ins}

@@ -2,7 +2,7 @@
 # compute-sanitizer over the tiny configuration (SURVEY §5): memcheck, then racecheck, on
 #   (a) __graft_entry__.smoke()  — one GCN training step through the Model API (SG, wgmma GEMMs, softmax, Adam)
 #   (b) every ScatterGather variant (registers / cp.async / TMA bulk-copy rings / producer-consumer ring) on the
-#       ragged test graph.
+#       ragged test graph, then one max-aggregation forward and backward.
 # Usage: tools/sanitize.sh [logdir]   (needs a GPU; `make sanitize`)
 set -u
 ROOT="$(cd "$(dirname "$0")/.." && pwd)"
@@ -25,6 +25,10 @@ for h in (41, 64, 200):
         outs.append(plan.forward(x, epilogue=3).clone())
     torch.cuda.synchronize()
     assert all(torch.equal(o.view(torch.int32), outs[0].view(torch.int32)) for o in outs), h
+    os.environ.pop("ROC_SG_VARIANT")
+    mx, arg = plan.minmax_forward(x, 1)                 # max aggregation and its backward (kernel A + fix-ups)
+    g = plan.minmax_backward(x, arg)
+    torch.cuda.synchronize()
 print("sg variants ok")
 PY
 rc=0

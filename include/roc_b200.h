@@ -392,6 +392,21 @@ int roc_linear_bwd_fused(const roc_linear_bwd_args* args, roc_stream_t stream);
 #define ROC_GEMM_PATH_SIMT 2
 int roc_last_gemm_path(int which);
 
+/* Test hook: how the calling thread's last Linear GEMM of kind `which` (as above) ran, so that a test can assert that
+ * a shape reached the kernel instantiation and pipeline regime it was chosen for.  On the SIMT path only `path` is
+ * set, and for dW also `splits` / `v_per_split` (the rest is 0).  Tensor cores:
+ *   nc        wgmma chunks of 32 columns per N tile (1, 2, 4; dW 1, 2, 4, 8)
+ *   epi       forward / dX epilogue instantiation: its EPI bit mask, or -1 for the generic kernel (dW: 0)
+ *   grid_x/y  forward / dX: persistent CTAs along the rows x N tiles;  dW: splits x 128-column M tiles
+ *   stages    depth of the TMA ring
+ *   splits, v_per_split   dW only: split-K ranges and the rows each holds (the partials are added in range order)
+ * Returns ROC_ERR_INVALID for a bad `which` or a NULL `info`. */
+typedef struct {
+  int path, nc, epi, grid_x, grid_y, stages, splits;
+  int64_t v_per_split;
+} roc_gemm_info;
+int roc_last_gemm_info(int which, roc_gemm_info* info);
+
 /* ------------------------------------------------------------ optimizer --- */
 
 /* Replaces adam_update, optimizer_kernel.cu:43-63 (launch :98-101).  alpha_t is

@@ -18,6 +18,8 @@ SG_EPI_NONE, SG_EPI_NORM, SG_EPI_RELU = 0, 1, 2
 AGGR_AVG, AGGR_MAX, AGGR_MIN, AGGR_SUM = 0, 1, 2, 3        # AggrType (gnn.h:75-80); ROC_SG_AGGR_MAX / _MIN = 1 / 2
 SG_NOARG = 0xFFFFFFFF                                      # arg of a row with no in-edge
 LINEAR_NORM_EPILOGUE = 1
+LINEAR_BWD_ONLY_DX, LINEAR_BWD_ONLY_DW = 1, 2
+GEMM_FWD, GEMM_DW, GEMM_DX = 0, 1, 2                       # `which` of roc_last_gemm_path / roc_last_gemm_info
 
 
 class LinearBwdArgs(C.Structure):
@@ -31,6 +33,15 @@ class LinearBwdArgs(C.Structure):
                 ("dropMask", C.c_void_p), ("ldMask", C.c_int64), ("dropRate", C.c_float),
                 ("dxReluOf", C.c_void_p), ("ldReluOf", C.c_int64),
                 ("dxNormRowEnd", C.c_void_p), ("colLeft", C.c_uint64), ("parts", C.c_int)]
+
+
+class GemmInfo(C.Structure):
+    """roc_gemm_info (include/roc_b200.h): how the last Linear GEMM of one kind was launched."""
+    _fields_ = [("path", C.c_int), ("nc", C.c_int), ("epi", C.c_int), ("grid_x", C.c_int), ("grid_y", C.c_int),
+                ("stages", C.c_int), ("splits", C.c_int), ("v_per_split", C.c_int64)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
 
 
 class PerfMetrics(C.Structure):
@@ -107,6 +118,7 @@ PROTOTYPES = {
     "roc_linear_bwd_dropout": (i32, [i64, i32, i32, vp, i64, vp, vp, i64, vp, i64, vp, vp, i64, i32, i32, vp, sz,
                                      vp, i64, f32, vp]),
     "roc_last_gemm_path": (i32, [i32]),
+    "roc_last_gemm_info": (i32, [i32, C.POINTER(GemmInfo)]),
     "roc_adam_update": (i32, [i64, f32, f32, f32, f32, f32, vp, vp, vp, vp, vp]),
     "roc_scale": (i32, [i64, f32, f32, vp, vp]),
     "roc_fill": (i32, [i64, i32, f32, vp, i64, vp]),
@@ -175,6 +187,13 @@ def check(rc, what=""):
         names = {-1: "ROC_ERR_INVALID", -2: "ROC_ERR_UNSUPPORTED", -3: "ROC_ERR_NOMEM", -4: "ROC_ERR_NO_DEVICE",
                  -5: "ROC_ERR_IO"}
         raise RocError("%s failed: %s" % (what or "roc call", names.get(rc, "cudaError %d" % rc)))
+
+
+def last_gemm_info(which):
+    """roc_last_gemm_info as a dict; which = 0 forward, 1 dW, 2 dX."""
+    info = GemmInfo()
+    check(lib.roc_last_gemm_info(which, C.byref(info)), "roc_last_gemm_info")
+    return info.as_dict()
 
 
 def device_count():

@@ -12,20 +12,23 @@ int simt_linear_dx(int64_t rows, int inDim, int outDim, const float* dY, int64_t
                    int64_t ldDX, int accumulate, const DropMask* dm, const float* reluOf, int64_t ldR,
                    const uint64_t* rowEnd, uint64_t colLeft, cudaStream_t st);
 int simt_linear_dw(int64_t rows, int inDim, int outDim, const float* X, int64_t ldX, const float* dY, int64_t ldDY,
-                   float* dW, float* workspace, size_t wsBytes, const DropMask* dm, cudaStream_t st);
+                   float* dW, float* workspace, size_t wsBytes, const DropMask* dm, cudaStream_t st,
+                   roc_gemm_info* info);
 int relu_bwd_inplace(int64_t rows, int H, const float* Y, int64_t ldY, float* dY, int64_t ldDY, cudaStream_t st);
 
 // tensor-core path (linear_tc.cu, linear_tc_dw.cu); each returns ROC_ERR_UNSUPPORTED when the
 // shape / alignment is outside what the wgmma kernels take.
+// They describe the launch they made in *info (roc_last_gemm_info).
 int tc_linear_fwd(int64_t rows, int inDim, int outDim, const float* X, int64_t ldX, const float* W, float* Y,
                   int64_t ldY, int relu, const uint64_t* rowEnd, uint64_t colLeft, const DropMask* dm,
-                  cudaStream_t st);
+                  cudaStream_t st, roc_gemm_info* info);
 int tc_linear_dx(int64_t rows, int inDim, int outDim, const float* dY, int64_t ldDY, const float* W, float* dX,
                  int64_t ldDX, int accumulate, const DropMask* dm, const float* reluOf, int64_t ldR,
-                 const uint64_t* rowEnd, uint64_t colLeft, cudaStream_t st);
+                 const uint64_t* rowEnd, uint64_t colLeft, cudaStream_t st, roc_gemm_info* info);
 size_t tc_dw_workspace_bytes(int64_t rows, int inDim, int outDim);
 int tc_linear_dw(int64_t rows, int inDim, int outDim, const float* X, int64_t ldX, const float* dY, int64_t ldDY,
-                 float* dW, float* workspace, size_t wsBytes, const DropMask* dm, cudaStream_t st);
+                 float* dW, float* workspace, size_t wsBytes, const DropMask* dm, cudaStream_t st,
+                 roc_gemm_info* info);
 
 // ROC_B200_GEMM=simt forces the exact-fp32 SIMT kernels (used by tests to
 // cross-check the tensor-core path).
@@ -34,10 +37,10 @@ static bool force_simt() {
   if (v < 0) { const char* e = getenv("ROC_B200_GEMM"); v = (e && e[0] == 's' && e[1] == 'i') ? 1 : 0; }
   return v == 1;
 }
-// which kernel family served the calling thread's last Linear GEMM of each kind (test hook: the tensor-core path
-// returns ROC_ERR_UNSUPPORTED for shapes it does not take and the dispatcher then uses SIMT — a test that means to
-// check the tensor cores must be able to see that it did)
-static thread_local int t_lastPath[3] = {0, 0, 0};   // fwd, dW, dX: 0 none, 1 tensor cores (wgmma), 2 SIMT
+// which kernel served the calling thread's last Linear GEMM of each kind, and how it was launched (test hook: the
+// tensor-core path returns ROC_ERR_UNSUPPORTED for shapes it does not take and the dispatcher then uses SIMT — a test
+// that means to check the tensor cores, or one instantiation / pipeline regime of them, must be able to see that it did)
+static thread_local roc_gemm_info t_last[3] = {};   // fwd, dW, dX; path 0 none, 1 tensor cores (wgmma), 2 SIMT
 }  // namespace roc
 
 using namespace roc;
@@ -63,10 +66,12 @@ static int linear_fwd_impl(int64_t rows, int inDim, int outDim, const float* X, 
   const uint64_t* re = (flags & ROC_LINEAR_NORM_EPILOGUE) ? rowEnd : nullptr;
   const int relu = activation == ROC_AC_MODE_RELU;
   if (!force_simt()) {
-    int rc = tc_linear_fwd(rows, inDim, outDim, X, ldX, W, Y, ldY, relu, re, colLeft, dm, as_stream(stream));
-    if (rc != ROC_ERR_UNSUPPORTED) { t_lastPath[0] = 1; return rc; }
+    roc_gemm_info info{};
+    int rc = tc_linear_fwd(rows, inDim, outDim, X, ldX, W, Y, ldY, relu, re, colLeft, dm, as_stream(stream), &info);
+    if (rc != ROC_ERR_UNSUPPORTED) { info.path = 1; t_last[0] = info; return rc; }
   }
-  t_lastPath[0] = 2;
+  t_last[0] = roc_gemm_info{};
+  t_last[0].path = 2;
   return simt_linear_fwd(rows, inDim, outDim, X, ldX, W, Y, ldY, relu, re, colLeft, dm, as_stream(stream));
 }
 
@@ -119,21 +124,25 @@ static int linear_bwd_impl(int64_t rows, int inDim, int outDim, const float* X, 
   int rc = ROC_OK;
   if (parts != ROC_LINEAR_BWD_ONLY_DX) {
     rc = ROC_ERR_UNSUPPORTED;
+    roc_gemm_info info{};
     if (!force_simt())
-      rc = tc_linear_dw(rows, inDim, outDim, X, ldX, dY, ldDY, dW, (float*)workspace, workspaceBytes, dm, st);
-    t_lastPath[1] = 1;
-    if (rc == ROC_ERR_UNSUPPORTED) t_lastPath[1] = 2;
+      rc = tc_linear_dw(rows, inDim, outDim, X, ldX, dY, ldDY, dW, (float*)workspace, workspaceBytes, dm, st, &info);
+    if (rc == ROC_ERR_UNSUPPORTED) info = roc_gemm_info{};
+    info.path = (rc == ROC_ERR_UNSUPPORTED) ? 2 : 1;
     if (rc == ROC_ERR_UNSUPPORTED)
-      rc = simt_linear_dw(rows, inDim, outDim, X, ldX, dY, ldDY, dW, (float*)workspace, workspaceBytes, dm, st);
+      rc = simt_linear_dw(rows, inDim, outDim, X, ldX, dY, ldDY, dW, (float*)workspace, workspaceBytes, dm, st, &info);
+    t_last[1] = info;
     if (rc != ROC_OK) return rc;
   }
   if (dX) {
     rc = ROC_ERR_UNSUPPORTED;
+    roc_gemm_info info{};
     if (!force_simt())
       rc = tc_linear_dx(rows, inDim, outDim, dY, ldDY, W, dX, ldDX, accumulate_dX, dm, dxReluOf, ldReluOf, dxRowEnd,
-                        colLeft, st);
-    t_lastPath[2] = 1;
-    if (rc == ROC_ERR_UNSUPPORTED) t_lastPath[2] = 2;
+                        colLeft, st, &info);
+    if (rc == ROC_ERR_UNSUPPORTED) info = roc_gemm_info{};
+    info.path = (rc == ROC_ERR_UNSUPPORTED) ? 2 : 1;
+    t_last[2] = info;
     if (rc == ROC_ERR_UNSUPPORTED)
       rc = simt_linear_dx(rows, inDim, outDim, dY, ldDY, W, dX, ldDX, accumulate_dX, dm, dxReluOf, ldReluOf, dxRowEnd,
                           colLeft, st);
@@ -176,4 +185,10 @@ extern "C" int roc_linear_bwd_fused(const roc_linear_bwd_args* a, roc_stream_t s
                          a->dxReluOf, a->ldReluOf, a->dxNormRowEnd, a->colLeft, stream, a->parts);
 }
 
-extern "C" int roc_last_gemm_path(int which) { return (which >= 0 && which < 3) ? t_lastPath[which] : 0; }
+extern "C" int roc_last_gemm_path(int which) { return (which >= 0 && which < 3) ? t_last[which].path : 0; }
+
+extern "C" int roc_last_gemm_info(int which, roc_gemm_info* info) {
+  if (which < 0 || which >= 3 || !info) return ROC_ERR_INVALID;
+  *info = t_last[which];
+  return ROC_OK;
+}

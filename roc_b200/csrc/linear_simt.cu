@@ -184,7 +184,8 @@ int simt_linear_dx(int64_t rows, int inDim, int outDim, const float* dY, int64_t
 }
 
 int simt_linear_dw(int64_t rows, int inDim, int outDim, const float* X, int64_t ldX, const float* dY, int64_t ldDY,
-                   float* dW, float* workspace, size_t wsBytes, const DropMask* dm, cudaStream_t st) {
+                   float* dW, float* workspace, size_t wsBytes, const DropMask* dm, cudaStream_t st,
+                   roc_gemm_info* info) {
   int splits = simt_dw_splits(rows, inDim, outDim);
   int64_t count = (int64_t)inDim * outDim;
   if (wsBytes < (size_t)splits * count * sizeof(float)) return ROC_ERR_INVALID;
@@ -194,6 +195,7 @@ int simt_linear_dw(int64_t rows, int inDim, int outDim, const float* X, int64_t 
   p.kPerSplit = ((rows + splits - 1) / splits + GB_K - 1) / GB_K * GB_K;
   p.splitStrideC = count; p.accumulate = 0;
   set_mask(p, dm, 2);
+  if (info) { info->splits = splits; info->v_per_split = p.kPerSplit; }
   dim3 grid((unsigned)((outDim + GB_M - 1) / GB_M), (unsigned)((inDim + GB_N - 1) / GB_N), (unsigned)splits);
   k_sgemm<false, false><<<grid, G_THREADS, 0, st>>>(p);
   ROC_LAUNCH_CHECK();

@@ -244,6 +244,12 @@ struct TsEpilogue {
   int accumulate = 0;
 };
 
+// the epilogue instantiation that serves `epi`: the combinations the GCN path produces have their own, anything else
+// takes the generic kernel (-1)
+static int tc_instance(int epi) {
+  return (epi == 0 || epi == EPI_NORM || epi == EPI_OMASK || epi == (EPI_OMASK | EPI_RELUOF | EPI_NORM)) ? epi : -1;
+}
+
 template <int NC>
 static int tc_launch(dim3 grid, size_t smemBytes, int epi, const CUtensorMap& mapA, const CUtensorMap& mapWhi,
                      const CUtensorMap& mapWlo, const TcParams& q, cudaStream_t st) {
@@ -253,7 +259,7 @@ static int tc_launch(dim3 grid, size_t smemBytes, int epi, const CUtensorMap& ma
     ROC_CUDA(ensure_dyn_smem(k_tc_linear<NC, E>, smemBytes, configured));                                         \
     k_tc_linear<NC, E><<<grid, TC_THREADS, smemBytes, st>>>(mapA, mapWhi, mapWlo, q);                             \
   } while (0)
-  switch (epi) {   // the combinations the GCN path produces; anything else takes the generic kernel
+  switch (tc_instance(epi)) {
     case 0: ROC_TC_LAUNCH(0); break;
     case EPI_NORM: ROC_TC_LAUNCH(EPI_NORM); break;
     case EPI_OMASK: ROC_TC_LAUNCH(EPI_OMASK); break;
@@ -267,7 +273,8 @@ static int tc_launch(dim3 grid, size_t smemBytes, int epi, const CUtensorMap& ma
 
 // Y[rows][N] (op)= A[rows][K] * B^T with B(n, k) taken from W as k_split_w describes
 static int ts_gemm(int64_t rows, int K, int N, const float* A, int64_t ldA, const float* W, int ldW, int transposed,
-                   float* Y, int64_t ldY, const DropMask* inMask, const TsEpilogue& e, cudaStream_t st) {
+                   float* Y, int64_t ldY, const DropMask* inMask, const TsEpilogue& e, cudaStream_t st,
+                   roc_gemm_info* info) {
   if (K < 8 || N < 1 || rows < 1) return ROC_ERR_UNSUPPORTED;
   if ((ldA % 4) || (ldY % 4) || !aligned16(A) || !aligned16(Y)) return ROC_ERR_UNSUPPORTED;
   if (e.reluOf && ((e.ldR % 4) || !aligned16(e.reluOf))) return ROC_ERR_UNSUPPORTED;
@@ -319,6 +326,10 @@ static int ts_gemm(int64_t rows, int K, int N, const float* A, int64_t ldA, cons
   dim3 grid((unsigned)gx, (unsigned)nTiles, 1);
   const int epi = (q.relu ? EPI_RELU : 0) | (q.omask ? EPI_OMASK : 0) | (q.reluOf ? EPI_RELUOF : 0) |
                   (q.rowEnd ? EPI_NORM : 0) | (q.accumulate ? EPI_ACC : 0);
+  if (info) {
+    info->nc = NC; info->epi = tc_instance(epi); info->grid_x = (int)grid.x; info->grid_y = (int)grid.y;
+    info->stages = stages;
+  }
   switch (NC) {
     case 1: return tc_launch<1>(grid, smemBytes, epi, mapA, mapWhi, mapWlo, q, st);
     case 2: return tc_launch<2>(grid, smemBytes, epi, mapA, mapWhi, mapWlo, q, st);
@@ -328,20 +339,20 @@ static int ts_gemm(int64_t rows, int K, int N, const float* A, int64_t ldA, cons
 
 int tc_linear_fwd(int64_t rows, int inDim, int outDim, const float* X, int64_t ldX, const float* W, float* Y,
                   int64_t ldY, int relu, const uint64_t* rowEnd, uint64_t colLeft, const DropMask* dm,
-                  cudaStream_t st) {
+                  cudaStream_t st, roc_gemm_info* info) {
   TsEpilogue e;
   e.relu = relu; e.rowEnd = rowEnd; e.colLeft = colLeft;
-  return ts_gemm(rows, inDim, outDim, X, ldX, W, inDim, 0, Y, ldY, dm, e, st);
+  return ts_gemm(rows, inDim, outDim, X, ldX, W, inDim, 0, Y, ldY, dm, e, st, info);
 }
 
 // dX (+)= dY W, optionally followed in the epilogue by the dropout backward of X's producer
 int tc_linear_dx(int64_t rows, int inDim, int outDim, const float* dY, int64_t ldDY, const float* W, float* dX,
                  int64_t ldDX, int accumulate, const DropMask* dm, const float* reluOf, int64_t ldR,
-                 const uint64_t* rowEnd, uint64_t colLeft, cudaStream_t st) {
+                 const uint64_t* rowEnd, uint64_t colLeft, cudaStream_t st, roc_gemm_info* info) {
   TsEpilogue e;
   e.outMask = dm; e.accumulate = accumulate;
   e.reluOf = reluOf; e.ldR = ldR; e.rowEnd = rowEnd; e.colLeft = colLeft;
-  return ts_gemm(rows, outDim, inDim, dY, ldDY, W, inDim, 1, dX, ldDX, nullptr, e, st);
+  return ts_gemm(rows, outDim, inDim, dY, ldDY, W, inDim, 1, dX, ldDX, nullptr, e, st, info);
 }
 
 }  // namespace roc

@@ -213,7 +213,8 @@ static int dw_launch(const DwPlan& q, const CUtensorMap& mapX, const CUtensorMap
 }
 
 int tc_linear_dw(int64_t rows, int inDim, int outDim, const float* X, int64_t ldX, const float* dY, int64_t ldDY,
-                 float* dW, float* workspace, size_t wsBytes, const DropMask* dm, cudaStream_t st) {
+                 float* dW, float* workspace, size_t wsBytes, const DropMask* dm, cudaStream_t st,
+                 roc_gemm_info* info) {
   DwPlan q;
   if (tc_dw_plan(rows, inDim, outDim, &q) != ROC_OK) return ROC_ERR_UNSUPPORTED;
   if ((ldX % 4) || (ldDY % 4) || !aligned16(X) || !aligned16(dY)) return ROC_ERR_UNSUPPORTED;
@@ -230,6 +231,10 @@ int tc_linear_dw(int64_t rows, int inDim, int outDim, const float* X, int64_t ld
   t.ws = workspace; t.rows = rows; t.inDim = inDim; t.outDim = outDim; t.stages = q.stages;
   t.vPerSplit = ((rows + q.splits - 1) / q.splits + DW_KS - 1) / DW_KS * DW_KS;
   if (dm) { t.mask = dm->bits; t.ldm = dm->ld; t.mscale = dm->scale; }
+  if (info) {
+    info->nc = q.NC; info->epi = 0; info->grid_x = q.splits; info->grid_y = q.MT; info->stages = q.stages;
+    info->splits = q.splits; info->v_per_split = t.vPerSplit;
+  }
   int rc;
   switch (q.NC) {
     case 1: rc = dw_launch<1>(q, mapX, mapDY, t, st); break;

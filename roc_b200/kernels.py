@@ -243,8 +243,9 @@ def linear_bwd_dropout(x, w, y, dy, dw, mask, rate, dx=None, activation=0, accum
 
 
 def linear_bwd_fused(x, w, y, dy, dw, dx, activation=0, mask=None, rate=0.0, relu_of=None, norm_row_end=None,
-                     col_left=0):
-    """roc_linear_bwd_fused: dX epilogue = dropout backward -> relu mask (relu_of > 0) -> / sqrt(deg)."""
+                     col_left=0, accumulate_dx=False, parts=0):
+    """roc_linear_bwd_fused: dX epilogue = dropout backward -> relu mask (relu_of > 0) -> / sqrt(deg) [-> += dx].
+    parts = 1 / 2 computes only dX / only dW (ROC_LINEAR_BWD_ONLY_DX / _ONLY_DW); dx may be None without dX."""
     ws_bytes = lib.roc_linear_bwd_workspace_bytes(x.shape[0], x.shape[1], w.shape[0])
     ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=x.device)
     a = _lib.LinearBwdArgs()
@@ -252,8 +253,9 @@ def linear_bwd_fused(x, w, y, dy, dw, dx, activation=0, mask=None, rate=0.0, rel
     a.X, a.ldX, a.W = x.data_ptr(), _ld(x), w.data_ptr()
     a.Y, a.ldY = (y.data_ptr(), _ld(y)) if y is not None else (None, 0)
     a.dY, a.ldDY, a.dW = dy.data_ptr(), _ld(dy), dw.data_ptr()
-    a.dX, a.ldDX = dx.data_ptr(), _ld(dx)
-    a.activation, a.accumulate_dX = activation, 0
+    a.dX, a.ldDX = (dx.data_ptr(), _ld(dx)) if dx is not None else (None, 0)
+    a.activation, a.accumulate_dX = activation, int(accumulate_dx)
+    a.parts = parts
     a.workspace, a.workspaceBytes = ws.data_ptr(), ws_bytes
     if mask is not None:
         a.dropMask, a.ldMask = mask.data_ptr(), mask.stride(0)

@@ -36,22 +36,42 @@ def test_no_undeclared_prototypes():
 
 
 def test_struct_layouts_match_the_header(tmp_path):
-    """The ctypes mirrors of the C structs (roc_linear_bwd_args, roc_perf_metrics) have the C layout:
+    """The ctypes mirrors of the C structs (roc_linear_bwd_args, roc_gemm_info, roc_perf_metrics) have the C layout:
     a tiny C program compiled against include/roc_b200.h prints sizeof / offsetof of every field."""
-    fields = [f for f, _ in _lib.LinearBwdArgs._fields_]
-    prog = ['#include <stdio.h>', '#include <stddef.h>', '#include "roc_b200.h"', 'int main(void) {',
-            '  printf("%zu\\n", sizeof(roc_linear_bwd_args));']
-    prog += ['  printf("%%zu\\n", offsetof(roc_linear_bwd_args, %s));' % f for f in fields]
+    structs = [("roc_linear_bwd_args", _lib.LinearBwdArgs), ("roc_gemm_info", _lib.GemmInfo)]
+    prog = ['#include <stdio.h>', '#include <stddef.h>', '#include "roc_b200.h"', 'int main(void) {']
+    for cname, py in structs:
+        prog += ['  printf("%%zu\\n", sizeof(%s));' % cname]
+        prog += ['  printf("%%zu\\n", offsetof(%s, %s));' % (cname, f) for f, _ in py._fields_]
     prog += ['  printf("%zu\\n", sizeof(roc_perf_metrics));', '  return 0;', '}']
     src = tmp_path / "layout.c"
     src.write_text("\n".join(prog))
     exe = tmp_path / "layout"
     subprocess.run(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)], check=True)
     out = [int(x) for x in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split()]
-    assert out[0] == C.sizeof(_lib.LinearBwdArgs)
-    for f, off in zip(fields, out[1:1 + len(fields)]):
-        assert getattr(_lib.LinearBwdArgs, f).offset == off, f
+    pos = 0
+    for cname, py in structs:
+        assert out[pos] == C.sizeof(py), cname
+        for f, _ in py._fields_:
+            pos += 1
+            assert getattr(py, f).offset == out[pos], (cname, f)
+        pos += 1
+    assert pos == len(out) - 1
     assert out[-1] == C.sizeof(_lib.PerfMetrics)
+
+
+def test_gemm_info_hook_without_a_gemm():
+    """roc_last_gemm_info rejects a bad kind and reports "none yet" on a thread that has run no Linear."""
+    info = _lib.GemmInfo()
+    assert _lib.lib.roc_last_gemm_info(3, C.byref(info)) == _lib.ROC_ERR_INVALID
+    assert _lib.lib.roc_last_gemm_info(0, None) == _lib.ROC_ERR_INVALID
+    import threading
+    got = []
+    t = threading.Thread(target=lambda: got.append(_lib.last_gemm_info(1)))
+    t.start()
+    t.join()
+    assert got == [{k: 0 for k, _ in _lib.GemmInfo._fields_}]
+    assert _lib.lib.roc_last_gemm_path(1) in (0, 1, 2) and _lib.lib.roc_last_gemm_path(7) == 0
 
 
 def test_library_is_sm90a_only():

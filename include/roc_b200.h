@@ -113,7 +113,7 @@ int roc_build_csr(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft,
 /* -------------------------------------------------------- ScatterGather --- */
 
 /* A plan holds the edge-balanced schedule for one partition's CSR: 64-edge
- * chunks, the first row of each chunk, carry slots for rows longer than a
+ * chunks, a start record per chunk, carry slots for rows longer than a
  * chunk.  It is a private, derived structure; rowEnd/colSrc stay the canonical
  * CSR and must outlive the plan.  Creation synchronises the stream. */
 typedef struct roc_sg_plan roc_sg_plan;
@@ -138,9 +138,8 @@ int roc_sg_plan_rows_sorted(const roc_sg_plan* plan, int* sorted, roc_stream_t s
  *   out[v-rowLeft][h] = sum_{e in in(v)} in[colSrc[e]][h],  h < H
  * `in` is indexed by whatever ids colSrc holds (global ids over the whole
  * [N][ldIn] matrix as in scattergather.cc:69-73, or local+halo ids).
- * Deterministic: the per-row summation order is fixed by the plan — and is the same in every kernel variant the
- * library may pick for a width (registers / cp.async / TMA bulk-copy rings; ROC_SG_VARIANT forces one), so results
- * do not depend on the variant either. */
+ * Deterministic: the per-row summation order is fixed by the plan and no atomics are used, so the same call on
+ * the same inputs gives the same bits every time. */
 int roc_sg_forward_planned(const roc_sg_plan* plan, int H, const float* in,
                            int64_t ldIn, float* out, int64_t ldOut, int epilogue,
                            roc_stream_t stream);
@@ -152,7 +151,7 @@ int roc_sg_forward_planned(const roc_sg_plan* plan, int H, const float* in,
  * A row starts with its first edge's value and id; a later value replaces them only if it is strictly greater
  * (smaller) or it is NaN and the current value is not, so NaN propagates as in torch.amax.  A row of degree 0 gets
  * out = 0 and arg = 0xFFFFFFFF.  Exact (no rounding) and independent of how the plan cuts rows into chunks.
- * `in` is indexed like roc_sg_forward_planned's.  Kernel A (registers) only: ROC_SG_VARIANT does not apply.
+ * `in` is indexed like roc_sg_forward_planned's.
  * ROC_ERR_INVALID for an aggr other than MAX / MIN, a NULL pointer or a leading dimension < H. */
 int roc_sg_minmax_forward_planned(const roc_sg_plan* plan, int aggr, int H, const float* in, int64_t ldIn,
                                   float* out, int64_t ldOut, roc_vid_t* arg, int64_t ldArg, roc_stream_t stream);

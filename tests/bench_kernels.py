@@ -50,7 +50,6 @@ def main():
     ap.add_argument("--epi", type=int, default=0, help="ROC_SG_EPI_* flags for our kernel")
     ap.add_argument("--zero-rows", type=float, default=0.0, help="fraction of input rows set to zero")
     ap.add_argument("--scale-in", type=float, default=1.0, help="multiply the input (e.g. 1e-30 for tiny values)")
-    ap.add_argument("--variants", default="", help="comma list of ROC_SG_VARIANT[:ROC_SG_TCFG] to time, e.g. a,c,t,t:1,b")
     a = ap.parse_args()
     dev = "cuda"
     if a.graph == "rmat":
@@ -75,22 +74,6 @@ def main():
             x[torch.rand(n, device=dev) < a.zero_rows] = 0
         out = K.padded(n, h, dev)
         plan.reserve(h)
-        if a.variants:
-            base = None
-            for spec in a.variants.split(","):
-                v, _, cfg = spec.partition(":")
-                os.environ["ROC_SG_VARIANT"] = v
-                if cfg:
-                    os.environ["ROC_SG_TCFG"] = cfg
-                else:
-                    os.environ.pop("ROC_SG_TCFG", None)
-                ms = timeit(lambda: plan.forward(x, out=out, epilogue=a.epi), a.iters, flush)
-                if base is None:
-                    base = out.clone()
-                print(json.dumps({"H": h, "variant": spec, "ms": round(ms, 4), "GBps": round(sg_bytes(n, e, h) / ms / 1e6, 1),
-                                  "same_bits_as_first": bool(torch.equal(out, base))}), flush=True)
-            os.environ.pop("ROC_SG_VARIANT", None)
-            os.environ.pop("ROC_SG_TCFG", None)
         ms = timeit(lambda: plan.forward(x, out=out, epilogue=a.epi), a.iters, flush)
         rec = {"H": h, "ours_ms": ms, "ours_GBps": sg_bytes(n, e, h) / ms / 1e6, "ours_Gedges_s": e / ms / 1e6}
         if use_ref and h <= 512:

@@ -1,4 +1,4 @@
-"""make_golden_sg.py — ScatterGather golden rows at the widths the kernel variants split on, minted on the GPU from
+"""make_golden_sg.py — ScatterGather golden rows at four widths (16 to 256 floats), minted on the GPU from
 the REFERENCE's own aggre_coop_kernel (oracle/_ref, scattergather_kernel.cu:20-76).
 
     python tests/golden/make_golden_sg.py [out.npz]        # needs a GPU and oracle/_ref/libroc_ref.so

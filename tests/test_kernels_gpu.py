@@ -45,7 +45,7 @@ def graph(kind):
 
 
 @pytest.mark.parametrize("kind", ["uniform", "rmat", "dense", "ragged", "single"])
-@pytest.mark.parametrize("h", [1, 4, 16, 41, 64, 100, 128, 256, 602])
+@pytest.mark.parametrize("h", [1, 4, 16, 41, 64, 100, 128, 200, 256, 602])
 def test_sg_planned_vs_oracle(kind, h):
     row_end, col = graph(kind)
     n = row_end.shape[0]
@@ -65,55 +65,46 @@ def test_sg_planned_vs_oracle(kind, h):
 
 
 @pytest.mark.parametrize("kind", ["uniform", "rmat", "dense", "ragged", "single"])
-@pytest.mark.parametrize("h", [4, 16, 41, 64, 100, 128, 200, 256, 602])
-def test_sg_variants_are_bitwise_identical(kind, h, monkeypatch):
-    """The register (A), cp.async (C), TMA bulk-copy (T) and producer/consumer ring (R) kernels share
-    the chunk plan and the per-row summation order, so they must agree bit for bit — with every ring shape of
-    variant T, every CTA-range split of variant R and with the fused epilogue — and the TMA paths must meet
-    the oracle exactly like the others."""
+@pytest.mark.parametrize("h", [65, 80, 100, 128, 129, 160, 200, 232, 256])
+def test_sg_variants_are_bitwise_identical(kind, h):
+    """Vectorised rows of 65..256 floats run on the bulk-copy ring kernel (sg_chunk_kernel_t: lane-held ids up to
+    128 floats, ids per stage above), every other width on the register kernel (sg_chunk_kernel).  Both follow the
+    plan's per-row summation order, so the ring kernel's result must equal, bit for bit, the first h columns of a
+    register-kernel launch at 512 floats over the same rows, with and without the fused epilogue."""
     row_end, col = graph(kind)
     n = row_end.shape[0]
-    x = np.random.RandomState(h).randn(n, h).astype(np.float32)
+    x = torch.from_numpy(np.random.RandomState(h).randn(n, 512).astype(np.float32)).to(DEV)
     d_re, d_col = to_dev(row_end, col)
     plan = K.SgPlan(0, n - 1, 0, d_re, d_col)
-    xp = K.padded(n, h, DEV, fill=torch.from_numpy(x).to(DEV))
-    monkeypatch.setenv("ROC_SG_VARIANT", "a")
-    base = plan.forward(xp).clone()
-    base_e = plan.forward(xp, epilogue=_lib.SG_EPI_NORM | _lib.SG_EPI_RELU).clone()
-    rel_close(base.cpu().numpy(), oracle.scatter_gather(0, n - 1, 0, row_end, col, x), what="A %s H=%d" % (kind, h))
-    for variant, cfgs in (("c", [None]), ("r", [None, 1, 4]), ("t", [None, 1, 2, 3, 4, 5, 6]), ("u", [None, 1, 2, 3]),
-                          ("b", [None, 1, 3])):
-        monkeypatch.setenv("ROC_SG_VARIANT", variant)
-        for cfg in cfgs:
-            if cfg is None:
-                monkeypatch.delenv("ROC_SG_TCFG", raising=False)
-            else:
-                monkeypatch.setenv("ROC_SG_TCFG", str(cfg))
-            got = plan.forward(xp)
-            got_e = plan.forward(xp, epilogue=_lib.SG_EPI_NORM | _lib.SG_EPI_RELU)
-            torch.cuda.synchronize()
-            assert torch.equal(got, base), "variant %s cfg %s differs from A (%s, H=%d)" % (variant, cfg, kind, h)
-            # as bit patterns: rows of degree 0 are 0 / sqrt(0) = NaN under the norm epilogue (quirk Q5)
-            assert torch.equal(got_e.contiguous().view(torch.int32), base_e.contiguous().view(torch.int32)), \
-                "variant %s cfg %s epilogue differs (%s, H=%d)" % (variant, cfg, kind, h)
-    monkeypatch.delenv("ROC_SG_TCFG", raising=False)
-    monkeypatch.delenv("ROC_SG_VARIANT", raising=False)
+    epi = _lib.SG_EPI_NORM | _lib.SG_EPI_RELU
+    wide, wide_e = plan.forward(x), plan.forward(x, epilogue=epi)
+    got, got_e = plan.forward(x[:, :h]), plan.forward(x[:, :h], epilogue=epi)     # ld = 512: the vector path
+    torch.cuda.synchronize()
+    assert torch.equal(got, wide[:, :h]), "ring kernel differs from the register kernel (%s, H=%d)" % (kind, h)
+    # as bit patterns: rows of degree 0 are 0 / sqrt(0) = NaN under the norm epilogue (quirk Q5)
+    assert torch.equal(got_e.contiguous().view(torch.int32), wide_e[:, :h].contiguous().view(torch.int32)), \
+        "ring kernel epilogue differs (%s, H=%d)" % (kind, h)
 
 
-@pytest.mark.parametrize("kind", ["uniform", "rmat", "dense"])
+@pytest.mark.parametrize("kind", ["uniform", "rmat", "dense", "ragged", "single"])
 def test_sg_epilogues(kind):
+    """The fused norm (and relu) must equal the oracle's norm applied to the kernel's own sum, at every kernel shape
+    (register and ring kernels, vector and scalar paths, one and two column blocks).  Rows of degree 0 are
+    0 / sqrt(0) = NaN under the norm (quirk Q5), so NaNs compare equal; their bit patterns may differ."""
     row_end, col = graph(kind)
-    n, h = row_end.shape[0], 64
-    x = np.random.RandomState(1).randn(n, h).astype(np.float32)
+    n = row_end.shape[0]
     d_re, d_col = to_dev(row_end, col)
     plan = K.SgPlan(0, n - 1, 0, d_re, d_col)
-    xd = torch.from_numpy(x).to(DEV)
-    raw = plan.forward(xd).cpu().numpy()
-    normed = oracle.indegree_norm(0, n - 1, 0, row_end, raw)
-    got = plan.forward(xd, epilogue=_lib.SG_EPI_NORM).cpu().numpy()
-    assert np.array_equal(got, normed), "fused norm must equal norm applied to the kernel's own sum"
-    got = plan.forward(xd, epilogue=_lib.SG_EPI_NORM | _lib.SG_EPI_RELU).cpu().numpy()
-    assert np.array_equal(got, np.maximum(normed, 0))
+    for h in (4, 16, 41, 64, 100, 128, 200, 256, 602):
+        x = np.random.RandomState(1).randn(n, h).astype(np.float32)
+        xd = torch.from_numpy(x).to(DEV)
+        raw = plan.forward(xd).cpu().numpy()
+        normed = oracle.indegree_norm(0, n - 1, 0, row_end, raw)
+        got = plan.forward(xd, epilogue=_lib.SG_EPI_NORM).cpu().numpy()
+        assert np.array_equal(got, normed, equal_nan=True), \
+            "fused norm must equal norm applied to the kernel's own sum (%s, H=%d)" % (kind, h)
+        got = plan.forward(xd, epilogue=_lib.SG_EPI_NORM | _lib.SG_EPI_RELU).cpu().numpy()
+        assert np.array_equal(got, np.maximum(normed, 0), equal_nan=True), "fused norm + relu (%s, H=%d)" % (kind, h)
 
 
 def test_sg_partition_slices_and_planless_abi():
@@ -493,8 +484,8 @@ SG_GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "
 
 
 def test_side_by_side_with_reference_kernel():
-    """R-MAT scale 14 at the widths the variants split on, against the reference's aggre_coop_kernel: the stored
-    rows of tests/golden/make_golden_sg.py always, and the whole output live when oracle/_ref is built."""
+    """R-MAT scale 14 at 16 / 64 / 128 / 256 floats, against the reference's aggre_coop_kernel: the stored rows of
+    tests/golden/make_golden_sg.py always, and the whole output live when oracle/_ref is built."""
     sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
     from make_golden_sg import graph, features
     row_end, col = graph()

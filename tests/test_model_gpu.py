@@ -183,8 +183,8 @@ def test_file_loaders_and_driver(tmp_path):
 
 
 def test_cfg5_shape_residual_wide_hidden_dense_graph():
-    """BASELINE.json configs[4] at a reduced size: 4 layers + the residual branch (5 dims), hidden 256 (the TMA
-    ring ScatterGather variant), dropout, on a graph whose every row is cut at chunk boundaries (mean degree
+    """BASELINE.json configs[4] at a reduced size: 4 layers + the residual branch (5 dims), hidden 256 (the bulk-copy
+    ring ScatterGather kernel), dropout, on a graph whose every row is cut at chunk boundaries (mean degree
     ~150: carries + fix-up on every row)."""
     layers = (40, 256, 256, 256, 9)
     re_t, col_t = datasets.powerlaw_graph(600, 60000, seed=4)

@@ -24,8 +24,9 @@
 //  * vectorised rows of 65..256 floats run on sg_chunk_kernel_t instead, which fetches them with cp.async.bulk
 //    copies into a shared-memory ring: it was faster there on a products-shaped graph (DESIGN.md §3.1).  It
 //    shares the plan and the per-row summation order, so its results are bit-identical to sg_chunk_kernel's.
-//  * min / max aggregation (roc_sg_minmax_*) runs the same kernel templated on the reduction, with its own fix-ups
-//    for the forward; its backward is the sum schedule with a second gathered row and a predicated add.
+//  * min / max aggregation (roc_sg_minmax_*) runs the same kernel and fix-ups templated on the reduction; its
+//    backward is the sum schedule with a second gathered row and a predicated add, finished by the sum's fix-ups.
+//    The three planned entry points check their arguments and share one column-block driver (run_planned).
 //
 // Algorithmic bytes per launch (DESIGN.md): E*(4H+4) + Nloc*(4H+8); min / max forward E*(4H+4) + Nloc*(8H+8),
 // backward E*(8H+4) + Nloc*(4H+8).
@@ -711,12 +712,24 @@ sg_chunk_kernel_t(const SgParams p) {
   while (cur + 1 < r1) { advance(); flush(); }
 }
 
-// ----------------------------------------------------------- fix-up kernel ---
-// One worker per heavy row: out[R] = epilogue(out[R] + sum_k carry[slot0 + k]), k ascending.
-template <int VEC, int L, int NCH, int U>
+// ---------------------------------------------------------- fix-up kernels ---
+// A row cut at chunk boundaries is finished from its owner's partial (out[R]; arg[R] for MAX / MIN) and its carries,
+// taken in chunk order: added for the sum (whose partials include the min / max backward's), combined by the
+// ordering rule for MAX / MIN.  Only the sum has an epilogue.
+// U carries are loaded per batch.  The carries are taken in chunk order whatever U is, so U never changes a result;
+// MAX / MIN take fewer per batch where their index carries would otherwise spill.
+__host__ __device__ constexpr int sg_fixup_u(int L, int NCH, int RED) {
+  return RED == SG_RED_SUM ? (NCH == 1 ? (L == 4 ? 4 : 8) : 8 / NCH) : (NCH <= 2 ? 4 : 1);
+}
+
+// One worker per heavy row.
+template <int VEC, int L, int NCH, int RED>
 __global__ void __launch_bounds__(SG_THREADS)
 sg_fixup_kernel(const SgParams p) {
   typedef typename V<VEC>::T T;
+  typedef typename V<VEC>::I I;
+  constexpr bool MM = RED != SG_RED_SUM;
+  constexpr int U = sg_fixup_u(L, NCH, RED);
   constexpr int WPB = SG_THREADS / L;
   constexpr uint32_t CH = SG_CH;
   const int lane = threadIdx.x % L;
@@ -729,151 +742,68 @@ sg_fixup_kernel(const SgParams p) {
   const uint32_t slot0 = p.carryIdx[c0 + 1];
   T* dst = reinterpret_cast<T*>(p.out) + (size_t)R * p.ldOut;
   const T* cbase = reinterpret_cast<const T*>(p.carry) + (size_t)slot0 * p.ldC;
+  I* adst = reinterpret_cast<I*>(p.arg) + (size_t)R * p.ldArg;
+  const I* abase = reinterpret_cast<const I*>(p.carryArg) + (size_t)slot0 * p.ldC;
   bool act[NCH];
   T acc[NCH];
+  I ai[NCH];
 #pragma unroll
   for (int ch = 0; ch < NCH; ch++) {
     act[ch] = (uint32_t)(lane + ch * L) < p.Q;
     acc[ch] = act[ch] ? V<VEC>::ld_plain(dst + lane + ch * L) : V<VEC>::zero();
+    if constexpr (MM) ai[ch] = act[ch] ? adst[lane + ch * L] : mm_noarg((I*)nullptr);
   }
   for (uint32_t k = 0; k < n; k += U) {
     T v[U][NCH];
+    I vi[MM ? U : 1][MM ? NCH : 1];
 #pragma unroll
     for (int u = 0; u < U; u++)
 #pragma unroll
-      for (int ch = 0; ch < NCH; ch++)
-        v[u][ch] = (k + u < n && act[ch]) ? V<VEC>::ld_plain(cbase + (size_t)(k + u) * p.ldC + lane + ch * L)
-                                          : V<VEC>::zero();
-#pragma unroll
-    for (int u = 0; u < U; u++)
-      if (k + u < n)
-#pragma unroll
-        for (int ch = 0; ch < NCH; ch++) V<VEC>::add(acc[ch], v[u][ch]);
-  }
-#pragma unroll
-  for (int ch = 0; ch < NCH; ch++)
-    if (act[ch]) epi_store<VEC>(acc[ch], dst + lane + ch * L, t - s, p.epi);
-}
-
-// Rows with more than SG_BIG carries (hubs: R-MAT-22's largest row spans 1 524 chunks) get a
-// whole CTA: each of the 256/L lane groups sums a contiguous block of the carries, the blocks
-// are combined in order through shared memory.  With one worker per row the hubs' serial
-// chains set the kernel's duration.
-constexpr uint32_t SG_BIG = 32;
-
-template <int VEC, int L, int NCH, int U>
-__global__ void __launch_bounds__(SG_THREADS)
-sg_fixup_big_kernel(const SgParams p) {
-  typedef typename V<VEC>::T T;
-  constexpr int WPB = SG_THREADS / L;
-  constexpr uint32_t CH = SG_CH;
-  __shared__ __align__(16) float part[WPB * NCH * L * VEC];
-  const int lane = threadIdx.x % L;
-  const int g = threadIdx.x / L;
-  const uint32_t R = p.bigRows[blockIdx.x];
-  const uint32_t s = p.rs[R], t = p.rs[R + 1];
-  const uint32_t c0 = s / CH, cLast = (t - 1) / CH;
-  const uint32_t n = cLast - c0;
-  const uint32_t slot0 = p.carryIdx[c0 + 1];
-  const T* cbase = reinterpret_cast<const T*>(p.carry) + (size_t)slot0 * p.ldC;
-  const uint32_t per = (n + WPB - 1) / WPB;
-  const uint32_t k0 = min(n, (uint32_t)g * per), k1 = min(n, k0 + per);
-  bool act[NCH];
-  T acc[NCH];
-#pragma unroll
-  for (int ch = 0; ch < NCH; ch++) { act[ch] = (uint32_t)(lane + ch * L) < p.Q; acc[ch] = V<VEC>::zero(); }
-  for (uint32_t k = k0; k < k1; k += U) {
-    T v[U][NCH];
-#pragma unroll
-    for (int u = 0; u < U; u++)
-#pragma unroll
-      for (int ch = 0; ch < NCH; ch++)
-        v[u][ch] = (k + u < k1 && act[ch]) ? V<VEC>::ld_plain(cbase + (size_t)(k + u) * p.ldC + lane + ch * L)
-                                           : V<VEC>::zero();
-#pragma unroll
-    for (int u = 0; u < U; u++)
-#pragma unroll
-      for (int ch = 0; ch < NCH; ch++) V<VEC>::add(acc[ch], v[u][ch]);
-  }
-  T* sp = reinterpret_cast<T*>(part);
-#pragma unroll
-  for (int ch = 0; ch < NCH; ch++) sp[(g * NCH + ch) * L + lane] = acc[ch];
-  __syncthreads();
-  if (g == 0) {
-    T* dst = reinterpret_cast<T*>(p.out) + (size_t)R * p.ldOut;
-#pragma unroll
-    for (int ch = 0; ch < NCH; ch++) {
-      if (act[ch]) {
-        T a = V<VEC>::ld_plain(dst + lane + ch * L);      // the owner chunk's raw partial
-        for (int gg = 0; gg < WPB; gg++) V<VEC>::add(a, sp[(gg * NCH + ch) * L + lane]);
-        epi_store<VEC>(a, dst + lane + ch * L, t - s, p.epi);
+      for (int ch = 0; ch < NCH; ch++) {
+        if constexpr (MM) {
+          const bool ok = k + u < n && act[ch];
+          v[u][ch] = ok ? V<VEC>::ld_plain(cbase + (size_t)(k + u) * p.ldC + lane + ch * L) : V<VEC>::zero();
+          vi[u][ch] = ok ? abase[(size_t)(k + u) * p.ldC + lane + ch * L] : mm_noarg((I*)nullptr);
+        } else {
+          v[u][ch] = (k + u < n && act[ch]) ? V<VEC>::ld_plain(cbase + (size_t)(k + u) * p.ldC + lane + ch * L)
+                                            : V<VEC>::zero();
+        }
       }
+#pragma unroll
+    for (int u = 0; u < U; u++)
+      if (MM || k + u < n)          // MAX / MIN: a carry past n has no index and is skipped
+#pragma unroll
+        for (int ch = 0; ch < NCH; ch++) {
+          if constexpr (MM) mm_combine<RED>(acc[ch], ai[ch], v[u][ch], vi[u][ch]);
+          else V<VEC>::add(acc[ch], v[u][ch]);
+        }
+  }
+#pragma unroll
+  for (int ch = 0; ch < NCH; ch++) {
+    if (act[ch]) {
+      if constexpr (MM) { V<VEC>::st(dst + lane + ch * L, acc[ch]); adst[lane + ch * L] = ai[ch]; }
+      else epi_store<VEC>(acc[ch], dst + lane + ch * L, t - s, p.epi);
     }
   }
 }
 
-// Min / max: one worker per heavy row takes the owner's partial (out[R], arg[R]), then the carries, k ascending,
-// with the same ordering rule.
-template <int VEC, int L, int NCH, int U, int RED>
-__global__ void __launch_bounds__(SG_THREADS)
-sg_fixup_minmax_kernel(const SgParams p) {
-  typedef typename V<VEC>::T T;
-  typedef typename V<VEC>::I I;
-  constexpr int WPB = SG_THREADS / L;
-  constexpr uint32_t CH = SG_CH;
-  const int lane = threadIdx.x % L;
-  const uint32_t w = blockIdx.x * WPB + threadIdx.x / L;
-  if (w >= p.numHeavy) return;
-  const uint32_t R = p.heavyRows[w];
-  const uint32_t s = p.rs[R], t = p.rs[R + 1];
-  const uint32_t c0 = s / CH, cLast = (t - 1) / CH;
-  const uint32_t n = cLast - c0;
-  const uint32_t slot0 = p.carryIdx[c0 + 1];
-  T* dst = reinterpret_cast<T*>(p.out) + (size_t)R * p.ldOut;
-  const T* cbase = reinterpret_cast<const T*>(p.carry) + (size_t)slot0 * p.ldC;
-  bool act[NCH];
-  T acc[NCH];
-  I* adst = reinterpret_cast<I*>(p.arg) + (size_t)R * p.ldArg;
-  const I* abase = reinterpret_cast<const I*>(p.carryArg) + (size_t)slot0 * p.ldC;
-  I ai[NCH];
-#pragma unroll
-  for (int ch = 0; ch < NCH; ch++) {
-    act[ch] = (uint32_t)(lane + ch * L) < p.Q;
-    acc[ch] = act[ch] ? V<VEC>::ld_plain(dst + lane + ch * L) : V<VEC>::zero();
-    ai[ch] = act[ch] ? adst[lane + ch * L] : mm_noarg((I*)nullptr);
-  }
-  for (uint32_t k = 0; k < n; k += U) {
-    T v[U][NCH];
-    I vi[U][NCH];
-#pragma unroll
-    for (int u = 0; u < U; u++)
-#pragma unroll
-      for (int ch = 0; ch < NCH; ch++) {
-        const bool ok = k + u < n && act[ch];
-        v[u][ch] = ok ? V<VEC>::ld_plain(cbase + (size_t)(k + u) * p.ldC + lane + ch * L) : V<VEC>::zero();
-        vi[u][ch] = ok ? abase[(size_t)(k + u) * p.ldC + lane + ch * L] : mm_noarg((I*)nullptr);
-      }
-#pragma unroll
-    for (int u = 0; u < U; u++)
-#pragma unroll
-      for (int ch = 0; ch < NCH; ch++) mm_combine<RED>(acc[ch], ai[ch], v[u][ch], vi[u][ch]);
-  }
-#pragma unroll
-  for (int ch = 0; ch < NCH; ch++)
-    if (act[ch]) { V<VEC>::st(dst + lane + ch * L, acc[ch]); adst[lane + ch * L] = ai[ch]; }
-}
+// Rows with more than SG_BIG carries (hubs: R-MAT-22's largest row spans 1 524 chunks) get a
+// whole CTA: each of the 256/L lane groups reduces a contiguous block of the carries, then group 0
+// takes the owner's partial and the groups' results in group order — chunk order again.  With one
+// worker per row the hubs' serial chains set the kernel's duration.
+constexpr uint32_t SG_BIG = 32;
 
-// Min / max rows with more than SG_BIG carries: each lane group reduces its block of carries in order, then group 0
-// takes the owner's partial and the groups' results in group order — chunk order again.
-template <int VEC, int L, int NCH, int U, int RED>
+template <int VEC, int L, int NCH, int RED>
 __global__ void __launch_bounds__(SG_THREADS)
-sg_fixup_big_minmax_kernel(const SgParams p) {
+sg_fixup_big_kernel(const SgParams p) {
   typedef typename V<VEC>::T T;
   typedef typename V<VEC>::I I;
+  constexpr bool MM = RED != SG_RED_SUM;
+  constexpr int U = sg_fixup_u(L, NCH, RED);
   constexpr int WPB = SG_THREADS / L;
   constexpr uint32_t CH = SG_CH;
   __shared__ __align__(16) float part[WPB * NCH * L * VEC];
-  __shared__ __align__(16) uint32_t parti[WPB * NCH * L * VEC];
+  __shared__ __align__(16) uint32_t parti[MM ? WPB * NCH * L * VEC : 1];   // MAX / MIN: the partials' indices
   const int lane = threadIdx.x % L;
   const int g = threadIdx.x / L;
   const uint32_t R = p.bigRows[blockIdx.x];
@@ -890,40 +820,56 @@ sg_fixup_big_minmax_kernel(const SgParams p) {
   I ai[NCH];
 #pragma unroll
   for (int ch = 0; ch < NCH; ch++) {
-    act[ch] = (uint32_t)(lane + ch * L) < p.Q; acc[ch] = V<VEC>::zero(); ai[ch] = mm_noarg((I*)nullptr);
+    act[ch] = (uint32_t)(lane + ch * L) < p.Q; acc[ch] = V<VEC>::zero();
+    if constexpr (MM) ai[ch] = mm_noarg((I*)nullptr);
   }
   for (uint32_t k = k0; k < k1; k += U) {
     T v[U][NCH];
-    I vi[U][NCH];
+    I vi[MM ? U : 1][MM ? NCH : 1];
 #pragma unroll
     for (int u = 0; u < U; u++)
 #pragma unroll
       for (int ch = 0; ch < NCH; ch++) {
-        const bool ok = k + u < k1 && act[ch];
-        v[u][ch] = ok ? V<VEC>::ld_plain(cbase + (size_t)(k + u) * p.ldC + lane + ch * L) : V<VEC>::zero();
-        vi[u][ch] = ok ? abase[(size_t)(k + u) * p.ldC + lane + ch * L] : mm_noarg((I*)nullptr);
+        if constexpr (MM) {
+          const bool ok = k + u < k1 && act[ch];
+          v[u][ch] = ok ? V<VEC>::ld_plain(cbase + (size_t)(k + u) * p.ldC + lane + ch * L) : V<VEC>::zero();
+          vi[u][ch] = ok ? abase[(size_t)(k + u) * p.ldC + lane + ch * L] : mm_noarg((I*)nullptr);
+        } else {
+          v[u][ch] = (k + u < k1 && act[ch]) ? V<VEC>::ld_plain(cbase + (size_t)(k + u) * p.ldC + lane + ch * L)
+                                            : V<VEC>::zero();
+        }
       }
 #pragma unroll
     for (int u = 0; u < U; u++)
 #pragma unroll
-      for (int ch = 0; ch < NCH; ch++) mm_combine<RED>(acc[ch], ai[ch], v[u][ch], vi[u][ch]);
+      for (int ch = 0; ch < NCH; ch++) {
+        if constexpr (MM) mm_combine<RED>(acc[ch], ai[ch], v[u][ch], vi[u][ch]);
+        else V<VEC>::add(acc[ch], v[u][ch]);
+      }
   }
   T* sp = reinterpret_cast<T*>(part);
   I* spi = reinterpret_cast<I*>(parti);
 #pragma unroll
-  for (int ch = 0; ch < NCH; ch++) { sp[(g * NCH + ch) * L + lane] = acc[ch]; spi[(g * NCH + ch) * L + lane] = ai[ch]; }
+  for (int ch = 0; ch < NCH; ch++) {
+    sp[(g * NCH + ch) * L + lane] = acc[ch];
+    if constexpr (MM) spi[(g * NCH + ch) * L + lane] = ai[ch];
+  }
   __syncthreads();
   if (g == 0) {
     T* dst = reinterpret_cast<T*>(p.out) + (size_t)R * p.ldOut;
     I* adst = reinterpret_cast<I*>(p.arg) + (size_t)R * p.ldArg;
 #pragma unroll
     for (int ch = 0; ch < NCH; ch++) {
-      if (act[ch]) {
-        T a = V<VEC>::ld_plain(dst + lane + ch * L);      // the owner chunk's partial
+      if (!act[ch]) continue;
+      T a = V<VEC>::ld_plain(dst + lane + ch * L);      // the owner chunk's partial
+      if constexpr (MM) {
         I ia = adst[lane + ch * L];
         for (int gg = 0; gg < WPB; gg++) mm_combine<RED>(a, ia, sp[(gg * NCH + ch) * L + lane], spi[(gg * NCH + ch) * L + lane]);
         V<VEC>::st(dst + lane + ch * L, a);
         adst[lane + ch * L] = ia;
+      } else {
+        for (int gg = 0; gg < WPB; gg++) V<VEC>::add(a, sp[(gg * NCH + ch) * L + lane]);
+        epi_store<VEC>(a, dst + lane + ch * L, t - s, p.epi);
       }
     }
   }
@@ -949,10 +895,10 @@ static int launch_ring(const SgParams& p, cudaStream_t st) {
 }
 
 // One ScatterGather launch: the main kernel (RING: sg_chunk_kernel_t), then the fix-ups of the rows it cut.  The
-// partials of the sum and of the min / max backward (MASK) are sums, so both use the sum fix-ups.
+// partials of the min / max backward (MASK) are sums, so it runs the sum's fix-ups.
 template <int VEC, int L, int NCH, int U, int MINB, int RED, bool RING = false>
 static int launch(const SgParams& p, cudaStream_t st) {
-  constexpr bool SUMS = RED == SG_RED_SUM || RED == SG_RED_MASK;
+  constexpr int FIX = RED == SG_RED_MASK ? SG_RED_SUM : RED;
   constexpr int WPB = SG_THREADS / L;
   if (p.numChunks) {
     if constexpr (RING) {
@@ -964,13 +910,11 @@ static int launch(const SgParams& p, cudaStream_t st) {
     }
   }
   if (p.numHeavy) {
-    if constexpr (SUMS) sg_fixup_kernel<VEC, L, NCH, U><<<(p.numHeavy + WPB - 1) / WPB, SG_THREADS, 0, st>>>(p);
-    else sg_fixup_minmax_kernel<VEC, L, NCH, U, RED><<<(p.numHeavy + WPB - 1) / WPB, SG_THREADS, 0, st>>>(p);
+    sg_fixup_kernel<VEC, L, NCH, FIX><<<(p.numHeavy + WPB - 1) / WPB, SG_THREADS, 0, st>>>(p);
     ROC_LAUNCH_CHECK();
   }
   if (p.numBig) {
-    if constexpr (SUMS) sg_fixup_big_kernel<VEC, L, NCH, U><<<p.numBig, SG_THREADS, 0, st>>>(p);
-    else sg_fixup_big_minmax_kernel<VEC, L, NCH, U, RED><<<p.numBig, SG_THREADS, 0, st>>>(p);
+    sg_fixup_big_kernel<VEC, L, NCH, FIX><<<p.numBig, SG_THREADS, 0, st>>>(p);
     ROC_LAUNCH_CHECK();
   }
   return ROC_OK;
@@ -1146,35 +1090,43 @@ static SgParams plan_params(const roc_sg_plan* pl) {
   return p;
 }
 
-extern "C" int roc_sg_forward_planned(const roc_sg_plan* plc, int H, const float* in, int64_t ldIn,
-                                      float* out, int64_t ldOut, int epilogue, roc_stream_t stream) {
-  roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
-  if (!pl || H <= 0 || !in || !out || ldIn < H || ldOut < H) return ROC_ERR_INVALID;
-  cudaStream_t st = as_stream(stream);
-  const bool vec = (ldIn % 4 == 0) && (ldOut % 4 == 0) && aligned16(in) && aligned16(out);
-  const int blockCols = vec ? 1024 : 256;     // the widest kernel: 256 T-columns
+// Reduction RED over the columns [0, H) of every row, in column blocks: 1,024 floats for the sum and 512 for min /
+// max when every leading dimension and pointer allows float4 rows, else 256.  `arg` holds the min / max indices
+// (written by the forward, gathered by the backward); the sum passes none.
+template <int RED>
+static int run_planned(roc_sg_plan* pl, int H, const float* in, int64_t ldIn, float* out, int64_t ldOut,
+                       const roc_vid_t* arg, int64_t ldArg, int epilogue, roc_vid_t selfBase, cudaStream_t st) {
+  const bool vec = (ldIn % 4 == 0) && (ldOut % 4 == 0) && (ldArg % 4 == 0) && aligned16(in) && aligned16(out) &&
+                   aligned16(arg);
+  const int vw = vec ? 4 : 1;                 // floats per T-column
+  const int blockCols = !vec ? 256 : RED == SG_RED_SUM ? 1024 : 512;
   {
     int need = H < blockCols ? H : blockCols;
     int rc = ensure_carry(pl, ((size_t)need + 3) / 4 * 4, st, true);
     if (rc != ROC_OK) return rc;
+    if constexpr (RED == SG_RED_MAX || RED == SG_RED_MIN) {
+      rc = ensure_carry_arg(pl, st);
+      if (rc != ROC_OK) return rc;
+    }
   }
   for (int c0 = 0; c0 < H; c0 += blockCols) {
     const int hb = (H - c0 < blockCols) ? H - c0 : blockCols;
     SgParams p = plan_params(pl);
-    p.in = in + c0; p.out = out + c0; p.epi = epilogue;
-    int rc;
-    if (vec) {
-      p.ldIn = (size_t)ldIn / 4; p.ldOut = (size_t)ldOut / 4; p.ldC = pl->carryLd / 4;
-      p.Q = ((uint32_t)hb + 3) / 4;
-      rc = dispatch<4, SG_RED_SUM>(p, st);
-    } else {
-      p.ldIn = (size_t)ldIn; p.ldOut = (size_t)ldOut; p.ldC = pl->carryLd;
-      p.Q = (uint32_t)hb;
-      rc = dispatch<1, SG_RED_SUM>(p, st);
-    }
+    p.in = in + c0; p.out = out + c0; p.epi = epilogue; p.selfBase = selfBase;
+    if (arg) p.arg = const_cast<roc_vid_t*>(arg) + c0;
+    p.ldIn = (size_t)ldIn / vw; p.ldOut = (size_t)ldOut / vw; p.ldArg = (size_t)ldArg / vw; p.ldC = pl->carryLd / vw;
+    p.Q = ((uint32_t)hb + vw - 1) / vw;
+    const int rc = vec ? dispatch<4, RED>(p, st) : dispatch<1, RED>(p, st);
     if (rc != ROC_OK) return rc;
   }
   return ROC_OK;
+}
+
+extern "C" int roc_sg_forward_planned(const roc_sg_plan* plc, int H, const float* in, int64_t ldIn,
+                                      float* out, int64_t ldOut, int epilogue, roc_stream_t stream) {
+  roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  if (!pl || H <= 0 || !in || !out || ldIn < H || ldOut < H) return ROC_ERR_INVALID;
+  return run_planned<SG_RED_SUM>(pl, H, in, ldIn, out, ldOut, nullptr, 0, epilogue, 0, as_stream(stream));
 }
 
 extern "C" int roc_sg_plan_rows_sorted(const roc_sg_plan* pl, int* sorted, roc_stream_t stream) {
@@ -1206,33 +1158,8 @@ extern "C" int roc_sg_minmax_forward_planned(const roc_sg_plan* plc, int aggr, i
       ldOut < H || ldArg < H)
     return ROC_ERR_INVALID;
   cudaStream_t st = as_stream(stream);
-  const bool vec = (ldIn % 4 == 0) && (ldOut % 4 == 0) && (ldArg % 4 == 0) && aligned16(in) && aligned16(out) &&
-                   aligned16(arg);
-  const int blockCols = vec ? 512 : 256;
-  {
-    int need = H < blockCols ? H : blockCols;
-    int rc = ensure_carry(pl, ((size_t)need + 3) / 4 * 4, st, true);
-    if (rc != ROC_OK) return rc;
-    rc = ensure_carry_arg(pl, st);
-    if (rc != ROC_OK) return rc;
-  }
-  for (int c0 = 0; c0 < H; c0 += blockCols) {
-    const int hb = (H - c0 < blockCols) ? H - c0 : blockCols;
-    SgParams p = plan_params(pl);
-    p.in = in + c0; p.out = out + c0; p.arg = arg + c0;
-    int rc;
-    if (vec) {
-      p.ldIn = (size_t)ldIn / 4; p.ldOut = (size_t)ldOut / 4; p.ldArg = (size_t)ldArg / 4; p.ldC = pl->carryLd / 4;
-      p.Q = ((uint32_t)hb + 3) / 4;
-      rc = aggr == ROC_SG_AGGR_MAX ? dispatch<4, SG_RED_MAX>(p, st) : dispatch<4, SG_RED_MIN>(p, st);
-    } else {
-      p.ldIn = (size_t)ldIn; p.ldOut = (size_t)ldOut; p.ldArg = (size_t)ldArg; p.ldC = pl->carryLd;
-      p.Q = (uint32_t)hb;
-      rc = aggr == ROC_SG_AGGR_MAX ? dispatch<1, SG_RED_MAX>(p, st) : dispatch<1, SG_RED_MIN>(p, st);
-    }
-    if (rc != ROC_OK) return rc;
-  }
-  return ROC_OK;
+  return aggr == ROC_SG_AGGR_MAX ? run_planned<SG_RED_MAX>(pl, H, in, ldIn, out, ldOut, arg, ldArg, 0, 0, st)
+                                 : run_planned<SG_RED_MIN>(pl, H, in, ldIn, out, ldOut, arg, ldArg, 0, 0, st);
 }
 
 extern "C" int roc_sg_minmax_backward_planned(const roc_sg_plan* plc, int H, roc_vid_t selfBase, const float* outGrad,
@@ -1240,32 +1167,7 @@ extern "C" int roc_sg_minmax_backward_planned(const roc_sg_plan* plc, int H, roc
                                               int64_t ldIn, roc_stream_t stream) {
   roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
   if (!pl || H <= 0 || !outGrad || !arg || !inGrad || ldG < H || ldArg < H || ldIn < H) return ROC_ERR_INVALID;
-  cudaStream_t st = as_stream(stream);
-  const bool vec = (ldG % 4 == 0) && (ldArg % 4 == 0) && (ldIn % 4 == 0) && aligned16(outGrad) && aligned16(arg) &&
-                   aligned16(inGrad);
-  const int blockCols = vec ? 512 : 256;
-  {
-    int need = H < blockCols ? H : blockCols;
-    int rc = ensure_carry(pl, ((size_t)need + 3) / 4 * 4, st, true);
-    if (rc != ROC_OK) return rc;
-  }
-  for (int c0 = 0; c0 < H; c0 += blockCols) {
-    const int hb = (H - c0 < blockCols) ? H - c0 : blockCols;
-    SgParams p = plan_params(pl);
-    p.in = outGrad + c0; p.out = inGrad + c0; p.arg = const_cast<roc_vid_t*>(arg) + c0; p.selfBase = selfBase;
-    int rc;
-    if (vec) {
-      p.ldIn = (size_t)ldG / 4; p.ldOut = (size_t)ldIn / 4; p.ldArg = (size_t)ldArg / 4; p.ldC = pl->carryLd / 4;
-      p.Q = ((uint32_t)hb + 3) / 4;
-      rc = dispatch<4, SG_RED_MASK>(p, st);
-    } else {
-      p.ldIn = (size_t)ldG; p.ldOut = (size_t)ldIn; p.ldArg = (size_t)ldArg; p.ldC = pl->carryLd;
-      p.Q = (uint32_t)hb;
-      rc = dispatch<1, SG_RED_MASK>(p, st);
-    }
-    if (rc != ROC_OK) return rc;
-  }
-  return ROC_OK;
+  return run_planned<SG_RED_MASK>(pl, H, outGrad, ldG, inGrad, ldIn, arg, ldArg, 0, selfBase, as_stream(stream));
 }
 
 extern "C" int roc_sg_forward(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft, int H,

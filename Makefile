@@ -42,6 +42,11 @@ oracle:
 sanitize: $(LIB)
 	tools/sanitize.sh
 
+# tensor-pipe rate of m64n32k8 against m64n64k8 / m64n128k8 (tf32, A from registers); needs a GPU to run
+$(BUILD)/bench_wgmma_n: tools/bench_wgmma_n.cu roc_b200/csrc/tc_common.cuh
+	@mkdir -p $(BUILD)
+	$(NVCC) $(ARCH) -O3 -std=c++17 -Iroc_b200/csrc $< -o $@
+
 clean:
 	rm -rf $(BUILD) $(LIB) $(BIN)
 	$(MAKE) -C oracle clean

@@ -395,9 +395,10 @@ int roc_last_gemm_path(int which);
  * a shape reached the kernel instantiation and pipeline regime it was chosen for.  On the SIMT path only `path` is
  * set, and for dW also `splits` / `v_per_split` (the rest is 0).  Tensor cores:
  *   nc        wgmma chunks of 32 columns per N tile (1, 2, 4; dW 1, 2, 4, 8)
- *   epi       forward / dX epilogue instantiation: its EPI bit mask, or -1 for the generic kernel (dW: 0)
+ *   epi       forward / dX epilogue instantiation: its EPI bit mask, or -1 for the generic kernel;  dW: the kernel,
+ *             1 the warp-specialised one (outDim <= 128), 0 the CTA-synchronised one (outDim > 128, ROC_B200_DW=sync)
  *   grid_x/y  forward / dX: persistent CTAs along the rows x N tiles;  dW: splits x 128-column M tiles
- *   stages    depth of the TMA ring
+ *   stages    depth of the TMA ring (dW: 32-vertex slots)
  *   splits, v_per_split   dW only: split-K ranges and the rows each holds (the partials are added in range order)
  * Returns ROC_ERR_INVALID for a bad `which` or a NULL `info`. */
 typedef struct {

@@ -1,6 +1,7 @@
 // linear.cu — C-ABI entry points of the Linear op and the kernel dispatcher.
 // Replaces Linear::forward_task / backward_task (linear_kernel.cu:19-118, 129-245).
 #include <cstdlib>
+#include <cstring>
 #include "common.cuh"
 
 namespace roc {
@@ -30,17 +31,31 @@ int tc_linear_dw(int64_t rows, int inDim, int outDim, const float* X, int64_t ld
                  float* dW, float* workspace, size_t wsBytes, const DropMask* dm, cudaStream_t st,
                  roc_gemm_info* info);
 
-// ROC_B200_GEMM=simt forces the exact-fp32 SIMT kernels (used by tests to
-// cross-check the tensor-core path).
-static bool force_simt() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("ROC_B200_GEMM"); v = (e && e[0] == 's' && e[1] == 'i') ? 1 : 0; }
-  return v == 1;
-}
 // which kernel served the calling thread's last Linear GEMM of each kind, and how it was launched (test hook: the
 // tensor-core path returns ROC_ERR_UNSUPPORTED for shapes it does not take and the dispatcher then uses SIMT — a test
 // that means to check the tensor cores, or one instantiation / pipeline regime of them, must be able to see that it did)
 static thread_local roc_gemm_info t_last[3] = {};   // fwd, dW, dX; path 0 none, 1 tensor cores (wgmma), 2 SIMT
+
+// GEMM `which` on the tensor cores, or on the exact-fp32 SIMT kernels when they do not take it (ROC_ERR_UNSUPPORTED)
+// or ROC_B200_GEMM=simt is set ("notc" is the same switch under its older name, still set by existing scripts and
+// tests).  The switch is read on every call, so a test can cross-check the two paths call by call.  Each path fills in
+// what it knows of its launch.
+template <class Tc, class Simt>
+static int run_gemm(int which, Tc&& tc, Simt&& simt) {
+  const char* e = getenv("ROC_B200_GEMM");
+  const bool forced = e && (strcmp(e, "simt") == 0 || strcmp(e, "notc") == 0);
+  roc_gemm_info info{};
+  int rc = forced ? ROC_ERR_UNSUPPORTED : tc(&info);
+  if (rc == ROC_ERR_UNSUPPORTED) {
+    info = roc_gemm_info{};
+    info.path = 2;
+    rc = simt(&info);
+  } else {
+    info.path = 1;
+  }
+  t_last[which] = info;
+  return rc;
+}
 }  // namespace roc
 
 using namespace roc;
@@ -65,14 +80,15 @@ static int linear_fwd_impl(int64_t rows, int inDim, int outDim, const float* X, 
   if (rows == 0) return ROC_OK;
   const uint64_t* re = (flags & ROC_LINEAR_NORM_EPILOGUE) ? rowEnd : nullptr;
   const int relu = activation == ROC_AC_MODE_RELU;
-  if (!force_simt()) {
-    roc_gemm_info info{};
-    int rc = tc_linear_fwd(rows, inDim, outDim, X, ldX, W, Y, ldY, relu, re, colLeft, dm, as_stream(stream), &info);
-    if (rc != ROC_ERR_UNSUPPORTED) { info.path = 1; t_last[0] = info; return rc; }
-  }
-  t_last[0] = roc_gemm_info{};
-  t_last[0].path = 2;
-  return simt_linear_fwd(rows, inDim, outDim, X, ldX, W, Y, ldY, relu, re, colLeft, dm, as_stream(stream));
+  cudaStream_t st = as_stream(stream);
+  return run_gemm(
+      0,
+      [&](roc_gemm_info* i) {
+        return tc_linear_fwd(rows, inDim, outDim, X, ldX, W, Y, ldY, relu, re, colLeft, dm, st, i);
+      },
+      [&](roc_gemm_info*) {
+        return simt_linear_fwd(rows, inDim, outDim, X, ldX, W, Y, ldY, relu, re, colLeft, dm, st);
+      });
 }
 
 extern "C" int roc_linear_fwd(int64_t rows, int inDim, int outDim, const float* X, int64_t ldX, const float* W,
@@ -121,33 +137,29 @@ static int linear_bwd_impl(int64_t rows, int inDim, int outDim, const float* X, 
     if (rc != ROC_OK) return rc;
   }
   if (!workspace) return ROC_ERR_INVALID;
-  int rc = ROC_OK;
+  float* ws = (float*)workspace;
   if (parts != ROC_LINEAR_BWD_ONLY_DX) {
-    rc = ROC_ERR_UNSUPPORTED;
-    roc_gemm_info info{};
-    if (!force_simt())
-      rc = tc_linear_dw(rows, inDim, outDim, X, ldX, dY, ldDY, dW, (float*)workspace, workspaceBytes, dm, st, &info);
-    if (rc == ROC_ERR_UNSUPPORTED) info = roc_gemm_info{};
-    info.path = (rc == ROC_ERR_UNSUPPORTED) ? 2 : 1;
-    if (rc == ROC_ERR_UNSUPPORTED)
-      rc = simt_linear_dw(rows, inDim, outDim, X, ldX, dY, ldDY, dW, (float*)workspace, workspaceBytes, dm, st, &info);
-    t_last[1] = info;
+    int rc = run_gemm(
+        1,
+        [&](roc_gemm_info* i) {
+          return tc_linear_dw(rows, inDim, outDim, X, ldX, dY, ldDY, dW, ws, workspaceBytes, dm, st, i);
+        },
+        [&](roc_gemm_info* i) {
+          return simt_linear_dw(rows, inDim, outDim, X, ldX, dY, ldDY, dW, ws, workspaceBytes, dm, st, i);
+        });
     if (rc != ROC_OK) return rc;
   }
-  if (dX) {
-    rc = ROC_ERR_UNSUPPORTED;
-    roc_gemm_info info{};
-    if (!force_simt())
-      rc = tc_linear_dx(rows, inDim, outDim, dY, ldDY, W, dX, ldDX, accumulate_dX, dm, dxReluOf, ldReluOf, dxRowEnd,
-                        colLeft, st, &info);
-    if (rc == ROC_ERR_UNSUPPORTED) info = roc_gemm_info{};
-    info.path = (rc == ROC_ERR_UNSUPPORTED) ? 2 : 1;
-    t_last[2] = info;
-    if (rc == ROC_ERR_UNSUPPORTED)
-      rc = simt_linear_dx(rows, inDim, outDim, dY, ldDY, W, dX, ldDX, accumulate_dX, dm, dxReluOf, ldReluOf, dxRowEnd,
-                          colLeft, st);
-    if (rc != ROC_OK) return rc;
-  }
+  if (dX)
+    return run_gemm(
+        2,
+        [&](roc_gemm_info* i) {
+          return tc_linear_dx(rows, inDim, outDim, dY, ldDY, W, dX, ldDX, accumulate_dX, dm, dxReluOf, ldReluOf,
+                              dxRowEnd, colLeft, st, i);
+        },
+        [&](roc_gemm_info*) {
+          return simt_linear_dx(rows, inDim, outDim, dY, ldDY, W, dX, ldDX, accumulate_dX, dm, dxReluOf, ldReluOf,
+                                dxRowEnd, colLeft, st);
+        });
   return ROC_OK;
 }
 

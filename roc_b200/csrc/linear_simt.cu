@@ -150,6 +150,15 @@ int simt_dw_splits(int64_t rows, int inDim, int outDim) {
   return want;
 }
 
+// dW += the `splits` partials of `part` ([splits][count]), for the SIMT and the tensor-core dW alike
+int splitk_reduce(int64_t count, int splits, const float* part, float* dW, cudaStream_t st) {
+  int64_t blocks = (count + 255) / 256;
+  if (blocks > sm_count() * 8) blocks = sm_count() * 8;
+  k_splitk_reduce<<<(unsigned)blocks, 256, 0, st>>>(count, splits, part, dW);
+  ROC_LAUNCH_CHECK();
+  return ROC_OK;
+}
+
 static void set_mask(GemmP& p, const DropMask* dm, int on) {
   if (!dm) return;
   p.mask = dm->bits; p.ldm = dm->ld; p.mscale = dm->scale; p.maskOn = on;
@@ -199,11 +208,7 @@ int simt_linear_dw(int64_t rows, int inDim, int outDim, const float* X, int64_t 
   dim3 grid((unsigned)((outDim + GB_M - 1) / GB_M), (unsigned)((inDim + GB_N - 1) / GB_N), (unsigned)splits);
   k_sgemm<false, false><<<grid, G_THREADS, 0, st>>>(p);
   ROC_LAUNCH_CHECK();
-  int64_t blocks = (count + 255) / 256;
-  if (blocks > sm_count() * 8) blocks = sm_count() * 8;
-  k_splitk_reduce<<<(unsigned)blocks, 256, 0, st>>>(count, splits, workspace, dW);
-  ROC_LAUNCH_CHECK();
-  return ROC_OK;
+  return splitk_reduce(count, splits, workspace, dW, st);
 }
 
 int relu_bwd_inplace(int64_t rows, int H, const float* Y, int64_t ldY, float* dY, int64_t ldDY, cudaStream_t st) {

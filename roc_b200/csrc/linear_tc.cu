@@ -253,22 +253,14 @@ static int tc_instance(int epi) {
 template <int NC>
 static int tc_launch(dim3 grid, size_t smemBytes, int epi, const CUtensorMap& mapA, const CUtensorMap& mapWhi,
                      const CUtensorMap& mapWlo, const TcParams& q, cudaStream_t st) {
-#define ROC_TC_LAUNCH(E)                                                                                          \
-  do {                                                                                                            \
-    static DynSmemCache configured;                                                                               \
-    ROC_CUDA(ensure_dyn_smem(k_tc_linear<NC, E>, smemBytes, configured));                                         \
-    k_tc_linear<NC, E><<<grid, TC_THREADS, smemBytes, st>>>(mapA, mapWhi, mapWlo, q);                             \
-  } while (0)
+  constexpr int E1 = EPI_NORM, E2 = EPI_OMASK, E3 = EPI_OMASK | EPI_RELUOF | EPI_NORM;
   switch (tc_instance(epi)) {
-    case 0: ROC_TC_LAUNCH(0); break;
-    case EPI_NORM: ROC_TC_LAUNCH(EPI_NORM); break;
-    case EPI_OMASK: ROC_TC_LAUNCH(EPI_OMASK); break;
-    case EPI_OMASK | EPI_RELUOF | EPI_NORM: ROC_TC_LAUNCH(EPI_OMASK | EPI_RELUOF | EPI_NORM); break;
-    default: ROC_TC_LAUNCH(-1); break;
+    case 0: return launch_dyn<k_tc_linear<NC, 0>>(grid, TC_THREADS, smemBytes, st, mapA, mapWhi, mapWlo, q);
+    case E1: return launch_dyn<k_tc_linear<NC, E1>>(grid, TC_THREADS, smemBytes, st, mapA, mapWhi, mapWlo, q);
+    case E2: return launch_dyn<k_tc_linear<NC, E2>>(grid, TC_THREADS, smemBytes, st, mapA, mapWhi, mapWlo, q);
+    case E3: return launch_dyn<k_tc_linear<NC, E3>>(grid, TC_THREADS, smemBytes, st, mapA, mapWhi, mapWlo, q);
+    default: return launch_dyn<k_tc_linear<NC, -1>>(grid, TC_THREADS, smemBytes, st, mapA, mapWhi, mapWlo, q);
   }
-#undef ROC_TC_LAUNCH
-  ROC_LAUNCH_CHECK();
-  return ROC_OK;
 }
 
 // Y[rows][N] (op)= A[rows][K] * B^T with B(n, k) taken from W as k_split_w describes
@@ -280,7 +272,6 @@ static int ts_gemm(int64_t rows, int K, int N, const float* A, int64_t ldA, cons
   if (e.reluOf && ((e.ldR % 4) || !aligned16(e.reluOf))) return ROC_ERR_UNSUPPORTED;
   if (rows > 0x7FFFFF00ll) return ROC_ERR_UNSUPPORTED;   // TMA coordinates are int32
   if (!encode_tiled_fn()) return ROC_ERR_UNSUPPORTED;
-  { const char* g = getenv("ROC_B200_GEMM"); if (g && g[0] == 'n' && g[1] == 'o') return ROC_ERR_UNSUPPORTED; }   // "notc"
   // N-tile of 32, 64 or 128 columns (wgmma chunks of 32): the widest tile streams A once per 128 output columns
   const int NC = (N <= 32) ? 1 : (N <= 64) ? 2 : 4;
   const int BN = 32 * NC;
@@ -304,12 +295,10 @@ static int ts_gemm(int64_t rows, int K, int N, const float* A, int64_t ldA, cons
   if (!make_tmap_f32_2d(&mapWhi, Whi, (uint64_t)Npad, (uint64_t)Kpad, (uint64_t)Kpad, (uint32_t)BN, TC_BK)) return ROC_ERR_UNSUPPORTED;
   if (!make_tmap_f32_2d(&mapWlo, Wlo, (uint64_t)Npad, (uint64_t)Kpad, (uint64_t)Kpad, (uint32_t)BN, TC_BK)) return ROC_ERR_UNSUPPORTED;
 
-  // as many stages as fit in the 227 KB an H100 block may use (beside the alignment slack and the barriers)
   const size_t stageBytes = (size_t)TC_BM * TC_BK * 4 + (size_t)2 * BN * TC_BK * 4;
   const size_t fixedBytes = 1024 /*align*/ + 256 /*barriers*/;
-  int stages = (int)(((size_t)227 * 1024 - fixedBytes) / stageBytes);
-  if (stages > TC_MAX_STAGES) stages = TC_MAX_STAGES;
-  if (stages < 2) return ROC_ERR_UNSUPPORTED;
+  const int stages = ring_stages(stageBytes, fixedBytes, TC_MAX_STAGES);
+  if (!stages) return ROC_ERR_UNSUPPORTED;
   TcParams q{};
   q.Y = Y; q.ldY = ldY; q.rows = rows; q.outDim = N; q.numKb = Kpad / TC_BK; q.stages = stages;
   q.accumulate = e.accumulate;

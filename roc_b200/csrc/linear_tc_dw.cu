@@ -15,8 +15,8 @@
 //       [N][KS] (hi, lo; 128-byte swizzle) that the MMAs of every consumer warpgroup read.
 //
 // Both kernels below do that arithmetic with the same per-element MMA order (blocks in vertex order, k8 steps 0..3,
-// then lo_x*hi_y, hi_x*lo_y, hi_x*hi_y), so every bit of dW is the same in both.  k_tc_linear_dw keeps its own
-// inline copy of the transpose / fragment / MMA / store steps so that its compiled code stays as it was.
+// then lo_x*hi_y, hi_x*lo_y, hi_x*hi_y), so every bit of dW is the same in both.  They share the per-block steps
+// (DwLane, dw_transpose, dw_fragments, dw_store) and differ in their pipelines and in how they issue the MMAs.
 //
 // k_tc_linear_dw_ws (N <= 128, the default there): one TMA producer warp and 1 or 2 consumer warpgroups.
 //   The producer fills a ring of stages (X boxes, the dY box and the [KS][4]-word box of the packed dropout
@@ -213,21 +213,12 @@ k_tc_linear_dw(const __grid_constant__ CUtensorMap mapX, const __grid_constant__
     for (int step = 0; step < p.stages && step < numSteps; step++) load(step);
 
   // ================================== consumers ===================================
-  const int g = lane >> 2, t = lane & 3;
-  const int ca = dw_col(warp, g, 0), cb = dw_col(warp, g, 1);   // X columns of this thread: i0 + ca and i0 + cb
-  // offsets of the fragment (k8 step 0) in the swizzled X boxes: (vertex t + 4 e, column c) at
-  // box(c) * 32 KS + (t + 4 e) * 32 + ((c % 32 / 4) ^ (t + 4 e)) * 4 + c % 4
-  int xo[2][2];
-#pragma unroll
-  for (int h = 0; h < 2; h++)
-#pragma unroll
-    for (int e = 0; e < 2; e++) {
-      const int c = h ? cb : ca, k = t + 4 * e;
-      xo[h][e] = (c / DW_XBOX) * (DW_KS * DW_XBOX) + k * DW_XBOX + ((((c % DW_XBOX) >> 2) ^ k) << 2) + (c & 3);
-    }
-  const bool masked = p.mask != nullptr && i0 + ca < p.inDim;   // (columns past inDim are zero-filled by TMA)
-  const int mcol = (i0 + ca) >> 5, mb0 = ca & 31, mb1 = cb & 31;
-  // dropout fused into the operand load: this thread's mask words of vertices v + 8 kk + t (+ 4)
+  const DwLane L(warp, lane);
+  const int t = lane & 3;
+  const bool masked = p.mask != nullptr && i0 + L.ca < p.inDim;   // (columns past inDim are zero-filled by TMA)
+  const int mcol = (i0 + L.ca) >> 5;
+  // dropout fused into the operand load: this thread's mask words of vertices v + 8 kk + t (+ 4); all ones for a
+  // column past inDim, as in k_tc_linear_dw_ws
   auto load_mask = [&](int step, uint32_t (&mw)[8]) {
     const int64_t v = v0 + (int64_t)step * DW_KS;
 #pragma unroll
@@ -236,43 +227,14 @@ k_tc_linear_dw(const __grid_constant__ CUtensorMap mapX, const __grid_constant__
       mw[q] = masked ? ((row < p.rows) ? __ldg(p.mask + row * p.ldm + mcol) : 0u) : 0xFFFFFFFFu;
     }
   };
-  // dY [KS][BN] of stage s -> dY^T hi / lo [BN][KS] of buffer b; 128-byte swizzle: element (o, k) at
-  // o*32 + ((k/4 ^ o%8) * 4) + k%4.  A thread takes 4 consecutive k of one o: 4 conflict-free loads, one 16-byte
-  // store per tile, and the 8 lanes of a store phase (8 consecutive o) fill the 32 banks.
-  auto transpose = [&](int s, int b) {
-    const float* ys = reinterpret_cast<const float*>(stages + (size_t)s * stageBytes + xBytes);
+  auto transpose = [&](int s, int b) {   // dY of stage s -> dY^T of buffer b
     float* hiT = bT + (size_t)(2 * b) * (BN * DW_KS);
-    float* loT = hiT + BN * DW_KS;
-#pragma unroll
-    for (int j = 0; j < NC; j++) {
-      const int idx = threadIdx.x + DW_THREADS * j;
-      const int q = idx / BN, o = idx - q * BN;
-      uint32_t h[4], l[4];
-#pragma unroll
-      for (int r = 0; r < 4; r++) split_tf32(ys[(4 * q + r) * BN + o], h[r], l[r]);
-      const int d = o * DW_KS + ((q ^ (o & 7)) << 2);
-      *reinterpret_cast<uint4*>(hiT + d) = make_uint4(h[0], h[1], h[2], h[3]);
-      *reinterpret_cast<uint4*>(loT + d) = make_uint4(l[0], l[1], l[2], l[3]);
-    }
-    fence_proxy_async_smem();
+    dw_transpose<NC, DW_THREADS>(reinterpret_cast<const float*>(stages + (size_t)s * stageBytes + xBytes), hiT,
+                                 hiT + BN * DW_KS, threadIdx.x);
   };
-  // A fragments (hi, lo) of every k8 step of the block in stage s
-  auto fragments = [&](int s, const uint32_t (&mw)[8], uint32_t (&fr)[DW_KS / 8][2][4]) {
-    const float* xs = reinterpret_cast<const float*>(stages + (size_t)s * stageBytes);
-#pragma unroll
-    for (int kk = 0; kk < DW_KS / 8; kk++) {
-      const int kb = kk * 8 * DW_XBOX;
-      float x[4] = {xs[kb + xo[0][0]], xs[kb + xo[1][0]], xs[kb + xo[0][1]], xs[kb + xo[1][1]]};
-      if (p.mask) {
-        const uint32_t m0 = mw[2 * kk], m1 = mw[2 * kk + 1];
-        x[0] = ((m0 >> mb0) & 1u) ? x[0] * p.mscale : 0.f;   // == k_dropout
-        x[1] = ((m0 >> mb1) & 1u) ? x[1] * p.mscale : 0.f;
-        x[2] = ((m1 >> mb0) & 1u) ? x[2] * p.mscale : 0.f;
-        x[3] = ((m1 >> mb1) & 1u) ? x[3] * p.mscale : 0.f;
-      }
-#pragma unroll
-      for (int i = 0; i < 4; i++) split_tf32(x[i], fr[kk][0][i], fr[kk][1][i]);
-    }
+  auto fragments = [&](int s, const uint32_t (&mw)[8], uint32_t (&fr)[DW_KS / 8][2][4]) {   // of the block in stage s
+    dw_fragments(reinterpret_cast<const float*>(stages + (size_t)s * stageBytes), L, p.mask != nullptr, p.mscale, mw,
+                 fr);
   };
   float acc[NC][16];
 #pragma unroll
@@ -335,22 +297,7 @@ k_tc_linear_dw(const __grid_constant__ CUtensorMap mapX, const __grid_constant__
   keep_live(frB);
 #pragma unroll
   for (int c = 0; c < NC; c++) wgmma_fence_acc(acc[c]);
-  // ---- epilogue: acc[c][4j + {0,1}] = (i0 + ca, o, o + 1), [4j + {2,3}] = (i0 + cb, ...), o = 32c + 8j + 2t
-  float* ws = p.ws + (size_t)blockIdx.x * ((size_t)p.inDim * p.outDim);
-  const int ia = i0 + ca, ib = i0 + cb;
-#pragma unroll
-  for (int c = 0; c < NC; c++)
-#pragma unroll
-    for (int j = 0; j < 4; j++) {
-      const int o = c * 32 + j * 8 + 2 * t;
-#pragma unroll
-      for (int h = 0; h < 2; h++) {
-        if (o + h >= p.outDim) continue;
-        float* col = ws + (size_t)(o + h) * p.inDim;
-        if (ia < p.inDim) col[ia] = acc[c][4 * j + h];
-        if (ib < p.inDim) col[ib] = acc[c][4 * j + 2 + h];
-      }
-    }
+  dw_store<NC>(p, L, i0, t, acc);
 }
 
 // WG consumer warpgroups (tile of 64 WG X columns) + one TMA producer warp
@@ -471,14 +418,7 @@ k_tc_linear_dw_ws(const __grid_constant__ CUtensorMap mapX, const __grid_constan
   dw_store<NC>(p, L, i0, t, acc);
 }
 
-__global__ void __launch_bounds__(256)
-k_tc_splitk_reduce(int64_t count, int splits, const float* __restrict__ part, float* __restrict__ dW) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x) {
-    float s = 0.f;
-    for (int z = 0; z < splits; z++) s += part[(int64_t)z * count + i];
-    dW[i] += s;
-  }
-}
+int splitk_reduce(int64_t count, int splits, const float* part, float* dW, cudaStream_t st);   // linear_simt.cu
 
 // ws: k_tc_linear_dw_ws with WG consumer warpgroups; otherwise k_tc_linear_dw
 struct DwPlan { int NC, MT, splits, stages; bool ws; int WG; size_t smemBytes; };
@@ -486,7 +426,6 @@ struct DwPlan { int NC, MT, splits, stages; bool ws; int WG; size_t smemBytes; }
 // maskOk: no mask, or one whose [KS][4]-word box TMA can load (16-byte aligned base)
 static int tc_dw_plan(int64_t rows, int inDim, int outDim, bool maskOk, DwPlan* q) {
   if (outDim > 256 || outDim < 1 || inDim < 4 || rows < 8) return ROC_ERR_UNSUPPORTED;
-  { const char* e = getenv("ROC_B200_GEMM"); if (e && e[0] == 'n' && e[1] == 'o') return ROC_ERR_UNSUPPORTED; }   // "notc"
   const int nc = (outDim + 31) / 32;
   q->NC = nc <= 1 ? 1 : nc <= 2 ? 2 : nc <= 4 ? 4 : 8;
   q->MT = (inDim + DW_BM - 1) / DW_BM;
@@ -502,11 +441,9 @@ static int tc_dw_plan(int64_t rows, int inDim, int outDim, bool maskOk, DwPlan* 
     stageBytes = (size_t)DW_KS * DW_BM * 4 + (size_t)DW_KS * bn * 4;
     fixedBytes = 1024 /*align*/ + 64 /*barriers*/ + 4 * bn * DW_KS * 4 /*two dY^T hi / lo buffers*/;
   }
-  int st = (int)(((size_t)227 * 1024 - fixedBytes) / stageBytes);
-  if (st > DW_MAX_STAGES) st = DW_MAX_STAGES;
-  if (st < 2) return ROC_ERR_UNSUPPORTED;
-  q->stages = st;
-  q->smemBytes = (size_t)st * stageBytes + fixedBytes;
+  q->stages = ring_stages(stageBytes, fixedBytes, DW_MAX_STAGES);
+  if (!q->stages) return ROC_ERR_UNSUPPORTED;
+  q->smemBytes = (size_t)q->stages * stageBytes + fixedBytes;
   int sp = sm_count() / q->MT;
   if (sp < 1) sp = 1;
   int64_t maxSp = (rows + 63) / 64;
@@ -526,26 +463,11 @@ static int dw_launch(const DwPlan& q, const CUtensorMap& mapX, const CUtensorMap
                      const TcDwParams& t, cudaStream_t st) {
   const dim3 grid((unsigned)q.splits, (unsigned)q.MT, 1);
   if constexpr (NC <= 4) {
-    if (q.ws && q.WG == 1) {
-      static DynSmemCache configured;
-      ROC_CUDA(ensure_dyn_smem(k_tc_linear_dw_ws<NC, 1>, q.smemBytes, configured));
-      k_tc_linear_dw_ws<NC, 1><<<grid, 128 + 32, q.smemBytes, st>>>(mapX, mapDY, mapM, t);
-      ROC_LAUNCH_CHECK();
-      return ROC_OK;
-    }
-    if (q.ws) {
-      static DynSmemCache configured;
-      ROC_CUDA(ensure_dyn_smem(k_tc_linear_dw_ws<NC, 2>, q.smemBytes, configured));
-      k_tc_linear_dw_ws<NC, 2><<<grid, 256 + 32, q.smemBytes, st>>>(mapX, mapDY, mapM, t);
-      ROC_LAUNCH_CHECK();
-      return ROC_OK;
-    }
+    if (q.ws && q.WG == 1)
+      return launch_dyn<k_tc_linear_dw_ws<NC, 1>>(grid, 128 + 32, q.smemBytes, st, mapX, mapDY, mapM, t);
+    if (q.ws) return launch_dyn<k_tc_linear_dw_ws<NC, 2>>(grid, 256 + 32, q.smemBytes, st, mapX, mapDY, mapM, t);
   }
-  static DynSmemCache configured;
-  ROC_CUDA(ensure_dyn_smem(k_tc_linear_dw<NC>, q.smemBytes, configured));
-  k_tc_linear_dw<NC><<<grid, DW_THREADS, q.smemBytes, st>>>(mapX, mapDY, t);
-  ROC_LAUNCH_CHECK();
-  return ROC_OK;
+  return launch_dyn<k_tc_linear_dw<NC>>(grid, DW_THREADS, q.smemBytes, st, mapX, mapDY, t);
 }
 
 int tc_linear_dw(int64_t rows, int inDim, int outDim, const float* X, int64_t ldX, const float* dY, int64_t ldDY,
@@ -586,11 +508,7 @@ int tc_linear_dw(int64_t rows, int inDim, int outDim, const float* X, int64_t ld
     default: rc = dw_launch<8>(q, mapX, mapDY, mapM, t, st); break;
   }
   if (rc != ROC_OK) return rc;
-  int64_t blocks = ((int64_t)count + 255) / 256;
-  if (blocks > sm_count() * 8) blocks = sm_count() * 8;
-  k_tc_splitk_reduce<<<(unsigned)blocks, 256, 0, st>>>((int64_t)count, q.splits, workspace, dW);
-  ROC_LAUNCH_CHECK();
-  return ROC_OK;
+  return splitk_reduce((int64_t)count, q.splits, workspace, dW, st);
 }
 
 }  // namespace roc

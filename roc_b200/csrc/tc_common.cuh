@@ -173,6 +173,16 @@ __device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) 
   lo = __float_as_uint(x - __uint_as_float(hi));
 }
 
+// ------------------------------------------------------- host: ring depth -----
+constexpr size_t SMEM_PER_BLOCK = 227 * 1024;   // the shared memory an H100 block may use
+
+// Stages of a TMA ring: as many of stageBytes as fit beside fixedBytes (alignment slack, barriers, buffers), at most
+// maxStages; 0 when fewer than 2 fit, since one stage cannot overlap the loads with the compute
+inline int ring_stages(size_t stageBytes, size_t fixedBytes, int maxStages) {
+  const int st = (int)((SMEM_PER_BLOCK - fixedBytes) / stageBytes);
+  return st < 2 ? 0 : st > maxStages ? maxStages : st;
+}
+
 // ------------------------------------------------------ host: tensor maps -----
 // cuTensorMapEncodeTiled through the runtime's driver entry point (no -lcuda).
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,

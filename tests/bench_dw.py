@@ -1,4 +1,4 @@
-"""bench_dw.py — micro-benchmark of the Linear weight gradient (k_tc_linear_dw + split-K reduce) alone (not a pytest
+"""bench_dw.py — micro-benchmark of the Linear weight gradient (k_tc_linear_dw + k_splitk_reduce) alone (not a pytest
 file).
 
 dW = dY^T X, plain and on dropout(X) with the keep-mask fused into the operand load (how the training step runs it),

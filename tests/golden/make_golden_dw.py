@@ -1,4 +1,4 @@
-"""make_golden_dw.py — SHA-256 digests of the tensor-core dW (k_tc_linear_dw + split-K reduce), bit for bit.
+"""make_golden_dw.py — SHA-256 digests of the tensor-core dW (k_tc_linear_dw + k_splitk_reduce), bit for bit.
 
     python tests/golden/make_golden_dw.py [out.npz]        # needs an H100; run on a build whose dW bits are the golden
 

@@ -1,7 +1,7 @@
 """GPU suite: the Linear GEMMs against an fp64 reference, element by element, at every kernel instantiation.
 
 The tensor-core kernels (k_tc_linear<NC, EPI> for forward and dX, k_tc_linear_dw<NC> for dW; 3xTF32 on wgmma) and
-the exact-fp32 SIMT kernels (ROC_B200_GEMM=notc) must meet the bound of tests/tf32_bound.py.  That bound is calibrated
+the exact-fp32 SIMT kernels (ROC_B200_GEMM=simt) must meet the bound of tests/tf32_bound.py.  That bound is calibrated
 on the CPU (test_tf32_bound_cpu.py) so that a correct kernel passes by a wide margin and a kernel that loses any one of
 its three MMAs fails by a wide margin.  For forward and dX that holds at every shape here (K = the layer width).  For
 dW, K is the row count, and the bound follows the kernel's split-K ranges; it keeps that power for ranges of 416 rows,
@@ -243,7 +243,7 @@ def check_fwd_launch(info, path, rows, n, epi, kind):
 @pytest.mark.parametrize("case", MATRIX, ids=_id)
 def test_fwd_dx_matrix(case, path, monkeypatch):
     if path == "notc":
-        monkeypatch.setenv("ROC_B200_GEMM", "notc")
+        monkeypatch.setenv("ROC_B200_GEMM", "simt")
     c = case
     what = "%s %s" % (path, _id(c))
     if c["kind"] == "fwd":
@@ -332,7 +332,7 @@ def _dw_id(c):
 @pytest.mark.parametrize("case", DW_MATRIX, ids=_dw_id)
 def test_dw_matrix(case, path, monkeypatch):
     if path == "notc":
-        monkeypatch.setenv("ROC_B200_GEMM", "notc")
+        monkeypatch.setenv("ROC_B200_GEMM", "simt")
     c = case
     what = "%s dW rows %d %d x %d" % (path, c["rows"], c["out"], c["inn"])
     r = run_dw(c["rows"], c["inn"], c["out"], c["family"], c["masked"], c["seed"])

@@ -68,7 +68,7 @@ def test_a_missing_mma_fails_by_a_wide_margin(family, m, k, n):
 @pytest.mark.parametrize("splits", [26, 132])
 def test_split_k_dw_keeps_its_power(family, splits):
     """dW sums over the vertices: K is the row count, split into ranges that accumulate on their own and are then added
-    in fp32 (k_tc_linear_dw, k_tc_splitk_reduce).  At the layout of the GPU matrix's ring-wrap cases (416 rows per
+    in fp32 (k_tc_linear_dw, k_splitk_reduce).  At the layout of the GPU matrix's ring-wrap cases (416 rows per
     split, 26 or 132 splits, the last short) the bound must still hold a correct kernel with margin and reject a lost
     MMA.  A bound that summed |partial sums| over all rows in one sequence would be ~sqrt(splits) times too loose
     for random signs: every lost lo term would pass."""

@@ -182,7 +182,7 @@ def round_toward_zero(x64):
 
 def emulate_split_k(a, b, split, mode):
     """emulate() of each range of `split` K-terms (the dW kernels' split-K), then the fp32 partials added in range
-    order, rounded to nearest (k_tc_splitk_reduce)"""
+    order, rounded to nearest (k_splitk_reduce)"""
     total = None
     for k0 in range(0, a.shape[1], split):
         part = emulate(a[:, k0:k0 + split], b[:, k0:k0 + split], mode)

@@ -164,6 +164,40 @@ int roc_sg_minmax_backward_planned(const roc_sg_plan* plan, int H, roc_vid_t sel
                                    const float* outGrad, int64_t ldG, const roc_vid_t* arg, int64_t ldArg,
                                    float* inGrad, int64_t ldIn, roc_stream_t stream);
 
+/* Attention aggregation (GAT, Velickovic et al. 2018).  `heads` heads over features of width H = heads * F; `score`
+ * has 2 * heads columns: column k is the destination score s_dst[.][k] of head k, column heads + k the source score
+ * s_src[.][k].  For plan row r with id i = selfBase + r and in-edges e in CSR order, sources j = colSrc[e]:
+ *   y(i,j,k)     = LeakyReLU_slope(s_dst[i][k] + s_src[j][k])          (z > 0 ? z : slope * z)
+ *   m[i][k]      = max_e y(i,j,k);   Z[i][k] = sum_e exp(y(i,j,k) - m[i][k])
+ *   a(i<-j,k)    = exp(y(i,j,k) - m[i][k]) / Z[i][k]
+ *   out[r][kF+f] = sum_e a(i<-j,k) * in[j][kF+f]
+ *   stats[r][k]  = m[i][k],   stats[r][heads+k] = 1 / Z[i][k]
+ * A row of degree 0 gets out = 0, m = 0 and 1/Z = 0, so its a is 0 wherever the backward recomputes it.  `in`,
+ * `score` and every per-node input of the backward are indexed by colSrc's ids (a whole graph, or a slice with global
+ * ids and selfBase = rowLeft).
+ * Backward, as gathers over the same CSR (quirk Q1: the true adjoint of the source-score and feature parts only on a
+ * symmetric graph; the destination-score part is exact on any graph).  G = outGrad, O = out, X = in, score and stats
+ * all indexed by colSrc's ids.  With D[i][k] = sum_f G[i][kF+f] O[i][kF+f], l = (s_dst[i][k] + s_src[j][k] > 0) ? 1 :
+ * slope and dz(i<-j,k) = a(i<-j,k) (sum_f G[i][kF+f] X[j][kF+f] - D[i][k]) l  (a recomputed from stats[i]):
+ *   scoreGrad[r][k]       = sum_{e in row r, j = col[e]} dz(i<-j,k)                 (d s_dst)
+ *   scoreGrad[r][heads+k] = sum_{e in row r, j = col[e]} dz(j<-i,k)                 (d s_src)
+ *   inGrad[r][kF+f]       = sum_{e in row r, j = col[e]} a(j<-i,k) G[j][kF+f]
+ * Shapes: heads in {1, 2, 4, 8}, H % heads == 0; for heads > 1, F is a power of two >= 4.  H <= 512 when every
+ * feature leading dimension is a multiple of 4 and every feature pointer 16-byte aligned, else H <= 256.  slope is
+ * finite and >= 0.  IEEE expf and divides; no atomics, so the same call on the same inputs returns the same bits.
+ * Both calls overwrite their outputs.  ROC_ERR_INVALID: a NULL pointer, a leading dimension too small (< H, or
+ * < 2 * heads for score / stats / scoreGrad), heads <= 0, H <= 0, a bad slope.  ROC_ERR_UNSUPPORTED: any other
+ * head layout or width.  The backward keeps a per-node record {s_dst, m, 1/Z, D} (16 bytes per head) in the plan;
+ * its first call finds the largest id in colSrc (one synchronisation of the stream). */
+int roc_sg_attn_forward_planned(const roc_sg_plan* plan, int heads, int H, float slope, roc_vid_t selfBase,
+                                const float* in, int64_t ldIn, const float* score, int64_t ldS,
+                                float* out, int64_t ldOut, float* stats, int64_t ldStats, roc_stream_t stream);
+int roc_sg_attn_backward_planned(const roc_sg_plan* plan, int heads, int H, float slope, roc_vid_t selfBase,
+                                 const float* in, int64_t ldIn, const float* score, int64_t ldS, const float* out,
+                                 int64_t ldOut, const float* stats, int64_t ldStats, const float* outGrad,
+                                 int64_t ldG, float* inGrad, int64_t ldInG, float* scoreGrad, int64_t ldSG,
+                                 roc_stream_t stream);
+
 /* Plan-less form with exactly the reference kernel's argument list
  * (scattergather_kernel.cu:21-28, EdgeStruct.dst dropped), dense ld == H.
  * Builds and frees a plan internally (synchronises); use the planned form in

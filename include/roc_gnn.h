@@ -189,6 +189,12 @@ public:
    * held the extreme.  That is the true gradient only on a symmetric graph without duplicate edges: init() refuses
    * a graph whose rows do not have strictly increasing sources.  Single partition only (exit(1) otherwise). */
   Tensor scatter_gather(const Tensor& _input, AggrType aggr);
+  /* Attention aggregation (GAT; roc_sg_attn_forward_planned): `scores` has 2 * heads columns, [s_dst | s_src] per
+   * head; the output has the input's width, each head's block of H / heads columns weighted by that head's
+   * softmax over the row's in-edges.  Its backward is a gather over the same CSR (quirk Q1): exact for the
+   * destination scores, the true gradient of the rest on a symmetric graph.  Never fused with neighbouring ops.
+   * Single partition only (exit(1) otherwise). */
+  Tensor attention_gather(const Tensor& input, const Tensor& scores, int heads, float negativeSlope = 0.2f);
   void softmax_cross_entropy(const Tensor& logits, const Tensor& labels, const Tensor& mask);
   Tensor indegree_norm(const Tensor& _input);
   Tensor linear(const Tensor& _input, int outDim, ActiMode activation, Initializer* initializer = NULL);
@@ -263,6 +269,19 @@ public:
   int epilogue;      /* ROC_SG_EPI_* the forward store applies (set by Model::init fusion) */
   int bwdEpilogue;   /* same for the backward launch */
   int fwdOut, bwdOut;/* region the fused forward / backward writes (-1: own output / input grad) */
+};
+
+class AttentionGather : public GnnOp {  /* not in the reference: Model::attention_gather */
+public:
+  AttentionGather(const Model& model, const Tensor& input, const Tensor& scores, int heads, float slope);
+  virtual void init(const Model& model);
+  virtual void forward(const Model& model);
+  virtual void backward(const Model& model);
+  int heads;
+  float slope;
+  float* stats;      /* [Nloc][statsLd] m | 1/Z per head of the last forward (Runtime arena) */
+  int64_t statsLd;
+  float* scratch[2]; /* gradients of an input that accumulates (or needs none), written here first (Runtime arena) */
 };
 
 class InDegreeNorm : public GnnOp {  /* gnn.h:244-261, graphnorm.cc */

@@ -87,6 +87,9 @@ PROTOTYPES = {
     "roc_sg_forward_planned": (i32, [vp, i32, vp, i64, vp, i64, i32, vp]),
     "roc_sg_minmax_forward_planned": (i32, [vp, i32, i32, vp, i64, vp, i64, vp, i64, vp]),
     "roc_sg_minmax_backward_planned": (i32, [vp, i32, u32, vp, i64, vp, i64, vp, i64, vp]),
+    "roc_sg_attn_forward_planned": (i32, [vp, i32, i32, f32, u32, vp, i64, vp, i64, vp, i64, vp, i64, vp]),
+    "roc_sg_attn_backward_planned": (i32, [vp, i32, i32, f32, u32, vp, i64, vp, i64, vp, i64, vp, i64, vp, i64, vp,
+                                           i64, vp, i64, vp]),
     "roc_sg_forward": (i32, [u32, u32, u64, i32, vp, vp, vp, vp, vp]),
     "roc_sg_backward": (i32, [u32, u32, u64, i32, vp, vp, vp, vp, vp]),
     "roc_halo_create": (i32, [u32, u32, u64, vp, vp, C.POINTER(vp)]),
@@ -141,6 +144,7 @@ PROTOTYPES = {
     "roc_host_indegree_norm": (i32, [vp, i32]),
     "roc_host_scatter_gather": (i32, [vp, i32]),
     "roc_host_scatter_gather_aggr": (i32, [vp, i32, i32]),
+    "roc_host_attention_gather": (i32, [vp, i32, i32, i32, f32]),
     "roc_host_get_aggr_index": (i32, [vp, i32, vp]),
     "roc_host_relu": (i32, [vp, i32]),
     "roc_host_sigmoid": (i32, [vp, i32]),

@@ -91,6 +91,9 @@ int roc_host_scatter_gather_aggr(roc_host* h, int t, int aggr) {
   if (aggr < AGGR_AVG || aggr > AGGR_SUM) ROC_FATAL("roc_host_scatter_gather_aggr: bad AggrType");
   return h->push(h->m().scatter_gather(h->at(t), (AggrType)aggr));
 }
+int roc_host_attention_gather(roc_host* h, int t, int scores, int heads, float slope) {
+  return h->push(h->m().attention_gather(h->at(t), h->at(scores), heads, slope));
+}
 int roc_host_get_aggr_index(roc_host* h, int t, uint32_t* host) { h->m().get_aggr_index(h->at(t), host); return 0; }
 int roc_host_relu(roc_host* h, int t) { return h->push(h->m().relu(h->at(t))); }
 int roc_host_sigmoid(roc_host* h, int t) { return h->push(h->m().sigmoid(h->at(t))); }

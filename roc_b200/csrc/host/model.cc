@@ -109,6 +109,13 @@ Tensor Model::scatter_gather(const Tensor& _input, AggrType aggr) {
   ROC_FATAL("scatter_gather: unknown AggrType");
   return Tensor();
 }
+Tensor Model::attention_gather(const Tensor& input, const Tensor& scores, int heads, float negativeSlope) {
+  if (ctx->numParts > 1)
+    ROC_FATAL("attention_gather: runs on one partition only (numParts > 1 is not supported)");
+  GnnOp* op = new AttentionGather(*this, input, scores, heads, negativeSlope);
+  layers.push_back(op);
+  return op->outputs[0];
+}
 void Model::get_aggr_index(const Tensor& out, uint32_t* host) const {
   for (GnnOp* op : layers) {
     ScatterGather* sg = dynamic_cast<ScatterGather*>(op);
@@ -380,7 +387,7 @@ bool Model::init(const Config& config) {
     const ScatterGather* sgl = as<ScatterGather>(layers[l]);
     const char* nm = sgl ? (sgl->aggr == AGGR_MAX ? "scatter_gather(max)" : sgl->aggr == AGGR_MIN ? "scatter_gather(min)"
                                                                                                   : "scatter_gather") :
-                     as<Linear>(layers[l]) ? "linear" :
+                     as<AttentionGather>(layers[l]) ? "attention_gather" : as<Linear>(layers[l]) ? "linear" :
                      as<InDegreeNorm>(layers[l]) ? "indegree_norm" : as<Activation>(layers[l]) ? "activation" :
                      as<Dropout>(layers[l]) ? "dropout" : as<Element>(layers[l]) ? "add" :
                      as<SoftmaxCrossEntropy>(layers[l]) ? "softmax_cross_entropy" : "op";
@@ -763,6 +770,73 @@ void ScatterGather::backward(const Model& model) {
   rt->sg_begin(H);
   ROC_CHECK(roc_sg_forward_planned(model.myGraph.plan, H, src, ld, dst, rt->t(dstRegion).ld, bwdEpilogue, rt->stream));
   rt->sg_end();
+}
+
+// ------------------------------------------------------- AttentionGather -----
+AttentionGather::AttentionGather(const Model& model, const Tensor& _input, const Tensor& _scores, int _heads, float _slope)
+    : GnnOp(_input, _scores), heads(_heads), slope(_slope), stats(nullptr), statsLd(0) {
+  scratch[0] = scratch[1] = nullptr;
+  ROC_ASSERT(_input.type == Tensor::NODE_TENSOR && _scores.type == Tensor::NODE_TENSOR);
+  ROC_ASSERT(_input.numDim == 2 && _scores.numDim == 2);
+  ROC_ASSERT(_input.dims[1] == model.myGraph.numNodes && _scores.dims[1] == model.myGraph.numNodes);
+  if (_heads <= 0 || _scores.dims[0] != 2 * (E_ID)_heads)
+    ROC_FATAL("attention_gather: the scores need 2 * heads columns ([s_dst | s_src] per head)");
+  if (!(_slope >= 0.0f) || !std::isfinite(_slope)) ROC_FATAL("attention_gather: the negative slope must be finite and >= 0");
+  // the layouts roc_sg_attn_* take on node tensors (rows padded to float4: the vector path)
+  const int64_t H = (int64_t)_input.dims[0], F = H / _heads;
+  if (_heads != 1 && _heads != 2 && _heads != 4 && _heads != 8)
+    ROC_FATAL("attention_gather: heads must be 1, 2, 4 or 8");
+  if (H % _heads || (_heads > 1 && (F < 4 || (F & (F - 1)))))
+    ROC_FATAL("attention_gather: with heads > 1, the input width must be heads * F with F a power of two >= 4");
+  if (H > 512) ROC_FATAL("attention_gather: the input width must be at most 512");
+  numOutputs = 1;
+  outputs[0] = model.create_node_tensor<DATATYPE>((int)_input.dims[0]);
+}
+void AttentionGather::init(const Model&) {}
+
+void AttentionGather::forward(const Model& model) {
+  RuntimeImpl* rt = model.ctx;
+  const int H = (int)inputs[0].dims[0];
+  if (!stats) {
+    statsLd = round_up4(2 * heads);
+    stats = (float*)rt->dmalloc((size_t)std::max<int64_t>(model.local_rows(), 1) * (size_t)statsLd * sizeof(float));
+  }
+  rt->sg_begin(H);
+  ROC_CHECK(roc_sg_attn_forward_planned(model.myGraph.plan, heads, H, slope, model.myGraph.rowLeft,
+                                        rt->data(inputs[0].region), rt->t(inputs[0].region).ld,
+                                        rt->data(inputs[1].region), rt->t(inputs[1].region).ld,
+                                        rt->data(outputs[0].region), rt->t(outputs[0].region).ld, stats, statsLd,
+                                        rt->stream));
+  rt->sg_end();
+}
+
+void AttentionGather::backward(const Model& model) {
+  RuntimeImpl* rt = model.ctx;
+  if (!rt->t(inputs[0].region).requiresGrad && !rt->t(inputs[1].region).requiresGrad) return;
+  const int H = (int)inputs[0].dims[0];
+  // The kernel overwrites both gradients.  An input whose gradient another op already wrote (the features feed the
+  // score Linear too) gets its part in scratch, added afterwards; so does one that needs no gradient.
+  float* dst[2];
+  for (int i = 0; i < 2; i++) {
+    const TensorImpl& x = rt->t(inputs[i].region);
+    if (x.requiresGrad && resetInputGrads[i]) { dst[i] = rt->grad(inputs[i].region); continue; }
+    if (!scratch[i]) scratch[i] = (float*)rt->dmalloc((size_t)std::max<int64_t>(model.local_rows(), 1) * (size_t)x.ld * sizeof(float));
+    dst[i] = scratch[i];
+  }
+  const int ox = outputs[0].region;
+  rt->sg_begin(H);
+  ROC_CHECK(roc_sg_attn_backward_planned(model.myGraph.plan, heads, H, slope, model.myGraph.rowLeft,
+                                         rt->data(inputs[0].region), rt->t(inputs[0].region).ld,
+                                         rt->data(inputs[1].region), rt->t(inputs[1].region).ld, rt->data(ox),
+                                         rt->t(ox).ld, stats, statsLd, rt->grad(ox), rt->t(ox).ld, dst[0],
+                                         rt->t(inputs[0].region).ld, dst[1], rt->t(inputs[1].region).ld, rt->stream));
+  rt->sg_end();
+  for (int i = 0; i < 2; i++) {
+    const TensorImpl& x = rt->t(inputs[i].region);
+    if (!x.requiresGrad || resetInputGrads[i]) continue;
+    float* g = rt->grad(inputs[i].region);
+    ROC_CHECK(roc_add_fwd(model.local_rows(), x.H, g, x.ld, scratch[i], x.ld, g, x.ld, rt->stream));
+  }
 }
 
 // --------------------------------------------------------- InDegreeNorm -----

@@ -32,6 +32,8 @@
 // backward E*(8H+4) + Nloc*(4H+8).
 #include <cub/cub.cuh>
 #include <thrust/iterator/counting_iterator.h>
+#include <algorithm>
+#include <cmath>
 #include <cstring>
 #include <new>
 #include "common.cuh"
@@ -56,6 +58,11 @@ struct roc_sg_plan {
   size_t carryLd = 0;
   uint32_t* carryArg = nullptr;   // [numCarries][carryLd] indices of the min / max carries (first use)
   size_t carryArgLd = 0;
+  float* carry2 = nullptr;        // [numCarries][16] attention: the heads-wide partials (first use)
+  float4* attnRec = nullptr;      // [recCap] attention backward: {s_dst, m, 1/Z, D} per (node id, head)
+  size_t recCap = 0;
+  uint64_t idEnd = 0;             // 1 + the largest id in col (found by the first attention backward)
+  bool idEndKnown = false;
   uint32_t* desc = nullptr;       // [numChunks][8] per-chunk start state of a worker (k_chunk_desc)
   int device = 0;
 };
@@ -198,7 +205,10 @@ template <> struct V<1> {
 // What a kernel does with each gathered row.  SUM adds it; MAX / MIN keep, per float, the value and the source id of
 // the first edge in CSR order that holds the extreme (roc_sg_minmax_forward_planned); MASK is the backward of those:
 // it adds the gathered gradient only where the gathered index names the row being computed.
-enum { SG_RED_SUM = 0, SG_RED_MAX = ROC_SG_AGGR_MAX, SG_RED_MIN = ROC_SG_AGGR_MIN, SG_RED_MASK = 3 };
+// The attention passes (roc_sg_attn_*): ASTAT gives each row's (m, Z) per head, ATTN the a-weighted sum, ADST the
+// destination-score gradient (heads wide), ASRC the input gradient and the source-score gradient.
+enum { SG_RED_SUM = 0, SG_RED_MAX = ROC_SG_AGGR_MAX, SG_RED_MIN = ROC_SG_AGGR_MIN, SG_RED_MASK = 3,
+       SG_RED_ASTAT = 4, SG_RED_ATTN = 5, SG_RED_ADST = 6, SG_RED_ASRC = 7 };
 constexpr uint32_t SG_NOARG = 0xFFFFFFFFu;   // index of a row that has no edge yet
 
 // The ordering rule: the candidate v replaces the current a iff it is strictly greater (smaller) or it is NaN and a
@@ -245,6 +255,49 @@ __device__ __forceinline__ void mask_add(float4& acc, const float4& g, const uin
 }
 __device__ __forceinline__ void mask_add(float& acc, float g, uint32_t a, uint32_t me) { acc += (a == me) ? g : 0.f; }
 
+// ------------------------------------------------------- attention helpers ---
+__device__ __forceinline__ float leaky(float z, float slope) { return z > 0.f ? z : slope * z; }
+// a = exp(y - m) / Z from the row's stats; a row of degree 0 (1/Z = 0) gives 0 whatever y is
+__device__ __forceinline__ float attn_alpha(float y, float m, float iz) { return iz == 0.f ? 0.f : expf(y - m) * iz; }
+// the product of two T-columns over their first nv floats (the rest of a partial last float4 is padding)
+__device__ __forceinline__ float dot_t(const float4& a, const float4& b, int nv) {
+  float s = a.x * b.x;
+  s += (nv > 1) ? a.y * b.y : 0.f;
+  s += (nv > 2) ? a.z * b.z : 0.f;
+  s += (nv > 3) ? a.w * b.w : 0.f;
+  return nv > 0 ? s : 0.f;
+}
+__device__ __forceinline__ float dot_t(float a, float b, int nv) { return nv > 0 ? a * b : 0.f; }
+__device__ __forceinline__ float4 attn_scale(float a, const float4& v) { return make_float4(a * v.x, a * v.y, a * v.z, a * v.w); }
+__device__ __forceinline__ float attn_scale(float a, float v) { return a * v; }
+// Per-head sums of d[ch] (lane `lane` holds T-column lane + ch*L; a head is 2^ftShift consecutive T-columns): first
+// across the chunks of one head in the lane (a pairwise tree), then across the head's lanes (an xor butterfly, whose
+// two operands are added in either order to the same bits, so every lane of the head ends with identical sums).
+// Every branch is uniform across the worker, as the shuffles need.
+template <int L, int NCH>
+__device__ __forceinline__ void head_sum(float (&d)[NCH], uint32_t ftShift, unsigned wmask) {
+  constexpr int LS = L == 4 ? 2 : L == 8 ? 3 : L == 16 ? 4 : 5;
+  const int gs = ftShift > (uint32_t)LS ? (int)min(ftShift - LS, 3u) : 0;     // log2 of the chunks per head
+#pragma unroll
+  for (int s = 0; (1 << s) < NCH; s++)
+#pragma unroll
+    for (int ch = 0; ch + (1 << s) < NCH; ch += 2 << s)
+      if (s < gs) d[ch] += d[ch + (1 << s)];
+  const int span = 1 << min((int)ftShift, LS);                               // lanes per head
+#pragma unroll
+  for (int ch = 0; ch < NCH; ch++)
+    if ((ch & ((1 << gs) - 1)) == 0)
+      for (int o = 1; o < span; o <<= 1) d[ch] += __shfl_xor_sync(wmask, d[ch], o, L);
+#pragma unroll
+  for (int ch = 1; ch < NCH; ch++) {            // every chunk takes its group's sum (indices resolved at compile time)
+    float v = d[ch];
+#pragma unroll
+    for (int g = 1; g <= 3; g++)
+      if (gs == g) v = d[ch & ~((1 << g) - 1)];
+    d[ch] = v;
+  }
+}
+
 struct SgParams {
   const uint32_t* rs;
   const uint32_t* firstRow;
@@ -264,8 +317,19 @@ struct SgParams {
   void* arg;            // MAX / MIN: [nloc][ldArg] indices written; MASK: [*][ldArg] indices gathered like `in`
   void* carryArg;       // MAX / MIN: [numCarries][ldC] indices of the carry partials
   size_t ldArg;         // in units of T
-  uint32_t selfBase;    // MASK: id of local row 0 in the id space of col
+  uint32_t selfBase;    // MASK, attention: id of local row 0 in the id space of col
+  // attention (units of float unless stated)
+  const float* score;   // [*][ldS]  s_dst | s_src, indexed like `in`
+  const float* stats;   // ATTN: [nloc][ldStats] m | 1/Z of the local rows
+  const float4* rec;    // ADST / ASRC: [*][heads] {s_dst, m, 1/Z, D}, indexed like `in`
+  const void* xrow;     // ADST: G, ASRC: X, the local row's own row (units of T, ldX), indexed like `in`
+  float* out2;          // ASTAT: unused; ADST / ASRC: heads-wide output [nloc][ldOut2]
+  float* carry2;        // [numCarries][SG_LDC2] heads-wide partials (ASTAT: m | Z)
+  size_t ldS, ldStats, ldX, ldOut2;
+  uint32_t heads, ftShift, H;   // ftShift: log2 of the T-columns per head (31 for one head)
+  float slope;
 };
+constexpr int SG_LDC2 = 16;     // 2 * the most heads
 
 // out[v] = relu?(acc / sqrtf(deg)) — what the model applies right after
 // scatter_gather (gnn.cc:84-85), IEEE sqrt and divide like graphnorm_kernel.cu:49-51.
@@ -292,11 +356,16 @@ sg_chunk_kernel(const SgParams p) {
   typedef typename V<VEC>::T T;
   typedef typename V<VEC>::I I;
   constexpr bool MM = RED == SG_RED_MAX || RED == SG_RED_MIN;
+  constexpr bool AT = RED >= SG_RED_ASTAT;                       // an attention pass
+  constexpr bool SV = RED == SG_RED_ATTN || RED == SG_RED_ADST;  // gathers s_src[j] beside in[j]
+  constexpr bool XI = RED == SG_RED_ADST || RED == SG_RED_ASRC;  // holds a row of its own row i, and heads-wide sums
   constexpr int WPB = SG_THREADS / L;
   constexpr uint32_t CH = SG_CH;
   const int lane = threadIdx.x % L;
   const uint32_t w = blockIdx.x * WPB + threadIdx.x / L;
   if (w >= p.numChunks) return;
+  const unsigned wmask = (L == 32) ? 0xffffffffu : (((1u << L) - 1u) << (((threadIdx.x & 31) / L) * L));
+  (void)wmask;
 
   const uint32_t* __restrict__ rs = p.rs;
   const uint32_t* __restrict__ col = p.col;
@@ -333,6 +402,43 @@ sg_chunk_kernel(const SgParams p) {
     if constexpr (MM) aidx[ch] = mm_noarg((I*)nullptr);
   }
 
+  // Attention: the head of each column chunk, its valid floats, and the current row's state (row_state).
+  constexpr int NA = AT ? NCH : 1;
+  uint32_t kh[NA];
+  int nv[NA];
+  float accS[NA];       // ASTAT: Z (acc holds m); ADST / ASRC: the heads-wide sums
+  float r0s[NA], r1s[NA], r2s[NA];   // ASTAT: s_dst[i]; ATTN: s_dst[i], m[i], 1/Z[i]; ASRC: s_src[i]
+  float4 rrec[RED == SG_RED_ADST ? NCH : 1];   // ADST: the record of row i
+  T xi[XI ? NCH : 1];   // ADST: G[i], ASRC: X[i]
+  if constexpr (AT) {
+#pragma unroll
+    for (int ch = 0; ch < NCH; ch++) {
+      const uint32_t c = (uint32_t)(lane + ch * L);
+      kh[ch] = min(c, p.Q - 1u) >> p.ftShift;
+      nv[ch] = (VEC == 4) ? max(0, min(4, (int)p.H - 4 * (int)c)) : (c < p.Q ? 1 : 0);
+      accS[ch] = 0.f;
+      if constexpr (RED == SG_RED_ASTAT) acc[ch] = -INFINITY;
+    }
+  }
+  auto row_state = [&]() {
+    if constexpr (AT) {
+      const uint64_t gi = (uint64_t)(p.selfBase + cur);
+#pragma unroll
+      for (int ch = 0; ch < NCH; ch++) {
+        if constexpr (RED == SG_RED_ASTAT || RED == SG_RED_ATTN) r0s[ch] = __ldg(p.score + gi * p.ldS + kh[ch]);
+        if constexpr (RED == SG_RED_ATTN) {
+          r1s[ch] = __ldg(p.stats + (uint64_t)cur * p.ldStats + kh[ch]);
+          r2s[ch] = __ldg(p.stats + (uint64_t)cur * p.ldStats + p.heads + kh[ch]);
+        }
+        if constexpr (RED == SG_RED_ASRC) r0s[ch] = __ldg(p.score + gi * p.ldS + p.heads + kh[ch]);
+        if constexpr (RED == SG_RED_ADST) rrec[ch] = __ldg(p.rec + gi * p.heads + kh[ch]);
+        if constexpr (XI)
+          xi[ch] = V<VEC>::ld(reinterpret_cast<const T*>(p.xrow) + gi * p.ldX + min((uint32_t)(lane + ch * L), p.Q - 1u));
+      }
+    }
+  };
+  row_state();
+
   // Row store.  The epilogue (IEEE sqrt + divides) lives in ONE out-of-line copy:
   // inlining it at every edge position made the kernel 4096 SASS instructions and
   // instruction-fetch bound.
@@ -358,6 +464,31 @@ sg_chunk_kernel(const SgParams p) {
       }
       return;
     }
+    if constexpr (RED == SG_RED_ASTAT) {
+      // lane k holds head k's (m, Z): a complete row stores m and 1/Z (0 and 0 with no edge), a cut row's parts their
+      // raw (m, Z) for sg_attn_stat_fixup
+      float* sdst = (kind == 0) ? p.carry2 + (uint64_t)carrySlot * SG_LDC2 : reinterpret_cast<float*>(p.out) + (uint64_t)cur * p.ldOut;
+      if (act[0]) {
+        const float m = acc[0], z = accS[0];
+        const bool done = kind == 1;
+        sdst[lane] = (done && !(z > 0.f)) ? 0.f : m;
+        sdst[p.heads + lane] = !done ? z : (z > 0.f ? 1.f / z : 0.f);
+      }
+      acc[0] = -INFINITY; accS[0] = 0.f;
+      return;
+    }
+    if constexpr (XI) {
+      // the heads-wide sums: the lane of a head's first column stores them
+      float* d2 = (kind == 0) ? p.carry2 + (uint64_t)carrySlot * SG_LDC2 : p.out2 + (uint64_t)cur * p.ldOut2;
+      const uint32_t ftMask = (p.ftShift >= 31u) ? 0x7FFFFFFFu : ((1u << p.ftShift) - 1u);
+#pragma unroll
+      for (int ch = 0; ch < NCH; ch++) {
+        const uint32_t c = (uint32_t)(lane + ch * L);
+        if (c < p.Q && (c & ftMask) == 0) d2[kh[ch]] = accS[ch];
+        accS[ch] = 0.f;
+      }
+      if constexpr (RED == SG_RED_ADST) return;
+    }
     const int epi = (kind == 1) ? p.epi : 0;
 #pragma unroll
     for (int ch = 0; ch < NCH; ch++) {
@@ -373,6 +504,7 @@ sg_chunk_kernel(const SgParams p) {
     bool heavy = curT - curS > CH;
     segEnd = heavy ? min(curT, ce) : curT;
     kind = heavy ? 2 : 1;
+    row_state();
   };
 
   // Every lane reads the source ids itself (same address across the worker: one broadcast
@@ -413,6 +545,8 @@ sg_chunk_kernel(const SgParams p) {
     }
     T v[U][NCH];
     I av[RED == SG_RED_MASK ? U : 1][RED == SG_RED_MASK ? NCH : 1];
+    float sv[SV ? U : 1][SV ? NCH : 1];                              // ATTN / ADST: s_src[j] of each chunk's head
+    float4 rv[RED == SG_RED_ASRC ? U : 1][RED == SG_RED_ASRC ? NCH : 1];   // ASRC: the record of j
 #pragma unroll
     for (int u = 0; u < U; u++) {
       const uint64_t off = (uint64_t)srcs[u] * rowBytes;
@@ -422,6 +556,14 @@ sg_chunk_kernel(const SgParams p) {
         const uint64_t aoff = (uint64_t)srcs[u] * argRowBytes;
 #pragma unroll
         for (int ch = 0; ch < NCH; ch++) av[u][ch] = __ldg(reinterpret_cast<const I*>(argl[ch] + aoff));
+      }
+      if constexpr (SV) {
+#pragma unroll
+        for (int ch = 0; ch < NCH; ch++) sv[u][ch] = __ldg(p.score + (uint64_t)srcs[u] * p.ldS + p.heads + kh[ch]);
+      }
+      if constexpr (RED == SG_RED_ASRC) {
+#pragma unroll
+        for (int ch = 0; ch < NCH; ch++) rv[u][ch] = __ldg(p.rec + (uint64_t)srcs[u] * p.heads + kh[ch]);
       }
     }
     {
@@ -437,11 +579,51 @@ sg_chunk_kernel(const SgParams p) {
 #pragma unroll
         for (int u = 0; u < U; u++) {
           if ((uint32_t)u >= pos && (uint32_t)u < lim) {
+            if constexpr (RED == SG_RED_ASTAT) {
+              // online (m, Z) of head `lane`: the running max is exact, Z is rescaled when it grows
+              const float y = leaky(r0s[0] + v[u][0], p.slope);
+              float& m = acc[0];
+              if (y > m) { accS[0] = accS[0] * expf(m - y) + 1.f; m = y; }
+              else accS[0] += expf(y - m);
+            } else if constexpr (RED == SG_RED_ATTN) {
 #pragma unroll
-            for (int ch = 0; ch < NCH; ch++) {
-              if constexpr (RED == SG_RED_SUM) V<VEC>::add(acc[ch], v[u][ch]);
-              else if constexpr (RED == SG_RED_MASK) mask_add(acc[ch], v[u][ch], av[u][ch], p.selfBase + cur);
-              else mm_add<RED>(acc[ch], aidx[ch], v[u][ch], srcs[u]);
+              for (int ch = 0; ch < NCH; ch++) {
+                const float a = attn_alpha(leaky(r0s[ch] + sv[u][ch], p.slope), r1s[ch], r2s[ch]);
+                V<VEC>::add(acc[ch], attn_scale(a, v[u][ch]));
+              }
+            } else if constexpr (RED == SG_RED_ADST) {
+              // dz(i<-j) = a(i<-j) (G[i].X[j] - D[i]) l: v is X[j], xi is G[i], rrec is {s_dst, m, 1/Z, D} of i
+              float d[NCH];
+#pragma unroll
+              for (int ch = 0; ch < NCH; ch++) d[ch] = dot_t(xi[ch], v[u][ch], nv[ch]);
+              head_sum<L, NCH>(d, p.ftShift, wmask);
+#pragma unroll
+              for (int ch = 0; ch < NCH; ch++) {
+                const float z = rrec[ch].x + sv[u][ch];
+                const float a = attn_alpha(leaky(z, p.slope), rrec[ch].y, rrec[ch].z);
+                accS[ch] += a * (d[ch] - rrec[ch].w) * (z > 0.f ? 1.f : p.slope);
+              }
+            } else if constexpr (RED == SG_RED_ASRC) {
+              // a(j<-i) G[j] and dz(j<-i) = a(j<-i) (G[j].X[i] - D[j]) l: v is G[j], xi is X[i], rv the record of j
+              float d[NCH];
+#pragma unroll
+              for (int ch = 0; ch < NCH; ch++) d[ch] = dot_t(v[u][ch], xi[ch], nv[ch]);
+              head_sum<L, NCH>(d, p.ftShift, wmask);
+#pragma unroll
+              for (int ch = 0; ch < NCH; ch++) {
+                const float4 r = rv[u][ch];
+                const float z = r.x + r0s[ch];
+                const float a = attn_alpha(leaky(z, p.slope), r.y, r.z);
+                V<VEC>::add(acc[ch], attn_scale(a, v[u][ch]));
+                accS[ch] += a * (d[ch] - r.w) * (z > 0.f ? 1.f : p.slope);
+              }
+            } else {
+#pragma unroll
+              for (int ch = 0; ch < NCH; ch++) {
+                if constexpr (RED == SG_RED_SUM) V<VEC>::add(acc[ch], v[u][ch]);
+                else if constexpr (RED == SG_RED_MASK) mask_add(acc[ch], v[u][ch], av[u][ch], p.selfBase + cur);
+                else mm_add<RED>(acc[ch], aidx[ch], v[u][ch], srcs[u]);
+              }
             }
           }
         }
@@ -948,6 +1130,161 @@ static int dispatch(const SgParams& p, cudaStream_t st) {
   return ROC_ERR_UNSUPPORTED;
 }
 
+// ------------------------------------------------------- attention kernels ---
+// (m, Z) partials of one head merged: the max is exact, each Z rescaled to it.  merge(a, b) and merge(b, a) give the
+// same bits, which the butterfly below relies on.  A partial with Z = 0 has no edge.
+__device__ __forceinline__ void attn_merge(float& m, float& z, float m2, float z2) {
+  if (!(z2 > 0.f)) return;
+  if (!(z > 0.f)) { m = m2; z = z2; return; }
+  const float M = fmaxf(m, m2);
+  z = z * expf(m - M) + z2 * expf(m2 - M);
+  m = M;
+}
+
+// Finishes the stats of every row the ASTAT pass cut (heavy and big rows alike): one warp per row, lane l merging
+// carries l, l + 32, ... in order, then an xor butterfly, then the owner's partial; stores m and 1/Z.  The order is
+// fixed by the plan, so the result is reproducible.
+__global__ void __launch_bounds__(SG_THREADS)
+sg_attn_stat_fixup(const SgParams p) {
+  constexpr uint32_t CH = SG_CH;
+  const uint32_t w = (blockIdx.x * SG_THREADS + threadIdx.x) / 32, lane = threadIdx.x % 32;
+  if (w >= p.numHeavy + p.numBig) return;
+  const uint32_t R = w < p.numHeavy ? p.heavyRows[w] : p.bigRows[w - p.numHeavy];
+  const uint32_t s = p.rs[R], t = p.rs[R + 1];
+  const uint32_t c0 = s / CH, n = (t - 1) / CH - c0;
+  const float* cb = p.carry2 + (uint64_t)p.carryIdx[c0 + 1] * SG_LDC2;
+  float* dst = reinterpret_cast<float*>(p.out) + (uint64_t)R * p.ldOut;
+  for (uint32_t k = 0; k < p.heads; k++) {
+    float m = 0.f, z = 0.f;
+    for (uint32_t i = lane; i < n; i += 32) attn_merge(m, z, cb[(uint64_t)i * SG_LDC2 + k], cb[(uint64_t)i * SG_LDC2 + p.heads + k]);
+#pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) {
+      const float m2 = __shfl_xor_sync(0xffffffffu, m, o), z2 = __shfl_xor_sync(0xffffffffu, z, o);
+      attn_merge(m, z, m2, z2);
+    }
+    if (lane == 0) {
+      float mo = dst[k], zo = dst[p.heads + k];
+      attn_merge(mo, zo, m, z);
+      dst[k] = mo;
+      dst[p.heads + k] = 1.f / zo;
+    }
+  }
+}
+
+// The backward's per-node record {s_dst, m, 1/Z, D} of ids [0, n): one worker of L lanes per node, D[k] = G[k] . O[k]
+// reduced per head like the gathers' dot products.
+template <int VEC, int L, int NCH>
+__global__ void __launch_bounds__(SG_THREADS)
+sg_attn_rec_kernel(const SgParams p, const void* G, size_t ldG, const void* O, size_t ldO, uint32_t n) {
+  typedef typename V<VEC>::T T;
+  constexpr int WPB = SG_THREADS / L;
+  const int lane = threadIdx.x % L;
+  const uint32_t v = blockIdx.x * WPB + threadIdx.x / L;
+  if (v >= n) return;
+  const unsigned wmask = (L == 32) ? 0xffffffffu : (((1u << L) - 1u) << (((threadIdx.x & 31) / L) * L));
+  const T* g = reinterpret_cast<const T*>(G) + (uint64_t)v * ldG;
+  const T* o = reinterpret_cast<const T*>(O) + (uint64_t)v * ldO;
+  float d[NCH];
+#pragma unroll
+  for (int ch = 0; ch < NCH; ch++) {
+    const uint32_t c = (uint32_t)(lane + ch * L);
+    const int nv = (VEC == 4) ? max(0, min(4, (int)p.H - 4 * (int)c)) : (c < p.Q ? 1 : 0);
+    const uint32_t cc = min(c, p.Q - 1u);
+    d[ch] = dot_t(V<VEC>::ld(g + cc), V<VEC>::ld(o + cc), nv);
+  }
+  head_sum<L, NCH>(d, p.ftShift, wmask);
+  const uint32_t ftMask = (p.ftShift >= 31u) ? 0x7FFFFFFFu : ((1u << p.ftShift) - 1u);
+#pragma unroll
+  for (int ch = 0; ch < NCH; ch++) {
+    const uint32_t c = (uint32_t)(lane + ch * L);
+    if (c < p.Q && (c & ftMask) == 0) {
+      const uint32_t k = c >> p.ftShift;
+      const_cast<float4*>(p.rec)[(uint64_t)v * p.heads + k] =
+          make_float4(p.score[(uint64_t)v * p.ldS + k], p.stats[(uint64_t)v * p.ldStats + k],
+                      p.stats[(uint64_t)v * p.ldStats + p.heads + k], d[ch]);
+    }
+  }
+}
+
+// One attention pass: the main kernel, then the fix-ups of the rows it cut.  ASTAT has its own; the H-wide partials
+// (ATTN, ASRC) and the heads-wide ones (ADST, ASRC; p2 = p with out2 / carry2 as a VEC = 1, Q = heads output) are
+// sums, finished by the sum's fix-ups.
+template <int VEC, int L, int NCH, int U, int MINB, int RED>
+static int launch_attn(const SgParams& p, cudaStream_t st) {
+  constexpr int WPB = SG_THREADS / L;
+  if (p.numChunks) {
+    sg_chunk_kernel<VEC, L, NCH, U, MINB, RED><<<(p.numChunks + WPB - 1) / WPB, SG_THREADS, 0, st>>>(p);
+    ROC_LAUNCH_CHECK();
+  }
+  if (RED == SG_RED_ASTAT) {
+    const uint32_t rows = p.numHeavy + p.numBig;
+    if (rows) {
+      sg_attn_stat_fixup<<<(rows + SG_THREADS / 32 - 1) / (SG_THREADS / 32), SG_THREADS, 0, st>>>(p);
+      ROC_LAUNCH_CHECK();
+    }
+    return ROC_OK;
+  }
+  if (RED != SG_RED_ADST) {
+    if (p.numHeavy) {
+      sg_fixup_kernel<VEC, L, NCH, SG_RED_SUM><<<(p.numHeavy + WPB - 1) / WPB, SG_THREADS, 0, st>>>(p);
+      ROC_LAUNCH_CHECK();
+    }
+    if (p.numBig) {
+      sg_fixup_big_kernel<VEC, L, NCH, SG_RED_SUM><<<p.numBig, SG_THREADS, 0, st>>>(p);
+      ROC_LAUNCH_CHECK();
+    }
+  }
+  if (RED == SG_RED_ADST || RED == SG_RED_ASRC) {
+    SgParams p2 = p;
+    p2.out = p.out2; p2.ldOut = p.ldOut2; p2.carry = p.carry2; p2.ldC = SG_LDC2; p2.Q = p.heads;
+    constexpr int L2 = 8, W2 = SG_THREADS / L2;
+    if (p.numHeavy) {
+      sg_fixup_kernel<1, L2, 1, SG_RED_SUM><<<(p.numHeavy + W2 - 1) / W2, SG_THREADS, 0, st>>>(p2);
+      ROC_LAUNCH_CHECK();
+    }
+    if (p.numBig) {
+      sg_fixup_big_kernel<1, L2, 1, SG_RED_SUM><<<p.numBig, SG_THREADS, 0, st>>>(p2);
+      ROC_LAUNCH_CHECK();
+    }
+  }
+  return ROC_OK;
+}
+
+// Kernel shape of an H-wide attention pass (or of the record kernel, REC) for Q T-columns: the sum's lane and chunk
+// counts, fewer gathers in flight where the second gathered value (s_src, the record) would otherwise spill.
+template <int VEC, int RED, bool REC = false>
+static int dispatch_attn(const SgParams& p, cudaStream_t st, const void* G = nullptr, size_t ldG = 0,
+                         const void* O = nullptr, size_t ldO = 0, uint32_t n = 0) {
+  constexpr int UB = RED == SG_RED_ASRC ? 2 : 4;     // gathers in flight at one chunk per lane
+  constexpr int MB2 = RED == SG_RED_ASRC ? 2 : 3;    // CTAs per SM at two chunks per lane, ...
+  constexpr int MB8 = RED == SG_RED_ATTN ? 2 : 1;    // ... and at eight (the row held in registers needs more)
+  const uint32_t Q = p.Q;
+#define SG_ATTN_SHAPE(L_, NCH_, U_, MINB_)                                                                    \
+  do {                                                                                                        \
+    if constexpr (REC) {                                                                                      \
+      if (n) {                                                                                                \
+        constexpr int W_ = SG_THREADS / (L_);                                                                 \
+        sg_attn_rec_kernel<VEC, L_, NCH_><<<(n + W_ - 1) / W_, SG_THREADS, 0, st>>>(p, G, ldG, O, ldO, n);     \
+        ROC_LAUNCH_CHECK();                                                                                   \
+      }                                                                                                       \
+      return ROC_OK;                                                                                          \
+    } else {                                                                                                  \
+      return launch_attn<VEC, L_, NCH_, U_, MINB_, RED>(p, st);                                               \
+    }                                                                                                         \
+  } while (0)
+  if (Q <= 4) SG_ATTN_SHAPE(4, 1, UB, 4);
+  if (Q <= 8) SG_ATTN_SHAPE(8, 1, UB, 4);
+  if (Q <= 16) SG_ATTN_SHAPE(16, 1, UB, 4);
+  if (Q <= 32) SG_ATTN_SHAPE(32, 1, UB, 4);
+  if (Q <= 64) SG_ATTN_SHAPE(32, 2, 2, MB2);
+  if (Q <= 128) SG_ATTN_SHAPE(32, 4, 1, 2);
+  if constexpr (VEC == 1) {
+    if (Q <= 256) SG_ATTN_SHAPE(32, 8, 1, MB8);
+  }
+#undef SG_ATTN_SHAPE
+  return ROC_ERR_UNSUPPORTED;
+}
+
 // Carry slots for rows cut at chunk boundaries.  roc_sg_plan_reserve sizes them up front (plain cudaMalloc, an
 // init-time call).  A launch that still finds them too small grows them on its own stream with stream-ordered
 // allocation: the old buffer is returned in stream order, after the launches that used it — no device
@@ -978,6 +1315,52 @@ static int ensure_carry_arg(roc_sg_plan* plan, cudaStream_t st) {
   cudaError_t e = cudaMallocAsync((void**)&plan->carryArg, bytes, st);
   if (e != cudaSuccess) { plan->carryArg = nullptr; plan->carryArgLd = 0; return (int)e; }
   plan->carryArgLd = plan->carryLd;
+  return ROC_OK;
+}
+
+// The heads-wide carries of the attention passes, [numCarries][SG_LDC2], allocated on first use like carryArg.
+static int ensure_carry2(roc_sg_plan* plan, cudaStream_t st) {
+  if (plan->numCarries == 0 || plan->carry2) return ROC_OK;
+  const size_t bytes = (size_t)plan->numCarries * SG_LDC2 * sizeof(float);
+  cudaError_t e = cudaMallocAsync((void**)&plan->carry2, bytes, st);
+  if (e != cudaSuccess) { plan->carry2 = nullptr; return (int)e; }
+  return ROC_OK;
+}
+
+// The attention backward's node records, grown in stream order to `n` entries.
+static int ensure_rec(roc_sg_plan* plan, size_t n, cudaStream_t st) {
+  if (n <= plan->recCap) return ROC_OK;
+  if (plan->attnRec) { ROC_CUDA(cudaFreeAsync(plan->attnRec, st)); plan->attnRec = nullptr; plan->recCap = 0; }
+  cudaError_t e = cudaMallocAsync((void**)&plan->attnRec, n * sizeof(float4), st);
+  if (e != cudaSuccess) { plan->attnRec = nullptr; return (int)e; }
+  plan->recCap = n;
+  return ROC_OK;
+}
+
+// 1 + the largest id in col, found once (one reduction and one synchronisation of the stream) and kept in the plan.
+static int find_id_end(roc_sg_plan* plan, cudaStream_t st) {
+  if (plan->idEndKnown) return ROC_OK;
+  uint64_t idEnd = 0;
+  if (plan->E) {
+    uint32_t* dmax = nullptr;
+    void* tmp = nullptr;
+    size_t tb = 0;
+    uint32_t h = 0;
+    cudaError_t e = cub::DeviceReduce::Max(nullptr, tb, plan->col, dmax, (int)plan->E, st);
+    if (e == cudaSuccess) e = cudaMallocAsync((void**)&dmax, 16 + (tb ? tb : 16), st);   // the max, then cub's scratch
+    if (e == cudaSuccess) {
+      tmp = reinterpret_cast<char*>(dmax) + 16;
+      e = cub::DeviceReduce::Max(tmp, tb, plan->col, dmax, (int)plan->E, st);
+      count_launch();
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&h, dmax, sizeof(uint32_t), cudaMemcpyDeviceToHost, st);
+    if (dmax) { cudaError_t f = cudaFreeAsync(dmax, st); if (e == cudaSuccess) e = f; }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return (int)e;
+    idEnd = (uint64_t)h + 1;
+  }
+  plan->idEnd = idEnd;
+  plan->idEndKnown = true;
   return ROC_OK;
 }
 
@@ -1061,7 +1444,7 @@ done:
 extern "C" void roc_sg_plan_destroy(roc_sg_plan* pl) {
   if (!pl) return;
   cudaFree(pl->rs); cudaFree(pl->firstRow); cudaFree(pl->carryIdx); cudaFree(pl->heavyRows); cudaFree(pl->bigRows); cudaFree(pl->carry); cudaFree(pl->desc);
-  cudaFree(pl->carryArg);
+  cudaFree(pl->carryArg); cudaFree(pl->carry2); cudaFree(pl->attnRec);
   delete pl;
 }
 
@@ -1168,6 +1551,102 @@ extern "C" int roc_sg_minmax_backward_planned(const roc_sg_plan* plc, int H, roc
   roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
   if (!pl || H <= 0 || !outGrad || !arg || !inGrad || ldG < H || ldArg < H || ldIn < H) return ROC_ERR_INVALID;
   return run_planned<SG_RED_MASK>(pl, H, outGrad, ldG, inGrad, ldIn, arg, ldArg, 0, selfBase, as_stream(stream));
+}
+
+// The head layout of an attention call whose pointers and leading dimensions are valid: ROC_ERR_INVALID for a bad
+// slope, ROC_ERR_UNSUPPORTED for a layout the kernels do not take; *ftShift = log2 of the T-columns per head.
+static int attn_layout(int heads, int H, float slope, bool vec, uint32_t* ftShift) {
+  if (!(slope >= 0.f) || !std::isfinite(slope)) return ROC_ERR_INVALID;
+  if ((heads != 1 && heads != 2 && heads != 4 && heads != 8) || H % heads) return ROC_ERR_UNSUPPORTED;
+  const int F = H / heads;
+  if (heads > 1 && (F < 4 || (F & (F - 1)))) return ROC_ERR_UNSUPPORTED;
+  if (H > (vec ? 512 : 256)) return ROC_ERR_UNSUPPORTED;
+  uint32_t fs = 0;
+  while ((1 << fs) < F / (vec ? 4 : 1)) fs++;
+  *ftShift = heads == 1 ? 31u : fs;
+  return ROC_OK;
+}
+
+// The parameters every attention pass shares (units of T set by the caller).
+static SgParams attn_params(const roc_sg_plan* pl, int heads, int H, float slope, roc_vid_t selfBase,
+                            const float* score, int64_t ldS, const float* stats, int64_t ldStats, uint32_t ftShift) {
+  SgParams p = plan_params(pl);
+  p.carry2 = pl->carry2; p.rec = pl->attnRec;
+  p.selfBase = selfBase; p.score = score; p.ldS = (size_t)ldS; p.stats = stats; p.ldStats = (size_t)ldStats;
+  p.heads = (uint32_t)heads; p.H = (uint32_t)H; p.slope = slope; p.ftShift = ftShift;
+  return p;
+}
+
+extern "C" int roc_sg_attn_forward_planned(const roc_sg_plan* plc, int heads, int H, float slope, roc_vid_t selfBase,
+                                           const float* in, int64_t ldIn, const float* score, int64_t ldS,
+                                           float* out, int64_t ldOut, float* stats, int64_t ldStats,
+                                           roc_stream_t stream) {
+  roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  if (!pl || !in || !score || !out || !stats || heads <= 0 || H <= 0 || ldIn < H || ldOut < H ||
+      ldS < 2 * (int64_t)heads || ldStats < 2 * (int64_t)heads)
+    return ROC_ERR_INVALID;
+  const bool vec = ldIn % 4 == 0 && ldOut % 4 == 0 && aligned16(in) && aligned16(out);
+  uint32_t fs = 0;
+  int rc = attn_layout(heads, H, slope, vec, &fs);
+  if (rc != ROC_OK) return rc;
+  cudaStream_t st = as_stream(stream);
+  if ((rc = ensure_carry(pl, ((size_t)H + 3) / 4 * 4, st, true)) != ROC_OK) return rc;
+  if ((rc = ensure_carry2(pl, st)) != ROC_OK) return rc;
+  // pass 1: (m, 1/Z) per row and head from the scores alone
+  SgParams a = attn_params(pl, heads, H, slope, selfBase, score, ldS, stats, ldStats, 0);
+  a.in = score + heads; a.ldIn = (size_t)ldS; a.out = stats; a.ldOut = (size_t)ldStats; a.Q = (uint32_t)heads;
+  rc = heads <= 4 ? launch_attn<1, 4, 1, 8, 4, SG_RED_ASTAT>(a, st) : launch_attn<1, 8, 1, 8, 4, SG_RED_ASTAT>(a, st);
+  if (rc != ROC_OK) return rc;
+  // pass 2: the a-weighted sum of the feature rows
+  const int vw = vec ? 4 : 1;
+  SgParams b = attn_params(pl, heads, H, slope, selfBase, score, ldS, stats, ldStats, fs);
+  b.in = in; b.ldIn = (size_t)ldIn / vw; b.out = out; b.ldOut = (size_t)ldOut / vw; b.ldC = pl->carryLd / vw;
+  b.Q = ((uint32_t)H + vw - 1) / vw;
+  return vec ? dispatch_attn<4, SG_RED_ATTN>(b, st) : dispatch_attn<1, SG_RED_ATTN>(b, st);
+}
+
+extern "C" int roc_sg_attn_backward_planned(const roc_sg_plan* plc, int heads, int H, float slope, roc_vid_t selfBase,
+                                            const float* in, int64_t ldIn, const float* score, int64_t ldS,
+                                            const float* out, int64_t ldOut, const float* stats, int64_t ldStats,
+                                            const float* outGrad, int64_t ldG, float* inGrad, int64_t ldInG,
+                                            float* scoreGrad, int64_t ldSG, roc_stream_t stream) {
+  roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  if (!pl || !in || !score || !out || !stats || !outGrad || !inGrad || !scoreGrad || heads <= 0 || H <= 0 ||
+      ldIn < H || ldOut < H || ldG < H || ldInG < H || ldS < 2 * (int64_t)heads || ldStats < 2 * (int64_t)heads ||
+      ldSG < 2 * (int64_t)heads)
+    return ROC_ERR_INVALID;
+  const bool vec = ldIn % 4 == 0 && ldOut % 4 == 0 && ldG % 4 == 0 && ldInG % 4 == 0 && aligned16(in) &&
+                   aligned16(out) && aligned16(outGrad) && aligned16(inGrad);
+  uint32_t fs = 0;
+  int rc = attn_layout(heads, H, slope, vec, &fs);
+  if (rc != ROC_OK) return rc;
+  cudaStream_t st = as_stream(stream);
+  if ((rc = find_id_end(pl, st)) != ROC_OK) return rc;
+  const uint64_t n64 = std::max<uint64_t>(pl->idEnd, (uint64_t)selfBase + pl->nloc);
+  if (n64 >= 0xFFFFFFF0ull) return ROC_ERR_UNSUPPORTED;
+  const uint32_t n = (uint32_t)n64;
+  if ((rc = ensure_rec(pl, (size_t)n * heads, st)) != ROC_OK) return rc;
+  if ((rc = ensure_carry(pl, ((size_t)H + 3) / 4 * 4, st, true)) != ROC_OK) return rc;
+  if ((rc = ensure_carry2(pl, st)) != ROC_OK) return rc;
+  const int vw = vec ? 4 : 1;
+  SgParams p = attn_params(pl, heads, H, slope, selfBase, score, ldS, stats, ldStats, fs);
+  p.ldC = pl->carryLd / vw;
+  p.Q = ((uint32_t)H + vw - 1) / vw;
+  // the node records {s_dst, m, 1/Z, D}
+  rc = vec ? dispatch_attn<4, SG_RED_ATTN, true>(p, st, outGrad, (size_t)ldG / 4, out, (size_t)ldOut / 4, n)
+           : dispatch_attn<1, SG_RED_ATTN, true>(p, st, outGrad, (size_t)ldG, out, (size_t)ldOut, n);
+  if (rc != ROC_OK) return rc;
+  // B1: d s_dst, gathering X[j] and s_src[j] against G[i]
+  SgParams b1 = p;
+  b1.in = in; b1.ldIn = (size_t)ldIn / vw; b1.xrow = outGrad; b1.ldX = (size_t)ldG / vw;
+  b1.out = nullptr; b1.out2 = scoreGrad; b1.ldOut2 = (size_t)ldSG;
+  rc = vec ? dispatch_attn<4, SG_RED_ADST>(b1, st) : dispatch_attn<1, SG_RED_ADST>(b1, st);
+  if (rc != ROC_OK) return rc;
+  // B2: inGrad and d s_src, gathering G[j] and the record of j against X[i]
+  SgParams b2 = p;
+  b2.in = outGrad; b2.ldIn = (size_t)ldG / vw; b2.xrow = in; b2.ldX = (size_t)ldIn / vw;
+  b2.out = inGrad; b2.ldOut = (size_t)ldInG / vw; b2.out2 = scoreGrad + heads; b2.ldOut2 = (size_t)ldSG;
+  return vec ? dispatch_attn<4, SG_RED_ASRC>(b2, st) : dispatch_attn<1, SG_RED_ASRC>(b2, st);
 }
 
 extern "C" int roc_sg_forward(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft, int H,

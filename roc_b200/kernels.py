@@ -100,6 +100,37 @@ class SgPlan:
               "roc_sg_minmax_backward_planned")
         return out
 
+    def attn_forward(self, x, scores, heads=1, slope=0.2, self_base=0, out=None, stats=None):
+        """Attention aggregation (include/roc_b200.h) -> (out [Nloc][H], stats [Nloc][2*heads] = m | 1/Z per head).
+        x and scores ([*][2*heads] = s_dst | s_src) are indexed like minmax_forward's input."""
+        nloc = self.row_right - self.row_left + 1
+        h = x.shape[1]
+        if out is None:
+            out = padded(nloc, h, x.device) if _ld(x) % 4 == 0 else torch.empty((nloc, h), device=x.device)
+        if stats is None:
+            stats = torch.empty((nloc, 2 * heads), device=x.device)
+        check(lib.roc_sg_attn_forward_planned(self.handle, int(heads), h, float(slope), int(self_base), _ptr(x), _ld(x),
+                                              _ptr(scores), _ld(scores), _ptr(out), _ld(out), _ptr(stats),
+                                              _ld(stats), _stream()), "roc_sg_attn_forward_planned")
+        return out, stats
+
+    def attn_backward(self, x, scores, out, stats, gy, heads=1, slope=0.2, self_base=0, in_grad=None,
+                      score_grad=None):
+        """Its backward -> (in_grad [Nloc][H], score_grad [Nloc][2*heads] = d s_dst | d s_src).  x, scores, out, stats
+        and gy are indexed like the forward's input (for a whole graph: the forward's own outputs)."""
+        nloc = self.row_right - self.row_left + 1
+        h = x.shape[1]
+        if in_grad is None:
+            in_grad = padded(nloc, h, x.device) if _ld(x) % 4 == 0 else torch.empty((nloc, h), device=x.device)
+        if score_grad is None:
+            score_grad = torch.empty((nloc, 2 * heads), device=x.device)
+        check(lib.roc_sg_attn_backward_planned(self.handle, int(heads), h, float(slope), int(self_base), _ptr(x),
+                                               _ld(x), _ptr(scores), _ld(scores), _ptr(out), _ld(out), _ptr(stats),
+                                               _ld(stats), _ptr(gy), _ld(gy), _ptr(in_grad), _ld(in_grad),
+                                               _ptr(score_grad), _ld(score_grad), _stream()),
+              "roc_sg_attn_backward_planned")
+        return in_grad, score_grad
+
     def close(self):
         if self.handle:
             lib.roc_sg_plan_destroy(self.handle)

@@ -99,6 +99,11 @@ class Model:
             return lib.roc_host_scatter_gather(self.h, t)
         return lib.roc_host_scatter_gather_aggr(self.h, t, int(aggr))
 
+    def attention_gather(self, t, scores, heads=1, negative_slope=0.2):
+        """GAT aggregation of t (H = heads * F columns) weighted by a per-head softmax over each row's in-edges of
+        LeakyReLU(s_dst[v] + s_src[u]); scores has 2 * heads columns [s_dst | s_src].  One partition only."""
+        return lib.roc_host_attention_gather(self.h, t, scores, int(heads), float(negative_slope))
+
     def relu(self, t):
         return lib.roc_host_relu(self.h, t)
 
@@ -325,3 +330,45 @@ def build_sage_pool(model, layers, dropout_rate, aggr=_lib.AGGR_MAX, lr=0.01, we
     model.init()
     return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs, "pools": pools,
             "pool_ins": pool_ins}
+
+
+def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01, weight_decay=0.05):
+    """GAT (Velickovic et al., 2018) built from the reference's ops plus attention_gather.  `heads` (an int, or one
+    value per hidden layer) applies to the hidden layers; the last layer has one head.  layers[i] is the width of
+    layer i's output, heads_i * F_i.  Per layer:
+
+        d  = dropout(t)
+        wh = linear(d, layers[i])                       # heads_i * F_i columns
+        sc = linear(wh, 2 * heads_i)                    # [s_dst | s_src] per head
+        t  = attention_gather(wh, sc, heads_i, slope)   # per head, softmax over N(v) + v (self loops are in A)
+        t  = relu(t)                                    # all but the last layer
+
+    Where this differs from the paper: there is no bias (the reference's Linear has none); ReLU replaces ELU (the
+    engine has no ELU); with heads > 1 each head's scores are a dense projection of all heads' features, where the
+    paper uses a per-head block.  With one head it is GAT exactly.  Single partition.  Returns the handles, with
+    `attn` (the attention_gather outputs), `attn_ins` (their feature inputs) and `scores`."""
+    L = len(layers)
+    hs = list(heads) if isinstance(heads, (list, tuple)) else [int(heads)] * (L - 2)
+    assert len(hs) == L - 2, "one head count per hidden layer"
+    hs.append(1)
+    x = model.create_node_tensor(layers[0])
+    label = model.create_node_tensor(layers[-1])
+    mask = model.create_node_tensor(1, is_int=True)
+    t = x
+    relu_outs, attn, attn_ins, scores = [], [], [], []
+    for i in range(1, L):
+        d = model.dropout(t, dropout_rate)
+        wh = model.linear(d, layers[i], _lib.AC_MODE_NONE)
+        sc = model.linear(wh, 2 * hs[i - 1], _lib.AC_MODE_NONE)
+        t = model.attention_gather(wh, sc, hs[i - 1], negative_slope)
+        attn_ins.append(wh)
+        scores.append(sc)
+        attn.append(t)
+        if i != L - 1:
+            t = model.relu(t)
+            relu_outs.append(t)
+    model.softmax_cross_entropy(t, label, mask)
+    model.adam(lr, weight_decay)
+    model.init()
+    return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs, "attn": attn,
+            "attn_ins": attn_ins, "scores": scores}

@@ -2,7 +2,9 @@
 # compute-sanitizer over the tiny configuration (SURVEY §5): memcheck, then racecheck, on
 #   (a) __graft_entry__.smoke()  — one GCN training step through the Model API (SG, wgmma GEMMs, softmax, Adam)
 #   (b) the ScatterGather sum with the fused epilogue on a small R-MAT graph at 41, 64, 100, 200 and 602 floats, each
-#       followed by one max-aggregation forward and backward;
+#       followed by one max-aggregation forward and backward; then the attention forward and backward at 41 and 64
+#       floats with one head and at 64 and 256 floats with eight, on float4 rows, and at 256 floats with two heads on
+#       rows of 257 floats (the scalar path);
 #   (c) the warp-specialised dW kernel at 602 x 64 with the dropout mask and at 64 x 41, on rows that wrap its ring
 #       and end in a partial block.
 # Usage: tools/sanitize.sh [logdir]   (needs a GPU; `make sanitize`)
@@ -25,6 +27,18 @@ for h in (41, 64, 100, 200, 602):
     mx, arg = plan.minmax_forward(x, 1)                 # max aggregation and its backward
     g = plan.minmax_backward(x, arg)
     torch.cuda.synchronize()
+for h, heads in ((41, 1), (64, 1), (64, 8), (256, 8)):
+    x = K.padded(n, h, "cuda", fill=torch.rand((n, h), device="cuda"))
+    sc = torch.randn((n, 2 * heads), device="cuda")
+    out, stats = plan.attn_forward(x, sc, heads)
+    plan.attn_backward(x, sc, out, stats, x, heads)
+    torch.cuda.synchronize()
+xs = torch.rand((n, 257), device="cuda")[:, :256]            # ld = 257: the scalar path
+sc = torch.randn((n, 4), device="cuda")
+out = torch.zeros((n, 257), device="cuda")[:, :256]
+out, stats = plan.attn_forward(xs, sc, 2, out=out)
+plan.attn_backward(xs, sc, out, stats, xs, 2, in_grad=torch.zeros((n, 257), device="cuda")[:, :256])
+torch.cuda.synchronize()
 print("sg ok")
 PY
 cat > "$LOG/dw.py" <<'PY'

@@ -1,4 +1,4 @@
-// sg.cu — ScatterGather (CSR row-parallel SpMM, sum aggregation) for sm_90a.
+// sg.cu — ScatterGather (CSR row-parallel SpMM: sum, min / max and attention aggregation) for sm_90a.
 //
 // Replaces aggre_coop_kernel + ScatterGather::{forward,backward}_task
 // (reference scattergather_kernel.cu:20-76, 78-170).  The reference walks one
@@ -20,22 +20,28 @@
 //  * the main kernel, sg_chunk_kernel, gathers the neighbour rows in registers.  A row is Q T-columns (float4
 //    when the rows are 16-byte aligned, else float); a worker is L = 4, 8, 16 or 32 lanes, the fewest that cover
 //    Q, and each lane loads its NCH = ceil(Q / L) columns of U rows per group.  A launch covers up to 256
-//    T-columns (1024 floats vectorised, 256 scalar); wider rows are split into column blocks.
+//    T-columns (1024 floats vectorised, 256 scalar); wider rows are split into column blocks.  One table
+//    (with_shape, sg_chunk_u, sg_chunk_minb) gives every reduction its shape, and one launcher (launch) runs the
+//    main kernel and the fix-ups the reduction needs.
 //  * vectorised rows of 65..256 floats run on sg_chunk_kernel_t instead, which fetches them with cp.async.bulk
 //    copies into a shared-memory ring: it was faster there on a products-shaped graph (DESIGN.md §3.1).  It
 //    shares the plan and the per-row summation order, so its results are bit-identical to sg_chunk_kernel's.
 //  * min / max aggregation (roc_sg_minmax_*) runs the same kernel and fix-ups templated on the reduction; its
 //    backward is the sum schedule with a second gathered row and a predicated add, finished by the sum's fix-ups.
-//    The three planned entry points check their arguments and share one column-block driver (run_planned).
+//    The sum and min / max entry points check their arguments and share one column-block driver (run_planned).
+//  * attention aggregation (roc_sg_attn_*) is more reductions of the same kernel: a stats pass and an a-weighted
+//    sum forward; a per-node record kernel and two gathers backward.  Both entry points share attn_setup.
 //
 // Algorithmic bytes per launch (DESIGN.md): E*(4H+4) + Nloc*(4H+8); min / max forward E*(4H+4) + Nloc*(8H+8),
-// backward E*(8H+4) + Nloc*(4H+8).
+// backward E*(8H+4) + Nloc*(4H+8); attention in DESIGN.md §3.1.
 #include <cub/cub.cuh>
 #include <thrust/iterator/counting_iterator.h>
 #include <algorithm>
 #include <cmath>
 #include <cstring>
+#include <initializer_list>
 #include <new>
+#include <type_traits>
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -54,13 +60,15 @@ struct roc_sg_plan {
   uint32_t* heavyRows = nullptr;  // [numHeavy]  rows with degree > CH and <= 32 carries (one worker each)
   uint32_t* bigRows = nullptr;    // [numBig]    rows with more carries (one CTA each)
   const uint32_t* col = nullptr;  // caller's colSrc
+  // Grown on demand (grow); each *Bytes is its buffer's capacity.
   float* carry = nullptr;         // [numCarries][carryLd]
-  size_t carryLd = 0;
-  uint32_t* carryArg = nullptr;   // [numCarries][carryLd] indices of the min / max carries (first use)
-  size_t carryArgLd = 0;
-  float* carry2 = nullptr;        // [numCarries][16] attention: the heads-wide partials (first use)
-  float4* attnRec = nullptr;      // [recCap] attention backward: {s_dst, m, 1/Z, D} per (node id, head)
-  size_t recCap = 0;
+  size_t carryBytes = 0, carryLd = 0;
+  uint32_t* carryArg = nullptr;   // [numCarries][carryLd] indices of the min / max carries
+  size_t carryArgBytes = 0;
+  float* carry2 = nullptr;        // [numCarries][16] attention: the heads-wide partials
+  size_t carry2Bytes = 0;
+  float4* attnRec = nullptr;      // attention backward: {s_dst, m, 1/Z, D} per (node id, head)
+  size_t attnRecBytes = 0;
   uint64_t idEnd = 0;             // 1 + the largest id in col (found by the first attention backward)
   bool idEndKnown = false;
   uint32_t* desc = nullptr;       // [numChunks][8] per-chunk start state of a worker (k_chunk_desc)
@@ -331,6 +339,22 @@ struct SgParams {
 };
 constexpr int SG_LDC2 = 16;     // 2 * the most heads
 
+// The lanes of the calling thread's L-lane worker within its warp: the mask of the worker's sub-warp shuffles.
+template <int L>
+__device__ __forceinline__ unsigned worker_mask() {
+  return (L == 32) ? 0xffffffffu : (((1u << L) - 1u) << (((threadIdx.x & 31) / L) * L));
+}
+// Attention: the floats of T-column c that hold features (the rest of a partial last float4 is padding; none past Q).
+template <int VEC>
+__device__ __forceinline__ int t_floats(uint32_t c, const SgParams& p) {
+  return (VEC == 4) ? max(0, min(4, (int)p.H - 4 * (int)c)) : (c < p.Q ? 1 : 0);
+}
+// Attention: the bits of a T-column's index within its head.  Column c is the head's first, whose lane stores the
+// head's sums, when c < Q and (c & head_mask(p)) == 0.
+__device__ __forceinline__ uint32_t head_mask(const SgParams& p) {
+  return (p.ftShift >= 31u) ? 0x7FFFFFFFu : ((1u << p.ftShift) - 1u);
+}
+
 // out[v] = relu?(acc / sqrtf(deg)) — what the model applies right after
 // scatter_gather (gnn.cc:84-85), IEEE sqrt and divide like graphnorm_kernel.cu:49-51.
 // The divisor is uniform over the row, so the divide is the row-uniform form of common.cuh
@@ -364,7 +388,7 @@ sg_chunk_kernel(const SgParams p) {
   const int lane = threadIdx.x % L;
   const uint32_t w = blockIdx.x * WPB + threadIdx.x / L;
   if (w >= p.numChunks) return;
-  const unsigned wmask = (L == 32) ? 0xffffffffu : (((1u << L) - 1u) << (((threadIdx.x & 31) / L) * L));
+  const unsigned wmask = worker_mask<L>();
   (void)wmask;
 
   const uint32_t* __restrict__ rs = p.rs;
@@ -415,7 +439,7 @@ sg_chunk_kernel(const SgParams p) {
     for (int ch = 0; ch < NCH; ch++) {
       const uint32_t c = (uint32_t)(lane + ch * L);
       kh[ch] = min(c, p.Q - 1u) >> p.ftShift;
-      nv[ch] = (VEC == 4) ? max(0, min(4, (int)p.H - 4 * (int)c)) : (c < p.Q ? 1 : 0);
+      nv[ch] = t_floats<VEC>(c, p);
       accS[ch] = 0.f;
       if constexpr (RED == SG_RED_ASTAT) acc[ch] = -INFINITY;
     }
@@ -480,7 +504,7 @@ sg_chunk_kernel(const SgParams p) {
     if constexpr (XI) {
       // the heads-wide sums: the lane of a head's first column stores them
       float* d2 = (kind == 0) ? p.carry2 + (uint64_t)carrySlot * SG_LDC2 : p.out2 + (uint64_t)cur * p.ldOut2;
-      const uint32_t ftMask = (p.ftShift >= 31u) ? 0x7FFFFFFFu : ((1u << p.ftShift) - 1u);
+      const uint32_t ftMask = head_mask(p);
 #pragma unroll
       for (int ch = 0; ch < NCH; ch++) {
         const uint32_t c = (uint32_t)(lane + ch * L);
@@ -705,8 +729,7 @@ sg_chunk_kernel_t(const SgParams p) {
   const int wi = threadIdx.x / L;
   const uint32_t w = blockIdx.x * WPB + wi;
   if (w >= p.numChunks) return;
-  const unsigned wmask = (L == 32) ? 0xffffffffu
-                                   : (((1u << L) - 1u) << (((threadIdx.x & 31) / L) * L));
+  const unsigned wmask = worker_mask<L>();
   const uint32_t smem0 = (uint32_t)__cvta_generic_to_shared(sg_smem_t);
   const uint32_t ring = smem0 + wi * RINGB;
   const uint32_t bars = smem0 + WPB * RINGB + wi * (P * 8);
@@ -1057,79 +1080,6 @@ sg_fixup_big_kernel(const SgParams p) {
   }
 }
 
-// sg_chunk_kernel_t's two shapes, the measured defaults (DESIGN.md §3.1), four workers per CTA: rows of 65..128 floats
-// (one float4 per lane) with lane-held ids and two stages of two four-row units per worker; rows of 129..256 floats
-// with the ids loaded per stage and two stages of one unit.
-template <int NCH>
-static int launch_ring(const SgParams& p, cudaStream_t st) {
-  constexpr int L = 32, P = 2, NT = 128;
-  constexpr int S = NCH == 1 ? 2 : 1, MINB = NCH == 1 ? 4 : 6, MODE = NCH == 1 ? 2 : 0;
-  constexpr int WPB = NT / L;
-  constexpr size_t smem = (size_t)WPB * P * S * 4 * NCH * L * 16 + (size_t)WPB * P * 8;
-  static std::atomic<uint64_t> configured{0};
-  ROC_CUDA(once_per_device(configured, [] {
-    return cudaFuncSetAttribute(sg_chunk_kernel_t<L, NCH, S, P, NT, MINB, MODE>,
-                                cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  }));
-  sg_chunk_kernel_t<L, NCH, S, P, NT, MINB, MODE><<<(p.numChunks + WPB - 1) / WPB, NT, smem, st>>>(p);
-  ROC_LAUNCH_CHECK();
-  return ROC_OK;
-}
-
-// One ScatterGather launch: the main kernel (RING: sg_chunk_kernel_t), then the fix-ups of the rows it cut.  The
-// partials of the min / max backward (MASK) are sums, so it runs the sum's fix-ups.
-template <int VEC, int L, int NCH, int U, int MINB, int RED, bool RING = false>
-static int launch(const SgParams& p, cudaStream_t st) {
-  constexpr int FIX = RED == SG_RED_MASK ? SG_RED_SUM : RED;
-  constexpr int WPB = SG_THREADS / L;
-  if (p.numChunks) {
-    if constexpr (RING) {
-      const int rc = launch_ring<NCH>(p, st);
-      if (rc != ROC_OK) return rc;
-    } else {
-      sg_chunk_kernel<VEC, L, NCH, U, MINB, RED><<<(p.numChunks + WPB - 1) / WPB, SG_THREADS, 0, st>>>(p);
-      ROC_LAUNCH_CHECK();
-    }
-  }
-  if (p.numHeavy) {
-    sg_fixup_kernel<VEC, L, NCH, FIX><<<(p.numHeavy + WPB - 1) / WPB, SG_THREADS, 0, st>>>(p);
-    ROC_LAUNCH_CHECK();
-  }
-  if (p.numBig) {
-    sg_fixup_big_kernel<VEC, L, NCH, FIX><<<p.numBig, SG_THREADS, 0, st>>>(p);
-    ROC_LAUNCH_CHECK();
-  }
-  return ROC_OK;
-}
-
-// Kernel shape for Q T-columns.  The sum takes up to 256 T-columns (1024 floats vectorised, 256 scalar); min / max
-// take 128 vectorised (512 floats: the big-row fix-up keeps values and indices of every lane group in static shared
-// memory).  Gathers in flight (U) are lowered for min / max where the index per float (forward) or the second
-// gathered row (backward) would otherwise spill under the kernel's occupancy.  The vectorised sum of 65..256 floats
-// runs on sg_chunk_kernel_t, which is faster there on a products-shaped graph (DESIGN.md §3.1).
-template <int VEC, int RED>
-static int dispatch(const SgParams& p, cudaStream_t st) {
-  constexpr bool S = RED == SG_RED_SUM;
-  constexpr bool B = RED == SG_RED_MASK;
-  const uint32_t Q = p.Q;
-  if (Q <= 4) return launch<VEC, 4, 1, 4, 4, RED>(p, st);
-  if (Q <= 8) return launch<VEC, 8, 1, S ? 8 : 4, 4, RED>(p, st);
-  if (Q <= 16) return launch<VEC, 16, 1, S ? 8 : 4, 4, RED>(p, st);
-  if (Q <= 32) {
-    if constexpr (VEC == 4 && S) return launch<VEC, 32, 1, 8, 4, RED, true>(p, st);
-    else return launch<VEC, 32, 1, S ? 8 : 4, 4, RED>(p, st);
-  }
-  if (Q <= 64) {
-    if constexpr (VEC == 4 && S) return launch<VEC, 32, 2, 4, 3, RED, true>(p, st);
-    else return launch<VEC, 32, 2, B ? 2 : 4, 3, RED>(p, st);
-  }
-  if (Q <= 128) return launch<VEC, 32, 4, S ? 2 : 1, 3, RED>(p, st);
-  if constexpr (S || VEC == 1) {
-    if (Q <= 256) return launch<VEC, 32, 8, 1, 2, RED>(p, st);
-  }
-  return ROC_ERR_UNSUPPORTED;
-}
-
 // ------------------------------------------------------- attention kernels ---
 // (m, Z) partials of one head merged: the max is exact, each Z rescaled to it.  merge(a, b) and merge(b, a) give the
 // same bits, which the butterfly below relies on.  A partial with Z = 0 has no edge.
@@ -1181,19 +1131,19 @@ sg_attn_rec_kernel(const SgParams p, const void* G, size_t ldG, const void* O, s
   const int lane = threadIdx.x % L;
   const uint32_t v = blockIdx.x * WPB + threadIdx.x / L;
   if (v >= n) return;
-  const unsigned wmask = (L == 32) ? 0xffffffffu : (((1u << L) - 1u) << (((threadIdx.x & 31) / L) * L));
+  const unsigned wmask = worker_mask<L>();
   const T* g = reinterpret_cast<const T*>(G) + (uint64_t)v * ldG;
   const T* o = reinterpret_cast<const T*>(O) + (uint64_t)v * ldO;
   float d[NCH];
 #pragma unroll
   for (int ch = 0; ch < NCH; ch++) {
     const uint32_t c = (uint32_t)(lane + ch * L);
-    const int nv = (VEC == 4) ? max(0, min(4, (int)p.H - 4 * (int)c)) : (c < p.Q ? 1 : 0);
+    const int nv = t_floats<VEC>(c, p);
     const uint32_t cc = min(c, p.Q - 1u);
     d[ch] = dot_t(V<VEC>::ld(g + cc), V<VEC>::ld(o + cc), nv);
   }
   head_sum<L, NCH>(d, p.ftShift, wmask);
-  const uint32_t ftMask = (p.ftShift >= 31u) ? 0x7FFFFFFFu : ((1u << p.ftShift) - 1u);
+  const uint32_t ftMask = head_mask(p);
 #pragma unroll
   for (int ch = 0; ch < NCH; ch++) {
     const uint32_t c = (uint32_t)(lane + ch * L);
@@ -1206,135 +1156,167 @@ sg_attn_rec_kernel(const SgParams p, const void* G, size_t ldG, const void* O, s
   }
 }
 
-// One attention pass: the main kernel, then the fix-ups of the rows it cut.  ASTAT has its own; the H-wide partials
-// (ATTN, ASRC) and the heads-wide ones (ADST, ASRC; p2 = p with out2 / carry2 as a VEC = 1, Q = heads output) are
-// sums, finished by the sum's fix-ups.
-template <int VEC, int L, int NCH, int U, int MINB, int RED>
-static int launch_attn(const SgParams& p, cudaStream_t st) {
+// ------------------------------------------------------------------ launches ---
+// sg_chunk_kernel_t's two shapes, the measured defaults (DESIGN.md §3.1), four workers per CTA: rows of 65..128 floats
+// (one float4 per lane) with lane-held ids and two stages of two four-row units per worker; rows of 129..256 floats
+// with the ids loaded per stage and two stages of one unit.
+template <int NCH>
+static int launch_ring(const SgParams& p, cudaStream_t st) {
+  constexpr int L = 32, P = 2, NT = 128;
+  constexpr int S = NCH == 1 ? 2 : 1, MINB = NCH == 1 ? 4 : 6, MODE = NCH == 1 ? 2 : 0;
+  constexpr int WPB = NT / L;
+  constexpr size_t smem = (size_t)WPB * P * S * 4 * NCH * L * 16 + (size_t)WPB * P * 8;
+  static std::atomic<uint64_t> configured{0};
+  ROC_CUDA(once_per_device(configured, [] {
+    return cudaFuncSetAttribute(sg_chunk_kernel_t<L, NCH, S, P, NT, MINB, MODE>,
+                                cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  }));
+  sg_chunk_kernel_t<L, NCH, S, P, NT, MINB, MODE><<<(p.numChunks + WPB - 1) / WPB, NT, smem, st>>>(p);
+  ROC_LAUNCH_CHECK();
+  return ROC_OK;
+}
+
+// The widest row, in T-columns, that one launch of RED takes: 256 (1024 floats vectorised, 256 scalar; wider rows are
+// split into column blocks), but 128 on float4 rows for every reduction except the sum (min / max: the big-row fix-up
+// keeps values and indices of every lane group in static shared memory).  ASTAT's row is one score per head.
+constexpr int sg_max_q(int VEC, int RED) {
+  return RED == SG_RED_ASTAT ? SG_LDC2 / 2 : (VEC == 4 && RED != SG_RED_SUM) ? 128 : 256;
+}
+
+// The row shape of every launch: calls f(L, NCH), as std::integral_constants, for rows of Q T-columns.  L is the
+// fewest of 4, 8, 16 or 32 lanes that cover Q; past 32 T-columns each lane takes NCH = 2, 4 or 8 chunks:
+// Q <= 4 -> (4, 1), <= 8 -> (8, 1), <= 16 -> (16, 1), <= 32 -> (32, 1), <= 64 -> (32, 2), <= 128 -> (32, 4),
+// <= 256 -> (32, 8).  Rows wider than QMAX are ROC_ERR_UNSUPPORTED.
+template <int QMAX, int QC = 4, class F>
+static int with_shape(uint32_t Q, F&& f) {
+  if constexpr (QC > QMAX) {
+    return ROC_ERR_UNSUPPORTED;
+  } else {
+    if (Q <= (uint32_t)QC)
+      return f(std::integral_constant<int, (QC < 32 ? QC : 32)>{}, std::integral_constant<int, (QC < 32 ? 1 : QC / 32)>{});
+    return with_shape<QMAX, 2 * QC>(Q, f);
+  }
+}
+
+// Gathers in flight (U) and CTAs per SM (MINB) of sg_chunk_kernel, per reduction at NCH = 1, 2, 4, 8 chunks per lane.
+// They are lower than the sum's where a second value held or gathered per float (the min / max index, the min / max
+// backward's index row, s_src, the record, the local row's own row) would otherwise spill under the occupancy.
+constexpr int SG_SHAPE_U[8][4] = {
+    {8, 4, 2, 1},   // SUM (U = 4 at L = 4)
+    {4, 4, 1, 1},   // MAX
+    {4, 4, 1, 1},   // MIN
+    {4, 2, 1, 1},   // MASK
+    {8, 0, 0, 0},   // ASTAT (one chunk: Q = heads)
+    {4, 2, 1, 1},   // ATTN
+    {4, 2, 1, 1},   // ADST
+    {2, 2, 1, 1}};  // ASRC
+constexpr int SG_SHAPE_MINB[8][4] = {
+    {4, 3, 3, 2}, {4, 3, 3, 2}, {4, 3, 3, 2}, {4, 3, 3, 2}, {4, 0, 0, 0}, {4, 3, 2, 2}, {4, 3, 2, 1}, {4, 2, 2, 1}};
+static_assert(SG_RED_MAX == 1 && SG_RED_MIN == 2, "SG_SHAPE_U / SG_SHAPE_MINB rows follow the SG_RED_* values");
+constexpr int sg_nch_index(int NCH) { return NCH == 1 ? 0 : NCH == 2 ? 1 : NCH == 4 ? 2 : 3; }
+constexpr int sg_chunk_u(int RED, int L, int NCH) {
+  return RED == SG_RED_SUM && L == 4 ? 4 : SG_SHAPE_U[RED][sg_nch_index(NCH)];
+}
+constexpr int sg_chunk_minb(int RED, int NCH) { return SG_SHAPE_MINB[RED][sg_nch_index(NCH)]; }
+
+// The fix-ups of the rows a main kernel cut, reduced by FIX over p's out / carry: one worker per heavy row, one CTA
+// per big row.
+template <int VEC, int L, int NCH, int FIX>
+static int launch_fixups(const SgParams& p, cudaStream_t st) {
   constexpr int WPB = SG_THREADS / L;
-  if (p.numChunks) {
-    sg_chunk_kernel<VEC, L, NCH, U, MINB, RED><<<(p.numChunks + WPB - 1) / WPB, SG_THREADS, 0, st>>>(p);
+  if (p.numHeavy) {
+    sg_fixup_kernel<VEC, L, NCH, FIX><<<(p.numHeavy + WPB - 1) / WPB, SG_THREADS, 0, st>>>(p);
     ROC_LAUNCH_CHECK();
   }
-  if (RED == SG_RED_ASTAT) {
+  if (p.numBig) {
+    sg_fixup_big_kernel<VEC, L, NCH, FIX><<<p.numBig, SG_THREADS, 0, st>>>(p);
+    ROC_LAUNCH_CHECK();
+  }
+  return ROC_OK;
+}
+
+// One ScatterGather launch: the main kernel (sg_chunk_kernel_t for the vectorised sum of 17..64 T-columns, which is
+// faster there on a products-shaped graph, DESIGN.md §3.1), then the fix-ups of the rows it cut.  MAX / MIN have their
+// own; ASTAT's stats have sg_attn_stat_fixup; the H-wide partials of the others are sums (the min / max backward's and
+// the attention gathers'), finished by the sum's.  ADST and ASRC then finish their heads-wide partials with the sum's
+// fix-ups on p2, p with out2 / carry2 as a VEC = 1, Q = heads output.
+template <int VEC, int RED, int L, int NCH>
+static int launch(const SgParams& p, cudaStream_t st) {
+  constexpr bool RING = VEC == 4 && RED == SG_RED_SUM && L == 32 && NCH <= 2;
+  constexpr int WPB = SG_THREADS / L;
+  int rc = ROC_OK;
+  if (p.numChunks) {
+    if constexpr (RING) {
+      if ((rc = launch_ring<NCH>(p, st)) != ROC_OK) return rc;
+    } else {
+      sg_chunk_kernel<VEC, L, NCH, sg_chunk_u(RED, L, NCH), sg_chunk_minb(RED, NCH), RED>
+          <<<(p.numChunks + WPB - 1) / WPB, SG_THREADS, 0, st>>>(p);
+      ROC_LAUNCH_CHECK();
+    }
+  }
+  if constexpr (RED == SG_RED_ASTAT) {
     const uint32_t rows = p.numHeavy + p.numBig;
     if (rows) {
       sg_attn_stat_fixup<<<(rows + SG_THREADS / 32 - 1) / (SG_THREADS / 32), SG_THREADS, 0, st>>>(p);
       ROC_LAUNCH_CHECK();
     }
-    return ROC_OK;
+  } else if constexpr (RED != SG_RED_ADST) {
+    constexpr int FIX = (RED == SG_RED_MAX || RED == SG_RED_MIN) ? RED : SG_RED_SUM;
+    if ((rc = launch_fixups<VEC, L, NCH, FIX>(p, st)) != ROC_OK) return rc;
   }
-  if (RED != SG_RED_ADST) {
-    if (p.numHeavy) {
-      sg_fixup_kernel<VEC, L, NCH, SG_RED_SUM><<<(p.numHeavy + WPB - 1) / WPB, SG_THREADS, 0, st>>>(p);
-      ROC_LAUNCH_CHECK();
-    }
-    if (p.numBig) {
-      sg_fixup_big_kernel<VEC, L, NCH, SG_RED_SUM><<<p.numBig, SG_THREADS, 0, st>>>(p);
-      ROC_LAUNCH_CHECK();
-    }
-  }
-  if (RED == SG_RED_ADST || RED == SG_RED_ASRC) {
+  if constexpr (RED == SG_RED_ADST || RED == SG_RED_ASRC) {
     SgParams p2 = p;
     p2.out = p.out2; p2.ldOut = p.ldOut2; p2.carry = p.carry2; p2.ldC = SG_LDC2; p2.Q = p.heads;
-    constexpr int L2 = 8, W2 = SG_THREADS / L2;
-    if (p.numHeavy) {
-      sg_fixup_kernel<1, L2, 1, SG_RED_SUM><<<(p.numHeavy + W2 - 1) / W2, SG_THREADS, 0, st>>>(p2);
+    rc = launch_fixups<1, 8, 1, SG_RED_SUM>(p2, st);
+  }
+  return rc;
+}
+
+// Reduction RED over rows of p.Q T-columns of VEC floats.
+template <int VEC, int RED>
+static int dispatch(const SgParams& p, cudaStream_t st) {
+  return with_shape<sg_max_q(VEC, RED)>(p.Q, [&](auto L, auto NCH) { return launch<VEC, RED, L, NCH>(p, st); });
+}
+
+// The attention backward's node records of ids [0, n), in the shape of its H-wide passes, from G = p.in (leading
+// dimension p.ldIn) and O = p.xrow (p.ldX).
+template <int VEC>
+static int launch_rec(const SgParams& p, uint32_t n, cudaStream_t st) {
+  return with_shape<sg_max_q(VEC, SG_RED_ATTN)>(p.Q, [&](auto L, auto NCH) {
+    if (n) {
+      constexpr int WPB = SG_THREADS / L;
+      sg_attn_rec_kernel<VEC, L, NCH><<<(n + WPB - 1) / WPB, SG_THREADS, 0, st>>>(p, p.in, p.ldIn, p.xrow, p.ldX, n);
       ROC_LAUNCH_CHECK();
     }
-    if (p.numBig) {
-      sg_fixup_big_kernel<1, L2, 1, SG_RED_SUM><<<p.numBig, SG_THREADS, 0, st>>>(p2);
-      ROC_LAUNCH_CHECK();
-    }
+    return ROC_OK;
+  });
+}
+
+// A plan buffer of at least `bytes`, `cap` its size in bytes.  roc_sg_plan_reserve sizes the carries up front (plain
+// cudaMalloc, an init-time call).  A launch that still finds a buffer too small grows it on its own stream with
+// stream-ordered allocation: the old buffer is returned in stream order, after the launches that used it — no device
+// synchronisation in the middle of a step.  A failed allocation leaves the buffer null with zero capacity.
+template <class T>
+static int grow(T*& buf, size_t& cap, size_t bytes, cudaStream_t st, bool inStream = true) {
+  if (bytes <= cap) return ROC_OK;
+  if (buf) {
+    if (inStream) ROC_CUDA(cudaFreeAsync(buf, st));
+    else { ROC_CUDA(cudaDeviceSynchronize()); ROC_CUDA(cudaFree(buf)); }
+    buf = nullptr; cap = 0;
   }
+  cudaError_t e = inStream ? cudaMallocAsync((void**)&buf, bytes, st) : cudaMalloc((void**)&buf, bytes);
+  if (e != cudaSuccess) { buf = nullptr; return (int)e; }
+  cap = bytes;
   return ROC_OK;
 }
 
-// Kernel shape of an H-wide attention pass (or of the record kernel, REC) for Q T-columns: the sum's lane and chunk
-// counts, fewer gathers in flight where the second gathered value (s_src, the record) would otherwise spill.
-template <int VEC, int RED, bool REC = false>
-static int dispatch_attn(const SgParams& p, cudaStream_t st, const void* G = nullptr, size_t ldG = 0,
-                         const void* O = nullptr, size_t ldO = 0, uint32_t n = 0) {
-  constexpr int UB = RED == SG_RED_ASRC ? 2 : 4;     // gathers in flight at one chunk per lane
-  constexpr int MB2 = RED == SG_RED_ASRC ? 2 : 3;    // CTAs per SM at two chunks per lane, ...
-  constexpr int MB8 = RED == SG_RED_ATTN ? 2 : 1;    // ... and at eight (the row held in registers needs more)
-  const uint32_t Q = p.Q;
-#define SG_ATTN_SHAPE(L_, NCH_, U_, MINB_)                                                                    \
-  do {                                                                                                        \
-    if constexpr (REC) {                                                                                      \
-      if (n) {                                                                                                \
-        constexpr int W_ = SG_THREADS / (L_);                                                                 \
-        sg_attn_rec_kernel<VEC, L_, NCH_><<<(n + W_ - 1) / W_, SG_THREADS, 0, st>>>(p, G, ldG, O, ldO, n);     \
-        ROC_LAUNCH_CHECK();                                                                                   \
-      }                                                                                                       \
-      return ROC_OK;                                                                                          \
-    } else {                                                                                                  \
-      return launch_attn<VEC, L_, NCH_, U_, MINB_, RED>(p, st);                                               \
-    }                                                                                                         \
-  } while (0)
-  if (Q <= 4) SG_ATTN_SHAPE(4, 1, UB, 4);
-  if (Q <= 8) SG_ATTN_SHAPE(8, 1, UB, 4);
-  if (Q <= 16) SG_ATTN_SHAPE(16, 1, UB, 4);
-  if (Q <= 32) SG_ATTN_SHAPE(32, 1, UB, 4);
-  if (Q <= 64) SG_ATTN_SHAPE(32, 2, 2, MB2);
-  if (Q <= 128) SG_ATTN_SHAPE(32, 4, 1, 2);
-  if constexpr (VEC == 1) {
-    if (Q <= 256) SG_ATTN_SHAPE(32, 8, 1, MB8);
-  }
-#undef SG_ATTN_SHAPE
-  return ROC_ERR_UNSUPPORTED;
-}
-
-// Carry slots for rows cut at chunk boundaries.  roc_sg_plan_reserve sizes them up front (plain cudaMalloc, an
-// init-time call).  A launch that still finds them too small grows them on its own stream with stream-ordered
-// allocation: the old buffer is returned in stream order, after the launches that used it — no device
-// synchronisation in the middle of a step.
-static int ensure_carry(roc_sg_plan* plan, size_t ldFloats, cudaStream_t st, bool inStream) {
-  if (plan->numCarries == 0 || ldFloats <= plan->carryLd) return ROC_OK;
-  if (plan->carry) {
-    if (inStream) ROC_CUDA(cudaFreeAsync(plan->carry, st));
-    else { ROC_CUDA(cudaDeviceSynchronize()); ROC_CUDA(cudaFree(plan->carry)); }
-    plan->carry = nullptr; plan->carryLd = 0;
-  }
-  const size_t bytes = (size_t)plan->numCarries * ldFloats * sizeof(float);
-  cudaError_t e = inStream ? cudaMallocAsync((void**)&plan->carry, bytes, st) : cudaMalloc((void**)&plan->carry, bytes);
-  if (e != cudaSuccess) { plan->carry = nullptr; plan->carryLd = 0; return (int)e; }
-  plan->carryLd = ldFloats;
-  return ROC_OK;
-}
-
-// The index carries of the min / max forward: u32 [numCarries][carryLd], the shape of the float carries (the kernels
-// address both with one leading dimension), grown the same way.
-static int ensure_carry_arg(roc_sg_plan* plan, cudaStream_t st) {
-  if (plan->numCarries == 0 || plan->carryArgLd == plan->carryLd) return ROC_OK;
-  if (plan->carryArg) {
-    ROC_CUDA(cudaFreeAsync(plan->carryArg, st));
-    plan->carryArg = nullptr; plan->carryArgLd = 0;
-  }
-  const size_t bytes = (size_t)plan->numCarries * plan->carryLd * sizeof(uint32_t);
-  cudaError_t e = cudaMallocAsync((void**)&plan->carryArg, bytes, st);
-  if (e != cudaSuccess) { plan->carryArg = nullptr; plan->carryArgLd = 0; return (int)e; }
-  plan->carryArgLd = plan->carryLd;
-  return ROC_OK;
-}
-
-// The heads-wide carries of the attention passes, [numCarries][SG_LDC2], allocated on first use like carryArg.
-static int ensure_carry2(roc_sg_plan* plan, cudaStream_t st) {
-  if (plan->numCarries == 0 || plan->carry2) return ROC_OK;
-  const size_t bytes = (size_t)plan->numCarries * SG_LDC2 * sizeof(float);
-  cudaError_t e = cudaMallocAsync((void**)&plan->carry2, bytes, st);
-  if (e != cudaSuccess) { plan->carry2 = nullptr; return (int)e; }
-  return ROC_OK;
-}
-
-// The attention backward's node records, grown in stream order to `n` entries.
-static int ensure_rec(roc_sg_plan* plan, size_t n, cudaStream_t st) {
-  if (n <= plan->recCap) return ROC_OK;
-  if (plan->attnRec) { ROC_CUDA(cudaFreeAsync(plan->attnRec, st)); plan->attnRec = nullptr; plan->recCap = 0; }
-  cudaError_t e = cudaMallocAsync((void**)&plan->attnRec, n * sizeof(float4), st);
-  if (e != cudaSuccess) { plan->attnRec = nullptr; return (int)e; }
-  plan->recCap = n;
-  return ROC_OK;
+// The carry slots of rows cut at chunk boundaries: [numCarries][carryLd] floats, carryLd at least `cols` rounded up
+// to float4 rows.
+static int grow_carries(roc_sg_plan* pl, int cols, cudaStream_t st, bool inStream = true) {
+  const size_t n = pl->numCarries, ld = ((size_t)cols + 3) / 4 * 4;
+  const int rc = grow(pl->carry, pl->carryBytes, n * ld * sizeof(float), st, inStream);
+  pl->carryLd = n ? pl->carryBytes / (n * sizeof(float)) : 0;
+  return rc;
 }
 
 // 1 + the largest id in col, found once (one reduction and one synchronisation of the stream) and kept in the plan.
@@ -1450,7 +1432,7 @@ extern "C" void roc_sg_plan_destroy(roc_sg_plan* pl) {
 
 extern "C" int roc_sg_plan_reserve(roc_sg_plan* pl, int maxH) {
   if (!pl || maxH <= 0) return ROC_ERR_INVALID;
-  return ensure_carry(pl, ((size_t)maxH + 3) / 4 * 4, nullptr, false);
+  return grow_carries(pl, maxH, nullptr, false);
 }
 
 extern "C" int roc_sg_plan_info(const roc_sg_plan* pl, uint64_t* numChunks, uint64_t* numCarries,
@@ -1462,15 +1444,32 @@ extern "C" int roc_sg_plan_info(const roc_sg_plan* pl, uint64_t* numChunks, uint
   return ROC_OK;
 }
 
-// The plan parameters shared by every launch of column block c0 (units of T applied by the caller).
+// The plan parameters shared by every launch, with the carries' leading dimension in floats like the caller's.
 static SgParams plan_params(const roc_sg_plan* pl) {
   SgParams p;
   memset(&p, 0, sizeof(p));
   p.rs = pl->rs; p.firstRow = pl->firstRow; p.carryIdx = pl->carryIdx; p.heavyRows = pl->heavyRows; p.bigRows = pl->bigRows;
-  p.col = pl->col; p.carry = pl->carry; p.carryArg = pl->carryArg;
+  p.col = pl->col; p.carry = pl->carry; p.carryArg = pl->carryArg; p.ldC = pl->carryLd;
   p.E = pl->E; p.numChunks = pl->numChunks; p.numHeavy = pl->numHeavy; p.numBig = pl->numBig; p.epi = 0;
   p.desc = pl->desc;
   return p;
+}
+
+// Whether rows can be read as float4 T-columns: every row pointer 16-byte aligned, every leading dimension a multiple
+// of 4 floats.
+static bool float4_rows(std::initializer_list<const void*> rows, std::initializer_list<int64_t> lds) {
+  for (const void* r : rows)
+    if (!aligned16(r)) return false;
+  for (int64_t ld : lds)
+    if (ld % 4) return false;
+  return true;
+}
+
+// Converts the leading dimensions of p's T-column rows (in, out, arg, xrow and the carries) from floats to T-columns
+// of vw floats, and sets Q for rows of `cols` floats.
+static void t_units(SgParams& p, int vw, int cols) {
+  p.ldIn /= vw; p.ldOut /= vw; p.ldArg /= vw; p.ldX /= vw; p.ldC /= vw;
+  p.Q = ((uint32_t)cols + vw - 1) / vw;
 }
 
 // Reduction RED over the columns [0, H) of every row, in column blocks: 1,024 floats for the sum and 512 for min /
@@ -1479,27 +1478,20 @@ static SgParams plan_params(const roc_sg_plan* pl) {
 template <int RED>
 static int run_planned(roc_sg_plan* pl, int H, const float* in, int64_t ldIn, float* out, int64_t ldOut,
                        const roc_vid_t* arg, int64_t ldArg, int epilogue, roc_vid_t selfBase, cudaStream_t st) {
-  const bool vec = (ldIn % 4 == 0) && (ldOut % 4 == 0) && (ldArg % 4 == 0) && aligned16(in) && aligned16(out) &&
-                   aligned16(arg);
-  const int vw = vec ? 4 : 1;                 // floats per T-column
+  const bool vec = float4_rows({in, out, arg}, {ldIn, ldOut, ldArg});
   const int blockCols = !vec ? 256 : RED == SG_RED_SUM ? 1024 : 512;
-  {
-    int need = H < blockCols ? H : blockCols;
-    int rc = ensure_carry(pl, ((size_t)need + 3) / 4 * 4, st, true);
-    if (rc != ROC_OK) return rc;
-    if constexpr (RED == SG_RED_MAX || RED == SG_RED_MIN) {
-      rc = ensure_carry_arg(pl, st);
-      if (rc != ROC_OK) return rc;
-    }
-  }
+  int rc = grow_carries(pl, std::min(H, blockCols), st);
+  // the min / max forward's index carries, which the kernels address with the float carries' leading dimension
+  if (rc == ROC_OK && (RED == SG_RED_MAX || RED == SG_RED_MIN))
+    rc = grow(pl->carryArg, pl->carryArgBytes, (size_t)pl->numCarries * pl->carryLd * sizeof(uint32_t), st);
+  if (rc != ROC_OK) return rc;
   for (int c0 = 0; c0 < H; c0 += blockCols) {
-    const int hb = (H - c0 < blockCols) ? H - c0 : blockCols;
     SgParams p = plan_params(pl);
     p.in = in + c0; p.out = out + c0; p.epi = epilogue; p.selfBase = selfBase;
     if (arg) p.arg = const_cast<roc_vid_t*>(arg) + c0;
-    p.ldIn = (size_t)ldIn / vw; p.ldOut = (size_t)ldOut / vw; p.ldArg = (size_t)ldArg / vw; p.ldC = pl->carryLd / vw;
-    p.Q = ((uint32_t)hb + vw - 1) / vw;
-    const int rc = vec ? dispatch<4, RED>(p, st) : dispatch<1, RED>(p, st);
+    p.ldIn = (size_t)ldIn; p.ldOut = (size_t)ldOut; p.ldArg = (size_t)ldArg;
+    t_units(p, vec ? 4 : 1, std::min(H - c0, blockCols));
+    rc = vec ? dispatch<4, RED>(p, st) : dispatch<1, RED>(p, st);
     if (rc != ROC_OK) return rc;
   }
   return ROC_OK;
@@ -1553,9 +1545,10 @@ extern "C" int roc_sg_minmax_backward_planned(const roc_sg_plan* plc, int H, roc
   return run_planned<SG_RED_MASK>(pl, H, outGrad, ldG, inGrad, ldIn, arg, ldArg, 0, selfBase, as_stream(stream));
 }
 
-// The head layout of an attention call whose pointers and leading dimensions are valid: ROC_ERR_INVALID for a bad
-// slope, ROC_ERR_UNSUPPORTED for a layout the kernels do not take; *ftShift = log2 of the T-columns per head.
-static int attn_layout(int heads, int H, float slope, bool vec, uint32_t* ftShift) {
+// What both attention entry points do once their own arguments are checked: ROC_ERR_INVALID for a bad slope,
+// ROC_ERR_UNSUPPORTED for a head layout the kernels do not take, then the carries of the H-wide and the heads-wide
+// partials.  *ftShift = log2 of the T-columns per head.
+static int attn_setup(roc_sg_plan* pl, int heads, int H, float slope, bool vec, cudaStream_t st, uint32_t* ftShift) {
   if (!(slope >= 0.f) || !std::isfinite(slope)) return ROC_ERR_INVALID;
   if ((heads != 1 && heads != 2 && heads != 4 && heads != 8) || H % heads) return ROC_ERR_UNSUPPORTED;
   const int F = H / heads;
@@ -1564,10 +1557,12 @@ static int attn_layout(int heads, int H, float slope, bool vec, uint32_t* ftShif
   uint32_t fs = 0;
   while ((1 << fs) < F / (vec ? 4 : 1)) fs++;
   *ftShift = heads == 1 ? 31u : fs;
-  return ROC_OK;
+  int rc = grow_carries(pl, H, st);
+  if (rc == ROC_OK) rc = grow(pl->carry2, pl->carry2Bytes, (size_t)pl->numCarries * SG_LDC2 * sizeof(float), st);
+  return rc;
 }
 
-// The parameters every attention pass shares (units of T set by the caller).
+// The parameters every attention pass shares (leading dimensions of T-column rows set by the pass, in floats).
 static SgParams attn_params(const roc_sg_plan* pl, int heads, int H, float slope, roc_vid_t selfBase,
                             const float* score, int64_t ldS, const float* stats, int64_t ldStats, uint32_t ftShift) {
   SgParams p = plan_params(pl);
@@ -1585,24 +1580,21 @@ extern "C" int roc_sg_attn_forward_planned(const roc_sg_plan* plc, int heads, in
   if (!pl || !in || !score || !out || !stats || heads <= 0 || H <= 0 || ldIn < H || ldOut < H ||
       ldS < 2 * (int64_t)heads || ldStats < 2 * (int64_t)heads)
     return ROC_ERR_INVALID;
-  const bool vec = ldIn % 4 == 0 && ldOut % 4 == 0 && aligned16(in) && aligned16(out);
-  uint32_t fs = 0;
-  int rc = attn_layout(heads, H, slope, vec, &fs);
-  if (rc != ROC_OK) return rc;
+  const bool vec = float4_rows({in, out}, {ldIn, ldOut});
   cudaStream_t st = as_stream(stream);
-  if ((rc = ensure_carry(pl, ((size_t)H + 3) / 4 * 4, st, true)) != ROC_OK) return rc;
-  if ((rc = ensure_carry2(pl, st)) != ROC_OK) return rc;
-  // pass 1: (m, 1/Z) per row and head from the scores alone
-  SgParams a = attn_params(pl, heads, H, slope, selfBase, score, ldS, stats, ldStats, 0);
-  a.in = score + heads; a.ldIn = (size_t)ldS; a.out = stats; a.ldOut = (size_t)ldStats; a.Q = (uint32_t)heads;
-  rc = heads <= 4 ? launch_attn<1, 4, 1, 8, 4, SG_RED_ASTAT>(a, st) : launch_attn<1, 8, 1, 8, 4, SG_RED_ASTAT>(a, st);
+  uint32_t fs = 0;
+  int rc = attn_setup(pl, heads, H, slope, vec, st, &fs);
   if (rc != ROC_OK) return rc;
+  // pass 1: (m, 1/Z) per row and head from the scores alone, one float per head
+  SgParams a = attn_params(pl, heads, H, slope, selfBase, score, ldS, stats, ldStats, 0);
+  a.in = score + heads; a.ldIn = (size_t)ldS; a.out = stats; a.ldOut = (size_t)ldStats;
+  t_units(a, 1, heads);
+  if ((rc = dispatch<1, SG_RED_ASTAT>(a, st)) != ROC_OK) return rc;
   // pass 2: the a-weighted sum of the feature rows
-  const int vw = vec ? 4 : 1;
   SgParams b = attn_params(pl, heads, H, slope, selfBase, score, ldS, stats, ldStats, fs);
-  b.in = in; b.ldIn = (size_t)ldIn / vw; b.out = out; b.ldOut = (size_t)ldOut / vw; b.ldC = pl->carryLd / vw;
-  b.Q = ((uint32_t)H + vw - 1) / vw;
-  return vec ? dispatch_attn<4, SG_RED_ATTN>(b, st) : dispatch_attn<1, SG_RED_ATTN>(b, st);
+  b.in = in; b.ldIn = (size_t)ldIn; b.out = out; b.ldOut = (size_t)ldOut;
+  t_units(b, vec ? 4 : 1, H);
+  return vec ? dispatch<4, SG_RED_ATTN>(b, st) : dispatch<1, SG_RED_ATTN>(b, st);
 }
 
 extern "C" int roc_sg_attn_backward_planned(const roc_sg_plan* plc, int heads, int H, float slope, roc_vid_t selfBase,
@@ -1615,38 +1607,37 @@ extern "C" int roc_sg_attn_backward_planned(const roc_sg_plan* plc, int heads, i
       ldIn < H || ldOut < H || ldG < H || ldInG < H || ldS < 2 * (int64_t)heads || ldStats < 2 * (int64_t)heads ||
       ldSG < 2 * (int64_t)heads)
     return ROC_ERR_INVALID;
-  const bool vec = ldIn % 4 == 0 && ldOut % 4 == 0 && ldG % 4 == 0 && ldInG % 4 == 0 && aligned16(in) &&
-                   aligned16(out) && aligned16(outGrad) && aligned16(inGrad);
-  uint32_t fs = 0;
-  int rc = attn_layout(heads, H, slope, vec, &fs);
-  if (rc != ROC_OK) return rc;
+  const bool vec = float4_rows({in, out, outGrad, inGrad}, {ldIn, ldOut, ldG, ldInG});
   cudaStream_t st = as_stream(stream);
+  uint32_t fs = 0;
+  int rc = attn_setup(pl, heads, H, slope, vec, st, &fs);
+  if (rc != ROC_OK) return rc;
   if ((rc = find_id_end(pl, st)) != ROC_OK) return rc;
   const uint64_t n64 = std::max<uint64_t>(pl->idEnd, (uint64_t)selfBase + pl->nloc);
   if (n64 >= 0xFFFFFFF0ull) return ROC_ERR_UNSUPPORTED;
   const uint32_t n = (uint32_t)n64;
-  if ((rc = ensure_rec(pl, (size_t)n * heads, st)) != ROC_OK) return rc;
-  if ((rc = ensure_carry(pl, ((size_t)H + 3) / 4 * 4, st, true)) != ROC_OK) return rc;
-  if ((rc = ensure_carry2(pl, st)) != ROC_OK) return rc;
+  if ((rc = grow(pl->attnRec, pl->attnRecBytes, (size_t)n * heads * sizeof(float4), st)) != ROC_OK) return rc;
   const int vw = vec ? 4 : 1;
-  SgParams p = attn_params(pl, heads, H, slope, selfBase, score, ldS, stats, ldStats, fs);
-  p.ldC = pl->carryLd / vw;
-  p.Q = ((uint32_t)H + vw - 1) / vw;
-  // the node records {s_dst, m, 1/Z, D}
-  rc = vec ? dispatch_attn<4, SG_RED_ATTN, true>(p, st, outGrad, (size_t)ldG / 4, out, (size_t)ldOut / 4, n)
-           : dispatch_attn<1, SG_RED_ATTN, true>(p, st, outGrad, (size_t)ldG, out, (size_t)ldOut, n);
+  const SgParams p = attn_params(pl, heads, H, slope, selfBase, score, ldS, stats, ldStats, fs);
+  // the node records {s_dst, m, 1/Z, D}, from G and O
+  SgParams r = p;
+  r.in = outGrad; r.ldIn = (size_t)ldG; r.xrow = out; r.ldX = (size_t)ldOut;
+  t_units(r, vw, H);
+  rc = vec ? launch_rec<4>(r, n, st) : launch_rec<1>(r, n, st);
   if (rc != ROC_OK) return rc;
   // B1: d s_dst, gathering X[j] and s_src[j] against G[i]
   SgParams b1 = p;
-  b1.in = in; b1.ldIn = (size_t)ldIn / vw; b1.xrow = outGrad; b1.ldX = (size_t)ldG / vw;
+  b1.in = in; b1.ldIn = (size_t)ldIn; b1.xrow = outGrad; b1.ldX = (size_t)ldG;
   b1.out = nullptr; b1.out2 = scoreGrad; b1.ldOut2 = (size_t)ldSG;
-  rc = vec ? dispatch_attn<4, SG_RED_ADST>(b1, st) : dispatch_attn<1, SG_RED_ADST>(b1, st);
+  t_units(b1, vw, H);
+  rc = vec ? dispatch<4, SG_RED_ADST>(b1, st) : dispatch<1, SG_RED_ADST>(b1, st);
   if (rc != ROC_OK) return rc;
   // B2: inGrad and d s_src, gathering G[j] and the record of j against X[i]
   SgParams b2 = p;
-  b2.in = outGrad; b2.ldIn = (size_t)ldG / vw; b2.xrow = in; b2.ldX = (size_t)ldIn / vw;
-  b2.out = inGrad; b2.ldOut = (size_t)ldInG / vw; b2.out2 = scoreGrad + heads; b2.ldOut2 = (size_t)ldSG;
-  return vec ? dispatch_attn<4, SG_RED_ASRC>(b2, st) : dispatch_attn<1, SG_RED_ASRC>(b2, st);
+  b2.in = outGrad; b2.ldIn = (size_t)ldG; b2.xrow = in; b2.ldX = (size_t)ldIn;
+  b2.out = inGrad; b2.ldOut = (size_t)ldInG; b2.out2 = scoreGrad + heads; b2.ldOut2 = (size_t)ldSG;
+  t_units(b2, vw, H);
+  return vec ? dispatch<4, SG_RED_ASRC>(b2, st) : dispatch<1, SG_RED_ASRC>(b2, st);
 }
 
 extern "C" int roc_sg_forward(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft, int H,

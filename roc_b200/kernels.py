@@ -44,6 +44,7 @@ class SgPlan:
         assert col_src.dtype in (torch.int32, torch.uint32)
         self.row_left, self.row_right, self.col_left = int(row_left), int(row_right), int(col_left)
         self.row_end, self.col_src = row_end, col_src   # keep alive
+        self.nloc = self.row_right - self.row_left + 1
         h = C.c_void_p()
         check(lib.roc_sg_plan_create(self.row_left, self.row_right, self.col_left, _ptr(row_end), _ptr(col_src),
                                      _stream(), C.byref(h)), "roc_sg_plan_create")
@@ -54,14 +55,21 @@ class SgPlan:
         check(lib.roc_sg_plan_info(self.handle, C.byref(a), C.byref(b), C.byref(c)))
         return {"chunks": a.value, "carries": b.value, "heavy_rows": c.value}
 
+    def _rows(self, like, dtype=torch.float32):
+        """A new [Nloc][H] output for an input `like` of width H: padded to float4 rows when like's rows are, else
+        dense."""
+        h = like.shape[1]
+        if _ld(like) % 4 == 0:
+            return padded(self.nloc, h, like.device, dtype=dtype)
+        return torch.empty((self.nloc, h), device=like.device, dtype=dtype)
+
     def reserve(self, max_h):
         check(lib.roc_sg_plan_reserve(self.handle, int(max_h)), "roc_sg_plan_reserve")
 
     def forward(self, x, out=None, epilogue=0):
-        nloc = self.row_right - self.row_left + 1
         h = x.shape[1]
         if out is None:
-            out = padded(nloc, h, x.device) if _ld(x) % 4 == 0 else torch.empty((nloc, h), device=x.device)
+            out = self._rows(x)
         check(lib.roc_sg_forward_planned(self.handle, h, _ptr(x), _ld(x), _ptr(out), _ld(out), int(epilogue),
                                          _stream()), "roc_sg_forward_planned")
         return out
@@ -76,14 +84,11 @@ class SgPlan:
         """Max (aggr = AGGR_MAX) or min (AGGR_MIN) aggregation -> (out [Nloc][H] fp32, arg [Nloc][H]): arg holds the
         source id of the first edge in CSR order with the extreme value (uint32 bits in int32 storage; SG_NOARG,
         i.e. -1, for a row with no edge)."""
-        nloc = self.row_right - self.row_left + 1
         h = x.shape[1]
-        vec = _ld(x) % 4 == 0
         if out is None:
-            out = padded(nloc, h, x.device) if vec else torch.empty((nloc, h), device=x.device)
+            out = self._rows(x)
         if arg is None:
-            arg = padded(nloc, h, x.device, dtype=torch.int32) if vec else \
-                torch.empty((nloc, h), device=x.device, dtype=torch.int32)
+            arg = self._rows(x, dtype=torch.int32)
         check(lib.roc_sg_minmax_forward_planned(self.handle, int(aggr), h, _ptr(x), _ld(x), _ptr(out), _ld(out),
                                                 _ptr(arg), _ld(arg), _stream()), "roc_sg_minmax_forward_planned")
         return out, arg
@@ -91,10 +96,9 @@ class SgPlan:
     def minmax_backward(self, gy, arg, self_base=0, out=None):
         """Gradient of minmax_forward's input: out[u] = sum over row u's edges e (v = col[e]) of gy[v] where
         arg[v] == self_base + u.  gy and arg are indexed like the forward's input."""
-        nloc = self.row_right - self.row_left + 1
         h = gy.shape[1]
         if out is None:
-            out = padded(nloc, h, gy.device) if _ld(gy) % 4 == 0 else torch.empty((nloc, h), device=gy.device)
+            out = self._rows(gy)
         check(lib.roc_sg_minmax_backward_planned(self.handle, h, int(self_base), _ptr(gy), _ld(gy), _ptr(arg),
                                                  _ld(arg), _ptr(out), _ld(out), _stream()),
               "roc_sg_minmax_backward_planned")
@@ -103,12 +107,11 @@ class SgPlan:
     def attn_forward(self, x, scores, heads=1, slope=0.2, self_base=0, out=None, stats=None):
         """Attention aggregation (include/roc_b200.h) -> (out [Nloc][H], stats [Nloc][2*heads] = m | 1/Z per head).
         x and scores ([*][2*heads] = s_dst | s_src) are indexed like minmax_forward's input."""
-        nloc = self.row_right - self.row_left + 1
         h = x.shape[1]
         if out is None:
-            out = padded(nloc, h, x.device) if _ld(x) % 4 == 0 else torch.empty((nloc, h), device=x.device)
+            out = self._rows(x)
         if stats is None:
-            stats = torch.empty((nloc, 2 * heads), device=x.device)
+            stats = torch.empty((self.nloc, 2 * heads), device=x.device)
         check(lib.roc_sg_attn_forward_planned(self.handle, int(heads), h, float(slope), int(self_base), _ptr(x), _ld(x),
                                               _ptr(scores), _ld(scores), _ptr(out), _ld(out), _ptr(stats),
                                               _ld(stats), _stream()), "roc_sg_attn_forward_planned")
@@ -118,12 +121,11 @@ class SgPlan:
                       score_grad=None):
         """Its backward -> (in_grad [Nloc][H], score_grad [Nloc][2*heads] = d s_dst | d s_src).  x, scores, out, stats
         and gy are indexed like the forward's input (for a whole graph: the forward's own outputs)."""
-        nloc = self.row_right - self.row_left + 1
         h = x.shape[1]
         if in_grad is None:
-            in_grad = padded(nloc, h, x.device) if _ld(x) % 4 == 0 else torch.empty((nloc, h), device=x.device)
+            in_grad = self._rows(x)
         if score_grad is None:
-            score_grad = torch.empty((nloc, 2 * heads), device=x.device)
+            score_grad = torch.empty((self.nloc, 2 * heads), device=x.device)
         check(lib.roc_sg_attn_backward_planned(self.handle, int(heads), h, float(slope), int(self_base), _ptr(x),
                                                _ld(x), _ptr(scores), _ld(scores), _ptr(out), _ld(out), _ptr(stats),
                                                _ld(stats), _ptr(gy), _ld(gy), _ptr(in_grad), _ld(in_grad),

@@ -211,6 +211,38 @@ int roc_sg_backward(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft, in
                     const roc_eid_t* rowEnd, const roc_vid_t* colSrc,
                     const float* outGrad, float* inGrad, roc_stream_t stream);
 
+/* Test hook: the kernel launches of the calling thread's last planned ScatterGather call (the roc_sg_*_planned entry
+ * points, and the plan-less forms through them), in launch order, so that a test can assert which instantiation of
+ * the row-shape table served a width and which fix-ups ran.  Column blocks and the passes of an attention call append
+ * to one list.  Each entry:
+ *   kind   ROC_SG_LAUNCH_*: the main kernel, its cp.async.bulk ring form (float4 sums of 17..64 T-columns), the
+ *          fix-up of rows with at most 32 carries (one worker each), of rows with more (one CTA each), the attention
+ *          stats fix-up, the attention backward's per-node record, and the fix-ups of its heads-wide partials
+ *   red    the reduction the kernel is instantiated for: 0 sum, 1 max, 2 min, 3 the min / max backward, 4 attention
+ *          stats, 5 the attention forward, 6 its d s_dst gather, 7 its input-gradient gather; -1 for the record,
+ *          which has none.  A sum fix-up finishing another reduction's partials reports 0.
+ *   vec    4 for float4 rows, else 1;  lanes, nch: the row shape (L lanes, chunks per lane);  grid: CTAs launched
+ * count is the number of launches; the first ROC_SG_MAX_LAUNCHES are stored.  Every planned call clears the list first,
+ * also one that fails before it launches anything.  ROC_ERR_INVALID for a NULL info. */
+#define ROC_SG_LAUNCH_MAIN 0
+#define ROC_SG_LAUNCH_RING 1
+#define ROC_SG_LAUNCH_FIXUP 2
+#define ROC_SG_LAUNCH_BIG_FIXUP 3
+#define ROC_SG_LAUNCH_STAT_FIXUP 4
+#define ROC_SG_LAUNCH_RECORD 5
+#define ROC_SG_LAUNCH_HEADS_FIXUP 6
+#define ROC_SG_LAUNCH_HEADS_BIG_FIXUP 7
+#define ROC_SG_MAX_LAUNCHES 32
+typedef struct {
+  int kind, red, vec, lanes, nch;
+  int64_t grid;
+} roc_sg_launch;
+typedef struct {
+  int count;
+  roc_sg_launch launch[ROC_SG_MAX_LAUNCHES];
+} roc_sg_call_info;
+int roc_sg_last_call_info(roc_sg_call_info* info);
+
 /* ----------------------------------------------------------------- halo --- */
 
 /* Boundary-node structures of one partition (multi-GPU).  The reference hands every

@@ -44,6 +44,23 @@ class GemmInfo(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+SG_LAUNCH_MAIN, SG_LAUNCH_RING, SG_LAUNCH_FIXUP, SG_LAUNCH_BIG_FIXUP = 0, 1, 2, 3      # roc_sg_launch.kind
+SG_LAUNCH_STAT_FIXUP, SG_LAUNCH_RECORD, SG_LAUNCH_HEADS_FIXUP, SG_LAUNCH_HEADS_BIG_FIXUP = 4, 5, 6, 7
+SG_LAUNCH_KINDS = ("main", "ring", "fixup", "big_fixup", "stat_fixup", "record", "heads_fixup", "heads_big_fixup")
+SG_MAX_LAUNCHES = 32
+
+
+class SgLaunch(C.Structure):
+    """roc_sg_launch (include/roc_b200.h): one kernel launch of a planned ScatterGather call."""
+    _fields_ = [("kind", C.c_int), ("red", C.c_int), ("vec", C.c_int), ("lanes", C.c_int), ("nch", C.c_int),
+                ("grid", C.c_int64)]
+
+
+class SgCallInfo(C.Structure):
+    """roc_sg_call_info (include/roc_b200.h): the launches of the calling thread's last planned ScatterGather call."""
+    _fields_ = [("count", C.c_int), ("launch", SgLaunch * SG_MAX_LAUNCHES)]
+
+
 class PerfMetrics(C.Structure):
     """PerfMetrics, softmax_kernel.cu:35-39."""
     _fields_ = [("trainLoss", C.c_float), ("trainAll", C.c_int), ("testAll", C.c_int), ("valAll", C.c_int),
@@ -92,6 +109,7 @@ PROTOTYPES = {
                                            i64, vp, i64, vp]),
     "roc_sg_forward": (i32, [u32, u32, u64, i32, vp, vp, vp, vp, vp]),
     "roc_sg_backward": (i32, [u32, u32, u64, i32, vp, vp, vp, vp, vp]),
+    "roc_sg_last_call_info": (i32, [C.POINTER(SgCallInfo)]),
     "roc_halo_create": (i32, [u32, u32, u64, vp, vp, C.POINTER(vp)]),
     "roc_halo_destroy": (None, [vp]),
     "roc_halo_size": (u32, [vp]),
@@ -198,6 +216,16 @@ def last_gemm_info(which):
     info = GemmInfo()
     check(lib.roc_last_gemm_info(which, C.byref(info)), "roc_last_gemm_info")
     return info.as_dict()
+
+
+def sg_last_call_info():
+    """roc_sg_last_call_info: the launches of the calling thread's last planned ScatterGather call, in order, as
+    dicts with the kind's name (SG_LAUNCH_KINDS) in "kind"."""
+    info = SgCallInfo()
+    check(lib.roc_sg_last_call_info(C.byref(info)), "roc_sg_last_call_info")
+    assert info.count <= SG_MAX_LAUNCHES, "%d launches, more than the hook stores" % info.count
+    return [dict({k: getattr(info.launch[i], k) for k, _ in SgLaunch._fields_},
+                 kind=SG_LAUNCH_KINDS[info.launch[i].kind]) for i in range(info.count)]
 
 
 def device_count():

@@ -1157,6 +1157,15 @@ sg_attn_rec_kernel(const SgParams p, const void* G, size_t ldG, const void* O, s
 }
 
 // ------------------------------------------------------------------ launches ---
+// The launches of the calling thread's last planned call (roc_sg_last_call_info): every planned entry point clears the
+// list, and every launch site below appends what it launched.
+static thread_local roc_sg_call_info t_call = {};
+static void clear_launches() { t_call.count = 0; }
+static void note_launch(int kind, int red, int vec, int lanes, int nch, uint32_t grid) {
+  if (t_call.count < ROC_SG_MAX_LAUNCHES) t_call.launch[t_call.count] = roc_sg_launch{kind, red, vec, lanes, nch, (int64_t)grid};
+  t_call.count++;
+}
+
 // sg_chunk_kernel_t's two shapes, the measured defaults (DESIGN.md §3.1), four workers per CTA: rows of 65..128 floats
 // (one float4 per lane) with lane-held ids and two stages of two four-row units per worker; rows of 129..256 floats
 // with the ids loaded per stage and two stages of one unit.
@@ -1171,8 +1180,10 @@ static int launch_ring(const SgParams& p, cudaStream_t st) {
     return cudaFuncSetAttribute(sg_chunk_kernel_t<L, NCH, S, P, NT, MINB, MODE>,
                                 cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   }));
-  sg_chunk_kernel_t<L, NCH, S, P, NT, MINB, MODE><<<(p.numChunks + WPB - 1) / WPB, NT, smem, st>>>(p);
+  const uint32_t grid = (p.numChunks + WPB - 1) / WPB;
+  sg_chunk_kernel_t<L, NCH, S, P, NT, MINB, MODE><<<grid, NT, smem, st>>>(p);
   ROC_LAUNCH_CHECK();
+  note_launch(ROC_SG_LAUNCH_RING, SG_RED_SUM, 4, L, NCH, grid);
   return ROC_OK;
 }
 
@@ -1220,17 +1231,20 @@ constexpr int sg_chunk_u(int RED, int L, int NCH) {
 constexpr int sg_chunk_minb(int RED, int NCH) { return SG_SHAPE_MINB[RED][sg_nch_index(NCH)]; }
 
 // The fix-ups of the rows a main kernel cut, reduced by FIX over p's out / carry: one worker per heavy row, one CTA
-// per big row.
+// per big row.  `heads`: p holds an attention gather's heads-wide partials.
 template <int VEC, int L, int NCH, int FIX>
-static int launch_fixups(const SgParams& p, cudaStream_t st) {
+static int launch_fixups(const SgParams& p, cudaStream_t st, bool heads = false) {
   constexpr int WPB = SG_THREADS / L;
   if (p.numHeavy) {
-    sg_fixup_kernel<VEC, L, NCH, FIX><<<(p.numHeavy + WPB - 1) / WPB, SG_THREADS, 0, st>>>(p);
+    const uint32_t grid = (p.numHeavy + WPB - 1) / WPB;
+    sg_fixup_kernel<VEC, L, NCH, FIX><<<grid, SG_THREADS, 0, st>>>(p);
     ROC_LAUNCH_CHECK();
+    note_launch(heads ? ROC_SG_LAUNCH_HEADS_FIXUP : ROC_SG_LAUNCH_FIXUP, FIX, VEC, L, NCH, grid);
   }
   if (p.numBig) {
     sg_fixup_big_kernel<VEC, L, NCH, FIX><<<p.numBig, SG_THREADS, 0, st>>>(p);
     ROC_LAUNCH_CHECK();
+    note_launch(heads ? ROC_SG_LAUNCH_HEADS_BIG_FIXUP : ROC_SG_LAUNCH_BIG_FIXUP, FIX, VEC, L, NCH, p.numBig);
   }
   return ROC_OK;
 }
@@ -1249,16 +1263,19 @@ static int launch(const SgParams& p, cudaStream_t st) {
     if constexpr (RING) {
       if ((rc = launch_ring<NCH>(p, st)) != ROC_OK) return rc;
     } else {
-      sg_chunk_kernel<VEC, L, NCH, sg_chunk_u(RED, L, NCH), sg_chunk_minb(RED, NCH), RED>
-          <<<(p.numChunks + WPB - 1) / WPB, SG_THREADS, 0, st>>>(p);
+      const uint32_t grid = (p.numChunks + WPB - 1) / WPB;
+      sg_chunk_kernel<VEC, L, NCH, sg_chunk_u(RED, L, NCH), sg_chunk_minb(RED, NCH), RED><<<grid, SG_THREADS, 0, st>>>(p);
       ROC_LAUNCH_CHECK();
+      note_launch(ROC_SG_LAUNCH_MAIN, RED, VEC, L, NCH, grid);
     }
   }
   if constexpr (RED == SG_RED_ASTAT) {
     const uint32_t rows = p.numHeavy + p.numBig;
     if (rows) {
-      sg_attn_stat_fixup<<<(rows + SG_THREADS / 32 - 1) / (SG_THREADS / 32), SG_THREADS, 0, st>>>(p);
+      const uint32_t grid = (rows + SG_THREADS / 32 - 1) / (SG_THREADS / 32);
+      sg_attn_stat_fixup<<<grid, SG_THREADS, 0, st>>>(p);
       ROC_LAUNCH_CHECK();
+      note_launch(ROC_SG_LAUNCH_STAT_FIXUP, SG_RED_ASTAT, 1, 32, 1, grid);
     }
   } else if constexpr (RED != SG_RED_ADST) {
     constexpr int FIX = (RED == SG_RED_MAX || RED == SG_RED_MIN) ? RED : SG_RED_SUM;
@@ -1267,7 +1284,7 @@ static int launch(const SgParams& p, cudaStream_t st) {
   if constexpr (RED == SG_RED_ADST || RED == SG_RED_ASRC) {
     SgParams p2 = p;
     p2.out = p.out2; p2.ldOut = p.ldOut2; p2.carry = p.carry2; p2.ldC = SG_LDC2; p2.Q = p.heads;
-    rc = launch_fixups<1, 8, 1, SG_RED_SUM>(p2, st);
+    rc = launch_fixups<1, 8, 1, SG_RED_SUM>(p2, st, true);
   }
   return rc;
 }
@@ -1285,8 +1302,10 @@ static int launch_rec(const SgParams& p, uint32_t n, cudaStream_t st) {
   return with_shape<sg_max_q(VEC, SG_RED_ATTN)>(p.Q, [&](auto L, auto NCH) {
     if (n) {
       constexpr int WPB = SG_THREADS / L;
-      sg_attn_rec_kernel<VEC, L, NCH><<<(n + WPB - 1) / WPB, SG_THREADS, 0, st>>>(p, p.in, p.ldIn, p.xrow, p.ldX, n);
+      const uint32_t grid = (n + WPB - 1) / WPB;
+      sg_attn_rec_kernel<VEC, L, NCH><<<grid, SG_THREADS, 0, st>>>(p, p.in, p.ldIn, p.xrow, p.ldX, n);
       ROC_LAUNCH_CHECK();
+      note_launch(ROC_SG_LAUNCH_RECORD, -1, VEC, L, NCH, grid);
     }
     return ROC_OK;
   });
@@ -1500,6 +1519,7 @@ static int run_planned(roc_sg_plan* pl, int H, const float* in, int64_t ldIn, fl
 extern "C" int roc_sg_forward_planned(const roc_sg_plan* plc, int H, const float* in, int64_t ldIn,
                                       float* out, int64_t ldOut, int epilogue, roc_stream_t stream) {
   roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  clear_launches();
   if (!pl || H <= 0 || !in || !out || ldIn < H || ldOut < H) return ROC_ERR_INVALID;
   return run_planned<SG_RED_SUM>(pl, H, in, ldIn, out, ldOut, nullptr, 0, epilogue, 0, as_stream(stream));
 }
@@ -1529,6 +1549,7 @@ extern "C" int roc_sg_minmax_forward_planned(const roc_sg_plan* plc, int aggr, i
                                              float* out, int64_t ldOut, roc_vid_t* arg, int64_t ldArg,
                                              roc_stream_t stream) {
   roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  clear_launches();
   if (!pl || (aggr != ROC_SG_AGGR_MAX && aggr != ROC_SG_AGGR_MIN) || H <= 0 || !in || !out || !arg || ldIn < H ||
       ldOut < H || ldArg < H)
     return ROC_ERR_INVALID;
@@ -1541,6 +1562,7 @@ extern "C" int roc_sg_minmax_backward_planned(const roc_sg_plan* plc, int H, roc
                                               int64_t ldG, const roc_vid_t* arg, int64_t ldArg, float* inGrad,
                                               int64_t ldIn, roc_stream_t stream) {
   roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  clear_launches();
   if (!pl || H <= 0 || !outGrad || !arg || !inGrad || ldG < H || ldArg < H || ldIn < H) return ROC_ERR_INVALID;
   return run_planned<SG_RED_MASK>(pl, H, outGrad, ldG, inGrad, ldIn, arg, ldArg, 0, selfBase, as_stream(stream));
 }
@@ -1577,6 +1599,7 @@ extern "C" int roc_sg_attn_forward_planned(const roc_sg_plan* plc, int heads, in
                                            float* out, int64_t ldOut, float* stats, int64_t ldStats,
                                            roc_stream_t stream) {
   roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  clear_launches();
   if (!pl || !in || !score || !out || !stats || heads <= 0 || H <= 0 || ldIn < H || ldOut < H ||
       ldS < 2 * (int64_t)heads || ldStats < 2 * (int64_t)heads)
     return ROC_ERR_INVALID;
@@ -1603,6 +1626,7 @@ extern "C" int roc_sg_attn_backward_planned(const roc_sg_plan* plc, int heads, i
                                             const float* outGrad, int64_t ldG, float* inGrad, int64_t ldInG,
                                             float* scoreGrad, int64_t ldSG, roc_stream_t stream) {
   roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  clear_launches();
   if (!pl || !in || !score || !out || !stats || !outGrad || !inGrad || !scoreGrad || heads <= 0 || H <= 0 ||
       ldIn < H || ldOut < H || ldG < H || ldInG < H || ldS < 2 * (int64_t)heads || ldStats < 2 * (int64_t)heads ||
       ldSG < 2 * (int64_t)heads)
@@ -1658,4 +1682,10 @@ extern "C" int roc_sg_backward(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t 
                                float* inGrad, roc_stream_t stream) {
   // Forward and backward do exactly the same thing (scattergather_kernel.cu:168-169).
   return roc_sg_forward(rowLeft, rowRight, colLeft, H, rowEnd, colSrc, outGrad, inGrad, stream);
+}
+
+extern "C" int roc_sg_last_call_info(roc_sg_call_info* info) {
+  if (!info) return ROC_ERR_INVALID;
+  *info = t_call;
+  return ROC_OK;
 }

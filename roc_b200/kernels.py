@@ -145,6 +145,12 @@ class SgPlan:
             pass
 
 
+def sg_launches():
+    """The kernel launches of this thread's last planned ScatterGather call (roc_sg_last_call_info): a list of dicts
+    kind ("main", "ring", "fixup", ...), red, vec, lanes, nch, grid."""
+    return _lib.sg_last_call_info()
+
+
 def sg_forward(row_left, row_right, col_left, row_end, col_src, x):
     """Plan-less form with the reference kernel's argument list; dense [N][H] in, [Nloc][H] out."""
     assert x.is_contiguous()

@@ -36,9 +36,11 @@ def test_no_undeclared_prototypes():
 
 
 def test_struct_layouts_match_the_header(tmp_path):
-    """The ctypes mirrors of the C structs (roc_linear_bwd_args, roc_gemm_info, roc_perf_metrics) have the C layout:
-    a tiny C program compiled against include/roc_b200.h prints sizeof / offsetof of every field."""
-    structs = [("roc_linear_bwd_args", _lib.LinearBwdArgs), ("roc_gemm_info", _lib.GemmInfo)]
+    """The ctypes mirrors of the C structs (roc_linear_bwd_args, roc_gemm_info, roc_sg_launch, roc_sg_call_info,
+    roc_perf_metrics) have the C layout: a tiny C program compiled against include/roc_b200.h prints sizeof / offsetof
+    of every field."""
+    structs = [("roc_linear_bwd_args", _lib.LinearBwdArgs), ("roc_gemm_info", _lib.GemmInfo),
+               ("roc_sg_launch", _lib.SgLaunch), ("roc_sg_call_info", _lib.SgCallInfo)]
     prog = ['#include <stdio.h>', '#include <stddef.h>', '#include "roc_b200.h"', 'int main(void) {']
     for cname, py in structs:
         prog += ['  printf("%%zu\\n", sizeof(%s));' % cname]
@@ -72,6 +74,22 @@ def test_gemm_info_hook_without_a_gemm():
     t.join()
     assert got == [{k: 0 for k, _ in _lib.GemmInfo._fields_}]
     assert _lib.lib.roc_last_gemm_path(1) in (0, 1, 2) and _lib.lib.roc_last_gemm_path(7) == 0
+
+
+def test_sg_call_info_hook_without_a_call():
+    """roc_sg_last_call_info rejects a NULL info, reports no launches on a thread that has made no ScatterGather call,
+    and its constants match the header's."""
+    assert _lib.lib.roc_sg_last_call_info(None) == _lib.ROC_ERR_INVALID
+    import threading
+    got = []
+    t = threading.Thread(target=lambda: got.append(_lib.sg_last_call_info()))
+    t.start()
+    t.join()
+    assert got == [[]]
+    hdr = open(os.path.join(ROOT, "include", "roc_b200.h")).read()
+    assert int(re.search(r"#define ROC_SG_MAX_LAUNCHES (\d+)", hdr).group(1)) == _lib.SG_MAX_LAUNCHES
+    for i, kind in enumerate(_lib.SG_LAUNCH_KINDS):
+        assert re.search(r"#define ROC_SG_LAUNCH_%s %d\b" % (kind.upper(), i), hdr), kind
 
 
 def test_library_is_sm90a_only():

@@ -198,6 +198,49 @@ int roc_sg_attn_backward_planned(const roc_sg_plan* plan, int heads, int H, floa
                                  int64_t ldG, float* inGrad, int64_t ldInG, float* scoreGrad, int64_t ldSG,
                                  roc_stream_t stream);
 
+/* Edge-weighted aggregation (GCN with edge weights, weighted graphs, edge saliency).  The reference declares edge
+ * tensors (gnn.h:178) but never reads them; these semantics are this library's own.  For plan row r with id
+ * i = selfBase + r and in-edges e in CSR order with sources j = colSrc[e], the edge's weight is w[e - colLeft]: a flat
+ * fp32 array in the plan's edge order.
+ *   out[r][h] = sum_e w[e] * in[j][h]
+ * accumulated as fmaf(w, in, acc) from +0 in the plan's fixed per-row order, with no atomics.  A row of degree 0 gets
+ * 0.  With every weight 1.0 the result is bit-identical to roc_sg_forward_planned with ROC_SG_EPI_NONE: both take the
+ * same column blocks (1,024 floats on float4 rows, else 256) and the same row shapes.  `in` is
+ * indexed like roc_sg_forward_planned's.  ROC_ERR_INVALID: a NULL pointer or a leading dimension < H. */
+int roc_sg_weighted_forward_planned(const roc_sg_plan* plan, int H, const float* in, int64_t ldIn, const float* w,
+                                    float* out, int64_t ldOut, roc_stream_t stream);
+/* The gradient of the edge weights (an SDDMM): for every edge e of the plan, with G = outGrad indexed by plan row
+ * and X = in indexed like the forward's input,
+ *   dw[e - colLeft] = sum_h G[r][h] * X[j][h]          (accumulate != 0: added to the value dw holds)
+ * in a fixed reduction order (columns in blocks of 512 floats on float4 rows, 256 otherwise, added in block order),
+ * so the same call gives the same bits.  ROC_ERR_INVALID: a NULL pointer or a leading dimension < H. */
+int roc_sg_edge_dot_planned(const roc_sg_plan* plan, int H, const float* outGrad, int64_t ldG, const float* in,
+                            int64_t ldIn, float* dw, int accumulate, roc_stream_t stream);
+/* The transpose of a whole graph's CSR (rows 0..numNodes-1, edges 0..rowEnd[numNodes-1], every id < numNodes), for
+ * the exact input gradient of the weighted aggregation on any graph (directed, asymmetric weights, duplicate edges):
+ *   rowEndT  u64[numNodes]  END offsets of node v's out-edges
+ *   colT     u32[E]         their destinations
+ *   perm     u32[E]         the original edge of each transposed edge
+ * built by a stable radix sort of (colSrc, edge index), so destinations increase within a transposed row; on a
+ * symmetric graph whose rows have strictly increasing sources (rowEndT, colT) equals (rowEnd, colSrc).  It holds a plan
+ * over (rowEndT, colT) and a buffer for the permuted weights.  rowEnd / colSrc must outlive it only during creation.
+ * Creation synchronises the stream three times: to read E, to check the ids after the sort, and in the plan build
+ * (roc_sg_plan_create).  ROC_ERR_INVALID: a NULL pointer or numNodes == 0; ROC_ERR_UNSUPPORTED: an id >= numNodes
+ * (as a slice with global ids has), or E > 2^31 - 1.  roc_sg_transpose_info returns its device arrays and plan (tests). */
+typedef struct roc_sg_transpose roc_sg_transpose;
+int roc_sg_transpose_create(roc_vid_t numNodes, const roc_eid_t* rowEnd, const roc_vid_t* colSrc,
+                            roc_stream_t stream, roc_sg_transpose** transpose);
+int roc_sg_transpose_info(const roc_sg_transpose* transpose, const roc_eid_t** rowEndT, const roc_vid_t** colT,
+                          const uint32_t** perm, const roc_sg_plan** planT);
+void roc_sg_transpose_destroy(roc_sg_transpose* transpose);
+/* The weighted aggregation's input gradient, exact on any graph:
+ *   inGrad[j][h] = sum_{e : colSrc[e] = j} w[e] * outGrad[dst(e)][h]
+ * computed as wT[t] = w[perm[t]] (one small kernel per call, into a buffer the transpose grows on the stream like a
+ * plan's carries, so that changed weights are always seen) and roc_sg_weighted_forward_planned over the transposed
+ * plan with wT.  outGrad and inGrad have numNodes rows.  ROC_ERR_INVALID: a NULL pointer or a leading dimension < H. */
+int roc_sg_weighted_backward_planned(roc_sg_transpose* transpose, int H, const float* outGrad, int64_t ldG,
+                                     const float* w, float* inGrad, int64_t ldIn, roc_stream_t stream);
+
 /* Plan-less form with exactly the reference kernel's argument list
  * (scattergather_kernel.cu:21-28, EdgeStruct.dst dropped), dense ld == H.
  * Builds and frees a plan internally (synchronises); use the planned form in
@@ -217,10 +260,12 @@ int roc_sg_backward(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft, in
  * to one list.  Each entry:
  *   kind   ROC_SG_LAUNCH_*: the main kernel, its cp.async.bulk ring form (float4 sums of 17..64 T-columns), the
  *          fix-up of rows with at most 32 carries (one worker each), of rows with more (one CTA each), the attention
- *          stats fix-up, the attention backward's per-node record, and the fix-ups of its heads-wide partials
+ *          stats fix-up, the attention backward's per-node record, the fix-ups of its heads-wide partials, and the
+ *          weighted backward's weight permutation (first in its list)
  *   red    the reduction the kernel is instantiated for: 0 sum, 1 max, 2 min, 3 the min / max backward, 4 attention
- *          stats, 5 the attention forward, 6 its d s_dst gather, 7 its input-gradient gather; -1 for the record,
- *          which has none.  A sum fix-up finishing another reduction's partials reports 0.
+ *          stats, 5 the attention forward, 6 its d s_dst gather, 7 its input-gradient gather, 8 the weighted sum
+ *          (forward and backward), 9 the edge-weight gradient; -1 for the record and the permutation, which have
+ *          none.  A sum fix-up finishing another reduction's partials reports 0.
  *   vec    4 for float4 rows, else 1;  lanes, nch: the row shape (L lanes, chunks per lane);  grid: CTAs launched
  * count is the number of launches; the first ROC_SG_MAX_LAUNCHES are stored.  Every planned call clears the list first,
  * also one that fails before it launches anything.  ROC_ERR_INVALID for a NULL info. */
@@ -232,6 +277,7 @@ int roc_sg_backward(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft, in
 #define ROC_SG_LAUNCH_RECORD 5
 #define ROC_SG_LAUNCH_HEADS_FIXUP 6
 #define ROC_SG_LAUNCH_HEADS_BIG_FIXUP 7
+#define ROC_SG_LAUNCH_PERMUTE 8
 #define ROC_SG_MAX_LAUNCHES 32
 typedef struct {
   int kind, red, vec, lanes, nch;

@@ -195,12 +195,27 @@ public:
    * destination scores, the true gradient of the rest on a symmetric graph.  Never fused with neighbouring ops.
    * Single partition only (exit(1) otherwise). */
   Tensor attention_gather(const Tensor& input, const Tensor& scores, int heads, float negativeSlope = 0.2f);
+  /* Edge-weighted aggregation (roc_sg_weighted_forward_planned): out[v] = sum over v's in-edges e of
+   * edgeWeights[e] * input[src(e)].  edgeWeights is an edge tensor (create_edge_tensor).  Its backward is exact on any
+   * graph: init() builds the graph's transpose once (roc_sg_transpose) the first time a model has such an op, and the
+   * input gradient runs over it.  The edge tensor's gradient is computed only after set_edge_grad(edges, true).
+   * Never fused with neighbouring ops.  Single partition only (exit(1) otherwise). */
+  Tensor scatter_gather(const Tensor& input, const Tensor& edgeWeights);
+  /* Opt-in gradient of an edge tensor (off by default, like the raw features').  When on, backward() leaves in its
+   * gradient twin the sum, over every weighted scatter_gather that reads it, of sum_h outGrad[v][h] * input[src][h]
+   * per edge (roc_sg_edge_dot_planned): the first op to run backward overwrites it and the others add, so the
+   * previous step's value is never kept.  Call it before init() when the op's input needs no gradient of its own. */
+  void set_edge_grad(const Tensor& edges, bool on);
   void softmax_cross_entropy(const Tensor& logits, const Tensor& labels, const Tensor& mask);
   Tensor indegree_norm(const Tensor& _input);
   Tensor linear(const Tensor& _input, int outDim, ActiMode activation, Initializer* initializer = NULL);
   Tensor relu(const Tensor& _input);
   Tensor sigmoid(const Tensor& _input);
   template <typename DT> Tensor create_node_tensor(int _numHidden) const;
+  /* gnn.h:178, gnn.cc:534-560: one value per edge of this partition, dims = {numHidden, numEdges}, stored as a dense
+   * fp32 array in the CSR's edge order, with a gradient twin allocated on first use.  Only DT = float and
+   * numHidden == 1 (exit(1) otherwise).  set_tensor / get_tensor move its local edge count of values. */
+  template <typename DT> Tensor create_edge_tensor(int numHidden) const;
   Tensor create_weight_tensor(int _inDim, int _outDim, Initializer* initializer) const;
   void load_features(const Tensor& input, const std::string& filename);
   void load_labels(const Tensor& label, const std::string& filename);
@@ -282,6 +297,15 @@ public:
   float* stats;      /* [Nloc][statsLd] m | 1/Z per head of the last forward (Runtime arena) */
   int64_t statsLd;
   float* scratch[2]; /* gradients of an input that accumulates (or needs none), written here first (Runtime arena) */
+};
+
+class WeightedScatterGather : public GnnOp {  /* not in the reference: Model::scatter_gather(input, edgeWeights) */
+public:
+  WeightedScatterGather(const Model& model, const Tensor& input, const Tensor& edgeWeights);
+  virtual void init(const Model& model);
+  virtual void forward(const Model& model);
+  virtual void backward(const Model& model);
+  float* scratch;    /* the input gradient when another op already wrote it (added afterwards; Runtime arena) */
 };
 
 class InDegreeNorm : public GnnOp {  /* gnn.h:244-261, graphnorm.cc */

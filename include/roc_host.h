@@ -44,6 +44,12 @@ int roc_host_scatter_gather(roc_host* h, int t);
 int roc_host_scatter_gather_aggr(roc_host* h, int t, int aggr);
 /* Model::attention_gather(t, scores, heads, slope); scores has 2 * heads columns */
 int roc_host_attention_gather(roc_host* h, int t, int scores, int heads, float slope);
+/* Model::create_edge_tensor<float>(hidden): rows = this partition's edge count */
+int roc_host_create_edge_tensor(roc_host* h, int hidden);
+/* Model::scatter_gather(t, edges): edge-weighted aggregation */
+int roc_host_scatter_gather_weighted(roc_host* h, int t, int edges);
+/* Model::set_edge_grad(edges, on) */
+int roc_host_set_edge_grad(roc_host* h, int edges, int on);
 int roc_host_relu(roc_host* h, int t);
 int roc_host_sigmoid(roc_host* h, int t);
 int roc_host_add(roc_host* h, int a, int b);

@@ -46,7 +46,9 @@ class GemmInfo(C.Structure):
 
 SG_LAUNCH_MAIN, SG_LAUNCH_RING, SG_LAUNCH_FIXUP, SG_LAUNCH_BIG_FIXUP = 0, 1, 2, 3      # roc_sg_launch.kind
 SG_LAUNCH_STAT_FIXUP, SG_LAUNCH_RECORD, SG_LAUNCH_HEADS_FIXUP, SG_LAUNCH_HEADS_BIG_FIXUP = 4, 5, 6, 7
-SG_LAUNCH_KINDS = ("main", "ring", "fixup", "big_fixup", "stat_fixup", "record", "heads_fixup", "heads_big_fixup")
+SG_LAUNCH_PERMUTE = 8
+SG_LAUNCH_KINDS = ("main", "ring", "fixup", "big_fixup", "stat_fixup", "record", "heads_fixup", "heads_big_fixup",
+                   "permute")
 SG_MAX_LAUNCHES = 32
 
 
@@ -107,6 +109,12 @@ PROTOTYPES = {
     "roc_sg_attn_forward_planned": (i32, [vp, i32, i32, f32, u32, vp, i64, vp, i64, vp, i64, vp, i64, vp]),
     "roc_sg_attn_backward_planned": (i32, [vp, i32, i32, f32, u32, vp, i64, vp, i64, vp, i64, vp, i64, vp, i64, vp,
                                            i64, vp, i64, vp]),
+    "roc_sg_weighted_forward_planned": (i32, [vp, i32, vp, i64, vp, vp, i64, vp]),
+    "roc_sg_edge_dot_planned": (i32, [vp, i32, vp, i64, vp, i64, vp, i32, vp]),
+    "roc_sg_transpose_create": (i32, [u32, vp, vp, vp, C.POINTER(vp)]),
+    "roc_sg_transpose_info": (i32, [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]),
+    "roc_sg_transpose_destroy": (None, [vp]),
+    "roc_sg_weighted_backward_planned": (i32, [vp, i32, vp, i64, vp, vp, i64, vp]),
     "roc_sg_forward": (i32, [u32, u32, u64, i32, vp, vp, vp, vp, vp]),
     "roc_sg_backward": (i32, [u32, u32, u64, i32, vp, vp, vp, vp, vp]),
     "roc_sg_last_call_info": (i32, [C.POINTER(SgCallInfo)]),
@@ -164,6 +172,9 @@ PROTOTYPES = {
     "roc_host_scatter_gather_aggr": (i32, [vp, i32, i32]),
     "roc_host_attention_gather": (i32, [vp, i32, i32, i32, f32]),
     "roc_host_get_aggr_index": (i32, [vp, i32, vp]),
+    "roc_host_create_edge_tensor": (i32, [vp, i32]),
+    "roc_host_scatter_gather_weighted": (i32, [vp, i32, i32]),
+    "roc_host_set_edge_grad": (i32, [vp, i32, i32]),
     "roc_host_relu": (i32, [vp, i32]),
     "roc_host_sigmoid": (i32, [vp, i32]),
     "roc_host_add": (i32, [vp, i32, i32]),

@@ -94,6 +94,11 @@ int roc_host_scatter_gather_aggr(roc_host* h, int t, int aggr) {
 int roc_host_attention_gather(roc_host* h, int t, int scores, int heads, float slope) {
   return h->push(h->m().attention_gather(h->at(t), h->at(scores), heads, slope));
 }
+int roc_host_create_edge_tensor(roc_host* h, int hidden) { return h->push(h->m().create_edge_tensor<DATATYPE>(hidden)); }
+int roc_host_scatter_gather_weighted(roc_host* h, int t, int edges) {
+  return h->push(h->m().scatter_gather(h->at(t), h->at(edges)));
+}
+int roc_host_set_edge_grad(roc_host* h, int edges, int on) { h->m().set_edge_grad(h->at(edges), on != 0); return 0; }
 int roc_host_get_aggr_index(roc_host* h, int t, uint32_t* host) { h->m().get_aggr_index(h->at(t), host); return 0; }
 int roc_host_relu(roc_host* h, int t) { return h->push(h->m().relu(h->at(t))); }
 int roc_host_sigmoid(roc_host* h, int t) { return h->push(h->m().sigmoid(h->at(t))); }

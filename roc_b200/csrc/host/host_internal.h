@@ -93,6 +93,7 @@ struct RuntimeImpl {
   void* linWs = nullptr; size_t linWsBytes = 0;           // split-K workspace of Linear backward
   void* staging = nullptr; size_t stagingBytes = 0;       // H2D staging for dense host rows -> padded rows
   float* flatGrad = nullptr; size_t flatGradCount = 0;    // all dW, one all-reduce
+  roc_sg_transpose* sgTranspose = nullptr;                // the graph's transpose, built by init() for weighted ops
   roc_perf_metrics* d_perf = nullptr;
   roc_perf_metrics h_perf{};
   uint32_t trainStep = 0;

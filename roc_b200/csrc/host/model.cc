@@ -58,6 +58,18 @@ Tensor Model::create_node_tensor<int>(int _numHidden) const {
   return t;
 }
 
+// gnn.cc:534-560: edge tensor = [numEdges][numHidden]; this process holds its partition's edges, in CSR order.
+template <>
+Tensor Model::create_edge_tensor<DATATYPE>(int numHidden) const {
+  if (numHidden != 1) ROC_FATAL("create_edge_tensor: only numHidden == 1 (one weight per edge) is supported");
+  Tensor t(Tensor::EDGE_TENSOR);
+  t.numDim = 2;
+  t.dims[0] = numHidden;
+  t.dims[1] = myGraph.numEdges;
+  t.region = ctx->new_tensor((int64_t)(myGraph.colRight - myGraph.colLeft + 1), numHidden, numHidden, false, false);
+  return t;
+}
+
 // gnn.cc:591-623: weight [inDim][outDim] (dim0 = inDim fastest => W_mem[o*inDim + i]).
 // The reference keeps one dW replica per GPU inside one region; here each process
 // owns its replica and replicas are summed by one NCCL all-reduce (Model::update).
@@ -115,6 +127,17 @@ Tensor Model::attention_gather(const Tensor& input, const Tensor& scores, int he
   GnnOp* op = new AttentionGather(*this, input, scores, heads, negativeSlope);
   layers.push_back(op);
   return op->outputs[0];
+}
+Tensor Model::scatter_gather(const Tensor& input, const Tensor& edgeWeights) {
+  if (ctx->numParts > 1)
+    ROC_FATAL("scatter_gather: edge-weighted aggregation runs on one partition only (numParts > 1 is not supported)");
+  GnnOp* op = new WeightedScatterGather(*this, input, edgeWeights);
+  layers.push_back(op);
+  return op->outputs[0];
+}
+void Model::set_edge_grad(const Tensor& edges, bool on) {
+  if (edges.type != Tensor::EDGE_TENSOR) ROC_FATAL("set_edge_grad: not an edge tensor");
+  ctx->t(edges.region).requiresGrad = on;
 }
 void Model::get_aggr_index(const Tensor& out, uint32_t* host) const {
   for (GnnOp* op : layers) {
@@ -387,7 +410,8 @@ bool Model::init(const Config& config) {
     const ScatterGather* sgl = as<ScatterGather>(layers[l]);
     const char* nm = sgl ? (sgl->aggr == AGGR_MAX ? "scatter_gather(max)" : sgl->aggr == AGGR_MIN ? "scatter_gather(min)"
                                                                                                   : "scatter_gather") :
-                     as<AttentionGather>(layers[l]) ? "attention_gather" : as<Linear>(layers[l]) ? "linear" :
+                     as<AttentionGather>(layers[l]) ? "attention_gather" :
+                     as<WeightedScatterGather>(layers[l]) ? "scatter_gather(weighted)" : as<Linear>(layers[l]) ? "linear" :
                      as<InDegreeNorm>(layers[l]) ? "indegree_norm" : as<Activation>(layers[l]) ? "activation" :
                      as<Dropout>(layers[l]) ? "dropout" : as<Element>(layers[l]) ? "add" :
                      as<SoftmaxCrossEntropy>(layers[l]) ? "softmax_cross_entropy" : "op";
@@ -837,6 +861,63 @@ void AttentionGather::backward(const Model& model) {
     float* g = rt->grad(inputs[i].region);
     ROC_CHECK(roc_add_fwd(model.local_rows(), x.H, g, x.ld, scratch[i], x.ld, g, x.ld, rt->stream));
   }
+}
+
+// ------------------------------------------------- WeightedScatterGather -----
+WeightedScatterGather::WeightedScatterGather(const Model& model, const Tensor& _input, const Tensor& _edges)
+    : GnnOp(_input, _edges), scratch(nullptr) {
+  ROC_ASSERT(_input.type == Tensor::NODE_TENSOR && _input.numDim == 2 && _input.dims[1] == model.myGraph.numNodes);
+  if (_edges.type != Tensor::EDGE_TENSOR || _edges.dims[0] != 1)
+    ROC_FATAL("scatter_gather: the weights must be an edge tensor with one value per edge");
+  trainableInputs[1] = false;
+  numOutputs = 1;
+  outputs[0] = model.create_node_tensor<DATATYPE>((int)_input.dims[0]);
+}
+// The first weighted op's init builds the graph's transpose (one synchronisation), which every weighted op shares.
+void WeightedScatterGather::init(const Model& model) {
+  RuntimeImpl* rt = model.ctx;
+  if (rt->sgTranspose) return;
+  const Graph& g = model.myGraph;
+  ROC_CHECK(roc_sg_transpose_create(g.numNodes, g.d_rowEnd, g.d_colSrc, rt->stream, &rt->sgTranspose));
+}
+
+void WeightedScatterGather::forward(const Model& model) {
+  RuntimeImpl* rt = model.ctx;
+  const int H = (int)inputs[0].dims[0];
+  const int x = inputs[0].region, y = outputs[0].region;
+  rt->sg_begin(H);
+  ROC_CHECK(roc_sg_weighted_forward_planned(model.myGraph.plan, H, rt->data(x), rt->t(x).ld, rt->data(inputs[1].region),
+                                            rt->data(y), rt->t(y).ld, rt->stream));
+  rt->sg_end();
+}
+
+// dX by the weighted sum over the transpose, then (opt-in) the edge gradient.  Both overwrite in the first op to run
+// backward on their input (resetInputGrads) and add in the others.
+void WeightedScatterGather::backward(const Model& model) {
+  RuntimeImpl* rt = model.ctx;
+  const int H = (int)inputs[0].dims[0];
+  const int x = inputs[0].region, e = inputs[1].region, y = outputs[0].region;
+  const bool wantX = rt->t(x).requiresGrad, wantE = rt->t(e).requiresGrad;
+  if (!rt->t(y).requiresGrad) {
+    if (wantE) ROC_FATAL("set_edge_grad: call it before init() when the weighted scatter_gather's input has no gradient");
+    return;
+  }
+  const int64_t ldY = rt->t(y).ld, ldX = rt->t(x).ld;
+  rt->sg_begin(H);
+  if (wantX) {
+    float* dst = rt->grad(x);
+    if (!resetInputGrads[0]) {
+      if (!scratch) scratch = (float*)rt->dmalloc((size_t)std::max<int64_t>(model.local_rows(), 1) * (size_t)ldX * sizeof(float));
+      dst = scratch;
+    }
+    ROC_CHECK(roc_sg_weighted_backward_planned(rt->sgTranspose, H, rt->grad(y), ldY, rt->data(e), dst, ldX, rt->stream));
+    if (!resetInputGrads[0])
+      ROC_CHECK(roc_add_fwd(model.local_rows(), H, rt->grad(x), ldX, scratch, ldX, rt->grad(x), ldX, rt->stream));
+  }
+  if (wantE)
+    ROC_CHECK(roc_sg_edge_dot_planned(model.myGraph.plan, H, rt->grad(y), ldY, rt->data(x), ldX, rt->grad(e),
+                                      resetInputGrads[1] ? 0 : 1, rt->stream));
+  rt->sg_end();
 }
 
 // --------------------------------------------------------- InDegreeNorm -----

@@ -399,6 +399,7 @@ Runtime::~Runtime() {
     for (size_t q = 0; q < x.peerGrad.size(); q++) if ((int)q != impl->myPart && x.peerGrad[q]) cudaIpcCloseMemHandle(x.peerGrad[q]);
   }
   impl->comm.destroy();
+  roc_sg_transpose_destroy(impl->sgTranspose);
   impl->dfree_all();
   for (cudaStream_t ps : impl->peerStreams) cudaStreamDestroy(ps);
   for (cudaEvent_t pe : impl->peerDone) cudaEventDestroy(pe);

@@ -31,9 +31,13 @@
 //    The sum and min / max entry points check their arguments and share one column-block driver (run_planned).
 //  * attention aggregation (roc_sg_attn_*) is more reductions of the same kernel: a stats pass and an a-weighted
 //    sum forward; a per-node record kernel and two gathers backward.  Both entry points share attn_setup.
+//  * edge-weighted aggregation (roc_sg_weighted_*, roc_sg_edge_dot_planned) is two more: WSUM, a sum with one FMA by
+//    each edge's weight, finished by the sum's fix-ups; EDOT, one dot product G[i] . X[j] per edge, which carries
+//    nothing.  The exact backward runs WSUM over a transposed CSR (roc_sg_transpose) with the weights permuted.
 //
 // Algorithmic bytes per launch (DESIGN.md): E*(4H+4) + Nloc*(4H+8); min / max forward E*(4H+4) + Nloc*(8H+8),
-// backward E*(8H+4) + Nloc*(4H+8); attention in DESIGN.md §3.1.
+// backward E*(8H+4) + Nloc*(4H+8); weighted forward E*(4H+8) + Nloc*(4H+8), edge dot E*(4H+8) + Nloc*4H; attention
+// in DESIGN.md §3.1.
 #include <cub/cub.cuh>
 #include <thrust/iterator/counting_iterator.h>
 #include <algorithm>
@@ -188,6 +192,9 @@ template <> struct V<4> {
   static __device__ __forceinline__ T ld_plain(const T* p) { return *p; }
   static __device__ __forceinline__ void st(T* p, const T& v) { *p = v; }
   static __device__ __forceinline__ void add(T& a, const T& b) { a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w; }
+  static __device__ __forceinline__ void fma(T& a, float w, const T& b) {
+    a.x = fmaf(w, b.x, a.x); a.y = fmaf(w, b.y, a.y); a.z = fmaf(w, b.z, a.z); a.w = fmaf(w, b.w, a.w);
+  }
   static __device__ __forceinline__ T rdiv(const T& a, const RowDiv& r) {
     float v[4] = {a.x, a.y, a.z, a.w};
     rowdiv4(v, r);          // one safety test for the four quotients
@@ -205,6 +212,7 @@ template <> struct V<1> {
   static __device__ __forceinline__ T ld_plain(const T* p) { return *p; }
   static __device__ __forceinline__ void st(T* p, const T& v) { *p = v; }
   static __device__ __forceinline__ void add(T& a, const T& b) { a += b; }
+  static __device__ __forceinline__ void fma(T& a, float w, const T& b) { a = fmaf(w, b, a); }
   static __device__ __forceinline__ T rdiv(const T& a, const RowDiv& r) { return rowdiv(a, r); }
   static __device__ __forceinline__ T relu(const T& a) { return relu_nanprop(a); }
 };
@@ -215,8 +223,10 @@ template <> struct V<1> {
 // it adds the gathered gradient only where the gathered index names the row being computed.
 // The attention passes (roc_sg_attn_*): ASTAT gives each row's (m, Z) per head, ATTN the a-weighted sum, ADST the
 // destination-score gradient (heads wide), ASRC the input gradient and the source-score gradient.
+// The edge-weighted passes (roc_sg_weighted_*, roc_sg_edge_dot_planned): WSUM the w-weighted sum, EDOT the per-edge
+// dot product G[i] . X[j] (the gradient of the edge weights).
 enum { SG_RED_SUM = 0, SG_RED_MAX = ROC_SG_AGGR_MAX, SG_RED_MIN = ROC_SG_AGGR_MIN, SG_RED_MASK = 3,
-       SG_RED_ASTAT = 4, SG_RED_ATTN = 5, SG_RED_ADST = 6, SG_RED_ASRC = 7 };
+       SG_RED_ASTAT = 4, SG_RED_ATTN = 5, SG_RED_ADST = 6, SG_RED_ASRC = 7, SG_RED_WSUM = 8, SG_RED_EDOT = 9 };
 constexpr uint32_t SG_NOARG = 0xFFFFFFFFu;   // index of a row that has no edge yet
 
 // The ordering rule: the candidate v replaces the current a iff it is strictly greater (smaller) or it is NaN and a
@@ -326,15 +336,18 @@ struct SgParams {
   void* carryArg;       // MAX / MIN: [numCarries][ldC] indices of the carry partials
   size_t ldArg;         // in units of T
   uint32_t selfBase;    // MASK, attention: id of local row 0 in the id space of col
-  // attention (units of float unless stated)
-  const float* score;   // [*][ldS]  s_dst | s_src, indexed like `in`
+  int dwAdd;            // EDOT: add to dw instead of overwriting it
+  // attention (units of float unless stated).  The edge-weighted passes use two of its slots (score, out2), so that
+  // the struct, every kernel's parameter block, keeps its layout (a union there changed the attention kernels' code).
+  const float* score;   // [*][ldS]  s_dst | s_src, indexed like `in`;  WSUM: [E] each local edge's weight
   const float* stats;   // ATTN: [nloc][ldStats] m | 1/Z of the local rows
   const float4* rec;    // ADST / ASRC: [*][heads] {s_dst, m, 1/Z, D}, indexed like `in`
-  const void* xrow;     // ADST: G, ASRC: X, the local row's own row (units of T, ldX), indexed like `in`
-  float* out2;          // ASTAT: unused; ADST / ASRC: heads-wide output [nloc][ldOut2]
+  const void* xrow;     // ADST, EDOT: G, ASRC: X, the local row's own row (units of T, ldX); EDOT: indexed by plan
+                        // row, else like `in`
+  float* out2;          // ASTAT: unused; ADST / ASRC: heads-wide output [nloc][ldOut2];  EDOT: [E] dw of each local edge
   float* carry2;        // [numCarries][SG_LDC2] heads-wide partials (ASTAT: m | Z)
   size_t ldS, ldStats, ldX, ldOut2;
-  uint32_t heads, ftShift, H;   // ftShift: log2 of the T-columns per head (31 for one head)
+  uint32_t heads, ftShift, H;   // ftShift: log2 of the T-columns per head (31 for one head); EDOT: H floats per row
   float slope;
 };
 constexpr int SG_LDC2 = 16;     // 2 * the most heads
@@ -380,9 +393,11 @@ sg_chunk_kernel(const SgParams p) {
   typedef typename V<VEC>::T T;
   typedef typename V<VEC>::I I;
   constexpr bool MM = RED == SG_RED_MAX || RED == SG_RED_MIN;
-  constexpr bool AT = RED >= SG_RED_ASTAT;                       // an attention pass
+  constexpr bool AT = RED >= SG_RED_ASTAT && RED <= SG_RED_ASRC; // an attention pass
   constexpr bool SV = RED == SG_RED_ATTN || RED == SG_RED_ADST;  // gathers s_src[j] beside in[j]
   constexpr bool XI = RED == SG_RED_ADST || RED == SG_RED_ASRC;  // holds a row of its own row i, and heads-wide sums
+  constexpr bool WS = RED == SG_RED_WSUM;                        // loads each edge's weight beside its source id
+  constexpr bool ED = RED == SG_RED_EDOT;                        // holds G[i], stores one dot product per edge
   constexpr int WPB = SG_THREADS / L;
   constexpr uint32_t CH = SG_CH;
   const int lane = threadIdx.x % L;
@@ -427,13 +442,17 @@ sg_chunk_kernel(const SgParams p) {
   }
 
   // Attention: the head of each column chunk, its valid floats, and the current row's state (row_state).
-  constexpr int NA = AT ? NCH : 1;
+  constexpr int NA = (AT || ED) ? NCH : 1;
   uint32_t kh[NA];
   int nv[NA];
   float accS[NA];       // ASTAT: Z (acc holds m); ADST / ASRC: the heads-wide sums
   float r0s[NA], r1s[NA], r2s[NA];   // ASTAT: s_dst[i]; ATTN: s_dst[i], m[i], 1/Z[i]; ASRC: s_src[i]
   float4 rrec[RED == SG_RED_ADST ? NCH : 1];   // ADST: the record of row i
-  T xi[XI ? NCH : 1];   // ADST: G[i], ASRC: X[i]
+  T xi[(XI || ED) ? NCH : 1];   // ADST, EDOT: G[i], ASRC: X[i]
+  if constexpr (ED) {
+#pragma unroll
+    for (int ch = 0; ch < NCH; ch++) nv[ch] = t_floats<VEC>((uint32_t)(lane + ch * L), p);
+  }
   if constexpr (AT) {
 #pragma unroll
     for (int ch = 0; ch < NCH; ch++) {
@@ -460,6 +479,11 @@ sg_chunk_kernel(const SgParams p) {
           xi[ch] = V<VEC>::ld(reinterpret_cast<const T*>(p.xrow) + gi * p.ldX + min((uint32_t)(lane + ch * L), p.Q - 1u));
       }
     }
+    if constexpr (ED) {
+#pragma unroll
+      for (int ch = 0; ch < NCH; ch++)
+        xi[ch] = V<VEC>::ld(reinterpret_cast<const T*>(p.xrow) + (uint64_t)cur * p.ldX + min((uint32_t)(lane + ch * L), p.Q - 1u));
+    }
   };
   row_state();
 
@@ -467,6 +491,7 @@ sg_chunk_kernel(const SgParams p) {
   // inlining it at every edge position made the kernel 4096 SASS instructions and
   // instruction-fetch bound.
   auto flush = [&]() {
+    if constexpr (ED) return;           // its outputs are per edge, stored as it goes
     char* dstb = (kind == 0)
         ? reinterpret_cast<char*>(reinterpret_cast<T*>(p.carry) + lane) + (uint64_t)carrySlot * ((uint32_t)p.ldC * (uint32_t)sizeof(T))
         : reinterpret_cast<char*>(out + lane) + (uint64_t)cur * ((uint32_t)p.ldOut * (uint32_t)sizeof(T));
@@ -559,13 +584,22 @@ sg_chunk_kernel(const SgParams p) {
   for (uint32_t base = e; base < ee; base += U) {
     const uint32_t cnt = min((uint32_t)U, ee - base);
     uint32_t srcs[U];
+    float wv[WS ? U : 1];                      // WSUM: each edge's weight, loaded like its source id
     if (cnt == (uint32_t)U) {
       const uint32_t* colp = col + base;       // full group: one address, immediate offsets
 #pragma unroll
       for (int u = 0; u < U; u++) srcs[u] = __ldg(colp + u);
+      if constexpr (WS) {
+#pragma unroll
+        for (int u = 0; u < U; u++) wv[u] = __ldg(p.score + base + u);
+      }
     } else {
 #pragma unroll
       for (int u = 0; u < U; u++) srcs[u] = __ldg(col + min(base + (uint32_t)u, eLast));
+      if constexpr (WS) {
+#pragma unroll
+        for (int u = 0; u < U; u++) wv[u] = __ldg(p.score + min(base + (uint32_t)u, eLast));
+      }
     }
     T v[U][NCH];
     I av[RED == SG_RED_MASK ? U : 1][RED == SG_RED_MASK ? NCH : 1];
@@ -640,6 +674,19 @@ sg_chunk_kernel(const SgParams p) {
                 const float a = attn_alpha(leaky(z, p.slope), r.y, r.z);
                 V<VEC>::add(acc[ch], attn_scale(a, v[u][ch]));
                 accS[ch] += a * (d[ch] - r.w) * (z > 0.f ? 1.f : p.slope);
+              }
+            } else if constexpr (WS) {
+#pragma unroll
+              for (int ch = 0; ch < NCH; ch++) V<VEC>::fma(acc[ch], wv[u], v[u][ch]);
+            } else if constexpr (ED) {
+              // dw(e) = G[i] . X[j]: v is X[j], xi is G[i]; the whole row reduced like one attention head
+              float d[NCH];
+#pragma unroll
+              for (int ch = 0; ch < NCH; ch++) d[ch] = dot_t(xi[ch], v[u][ch], nv[ch]);
+              head_sum<L, NCH>(d, 31u, wmask);
+              if (lane == 0) {
+                float* q = p.out2 + base + (uint32_t)u;
+                *q = p.dwAdd ? *q + d[0] : d[0];
               }
             } else {
 #pragma unroll
@@ -1188,10 +1235,12 @@ static int launch_ring(const SgParams& p, cudaStream_t st) {
 }
 
 // The widest row, in T-columns, that one launch of RED takes: 256 (1024 floats vectorised, 256 scalar; wider rows are
-// split into column blocks), but 128 on float4 rows for every reduction except the sum (min / max: the big-row fix-up
-// keeps values and indices of every lane group in static shared memory).  ASTAT's row is one score per head.
+// split into column blocks), but 128 on float4 rows for every reduction except the sum and the weighted sum (min /
+// max: the big-row fix-up keeps values and indices of every lane group in static shared memory).  The weighted sum
+// takes the sum's column blocks, so that with all-ones weights it gives the sum's bits at every width (the big-row
+// fix-up groups a row's carries by the block's lane count).  ASTAT's row is one score per head.
 constexpr int sg_max_q(int VEC, int RED) {
-  return RED == SG_RED_ASTAT ? SG_LDC2 / 2 : (VEC == 4 && RED != SG_RED_SUM) ? 128 : 256;
+  return RED == SG_RED_ASTAT ? SG_LDC2 / 2 : (VEC == 4 && RED != SG_RED_SUM && RED != SG_RED_WSUM) ? 128 : 256;
 }
 
 // The row shape of every launch: calls f(L, NCH), as std::integral_constants, for rows of Q T-columns.  L is the
@@ -1212,7 +1261,8 @@ static int with_shape(uint32_t Q, F&& f) {
 // Gathers in flight (U) and CTAs per SM (MINB) of sg_chunk_kernel, per reduction at NCH = 1, 2, 4, 8 chunks per lane.
 // They are lower than the sum's where a second value held or gathered per float (the min / max index, the min / max
 // backward's index row, s_src, the record, the local row's own row) would otherwise spill under the occupancy.
-constexpr int SG_SHAPE_U[8][4] = {
+// WSUM keeps the sum's U and holds U weights beside them, so at one chunk per lane it runs three CTAs per SM.
+constexpr int SG_SHAPE_U[10][4] = {
     {8, 4, 2, 1},   // SUM (U = 4 at L = 4)
     {4, 4, 1, 1},   // MAX
     {4, 4, 1, 1},   // MIN
@@ -1220,9 +1270,12 @@ constexpr int SG_SHAPE_U[8][4] = {
     {8, 0, 0, 0},   // ASTAT (one chunk: Q = heads)
     {4, 2, 1, 1},   // ATTN
     {4, 2, 1, 1},   // ADST
-    {2, 2, 1, 1}};  // ASRC
-constexpr int SG_SHAPE_MINB[8][4] = {
-    {4, 3, 3, 2}, {4, 3, 3, 2}, {4, 3, 3, 2}, {4, 3, 3, 2}, {4, 0, 0, 0}, {4, 3, 2, 2}, {4, 3, 2, 1}, {4, 2, 2, 1}};
+    {2, 2, 1, 1},   // ASRC
+    {8, 4, 2, 1},   // WSUM
+    {4, 2, 1, 1}};  // EDOT
+constexpr int SG_SHAPE_MINB[10][4] = {
+    {4, 3, 3, 2}, {4, 3, 3, 2}, {4, 3, 3, 2}, {4, 3, 3, 2}, {4, 0, 0, 0}, {4, 3, 2, 2}, {4, 3, 2, 1}, {4, 2, 2, 1},
+    {3, 3, 3, 2}, {4, 3, 2, 1}};
 static_assert(SG_RED_MAX == 1 && SG_RED_MIN == 2, "SG_SHAPE_U / SG_SHAPE_MINB rows follow the SG_RED_* values");
 constexpr int sg_nch_index(int NCH) { return NCH == 1 ? 0 : NCH == 2 ? 1 : NCH == 4 ? 2 : 3; }
 constexpr int sg_chunk_u(int RED, int L, int NCH) {
@@ -1277,7 +1330,7 @@ static int launch(const SgParams& p, cudaStream_t st) {
       ROC_LAUNCH_CHECK();
       note_launch(ROC_SG_LAUNCH_STAT_FIXUP, SG_RED_ASTAT, 1, 32, 1, grid);
     }
-  } else if constexpr (RED != SG_RED_ADST) {
+  } else if constexpr (RED != SG_RED_ADST && RED != SG_RED_EDOT) {   // EDOT's outputs are per edge: nothing carried
     constexpr int FIX = (RED == SG_RED_MAX || RED == SG_RED_MIN) ? RED : SG_RED_SUM;
     if ((rc = launch_fixups<VEC, L, NCH, FIX>(p, st)) != ROC_OK) return rc;
   }
@@ -1365,7 +1418,58 @@ static int find_id_end(roc_sg_plan* plan, cudaStream_t st) {
   return ROC_OK;
 }
 
+// ------------------------------------------------------- transposed CSR ---
+// From the stable sort of (colSrc, edge index): perm[t] is the original edge of transposed edge t, srcSorted[t] its
+// source.  Transposed row v (node v's out-edges) is [rowEndT[v - 1], rowEndT[v]); colT[t] is the destination of
+// perm[t], the row whose [start, end) holds it.
+__global__ void k_iota(uint32_t n, uint32_t* __restrict__ a) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) a[i] = i;
+}
+
+__global__ void k_transpose_col(uint32_t E, uint32_t N, const uint64_t* __restrict__ rowEnd,
+                                const uint32_t* __restrict__ perm, uint32_t* __restrict__ colT) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= E) return;
+  const uint64_t e = perm[t];
+  uint32_t lo = 0, hi = N;        // the first row r with rowEnd[r] > e
+  while (lo < hi) {
+    const uint32_t mid = lo + ((hi - lo) >> 1);
+    if (rowEnd[mid] > e) hi = mid; else lo = mid + 1;
+  }
+  colT[t] = lo;
+}
+
+__global__ void k_transpose_row_end(uint32_t N, uint32_t E, const uint32_t* __restrict__ srcSorted,
+                                    uint64_t* __restrict__ rowEndT) {
+  const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= N) return;
+  uint32_t lo = 0, hi = E;        // the number of sources <= v
+  while (lo < hi) {
+    const uint32_t mid = lo + ((hi - lo) >> 1);
+    if (srcSorted[mid] <= v) lo = mid + 1; else hi = mid;
+  }
+  rowEndT[v] = lo;
+}
+
+// wT[t] = w[perm[t]]: the weights in the transposed plan's edge order
+__global__ void k_permute(uint32_t E, const uint32_t* __restrict__ perm, const float* __restrict__ w,
+                          float* __restrict__ wT) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t < E) wT[t] = __ldg(w + perm[t]);
+}
+
 }  // namespace roc
+
+struct roc_sg_transpose {
+  uint32_t N = 0, E = 0;
+  uint64_t* rowEndT = nullptr;    // [N]
+  uint32_t* colT = nullptr;       // [E]
+  uint32_t* perm = nullptr;       // [E]
+  roc_sg_plan* planT = nullptr;   // the plan over (rowEndT, colT)
+  float* wT = nullptr;            // [E] the permuted weights of the last backward, grown on demand (grow)
+  size_t wTBytes = 0;
+};
 
 using namespace roc;
 
@@ -1491,24 +1595,39 @@ static void t_units(SgParams& p, int vw, int cols) {
   p.Q = ((uint32_t)cols + vw - 1) / vw;
 }
 
-// Reduction RED over the columns [0, H) of every row, in column blocks: 1,024 floats for the sum and 512 for min /
-// max when every leading dimension and pointer allows float4 rows, else 256.  `arg` holds the min / max indices
-// (written by the forward, gathered by the backward); the sum passes none.
+// The edge-weighted operands of run_planned: WSUM's weights, EDOT's G rows (indexed by plan row) and its output.
+struct SgEdge {
+  const float* w = nullptr;
+  const float* g = nullptr;
+  int64_t ldG = 0;
+  float* dw = nullptr;
+  bool accumulate = false;
+};
+
+// Reduction RED over the columns [0, H) of every row, in column blocks: 1,024 floats for the sum and the weighted sum
+// and 512 for the others when every leading dimension and pointer allows float4 rows, else 256.  `arg` holds the min / max indices
+// (written by the forward, gathered by the backward); the sum passes none.  EDOT's column blocks add their partial
+// dot products to dw in block order: the first overwrites it (or adds, with ed.accumulate), the later ones add.
 template <int RED>
 static int run_planned(roc_sg_plan* pl, int H, const float* in, int64_t ldIn, float* out, int64_t ldOut,
-                       const roc_vid_t* arg, int64_t ldArg, int epilogue, roc_vid_t selfBase, cudaStream_t st) {
-  const bool vec = float4_rows({in, out, arg}, {ldIn, ldOut, ldArg});
-  const int blockCols = !vec ? 256 : RED == SG_RED_SUM ? 1024 : 512;
-  int rc = grow_carries(pl, std::min(H, blockCols), st);
+                       const roc_vid_t* arg, int64_t ldArg, int epilogue, roc_vid_t selfBase, cudaStream_t st,
+                       const SgEdge& ed = SgEdge()) {
+  const bool vec = float4_rows({in, out, arg, ed.g}, {ldIn, ldOut, ldArg, ed.ldG});
+  const int blockCols = !vec ? 256 : (RED == SG_RED_SUM || RED == SG_RED_WSUM) ? 1024 : 512;
+  // EDOT carries nothing
+  int rc = RED == SG_RED_EDOT ? ROC_OK : grow_carries(pl, std::min(H, blockCols), st);
   // the min / max forward's index carries, which the kernels address with the float carries' leading dimension
   if (rc == ROC_OK && (RED == SG_RED_MAX || RED == SG_RED_MIN))
     rc = grow(pl->carryArg, pl->carryArgBytes, (size_t)pl->numCarries * pl->carryLd * sizeof(uint32_t), st);
   if (rc != ROC_OK) return rc;
   for (int c0 = 0; c0 < H; c0 += blockCols) {
     SgParams p = plan_params(pl);
-    p.in = in + c0; p.out = out + c0; p.epi = epilogue; p.selfBase = selfBase;
+    p.in = in + c0; p.out = out ? out + c0 : nullptr; p.epi = epilogue; p.selfBase = selfBase;
     if (arg) p.arg = const_cast<roc_vid_t*>(arg) + c0;
     p.ldIn = (size_t)ldIn; p.ldOut = (size_t)ldOut; p.ldArg = (size_t)ldArg;
+    p.score = ed.w; p.out2 = ed.dw; p.dwAdd = (ed.accumulate || c0 > 0) ? 1 : 0;
+    if (ed.g) { p.xrow = ed.g + c0; p.ldX = (size_t)ed.ldG; }
+    p.H = (uint32_t)std::min(H - c0, blockCols);
     t_units(p, vec ? 4 : 1, std::min(H - c0, blockCols));
     rc = vec ? dispatch<4, RED>(p, st) : dispatch<1, RED>(p, st);
     if (rc != ROC_OK) return rc;
@@ -1662,6 +1781,114 @@ extern "C" int roc_sg_attn_backward_planned(const roc_sg_plan* plc, int heads, i
   b2.out = inGrad; b2.ldOut = (size_t)ldInG; b2.out2 = scoreGrad + heads; b2.ldOut2 = (size_t)ldSG;
   t_units(b2, vw, H);
   return vec ? dispatch<4, SG_RED_ASRC>(b2, st) : dispatch<1, SG_RED_ASRC>(b2, st);
+}
+
+extern "C" int roc_sg_weighted_forward_planned(const roc_sg_plan* plc, int H, const float* in, int64_t ldIn,
+                                               const float* w, float* out, int64_t ldOut, roc_stream_t stream) {
+  roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  clear_launches();
+  if (!pl || H <= 0 || !in || !w || !out || ldIn < H || ldOut < H) return ROC_ERR_INVALID;
+  SgEdge ed;
+  ed.w = w;
+  return run_planned<SG_RED_WSUM>(pl, H, in, ldIn, out, ldOut, nullptr, 0, 0, 0, as_stream(stream), ed);
+}
+
+extern "C" int roc_sg_edge_dot_planned(const roc_sg_plan* plc, int H, const float* outGrad, int64_t ldG,
+                                       const float* in, int64_t ldIn, float* dw, int accumulate, roc_stream_t stream) {
+  roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  clear_launches();
+  if (!pl || H <= 0 || !outGrad || !in || !dw || ldG < H || ldIn < H) return ROC_ERR_INVALID;
+  SgEdge ed;
+  ed.g = outGrad; ed.ldG = ldG; ed.dw = dw; ed.accumulate = accumulate != 0;
+  return run_planned<SG_RED_EDOT>(pl, H, in, ldIn, nullptr, 0, nullptr, 0, 0, 0, as_stream(stream), ed);
+}
+
+extern "C" void roc_sg_transpose_destroy(roc_sg_transpose* tr) {
+  if (!tr) return;
+  roc_sg_plan_destroy(tr->planT);
+  cudaFree(tr->rowEndT); cudaFree(tr->colT); cudaFree(tr->perm); cudaFree(tr->wT);
+  delete tr;
+}
+
+extern "C" int roc_sg_transpose_create(roc_vid_t numNodes, const roc_eid_t* rowEnd, const roc_vid_t* colSrc,
+                                       roc_stream_t stream, roc_sg_transpose** out) {
+  if (!out || !rowEnd || numNodes == 0) return ROC_ERR_INVALID;
+  if (roc_device_count() <= 0) return ROC_ERR_NO_DEVICE;
+  if (numNodes >= 0xFFFFFFF0u) return ROC_ERR_UNSUPPORTED;
+  cudaStream_t st = as_stream(stream);
+  uint64_t E64 = 0;
+  ROC_CUDA(cudaMemcpyAsync(&E64, rowEnd + (numNodes - 1), sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  ROC_CUDA(cudaStreamSynchronize(st));
+  if (E64 > 0x7FFFFFFFull) return ROC_ERR_UNSUPPORTED;   // cub's sort counts items in an int
+  if (E64 > 0 && !colSrc) return ROC_ERR_INVALID;
+  roc_sg_transpose* tr = new (std::nothrow) roc_sg_transpose();
+  if (!tr) return ROC_ERR_NOMEM;
+  tr->N = numNodes; tr->E = (uint32_t)E64;
+  const uint32_t N = tr->N, E = tr->E;
+  uint32_t* iota = nullptr; uint32_t* srcSorted = nullptr; void* tmp = nullptr;
+  uint32_t maxSrc = 0;
+  int rc = ROC_OK;
+#define TR_CUDA(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { rc = (int)e_; goto done; } } while (0)
+  {
+    const int T = 256;
+    TR_CUDA(cudaMalloc(&tr->rowEndT, sizeof(uint64_t) * (size_t)N));
+    TR_CUDA(cudaMalloc(&tr->colT, sizeof(uint32_t) * std::max<size_t>(E, 1)));
+    TR_CUDA(cudaMalloc(&tr->perm, sizeof(uint32_t) * std::max<size_t>(E, 1)));
+    if (E) {
+      TR_CUDA(cudaMalloc(&iota, sizeof(uint32_t) * (size_t)E));
+      TR_CUDA(cudaMalloc(&srcSorted, sizeof(uint32_t) * (size_t)E));
+      k_iota<<<(E + T - 1) / T, T, 0, st>>>(E, iota);
+      count_launch();
+      size_t tb = 0;
+      TR_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, colSrc, srcSorted, iota, tr->perm, (int)E, 0, 32, st));
+      TR_CUDA(cudaMalloc(&tmp, tb ? tb : 16));
+      TR_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb, colSrc, srcSorted, iota, tr->perm, (int)E, 0, 32, st));
+      count_launch(4);
+      TR_CUDA(cudaMemcpyAsync(&maxSrc, srcSorted + (E - 1), sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+      TR_CUDA(cudaStreamSynchronize(st));
+      if (maxSrc >= N) { rc = ROC_ERR_UNSUPPORTED; goto done; }   // a slice (global ids) or a bad id
+      k_transpose_col<<<(E + T - 1) / T, T, 0, st>>>(E, N, rowEnd, tr->perm, tr->colT);
+      count_launch();
+    }
+    k_transpose_row_end<<<(N + T - 1) / T, T, 0, st>>>(N, E, srcSorted, tr->rowEndT);
+    count_launch();
+    TR_CUDA(cudaGetLastError());
+    rc = roc_sg_plan_create(0, N - 1, 0, tr->rowEndT, tr->colT, stream, &tr->planT);
+  }
+done:
+#undef TR_CUDA
+  cudaFree(iota); cudaFree(srcSorted); cudaFree(tmp);
+  if (rc != ROC_OK) { roc_sg_transpose_destroy(tr); return rc; }
+  *out = tr;
+  return ROC_OK;
+}
+
+extern "C" int roc_sg_transpose_info(const roc_sg_transpose* tr, const roc_eid_t** rowEndT, const roc_vid_t** colT,
+                                     const uint32_t** perm, const roc_sg_plan** planT) {
+  if (!tr) return ROC_ERR_INVALID;
+  if (rowEndT) *rowEndT = tr->rowEndT;
+  if (colT) *colT = tr->colT;
+  if (perm) *perm = tr->perm;
+  if (planT) *planT = tr->planT;
+  return ROC_OK;
+}
+
+extern "C" int roc_sg_weighted_backward_planned(roc_sg_transpose* tr, int H, const float* outGrad, int64_t ldG,
+                                                const float* w, float* inGrad, int64_t ldIn, roc_stream_t stream) {
+  clear_launches();
+  if (!tr || H <= 0 || !outGrad || !w || !inGrad || ldG < H || ldIn < H) return ROC_ERR_INVALID;
+  cudaStream_t st = as_stream(stream);
+  int rc = grow(tr->wT, tr->wTBytes, sizeof(float) * std::max<size_t>(tr->E, 1), st);
+  if (rc != ROC_OK) return rc;
+  if (tr->E) {
+    const uint32_t grid = (tr->E + 255) / 256;
+    k_permute<<<grid, 256, 0, st>>>(tr->E, tr->perm, w, tr->wT);
+    ROC_LAUNCH_CHECK();
+    note_launch(ROC_SG_LAUNCH_PERMUTE, -1, 1, 1, 1, grid);
+  }
+  SgEdge ed;
+  ed.w = tr->wT;
+  return run_planned<SG_RED_WSUM>(tr->planT, H, outGrad, ldG, inGrad, ldIn, nullptr, 0, 0, 0, st, ed);
 }
 
 extern "C" int roc_sg_forward(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft, int H,

@@ -142,3 +142,19 @@ def write_dataset(prefix, row_end, col_src, feats, labels, mask):
     write_feats_bin(prefix, feats)
     write_labels(prefix, labels)
     write_mask(prefix, mask)
+
+
+def gcn_edge_weights(row_end, col, w):
+    """GCN's symmetric normalisation of edge weights: w_e / sqrt(d_i d_j) for edge e = (i <- j), where d is the
+    weighted in-degree (the sum of a row's weights).  Weights are >= 0; an edge whose d_i d_j is 0 gets 0.  Computed
+    once per graph in fp64 on the host and returned as fp32 in the CSR's edge order."""
+    t = np.asarray(row_end, dtype=np.int64)
+    deg = np.diff(np.concatenate([[0], t]))
+    dst = np.repeat(np.arange(t.shape[0]), deg)
+    w = np.asarray(w, dtype=np.float64)
+    assert w.shape[0] == t[-1] and (w >= 0).all(), "one weight >= 0 per edge"
+    d = np.bincount(dst, weights=w, minlength=t.shape[0])
+    dd = d[dst] * d[np.asarray(col, dtype=np.int64)]
+    out = np.zeros_like(w)
+    np.divide(w, np.sqrt(dd), out=out, where=dd > 0)
+    return out.astype(np.float32)

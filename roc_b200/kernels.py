@@ -133,9 +133,89 @@ class SgPlan:
               "roc_sg_attn_backward_planned")
         return in_grad, score_grad
 
+    def weighted_forward(self, x, w, out=None):
+        """Edge-weighted sum: out[r] = sum over row r's edges e of w[e - col_left] * x[col[e]]; w is a flat fp32 array in
+        the plan's edge order, x is indexed like forward's input."""
+        h = x.shape[1]
+        if out is None:
+            out = self._rows(x)
+        check(lib.roc_sg_weighted_forward_planned(self.handle, h, _ptr(x), _ld(x), _ptr(w), _ptr(out), _ld(out),
+                                                  _stream()), "roc_sg_weighted_forward_planned")
+        return out
+
+    def edge_dot(self, gy, x, dw=None, accumulate=False):
+        """Gradient of weighted_forward's weights: dw[e - col_left] (+)= gy[r] . x[col[e]] for every edge e of row r;
+        gy has the plan's rows, x is indexed like the forward's input."""
+        if dw is None:
+            dw = torch.empty(max(self.num_edges(), 1), device=gy.device)
+        check(lib.roc_sg_edge_dot_planned(self.handle, gy.shape[1], _ptr(gy), _ld(gy), _ptr(x), _ld(x), _ptr(dw),
+                                          int(bool(accumulate)), _stream()), "roc_sg_edge_dot_planned")
+        return dw
+
+    def num_edges(self):
+        return int(self.row_end[-1].item()) - self.col_left if self.nloc else 0
+
     def close(self):
         if self.handle:
             lib.roc_sg_plan_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class _DeviceArray:
+    """A borrowed device array, for torch.as_tensor through __cuda_array_interface__."""
+
+    def __init__(self, ptr, n, typestr):
+        self.__cuda_array_interface__ = {"shape": (n,), "typestr": typestr, "data": (ptr or 0, False), "version": 2}
+
+
+class SgTranspose:
+    """roc_sg_transpose of a whole graph's CSR (row_end: N END offsets, col: E sources, every id < N): the exact input
+    gradient of the edge-weighted sum on any graph."""
+
+    def __init__(self, row_end, col):
+        _lib.require_device()
+        assert row_end.dtype in (torch.int64, torch.uint64) and col.dtype in (torch.int32, torch.uint32)
+        self.row_end, self.col = row_end, col
+        self.n = row_end.shape[0]
+        self.num_edges = int(row_end[-1].item()) if self.n else 0
+        h = C.c_void_p()
+        check(lib.roc_sg_transpose_create(self.n, _ptr(row_end), _ptr(col), _stream(), C.byref(h)),
+              "roc_sg_transpose_create")
+        self.handle = h
+
+    def backward(self, gy, w, out=None):
+        """in_grad[j] = sum over the edges e with col[e] = j of w[e] * gy[dst(e)]; gy and in_grad have N rows."""
+        h = gy.shape[1]
+        if out is None:
+            out = padded(self.n, h, gy.device) if _ld(gy) % 4 == 0 else torch.empty((self.n, h), device=gy.device)
+        check(lib.roc_sg_weighted_backward_planned(self.handle, h, _ptr(gy), _ld(gy), _ptr(w), _ptr(out), _ld(out),
+                                                   _stream()), "roc_sg_weighted_backward_planned")
+        return out
+
+    def info(self):
+        """Copies of the transposed CSR: {"row_end": int64 [N], "col": int32 [E], "perm": int32 [E]} (the uint32 /
+        uint64 bits in signed storage) on the device."""
+        re_, col, perm = C.c_void_p(), C.c_void_p(), C.c_void_p()
+        check(lib.roc_sg_transpose_info(self.handle, C.byref(re_), C.byref(col), C.byref(perm), None),
+              "roc_sg_transpose_info")
+        torch.cuda.current_stream().synchronize()
+
+        def copy(p, n, typestr):
+            if n == 0:
+                return torch.empty(0, dtype=torch.int64 if typestr == "<i8" else torch.int32, device="cuda")
+            return torch.as_tensor(_DeviceArray(p.value, n, typestr), device="cuda").clone()
+        return {"row_end": copy(re_, self.n, "<i8"), "col": copy(col, self.num_edges, "<i4"),
+                "perm": copy(perm, self.num_edges, "<i4")}
+
+    def close(self):
+        if self.handle:
+            lib.roc_sg_transpose_destroy(self.handle)
             self.handle = None
 
     def __del__(self):

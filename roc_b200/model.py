@@ -92,9 +92,22 @@ class Model:
     def indegree_norm(self, t):
         return lib.roc_host_indegree_norm(self.h, t)
 
-    def scatter_gather(self, t, aggr=_lib.AGGR_SUM):
+    def create_edge_tensor(self, hidden=1):
+        """One fp32 value per edge of this partition, in CSR order (Model::create_edge_tensor); hidden must be 1."""
+        return lib.roc_host_create_edge_tensor(self.h, int(hidden))
+
+    def set_edge_grad(self, edges, on=True):
+        """Compute the edge tensor's gradient in backward (off by default): the sum over the weighted scatter_gathers
+        that read it.  Call before init() when the weighted op's input has no gradient of its own."""
+        check(lib.roc_host_set_edge_grad(self.h, edges, int(bool(on))))
+
+    def scatter_gather(self, t, aggr=_lib.AGGR_SUM, weights=None):
         """aggr: AGGR_SUM (the reference's op), AGGR_AVG (sum -> indegree_norm -> indegree_norm), AGGR_MAX / AGGR_MIN
-        (per feature over the in-neighbours; one partition only)."""
+        (per feature over the in-neighbours; one partition only).  weights: an edge tensor (create_edge_tensor) for
+        the edge-weighted sum over each row's in-edges, whose backward is exact on any graph (one partition only)."""
+        if weights is not None:
+            assert aggr == _lib.AGGR_SUM, "edge weights go with the sum"
+            return lib.roc_host_scatter_gather_weighted(self.h, t, weights)
         if aggr == _lib.AGGR_SUM:
             return lib.roc_host_scatter_gather(self.h, t)
         return lib.roc_host_scatter_gather_aggr(self.h, t, int(aggr))
@@ -372,3 +385,33 @@ def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01,
     model.init()
     return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs, "attn": attn,
             "attn_ins": attn_ins, "scores": scores}
+
+
+def build_gcn_weighted(model, layers, dropout_rate, edge_weights, edge_grad=False, lr=0.01, weight_decay=0.05):
+    """GCN with edge weights (e.g. datasets.gcn_edge_weights, which folds in the symmetric normalisation).  Per layer
+
+        t = relu(scatter_gather(linear(dropout(t), layers[i]), weights=e))     # no relu on the last layer
+
+    with one edge tensor e shared by every layer.  edge_weights: one fp32 value per edge in CSR order, loaded after
+    init().  edge_grad: compute e's gradient in backward (the sum of the layers' contributions).  Single partition.
+    Returns the handles, with `edges` and the aggregations' inputs `sg_ins` and outputs `sg_outs`."""
+    L = len(layers)
+    x = model.create_node_tensor(layers[0])
+    label = model.create_node_tensor(layers[-1])
+    mask = model.create_node_tensor(1, is_int=True)
+    e = model.create_edge_tensor(1)
+    t = x
+    sg_ins, sg_outs = [], []
+    for i in range(1, L):
+        t = model.linear(model.dropout(t, dropout_rate), layers[i], _lib.AC_MODE_NONE)
+        sg_ins.append(t)
+        t = model.scatter_gather(t, weights=e)
+        sg_outs.append(t)
+        if i != L - 1:
+            t = model.relu(t)
+    model.softmax_cross_entropy(t, label, mask)
+    model.adam(lr, weight_decay)
+    model.set_edge_grad(e, edge_grad)
+    model.init()
+    model.set_tensor(e, np.asarray(edge_weights, dtype=np.float32))
+    return {"input": x, "label": label, "mask": mask, "logits": t, "edges": e, "sg_ins": sg_ins, "sg_outs": sg_outs}

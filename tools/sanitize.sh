@@ -4,7 +4,8 @@
 #   (b) the ScatterGather sum with the fused epilogue on a small R-MAT graph at 41, 64, 100, 200 and 602 floats, each
 #       followed by one max-aggregation forward and backward; then the attention forward and backward at 41 and 64
 #       floats with one head and at 64 and 256 floats with eight, on float4 rows, and at 256 floats with two heads on
-#       rows of 257 floats (the scalar path);
+#       rows of 257 floats (the scalar path); then the edge-weighted forward, its transposed backward and the edge
+#       dot (overwriting, then accumulating) at 41, 64, 200 and 602 floats;
 #   (c) the warp-specialised dW kernel at 602 x 64 with the dropout mask and at 64 x 41, on rows that wrap its ring
 #       and end in a partial block.
 # Usage: tools/sanitize.sh [logdir]   (needs a GPU; `make sanitize`)
@@ -39,6 +40,16 @@ out = torch.zeros((n, 257), device="cuda")[:, :256]
 out, stats = plan.attn_forward(xs, sc, 2, out=out)
 plan.attn_backward(xs, sc, out, stats, xs, 2, in_grad=torch.zeros((n, 257), device="cuda")[:, :256])
 torch.cuda.synchronize()
+tr = K.SgTranspose(re.cuda(), col.cuda())
+w = torch.rand(col.shape[0], device="cuda")
+for h in (41, 64, 200, 602):
+    x = K.padded(n, h, "cuda", fill=torch.rand((n, h), device="cuda"))
+    y = plan.weighted_forward(x, w)
+    tr.backward(y, w)
+    dw = plan.edge_dot(y, x)
+    plan.edge_dot(y, x, dw=dw, accumulate=True)
+    torch.cuda.synchronize()
+tr.close()
 print("sg ok")
 PY
 cat > "$LOG/dw.py" <<'PY'

@@ -241,6 +241,40 @@ void roc_sg_transpose_destroy(roc_sg_transpose* transpose);
 int roc_sg_weighted_backward_planned(roc_sg_transpose* transpose, int H, const float* outGrad, int64_t ldG,
                                      const float* w, float* inGrad, int64_t ldIn, roc_stream_t stream);
 
+/* Exact backwards of the sum, max / min and attention aggregations on any whole graph (directed, with duplicate edges
+ * or nodes without in- or out-edges), over the transpose.  The gathers over the same CSR above (quirk Q1) stay the
+ * default; these are the opt-in alternative (Model::set_exact_backward).  dst(e) is the row that owns edge e, and
+ * transposed row j lists j's out-edges in the transpose's stable order.  outGrad, arg, inGrad and every per-node input
+ * have numNodes rows.  On a symmetric graph whose rows have strictly increasing sources the transposed CSR is the CSR,
+ * and each call returns exactly the bits of its counterpart named below.  They take the same row shapes and column
+ * blocks as those, run in the plan's fixed order with no atomics (the same call gives the same bits), and report their
+ * launches through roc_sg_last_call_info.  ROC_ERR_INVALID: a NULL pointer or a leading dimension < H.
+ *
+ * Sum (counterpart roc_sg_forward_planned with the same epilogue):
+ *   inGrad[j][h] = epi( sum_{e : colSrc[e] = j} outGrad[dst(e)][h] )
+ * NORM divides by sqrtf of j's IN-degree in the original graph, read from its rowEnd (required with NORM, else
+ * ROC_ERR_INVALID), in the form that gives roc_indegree_norm's bits; RELU as in the forward. */
+int roc_sg_transpose_sum_backward(roc_sg_transpose* transpose, int H, const float* outGrad, int64_t ldG, float* inGrad,
+                                  int64_t ldIn, int epilogue, const roc_eid_t* rowEnd, roc_stream_t stream);
+/* Max / min (counterpart roc_sg_minmax_backward_planned with selfBase 0), for arg from roc_sg_minmax_forward_planned:
+ *   inGrad[j][h] = sum over the DISTINCT destinations i of j's out-edges of (arg[i][h] == j ? outGrad[i][h] : 0)
+ * A duplicate edge j -> i lies next to its twin in transposed row j; an entry whose destination equals the previous
+ * entry's in the same row adds nothing, so the result is the true adjoint on multigraphs too. */
+int roc_sg_transpose_minmax_backward(roc_sg_transpose* transpose, int H, const float* outGrad, int64_t ldG,
+                                     const roc_vid_t* arg, int64_t ldArg, float* inGrad, int64_t ldIn,
+                                     roc_stream_t stream);
+/* Attention (counterpart roc_sg_attn_backward_planned with selfBase 0), `plan` the whole graph's forward plan:
+ *   scoreGrad[i][k]       = sum_{e : dst(e) = i, j = colSrc[e]} dz(i<-j,k)              (d s_dst, over `plan`)
+ *   scoreGrad[j][heads+k] = sum_{e : colSrc[e] = j, i = dst(e)} dz(i<-j,k)              (d s_src)
+ *   inGrad[j][kF+f]       = sum_{e : colSrc[e] = j, i = dst(e)} a(i<-j,k) G[i][kF+f]
+ * with a, dz and the per-node record as in roc_sg_attn_backward_planned; a duplicate edge counts once per edge, as in
+ * the forward.  The records cover ids [0, numNodes): no id scan, no synchronisation.  Head layouts and widths are
+ * refused exactly as there; ROC_ERR_INVALID also when `plan` does not have the transpose's rows and edges. */
+int roc_sg_attn_backward_exact(const roc_sg_plan* plan, roc_sg_transpose* transpose, int heads, int H, float slope,
+                               const float* in, int64_t ldIn, const float* score, int64_t ldS, const float* out,
+                               int64_t ldOut, const float* stats, int64_t ldStats, const float* outGrad, int64_t ldG,
+                               float* inGrad, int64_t ldInG, float* scoreGrad, int64_t ldSG, roc_stream_t stream);
+
 /* Plan-less form with exactly the reference kernel's argument list
  * (scattergather_kernel.cu:21-28, EdgeStruct.dst dropped), dense ld == H.
  * Builds and frees a plan internally (synchronises); use the planned form in
@@ -264,8 +298,10 @@ int roc_sg_backward(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft, in
  *          weighted backward's weight permutation (first in its list)
  *   red    the reduction the kernel is instantiated for: 0 sum, 1 max, 2 min, 3 the min / max backward, 4 attention
  *          stats, 5 the attention forward, 6 its d s_dst gather, 7 its input-gradient gather, 8 the weighted sum
- *          (forward and backward), 9 the edge-weight gradient; -1 for the record and the permutation, which have
- *          none.  A sum fix-up finishing another reduction's partials reports 0.
+ *          (forward and backward), 9 the edge-weight gradient, 10 the exact sum backward with NORM (the sum whose
+ *          epilogue divides by the original graph's in-degree; its main kernel, ring and fix-ups), 11 the exact max /
+ *          min backward; -1 for the record and the permutation, which have none.  A sum fix-up finishing another
+ *          reduction's partials reports 0.
  *   vec    4 for float4 rows, else 1;  lanes, nch: the row shape (L lanes, chunks per lane);  grid: CTAs launched
  * count is the number of launches; the first ROC_SG_MAX_LAUNCHES are stored.  Every planned call clears the list first,
  * also one that fails before it launches anything.  ROC_ERR_INVALID for a NULL info. */

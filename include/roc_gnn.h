@@ -236,6 +236,12 @@ public:
   void set_labels(const Tensor& label, const int* host_class_idx);
   roc_perf_metrics last_metrics(void) const;   /* PerfMetrics of the latest softmax pass */
   void set_fusion(bool on) { fuse = on; }
+  /* Opt-in exact backward (off by default) for the sum (and so AGGR_AVG), max / min and attention aggregations on
+   * directed graphs: their input gradients run over the graph's transpose (roc_sg_transpose_sum_backward,
+   * roc_sg_transpose_minmax_backward, roc_sg_attn_backward_exact) instead of the same CSR (quirk Q1, the true gradient
+   * only on a symmetric graph).  init() then builds the transpose once, shared with the weighted ops, and max / min
+   * accept graphs with duplicate edges.  Call it before init().  Single partition only (exit(1) otherwise). */
+  void set_exact_backward(bool on);
   /* the source ids a max / min scatter_gather chose (its `arg`), [rows_local][H] u32; `out` is its output tensor */
   void get_aggr_index(const Tensor& out, uint32_t* host) const;
   int64_t local_rows(void) const { return (int64_t)myGraph.rowRight - myGraph.rowLeft + 1; }
@@ -251,6 +257,7 @@ public:
   int epoch_num;
   bool fuse;          /* fuse linear->norm and SG->norm->relu into kernel epilogues (default on) */
   bool printMetrics;  /* print the [INFER] accuracy line like softmax_kernel.cu:141-152 (default on) */
+  bool exactBackward; /* set_exact_backward (default off) */
 };
 
 class GnnOp {  /* gnn.h:205-222 */

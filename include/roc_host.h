@@ -60,6 +60,8 @@ int roc_host_set_lr(roc_host* h, double lr);
 double roc_host_get_lr(roc_host* h);
 void roc_host_srand(unsigned seed);               /* std::srand(config.seed), gnn.cc:56 */
 int roc_host_set_fusion(roc_host* h, int on);
+/* Model::set_exact_backward(on); before roc_host_init */
+int roc_host_set_exact_backward(roc_host* h, int on);
 int roc_host_init(roc_host* h);
 
 /* data: dense host buffers of this partition's rows ([rows][hidden]) */

@@ -115,6 +115,10 @@ PROTOTYPES = {
     "roc_sg_transpose_info": (i32, [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]),
     "roc_sg_transpose_destroy": (None, [vp]),
     "roc_sg_weighted_backward_planned": (i32, [vp, i32, vp, i64, vp, vp, i64, vp]),
+    "roc_sg_transpose_sum_backward": (i32, [vp, i32, vp, i64, vp, i64, i32, vp, vp]),
+    "roc_sg_transpose_minmax_backward": (i32, [vp, i32, vp, i64, vp, i64, vp, i64, vp]),
+    "roc_sg_attn_backward_exact": (i32, [vp, vp, i32, i32, f32, vp, i64, vp, i64, vp, i64, vp, i64, vp, i64, vp, i64,
+                                         vp, i64, vp]),
     "roc_sg_forward": (i32, [u32, u32, u64, i32, vp, vp, vp, vp, vp]),
     "roc_sg_backward": (i32, [u32, u32, u64, i32, vp, vp, vp, vp, vp]),
     "roc_sg_last_call_info": (i32, [C.POINTER(SgCallInfo)]),
@@ -184,6 +188,7 @@ PROTOTYPES = {
     "roc_host_get_lr": (f64, [vp]),
     "roc_host_srand": (None, [C.c_uint]),
     "roc_host_set_fusion": (i32, [vp, i32]),
+    "roc_host_set_exact_backward": (i32, [vp, i32]),
     "roc_host_init": (i32, [vp]),
     "roc_host_load_features": (i32, [vp, i32, C.c_char_p]),
     "roc_host_load_labels": (i32, [vp, i32, C.c_char_p]),

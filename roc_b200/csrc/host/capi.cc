@@ -118,6 +118,7 @@ int roc_host_set_lr(roc_host* h, double lr) { if (!h->adam) return -1; h->adam->
 double roc_host_get_lr(roc_host* h) { return h->adam ? h->adam->alpha : 0.0; }
 void roc_host_srand(unsigned seed) { std::srand(seed); }
 int roc_host_set_fusion(roc_host* h, int on) { h->m().set_fusion(on != 0); return 0; }
+int roc_host_set_exact_backward(roc_host* h, int on) { h->m().set_exact_backward(on != 0); return 0; }
 int roc_host_init(roc_host* h) { return h->m().init(h->config) ? 0 : -1; }
 
 int roc_host_load_features(roc_host* h, int t, const char* prefix) { h->m().load_features(h->at(t), prefix); return 0; }

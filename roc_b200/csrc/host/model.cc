@@ -36,7 +36,7 @@ GnnOp::GnnOp(const Tensor& _input1, const Tensor& _input2, const Tensor& _input3
 // ------------------------------------------------------------------ Model ---
 Model::Model(const Graph& _graph, Context _ctx, Runtime* _runtime)
     : mode(MD_MODE_TRAIN), myGraph(_graph), ctx(_ctx), runtime(_runtime), optimizer(NULL), epoch_num(0),
-      fuse(true), printMetrics(true) {}
+      fuse(true), printMetrics(true), exactBackward(false) {}
 
 // gnn.cc:475-532: node tensor = [numNodes][H]; this process holds its vertex range.
 template <>
@@ -138,6 +138,12 @@ Tensor Model::scatter_gather(const Tensor& input, const Tensor& edgeWeights) {
 void Model::set_edge_grad(const Tensor& edges, bool on) {
   if (edges.type != Tensor::EDGE_TENSOR) ROC_FATAL("set_edge_grad: not an edge tensor");
   ctx->t(edges.region).requiresGrad = on;
+}
+void Model::set_exact_backward(bool on) {
+  if (on && ctx->numParts > 1)
+    ROC_FATAL("set_exact_backward: the exact backward runs on one partition only (numParts > 1 is not supported)");
+  if (ctx->flatGrad) ROC_FATAL("set_exact_backward: call it before init()");
+  exactBackward = on;
 }
 void Model::get_aggr_index(const Tensor& out, uint32_t* host) const {
   for (GnnOp* op : layers) {
@@ -258,14 +264,30 @@ bool Model::init(const Config& config) {
   }
   rt->ensure_lin_ws(ws);
   // max / min aggregation sends each gradient to one source per (row, feature): a duplicate edge would receive it
-  // twice.  Strictly increasing sources per row rule duplicates out.
-  for (size_t l = 0; l < layers.size(); l++) {
+  // twice.  Strictly increasing sources per row rule duplicates out.  The exact backward takes each distinct edge once
+  // and needs no such rule.
+  for (size_t l = 0; l < layers.size() && !exactBackward; l++) {
     ScatterGather* sg = as<ScatterGather>(layers[l]);
     if (!sg || (sg->aggr != AGGR_MAX && sg->aggr != AGGR_MIN)) continue;
     int sorted = 0;
     ROC_CHECK(roc_sg_plan_rows_sorted(myGraph.plan, &sorted, rt->stream));
     if (!sorted) ROC_FATAL("scatter_gather(max / min): every row's sources must be strictly increasing (no duplicate edges)");
     break;
+  }
+  // the exact backward's transpose, built once and shared with the weighted ops, its plan's carries reserved for the
+  // widest aggregation it serves, as the forward plan's are
+  if (exactBackward) {
+    int maxT = 0;
+    for (size_t l = 0; l < layers.size(); l++)
+      if (as<ScatterGather>(layers[l]) || as<AttentionGather>(layers[l]))
+        maxT = std::max(maxT, (int)layers[l]->inputs[0].dims[0]);
+    if (maxT > 0) {
+      if (!rt->sgTranspose)
+        ROC_CHECK(roc_sg_transpose_create(myGraph.numNodes, myGraph.d_rowEnd, myGraph.d_colSrc, rt->stream, &rt->sgTranspose));
+      const roc_sg_plan* planT = nullptr;
+      ROC_CHECK(roc_sg_transpose_info(rt->sgTranspose, nullptr, nullptr, nullptr, &planT));
+      ROC_CHECK(roc_sg_plan_reserve(const_cast<roc_sg_plan*>(planT), maxT));
+    }
   }
   if (maxSg > 0) {
     ROC_CHECK(roc_sg_plan_reserve(myGraph.plan, maxSg));
@@ -777,22 +799,32 @@ void ScatterGather::backward(const Model& model) {
   const int H = (int)inputs[0].dims[0];
   const int64_t ld = rt->t(outputs[0].region).ld;
   if (aggr == AGGR_MAX || aggr == AGGR_MIN) {
-    // each output gradient goes to the source its forward chose; a gather over the same CSR (no atomics)
+    // each output gradient goes to the source its forward chose; a gather over the same CSR (no atomics), or over the
+    // transpose with the exact backward
     const int src = inputs[0].region;
     rt->sg_begin(H);
-    ROC_CHECK(roc_sg_minmax_backward_planned(model.myGraph.plan, H, model.myGraph.rowLeft, rt->grad(outputs[0].region),
-                                             ld, arg, argLd, rt->grad(src), rt->t(src).ld, rt->stream));
+    if (model.exactBackward)
+      ROC_CHECK(roc_sg_transpose_minmax_backward(rt->sgTranspose, H, rt->grad(outputs[0].region), ld, arg, argLd,
+                                                 rt->grad(src), rt->t(src).ld, rt->stream));
+    else
+      ROC_CHECK(roc_sg_minmax_backward_planned(model.myGraph.plan, H, model.myGraph.rowLeft, rt->grad(outputs[0].region),
+                                               ld, arg, argLd, rt->grad(src), rt->t(src).ld, rt->stream));
     rt->sg_end();
     return;
   }
   const int dstRegion = bwdOut >= 0 ? bwdOut : inputs[0].region;
-  // Forward and backward do exactly the same thing, on gradients (scattergather_kernel.cu:168-169)
+  // Forward and backward do exactly the same thing, on gradients (scattergather_kernel.cu:168-169); the exact backward
+  // sums over the transpose instead, its fused NORM dividing by the in-degree of the graph's rowEnd
   rt->sg_begin(-H);
   const float* src = gathered(model, rt->grad(outputs[0].region), ld, H, &rt->t(outputs[0].region), true);
   rt->sg_end();
   float* dst = rt->grad(dstRegion);
   rt->sg_begin(H);
-  ROC_CHECK(roc_sg_forward_planned(model.myGraph.plan, H, src, ld, dst, rt->t(dstRegion).ld, bwdEpilogue, rt->stream));
+  if (model.exactBackward)
+    ROC_CHECK(roc_sg_transpose_sum_backward(rt->sgTranspose, H, src, ld, dst, rt->t(dstRegion).ld, bwdEpilogue,
+                                            model.myGraph.d_rowEnd, rt->stream));
+  else
+    ROC_CHECK(roc_sg_forward_planned(model.myGraph.plan, H, src, ld, dst, rt->t(dstRegion).ld, bwdEpilogue, rt->stream));
   rt->sg_end();
 }
 
@@ -849,11 +881,18 @@ void AttentionGather::backward(const Model& model) {
   }
   const int ox = outputs[0].region;
   rt->sg_begin(H);
-  ROC_CHECK(roc_sg_attn_backward_planned(model.myGraph.plan, heads, H, slope, model.myGraph.rowLeft,
+  if (model.exactBackward)
+    ROC_CHECK(roc_sg_attn_backward_exact(model.myGraph.plan, rt->sgTranspose, heads, H, slope,
                                          rt->data(inputs[0].region), rt->t(inputs[0].region).ld,
                                          rt->data(inputs[1].region), rt->t(inputs[1].region).ld, rt->data(ox),
                                          rt->t(ox).ld, stats, statsLd, rt->grad(ox), rt->t(ox).ld, dst[0],
                                          rt->t(inputs[0].region).ld, dst[1], rt->t(inputs[1].region).ld, rt->stream));
+  else
+    ROC_CHECK(roc_sg_attn_backward_planned(model.myGraph.plan, heads, H, slope, model.myGraph.rowLeft,
+                                           rt->data(inputs[0].region), rt->t(inputs[0].region).ld,
+                                           rt->data(inputs[1].region), rt->t(inputs[1].region).ld, rt->data(ox),
+                                           rt->t(ox).ld, stats, statsLd, rt->grad(ox), rt->t(ox).ld, dst[0],
+                                           rt->t(inputs[0].region).ld, dst[1], rt->t(inputs[1].region).ld, rt->stream));
   rt->sg_end();
   for (int i = 0; i < 2; i++) {
     const TensorImpl& x = rt->t(inputs[i].region);

@@ -34,6 +34,10 @@
 //  * edge-weighted aggregation (roc_sg_weighted_*, roc_sg_edge_dot_planned) is two more: WSUM, a sum with one FMA by
 //    each edge's weight, finished by the sum's fix-ups; EDOT, one dot product G[i] . X[j] per edge, which carries
 //    nothing.  The exact backward runs WSUM over a transposed CSR (roc_sg_transpose) with the weights permuted.
+//  * the exact backwards of the other aggregations run over the same transpose (roc_sg_transpose_*_backward,
+//    roc_sg_attn_backward_exact): TSUM is the sum whose NORM epilogue divides by the original graph's in-degree,
+//    TMASK the min / max backward that skips a repeated destination (a duplicate edge), and the attention input
+//    gradient is the ASRC gather itself, run over the transposed plan.
 //
 // Algorithmic bytes per launch (DESIGN.md): E*(4H+4) + Nloc*(4H+8); min / max forward E*(4H+4) + Nloc*(8H+8),
 // backward E*(8H+4) + Nloc*(4H+8); weighted forward E*(4H+8) + Nloc*(4H+8), edge dot E*(4H+8) + Nloc*4H; attention
@@ -225,8 +229,12 @@ template <> struct V<1> {
 // destination-score gradient (heads wide), ASRC the input gradient and the source-score gradient.
 // The edge-weighted passes (roc_sg_weighted_*, roc_sg_edge_dot_planned): WSUM the w-weighted sum, EDOT the per-edge
 // dot product G[i] . X[j] (the gradient of the edge weights).
+// The exact backwards over a transposed plan (roc_sg_transpose_*_backward): TSUM is the sum whose NORM epilogue
+// divides by the in-degree of the original graph (its row ends in p.xrow) instead of the plan's row length; TMASK is
+// MASK where an entry whose destination repeats the previous entry's in the same row (a duplicate edge) adds nothing.
 enum { SG_RED_SUM = 0, SG_RED_MAX = ROC_SG_AGGR_MAX, SG_RED_MIN = ROC_SG_AGGR_MIN, SG_RED_MASK = 3,
-       SG_RED_ASTAT = 4, SG_RED_ATTN = 5, SG_RED_ADST = 6, SG_RED_ASRC = 7, SG_RED_WSUM = 8, SG_RED_EDOT = 9 };
+       SG_RED_ASTAT = 4, SG_RED_ATTN = 5, SG_RED_ADST = 6, SG_RED_ASRC = 7, SG_RED_WSUM = 8, SG_RED_EDOT = 9,
+       SG_RED_TSUM = 10, SG_RED_TMASK = 11 };
 constexpr uint32_t SG_NOARG = 0xFFFFFFFFu;   // index of a row that has no edge yet
 
 // The ordering rule: the candidate v replaces the current a iff it is strictly greater (smaller) or it is NaN and a
@@ -343,7 +351,7 @@ struct SgParams {
   const float* stats;   // ATTN: [nloc][ldStats] m | 1/Z of the local rows
   const float4* rec;    // ADST / ASRC: [*][heads] {s_dst, m, 1/Z, D}, indexed like `in`
   const void* xrow;     // ADST, EDOT: G, ASRC: X, the local row's own row (units of T, ldX); EDOT: indexed by plan
-                        // row, else like `in`
+                        // row, else like `in`.  TSUM: the original graph's rowEnd (u64), for in_degree
   float* out2;          // ASTAT: unused; ADST / ASRC: heads-wide output [nloc][ldOut2];  EDOT: [E] dw of each local edge
   float* carry2;        // [numCarries][SG_LDC2] heads-wide partials (ASTAT: m | Z)
   size_t ldS, ldStats, ldX, ldOut2;
@@ -383,6 +391,18 @@ __device__ __forceinline__ void epi_store(typename V<VEC>::T v, typename V<VEC>:
   V<VEC>::st(dst, v);
 }
 
+// TSUM: the in-degree of node r in the original whole graph, from its row ends (what roc_indegree_norm divides by).
+__device__ __forceinline__ uint32_t in_degree(const SgParams& p, uint32_t r) {
+  const uint64_t* re = static_cast<const uint64_t*>(p.xrow);
+  return (uint32_t)(__ldg(re + r) - (r ? __ldg(re + r - 1) : 0ull));
+}
+// What the NORM epilogue of plan row r, of `len` edges, divides by the square root of.
+template <int RED>
+__device__ __forceinline__ uint32_t norm_deg(const SgParams& p, uint32_t r, uint32_t len) {
+  if constexpr (RED == SG_RED_TSUM) return in_degree(p, r);
+  else return len;
+}
+
 // ------------------------------------------------------------- main kernel ---
 // One worker (L lanes) per chunk.  Lane `lane` owns T-columns lane + ch*L.
 // RED (SG_RED_*) changes only what is done with a gathered row and what the row store writes; the schedule, the
@@ -398,6 +418,7 @@ sg_chunk_kernel(const SgParams p) {
   constexpr bool XI = RED == SG_RED_ADST || RED == SG_RED_ASRC;  // holds a row of its own row i, and heads-wide sums
   constexpr bool WS = RED == SG_RED_WSUM;                        // loads each edge's weight beside its source id
   constexpr bool ED = RED == SG_RED_EDOT;                        // holds G[i], stores one dot product per edge
+  constexpr bool MK = RED == SG_RED_MASK || RED == SG_RED_TMASK; // gathers an index row beside each gradient row
   constexpr int WPB = SG_THREADS / L;
   constexpr uint32_t CH = SG_CH;
   const int lane = threadIdx.x % L;
@@ -542,7 +563,7 @@ sg_chunk_kernel(const SgParams p) {
 #pragma unroll
     for (int ch = 0; ch < NCH; ch++) {
       if (act[ch]) {
-        if (epi) epi_store<VEC>(acc[ch], dst + ch * L, curT - curS, epi);
+        if (epi) epi_store<VEC>(acc[ch], dst + ch * L, norm_deg<RED>(p, cur, curT - curS), epi);
         else V<VEC>::st(dst + ch * L, acc[ch]);
       }
       acc[ch] = V<VEC>::zero();
@@ -571,9 +592,9 @@ sg_chunk_kernel(const SgParams p) {
     inl[ch] = reinterpret_cast<const char*>(in + min((uint32_t)(lane + ch * L), p.Q - 1u));
   const uint32_t rowBytes = (uint32_t)p.ldIn * (uint32_t)sizeof(T);
   // MASK: the index row of each edge's source is gathered next to its gradient row
-  const char* argl[RED == SG_RED_MASK ? NCH : 1];
+  const char* argl[MK ? NCH : 1];
   uint32_t argRowBytes = 0;
-  if constexpr (RED == SG_RED_MASK) {
+  if constexpr (MK) {
 #pragma unroll
     for (int ch = 0; ch < NCH; ch++)
       argl[ch] = reinterpret_cast<const char*>(reinterpret_cast<const I*>(p.arg) + min((uint32_t)(lane + ch * L), p.Q - 1u));
@@ -601,8 +622,20 @@ sg_chunk_kernel(const SgParams p) {
         for (int u = 0; u < U; u++) wv[u] = __ldg(p.score + min(base + (uint32_t)u, eLast));
       }
     }
+    // TMASK: bit u is set when edge base + u has the destination of the edge before it (for u = 0 the edge before the
+    // group, which may lie in an earlier chunk of the same row); whether that edge is in the same row is checked when
+    // the edge is added
+    [[maybe_unused]] uint32_t repeat = 0;
+    if constexpr (RED == SG_RED_TMASK) {
+      uint32_t prev = __ldg(col + (base ? base - 1u : 0u));
+#pragma unroll
+      for (int u = 0; u < U; u++) {
+        repeat |= (srcs[u] == prev ? 1u : 0u) << u;
+        prev = srcs[u];
+      }
+    }
     T v[U][NCH];
-    I av[RED == SG_RED_MASK ? U : 1][RED == SG_RED_MASK ? NCH : 1];
+    I av[MK ? U : 1][MK ? NCH : 1];
     float sv[SV ? U : 1][SV ? NCH : 1];                              // ATTN / ADST: s_src[j] of each chunk's head
     float4 rv[RED == SG_RED_ASRC ? U : 1][RED == SG_RED_ASRC ? NCH : 1];   // ASRC: the record of j
 #pragma unroll
@@ -610,7 +643,7 @@ sg_chunk_kernel(const SgParams p) {
       const uint64_t off = (uint64_t)srcs[u] * rowBytes;
 #pragma unroll
       for (int ch = 0; ch < NCH; ch++) v[u][ch] = V<VEC>::ld(reinterpret_cast<const T*>(inl[ch] + off));
-      if constexpr (RED == SG_RED_MASK) {
+      if constexpr (MK) {
         const uint64_t aoff = (uint64_t)srcs[u] * argRowBytes;
 #pragma unroll
         for (int ch = 0; ch < NCH; ch++) av[u][ch] = __ldg(reinterpret_cast<const I*>(argl[ch] + aoff));
@@ -688,10 +721,17 @@ sg_chunk_kernel(const SgParams p) {
                 float* q = p.out2 + base + (uint32_t)u;
                 *q = p.dwAdd ? *q + d[0] : d[0];
               }
+            } else if constexpr (RED == SG_RED_TMASK) {
+              // a duplicate edge j -> i sits right after its twin in transposed row j (the sort is stable): only the
+              // first of them adds, so each distinct destination's gradient is taken once
+              if (base + (uint32_t)u == curS || !((repeat >> u) & 1u)) {
+#pragma unroll
+                for (int ch = 0; ch < NCH; ch++) mask_add(acc[ch], v[u][ch], av[u][ch], p.selfBase + cur);
+              }
             } else {
 #pragma unroll
               for (int ch = 0; ch < NCH; ch++) {
-                if constexpr (RED == SG_RED_SUM) V<VEC>::add(acc[ch], v[u][ch]);
+                if constexpr (RED == SG_RED_SUM || RED == SG_RED_TSUM) V<VEC>::add(acc[ch], v[u][ch]);
                 else if constexpr (RED == SG_RED_MASK) mask_add(acc[ch], v[u][ch], av[u][ch], p.selfBase + cur);
                 else mm_add<RED>(acc[ch], aidx[ch], v[u][ch], srcs[u]);
               }
@@ -720,7 +760,7 @@ sg_chunk_kernel(const SgParams p) {
 // bytes in flight are well under half of its peak; the ring is refilled stage by stage, so it
 // stays full.  (2) the copies are issued by one lane instead of an index load + IMAD.WIDE +
 // LDG.128 per lane group.  MODE 0 (T) loads the source ids of a stage when it issues it; MODE 2 (U) holds them in
-// the lanes that issue them.
+// the lanes that issue them.  MODE bit 4 makes it TSUM (the NORM epilogue divides by in_degree).
 // A row slot is L*NCH*16 bytes (the worker's whole lane span), so the shared-memory row pitch is a
 // compile-time constant and the adds are unpredicated; lanes past the row's end add stale slot
 // contents they never store.
@@ -836,7 +876,8 @@ sg_chunk_kernel_t(const SgParams p) {
 #pragma unroll
     for (int ch = 0; ch < NCH; ch++) {
       if (act[ch]) {
-        if (epi) epi_store<4>(acc[ch], dst + ch * L, curT - curS, epi);
+        if (epi)
+          epi_store<4>(acc[ch], dst + ch * L, norm_deg<(MODE & 4) ? SG_RED_TSUM : SG_RED_SUM>(p, cur, curT - curS), epi);
         else *(dst + ch * L) = acc[ch];
       }
       acc[ch] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -858,9 +899,9 @@ sg_chunk_kernel_t(const SgParams p) {
   // ids of units j, j + L, ... of the worker's edge range (a worker has at most 127 edges = 32 units) and
   // issues those units itself when their ring slot frees (on MODE 0 the id load of the stage about to be issued
   // is a large share of the stalls).
-  constexpr int NU = (MODE == 2) ? (32 / L) : 1;
+  constexpr int NU = (MODE & 2) ? (32 / L) : 1;
   uint4 ids[NU];
-  if (MODE == 2 && nE) {
+  if ((MODE & 2) && nE) {
 #pragma unroll
     for (int n = 0; n < NU; n++) {
       const uint32_t e4 = 4u * ((uint32_t)lane + (uint32_t)n * L);
@@ -871,7 +912,7 @@ sg_chunk_kernel_t(const SgParams p) {
     }
   }
   auto issue = [&](uint32_t k, uint32_t slot) {
-    if (MODE == 2) {
+    if (MODE & 2) {
       if (k < nStages) {
         const uint32_t off = k * G;
         const uint32_t bar = bars + slot * 8;
@@ -971,7 +1012,7 @@ sg_chunk_kernel_t(const SgParams p) {
 // U carries are loaded per batch.  The carries are taken in chunk order whatever U is, so U never changes a result;
 // MAX / MIN take fewer per batch where their index carries would otherwise spill.
 __host__ __device__ constexpr int sg_fixup_u(int L, int NCH, int RED) {
-  return RED == SG_RED_SUM ? (NCH == 1 ? (L == 4 ? 4 : 8) : 8 / NCH) : (NCH <= 2 ? 4 : 1);
+  return (RED == SG_RED_SUM || RED == SG_RED_TSUM) ? (NCH == 1 ? (L == 4 ? 4 : 8) : 8 / NCH) : (NCH <= 2 ? 4 : 1);
 }
 
 // One worker per heavy row.
@@ -980,7 +1021,7 @@ __global__ void __launch_bounds__(SG_THREADS)
 sg_fixup_kernel(const SgParams p) {
   typedef typename V<VEC>::T T;
   typedef typename V<VEC>::I I;
-  constexpr bool MM = RED != SG_RED_SUM;
+  constexpr bool MM = RED == SG_RED_MAX || RED == SG_RED_MIN;
   constexpr int U = sg_fixup_u(L, NCH, RED);
   constexpr int WPB = SG_THREADS / L;
   constexpr uint32_t CH = SG_CH;
@@ -1034,7 +1075,7 @@ sg_fixup_kernel(const SgParams p) {
   for (int ch = 0; ch < NCH; ch++) {
     if (act[ch]) {
       if constexpr (MM) { V<VEC>::st(dst + lane + ch * L, acc[ch]); adst[lane + ch * L] = ai[ch]; }
-      else epi_store<VEC>(acc[ch], dst + lane + ch * L, t - s, p.epi);
+      else epi_store<VEC>(acc[ch], dst + lane + ch * L, norm_deg<RED>(p, R, t - s), p.epi);
     }
   }
 }
@@ -1050,7 +1091,7 @@ __global__ void __launch_bounds__(SG_THREADS)
 sg_fixup_big_kernel(const SgParams p) {
   typedef typename V<VEC>::T T;
   typedef typename V<VEC>::I I;
-  constexpr bool MM = RED != SG_RED_SUM;
+  constexpr bool MM = RED == SG_RED_MAX || RED == SG_RED_MIN;
   constexpr int U = sg_fixup_u(L, NCH, RED);
   constexpr int WPB = SG_THREADS / L;
   constexpr uint32_t CH = SG_CH;
@@ -1121,7 +1162,7 @@ sg_fixup_big_kernel(const SgParams p) {
         adst[lane + ch * L] = ia;
       } else {
         for (int gg = 0; gg < WPB; gg++) V<VEC>::add(a, sp[(gg * NCH + ch) * L + lane]);
-        epi_store<VEC>(a, dst + lane + ch * L, t - s, p.epi);
+        epi_store<VEC>(a, dst + lane + ch * L, norm_deg<RED>(p, R, t - s), p.epi);
       }
     }
   }
@@ -1215,11 +1256,11 @@ static void note_launch(int kind, int red, int vec, int lanes, int nch, uint32_t
 
 // sg_chunk_kernel_t's two shapes, the measured defaults (DESIGN.md §3.1), four workers per CTA: rows of 65..128 floats
 // (one float4 per lane) with lane-held ids and two stages of two four-row units per worker; rows of 129..256 floats
-// with the ids loaded per stage and two stages of one unit.
-template <int NCH>
+// with the ids loaded per stage and two stages of one unit.  TS: the TSUM form.
+template <int NCH, bool TS>
 static int launch_ring(const SgParams& p, cudaStream_t st) {
   constexpr int L = 32, P = 2, NT = 128;
-  constexpr int S = NCH == 1 ? 2 : 1, MINB = NCH == 1 ? 4 : 6, MODE = NCH == 1 ? 2 : 0;
+  constexpr int S = NCH == 1 ? 2 : 1, MINB = NCH == 1 ? 4 : 6, MODE = (NCH == 1 ? 2 : 0) | (TS ? 4 : 0);
   constexpr int WPB = NT / L;
   constexpr size_t smem = (size_t)WPB * P * S * 4 * NCH * L * 16 + (size_t)WPB * P * 8;
   static std::atomic<uint64_t> configured{0};
@@ -1230,17 +1271,18 @@ static int launch_ring(const SgParams& p, cudaStream_t st) {
   const uint32_t grid = (p.numChunks + WPB - 1) / WPB;
   sg_chunk_kernel_t<L, NCH, S, P, NT, MINB, MODE><<<grid, NT, smem, st>>>(p);
   ROC_LAUNCH_CHECK();
-  note_launch(ROC_SG_LAUNCH_RING, SG_RED_SUM, 4, L, NCH, grid);
+  note_launch(ROC_SG_LAUNCH_RING, TS ? SG_RED_TSUM : SG_RED_SUM, 4, L, NCH, grid);
   return ROC_OK;
 }
 
 // The widest row, in T-columns, that one launch of RED takes: 256 (1024 floats vectorised, 256 scalar; wider rows are
-// split into column blocks), but 128 on float4 rows for every reduction except the sum and the weighted sum (min /
-// max: the big-row fix-up keeps values and indices of every lane group in static shared memory).  The weighted sum
-// takes the sum's column blocks, so that with all-ones weights it gives the sum's bits at every width (the big-row
-// fix-up groups a row's carries by the block's lane count).  ASTAT's row is one score per head.
+// split into column blocks), but 128 on float4 rows for every reduction except the sums (min / max: the big-row
+// fix-up keeps values and indices of every lane group in static shared memory).  The weighted sum and TSUM take the
+// sum's column blocks, so that with all-ones weights (on a symmetric graph) they give the sum's bits at every width
+// (the big-row fix-up groups a row's carries by the block's lane count).  ASTAT's row is one score per head.
 constexpr int sg_max_q(int VEC, int RED) {
-  return RED == SG_RED_ASTAT ? SG_LDC2 / 2 : (VEC == 4 && RED != SG_RED_SUM && RED != SG_RED_WSUM) ? 128 : 256;
+  return RED == SG_RED_ASTAT ? SG_LDC2 / 2
+         : (VEC == 4 && RED != SG_RED_SUM && RED != SG_RED_WSUM && RED != SG_RED_TSUM) ? 128 : 256;
 }
 
 // The row shape of every launch: calls f(L, NCH), as std::integral_constants, for rows of Q T-columns.  L is the
@@ -1262,7 +1304,9 @@ static int with_shape(uint32_t Q, F&& f) {
 // They are lower than the sum's where a second value held or gathered per float (the min / max index, the min / max
 // backward's index row, s_src, the record, the local row's own row) would otherwise spill under the occupancy.
 // WSUM keeps the sum's U and holds U weights beside them, so at one chunk per lane it runs three CTAs per SM.
-constexpr int SG_SHAPE_U[10][4] = {
+// TSUM and TMASK take the shapes of SUM and MASK, but TMASK, which also holds each group's repeated-destination bits,
+// runs three CTAs per SM at one chunk per lane.
+constexpr int SG_SHAPE_U[12][4] = {
     {8, 4, 2, 1},   // SUM (U = 4 at L = 4)
     {4, 4, 1, 1},   // MAX
     {4, 4, 1, 1},   // MIN
@@ -1272,14 +1316,17 @@ constexpr int SG_SHAPE_U[10][4] = {
     {4, 2, 1, 1},   // ADST
     {2, 2, 1, 1},   // ASRC
     {8, 4, 2, 1},   // WSUM
-    {4, 2, 1, 1}};  // EDOT
-constexpr int SG_SHAPE_MINB[10][4] = {
+    {4, 2, 1, 1},   // EDOT
+    {8, 4, 2, 1},   // TSUM (U = 4 at L = 4)
+    {4, 2, 1, 1}};  // TMASK
+constexpr int SG_SHAPE_MINB[12][4] = {
     {4, 3, 3, 2}, {4, 3, 3, 2}, {4, 3, 3, 2}, {4, 3, 3, 2}, {4, 0, 0, 0}, {4, 3, 2, 2}, {4, 3, 2, 1}, {4, 2, 2, 1},
-    {3, 3, 3, 2}, {4, 3, 2, 1}};
-static_assert(SG_RED_MAX == 1 && SG_RED_MIN == 2, "SG_SHAPE_U / SG_SHAPE_MINB rows follow the SG_RED_* values");
+    {3, 3, 3, 2}, {4, 3, 2, 1}, {4, 3, 3, 2}, {3, 3, 3, 2}};
+static_assert(SG_RED_MAX == 1 && SG_RED_MIN == 2 && SG_RED_TMASK == 11,
+              "SG_SHAPE_U / SG_SHAPE_MINB rows follow the SG_RED_* values");
 constexpr int sg_nch_index(int NCH) { return NCH == 1 ? 0 : NCH == 2 ? 1 : NCH == 4 ? 2 : 3; }
 constexpr int sg_chunk_u(int RED, int L, int NCH) {
-  return RED == SG_RED_SUM && L == 4 ? 4 : SG_SHAPE_U[RED][sg_nch_index(NCH)];
+  return (RED == SG_RED_SUM || RED == SG_RED_TSUM) && L == 4 ? 4 : SG_SHAPE_U[RED][sg_nch_index(NCH)];
 }
 constexpr int sg_chunk_minb(int RED, int NCH) { return SG_SHAPE_MINB[RED][sg_nch_index(NCH)]; }
 
@@ -1303,18 +1350,18 @@ static int launch_fixups(const SgParams& p, cudaStream_t st, bool heads = false)
 }
 
 // One ScatterGather launch: the main kernel (sg_chunk_kernel_t for the vectorised sum of 17..64 T-columns, which is
-// faster there on a products-shaped graph, DESIGN.md §3.1), then the fix-ups of the rows it cut.  MAX / MIN have their
-// own; ASTAT's stats have sg_attn_stat_fixup; the H-wide partials of the others are sums (the min / max backward's and
-// the attention gathers'), finished by the sum's.  ADST and ASRC then finish their heads-wide partials with the sum's
+// faster there on a products-shaped graph, DESIGN.md §3.1; for TSUM too), then the fix-ups of the rows it cut.  MAX /
+// MIN and TSUM (whose epilogue divides by the in-degree) have their own; ASTAT's stats have sg_attn_stat_fixup; the
+// H-wide partials of the others are sums (the min / max backwards' and the attention gathers'), finished by the sum's.  ADST and ASRC then finish their heads-wide partials with the sum's
 // fix-ups on p2, p with out2 / carry2 as a VEC = 1, Q = heads output.
 template <int VEC, int RED, int L, int NCH>
 static int launch(const SgParams& p, cudaStream_t st) {
-  constexpr bool RING = VEC == 4 && RED == SG_RED_SUM && L == 32 && NCH <= 2;
+  constexpr bool RING = VEC == 4 && (RED == SG_RED_SUM || RED == SG_RED_TSUM) && L == 32 && NCH <= 2;
   constexpr int WPB = SG_THREADS / L;
   int rc = ROC_OK;
   if (p.numChunks) {
     if constexpr (RING) {
-      if ((rc = launch_ring<NCH>(p, st)) != ROC_OK) return rc;
+      if ((rc = launch_ring<NCH, RED == SG_RED_TSUM>(p, st)) != ROC_OK) return rc;
     } else {
       const uint32_t grid = (p.numChunks + WPB - 1) / WPB;
       sg_chunk_kernel<VEC, L, NCH, sg_chunk_u(RED, L, NCH), sg_chunk_minb(RED, NCH), RED><<<grid, SG_THREADS, 0, st>>>(p);
@@ -1331,7 +1378,7 @@ static int launch(const SgParams& p, cudaStream_t st) {
       note_launch(ROC_SG_LAUNCH_STAT_FIXUP, SG_RED_ASTAT, 1, 32, 1, grid);
     }
   } else if constexpr (RED != SG_RED_ADST && RED != SG_RED_EDOT) {   // EDOT's outputs are per edge: nothing carried
-    constexpr int FIX = (RED == SG_RED_MAX || RED == SG_RED_MIN) ? RED : SG_RED_SUM;
+    constexpr int FIX = (RED == SG_RED_MAX || RED == SG_RED_MIN || RED == SG_RED_TSUM) ? RED : SG_RED_SUM;
     if ((rc = launch_fixups<VEC, L, NCH, FIX>(p, st)) != ROC_OK) return rc;
   }
   if constexpr (RED == SG_RED_ADST || RED == SG_RED_ASRC) {
@@ -1595,13 +1642,15 @@ static void t_units(SgParams& p, int vw, int cols) {
   p.Q = ((uint32_t)cols + vw - 1) / vw;
 }
 
-// The edge-weighted operands of run_planned: WSUM's weights, EDOT's G rows (indexed by plan row) and its output.
+// The operands of run_planned only some reductions take: WSUM's weights, EDOT's G rows (indexed by plan row) and its
+// output, TSUM's row ends of the original graph.
 struct SgEdge {
   const float* w = nullptr;
   const float* g = nullptr;
   int64_t ldG = 0;
   float* dw = nullptr;
   bool accumulate = false;
+  const roc_eid_t* rowEnd = nullptr;
 };
 
 // Reduction RED over the columns [0, H) of every row, in column blocks: 1,024 floats for the sum and the weighted sum
@@ -1613,7 +1662,7 @@ static int run_planned(roc_sg_plan* pl, int H, const float* in, int64_t ldIn, fl
                        const roc_vid_t* arg, int64_t ldArg, int epilogue, roc_vid_t selfBase, cudaStream_t st,
                        const SgEdge& ed = SgEdge()) {
   const bool vec = float4_rows({in, out, arg, ed.g}, {ldIn, ldOut, ldArg, ed.ldG});
-  const int blockCols = !vec ? 256 : (RED == SG_RED_SUM || RED == SG_RED_WSUM) ? 1024 : 512;
+  const int blockCols = !vec ? 256 : (RED == SG_RED_SUM || RED == SG_RED_WSUM || RED == SG_RED_TSUM) ? 1024 : 512;
   // EDOT carries nothing
   int rc = RED == SG_RED_EDOT ? ROC_OK : grow_carries(pl, std::min(H, blockCols), st);
   // the min / max forward's index carries, which the kernels address with the float carries' leading dimension
@@ -1627,6 +1676,7 @@ static int run_planned(roc_sg_plan* pl, int H, const float* in, int64_t ldIn, fl
     p.ldIn = (size_t)ldIn; p.ldOut = (size_t)ldOut; p.ldArg = (size_t)ldArg;
     p.score = ed.w; p.out2 = ed.dw; p.dwAdd = (ed.accumulate || c0 > 0) ? 1 : 0;
     if (ed.g) { p.xrow = ed.g + c0; p.ldX = (size_t)ed.ldG; }
+    if (ed.rowEnd) p.xrow = ed.rowEnd;
     p.H = (uint32_t)std::min(H - c0, blockCols);
     t_units(p, vec ? 4 : 1, std::min(H - c0, blockCols));
     rc = vec ? dispatch<4, RED>(p, st) : dispatch<1, RED>(p, st);
@@ -1713,6 +1763,41 @@ static SgParams attn_params(const roc_sg_plan* pl, int heads, int H, float slope
   return p;
 }
 
+// The attention backward's passes once its arguments are checked and both plans' carries grown: the node records of
+// ids [0, n) and B1 (d s_dst) over `pl`, B2 (inGrad, d s_src) over `plB2`.  With plB2 = pl, B2 is the gather over the
+// same CSR (quirk Q1); over the transposed plan its row j gathers the destinations i of j's out-edges, where the same
+// formula, a(i<-j) G[i] against the record of i, is the true adjoint.
+static int attn_backward_passes(roc_sg_plan* pl, roc_sg_plan* plB2, uint32_t n, int heads, int H, float slope,
+                                roc_vid_t selfBase, uint32_t fs, bool vec, const float* in, int64_t ldIn,
+                                const float* score, int64_t ldS, const float* out, int64_t ldOut, const float* stats,
+                                int64_t ldStats, const float* outGrad, int64_t ldG, float* inGrad, int64_t ldInG,
+                                float* scoreGrad, int64_t ldSG, cudaStream_t st) {
+  int rc = grow(pl->attnRec, pl->attnRecBytes, (size_t)n * heads * sizeof(float4), st);
+  if (rc != ROC_OK) return rc;
+  const int vw = vec ? 4 : 1;
+  const SgParams p = attn_params(pl, heads, H, slope, selfBase, score, ldS, stats, ldStats, fs);
+  // the node records {s_dst, m, 1/Z, D}, from G and O
+  SgParams r = p;
+  r.in = outGrad; r.ldIn = (size_t)ldG; r.xrow = out; r.ldX = (size_t)ldOut;
+  t_units(r, vw, H);
+  rc = vec ? launch_rec<4>(r, n, st) : launch_rec<1>(r, n, st);
+  if (rc != ROC_OK) return rc;
+  // B1: d s_dst, gathering X[j] and s_src[j] against G[i]
+  SgParams b1 = p;
+  b1.in = in; b1.ldIn = (size_t)ldIn; b1.xrow = outGrad; b1.ldX = (size_t)ldG;
+  b1.out = nullptr; b1.out2 = scoreGrad; b1.ldOut2 = (size_t)ldSG;
+  t_units(b1, vw, H);
+  rc = vec ? dispatch<4, SG_RED_ADST>(b1, st) : dispatch<1, SG_RED_ADST>(b1, st);
+  if (rc != ROC_OK) return rc;
+  // B2: inGrad and d s_src, gathering G[j] and the record of j against X[i]
+  SgParams b2 = attn_params(plB2, heads, H, slope, selfBase, score, ldS, stats, ldStats, fs);
+  b2.rec = pl->attnRec;
+  b2.in = outGrad; b2.ldIn = (size_t)ldG; b2.xrow = in; b2.ldX = (size_t)ldIn;
+  b2.out = inGrad; b2.ldOut = (size_t)ldInG; b2.out2 = scoreGrad + heads; b2.ldOut2 = (size_t)ldSG;
+  t_units(b2, vw, H);
+  return vec ? dispatch<4, SG_RED_ASRC>(b2, st) : dispatch<1, SG_RED_ASRC>(b2, st);
+}
+
 extern "C" int roc_sg_attn_forward_planned(const roc_sg_plan* plc, int heads, int H, float slope, roc_vid_t selfBase,
                                            const float* in, int64_t ldIn, const float* score, int64_t ldS,
                                            float* out, int64_t ldOut, float* stats, int64_t ldStats,
@@ -1758,29 +1843,30 @@ extern "C" int roc_sg_attn_backward_planned(const roc_sg_plan* plc, int heads, i
   if ((rc = find_id_end(pl, st)) != ROC_OK) return rc;
   const uint64_t n64 = std::max<uint64_t>(pl->idEnd, (uint64_t)selfBase + pl->nloc);
   if (n64 >= 0xFFFFFFF0ull) return ROC_ERR_UNSUPPORTED;
-  const uint32_t n = (uint32_t)n64;
-  if ((rc = grow(pl->attnRec, pl->attnRecBytes, (size_t)n * heads * sizeof(float4), st)) != ROC_OK) return rc;
-  const int vw = vec ? 4 : 1;
-  const SgParams p = attn_params(pl, heads, H, slope, selfBase, score, ldS, stats, ldStats, fs);
-  // the node records {s_dst, m, 1/Z, D}, from G and O
-  SgParams r = p;
-  r.in = outGrad; r.ldIn = (size_t)ldG; r.xrow = out; r.ldX = (size_t)ldOut;
-  t_units(r, vw, H);
-  rc = vec ? launch_rec<4>(r, n, st) : launch_rec<1>(r, n, st);
+  return attn_backward_passes(pl, pl, (uint32_t)n64, heads, H, slope, selfBase, fs, vec, in, ldIn, score, ldS, out,
+                              ldOut, stats, ldStats, outGrad, ldG, inGrad, ldInG, scoreGrad, ldSG, st);
+}
+
+extern "C" int roc_sg_attn_backward_exact(const roc_sg_plan* plc, roc_sg_transpose* tr, int heads, int H, float slope,
+                                          const float* in, int64_t ldIn, const float* score, int64_t ldS,
+                                          const float* out, int64_t ldOut, const float* stats, int64_t ldStats,
+                                          const float* outGrad, int64_t ldG, float* inGrad, int64_t ldInG,
+                                          float* scoreGrad, int64_t ldSG, roc_stream_t stream) {
+  roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  clear_launches();
+  if (!pl || !tr || !in || !score || !out || !stats || !outGrad || !inGrad || !scoreGrad || heads <= 0 || H <= 0 ||
+      ldIn < H || ldOut < H || ldG < H || ldInG < H || ldS < 2 * (int64_t)heads || ldStats < 2 * (int64_t)heads ||
+      ldSG < 2 * (int64_t)heads || pl->nloc != tr->N || pl->E != tr->E)
+    return ROC_ERR_INVALID;
+  const bool vec = float4_rows({in, out, outGrad, inGrad}, {ldIn, ldOut, ldG, ldInG});
+  cudaStream_t st = as_stream(stream);
+  uint32_t fs = 0;
+  int rc = attn_setup(pl, heads, H, slope, vec, st, &fs);
+  if (rc == ROC_OK) rc = attn_setup(tr->planT, heads, H, slope, vec, st, &fs);
   if (rc != ROC_OK) return rc;
-  // B1: d s_dst, gathering X[j] and s_src[j] against G[i]
-  SgParams b1 = p;
-  b1.in = in; b1.ldIn = (size_t)ldIn; b1.xrow = outGrad; b1.ldX = (size_t)ldG;
-  b1.out = nullptr; b1.out2 = scoreGrad; b1.ldOut2 = (size_t)ldSG;
-  t_units(b1, vw, H);
-  rc = vec ? dispatch<4, SG_RED_ADST>(b1, st) : dispatch<1, SG_RED_ADST>(b1, st);
-  if (rc != ROC_OK) return rc;
-  // B2: inGrad and d s_src, gathering G[j] and the record of j against X[i]
-  SgParams b2 = p;
-  b2.in = outGrad; b2.ldIn = (size_t)ldG; b2.xrow = in; b2.ldX = (size_t)ldIn;
-  b2.out = inGrad; b2.ldOut = (size_t)ldInG; b2.out2 = scoreGrad + heads; b2.ldOut2 = (size_t)ldSG;
-  t_units(b2, vw, H);
-  return vec ? dispatch<4, SG_RED_ASRC>(b2, st) : dispatch<1, SG_RED_ASRC>(b2, st);
+  // a whole graph: every id is below N, so the records cover [0, N) with no id scan
+  return attn_backward_passes(pl, tr->planT, tr->N, heads, H, slope, 0, fs, vec, in, ldIn, score, ldS, out, ldOut,
+                              stats, ldStats, outGrad, ldG, inGrad, ldInG, scoreGrad, ldSG, st);
 }
 
 extern "C" int roc_sg_weighted_forward_planned(const roc_sg_plan* plc, int H, const float* in, int64_t ldIn,
@@ -1889,6 +1975,29 @@ extern "C" int roc_sg_weighted_backward_planned(roc_sg_transpose* tr, int H, con
   SgEdge ed;
   ed.w = tr->wT;
   return run_planned<SG_RED_WSUM>(tr->planT, H, outGrad, ldG, inGrad, ldIn, nullptr, 0, 0, 0, st, ed);
+}
+
+extern "C" int roc_sg_transpose_sum_backward(roc_sg_transpose* tr, int H, const float* outGrad, int64_t ldG,
+                                             float* inGrad, int64_t ldIn, int epilogue, const roc_eid_t* rowEnd,
+                                             roc_stream_t stream) {
+  clear_launches();
+  if (!tr || H <= 0 || !outGrad || !inGrad || ldG < H || ldIn < H || ((epilogue & ROC_SG_EPI_NORM) && !rowEnd))
+    return ROC_ERR_INVALID;
+  cudaStream_t st = as_stream(stream);
+  // without NORM the transposed plan's own sum is the whole computation
+  if (!(epilogue & ROC_SG_EPI_NORM))
+    return run_planned<SG_RED_SUM>(tr->planT, H, outGrad, ldG, inGrad, ldIn, nullptr, 0, epilogue, 0, st);
+  SgEdge ed;
+  ed.rowEnd = rowEnd;
+  return run_planned<SG_RED_TSUM>(tr->planT, H, outGrad, ldG, inGrad, ldIn, nullptr, 0, epilogue, 0, st, ed);
+}
+
+extern "C" int roc_sg_transpose_minmax_backward(roc_sg_transpose* tr, int H, const float* outGrad, int64_t ldG,
+                                                const roc_vid_t* arg, int64_t ldArg, float* inGrad, int64_t ldIn,
+                                                roc_stream_t stream) {
+  clear_launches();
+  if (!tr || H <= 0 || !outGrad || !arg || !inGrad || ldG < H || ldArg < H || ldIn < H) return ROC_ERR_INVALID;
+  return run_planned<SG_RED_TMASK>(tr->planT, H, outGrad, ldG, inGrad, ldIn, arg, ldArg, 0, 0, as_stream(stream));
 }
 
 extern "C" int roc_sg_forward(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft, int H,

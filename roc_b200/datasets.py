@@ -3,7 +3,9 @@
 Graphs are symmetrised (the reference's backward multiplies by A, not A^T —
 scattergather_kernel.cu:160-170 — which is the true adjoint only for symmetric
 A), de-duplicated, given self loops (the `.add_self_edge.lux` convention,
-gnn.cc:756) and sorted by (dst, src).  CSR convention: rowEnd[v] = inclusive
+gnn.cc:756) and sorted by (dst, src).  directed=True skips the symmetrisation, for
+models trained with Model.set_exact_backward, whose backward runs over the transposed
+graph.  CSR convention: rowEnd[v] = inclusive
 prefix sum of in-degrees (u64), col[e] = source (u32).
 
 Generators run on whatever torch device is passed (CPU in tests, the GPU in
@@ -15,12 +17,16 @@ import numpy as np
 import torch
 
 
-def _csr_from_pairs(src, dst, n):
-    """Symmetrise + self loops + dedup + sort by (dst, src).  src/dst: int64 tensors."""
+def _csr_from_pairs(src, dst, n, directed=False):
+    """Symmetrise (unless directed) + self loops + dedup + sort by (dst, src).  src/dst: int64 tensors."""
     dev = src.device
     loops = torch.arange(n, device=dev, dtype=torch.int64)
-    s = torch.cat([src, dst, loops])
-    d = torch.cat([dst, src, loops])
+    if directed:
+        s = torch.cat([src, loops])
+        d = torch.cat([dst, loops])
+    else:
+        s = torch.cat([src, dst, loops])
+        d = torch.cat([dst, src, loops])
     key = torch.unique(d * n + s)          # sorted by dst then src, duplicates removed
     d = key // n
     s = key - d * n
@@ -29,17 +35,19 @@ def _csr_from_pairs(src, dst, n):
     return row_end.to(torch.int64), s.to(torch.int32)
 
 
-def uniform_graph(n, n_pairs, seed=1, device="cpu"):
+def uniform_graph(n, n_pairs, seed=1, device="cpu", directed=False):
+    """directed=True keeps each pair's orientation (src -> dst): no reverse edges are added."""
     g = torch.Generator(device=device)
     g.manual_seed(seed)
     src = torch.randint(0, n, (n_pairs,), generator=g, device=device, dtype=torch.int64)
     dst = torch.randint(0, n, (n_pairs,), generator=g, device=device, dtype=torch.int64)
-    return _csr_from_pairs(src, dst, n)
+    return _csr_from_pairs(src, dst, n, directed)
 
 
-def rmat_graph(scale, n_pairs, seed=1, abcd=(0.57, 0.19, 0.19, 0.05), permute=True, device="cpu"):
+def rmat_graph(scale, n_pairs, seed=1, abcd=(0.57, 0.19, 0.19, 0.05), permute=True, device="cpu", directed=False):
     """R-MAT (Chakrabarti et al.) with Graph500's (a,b,c,d); n = 2^scale vertices,
-    n_pairs undirected pairs drawn before symmetrisation / dedup."""
+    n_pairs undirected pairs drawn before symmetrisation / dedup.  directed=True keeps each pair's orientation
+    (src -> dst): the graph gets no reverse edges, so it has about half the edges of the symmetric one."""
     n = 1 << scale
     g = torch.Generator(device=device)
     g.manual_seed(seed)
@@ -55,7 +63,7 @@ def rmat_graph(scale, n_pairs, seed=1, abcd=(0.57, 0.19, 0.19, 0.05), permute=Tr
     if permute:
         perm = torch.randperm(n, generator=g, device=device)
         src, dst = perm[src], perm[dst]
-    return _csr_from_pairs(src, dst, n)
+    return _csr_from_pairs(src, dst, n, directed)
 
 
 def powerlaw_graph(n, n_pairs, alpha=1.6, seed=1, device="cpu"):

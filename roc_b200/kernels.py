@@ -176,7 +176,7 @@ class _DeviceArray:
 
 class SgTranspose:
     """roc_sg_transpose of a whole graph's CSR (row_end: N END offsets, col: E sources, every id < N): the exact input
-    gradient of the edge-weighted sum on any graph."""
+    gradients of the edge-weighted sum, the sum, max / min and attention on any graph."""
 
     def __init__(self, row_end, col):
         _lib.require_device()
@@ -197,6 +197,45 @@ class SgTranspose:
         check(lib.roc_sg_weighted_backward_planned(self.handle, h, _ptr(gy), _ld(gy), _ptr(w), _ptr(out), _ld(out),
                                                    _stream()), "roc_sg_weighted_backward_planned")
         return out
+
+    def _rows(self, like):
+        """A new [N][H] output for an input `like`: padded to float4 rows when like's rows are, else dense."""
+        h = like.shape[1]
+        return padded(self.n, h, like.device) if _ld(like) % 4 == 0 else torch.empty((self.n, h), device=like.device)
+
+    def sum_backward(self, gy, epilogue=0, row_end=None, out=None):
+        """The sum's exact input gradient: out[j] = epi(sum over the edges e with col[e] = j of gy[dst(e)]).  With
+        SG_EPI_NORM, row_end (the graph's, u64 END offsets) is required: NORM divides by j's in-degree in it."""
+        h = gy.shape[1]
+        if out is None:
+            out = self._rows(gy)
+        check(lib.roc_sg_transpose_sum_backward(self.handle, h, _ptr(gy), _ld(gy), _ptr(out), _ld(out), int(epilogue),
+                                                _ptr(row_end), _stream()), "roc_sg_transpose_sum_backward")
+        return out
+
+    def minmax_backward(self, gy, arg, out=None):
+        """Max / min's exact input gradient for arg from SgPlan.minmax_forward: out[j] = sum over the distinct
+        destinations i of j's out-edges of gy[i] where arg[i] == j (a duplicate edge counts once)."""
+        h = gy.shape[1]
+        if out is None:
+            out = self._rows(gy)
+        check(lib.roc_sg_transpose_minmax_backward(self.handle, h, _ptr(gy), _ld(gy), _ptr(arg), _ld(arg), _ptr(out),
+                                                   _ld(out), _stream()), "roc_sg_transpose_minmax_backward")
+        return out
+
+    def attn_backward(self, plan, x, scores, out, stats, gy, heads=1, slope=0.2, in_grad=None, score_grad=None):
+        """Attention's exact backward -> (in_grad [N][H], score_grad [N][2*heads] = d s_dst | d s_src), with `plan` the
+        whole graph's SgPlan and the other arguments as SgPlan.attn_backward's."""
+        h = x.shape[1]
+        if in_grad is None:
+            in_grad = self._rows(x)
+        if score_grad is None:
+            score_grad = torch.empty((self.n, 2 * heads), device=x.device)
+        check(lib.roc_sg_attn_backward_exact(plan.handle, self.handle, int(heads), h, float(slope), _ptr(x), _ld(x),
+                                             _ptr(scores), _ld(scores), _ptr(out), _ld(out), _ptr(stats), _ld(stats),
+                                             _ptr(gy), _ld(gy), _ptr(in_grad), _ld(in_grad), _ptr(score_grad),
+                                             _ld(score_grad), _stream()), "roc_sg_attn_backward_exact")
+        return in_grad, score_grad
 
     def info(self):
         """Copies of the transposed CSR: {"row_end": int64 [N], "col": int32 [E], "perm": int32 [E]} (the uint32 /

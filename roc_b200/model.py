@@ -143,6 +143,12 @@ class Model:
     def set_fusion(self, on):
         check(lib.roc_host_set_fusion(self.h, int(on)))
 
+    def set_exact_backward(self, on=True):
+        """Train the sum (and mean), max / min and attention aggregations on their exact gradient over the graph's
+        transpose, which is right on directed graphs and multigraphs (off by default: the gather over the same CSR,
+        exact only on a symmetric graph).  Call before init().  One partition only."""
+        check(lib.roc_host_set_exact_backward(self.h, int(bool(on))))
+
     def init(self):
         check(lib.roc_host_init(self.h))
 
@@ -248,8 +254,10 @@ class Model:
         return pm.as_dict()
 
 
-def build_gcn(model, layers, dropout_rate, lr=0.01, weight_decay=0.05):
-    """The model script of gnn.cc:65-98 for `-layers a-b-...-c`.  Returns the handles."""
+def build_gcn(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exact_backward=False):
+    """The model script of gnn.cc:65-98 for `-layers a-b-...-c`.  Returns the handles.  exact_backward: train on the
+    exact gradient over the graph's transpose (Model.set_exact_backward), for directed graphs; the same keyword on
+    build_sage_mean, build_sage_pool and build_gat."""
     L = len(layers)
     x = model.create_node_tensor(layers[0])
     label = model.create_node_tensor(layers[-1])
@@ -271,11 +279,13 @@ def build_gcn(model, layers, dropout_rate, lr=0.01, weight_decay=0.05):
             t = model.add(t, skip)
     model.softmax_cross_entropy(t, label, mask)
     model.adam(lr, weight_decay)
+    if exact_backward:
+        model.set_exact_backward(True)
     model.init()
     return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs}
 
 
-def build_sage_mean(model, layers, dropout_rate, lr=0.01, weight_decay=0.05):
+def build_sage_mean(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exact_backward=False):
     """GraphSAGE with the mean aggregator (BASELINE.json configs[2]) composed from the reference's own ops
     (gnn.h:165-179; AGGR_AVG is declared at gnn.h:75-80 but the reference's ScatterGather only sums):
 
@@ -306,11 +316,13 @@ def build_sage_mean(model, layers, dropout_rate, lr=0.01, weight_decay=0.05):
             relu_outs.append(t)
     model.softmax_cross_entropy(t, label, mask)
     model.adam(lr, weight_decay)
+    if exact_backward:
+        model.set_exact_backward(True)
     model.init()
     return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs}
 
 
-def build_sage_pool(model, layers, dropout_rate, aggr=_lib.AGGR_MAX, lr=0.01, weight_decay=0.05):
+def build_sage_pool(model, layers, dropout_rate, aggr=_lib.AGGR_MAX, lr=0.01, weight_decay=0.05, exact_backward=False):
     """GraphSAGE with the pooling aggregator (Hamilton et al., 2017) composed from the reference's ops plus the max
     (or min) ScatterGather.  The reference's Linear has no bias, so neither has this.  Per layer:
 
@@ -340,12 +352,15 @@ def build_sage_pool(model, layers, dropout_rate, aggr=_lib.AGGR_MAX, lr=0.01, we
             relu_outs.append(t)
     model.softmax_cross_entropy(t, label, mask)
     model.adam(lr, weight_decay)
+    if exact_backward:
+        model.set_exact_backward(True)
     model.init()
     return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs, "pools": pools,
             "pool_ins": pool_ins}
 
 
-def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01, weight_decay=0.05):
+def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01, weight_decay=0.05,
+              exact_backward=False):
     """GAT (Velickovic et al., 2018) built from the reference's ops plus attention_gather.  `heads` (an int, or one
     value per hidden layer) applies to the hidden layers; the last layer has one head.  layers[i] is the width of
     layer i's output, heads_i * F_i.  Per layer:
@@ -382,6 +397,8 @@ def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01,
             relu_outs.append(t)
     model.softmax_cross_entropy(t, label, mask)
     model.adam(lr, weight_decay)
+    if exact_backward:
+        model.set_exact_backward(True)
     model.init()
     return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs, "attn": attn,
             "attn_ins": attn_ins, "scores": scores}

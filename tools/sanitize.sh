@@ -5,7 +5,9 @@
 #       followed by one max-aggregation forward and backward; then the attention forward and backward at 41 and 64
 #       floats with one head and at 64 and 256 floats with eight, on float4 rows, and at 256 floats with two heads on
 #       rows of 257 floats (the scalar path); then the edge-weighted forward, its transposed backward and the edge
-#       dot (overwriting, then accumulating) at 41, 64, 200 and 602 floats;
+#       dot (overwriting, then accumulating) at 41, 64, 200 and 602 floats; then the exact sum (with norm and relu)
+#       and min backwards over the transpose at the same widths, and the exact attention backward at 41 floats with
+#       one head and 64 with eight;
 #   (c) the warp-specialised dW kernel at 602 x 64 with the dropout mask and at 64 x 41, on rows that wrap its ring
 #       and end in a partial block.
 # Usage: tools/sanitize.sh [logdir]   (needs a GPU; `make sanitize`)
@@ -48,6 +50,18 @@ for h in (41, 64, 200, 602):
     tr.backward(y, w)
     dw = plan.edge_dot(y, x)
     plan.edge_dot(y, x, dw=dw, accumulate=True)
+    torch.cuda.synchronize()
+for h in (41, 64, 200, 602):                                 # the exact backwards over the same transpose
+    x = K.padded(n, h, "cuda", fill=torch.rand((n, h), device="cuda"))
+    tr.sum_backward(x, epilogue=3, row_end=re.cuda())
+    mx, arg = plan.minmax_forward(x, 2)
+    tr.minmax_backward(x, arg)
+    torch.cuda.synchronize()
+for h, heads in ((41, 1), (64, 8)):
+    x = K.padded(n, h, "cuda", fill=torch.rand((n, h), device="cuda"))
+    sc = torch.randn((n, 2 * heads), device="cuda")
+    out, stats = plan.attn_forward(x, sc, heads)
+    tr.attn_backward(plan, x, sc, out, stats, x, heads)
     torch.cuda.synchronize()
 tr.close()
 print("sg ok")

@@ -354,7 +354,7 @@ int roc_halo_send_layout(int numParts, int myPart, const int32_t* host_allCounts
                          uint64_t* sendOffs, uint64_t* numSendRows);
 /* roc_pack_rows for a subset: dst[sel[t]] = src[rows[sel[t]]] for t < nSel — the send-list entries of one row
  * block, written to their places in the send buffer, so that the block can travel (copy engines, peer slabs) while
- * the producer computes the next one. */
+ * the producer computes the next one.  Writes the float4 pad columns [H, round_up(H, 4)) as roc_pack_rows does. */
 int roc_pack_rows_at(int64_t nSel, int H, const roc_vid_t* sel, const roc_vid_t* rows, const float* src,
                      int64_t ldSrc, float* dst, int64_t ldDst, roc_stream_t stream);
 /* Fused pack + exchange over peer memory: row srcRows[j] of `src` is stored to
@@ -365,12 +365,18 @@ int roc_pack_rows_at(int64_t nSel, int H, const roc_vid_t* sel, const roc_vid_t*
  * host_peerBase is a HOST array of numPeers <= ROC_MAX_PEERS device pointers (entries never named by peer[] may be
  * NULL).  smLimit > 0 sizes the grid for that many SMs (the ones a producer running beside it left free, see
  * roc_set_sm_reserve); 0 = whole chip.  The caller orders the consumer after every producer (a barrier across
- * the partitions). */
+ * the partitions).  With ldSrc, ldDst, src and every non-NULL peer base 16-byte aligned, each row is stored as whole
+ * float4s: columns [H, round_up(H, 4)) of the destination row receive the source row's pad columns; columns from
+ * round_up(H, 4) on are never written.  Otherwise exactly columns [0, H) are. */
 #define ROC_MAX_PEERS 16
 int roc_push_rows(int64_t nRows, int H, const roc_vid_t* srcRows, const uint8_t* peer, const roc_vid_t* dstRow,
                   const float* src, int64_t ldSrc, float* const* host_peerBase, int numPeers, int64_t ldDst,
                   int smLimit, roc_stream_t stream);
-/* dst[j][0:H] = src[rows[j]][0:H]: packs the rows another partition asked for into a send buffer. */
+/* dst[j][0:H] = src[rows[j]][0:H]: packs the rows another partition asked for into a send buffer.
+ * Pad columns: when ldSrc and ldDst are multiples of 4 and both bases are 16-byte aligned, the rows travel as whole
+ * float4s, so dst[j][H:round_up(H, 4)] also receives src[rows[j]][H:round_up(H, 4)]; columns from round_up(H, 4) on
+ * are never written.  Otherwise exactly dst[j][0:H] is written.  The same holds for roc_pack_rows_at and, with every
+ * peer base aligned, for roc_push_rows: callers pass whole padded rows. */
 int roc_pack_rows(int64_t nRows, int H, const roc_vid_t* rows, const float* src, int64_t ldSrc,
                   float* dst, int64_t ldDst, roc_stream_t stream);
 
@@ -380,7 +386,12 @@ int roc_pack_rows(int64_t nRows, int H, const roc_vid_t* rows, const float* src,
  * out[n][h] = in[n][h] / sqrtf((float)deg(n)); in/out are the partition's rows.
  * If `also_relu_mask_of` is non-NULL (fused backward of relu∘norm, gnn.cc:84-85):
  * out = (also_relu_mask_of > 0 ? in : 0) / sqrtf(deg); it has `in`'s shape and
- * leading dimension (it is the relu output whose gradient `in` is). */
+ * leading dimension (it is the relu output whose gradient `in` is).
+ * Pad columns: when ldIn and ldOut are multiples of 4 and in, out and the mask are 16-byte
+ * aligned, rows are processed as whole float4s, whatever H is: columns [H, round_up(H, 4))
+ * of each output row receive that row's input pad columns, masked and divided the same
+ * way (a NaN pad gives NaN, a zero pad 0, or NaN in a row of degree 0).  Columns from
+ * round_up(H, 4) on are never written.  Otherwise exactly columns [0, H) are. */
 int roc_indegree_norm(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft, int H,
                       const roc_eid_t* rowEnd, const float* in, int64_t ldIn,
                       float* out, int64_t ldOut, const float* also_relu_mask_of,

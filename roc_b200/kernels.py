@@ -358,10 +358,7 @@ def softmax_xent_bwd(logits, labels, mask, compact=False):
     else:
         check(lib.roc_softmax_xent_bwd(logits.shape[0], logits.shape[1], _ptr(logits), _ld(logits), _ptr(labels),
                                        _ld(labels), _ptr(mask), _ptr(g), _ld(g), _ptr(perf), _stream()))
-    p = perf.cpu()
-    d = {"trainLoss": float(p[:1].view(torch.float32)[0]), "trainAll": int(p[1]), "testAll": int(p[2]),
-         "valAll": int(p[3]), "trainCorrect": int(p[4]), "testCorrect": int(p[5]), "valCorrect": int(p[6])}
-    return g, d
+    return g, _perf_dict(perf)
 
 
 def linear_fwd(x, w, activation=0, norm_row_end=None, col_left=0, out=None):
@@ -426,15 +423,22 @@ def linear_bwd_fused(x, w, y, dy, dw, dx, activation=0, mask=None, rate=0.0, rel
     return dw, dx
 
 
-def softmax_xent_bwd_norm(logits, labels, mask, row_end, col_left=0, compact=False):
-    """softmax_xent_bwd with the logits' InDegreeNorm backward fused: grad rows divided by sqrt(deg)."""
+def _perf_dict(perf):
+    p = perf.cpu()
+    return {"trainLoss": float(p[:1].view(torch.float32)[0]), "trainAll": int(p[1]), "testAll": int(p[2]),
+            "valAll": int(p[3]), "trainCorrect": int(p[4]), "testCorrect": int(p[5]), "valCorrect": int(p[6])}
+
+
+def softmax_xent_bwd_norm(logits, labels, mask, row_end, col_left=0, compact=False, with_perf=False):
+    """softmax_xent_bwd with the logits' InDegreeNorm backward fused: grad rows divided by sqrt(deg).  Returns the
+    gradient, or (gradient, metrics dict as softmax_xent_bwd's) with with_perf=True."""
     g = torch.empty_like(logits)
     perf = torch.zeros(7, dtype=torch.int32, device=logits.device)
     check(lib.roc_softmax_xent_bwd_norm(logits.shape[0], logits.shape[1], _ptr(logits), _ld(logits),
                                         None if compact else _ptr(labels), 0 if compact else _ld(labels),
                                         _ptr(labels) if compact else None, _ptr(mask), _ptr(g), _ld(g),
                                         _ptr(row_end), col_left, _ptr(perf), _stream()), "roc_softmax_xent_bwd_norm")
-    return g
+    return (g, _perf_dict(perf)) if with_perf else g
 
 
 def linear_bwd(x, w, y, dy, dw, dx=None, activation=0, accumulate_dx=False):

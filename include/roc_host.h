@@ -80,6 +80,39 @@ int roc_host_parameter_shape(roc_host* h, int p, int64_t out[2]); /* inDim, outD
 int roc_host_get_parameter(roc_host* h, int p, float* host, int which); /* 0 W, 1 dW, 2 m, 3 v */
 int roc_host_set_parameter(roc_host* h, int p, const float* host);
 
+/* What Model::init decided for each layer (read-only; call after roc_host_init).  Layers are numbered in creation
+ * order (AGGR_AVG appends three).  Every tensor field is a tensor handle, -1 for none, or -2 for a tensor the
+ * caller holds no handle for (the inner tensors of AGGR_AVG).  Returns ROC_ERR_INVALID for a bad layer or NULL out. */
+#define ROC_HOST_OP_LINEAR 0
+#define ROC_HOST_OP_INDEGREE_NORM 1
+#define ROC_HOST_OP_SCATTER_GATHER 2          /* the sum */
+#define ROC_HOST_OP_SCATTER_GATHER_MAX 3
+#define ROC_HOST_OP_SCATTER_GATHER_MIN 4
+#define ROC_HOST_OP_SCATTER_GATHER_WEIGHTED 5
+#define ROC_HOST_OP_ATTENTION_GATHER 6
+#define ROC_HOST_OP_RELU 7
+#define ROC_HOST_OP_SIGMOID 8
+#define ROC_HOST_OP_ADD 9
+#define ROC_HOST_OP_DROPOUT 10
+#define ROC_HOST_OP_SOFTMAX_CROSS_ENTROPY 11
+struct roc_host_op_info {   /* a struct tag only: roc_host_op_info is also the function's name */
+  int kind;          /* ROC_HOST_OP_* */
+  int fusedInto;     /* >= 0: the layer whose kernel does this op's forward */
+  int bwdFused;      /* norm: its backward is done by a Linear's dX epilogue or by the softmax */
+  int epilogue;      /* sum ScatterGather: ROC_SG_EPI_* of the forward store */
+  int bwdEpilogue;   /*   ... and of the backward store */
+  int fwdOut;        /*   the tensor the forward writes (-1: its own output); also a Linear's */
+  int bwdOut;        /*   the tensor whose gradient the backward writes (-1: its input's) */
+  int flags;         /* Linear: ROC_LINEAR_* of the forward */
+  int dropOp;        /*   >= 0: the Dropout layer applied while X is loaded */
+  int dxOut;         /*   the tensor whose gradient dX goes to (-1: its input's) */
+  int dxReluOf;      /*   the tensor whose relu mask the dX epilogue applies (-1: none) */
+  int dxNorm;        /*   the dX epilogue divides by sqrt(in-degree) */
+  int gradOut;       /* softmax: the tensor whose gradient it writes, divided by sqrt(in-degree) (-1: the logits') */
+};
+int roc_host_num_ops(roc_host* h);
+int roc_host_op_info(roc_host* h, int layer, struct roc_host_op_info* out);
+
 /* train loop (gnn.cc:99-111) */
 int roc_host_train_mode(roc_host* h);
 int roc_host_infer_mode(roc_host* h);

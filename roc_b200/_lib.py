@@ -72,6 +72,22 @@ class PerfMetrics(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+HOST_OPS = ("linear", "indegree_norm", "scatter_gather", "scatter_gather_max", "scatter_gather_min",
+            "scatter_gather_weighted", "attention_gather", "relu", "sigmoid", "add", "dropout",
+            "softmax_cross_entropy")                       # ROC_HOST_OP_* by value
+
+
+class HostOpInfo(C.Structure):
+    """roc_host_op_info (include/roc_host.h): one layer's kind and the fusion decisions Model::init made."""
+    _fields_ = [(k, C.c_int) for k in ("kind", "fusedInto", "bwdFused", "epilogue", "bwdEpilogue", "fwdOut", "bwdOut",
+                                       "flags", "dropOp", "dxOut", "dxReluOf", "dxNorm", "gradOut")]
+
+    def as_dict(self):
+        d = {k: getattr(self, k) for k, _ in self._fields_}
+        d["kind"] = HOST_OPS[self.kind]
+        return d
+
+
 class RocError(RuntimeError):
     pass
 
@@ -202,6 +218,8 @@ PROTOTYPES = {
     "roc_host_parameter_shape": (i32, [vp, i32, vp]),
     "roc_host_get_parameter": (i32, [vp, i32, vp, i32]),
     "roc_host_set_parameter": (i32, [vp, i32, vp]),
+    "roc_host_num_ops": (i32, [vp]),
+    "roc_host_op_info": (i32, [vp, i32, C.POINTER(HostOpInfo)]),
     "roc_host_train_mode": (i32, [vp]),
     "roc_host_infer_mode": (i32, [vp]),
     "roc_host_zero_gradients": (i32, [vp]),

@@ -117,8 +117,9 @@ k_map(int64_t rows, int Wq, const float* __restrict__ a, int64_t lda, const floa
 // add backward: dA (+)= dY ; dB (+)= dY in one pass over dY
 template <int VEC>
 __global__ void __launch_bounds__(EW_T)
-k_add_bwd(int64_t rows, int Wq, const float* __restrict__ dy, int64_t ldy, float* __restrict__ da,
-          int64_t lda, int accA, float* __restrict__ db, int64_t ldb, int accB) {
+k_add_bwd(int64_t rows, int Wq, const float* __restrict__ dy, int64_t ldy, float* da, int64_t lda, int accA,
+          float* db, int64_t ldb, int accB) {
+  // da and db alias for add(t, t) (accA = 0, accB = 1): no __restrict__ on them, so db's load follows da's store
   const int64_t total = rows * (int64_t)Wq;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total;
        i += (int64_t)gridDim.x * blockDim.x) {

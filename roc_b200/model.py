@@ -217,6 +217,16 @@ class Model:
         assert w.shape == (o, i)
         check(lib.roc_host_set_parameter(self.h, p, w.ctypes.data))
 
+    def op_info(self):
+        """Per layer, in creation order, what init() decided: the op kind and its fusion fields (roc_host_op_info),
+        tensors as handles or -1."""
+        out = []
+        for layer in range(lib.roc_host_num_ops(self.h)):
+            info = _lib.HostOpInfo()
+            check(lib.roc_host_op_info(self.h, layer, C.byref(info)), "roc_host_op_info")
+            out.append(info.as_dict())
+        return out
+
     # ---- train loop (gnn.cc:99-111)
     def train_mode(self):
         check(lib.roc_host_train_mode(self.h))

@@ -37,11 +37,12 @@ def test_no_undeclared_prototypes():
 
 def test_struct_layouts_match_the_header(tmp_path):
     """The ctypes mirrors of the C structs (roc_linear_bwd_args, roc_gemm_info, roc_sg_launch, roc_sg_call_info,
-    roc_perf_metrics) have the C layout: a tiny C program compiled against include/roc_b200.h prints sizeof / offsetof
-    of every field."""
+    roc_host_op_info, roc_perf_metrics) have the C layout: a tiny C program compiled against include/roc_host.h prints
+    sizeof / offsetof of every field."""
     structs = [("roc_linear_bwd_args", _lib.LinearBwdArgs), ("roc_gemm_info", _lib.GemmInfo),
-               ("roc_sg_launch", _lib.SgLaunch), ("roc_sg_call_info", _lib.SgCallInfo)]
-    prog = ['#include <stdio.h>', '#include <stddef.h>', '#include "roc_b200.h"', 'int main(void) {']
+               ("roc_sg_launch", _lib.SgLaunch), ("roc_sg_call_info", _lib.SgCallInfo),
+               ("struct roc_host_op_info", _lib.HostOpInfo)]
+    prog = ['#include <stdio.h>', '#include <stddef.h>', '#include "roc_host.h"', 'int main(void) {']
     for cname, py in structs:
         prog += ['  printf("%%zu\\n", sizeof(%s));' % cname]
         prog += ['  printf("%%zu\\n", offsetof(%s, %s));' % (cname, f) for f, _ in py._fields_]
@@ -60,6 +61,13 @@ def test_struct_layouts_match_the_header(tmp_path):
         pos += 1
     assert pos == len(out) - 1
     assert out[-1] == C.sizeof(_lib.PerfMetrics)
+
+
+def test_host_op_kinds_match_the_header():
+    hdr = open(os.path.join(ROOT, "include", "roc_host.h")).read()
+    for i, kind in enumerate(_lib.HOST_OPS):
+        assert re.search(r"#define ROC_HOST_OP_%s %d\b" % (kind.upper(), i), hdr), kind
+    assert len(re.findall(r"#define ROC_HOST_OP_", hdr)) == len(_lib.HOST_OPS)
 
 
 def test_gemm_info_hook_without_a_gemm():

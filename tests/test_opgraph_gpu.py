@@ -1,0 +1,768 @@
+"""Model op graphs, fused and unfused, against the fp64 interpreter of tests/opgraph.py over three Adam steps.
+
+Model::init decides which tensors need a gradient, who overwrites a gradient and who adds to it (resetInputGrads,
+set in reverse layer order by Model::backward), and five peephole fusions that reroute where a gradient is written
+and switch other ops' forward or backward off.  This file builds op graphs through a Recorder and checks, per case:
+
+- the fusion report (Model.op_info) of both schedules: the hand-listed cases state it exactly, the unfused schedule
+  has none;
+- against the witness at each step's weights: the logits at the parity bar, every dW and every edge gradient at
+  rtol 2e-4 with atol_scale 2e-5 (the bars of test_exact_model_gpu.py);
+- between the schedules, bit for bit: logits, dW, edge gradients and the weights after each update;
+- after training, an infer-mode forward: equal metrics in both schedules (except trainLoss, an atomic sum), and the
+  *All counts equal to the mask's counts.
+
+Wirings that break Q7 (below) run in a subprocess: both schedules must exit non-zero at the first backward() with
+the same assertion.
+
+The rules every generated graph obeys, derived from model.cc:
+- Q7 as implemented.  ScatterGather::backward and InDegreeNorm::backward assert resetInputGrads[0] before they check
+  requiresGrad, so each must be the last-created consumer of its input, even when that input is a leaf.
+  Dropout::backward checks requiresGrad first: the rule binds a dropout only when its input needs a gradient.  Every
+  other op adds into a gradient another op already wrote.
+- Q1: without set_exact_backward, the sum, max / min and attention backwards gather over the forward CSR, the true
+  adjoint only on a symmetric graph; so only exact-mode cases run on the directed multigraph.
+- Max / min without the exact mode need strictly increasing sources per row (the symmetric graphs have them).
+- attention_gather: scores of 2 * heads columns; heads 1, 2, 4 or 8; with heads > 1 the width is heads * F with F a
+  power of two >= 4; width <= 512.
+- One loss."""
+import itertools
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+import pytest
+
+from conftest import ROOT
+from opgraph import Recorder, witness
+from roc_b200 import _lib, datasets
+from roc_b200.model import Host, Model
+
+pytestmark = pytest.mark.gpu
+NONE, RELU = _lib.AC_MODE_NONE, _lib.AC_MODE_RELU
+SEEN = set()               # what the cases reached: op kinds, fusions, near-misses, width classes
+WORST = {}                 # output family -> worst |error| / bound
+T0 = time.time()
+
+
+# ------------------------------------------------------------------------------------------------------ graphs ---
+def symmetric(n, pairs, seed, hub=False):
+    """Symmetric, deduplicated, a self loop on every node, sources strictly increasing per row.  hub: node 0 is
+    joined to every node, so its row has n > 2,112 in-edges (cut rows and the big-row fix-up)."""
+    rng = np.random.RandomState(seed)
+    s, d = rng.randint(0, n, size=pairs), rng.randint(0, n, size=pairs)
+    if hub:
+        s, d = np.concatenate([s, np.arange(n)]), np.concatenate([d, np.zeros(n, dtype=np.int64)])
+    s, d = np.concatenate([s, d, np.arange(n)]), np.concatenate([d, s, np.arange(n)])
+    key = np.unique(d.astype(np.int64) * n + s)
+    d, s = key // n, key % n
+    return np.cumsum(np.bincount(d, minlength=n)).astype(np.uint64), s.astype(np.uint32)
+
+
+def directed_multigraph(n=250, e=1800, seed=3):
+    """Directed, with duplicate edges, a heavy row and a self loop on every node."""
+    rng = np.random.RandomState(seed)
+    dst = rng.randint(0, n, size=e)
+    src = (rng.zipf(1.6, size=e) - 1) % n
+    src[1::4], dst[1::4] = src[0::4][:src[1::4].shape[0]], dst[0::4][:dst[1::4].shape[0]]
+    dst[:120] = 9
+    dst, src = np.concatenate([dst, np.arange(n)]), np.concatenate([src, np.arange(n)])
+    order = np.argsort(dst, kind="stable")
+    return np.cumsum(np.bincount(dst[order], minlength=n)).astype(np.uint64), src[order].astype(np.uint32)
+
+
+GRAPHS = {}
+
+
+def graph(kind):
+    if kind not in GRAPHS:
+        GRAPHS[kind] = {"sym": lambda: symmetric(300, 1200, 1), "hub": lambda: symmetric(2300, 3000, 2, hub=True),
+                        "directed": directed_multigraph}[kind]()
+        if kind == "hub":
+            assert np.diff(np.concatenate([[0], GRAPHS[kind][0].astype(np.int64)])).max() > 2112
+    return GRAPHS[kind]
+
+
+# --------------------------------------------------------------------------------------------------- the runner ---
+DEFAULTS = dict(fusedInto=-1, bwdFused=0, epilogue=0, bwdEpilogue=0, fwdOut=-1, bwdOut=-1, flags=0, dropOp=-1,
+                dxOut=-1, dxReluOf=-1, dxNorm=0, gradOut=-1)
+
+
+def fusions(infos):
+    """{layer: the fields init() changed from their defaults}."""
+    out = {}
+    for layer, info in enumerate(infos):
+        d = {k: v for k, v in info.items() if k != "kind" and v != DEFAULTS[k]}
+        if d:
+            out[layer] = d
+    return out
+
+
+def note_fusions(fz, ir):
+    for layer, d in fz.items():
+        kind = ir.nodes[layer]["kind"]
+        if kind == "linear" and d.get("flags"):
+            SEEN.add("fusion:linear_norm_sg")
+        if kind == "scatter_gather" and "epilogue" in d:
+            SEEN.add("fusion:sg_norm" if d["epilogue"] == _lib.SG_EPI_NORM else "fusion:sg_norm_relu")
+        if kind == "linear" and d.get("dropOp", -1) >= 0:
+            SEEN.add("fusion:dropout_linear")
+        if kind == "softmax_cross_entropy":
+            SEEN.add("fusion:norm_softmax")
+        if kind == "linear" and d.get("dxNorm"):
+            SEEN.add("fusion:norm_relu_linear" if ir.nodes[layer - 1]["kind"] == "relu" else
+                     "fusion:norm_relu_dropout_linear")
+
+
+def note_widths(ir):
+    for nd in ir.nodes:
+        k = nd["kind"]
+        SEEN.add("op:" + k)
+        if k == "linear":
+            i, o = ir.width[nd["ins"][0]], nd["attrs"]["out_dim"]
+            SEEN.add("op:linear_relu" if nd["attrs"]["activation"] == RELU else "op:linear_none")
+            if i % 4:
+                SEEN.add("width:linear_in_not_float4")
+            if o > 128:
+                SEEN.add("width:linear_out_over_128")
+        w = ir.width.get(nd["ins"][0], 0)
+        if k.startswith("scatter_gather") or k == "attention_gather":
+            if w % 4 and w <= 16:
+                SEEN.add("width:sg_H_not_float4")
+            if 65 <= w <= 128:
+                SEEN.add("width:sg_65_128")
+            if 129 <= w <= 256:
+                SEEN.add("width:sg_129_256")
+        if k == "softmax_cross_entropy":
+            SEEN.add("width:softmax_C_%d" % w)
+
+
+def family(name, got, want, rtol, atol_scale):
+    """rel_close, keeping the worst |error| / bound of each output family.  A dW row that vanishes identically (the
+    destination-score rows of an attention score Linear when every edge's LeakyReLU is on one side: the softmax does
+    not change when a row's scores shift together) holds only fp32 rounding of terms that cancel; such a row, below
+    1e-12 of the matrix's largest entry in fp64, is held to 1e-4 of that entry instead."""
+    got, want = np.asarray(got, dtype=np.float64), np.asarray(want, dtype=np.float64)
+    assert got.shape == want.shape, name
+    scale = np.abs(want).max() if want.size else 0.0
+    bound = rtol * np.abs(want) + atol_scale * scale + 1e-30
+    if want.ndim == 2 and want.size:
+        zero_rows = np.abs(want).max(axis=1) <= 1e-12 * scale
+        bound[zero_rows] = 1e-4 * scale + 1e-30
+    r = float((np.abs(got - want) / bound).max()) if want.size else 0.0
+    WORST[name] = max(WORST.get(name, 0.0), r)
+    return r
+
+
+def run(build, gkind, fuse, steps=3, feats_seed=5):
+    """Build with `build(ir)` (it makes the graph and the loss, returns its handles), train `steps` Adam steps and
+    run one infer forward.  Per step: weights before it, logits, dW, edge gradients, weights after it, the relu masks
+    and max / min choices; then the infer metrics and the fusion report."""
+    row_end, col = graph(gkind)
+    n = row_end.shape[0]
+    host = Host(0, 0, 1)
+    host.graph_from_arrays(row_end, col)
+    m = Model(host, seed=1)
+    m.set_fusion(fuse)
+    ir = Recorder(m)
+    h = build(ir)
+    ir.adam(0.01, 0.05)
+    ir.init()
+    loss = ir.loss_node()
+    logits_t, label_t, mask_t = loss["ins"]
+    rng = np.random.RandomState(feats_seed)
+    feats = {t: rng.uniform(-1, 1, size=(n, ir.width[t])).astype(np.float32) for t in ir.leaves if t != label_t}
+    for t, a in feats.items():
+        m.set_tensor(t, a)
+    _, labels, mask = datasets.node_data(n, 1, ir.width[logits_t], seed=feats_seed)
+    labels, mask = labels.numpy(), mask.numpy()
+    m.set_labels(label_t, labels)
+    m.set_tensor(mask_t, mask.astype(np.int32))
+    ev = {}
+    for e in ir.edges:
+        ev[e] = np.random.RandomState(e).uniform(0.05, 0.6, size=col.shape[0]).astype(np.float32)
+        m.set_tensor(e, ev[e])
+    relu_of = {nd["layer"]: nd["out"] for nd in ir.nodes
+               if nd["kind"] == "relu" or (nd["kind"] == "linear" and nd["attrs"]["activation"] == RELU)}
+    minmax = {nd["layer"]: nd["out"] for nd in ir.nodes if nd["kind"] in ("scatter_gather_max", "scatter_gather_min")}
+    out = dict(steps=[], ir=ir, h=h, feats=feats, labels=labels, mask=mask, edges=ev, info=m.op_info())
+    for _ in range(steps):
+        w0 = [m.get_parameter(p) for p in range(m.num_parameters())]
+        m.train_mode(); m.zero_gradients(); m.forward()
+        st = dict(w0=w0, logits=m.get_tensor(logits_t),
+                  relu={l: m.get_tensor(t) > 0 for l, t in relu_of.items()},
+                  args={l: m.get_aggr_index(t) for l, t in minmax.items()})
+        m.backward()
+        st["dw"] = [m.get_parameter(p, "grad") for p in range(m.num_parameters())]
+        st["de"] = {e: m.get_tensor(e, grad=True)[:, 0].copy() for e in ir.edges if ir.edge_grad[e]}
+        m.update()
+        st["w1"] = [m.get_parameter(p) for p in range(m.num_parameters())]
+        out["steps"].append(st)
+    m.infer_mode(); m.forward()
+    out["metrics"] = m.metrics()
+    host.close()
+    return out
+
+
+def check_case(build, gkind="sym", expect=None):
+    """Both schedules against the witness and each other; `expect(h)`: the fused schedule's fusion report."""
+    fused, unfused = run(build, gkind, True), run(build, gkind, False)
+    ir = fused["ir"]
+    row_end, col = graph(gkind)
+    fz = fusions(fused["info"])
+    assert fusions(unfused["info"]) == {}, "the unfused schedule fused something"
+    if expect is not None:
+        assert fz == expect(fused["h"]), fz
+    note_fusions(fz, ir)
+    note_widths(ir)
+    for r in (fused, unfused):
+        for step, st in enumerate(r["steps"]):
+            what = "%s step %d" % ("fused" if r is fused else "unfused", step)
+            wit = witness(ir, (row_end, col), r["feats"], r["labels"], r["mask"], st["w0"], r["edges"], step=step + 1,
+                          relu_masks=st["relu"], aggr_args=st["args"])
+            assert family("logits", st["logits"], wit["logits"], 1e-4, 1e-5) <= 1, what + " logits vs fp64"
+            for p, (a, b) in enumerate(zip(st["dw"], wit["dW"])):
+                assert family("dW", a, b, 2e-4, 2e-5) <= 1, what + " dW[%d] vs fp64" % p
+            for e, g in st["de"].items():
+                assert family("edge gradient", g, wit["edge_grad"][e], 2e-4, 2e-5) <= 1, what + " edge gradient"
+    for step, (a, b) in enumerate(zip(fused["steps"], unfused["steps"])):
+        assert np.array_equal(a["logits"], b["logits"]), "step %d: logits differ between the schedules" % step
+        for p in range(len(a["dw"])):
+            assert np.array_equal(a["dw"][p], b["dw"][p]), "step %d: dW[%d] differs between the schedules" % (step, p)
+            assert np.array_equal(a["w1"][p], b["w1"][p]), "step %d: W[%d] differs between the schedules" % (step, p)
+        for e in a["de"]:
+            assert np.array_equal(a["de"][e], b["de"][e]), "step %d: edge gradient differs" % step
+    fm, um = dict(fused["metrics"]), dict(unfused["metrics"])
+    fm.pop("trainLoss"), um.pop("trainLoss")
+    assert fm == um, (fm, um)
+    mask = fused["mask"]
+    assert (fm["trainAll"], fm["valAll"], fm["testAll"]) == tuple(int((mask == k).sum()) for k in (0, 1, 2)), fm
+    return fz
+
+
+def loss(ir, t):
+    ir.softmax_cross_entropy(t, ir.create_node_tensor(ir.width[t]), ir.create_node_tensor(1, is_int=True))
+
+
+# ------------------------------------------------------------------------------------------ (a) hand-listed cases ---
+def lin_norm_sg(ir):
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 16); n = ir.indegree_norm(t); s = ir.scatter_gather(n)
+    loss(ir, s)
+    return dict(t=t, n=n, s=s)
+
+
+def sg_norm(ir):
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 16); s = ir.scatter_gather(t); n = ir.indegree_norm(s)
+    loss(ir, n)
+    return dict(t=t, s=s, n=n)
+
+
+def sg_norm_relu(ir):
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 16); s = ir.scatter_gather(t); n = ir.indegree_norm(s); r = ir.relu(n)
+    loss(ir, r)
+    return dict(s=s, n=n, r=r)
+
+
+def dropout_linear(ir):
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 16); d = ir.dropout(t, 0.5, seed=3); y = ir.linear(d, 5)
+    loss(ir, y)
+    return dict(t=t, d=d)
+
+
+def norm_softmax(ir):
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 5); n = ir.indegree_norm(t)
+    loss(ir, n)
+    return dict(t=t, n=n)
+
+
+def norm_relu_linear(ir, drop=False):
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 16); s = ir.scatter_gather(t); n = ir.indegree_norm(s); r = ir.relu(n)
+    d = ir.dropout(r, 0.5, seed=1) if drop else r
+    y = ir.linear(d, 5)
+    loss(ir, y)
+    return dict(s=s, n=n, r=r)
+
+
+def expect_fused_chain(h, sg_layer, relu=True):
+    """sg -> norm [-> relu] as the downstream SG fusion leaves it (the layers follow the SG)."""
+    e = {sg_layer: dict(epilogue=_lib.SG_EPI_NORM | (_lib.SG_EPI_RELU if relu else 0), fwdOut=h["r"] if relu
+                        else h["n"]), sg_layer + 1: dict(fusedInto=sg_layer)}
+    if relu:
+        e[sg_layer + 2] = dict(fusedInto=sg_layer)
+    return e
+
+
+HAND = {
+    # each fusion alone, in its minimal pattern
+    "lin_norm_sg": (lin_norm_sg, lambda h: {0: dict(flags=_lib.LINEAR_NORM_EPILOGUE, fwdOut=h["n"]), 1: dict(fusedInto=0),
+                                            2: dict(bwdEpilogue=_lib.SG_EPI_NORM, bwdOut=h["t"])}),
+    # the norm feeds the loss: the softmax takes its backward too
+    "sg_norm": (sg_norm, lambda h: {1: dict(epilogue=_lib.SG_EPI_NORM, fwdOut=h["n"]), 2: dict(fusedInto=1, bwdFused=1),
+                                    3: dict(gradOut=h["s"])}),
+    "sg_norm_relu": (sg_norm_relu, lambda h: expect_fused_chain(h, 1)),
+    "dropout_linear": (dropout_linear, lambda h: {1: dict(fusedInto=2), 2: dict(dropOp=1)}),
+    "norm_softmax": (norm_softmax, lambda h: {1: dict(bwdFused=1), 2: dict(gradOut=h["t"])}),
+    "norm_relu_linear": (norm_relu_linear, lambda h: {**expect_fused_chain(h, 1),
+                                                      2: dict(fusedInto=1, bwdFused=1),
+                                                      4: dict(dxReluOf=h["r"], dxNorm=1, dxOut=h["s"])}),
+    "norm_relu_dropout_linear": (lambda ir: norm_relu_linear(ir, drop=True),
+                                 lambda h: {**expect_fused_chain(h, 1), 2: dict(fusedInto=1, bwdFused=1),
+                                            4: dict(fusedInto=5),
+                                            5: dict(dropOp=4, dxReluOf=h["r"], dxNorm=1, dxOut=h["s"])}),
+}
+
+
+def near(name):
+    SEEN.add("near:" + name)
+
+
+def nm_linear_out_twice(ir):
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 16); r = ir.relu(t); n = ir.indegree_norm(t); s = ir.scatter_gather(n)
+    loss(ir, ir.linear(ir.add(s, r), 5))
+
+
+def nm_norm1_out_twice(ir):
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 16); n = ir.indegree_norm(t); r = ir.relu(n); s = ir.scatter_gather(n)
+    loss(ir, ir.linear(ir.add(s, r), 5))
+
+
+def nm_sg_out_twice(ir):
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 16); s = ir.scatter_gather(t); r = ir.relu(s); n = ir.indegree_norm(s)
+    loss(ir, ir.linear(ir.add(n, r), 5))
+
+
+def nm_norm2_out_twice(ir):
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 16); s = ir.scatter_gather(t); n = ir.indegree_norm(s); g = ir.sigmoid(n); r = ir.relu(n)
+    loss(ir, ir.linear(ir.add(r, g), 5))
+    return dict(n=n)
+
+
+def nm_relu_out_twice(ir):
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 16); s = ir.scatter_gather(t); n = ir.indegree_norm(s); r = ir.relu(n)
+    loss(ir, ir.add(ir.linear(r, 5), ir.linear(r, 5)))
+    return dict(n=n, r=r)
+
+
+def nm_linear_relu(ir):
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 16, RELU); n = ir.indegree_norm(t); s = ir.scatter_gather(n)
+    loss(ir, ir.linear(s, 5))
+
+
+def nm_aggr(aggr):
+    def build(ir):
+        x = ir.create_node_tensor(12)
+        t = ir.linear(x, 16); n = ir.indegree_norm(t)
+        s = ir.scatter_gather(n, weights=ir.create_edge_tensor()) if aggr == "weighted" else ir.scatter_gather(n, aggr)
+        n2 = ir.indegree_norm(s); r = ir.relu(n2)
+        loss(ir, ir.linear(r, 5))
+    return build
+
+
+def nm_sigmoid(ir):
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 16); s = ir.scatter_gather(t); n = ir.indegree_norm(s); g = ir.sigmoid(n)
+    loss(ir, ir.linear(g, 5))
+    return dict(n=n)
+
+
+def nm_dropout_twice(ir):
+    x = ir.create_node_tensor(12)
+    d = ir.dropout(x, 0.5, seed=2)
+    loss(ir, ir.add(ir.linear(d, 5), ir.linear(d, 5)))
+
+
+def nm_dropout_non_linear(ir):
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 16); d = ir.dropout(t, 0.5, seed=2); r = ir.relu(d)
+    loss(ir, ir.linear(r, 5))
+
+
+def nm_norm_softmax_no_grad(ir):
+    x = ir.create_node_tensor(5)
+    ir.linear(x, 4)                          # a dead parameter; the norm must be x's last consumer
+    loss(ir, ir.indegree_norm(x))
+
+
+def nm_norm_in_linear_feeds_softmax(ir):
+    """model.cc's guard against a norm fused into a Linear feeding the softmax: the upstream fusion needs the norm's
+    output read once (by the SG), the softmax fusion needs it read once (by the softmax), so the two never meet.
+    With both readers the upstream fusion is refused; the SG comes after the loss so that it is the norm output's
+    last consumer, and its output is dead."""
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 5); n = ir.indegree_norm(t)
+    loss(ir, n)
+    ir.scatter_gather(n)
+
+
+def nm_competing_norm(ir):
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 16); n1 = ir.indegree_norm(t); s1 = ir.scatter_gather(n1); n2 = ir.indegree_norm(s1)
+    s2 = ir.scatter_gather(n2)
+    loss(ir, ir.linear(s2, 5))
+    return dict(t=t, n1=n1, n2=n2)
+
+
+NEAR = {
+    "linear_out_read_twice": (nm_linear_out_twice, lambda h: {}),
+    "norm1_out_read_twice": (nm_norm1_out_twice, lambda h: {}),
+    "sg_out_read_twice": (nm_sg_out_twice, lambda h: {}),
+    "norm2_out_read_twice": (nm_norm2_out_twice, lambda h: {1: dict(epilogue=_lib.SG_EPI_NORM, fwdOut=h["n"]),
+                                                            2: dict(fusedInto=1)}),
+    "relu_out_read_twice": (nm_relu_out_twice, lambda h: expect_fused_chain(h, 1)),
+    "linear_relu_upstream": (nm_linear_relu, lambda h: {}),
+    "max_instead_of_sum": (nm_aggr(_lib.AGGR_MAX), lambda h: {}),
+    "min_instead_of_sum": (nm_aggr(_lib.AGGR_MIN), lambda h: {}),
+    "weighted_instead_of_sum": (nm_aggr("weighted"), lambda h: {}),
+    "sigmoid_instead_of_relu": (nm_sigmoid, lambda h: {1: dict(epilogue=_lib.SG_EPI_NORM, fwdOut=h["n"]),
+                                                       2: dict(fusedInto=1)}),
+    "dropout_read_twice": (nm_dropout_twice, lambda h: {}),
+    "dropout_feeds_non_linear": (nm_dropout_non_linear, lambda h: {}),
+    "norm_softmax_input_needs_no_grad": (nm_norm_softmax_no_grad, lambda h: {}),
+    "norm_in_linear_feeds_softmax": (nm_norm_in_linear_feeds_softmax, lambda h: {}),
+    # lin -> n1 -> sg1 -> n2 -> sg2: n2 goes to sg1's epilogue, so sg2 cannot take it for its upstream fusion
+    "competing_norm": (nm_competing_norm, lambda h: {0: dict(flags=_lib.LINEAR_NORM_EPILOGUE, fwdOut=h["n1"]),
+                                                     1: dict(fusedInto=0),
+                                                     2: dict(bwdEpilogue=_lib.SG_EPI_NORM, bwdOut=h["t"],
+                                                             epilogue=_lib.SG_EPI_NORM, fwdOut=h["n2"]),
+                                                     3: dict(fusedInto=2)}),
+}
+
+
+def add_t_t(ir):
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 5)
+    loss(ir, ir.add(t, t))
+
+
+def attention_t_t(ir):
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 2)
+    loss(ir, ir.linear(ir.attention_gather(t, t, heads=1), 5))
+
+
+def three_readers(order):
+    def build(ir):
+        x = ir.create_node_tensor(12)
+        t = ir.linear(x, 16)
+        make = {"relu": lambda: ir.relu(t), "sigmoid": lambda: ir.sigmoid(t), "linear": lambda: ir.linear(t, 16)}
+        outs = [make[k]() for k in order]
+        loss(ir, ir.linear(ir.add(ir.add(outs[0], outs[1]), outs[2]), 5))
+    return build
+
+
+def linear_relu_sigmoid(ir):
+    x = ir.create_node_tensor(12)
+    loss(ir, ir.linear(ir.sigmoid(ir.linear(x, 16, RELU)), 5, RELU))
+
+
+def sgc(ir):
+    x = ir.create_node_tensor(12)
+    s = ir.scatter_gather(x); n = ir.indegree_norm(s)
+    loss(ir, ir.linear(n, 5))
+    return dict(n=n)
+
+
+def shared_edges(grad):
+    def build(ir):
+        x = ir.create_node_tensor(12)
+        e = ir.create_edge_tensor()
+        a = ir.scatter_gather(ir.linear(x, 16), weights=e)
+        b = ir.scatter_gather(ir.relu(a), weights=e)
+        loss(ir, ir.linear(b, 5))
+        ir.set_edge_grad(e, grad)
+    return build
+
+
+def dead_branch(ir):
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 16)
+    y = ir.linear(t, 5)
+    ir.relu(ir.linear(t, 8))          # created after y: its backward runs first and writes t's gradient
+    loss(ir, y)
+
+
+SHARED = {
+    "add_t_t": (add_t_t, lambda h: {}),
+    "attention_t_t_H2": (attention_t_t, lambda h: {}),
+    "linear_relu_and_sigmoid": (linear_relu_sigmoid, lambda h: {}),
+    "sgc_raw_features": (sgc, lambda h: {0: dict(epilogue=_lib.SG_EPI_NORM, fwdOut=h["n"]), 1: dict(fusedInto=0)}),
+    "shared_edges_grad_on": (shared_edges(True), lambda h: {}),
+    "shared_edges_grad_off": (shared_edges(False), lambda h: {}),
+    "dead_branch": (dead_branch, lambda h: {}),
+}
+for _o in itertools.permutations(("relu", "sigmoid", "linear")):
+    SHARED["three_readers_" + "_".join(_o)] = (three_readers(_o), lambda h: {})
+
+
+def exact_gcn(ir):
+    ir.set_exact_backward(True)
+    x = ir.create_node_tensor(12)
+    t = ir.linear(ir.dropout(x, 0.5), 16); s = ir.scatter_gather(ir.indegree_norm(t)); r = ir.relu(ir.indegree_norm(s))
+    t2 = ir.linear(ir.dropout(r, 0.5), 5)
+    loss(ir, ir.indegree_norm(ir.scatter_gather(ir.indegree_norm(t2))))
+
+
+def exact_pool(aggr):
+    def build(ir):
+        ir.set_exact_backward(True)
+        x = ir.create_node_tensor(12)
+        p = ir.relu(ir.linear(x, 16))
+        loss(ir, ir.add(ir.linear(ir.scatter_gather(p, aggr), 5), ir.linear(x, 5)))
+    return build
+
+
+def exact_attention_weighted(ir):
+    ir.set_exact_backward(True)
+    x = ir.create_node_tensor(12)
+    e = ir.create_edge_tensor()
+    wh = ir.linear(x, 16)
+    a = ir.relu(ir.attention_gather(wh, ir.linear(wh, 8), heads=4))
+    b = ir.scatter_gather(ir.scatter_gather(a, _lib.AGGR_AVG), weights=e)
+    ir.set_edge_grad(e, True)
+    loss(ir, ir.linear(b, 5))
+
+
+EXACT = {"gcn_dropout": exact_gcn, "pool_max": exact_pool(_lib.AGGR_MAX), "pool_min": exact_pool(_lib.AGGR_MIN),
+         "attention_avg_weighted": exact_attention_weighted}
+
+
+@pytest.mark.parametrize("name", list(HAND))
+def test_each_fusion_alone(name):
+    build, expect = HAND[name]
+    check_case(build, expect=expect)
+
+
+@pytest.mark.parametrize("name", list(NEAR))
+def test_fusion_near_miss(name):
+    build, expect = NEAR[name]
+    check_case(build, expect=expect)
+    near(name)
+
+
+@pytest.mark.parametrize("name", list(SHARED))
+def test_shared_and_aliased(name):
+    build, expect = SHARED[name]
+    check_case(build, expect=expect)
+    SEEN.add("shared:" + name)
+
+
+@pytest.mark.parametrize("name", list(EXACT))
+def test_exact_mode_on_a_directed_multigraph(name):
+    check_case(EXACT[name], gkind="directed")
+    SEEN.add("exact:" + name)
+
+
+# ------------------------------------------------------------------------------------------ (b) random graphs ---
+SMALL, RING_U, RING_T = (3, 5, 7, 12, 16), (72, 100, 128), (132, 160, 256)
+CLASSES = (5, 32, 33, 64, 65, 128, 129)
+
+
+def random_graph(seed):
+    """A seeded DAG over every op, obeying the rules in the module docstring.  Tensors a ScatterGather, a norm or a
+    dropout (whose input needs a gradient) have read are closed: nothing reads them again.  Every tensor nothing
+    reads at the end goes through a Linear into one sum that feeds the loss, except, now and then, a dead one."""
+    exact = seed % 6 == 5
+    gkind = "directed" if exact else ("hub" if seed % 8 == 3 else "sym")
+
+    def build(ir):                       # called once per schedule: the same graph each time
+        rng = np.random.RandomState(seed)
+        if exact:
+            ir.set_exact_backward(True)
+        open_, grad, closed = [], {}, set()
+        edges = []
+
+        def take(t, closes):
+            open_.remove(t) if closes and t in open_ else None
+            if closes:
+                closed.add(t)
+
+        def new(t, g):
+            open_.append(t)
+            grad[t] = g
+            return t
+
+        x = ir.create_node_tensor(int(rng.choice((7, 12, 16, 33))))
+        new(x, False)
+        for _ in range(rng.randint(3, 9)):
+            t = open_[rng.randint(len(open_))]
+            w = ir.width[t]
+            k = rng.choice(["linear", "linear", "norm", "sg", "sg_mm", "sg_w", "attn", "relu", "sigmoid", "add",
+                            "dropout"])
+            if k == "linear":
+                pick = rng.randint(4)
+                o = int(rng.choice(SMALL + (136, 7) if pick == 0 else RING_U if pick == 1 else RING_T if pick == 2
+                                   else SMALL))
+                new(ir.linear(t, o, RELU if rng.rand() < 0.3 else NONE), True)
+            elif k == "norm":
+                take(t, True)
+                new(ir.indegree_norm(t), grad[t])
+            elif k == "sg":
+                take(t, True)
+                new(ir.scatter_gather(t, _lib.AGGR_AVG if rng.rand() < 0.25 else _lib.AGGR_SUM), grad[t])
+            elif k == "sg_mm":
+                take(t, True)
+                new(ir.scatter_gather(t, _lib.AGGR_MAX if rng.rand() < 0.5 else _lib.AGGR_MIN), grad[t])
+            elif k == "sg_w":
+                if not edges or rng.rand() < 0.3:
+                    edges.append(ir.create_edge_tensor())
+                e = edges[rng.randint(len(edges))]
+                new(ir.scatter_gather(t, weights=e), True)     # WeightedScatterGather adds where it must: no closing
+            elif k == "attn":
+                heads = int(rng.choice([h for h in (1, 2, 4, 8) if h == 1 or (w % h == 0 and w // h >= 4 and
+                                                                               (w // h) & (w // h - 1) == 0)]))
+                if w > 512:
+                    continue
+                sc = ir.linear(t, 2 * heads)
+                new(ir.attention_gather(t, sc, heads=heads), True)
+            elif k in ("relu", "sigmoid"):
+                new(getattr(ir, k)(t), grad[t])
+            elif k == "add":
+                same = [u for u in open_ if ir.width[u] == w]
+                u = same[rng.randint(len(same))]
+                new(ir.add(t, u), grad[t] or grad[u])
+            else:
+                take(t, grad[t])
+                new(ir.dropout(t, float(rng.choice([0.0, 0.5])), seed=int(rng.randint(4))), grad[t])
+        C = int(rng.choice(CLASSES))
+        sinks = [t for t in open_ if t != x or len(open_) == 1]
+        if len(sinks) > 1 and rng.rand() < 0.25:
+            sinks = sinks[1:]                                     # the first one stays dead
+        z = None
+        for t in sinks:
+            y = ir.linear(t, C)
+            z = y if z is None else ir.add(z, y)
+        if rng.rand() < 0.3:
+            z = ir.indegree_norm(z)
+        loss(ir, z)
+        for e in edges:
+            ir.set_edge_grad(e, bool(rng.rand() < 0.7))
+    return build, gkind
+
+
+@pytest.mark.parametrize("seed", range(48))
+def test_random_graph(seed):
+    build, gkind = random_graph(seed)
+    check_case(build, gkind=gkind)
+    SEEN.add("random")
+    if gkind == "hub":
+        SEEN.add("graph:hub")
+
+
+# ----------------------------------------------------------------------------------------------- (e) refusals ---
+def rf_sg(leaf):
+    def build(ir):
+        x = ir.create_node_tensor(12)
+        t = x if leaf else ir.linear(x, 16)
+        s = ir.scatter_gather(t)
+        loss(ir, ir.add(ir.linear(s, 5), ir.linear(t, 5)))     # t read again after the SG
+    return build
+
+
+def rf_norm(leaf):
+    def build(ir):
+        x = ir.create_node_tensor(12)
+        t = x if leaf else ir.linear(x, 16)
+        n = ir.indegree_norm(t)
+        loss(ir, ir.add(ir.linear(n, 5), ir.linear(t, 5)))
+    return build
+
+
+def rf_dropout(into_linear):
+    def build(ir):
+        x = ir.create_node_tensor(12)
+        t = ir.linear(x, 16)
+        d = ir.dropout(t, 0.5)
+        y = ir.linear(d, 5) if into_linear else ir.linear(ir.relu(d), 5)
+        loss(ir, ir.add(y, ir.linear(t, 5)))
+    return build
+
+
+def rf_norm_softmax(ir):
+    """The softmax takes the norm's backward (gradOut); a reader of the norm's input created after the loss."""
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 5)
+    loss(ir, ir.indegree_norm(t))
+    ir.relu(t)
+
+
+REFUSE = {"sg_not_last": rf_sg(False), "sg_on_leaf_not_last": rf_sg(True), "norm_not_last": rf_norm(False),
+          "norm_on_leaf_not_last": rf_norm(True), "dropout_not_last": rf_dropout(False),
+          "dropout_into_linear_not_last": rf_dropout(True), "norm_into_softmax_not_last": rf_norm_softmax}
+
+
+def refusal_prog(name, fuse):
+    """Run in a subprocess: build case `name`, forward, backward."""
+    row_end, col = graph("sym")
+    host = Host(0, 0, 1)
+    host.graph_from_arrays(row_end, col)
+    m = Model(host, seed=1)
+    m.set_fusion(fuse)
+    ir = Recorder(m)
+    REFUSE[name](ir)
+    ir.adam(0.01, 0.05)
+    ir.init()
+    n = row_end.shape[0]
+    logits_t, label_t, mask_t = ir.loss_node()["ins"]
+    for t in ir.leaves:
+        if t != label_t:
+            m.set_tensor(t, np.random.RandomState(t).uniform(-1, 1, size=(n, ir.width[t])).astype(np.float32))
+    m.set_labels(label_t, np.arange(n, dtype=np.int32) % ir.width[logits_t])
+    m.set_tensor(mask_t, np.zeros(n, dtype=np.int32))
+    m.train_mode(); m.zero_gradients(); m.forward()
+    print("forward done", flush=True)
+    m.backward()
+    host.synchronize()
+    print("backward done", flush=True)
+
+
+def run_refusal(name, fuse):
+    prog = "\n".join(["import sys; sys.path.insert(0, %r); sys.path.insert(0, %r)" % (ROOT, os.path.join(ROOT, "tests")),
+                      "from test_opgraph_gpu import refusal_prog",
+                      "refusal_prog(%r, %r)" % (name, fuse)])
+    return subprocess.run([sys.executable, "-c", prog], capture_output=True, text=True, timeout=300, cwd=ROOT,
+                          env=dict(os.environ))
+
+
+@pytest.mark.parametrize("name", list(REFUSE))
+def test_q7_refusal_is_the_same_in_both_schedules(name):
+    got = {}
+    for fuse in (True, False):
+        p = run_refusal(name, fuse)
+        assert p.returncode != 0, "%s (fuse=%s) trained where Q7 refuses:\n%s" % (name, fuse, p.stdout)
+        assert p.stdout.strip().splitlines()[-1:] == ["forward done"], (fuse, p.stdout, p.stderr[-2000:])
+        lines = p.stderr.strip().splitlines()
+        assert len(lines) >= 3 and lines[-3].startswith("assertion failed: resetInputGrads[0]"), p.stderr[-2000:]
+        got[fuse] = lines[-3:-1]
+    assert got[True] == got[False], got
+    SEEN.add("refusal:" + name)
+
+
+# ------------------------------------------------------------------------------------------------ (f) coverage ---
+def test_opgraph_covered():
+    """Every op kind, fusion, near-miss and width class was reached (run the whole file: this test comes last)."""
+    want = {"op:" + k for k in _lib.HOST_OPS} | {"op:linear_relu", "op:linear_none"}
+    want |= {"fusion:" + f for f in ("linear_norm_sg", "sg_norm", "sg_norm_relu", "dropout_linear", "norm_softmax",
+                                     "norm_relu_linear", "norm_relu_dropout_linear")}
+    want |= {"near:" + n for n in NEAR} | {"shared:" + s for s in SHARED} | {"exact:" + e for e in EXACT}
+    want |= {"refusal:" + r for r in REFUSE} | {"random", "graph:hub"}
+    want |= {"width:" + w for w in ("linear_in_not_float4", "linear_out_over_128", "sg_H_not_float4", "sg_65_128",
+                                    "sg_129_256")}
+    want |= {"width:softmax_C_%d" % c for c in CLASSES}
+    missing = sorted(want - SEEN)
+    assert not missing, missing
+    print("\nworst |error| / bound: %s; %.0f s" % (", ".join("%s %.3f" % kv for kv in sorted(WORST.items())),
+                                                  time.time() - T0))

@@ -20,9 +20,10 @@
 //  * the main kernel, sg_chunk_kernel, gathers the neighbour rows in registers.  A row is Q T-columns (float4
 //    when the rows are 16-byte aligned, else float); a worker is L = 4, 8, 16 or 32 lanes, the fewest that cover
 //    Q, and each lane loads its NCH = ceil(Q / L) columns of U rows per group.  A launch covers up to 256
-//    T-columns (1024 floats vectorised, 256 scalar); wider rows are split into column blocks.  One table
-//    (with_shape, sg_chunk_u, sg_chunk_minb) gives every reduction its shape, and one launcher (launch) runs the
-//    main kernel and the fix-ups the reduction needs.
+//    T-columns (1024 floats vectorised, 256 scalar); wider rows are split into column blocks.  with_shape picks L
+//    and NCH; one row per reduction of the table SG_REDS gives its widest row, its gathers in flight and CTAs per SM,
+//    the fix-ups and carries it needs, and whether it has a ring form.  One launcher (launch) runs the main kernel
+//    and the fix-ups the row names.
 //  * vectorised rows of 65..256 floats run on sg_chunk_kernel_t instead, which fetches them with cp.async.bulk
 //    copies into a shared-memory ring: it was faster there on a products-shaped graph (DESIGN.md §3.1).  It
 //    shares the plan and the per-row summation order, so its results are bit-identical to sg_chunk_kernel's.
@@ -1254,13 +1255,78 @@ static void note_launch(int kind, int red, int vec, int lanes, int nch, uint32_t
   t_call.count++;
 }
 
+// ----------------------------------------------------------- reduction table ---
+// Everything the host needs to know to launch a reduction: one row per SG_RED_* value.
+enum SgFix {
+  SG_FIX_NONE,    // nothing carried (EDOT's outputs are per edge), or only heads-wide partials (ADST)
+  SG_FIX_OWN,     // the fix-ups instantiated for the reduction itself
+  SG_FIX_SUM,     // the H-wide partials are plain sums, finished by the sum's fix-ups
+  SG_FIX_STATS    // sg_attn_stat_fixup
+};
+enum SgCarry {
+  SG_CARRY_NONE,
+  SG_CARRY_FLOAT,
+  SG_CARRY_INDEX  // the float carries plus the min / max index carries
+};
+struct SgRed {
+  int red;          // the SG_RED_* value this row describes
+  // The widest row, in T-columns, one launch takes, on float4 rows and on scalar rows; run_planned cuts wider rows
+  // into column blocks of VEC * maxQ floats.
+  int maxQ4, maxQ1;
+  // -1: every row runs on sg_chunk_kernel.  Otherwise vectorised rows at L = 32, NCH <= 2 run on sg_chunk_kernel_t,
+  // and this is the MODE bit the reduction adds there (4: TSUM's NORM epilogue divides by in_degree).
+  int ring;
+  SgFix fix;        // the fix-up of the H-wide partials of the rows the main kernel cut
+  bool headsFix;    // the heads-wide partials (out2 / carry2) also go through the sum's fix-ups
+  SgCarry carry;
+  int u4;           // sg_chunk_kernel's gathers in flight (U) at L = 4
+  int u[4];         // U at NCH = 1 (L = 8..32), 2, 4, 8 chunks per lane
+  int minb[4];      // CTAs per SM at NCH = 1, 2, 4, 8
+};
+
+// maxQ: 256 T-columns (1024 floats vectorised, 256 scalar), but 128 on float4 rows for every reduction except the sums
+// (min / max: the big-row fix-up keeps values and indices of every lane group in static shared memory).  The weighted
+// sum and TSUM take the sum's column blocks, so that with all-ones weights (on a symmetric graph) they give the sum's
+// bits at every width (the big-row fix-up groups a row's carries by the block's lane count).  ASTAT's row is one
+// score per head, on scalar rows only.
+// U and MINB are lower than the sum's where a second value held or gathered per float (the min / max index, the
+// min / max backward's index row, s_src, the record, the local row's own row) would otherwise spill under the
+// occupancy.  WSUM keeps the sum's U and holds U weights beside them, so at one chunk per lane it runs three CTAs per
+// SM.  TSUM and TMASK take the shapes of SUM and MASK, but TMASK, which also holds each group's repeated-destination
+// bits, runs three CTAs per SM at one chunk per lane.
+constexpr SgRed SG_REDS[] = {
+    // red           maxQ4 maxQ1 ring fix           heads  carry           u4  u             minb
+    {SG_RED_SUM,     256,  256,  0,   SG_FIX_SUM,   false, SG_CARRY_FLOAT, 4, {8, 4, 2, 1}, {4, 3, 3, 2}},
+    {SG_RED_MAX,     128,  256,  -1,  SG_FIX_OWN,   false, SG_CARRY_INDEX, 4, {4, 4, 1, 1}, {4, 3, 3, 2}},
+    {SG_RED_MIN,     128,  256,  -1,  SG_FIX_OWN,   false, SG_CARRY_INDEX, 4, {4, 4, 1, 1}, {4, 3, 3, 2}},
+    {SG_RED_MASK,    128,  256,  -1,  SG_FIX_SUM,   false, SG_CARRY_FLOAT, 4, {4, 2, 1, 1}, {4, 3, 3, 2}},
+    {SG_RED_ASTAT,   0,    SG_LDC2 / 2, -1, SG_FIX_STATS, false, SG_CARRY_FLOAT, 8, {8, 0, 0, 0}, {4, 0, 0, 0}},
+    {SG_RED_ATTN,    128,  256,  -1,  SG_FIX_SUM,   false, SG_CARRY_FLOAT, 4, {4, 2, 1, 1}, {4, 3, 2, 2}},
+    {SG_RED_ADST,    128,  256,  -1,  SG_FIX_NONE,  true,  SG_CARRY_FLOAT, 4, {4, 2, 1, 1}, {4, 3, 2, 1}},
+    {SG_RED_ASRC,    128,  256,  -1,  SG_FIX_SUM,   true,  SG_CARRY_FLOAT, 2, {2, 2, 1, 1}, {4, 2, 2, 1}},
+    {SG_RED_WSUM,    256,  256,  -1,  SG_FIX_SUM,   false, SG_CARRY_FLOAT, 8, {8, 4, 2, 1}, {3, 3, 3, 2}},
+    {SG_RED_EDOT,    128,  256,  -1,  SG_FIX_NONE,  false, SG_CARRY_NONE,  4, {4, 2, 1, 1}, {4, 3, 2, 1}},
+    {SG_RED_TSUM,    256,  256,  4,   SG_FIX_OWN,   false, SG_CARRY_FLOAT, 4, {8, 4, 2, 1}, {4, 3, 3, 2}},
+    {SG_RED_TMASK,   128,  256,  -1,  SG_FIX_SUM,   false, SG_CARRY_FLOAT, 4, {4, 2, 1, 1}, {3, 3, 3, 2}}};
+constexpr bool sg_reds_in_order() {
+  for (int i = 0; i < (int)(sizeof(SG_REDS) / sizeof(SG_REDS[0])); i++)
+    if (SG_REDS[i].red != i) return false;
+  return sizeof(SG_REDS) / sizeof(SG_REDS[0]) == SG_RED_TMASK + 1;
+}
+static_assert(sg_reds_in_order(), "SG_REDS has one row per SG_RED_* value, in order");
+
+constexpr int sg_max_q(int VEC, int RED) { return VEC == 4 ? SG_REDS[RED].maxQ4 : SG_REDS[RED].maxQ1; }
+constexpr int sg_nch_index(int NCH) { return NCH == 1 ? 0 : NCH == 2 ? 1 : NCH == 4 ? 2 : 3; }
+constexpr int sg_chunk_u(int RED, int L, int NCH) { return L == 4 ? SG_REDS[RED].u4 : SG_REDS[RED].u[sg_nch_index(NCH)]; }
+constexpr int sg_chunk_minb(int RED, int NCH) { return SG_REDS[RED].minb[sg_nch_index(NCH)]; }
+
 // sg_chunk_kernel_t's two shapes, the measured defaults (DESIGN.md §3.1), four workers per CTA: rows of 65..128 floats
 // (one float4 per lane) with lane-held ids and two stages of two four-row units per worker; rows of 129..256 floats
-// with the ids loaded per stage and two stages of one unit.  TS: the TSUM form.
-template <int NCH, bool TS>
+// with the ids loaded per stage and two stages of one unit.
+template <int NCH, int RED>
 static int launch_ring(const SgParams& p, cudaStream_t st) {
   constexpr int L = 32, P = 2, NT = 128;
-  constexpr int S = NCH == 1 ? 2 : 1, MINB = NCH == 1 ? 4 : 6, MODE = (NCH == 1 ? 2 : 0) | (TS ? 4 : 0);
+  constexpr int S = NCH == 1 ? 2 : 1, MINB = NCH == 1 ? 4 : 6, MODE = (NCH == 1 ? 2 : 0) | SG_REDS[RED].ring;
   constexpr int WPB = NT / L;
   constexpr size_t smem = (size_t)WPB * P * S * 4 * NCH * L * 16 + (size_t)WPB * P * 8;
   static std::atomic<uint64_t> configured{0};
@@ -1271,18 +1337,8 @@ static int launch_ring(const SgParams& p, cudaStream_t st) {
   const uint32_t grid = (p.numChunks + WPB - 1) / WPB;
   sg_chunk_kernel_t<L, NCH, S, P, NT, MINB, MODE><<<grid, NT, smem, st>>>(p);
   ROC_LAUNCH_CHECK();
-  note_launch(ROC_SG_LAUNCH_RING, TS ? SG_RED_TSUM : SG_RED_SUM, 4, L, NCH, grid);
+  note_launch(ROC_SG_LAUNCH_RING, RED, 4, L, NCH, grid);
   return ROC_OK;
-}
-
-// The widest row, in T-columns, that one launch of RED takes: 256 (1024 floats vectorised, 256 scalar; wider rows are
-// split into column blocks), but 128 on float4 rows for every reduction except the sums (min / max: the big-row
-// fix-up keeps values and indices of every lane group in static shared memory).  The weighted sum and TSUM take the
-// sum's column blocks, so that with all-ones weights (on a symmetric graph) they give the sum's bits at every width
-// (the big-row fix-up groups a row's carries by the block's lane count).  ASTAT's row is one score per head.
-constexpr int sg_max_q(int VEC, int RED) {
-  return RED == SG_RED_ASTAT ? SG_LDC2 / 2
-         : (VEC == 4 && RED != SG_RED_SUM && RED != SG_RED_WSUM && RED != SG_RED_TSUM) ? 128 : 256;
 }
 
 // The row shape of every launch: calls f(L, NCH), as std::integral_constants, for rows of Q T-columns.  L is the
@@ -1299,36 +1355,6 @@ static int with_shape(uint32_t Q, F&& f) {
     return with_shape<QMAX, 2 * QC>(Q, f);
   }
 }
-
-// Gathers in flight (U) and CTAs per SM (MINB) of sg_chunk_kernel, per reduction at NCH = 1, 2, 4, 8 chunks per lane.
-// They are lower than the sum's where a second value held or gathered per float (the min / max index, the min / max
-// backward's index row, s_src, the record, the local row's own row) would otherwise spill under the occupancy.
-// WSUM keeps the sum's U and holds U weights beside them, so at one chunk per lane it runs three CTAs per SM.
-// TSUM and TMASK take the shapes of SUM and MASK, but TMASK, which also holds each group's repeated-destination bits,
-// runs three CTAs per SM at one chunk per lane.
-constexpr int SG_SHAPE_U[12][4] = {
-    {8, 4, 2, 1},   // SUM (U = 4 at L = 4)
-    {4, 4, 1, 1},   // MAX
-    {4, 4, 1, 1},   // MIN
-    {4, 2, 1, 1},   // MASK
-    {8, 0, 0, 0},   // ASTAT (one chunk: Q = heads)
-    {4, 2, 1, 1},   // ATTN
-    {4, 2, 1, 1},   // ADST
-    {2, 2, 1, 1},   // ASRC
-    {8, 4, 2, 1},   // WSUM
-    {4, 2, 1, 1},   // EDOT
-    {8, 4, 2, 1},   // TSUM (U = 4 at L = 4)
-    {4, 2, 1, 1}};  // TMASK
-constexpr int SG_SHAPE_MINB[12][4] = {
-    {4, 3, 3, 2}, {4, 3, 3, 2}, {4, 3, 3, 2}, {4, 3, 3, 2}, {4, 0, 0, 0}, {4, 3, 2, 2}, {4, 3, 2, 1}, {4, 2, 2, 1},
-    {3, 3, 3, 2}, {4, 3, 2, 1}, {4, 3, 3, 2}, {3, 3, 3, 2}};
-static_assert(SG_RED_MAX == 1 && SG_RED_MIN == 2 && SG_RED_TMASK == 11,
-              "SG_SHAPE_U / SG_SHAPE_MINB rows follow the SG_RED_* values");
-constexpr int sg_nch_index(int NCH) { return NCH == 1 ? 0 : NCH == 2 ? 1 : NCH == 4 ? 2 : 3; }
-constexpr int sg_chunk_u(int RED, int L, int NCH) {
-  return (RED == SG_RED_SUM || RED == SG_RED_TSUM) && L == 4 ? 4 : SG_SHAPE_U[RED][sg_nch_index(NCH)];
-}
-constexpr int sg_chunk_minb(int RED, int NCH) { return SG_SHAPE_MINB[RED][sg_nch_index(NCH)]; }
 
 // The fix-ups of the rows a main kernel cut, reduced by FIX over p's out / carry: one worker per heavy row, one CTA
 // per big row.  `heads`: p holds an attention gather's heads-wide partials.
@@ -1349,19 +1375,18 @@ static int launch_fixups(const SgParams& p, cudaStream_t st, bool heads = false)
   return ROC_OK;
 }
 
-// One ScatterGather launch: the main kernel (sg_chunk_kernel_t for the vectorised sum of 17..64 T-columns, which is
-// faster there on a products-shaped graph, DESIGN.md §3.1; for TSUM too), then the fix-ups of the rows it cut.  MAX /
-// MIN and TSUM (whose epilogue divides by the in-degree) have their own; ASTAT's stats have sg_attn_stat_fixup; the
-// H-wide partials of the others are sums (the min / max backwards' and the attention gathers'), finished by the sum's.  ADST and ASRC then finish their heads-wide partials with the sum's
-// fix-ups on p2, p with out2 / carry2 as a VEC = 1, Q = heads output.
+// One ScatterGather launch: the main kernel (sg_chunk_kernel_t for the ring reductions' vectorised rows of 17..64
+// T-columns, where it is faster on a products-shaped graph, DESIGN.md §3.1), then the fix-ups of the rows it cut, as
+// the reduction's row of SG_REDS says.  Heads-wide partials are finished by the sum's fix-ups on p2, p with
+// out2 / carry2 as a VEC = 1, Q = heads output.
 template <int VEC, int RED, int L, int NCH>
 static int launch(const SgParams& p, cudaStream_t st) {
-  constexpr bool RING = VEC == 4 && (RED == SG_RED_SUM || RED == SG_RED_TSUM) && L == 32 && NCH <= 2;
+  constexpr SgRed R = SG_REDS[RED];
   constexpr int WPB = SG_THREADS / L;
   int rc = ROC_OK;
   if (p.numChunks) {
-    if constexpr (RING) {
-      if ((rc = launch_ring<NCH, RED == SG_RED_TSUM>(p, st)) != ROC_OK) return rc;
+    if constexpr (VEC == 4 && R.ring >= 0 && L == 32 && NCH <= 2) {
+      if ((rc = launch_ring<NCH, RED>(p, st)) != ROC_OK) return rc;
     } else {
       const uint32_t grid = (p.numChunks + WPB - 1) / WPB;
       sg_chunk_kernel<VEC, L, NCH, sg_chunk_u(RED, L, NCH), sg_chunk_minb(RED, NCH), RED><<<grid, SG_THREADS, 0, st>>>(p);
@@ -1369,19 +1394,18 @@ static int launch(const SgParams& p, cudaStream_t st) {
       note_launch(ROC_SG_LAUNCH_MAIN, RED, VEC, L, NCH, grid);
     }
   }
-  if constexpr (RED == SG_RED_ASTAT) {
+  if constexpr (R.fix == SG_FIX_STATS) {
     const uint32_t rows = p.numHeavy + p.numBig;
     if (rows) {
       const uint32_t grid = (rows + SG_THREADS / 32 - 1) / (SG_THREADS / 32);
       sg_attn_stat_fixup<<<grid, SG_THREADS, 0, st>>>(p);
       ROC_LAUNCH_CHECK();
-      note_launch(ROC_SG_LAUNCH_STAT_FIXUP, SG_RED_ASTAT, 1, 32, 1, grid);
+      note_launch(ROC_SG_LAUNCH_STAT_FIXUP, RED, 1, 32, 1, grid);
     }
-  } else if constexpr (RED != SG_RED_ADST && RED != SG_RED_EDOT) {   // EDOT's outputs are per edge: nothing carried
-    constexpr int FIX = (RED == SG_RED_MAX || RED == SG_RED_MIN || RED == SG_RED_TSUM) ? RED : SG_RED_SUM;
-    if ((rc = launch_fixups<VEC, L, NCH, FIX>(p, st)) != ROC_OK) return rc;
+  } else if constexpr (R.fix != SG_FIX_NONE) {
+    if ((rc = launch_fixups<VEC, L, NCH, R.fix == SG_FIX_OWN ? RED : SG_RED_SUM>(p, st)) != ROC_OK) return rc;
   }
-  if constexpr (RED == SG_RED_ADST || RED == SG_RED_ASRC) {
+  if constexpr (R.headsFix) {
     SgParams p2 = p;
     p2.out = p.out2; p2.ldOut = p.ldOut2; p2.carry = p.carry2; p2.ldC = SG_LDC2; p2.Q = p.heads;
     rc = launch_fixups<1, 8, 1, SG_RED_SUM>(p2, st, true);
@@ -1653,20 +1677,20 @@ struct SgEdge {
   const roc_eid_t* rowEnd = nullptr;
 };
 
-// Reduction RED over the columns [0, H) of every row, in column blocks: 1,024 floats for the sum and the weighted sum
-// and 512 for the others when every leading dimension and pointer allows float4 rows, else 256.  `arg` holds the min / max indices
+// Reduction RED over the columns [0, H) of every row, in column blocks of the widest row one launch takes (SG_REDS),
+// on float4 rows when every leading dimension and pointer allows them.  `arg` holds the min / max indices
 // (written by the forward, gathered by the backward); the sum passes none.  EDOT's column blocks add their partial
 // dot products to dw in block order: the first overwrites it (or adds, with ed.accumulate), the later ones add.
 template <int RED>
 static int run_planned(roc_sg_plan* pl, int H, const float* in, int64_t ldIn, float* out, int64_t ldOut,
                        const roc_vid_t* arg, int64_t ldArg, int epilogue, roc_vid_t selfBase, cudaStream_t st,
                        const SgEdge& ed = SgEdge()) {
+  constexpr SgCarry CARRY = SG_REDS[RED].carry;
   const bool vec = float4_rows({in, out, arg, ed.g}, {ldIn, ldOut, ldArg, ed.ldG});
-  const int blockCols = !vec ? 256 : (RED == SG_RED_SUM || RED == SG_RED_WSUM || RED == SG_RED_TSUM) ? 1024 : 512;
-  // EDOT carries nothing
-  int rc = RED == SG_RED_EDOT ? ROC_OK : grow_carries(pl, std::min(H, blockCols), st);
+  const int blockCols = vec ? 4 * sg_max_q(4, RED) : sg_max_q(1, RED);
+  int rc = CARRY == SG_CARRY_NONE ? ROC_OK : grow_carries(pl, std::min(H, blockCols), st);
   // the min / max forward's index carries, which the kernels address with the float carries' leading dimension
-  if (rc == ROC_OK && (RED == SG_RED_MAX || RED == SG_RED_MIN))
+  if (rc == ROC_OK && CARRY == SG_CARRY_INDEX)
     rc = grow(pl->carryArg, pl->carryArgBytes, (size_t)pl->numCarries * pl->carryLd * sizeof(uint32_t), st);
   if (rc != ROC_OK) return rc;
   for (int c0 = 0; c0 < H; c0 += blockCols) {

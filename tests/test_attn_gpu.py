@@ -16,16 +16,13 @@ from roc_b200 import _lib, datasets
 from roc_b200 import kernels as K
 from roc_b200.model import Host, Model, build_gat
 from sg_graphs import graph, to_dev
+from sg_matrix import close_terms, valid_heads
 import witness_gat as wg
 from witness_gat import gat_witness
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
 SLOPE = 0.2
-
-
-def valid_heads(h):
-    return [k for k in (1, 2, 4, 8) if k == 1 or (h % k == 0 and (h // k) >= 4 and (h // k) & (h // k - 1) == 0)]
 
 
 def bits(t):
@@ -46,16 +43,6 @@ def dev(a, vec):
     t.copy_(torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32)))
     assert (t.stride(0) % 4 == 0) == vec
     return t
-
-
-def close_terms(got, want, mag, what, eps):
-    """The parity bar, plus `eps` of the magnitude of the summed terms (`mag`: the same sums over |terms|).  A sum
-    whose terms cancel is only good to its rounding relative to them, not to the result."""
-    err = np.abs(np.asarray(got, dtype=np.float64) - want)
-    bound = 1e-4 * np.abs(want) + 1e-5 * np.abs(want).max() + eps * mag + 1e-30
-    bad = err > bound
-    assert not bad.any(), "%s: %d/%d elements off; worst err %.3e at %s" % (
-        what, int(bad.sum()), bad.size, float(err.max()), np.unravel_index((err - bound).argmax(), err.shape))
 
 
 def check(plan, row_end, col, x, s, g, heads, vec, what, self_base=0, col_left=0, full=None, eps_a=0.0):

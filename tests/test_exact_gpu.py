@@ -17,97 +17,16 @@ import exact_oracle as xo
 import minmax_oracle as mmo
 from roc_b200 import _lib
 from roc_b200 import kernels as K
-from test_attn_gpu import close_terms, valid_heads
-from test_sg_matrix_gpu import (ADST, ASRC, CH, MASK, NORM, RELU, RUNGS, SCALAR, SLOPE, SUM, Guarded, cdiv, dev_in,
-                                exact, guarded, no_new_nan, scores_dev, shape)
-from test_weighted_gpu import WGraph, symmetric_sorted, wgraphs
+from sg_matrix import (DEV, NORM, RELU, SCALAR, SLOPE, SUM, TMASK, TSUM, Guarded, WGraph, attn_backward, check_bits,
+                       close_terms, dev_in, every_instantiation, exact, guarded, launches, no_new_nan, planned,
+                       same_bits, scores_dev, symmetric_sorted, valid_heads, xgraphs)
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda"
-TSUM, TMASK = 10, 11
 SUM_V = [1, 16, 17, 32, 33, 64, 65, 128, 129, 256, 257, 1024, 1025, 2051]
 MM_V = [1, 16, 17, 32, 33, 64, 65, 128, 129, 256, 257, 512, 513, 700]
 ATTN_V = [1, 16, 17, 32, 33, 64, 65, 128, 129, 256, 257, 512]
 ATTN_S = [1, 4, 5, 8, 9, 16, 17, 32, 33, 64, 65, 128, 129, 256]
 SEEN, RAN = set(), set()
-
-_G = None
-
-
-def xgraphs():
-    """Every whole graph of test_weighted_gpu.wgraphs() plus the fan-out graph."""
-    global _G
-    if _G is None:
-        _G = {k: g for k, g in wgraphs().items() if g.whole}
-        n = 4000
-        rng = np.random.RandomState(17)
-        deg = rng.randint(0, 4, size=n)
-        deg[:3000] += 1                                      # rows 0..2999 each take an edge from the hub 3999
-        deg[3000:3100] = 0
-        col = []
-        for r in range(n):
-            k = int(deg[r])
-            srcs = list(rng.randint(0, 3000, size=k - 1 if r < 3000 else k)) + ([3999] if r < 3000 else [])
-            rng.shuffle(srcs)
-            col += srcs
-        _G["fanout"] = WGraph("fanout", np.cumsum(deg).astype(np.uint64), np.array(col, np.uint32), n)
-        assert _G["fanout"].sched_t[2] >= 1                 # a big transposed row
-    return _G
-
-
-def launches(what, want):
-    got = [(l["kind"], l["red"], l["vec"], l["lanes"], l["nch"], l["grid"]) for l in K.sg_launches()]
-    assert got == want, "%s: launched\n  %s\nexpected\n  %s" % (what, got, want)
-    SEEN.update(x[:5] for x in got)
-
-
-def fixups(sched, fix, vec, lanes, nch, heads=False):
-    _, heavy, big = sched
-    out = []
-    if heavy:
-        out.append(("heads_fixup" if heads else "fixup", fix, vec, lanes, nch, cdiv(heavy, 256 // lanes)))
-    if big:
-        out.append(("heads_big_fixup" if heads else "big_fixup", fix, vec, lanes, nch, big))
-    return out
-
-
-def main_launch(sched, red, vec, q):
-    lanes, nch = shape(q)
-    if vec == 4 and red in (SUM, TSUM) and lanes == 32 and nch <= 2:
-        return [("ring", red, 4, 32, nch, cdiv(sched[0], 4))]
-    return [("main", red, vec, lanes, nch, cdiv(sched[0], 256 // lanes))]
-
-
-def expect(sched, red, vec, h):
-    """The sums and the max / min backward over the transposed plan: per column block the main kernel, then the
-    fix-ups (TSUM's own; the max / min backward's are the sum's)."""
-    vw = 4 if vec else 1
-    block = 256 if not vec else 1024 if red in (SUM, TSUM) else 512
-    want = []
-    for c0 in range(0, h, block):
-        q = cdiv(min(h - c0, block), vw)
-        want += main_launch(sched, red, vw, q) + fixups(sched, TSUM if red == TSUM else SUM, vw, *shape(q))
-    return want
-
-
-def expect_attn(g, vec, h, heads):
-    vw = 4 if vec else 1
-    q = cdiv(h, vw)
-    lanes, nch = shape(q)
-    want = [("record", -1, vw, lanes, nch, cdiv(g.n, 256 // lanes))]
-    want += main_launch(g.sched, ADST, vw, q) + fixups(g.sched, SUM, 1, 8, 1, heads=True)
-    want += main_launch(g.sched_t, ASRC, vw, q) + fixups(g.sched_t, SUM, vw, lanes, nch)
-    return want + fixups(g.sched_t, SUM, 1, 8, 1, heads=True)
-
-
-def bits_same(a, b, what):
-    assert np.array_equal(a.bits(), b.bits()), "%s: a repeated call gave different bits" % what
-
-
-def check_bits(got, want, what):
-    bad = ~((got == want) | (np.isnan(got) & np.isnan(want)))
-    assert not bad.any(), "%s: %d/%d elements differ from the exact reference, first at %s (%r vs %r)" % (
-        what, int(bad.sum()), bad.size, np.argwhere(bad)[0], got[bad][0], want[bad][0])
 
 
 # --------------------------------------------------------------------------------------------------------- calls ---
@@ -116,9 +35,9 @@ def sum_call(g, gd, h, vec, epi, what):
     for _ in range(2):
         o = guarded(g.n, h, vec)
         g.tr.sum_backward(gd, epilogue=epi, row_end=g.d_re if epi & NORM else None, out=o.view)
-        launches(what, expect(g.sched_t, TSUM if epi & NORM else SUM, vec, h))
+        launches(what, planned(g.sched_t, TSUM if epi & NORM else SUM, vec, h), SEEN)
         outs.append(o)
-    bits_same(outs[0], outs[1], what)
+    same_bits(outs[0], outs[1], what)
     outs[0].check_guards(what)
     return outs[0].host()
 
@@ -128,9 +47,9 @@ def minmax_call(g, gd, arg, h, vec, what):
     for _ in range(2):
         o = guarded(g.n, h, vec)
         g.tr.minmax_backward(gd, arg, out=o.view)
-        launches(what, expect(g.sched_t, TMASK, vec, h))
+        launches(what, planned(g.sched_t, TMASK, vec, h), SEEN)
         outs.append(o)
-    bits_same(outs[0], outs[1], what)
+    same_bits(outs[0], outs[1], what)
     outs[0].check_guards(what)
     return outs[0].host()
 
@@ -140,10 +59,10 @@ def attn_call(g, xd, sd, od, std, gd, heads, h, vec, what):
     for _ in range(2):
         ig, sg = guarded(g.n, h, vec), Guarded(g.n, 2 * heads, 2 * heads + 4, 2 * heads)
         g.tr.attn_backward(g.plan, xd, sd, od, std, gd, heads, SLOPE, in_grad=ig.view, score_grad=sg.view)
-        launches(what, expect_attn(g, vec, h, heads))
+        launches(what, attn_backward(g.sched, g.sched_t, vec, h, g.n), SEEN)
         runs.append((ig, sg))
     for a, b in zip(*runs):
-        bits_same(a, b, what)
+        same_bits(a, b, what)
         a.check_guards(what)
     return runs[0][0].host(), runs[0][1].host()
 
@@ -371,22 +290,11 @@ def test_refusals():
 
 
 # ----------------------------------------------------------------------------------------------------- coverage ---
-def every_instantiation():
-    want = set()
-    for vec in (4, 1):
-        for qc, lanes, nch in RUNGS:
-            ring = vec == 4 and lanes == 32 and nch <= 2
-            want.add(("ring" if ring else "main", TSUM, vec, lanes, nch))
-            want |= {(k, TSUM, vec, lanes, nch) for k in ("fixup", "big_fixup")}
-            if qc <= (128 if vec == 4 else 256):
-                want.add(("main", TMASK, vec, lanes, nch))
-    return want
-
-
 def test_exact_covered():
     wanted = {(k, v, h) for k, ws in (("sum", SUM_V), ("minmax", MM_V), ("attn", ATTN_V)) for v, hs in
               ((True, ws), (False, ATTN_S if k == "attn" else SCALAR)) for h in hs}
     if not wanted <= RAN:
         pytest.skip("%d of the matrix cases did not run in this process" % len(wanted - RAN))
-    missing = every_instantiation() - SEEN
+    # TMASK's fix-ups are the sum's, which test_sg_matrix_gpu covers
+    missing = {x for x in every_instantiation((TSUM, TMASK)) if x[1] != SUM} - SEEN
     assert not missing, "never launched: %s" % sorted(missing)

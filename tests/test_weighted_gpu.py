@@ -1,6 +1,6 @@
 """Edge-weighted ScatterGather on the GPU: the weighted forward, its transposed backward and the edge-weight gradient
 (include/roc_b200.h) at both ends of every rung of the row-shape table and past the widest in column blocks, on every
-graph of the ScatterGather matrix (test_sg_matrix_gpu.py) and on directed graphs with duplicate edges and nodes with
+graph of the ScatterGather matrix (sg_matrix.py) and on directed graphs with duplicate edges and nodes with
 no out-edge.
 
 Exact data: features are multiples of 1/16 in [-8, 8], weights multiples of 1/2 in [-4, 4], the gradients of the
@@ -19,79 +19,13 @@ import weighted_oracle as wo
 from roc_b200 import _lib
 from roc_b200 import kernels as K
 from sg_graphs import to_dev
-from test_sg_matrix_gpu import (CH, BIG, RUNGS, SCALAR, SUM, Guarded, cdiv, dev_in, exact, graphs, guarded, shape)
+from sg_matrix import (DEV, EDOT, SCALAR, SENT_F, WSUM, WGraph, dev_in, every_instantiation, exact, guarded, launches,
+                       planned, same_bits, symmetric_sorted, weighted_backward, wgraphs)
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda"
-WSUM, EDOT = 8, 9
 VEC_W = [1, 16, 17, 32, 33, 64, 65, 128, 129, 256, 257, 512, 513, 700, 1024, 1025, 1100, 2051]
-SENT = -1234.5
 SEEN = set()
 RAN = set()
-
-
-# ------------------------------------------------------------------------------------------------------ graphs ---
-def schedule(row_end, col_left=0):
-    """(chunks, heavy, big) of a plan over row_end, from the definitions in sg.cu."""
-    t = np.asarray(row_end, dtype=np.int64) - col_left
-    s = np.concatenate([[0], t[:-1]])
-    deg = t - s
-    carries = np.where(deg > CH, (t - 1) // CH - s // CH, 0)
-    e = int(t[-1]) if t.shape[0] else 0
-    return e // CH + 1, int(((deg > CH) & (carries <= BIG)).sum()), int((carries > BIG).sum())
-
-
-class WGraph:
-    """A graph of the matrix (or a new one) with its transpose when it is a whole graph."""
-
-    def __init__(self, name, row_end, col, n, row_left=0, col_left=0, plan=None):
-        self.name, self.n, self.row_left, self.col_left = name, n, row_left, col_left
-        self.row_end, self.col = np.asarray(row_end, np.uint64), np.asarray(col, np.uint32)
-        self.nloc, self.E = self.row_end.shape[0], self.col.shape[0]
-        self.d_re, self.d_col = to_dev(self.row_end, self.col)
-        self.plan = plan or K.SgPlan(row_left, row_left + self.nloc - 1, col_left, self.d_re, self.d_col)
-        self.sched = schedule(self.row_end, col_left)
-        self.whole = row_left == 0 and col_left == 0 and self.nloc == n
-        self.tr = None
-        if self.whole:
-            self.tr = K.SgTranspose(self.d_re, self.d_col)
-            self.re_t, self.col_t, self.perm = wo.transpose(self.row_end, self.col, n)
-            self.sched_t = schedule(self.re_t)
-        self.deg = np.diff(np.concatenate([[0], self.row_end.astype(np.int64) - col_left]))
-
-
-def directed_dup(n, e, seed):
-    rng = np.random.RandomState(seed)
-    dst = np.sort(rng.randint(0, n, size=e))
-    src = rng.randint(0, n - 3, size=e)                     # the last three nodes have no out-edge
-    src[1::3] = src[0::3][:src[1::3].shape[0]]              # duplicate edges
-    dst[:200] = 5                                           # one heavy row of duplicates
-    dst = np.sort(dst)
-    order = np.lexsort((src, dst))
-    return np.cumsum(np.bincount(dst, minlength=n)).astype(np.uint64), src[order].astype(np.uint32)
-
-
-_G = None
-
-
-def wgraphs():
-    global _G
-    if _G is None:
-        _G = {}
-        for g in graphs().values():
-            _G[g.name] = WGraph(g.name, g.row_end, g.col, g.n, g.row_left, g.col_left, plan=g.plan)
-        _G["directed"] = WGraph("directed", *directed_dup(3000, 40000, 21), 3000)
-        hub = np.zeros(300, dtype=np.int64)
-        hub[7] = 4000                                       # a hub whose sources fan out: long transposed rows too
-        re_ = np.cumsum(hub).astype(np.uint64)
-        col = np.random.RandomState(3).randint(0, 40, size=4000).astype(np.uint32)
-        _G["hub"] = WGraph("hub", re_, col, 300)
-        d = _G["directed"]
-        assert d.re_t[-1] == d.re_t[-4]                     # empty transposed rows
-        dst = np.repeat(np.arange(d.n), d.deg)
-        pairs = dst.astype(np.int64) * d.n + d.col
-        assert np.unique(pairs).shape[0] < pairs.shape[0]  # duplicate (dst, src) edges
-    return _G
 
 
 # --------------------------------------------------------------------------------------------------------- data ---
@@ -121,45 +55,6 @@ def test_exact_bound():
     assert (max(VEC_W) * 1 * 8 + 4) * 256 < 2 ** 24        # |gy| <= 1, |x| <= 8, granularity 1/256, |dw0| <= 4
 
 
-# ------------------------------------------------------------------------------------------------- launch lists ---
-def launches(what, want):
-    got = [(l["kind"], l["red"], l["vec"], l["lanes"], l["nch"], l["grid"]) for l in K.sg_launches()]
-    assert got == want, "%s: launched\n  %s\nexpected\n  %s" % (what, got, want)
-    SEEN.update(x[:5] for x in got)
-
-
-def expect(sched, red, vec, h):
-    chunks, heavy, big = sched
-    vw = 4 if vec else 1
-    block = (1024 if red == WSUM else 512) if vec else 256
-    want = []
-    for c0 in range(0, h, block):
-        lanes, nch = shape(cdiv(min(h - c0, block), vw))
-        want.append(("main", red, vw, lanes, nch, cdiv(chunks, 256 // lanes)))
-        if red == WSUM:
-            if heavy:
-                want.append(("fixup", SUM, vw, lanes, nch, cdiv(heavy, 256 // lanes)))
-            if big:
-                want.append(("big_fixup", SUM, vw, lanes, nch, big))
-    return want
-
-
-def expect_bwd(g, vec, h):
-    pre = [("permute", -1, 1, 1, 1, cdiv(g.E, 256))] if g.E else []
-    return pre + expect(g.sched_t, WSUM, vec, h)
-
-
-def every_instantiation():
-    want = set()
-    for vec, qmax in ((4, 256), (1, 256)):
-        for qc, lanes, nch in RUNGS:
-            if qc <= qmax:
-                want |= {("main", WSUM, vec, lanes, nch)} | {(k, SUM, vec, lanes, nch) for k in ("fixup", "big_fixup")}
-            if qc <= (128 if vec == 4 else 256):
-                want.add(("main", EDOT, vec, lanes, nch))
-    return want | {("permute", -1, 1, 1, 1)}
-
-
 # ------------------------------------------------------------------------------------------------------- calls ---
 def bits_equal(a, b):
     return np.array_equal(np.asarray(a, np.float32).view(np.int32), np.asarray(b, np.float32).view(np.int32))
@@ -178,9 +73,9 @@ def fwd(g, xd, wd, h, vec):
     for _ in range(2):
         o = guarded(g.nloc, h, vec)
         g.plan.weighted_forward(xd, wd, out=o.view)
-        launches("%s forward H=%d" % (g.name, h), expect(g.sched, WSUM, vec, h))
+        launches("%s forward H=%d" % (g.name, h), planned(g.sched, WSUM, vec, h), SEEN)
         outs.append(o)
-    assert np.array_equal(outs[0].bits(), outs[1].bits()), "%s forward: repeated call differs" % g.name
+    same_bits(outs[0], outs[1], "%s forward" % g.name)
     outs[0].check_guards("%s forward" % g.name)
     return outs[0].host()
 
@@ -190,9 +85,9 @@ def bwd(g, gd, wd, h, vec):
     for _ in range(2):
         o = guarded(g.n, h, vec)
         g.tr.backward(gd, wd, out=o.view)
-        launches("%s backward H=%d" % (g.name, h), expect_bwd(g, vec, h))
+        launches("%s backward H=%d" % (g.name, h), weighted_backward(g, vec, h), SEEN)
         outs.append(o)
-    assert np.array_equal(outs[0].bits(), outs[1].bits()), "%s backward: repeated call differs" % g.name
+    same_bits(outs[0], outs[1], "%s backward" % g.name)
     outs[0].check_guards("%s backward" % g.name)
     return outs[0].host()
 
@@ -201,13 +96,13 @@ def edot(g, gd, xd, h, vec, dw0=None):
     """dw into a guarded flat buffer; with dw0, accumulated onto it."""
     res = []
     for _ in range(2):
-        buf = torch.full((g.E + 8,), SENT, device=DEV)
+        buf = torch.full((g.E + 8,), SENT_F, device=DEV)
         if dw0 is not None:
             buf[4:4 + g.E] = torch.from_numpy(dw0[:g.E]).to(DEV)
         g.plan.edge_dot(gd, xd, dw=buf[4:], accumulate=dw0 is not None)
-        launches("%s edge dot H=%d" % (g.name, h), expect(g.sched, EDOT, vec, h))
+        launches("%s edge dot H=%d" % (g.name, h), planned(g.sched, EDOT, vec, h), SEEN)
         b = buf.cpu().numpy()
-        assert bits_equal(b[:4], [SENT] * 4) and bits_equal(b[4 + g.E:], [SENT] * 4), "%s edge dot: guards" % g.name
+        assert bits_equal(b[:4], [SENT_F] * 4) and bits_equal(b[4 + g.E:], [SENT_F] * 4), "%s edge dot: guards" % g.name
         res.append(b[4:4 + g.E])
     assert bits_equal(res[0], res[1]), "%s edge dot: repeated call differs" % g.name
     return res[0]
@@ -288,15 +183,6 @@ def test_all_ones_is_the_sum(h):
             g.plan.forward(xd, out=b.view)
             assert np.array_equal(a.bits(), b.bits()), "%s H=%d: the all-ones weighted sum differs from the sum" % (
                 g.name, h)
-
-
-def symmetric_sorted(n, p, seed):
-    rng = np.random.RandomState(seed)
-    a = rng.rand(n, n) < p
-    a = a | a.T
-    a[:40, :40] = True                                      # heavy rows
-    return (np.cumsum(a.sum(axis=1)).astype(np.uint64),
-            np.concatenate([np.nonzero(a[i])[0] for i in range(n)]).astype(np.uint32))
 
 
 @pytest.mark.parametrize("h", [5, 64, 200, 602])
@@ -390,6 +276,7 @@ def test_weighted_covered():
     wanted = {("vec", h) for h in VEC_W} | {("scalar", h) for h in SCALAR}
     if not wanted <= RAN:
         pytest.skip("%d of the matrix cases did not run in this process" % len(wanted - RAN))
-    missing = every_instantiation() - SEEN
+    want = every_instantiation((WSUM, EDOT)) | {("permute", -1, 1, 1, 1)}
+    missing = want - SEEN
     assert not missing, "never launched: %s" % sorted(missing)
-    assert SEEN <= every_instantiation(), "launched outside the table: %s" % sorted(SEEN - every_instantiation())
+    assert SEEN <= want, "launched outside the table: %s" % sorted(SEEN - want)

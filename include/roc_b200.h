@@ -559,10 +559,15 @@ int roc_last_gemm_path(int which);
  *   grid_x/y  forward / dX: persistent CTAs along the rows x N tiles;  dW: splits x 128-column M tiles
  *   stages    depth of the TMA ring (dW: 32-vertex slots)
  *   splits, v_per_split   dW only: split-K ranges and the rows each holds (the partials are added in range order)
+ *   w_resident  forward / dX: 1 when the CTA's W_hi / W_lo slice is loaded into shared memory once (the ring carries
+ *             only the streaming operand), 0 when W streams through the ring with it
+ *   epi_bufs  forward / dX: shared-memory buffers of the epilogue operands (relu-mask source, output-mask words) the
+ *             producer loads ahead of each tile: 0 when the epilogue has none, else 1 or 2
  * Returns ROC_ERR_INVALID for a bad `which` or a NULL `info`. */
 typedef struct {
   int path, nc, epi, grid_x, grid_y, stages, splits;
   int64_t v_per_split;
+  int w_resident, epi_bufs;
 } roc_gemm_info;
 int roc_last_gemm_info(int which, roc_gemm_info* info);
 

@@ -38,7 +38,8 @@ class LinearBwdArgs(C.Structure):
 class GemmInfo(C.Structure):
     """roc_gemm_info (include/roc_b200.h): how the last Linear GEMM of one kind was launched."""
     _fields_ = [("path", C.c_int), ("nc", C.c_int), ("epi", C.c_int), ("grid_x", C.c_int), ("grid_y", C.c_int),
-                ("stages", C.c_int), ("splits", C.c_int), ("v_per_split", C.c_int64)]
+                ("stages", C.c_int), ("splits", C.c_int), ("v_per_split", C.c_int64),
+                ("w_resident", C.c_int), ("epi_bufs", C.c_int)]
 
     def as_dict(self):
         return {k: getattr(self, k) for k, _ in self._fields_}

@@ -17,13 +17,22 @@
 // so the tile crosses shared memory once.  W_hi / W_lo come from shared memory (K-major,
 // 128-byte swizzle).  One persistent CTA per SM (x N-tiles of <= 128 columns in grid.y):
 //   warps 0-7  two consumer warpgroups, 64 rows of the 128-row tile each: fragment load,
-//              [dropout mask ->] hi/lo split, 3 x wgmma m64n32k8 per 32-column chunk and k8
-//              step, then the epilogue (relu / dropout-backward mask / relu mask / row norm /
-//              accumulate) straight from the accumulator registers
-//   warp 8     TMA producer (A tile [128 rows][32 k] + W_hi + W_lo tile per stage)
-// HBM-bound on A (rows*K*4 bytes read once); W (tens of KB) stays in L2.
+//              [dropout mask ->] hi/lo split, per k8 step one wgmma m64n(32 NC)k8 per operand pair,
+//              then the epilogue (relu / dropout-backward mask / relu mask / row norm / accumulate)
+//              from the accumulator registers
+//   warp 8     TMA producer: per tile the epilogue operands (reluOf boxes and output-mask words, into
+//              one of 1 or 2 buffers), then per k-block the A tile [128 rows][32 k], with W_hi + W_lo
+//              of the k-block when W does not stay resident
+// The mainloop keeps two k-blocks of MMAs in flight: the fragments of k-block kb and kb - 1 live in two
+// register sets, `wgmma.wait_group 1` after kb's issue retires kb - 1 and frees its stage, and the queue
+// drains only at the end of a tile.  The input-mask words are loaded a k-block ahead of their use and the
+// row-norm divisors at the top of the tile, so no global load waits in front of an MMA.
+// When the CTA's W_hi / W_lo slice (2 * 32 NC * Kpad floats) fits beside the epilogue buffers and a ring
+// of TC_RES_MIN_STAGES A stages, it is loaded once per CTA and the ring carries A alone; otherwise W streams
+// through the ring with A, from L2.  HBM-bound on A (rows*K*4 bytes read once).
 #include <cstdio>
 #include <cstdlib>
+#include <cstring>
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -35,6 +44,7 @@ constexpr int TC_BM = 128;        // rows per tile: two consumer warpgroups of 6
 constexpr int TC_BK = 32;         // fp32 per k-block = one 128-byte swizzle row
 constexpr int TC_THREADS = 288;   // 8 consumer warps + 1 producer warp
 constexpr int TC_MAX_STAGES = 8;
+constexpr int TC_RES_MIN_STAGES = 4;  // A stages a resident W must leave room for: 64 KB in flight per SM
 
 // Whi/Wlo[n][k] (n < Npad, k < Kpad, zero padded) = split of B(n, k), where
 //   transposed == 0: B(n, k) = W[n * ldW + k]   (fwd: n = output o, k = input i, ldW = inDim)
@@ -58,10 +68,16 @@ struct TcParams {
   const uint32_t* mask; int64_t ldm; float mscale;      // dropout of A fused into the operand load (NULL = none)
   // epilogue, applied in this order to acc(row, col):
   int relu;                                             //   relu (Linear's activation, linear_kernel.cu:83-104)
-  const uint32_t* omask; int64_t oldm; float oscale;    //   dropout backward: keep ? x * scale : 0
-  const float* reluOf; int64_t ldR;                     //   relu backward: reluOf(row, col) > 0 ? x : 0
+  const uint32_t* omask; float oscale;                  //   dropout backward: keep ? x * scale : 0 (words by TMA)
+  const float* reluOf;                                  //   relu backward: reluOf(row, col) > 0 ? x : 0 (by TMA)
   const uint64_t* rowEnd; uint64_t colLeft;             //   indegree norm: x / sqrtf(deg(row))
   int accumulate;                                       //   Y += x instead of Y = x
+  // shared memory (offsets from the 1024-aligned base): [W_hi | W_lo of every k-block when wres] [ring] [epilogue
+  // operand buffers] [barriers]
+  int wres;                                             // W resident: the ring stages carry only A
+  uint32_t stageOff, stageBytes;
+  uint32_t eOff, eBytes, eMaskOff; int eb;              // eb buffers of eBytes: [NC][128][32] reluOf, [128][4] mask words
+  uint32_t barOff;
 };
 
 // Epilogue stage switches: compile-time when the kernel is instantiated for a fixed combination
@@ -80,53 +96,37 @@ __device__ __forceinline__ float row_norm_divisor(const TcParams& p, int64_t row
   return sqrtf((float)(uint32_t)(p.rowEnd[row] - st));
 }
 
-// Epilogue of two adjacent columns (col even) of one row: the accumulator pair a thread holds.
-template <int EPI>
-__device__ __forceinline__ void tc_store_pair(const TcParams& p, int64_t row, int col, float x0, float x1,
-                                              const RowDiv& rd) {
-  EPI_FLAGS(EPI, p)
+// Y[row][col, col + 1] (+)= x0, x1 (col even): the accumulator pair a thread holds, after the rest of the epilogue
+__device__ __forceinline__ void tc_store_pair(const TcParams& p, bool fAcc, int64_t row, int col, float x0, float x1) {
   if (row >= p.rows || col >= p.outDim) return;
-  const bool two = col + 1 < p.outDim;
   float* y = p.Y + row * p.ldY + col;
-  uint32_t mw = 3u;                 // col is even: col and col + 1 sit in one mask word
-  if (fOmask) mw = __ldg(p.omask + row * p.oldm + (col >> 5)) >> (col & 31);
-  float old[2] = {0.f, 0.f}, ro[2] = {1.f, 1.f};
-  if (fAcc) {
-    if (two) { const float2 o = *reinterpret_cast<const float2*>(y); old[0] = o.x; old[1] = o.y; }
-    else old[0] = y[0];
+  if (col + 1 < p.outDim) {
+    if (fAcc) { const float2 o = *reinterpret_cast<const float2*>(y); x0 = o.x + x0; x1 = o.y + x1; }
+    *reinterpret_cast<float2*>(y) = make_float2(x0, x1);
+  } else {
+    y[0] = fAcc ? y[0] + x0 : x0;
   }
-  if (fReluOf) {
-    const float* rp = p.reluOf + row * p.ldR + col;
-    if (two) { const float2 o = __ldg(reinterpret_cast<const float2*>(rp)); ro[0] = o.x; ro[1] = o.y; }
-    else ro[0] = rp[0];
-  }
-  float v[2] = {x0, x1};
-#pragma unroll
-  for (int k = 0; k < 2; k++) {
-    float x = v[k];
-    if (fRelu) x = relu_nanprop(x);
-    if (fOmask) x = ((mw >> k) & 1u) ? x * p.oscale : 0.f;
-    if (fReluOf) x = (ro[k] > 0.f) ? x : 0.f;
-    if (fNorm) x = rowdiv(x, rd);   // == x / d bit for bit (common.cuh)
-    if (fAcc) x = old[k] + x;
-    v[k] = x;
-  }
-  if (two) *reinterpret_cast<float2*>(y) = make_float2(v[0], v[1]);
-  else y[0] = v[0];
 }
+
+__device__ __forceinline__ void wgmma_wait_1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 
 template <int NC, int EPI>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_tc_linear(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapWhi,
-            const __grid_constant__ CUtensorMap mapWlo, const TcParams p) {
+            const __grid_constant__ CUtensorMap mapWlo, const __grid_constant__ CUtensorMap mapR,
+            const __grid_constant__ CUtensorMap mapM, const TcParams p) {
   constexpr int BN = 32 * NC;
   constexpr uint32_t aBytes = TC_BM * TC_BK * 4;       // 16 KB of A per stage
-  constexpr uint32_t bBytes = BN * TC_BK * 4;
-  constexpr uint32_t stageBytes = aBytes + 2 * bBytes;
+  constexpr uint32_t bBytes = BN * TC_BK * 4;          // one k-block of W_hi (or W_lo)
+  constexpr uint32_t rBytes = TC_BM * 32 * 4;          // one 32-column box of reluOf
+  EPI_FLAGS(EPI, p)
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * stageBytes);   // [stages] TMA landed
-  uint64_t* empty = full + TC_MAX_STAGES;                                                // [stages] consumers done
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.barOff);   // [stages] TMA landed
+  uint64_t* empty = full + TC_MAX_STAGES;                          // [stages] consumers done
+  uint64_t* efull = empty + TC_MAX_STAGES;                         // [eb] epilogue operands landed
+  uint64_t* eempty = efull + 2;                                    // [eb] consumers have read them
+  uint64_t* wfull = eempty + 2;                                    // resident W landed
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t numTiles = (p.rows + TC_BM - 1) / TC_BM;
@@ -134,23 +134,53 @@ k_tc_linear(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&mapA); tma_prefetch_desc(&mapWhi); tma_prefetch_desc(&mapWlo);
+    if (fReluOf) tma_prefetch_desc(&mapR);
+    if (fOmask) tma_prefetch_desc(&mapM);
     for (int s = 0; s < p.stages; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
+    for (int e = 0; e < p.eb; e++) { mbar_init(&efull[e], 1); mbar_init(&eempty[e], 8); }
+    mbar_init(wfull, 1);
     fence_barrier_init();
   }
   __syncthreads();
 
   if (warp == 8) {
     // ================================ TMA producer ================================
+    if (p.wres) {
+      if (elect_one()) {
+        mbar_arrive_expect_tx(wfull, 2u * p.numKb * bBytes);
+        for (int kb = 0; kb < p.numKb; kb++) {
+          tma_load_2d(smem + (size_t)kb * bBytes, &mapWhi, kb * TC_BK, n0, wfull);
+          tma_load_2d(smem + (size_t)(p.numKb + kb) * bBytes, &mapWlo, kb * TC_BK, n0, wfull);
+        }
+      }
+      __syncwarp();
+    }
     int s = 0; uint32_t ph = 0;
+    int e = 0; uint32_t eph = 0;
     for (int64_t tile = blockIdx.x; tile < numTiles; tile += gridDim.x) {
+      const int r0 = (int)(tile * TC_BM);
+      if (p.eb) {   // the tile's epilogue operands, ahead of its A stages
+        mbar_wait(&eempty[e], eph ^ 1);
+        if (elect_one()) {
+          uint8_t* eb = smem + p.eOff + (size_t)e * p.eBytes;
+          mbar_arrive_expect_tx(&efull[e], p.eBytes);
+          if (fReluOf)
+            for (int c = 0; c < NC; c++) tma_load_2d(eb + c * rBytes, &mapR, n0 + 32 * c, r0, &efull[e]);
+          if (fOmask) tma_load_2d(eb + p.eMaskOff, &mapM, n0 / 32, r0, &efull[e]);
+        }
+        __syncwarp();
+        if (++e == p.eb) { e = 0; eph ^= 1; }
+      }
       for (int kb = 0; kb < p.numKb; kb++) {
         mbar_wait(&empty[s], ph ^ 1);
-        uint8_t* st = smem + (size_t)s * stageBytes;
+        uint8_t* st = smem + p.stageOff + (size_t)s * p.stageBytes;
         if (elect_one()) {
-          mbar_arrive_expect_tx(&full[s], stageBytes);
-          tma_load_2d(st, &mapA, kb * TC_BK, (int)(tile * TC_BM), &full[s]);
-          tma_load_2d(st + aBytes, &mapWhi, kb * TC_BK, n0, &full[s]);
-          tma_load_2d(st + aBytes + bBytes, &mapWlo, kb * TC_BK, n0, &full[s]);
+          mbar_arrive_expect_tx(&full[s], p.stageBytes);
+          tma_load_2d(st, &mapA, kb * TC_BK, r0, &full[s]);
+          if (!p.wres) {
+            tma_load_2d(st + aBytes, &mapWhi, kb * TC_BK, n0, &full[s]);
+            tma_load_2d(st + aBytes + bBytes, &mapWlo, kb * TC_BK, n0, &full[s]);
+          }
         }
         __syncwarp();
         if (++s == p.stages) { s = 0; ph ^= 1; }
@@ -160,11 +190,21 @@ k_tc_linear(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
   }
 
   // ================================== consumers ===================================
-  const bool fNorm = (EPI) < 0 ? p.rowEnd != nullptr : ((EPI) & EPI_NORM) != 0;
   const int g = lane >> 2, t = lane & 3;
   const int rl = (warp >> 2) * 64 + (warp & 3) * 16 + g;    // tile rows of this thread: rl and rl + 8 (both == g mod 8)
   const bool masked = p.mask != nullptr;
+  auto mask_word = [&](int64_t row, int kb) { return (row < p.rows) ? __ldg(p.mask + row * p.ldm + kb) : 0u; };
+  if (p.wres) mbar_wait(wfull, 0);
   int s = 0; uint32_t ph = 0;
+  int e = 0; uint32_t eph = 0;
+  // dropout fused into the operand load: bit c of mask[row][kb] keeps column 32 kb + c.  The words of the next k-block
+  // (of the next tile after the last one) are loaded a whole k-block ahead, so their latency stays off the MMAs.
+  uint32_t mn0 = 0xFFFFFFFFu, mn1 = 0xFFFFFFFFu;
+  if (masked && blockIdx.x < numTiles) {
+    mn0 = mask_word(blockIdx.x * TC_BM + rl, 0);
+    mn1 = mask_word(blockIdx.x * TC_BM + rl + 8, 0);
+  }
+  uint32_t frA[TC_BK / 8][2][4], frB[TC_BK / 8][2][4] = {};   // A fragments (hi, lo) of two k-blocks in flight
   for (int64_t tile = blockIdx.x; tile < numTiles; tile += gridDim.x) {
     const int64_t row0 = tile * TC_BM + rl, row1 = row0 + 8;
     // the rows' norm divisors are fetched before the main loop so their DRAM latency overlaps it
@@ -175,17 +215,24 @@ k_tc_linear(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
     for (int c = 0; c < NC; c++)
 #pragma unroll
       for (int i = 0; i < 16; i++) acc[c][i] = 0.f;
-    for (int kb = 0; kb < p.numKb; kb++) {
-      // dropout fused into the operand load: bit c of mask[row][kb] keeps column 32 kb + c
-      uint32_t mw0 = 0xFFFFFFFFu, mw1 = 0xFFFFFFFFu;
+    int sPrev = 0;
+    // k-block kb: its A fragments go to `fr`, whose MMAs (k-block kb - 2) retired in the previous step; the MMAs of
+    // kb - 1 (fragments in `frPrev`) may run until the wait_group 1 that follows kb's issue, which then frees kb - 1's
+    // stage.  The MMA queue drains only at the end of the tile.
+    auto body = [&](int kb, uint32_t (&fr)[TC_BK / 8][2][4], uint32_t (&frPrev)[TC_BK / 8][2][4]) {
+      const uint32_t mw0 = mn0, mw1 = mn1;
       if (masked) {
-        mw0 = (row0 < p.rows) ? __ldg(p.mask + row0 * p.ldm + kb) : 0u;
-        mw1 = (row1 < p.rows) ? __ldg(p.mask + row1 * p.ldm + kb) : 0u;
+        if (kb + 1 < p.numKb) { mn0 = mask_word(row0, kb + 1); mn1 = mask_word(row1, kb + 1); }
+        else if (tile + gridDim.x < numTiles) {
+          const int64_t nr = row0 + (int64_t)gridDim.x * TC_BM;
+          mn0 = mask_word(nr, 0); mn1 = mask_word(nr + 8, 0);
+        }
       }
       mbar_wait(&full[s], ph);
-      const float* as = reinterpret_cast<const float*>(smem + (size_t)s * stageBytes);
-      const uint32_t bHi = smem_u32(smem + (size_t)s * stageBytes + aBytes), bLo = bHi + bBytes;
-      uint32_t fr[TC_BK / 8][2][4];    // A fragments (hi, lo) of every k8 step: live until the MMAs are retired
+      const uint8_t* st = smem + p.stageOff + (size_t)s * p.stageBytes;
+      const float* as = reinterpret_cast<const float*>(st);
+      const uint32_t bHi = p.wres ? smem_u32(smem + (size_t)kb * bBytes) : smem_u32(st + aBytes);
+      const uint32_t bLo = p.wres ? bHi + (uint32_t)p.numKb * bBytes : bHi + bBytes;
 #pragma unroll
       for (int kk = 0; kk < TC_BK / 8; kk++) {
         // 128B swizzle: 16-byte chunk j of row r sits at chunk j ^ (r & 7); columns 8 kk + t and 8 kk + t + 4
@@ -200,34 +247,86 @@ k_tc_linear(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
         }
 #pragma unroll
         for (int i = 0; i < 4; i++) split_tf32(x[i], fr[kk][0][i], fr[kk][1][i]);
-        wgmma_fence();
+      }
+      // per k8 step one m64n(32 NC)k8 per operand pair, lo*hi, hi*lo, hi*hi: each element gets the products of its
+      // n32 chunk in the same order
 #pragma unroll
-        for (int c = 0; c < NC; c++) {
-          const uint32_t off = (uint32_t)c * 32u * 128u + (uint32_t)kk * 32u;
-          const uint64_t dBh = make_sdesc_sw128(bHi + off), dBl = make_sdesc_sw128(bLo + off);
-          wgmma_m64n32k8_tf32(acc[c], fr[kk][1], dBh);
-          wgmma_m64n32k8_tf32(acc[c], fr[kk][0], dBl);
-          wgmma_m64n32k8_tf32(acc[c], fr[kk][0], dBh);
-        }
+      for (int kk = 0; kk < TC_BK / 8; kk++) {
+        wgmma_fence();
+        const uint64_t dBh = make_sdesc_sw128(bHi + kk * 32u), dBl = make_sdesc_sw128(bLo + kk * 32u);
+        wgmma_m64nNk8_tf32<NC>(acc, fr[kk][1], dBh);
+        wgmma_m64nNk8_tf32<NC>(acc, fr[kk][0], dBl);
+        wgmma_m64nNk8_tf32<NC>(acc, fr[kk][0], dBh);
       }
       wgmma_commit();
-      wgmma_wait_all();
-      keep_live(fr);
-#pragma unroll
-      for (int c = 0; c < NC; c++) wgmma_fence_acc(acc[c]);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty[s]);
+      wgmma_wait_1();
+      keep_live(frPrev);
+      if (kb > 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[sPrev]);
+      }
+      sPrev = s;
       if (++s == p.stages) { s = 0; ph ^= 1; }
+    };
+    for (int kb = 0; kb < p.numKb; kb += 2) {
+      body(kb, frA, frB);
+      if (kb + 1 < p.numKb) body(kb + 1, frB, frA);
     }
-    // epilogue: acc[c][4j + {0,1}] = (row0, col, col + 1), acc[c][4j + {2,3}] = (row1, ...), col = n0 + 32c + 8j + 2t
-    const RowDiv rd0 = rowdiv_make(d0), rd1 = rowdiv_make(d1);
+    wgmma_wait_all();
+    keep_live(frA);
+    keep_live(frB);
+#pragma unroll
+    for (int c = 0; c < NC; c++) wgmma_fence_acc(acc[c]);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[sPrev]);
+
+    // epilogue: acc[c][4j + {0,1}] = (row0, col, col + 1), acc[c][4j + {2,3}] = (row1, ...), col = n0 + 32c + 8j + 2t.
+    // The reluOf boxes ([128][32], 128-byte swizzle) and mask words ([128][4]) of the tile are in shared memory.
+    const RowDiv rd[2] = {rowdiv_make(d0), rowdiv_make(d1)};
+    const float* eo = nullptr;
+    const uint32_t* em = nullptr;
+    if (p.eb) {
+      mbar_wait(&efull[e], eph);
+      const uint8_t* eb = smem + p.eOff + (size_t)e * p.eBytes;
+      eo = reinterpret_cast<const float*>(eb);
+      em = reinterpret_cast<const uint32_t*>(eb + p.eMaskOff);
+    }
+#pragma unroll
+    for (int c = 0; c < NC; c++)
+#pragma unroll
+      for (int j = 0; j < 4; j++)
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+          const int r = rl + 8 * h, cc = 8 * j + 2 * t;   // tile row, column in chunk c
+          const uint32_t mw = fOmask ? em[r * 4 + c] >> cc : 3u;
+          float2 ro = make_float2(1.f, 1.f);
+          if (fReluOf) ro = *reinterpret_cast<const float2*>(eo + c * (rBytes / 4) + r * 32 + (((cc >> 2) ^ g) << 2) + (cc & 3));
+          float v[2] = {acc[c][4 * j + 2 * h], acc[c][4 * j + 2 * h + 1]};
+          const float rov[2] = {ro.x, ro.y};
+#pragma unroll
+          for (int k = 0; k < 2; k++) {
+            float x = v[k];
+            if (fRelu) x = relu_nanprop(x);
+            if (fOmask) x = ((mw >> k) & 1u) ? x * p.oscale : 0.f;
+            if (fReluOf) x = (rov[k] > 0.f) ? x : 0.f;
+            if (fNorm) x = rowdiv(x, rd[h]);   // == x / d bit for bit (common.cuh)
+            v[k] = x;
+          }
+          acc[c][4 * j + 2 * h] = v[0];
+          acc[c][4 * j + 2 * h + 1] = v[1];
+        }
+    if (p.eb) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&eempty[e]);
+      if (++e == p.eb) { e = 0; eph ^= 1; }
+    }
 #pragma unroll
     for (int c = 0; c < NC; c++)
 #pragma unroll
       for (int j = 0; j < 4; j++) {
         const int col = n0 + c * 32 + j * 8 + 2 * t;
-        tc_store_pair<EPI>(p, row0, col, acc[c][4 * j], acc[c][4 * j + 1], rd0);
-        tc_store_pair<EPI>(p, row1, col, acc[c][4 * j + 2], acc[c][4 * j + 3], rd1);
+        tc_store_pair(p, fAcc, row0, col, acc[c][4 * j], acc[c][4 * j + 1]);
+        tc_store_pair(p, fAcc, row1, col, acc[c][4 * j + 2], acc[c][4 * j + 3]);
       }
   }
 }
@@ -250,16 +349,17 @@ static int tc_instance(int epi) {
   return (epi == 0 || epi == EPI_NORM || epi == EPI_OMASK || epi == (EPI_OMASK | EPI_RELUOF | EPI_NORM)) ? epi : -1;
 }
 
+struct TcMaps { CUtensorMap A, Whi, Wlo, R, M; };
+
 template <int NC>
-static int tc_launch(dim3 grid, size_t smemBytes, int epi, const CUtensorMap& mapA, const CUtensorMap& mapWhi,
-                     const CUtensorMap& mapWlo, const TcParams& q, cudaStream_t st) {
+static int tc_launch(dim3 grid, size_t smemBytes, int epi, const TcMaps& m, const TcParams& q, cudaStream_t st) {
   constexpr int E1 = EPI_NORM, E2 = EPI_OMASK, E3 = EPI_OMASK | EPI_RELUOF | EPI_NORM;
   switch (tc_instance(epi)) {
-    case 0: return launch_dyn<k_tc_linear<NC, 0>>(grid, TC_THREADS, smemBytes, st, mapA, mapWhi, mapWlo, q);
-    case E1: return launch_dyn<k_tc_linear<NC, E1>>(grid, TC_THREADS, smemBytes, st, mapA, mapWhi, mapWlo, q);
-    case E2: return launch_dyn<k_tc_linear<NC, E2>>(grid, TC_THREADS, smemBytes, st, mapA, mapWhi, mapWlo, q);
-    case E3: return launch_dyn<k_tc_linear<NC, E3>>(grid, TC_THREADS, smemBytes, st, mapA, mapWhi, mapWlo, q);
-    default: return launch_dyn<k_tc_linear<NC, -1>>(grid, TC_THREADS, smemBytes, st, mapA, mapWhi, mapWlo, q);
+    case 0: return launch_dyn<k_tc_linear<NC, 0>>(grid, TC_THREADS, smemBytes, st, m.A, m.Whi, m.Wlo, m.R, m.M, q);
+    case E1: return launch_dyn<k_tc_linear<NC, E1>>(grid, TC_THREADS, smemBytes, st, m.A, m.Whi, m.Wlo, m.R, m.M, q);
+    case E2: return launch_dyn<k_tc_linear<NC, E2>>(grid, TC_THREADS, smemBytes, st, m.A, m.Whi, m.Wlo, m.R, m.M, q);
+    case E3: return launch_dyn<k_tc_linear<NC, E3>>(grid, TC_THREADS, smemBytes, st, m.A, m.Whi, m.Wlo, m.R, m.M, q);
+    default: return launch_dyn<k_tc_linear<NC, -1>>(grid, TC_THREADS, smemBytes, st, m.A, m.Whi, m.Wlo, m.R, m.M, q);
   }
 }
 
@@ -270,6 +370,7 @@ static int ts_gemm(int64_t rows, int K, int N, const float* A, int64_t ldA, cons
   if (K < 8 || N < 1 || rows < 1) return ROC_ERR_UNSUPPORTED;
   if ((ldA % 4) || (ldY % 4) || !aligned16(A) || !aligned16(Y)) return ROC_ERR_UNSUPPORTED;
   if (e.reluOf && ((e.ldR % 4) || !aligned16(e.reluOf))) return ROC_ERR_UNSUPPORTED;
+  if (e.outMask && !aligned16(e.outMask->bits)) return ROC_ERR_UNSUPPORTED;   // TMA takes the words [128][4] per tile
   if (rows > 0x7FFFFF00ll) return ROC_ERR_UNSUPPORTED;   // TMA coordinates are int32
   if (!encode_tiled_fn()) return ROC_ERR_UNSUPPORTED;
   // N-tile of 32, 64 or 128 columns (wgmma chunks of 32): the widest tile streams A once per 128 output columns
@@ -290,24 +391,44 @@ static int ts_gemm(int64_t rows, int K, int N, const float* A, int64_t ldA, cons
   k_split_w<<<(Npad * Kpad + 255) / 256, 256, 0, st>>>(N, K, Npad, Kpad, ldW, transposed, W, Whi, Wlo);
   ROC_LAUNCH_CHECK();
 
-  CUtensorMap mapA, mapWhi, mapWlo;
-  if (!make_tmap_f32_2d(&mapA, A, (uint64_t)rows, (uint64_t)K, (uint64_t)ldA, TC_BM, TC_BK)) return ROC_ERR_UNSUPPORTED;
-  if (!make_tmap_f32_2d(&mapWhi, Whi, (uint64_t)Npad, (uint64_t)Kpad, (uint64_t)Kpad, (uint32_t)BN, TC_BK)) return ROC_ERR_UNSUPPORTED;
-  if (!make_tmap_f32_2d(&mapWlo, Wlo, (uint64_t)Npad, (uint64_t)Kpad, (uint64_t)Kpad, (uint32_t)BN, TC_BK)) return ROC_ERR_UNSUPPORTED;
+  TcMaps m;
+  memset(&m, 0, sizeof(m));
+  if (!make_tmap_f32_2d(&m.A, A, (uint64_t)rows, (uint64_t)K, (uint64_t)ldA, TC_BM, TC_BK)) return ROC_ERR_UNSUPPORTED;
+  if (!make_tmap_f32_2d(&m.Whi, Whi, (uint64_t)Npad, (uint64_t)Kpad, (uint64_t)Kpad, (uint32_t)BN, TC_BK)) return ROC_ERR_UNSUPPORTED;
+  if (!make_tmap_f32_2d(&m.Wlo, Wlo, (uint64_t)Npad, (uint64_t)Kpad, (uint64_t)Kpad, (uint32_t)BN, TC_BK)) return ROC_ERR_UNSUPPORTED;
+  if (e.reluOf && !make_tmap_f32_2d(&m.R, e.reluOf, (uint64_t)rows, (uint64_t)N, (uint64_t)e.ldR, TC_BM, 32))
+    return ROC_ERR_UNSUPPORTED;
+  if (e.outMask && !make_tmap_u32_2d(&m.M, e.outMask->bits, (uint64_t)rows, (uint64_t)e.outMask->ld,
+                                     (uint64_t)e.outMask->ld, TC_BM, 4))
+    return ROC_ERR_UNSUPPORTED;
 
-  const size_t stageBytes = (size_t)TC_BM * TC_BK * 4 + (size_t)2 * BN * TC_BK * 4;
+  // Shared memory: W resident when its slice fits beside both epilogue buffers and a ring of TC_RES_MIN_STAGES A
+  // stages; then two epilogue buffers when they leave a ring of 2, else one.
+  const int numKb = Kpad / TC_BK;
+  const size_t aBytes = (size_t)TC_BM * TC_BK * 4, bBytes = (size_t)BN * TC_BK * 4;
+  const size_t wBytes = 2 * (size_t)numKb * bBytes;
+  const size_t eBytes = (e.reluOf ? (size_t)TC_BM * BN * 4 : 0) + (e.outMask ? (size_t)TC_BM * 4 * 4 : 0);
   const size_t fixedBytes = 1024 /*align*/ + 256 /*barriers*/;
-  const int stages = ring_stages(stageBytes, fixedBytes, TC_MAX_STAGES);
+  const bool wres = ring_stages(aBytes, fixedBytes + wBytes + 2 * eBytes, TC_MAX_STAGES) >= TC_RES_MIN_STAGES;
+  const size_t stageBytes = aBytes + (wres ? 0 : 2 * bBytes);
+  const size_t wUsed = wres ? wBytes : 0;
+  const int eb = !eBytes ? 0 : ring_stages(stageBytes, fixedBytes + wUsed + 2 * eBytes, TC_MAX_STAGES) ? 2 : 1;
+  const int stages = ring_stages(stageBytes, fixedBytes + wUsed + eb * eBytes, TC_MAX_STAGES);
   if (!stages) return ROC_ERR_UNSUPPORTED;
   TcParams q{};
-  q.Y = Y; q.ldY = ldY; q.rows = rows; q.outDim = N; q.numKb = Kpad / TC_BK; q.stages = stages;
+  q.Y = Y; q.ldY = ldY; q.rows = rows; q.outDim = N; q.numKb = numKb; q.stages = stages;
   q.accumulate = e.accumulate;
   if (inMask) { q.mask = inMask->bits; q.ldm = inMask->ld; q.mscale = inMask->scale; }
   q.relu = e.relu;
-  if (e.outMask) { q.omask = e.outMask->bits; q.oldm = e.outMask->ld; q.oscale = e.outMask->scale; }
-  q.reluOf = e.reluOf; q.ldR = e.ldR;
+  if (e.outMask) { q.omask = e.outMask->bits; q.oscale = e.outMask->scale; }
+  q.reluOf = e.reluOf;
   q.rowEnd = e.rowEnd; q.colLeft = e.colLeft;
-  const size_t smemBytes = (size_t)stages * stageBytes + fixedBytes;
+  q.wres = wres;
+  q.stageOff = (uint32_t)wUsed; q.stageBytes = (uint32_t)stageBytes;
+  q.eOff = q.stageOff + (uint32_t)(stages * stageBytes); q.eBytes = (uint32_t)eBytes; q.eb = eb;
+  q.eMaskOff = e.reluOf ? (uint32_t)(TC_BM * BN * 4) : 0u;
+  q.barOff = q.eOff + (uint32_t)(eb * eBytes);
+  const size_t smemBytes = (size_t)q.barOff + fixedBytes;
   const int64_t numTiles = (rows + TC_BM - 1) / TC_BM;
   int gx = sm_count() / nTiles;
   if (gx < 1) gx = 1;
@@ -317,12 +438,12 @@ static int ts_gemm(int64_t rows, int K, int N, const float* A, int64_t ldA, cons
                   (q.rowEnd ? EPI_NORM : 0) | (q.accumulate ? EPI_ACC : 0);
   if (info) {
     info->nc = NC; info->epi = tc_instance(epi); info->grid_x = (int)grid.x; info->grid_y = (int)grid.y;
-    info->stages = stages;
+    info->stages = stages; info->w_resident = wres; info->epi_bufs = eb;
   }
   switch (NC) {
-    case 1: return tc_launch<1>(grid, smemBytes, epi, mapA, mapWhi, mapWlo, q, st);
-    case 2: return tc_launch<2>(grid, smemBytes, epi, mapA, mapWhi, mapWlo, q, st);
-    default: return tc_launch<4>(grid, smemBytes, epi, mapA, mapWhi, mapWlo, q, st);
+    case 1: return tc_launch<1>(grid, smemBytes, epi, m, q, st);
+    case 2: return tc_launch<2>(grid, smemBytes, epi, m, q, st);
+    default: return tc_launch<4>(grid, smemBytes, epi, m, q, st);
   }
 }
 

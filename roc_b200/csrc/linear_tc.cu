@@ -19,14 +19,15 @@
 //   warps 0-7  two consumer warpgroups, 64 rows of the 128-row tile each: fragment load,
 //              [dropout mask ->] hi/lo split, per k8 step one wgmma m64n(32 NC)k8 per operand pair,
 //              then the epilogue (relu / dropout-backward mask / relu mask / row norm / accumulate)
-//              from the accumulator registers
+//              from the accumulator registers; at NC <= 2 a written (not accumulated) Y leaves through
+//              a shared-memory staging tile by TMA stores
 //   warp 8     TMA producer: per tile the epilogue operands (reluOf boxes and output-mask words, into
-//              one of 1 or 2 buffers), then per k-block the A tile [128 rows][32 k], with W_hi + W_lo
-//              of the k-block when W does not stay resident
+//              one of 1 or 2 buffers), then per k-block the A tile [128 rows][32 k] and its input-mask
+//              words, with W_hi + W_lo of the k-block when W does not stay resident
 // The mainloop keeps two k-blocks of MMAs in flight: the fragments of k-block kb and kb - 1 live in two
 // register sets, `wgmma.wait_group 1` after kb's issue retires kb - 1 and frees its stage, and the queue
-// drains only at the end of a tile.  The input-mask words are loaded a k-block ahead of their use and the
-// row-norm divisors at the top of the tile, so no global load waits in front of an MMA.
+// drains only at the end of a tile.  The row ends of the norm divisors are loaded a tile ahead of their use,
+// so no global load waits in front of an MMA.
 // When the CTA's W_hi / W_lo slice (2 * 32 NC * Kpad floats) fits beside the epilogue buffers and a ring
 // of TC_RES_MIN_STAGES A stages, it is loaded once per CTA and the ring carries A alone; otherwise W streams
 // through the ring with A, from L2.  HBM-bound on A (rows*K*4 bytes read once).
@@ -73,10 +74,13 @@ struct TcParams {
   const uint64_t* rowEnd; uint64_t colLeft;             //   indegree norm: x / sqrtf(deg(row))
   int accumulate;                                       //   Y += x instead of Y = x
   // shared memory (offsets from the 1024-aligned base): [W_hi | W_lo of every k-block when wres] [ring] [epilogue
-  // operand buffers] [barriers]
-  int wres;                                             // W resident: the ring stages carry only A
-  uint32_t stageOff, stageBytes;
+  // operand buffers] [Y staging tile] [barriers]
+  int wres;                                             // W resident: the ring stages carry only A (and mask words)
+  uint32_t stageOff, stageBytes, mOff;                  // stage: A [128][32], W_hi + W_lo unless wres, at mOff the
+                                                        // input-mask words [128][4] when mask
   uint32_t eOff, eBytes, eMaskOff; int eb;              // eb buffers of eBytes: [NC][128][32] reluOf, [128][4] mask words
+  int ystage; uint32_t yOff; int yCols;                 // Y leaves through [NC][128][32] at yOff, columns < yCols by
+                                                        // TMA stores
   uint32_t barOff;
 };
 
@@ -90,11 +94,13 @@ enum { EPI_RELU = 1, EPI_OMASK = 2, EPI_RELUOF = 4, EPI_NORM = 8, EPI_ACC = 16 }
   const bool fNorm = (EPI) < 0 ? (p).rowEnd != nullptr : ((EPI) & EPI_NORM) != 0;  \
   const bool fAcc = (EPI) < 0 ? (p).accumulate != 0 : ((EPI) & EPI_ACC) != 0;
 
-__device__ __forceinline__ float row_norm_divisor(const TcParams& p, int64_t row) {
-  if (!p.rowEnd || row >= p.rows) return 1.0f;
-  const uint64_t st = (row == 0) ? p.colLeft : p.rowEnd[row - 1];
-  return sqrtf((float)(uint32_t)(p.rowEnd[row] - st));
+// b = the low words of the row's (start, end) offsets, so that end - start is its indegree; (0, 1) past the last row
+__device__ __forceinline__ void row_bounds(const TcParams& p, int64_t row, uint32_t (&b)[2]) {
+  if (!p.rowEnd || row >= p.rows) { b[0] = 0u; b[1] = 1u; return; }
+  b[0] = (uint32_t)((row == 0) ? p.colLeft : p.rowEnd[row - 1]);
+  b[1] = (uint32_t)p.rowEnd[row];
 }
+__device__ __forceinline__ float row_norm_divisor(const uint32_t (&b)[2]) { return sqrtf((float)(b[1] - b[0])); }
 
 // Y[row][col, col + 1] (+)= x0, x1 (col even): the accumulator pair a thread holds, after the rest of the epilogue
 __device__ __forceinline__ void tc_store_pair(const TcParams& p, bool fAcc, int64_t row, int col, float x0, float x1) {
@@ -114,7 +120,9 @@ template <int NC, int EPI>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_tc_linear(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapWhi,
             const __grid_constant__ CUtensorMap mapWlo, const __grid_constant__ CUtensorMap mapR,
-            const __grid_constant__ CUtensorMap mapM, const TcParams p) {
+            const __grid_constant__ CUtensorMap mapM, const __grid_constant__ CUtensorMap mapIM,
+            const __grid_constant__ CUtensorMap mapY,
+            const TcParams p) {
   constexpr int BN = 32 * NC;
   constexpr uint32_t aBytes = TC_BM * TC_BK * 4;       // 16 KB of A per stage
   constexpr uint32_t bBytes = BN * TC_BK * 4;          // one k-block of W_hi (or W_lo)
@@ -131,11 +139,13 @@ k_tc_linear(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t numTiles = (p.rows + TC_BM - 1) / TC_BM;
   const int n0 = blockIdx.y * BN;          // this CTA's slice of the N (output column) dimension
+  const bool masked = p.mask != nullptr;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&mapA); tma_prefetch_desc(&mapWhi); tma_prefetch_desc(&mapWlo);
     if (fReluOf) tma_prefetch_desc(&mapR);
     if (fOmask) tma_prefetch_desc(&mapM);
+    if (masked) tma_prefetch_desc(&mapIM);
     for (int s = 0; s < p.stages; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
     for (int e = 0; e < p.eb; e++) { mbar_init(&efull[e], 1); mbar_init(&eempty[e], 8); }
     mbar_init(wfull, 1);
@@ -177,6 +187,8 @@ k_tc_linear(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
         if (elect_one()) {
           mbar_arrive_expect_tx(&full[s], p.stageBytes);
           tma_load_2d(st, &mapA, kb * TC_BK, r0, &full[s]);
+          // the box starts 16-byte aligned in global memory: words (kb & ~3) .. + 3, of which word kb is used
+          if (masked) tma_load_2d(st + p.mOff, &mapIM, kb & ~3, r0, &full[s]);
           if (!p.wres) {
             tma_load_2d(st + aBytes, &mapWhi, kb * TC_BK, n0, &full[s]);
             tma_load_2d(st + aBytes + bBytes, &mapWlo, kb * TC_BK, n0, &full[s]);
@@ -192,24 +204,23 @@ k_tc_linear(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
   // ================================== consumers ===================================
   const int g = lane >> 2, t = lane & 3;
   const int rl = (warp >> 2) * 64 + (warp & 3) * 16 + g;    // tile rows of this thread: rl and rl + 8 (both == g mod 8)
-  const bool masked = p.mask != nullptr;
-  auto mask_word = [&](int64_t row, int kb) { return (row < p.rows) ? __ldg(p.mask + row * p.ldm + kb) : 0u; };
   if (p.wres) mbar_wait(wfull, 0);
   int s = 0; uint32_t ph = 0;
   int e = 0; uint32_t eph = 0;
-  // dropout fused into the operand load: bit c of mask[row][kb] keeps column 32 kb + c.  The words of the next k-block
-  // (of the next tile after the last one) are loaded a whole k-block ahead, so their latency stays off the MMAs.
-  uint32_t mn0 = 0xFFFFFFFFu, mn1 = 0xFFFFFFFFu;
-  if (masked && blockIdx.x < numTiles) {
-    mn0 = mask_word(blockIdx.x * TC_BM + rl, 0);
-    mn1 = mask_word(blockIdx.x * TC_BM + rl + 8, 0);
+  // The row ends of the norm divisors are loaded a whole tile ahead of their use, into registers.
+  uint32_t nb0[2] = {0u, 1u}, nb1[2] = {0u, 1u};
+  if (fNorm) {
+    row_bounds(p, (int64_t)blockIdx.x * TC_BM + rl, nb0);
+    row_bounds(p, (int64_t)blockIdx.x * TC_BM + rl + 8, nb1);
   }
   uint32_t frA[TC_BK / 8][2][4], frB[TC_BK / 8][2][4] = {};   // A fragments (hi, lo) of two k-blocks in flight
   for (int64_t tile = blockIdx.x; tile < numTiles; tile += gridDim.x) {
     const int64_t row0 = tile * TC_BM + rl, row1 = row0 + 8;
-    // the rows' norm divisors are fetched before the main loop so their DRAM latency overlaps it
-    const float d0 = fNorm ? row_norm_divisor(p, row0) : 1.0f;
-    const float d1 = fNorm ? row_norm_divisor(p, row1) : 1.0f;
+    const uint32_t rb0[2] = {nb0[0], nb0[1]}, rb1[2] = {nb1[0], nb1[1]};   // this tile's
+    if (fNorm) {
+      row_bounds(p, row0 + (int64_t)gridDim.x * TC_BM, nb0);
+      row_bounds(p, row1 + (int64_t)gridDim.x * TC_BM, nb1);
+    }
     float acc[NC][16];
 #pragma unroll
     for (int c = 0; c < NC; c++)
@@ -220,19 +231,19 @@ k_tc_linear(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
     // kb - 1 (fragments in `frPrev`) may run until the wait_group 1 that follows kb's issue, which then frees kb - 1's
     // stage.  The MMA queue drains only at the end of the tile.
     auto body = [&](int kb, uint32_t (&fr)[TC_BK / 8][2][4], uint32_t (&frPrev)[TC_BK / 8][2][4]) {
-      const uint32_t mw0 = mn0, mw1 = mn1;
-      if (masked) {
-        if (kb + 1 < p.numKb) { mn0 = mask_word(row0, kb + 1); mn1 = mask_word(row1, kb + 1); }
-        else if (tile + gridDim.x < numTiles) {
-          const int64_t nr = row0 + (int64_t)gridDim.x * TC_BM;
-          mn0 = mask_word(nr, 0); mn1 = mask_word(nr + 8, 0);
-        }
-      }
       mbar_wait(&full[s], ph);
       const uint8_t* st = smem + p.stageOff + (size_t)s * p.stageBytes;
       const float* as = reinterpret_cast<const float*>(st);
       const uint32_t bHi = p.wres ? smem_u32(smem + (size_t)kb * bBytes) : smem_u32(st + aBytes);
       const uint32_t bLo = p.wres ? bHi + (uint32_t)p.numKb * bBytes : bHi + bBytes;
+      // dropout fused into the operand load: bit c of mask[row][kb] keeps column 32 kb + c ([128][4] words by TMA,
+      // with the stage)
+      uint32_t mw0 = 0u, mw1 = 0u;
+      if (masked) {
+        const uint32_t* mw = reinterpret_cast<const uint32_t*>(st + p.mOff);
+        mw0 = mw[rl * 4 + (kb & 3)];
+        mw1 = mw[(rl + 8) * 4 + (kb & 3)];
+      }
 #pragma unroll
       for (int kk = 0; kk < TC_BK / 8; kk++) {
         // 128B swizzle: 16-byte chunk j of row r sits at chunk j ^ (r & 7); columns 8 kk + t and 8 kk + t + 4
@@ -282,7 +293,7 @@ k_tc_linear(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
 
     // epilogue: acc[c][4j + {0,1}] = (row0, col, col + 1), acc[c][4j + {2,3}] = (row1, ...), col = n0 + 32c + 8j + 2t.
     // The reluOf boxes ([128][32], 128-byte swizzle) and mask words ([128][4]) of the tile are in shared memory.
-    const RowDiv rd[2] = {rowdiv_make(d0), rowdiv_make(d1)};
+    const RowDiv rd[2] = {rowdiv_make(row_norm_divisor(rb0)), rowdiv_make(row_norm_divisor(rb1))};
     const float* eo = nullptr;
     const uint32_t* em = nullptr;
     if (p.eb) {
@@ -320,15 +331,56 @@ k_tc_linear(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
       if (lane == 0) mbar_arrive(&eempty[e]);
       if (++e == p.eb) { e = 0; eph ^= 1; }
     }
+    if (NC <= 2 && p.ystage) {
+      // The tile leaves through shared memory: each warpgroup writes its 64 rows of every chunk ([64][32], 128-byte
+      // swizzle) and one of its threads stores them by TMA, which skips the rows past Y's last.  The stores run on
+      // while the next tile is computed; the buffer is refilled once they have read it.
+      const int wg = warp >> 2;
+      const bool leader = (threadIdx.x & 127) == 0;
+      float* yb = reinterpret_cast<float*>(smem + p.yOff) + wg * 64 * 32;   // chunk c at + c * TC_BM * 32
+      if (leader) bulk_wait_read();
+      named_barrier(1 + wg, 128);
 #pragma unroll
-    for (int c = 0; c < NC; c++)
+      for (int c = 0; c < NC; c++)
 #pragma unroll
-      for (int j = 0; j < 4; j++) {
-        const int col = n0 + c * 32 + j * 8 + 2 * t;
-        tc_store_pair(p, fAcc, row0, col, acc[c][4 * j], acc[c][4 * j + 1]);
-        tc_store_pair(p, fAcc, row1, col, acc[c][4 * j + 2], acc[c][4 * j + 3]);
+        for (int j = 0; j < 4; j++)
+#pragma unroll
+          for (int h = 0; h < 2; h++) {
+            const int r = (rl & 63) + 8 * h, cc = 8 * j + 2 * t;
+            *reinterpret_cast<float2*>(yb + c * TC_BM * 32 + r * 32 + (((cc >> 2) ^ g) << 2) + (cc & 3)) =
+                make_float2(acc[c][4 * j + 2 * h], acc[c][4 * j + 2 * h + 1]);
+          }
+      fence_proxy_async_smem();
+      named_barrier(1 + wg, 128);
+      if (leader) {
+        for (int c = 0; c < NC; c++)
+          tma_store_2d(&mapY, yb + c * TC_BM * 32, n0 + 32 * c, (int)(tile * TC_BM) + 64 * wg);
+        bulk_commit();
       }
+      // The TMA store covers the columns below p.yCols, a multiple of 4: it writes whole 16-byte units, so past a
+      // column count that is not a multiple of 4 it would overwrite Y's padding.  The last 1-3 columns go directly.
+#pragma unroll
+      for (int c = 0; c < NC; c++)
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+          const int col = n0 + c * 32 + j * 8 + 2 * t;
+          if (col >= p.yCols) {
+            tc_store_pair(p, false, row0, col, acc[c][4 * j], acc[c][4 * j + 1]);
+            tc_store_pair(p, false, row1, col, acc[c][4 * j + 2], acc[c][4 * j + 3]);
+          }
+        }
+    } else {
+#pragma unroll
+      for (int c = 0; c < NC; c++)
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+          const int col = n0 + c * 32 + j * 8 + 2 * t;
+          tc_store_pair(p, fAcc, row0, col, acc[c][4 * j], acc[c][4 * j + 1]);
+          tc_store_pair(p, fAcc, row1, col, acc[c][4 * j + 2], acc[c][4 * j + 3]);
+        }
+    }
   }
+  if (NC <= 2 && p.ystage && (threadIdx.x & 127) == 0) bulk_wait();   // the last stores have landed
 }
 
 // The split weights (W_hi / W_lo, padded) live in a stream-ordered allocation made for this call
@@ -349,17 +401,22 @@ static int tc_instance(int epi) {
   return (epi == 0 || epi == EPI_NORM || epi == EPI_OMASK || epi == (EPI_OMASK | EPI_RELUOF | EPI_NORM)) ? epi : -1;
 }
 
-struct TcMaps { CUtensorMap A, Whi, Wlo, R, M; };
+struct TcMaps { CUtensorMap A, Whi, Wlo, R, M, IM, Y; };
+
+template <int NC, int EPI>
+static int tc_launch_epi(dim3 grid, size_t smemBytes, const TcMaps& m, const TcParams& q, cudaStream_t st) {
+  return launch_dyn<k_tc_linear<NC, EPI>>(grid, TC_THREADS, smemBytes, st, m.A, m.Whi, m.Wlo, m.R, m.M, m.IM, m.Y, q);
+}
 
 template <int NC>
 static int tc_launch(dim3 grid, size_t smemBytes, int epi, const TcMaps& m, const TcParams& q, cudaStream_t st) {
   constexpr int E1 = EPI_NORM, E2 = EPI_OMASK, E3 = EPI_OMASK | EPI_RELUOF | EPI_NORM;
   switch (tc_instance(epi)) {
-    case 0: return launch_dyn<k_tc_linear<NC, 0>>(grid, TC_THREADS, smemBytes, st, m.A, m.Whi, m.Wlo, m.R, m.M, q);
-    case E1: return launch_dyn<k_tc_linear<NC, E1>>(grid, TC_THREADS, smemBytes, st, m.A, m.Whi, m.Wlo, m.R, m.M, q);
-    case E2: return launch_dyn<k_tc_linear<NC, E2>>(grid, TC_THREADS, smemBytes, st, m.A, m.Whi, m.Wlo, m.R, m.M, q);
-    case E3: return launch_dyn<k_tc_linear<NC, E3>>(grid, TC_THREADS, smemBytes, st, m.A, m.Whi, m.Wlo, m.R, m.M, q);
-    default: return launch_dyn<k_tc_linear<NC, -1>>(grid, TC_THREADS, smemBytes, st, m.A, m.Whi, m.Wlo, m.R, m.M, q);
+    case 0: return tc_launch_epi<NC, 0>(grid, smemBytes, m, q, st);
+    case E1: return tc_launch_epi<NC, E1>(grid, smemBytes, m, q, st);
+    case E2: return tc_launch_epi<NC, E2>(grid, smemBytes, m, q, st);
+    case E3: return tc_launch_epi<NC, E3>(grid, smemBytes, m, q, st);
+    default: return tc_launch_epi<NC, -1>(grid, smemBytes, m, q, st);
   }
 }
 
@@ -371,6 +428,7 @@ static int ts_gemm(int64_t rows, int K, int N, const float* A, int64_t ldA, cons
   if ((ldA % 4) || (ldY % 4) || !aligned16(A) || !aligned16(Y)) return ROC_ERR_UNSUPPORTED;
   if (e.reluOf && ((e.ldR % 4) || !aligned16(e.reluOf))) return ROC_ERR_UNSUPPORTED;
   if (e.outMask && !aligned16(e.outMask->bits)) return ROC_ERR_UNSUPPORTED;   // TMA takes the words [128][4] per tile
+  if (inMask && !aligned16(inMask->bits)) return ROC_ERR_UNSUPPORTED;         // and [128][4] per k-block
   if (rows > 0x7FFFFF00ll) return ROC_ERR_UNSUPPORTED;   // TMA coordinates are int32
   if (!encode_tiled_fn()) return ROC_ERR_UNSUPPORTED;
   // N-tile of 32, 64 or 128 columns (wgmma chunks of 32): the widest tile streams A once per 128 output columns
@@ -401,16 +459,27 @@ static int ts_gemm(int64_t rows, int K, int N, const float* A, int64_t ldA, cons
   if (e.outMask && !make_tmap_u32_2d(&m.M, e.outMask->bits, (uint64_t)rows, (uint64_t)e.outMask->ld,
                                      (uint64_t)e.outMask->ld, TC_BM, 4))
     return ROC_ERR_UNSUPPORTED;
+  if (inMask && !make_tmap_u32_2d(&m.IM, inMask->bits, (uint64_t)rows, (uint64_t)inMask->ld, (uint64_t)inMask->ld,
+                                  TC_BM, 4))
+    return ROC_ERR_UNSUPPORTED;
+  // Y leaves by TMA stores from a staging tile when it is written, not accumulated, and the tile is <= 64 columns wide
+  // (the 128-wide tile keeps its shared memory for the ring)
+  const int yCols = N & ~3;
+  const bool ystage = !e.accumulate && NC <= 2 && yCols > 0;
+  if (ystage && !make_tmap_f32_2d(&m.Y, Y, (uint64_t)rows, (uint64_t)yCols, (uint64_t)ldY, TC_BM / 2, 32))
+    return ROC_ERR_UNSUPPORTED;
 
-  // Shared memory: W resident when its slice fits beside both epilogue buffers and a ring of TC_RES_MIN_STAGES A
-  // stages; then two epilogue buffers when they leave a ring of 2, else one.
+  // Shared memory: W resident when its slice fits beside both epilogue buffers, the Y staging tile and a ring of
+  // TC_RES_MIN_STAGES A stages; then two epilogue buffers when they leave a ring of 2, else one.
   const int numKb = Kpad / TC_BK;
   const size_t aBytes = (size_t)TC_BM * TC_BK * 4, bBytes = (size_t)BN * TC_BK * 4;
+  const size_t mBytes = inMask ? (size_t)TC_BM * 4 * 4 : 0;
   const size_t wBytes = 2 * (size_t)numKb * bBytes;
   const size_t eBytes = (e.reluOf ? (size_t)TC_BM * BN * 4 : 0) + (e.outMask ? (size_t)TC_BM * 4 * 4 : 0);
-  const size_t fixedBytes = 1024 /*align*/ + 256 /*barriers*/;
-  const bool wres = ring_stages(aBytes, fixedBytes + wBytes + 2 * eBytes, TC_MAX_STAGES) >= TC_RES_MIN_STAGES;
-  const size_t stageBytes = aBytes + (wres ? 0 : 2 * bBytes);
+  const size_t yBytes = ystage ? (size_t)TC_BM * BN * 4 : 0;
+  const size_t fixedBytes = 1024 /*align*/ + 256 /*barriers*/ + yBytes;
+  const bool wres = ring_stages(aBytes + mBytes, fixedBytes + wBytes + 2 * eBytes, TC_MAX_STAGES) >= TC_RES_MIN_STAGES;
+  const size_t stageBytes = aBytes + (wres ? 0 : 2 * bBytes) + mBytes;
   const size_t wUsed = wres ? wBytes : 0;
   const int eb = !eBytes ? 0 : ring_stages(stageBytes, fixedBytes + wUsed + 2 * eBytes, TC_MAX_STAGES) ? 2 : 1;
   const int stages = ring_stages(stageBytes, fixedBytes + wUsed + eb * eBytes, TC_MAX_STAGES);
@@ -424,11 +493,12 @@ static int ts_gemm(int64_t rows, int K, int N, const float* A, int64_t ldA, cons
   q.reluOf = e.reluOf;
   q.rowEnd = e.rowEnd; q.colLeft = e.colLeft;
   q.wres = wres;
-  q.stageOff = (uint32_t)wUsed; q.stageBytes = (uint32_t)stageBytes;
+  q.stageOff = (uint32_t)wUsed; q.stageBytes = (uint32_t)stageBytes; q.mOff = (uint32_t)(stageBytes - mBytes);
   q.eOff = q.stageOff + (uint32_t)(stages * stageBytes); q.eBytes = (uint32_t)eBytes; q.eb = eb;
   q.eMaskOff = e.reluOf ? (uint32_t)(TC_BM * BN * 4) : 0u;
-  q.barOff = q.eOff + (uint32_t)(eb * eBytes);
-  const size_t smemBytes = (size_t)q.barOff + fixedBytes;
+  q.ystage = ystage; q.yCols = yCols; q.yOff = q.eOff + (uint32_t)(eb * eBytes);
+  q.barOff = q.yOff + (uint32_t)yBytes;
+  const size_t smemBytes = (size_t)q.barOff + fixedBytes - yBytes;
   const int64_t numTiles = (rows + TC_BM - 1) / TC_BM;
   int gx = sm_count() / nTiles;
   if (gx < 1) gx = 1;

@@ -68,6 +68,21 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1), "r"(smem_u32(bar))
       : "memory");
 }
+// 2-D tile store from shared memory (elements outside the tensor are not written), tracked by the issuing thread's
+// bulk groups: bulk_commit() closes a group, bulk_wait_read() waits until its groups have read their shared memory,
+// bulk_wait() until their writes are done
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// barrier `id` (1..15) over `threads` threads of the CTA (a multiple of 32)
+__device__ __forceinline__ void named_barrier(uint32_t id, uint32_t threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
 
 // -------------------------------------------------------------------- wgmma ---
 // Warpgroup MMA (sm_90a): the 128 threads of a warpgroup issue together; the accumulator lives in

@@ -429,6 +429,12 @@ int roc_dropout_fwd(int64_t rows, int H, int64_t firstRow, float rate, uint64_t 
 int roc_dropout_bwd(int64_t rows, int H, int64_t firstRow, float rate, uint64_t seed,
                     uint32_t step, const float* dY, int64_t ldDY, float* dX,
                     int64_t ldDX, roc_stream_t stream);
+/* roc_dropout_fwd on a bf16 x (raw bits, see roc_f32_to_bf16), writing fp32 y.  Each element
+ * widens to fp32 exactly, so y is bit-identical to roc_dropout_fwd on the widened x (same
+ * mask, same scale).  rate == 0 is the widening copy. */
+int roc_dropout_fwd_bf16(int64_t rows, int H, int64_t firstRow, float rate, uint64_t seed,
+                         uint32_t step, const uint16_t* x, int64_t ldX, float* y, int64_t ldY,
+                         roc_stream_t stream);
 
 /* The same mask, packed one bit per element: bit (h & 31) of
  * mask[row * ldMask + (h >> 5)] = keep(firstRow + row, h).  ldMask (32-bit words per
@@ -493,6 +499,32 @@ int roc_linear_fwd_dropout(int64_t rows, int inDim, int outDim, const float* X, 
                            const float* W, float* Y, int64_t ldY, int activation, int flags,
                            const roc_eid_t* rowEnd, roc_eid_t colLeft, const uint32_t* mask,
                            int64_t ldMask, float rate, roc_stream_t stream);
+
+/* ---- bf16 input features.  A leaf node tensor (the raw features X) may be stored in bf16:
+ * raw bits as uint16_t, round-to-nearest-even from fp32 (roc_f32_to_bf16), rows of
+ * ld >= inDim elements.  The tensor-core kernels read it by TMA and take ld a multiple of 8
+ * (16-byte rows) and a 16-byte aligned base; other layouts, and the shapes they refuse, run on
+ * the SIMT kernels as the fp32 entry points do (roc_last_gemm_info tells which).  A bf16 value
+ * has 8 significant bits, so it widens to fp32 exactly and its TF32 split has a zero low part:
+ * each kernel widens X as it reads it and then computes what it computes in fp32.
+ *
+ * roc_linear_fwd_dropout with a bf16 X: mask == NULL and rate == 0 means no dropout.  Y is
+ * bit-identical to roc_linear_fwd_dropout on the widened X (on the same path, tensor cores or
+ * SIMT). */
+int roc_linear_fwd_bf16(int64_t rows, int inDim, int outDim, const uint16_t* X, int64_t ldX,
+                        const float* W, float* Y, int64_t ldY, int activation, int flags,
+                        const roc_eid_t* rowEnd, roc_eid_t colLeft, const uint32_t* mask,
+                        int64_t ldMask, float rate, roc_stream_t stream);
+/* dW of a Linear whose input is a bf16 X (a leaf: there is no dX):
+ *   if activation == RELU: dY = (Y > 0) ? dY : 0 in place
+ *   dW[o*inDim+i] += sum_v dropout(X)[v][i] * dY[v][o]
+ * with the dropout as in roc_linear_fwd_bf16 and `workspace` sized by
+ * roc_linear_bwd_workspace_bytes.  dY and dW are bit-identical to roc_linear_bwd_dropout with
+ * dX == NULL on the widened X (on the same path and dW kernel). */
+int roc_linear_dw_bf16(int64_t rows, int inDim, int outDim, const uint16_t* X, int64_t ldX,
+                       const float* Y, int64_t ldY, float* dY, int64_t ldDY, float* dW,
+                       int activation, void* workspace, size_t workspaceBytes,
+                       const uint32_t* mask, int64_t ldMask, float rate, roc_stream_t stream);
 
 size_t roc_linear_bwd_workspace_bytes(int64_t rows, int inDim, int outDim);
 int roc_linear_bwd(int64_t rows, int inDim, int outDim, const float* X, int64_t ldX,
@@ -597,6 +629,15 @@ int roc_selftest_rowdiv(float d, uint64_t firstBits, uint64_t count, uint64_t* d
  * the [rows][H] window between tensors of different leading dimensions. */
 int roc_copy2d(int64_t rows, int H, const float* src, int64_t ldSrc, float* dst, int64_t ldDst,
                roc_stream_t stream);
+/* fp32 -> bf16 (raw bits) of the [rows][H] window, round to nearest even, as torch's
+ * Tensor.to(torch.bfloat16): a finite value past the largest bf16 rounds to +-inf, and a NaN
+ * becomes the quiet NaN 0x7FC0 (sign and payload are not kept).  Writes whole destination rows: columns [H, ldDst) get zero.  Uploads
+ * convert staged fp32 chunks with it, so no full-size fp32 copy is ever on the device. */
+int roc_f32_to_bf16(int64_t rows, int H, const float* src, int64_t ldSrc, uint16_t* dst,
+                    int64_t ldDst, roc_stream_t stream);
+/* bf16 -> fp32 of the [rows][H] window: exact. */
+int roc_bf16_to_f32(int64_t rows, int H, const uint16_t* src, int64_t ldSrc, float* dst,
+                    int64_t ldDst, roc_stream_t stream);
 
 #ifdef __cplusplus
 }

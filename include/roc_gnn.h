@@ -211,6 +211,10 @@ public:
   Tensor linear(const Tensor& _input, int outDim, ActiMode activation, Initializer* initializer = NULL);
   Tensor relu(const Tensor& _input);
   Tensor sigmoid(const Tensor& _input);
+  /* DT = DATATYPE (fp32), int (masks), or __nv_bfloat16 (<cuda_bf16.h>): a leaf feature matrix stored in bf16, rounded
+   * to nearest even, rows of round_up(H, 8) elements.  It never has a gradient and is never an op's output; linear and
+   * dropout read it (bit-identical to the same model on an fp32 input holding the widened values), and init() refuses
+   * any other op that reads it.  Untested at more than one partition. */
   template <typename DT> Tensor create_node_tensor(int _numHidden) const;
   /* gnn.h:178, gnn.cc:534-560: one value per edge of this partition, dims = {numHidden, numEdges}, stored as a dense
    * fp32 array in the CSR's edge order, with a gradient twin allocated on first use.  Only DT = float and
@@ -229,9 +233,13 @@ public:
   void zero_gradients(void);
 
   /* ---- additions (not in gnn.h): host<->device access to this partition's rows ---- */
-  /* Copy `rows_local x H` values between a dense host buffer and the tensor. */
+  /* Copy `rows_local x H` values between a dense host buffer and the tensor.  A bf16 tensor takes and returns fp32
+   * rows (set: rounded to nearest even on the device; get: widened exactly); grad = true on it is an error. */
   void set_tensor(const Tensor& t, const void* host, bool grad = false);
   void get_tensor(const Tensor& t, void* host, bool grad = false) const;
+  /* a bf16 tensor's raw bits, `rows_local x H` uint16 values, copied as they are */
+  void set_tensor_bf16(const Tensor& t, const uint16_t* host);
+  void get_tensor_bf16(const Tensor& t, uint16_t* host) const;
   /* labels as class indices (what load_labels parses, load_task.cu:118-123) */
   void set_labels(const Tensor& label, const int* host_class_idx);
   roc_perf_metrics last_metrics(void) const;   /* PerfMetrics of the latest softmax pass */

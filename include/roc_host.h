@@ -36,6 +36,9 @@ const roc_sg_plan* roc_host_graph_plan(roc_host* h);
 
 /* Model builder — returns a tensor handle (>= 0). */
 int roc_host_create_node_tensor(roc_host* h, int hidden, int is_int);
+/* a leaf feature tensor stored in bf16 (Model::create_node_tensor<__nv_bfloat16>): only linear and dropout may read
+ * it; set_tensor / get_tensor move fp32 rows (rounded / widened), the _bf16 calls below its raw bits */
+int roc_host_create_node_tensor_bf16(roc_host* h, int hidden);
 int roc_host_dropout(roc_host* h, int t, float rate, int seed);
 int roc_host_linear(roc_host* h, int t, int outDim, int activation);
 int roc_host_indegree_norm(roc_host* h, int t);
@@ -70,11 +73,13 @@ int roc_host_load_labels(roc_host* h, int t, const char* prefix);
 int roc_host_load_train_mask(roc_host* h, int t, const char* prefix);
 int roc_host_set_tensor(roc_host* h, int t, const void* host, int grad);
 int roc_host_get_tensor(roc_host* h, int t, void* host, int grad);
+int roc_host_set_tensor_bf16(roc_host* h, int t, const uint16_t* host);   /* raw bf16 bits, rows x hidden */
+int roc_host_get_tensor_bf16(roc_host* h, int t, uint16_t* host);
 int roc_host_set_labels(roc_host* h, int t, const int32_t* host_class_idx);
 /* the source ids a max / min scatter_gather output t was taken from, [rows][hidden] u32 (Model::get_aggr_index) */
 int roc_host_get_aggr_index(roc_host* h, int t, uint32_t* host);
 int roc_host_tensor_shape(roc_host* h, int t, int64_t out[3]);   /* rows, hidden, ld */
-void* roc_host_tensor_ptr(roc_host* h, int t, int grad);          /* device pointer */
+void* roc_host_tensor_ptr(roc_host* h, int t, int grad);          /* device pointer (a bf16 tensor: its bits) */
 int roc_host_num_parameters(roc_host* h);
 int roc_host_parameter_shape(roc_host* h, int p, int64_t out[2]); /* inDim, outDim */
 int roc_host_get_parameter(roc_host* h, int p, float* host, int which); /* 0 W, 1 dW, 2 m, 3 v */

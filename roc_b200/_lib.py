@@ -157,6 +157,7 @@ PROTOTYPES = {
     "roc_dropout_fwd": (i32, [i64, i32, i64, f32, u64, u32, vp, i64, vp, i64, vp]),
     "roc_dropout_bwd": (i32, [i64, i32, i64, f32, u64, u32, vp, i64, vp, i64, vp]),
     "roc_dropout_mask": (i32, [i64, i32, i64, f32, u64, u32, vp, i64, vp]),
+    "roc_dropout_fwd_bf16": (i32, [i64, i32, i64, f32, u64, u32, vp, i64, vp, i64, vp]),
     "roc_softmax_xent_bwd": (i32, [i64, i32, vp, i64, vp, i64, vp, vp, i64, vp, vp]),
     "roc_softmax_xent_bwd_idx": (i32, [i64, i32, vp, i64, vp, vp, vp, i64, vp, vp]),
     "roc_softmax_xent_bwd_norm": (i32, [i64, i32, vp, i64, vp, i64, vp, vp, vp, i64, vp, u64, vp, vp]),
@@ -167,12 +168,16 @@ PROTOTYPES = {
     "roc_linear_fwd_dropout": (i32, [i64, i32, i32, vp, i64, vp, vp, i64, i32, i32, vp, u64, vp, i64, f32, vp]),
     "roc_linear_bwd_dropout": (i32, [i64, i32, i32, vp, i64, vp, vp, i64, vp, i64, vp, vp, i64, i32, i32, vp, sz,
                                      vp, i64, f32, vp]),
+    "roc_linear_fwd_bf16": (i32, [i64, i32, i32, vp, i64, vp, vp, i64, i32, i32, vp, u64, vp, i64, f32, vp]),
+    "roc_linear_dw_bf16": (i32, [i64, i32, i32, vp, i64, vp, i64, vp, i64, vp, i32, vp, sz, vp, i64, f32, vp]),
     "roc_last_gemm_path": (i32, [i32]),
     "roc_last_gemm_info": (i32, [i32, C.POINTER(GemmInfo)]),
     "roc_adam_update": (i32, [i64, f32, f32, f32, f32, f32, vp, vp, vp, vp, vp]),
     "roc_scale": (i32, [i64, f32, f32, vp, vp]),
     "roc_fill": (i32, [i64, i32, f32, vp, i64, vp]),
     "roc_copy2d": (i32, [i64, i32, vp, i64, vp, i64, vp]),
+    "roc_f32_to_bf16": (i32, [i64, i32, vp, i64, vp, i64, vp]),
+    "roc_bf16_to_f32": (i32, [i64, i32, vp, i64, vp, i64, vp]),
     "roc_selftest_rowdiv": (i32, [f32, u64, u64, vp, vp]),
     # ---- roc_host.h
     "roc_host_create": (vp, [i32, i32, i32]),
@@ -186,6 +191,7 @@ PROTOTYPES = {
     "roc_host_graph_info": (i32, [vp, vp]),
     "roc_host_graph_plan": (vp, [vp]),
     "roc_host_create_node_tensor": (i32, [vp, i32, i32]),
+    "roc_host_create_node_tensor_bf16": (i32, [vp, i32]),
     "roc_host_dropout": (i32, [vp, i32, f32, i32]),
     "roc_host_linear": (i32, [vp, i32, i32, i32]),
     "roc_host_indegree_norm": (i32, [vp, i32]),
@@ -212,6 +218,8 @@ PROTOTYPES = {
     "roc_host_load_train_mask": (i32, [vp, i32, C.c_char_p]),
     "roc_host_set_tensor": (i32, [vp, i32, vp, i32]),
     "roc_host_get_tensor": (i32, [vp, i32, vp, i32]),
+    "roc_host_set_tensor_bf16": (i32, [vp, i32, vp]),
+    "roc_host_get_tensor_bf16": (i32, [vp, i32, vp]),
     "roc_host_set_labels": (i32, [vp, i32, vp]),
     "roc_host_tensor_shape": (i32, [vp, i32, vp]),
     "roc_host_tensor_ptr": (vp, [vp, i32, i32]),

@@ -169,11 +169,11 @@ __device__ __forceinline__ uint32_t dropout_keep8(uint64_t row, uint32_t grp, ui
 
 // One thread handles the 8 columns of one Philox block of UNR different (row, block) items per
 // iteration, all loads issued before the Philox rounds.  VEC == 1 is the scalar fallback for
-// unpadded layouts.
-template <int VEC, int UNR>
+// unpadded layouts and for a bf16 x (TX = uint16_t, widened exactly as it is loaded).
+template <int VEC, int UNR, class TX = float>
 __global__ void __launch_bounds__(EW_T)
 k_dropout(int64_t rows, int H, int64_t firstRow, uint32_t thresh16, float scale, uint32_t seedLo,
-          uint32_t seedHi, uint32_t step, const float* __restrict__ x, int64_t ldx,
+          uint32_t seedHi, uint32_t step, const TX* __restrict__ x, int64_t ldx,
           float* __restrict__ y, int64_t ldy) {
   const int Wq = (H + 7) / 8;
   const int64_t total = rows * (int64_t)Wq;
@@ -195,7 +195,7 @@ k_dropout(int64_t rows, int H, int64_t firstRow, uint32_t thresh16, float scale,
           *reinterpret_cast<float4*>(&xv[u][4 * h]) = *reinterpret_cast<const float4*>(x + r * ldx + ch);
         else
 #pragma unroll
-          for (int j = 0; j < 4; j++) xv[u][4 * h + j] = (ok && ch + j < H) ? x[r * ldx + ch + j] : 0.f;
+          for (int j = 0; j < 4; j++) xv[u][4 * h + j] = (ok && ch + j < H) ? to_f32(x[r * ldx + ch + j]) : 0.f;
       }
     }
 #pragma unroll
@@ -703,6 +703,18 @@ extern "C" int roc_dropout_fwd(int64_t rows, int H, int64_t firstRow, float rate
   return dropout_launch(rows, H, firstRow, rate, seed, step, x, ldX, y, ldY, as_stream(stream));
 }
 
+extern "C" int roc_dropout_fwd_bf16(int64_t rows, int H, int64_t firstRow, float rate, uint64_t seed,
+                                    uint32_t step, const uint16_t* x, int64_t ldX, float* y, int64_t ldY,
+                                    roc_stream_t stream) {
+  if (!x || !y || rows < 0 || H <= 0 || ldX < H || ldY < H || rate < 0.f || rate >= 1.f) return ROC_ERR_INVALID;
+  if (rows == 0) return ROC_OK;
+  k_dropout<1, 2, uint16_t><<<ew_grid((rows * ((H + 7) / 8) + 1) / 2, EW_T), EW_T, 0, as_stream(stream)>>>(
+      rows, H, firstRow, dropout_thresh16(rate), 1.0f / (1.0f - rate), (uint32_t)seed, (uint32_t)(seed >> 32), step,
+      x, ldX, y, ldY);
+  ROC_LAUNCH_CHECK();
+  return ROC_OK;
+}
+
 extern "C" int roc_dropout_bwd(int64_t rows, int H, int64_t firstRow, float rate, uint64_t seed, uint32_t step,
                                const float* dY, int64_t ldDY, float* dX, int64_t ldDX, roc_stream_t stream) {
   // dX = dY * keep / (1 - rate): the same map as forward (dropout_kernel.cu:149-150)
@@ -806,6 +818,56 @@ extern "C" int roc_fill(int64_t rows, int H, float value, float* x, int64_t ld, 
   if (!x || rows < 0 || H <= 0 || ld < H) return ROC_ERR_INVALID;
   if (rows == 0) return ROC_OK;
   k_fill<<<ew_grid(rows * H, EW_T), EW_T, 0, as_stream(stream)>>>(rows, H, value, x, ld);
+  ROC_LAUNCH_CHECK();
+  return ROC_OK;
+}
+
+// ------------------------------------------------------------------- bf16 ---
+// fp32 -> bf16, round to nearest even as torch's Tensor.to(torch.bfloat16): a finite value past the largest bf16 rounds
+// to +-inf, a NaN becomes the quiet NaN 0x7FC0.  Writes every column of the
+// [rows][ldDst] destination: the pad columns [H, ldDst) get zero.
+__device__ __forceinline__ uint16_t f32_to_bf16_rne(float f) {
+  const uint32_t u = __float_as_uint(f);
+  if (f != f) return (uint16_t)0x7FC0u;
+  return (uint16_t)((u + 0x7FFFu + ((u >> 16) & 1u)) >> 16);
+}
+
+__global__ void __launch_bounds__(EW_T)
+k_f32_to_bf16(int64_t rows, int H, const float* __restrict__ src, int64_t ldSrc, uint16_t* __restrict__ dst,
+              int64_t ldDst) {
+  const int64_t total = rows * ldDst;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = i / ldDst;
+    const int c = (int)(i - r * ldDst);
+    dst[i] = c < H ? f32_to_bf16_rne(src[r * ldSrc + c]) : (uint16_t)0u;
+  }
+}
+
+__global__ void __launch_bounds__(EW_T)
+k_bf16_to_f32(int64_t rows, int H, const uint16_t* __restrict__ src, int64_t ldSrc, float* __restrict__ dst,
+              int64_t ldDst) {
+  const int64_t total = rows * (int64_t)H;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = i / H;
+    const int c = (int)(i - r * H);
+    dst[r * ldDst + c] = to_f32(src[r * ldSrc + c]);
+  }
+}
+
+extern "C" int roc_f32_to_bf16(int64_t rows, int H, const float* src, int64_t ldSrc, uint16_t* dst, int64_t ldDst,
+                               roc_stream_t stream) {
+  if (!src || !dst || rows < 0 || H <= 0 || ldSrc < H || ldDst < H) return ROC_ERR_INVALID;
+  if (rows == 0) return ROC_OK;
+  k_f32_to_bf16<<<ew_grid(rows * ldDst, EW_T), EW_T, 0, as_stream(stream)>>>(rows, H, src, ldSrc, dst, ldDst);
+  ROC_LAUNCH_CHECK();
+  return ROC_OK;
+}
+
+extern "C" int roc_bf16_to_f32(int64_t rows, int H, const uint16_t* src, int64_t ldSrc, float* dst, int64_t ldDst,
+                               roc_stream_t stream) {
+  if (!src || !dst || rows < 0 || H <= 0 || ldSrc < H || ldDst < H) return ROC_ERR_INVALID;
+  if (rows == 0) return ROC_OK;
+  k_bf16_to_f32<<<ew_grid(rows * H, EW_T), EW_T, 0, as_stream(stream)>>>(rows, H, src, ldSrc, dst, ldDst);
   ROC_LAUNCH_CHECK();
   return ROC_OK;
 }

@@ -1,4 +1,5 @@
 // capi.cc — roc_host_* : C ABI over the C++ host for Python / bench / tests.
+#include <cuda_bf16.h>
 #include <cstring>
 
 #include "host_internal.h"
@@ -81,6 +82,9 @@ const roc_sg_plan* roc_host_graph_plan(roc_host* h) { return h->graph ? h->graph
 int roc_host_create_node_tensor(roc_host* h, int hidden, int is_int) {
   return h->push(is_int ? h->m().create_node_tensor<int>(hidden) : h->m().create_node_tensor<DATATYPE>(hidden));
 }
+int roc_host_create_node_tensor_bf16(roc_host* h, int hidden) {
+  return h->push(h->m().create_node_tensor<__nv_bfloat16>(hidden));
+}
 int roc_host_dropout(roc_host* h, int t, float rate, int seed) { return h->push(h->m().dropout(h->at(t), rate, seed)); }
 int roc_host_linear(roc_host* h, int t, int outDim, int activation) {
   return h->push(h->m().linear(h->at(t), outDim, (ActiMode)activation));
@@ -126,6 +130,8 @@ int roc_host_load_labels(roc_host* h, int t, const char* prefix) { h->m().load_l
 int roc_host_load_train_mask(roc_host* h, int t, const char* prefix) { h->m().load_train_mask(h->at(t), prefix); return 0; }
 int roc_host_set_tensor(roc_host* h, int t, const void* host, int grad) { h->m().set_tensor(h->at(t), host, grad != 0); return 0; }
 int roc_host_get_tensor(roc_host* h, int t, void* host, int grad) { h->m().get_tensor(h->at(t), host, grad != 0); return 0; }
+int roc_host_set_tensor_bf16(roc_host* h, int t, const uint16_t* host) { h->m().set_tensor_bf16(h->at(t), host); return 0; }
+int roc_host_get_tensor_bf16(roc_host* h, int t, uint16_t* host) { h->m().get_tensor_bf16(h->at(t), host); return 0; }
 int roc_host_set_labels(roc_host* h, int t, const int32_t* cls) { h->m().set_labels(h->at(t), cls); return 0; }
 
 int roc_host_tensor_shape(roc_host* h, int t, int64_t out[3]) {
@@ -134,6 +140,8 @@ int roc_host_tensor_shape(roc_host* h, int t, int64_t out[3]) {
   return 0;
 }
 void* roc_host_tensor_ptr(roc_host* h, int t, int grad) {
+  RuntimeImpl* rt = h->rt->impl;
+  if (!grad && rt->t(h->at(t).region).isBf16) return (void*)rt->data_bf16(h->at(t).region);
   return grad ? (void*)h->rt->impl->grad(h->at(t).region) : (void*)h->rt->impl->data(h->at(t).region);
 }
 

@@ -32,6 +32,8 @@ struct TensorImpl {
   int H = 0;              // logical width (node: hidden; weight: inDim, stored [out][in])
   int64_t ld = 0;         // floats between rows (H rounded up to 4 for node tensors)
   bool isInt = false;     // create_node_tensor<int> (mask)
+  bool isBf16 = false;    // create_node_tensor<__nv_bfloat16>: a leaf feature matrix held as bf16 bits, ld elements
+                          // per row (H rounded up to 8); reached only through RuntimeImpl::data_bf16, never as float*
   bool isWeight = false;
   bool requiresGrad = false;
   bool produced = false;  // output of some op
@@ -117,8 +119,9 @@ struct RuntimeImpl {
   void* dmalloc(size_t bytes);
   void dfree_all();
   int new_tensor(int64_t rows, int H, int64_t ld, bool isInt, bool isWeight);
-  float* data(int region);   // allocates on first use, zero-filled
-  float* grad(int region);
+  float* data(int region);   // allocates on first use, zero-filled; a bf16 tensor is an error
+  float* grad(int region);   // a bf16 tensor has no gradient: an error
+  uint16_t* data_bf16(int region);   // the bf16 tensor's bits, allocated on first use, zero-filled
   // append `halo` rows to the data / grad buffer of x (re-allocating and copying if it already exists)
   void grow_halo(TensorImpl& x, bool grad, int64_t halo);
   // map the other partitions' copies of x's data / grad buffer (collective: every rank calls it for the same tensor)
@@ -130,6 +133,7 @@ struct RuntimeImpl {
 };
 
 inline int64_t round_up4(int64_t x) { return (x + 3) / 4 * 4; }
+inline int64_t round_up8(int64_t x) { return (x + 7) / 8 * 8; }
 
 }  // namespace host
 }  // namespace roc

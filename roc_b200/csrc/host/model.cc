@@ -2,6 +2,7 @@
 // Mirrors gnn.cc:433-749 and the per-op .cc files of the reference; each op's
 // forward/backward enqueues C-ABI kernels (roc_b200.h) on the Runtime's stream
 // instead of launching a Legion index task.
+#include <cuda_bf16.h>
 #include <curand.h>
 #include <algorithm>
 #include <cmath>
@@ -46,6 +47,16 @@ Tensor Model::create_node_tensor<DATATYPE>(int _numHidden) const {
   t.dims[0] = _numHidden;
   t.dims[1] = myGraph.numNodes;
   t.region = ctx->new_tensor(local_rows(), _numHidden, round_up4(_numHidden), false, false);
+  return t;
+}
+template <>
+Tensor Model::create_node_tensor<__nv_bfloat16>(int _numHidden) const {
+  Tensor t(Tensor::NODE_TENSOR);
+  t.numDim = 2;
+  t.dims[0] = _numHidden;
+  t.dims[1] = myGraph.numNodes;
+  t.region = ctx->new_tensor(local_rows(), _numHidden, round_up8(_numHidden), false, false);
+  ctx->t(t.region).isBf16 = true;
   return t;
 }
 template <>
@@ -222,6 +233,24 @@ ScatterGather* as_sum_sg(GnnOp* op) {
 bool Model::init(const Config& config) {
   (void)config;
   RuntimeImpl* rt = ctx;
+  // a bf16 tensor is read by linear (its X) and dropout only; any other op would need an fp32 view of it
+  for (size_t l = 0; l < layers.size(); l++) {
+    GnnOp* op = layers[l];
+    const bool takesBf16 = as<Linear>(op) || as<Dropout>(op);
+    for (int j = 0; j < op->numInputs; j++) {
+      const int r = op->inputs[j].region;
+      if (r < 0 || !rt->t(r).isBf16 || (takesBf16 && j == 0)) continue;
+      const ScatterGather* sgl = as<ScatterGather>(op);
+      const char* nm = sgl ? (sgl->aggr == AGGR_MAX ? "scatter_gather(max)" : sgl->aggr == AGGR_MIN ? "scatter_gather(min)"
+                                                                                                    : "scatter_gather") :
+                       as<AttentionGather>(op) ? "attention_gather" :
+                       as<WeightedScatterGather>(op) ? "scatter_gather(weighted)" :
+                       as<InDegreeNorm>(op) ? "indegree_norm" :
+                       as<Activation>(op) ? (as<Activation>(op)->actiMode == AC_MODE_RELU ? "relu" : "sigmoid") :
+                       as<Element>(op) ? "add" : as<SoftmaxCrossEntropy>(op) ? "softmax_cross_entropy" : "op";
+      ROC_FATAL((std::string(nm) + " cannot read a bf16 tensor: only linear and dropout take bf16 input").c_str());
+    }
+  }
   myGraph.maxHidden = 0;
   for (size_t i = 0; i < layers.size(); i++) {
     for (int j = 0; j < layers[i]->numOutputs; j++)
@@ -496,6 +525,21 @@ void Model::zero_gradients(void) {
 void Model::set_tensor(const Tensor& t, const void* host, bool grad) {
   RuntimeImpl* rt = ctx;
   TensorImpl& x = rt->t(t.region);
+  if (x.isBf16) {
+    // fp32 host rows, rounded on the device chunk by chunk: no full-size fp32 copy is ever resident
+    if (grad) ROC_FATAL("set_tensor(grad=true): a bf16 tensor has no gradient");
+    uint16_t* dst = rt->data_bf16(t.region);
+    const int64_t chunkRows = std::max<int64_t>(1, (int64_t)(64u << 20) / x.H);
+    rt->ensure_staging((size_t)std::min<int64_t>(chunkRows, x.rows) * x.H * sizeof(float));
+    const float* h = static_cast<const float*>(host);
+    for (int64_t r0 = 0; r0 < x.rows; r0 += chunkRows) {
+      const int64_t nr = std::min<int64_t>(chunkRows, x.rows - r0);
+      ROC_CHECK(cudaMemcpyAsync(rt->staging, h + r0 * x.H, (size_t)nr * x.H * 4, cudaMemcpyHostToDevice, rt->stream));
+      ROC_CHECK(roc_f32_to_bf16(nr, x.H, (const float*)rt->staging, x.H, dst + r0 * x.ld, x.ld, rt->stream));
+    }
+    ROC_CHECK(cudaStreamSynchronize(rt->stream));
+    return;
+  }
   float* dst = grad ? rt->grad(t.region) : rt->data(t.region);
   if (x.ld == x.H || x.isInt) {
     ROC_CHECK(cudaMemcpyAsync(dst, host, (size_t)x.rows * x.H * 4, cudaMemcpyHostToDevice, rt->stream));
@@ -518,9 +562,42 @@ void Model::set_tensor(const Tensor& t, const void* host, bool grad) {
 void Model::get_tensor(const Tensor& t, void* host, bool grad) const {
   RuntimeImpl* rt = ctx;
   TensorImpl& x = rt->t(t.region);
+  if (x.isBf16) {
+    // widened exactly on the device into staging, chunk by chunk
+    if (grad) ROC_FATAL("get_tensor(grad=true): a bf16 tensor has no gradient");
+    const uint16_t* src = rt->data_bf16(t.region);
+    const int64_t chunkRows = std::max<int64_t>(1, (int64_t)(64u << 20) / x.H);
+    rt->ensure_staging((size_t)std::min<int64_t>(chunkRows, x.rows) * x.H * sizeof(float));
+    float* h = static_cast<float*>(host);
+    for (int64_t r0 = 0; r0 < x.rows; r0 += chunkRows) {
+      const int64_t nr = std::min<int64_t>(chunkRows, x.rows - r0);
+      ROC_CHECK(roc_bf16_to_f32(nr, x.H, src + r0 * x.ld, x.ld, (float*)rt->staging, x.H, rt->stream));
+      ROC_CHECK(cudaMemcpyAsync(h + r0 * x.H, rt->staging, (size_t)nr * x.H * 4, cudaMemcpyDeviceToHost, rt->stream));
+      ROC_CHECK(cudaStreamSynchronize(rt->stream));   // the next chunk reuses the staging buffer
+    }
+    return;
+  }
   const float* src = grad ? rt->grad(t.region) : rt->data(t.region);
   ROC_CHECK(cudaMemcpy2DAsync(host, (size_t)x.H * 4, src, (size_t)x.ld * 4, (size_t)x.H * 4, (size_t)x.rows,
                               cudaMemcpyDeviceToHost, rt->stream));
+  ROC_CHECK(cudaStreamSynchronize(rt->stream));
+}
+
+void Model::set_tensor_bf16(const Tensor& t, const uint16_t* host) {
+  RuntimeImpl* rt = ctx;
+  TensorImpl& x = rt->t(t.region);
+  if (!x.isBf16) ROC_FATAL("set_tensor_bf16: not a bf16 tensor");
+  ROC_CHECK(cudaMemcpy2DAsync(rt->data_bf16(t.region), (size_t)x.ld * 2, host, (size_t)x.H * 2, (size_t)x.H * 2,
+                              (size_t)x.rows, cudaMemcpyHostToDevice, rt->stream));
+  ROC_CHECK(cudaStreamSynchronize(rt->stream));
+}
+
+void Model::get_tensor_bf16(const Tensor& t, uint16_t* host) const {
+  RuntimeImpl* rt = ctx;
+  TensorImpl& x = rt->t(t.region);
+  if (!x.isBf16) ROC_FATAL("get_tensor_bf16: not a bf16 tensor");
+  ROC_CHECK(cudaMemcpy2DAsync(host, (size_t)x.H * 2, rt->data_bf16(t.region), (size_t)x.ld * 2, (size_t)x.H * 2,
+                              (size_t)x.rows, cudaMemcpyDeviceToHost, rt->stream));
   ROC_CHECK(cudaStreamSynchronize(rt->stream));
 }
 
@@ -1042,8 +1119,19 @@ void Linear::forward(const Model& model) {
     if (f.rate > 0.0f)
       ROC_CHECK(roc_dropout_mask(model.local_rows(), inDim, g.rowLeft, f.rate, f.key, rt->trainStep,
                                  dropMask, dropLd, rt->stream));
-    const float* X = rt->data(f.inRegion);
     const int64_t ldX = rt->t(f.inRegion).ld;
+    if (rt->t(f.inRegion).isBf16) {
+      const uint16_t* Xb = rt->data_bf16(f.inRegion);
+      for (size_t k = 0; k < pipe.blocks(); k++) {
+        const int64_t r0 = pipe.row0(k), nr = pipe.rows(k, model.local_rows());
+        ROC_CHECK(roc_linear_fwd_bf16(nr, inDim, outDim, Xb + r0 * ldX, ldX, rt->data(weight.region), Y + r0 * ldY, ldY,
+                                      (int)activation, flags, g.d_rowEnd + r0, pipe.colLeft(k),
+                                      f.rate > 0.0f ? dropMask + r0 * dropLd : NULL, dropLd, f.rate, rt->stream));
+        pipe.pushed(k, Y, ldY, outDim);
+      }
+      return;
+    }
+    const float* X = rt->data(f.inRegion);
     for (size_t k = 0; k < pipe.blocks(); k++) {
       const int64_t r0 = pipe.row0(k), nr = pipe.rows(k, model.local_rows());
       ROC_CHECK(roc_linear_fwd_dropout(nr, inDim, outDim, X + r0 * ldX, ldX, rt->data(weight.region), Y + r0 * ldY, ldY,
@@ -1053,8 +1141,19 @@ void Linear::forward(const Model& model) {
     }
     return;
   }
-  const float* X = rt->data(inputs[0].region);
   const int64_t ldX = rt->t(inputs[0].region).ld;
+  if (rt->t(inputs[0].region).isBf16) {   // a bf16 leaf X, read directly by the GEMM
+    const uint16_t* Xb = rt->data_bf16(inputs[0].region);
+    for (size_t k = 0; k < pipe.blocks(); k++) {
+      const int64_t r0 = pipe.row0(k), nr = pipe.rows(k, model.local_rows());
+      ROC_CHECK(roc_linear_fwd_bf16(nr, inDim, outDim, Xb + r0 * ldX, ldX, rt->data(weight.region), Y + r0 * ldY, ldY,
+                                    (int)activation, flags, g.d_rowEnd + r0, pipe.colLeft(k), NULL, 0, 0.0f,
+                                    rt->stream));
+      pipe.pushed(k, Y, ldY, outDim);
+    }
+    return;
+  }
+  const float* X = rt->data(inputs[0].region);
   for (size_t k = 0; k < pipe.blocks(); k++) {
     const int64_t r0 = pipe.row0(k), nr = pipe.rows(k, model.local_rows());
     ROC_CHECK(roc_linear_fwd(nr, inDim, outDim, X + r0 * ldX, ldX, rt->data(weight.region), Y + r0 * ldY, ldY,
@@ -1079,6 +1178,17 @@ void Linear::backward(const Model& model) {
     xRegion = f.inRegion;
     a.accumulate_dX = 0;
     a.dropMask = dropMask; a.ldMask = dropLd; a.dropRate = f.rate;
+  }
+  if (rt->t(xRegion).isBf16) {
+    // a bf16 X is a leaf: dW only (with the relu backward of dY when activation is RELU); the same bits as the fp32
+    // path on the widened X
+    ROC_ASSERT(!rt->t(xRegion).requiresGrad);
+    const int yr = outputs[0].region;
+    ROC_CHECK(roc_linear_dw_bf16(model.local_rows(), (int)weight.dims[0], (int)weight.dims[1], rt->data_bf16(xRegion),
+                                 rt->t(xRegion).ld, activation != AC_MODE_NONE ? rt->data(yr) : NULL, rt->t(yr).ld,
+                                 rt->grad(gy), rt->t(gy).ld, rt->grad(weight.region), (int)activation, rt->linWs,
+                                 rt->linWsBytes, a.dropMask, a.ldMask, a.dropRate, rt->stream));
+    return;
   }
   const int dxRegion = dxOut >= 0 ? dxOut : xRegion;
   a.rows = model.local_rows(); a.inDim = (int)weight.dims[0]; a.outDim = (int)weight.dims[1];
@@ -1184,6 +1294,12 @@ void Dropout::forward(const Model& model) {
   // train: masked scale (dropout_kernel.cu:98-99); infer: plain copy (:159-180)
   const float r = (model.mode == MD_MODE_TRAIN) ? rate : 0.0f;
   const uint64_t key = ((uint64_t)(uint32_t)seed << 32) | (uint32_t)opIndex;
+  if (rt->t(inputs[0].region).isBf16) {   // bf16 in, fp32 out; rate 0 is the widening copy
+    ROC_CHECK(roc_dropout_fwd_bf16(model.local_rows(), (int)inputs[0].dims[0], model.myGraph.rowLeft, r, key,
+                                   rt->trainStep, rt->data_bf16(inputs[0].region), rt->t(inputs[0].region).ld,
+                                   rt->data(outputs[0].region), rt->t(outputs[0].region).ld, rt->stream));
+    return;
+  }
   ROC_CHECK(roc_dropout_fwd(model.local_rows(), (int)inputs[0].dims[0], model.myGraph.rowLeft, r, key, rt->trainStep,
                             rt->data(inputs[0].region), rt->t(inputs[0].region).ld, rt->data(outputs[0].region),
                             rt->t(outputs[0].region).ld, rt->stream));

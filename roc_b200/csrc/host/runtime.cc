@@ -46,6 +46,7 @@ int RuntimeImpl::new_tensor(int64_t rows, int H, int64_t ld, bool isInt, bool is
 
 float* RuntimeImpl::data(int region) {
   TensorImpl& x = t(region);
+  if (x.isBf16) ROC_FATAL("a bf16 node tensor was read as fp32: only linear and dropout take bf16 input");
   if (!x.data) {
     size_t bytes = (size_t)(x.rows + x.haloData) * (size_t)x.ld * sizeof(float);
     x.data = (float*)dmalloc(bytes);
@@ -54,8 +55,20 @@ float* RuntimeImpl::data(int region) {
   return x.data;
 }
 
+uint16_t* RuntimeImpl::data_bf16(int region) {
+  TensorImpl& x = t(region);
+  ROC_ASSERT(x.isBf16);
+  if (!x.data) {
+    size_t bytes = (size_t)x.rows * (size_t)x.ld * sizeof(uint16_t);
+    x.data = (float*)dmalloc(bytes);   // the untyped buffer; every access goes through this accessor
+    ROC_CHECK(cudaMemsetAsync(x.data, 0, bytes ? bytes : 16, stream));
+  }
+  return reinterpret_cast<uint16_t*>(x.data);
+}
+
 float* RuntimeImpl::grad(int region) {
   TensorImpl& x = t(region);
+  if (x.isBf16) ROC_FATAL("a bf16 node tensor has no gradient");
   if (!x.grad) {
     size_t bytes = (size_t)(x.rows + x.haloGrad) * (size_t)x.ld * sizeof(float);
     x.grad = (float*)dmalloc(bytes);

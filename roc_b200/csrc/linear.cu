@@ -6,29 +6,30 @@
 
 namespace roc {
 int simt_dw_splits(int64_t rows, int inDim, int outDim);
-int simt_linear_fwd(int64_t rows, int inDim, int outDim, const float* X, int64_t ldX, const float* W, float* Y,
-                    int64_t ldY, int relu, const uint64_t* rowEnd, uint64_t colLeft, const DropMask* dm,
+// X / ldX of the forward and dW: fp32, or bf16 (raw bits) when xBf16
+int simt_linear_fwd(int64_t rows, int inDim, int outDim, const void* X, bool xBf16, int64_t ldX, const float* W,
+                    float* Y, int64_t ldY, int relu, const uint64_t* rowEnd, uint64_t colLeft, const DropMask* dm,
                     cudaStream_t st);
 int simt_linear_dx(int64_t rows, int inDim, int outDim, const float* dY, int64_t ldDY, const float* W, float* dX,
                    int64_t ldDX, int accumulate, const DropMask* dm, const float* reluOf, int64_t ldR,
                    const uint64_t* rowEnd, uint64_t colLeft, cudaStream_t st);
-int simt_linear_dw(int64_t rows, int inDim, int outDim, const float* X, int64_t ldX, const float* dY, int64_t ldDY,
-                   float* dW, float* workspace, size_t wsBytes, const DropMask* dm, cudaStream_t st,
+int simt_linear_dw(int64_t rows, int inDim, int outDim, const void* X, bool xBf16, int64_t ldX, const float* dY,
+                   int64_t ldDY, float* dW, float* workspace, size_t wsBytes, const DropMask* dm, cudaStream_t st,
                    roc_gemm_info* info);
 int relu_bwd_inplace(int64_t rows, int H, const float* Y, int64_t ldY, float* dY, int64_t ldDY, cudaStream_t st);
 
 // tensor-core path (linear_tc.cu, linear_tc_dw.cu); each returns ROC_ERR_UNSUPPORTED when the
 // shape / alignment is outside what the wgmma kernels take.
 // They describe the launch they made in *info (roc_last_gemm_info).
-int tc_linear_fwd(int64_t rows, int inDim, int outDim, const float* X, int64_t ldX, const float* W, float* Y,
-                  int64_t ldY, int relu, const uint64_t* rowEnd, uint64_t colLeft, const DropMask* dm,
+int tc_linear_fwd(int64_t rows, int inDim, int outDim, const void* X, bool xBf16, int64_t ldX, const float* W,
+                  float* Y, int64_t ldY, int relu, const uint64_t* rowEnd, uint64_t colLeft, const DropMask* dm,
                   cudaStream_t st, roc_gemm_info* info);
 int tc_linear_dx(int64_t rows, int inDim, int outDim, const float* dY, int64_t ldDY, const float* W, float* dX,
                  int64_t ldDX, int accumulate, const DropMask* dm, const float* reluOf, int64_t ldR,
                  const uint64_t* rowEnd, uint64_t colLeft, cudaStream_t st, roc_gemm_info* info);
 size_t tc_dw_workspace_bytes(int64_t rows, int inDim, int outDim);
-int tc_linear_dw(int64_t rows, int inDim, int outDim, const float* X, int64_t ldX, const float* dY, int64_t ldDY,
-                 float* dW, float* workspace, size_t wsBytes, const DropMask* dm, cudaStream_t st,
+int tc_linear_dw(int64_t rows, int inDim, int outDim, const void* X, bool xBf16, int64_t ldX, const float* dY,
+                 int64_t ldDY, float* dW, float* workspace, size_t wsBytes, const DropMask* dm, cudaStream_t st,
                  roc_gemm_info* info);
 
 // which kernel served the calling thread's last Linear GEMM of each kind, and how it was launched (test hook: the
@@ -71,8 +72,8 @@ static int mask_args(const uint32_t* mask, int64_t ldMask, float rate, int inDim
   return ROC_OK;
 }
 
-static int linear_fwd_impl(int64_t rows, int inDim, int outDim, const float* X, int64_t ldX, const float* W,
-                           float* Y, int64_t ldY, int activation, int flags, const roc_eid_t* rowEnd,
+static int linear_fwd_impl(int64_t rows, int inDim, int outDim, const void* X, bool xBf16, int64_t ldX,
+                           const float* W, float* Y, int64_t ldY, int activation, int flags, const roc_eid_t* rowEnd,
                            roc_eid_t colLeft, const DropMask* dm, roc_stream_t stream) {
   if (!X || !W || !Y || rows < 0 || inDim <= 0 || outDim <= 0 || ldX < inDim || ldY < outDim) return ROC_ERR_INVALID;
   if (activation != ROC_AC_MODE_NONE && activation != ROC_AC_MODE_RELU) return ROC_ERR_UNSUPPORTED;  // linear_kernel.cu:96
@@ -84,17 +85,18 @@ static int linear_fwd_impl(int64_t rows, int inDim, int outDim, const float* X, 
   return run_gemm(
       0,
       [&](roc_gemm_info* i) {
-        return tc_linear_fwd(rows, inDim, outDim, X, ldX, W, Y, ldY, relu, re, colLeft, dm, st, i);
+        return tc_linear_fwd(rows, inDim, outDim, X, xBf16, ldX, W, Y, ldY, relu, re, colLeft, dm, st, i);
       },
       [&](roc_gemm_info*) {
-        return simt_linear_fwd(rows, inDim, outDim, X, ldX, W, Y, ldY, relu, re, colLeft, dm, st);
+        return simt_linear_fwd(rows, inDim, outDim, X, xBf16, ldX, W, Y, ldY, relu, re, colLeft, dm, st);
       });
 }
 
 extern "C" int roc_linear_fwd(int64_t rows, int inDim, int outDim, const float* X, int64_t ldX, const float* W,
                               float* Y, int64_t ldY, int activation, int flags, const roc_eid_t* rowEnd,
                               roc_eid_t colLeft, roc_stream_t stream) {
-  return linear_fwd_impl(rows, inDim, outDim, X, ldX, W, Y, ldY, activation, flags, rowEnd, colLeft, nullptr, stream);
+  return linear_fwd_impl(rows, inDim, outDim, X, false, ldX, W, Y, ldY, activation, flags, rowEnd, colLeft, nullptr,
+                         stream);
 }
 
 extern "C" int roc_linear_fwd_dropout(int64_t rows, int inDim, int outDim, const float* X, int64_t ldX,
@@ -104,7 +106,21 @@ extern "C" int roc_linear_fwd_dropout(int64_t rows, int inDim, int outDim, const
   DropMask dm; const DropMask* use;
   int rc = mask_args(mask, ldMask, rate, inDim, &dm, &use);
   if (rc != ROC_OK) return rc;
-  return linear_fwd_impl(rows, inDim, outDim, X, ldX, W, Y, ldY, activation, flags, rowEnd, colLeft, use, stream);
+  return linear_fwd_impl(rows, inDim, outDim, X, false, ldX, W, Y, ldY, activation, flags, rowEnd, colLeft, use,
+                         stream);
+}
+
+extern "C" int roc_linear_fwd_bf16(int64_t rows, int inDim, int outDim, const uint16_t* X, int64_t ldX,
+                                   const float* W, float* Y, int64_t ldY, int activation, int flags,
+                                   const roc_eid_t* rowEnd, roc_eid_t colLeft, const uint32_t* mask, int64_t ldMask,
+                                   float rate, roc_stream_t stream) {
+  DropMask dm; const DropMask* use = nullptr;
+  if (mask || rate != 0.f) {
+    int rc = mask_args(mask, ldMask, rate, inDim, &dm, &use);
+    if (rc != ROC_OK) return rc;
+  }
+  return linear_fwd_impl(rows, inDim, outDim, X, true, ldX, W, Y, ldY, activation, flags, rowEnd, colLeft, use,
+                         stream);
 }
 
 extern "C" size_t roc_linear_bwd_workspace_bytes(int64_t rows, int inDim, int outDim) {
@@ -142,10 +158,10 @@ static int linear_bwd_impl(int64_t rows, int inDim, int outDim, const float* X, 
     int rc = run_gemm(
         1,
         [&](roc_gemm_info* i) {
-          return tc_linear_dw(rows, inDim, outDim, X, ldX, dY, ldDY, dW, ws, workspaceBytes, dm, st, i);
+          return tc_linear_dw(rows, inDim, outDim, X, false, ldX, dY, ldDY, dW, ws, workspaceBytes, dm, st, i);
         },
         [&](roc_gemm_info* i) {
-          return simt_linear_dw(rows, inDim, outDim, X, ldX, dY, ldDY, dW, ws, workspaceBytes, dm, st, i);
+          return simt_linear_dw(rows, inDim, outDim, X, false, ldX, dY, ldDY, dW, ws, workspaceBytes, dm, st, i);
         });
     if (rc != ROC_OK) return rc;
   }
@@ -195,6 +211,36 @@ extern "C" int roc_linear_bwd_fused(const roc_linear_bwd_args* a, roc_stream_t s
   return linear_bwd_impl(a->rows, a->inDim, a->outDim, a->X, a->ldX, a->W, a->Y, a->ldY, a->dY, a->ldDY, a->dW,
                          a->dX, a->ldDX, a->activation, a->accumulate_dX, a->workspace, a->workspaceBytes, use,
                          a->dxReluOf, a->ldReluOf, a->dxNormRowEnd, a->colLeft, stream, a->parts);
+}
+
+extern "C" int roc_linear_dw_bf16(int64_t rows, int inDim, int outDim, const uint16_t* X, int64_t ldX,
+                                  const float* Y, int64_t ldY, float* dY, int64_t ldDY, float* dW, int activation,
+                                  void* workspace, size_t workspaceBytes, const uint32_t* mask, int64_t ldMask,
+                                  float rate, roc_stream_t stream) {
+  DropMask dm; const DropMask* use = nullptr;
+  if (mask || rate != 0.f) {
+    int rc = mask_args(mask, ldMask, rate, inDim, &dm, &use);
+    if (rc != ROC_OK) return rc;
+  }
+  if (!X || !dY || !dW || !workspace || rows < 0 || inDim <= 0 || outDim <= 0 || ldX < inDim || ldDY < outDim)
+    return ROC_ERR_INVALID;
+  if (activation != ROC_AC_MODE_NONE && activation != ROC_AC_MODE_RELU) return ROC_ERR_UNSUPPORTED;
+  if (rows == 0) return ROC_OK;
+  cudaStream_t st = as_stream(stream);
+  if (activation == ROC_AC_MODE_RELU) {   // as roc_linear_bwd: dY = (Y > 0) ? dY : 0 in place
+    if (!Y || ldY < outDim) return ROC_ERR_INVALID;
+    int rc = relu_bwd_inplace(rows, outDim, Y, ldY, dY, ldDY, st);
+    if (rc != ROC_OK) return rc;
+  }
+  float* ws = (float*)workspace;
+  return run_gemm(
+      1,
+      [&](roc_gemm_info* i) {
+        return tc_linear_dw(rows, inDim, outDim, X, true, ldX, dY, ldDY, dW, ws, workspaceBytes, use, st, i);
+      },
+      [&](roc_gemm_info* i) {
+        return simt_linear_dw(rows, inDim, outDim, X, true, ldX, dY, ldDY, dW, ws, workspaceBytes, use, st, i);
+      });
 }
 
 extern "C" int roc_last_gemm_path(int which) { return (which >= 0 && which < 3) ? t_last[which].path : 0; }

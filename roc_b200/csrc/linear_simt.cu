@@ -16,8 +16,8 @@ constexpr int GB_M = 128, GB_N = 64, GB_K = 16, GT_M = 8, GT_N = 4;
 constexpr int G_THREADS = (GB_M / GT_M) * (GB_N / GT_N);  // 256
 
 struct GemmP {
-  const float* A; int64_t lda;
-  const float* B; int64_t ldb;
+  const void* A; int64_t lda;   // TA / TB elements (fp32, or bf16 bits for a bf16 X)
+  const void* B; int64_t ldb;
   float* C; int64_t ldc;
   int64_t M; int N; int64_t K;
   int64_t kPerSplit;      // K range per blockIdx.z
@@ -32,9 +32,12 @@ struct GemmP {
   const float* reluOf; int64_t ldR;   // epilogue relu backward: reluOf(m, n) > 0 ? v : 0 (NULL = none)
 };
 
-template <bool A_KCONTIG, bool B_KCONTIG>
+// TA / TB: element type of A / B, float or uint16_t (a bf16 X, widened exactly as it is loaded)
+template <bool A_KCONTIG, bool B_KCONTIG, class TA = float, class TB = float>
 __global__ void __launch_bounds__(G_THREADS)
 k_sgemm(const GemmP p) {
+  const TA* pA = static_cast<const TA*>(p.A);
+  const TB* pB = static_cast<const TB*>(p.B);
   __shared__ float As[GB_K][GB_M + 4];
   __shared__ float Bs[GB_K][GB_N + 4];
   const int tid = threadIdx.x;
@@ -59,7 +62,7 @@ k_sgemm(const GemmP p) {
       int64_t m = m0 + mm, k = k0 + kk;
       float v = 0.f;
       if (m < p.M && k < kEnd) {
-        v = A_KCONTIG ? p.A[m * p.lda + k] : p.A[k * p.lda + m];
+        v = to_f32(A_KCONTIG ? pA[m * p.lda + k] : pA[k * p.lda + m]);
         if (p.maskOn == 1) v = drop_apply(p.mask, p.ldm, p.mscale, m, (int)k, v);
       }
       As[kk][mm] = v;
@@ -72,7 +75,7 @@ k_sgemm(const GemmP p) {
       int n = n0 + nn; int64_t k = k0 + kk;
       float v = 0.f;
       if (n < p.N && k < kEnd) {
-        v = B_KCONTIG ? p.B[(int64_t)n * p.ldb + k] : p.B[k * p.ldb + n];
+        v = to_f32(B_KCONTIG ? pB[(int64_t)n * p.ldb + k] : pB[k * p.ldb + n]);
         if (p.maskOn == 2) v = drop_apply(p.mask, p.ldm, p.mscale, k, n, v);
       }
       Bs[kk][nn] = v;
@@ -164,8 +167,9 @@ static void set_mask(GemmP& p, const DropMask* dm, int on) {
   p.mask = dm->bits; p.ldm = dm->ld; p.mscale = dm->scale; p.maskOn = on;
 }
 
-int simt_linear_fwd(int64_t rows, int inDim, int outDim, const float* X, int64_t ldX, const float* W, float* Y,
-                    int64_t ldY, int relu, const uint64_t* rowEnd, uint64_t colLeft, const DropMask* dm,
+// X is fp32, or bf16 (raw bits) when xBf16
+int simt_linear_fwd(int64_t rows, int inDim, int outDim, const void* X, bool xBf16, int64_t ldX, const float* W,
+                    float* Y, int64_t ldY, int relu, const uint64_t* rowEnd, uint64_t colLeft, const DropMask* dm,
                     cudaStream_t st) {
   GemmP p{};
   p.A = X; p.lda = ldX; p.B = W; p.ldb = inDim; p.C = Y; p.ldc = ldY;
@@ -173,7 +177,8 @@ int simt_linear_fwd(int64_t rows, int inDim, int outDim, const float* X, int64_t
   p.accumulate = 0; p.relu = relu; p.rowEnd = rowEnd; p.colLeft = colLeft;
   set_mask(p, dm, 1);
   dim3 grid((unsigned)((rows + GB_M - 1) / GB_M), (unsigned)((outDim + GB_N - 1) / GB_N), 1);
-  k_sgemm<true, true><<<grid, G_THREADS, 0, st>>>(p);
+  if (xBf16) k_sgemm<true, true, uint16_t, float><<<grid, G_THREADS, 0, st>>>(p);
+  else k_sgemm<true, true><<<grid, G_THREADS, 0, st>>>(p);
   ROC_LAUNCH_CHECK();
   return ROC_OK;
 }
@@ -192,8 +197,8 @@ int simt_linear_dx(int64_t rows, int inDim, int outDim, const float* dY, int64_t
   return ROC_OK;
 }
 
-int simt_linear_dw(int64_t rows, int inDim, int outDim, const float* X, int64_t ldX, const float* dY, int64_t ldDY,
-                   float* dW, float* workspace, size_t wsBytes, const DropMask* dm, cudaStream_t st,
+int simt_linear_dw(int64_t rows, int inDim, int outDim, const void* X, bool xBf16, int64_t ldX, const float* dY,
+                   int64_t ldDY, float* dW, float* workspace, size_t wsBytes, const DropMask* dm, cudaStream_t st,
                    roc_gemm_info* info) {
   int splits = simt_dw_splits(rows, inDim, outDim);
   int64_t count = (int64_t)inDim * outDim;
@@ -206,7 +211,8 @@ int simt_linear_dw(int64_t rows, int inDim, int outDim, const float* X, int64_t 
   set_mask(p, dm, 2);
   if (info) { info->splits = splits; info->v_per_split = p.kPerSplit; }
   dim3 grid((unsigned)((outDim + GB_M - 1) / GB_M), (unsigned)((inDim + GB_N - 1) / GB_N), (unsigned)splits);
-  k_sgemm<false, false><<<grid, G_THREADS, 0, st>>>(p);
+  if (xBf16) k_sgemm<false, false, float, uint16_t><<<grid, G_THREADS, 0, st>>>(p);
+  else k_sgemm<false, false><<<grid, G_THREADS, 0, st>>>(p);
   ROC_LAUNCH_CHECK();
   return splitk_reduce(count, splits, workspace, dW, st);
 }

@@ -29,8 +29,9 @@
 // drains only at the end of a tile.  The row ends of the norm divisors are loaded a tile ahead of their use,
 // so no global load waits in front of an MMA.
 // When the CTA's W_hi / W_lo slice (2 * 32 NC * Kpad floats) fits beside the epilogue buffers and a ring
-// of TC_RES_MIN_STAGES A stages, it is loaded once per CTA and the ring carries A alone; otherwise W streams
-// through the ring with A, from L2.  HBM-bound on A (rows*K*4 bytes read once).
+// of TC_RES_MIN_A_BYTES of A, it is loaded once per CTA and the ring carries A alone; otherwise W streams
+// through the ring with A, from L2.  A is read once (rows*K*4 bytes, or rows*K*2 for a bf16 A).
+// The forward of a leaf bf16 X runs the same kernel with TA = uint16_t (see k_tc_linear).
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -42,10 +43,12 @@ namespace roc {
 using namespace tc;
 
 constexpr int TC_BM = 128;        // rows per tile: two consumer warpgroups of 64
-constexpr int TC_BK = 32;         // fp32 per k-block = one 128-byte swizzle row
+constexpr int TC_BK = 32;         // k per k-block: one 128-byte swizzle row of fp32 A and of W, a 64-byte one of bf16 A
 constexpr int TC_THREADS = 288;   // 8 consumer warps + 1 producer warp
-constexpr int TC_MAX_STAGES = 8;
-constexpr int TC_RES_MIN_STAGES = 4;  // A stages a resident W must leave room for: 64 KB in flight per SM
+constexpr int TC_MAX_STAGES = 8;        // ring depth with fp32 A (16 KB of A per stage)
+constexpr int TC_MAX_STAGES_BF16 = 12;  // with bf16 A (8 KB per stage)
+constexpr int TC_BAR_STAGES = 12;       // full / empty barrier slots: the deeper of the two rings
+constexpr size_t TC_RES_MIN_A_BYTES = 64 * 1024;  // A in flight a resident W must leave room for, per SM
 
 // Whi/Wlo[n][k] (n < Npad, k < Kpad, zero padded) = split of B(n, k), where
 //   transposed == 0: B(n, k) = W[n * ldW + k]   (fwd: n = output o, k = input i, ldW = inDim)
@@ -116,7 +119,10 @@ __device__ __forceinline__ void tc_store_pair(const TcParams& p, bool fAcc, int6
 
 __device__ __forceinline__ void wgmma_wait_1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 
-template <int NC, int EPI>
+// TA: float, or uint16_t for an A in bf16 (the forward of a leaf bf16 X): its [128][32] box has 64-byte rows with the
+// 64-byte swizzle, and each element is widened exactly as the fragment is read, so everything after the load is the
+// fp32 kernel's arithmetic on A.float().
+template <int NC, int EPI, class TA>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_tc_linear(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapWhi,
             const __grid_constant__ CUtensorMap mapWlo, const __grid_constant__ CUtensorMap mapR,
@@ -124,15 +130,15 @@ k_tc_linear(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
             const __grid_constant__ CUtensorMap mapY,
             const TcParams p) {
   constexpr int BN = 32 * NC;
-  constexpr uint32_t aBytes = TC_BM * TC_BK * 4;       // 16 KB of A per stage
+  constexpr uint32_t aBytes = TC_BM * TC_BK * sizeof(TA);   // 16 KB (fp32) or 8 KB (bf16) of A per stage
   constexpr uint32_t bBytes = BN * TC_BK * 4;          // one k-block of W_hi (or W_lo)
   constexpr uint32_t rBytes = TC_BM * 32 * 4;          // one 32-column box of reluOf
   EPI_FLAGS(EPI, p)
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.barOff);   // [stages] TMA landed
-  uint64_t* empty = full + TC_MAX_STAGES;                          // [stages] consumers done
-  uint64_t* efull = empty + TC_MAX_STAGES;                         // [eb] epilogue operands landed
+  uint64_t* empty = full + TC_BAR_STAGES;                          // [stages] consumers done
+  uint64_t* efull = empty + TC_BAR_STAGES;                         // [eb] epilogue operands landed
   uint64_t* eempty = efull + 2;                                    // [eb] consumers have read them
   uint64_t* wfull = eempty + 2;                                    // resident W landed
 
@@ -233,7 +239,7 @@ k_tc_linear(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
     auto body = [&](int kb, uint32_t (&fr)[TC_BK / 8][2][4], uint32_t (&frPrev)[TC_BK / 8][2][4]) {
       mbar_wait(&full[s], ph);
       const uint8_t* st = smem + p.stageOff + (size_t)s * p.stageBytes;
-      const float* as = reinterpret_cast<const float*>(st);
+      const TA* as = reinterpret_cast<const TA*>(st);
       const uint32_t bHi = p.wres ? smem_u32(smem + (size_t)kb * bBytes) : smem_u32(st + aBytes);
       const uint32_t bLo = p.wres ? bHi + (uint32_t)p.numKb * bBytes : bHi + bBytes;
       // dropout fused into the operand load: bit c of mask[row][kb] keeps column 32 kb + c ([128][4] words by TMA,
@@ -246,9 +252,17 @@ k_tc_linear(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
       }
 #pragma unroll
       for (int kk = 0; kk < TC_BK / 8; kk++) {
-        // 128B swizzle: 16-byte chunk j of row r sits at chunk j ^ (r & 7); columns 8 kk + t and 8 kk + t + 4
-        const int o0 = (((2 * kk) ^ g) << 2) + t, o1 = (((2 * kk + 1) ^ g) << 2) + t;
-        float x[4] = {as[rl * TC_BK + o0], as[(rl + 8) * TC_BK + o0], as[rl * TC_BK + o1], as[(rl + 8) * TC_BK + o1]};
+        // columns 8 kk + t and 8 kk + t + 4 of rows rl and rl + 8.  fp32, 128B swizzle: 16-byte chunk j of row r sits
+        // at chunk j ^ (r & 7).  bf16, 64B swizzle: chunk j (8 elements) of row r at j ^ ((r >> 1) & 3), the same for
+        // rl and rl + 8; the 8 rows of a warp then read 8 distinct 4-bank groups
+        int o0, o1;
+        if constexpr (sizeof(TA) == 4) {
+          o0 = (((2 * kk) ^ g) << 2) + t; o1 = (((2 * kk + 1) ^ g) << 2) + t;
+        } else {
+          o0 = ((kk ^ ((rl >> 1) & 3)) << 3) + t; o1 = o0 + 4;
+        }
+        float x[4] = {to_f32(as[rl * TC_BK + o0]), to_f32(as[(rl + 8) * TC_BK + o0]), to_f32(as[rl * TC_BK + o1]),
+                      to_f32(as[(rl + 8) * TC_BK + o1])};
         if (masked) {
           const int b0 = 8 * kk + t, b1 = b0 + 4;
           x[0] = ((mw0 >> b0) & 1u) ? x[0] * p.mscale : 0.f;   // == k_dropout
@@ -403,29 +417,40 @@ static int tc_instance(int epi) {
 
 struct TcMaps { CUtensorMap A, Whi, Wlo, R, M, IM, Y; };
 
-template <int NC, int EPI>
+template <int NC, int EPI, class TA>
 static int tc_launch_epi(dim3 grid, size_t smemBytes, const TcMaps& m, const TcParams& q, cudaStream_t st) {
-  return launch_dyn<k_tc_linear<NC, EPI>>(grid, TC_THREADS, smemBytes, st, m.A, m.Whi, m.Wlo, m.R, m.M, m.IM, m.Y, q);
+  return launch_dyn<k_tc_linear<NC, EPI, TA>>(grid, TC_THREADS, smemBytes, st, m.A, m.Whi, m.Wlo, m.R, m.M, m.IM, m.Y,
+                                              q);
 }
 
-template <int NC>
+template <int NC, class TA>
 static int tc_launch(dim3 grid, size_t smemBytes, int epi, const TcMaps& m, const TcParams& q, cudaStream_t st) {
   constexpr int E1 = EPI_NORM, E2 = EPI_OMASK, E3 = EPI_OMASK | EPI_RELUOF | EPI_NORM;
-  switch (tc_instance(epi)) {
-    case 0: return tc_launch_epi<NC, 0>(grid, smemBytes, m, q, st);
-    case E1: return tc_launch_epi<NC, E1>(grid, smemBytes, m, q, st);
-    case E2: return tc_launch_epi<NC, E2>(grid, smemBytes, m, q, st);
-    case E3: return tc_launch_epi<NC, E3>(grid, smemBytes, m, q, st);
-    default: return tc_launch_epi<NC, -1>(grid, smemBytes, m, q, st);
+  if constexpr (sizeof(TA) == 2) {
+    // a bf16 A is a leaf X in a forward: its epilogues are relu and the norm, so the dX instantiations are not built
+    switch (tc_instance(epi)) {
+      case 0: return tc_launch_epi<NC, 0, TA>(grid, smemBytes, m, q, st);
+      case E1: return tc_launch_epi<NC, E1, TA>(grid, smemBytes, m, q, st);
+      default: return tc_launch_epi<NC, -1, TA>(grid, smemBytes, m, q, st);
+    }
+  } else {
+    switch (tc_instance(epi)) {
+      case 0: return tc_launch_epi<NC, 0, TA>(grid, smemBytes, m, q, st);
+      case E1: return tc_launch_epi<NC, E1, TA>(grid, smemBytes, m, q, st);
+      case E2: return tc_launch_epi<NC, E2, TA>(grid, smemBytes, m, q, st);
+      case E3: return tc_launch_epi<NC, E3, TA>(grid, smemBytes, m, q, st);
+      default: return tc_launch_epi<NC, -1, TA>(grid, smemBytes, m, q, st);
+    }
   }
 }
 
-// Y[rows][N] (op)= A[rows][K] * B^T with B(n, k) taken from W as k_split_w describes
-static int ts_gemm(int64_t rows, int K, int N, const float* A, int64_t ldA, const float* W, int ldW, int transposed,
-                   float* Y, int64_t ldY, const DropMask* inMask, const TsEpilogue& e, cudaStream_t st,
-                   roc_gemm_info* info) {
+// Y[rows][N] (op)= A[rows][K] * B^T with B(n, k) taken from W as k_split_w describes; A is fp32, or bf16 (raw bits)
+// when aBf16
+static int ts_gemm(int64_t rows, int K, int N, const void* A, bool aBf16, int64_t ldA, const float* W, int ldW,
+                   int transposed, float* Y, int64_t ldY, const DropMask* inMask, const TsEpilogue& e,
+                   cudaStream_t st, roc_gemm_info* info) {
   if (K < 8 || N < 1 || rows < 1) return ROC_ERR_UNSUPPORTED;
-  if ((ldA % 4) || (ldY % 4) || !aligned16(A) || !aligned16(Y)) return ROC_ERR_UNSUPPORTED;
+  if ((ldA % (aBf16 ? 8 : 4)) || (ldY % 4) || !aligned16(A) || !aligned16(Y)) return ROC_ERR_UNSUPPORTED;
   if (e.reluOf && ((e.ldR % 4) || !aligned16(e.reluOf))) return ROC_ERR_UNSUPPORTED;
   if (e.outMask && !aligned16(e.outMask->bits)) return ROC_ERR_UNSUPPORTED;   // TMA takes the words [128][4] per tile
   if (inMask && !aligned16(inMask->bits)) return ROC_ERR_UNSUPPORTED;         // and [128][4] per k-block
@@ -451,7 +476,11 @@ static int ts_gemm(int64_t rows, int K, int N, const float* A, int64_t ldA, cons
 
   TcMaps m;
   memset(&m, 0, sizeof(m));
-  if (!make_tmap_f32_2d(&m.A, A, (uint64_t)rows, (uint64_t)K, (uint64_t)ldA, TC_BM, TC_BK)) return ROC_ERR_UNSUPPORTED;
+  if (aBf16 ? !make_tmap_bf16_2d(&m.A, static_cast<const uint16_t*>(A), (uint64_t)rows, (uint64_t)K, (uint64_t)ldA,
+                                 TC_BM, TC_BK)
+            : !make_tmap_f32_2d(&m.A, static_cast<const float*>(A), (uint64_t)rows, (uint64_t)K, (uint64_t)ldA, TC_BM,
+                                TC_BK))
+    return ROC_ERR_UNSUPPORTED;
   if (!make_tmap_f32_2d(&m.Whi, Whi, (uint64_t)Npad, (uint64_t)Kpad, (uint64_t)Kpad, (uint32_t)BN, TC_BK)) return ROC_ERR_UNSUPPORTED;
   if (!make_tmap_f32_2d(&m.Wlo, Wlo, (uint64_t)Npad, (uint64_t)Kpad, (uint64_t)Kpad, (uint32_t)BN, TC_BK)) return ROC_ERR_UNSUPPORTED;
   if (e.reluOf && !make_tmap_f32_2d(&m.R, e.reluOf, (uint64_t)rows, (uint64_t)N, (uint64_t)e.ldR, TC_BM, 32))
@@ -469,20 +498,23 @@ static int ts_gemm(int64_t rows, int K, int N, const float* A, int64_t ldA, cons
   if (ystage && !make_tmap_f32_2d(&m.Y, Y, (uint64_t)rows, (uint64_t)yCols, (uint64_t)ldY, TC_BM / 2, 32))
     return ROC_ERR_UNSUPPORTED;
 
-  // Shared memory: W resident when its slice fits beside both epilogue buffers, the Y staging tile and a ring of
-  // TC_RES_MIN_STAGES A stages; then two epilogue buffers when they leave a ring of 2, else one.
+  // Shared memory: W resident when its slice fits beside both epilogue buffers, the Y staging tile and a ring that
+  // holds TC_RES_MIN_A_BYTES of A (4 fp32 stages, 8 bf16 ones); then two epilogue buffers when they leave a ring of 2,
+  // else one.  A bf16 stage is half as large, so its ring may be deeper, up to the same bytes of A as fp32's 8 stages.
   const int numKb = Kpad / TC_BK;
-  const size_t aBytes = (size_t)TC_BM * TC_BK * 4, bBytes = (size_t)BN * TC_BK * 4;
+  const size_t aBytes = (size_t)TC_BM * TC_BK * (aBf16 ? 2 : 4), bBytes = (size_t)BN * TC_BK * 4;
+  const int maxStages = aBf16 ? TC_MAX_STAGES_BF16 : TC_MAX_STAGES;
+  const int resMinStages = (int)(TC_RES_MIN_A_BYTES / aBytes);
   const size_t mBytes = inMask ? (size_t)TC_BM * 4 * 4 : 0;
   const size_t wBytes = 2 * (size_t)numKb * bBytes;
   const size_t eBytes = (e.reluOf ? (size_t)TC_BM * BN * 4 : 0) + (e.outMask ? (size_t)TC_BM * 4 * 4 : 0);
   const size_t yBytes = ystage ? (size_t)TC_BM * BN * 4 : 0;
   const size_t fixedBytes = 1024 /*align*/ + 256 /*barriers*/ + yBytes;
-  const bool wres = ring_stages(aBytes + mBytes, fixedBytes + wBytes + 2 * eBytes, TC_MAX_STAGES) >= TC_RES_MIN_STAGES;
+  const bool wres = ring_stages(aBytes + mBytes, fixedBytes + wBytes + 2 * eBytes, maxStages) >= resMinStages;
   const size_t stageBytes = aBytes + (wres ? 0 : 2 * bBytes) + mBytes;
   const size_t wUsed = wres ? wBytes : 0;
-  const int eb = !eBytes ? 0 : ring_stages(stageBytes, fixedBytes + wUsed + 2 * eBytes, TC_MAX_STAGES) ? 2 : 1;
-  const int stages = ring_stages(stageBytes, fixedBytes + wUsed + eb * eBytes, TC_MAX_STAGES);
+  const int eb = !eBytes ? 0 : ring_stages(stageBytes, fixedBytes + wUsed + 2 * eBytes, maxStages) ? 2 : 1;
+  const int stages = ring_stages(stageBytes, fixedBytes + wUsed + eb * eBytes, maxStages);
   if (!stages) return ROC_ERR_UNSUPPORTED;
   TcParams q{};
   q.Y = Y; q.ldY = ldY; q.rows = rows; q.outDim = N; q.numKb = numKb; q.stages = stages;
@@ -510,19 +542,27 @@ static int ts_gemm(int64_t rows, int K, int N, const float* A, int64_t ldA, cons
     info->nc = NC; info->epi = tc_instance(epi); info->grid_x = (int)grid.x; info->grid_y = (int)grid.y;
     info->stages = stages; info->w_resident = wres; info->epi_bufs = eb;
   }
+  if (aBf16) {
+    switch (NC) {
+      case 1: return tc_launch<1, uint16_t>(grid, smemBytes, epi, m, q, st);
+      case 2: return tc_launch<2, uint16_t>(grid, smemBytes, epi, m, q, st);
+      default: return tc_launch<4, uint16_t>(grid, smemBytes, epi, m, q, st);
+    }
+  }
   switch (NC) {
-    case 1: return tc_launch<1>(grid, smemBytes, epi, m, q, st);
-    case 2: return tc_launch<2>(grid, smemBytes, epi, m, q, st);
-    default: return tc_launch<4>(grid, smemBytes, epi, m, q, st);
+    case 1: return tc_launch<1, float>(grid, smemBytes, epi, m, q, st);
+    case 2: return tc_launch<2, float>(grid, smemBytes, epi, m, q, st);
+    default: return tc_launch<4, float>(grid, smemBytes, epi, m, q, st);
   }
 }
 
-int tc_linear_fwd(int64_t rows, int inDim, int outDim, const float* X, int64_t ldX, const float* W, float* Y,
-                  int64_t ldY, int relu, const uint64_t* rowEnd, uint64_t colLeft, const DropMask* dm,
+// X is fp32, or bf16 (raw bits) when xBf16
+int tc_linear_fwd(int64_t rows, int inDim, int outDim, const void* X, bool xBf16, int64_t ldX, const float* W,
+                  float* Y, int64_t ldY, int relu, const uint64_t* rowEnd, uint64_t colLeft, const DropMask* dm,
                   cudaStream_t st, roc_gemm_info* info) {
   TsEpilogue e;
   e.relu = relu; e.rowEnd = rowEnd; e.colLeft = colLeft;
-  return ts_gemm(rows, inDim, outDim, X, ldX, W, inDim, 0, Y, ldY, dm, e, st, info);
+  return ts_gemm(rows, inDim, outDim, X, xBf16, ldX, W, inDim, 0, Y, ldY, dm, e, st, info);
 }
 
 // dX (+)= dY W, optionally followed in the epilogue by the dropout backward of X's producer
@@ -532,7 +572,7 @@ int tc_linear_dx(int64_t rows, int inDim, int outDim, const float* dY, int64_t l
   TsEpilogue e;
   e.outMask = dm; e.accumulate = accumulate;
   e.reluOf = reluOf; e.ldR = ldR; e.rowEnd = rowEnd; e.colLeft = colLeft;
-  return ts_gemm(rows, outDim, inDim, dY, ldDY, W, inDim, 1, dX, ldDX, nullptr, e, st, info);
+  return ts_gemm(rows, outDim, inDim, dY, false, ldDY, W, inDim, 1, dX, ldDX, nullptr, e, st, info);
 }
 
 }  // namespace roc

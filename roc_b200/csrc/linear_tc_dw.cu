@@ -35,6 +35,8 @@
 //   into a second register set.  One CTA-wide barrier per block publishes the next dY^T buffer and certifies
 //   that both warpgroups' MMAs of the previous block have retired (which frees that buffer and the ring
 //   stage).
+// A bf16 X (a leaf node tensor) takes the same two kernels with 64-byte X box rows and the 64-byte swizzle; each
+// element is widened exactly as its fragment is read, so dW is the fp32 kernel's on X.float(), bit for bit.
 #include <cstdlib>
 #include <cstring>
 #include "common.cuh"
@@ -72,9 +74,12 @@ __device__ __forceinline__ int dw_col(int w, int g, int h) {
   return (w >> 1) * DW_XBOX + (g >> 2) * 16 + (w & 1) * 8 + h * 4 + (g & 3);
 }
 
-// What a consumer thread needs to find its A fragment: the offsets of (vertex t + 4 e, column c) of k8 step 0 in the
-// swizzled X boxes, box(c) * 32 KS + (t + 4 e) * 32 + ((c % 32 / 4) ^ (t + 4 e)) * 4 + c % 4, and the mask bits of
-// its two columns.
+// What a consumer thread needs to find its A fragment: the element offsets of (vertex k = t + 4 e, column c) of k8
+// step 0 in the swizzled X boxes, and the mask bits of its two columns.  fp32 X (TX = float, 128-byte swizzle):
+// box(c) * 32 KS + k * 32 + ((c % 32 / 4) ^ k) * 4 + c % 4.  bf16 X (TX = uint16_t, rows of 64 bytes, 64-byte
+// swizzle): box(c) * 32 KS + k * 32 + ((c % 32 / 8) ^ ((k / 2) % 4)) * 8 + c % 8.  Either swizzle term is the same
+// for vertex k + 8 kk, so the k8 steps add 8 kk * 32 elements.
+template <class TX>
 struct DwLane {
   int ca, cb;       // X columns of this thread in the tile
   int xo[2][2];
@@ -87,7 +92,11 @@ struct DwLane {
 #pragma unroll
       for (int e = 0; e < 2; e++) {
         const int c = h ? cb : ca, k = t + 4 * e;
-        xo[h][e] = (c / DW_XBOX) * (DW_KS * DW_XBOX) + k * DW_XBOX + ((((c % DW_XBOX) >> 2) ^ k) << 2) + (c & 3);
+        if constexpr (sizeof(TX) == 4)
+          xo[h][e] = (c / DW_XBOX) * (DW_KS * DW_XBOX) + k * DW_XBOX + ((((c % DW_XBOX) >> 2) ^ k) << 2) + (c & 3);
+        else
+          xo[h][e] = (c / DW_XBOX) * (DW_KS * DW_XBOX) + k * DW_XBOX + ((((c % DW_XBOX) >> 3) ^ ((k >> 1) & 3)) << 3) +
+                     (c & 7);
       }
     mb0 = ca & 31; mb1 = cb & 31;
   }
@@ -114,13 +123,15 @@ __device__ __forceinline__ void dw_transpose(const float* ys, float* hiT, float*
 }
 
 // A fragments (hi, lo) of every k8 step of the block whose X boxes start at xs; mw[2 kk + e] is the mask word of
-// vertex 8 kk + 4 e + t (all ones without a mask)
-__device__ __forceinline__ void dw_fragments(const float* xs, const DwLane& L, bool masked, float mscale,
+// vertex 8 kk + 4 e + t (all ones without a mask).  A bf16 X is widened exactly as it is read.
+template <class TX>
+__device__ __forceinline__ void dw_fragments(const TX* xs, const DwLane<TX>& L, bool masked, float mscale,
                                              const uint32_t (&mw)[8], uint32_t (&fr)[DW_KS / 8][2][4]) {
 #pragma unroll
   for (int kk = 0; kk < DW_KS / 8; kk++) {
     const int kb = kk * 8 * DW_XBOX;
-    float x[4] = {xs[kb + L.xo[0][0]], xs[kb + L.xo[1][0]], xs[kb + L.xo[0][1]], xs[kb + L.xo[1][1]]};
+    float x[4] = {to_f32(xs[kb + L.xo[0][0]]), to_f32(xs[kb + L.xo[1][0]]), to_f32(xs[kb + L.xo[0][1]]),
+                  to_f32(xs[kb + L.xo[1][1]])};
     if (masked) {
       const uint32_t m0 = mw[2 * kk], m1 = mw[2 * kk + 1];
       x[0] = ((m0 >> L.mb0) & 1u) ? x[0] * mscale : 0.f;   // == k_dropout
@@ -152,8 +163,8 @@ __device__ __forceinline__ void dw_mmas(float (&acc)[NC][16], uint32_t dHi, uint
 }
 
 // acc[c][4j + {0,1}] = (i0 + ca, o, o + 1), [4j + {2,3}] = (i0 + cb, ...), o = 32c + 8j + 2t -> this split's partial
-template <int NC>
-__device__ __forceinline__ void dw_store(const TcDwParams& p, const DwLane& L, int i0, int t,
+template <int NC, class TX>
+__device__ __forceinline__ void dw_store(const TcDwParams& p, const DwLane<TX>& L, int i0, int t,
                                          const float (&acc)[NC][16]) {
   float* ws = p.ws + (size_t)blockIdx.x * ((size_t)p.inDim * p.outDim);
   const int ia = i0 + L.ca, ib = i0 + L.cb;
@@ -172,13 +183,14 @@ __device__ __forceinline__ void dw_store(const TcDwParams& p, const DwLane& L, i
     }
 }
 
-template <int NC>
+// TX: float, or uint16_t for a bf16 X (boxes of 64-byte rows, 64-byte swizzle), in both kernels below
+template <int NC, class TX>
 __global__ void __launch_bounds__(DW_THREADS, 1)
 k_tc_linear_dw(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CUtensorMap mapDY,
                const TcDwParams p) {
   constexpr int BN = 32 * NC;
-  constexpr uint32_t xBytes = DW_KS * DW_BM * 4;      // four [KS][32] boxes of X
-  constexpr uint32_t xBoxBytes = DW_KS * DW_XBOX * 4;
+  constexpr uint32_t xBytes = DW_KS * DW_BM * sizeof(TX);      // four [KS][32] boxes of X
+  constexpr uint32_t xBoxBytes = DW_KS * DW_XBOX * sizeof(TX);
   constexpr uint32_t yBytes = DW_KS * BN * 4;         // [KS][BN] of dY
   constexpr uint32_t stageBytes = xBytes + yBytes;
   constexpr uint32_t bBytes = BN * DW_KS * 4;         // one dY^T tile; buffer b holds hi at 2b, lo at 2b + 1
@@ -213,7 +225,7 @@ k_tc_linear_dw(const __grid_constant__ CUtensorMap mapX, const __grid_constant__
     for (int step = 0; step < p.stages && step < numSteps; step++) load(step);
 
   // ================================== consumers ===================================
-  const DwLane L(warp, lane);
+  const DwLane<TX> L(warp, lane);
   const int t = lane & 3;
   const bool masked = p.mask != nullptr && i0 + L.ca < p.inDim;   // (columns past inDim are zero-filled by TMA)
   const int mcol = (i0 + L.ca) >> 5;
@@ -233,8 +245,7 @@ k_tc_linear_dw(const __grid_constant__ CUtensorMap mapX, const __grid_constant__
                                  hiT + BN * DW_KS, threadIdx.x);
   };
   auto fragments = [&](int s, const uint32_t (&mw)[8], uint32_t (&fr)[DW_KS / 8][2][4]) {   // of the block in stage s
-    dw_fragments(reinterpret_cast<const float*>(stages + (size_t)s * stageBytes), L, p.mask != nullptr, p.mscale, mw,
-                 fr);
+    dw_fragments(reinterpret_cast<const TX*>(stages + (size_t)s * stageBytes), L, p.mask != nullptr, p.mscale, mw, fr);
   };
   float acc[NC][16];
 #pragma unroll
@@ -301,14 +312,14 @@ k_tc_linear_dw(const __grid_constant__ CUtensorMap mapX, const __grid_constant__
 }
 
 // WG consumer warpgroups (tile of 64 WG X columns) + one TMA producer warp
-template <int NC, int WG>
+template <int NC, int WG, class TX>
 __global__ void __launch_bounds__(128 * WG + 32, 1)
 k_tc_linear_dw_ws(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CUtensorMap mapDY,
                   const __grid_constant__ CUtensorMap mapM, const TcDwParams p) {
   constexpr int BN = 32 * NC;
   constexpr int CT = 128 * WG, CW = 4 * WG;            // consumer threads, warps
   constexpr int BM = 64 * WG;                          // X columns of the tile
-  constexpr uint32_t xBoxBytes = DW_KS * DW_XBOX * 4;
+  constexpr uint32_t xBoxBytes = DW_KS * DW_XBOX * sizeof(TX);
   constexpr uint32_t xBytes = (BM / DW_XBOX) * xBoxBytes;
   constexpr uint32_t yBytes = DW_KS * BN * 4;          // [KS][BN] of dY
   constexpr uint32_t stageBytes = xBytes + yBytes;     // a multiple of 1024: every box stays swizzle-aligned
@@ -363,7 +374,7 @@ k_tc_linear_dw_ws(const __grid_constant__ CUtensorMap mapX, const __grid_constan
   }
 
   // ================================== consumers ===================================
-  const DwLane L(warp, lane);
+  const DwLane<TX> L(warp, lane);
   const int t = lane & 3;
   // Mask word of the thread's two columns for vertex r of the stage: masks[s][r][ca / 32].  A column past inDim is
   // zero-filled by TMA and keeps all bits, as in k_tc_linear_dw; rows past `rows` read the TMA zero fill (dropped).
@@ -392,7 +403,7 @@ k_tc_linear_dw_ws(const __grid_constant__ CUtensorMap mapX, const __grid_constan
     const uint32_t* ms = masks + (size_t)s * (DW_KS * DW_MASK_WORDS);
 #pragma unroll
     for (int q = 0; q < 8; q++) mw[q] = masked ? (ms[(4 * q + t) * DW_MASK_WORDS + mcol] | mpast) : 0xFFFFFFFFu;
-    dw_fragments(reinterpret_cast<const float*>(st), L, masked, p.mscale, mw, fr);
+    dw_fragments(reinterpret_cast<const TX*>(st), L, masked, p.mscale, mw, fr);
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[s]);
     mbar_wait(&bfull[b], bph);          // every warp's share of block step's dY^T is written
@@ -423,8 +434,9 @@ int splitk_reduce(int64_t count, int splits, const float* part, float* dW, cudaS
 // ws: k_tc_linear_dw_ws with WG consumer warpgroups; otherwise k_tc_linear_dw
 struct DwPlan { int NC, MT, splits, stages; bool ws; int WG; size_t smemBytes; };
 
-// maskOk: no mask, or one whose [KS][4]-word box TMA can load (16-byte aligned base)
-static int tc_dw_plan(int64_t rows, int inDim, int outDim, bool maskOk, DwPlan* q) {
+// maskOk: no mask, or one whose [KS][4]-word box TMA can load (16-byte aligned base); xElem: bytes per X element (4,
+// or 2 for bf16).  The split count does not depend on xElem, so one workspace size serves both.
+static int tc_dw_plan(int64_t rows, int inDim, int outDim, bool maskOk, size_t xElem, DwPlan* q) {
   if (outDim > 256 || outDim < 1 || inDim < 4 || rows < 8) return ROC_ERR_UNSUPPORTED;
   const int nc = (outDim + 31) / 32;
   q->NC = nc <= 1 ? 1 : nc <= 2 ? 2 : nc <= 4 ? 4 : 8;
@@ -435,10 +447,10 @@ static int tc_dw_plan(int64_t rows, int inDim, int outDim, bool maskOk, DwPlan* 
   const size_t bn = (size_t)32 * q->NC;
   size_t stageBytes, fixedBytes;
   if (q->ws) {
-    stageBytes = (size_t)DW_KS * 64 * q->WG * 4 + (size_t)DW_KS * bn * 4 + (size_t)DW_KS * DW_MASK_WORDS * 4;
+    stageBytes = (size_t)DW_KS * 64 * q->WG * xElem + (size_t)DW_KS * bn * 4 + (size_t)DW_KS * DW_MASK_WORDS * 4;
     fixedBytes = 1024 /*align*/ + 128 /*barriers*/ + (size_t)2 * dw_ws_bufs(q->NC) * bn * DW_KS * 4 /*dY^T hi / lo*/;
   } else {
-    stageBytes = (size_t)DW_KS * DW_BM * 4 + (size_t)DW_KS * bn * 4;
+    stageBytes = (size_t)DW_KS * DW_BM * xElem + (size_t)DW_KS * bn * 4;
     fixedBytes = 1024 /*align*/ + 64 /*barriers*/ + 4 * bn * DW_KS * 4 /*two dY^T hi / lo buffers*/;
   }
   q->stages = ring_stages(stageBytes, fixedBytes, DW_MAX_STAGES);
@@ -454,37 +466,52 @@ static int tc_dw_plan(int64_t rows, int inDim, int outDim, bool maskOk, DwPlan* 
 
 size_t tc_dw_workspace_bytes(int64_t rows, int inDim, int outDim) {
   DwPlan q;
-  if (tc_dw_plan(rows, inDim, outDim, true, &q) != ROC_OK) return 0;
+  if (tc_dw_plan(rows, inDim, outDim, true, 4, &q) != ROC_OK) return 0;
   return (size_t)q.splits * (size_t)inDim * (size_t)outDim * sizeof(float);
 }
 
-template <int NC>
+template <int NC, class TX>
 static int dw_launch(const DwPlan& q, const CUtensorMap& mapX, const CUtensorMap& mapDY, const CUtensorMap& mapM,
                      const TcDwParams& t, cudaStream_t st) {
   const dim3 grid((unsigned)q.splits, (unsigned)q.MT, 1);
   if constexpr (NC <= 4) {
     if (q.ws && q.WG == 1)
-      return launch_dyn<k_tc_linear_dw_ws<NC, 1>>(grid, 128 + 32, q.smemBytes, st, mapX, mapDY, mapM, t);
-    if (q.ws) return launch_dyn<k_tc_linear_dw_ws<NC, 2>>(grid, 256 + 32, q.smemBytes, st, mapX, mapDY, mapM, t);
+      return launch_dyn<k_tc_linear_dw_ws<NC, 1, TX>>(grid, 128 + 32, q.smemBytes, st, mapX, mapDY, mapM, t);
+    if (q.ws) return launch_dyn<k_tc_linear_dw_ws<NC, 2, TX>>(grid, 256 + 32, q.smemBytes, st, mapX, mapDY, mapM, t);
   }
-  return launch_dyn<k_tc_linear_dw<NC>>(grid, DW_THREADS, q.smemBytes, st, mapX, mapDY, t);
+  return launch_dyn<k_tc_linear_dw<NC, TX>>(grid, DW_THREADS, q.smemBytes, st, mapX, mapDY, t);
 }
 
-int tc_linear_dw(int64_t rows, int inDim, int outDim, const float* X, int64_t ldX, const float* dY, int64_t ldDY,
-                 float* dW, float* workspace, size_t wsBytes, const DropMask* dm, cudaStream_t st,
+template <class TX>
+static int dw_launch_nc(const DwPlan& q, const CUtensorMap& mapX, const CUtensorMap& mapDY, const CUtensorMap& mapM,
+                        const TcDwParams& t, cudaStream_t st) {
+  switch (q.NC) {
+    case 1: return dw_launch<1, TX>(q, mapX, mapDY, mapM, t, st);
+    case 2: return dw_launch<2, TX>(q, mapX, mapDY, mapM, t, st);
+    case 4: return dw_launch<4, TX>(q, mapX, mapDY, mapM, t, st);
+    default: return dw_launch<8, TX>(q, mapX, mapDY, mapM, t, st);
+  }
+}
+
+// X is fp32, or bf16 (raw bits) when xBf16
+int tc_linear_dw(int64_t rows, int inDim, int outDim, const void* X, bool xBf16, int64_t ldX, const float* dY,
+                 int64_t ldDY, float* dW, float* workspace, size_t wsBytes, const DropMask* dm, cudaStream_t st,
                  roc_gemm_info* info) {
   // the mask box is [KS vertices][4 words]: TMA wants a 16-byte aligned base (the row stride is a multiple of 4 words,
   // which the C ABI requires), so a mask that starts elsewhere goes to k_tc_linear_dw, which loads it word by word
   const bool maskOk = !dm || aligned16(dm->bits);
   DwPlan q;
-  if (tc_dw_plan(rows, inDim, outDim, maskOk, &q) != ROC_OK) return ROC_ERR_UNSUPPORTED;
-  if ((ldX % 4) || (ldDY % 4) || !aligned16(X) || !aligned16(dY)) return ROC_ERR_UNSUPPORTED;
+  if (tc_dw_plan(rows, inDim, outDim, maskOk, xBf16 ? 2 : 4, &q) != ROC_OK) return ROC_ERR_UNSUPPORTED;
+  if ((ldX % (xBf16 ? 8 : 4)) || (ldDY % 4) || !aligned16(X) || !aligned16(dY)) return ROC_ERR_UNSUPPORTED;
   if (rows > 0x7FFFFF00ll || !encode_tiled_fn()) return ROC_ERR_UNSUPPORTED;
   const size_t count = (size_t)inDim * outDim;
   if (wsBytes < (size_t)q.splits * count * sizeof(float)) return ROC_ERR_INVALID;
   CUtensorMap mapX, mapDY, mapM;
   memset(&mapM, 0, sizeof(mapM));
-  if (!make_tmap_f32_2d(&mapX, X, (uint64_t)rows, (uint64_t)inDim, (uint64_t)ldX, DW_KS, DW_XBOX))
+  if (xBf16 ? !make_tmap_bf16_2d(&mapX, static_cast<const uint16_t*>(X), (uint64_t)rows, (uint64_t)inDim,
+                                 (uint64_t)ldX, DW_KS, DW_XBOX)
+            : !make_tmap_f32_2d(&mapX, static_cast<const float*>(X), (uint64_t)rows, (uint64_t)inDim, (uint64_t)ldX,
+                                DW_KS, DW_XBOX))
     return ROC_ERR_UNSUPPORTED;
   if (!make_tmap_f32_2d(&mapDY, dY, (uint64_t)rows, (uint64_t)outDim, (uint64_t)ldDY, DW_KS, (uint32_t)(32 * q.NC),
                         CU_TENSOR_MAP_SWIZZLE_NONE))
@@ -500,13 +527,8 @@ int tc_linear_dw(int64_t rows, int inDim, int outDim, const float* X, int64_t ld
     info->nc = q.NC; info->epi = q.ws ? 1 : 0; info->grid_x = q.splits; info->grid_y = q.MT; info->stages = q.stages;
     info->splits = q.splits; info->v_per_split = t.vPerSplit;
   }
-  int rc;
-  switch (q.NC) {
-    case 1: rc = dw_launch<1>(q, mapX, mapDY, mapM, t, st); break;
-    case 2: rc = dw_launch<2>(q, mapX, mapDY, mapM, t, st); break;
-    case 4: rc = dw_launch<4>(q, mapX, mapDY, mapM, t, st); break;
-    default: rc = dw_launch<8>(q, mapX, mapDY, mapM, t, st); break;
-  }
+  const int rc = xBf16 ? dw_launch_nc<uint16_t>(q, mapX, mapDY, mapM, t, st)
+                        : dw_launch_nc<float>(q, mapX, mapDY, mapM, t, st);
   if (rc != ROC_OK) return rc;
   return splitk_reduce((int64_t)count, q.splits, workspace, dW, st);
 }

@@ -192,10 +192,13 @@ __device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) 
 constexpr size_t SMEM_PER_BLOCK = 227 * 1024;   // the shared memory an H100 block may use
 
 // Stages of a TMA ring: as many of stageBytes as fit beside fixedBytes (alignment slack, barriers, buffers), at most
-// maxStages; 0 when fewer than 2 fit, since one stage cannot overlap the loads with the compute
+// maxStages; 0 when fewer than 2 fit, since one stage cannot overlap the loads with the compute (and when fixedBytes
+// alone exceeds shared memory)
 inline int ring_stages(size_t stageBytes, size_t fixedBytes, int maxStages) {
-  const int st = (int)((SMEM_PER_BLOCK - fixedBytes) / stageBytes);
-  return st < 2 ? 0 : st > maxStages ? maxStages : st;
+  if (fixedBytes >= SMEM_PER_BLOCK) return 0;
+  const size_t fit = (SMEM_PER_BLOCK - fixedBytes) / stageBytes;
+  const int st = fit > (size_t)maxStages ? maxStages : (int)fit;
+  return st < 2 ? 0 : st;
 }
 
 // ------------------------------------------------------ host: tensor maps -----
@@ -237,6 +240,22 @@ inline bool make_tmap_f32_2d(CUtensorMap* m, const float* base, uint64_t rows, u
                              uint32_t boxRows, uint32_t boxCols,
                              CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
   return make_tmap_32b_2d(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, base, rows, cols, ld, boxRows, boxCols, swizzle);
+}
+// bf16 row-major [rows][cols] (raw bits) with `ld` elements between rows (a multiple of 8: TMA strides are whole
+// 16-byte units); box = [boxRows][boxCols], 64-byte swizzle (boxCols * 2 must be 64), out-of-bounds elements read as
+// zero
+inline bool make_tmap_bf16_2d(CUtensorMap* m, const uint16_t* base, uint64_t rows, uint64_t cols, uint64_t ld,
+                              uint32_t boxRows, uint32_t boxCols) {
+  EncodeTiledFn fn = encode_tiled_fn();
+  if (!fn) return false;
+  cuuint64_t dims[2] = {cols, rows};
+  cuuint64_t strides[1] = {ld * 2};
+  cuuint32_t box[2] = {boxCols, boxRows};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<uint16_t*>(base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS;
 }
 // uint32 row-major [rows][cols] (the packed dropout mask), no swizzle
 inline bool make_tmap_u32_2d(CUtensorMap* m, const uint32_t* base, uint64_t rows, uint64_t cols, uint64_t ld,

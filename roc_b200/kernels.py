@@ -385,6 +385,67 @@ def linear_fwd_dropout(x, w, mask, rate, activation=0, norm_row_end=None, col_le
     return out
 
 
+def bf16_padded(rows, h, device="cuda"):
+    """[rows][h] view of a zeroed bf16 [rows][round_up(h, 8)] allocation (the bf16 node-tensor layout)."""
+    ld = (h + 7) // 8 * 8
+    return torch.zeros((rows, ld), device=device, dtype=torch.bfloat16)[:, :h]
+
+
+def f32_to_bf16(x, out=None):
+    """roc_f32_to_bf16: fp32 [rows][h] -> bf16 (round to nearest even); the pad columns of `out`'s rows are zeroed."""
+    if out is None:
+        out = bf16_padded(x.shape[0], x.shape[1], x.device)
+    assert out.dtype == torch.bfloat16
+    check(lib.roc_f32_to_bf16(x.shape[0], x.shape[1], _ptr(x), _ld(x), _ptr(out), _ld(out), _stream()),
+          "roc_f32_to_bf16")
+    return out
+
+
+def bf16_to_f32(x, out=None):
+    """roc_bf16_to_f32: bf16 [rows][h] -> fp32, exactly."""
+    assert x.dtype == torch.bfloat16
+    if out is None:
+        out = padded(x.shape[0], x.shape[1], x.device)
+    check(lib.roc_bf16_to_f32(x.shape[0], x.shape[1], _ptr(x), _ld(x), _ptr(out), _ld(out), _stream()),
+          "roc_bf16_to_f32")
+    return out
+
+
+def dropout_fwd_bf16(x, first_row, rate, seed, step, out=None):
+    """roc_dropout_fwd_bf16: dropout of a bf16 x into fp32."""
+    assert x.dtype == torch.bfloat16
+    if out is None:
+        out = padded(x.shape[0], x.shape[1], x.device)
+    check(lib.roc_dropout_fwd_bf16(x.shape[0], x.shape[1], first_row, rate, seed, step, _ptr(x), _ld(x), _ptr(out),
+                                   _ld(out), _stream()), "roc_dropout_fwd_bf16")
+    return out
+
+
+def linear_fwd_bf16(x, w, mask=None, rate=0.0, activation=0, norm_row_end=None, col_left=0, out=None):
+    """roc_linear_fwd_bf16: linear_fwd_dropout with a bf16 x."""
+    assert x.dtype == torch.bfloat16 and w.is_contiguous()
+    if out is None:
+        out = padded(x.shape[0], w.shape[0], x.device)
+    flags = _lib.LINEAR_NORM_EPILOGUE if norm_row_end is not None else 0
+    check(lib.roc_linear_fwd_bf16(x.shape[0], x.shape[1], w.shape[0], _ptr(x), _ld(x), _ptr(w), _ptr(out), _ld(out),
+                                  activation, flags, _ptr(norm_row_end), col_left, _ptr(mask),
+                                  mask.stride(0) if mask is not None else 0, rate, _stream()), "roc_linear_fwd_bf16")
+    return out
+
+
+def linear_dw_bf16(x, dy, dw, mask=None, rate=0.0, y=None, activation=0):
+    """roc_linear_dw_bf16: dW += dY^T dropout(x) for a bf16 x (with the in-place relu backward of dy first when
+    activation is RELU)."""
+    assert x.dtype == torch.bfloat16
+    ws_bytes = lib.roc_linear_bwd_workspace_bytes(x.shape[0], x.shape[1], dy.shape[1])
+    ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=x.device)
+    check(lib.roc_linear_dw_bf16(x.shape[0], x.shape[1], dy.shape[1], _ptr(x), _ld(x), _ptr(y),
+                                 _ld(y) if y is not None else 0, _ptr(dy), _ld(dy), _ptr(dw), activation, _ptr(ws),
+                                 ws_bytes, _ptr(mask), mask.stride(0) if mask is not None else 0, rate, _stream()),
+          "roc_linear_dw_bf16")
+    return dw
+
+
 def linear_bwd_dropout(x, w, y, dy, dw, mask, rate, dx=None, activation=0, accumulate_dx=False):
     """linear_bwd where the forward input was dropout(x); dx is the gradient of x (pre-dropout)."""
     ws_bytes = lib.roc_linear_bwd_workspace_bytes(x.shape[0], x.shape[1], w.shape[0])

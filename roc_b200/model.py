@@ -76,12 +76,26 @@ class Model:
     def __init__(self, host, seed=None):
         self.host = host
         self.h = host.h
+        self._bf16 = set()               # handles of the bf16 node tensors
         if seed is not None:
             lib.roc_host_srand(seed)     # std::srand(config.seed), gnn.cc:56
 
     # ---- builders (gnn.h:165-179)
-    def create_node_tensor(self, hidden, is_int=False):
+    def create_node_tensor(self, hidden, is_int=False, dtype="float32"):
+        """dtype "float32" (every tensor) or "bfloat16": a leaf feature tensor held in bf16 (rounded to nearest even,
+        half the memory), which only linear and dropout may read; init() refuses any other op on it.  It has no
+        gradient.  set_tensor takes fp32 rows or a torch.bfloat16 tensor, get_tensor returns fp32 (raw=True: the
+        bits as uint16)."""
+        if dtype in ("bfloat16", "bf16"):
+            assert not is_int
+            t = lib.roc_host_create_node_tensor_bf16(self.h, hidden)
+            self._bf16.add(t)
+            return t
+        assert dtype in ("float32", np.float32), dtype
         return lib.roc_host_create_node_tensor(self.h, hidden, int(is_int))
+
+    def is_bf16(self, t):
+        return t in self._bf16
 
     def dropout(self, t, rate, seed=0):
         return lib.roc_host_dropout(self.h, t, rate, seed)
@@ -172,6 +186,16 @@ class Model:
 
     def set_tensor(self, t, arr, grad=False):
         rows, hidden, _ = self.tensor_shape(t)
+        if t in self._bf16:
+            if grad:
+                raise _lib.RocError("set_tensor(grad=True): a bf16 tensor has no gradient")
+            if str(getattr(arr, "dtype", "")) == "torch.bfloat16":
+                import torch   # only a torch tensor can carry bf16 rows
+                bits = np.ascontiguousarray(arr.detach().contiguous().cpu().view(torch.int16).numpy())   # copied as is
+                assert bits.size == rows * hidden, (bits.shape, rows, hidden)
+                check(lib.roc_host_set_tensor_bf16(self.h, t, bits.ctypes.data))
+                return
+            arr = np.ascontiguousarray(arr, dtype=np.float32)   # fp32 rows, rounded on the device
         arr = np.ascontiguousarray(arr)
         assert arr.itemsize == 4 and arr.size == rows * hidden, (arr.shape, rows, hidden)
         check(lib.roc_host_set_tensor(self.h, t, arr.ctypes.data, int(grad)))
@@ -180,8 +204,16 @@ class Model:
         """ptr: address of a dense [rows][hidden] 4-byte host buffer (e.g. pinned torch memory)."""
         check(lib.roc_host_set_tensor(self.h, t, C.c_void_p(ptr), int(grad)))
 
-    def get_tensor(self, t, grad=False, dtype=np.float32):
+    def get_tensor(self, t, grad=False, dtype=np.float32, raw=False):
+        """the tensor's rows as fp32 (a bf16 tensor widened exactly); raw=True on a bf16 tensor: its bits (uint16)"""
         rows, hidden, _ = self.tensor_shape(t)
+        if t in self._bf16:
+            if grad:
+                raise _lib.RocError("get_tensor(grad=True): a bf16 tensor has no gradient")
+            if raw:
+                out = np.empty((rows, hidden), dtype=np.uint16)
+                check(lib.roc_host_get_tensor_bf16(self.h, t, out.ctypes.data))
+                return out
         out = np.empty((rows, hidden), dtype=dtype)
         check(lib.roc_host_get_tensor(self.h, t, out.ctypes.data, int(grad)))
         return out
@@ -264,12 +296,21 @@ class Model:
         return pm.as_dict()
 
 
-def build_gcn(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exact_backward=False):
+def _input_tensor(model, hidden, features):
+    """the builders' input features: fp32, or bf16 with features="bfloat16" (the plain call for fp32, so that any object
+    with the builder methods can stand in for a Model)"""
+    if features == "float32":
+        return model.create_node_tensor(hidden)
+    return model.create_node_tensor(hidden, dtype=features)
+
+
+def build_gcn(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exact_backward=False, features="float32"):
     """The model script of gnn.cc:65-98 for `-layers a-b-...-c`.  Returns the handles.  exact_backward: train on the
     exact gradient over the graph's transpose (Model.set_exact_backward), for directed graphs; the same keyword on
-    build_sage_mean, build_sage_pool and build_gat."""
+    build_sage_mean, build_sage_pool and build_gat.  features="bfloat16" keeps the input features in bf16
+    (Model.create_node_tensor); the same keyword on every builder."""
     L = len(layers)
-    x = model.create_node_tensor(layers[0])
+    x = _input_tensor(model, layers[0], features)
     label = model.create_node_tensor(layers[-1])
     mask = model.create_node_tensor(1, is_int=True)
     t = x
@@ -295,7 +336,8 @@ def build_gcn(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exact_bac
     return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs}
 
 
-def build_sage_mean(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exact_backward=False):
+def build_sage_mean(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exact_backward=False,
+                    features="float32"):
     """GraphSAGE with the mean aggregator (BASELINE.json configs[2]) composed from the reference's own ops
     (gnn.h:165-179; AGGR_AVG is declared at gnn.h:75-80 but the reference's ScatterGather only sums):
 
@@ -308,7 +350,7 @@ def build_sage_mean(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exa
     x / sqrt(deg) / sqrt(deg) is the mean to within one fp32 rounding.  Same wiring as the reference's residual
     GCN layer (gnn.cc:79-90) with both norms after the aggregation."""
     L = len(layers)
-    x = model.create_node_tensor(layers[0])
+    x = _input_tensor(model, layers[0], features)
     label = model.create_node_tensor(layers[-1])
     mask = model.create_node_tensor(1, is_int=True)
     t = x
@@ -332,7 +374,8 @@ def build_sage_mean(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exa
     return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs}
 
 
-def build_sage_pool(model, layers, dropout_rate, aggr=_lib.AGGR_MAX, lr=0.01, weight_decay=0.05, exact_backward=False):
+def build_sage_pool(model, layers, dropout_rate, aggr=_lib.AGGR_MAX, lr=0.01, weight_decay=0.05, exact_backward=False,
+                    features="float32"):
     """GraphSAGE with the pooling aggregator (Hamilton et al., 2017) composed from the reference's ops plus the max
     (or min) ScatterGather.  The reference's Linear has no bias, so neither has this.  Per layer:
 
@@ -345,7 +388,7 @@ def build_sage_pool(model, layers, dropout_rate, aggr=_lib.AGGR_MAX, lr=0.01, we
     Single partition; init refuses a graph with a duplicate edge in a row.  Returns the handles, with `pools`
     (the scatter_gather outputs, for get_aggr_index) and `pool_ins` (their inputs)."""
     L = len(layers)
-    x = model.create_node_tensor(layers[0])
+    x = _input_tensor(model, layers[0], features)
     label = model.create_node_tensor(layers[-1])
     mask = model.create_node_tensor(1, is_int=True)
     t = x
@@ -370,7 +413,7 @@ def build_sage_pool(model, layers, dropout_rate, aggr=_lib.AGGR_MAX, lr=0.01, we
 
 
 def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01, weight_decay=0.05,
-              exact_backward=False):
+              exact_backward=False, features="float32"):
     """GAT (Velickovic et al., 2018) built from the reference's ops plus attention_gather.  `heads` (an int, or one
     value per hidden layer) applies to the hidden layers; the last layer has one head.  layers[i] is the width of
     layer i's output, heads_i * F_i.  Per layer:
@@ -389,7 +432,7 @@ def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01,
     hs = list(heads) if isinstance(heads, (list, tuple)) else [int(heads)] * (L - 2)
     assert len(hs) == L - 2, "one head count per hidden layer"
     hs.append(1)
-    x = model.create_node_tensor(layers[0])
+    x = _input_tensor(model, layers[0], features)
     label = model.create_node_tensor(layers[-1])
     mask = model.create_node_tensor(1, is_int=True)
     t = x
@@ -414,7 +457,8 @@ def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01,
             "attn_ins": attn_ins, "scores": scores}
 
 
-def build_gcn_weighted(model, layers, dropout_rate, edge_weights, edge_grad=False, lr=0.01, weight_decay=0.05):
+def build_gcn_weighted(model, layers, dropout_rate, edge_weights, edge_grad=False, lr=0.01, weight_decay=0.05,
+                       features="float32"):
     """GCN with edge weights (e.g. datasets.gcn_edge_weights, which folds in the symmetric normalisation).  Per layer
 
         t = relu(scatter_gather(linear(dropout(t), layers[i]), weights=e))     # no relu on the last layer
@@ -423,7 +467,7 @@ def build_gcn_weighted(model, layers, dropout_rate, edge_weights, edge_grad=Fals
     init().  edge_grad: compute e's gradient in backward (the sum of the layers' contributions).  Single partition.
     Returns the handles, with `edges` and the aggregations' inputs `sg_ins` and outputs `sg_outs`."""
     L = len(layers)
-    x = model.create_node_tensor(layers[0])
+    x = _input_tensor(model, layers[0], features)
     label = model.create_node_tensor(layers[-1])
     mask = model.create_node_tensor(1, is_int=True)
     e = model.create_edge_tensor(1)

@@ -142,14 +142,17 @@ class Recorder:
 
 
 def _relu_with_mask(pre, product_mask, what):
-    """ReLU whose mask is the product's where fp32 and fp64 disagree at a pre-activation within rounding of 0."""
+    """ReLU whose mask is the product's where fp32 and fp64 disagree at a pre-activation within rounding of 0.
+    product_mask: a bool array or tensor (moved to pre's device).  The result saves a bool mask for autograd, not a
+    float one, so that tests/scale_witness.py can use it at full size."""
     if product_mask is None:
         return torch.relu(pre)
-    p = pre.detach().numpy()
-    diff = (p > 0) != product_mask
+    p = pre.detach()
+    pm = torch.as_tensor(product_mask).to(p.device, torch.bool)
+    diff = (p > 0) != pm
     if diff.any():
-        assert np.abs(p[diff]).max() <= 1e-4 * np.abs(p).max(), "%s: relu masks differ away from zero" % what
-    return pre * torch.from_numpy(product_mask.astype(np.float64))
+        assert p[diff].abs().max() <= 1e-4 * p.abs().max(), "%s: relu masks differ away from zero" % what
+    return torch.where(pm, pre, 0.0)
 
 
 def _extreme_sources(row_end, col, x, is_max, product_args, what):

@@ -8,7 +8,6 @@ launches, one JSON line per kernel and a total.  Run it on its own: the tracer s
 bench.py's.  With --out the per-kernel table is also written to DIR/profile_step_cfg<N>.json.
 """
 import argparse
-import importlib.util
 import json
 import os
 import sys
@@ -19,12 +18,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-
-def bench_module():
-    spec = importlib.util.spec_from_file_location("roc_bench", os.path.join(ROOT, "bench.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
+from bench_inputs import bench_module, node_inputs  # noqa: E402  (tests/ is this script's directory)
 
 
 def card():
@@ -60,21 +54,7 @@ def main():
     nloc = info["rowRight"] - info["rowLeft"] + 1
     m = Model(host, seed=1)
     hnd = B.build_model(m, a.config)
-    # the inputs of bench.py's run_ours (rank 0)
-    g = torch.Generator(device="cpu"); g.manual_seed(1000)
-    feats = torch.empty((nloc, layers[0]), dtype=torch.float32, pin_memory=True)
-    dg = torch.Generator(device=dev); dg.manual_seed(1000)
-    chunk = 1 << 18
-    for r0 in range(0, nloc, chunk):
-        r1 = min(nloc, r0 + chunk)
-        feats[r0:r1].copy_(torch.rand((r1 - r0, layers[0]), device=dev, generator=dg) * 2 - 1)
-    labels = torch.randint(0, layers[-1], (nloc,), generator=g, dtype=torch.int32).pin_memory()
-    u = torch.rand(nloc, generator=g)
-    mask = torch.full((nloc,), 2, dtype=torch.int32)
-    mask[u < 0.76] = 1
-    mask[u < 0.66] = 0
-    mask = mask.pin_memory()
-    torch.cuda.synchronize()
+    feats, labels, mask = node_inputs(nloc, layers, dev)      # the inputs of bench.py's run_ours (rank 0)
     m.set_tensor_from_host_ptr(hnd["input"], feats.data_ptr())
     m.set_labels(hnd["label"], labels.numpy())
     m.set_tensor_from_host_ptr(hnd["mask"], mask.data_ptr())

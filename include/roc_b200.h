@@ -143,6 +143,14 @@ int roc_sg_plan_rows_sorted(const roc_sg_plan* plan, int* sorted, roc_stream_t s
 int roc_sg_forward_planned(const roc_sg_plan* plan, int H, const float* in,
                            int64_t ldIn, float* out, int64_t ldOut, int epilogue,
                            roc_stream_t stream);
+/* roc_sg_forward_planned over bf16 rows (raw bits, see roc_f32_to_bf16): half the bytes per gathered row, each value
+ * widened exactly in registers and accumulated in fp32, with the same epilogues and the same fp32 output.  `in` is
+ * 16-byte aligned and ldIn (in elements) is a multiple of 8, else ROC_ERR_INVALID.  The result is bit-identical to
+ * roc_sg_forward_planned on roc_bf16_to_f32(in) written to a 16-byte aligned buffer with a leading dimension that is a
+ * multiple of 4: the plan, the row shapes, the column blocks, the per-float add order, the carries and the fix-ups are
+ * that call's.  Its launches report reduction 12 (the sum over bf16 rows) in roc_sg_last_call_info. */
+int roc_sg_forward_planned_bf16(const roc_sg_plan* plan, int H, const uint16_t* in, int64_t ldIn, float* out,
+                                int64_t ldOut, int epilogue, roc_stream_t stream);
 
 /* Max / min aggregation (GraphSAGE-pool).  The reference declares AGGR_MAX / AGGR_MIN but never implements them;
  * these semantics are this library's own.  For a row v with in-edges e in CSR order:
@@ -300,7 +308,8 @@ int roc_sg_backward(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft, in
  *          stats, 5 the attention forward, 6 its d s_dst gather, 7 its input-gradient gather, 8 the weighted sum
  *          (forward and backward), 9 the edge-weight gradient, 10 the exact sum backward with NORM (the sum whose
  *          epilogue divides by the original graph's in-degree; its main kernel, ring and fix-ups), 11 the exact max /
- *          min backward; -1 for the record and the permutation, which have none.  A sum fix-up finishing another
+ *          min backward, 12 the sum over bf16 rows (its main kernel and ring); -1 for the record and the
+ *          permutation, which have none.  A sum fix-up finishing another
  *          reduction's partials reports 0.
  *   vec    4 for float4 rows, else 1;  lanes, nch: the row shape (L lanes, chunks per lane);  grid: CTAs launched
  * count is the number of launches; the first ROC_SG_MAX_LAUNCHES are stored.  Every planned call clears the list first,
@@ -481,6 +490,12 @@ int roc_softmax_xent_bwd_norm(int64_t rows, int C, const float* logits, int64_t 
  * indegree_norm that follows linear in the model, gnn.cc:81-82); then needs
  * rowLeft-relative rowEnd/colLeft (else pass NULL/0). */
 #define ROC_LINEAR_NORM_EPILOGUE 1
+/* ROC_LINEAR_Y_BF16 (roc_linear_fwd, roc_linear_fwd_dropout, roc_linear_fwd_bf16): Y holds bf16 bits (pass a
+ * uint16_t buffer cast to float*), ldY is in elements and a multiple of 8, else ROC_ERR_INVALID.  Each stored value is
+ * exactly roc_f32_to_bf16 of what the same call stores without the flag, and the columns [outDim, ldY) are never
+ * written.  The wgmma kernel stores a tile of at most 64 columns through a bf16 staging tile by TMA, wider ones and
+ * the last outDim % 8 columns directly; the SIMT kernel narrows as it stores. */
+#define ROC_LINEAR_Y_BF16 2
 int roc_linear_fwd(int64_t rows, int inDim, int outDim, const float* X, int64_t ldX,
                    const float* W, float* Y, int64_t ldY, int activation, int flags,
                    const roc_eid_t* rowEnd, roc_eid_t colLeft, roc_stream_t stream);

@@ -234,7 +234,8 @@ public:
 
   /* ---- additions (not in gnn.h): host<->device access to this partition's rows ---- */
   /* Copy `rows_local x H` values between a dense host buffer and the tensor.  A bf16 tensor takes and returns fp32
-   * rows (set: rounded to nearest even on the device; get: widened exactly); grad = true on it is an error. */
+   * rows (set: rounded to nearest even on the device; get: widened exactly); grad = true is an error on a bf16 leaf and
+   * reaches the fp32 gradient of a bf16 tensor an op produces (set_bf16_aggregation). */
   void set_tensor(const Tensor& t, const void* host, bool grad = false);
   void get_tensor(const Tensor& t, void* host, bool grad = false) const;
   /* a bf16 tensor's raw bits, `rows_local x H` uint16 values, copied as they are */
@@ -250,6 +251,13 @@ public:
    * only on a symmetric graph).  init() then builds the transpose once, shared with the weighted ops, and max / min
    * accept graphs with duplicate edges.  Call it before init().  Single partition only (exit(1) otherwise). */
   void set_exact_backward(bool on);
+  /* Opt-in bf16 aggregation inputs (off by default).  At init(), after fusion, each tensor that a Linear with
+   * AC_MODE_NONE writes in its forward (its own output, or the output of an indegree_norm fused into its epilogue) and
+   * that one sum scatter_gather alone reads is stored in bf16: the Linear rounds its fp32 result to nearest even as it
+   * stores it, and the scatter_gather gathers the rows at half width and accumulates them in fp32.  The gradient of
+   * such a tensor is an ordinary fp32 tensor; every other tensor stays fp32.  Call it before init().  Single partition
+   * only (init() exits otherwise). */
+  void set_bf16_aggregation(bool on);
   /* the source ids a max / min scatter_gather chose (its `arg`), [rows_local][H] u32; `out` is its output tensor */
   void get_aggr_index(const Tensor& out, uint32_t* host) const;
   int64_t local_rows(void) const { return (int64_t)myGraph.rowRight - myGraph.rowLeft + 1; }
@@ -266,6 +274,7 @@ public:
   bool fuse;          /* fuse linear->norm and SG->norm->relu into kernel epilogues (default on) */
   bool printMetrics;  /* print the [INFER] accuracy line like softmax_kernel.cu:141-152 (default on) */
   bool exactBackward; /* set_exact_backward (default off) */
+  bool bf16Aggregation; /* set_bf16_aggregation (default off) */
 };
 
 class GnnOp {  /* gnn.h:205-222 */

@@ -65,6 +65,8 @@ void roc_host_srand(unsigned seed);               /* std::srand(config.seed), gn
 int roc_host_set_fusion(roc_host* h, int on);
 /* Model::set_exact_backward(on); before roc_host_init */
 int roc_host_set_exact_backward(roc_host* h, int on);
+/* Model::set_bf16_aggregation(on); before roc_host_init */
+int roc_host_set_bf16_aggregation(roc_host* h, int on);
 int roc_host_init(roc_host* h);
 
 /* data: dense host buffers of this partition's rows ([rows][hidden]) */
@@ -80,6 +82,12 @@ int roc_host_set_labels(roc_host* h, int t, const int32_t* host_class_idx);
 int roc_host_get_aggr_index(roc_host* h, int t, uint32_t* host);
 int roc_host_tensor_shape(roc_host* h, int t, int64_t out[3]);   /* rows, hidden, ld */
 void* roc_host_tensor_ptr(roc_host* h, int t, int grad);          /* device pointer (a bf16 tensor: its bits) */
+/* how the tensor's data is stored: ROC_HOST_DTYPE_*.  After roc_host_init it shows which tensors
+ * set_bf16_aggregation made bf16 (their gradients stay fp32). */
+#define ROC_HOST_DTYPE_FLOAT32 0
+#define ROC_HOST_DTYPE_BFLOAT16 1
+#define ROC_HOST_DTYPE_INT32 2
+int roc_host_tensor_dtype(roc_host* h, int t);
 int roc_host_num_parameters(roc_host* h);
 int roc_host_parameter_shape(roc_host* h, int p, int64_t out[2]); /* inDim, outDim */
 int roc_host_get_parameter(roc_host* h, int p, float* host, int which); /* 0 W, 1 dW, 2 m, 3 v */

@@ -18,6 +18,9 @@ SG_EPI_NONE, SG_EPI_NORM, SG_EPI_RELU = 0, 1, 2
 AGGR_AVG, AGGR_MAX, AGGR_MIN, AGGR_SUM = 0, 1, 2, 3        # AggrType (gnn.h:75-80); ROC_SG_AGGR_MAX / _MIN = 1 / 2
 SG_NOARG = 0xFFFFFFFF                                      # arg of a row with no in-edge
 LINEAR_NORM_EPILOGUE = 1
+LINEAR_Y_BF16 = 2                                          # Y holds bf16 bits
+SG_RED_BSUM = 12                                           # roc_sg_launch.red of the sum over bf16 rows
+HOST_DTYPES = ("float32", "bfloat16", "int32")             # ROC_HOST_DTYPE_* by value
 LINEAR_BWD_ONLY_DX, LINEAR_BWD_ONLY_DW = 1, 2
 GEMM_FWD, GEMM_DW, GEMM_DX = 0, 1, 2                       # `which` of roc_last_gemm_path / roc_last_gemm_info
 
@@ -121,6 +124,7 @@ PROTOTYPES = {
     "roc_sg_plan_info": (i32, [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]),
     "roc_sg_plan_rows_sorted": (i32, [vp, C.POINTER(i32), vp]),
     "roc_sg_forward_planned": (i32, [vp, i32, vp, i64, vp, i64, i32, vp]),
+    "roc_sg_forward_planned_bf16": (i32, [vp, i32, vp, i64, vp, i64, i32, vp]),
     "roc_sg_minmax_forward_planned": (i32, [vp, i32, i32, vp, i64, vp, i64, vp, i64, vp]),
     "roc_sg_minmax_backward_planned": (i32, [vp, i32, u32, vp, i64, vp, i64, vp, i64, vp]),
     "roc_sg_attn_forward_planned": (i32, [vp, i32, i32, f32, u32, vp, i64, vp, i64, vp, i64, vp, i64, vp]),
@@ -212,6 +216,7 @@ PROTOTYPES = {
     "roc_host_srand": (None, [C.c_uint]),
     "roc_host_set_fusion": (i32, [vp, i32]),
     "roc_host_set_exact_backward": (i32, [vp, i32]),
+    "roc_host_set_bf16_aggregation": (i32, [vp, i32]),
     "roc_host_init": (i32, [vp]),
     "roc_host_load_features": (i32, [vp, i32, C.c_char_p]),
     "roc_host_load_labels": (i32, [vp, i32, C.c_char_p]),
@@ -223,6 +228,7 @@ PROTOTYPES = {
     "roc_host_set_labels": (i32, [vp, i32, vp]),
     "roc_host_tensor_shape": (i32, [vp, i32, vp]),
     "roc_host_tensor_ptr": (vp, [vp, i32, i32]),
+    "roc_host_tensor_dtype": (i32, [vp, i32]),
     "roc_host_num_parameters": (i32, [vp]),
     "roc_host_parameter_shape": (i32, [vp, i32, vp]),
     "roc_host_get_parameter": (i32, [vp, i32, vp, i32]),

@@ -823,15 +823,8 @@ extern "C" int roc_fill(int64_t rows, int H, float value, float* x, int64_t ld, 
 }
 
 // ------------------------------------------------------------------- bf16 ---
-// fp32 -> bf16, round to nearest even as torch's Tensor.to(torch.bfloat16): a finite value past the largest bf16 rounds
-// to +-inf, a NaN becomes the quiet NaN 0x7FC0.  Writes every column of the
-// [rows][ldDst] destination: the pad columns [H, ldDst) get zero.
-__device__ __forceinline__ uint16_t f32_to_bf16_rne(float f) {
-  const uint32_t u = __float_as_uint(f);
-  if (f != f) return (uint16_t)0x7FC0u;
-  return (uint16_t)((u + 0x7FFFu + ((u >> 16) & 1u)) >> 16);
-}
-
+// fp32 -> bf16 by f32_to_bf16_rne (common.cuh).  Writes every column of the [rows][ldDst] destination: the pad columns
+// [H, ldDst) get zero.
 __global__ void __launch_bounds__(EW_T)
 k_f32_to_bf16(int64_t rows, int H, const float* __restrict__ src, int64_t ldSrc, uint16_t* __restrict__ dst,
               int64_t ldDst) {

@@ -123,6 +123,7 @@ double roc_host_get_lr(roc_host* h) { return h->adam ? h->adam->alpha : 0.0; }
 void roc_host_srand(unsigned seed) { std::srand(seed); }
 int roc_host_set_fusion(roc_host* h, int on) { h->m().set_fusion(on != 0); return 0; }
 int roc_host_set_exact_backward(roc_host* h, int on) { h->m().set_exact_backward(on != 0); return 0; }
+int roc_host_set_bf16_aggregation(roc_host* h, int on) { h->m().set_bf16_aggregation(on != 0); return 0; }
 int roc_host_init(roc_host* h) { return h->m().init(h->config) ? 0 : -1; }
 
 int roc_host_load_features(roc_host* h, int t, const char* prefix) { h->m().load_features(h->at(t), prefix); return 0; }
@@ -143,6 +144,11 @@ void* roc_host_tensor_ptr(roc_host* h, int t, int grad) {
   RuntimeImpl* rt = h->rt->impl;
   if (!grad && rt->t(h->at(t).region).isBf16) return (void*)rt->data_bf16(h->at(t).region);
   return grad ? (void*)h->rt->impl->grad(h->at(t).region) : (void*)h->rt->impl->data(h->at(t).region);
+}
+
+int roc_host_tensor_dtype(roc_host* h, int t) {
+  const TensorImpl& x = h->rt->impl->t(h->at(t).region);
+  return x.isBf16 ? ROC_HOST_DTYPE_BFLOAT16 : x.isInt ? ROC_HOST_DTYPE_INT32 : ROC_HOST_DTYPE_FLOAT32;
 }
 
 int roc_host_num_parameters(roc_host* h) { return (int)h->m().parameters.size(); }

@@ -33,7 +33,9 @@ struct TensorImpl {
   int64_t ld = 0;         // floats between rows (H rounded up to 4 for node tensors)
   bool isInt = false;     // create_node_tensor<int> (mask)
   bool isBf16 = false;    // create_node_tensor<__nv_bfloat16>: a leaf feature matrix held as bf16 bits, ld elements
-                          // per row (H rounded up to 8); reached only through RuntimeImpl::data_bf16, never as float*
+                          // per row (H rounded up to 8); or, with Model::set_bf16_aggregation, a Linear output that
+                          // only a sum ScatterGather reads (its gradient stays fp32, with the same ld).  The bits are
+                          // reached only through RuntimeImpl::data_bf16, never as float*
   bool isWeight = false;
   bool requiresGrad = false;
   bool produced = false;  // output of some op
@@ -120,7 +122,7 @@ struct RuntimeImpl {
   void dfree_all();
   int new_tensor(int64_t rows, int H, int64_t ld, bool isInt, bool isWeight);
   float* data(int region);   // allocates on first use, zero-filled; a bf16 tensor is an error
-  float* grad(int region);   // a bf16 tensor has no gradient: an error
+  float* grad(int region);   // a bf16 leaf has no gradient: an error
   uint16_t* data_bf16(int region);   // the bf16 tensor's bits, allocated on first use, zero-filled
   // append `halo` rows to the data / grad buffer of x (re-allocating and copying if it already exists)
   void grow_halo(TensorImpl& x, bool grad, int64_t halo);

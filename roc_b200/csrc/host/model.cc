@@ -37,7 +37,7 @@ GnnOp::GnnOp(const Tensor& _input1, const Tensor& _input2, const Tensor& _input3
 // ------------------------------------------------------------------ Model ---
 Model::Model(const Graph& _graph, Context _ctx, Runtime* _runtime)
     : mode(MD_MODE_TRAIN), myGraph(_graph), ctx(_ctx), runtime(_runtime), optimizer(NULL), epoch_num(0),
-      fuse(true), printMetrics(true), exactBackward(false) {}
+      fuse(true), printMetrics(true), exactBackward(false), bf16Aggregation(false) {}
 
 // gnn.cc:475-532: node tensor = [numNodes][H]; this process holds its vertex range.
 template <>
@@ -156,6 +156,10 @@ void Model::set_exact_backward(bool on) {
   if (ctx->flatGrad) ROC_FATAL("set_exact_backward: call it before init()");
   exactBackward = on;
 }
+void Model::set_bf16_aggregation(bool on) {
+  if (ctx->flatGrad) ROC_FATAL("set_bf16_aggregation: call it before init()");
+  bf16Aggregation = on;
+}
 void Model::get_aggr_index(const Tensor& out, uint32_t* host) const {
   for (GnnOp* op : layers) {
     ScatterGather* sg = dynamic_cast<ScatterGather*>(op);
@@ -233,6 +237,8 @@ ScatterGather* as_sum_sg(GnnOp* op) {
 bool Model::init(const Config& config) {
   (void)config;
   RuntimeImpl* rt = ctx;
+  if (bf16Aggregation && rt->numParts > 1)
+    ROC_FATAL("set_bf16_aggregation: bf16 aggregation inputs run on one partition only (numParts > 1 is not supported)");
   // a bf16 tensor is read by linear (its X) and dropout only; any other op would need an fp32 view of it
   for (size_t l = 0; l < layers.size(); l++) {
     GnnOp* op = layers[l];
@@ -455,6 +461,21 @@ bool Model::init(const Config& config) {
       n->bwdFused = true;
     }
   }
+  // ---- bf16 aggregation inputs: what a Linear(NONE) writes (its output, or the fused norm's) and one sum
+  //      scatter_gather alone reads is stored in bf16, rows of round_up(H, 8) elements; its gradient twin keeps that ld
+  if (bf16Aggregation) {
+    Wiring w = wire(layers);
+    for (size_t l = 0; l < layers.size(); l++) {
+      Linear* lin = as<Linear>(layers[l]);
+      if (!lin || lin->activation != AC_MODE_NONE) continue;
+      const int r = lin->fwdOut >= 0 ? lin->fwdOut : lin->outputs[0].region;
+      if (w.consumers[r] != 1 || !as_sum_sg(layers[w.consumerOp[r]])) continue;
+      TensorImpl& x = rt->t(r);
+      if (x.data || x.grad) ROC_FATAL("set_bf16_aggregation: a tensor that becomes bf16 was already allocated");
+      x.isBf16 = true;
+      x.ld = round_up8(x.H);
+    }
+  }
   for (size_t l = 0; l < layers.size(); l++) layers[l]->init(*this);
   rt->opNames.clear();
   for (size_t l = 0; l < layers.size(); l++) {
@@ -525,9 +546,9 @@ void Model::zero_gradients(void) {
 void Model::set_tensor(const Tensor& t, const void* host, bool grad) {
   RuntimeImpl* rt = ctx;
   TensorImpl& x = rt->t(t.region);
-  if (x.isBf16) {
+  if (x.isBf16 && !(grad && x.produced)) {
     // fp32 host rows, rounded on the device chunk by chunk: no full-size fp32 copy is ever resident
-    if (grad) ROC_FATAL("set_tensor(grad=true): a bf16 tensor has no gradient");
+    if (grad) ROC_FATAL("set_tensor(grad=true): a bf16 leaf tensor has no gradient");
     uint16_t* dst = rt->data_bf16(t.region);
     const int64_t chunkRows = std::max<int64_t>(1, (int64_t)(64u << 20) / x.H);
     rt->ensure_staging((size_t)std::min<int64_t>(chunkRows, x.rows) * x.H * sizeof(float));
@@ -562,9 +583,9 @@ void Model::set_tensor(const Tensor& t, const void* host, bool grad) {
 void Model::get_tensor(const Tensor& t, void* host, bool grad) const {
   RuntimeImpl* rt = ctx;
   TensorImpl& x = rt->t(t.region);
-  if (x.isBf16) {
+  if (x.isBf16 && !(grad && x.produced)) {
     // widened exactly on the device into staging, chunk by chunk
-    if (grad) ROC_FATAL("get_tensor(grad=true): a bf16 tensor has no gradient");
+    if (grad) ROC_FATAL("get_tensor(grad=true): a bf16 leaf tensor has no gradient");
     const uint16_t* src = rt->data_bf16(t.region);
     const int64_t chunkRows = std::max<int64_t>(1, (int64_t)(64u << 20) / x.H);
     rt->ensure_staging((size_t)std::min<int64_t>(chunkRows, x.rows) * x.H * sizeof(float));
@@ -861,6 +882,15 @@ void ScatterGather::forward(const Model& model) {
   }
   const int outRegion = fwdOut >= 0 ? fwdOut : outputs[0].region;
   rt->sg_begin(-H);          // negative width = the exposed part of the halo exchange (profile mode only)
+  if (rt->t(inputs[0].region).isBf16) {   // set_bf16_aggregation: one partition, nothing to exchange
+    rt->sg_end();
+    float* dst = rt->data(outRegion);
+    rt->sg_begin(H);
+    ROC_CHECK(roc_sg_forward_planned_bf16(model.myGraph.plan, H, rt->data_bf16(inputs[0].region), ldIn, dst,
+                                          rt->t(outRegion).ld, epilogue, rt->stream));
+    rt->sg_end();
+    return;
+  }
   const float* src = gathered(model, rt->data(inputs[0].region), ldIn, H, &rt->t(inputs[0].region), false);
   rt->sg_end();
   float* dst = rt->data(outRegion);
@@ -1110,8 +1140,14 @@ void Linear::forward(const Model& model) {
   // and block k's boundary rows travel while block k + 1 is computed; otherwise one block = all rows.
   PushPipe pipe(model, outRegion, /*grad=*/false);
   const int inDim = (int)weight.dims[0], outDim = (int)weight.dims[1];
-  float* Y = rt->data(outRegion);
   const int64_t ldY = rt->t(outRegion).ld;
+  // a bf16 Y (set_bf16_aggregation) holds bits: rows of ldY elements, stored by the kernels under ROC_LINEAR_Y_BF16
+  const bool yBf16 = rt->t(outRegion).isBf16;
+  float* Y = yBf16 ? reinterpret_cast<float*>(rt->data_bf16(outRegion)) : rt->data(outRegion);
+  auto yRow = [&](int64_t r0) {
+    return yBf16 ? reinterpret_cast<float*>(rt->data_bf16(outRegion) + r0 * ldY) : Y + r0 * ldY;
+  };
+  const int flags = this->flags | (yBf16 ? ROC_LINEAR_Y_BF16 : 0);
   if (dropOp >= 0) {
     // dropout -> linear: the mask is generated packed (1 bit / element) and applied while the GEMM
     // loads X, so the dropped copy of X is never materialised
@@ -1124,7 +1160,7 @@ void Linear::forward(const Model& model) {
       const uint16_t* Xb = rt->data_bf16(f.inRegion);
       for (size_t k = 0; k < pipe.blocks(); k++) {
         const int64_t r0 = pipe.row0(k), nr = pipe.rows(k, model.local_rows());
-        ROC_CHECK(roc_linear_fwd_bf16(nr, inDim, outDim, Xb + r0 * ldX, ldX, rt->data(weight.region), Y + r0 * ldY, ldY,
+        ROC_CHECK(roc_linear_fwd_bf16(nr, inDim, outDim, Xb + r0 * ldX, ldX, rt->data(weight.region), yRow(r0), ldY,
                                       (int)activation, flags, g.d_rowEnd + r0, pipe.colLeft(k),
                                       f.rate > 0.0f ? dropMask + r0 * dropLd : NULL, dropLd, f.rate, rt->stream));
         pipe.pushed(k, Y, ldY, outDim);
@@ -1134,7 +1170,7 @@ void Linear::forward(const Model& model) {
     const float* X = rt->data(f.inRegion);
     for (size_t k = 0; k < pipe.blocks(); k++) {
       const int64_t r0 = pipe.row0(k), nr = pipe.rows(k, model.local_rows());
-      ROC_CHECK(roc_linear_fwd_dropout(nr, inDim, outDim, X + r0 * ldX, ldX, rt->data(weight.region), Y + r0 * ldY, ldY,
+      ROC_CHECK(roc_linear_fwd_dropout(nr, inDim, outDim, X + r0 * ldX, ldX, rt->data(weight.region), yRow(r0), ldY,
                                        (int)activation, flags, g.d_rowEnd + r0, pipe.colLeft(k), dropMask + r0 * dropLd,
                                        dropLd, f.rate, rt->stream));
       pipe.pushed(k, Y, ldY, outDim);
@@ -1146,7 +1182,7 @@ void Linear::forward(const Model& model) {
     const uint16_t* Xb = rt->data_bf16(inputs[0].region);
     for (size_t k = 0; k < pipe.blocks(); k++) {
       const int64_t r0 = pipe.row0(k), nr = pipe.rows(k, model.local_rows());
-      ROC_CHECK(roc_linear_fwd_bf16(nr, inDim, outDim, Xb + r0 * ldX, ldX, rt->data(weight.region), Y + r0 * ldY, ldY,
+      ROC_CHECK(roc_linear_fwd_bf16(nr, inDim, outDim, Xb + r0 * ldX, ldX, rt->data(weight.region), yRow(r0), ldY,
                                     (int)activation, flags, g.d_rowEnd + r0, pipe.colLeft(k), NULL, 0, 0.0f,
                                     rt->stream));
       pipe.pushed(k, Y, ldY, outDim);
@@ -1156,7 +1192,7 @@ void Linear::forward(const Model& model) {
   const float* X = rt->data(inputs[0].region);
   for (size_t k = 0; k < pipe.blocks(); k++) {
     const int64_t r0 = pipe.row0(k), nr = pipe.rows(k, model.local_rows());
-    ROC_CHECK(roc_linear_fwd(nr, inDim, outDim, X + r0 * ldX, ldX, rt->data(weight.region), Y + r0 * ldY, ldY,
+    ROC_CHECK(roc_linear_fwd(nr, inDim, outDim, X + r0 * ldX, ldX, rt->data(weight.region), yRow(r0), ldY,
                              (int)activation, flags, g.d_rowEnd + r0, pipe.colLeft(k), rt->stream));
     pipe.pushed(k, Y, ldY, outDim);
   }

@@ -68,7 +68,7 @@ uint16_t* RuntimeImpl::data_bf16(int region) {
 
 float* RuntimeImpl::grad(int region) {
   TensorImpl& x = t(region);
-  if (x.isBf16) ROC_FATAL("a bf16 node tensor has no gradient");
+  if (x.isBf16 && !x.produced) ROC_FATAL("a bf16 leaf tensor has no gradient");   // a produced one has an fp32 twin
   if (!x.grad) {
     size_t bytes = (size_t)(x.rows + x.haloGrad) * (size_t)x.ld * sizeof(float);
     x.grad = (float*)dmalloc(bytes);

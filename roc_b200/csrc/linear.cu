@@ -8,8 +8,8 @@ namespace roc {
 int simt_dw_splits(int64_t rows, int inDim, int outDim);
 // X / ldX of the forward and dW: fp32, or bf16 (raw bits) when xBf16
 int simt_linear_fwd(int64_t rows, int inDim, int outDim, const void* X, bool xBf16, int64_t ldX, const float* W,
-                    float* Y, int64_t ldY, int relu, const uint64_t* rowEnd, uint64_t colLeft, const DropMask* dm,
-                    cudaStream_t st);
+                    void* Y, bool yBf16, int64_t ldY, int relu, const uint64_t* rowEnd, uint64_t colLeft,
+                    const DropMask* dm, cudaStream_t st);
 int simt_linear_dx(int64_t rows, int inDim, int outDim, const float* dY, int64_t ldDY, const float* W, float* dX,
                    int64_t ldDX, int accumulate, const DropMask* dm, const float* reluOf, int64_t ldR,
                    const uint64_t* rowEnd, uint64_t colLeft, cudaStream_t st);
@@ -21,9 +21,10 @@ int relu_bwd_inplace(int64_t rows, int H, const float* Y, int64_t ldY, float* dY
 // tensor-core path (linear_tc.cu, linear_tc_dw.cu); each returns ROC_ERR_UNSUPPORTED when the
 // shape / alignment is outside what the wgmma kernels take.
 // They describe the launch they made in *info (roc_last_gemm_info).
+// Y is fp32, or bf16 (raw bits) when yBf16
 int tc_linear_fwd(int64_t rows, int inDim, int outDim, const void* X, bool xBf16, int64_t ldX, const float* W,
-                  float* Y, int64_t ldY, int relu, const uint64_t* rowEnd, uint64_t colLeft, const DropMask* dm,
-                  cudaStream_t st, roc_gemm_info* info);
+                  void* Y, bool yBf16, int64_t ldY, int relu, const uint64_t* rowEnd, uint64_t colLeft,
+                  const DropMask* dm, cudaStream_t st, roc_gemm_info* info);
 int tc_linear_dx(int64_t rows, int inDim, int outDim, const float* dY, int64_t ldDY, const float* W, float* dX,
                  int64_t ldDX, int accumulate, const DropMask* dm, const float* reluOf, int64_t ldR,
                  const uint64_t* rowEnd, uint64_t colLeft, cudaStream_t st, roc_gemm_info* info);
@@ -78,6 +79,8 @@ static int linear_fwd_impl(int64_t rows, int inDim, int outDim, const void* X, b
   if (!X || !W || !Y || rows < 0 || inDim <= 0 || outDim <= 0 || ldX < inDim || ldY < outDim) return ROC_ERR_INVALID;
   if (activation != ROC_AC_MODE_NONE && activation != ROC_AC_MODE_RELU) return ROC_ERR_UNSUPPORTED;  // linear_kernel.cu:96
   if ((flags & ROC_LINEAR_NORM_EPILOGUE) && !rowEnd) return ROC_ERR_INVALID;
+  const bool yBf16 = (flags & ROC_LINEAR_Y_BF16) != 0;
+  if (yBf16 && (ldY % 8)) return ROC_ERR_INVALID;
   if (rows == 0) return ROC_OK;
   const uint64_t* re = (flags & ROC_LINEAR_NORM_EPILOGUE) ? rowEnd : nullptr;
   const int relu = activation == ROC_AC_MODE_RELU;
@@ -85,10 +88,10 @@ static int linear_fwd_impl(int64_t rows, int inDim, int outDim, const void* X, b
   return run_gemm(
       0,
       [&](roc_gemm_info* i) {
-        return tc_linear_fwd(rows, inDim, outDim, X, xBf16, ldX, W, Y, ldY, relu, re, colLeft, dm, st, i);
+        return tc_linear_fwd(rows, inDim, outDim, X, xBf16, ldX, W, Y, yBf16, ldY, relu, re, colLeft, dm, st, i);
       },
       [&](roc_gemm_info*) {
-        return simt_linear_fwd(rows, inDim, outDim, X, xBf16, ldX, W, Y, ldY, relu, re, colLeft, dm, st);
+        return simt_linear_fwd(rows, inDim, outDim, X, xBf16, ldX, W, Y, yBf16, ldY, relu, re, colLeft, dm, st);
       });
 }
 

@@ -32,8 +32,9 @@ struct GemmP {
   const float* reluOf; int64_t ldR;   // epilogue relu backward: reluOf(m, n) > 0 ? v : 0 (NULL = none)
 };
 
-// TA / TB: element type of A / B, float or uint16_t (a bf16 X, widened exactly as it is loaded)
-template <bool A_KCONTIG, bool B_KCONTIG, class TA = float, class TB = float>
+// TA / TB: element type of A / B, float or uint16_t (a bf16 X, widened exactly as it is loaded).  TC: of C, float or
+// uint16_t (a forward Y stored in bf16: each result is narrowed by f32_to_bf16_rne as it is stored).
+template <bool A_KCONTIG, bool B_KCONTIG, class TA = float, class TB = float, class TC = float>
 __global__ void __launch_bounds__(G_THREADS)
 k_sgemm(const GemmP p) {
   const TA* pA = static_cast<const TA*>(p.A);
@@ -115,8 +116,12 @@ k_sgemm(const GemmP p) {
       if (p.maskOn == 3) v = drop_apply(p.mask, p.ldm, p.mscale, m, n, v);
       if (p.reluOf) v = (p.reluOf[m * p.ldR + n] > 0.f) ? v : 0.f;
       if (p.rowEnd) v = v / d;           // fwd: the model's indegree_norm (gnn.cc:82)
-      float* dst = C + m * p.ldc + n;
-      *dst = p.accumulate ? *dst + v : v;
+      if constexpr (sizeof(TC) == 2) {
+        reinterpret_cast<uint16_t*>(p.C)[m * p.ldc + n] = f32_to_bf16_rne(v);
+      } else {
+        float* dst = C + m * p.ldc + n;
+        *dst = p.accumulate ? *dst + v : v;
+      }
     }
   }
 }
@@ -167,17 +172,19 @@ static void set_mask(GemmP& p, const DropMask* dm, int on) {
   p.mask = dm->bits; p.ldm = dm->ld; p.mscale = dm->scale; p.maskOn = on;
 }
 
-// X is fp32, or bf16 (raw bits) when xBf16
+// X is fp32, or bf16 (raw bits) when xBf16; Y likewise with yBf16
 int simt_linear_fwd(int64_t rows, int inDim, int outDim, const void* X, bool xBf16, int64_t ldX, const float* W,
-                    float* Y, int64_t ldY, int relu, const uint64_t* rowEnd, uint64_t colLeft, const DropMask* dm,
-                    cudaStream_t st) {
+                    void* Y, bool yBf16, int64_t ldY, int relu, const uint64_t* rowEnd, uint64_t colLeft,
+                    const DropMask* dm, cudaStream_t st) {
   GemmP p{};
-  p.A = X; p.lda = ldX; p.B = W; p.ldb = inDim; p.C = Y; p.ldc = ldY;
+  p.A = X; p.lda = ldX; p.B = W; p.ldb = inDim; p.C = static_cast<float*>(Y); p.ldc = ldY;
   p.M = rows; p.N = outDim; p.K = inDim; p.kPerSplit = inDim; p.splitStrideC = 0;
   p.accumulate = 0; p.relu = relu; p.rowEnd = rowEnd; p.colLeft = colLeft;
   set_mask(p, dm, 1);
   dim3 grid((unsigned)((rows + GB_M - 1) / GB_M), (unsigned)((outDim + GB_N - 1) / GB_N), 1);
-  if (xBf16) k_sgemm<true, true, uint16_t, float><<<grid, G_THREADS, 0, st>>>(p);
+  if (xBf16 && yBf16) k_sgemm<true, true, uint16_t, float, uint16_t><<<grid, G_THREADS, 0, st>>>(p);
+  else if (yBf16) k_sgemm<true, true, float, float, uint16_t><<<grid, G_THREADS, 0, st>>>(p);
+  else if (xBf16) k_sgemm<true, true, uint16_t, float><<<grid, G_THREADS, 0, st>>>(p);
   else k_sgemm<true, true><<<grid, G_THREADS, 0, st>>>(p);
   ROC_LAUNCH_CHECK();
   return ROC_OK;

@@ -88,14 +88,18 @@ struct TcParams {
 };
 
 // Epilogue stage switches: compile-time when the kernel is instantiated for a fixed combination
-// (EPI >= 0, a bit mask), read from the parameters for the generic instantiation (EPI < 0).
-enum { EPI_RELU = 1, EPI_OMASK = 2, EPI_RELUOF = 4, EPI_NORM = 8, EPI_ACC = 16 };
+// (EPI >= 0, a bit mask), read from the parameters for the generic instantiation (EPI < 0, or EPI_GEN with
+// EPI_YBF16).  EPI_YBF16 stores Y in bf16 (ROC_LINEAR_Y_BF16): always compile-time, so the fp32 instantiations do not
+// change.
+enum { EPI_RELU = 1, EPI_OMASK = 2, EPI_RELUOF = 4, EPI_NORM = 8, EPI_ACC = 16, EPI_YBF16 = 32, EPI_GEN = 64 };
 #define EPI_FLAGS(EPI, p)                                                        \
-  const bool fRelu = (EPI) < 0 ? (p).relu != 0 : ((EPI) & EPI_RELU) != 0;         \
-  const bool fOmask = (EPI) < 0 ? (p).omask != nullptr : ((EPI) & EPI_OMASK) != 0; \
-  const bool fReluOf = (EPI) < 0 ? (p).reluOf != nullptr : ((EPI) & EPI_RELUOF) != 0; \
-  const bool fNorm = (EPI) < 0 ? (p).rowEnd != nullptr : ((EPI) & EPI_NORM) != 0;  \
-  const bool fAcc = (EPI) < 0 ? (p).accumulate != 0 : ((EPI) & EPI_ACC) != 0;
+  constexpr bool fGen = (EPI) < 0 || ((EPI) & EPI_GEN) != 0;                     \
+  constexpr bool fYb = (EPI) >= 0 && ((EPI) & EPI_YBF16) != 0;                   \
+  const bool fRelu = fGen ? (p).relu != 0 : ((EPI) & EPI_RELU) != 0;              \
+  const bool fOmask = fGen ? (p).omask != nullptr : ((EPI) & EPI_OMASK) != 0;      \
+  const bool fReluOf = fGen ? (p).reluOf != nullptr : ((EPI) & EPI_RELUOF) != 0;   \
+  const bool fNorm = fGen ? (p).rowEnd != nullptr : ((EPI) & EPI_NORM) != 0;       \
+  const bool fAcc = fGen ? (p).accumulate != 0 : ((EPI) & EPI_ACC) != 0;
 
 // b = the low words of the row's (start, end) offsets, so that end - start is its indegree; (0, 1) past the last row
 __device__ __forceinline__ void row_bounds(const TcParams& p, int64_t row, uint32_t (&b)[2]) {
@@ -115,6 +119,17 @@ __device__ __forceinline__ void tc_store_pair(const TcParams& p, bool fAcc, int6
   } else {
     y[0] = fAcc ? y[0] + x0 : x0;
   }
+}
+
+// The same for a bf16 Y (EPI_YBF16, never accumulated): each value narrowed by f32_to_bf16_rne
+__device__ __forceinline__ uint32_t pack_bf16x2(float x0, float x1) {
+  return (uint32_t)f32_to_bf16_rne(x0) | ((uint32_t)f32_to_bf16_rne(x1) << 16);
+}
+__device__ __forceinline__ void tc_store_pair_bf16(const TcParams& p, int64_t row, int col, float x0, float x1) {
+  if (row >= p.rows || col >= p.outDim) return;
+  uint16_t* y = reinterpret_cast<uint16_t*>(p.Y) + row * p.ldY + col;
+  if (col + 1 < p.outDim) *reinterpret_cast<uint32_t*>(y) = pack_bf16x2(x0, x1);
+  else y[0] = f32_to_bf16_rne(x0);
 }
 
 __device__ __forceinline__ void wgmma_wait_1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
@@ -352,6 +367,7 @@ k_tc_linear(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
       const int wg = warp >> 2;
       const bool leader = (threadIdx.x & 127) == 0;
       float* yb = reinterpret_cast<float*>(smem + p.yOff) + wg * 64 * 32;   // chunk c at + c * TC_BM * 32
+      uint16_t* ybh = reinterpret_cast<uint16_t*>(smem + p.yOff) + wg * 64 * 32;   // the same for a bf16 Y
       if (leader) bulk_wait_read();
       named_barrier(1 + wg, 128);
 #pragma unroll
@@ -361,26 +377,40 @@ k_tc_linear(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
 #pragma unroll
           for (int h = 0; h < 2; h++) {
             const int r = (rl & 63) + 8 * h, cc = 8 * j + 2 * t;
-            *reinterpret_cast<float2*>(yb + c * TC_BM * 32 + r * 32 + (((cc >> 2) ^ g) << 2) + (cc & 3)) =
-                make_float2(acc[c][4 * j + 2 * h], acc[c][4 * j + 2 * h + 1]);
+            if constexpr (fYb) {
+              // [64][32] bf16, 64-byte rows with the 64-byte swizzle: 16-byte unit j of row r at j ^ ((r >> 1) & 3)
+              *reinterpret_cast<uint32_t*>(ybh + c * TC_BM * 32 + r * 32 + ((j ^ ((r >> 1) & 3)) << 3) + 2 * t) =
+                  pack_bf16x2(acc[c][4 * j + 2 * h], acc[c][4 * j + 2 * h + 1]);
+            } else {
+              *reinterpret_cast<float2*>(yb + c * TC_BM * 32 + r * 32 + (((cc >> 2) ^ g) << 2) + (cc & 3)) =
+                  make_float2(acc[c][4 * j + 2 * h], acc[c][4 * j + 2 * h + 1]);
+            }
           }
       fence_proxy_async_smem();
       named_barrier(1 + wg, 128);
       if (leader) {
-        for (int c = 0; c < NC; c++)
-          tma_store_2d(&mapY, yb + c * TC_BM * 32, n0 + 32 * c, (int)(tile * TC_BM) + 64 * wg);
+        for (int c = 0; c < NC; c++) {
+          if constexpr (fYb) tma_store_2d(&mapY, ybh + c * TC_BM * 32, n0 + 32 * c, (int)(tile * TC_BM) + 64 * wg);
+          else tma_store_2d(&mapY, yb + c * TC_BM * 32, n0 + 32 * c, (int)(tile * TC_BM) + 64 * wg);
+        }
         bulk_commit();
       }
-      // The TMA store covers the columns below p.yCols, a multiple of 4: it writes whole 16-byte units, so past a
-      // column count that is not a multiple of 4 it would overwrite Y's padding.  The last 1-3 columns go directly.
+      // The TMA store covers the columns below p.yCols, a multiple of 4 (8 for a bf16 Y): it writes whole 16-byte
+      // units, so past a column count that is not such a multiple it would overwrite Y's padding.  The last columns go
+      // directly.
 #pragma unroll
       for (int c = 0; c < NC; c++)
 #pragma unroll
         for (int j = 0; j < 4; j++) {
           const int col = n0 + c * 32 + j * 8 + 2 * t;
           if (col >= p.yCols) {
-            tc_store_pair(p, false, row0, col, acc[c][4 * j], acc[c][4 * j + 1]);
-            tc_store_pair(p, false, row1, col, acc[c][4 * j + 2], acc[c][4 * j + 3]);
+            if constexpr (fYb) {
+              tc_store_pair_bf16(p, row0, col, acc[c][4 * j], acc[c][4 * j + 1]);
+              tc_store_pair_bf16(p, row1, col, acc[c][4 * j + 2], acc[c][4 * j + 3]);
+            } else {
+              tc_store_pair(p, false, row0, col, acc[c][4 * j], acc[c][4 * j + 1]);
+              tc_store_pair(p, false, row1, col, acc[c][4 * j + 2], acc[c][4 * j + 3]);
+            }
           }
         }
     } else {
@@ -389,8 +419,13 @@ k_tc_linear(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
 #pragma unroll
         for (int j = 0; j < 4; j++) {
           const int col = n0 + c * 32 + j * 8 + 2 * t;
-          tc_store_pair(p, fAcc, row0, col, acc[c][4 * j], acc[c][4 * j + 1]);
-          tc_store_pair(p, fAcc, row1, col, acc[c][4 * j + 2], acc[c][4 * j + 3]);
+          if constexpr (fYb) {
+            tc_store_pair_bf16(p, row0, col, acc[c][4 * j], acc[c][4 * j + 1]);
+            tc_store_pair_bf16(p, row1, col, acc[c][4 * j + 2], acc[c][4 * j + 3]);
+          } else {
+            tc_store_pair(p, fAcc, row0, col, acc[c][4 * j], acc[c][4 * j + 1]);
+            tc_store_pair(p, fAcc, row1, col, acc[c][4 * j + 2], acc[c][4 * j + 3]);
+          }
         }
     }
   }
@@ -410,8 +445,12 @@ struct TsEpilogue {
 };
 
 // the epilogue instantiation that serves `epi`: the combinations the GCN path produces have their own, anything else
-// takes the generic kernel (-1)
+// takes the generic kernel (-1).  A bf16 Y (a forward) has its own for no epilogue and the norm, and a generic one.
 static int tc_instance(int epi) {
+  if (epi & EPI_YBF16) {
+    const int b = epi & ~EPI_YBF16;
+    return EPI_YBF16 | ((b == 0 || b == EPI_NORM) ? b : EPI_GEN);
+  }
   return (epi == 0 || epi == EPI_NORM || epi == EPI_OMASK || epi == (EPI_OMASK | EPI_RELUOF | EPI_NORM)) ? epi : -1;
 }
 
@@ -426,6 +465,13 @@ static int tc_launch_epi(dim3 grid, size_t smemBytes, const TcMaps& m, const TcP
 template <int NC, class TA>
 static int tc_launch(dim3 grid, size_t smemBytes, int epi, const TcMaps& m, const TcParams& q, cudaStream_t st) {
   constexpr int E1 = EPI_NORM, E2 = EPI_OMASK, E3 = EPI_OMASK | EPI_RELUOF | EPI_NORM;
+  constexpr int Y0 = EPI_YBF16, Y1 = EPI_YBF16 | EPI_NORM, YG = EPI_YBF16 | EPI_GEN;
+  switch (tc_instance(epi)) {   // a bf16 Y: a forward, of an fp32 or a bf16 A
+    case Y0: return tc_launch_epi<NC, Y0, TA>(grid, smemBytes, m, q, st);
+    case Y1: return tc_launch_epi<NC, Y1, TA>(grid, smemBytes, m, q, st);
+    case YG: return tc_launch_epi<NC, YG, TA>(grid, smemBytes, m, q, st);
+    default: break;
+  }
   if constexpr (sizeof(TA) == 2) {
     // a bf16 A is a leaf X in a forward: its epilogues are relu and the norm, so the dX instantiations are not built
     switch (tc_instance(epi)) {
@@ -445,12 +491,12 @@ static int tc_launch(dim3 grid, size_t smemBytes, int epi, const TcMaps& m, cons
 }
 
 // Y[rows][N] (op)= A[rows][K] * B^T with B(n, k) taken from W as k_split_w describes; A is fp32, or bf16 (raw bits)
-// when aBf16
+// when aBf16; Y likewise with yBf16 (written, never accumulated)
 static int ts_gemm(int64_t rows, int K, int N, const void* A, bool aBf16, int64_t ldA, const float* W, int ldW,
-                   int transposed, float* Y, int64_t ldY, const DropMask* inMask, const TsEpilogue& e,
+                   int transposed, void* Y, bool yBf16, int64_t ldY, const DropMask* inMask, const TsEpilogue& e,
                    cudaStream_t st, roc_gemm_info* info) {
   if (K < 8 || N < 1 || rows < 1) return ROC_ERR_UNSUPPORTED;
-  if ((ldA % (aBf16 ? 8 : 4)) || (ldY % 4) || !aligned16(A) || !aligned16(Y)) return ROC_ERR_UNSUPPORTED;
+  if ((ldA % (aBf16 ? 8 : 4)) || (ldY % (yBf16 ? 8 : 4)) || !aligned16(A) || !aligned16(Y)) return ROC_ERR_UNSUPPORTED;
   if (e.reluOf && ((e.ldR % 4) || !aligned16(e.reluOf))) return ROC_ERR_UNSUPPORTED;
   if (e.outMask && !aligned16(e.outMask->bits)) return ROC_ERR_UNSUPPORTED;   // TMA takes the words [128][4] per tile
   if (inMask && !aligned16(inMask->bits)) return ROC_ERR_UNSUPPORTED;         // and [128][4] per k-block
@@ -492,10 +538,13 @@ static int ts_gemm(int64_t rows, int K, int N, const void* A, bool aBf16, int64_
                                   TC_BM, 4))
     return ROC_ERR_UNSUPPORTED;
   // Y leaves by TMA stores from a staging tile when it is written, not accumulated, and the tile is <= 64 columns wide
-  // (the 128-wide tile keeps its shared memory for the ring)
-  const int yCols = N & ~3;
+  // (the 128-wide tile keeps its shared memory for the ring).  A bf16 tile is [64][32] with 64-byte rows.
+  const int yCols = N & (yBf16 ? ~7 : ~3);
   const bool ystage = !e.accumulate && NC <= 2 && yCols > 0;
-  if (ystage && !make_tmap_f32_2d(&m.Y, Y, (uint64_t)rows, (uint64_t)yCols, (uint64_t)ldY, TC_BM / 2, 32))
+  if (ystage && !(yBf16 ? make_tmap_bf16_2d(&m.Y, static_cast<const uint16_t*>(Y), (uint64_t)rows, (uint64_t)yCols,
+                                            (uint64_t)ldY, TC_BM / 2, 32)
+                        : make_tmap_f32_2d(&m.Y, static_cast<const float*>(Y), (uint64_t)rows, (uint64_t)yCols,
+                                           (uint64_t)ldY, TC_BM / 2, 32)))
     return ROC_ERR_UNSUPPORTED;
 
   // Shared memory: W resident when its slice fits beside both epilogue buffers, the Y staging tile and a ring that
@@ -508,7 +557,7 @@ static int ts_gemm(int64_t rows, int K, int N, const void* A, bool aBf16, int64_
   const size_t mBytes = inMask ? (size_t)TC_BM * 4 * 4 : 0;
   const size_t wBytes = 2 * (size_t)numKb * bBytes;
   const size_t eBytes = (e.reluOf ? (size_t)TC_BM * BN * 4 : 0) + (e.outMask ? (size_t)TC_BM * 4 * 4 : 0);
-  const size_t yBytes = ystage ? (size_t)TC_BM * BN * 4 : 0;
+  const size_t yBytes = ystage ? (size_t)TC_BM * BN * (yBf16 ? 2 : 4) : 0;
   const size_t fixedBytes = 1024 /*align*/ + 256 /*barriers*/ + yBytes;
   const bool wres = ring_stages(aBytes + mBytes, fixedBytes + wBytes + 2 * eBytes, maxStages) >= resMinStages;
   const size_t stageBytes = aBytes + (wres ? 0 : 2 * bBytes) + mBytes;
@@ -517,7 +566,7 @@ static int ts_gemm(int64_t rows, int K, int N, const void* A, bool aBf16, int64_
   const int stages = ring_stages(stageBytes, fixedBytes + wUsed + eb * eBytes, maxStages);
   if (!stages) return ROC_ERR_UNSUPPORTED;
   TcParams q{};
-  q.Y = Y; q.ldY = ldY; q.rows = rows; q.outDim = N; q.numKb = numKb; q.stages = stages;
+  q.Y = static_cast<float*>(Y); q.ldY = ldY; q.rows = rows; q.outDim = N; q.numKb = numKb; q.stages = stages;
   q.accumulate = e.accumulate;
   if (inMask) { q.mask = inMask->bits; q.ldm = inMask->ld; q.mscale = inMask->scale; }
   q.relu = e.relu;
@@ -537,7 +586,7 @@ static int ts_gemm(int64_t rows, int K, int N, const void* A, bool aBf16, int64_
   if (numTiles < gx) gx = (int)numTiles;
   dim3 grid((unsigned)gx, (unsigned)nTiles, 1);
   const int epi = (q.relu ? EPI_RELU : 0) | (q.omask ? EPI_OMASK : 0) | (q.reluOf ? EPI_RELUOF : 0) |
-                  (q.rowEnd ? EPI_NORM : 0) | (q.accumulate ? EPI_ACC : 0);
+                  (q.rowEnd ? EPI_NORM : 0) | (q.accumulate ? EPI_ACC : 0) | (yBf16 ? EPI_YBF16 : 0);
   if (info) {
     info->nc = NC; info->epi = tc_instance(epi); info->grid_x = (int)grid.x; info->grid_y = (int)grid.y;
     info->stages = stages; info->w_resident = wres; info->epi_bufs = eb;
@@ -556,13 +605,13 @@ static int ts_gemm(int64_t rows, int K, int N, const void* A, bool aBf16, int64_
   }
 }
 
-// X is fp32, or bf16 (raw bits) when xBf16
+// X is fp32, or bf16 (raw bits) when xBf16; Y likewise with yBf16
 int tc_linear_fwd(int64_t rows, int inDim, int outDim, const void* X, bool xBf16, int64_t ldX, const float* W,
-                  float* Y, int64_t ldY, int relu, const uint64_t* rowEnd, uint64_t colLeft, const DropMask* dm,
-                  cudaStream_t st, roc_gemm_info* info) {
+                  void* Y, bool yBf16, int64_t ldY, int relu, const uint64_t* rowEnd, uint64_t colLeft,
+                  const DropMask* dm, cudaStream_t st, roc_gemm_info* info) {
   TsEpilogue e;
   e.relu = relu; e.rowEnd = rowEnd; e.colLeft = colLeft;
-  return ts_gemm(rows, inDim, outDim, X, xBf16, ldX, W, inDim, 0, Y, ldY, dm, e, st, info);
+  return ts_gemm(rows, inDim, outDim, X, xBf16, ldX, W, inDim, 0, Y, yBf16, ldY, dm, e, st, info);
 }
 
 // dX (+)= dY W, optionally followed in the epilogue by the dropout backward of X's producer
@@ -572,7 +621,7 @@ int tc_linear_dx(int64_t rows, int inDim, int outDim, const float* dY, int64_t l
   TsEpilogue e;
   e.outMask = dm; e.accumulate = accumulate;
   e.reluOf = reluOf; e.ldR = ldR; e.rowEnd = rowEnd; e.colLeft = colLeft;
-  return ts_gemm(rows, outDim, inDim, dY, false, ldDY, W, inDim, 1, dX, ldDX, nullptr, e, st, info);
+  return ts_gemm(rows, outDim, inDim, dY, false, ldDY, W, inDim, 1, dX, false, ldDX, nullptr, e, st, info);
 }
 
 }  // namespace roc

@@ -39,9 +39,11 @@
 //    roc_sg_attn_backward_exact): TSUM is the sum whose NORM epilogue divides by the original graph's in-degree,
 //    TMASK the min / max backward that skips a repeated destination (a duplicate edge), and the attention input
 //    gradient is the ASRC gather itself, run over the transposed plan.
+//  * the sum over bf16 rows (roc_sg_forward_planned_bf16) is BSUM: SUM's row of the table with half-width loads,
+//    widened in registers, on both the register and the ring kernel.
 //
 // Algorithmic bytes per launch (DESIGN.md): E*(4H+4) + Nloc*(4H+8); min / max forward E*(4H+4) + Nloc*(8H+8),
-// backward E*(8H+4) + Nloc*(4H+8); weighted forward E*(4H+8) + Nloc*(4H+8), edge dot E*(4H+8) + Nloc*4H; attention
+// backward E*(8H+4) + Nloc*(4H+8); the sum over bf16 rows E*(2H+4) + Nloc*(4H+8); weighted forward E*(4H+8) + Nloc*(4H+8), edge dot E*(4H+8) + Nloc*4H; attention
 // in DESIGN.md §3.1.
 #include <cub/cub.cuh>
 #include <thrust/iterator/counting_iterator.h>
@@ -222,6 +224,18 @@ template <> struct V<1> {
   static __device__ __forceinline__ T relu(const T& a) { return relu_nanprop(a); }
 };
 
+// One T-column of a bf16 row (BSUM): VEC bf16 values (2 * VEC bytes, element 0 in the low half of the first word),
+// each widened exactly, as to_f32 does.
+__device__ __forceinline__ float4 widen_bf16x4(uint2 u) {
+  return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xFFFF0000u), __uint_as_float(u.y << 16),
+                     __uint_as_float(u.y & 0xFFFF0000u));
+}
+template <int VEC>
+__device__ __forceinline__ typename V<VEC>::T ld_bf16(const char* p) {
+  if constexpr (VEC == 4) return widen_bf16x4(__ldg(reinterpret_cast<const uint2*>(p)));
+  else return to_f32(__ldg(reinterpret_cast<const unsigned short*>(p)));
+}
+
 // ------------------------------------------------------- min / max reduction ---
 // What a kernel does with each gathered row.  SUM adds it; MAX / MIN keep, per float, the value and the source id of
 // the first edge in CSR order that holds the extreme (roc_sg_minmax_forward_planned); MASK is the backward of those:
@@ -233,9 +247,11 @@ template <> struct V<1> {
 // The exact backwards over a transposed plan (roc_sg_transpose_*_backward): TSUM is the sum whose NORM epilogue
 // divides by the in-degree of the original graph (its row ends in p.xrow) instead of the plan's row length; TMASK is
 // MASK where an entry whose destination repeats the previous entry's in the same row (a duplicate edge) adds nothing.
+// BSUM is the sum over bf16 rows (roc_sg_forward_planned_bf16): only its loads differ from SUM's, each T-column of VEC
+// bf16 values widened exactly in registers, so it adds the same floats in the same order.
 enum { SG_RED_SUM = 0, SG_RED_MAX = ROC_SG_AGGR_MAX, SG_RED_MIN = ROC_SG_AGGR_MIN, SG_RED_MASK = 3,
        SG_RED_ASTAT = 4, SG_RED_ATTN = 5, SG_RED_ADST = 6, SG_RED_ASRC = 7, SG_RED_WSUM = 8, SG_RED_EDOT = 9,
-       SG_RED_TSUM = 10, SG_RED_TMASK = 11 };
+       SG_RED_TSUM = 10, SG_RED_TMASK = 11, SG_RED_BSUM = 12 };
 constexpr uint32_t SG_NOARG = 0xFFFFFFFFu;   // index of a row that has no edge yet
 
 // The ordering rule: the candidate v replaces the current a iff it is strictly greater (smaller) or it is NaN and a
@@ -420,6 +436,8 @@ sg_chunk_kernel(const SgParams p) {
   constexpr bool WS = RED == SG_RED_WSUM;                        // loads each edge's weight beside its source id
   constexpr bool ED = RED == SG_RED_EDOT;                        // holds G[i], stores one dot product per edge
   constexpr bool MK = RED == SG_RED_MASK || RED == SG_RED_TMASK; // gathers an index row beside each gradient row
+  constexpr bool BF = RED == SG_RED_BSUM;                        // gathers bf16 rows
+  constexpr uint32_t TB = BF ? 2 * VEC : sizeof(T);              // bytes of one T-column of `in`
   constexpr int WPB = SG_THREADS / L;
   constexpr uint32_t CH = SG_CH;
   const int lane = threadIdx.x % L;
@@ -589,9 +607,13 @@ sg_chunk_kernel(const SgParams p) {
   // traffic): their sums are never stored (flush tests act[]), and no load needs a predicate
   const char* inl[NCH];
 #pragma unroll
-  for (int ch = 0; ch < NCH; ch++)
-    inl[ch] = reinterpret_cast<const char*>(in + min((uint32_t)(lane + ch * L), p.Q - 1u));
-  const uint32_t rowBytes = (uint32_t)p.ldIn * (uint32_t)sizeof(T);
+  for (int ch = 0; ch < NCH; ch++) {
+    if constexpr (BF)
+      inl[ch] = reinterpret_cast<const char*>(p.in) + (size_t)min((uint32_t)(lane + ch * L), p.Q - 1u) * TB;
+    else
+      inl[ch] = reinterpret_cast<const char*>(in + min((uint32_t)(lane + ch * L), p.Q - 1u));
+  }
+  const uint32_t rowBytes = (uint32_t)p.ldIn * TB;
   // MASK: the index row of each edge's source is gathered next to its gradient row
   const char* argl[MK ? NCH : 1];
   uint32_t argRowBytes = 0;
@@ -643,7 +665,10 @@ sg_chunk_kernel(const SgParams p) {
     for (int u = 0; u < U; u++) {
       const uint64_t off = (uint64_t)srcs[u] * rowBytes;
 #pragma unroll
-      for (int ch = 0; ch < NCH; ch++) v[u][ch] = V<VEC>::ld(reinterpret_cast<const T*>(inl[ch] + off));
+      for (int ch = 0; ch < NCH; ch++) {
+        if constexpr (BF) v[u][ch] = ld_bf16<VEC>(inl[ch] + off);
+        else v[u][ch] = V<VEC>::ld(reinterpret_cast<const T*>(inl[ch] + off));
+      }
       if constexpr (MK) {
         const uint64_t aoff = (uint64_t)srcs[u] * argRowBytes;
 #pragma unroll
@@ -732,7 +757,7 @@ sg_chunk_kernel(const SgParams p) {
             } else {
 #pragma unroll
               for (int ch = 0; ch < NCH; ch++) {
-                if constexpr (RED == SG_RED_SUM || RED == SG_RED_TSUM) V<VEC>::add(acc[ch], v[u][ch]);
+                if constexpr (RED == SG_RED_SUM || RED == SG_RED_TSUM || BF) V<VEC>::add(acc[ch], v[u][ch]);
                 else if constexpr (RED == SG_RED_MASK) mask_add(acc[ch], v[u][ch], av[u][ch], p.selfBase + cur);
                 else mm_add<RED>(acc[ch], aidx[ch], v[u][ch], srcs[u]);
               }
@@ -761,14 +786,21 @@ sg_chunk_kernel(const SgParams p) {
 // bytes in flight are well under half of its peak; the ring is refilled stage by stage, so it
 // stays full.  (2) the copies are issued by one lane instead of an index load + IMAD.WIDE +
 // LDG.128 per lane group.  MODE 0 (T) loads the source ids of a stage when it issues it; MODE 2 (U) holds them in
-// the lanes that issue them.  MODE bit 4 makes it TSUM (the NORM epilogue divides by in_degree).
-// A row slot is L*NCH*16 bytes (the worker's whole lane span), so the shared-memory row pitch is a
+// the lanes that issue them.  MODE bit 4 makes it TSUM (the NORM epilogue divides by in_degree); bit 8 makes it
+// BSUM: the copies carry bf16 rows (8 bytes per T-column, rounded up to whole 16-byte units, which stay inside a row
+// whose leading dimension is a multiple of 8 elements), and each lane widens its T-column as it reads it.
+// A row slot is L*NCH*16 bytes (8 for bf16; the worker's whole lane span), so the shared-memory row pitch is a
 // compile-time constant and the adds are unpredicated; lanes past the row's end add stale slot
 // contents they never store.
 __device__ __forceinline__ float4 lds128(uint32_t saddr) {
   float4 v;
   asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(saddr) : "memory");
   return v;
+}
+__device__ __forceinline__ float4 lds_bf16x4(uint32_t saddr) {
+  uint2 u;
+  asm volatile("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(u.x), "=r"(u.y) : "r"(saddr) : "memory");
+  return widen_bf16x4(u);
 }
 __device__ __forceinline__ void mbar_init_a(uint32_t bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
@@ -808,7 +840,9 @@ sg_chunk_kernel_t(const SgParams p) {
   constexpr int WPB = NT / L;
   constexpr uint32_t CH = SG_CH;
   constexpr int G = 4 * S;                       // edges per stage
-  constexpr uint32_t SLOTB = NCH * L * 16;       // shared-memory bytes per gathered row
+  constexpr bool BF = (MODE & 8) != 0;           // bf16 rows
+  constexpr uint32_t CB = BF ? 8 : 16;           // bytes of one T-column
+  constexpr uint32_t SLOTB = NCH * L * CB;       // shared-memory bytes per gathered row
   constexpr uint32_t G4B = 4 * SLOTB;            // one four-row unit
   constexpr uint32_t STAGEB = S * G4B;
   constexpr uint32_t RINGB = P * STAGEB;
@@ -894,8 +928,8 @@ sg_chunk_kernel_t(const SgParams p) {
   // stage k -> ring slot `slot`: issued by the worker's first lane.  A stage that runs past the
   // worker's last edge repeats that edge's source (a duplicate row, L2-resident; never added).
   const char* inB = reinterpret_cast<const char*>(p.in);
-  const uint32_t strideB = (uint32_t)p.ldIn * 16u;
-  const uint32_t rowB = p.Q * 16u;
+  const uint32_t strideB = (uint32_t)p.ldIn * CB;
+  const uint32_t rowB = BF ? (p.Q * 8u + 15u) & ~15u : p.Q * 16u;
   // MODE 2: the source ids never sit in front of the issue.  Lane j of the worker loads, once and up front, the
   // ids of units j, j + L, ... of the worker's edge range (a worker has at most 127 edges = 32 units) and
   // issues those units itself when their ring slot frees (on MODE 0 the id load of the stage about to be issued
@@ -965,14 +999,18 @@ sg_chunk_kernel_t(const SgParams p) {
   for (uint32_t k = 0; k < nStages; k++) {
     mbar_wait_a(bars + slot * 8, parity);
     const uint32_t e0 = eb + k * G;
-    const uint32_t sa = ring + slot * STAGEB + lane * 16;
+    const uint32_t sa = ring + slot * STAGEB + lane * CB;
+    auto lds = [&](int u, int ch) {
+      if constexpr (BF) return lds_bf16x4(sa + u * SLOTB + ch * L * CB);
+      else return lds128(sa + u * SLOTB + ch * L * 16);
+    };
     if (segEnd - e0 >= (uint32_t)G) {
       // the whole stage lies inside the current row segment
 #pragma unroll
       for (int u = 0; u < G; u++)
 #pragma unroll
         for (int ch = 0; ch < NCH; ch++) {
-          const float4 v = lds128(sa + u * SLOTB + ch * L * 16);
+          const float4 v = lds(u, ch);
           acc[ch].x += v.x; acc[ch].y += v.y; acc[ch].z += v.z; acc[ch].w += v.w;
         }
     } else {
@@ -986,7 +1024,7 @@ sg_chunk_kernel_t(const SgParams p) {
           if ((uint32_t)u >= pos && (uint32_t)u < lim) {
 #pragma unroll
             for (int ch = 0; ch < NCH; ch++) {
-              const float4 v = lds128(sa + u * SLOTB + ch * L * 16);
+              const float4 v = lds(u, ch);
               acc[ch].x += v.x; acc[ch].y += v.y; acc[ch].z += v.z; acc[ch].w += v.w;
             }
           }
@@ -1274,7 +1312,7 @@ struct SgRed {
   // into column blocks of VEC * maxQ floats.
   int maxQ4, maxQ1;
   // -1: every row runs on sg_chunk_kernel.  Otherwise vectorised rows at L = 32, NCH <= 2 run on sg_chunk_kernel_t,
-  // and this is the MODE bit the reduction adds there (4: TSUM's NORM epilogue divides by in_degree).
+  // and this is the MODE bit the reduction adds there (4: TSUM's NORM epilogue divides by in_degree; 8: bf16 rows).
   int ring;
   SgFix fix;        // the fix-up of the H-wide partials of the rows the main kernel cut
   bool headsFix;    // the heads-wide partials (out2 / carry2) also go through the sum's fix-ups
@@ -1293,7 +1331,8 @@ struct SgRed {
 // min / max backward's index row, s_src, the record, the local row's own row) would otherwise spill under the
 // occupancy.  WSUM keeps the sum's U and holds U weights beside them, so at one chunk per lane it runs three CTAs per
 // SM.  TSUM and TMASK take the shapes of SUM and MASK, but TMASK, which also holds each group's repeated-destination
-// bits, runs three CTAs per SM at one chunk per lane.
+// bits, runs three CTAs per SM at one chunk per lane.  BSUM is SUM's row with bf16 loads (ring MODE bit 8): the same
+// column blocks, shapes and sum fix-ups, so that its results are SUM's bits on the widened rows.
 constexpr SgRed SG_REDS[] = {
     // red           maxQ4 maxQ1 ring fix           heads  carry           u4  u             minb
     {SG_RED_SUM,     256,  256,  0,   SG_FIX_SUM,   false, SG_CARRY_FLOAT, 4, {8, 4, 2, 1}, {4, 3, 3, 2}},
@@ -1307,11 +1346,12 @@ constexpr SgRed SG_REDS[] = {
     {SG_RED_WSUM,    256,  256,  -1,  SG_FIX_SUM,   false, SG_CARRY_FLOAT, 8, {8, 4, 2, 1}, {3, 3, 3, 2}},
     {SG_RED_EDOT,    128,  256,  -1,  SG_FIX_NONE,  false, SG_CARRY_NONE,  4, {4, 2, 1, 1}, {4, 3, 2, 1}},
     {SG_RED_TSUM,    256,  256,  4,   SG_FIX_OWN,   false, SG_CARRY_FLOAT, 4, {8, 4, 2, 1}, {4, 3, 3, 2}},
-    {SG_RED_TMASK,   128,  256,  -1,  SG_FIX_SUM,   false, SG_CARRY_FLOAT, 4, {4, 2, 1, 1}, {3, 3, 3, 2}}};
+    {SG_RED_TMASK,   128,  256,  -1,  SG_FIX_SUM,   false, SG_CARRY_FLOAT, 4, {4, 2, 1, 1}, {3, 3, 3, 2}},
+    {SG_RED_BSUM,    256,  256,  8,   SG_FIX_SUM,   false, SG_CARRY_FLOAT, 4, {8, 4, 2, 1}, {4, 3, 3, 2}}};
 constexpr bool sg_reds_in_order() {
   for (int i = 0; i < (int)(sizeof(SG_REDS) / sizeof(SG_REDS[0])); i++)
     if (SG_REDS[i].red != i) return false;
-  return sizeof(SG_REDS) / sizeof(SG_REDS[0]) == SG_RED_TMASK + 1;
+  return sizeof(SG_REDS) / sizeof(SG_REDS[0]) == SG_RED_BSUM + 1;
 }
 static_assert(sg_reds_in_order(), "SG_REDS has one row per SG_RED_* value, in order");
 
@@ -1328,7 +1368,7 @@ static int launch_ring(const SgParams& p, cudaStream_t st) {
   constexpr int L = 32, P = 2, NT = 128;
   constexpr int S = NCH == 1 ? 2 : 1, MINB = NCH == 1 ? 4 : 6, MODE = (NCH == 1 ? 2 : 0) | SG_REDS[RED].ring;
   constexpr int WPB = NT / L;
-  constexpr size_t smem = (size_t)WPB * P * S * 4 * NCH * L * 16 + (size_t)WPB * P * 8;
+  constexpr size_t smem = (size_t)WPB * P * S * 4 * NCH * L * ((MODE & 8) ? 8 : 16) + (size_t)WPB * P * 8;
   static std::atomic<uint64_t> configured{0};
   ROC_CUDA(once_per_device(configured, [] {
     return cudaFuncSetAttribute(sg_chunk_kernel_t<L, NCH, S, P, NT, MINB, MODE>,
@@ -1681,8 +1721,9 @@ struct SgEdge {
 // on float4 rows when every leading dimension and pointer allows them.  `arg` holds the min / max indices
 // (written by the forward, gathered by the backward); the sum passes none.  EDOT's column blocks add their partial
 // dot products to dw in block order: the first overwrites it (or adds, with ed.accumulate), the later ones add.
+// `in` holds fp32 rows, bf16 ones (raw bits) for BSUM; its leading dimension is in elements either way.
 template <int RED>
-static int run_planned(roc_sg_plan* pl, int H, const float* in, int64_t ldIn, float* out, int64_t ldOut,
+static int run_planned(roc_sg_plan* pl, int H, const void* in, int64_t ldIn, float* out, int64_t ldOut,
                        const roc_vid_t* arg, int64_t ldArg, int epilogue, roc_vid_t selfBase, cudaStream_t st,
                        const SgEdge& ed = SgEdge()) {
   constexpr SgCarry CARRY = SG_REDS[RED].carry;
@@ -1695,7 +1736,8 @@ static int run_planned(roc_sg_plan* pl, int H, const float* in, int64_t ldIn, fl
   if (rc != ROC_OK) return rc;
   for (int c0 = 0; c0 < H; c0 += blockCols) {
     SgParams p = plan_params(pl);
-    p.in = in + c0; p.out = out ? out + c0 : nullptr; p.epi = epilogue; p.selfBase = selfBase;
+    p.in = static_cast<const char*>(in) + (size_t)c0 * (RED == SG_RED_BSUM ? 2 : 4);
+    p.out = out ? out + c0 : nullptr; p.epi = epilogue; p.selfBase = selfBase;
     if (arg) p.arg = const_cast<roc_vid_t*>(arg) + c0;
     p.ldIn = (size_t)ldIn; p.ldOut = (size_t)ldOut; p.ldArg = (size_t)ldArg;
     p.score = ed.w; p.out2 = ed.dw; p.dwAdd = (ed.accumulate || c0 > 0) ? 1 : 0;
@@ -1715,6 +1757,17 @@ extern "C" int roc_sg_forward_planned(const roc_sg_plan* plc, int H, const float
   clear_launches();
   if (!pl || H <= 0 || !in || !out || ldIn < H || ldOut < H) return ROC_ERR_INVALID;
   return run_planned<SG_RED_SUM>(pl, H, in, ldIn, out, ldOut, nullptr, 0, epilogue, 0, as_stream(stream));
+}
+
+// A 16-byte aligned `in` with ldIn a multiple of 8 is read as float4 T-columns whenever `out` allows it, as the fp32
+// call does for the widened copy of `in` (roc_bf16_to_f32 into any 16-byte aligned buffer whose leading dimension is
+// a multiple of 4): the same column blocks and row shapes, hence the same bits.
+extern "C" int roc_sg_forward_planned_bf16(const roc_sg_plan* plc, int H, const uint16_t* in, int64_t ldIn,
+                                           float* out, int64_t ldOut, int epilogue, roc_stream_t stream) {
+  roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  clear_launches();
+  if (!pl || H <= 0 || !in || !out || ldIn < H || ldOut < H || (ldIn % 8) || !aligned16(in)) return ROC_ERR_INVALID;
+  return run_planned<SG_RED_BSUM>(pl, H, in, ldIn, out, ldOut, nullptr, 0, epilogue, 0, as_stream(stream));
 }
 
 extern "C" int roc_sg_plan_rows_sorted(const roc_sg_plan* pl, int* sorted, roc_stream_t stream) {

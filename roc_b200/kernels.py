@@ -74,6 +74,16 @@ class SgPlan:
                                          _stream()), "roc_sg_forward_planned")
         return out
 
+    def forward_bf16(self, x, out=None, epilogue=0):
+        """roc_sg_forward_planned_bf16: forward() over bf16 rows (16-byte aligned, ld a multiple of 8, as bf16_padded
+        makes them), accumulated in fp32 into an fp32 `out`."""
+        assert x.dtype == torch.bfloat16
+        if out is None:
+            out = padded(self.nloc, x.shape[1], x.device)
+        check(lib.roc_sg_forward_planned_bf16(self.handle, x.shape[1], _ptr(x), _ld(x), _ptr(out), _ld(out),
+                                              int(epilogue), _stream()), "roc_sg_forward_planned_bf16")
+        return out
+
     def rows_sorted(self):
         """True if every row's sources are strictly increasing (no duplicate edges)."""
         ok = C.c_int()
@@ -361,23 +371,31 @@ def softmax_xent_bwd(logits, labels, mask, compact=False):
     return g, _perf_dict(perf)
 
 
-def linear_fwd(x, w, activation=0, norm_row_end=None, col_left=0, out=None):
-    """x [N][in] (ld-padded ok), w [out][in] contiguous (= W_mem[o*in + i]) -> [N][out]."""
-    assert w.is_contiguous()
+def _linear_out(x, w, out, y_bf16):
+    """The output of a forward Linear and its flags beyond the norm: fp32 rows padded to 4, or with y_bf16 bf16 rows
+    padded to 8 (ROC_LINEAR_Y_BF16)."""
     if out is None:
-        out = padded(x.shape[0], w.shape[0], x.device)
-    flags = _lib.LINEAR_NORM_EPILOGUE if norm_row_end is not None else 0
+        out = bf16_padded(x.shape[0], w.shape[0], x.device) if y_bf16 else padded(x.shape[0], w.shape[0], x.device)
+    assert (out.dtype == torch.bfloat16) == bool(y_bf16)
+    return out, (_lib.LINEAR_Y_BF16 if y_bf16 else 0)
+
+
+def linear_fwd(x, w, activation=0, norm_row_end=None, col_left=0, out=None, y_bf16=False):
+    """x [N][in] (ld-padded ok), w [out][in] contiguous (= W_mem[o*in + i]) -> [N][out]; with y_bf16 the result is
+    stored in bf16 (round to nearest even)."""
+    assert w.is_contiguous()
+    out, yflag = _linear_out(x, w, out, y_bf16)
+    flags = (_lib.LINEAR_NORM_EPILOGUE if norm_row_end is not None else 0) | yflag
     check(lib.roc_linear_fwd(x.shape[0], x.shape[1], w.shape[0], _ptr(x), _ld(x), _ptr(w), _ptr(out), _ld(out),
                              activation, flags, _ptr(norm_row_end), col_left, _stream()), "roc_linear_fwd")
     return out
 
 
-def linear_fwd_dropout(x, w, mask, rate, activation=0, norm_row_end=None, col_left=0, out=None):
+def linear_fwd_dropout(x, w, mask, rate, activation=0, norm_row_end=None, col_left=0, out=None, y_bf16=False):
     """linear_fwd(dropout(x)) with the dropout applied while loading x (mask from dropout_mask)."""
     assert w.is_contiguous()
-    if out is None:
-        out = padded(x.shape[0], w.shape[0], x.device)
-    flags = _lib.LINEAR_NORM_EPILOGUE if norm_row_end is not None else 0
+    out, yflag = _linear_out(x, w, out, y_bf16)
+    flags = (_lib.LINEAR_NORM_EPILOGUE if norm_row_end is not None else 0) | yflag
     check(lib.roc_linear_fwd_dropout(x.shape[0], x.shape[1], w.shape[0], _ptr(x), _ld(x), _ptr(w), _ptr(out),
                                      _ld(out), activation, flags, _ptr(norm_row_end), col_left, _ptr(mask),
                                      mask.stride(0) if mask is not None else 0, rate, _stream()),
@@ -421,12 +439,11 @@ def dropout_fwd_bf16(x, first_row, rate, seed, step, out=None):
     return out
 
 
-def linear_fwd_bf16(x, w, mask=None, rate=0.0, activation=0, norm_row_end=None, col_left=0, out=None):
+def linear_fwd_bf16(x, w, mask=None, rate=0.0, activation=0, norm_row_end=None, col_left=0, out=None, y_bf16=False):
     """roc_linear_fwd_bf16: linear_fwd_dropout with a bf16 x."""
     assert x.dtype == torch.bfloat16 and w.is_contiguous()
-    if out is None:
-        out = padded(x.shape[0], w.shape[0], x.device)
-    flags = _lib.LINEAR_NORM_EPILOGUE if norm_row_end is not None else 0
+    out, yflag = _linear_out(x, w, out, y_bf16)
+    flags = (_lib.LINEAR_NORM_EPILOGUE if norm_row_end is not None else 0) | yflag
     check(lib.roc_linear_fwd_bf16(x.shape[0], x.shape[1], w.shape[0], _ptr(x), _ld(x), _ptr(w), _ptr(out), _ld(out),
                                   activation, flags, _ptr(norm_row_end), col_left, _ptr(mask),
                                   mask.stride(0) if mask is not None else 0, rate, _stream()), "roc_linear_fwd_bf16")

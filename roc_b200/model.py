@@ -163,6 +163,13 @@ class Model:
         exact only on a symmetric graph).  Call before init().  One partition only."""
         check(lib.roc_host_set_exact_backward(self.h, int(bool(on))))
 
+    def set_bf16_aggregation(self, on=True):
+        """Store in bf16 each tensor that a Linear without activation writes (its output, or the indegree_norm fused
+        into it) and that one sum scatter_gather alone reads: the Linear rounds as it stores, the scatter_gather
+        gathers half-width rows and accumulates in fp32.  Gradients and every other tensor stay fp32; tensor_dtype()
+        shows which tensors init() chose.  Call before init().  One partition only."""
+        check(lib.roc_host_set_bf16_aggregation(self.h, int(bool(on))))
+
     def init(self):
         check(lib.roc_host_init(self.h))
 
@@ -184,11 +191,15 @@ class Model:
     def tensor_ptr(self, t, grad=False):
         return lib.roc_host_tensor_ptr(self.h, t, int(grad))
 
+    def tensor_dtype(self, t):
+        """How the tensor's data is stored: "float32", "bfloat16" or "int32" (gradients are always fp32)."""
+        return _lib.HOST_DTYPES[lib.roc_host_tensor_dtype(self.h, t)]
+
     def set_tensor(self, t, arr, grad=False):
         rows, hidden, _ = self.tensor_shape(t)
-        if t in self._bf16:
+        if t in self._bf16 or (not grad and self.tensor_dtype(t) == "bfloat16"):
             if grad:
-                raise _lib.RocError("set_tensor(grad=True): a bf16 tensor has no gradient")
+                raise _lib.RocError("set_tensor(grad=True): a bf16 leaf tensor has no gradient")
             if str(getattr(arr, "dtype", "")) == "torch.bfloat16":
                 import torch   # only a torch tensor can carry bf16 rows
                 bits = np.ascontiguousarray(arr.detach().contiguous().cpu().view(torch.int16).numpy())   # copied as is
@@ -205,11 +216,12 @@ class Model:
         check(lib.roc_host_set_tensor(self.h, t, C.c_void_p(ptr), int(grad)))
 
     def get_tensor(self, t, grad=False, dtype=np.float32, raw=False):
-        """the tensor's rows as fp32 (a bf16 tensor widened exactly); raw=True on a bf16 tensor: its bits (uint16)"""
+        """the tensor's rows as fp32 (a bf16 tensor widened exactly); raw=True on a bf16 tensor: its bits (uint16).
+        grad=True on a bf16 tensor an op produces (set_bf16_aggregation) gives its fp32 gradient."""
         rows, hidden, _ = self.tensor_shape(t)
-        if t in self._bf16:
+        if t in self._bf16 or (not grad and self.tensor_dtype(t) == "bfloat16"):
             if grad:
-                raise _lib.RocError("get_tensor(grad=True): a bf16 tensor has no gradient")
+                raise _lib.RocError("get_tensor(grad=True): a bf16 leaf tensor has no gradient")
             if raw:
                 out = np.empty((rows, hidden), dtype=np.uint16)
                 check(lib.roc_host_get_tensor_bf16(self.h, t, out.ctypes.data))
@@ -304,11 +316,22 @@ def _input_tensor(model, hidden, features):
     return model.create_node_tensor(hidden, dtype=features)
 
 
-def build_gcn(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exact_backward=False, features="float32"):
+def _aggregation(model, aggregation):
+    """aggregation="bfloat16": Model.set_bf16_aggregation; "float32" (the default) leaves the model as it is."""
+    if aggregation not in ("float32", "bfloat16"):
+        raise ValueError("aggregation must be \"float32\" or \"bfloat16\"")
+    if aggregation == "bfloat16":
+        model.set_bf16_aggregation(True)
+
+
+def build_gcn(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exact_backward=False, features="float32",
+              aggregation="float32"):
     """The model script of gnn.cc:65-98 for `-layers a-b-...-c`.  Returns the handles.  exact_backward: train on the
     exact gradient over the graph's transpose (Model.set_exact_backward), for directed graphs; the same keyword on
     build_sage_mean, build_sage_pool and build_gat.  features="bfloat16" keeps the input features in bf16
-    (Model.create_node_tensor); the same keyword on every builder."""
+    (Model.create_node_tensor); the same keyword on every builder.  aggregation="bfloat16" stores the fused
+    linear -> indegree_norm output each scatter_gather reads in bf16 (Model.set_bf16_aggregation); the same keyword
+    on build_sage_mean."""
     L = len(layers)
     x = _input_tensor(model, layers[0], features)
     label = model.create_node_tensor(layers[-1])
@@ -332,12 +355,13 @@ def build_gcn(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exact_bac
     model.adam(lr, weight_decay)
     if exact_backward:
         model.set_exact_backward(True)
+    _aggregation(model, aggregation)
     model.init()
     return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs}
 
 
 def build_sage_mean(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exact_backward=False,
-                    features="float32"):
+                    features="float32", aggregation="float32"):
     """GraphSAGE with the mean aggregator (BASELINE.json configs[2]) composed from the reference's own ops
     (gnn.h:165-179; AGGR_AVG is declared at gnn.h:75-80 but the reference's ScatterGather only sums):
 
@@ -348,7 +372,8 @@ def build_sage_mean(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exa
         t    = relu(t)                                                         # all but the last layer
 
     x / sqrt(deg) / sqrt(deg) is the mean to within one fp32 rounding.  Same wiring as the reference's residual
-    GCN layer (gnn.cc:79-90) with both norms after the aggregation."""
+    GCN layer (gnn.cc:79-90) with both norms after the aggregation.  aggregation="bfloat16" stores linear(D, d_i),
+    which only the scatter_gather reads, in bf16 (Model.set_bf16_aggregation)."""
     L = len(layers)
     x = _input_tensor(model, layers[0], features)
     label = model.create_node_tensor(layers[-1])
@@ -370,6 +395,7 @@ def build_sage_mean(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exa
     model.adam(lr, weight_decay)
     if exact_backward:
         model.set_exact_backward(True)
+    _aggregation(model, aggregation)
     model.init()
     return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs}
 

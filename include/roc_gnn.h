@@ -338,8 +338,8 @@ public:
   virtual void init(const Model& model);
   virtual void forward(const Model& model);
   virtual void backward(const Model& model);
-  int reluMaskOf;   /* backward: also apply the relu mask of this region's values (-1: none) */
-  int bwdIn;        /* region whose grad is read in backward (-1: own output) */
+  int reluOut;      /* a relu fused into the forward: its output region, whose grad the backward reads and whose
+                       values' mask it applies (-1: none; the backward reads its own output's grad) */
   bool bwdFused;    /* backward done in another op's epilogue (a Linear's dX or the softmax) */
 };
 
@@ -354,7 +354,6 @@ public:
   Tensor weight;
   int flags;        /* ROC_LINEAR_* (norm epilogue fused) */
   int fwdOut;       /* region the forward writes (-1: own output) */
-  int bwdIn;        /* region whose grad feeds backward (-1: own output) */
   int dropOp;       /* >= 0: layers[dropOp] is the Dropout feeding this op, applied while X is loaded */
   uint32_t* dropMask;      /* packed keep-mask of that dropout, [rows][dropLd] (roc_dropout_mask) */
   int64_t dropLd;

@@ -196,29 +196,18 @@ int roc_host_op_info(roc_host* h, int layer, struct roc_host_op_info* out) {
   struct roc_host_op_info r;
   memset(&r, 0, sizeof(r));
   r.fusedInto = op->fusedInto;
+  r.kind = op_kind(op);
   r.fwdOut = r.bwdOut = r.dropOp = r.dxOut = r.dxReluOf = r.gradOut = -1;
   if (const ScatterGather* sg = dynamic_cast<const ScatterGather*>(op)) {
-    r.kind = sg->aggr == AGGR_MAX ? ROC_HOST_OP_SCATTER_GATHER_MAX
-             : sg->aggr == AGGR_MIN ? ROC_HOST_OP_SCATTER_GATHER_MIN : ROC_HOST_OP_SCATTER_GATHER;
     r.epilogue = sg->epilogue; r.bwdEpilogue = sg->bwdEpilogue;
     r.fwdOut = handle(sg->fwdOut); r.bwdOut = handle(sg->bwdOut);
   } else if (const Linear* lin = dynamic_cast<const Linear*>(op)) {
-    r.kind = ROC_HOST_OP_LINEAR;
     r.flags = lin->flags; r.fwdOut = handle(lin->fwdOut); r.dropOp = lin->dropOp; r.dxOut = handle(lin->dxOut); r.dxReluOf = handle(lin->dxReluOf);
     r.dxNorm = lin->dxNorm ? 1 : 0;
   } else if (const InDegreeNorm* n = dynamic_cast<const InDegreeNorm*>(op)) {
-    r.kind = ROC_HOST_OP_INDEGREE_NORM;
     r.bwdFused = n->bwdFused ? 1 : 0;
   } else if (const SoftmaxCrossEntropy* s = dynamic_cast<const SoftmaxCrossEntropy*>(op)) {
-    r.kind = ROC_HOST_OP_SOFTMAX_CROSS_ENTROPY;
     r.gradOut = handle(s->gradOut);
-  } else if (const Activation* a = dynamic_cast<const Activation*>(op)) {
-    r.kind = a->actiMode == AC_MODE_RELU ? ROC_HOST_OP_RELU : ROC_HOST_OP_SIGMOID;
-  } else {
-    r.kind = dynamic_cast<const WeightedScatterGather*>(op) ? ROC_HOST_OP_SCATTER_GATHER_WEIGHTED
-             : dynamic_cast<const AttentionGather*>(op)     ? ROC_HOST_OP_ATTENTION_GATHER
-             : dynamic_cast<const Dropout*>(op)             ? ROC_HOST_OP_DROPOUT
-                                                            : ROC_HOST_OP_ADD;
   }
   *out = r;
   return 0;

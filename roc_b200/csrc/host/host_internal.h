@@ -8,6 +8,7 @@
 #include <vector>
 
 #include "roc_gnn.h"
+#include "roc_host.h"
 
 namespace roc {
 namespace host {
@@ -97,7 +98,7 @@ struct RuntimeImpl {
   void* linWs = nullptr; size_t linWsBytes = 0;           // split-K workspace of Linear backward
   void* staging = nullptr; size_t stagingBytes = 0;       // H2D staging for dense host rows -> padded rows
   float* flatGrad = nullptr; size_t flatGradCount = 0;    // all dW, one all-reduce
-  roc_sg_transpose* sgTranspose = nullptr;                // the graph's transpose, built by init() for weighted ops
+  roc_sg_transpose* sgTranspose = nullptr;                // the graph's transpose: exact backward, weighted ops
   roc_perf_metrics* d_perf = nullptr;
   roc_perf_metrics h_perf{};
   uint32_t trainStep = 0;
@@ -136,6 +137,10 @@ struct RuntimeImpl {
 
 inline int64_t round_up4(int64_t x) { return (x + 3) / 4 * 4; }
 inline int64_t round_up8(int64_t x) { return (x + 7) / 8 * 8; }
+
+// an op's ROC_HOST_OP_* kind (roc_host_op_info), and each kind's name in refusals and the per-op trace / profile
+int op_kind(const GnnOp* op);
+extern const char* const opKindNames[ROC_HOST_OP_SOFTMAX_CROSS_ENTROPY + 1];
 
 }  // namespace host
 }  // namespace roc

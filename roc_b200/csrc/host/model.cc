@@ -202,6 +202,25 @@ Tensor Model::sigmoid(const Tensor& _input) {
 void Model::train_mode(void) { mode = MD_MODE_TRAIN; }
 void Model::infer_mode(void) { mode = MD_MODE_INFER; }
 
+const char* const roc::host::opKindNames[ROC_HOST_OP_SOFTMAX_CROSS_ENTROPY + 1] = {
+    "linear", "indegree_norm", "scatter_gather", "scatter_gather(max)", "scatter_gather(min)",
+    "scatter_gather(weighted)", "attention_gather", "relu", "sigmoid", "add", "dropout", "softmax_cross_entropy"};
+int roc::host::op_kind(const GnnOp* op) {
+  if (const ScatterGather* sg = dynamic_cast<const ScatterGather*>(op))
+    return sg->aggr == AGGR_MAX   ? ROC_HOST_OP_SCATTER_GATHER_MAX
+           : sg->aggr == AGGR_MIN ? ROC_HOST_OP_SCATTER_GATHER_MIN
+                                  : ROC_HOST_OP_SCATTER_GATHER;
+  if (const Activation* a = dynamic_cast<const Activation*>(op))
+    return a->actiMode == AC_MODE_RELU ? ROC_HOST_OP_RELU : ROC_HOST_OP_SIGMOID;
+  return dynamic_cast<const Linear*>(op)                  ? ROC_HOST_OP_LINEAR
+         : dynamic_cast<const InDegreeNorm*>(op)          ? ROC_HOST_OP_INDEGREE_NORM
+         : dynamic_cast<const WeightedScatterGather*>(op) ? ROC_HOST_OP_SCATTER_GATHER_WEIGHTED
+         : dynamic_cast<const AttentionGather*>(op)       ? ROC_HOST_OP_ATTENTION_GATHER
+         : dynamic_cast<const Dropout*>(op)               ? ROC_HOST_OP_DROPOUT
+         : dynamic_cast<const SoftmaxCrossEntropy*>(op)   ? ROC_HOST_OP_SOFTMAX_CROSS_ENTROPY
+                                                          : ROC_HOST_OP_ADD;
+}
+
 namespace {
 struct Wiring {
   std::map<int, int> producer;    // region -> layer index
@@ -230,44 +249,28 @@ ScatterGather* as_sum_sg(GnnOp* op) {
 }
 }  // namespace
 
-// gnn.cc:625-673.  No graph loading / ResourceManager creation left to do here
-// (Graph's constructor already built the device CSR); what remains is sizing the
-// shared scratch, deciding which tensors need gradients, laying the dW replicas
-// out in one flat buffer and fusing the GCN aggregate block.
-bool Model::init(const Config& config) {
-  (void)config;
-  RuntimeImpl* rt = ctx;
-  if (bf16Aggregation && rt->numParts > 1)
+// ---- the passes of Model::init, in the order it runs them
+
+// a bf16 tensor is read by linear (its X) and dropout only; any other op would need an fp32 view of it
+static void check_bf16_readers(const Model& m) {
+  RuntimeImpl* rt = m.ctx;
+  if (m.bf16Aggregation && rt->numParts > 1)
     ROC_FATAL("set_bf16_aggregation: bf16 aggregation inputs run on one partition only (numParts > 1 is not supported)");
-  // a bf16 tensor is read by linear (its X) and dropout only; any other op would need an fp32 view of it
-  for (size_t l = 0; l < layers.size(); l++) {
-    GnnOp* op = layers[l];
+  for (GnnOp* op : m.layers) {
     const bool takesBf16 = as<Linear>(op) || as<Dropout>(op);
     for (int j = 0; j < op->numInputs; j++) {
       const int r = op->inputs[j].region;
       if (r < 0 || !rt->t(r).isBf16 || (takesBf16 && j == 0)) continue;
-      const ScatterGather* sgl = as<ScatterGather>(op);
-      const char* nm = sgl ? (sgl->aggr == AGGR_MAX ? "scatter_gather(max)" : sgl->aggr == AGGR_MIN ? "scatter_gather(min)"
-                                                                                                    : "scatter_gather") :
-                       as<AttentionGather>(op) ? "attention_gather" :
-                       as<WeightedScatterGather>(op) ? "scatter_gather(weighted)" :
-                       as<InDegreeNorm>(op) ? "indegree_norm" :
-                       as<Activation>(op) ? (as<Activation>(op)->actiMode == AC_MODE_RELU ? "relu" : "sigmoid") :
-                       as<Element>(op) ? "add" : as<SoftmaxCrossEntropy>(op) ? "softmax_cross_entropy" : "op";
-      ROC_FATAL((std::string(nm) + " cannot read a bf16 tensor: only linear and dropout take bf16 input").c_str());
+      ROC_FATAL((std::string(opKindNames[op_kind(op)]) +
+                 " cannot read a bf16 tensor: only linear and dropout take bf16 input").c_str());
     }
   }
-  myGraph.maxHidden = 0;
-  for (size_t i = 0; i < layers.size(); i++) {
-    for (int j = 0; j < layers[i]->numOutputs; j++)
-      myGraph.maxHidden = std::max(myGraph.maxHidden, (int)layers[i]->outputs[j].dims[0]);
-    for (int j = 0; j < layers[i]->numInputs; j++)
-      if (layers[i]->inputs[j].numDim == 2)
-        myGraph.maxHidden = std::max(myGraph.maxHidden, (int)layers[i]->inputs[j].dims[0]);
-  }
-  // which tensors carry gradients: anything downstream of a parameter
-  for (size_t l = 0; l < layers.size(); l++) {
-    GnnOp* op = layers[l];
+}
+
+// which tensors carry gradients: anything downstream of a parameter
+static void mark_gradients(const Model& m) {
+  RuntimeImpl* rt = m.ctx;
+  for (GnnOp* op : m.layers) {
     bool any = false;
     for (int j = 0; j < op->numInputs; j++)
       if (op->inputs[j].region >= 0) any = any || rt->t(op->inputs[j].region).requiresGrad;
@@ -277,8 +280,11 @@ bool Model::init(const Config& config) {
       rt->t(op->outputs[j].region).produced = true;
     }
   }
-  // flat dW buffer (one all-reduce per step instead of the reference's serial
-  // replica sum, optimizer_kernel.cu:88-94)
+}
+
+// flat dW buffer (one all-reduce per step instead of the reference's serial
+// replica sum, optimizer_kernel.cu:88-94)
+static void lay_out_flat_dw(RuntimeImpl* rt, const std::vector<Tensor>& parameters) {
   size_t total = 0;
   for (size_t p = 0; p < parameters.size(); p++) total += (size_t)parameters[p].dims[0] * parameters[p].dims[1];
   rt->flatGradCount = total;
@@ -289,41 +295,65 @@ bool Model::init(const Config& config) {
     rt->t(parameters[p].region).grad = rt->flatGrad + off;
     off += (size_t)parameters[p].dims[0] * parameters[p].dims[1];
   }
-  // scratch: Linear split-K workspace, SG carry slots, the gathered feature matrix
+}
+
+// scratch: Linear split-K workspace, SG carry slots, the gathered feature matrix.  Returns the widest ScatterGather
+// input, the width the graph's plan reserves its carries for (set_up_halo).
+static int size_scratch_and_plans(Model& m) {
+  RuntimeImpl* rt = m.ctx;
+  Graph& g = m.myGraph;
+  g.maxHidden = 0;
   size_t ws = 0;
   int maxSg = 0;
-  for (size_t l = 0; l < layers.size(); l++) {
-    if (Linear* lin = as<Linear>(layers[l]))
-      ws = std::max(ws, roc_linear_bwd_workspace_bytes(local_rows(), (int)lin->weight.dims[0], (int)lin->weight.dims[1]));
-    if (as<ScatterGather>(layers[l])) maxSg = std::max(maxSg, (int)layers[l]->inputs[0].dims[0]);
+  bool minmax = false;
+  for (GnnOp* op : m.layers) {
+    for (int j = 0; j < op->numOutputs; j++) g.maxHidden = std::max(g.maxHidden, (int)op->outputs[j].dims[0]);
+    for (int j = 0; j < op->numInputs; j++)
+      if (op->inputs[j].numDim == 2) g.maxHidden = std::max(g.maxHidden, (int)op->inputs[j].dims[0]);
+    if (Linear* lin = as<Linear>(op))
+      ws = std::max(ws, roc_linear_bwd_workspace_bytes(m.local_rows(), (int)lin->weight.dims[0], (int)lin->weight.dims[1]));
+    if (ScatterGather* sg = as<ScatterGather>(op)) {
+      maxSg = std::max(maxSg, (int)sg->inputs[0].dims[0]);
+      minmax = minmax || sg->aggr == AGGR_MAX || sg->aggr == AGGR_MIN;
+    }
   }
   rt->ensure_lin_ws(ws);
   // max / min aggregation sends each gradient to one source per (row, feature): a duplicate edge would receive it
   // twice.  Strictly increasing sources per row rule duplicates out.  The exact backward takes each distinct edge once
   // and needs no such rule.
-  for (size_t l = 0; l < layers.size() && !exactBackward; l++) {
-    ScatterGather* sg = as<ScatterGather>(layers[l]);
-    if (!sg || (sg->aggr != AGGR_MAX && sg->aggr != AGGR_MIN)) continue;
+  if (minmax && !m.exactBackward) {
     int sorted = 0;
-    ROC_CHECK(roc_sg_plan_rows_sorted(myGraph.plan, &sorted, rt->stream));
+    ROC_CHECK(roc_sg_plan_rows_sorted(g.plan, &sorted, rt->stream));
     if (!sorted) ROC_FATAL("scatter_gather(max / min): every row's sources must be strictly increasing (no duplicate edges)");
-    break;
   }
-  // the exact backward's transpose, built once and shared with the weighted ops, its plan's carries reserved for the
-  // widest aggregation it serves, as the forward plan's are
-  if (exactBackward) {
-    int maxT = 0;
-    for (size_t l = 0; l < layers.size(); l++)
-      if (as<ScatterGather>(layers[l]) || as<AttentionGather>(layers[l]))
-        maxT = std::max(maxT, (int)layers[l]->inputs[0].dims[0]);
-    if (maxT > 0) {
-      if (!rt->sgTranspose)
-        ROC_CHECK(roc_sg_transpose_create(myGraph.numNodes, myGraph.d_rowEnd, myGraph.d_colSrc, rt->stream, &rt->sgTranspose));
-      const roc_sg_plan* planT = nullptr;
-      ROC_CHECK(roc_sg_transpose_info(rt->sgTranspose, nullptr, nullptr, nullptr, &planT));
-      ROC_CHECK(roc_sg_plan_reserve(const_cast<roc_sg_plan*>(planT), maxT));
-    }
+  return maxSg;
+}
+
+// the graph's transpose, built once and shared by the exact backward and the weighted ops, its plan's carries reserved
+// for the widest aggregation the exact backward serves, as the forward plan's are
+static void build_transpose(const Model& m) {
+  RuntimeImpl* rt = m.ctx;
+  const Graph& g = m.myGraph;
+  int maxT = 0;
+  bool weighted = false;
+  for (GnnOp* op : m.layers) {
+    if (m.exactBackward && (as<ScatterGather>(op) || as<AttentionGather>(op)))
+      maxT = std::max(maxT, (int)op->inputs[0].dims[0]);
+    weighted = weighted || as<WeightedScatterGather>(op);
   }
+  if (maxT == 0 && !weighted) return;
+  if (!rt->sgTranspose)
+    ROC_CHECK(roc_sg_transpose_create(g.numNodes, g.d_rowEnd, g.d_colSrc, rt->stream, &rt->sgTranspose));
+  if (maxT > 0) {
+    const roc_sg_plan* planT = nullptr;
+    ROC_CHECK(roc_sg_transpose_info(rt->sgTranspose, nullptr, nullptr, nullptr, &planT));
+    ROC_CHECK(roc_sg_plan_reserve(const_cast<roc_sg_plan*>(planT), maxT));
+  }
+}
+
+// the plan's carries for the widest ScatterGather; with more than one partition, the gathered matrix, or the halo
+// slabs behind the tensors a ScatterGather reads and the way they are exchanged
+static void set_up_halo(RuntimeImpl* rt, const Graph& myGraph, const std::vector<GnnOp*>& layers, int maxSg) {
   if (maxSg > 0) {
     ROC_CHECK(roc_sg_plan_reserve(myGraph.plan, maxSg));
     if (rt->numParts > 1 && !myGraph.halo) rt->ensure_gather((size_t)myGraph.numNodes * (size_t)round_up4(maxSg));
@@ -365,131 +395,141 @@ bool Model::init(const Config& config) {
                                      : "roc_push_rows peer writes (CUDA IPC over NVLink), pipelined with the producer");
     }
   }
-  // ---- fusion of  linear -> indegree_norm -> scatter_gather -> indegree_norm -> relu  (gnn.cc:81-85)
-  if (fuse) {
-    Wiring w = wire(layers);
-    for (size_t l = 0; l < layers.size(); l++) {
-      ScatterGather* sg = as_sum_sg(layers[l]);
-      if (!sg) continue;
-      // upstream: Linear(NONE) -> InDegreeNorm -> SG, each feeding only the next
-      int rin = sg->inputs[0].region;
-      if (w.producer.count(rin) && w.consumers[rin] == 1) {
-        InDegreeNorm* n1 = as<InDegreeNorm>(layers[w.producer[rin]]);
-        if (n1 && n1->fusedInto < 0) {
-          int rl = n1->inputs[0].region;
-          if (w.producer.count(rl) && w.consumers[rl] == 1) {
-            Linear* lin = as<Linear>(layers[w.producer[rl]]);
-            if (lin && lin->activation == AC_MODE_NONE && lin->fwdOut < 0) {
-              lin->flags |= ROC_LINEAR_NORM_EPILOGUE;
-              lin->fwdOut = n1->outputs[0].region;       // linear writes the normalised rows
-              n1->fusedInto = w.producer[rl];
-              sg->bwdEpilogue = ROC_SG_EPI_NORM;          // SG backward writes d(linear out)
-              sg->bwdOut = lin->outputs[0].region;
-            }
-          }
-        }
-      }
-      // downstream: SG -> InDegreeNorm -> [relu]
-      int rout = sg->outputs[0].region;
-      if (w.consumers[rout] == 1) {
-        InDegreeNorm* n2 = as<InDegreeNorm>(layers[w.consumerOp[rout]]);
-        if (n2 && n2->fusedInto < 0) {
-          sg->epilogue = ROC_SG_EPI_NORM;
-          sg->fwdOut = n2->outputs[0].region;
-          n2->fusedInto = (int)l;   // forward only; its backward kernel still runs
-          int rn = n2->outputs[0].region;
-          if (w.consumers[rn] == 1) {
-            Activation* act = as<Activation>(layers[w.consumerOp[rn]]);
-            if (act && act->actiMode == AC_MODE_RELU && act->fusedInto < 0) {
-              sg->epilogue |= ROC_SG_EPI_RELU;
-              sg->fwdOut = act->outputs[0].region;
-              act->fusedInto = (int)l;
-              n2->reluMaskOf = act->outputs[0].region;   // backward: relu mask + norm in one pass
-              n2->bwdIn = act->outputs[0].region;
-            }
-          }
-        }
-      }
-    }
-  }
-  // ---- fusion of  dropout -> linear  (gnn.cc:79-81, 86-88): the dropout output feeds only the linear
-  if (fuse) {
-    Wiring w = wire(layers);
-    for (size_t l = 0; l < layers.size(); l++) {
-      Dropout* d = as<Dropout>(layers[l]);
-      if (!d || d->fusedInto >= 0) continue;
-      const int ro = d->outputs[0].region;
-      if (w.consumers[ro] != 1) continue;
-      Linear* lin = as<Linear>(layers[w.consumerOp[ro]]);
-      if (!lin || lin->dropOp >= 0 || lin->inputs[0].region != ro) continue;
-      lin->dropOp = (int)l;
-      d->fusedInto = w.consumerOp[ro];
-    }
-  }
-  // ---- backward-only fusions into epilogues
-  if (fuse) {
-    Wiring w = wire(layers);
-    for (size_t l = 0; l < layers.size(); l++) {
-      // (a) ... -> indegree_norm -> softmax_cross_entropy: the softmax kernel divides the logits'
-      //     gradient by sqrt(deg) and writes it where the norm's input gradient lives
-      if (SoftmaxCrossEntropy* sce = as<SoftmaxCrossEntropy>(layers[l])) {
-        const int rz = sce->inputs[0].region;
-        if (!w.producer.count(rz) || w.consumers[rz] != 1) continue;
-        InDegreeNorm* n = as<InDegreeNorm>(layers[w.producer[rz]]);
-        if (!n || n->bwdFused || n->reluMaskOf >= 0 || n->bwdIn >= 0) continue;
-        if (n->fusedInto >= 0 && as<Linear>(layers[(size_t)n->fusedInto])) continue;   // handled by the SG epilogue
-        if (!rt->t(n->inputs[0].region).requiresGrad) continue;
-        sce->gradOut = n->inputs[0].region;
-        n->bwdFused = true;
-        continue;
-      }
-      // (b) indegree_norm -> relu -> [dropout ->] linear: the linear's dX epilogue applies the dropout
-      //     backward, the relu mask and the norm, and writes the norm's input gradient directly
-      Linear* lin = as<Linear>(layers[l]);
-      if (!lin || lin->dxOut >= 0) continue;
-      const int rin = lin->dropOp >= 0 ? layers[(size_t)lin->dropOp]->inputs[0].region : lin->inputs[0].region;
-      if (!rt->t(rin).requiresGrad || !w.producer.count(rin) || w.consumers[rin] != 1) continue;
-      Activation* act = as<Activation>(layers[w.producer[rin]]);
-      if (!act || act->actiMode != AC_MODE_RELU || act->fusedInto < 0) continue;
-      const int rn = act->inputs[0].region;
-      if (!w.producer.count(rn)) continue;
-      InDegreeNorm* n = as<InDegreeNorm>(layers[w.producer[rn]]);
-      if (!n || n->bwdFused || n->reluMaskOf != rin || n->bwdIn != rin) continue;
-      lin->dxReluOf = rin;
-      lin->dxNorm = true;
-      lin->dxOut = n->inputs[0].region;
-      n->bwdFused = true;
-    }
-  }
-  // ---- bf16 aggregation inputs: what a Linear(NONE) writes (its output, or the fused norm's) and one sum
-  //      scatter_gather alone reads is stored in bf16, rows of round_up(H, 8) elements; its gradient twin keeps that ld
-  if (bf16Aggregation) {
-    Wiring w = wire(layers);
-    for (size_t l = 0; l < layers.size(); l++) {
-      Linear* lin = as<Linear>(layers[l]);
-      if (!lin || lin->activation != AC_MODE_NONE) continue;
-      const int r = lin->fwdOut >= 0 ? lin->fwdOut : lin->outputs[0].region;
-      if (w.consumers[r] != 1 || !as_sum_sg(layers[w.consumerOp[r]])) continue;
-      TensorImpl& x = rt->t(r);
-      if (x.data || x.grad) ROC_FATAL("set_bf16_aggregation: a tensor that becomes bf16 was already allocated");
-      x.isBf16 = true;
-      x.ld = round_up8(x.H);
-    }
-  }
-  for (size_t l = 0; l < layers.size(); l++) layers[l]->init(*this);
-  rt->opNames.clear();
+}
+
+// ---- fusion of  linear -> indegree_norm -> scatter_gather -> indegree_norm -> relu  (gnn.cc:81-85)
+static void fuse_gcn_block(const std::vector<GnnOp*>& layers, Wiring& w) {
   for (size_t l = 0; l < layers.size(); l++) {
-    const ScatterGather* sgl = as<ScatterGather>(layers[l]);
-    const char* nm = sgl ? (sgl->aggr == AGGR_MAX ? "scatter_gather(max)" : sgl->aggr == AGGR_MIN ? "scatter_gather(min)"
-                                                                                                  : "scatter_gather") :
-                     as<AttentionGather>(layers[l]) ? "attention_gather" :
-                     as<WeightedScatterGather>(layers[l]) ? "scatter_gather(weighted)" : as<Linear>(layers[l]) ? "linear" :
-                     as<InDegreeNorm>(layers[l]) ? "indegree_norm" : as<Activation>(layers[l]) ? "activation" :
-                     as<Dropout>(layers[l]) ? "dropout" : as<Element>(layers[l]) ? "add" :
-                     as<SoftmaxCrossEntropy>(layers[l]) ? "softmax_cross_entropy" : "op";
-    rt->opNames.push_back(std::string(nm) + (layers[l]->fusedInto >= 0 ? " (fused)" : ""));
+    ScatterGather* sg = as_sum_sg(layers[l]);
+    if (!sg) continue;
+    // upstream: Linear(NONE) -> InDegreeNorm -> SG, each feeding only the next
+    int rin = sg->inputs[0].region;
+    if (w.producer.count(rin) && w.consumers[rin] == 1) {
+      InDegreeNorm* n1 = as<InDegreeNorm>(layers[w.producer[rin]]);
+      if (n1 && n1->fusedInto < 0) {
+        int rl = n1->inputs[0].region;
+        if (w.producer.count(rl) && w.consumers[rl] == 1) {
+          Linear* lin = as<Linear>(layers[w.producer[rl]]);
+          if (lin && lin->activation == AC_MODE_NONE && lin->fwdOut < 0) {
+            lin->flags |= ROC_LINEAR_NORM_EPILOGUE;
+            lin->fwdOut = n1->outputs[0].region;       // linear writes the normalised rows
+            n1->fusedInto = w.producer[rl];
+            sg->bwdEpilogue = ROC_SG_EPI_NORM;          // SG backward writes d(linear out)
+            sg->bwdOut = lin->outputs[0].region;
+          }
+        }
+      }
+    }
+    // downstream: SG -> InDegreeNorm -> [relu]
+    int rout = sg->outputs[0].region;
+    if (w.consumers[rout] == 1) {
+      InDegreeNorm* n2 = as<InDegreeNorm>(layers[w.consumerOp[rout]]);
+      if (n2 && n2->fusedInto < 0) {
+        sg->epilogue = ROC_SG_EPI_NORM;
+        sg->fwdOut = n2->outputs[0].region;
+        n2->fusedInto = (int)l;   // forward only; its backward kernel still runs
+        int rn = n2->outputs[0].region;
+        if (w.consumers[rn] == 1) {
+          Activation* act = as<Activation>(layers[w.consumerOp[rn]]);
+          if (act && act->actiMode == AC_MODE_RELU && act->fusedInto < 0) {
+            sg->epilogue |= ROC_SG_EPI_RELU;
+            sg->fwdOut = act->outputs[0].region;
+            act->fusedInto = (int)l;
+            n2->reluOut = act->outputs[0].region;   // backward: relu mask + norm in one pass
+          }
+        }
+      }
+    }
   }
-  ROC_CHECK(cudaStreamSynchronize(rt->stream));
+}
+
+// ---- fusion of  dropout -> linear  (gnn.cc:79-81, 86-88): the dropout output feeds only the linear
+static void fuse_dropout_into_linear(const std::vector<GnnOp*>& layers, Wiring& w) {
+  for (size_t l = 0; l < layers.size(); l++) {
+    Dropout* d = as<Dropout>(layers[l]);
+    if (!d || d->fusedInto >= 0) continue;
+    const int ro = d->outputs[0].region;
+    if (w.consumers[ro] != 1) continue;
+    Linear* lin = as<Linear>(layers[w.consumerOp[ro]]);
+    if (!lin || lin->dropOp >= 0 || lin->inputs[0].region != ro) continue;
+    lin->dropOp = (int)l;
+    d->fusedInto = w.consumerOp[ro];
+  }
+}
+
+// ---- backward-only fusions into epilogues
+static void fuse_backward_epilogues(RuntimeImpl* rt, const std::vector<GnnOp*>& layers, Wiring& w) {
+  for (size_t l = 0; l < layers.size(); l++) {
+    // (a) ... -> indegree_norm -> softmax_cross_entropy: the softmax kernel divides the logits'
+    //     gradient by sqrt(deg) and writes it where the norm's input gradient lives
+    if (SoftmaxCrossEntropy* sce = as<SoftmaxCrossEntropy>(layers[l])) {
+      const int rz = sce->inputs[0].region;
+      if (!w.producer.count(rz) || w.consumers[rz] != 1) continue;
+      InDegreeNorm* n = as<InDegreeNorm>(layers[w.producer[rz]]);
+      if (!n || n->bwdFused || n->reluOut >= 0) continue;
+      if (n->fusedInto >= 0 && as<Linear>(layers[(size_t)n->fusedInto])) continue;   // handled by the SG epilogue
+      if (!rt->t(n->inputs[0].region).requiresGrad) continue;
+      sce->gradOut = n->inputs[0].region;
+      n->bwdFused = true;
+      continue;
+    }
+    // (b) indegree_norm -> relu -> [dropout ->] linear: the linear's dX epilogue applies the dropout
+    //     backward, the relu mask and the norm, and writes the norm's input gradient directly
+    Linear* lin = as<Linear>(layers[l]);
+    if (!lin || lin->dxOut >= 0) continue;
+    const int rin = lin->dropOp >= 0 ? layers[(size_t)lin->dropOp]->inputs[0].region : lin->inputs[0].region;
+    if (!rt->t(rin).requiresGrad || !w.producer.count(rin) || w.consumers[rin] != 1) continue;
+    Activation* act = as<Activation>(layers[w.producer[rin]]);
+    if (!act || act->actiMode != AC_MODE_RELU || act->fusedInto < 0) continue;
+    const int rn = act->inputs[0].region;
+    if (!w.producer.count(rn)) continue;
+    InDegreeNorm* n = as<InDegreeNorm>(layers[w.producer[rn]]);
+    if (!n || n->bwdFused || n->reluOut != rin) continue;
+    lin->dxReluOf = rin;
+    lin->dxNorm = true;
+    lin->dxOut = n->inputs[0].region;
+    n->bwdFused = true;
+  }
+}
+
+// ---- bf16 aggregation inputs: what a Linear(NONE) writes (its output, or the fused norm's) and one sum
+//      scatter_gather alone reads is stored in bf16, rows of round_up(H, 8) elements; its gradient twin keeps that ld
+static void choose_bf16_aggregation(RuntimeImpl* rt, const std::vector<GnnOp*>& layers, Wiring& w) {
+  for (size_t l = 0; l < layers.size(); l++) {
+    Linear* lin = as<Linear>(layers[l]);
+    if (!lin || lin->activation != AC_MODE_NONE) continue;
+    const int r = lin->fwdOut >= 0 ? lin->fwdOut : lin->outputs[0].region;
+    if (w.consumers[r] != 1 || !as_sum_sg(layers[w.consumerOp[r]])) continue;
+    TensorImpl& x = rt->t(r);
+    if (x.data || x.grad) ROC_FATAL("set_bf16_aggregation: a tensor that becomes bf16 was already allocated");
+    x.isBf16 = true;
+    x.ld = round_up8(x.H);
+  }
+}
+
+// gnn.cc:625-673.  No graph loading / ResourceManager creation left to do here
+// (Graph's constructor already built the device CSR); what remains are the passes
+// above, in an order each later one relies on (a fusion sees the earlier ones'
+// decisions, op_info reports them all).
+bool Model::init(const Config&) {
+  check_bf16_readers(*this);
+  mark_gradients(*this);
+  lay_out_flat_dw(ctx, parameters);
+  const int maxSg = size_scratch_and_plans(*this);
+  build_transpose(*this);
+  set_up_halo(ctx, myGraph, layers, maxSg);
+  Wiring w = wire(layers);   // the passes below change no op's inputs or outputs
+  if (fuse) {
+    fuse_gcn_block(layers, w);
+    fuse_dropout_into_linear(layers, w);
+    fuse_backward_epilogues(ctx, layers, w);
+  }
+  if (bf16Aggregation) choose_bf16_aggregation(ctx, layers, w);
+  for (size_t l = 0; l < layers.size(); l++) layers[l]->init(*this);
+  ctx->opNames.clear();
+  for (size_t l = 0; l < layers.size(); l++)
+    ctx->opNames.push_back(std::string(opKindNames[op_kind(layers[l])]) + (layers[l]->fusedInto >= 0 ? " (fused)" : ""));
+  ROC_CHECK(cudaStreamSynchronize(ctx->stream));
   return true;
 }
 
@@ -543,21 +583,34 @@ void Model::zero_gradients(void) {
     ROC_CHECK(cudaMemsetAsync(rt->flatGrad, 0, rt->flatGradCount * sizeof(float), rt->stream));
 }
 
+// Dense fp32 host rows <-> x's rows through the staging buffer, ~256 MB of floats at a time, so no full-size fp32 copy
+// is ever resident.  Each chunk of rows [r0, r0 + nr) goes from `in` into staging before convert(r0, nr), or from
+// staging to `out` after it (waited for: the next chunk reuses the buffer); one of `in` / `out` is null.
+template <typename Convert>
+static void staged_rows(RuntimeImpl* rt, const TensorImpl& x, const float* in, float* out, Convert convert) {
+  const int64_t chunkRows = std::max<int64_t>(1, (int64_t)(64u << 20) / x.H);
+  rt->ensure_staging((size_t)std::min<int64_t>(chunkRows, x.rows) * x.H * sizeof(float));
+  for (int64_t r0 = 0; r0 < x.rows; r0 += chunkRows) {
+    const int64_t nr = std::min<int64_t>(chunkRows, x.rows - r0);
+    if (in) ROC_CHECK(cudaMemcpyAsync(rt->staging, in + r0 * x.H, (size_t)nr * x.H * 4, cudaMemcpyHostToDevice, rt->stream));
+    convert(r0, nr);
+    if (out) {
+      ROC_CHECK(cudaMemcpyAsync(out + r0 * x.H, rt->staging, (size_t)nr * x.H * 4, cudaMemcpyDeviceToHost, rt->stream));
+      ROC_CHECK(cudaStreamSynchronize(rt->stream));
+    }
+  }
+}
+
 void Model::set_tensor(const Tensor& t, const void* host, bool grad) {
   RuntimeImpl* rt = ctx;
   TensorImpl& x = rt->t(t.region);
   if (x.isBf16 && !(grad && x.produced)) {
-    // fp32 host rows, rounded on the device chunk by chunk: no full-size fp32 copy is ever resident
+    // fp32 host rows, rounded on the device chunk by chunk
     if (grad) ROC_FATAL("set_tensor(grad=true): a bf16 leaf tensor has no gradient");
     uint16_t* dst = rt->data_bf16(t.region);
-    const int64_t chunkRows = std::max<int64_t>(1, (int64_t)(64u << 20) / x.H);
-    rt->ensure_staging((size_t)std::min<int64_t>(chunkRows, x.rows) * x.H * sizeof(float));
-    const float* h = static_cast<const float*>(host);
-    for (int64_t r0 = 0; r0 < x.rows; r0 += chunkRows) {
-      const int64_t nr = std::min<int64_t>(chunkRows, x.rows - r0);
-      ROC_CHECK(cudaMemcpyAsync(rt->staging, h + r0 * x.H, (size_t)nr * x.H * 4, cudaMemcpyHostToDevice, rt->stream));
+    staged_rows(rt, x, static_cast<const float*>(host), nullptr, [&](int64_t r0, int64_t nr) {
       ROC_CHECK(roc_f32_to_bf16(nr, x.H, (const float*)rt->staging, x.H, dst + r0 * x.ld, x.ld, rt->stream));
-    }
+    });
     ROC_CHECK(cudaStreamSynchronize(rt->stream));
     return;
   }
@@ -568,14 +621,9 @@ void Model::set_tensor(const Tensor& t, const void* host, bool grad) {
     // Dense host rows -> padded device rows.  A strided cudaMemcpy2D of 2.4 KB rows runs at
     // ~17 GB/s; contiguous chunks into a staging buffer run at PCIe speed and the re-pitch
     // is a device copy at HBM speed.
-    const int64_t chunkRows = std::max<int64_t>(1, (int64_t)(64u << 20) / x.H);   // ~256 MB of floats
-    rt->ensure_staging((size_t)std::min<int64_t>(chunkRows, x.rows) * x.H * sizeof(float));
-    const float* h = static_cast<const float*>(host);
-    for (int64_t r0 = 0; r0 < x.rows; r0 += chunkRows) {
-      const int64_t nr = std::min<int64_t>(chunkRows, x.rows - r0);
-      ROC_CHECK(cudaMemcpyAsync(rt->staging, h + r0 * x.H, (size_t)nr * x.H * 4, cudaMemcpyHostToDevice, rt->stream));
+    staged_rows(rt, x, static_cast<const float*>(host), nullptr, [&](int64_t r0, int64_t nr) {
       ROC_CHECK(roc_copy2d(nr, x.H, (const float*)rt->staging, x.H, dst + r0 * x.ld, x.ld, rt->stream));
-    }
+    });
   }
   ROC_CHECK(cudaStreamSynchronize(rt->stream));
 }
@@ -587,15 +635,9 @@ void Model::get_tensor(const Tensor& t, void* host, bool grad) const {
     // widened exactly on the device into staging, chunk by chunk
     if (grad) ROC_FATAL("get_tensor(grad=true): a bf16 leaf tensor has no gradient");
     const uint16_t* src = rt->data_bf16(t.region);
-    const int64_t chunkRows = std::max<int64_t>(1, (int64_t)(64u << 20) / x.H);
-    rt->ensure_staging((size_t)std::min<int64_t>(chunkRows, x.rows) * x.H * sizeof(float));
-    float* h = static_cast<float*>(host);
-    for (int64_t r0 = 0; r0 < x.rows; r0 += chunkRows) {
-      const int64_t nr = std::min<int64_t>(chunkRows, x.rows - r0);
+    staged_rows(rt, x, nullptr, static_cast<float*>(host), [&](int64_t r0, int64_t nr) {
       ROC_CHECK(roc_bf16_to_f32(nr, x.H, src + r0 * x.ld, x.ld, (float*)rt->staging, x.H, rt->stream));
-      ROC_CHECK(cudaMemcpyAsync(h + r0 * x.H, rt->staging, (size_t)nr * x.H * 4, cudaMemcpyDeviceToHost, rt->stream));
-      ROC_CHECK(cudaStreamSynchronize(rt->stream));   // the next chunk reuses the staging buffer
-    }
+    });
     return;
   }
   const float* src = grad ? rt->grad(t.region) : rt->data(t.region);
@@ -881,21 +923,18 @@ void ScatterGather::forward(const Model& model) {
     return;
   }
   const int outRegion = fwdOut >= 0 ? fwdOut : outputs[0].region;
+  const bool xBf16 = rt->t(inputs[0].region).isBf16;   // set_bf16_aggregation: one partition, nothing to exchange
   rt->sg_begin(-H);          // negative width = the exposed part of the halo exchange (profile mode only)
-  if (rt->t(inputs[0].region).isBf16) {   // set_bf16_aggregation: one partition, nothing to exchange
-    rt->sg_end();
-    float* dst = rt->data(outRegion);
-    rt->sg_begin(H);
-    ROC_CHECK(roc_sg_forward_planned_bf16(model.myGraph.plan, H, rt->data_bf16(inputs[0].region), ldIn, dst,
-                                          rt->t(outRegion).ld, epilogue, rt->stream));
-    rt->sg_end();
-    return;
-  }
-  const float* src = gathered(model, rt->data(inputs[0].region), ldIn, H, &rt->t(inputs[0].region), false);
+  const float* src =
+      xBf16 ? nullptr : gathered(model, rt->data(inputs[0].region), ldIn, H, &rt->t(inputs[0].region), false);
   rt->sg_end();
   float* dst = rt->data(outRegion);
   rt->sg_begin(H);
-  ROC_CHECK(roc_sg_forward_planned(model.myGraph.plan, H, src, ldIn, dst, rt->t(outRegion).ld, epilogue, rt->stream));
+  if (xBf16)
+    ROC_CHECK(roc_sg_forward_planned_bf16(model.myGraph.plan, H, rt->data_bf16(inputs[0].region), ldIn, dst,
+                                          rt->t(outRegion).ld, epilogue, rt->stream));
+  else
+    ROC_CHECK(roc_sg_forward_planned(model.myGraph.plan, H, src, ldIn, dst, rt->t(outRegion).ld, epilogue, rt->stream));
   rt->sg_end();
 }
 
@@ -933,6 +972,22 @@ void ScatterGather::backward(const Model& model) {
   else
     ROC_CHECK(roc_sg_forward_planned(model.myGraph.plan, H, src, ld, dst, rt->t(dstRegion).ld, bwdEpilogue, rt->stream));
   rt->sg_end();
+}
+
+// An op whose kernel overwrites an input gradient writes it into the gradient itself when `direct`, else into
+// `scratch` (allocated on first use), which add_scratch then adds to the gradient another op already wrote.
+static float* grad_or_scratch(const Model& model, int region, bool direct, float*& scratch) {
+  RuntimeImpl* rt = model.ctx;
+  if (direct) return rt->grad(region);
+  if (!scratch)
+    scratch = (float*)rt->dmalloc((size_t)std::max<int64_t>(model.local_rows(), 1) * (size_t)rt->t(region).ld * sizeof(float));
+  return scratch;
+}
+static void add_scratch(const Model& model, int region, const float* scratch) {
+  RuntimeImpl* rt = model.ctx;
+  const TensorImpl& x = rt->t(region);
+  float* g = rt->grad(region);
+  ROC_CHECK(roc_add_fwd(model.local_rows(), x.H, g, x.ld, scratch, x.ld, g, x.ld, rt->stream));
 }
 
 // ------------------------------------------------------- AttentionGather -----
@@ -980,12 +1035,8 @@ void AttentionGather::backward(const Model& model) {
   // The kernel overwrites both gradients.  An input whose gradient another op already wrote (the features feed the
   // score Linear too) gets its part in scratch, added afterwards; so does one that needs no gradient.
   float* dst[2];
-  for (int i = 0; i < 2; i++) {
-    const TensorImpl& x = rt->t(inputs[i].region);
-    if (x.requiresGrad && resetInputGrads[i]) { dst[i] = rt->grad(inputs[i].region); continue; }
-    if (!scratch[i]) scratch[i] = (float*)rt->dmalloc((size_t)std::max<int64_t>(model.local_rows(), 1) * (size_t)x.ld * sizeof(float));
-    dst[i] = scratch[i];
-  }
+  for (int i = 0; i < 2; i++)
+    dst[i] = grad_or_scratch(model, inputs[i].region, rt->t(inputs[i].region).requiresGrad && resetInputGrads[i], scratch[i]);
   const int ox = outputs[0].region;
   rt->sg_begin(H);
   if (model.exactBackward)
@@ -1001,12 +1052,8 @@ void AttentionGather::backward(const Model& model) {
                                            rt->t(ox).ld, stats, statsLd, rt->grad(ox), rt->t(ox).ld, dst[0],
                                            rt->t(inputs[0].region).ld, dst[1], rt->t(inputs[1].region).ld, rt->stream));
   rt->sg_end();
-  for (int i = 0; i < 2; i++) {
-    const TensorImpl& x = rt->t(inputs[i].region);
-    if (!x.requiresGrad || resetInputGrads[i]) continue;
-    float* g = rt->grad(inputs[i].region);
-    ROC_CHECK(roc_add_fwd(model.local_rows(), x.H, g, x.ld, scratch[i], x.ld, g, x.ld, rt->stream));
-  }
+  for (int i = 0; i < 2; i++)
+    if (rt->t(inputs[i].region).requiresGrad && !resetInputGrads[i]) add_scratch(model, inputs[i].region, scratch[i]);
 }
 
 // ------------------------------------------------- WeightedScatterGather -----
@@ -1019,13 +1066,7 @@ WeightedScatterGather::WeightedScatterGather(const Model& model, const Tensor& _
   numOutputs = 1;
   outputs[0] = model.create_node_tensor<DATATYPE>((int)_input.dims[0]);
 }
-// The first weighted op's init builds the graph's transpose (one synchronisation), which every weighted op shares.
-void WeightedScatterGather::init(const Model& model) {
-  RuntimeImpl* rt = model.ctx;
-  if (rt->sgTranspose) return;
-  const Graph& g = model.myGraph;
-  ROC_CHECK(roc_sg_transpose_create(g.numNodes, g.d_rowEnd, g.d_colSrc, rt->stream, &rt->sgTranspose));
-}
+void WeightedScatterGather::init(const Model&) {}
 
 void WeightedScatterGather::forward(const Model& model) {
   RuntimeImpl* rt = model.ctx;
@@ -1051,14 +1092,9 @@ void WeightedScatterGather::backward(const Model& model) {
   const int64_t ldY = rt->t(y).ld, ldX = rt->t(x).ld;
   rt->sg_begin(H);
   if (wantX) {
-    float* dst = rt->grad(x);
-    if (!resetInputGrads[0]) {
-      if (!scratch) scratch = (float*)rt->dmalloc((size_t)std::max<int64_t>(model.local_rows(), 1) * (size_t)ldX * sizeof(float));
-      dst = scratch;
-    }
+    float* dst = grad_or_scratch(model, x, resetInputGrads[0], scratch);
     ROC_CHECK(roc_sg_weighted_backward_planned(rt->sgTranspose, H, rt->grad(y), ldY, rt->data(e), dst, ldX, rt->stream));
-    if (!resetInputGrads[0])
-      ROC_CHECK(roc_add_fwd(model.local_rows(), H, rt->grad(x), ldX, scratch, ldX, rt->grad(x), ldX, rt->stream));
+    if (!resetInputGrads[0]) add_scratch(model, x, scratch);
   }
   if (wantE)
     ROC_CHECK(roc_sg_edge_dot_planned(model.myGraph.plan, H, rt->grad(y), ldY, rt->data(x), ldX, rt->grad(e),
@@ -1068,7 +1104,7 @@ void WeightedScatterGather::backward(const Model& model) {
 
 // --------------------------------------------------------- InDegreeNorm -----
 InDegreeNorm::InDegreeNorm(const Model& model, const Tensor& _input)
-    : GnnOp(_input), reluMaskOf(-1), bwdIn(-1), bwdFused(false) {
+    : GnnOp(_input), reluOut(-1), bwdFused(false) {
   ROC_ASSERT(inputs[0].type == Tensor::NODE_TENSOR);   // graphnorm.cc:33-35
   ROC_ASSERT(inputs[0].numDim == 2);
   ROC_ASSERT(inputs[0].dims[1] == model.myGraph.numNodes);
@@ -1095,15 +1131,15 @@ void InDegreeNorm::backward(const Model& model) {
   if (fusedInto >= 0 && dynamic_cast<Linear*>(model.layers[(size_t)fusedInto])) return;
   if (bwdFused) return;   // a Linear's dX epilogue / the softmax already wrote this gradient
   const Graph& g = model.myGraph;
-  const int src = bwdIn >= 0 ? bwdIn : outputs[0].region;
+  const int src = reluOut >= 0 ? reluOut : outputs[0].region;
   ROC_CHECK(roc_indegree_norm(g.rowLeft, g.rowRight, g.colLeft, (int)inputs[0].dims[0], g.d_rowEnd, rt->grad(src),
                               rt->t(src).ld, rt->grad(inputs[0].region), rt->t(inputs[0].region).ld,
-                              reluMaskOf >= 0 ? rt->data(reluMaskOf) : NULL, rt->stream));
+                              reluOut >= 0 ? rt->data(reluOut) : NULL, rt->stream));
 }
 
 // ----------------------------------------------------------------- Linear ---
 Linear::Linear(const Model& model, const Tensor& _input, int outDim, ActiMode _activation, Initializer* initializer)
-    : GnnOp(_input), activation(_activation), flags(0), fwdOut(-1), bwdIn(-1), dropOp(-1), dropMask(nullptr), dropLd(0),
+    : GnnOp(_input), activation(_activation), flags(0), fwdOut(-1), dropOp(-1), dropMask(nullptr), dropLd(0),
       dxReluOf(-1), dxNorm(false), dxOut(-1) {
   ROC_ASSERT(_input.numDim == 2);   // linear.cc:41-42
   ROC_ASSERT(_input.dims[1] == model.myGraph.numNodes);
@@ -1119,16 +1155,10 @@ void Linear::init(const Model& model) {
 }
 
 namespace {
-// the Dropout folded into a Linear: its rate in the current mode and its Philox key
-struct FusedDrop { const Dropout* op; float rate; uint64_t key; int inRegion; };
-FusedDrop fused_drop(const Model& model, int dropOp) {
-  const Dropout* d = static_cast<const Dropout*>(model.layers[(size_t)dropOp]);
-  FusedDrop f;
-  f.op = d;
-  f.rate = (model.mode == MD_MODE_TRAIN) ? d->rate : 0.0f;    // infer: dropout is a copy (dropout_kernel.cu:159-180)
-  f.key = ((uint64_t)(uint32_t)d->seed << 32) | (uint32_t)d->opIndex;
-  f.inRegion = d->inputs[0].region;
-  return f;
+// a Dropout's rate in the current mode (infer: dropout is a copy, dropout_kernel.cu:159-180) and its Philox key
+struct DropDraw { float rate; uint64_t key; };
+DropDraw drop_draw(const Model& model, const Dropout& d) {
+  return {model.mode == MD_MODE_TRAIN ? d.rate : 0.0f, ((uint64_t)(uint32_t)d.seed << 32) | (uint32_t)d.opIndex};
 }
 }  // namespace
 
@@ -1148,52 +1178,33 @@ void Linear::forward(const Model& model) {
     return yBf16 ? reinterpret_cast<float*>(rt->data_bf16(outRegion) + r0 * ldY) : Y + r0 * ldY;
   };
   const int flags = this->flags | (yBf16 ? ROC_LINEAR_Y_BF16 : 0);
+  int xRegion = inputs[0].region;
+  float rate = 0.0f;
   if (dropOp >= 0) {
     // dropout -> linear: the mask is generated packed (1 bit / element) and applied while the GEMM
     // loads X, so the dropped copy of X is never materialised
-    const FusedDrop f = fused_drop(model, dropOp);
+    const Dropout* d = static_cast<const Dropout*>(model.layers[(size_t)dropOp]);
+    const DropDraw f = drop_draw(model, *d);
     if (f.rate > 0.0f)
       ROC_CHECK(roc_dropout_mask(model.local_rows(), inDim, g.rowLeft, f.rate, f.key, rt->trainStep,
                                  dropMask, dropLd, rt->stream));
-    const int64_t ldX = rt->t(f.inRegion).ld;
-    if (rt->t(f.inRegion).isBf16) {
-      const uint16_t* Xb = rt->data_bf16(f.inRegion);
-      for (size_t k = 0; k < pipe.blocks(); k++) {
-        const int64_t r0 = pipe.row0(k), nr = pipe.rows(k, model.local_rows());
-        ROC_CHECK(roc_linear_fwd_bf16(nr, inDim, outDim, Xb + r0 * ldX, ldX, rt->data(weight.region), yRow(r0), ldY,
-                                      (int)activation, flags, g.d_rowEnd + r0, pipe.colLeft(k),
-                                      f.rate > 0.0f ? dropMask + r0 * dropLd : NULL, dropLd, f.rate, rt->stream));
-        pipe.pushed(k, Y, ldY, outDim);
-      }
-      return;
-    }
-    const float* X = rt->data(f.inRegion);
-    for (size_t k = 0; k < pipe.blocks(); k++) {
-      const int64_t r0 = pipe.row0(k), nr = pipe.rows(k, model.local_rows());
-      ROC_CHECK(roc_linear_fwd_dropout(nr, inDim, outDim, X + r0 * ldX, ldX, rt->data(weight.region), yRow(r0), ldY,
-                                       (int)activation, flags, g.d_rowEnd + r0, pipe.colLeft(k), dropMask + r0 * dropLd,
-                                       dropLd, f.rate, rt->stream));
-      pipe.pushed(k, Y, ldY, outDim);
-    }
-    return;
+    xRegion = d->inputs[0].region;
+    rate = f.rate;
   }
-  const int64_t ldX = rt->t(inputs[0].region).ld;
-  if (rt->t(inputs[0].region).isBf16) {   // a bf16 leaf X, read directly by the GEMM
-    const uint16_t* Xb = rt->data_bf16(inputs[0].region);
-    for (size_t k = 0; k < pipe.blocks(); k++) {
-      const int64_t r0 = pipe.row0(k), nr = pipe.rows(k, model.local_rows());
-      ROC_CHECK(roc_linear_fwd_bf16(nr, inDim, outDim, Xb + r0 * ldX, ldX, rt->data(weight.region), yRow(r0), ldY,
-                                    (int)activation, flags, g.d_rowEnd + r0, pipe.colLeft(k), NULL, 0, 0.0f,
-                                    rt->stream));
-      pipe.pushed(k, Y, ldY, outDim);
-    }
-    return;
-  }
-  const float* X = rt->data(inputs[0].region);
+  const int64_t ldX = rt->t(xRegion).ld;
+  // a bf16 X (a leaf) is read directly by the GEMM
+  const bool xBf16 = rt->t(xRegion).isBf16;
   for (size_t k = 0; k < pipe.blocks(); k++) {
     const int64_t r0 = pipe.row0(k), nr = pipe.rows(k, model.local_rows());
-    ROC_CHECK(roc_linear_fwd(nr, inDim, outDim, X + r0 * ldX, ldX, rt->data(weight.region), yRow(r0), ldY,
-                             (int)activation, flags, g.d_rowEnd + r0, pipe.colLeft(k), rt->stream));
+    const uint32_t* mask = rate > 0.0f ? dropMask + r0 * dropLd : NULL;
+    if (xBf16)
+      ROC_CHECK(roc_linear_fwd_bf16(nr, inDim, outDim, rt->data_bf16(xRegion) + r0 * ldX, ldX, rt->data(weight.region),
+                                    yRow(r0), ldY, (int)activation, flags, g.d_rowEnd + r0, pipe.colLeft(k), mask,
+                                    dropLd, rate, rt->stream));
+    else
+      ROC_CHECK(roc_linear_fwd_dropout(nr, inDim, outDim, rt->data(xRegion) + r0 * ldX, ldX, rt->data(weight.region),
+                                       yRow(r0), ldY, (int)activation, flags, g.d_rowEnd + r0, pipe.colLeft(k), mask,
+                                       dropLd, rate, rt->stream));
     pipe.pushed(k, Y, ldY, outDim);
   }
 }
@@ -1201,7 +1212,6 @@ void Linear::forward(const Model& model) {
 void Linear::backward(const Model& model) {
   RuntimeImpl* rt = model.ctx;
   const Graph& g = model.myGraph;
-  const int gy = bwdIn >= 0 ? bwdIn : outputs[0].region;
   roc_linear_bwd_args a;
   memset(&a, 0, sizeof(a));
   int xRegion = inputs[0].region;
@@ -1209,34 +1219,33 @@ void Linear::backward(const Model& model) {
   if (dropOp >= 0) {
     // dW from the masked X; dX lands directly in the gradient of the dropout's input (the dropout
     // backward, dropout_kernel.cu:149-150, runs in the dX epilogue; it always overwrites, :119)
-    const FusedDrop f = fused_drop(model, dropOp);
+    const Dropout* d = static_cast<const Dropout*>(model.layers[(size_t)dropOp]);
     ROC_ASSERT(resetInputGrads[0]);
-    xRegion = f.inRegion;
+    xRegion = d->inputs[0].region;
     a.accumulate_dX = 0;
-    a.dropMask = dropMask; a.ldMask = dropLd; a.dropRate = f.rate;
+    a.dropMask = dropMask; a.ldMask = dropLd; a.dropRate = drop_draw(model, *d).rate;
   }
-  if (rt->t(xRegion).isBf16) {
-    // a bf16 X is a leaf: dW only (with the relu backward of dY when activation is RELU); the same bits as the fp32
-    // path on the widened X
-    ROC_ASSERT(!rt->t(xRegion).requiresGrad);
-    const int yr = outputs[0].region;
-    ROC_CHECK(roc_linear_dw_bf16(model.local_rows(), (int)weight.dims[0], (int)weight.dims[1], rt->data_bf16(xRegion),
-                                 rt->t(xRegion).ld, activation != AC_MODE_NONE ? rt->data(yr) : NULL, rt->t(yr).ld,
-                                 rt->grad(gy), rt->t(gy).ld, rt->grad(weight.region), (int)activation, rt->linWs,
-                                 rt->linWsBytes, a.dropMask, a.ldMask, a.dropRate, rt->stream));
-    return;
-  }
+  // a bf16 X is a leaf: dW only (with the relu backward of dY when activation is RELU); the same bits as the fp32
+  // path on the widened X
+  const bool xBf16 = rt->t(xRegion).isBf16;
+  if (xBf16) ROC_ASSERT(!rt->t(xRegion).requiresGrad);
   const int dxRegion = dxOut >= 0 ? dxOut : xRegion;
   a.rows = model.local_rows(); a.inDim = (int)weight.dims[0]; a.outDim = (int)weight.dims[1];
-  a.X = rt->data(xRegion); a.ldX = rt->t(xRegion).ld;
+  a.X = xBf16 ? NULL : rt->data(xRegion); a.ldX = rt->t(xRegion).ld;
   a.W = rt->data(weight.region);
   a.Y = (activation != AC_MODE_NONE) ? rt->data(outputs[0].region) : NULL; a.ldY = rt->t(outputs[0].region).ld;
-  a.dY = rt->grad(gy); a.ldDY = rt->t(gy).ld;
+  a.dY = rt->grad(outputs[0].region); a.ldDY = rt->t(outputs[0].region).ld;
   a.dW = rt->grad(weight.region);
   a.dX = rt->t(xRegion).requiresGrad ? rt->grad(dxRegion) : NULL;   // Q8: leaf grads skipped
   a.ldDX = rt->t(dxRegion).ld;
   a.activation = (int)activation;
   a.workspace = rt->linWs; a.workspaceBytes = rt->linWsBytes;
+  if (xBf16) {
+    ROC_CHECK(roc_linear_dw_bf16(a.rows, a.inDim, a.outDim, rt->data_bf16(xRegion), a.ldX, a.Y, a.ldY, a.dY, a.ldDY,
+                                 a.dW, a.activation, a.workspace, a.workspaceBytes, a.dropMask, a.ldMask, a.dropRate,
+                                 rt->stream));
+    return;
+  }
   if (a.dX && dxReluOf >= 0) { a.dxReluOf = rt->data(dxReluOf); a.ldReluOf = rt->t(dxReluOf).ld; }
   if (a.dX && dxNorm) { a.dxNormRowEnd = g.d_rowEnd; a.colLeft = g.colLeft; }
   // dX feeds a ScatterGather backward on other GPUs (peer-mapped slabs): dX in row blocks, each pushed while the
@@ -1258,8 +1267,6 @@ void Linear::backward(const Model& model) {
       pipe.pushed(k, a.dX, a.ldDX, a.inDim);
     }
     a.parts = ROC_LINEAR_BWD_ONLY_DW;
-    ROC_CHECK(roc_linear_bwd_fused(&a, rt->stream));
-    return;
   }
   ROC_CHECK(roc_linear_bwd_fused(&a, rt->stream));
 }
@@ -1328,28 +1335,26 @@ void Dropout::forward(const Model& model) {
   if (fusedInto >= 0) return;   // applied by the consuming Linear while it loads X
   RuntimeImpl* rt = model.ctx;
   // train: masked scale (dropout_kernel.cu:98-99); infer: plain copy (:159-180)
-  const float r = (model.mode == MD_MODE_TRAIN) ? rate : 0.0f;
-  const uint64_t key = ((uint64_t)(uint32_t)seed << 32) | (uint32_t)opIndex;
+  const DropDraw d = drop_draw(model, *this);
   if (rt->t(inputs[0].region).isBf16) {   // bf16 in, fp32 out; rate 0 is the widening copy
-    ROC_CHECK(roc_dropout_fwd_bf16(model.local_rows(), (int)inputs[0].dims[0], model.myGraph.rowLeft, r, key,
+    ROC_CHECK(roc_dropout_fwd_bf16(model.local_rows(), (int)inputs[0].dims[0], model.myGraph.rowLeft, d.rate, d.key,
                                    rt->trainStep, rt->data_bf16(inputs[0].region), rt->t(inputs[0].region).ld,
                                    rt->data(outputs[0].region), rt->t(outputs[0].region).ld, rt->stream));
     return;
   }
-  ROC_CHECK(roc_dropout_fwd(model.local_rows(), (int)inputs[0].dims[0], model.myGraph.rowLeft, r, key, rt->trainStep,
-                            rt->data(inputs[0].region), rt->t(inputs[0].region).ld, rt->data(outputs[0].region),
-                            rt->t(outputs[0].region).ld, rt->stream));
+  ROC_CHECK(roc_dropout_fwd(model.local_rows(), (int)inputs[0].dims[0], model.myGraph.rowLeft, d.rate, d.key,
+                            rt->trainStep, rt->data(inputs[0].region), rt->t(inputs[0].region).ld,
+                            rt->data(outputs[0].region), rt->t(outputs[0].region).ld, rt->stream));
 }
 void Dropout::backward(const Model& model) {
   RuntimeImpl* rt = model.ctx;
   if (!rt->t(inputs[0].region).requiresGrad) return;   // leaf input (Q8)
   ROC_ASSERT(resetInputGrads[0]);   // dropout_kernel.cu:119
   if (fusedInto >= 0) return;       // the consuming Linear's dX epilogue already wrote this gradient
-  const float r = (model.mode == MD_MODE_TRAIN) ? rate : 0.0f;
-  const uint64_t key = ((uint64_t)(uint32_t)seed << 32) | (uint32_t)opIndex;
-  ROC_CHECK(roc_dropout_bwd(model.local_rows(), (int)inputs[0].dims[0], model.myGraph.rowLeft, r, key, rt->trainStep,
-                            rt->grad(outputs[0].region), rt->t(outputs[0].region).ld, rt->grad(inputs[0].region),
-                            rt->t(inputs[0].region).ld, rt->stream));
+  const DropDraw d = drop_draw(model, *this);
+  ROC_CHECK(roc_dropout_bwd(model.local_rows(), (int)inputs[0].dims[0], model.myGraph.rowLeft, d.rate, d.key,
+                            rt->trainStep, rt->grad(outputs[0].region), rt->t(outputs[0].region).ld,
+                            rt->grad(inputs[0].region), rt->t(inputs[0].region).ld, rt->stream));
 }
 
 // ---------------------------------------------------- SoftmaxCrossEntropy ---

@@ -163,6 +163,14 @@ int roc_sg_forward_planned_bf16(const roc_sg_plan* plan, int H, const uint16_t* 
  * ROC_ERR_INVALID for an aggr other than MAX / MIN, a NULL pointer or a leading dimension < H. */
 int roc_sg_minmax_forward_planned(const roc_sg_plan* plan, int aggr, int H, const float* in, int64_t ldIn,
                                   float* out, int64_t ldOut, roc_vid_t* arg, int64_t ldArg, roc_stream_t stream);
+/* roc_sg_minmax_forward_planned over bf16 rows (raw bits, see roc_f32_to_bf16), each value widened exactly in
+ * registers: the same fp32 out and the same arg. `in` is 16-byte aligned and ldIn (in elements) is a multiple of 8,
+ * else ROC_ERR_INVALID. The result is bit-identical to roc_sg_minmax_forward_planned on roc_bf16_to_f32(in) written
+ * to a 16-byte aligned buffer with a leading dimension that is a multiple of 4: the plan, the row shapes, the column
+ * blocks, the per-float order, the carries and the fix-ups are that call's. Its main launches report reduction 17
+ * (max) or 18 (min) in roc_sg_last_call_info. */
+int roc_sg_minmax_forward_planned_bf16(const roc_sg_plan* plan, int aggr, int H, const uint16_t* in, int64_t ldIn,
+                                       float* out, int64_t ldOut, roc_vid_t* arg, int64_t ldArg, roc_stream_t stream);
 /* Its backward, as a gather over the same CSR (like the sum's, quirk Q1), in the plan's fixed order, no atomics:
  *   inGrad[u][h] = sum_{e in row u, v = colSrc[e]} (arg[v][h] == selfBase + u ? outGrad[v][h] : 0)
  * outGrad and arg are indexed by colSrc's ids; selfBase + u is local row u's id in that space (0 for a whole graph,
@@ -205,6 +213,23 @@ int roc_sg_attn_backward_planned(const roc_sg_plan* plan, int heads, int H, floa
                                  int64_t ldOut, const float* stats, int64_t ldStats, const float* outGrad,
                                  int64_t ldG, float* inGrad, int64_t ldInG, float* scoreGrad, int64_t ldSG,
                                  roc_stream_t stream);
+/* The attention forward and its backward over bf16 feature rows X = in (raw bits, see roc_f32_to_bf16), each value
+ * widened exactly in registers; score, stats, out, outGrad and every output stay fp32. The forward gathers X[j] at
+ * half width (its stats pass reads only the scores); the backward gathers X[j] in its d s_dst pass and reads X[i],
+ * the row's own row, in its input-gradient pass. `in` is 16-byte aligned and ldIn (in elements) is a multiple of 8,
+ * else ROC_ERR_INVALID. The result is bit-identical to the fp32 call on roc_bf16_to_f32(in) written to a 16-byte
+ * aligned buffer with a leading dimension that is a multiple of 4: the plan, the row shapes, the column blocks, the
+ * per-float order, the carries and the fix-ups are that call's. Their main launches report reduction 21 (the
+ * forward's weighted sum), 22 (d s_dst) and 23 (the input gradient) in roc_sg_last_call_info; the stats pass, the
+ * record and the fix-ups are the fp32 call's and report as there. */
+int roc_sg_attn_forward_planned_bf16(const roc_sg_plan* plan, int heads, int H, float slope, roc_vid_t selfBase,
+                                     const uint16_t* in, int64_t ldIn, const float* score, int64_t ldS, float* out,
+                                     int64_t ldOut, float* stats, int64_t ldStats, roc_stream_t stream);
+int roc_sg_attn_backward_planned_bf16(const roc_sg_plan* plan, int heads, int H, float slope, roc_vid_t selfBase,
+                                      const uint16_t* in, int64_t ldIn, const float* score, int64_t ldS,
+                                      const float* out, int64_t ldOut, const float* stats, int64_t ldStats,
+                                      const float* outGrad, int64_t ldG, float* inGrad, int64_t ldInG,
+                                      float* scoreGrad, int64_t ldSG, roc_stream_t stream);
 
 /* Edge-weighted aggregation (GCN with edge weights, weighted graphs, edge saliency).  The reference declares edge
  * tensors (gnn.h:178) but never reads them; these semantics are this library's own.  For plan row r with id
@@ -217,6 +242,14 @@ int roc_sg_attn_backward_planned(const roc_sg_plan* plan, int heads, int H, floa
  * indexed like roc_sg_forward_planned's.  ROC_ERR_INVALID: a NULL pointer or a leading dimension < H. */
 int roc_sg_weighted_forward_planned(const roc_sg_plan* plan, int H, const float* in, int64_t ldIn, const float* w,
                                     float* out, int64_t ldOut, roc_stream_t stream);
+/* roc_sg_weighted_forward_planned over bf16 rows (raw bits, see roc_f32_to_bf16), each value widened exactly in
+ * registers and accumulated in fp32. `in` is 16-byte aligned and ldIn (in elements) is a multiple of 8, else
+ * ROC_ERR_INVALID. The result is bit-identical to roc_sg_weighted_forward_planned on roc_bf16_to_f32(in) written to a
+ * 16-byte aligned buffer with a leading dimension that is a multiple of 4: the plan, the row shapes, the column
+ * blocks, the per-float order, the carries and the fix-ups are that call's. Its main launches report reduction 24 in
+ * roc_sg_last_call_info. */
+int roc_sg_weighted_forward_planned_bf16(const roc_sg_plan* plan, int H, const uint16_t* in, int64_t ldIn,
+                                         const float* w, float* out, int64_t ldOut, roc_stream_t stream);
 /* The gradient of the edge weights (an SDDMM): for every edge e of the plan, with G = outGrad indexed by plan row
  * and X = in indexed like the forward's input,
  *   dw[e - colLeft] = sum_h G[r][h] * X[j][h]          (accumulate != 0: added to the value dw holds)
@@ -224,6 +257,14 @@ int roc_sg_weighted_forward_planned(const roc_sg_plan* plan, int H, const float*
  * so the same call gives the same bits.  ROC_ERR_INVALID: a NULL pointer or a leading dimension < H. */
 int roc_sg_edge_dot_planned(const roc_sg_plan* plan, int H, const float* outGrad, int64_t ldG, const float* in,
                             int64_t ldIn, float* dw, int accumulate, roc_stream_t stream);
+/* roc_sg_edge_dot_planned with X = in in bf16 (raw bits, see roc_f32_to_bf16), each value widened exactly in
+ * registers; G and dw stay fp32. `in` is 16-byte aligned and ldIn (in elements) is a multiple of 8, else
+ * ROC_ERR_INVALID. The result is bit-identical to roc_sg_edge_dot_planned on roc_bf16_to_f32(in) written to a 16-byte
+ * aligned buffer with a leading dimension that is a multiple of 4: the plan, the row shapes, the column blocks, the
+ * per-float order, the carries and the fix-ups are that call's. Its launches report reduction 25 in
+ * roc_sg_last_call_info. */
+int roc_sg_edge_dot_planned_bf16(const roc_sg_plan* plan, int H, const float* outGrad, int64_t ldG,
+                                 const uint16_t* in, int64_t ldIn, float* dw, int accumulate, roc_stream_t stream);
 /* The transpose of a whole graph's CSR (rows 0..numNodes-1, edges 0..rowEnd[numNodes-1], every id < numNodes), for
  * the exact input gradient of the weighted aggregation on any graph (directed, asymmetric weights, duplicate edges):
  *   rowEndT  u64[numNodes]  END offsets of node v's out-edges
@@ -282,6 +323,14 @@ int roc_sg_attn_backward_exact(const roc_sg_plan* plan, roc_sg_transpose* transp
                                const float* in, int64_t ldIn, const float* score, int64_t ldS, const float* out,
                                int64_t ldOut, const float* stats, int64_t ldStats, const float* outGrad, int64_t ldG,
                                float* inGrad, int64_t ldInG, float* scoreGrad, int64_t ldSG, roc_stream_t stream);
+/* roc_sg_attn_backward_exact over bf16 feature rows X = in, as roc_sg_attn_backward_planned_bf16 is to
+ * roc_sg_attn_backward_planned: bit-identical to roc_sg_attn_backward_exact on the widened rows, under the same input
+ * rules, with its main launches reporting 22 and 23. */
+int roc_sg_attn_backward_exact_bf16(const roc_sg_plan* plan, roc_sg_transpose* transpose, int heads, int H,
+                                    float slope, const uint16_t* in, int64_t ldIn, const float* score, int64_t ldS,
+                                    const float* out, int64_t ldOut, const float* stats, int64_t ldStats,
+                                    const float* outGrad, int64_t ldG, float* inGrad, int64_t ldInG, float* scoreGrad,
+                                    int64_t ldSG, roc_stream_t stream);
 
 /* Plan-less form with exactly the reference kernel's argument list
  * (scattergather_kernel.cu:21-28, EdgeStruct.dst dropped), dense ld == H.
@@ -308,8 +357,10 @@ int roc_sg_backward(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft, in
  *          stats, 5 the attention forward, 6 its d s_dst gather, 7 its input-gradient gather, 8 the weighted sum
  *          (forward and backward), 9 the edge-weight gradient, 10 the exact sum backward with NORM (the sum whose
  *          epilogue divides by the original graph's in-degree; its main kernel, ring and fix-ups), 11 the exact max /
- *          min backward, 12 the sum over bf16 rows (its main kernel and ring); -1 for the record and the
- *          permutation, which have none.  A sum fix-up finishing another
+ *          min backward, 12 the sum over bf16 rows (its main kernel and ring); 16 + r for the main kernel of
+ *          reduction r over bf16 feature rows (17 max, 18 min, 21 attention forward, 22 d s_dst, 23 input gradient,
+ *          24 weighted sum, 25 edge-weight gradient: the roc_sg_*_bf16 calls), whose fix-ups are reduction r's and
+ *          report as there; -1 for the record and the permutation, which have none.  A sum fix-up finishing another
  *          reduction's partials reports 0.
  *   vec    4 for float4 rows, else 1;  lanes, nch: the row shape (L lanes, chunks per lane);  grid: CTAs launched
  * count is the number of launches; the first ROC_SG_MAX_LAUNCHES are stored.  Every planned call clears the list first,
@@ -414,6 +465,15 @@ int roc_activation_fwd(int64_t rows, int H, int mode, const float* x, int64_t ld
 int roc_activation_bwd(int64_t rows, int H, int mode, const float* y, int64_t ldY,
                        const float* dY, int64_t ldDY, float* dX, int64_t ldDX,
                        int accumulate, roc_stream_t stream);
+/* ROC_AC_MODE_RELU with a bf16 output (raw bits, see roc_f32_to_bf16): fwd stores exactly roc_f32_to_bf16 of what
+ * roc_activation_fwd stores, in columns [0, H) (the rest of each row is never written); bwd is roc_activation_bwd on
+ * the widened y, so its mask is the stored bf16 value's.  That mask differs from the fp32 value's in one case only: a
+ * positive fp32 value no larger than 2^-134 (half of bf16's smallest subnormal) rounds to +0 and masks its gradient.
+ * Any other mode is ROC_ERR_UNSUPPORTED. */
+int roc_activation_fwd_y_bf16(int64_t rows, int H, int mode, const float* x, int64_t ldX, uint16_t* y, int64_t ldY,
+                              roc_stream_t stream);
+int roc_activation_bwd_y_bf16(int64_t rows, int H, int mode, const uint16_t* y, int64_t ldY, const float* dY,
+                              int64_t ldDY, float* dX, int64_t ldDX, int accumulate, roc_stream_t stream);
 
 /* Replaces op_kernel (EW_TYPE_ADD), element_kernel.cu:19-39, and its backward
  * add_kernel pair, :93-101. */

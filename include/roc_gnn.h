@@ -251,12 +251,16 @@ public:
    * only on a symmetric graph).  init() then builds the transpose once, shared with the weighted ops, and max / min
    * accept graphs with duplicate edges.  Call it before init().  Single partition only (exit(1) otherwise). */
   void set_exact_backward(bool on);
-  /* Opt-in bf16 aggregation inputs (off by default).  At init(), after fusion, each tensor that a Linear with
-   * AC_MODE_NONE writes in its forward (its own output, or the output of an indegree_norm fused into its epilogue) and
-   * that one sum scatter_gather alone reads is stored in bf16: the Linear rounds its fp32 result to nearest even as it
-   * stores it, and the scatter_gather gathers the rows at half width and accumulates them in fp32.  The gradient of
-   * such a tensor is an ordinary fp32 tensor; every other tensor stays fp32.  Call it before init().  Single partition
-   * only (init() exits otherwise). */
+  /* Opt-in bf16 aggregation inputs (off by default).  At init(), after fusion, a tensor is stored in bf16 when
+   *  - a Linear with AC_MODE_NONE writes it in its forward (its own output, or the output of an indegree_norm fused
+   *    into its epilogue) and one sum scatter_gather alone reads it; or
+   *  - a Linear with AC_MODE_NONE or an unfused relu writes it, at least one max / min scatter_gather, weighted
+   *    scatter_gather or attention_gather reads it as its feature input, and every other reader is one of those or a
+   *    Linear reading it as X with no fused dropout (GAT's score Linear).
+   * Its producer rounds the fp32 result to nearest even as it stores it (a relu's gradient then takes its mask from the
+   * stored bf16 value), the aggregations read the rows at half width and compute in fp32, and a Linear reads them as a
+   * bf16 X.  The gradient of such a tensor is an ordinary fp32 tensor; every other tensor stays fp32.  Call it before
+   * init().  Single partition only (init() exits otherwise). */
   void set_bf16_aggregation(bool on);
   /* the source ids a max / min scatter_gather chose (its `arg`), [rows_local][H] u32; `out` is its output tensor */
   void get_aggr_index(const Tensor& out, uint32_t* host) const;

@@ -20,6 +20,7 @@ SG_NOARG = 0xFFFFFFFF                                      # arg of a row with n
 LINEAR_NORM_EPILOGUE = 1
 LINEAR_Y_BF16 = 2                                          # Y holds bf16 bits
 SG_RED_BSUM = 12                                           # roc_sg_launch.red of the sum over bf16 rows
+SG_RED_BF16 = 16                                           # + r: roc_sg_launch.red of reduction r's bf16 form
 HOST_DTYPES = ("float32", "bfloat16", "int32")             # ROC_HOST_DTYPE_* by value
 LINEAR_BWD_ONLY_DX, LINEAR_BWD_ONLY_DW = 1, 2
 GEMM_FWD, GEMM_DW, GEMM_DX = 0, 1, 2                       # `which` of roc_last_gemm_path / roc_last_gemm_info
@@ -126,12 +127,18 @@ PROTOTYPES = {
     "roc_sg_forward_planned": (i32, [vp, i32, vp, i64, vp, i64, i32, vp]),
     "roc_sg_forward_planned_bf16": (i32, [vp, i32, vp, i64, vp, i64, i32, vp]),
     "roc_sg_minmax_forward_planned": (i32, [vp, i32, i32, vp, i64, vp, i64, vp, i64, vp]),
+    "roc_sg_minmax_forward_planned_bf16": (i32, [vp, i32, i32, vp, i64, vp, i64, vp, i64, vp]),
     "roc_sg_minmax_backward_planned": (i32, [vp, i32, u32, vp, i64, vp, i64, vp, i64, vp]),
     "roc_sg_attn_forward_planned": (i32, [vp, i32, i32, f32, u32, vp, i64, vp, i64, vp, i64, vp, i64, vp]),
+    "roc_sg_attn_forward_planned_bf16": (i32, [vp, i32, i32, f32, u32, vp, i64, vp, i64, vp, i64, vp, i64, vp]),
     "roc_sg_attn_backward_planned": (i32, [vp, i32, i32, f32, u32, vp, i64, vp, i64, vp, i64, vp, i64, vp, i64, vp,
                                            i64, vp, i64, vp]),
+    "roc_sg_attn_backward_planned_bf16": (i32, [vp, i32, i32, f32, u32, vp, i64, vp, i64, vp, i64, vp, i64, vp, i64,
+                                                vp, i64, vp, i64, vp]),
     "roc_sg_weighted_forward_planned": (i32, [vp, i32, vp, i64, vp, vp, i64, vp]),
     "roc_sg_edge_dot_planned": (i32, [vp, i32, vp, i64, vp, i64, vp, i32, vp]),
+    "roc_sg_weighted_forward_planned_bf16": (i32, [vp, i32, vp, i64, vp, vp, i64, vp]),
+    "roc_sg_edge_dot_planned_bf16": (i32, [vp, i32, vp, i64, vp, i64, vp, i32, vp]),
     "roc_sg_transpose_create": (i32, [u32, vp, vp, vp, C.POINTER(vp)]),
     "roc_sg_transpose_info": (i32, [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]),
     "roc_sg_transpose_destroy": (None, [vp]),
@@ -140,6 +147,8 @@ PROTOTYPES = {
     "roc_sg_transpose_minmax_backward": (i32, [vp, i32, vp, i64, vp, i64, vp, i64, vp]),
     "roc_sg_attn_backward_exact": (i32, [vp, vp, i32, i32, f32, vp, i64, vp, i64, vp, i64, vp, i64, vp, i64, vp, i64,
                                          vp, i64, vp]),
+    "roc_sg_attn_backward_exact_bf16": (i32, [vp, vp, i32, i32, f32, vp, i64, vp, i64, vp, i64, vp, i64, vp, i64, vp,
+                                              i64, vp, i64, vp]),
     "roc_sg_forward": (i32, [u32, u32, u64, i32, vp, vp, vp, vp, vp]),
     "roc_sg_backward": (i32, [u32, u32, u64, i32, vp, vp, vp, vp, vp]),
     "roc_sg_last_call_info": (i32, [C.POINTER(SgCallInfo)]),
@@ -156,6 +165,8 @@ PROTOTYPES = {
     "roc_indegree_norm": (i32, [u32, u32, u64, i32, vp, vp, i64, vp, i64, vp, vp]),
     "roc_activation_fwd": (i32, [i64, i32, i32, vp, i64, vp, i64, vp]),
     "roc_activation_bwd": (i32, [i64, i32, i32, vp, i64, vp, i64, vp, i64, i32, vp]),
+    "roc_activation_fwd_y_bf16": (i32, [i64, i32, i32, vp, i64, vp, i64, vp]),
+    "roc_activation_bwd_y_bf16": (i32, [i64, i32, i32, vp, i64, vp, i64, vp, i64, i32, vp]),
     "roc_add_fwd": (i32, [i64, i32, vp, i64, vp, i64, vp, i64, vp]),
     "roc_add_bwd": (i32, [i64, i32, vp, i64, vp, i64, i32, vp, i64, i32, vp]),
     "roc_dropout_fwd": (i32, [i64, i32, i64, f32, u64, u32, vp, i64, vp, i64, vp]),

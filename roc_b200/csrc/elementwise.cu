@@ -864,3 +864,53 @@ extern "C" int roc_bf16_to_f32(int64_t rows, int H, const uint16_t* src, int64_t
   ROC_LAUNCH_CHECK();
   return ROC_OK;
 }
+
+// relu with its output y stored in bf16 (the value the model keeps), and its backward with the mask read from that y.
+// Columns [H, ldY) of y are never written.
+__global__ void __launch_bounds__(EW_T)
+k_relu_fwd_y_bf16(int64_t rows, int H, const float* __restrict__ x, int64_t ldX, uint16_t* __restrict__ y,
+                  int64_t ldY) {
+  const int64_t total = rows * (int64_t)H;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = i / H;
+    const int c = (int)(i - r * H);
+    y[r * ldY + c] = f32_to_bf16_rne(relu_nanprop(x[r * ldX + c]));
+  }
+}
+
+template <bool ACC>
+__global__ void __launch_bounds__(EW_T)
+k_relu_bwd_y_bf16(int64_t rows, int H, const uint16_t* __restrict__ y, int64_t ldY, const float* __restrict__ dy,
+                  int64_t ldDY, float* __restrict__ dx, int64_t ldDX) {
+  const int64_t total = rows * (int64_t)H;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = i / H;
+    const int c = (int)(i - r * H);
+    const float g = (to_f32(y[r * ldY + c]) > 0.f) ? dy[r * ldDY + c] : 0.f;
+    dx[r * ldDX + c] = ACC ? dx[r * ldDX + c] + g : g;
+  }
+}
+
+extern "C" int roc_activation_fwd_y_bf16(int64_t rows, int H, int mode, const float* x, int64_t ldX, uint16_t* y,
+                                         int64_t ldY, roc_stream_t stream) {
+  if (!x || !y || rows < 0 || H <= 0 || ldX < H || ldY < H) return ROC_ERR_INVALID;
+  if (mode != ROC_AC_MODE_RELU) return ROC_ERR_UNSUPPORTED;
+  if (rows == 0) return ROC_OK;
+  k_relu_fwd_y_bf16<<<ew_grid(rows * H, EW_T), EW_T, 0, as_stream(stream)>>>(rows, H, x, ldX, y, ldY);
+  ROC_LAUNCH_CHECK();
+  return ROC_OK;
+}
+
+extern "C" int roc_activation_bwd_y_bf16(int64_t rows, int H, int mode, const uint16_t* y, int64_t ldY,
+                                         const float* dY, int64_t ldDY, float* dX, int64_t ldDX, int accumulate,
+                                         roc_stream_t stream) {
+  if (!y || !dY || !dX || rows < 0 || H <= 0 || ldY < H || ldDY < H || ldDX < H) return ROC_ERR_INVALID;
+  if (mode != ROC_AC_MODE_RELU) return ROC_ERR_UNSUPPORTED;
+  if (rows == 0) return ROC_OK;
+  cudaStream_t st = as_stream(stream);
+  const unsigned grid = ew_grid(rows * H, EW_T);
+  if (accumulate) k_relu_bwd_y_bf16<true><<<grid, EW_T, 0, st>>>(rows, H, y, ldY, dY, ldDY, dX, ldDX);
+  else k_relu_bwd_y_bf16<false><<<grid, EW_T, 0, st>>>(rows, H, y, ldY, dY, ldDY, dX, ldDX);
+  ROC_LAUNCH_CHECK();
+  return ROC_OK;
+}

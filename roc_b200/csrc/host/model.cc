@@ -494,16 +494,41 @@ static void fuse_backward_epilogues(RuntimeImpl* rt, const std::vector<GnnOp*>& 
 
 // ---- bf16 aggregation inputs: what a Linear(NONE) writes (its output, or the fused norm's) and one sum
 //      scatter_gather alone reads is stored in bf16, rows of round_up(H, 8) elements; its gradient twin keeps that ld
+static void make_bf16(RuntimeImpl* rt, int r) {
+  TensorImpl& x = rt->t(r);
+  if (x.data || x.grad) ROC_FATAL("set_bf16_aggregation: a tensor that becomes bf16 was already allocated");
+  x.isBf16 = true;
+  x.ld = round_up8(x.H);
+}
 static void choose_bf16_aggregation(RuntimeImpl* rt, const std::vector<GnnOp*>& layers, Wiring& w) {
   for (size_t l = 0; l < layers.size(); l++) {
     Linear* lin = as<Linear>(layers[l]);
     if (!lin || lin->activation != AC_MODE_NONE) continue;
     const int r = lin->fwdOut >= 0 ? lin->fwdOut : lin->outputs[0].region;
     if (w.consumers[r] != 1 || !as_sum_sg(layers[w.consumerOp[r]])) continue;
-    TensorImpl& x = rt->t(r);
-    if (x.data || x.grad) ROC_FATAL("set_bf16_aggregation: a tensor that becomes bf16 was already allocated");
-    x.isBf16 = true;
-    x.ld = round_up8(x.H);
+    make_bf16(rt, r);
+  }
+  // ... and what a Linear(NONE) or an unfused relu writes when a max / min, weighted or attention aggregation reads it
+  // as its feature input, and every other reader is one of those or a Linear reading it as X (no fused dropout)
+  for (size_t l = 0; l < layers.size(); l++) {
+    int r = -1;
+    if (Linear* lin = as<Linear>(layers[l]))
+      r = lin->activation == AC_MODE_NONE ? (lin->fwdOut >= 0 ? lin->fwdOut : lin->outputs[0].region) : -1;
+    else if (Activation* act = as<Activation>(layers[l]))
+      r = (act->actiMode == AC_MODE_RELU && act->fusedInto < 0) ? act->outputs[0].region : -1;
+    if (r < 0 || rt->t(r).isBf16) continue;
+    bool aggregated = false, others = true;
+    for (GnnOp* op : layers)
+      for (int j = 0; j < op->numInputs; j++) {
+        if (op->inputs[j].region != r) continue;
+        ScatterGather* sg = as<ScatterGather>(op);
+        Linear* lin = as<Linear>(op);
+        if (j == 0 && ((sg && sg->aggr != AGGR_SUM) || as<WeightedScatterGather>(op) || as<AttentionGather>(op)))
+          aggregated = true;
+        else if (!(j == 0 && lin && lin->dropOp < 0))
+          others = false;
+      }
+    if (aggregated && others) make_bf16(rt, r);
   }
 }
 
@@ -915,10 +940,14 @@ void ScatterGather::forward(const Model& model) {
       argLd = ldOut;
       arg = (uint32_t*)rt->dmalloc((size_t)model.local_rows() * (size_t)argLd * sizeof(uint32_t));
     }
+    const int how = aggr == AGGR_MAX ? ROC_SG_AGGR_MAX : ROC_SG_AGGR_MIN;
     rt->sg_begin(H);
-    ROC_CHECK(roc_sg_minmax_forward_planned(model.myGraph.plan, aggr == AGGR_MAX ? ROC_SG_AGGR_MAX : ROC_SG_AGGR_MIN, H,
-                                            rt->data(inputs[0].region), ldIn, rt->data(outputs[0].region), ldOut, arg,
-                                            argLd, rt->stream));
+    if (rt->t(inputs[0].region).isBf16)
+      ROC_CHECK(roc_sg_minmax_forward_planned_bf16(model.myGraph.plan, how, H, rt->data_bf16(inputs[0].region), ldIn,
+                                                   rt->data(outputs[0].region), ldOut, arg, argLd, rt->stream));
+    else
+      ROC_CHECK(roc_sg_minmax_forward_planned(model.myGraph.plan, how, H, rt->data(inputs[0].region), ldIn,
+                                              rt->data(outputs[0].region), ldOut, arg, argLd, rt->stream));
     rt->sg_end();
     return;
   }
@@ -1019,12 +1048,16 @@ void AttentionGather::forward(const Model& model) {
     statsLd = round_up4(2 * heads);
     stats = (float*)rt->dmalloc((size_t)std::max<int64_t>(model.local_rows(), 1) * (size_t)statsLd * sizeof(float));
   }
+  const int x = inputs[0].region, sc = inputs[1].region, y = outputs[0].region;
   rt->sg_begin(H);
-  ROC_CHECK(roc_sg_attn_forward_planned(model.myGraph.plan, heads, H, slope, model.myGraph.rowLeft,
-                                        rt->data(inputs[0].region), rt->t(inputs[0].region).ld,
-                                        rt->data(inputs[1].region), rt->t(inputs[1].region).ld,
-                                        rt->data(outputs[0].region), rt->t(outputs[0].region).ld, stats, statsLd,
-                                        rt->stream));
+  if (rt->t(x).isBf16)
+    ROC_CHECK(roc_sg_attn_forward_planned_bf16(model.myGraph.plan, heads, H, slope, model.myGraph.rowLeft,
+                                               rt->data_bf16(x), rt->t(x).ld, rt->data(sc), rt->t(sc).ld, rt->data(y),
+                                               rt->t(y).ld, stats, statsLd, rt->stream));
+  else
+    ROC_CHECK(roc_sg_attn_forward_planned(model.myGraph.plan, heads, H, slope, model.myGraph.rowLeft, rt->data(x),
+                                          rt->t(x).ld, rt->data(sc), rt->t(sc).ld, rt->data(y), rt->t(y).ld, stats,
+                                          statsLd, rt->stream));
   rt->sg_end();
 }
 
@@ -1037,20 +1070,26 @@ void AttentionGather::backward(const Model& model) {
   float* dst[2];
   for (int i = 0; i < 2; i++)
     dst[i] = grad_or_scratch(model, inputs[i].region, rt->t(inputs[i].region).requiresGrad && resetInputGrads[i], scratch[i]);
-  const int ox = outputs[0].region;
+  const int ox = outputs[0].region, x = inputs[0].region, sc = inputs[1].region;
+  const int64_t ldX = rt->t(x).ld, ldS = rt->t(sc).ld, ldO = rt->t(ox).ld;
+  const bool xBf16 = rt->t(x).isBf16;
   rt->sg_begin(H);
-  if (model.exactBackward)
-    ROC_CHECK(roc_sg_attn_backward_exact(model.myGraph.plan, rt->sgTranspose, heads, H, slope,
-                                         rt->data(inputs[0].region), rt->t(inputs[0].region).ld,
-                                         rt->data(inputs[1].region), rt->t(inputs[1].region).ld, rt->data(ox),
-                                         rt->t(ox).ld, stats, statsLd, rt->grad(ox), rt->t(ox).ld, dst[0],
-                                         rt->t(inputs[0].region).ld, dst[1], rt->t(inputs[1].region).ld, rt->stream));
+  if (model.exactBackward && xBf16)
+    ROC_CHECK(roc_sg_attn_backward_exact_bf16(model.myGraph.plan, rt->sgTranspose, heads, H, slope, rt->data_bf16(x),
+                                              ldX, rt->data(sc), ldS, rt->data(ox), ldO, stats, statsLd, rt->grad(ox),
+                                              ldO, dst[0], ldX, dst[1], ldS, rt->stream));
+  else if (model.exactBackward)
+    ROC_CHECK(roc_sg_attn_backward_exact(model.myGraph.plan, rt->sgTranspose, heads, H, slope, rt->data(x), ldX,
+                                         rt->data(sc), ldS, rt->data(ox), ldO, stats, statsLd, rt->grad(ox), ldO,
+                                         dst[0], ldX, dst[1], ldS, rt->stream));
+  else if (xBf16)
+    ROC_CHECK(roc_sg_attn_backward_planned_bf16(model.myGraph.plan, heads, H, slope, model.myGraph.rowLeft,
+                                                rt->data_bf16(x), ldX, rt->data(sc), ldS, rt->data(ox), ldO, stats,
+                                                statsLd, rt->grad(ox), ldO, dst[0], ldX, dst[1], ldS, rt->stream));
   else
-    ROC_CHECK(roc_sg_attn_backward_planned(model.myGraph.plan, heads, H, slope, model.myGraph.rowLeft,
-                                           rt->data(inputs[0].region), rt->t(inputs[0].region).ld,
-                                           rt->data(inputs[1].region), rt->t(inputs[1].region).ld, rt->data(ox),
-                                           rt->t(ox).ld, stats, statsLd, rt->grad(ox), rt->t(ox).ld, dst[0],
-                                           rt->t(inputs[0].region).ld, dst[1], rt->t(inputs[1].region).ld, rt->stream));
+    ROC_CHECK(roc_sg_attn_backward_planned(model.myGraph.plan, heads, H, slope, model.myGraph.rowLeft, rt->data(x),
+                                           ldX, rt->data(sc), ldS, rt->data(ox), ldO, stats, statsLd, rt->grad(ox),
+                                           ldO, dst[0], ldX, dst[1], ldS, rt->stream));
   rt->sg_end();
   for (int i = 0; i < 2; i++)
     if (rt->t(inputs[i].region).requiresGrad && !resetInputGrads[i]) add_scratch(model, inputs[i].region, scratch[i]);
@@ -1073,8 +1112,12 @@ void WeightedScatterGather::forward(const Model& model) {
   const int H = (int)inputs[0].dims[0];
   const int x = inputs[0].region, y = outputs[0].region;
   rt->sg_begin(H);
-  ROC_CHECK(roc_sg_weighted_forward_planned(model.myGraph.plan, H, rt->data(x), rt->t(x).ld, rt->data(inputs[1].region),
-                                            rt->data(y), rt->t(y).ld, rt->stream));
+  if (rt->t(x).isBf16)
+    ROC_CHECK(roc_sg_weighted_forward_planned_bf16(model.myGraph.plan, H, rt->data_bf16(x), rt->t(x).ld,
+                                                   rt->data(inputs[1].region), rt->data(y), rt->t(y).ld, rt->stream));
+  else
+    ROC_CHECK(roc_sg_weighted_forward_planned(model.myGraph.plan, H, rt->data(x), rt->t(x).ld,
+                                              rt->data(inputs[1].region), rt->data(y), rt->t(y).ld, rt->stream));
   rt->sg_end();
 }
 
@@ -1096,7 +1139,10 @@ void WeightedScatterGather::backward(const Model& model) {
     ROC_CHECK(roc_sg_weighted_backward_planned(rt->sgTranspose, H, rt->grad(y), ldY, rt->data(e), dst, ldX, rt->stream));
     if (!resetInputGrads[0]) add_scratch(model, x, scratch);
   }
-  if (wantE)
+  if (wantE && rt->t(x).isBf16)
+    ROC_CHECK(roc_sg_edge_dot_planned_bf16(model.myGraph.plan, H, rt->grad(y), ldY, rt->data_bf16(x), ldX, rt->grad(e),
+                                           resetInputGrads[1] ? 0 : 1, rt->stream));
+  else if (wantE)
     ROC_CHECK(roc_sg_edge_dot_planned(model.myGraph.plan, H, rt->grad(y), ldY, rt->data(x), ldX, rt->grad(e),
                                       resetInputGrads[1] ? 0 : 1, rt->stream));
   rt->sg_end();
@@ -1225,10 +1271,9 @@ void Linear::backward(const Model& model) {
     a.accumulate_dX = 0;
     a.dropMask = dropMask; a.ldMask = dropLd; a.dropRate = drop_draw(model, *d).rate;
   }
-  // a bf16 X is a leaf: dW only (with the relu backward of dY when activation is RELU); the same bits as the fp32
-  // path on the widened X
+  // a bf16 X: dW by the bf16 kernel (with the relu backward of dY when activation is RELU), the same bits as the fp32
+  // path on the widened X; only one an op produced (set_bf16_aggregation) has a gradient
   const bool xBf16 = rt->t(xRegion).isBf16;
-  if (xBf16) ROC_ASSERT(!rt->t(xRegion).requiresGrad);
   const int dxRegion = dxOut >= 0 ? dxOut : xRegion;
   a.rows = model.local_rows(); a.inDim = (int)weight.dims[0]; a.outDim = (int)weight.dims[1];
   a.X = xBf16 ? NULL : rt->data(xRegion); a.ldX = rt->t(xRegion).ld;
@@ -1244,10 +1289,19 @@ void Linear::backward(const Model& model) {
     ROC_CHECK(roc_linear_dw_bf16(a.rows, a.inDim, a.outDim, rt->data_bf16(xRegion), a.ldX, a.Y, a.ldY, a.dY, a.ldDY,
                                  a.dW, a.activation, a.workspace, a.workspaceBytes, a.dropMask, a.ldMask, a.dropRate,
                                  rt->stream));
-    return;
+    if (!a.dX) return;
   }
   if (a.dX && dxReluOf >= 0) { a.dxReluOf = rt->data(dxReluOf); a.ldReluOf = rt->t(dxReluOf).ld; }
   if (a.dX && dxNorm) { a.dxNormRowEnd = g.d_rowEnd; a.colLeft = g.colLeft; }
+  if (xBf16) {
+    // dX by the fp32 kernel, which never reads X (the bf16 rows stand in for it in the argument check) and takes dY
+    // as the dW call left it, relu-masked in place; one partition, so no pipelined row blocks
+    a.parts = ROC_LINEAR_BWD_ONLY_DX;
+    a.activation = AC_MODE_NONE;
+    a.X = reinterpret_cast<const float*>(rt->data_bf16(xRegion));
+    ROC_CHECK(roc_linear_bwd_fused(&a, rt->stream));
+    return;
+  }
   // dX feeds a ScatterGather backward on other GPUs (peer-mapped slabs): dX in row blocks, each pushed while the
   // next is computed, then dW — which nothing downstream waits for — while the last rows travel.
   PushPipe pipe(model, (a.dX && activation == AC_MODE_NONE) ? dxRegion : -1, /*grad=*/true);
@@ -1282,18 +1336,26 @@ void Activation::init(const Model&) {}
 void Activation::forward(const Model& model) {
   if (fusedInto >= 0) return;
   RuntimeImpl* rt = model.ctx;
-  ROC_CHECK(roc_activation_fwd(model.local_rows(), (int)inputs[0].dims[0], (int)actiMode, rt->data(inputs[0].region),
-                               rt->t(inputs[0].region).ld, rt->data(outputs[0].region), rt->t(outputs[0].region).ld,
-                               rt->stream));
+  const int x = inputs[0].region, y = outputs[0].region;
+  if (rt->t(y).isBf16)   // set_bf16_aggregation: a relu output that an aggregation reads
+    ROC_CHECK(roc_activation_fwd_y_bf16(model.local_rows(), (int)inputs[0].dims[0], (int)actiMode, rt->data(x),
+                                        rt->t(x).ld, rt->data_bf16(y), rt->t(y).ld, rt->stream));
+  else
+    ROC_CHECK(roc_activation_fwd(model.local_rows(), (int)inputs[0].dims[0], (int)actiMode, rt->data(x), rt->t(x).ld,
+                                 rt->data(y), rt->t(y).ld, rt->stream));
 }
 void Activation::backward(const Model& model) {
   if (fusedInto >= 0) return;   // mask applied by the fused indegree_norm backward
   RuntimeImpl* rt = model.ctx;
   if (!rt->t(inputs[0].region).requiresGrad) return;
-  ROC_CHECK(roc_activation_bwd(model.local_rows(), (int)inputs[0].dims[0], (int)actiMode, rt->data(outputs[0].region),
-                               rt->t(outputs[0].region).ld, rt->grad(outputs[0].region), rt->t(outputs[0].region).ld,
-                               rt->grad(inputs[0].region), rt->t(inputs[0].region).ld, resetInputGrads[0] ? 0 : 1,
-                               rt->stream));
+  const int x = inputs[0].region, y = outputs[0].region;
+  const int rows = model.local_rows(), H = (int)inputs[0].dims[0], acc = resetInputGrads[0] ? 0 : 1;
+  if (rt->t(y).isBf16)   // the mask of the stored bf16 y
+    ROC_CHECK(roc_activation_bwd_y_bf16(rows, H, (int)actiMode, rt->data_bf16(y), rt->t(y).ld, rt->grad(y), rt->t(y).ld,
+                                        rt->grad(x), rt->t(x).ld, acc, rt->stream));
+  else
+    ROC_CHECK(roc_activation_bwd(rows, H, (int)actiMode, rt->data(y), rt->t(y).ld, rt->grad(y), rt->t(y).ld,
+                                 rt->grad(x), rt->t(x).ld, acc, rt->stream));
 }
 
 // ---------------------------------------------------------------- Element ---

@@ -41,6 +41,9 @@
 //    gradient is the ASRC gather itself, run over the transposed plan.
 //  * the sum over bf16 rows (roc_sg_forward_planned_bf16) is BSUM: SUM's row of the table with half-width loads,
 //    widened in registers, on both the register and the ring kernel.
+//  * the max / min, weighted, edge-dot and attention calls over bf16 feature rows (roc_sg_*_bf16) are those
+//    reductions plus SG_RED_BF16: the same row of the table and the same fix-ups, with the feature rows loaded at half
+//    width and widened in registers as BSUM's are.  Their bytes per gathered row fall from 4H to 2H.
 //
 // Algorithmic bytes per launch (DESIGN.md): E*(4H+4) + Nloc*(4H+8); min / max forward E*(4H+4) + Nloc*(8H+8),
 // backward E*(8H+4) + Nloc*(4H+8); the sum over bf16 rows E*(2H+4) + Nloc*(4H+8); weighted forward E*(4H+8) + Nloc*(4H+8), edge dot E*(4H+8) + Nloc*4H; attention
@@ -249,9 +252,18 @@ __device__ __forceinline__ typename V<VEC>::T ld_bf16(const char* p) {
 // MASK where an entry whose destination repeats the previous entry's in the same row (a duplicate edge) adds nothing.
 // BSUM is the sum over bf16 rows (roc_sg_forward_planned_bf16): only its loads differ from SUM's, each T-column of VEC
 // bf16 values widened exactly in registers, so it adds the same floats in the same order.
+// SG_RED_BF16 added to MAX, MIN, ATTN, ADST, ASRC, WSUM or EDOT is that reduction's bf16 form (the roc_sg_*_bf16
+// calls): the feature rows X it reads (gathered, or ASRC's own row i) are bf16, loaded and widened as BSUM's are, and
+// everything else is the fp32 reduction's, its row of SG_REDS included.
 enum { SG_RED_SUM = 0, SG_RED_MAX = ROC_SG_AGGR_MAX, SG_RED_MIN = ROC_SG_AGGR_MIN, SG_RED_MASK = 3,
        SG_RED_ASTAT = 4, SG_RED_ATTN = 5, SG_RED_ADST = 6, SG_RED_ASRC = 7, SG_RED_WSUM = 8, SG_RED_EDOT = 9,
        SG_RED_TSUM = 10, SG_RED_TMASK = 11, SG_RED_BSUM = 12 };
+constexpr int SG_RED_BF16 = 16;
+__host__ __device__ constexpr int sg_red_base(int RF) { return RF & (SG_RED_BF16 - 1); }
+// the rows gathered as `in` are bf16 (every bf16 form but ASRC's, which gathers fp32 gradients)
+__host__ __device__ constexpr bool sg_bf16_in(int RF) {
+  return RF == SG_RED_BSUM || ((RF & SG_RED_BF16) && sg_red_base(RF) != SG_RED_ASRC);
+}
 constexpr uint32_t SG_NOARG = 0xFFFFFFFFu;   // index of a row that has no edge yet
 
 // The ordering rule: the candidate v replaces the current a iff it is strictly greater (smaller) or it is NaN and a
@@ -423,12 +435,13 @@ __device__ __forceinline__ uint32_t norm_deg(const SgParams& p, uint32_t r, uint
 // ------------------------------------------------------------- main kernel ---
 // One worker (L lanes) per chunk.  Lane `lane` owns T-columns lane + ch*L.
 // RED (SG_RED_*) changes only what is done with a gathered row and what the row store writes; the schedule, the
-// gathers and the single store site are the same for every reduction.
-template <int VEC, int L, int NCH, int U, int MINB, int RED = SG_RED_SUM>
+// gathers and the single store site are the same for every reduction.  RF is RED, plus SG_RED_BF16 for its bf16 form.
+template <int VEC, int L, int NCH, int U, int MINB, int RF = SG_RED_SUM>
 __global__ void __launch_bounds__(SG_THREADS, MINB)
 sg_chunk_kernel(const SgParams p) {
   typedef typename V<VEC>::T T;
   typedef typename V<VEC>::I I;
+  constexpr int RED = sg_red_base(RF);
   constexpr bool MM = RED == SG_RED_MAX || RED == SG_RED_MIN;
   constexpr bool AT = RED >= SG_RED_ASTAT && RED <= SG_RED_ASRC; // an attention pass
   constexpr bool SV = RED == SG_RED_ATTN || RED == SG_RED_ADST;  // gathers s_src[j] beside in[j]
@@ -436,7 +449,8 @@ sg_chunk_kernel(const SgParams p) {
   constexpr bool WS = RED == SG_RED_WSUM;                        // loads each edge's weight beside its source id
   constexpr bool ED = RED == SG_RED_EDOT;                        // holds G[i], stores one dot product per edge
   constexpr bool MK = RED == SG_RED_MASK || RED == SG_RED_TMASK; // gathers an index row beside each gradient row
-  constexpr bool BF = RED == SG_RED_BSUM;                        // gathers bf16 rows
+  constexpr bool BX = (RF & SG_RED_BF16) && RED == SG_RED_ASRC;  // its own row X[i] (xrow) is bf16
+  constexpr bool BF = sg_bf16_in(RF);                            // gathers bf16 rows
   constexpr uint32_t TB = BF ? 2 * VEC : sizeof(T);              // bytes of one T-column of `in`
   constexpr int WPB = SG_THREADS / L;
   constexpr uint32_t CH = SG_CH;
@@ -515,7 +529,10 @@ sg_chunk_kernel(const SgParams p) {
         }
         if constexpr (RED == SG_RED_ASRC) r0s[ch] = __ldg(p.score + gi * p.ldS + p.heads + kh[ch]);
         if constexpr (RED == SG_RED_ADST) rrec[ch] = __ldg(p.rec + gi * p.heads + kh[ch]);
-        if constexpr (XI)
+        if constexpr (BX)
+          xi[ch] = ld_bf16<VEC>(static_cast<const char*>(p.xrow) +
+                                (gi * p.ldX + min((uint32_t)(lane + ch * L), p.Q - 1u)) * (2 * VEC));
+        else if constexpr (XI)
           xi[ch] = V<VEC>::ld(reinterpret_cast<const T*>(p.xrow) + gi * p.ldX + min((uint32_t)(lane + ch * L), p.Q - 1u));
       }
     }
@@ -757,7 +774,7 @@ sg_chunk_kernel(const SgParams p) {
             } else {
 #pragma unroll
               for (int ch = 0; ch < NCH; ch++) {
-                if constexpr (RED == SG_RED_SUM || RED == SG_RED_TSUM || BF) V<VEC>::add(acc[ch], v[u][ch]);
+                if constexpr (RED == SG_RED_SUM || RED == SG_RED_TSUM || RED == SG_RED_BSUM) V<VEC>::add(acc[ch], v[u][ch]);
                 else if constexpr (RED == SG_RED_MASK) mask_add(acc[ch], v[u][ch], av[u][ch], p.selfBase + cur);
                 else mm_add<RED>(acc[ch], aidx[ch], v[u][ch], srcs[u]);
               }
@@ -1332,7 +1349,8 @@ struct SgRed {
 // occupancy.  WSUM keeps the sum's U and holds U weights beside them, so at one chunk per lane it runs three CTAs per
 // SM.  TSUM and TMASK take the shapes of SUM and MASK, but TMASK, which also holds each group's repeated-destination
 // bits, runs three CTAs per SM at one chunk per lane.  BSUM is SUM's row with bf16 loads (ring MODE bit 8): the same
-// column blocks, shapes and sum fix-ups, so that its results are SUM's bits on the widened rows.
+// column blocks, shapes and sum fix-ups, so that its results are SUM's bits on the widened rows.  The other bf16 forms
+// (SG_RED_BF16) have no row of their own: they take their reduction's, fix-ups included, for the same reason.
 constexpr SgRed SG_REDS[] = {
     // red           maxQ4 maxQ1 ring fix           heads  carry           u4  u             minb
     {SG_RED_SUM,     256,  256,  0,   SG_FIX_SUM,   false, SG_CARRY_FLOAT, 4, {8, 4, 2, 1}, {4, 3, 3, 2}},
@@ -1355,10 +1373,12 @@ constexpr bool sg_reds_in_order() {
 }
 static_assert(sg_reds_in_order(), "SG_REDS has one row per SG_RED_* value, in order");
 
-constexpr int sg_max_q(int VEC, int RED) { return VEC == 4 ? SG_REDS[RED].maxQ4 : SG_REDS[RED].maxQ1; }
+// A bf16 form (SG_RED_BF16) takes its reduction's row.
+constexpr const SgRed& sg_red(int RF) { return SG_REDS[sg_red_base(RF)]; }
+constexpr int sg_max_q(int VEC, int RED) { return VEC == 4 ? sg_red(RED).maxQ4 : sg_red(RED).maxQ1; }
 constexpr int sg_nch_index(int NCH) { return NCH == 1 ? 0 : NCH == 2 ? 1 : NCH == 4 ? 2 : 3; }
-constexpr int sg_chunk_u(int RED, int L, int NCH) { return L == 4 ? SG_REDS[RED].u4 : SG_REDS[RED].u[sg_nch_index(NCH)]; }
-constexpr int sg_chunk_minb(int RED, int NCH) { return SG_REDS[RED].minb[sg_nch_index(NCH)]; }
+constexpr int sg_chunk_u(int RED, int L, int NCH) { return L == 4 ? sg_red(RED).u4 : sg_red(RED).u[sg_nch_index(NCH)]; }
+constexpr int sg_chunk_minb(int RED, int NCH) { return sg_red(RED).minb[sg_nch_index(NCH)]; }
 
 // sg_chunk_kernel_t's two shapes, the measured defaults (DESIGN.md §3.1), four workers per CTA: rows of 65..128 floats
 // (one float4 per lane) with lane-held ids and two stages of two four-row units per worker; rows of 129..256 floats
@@ -1421,7 +1441,7 @@ static int launch_fixups(const SgParams& p, cudaStream_t st, bool heads = false)
 // out2 / carry2 as a VEC = 1, Q = heads output.
 template <int VEC, int RED, int L, int NCH>
 static int launch(const SgParams& p, cudaStream_t st) {
-  constexpr SgRed R = SG_REDS[RED];
+  constexpr SgRed R = sg_red(RED);
   constexpr int WPB = SG_THREADS / L;
   int rc = ROC_OK;
   if (p.numChunks) {
@@ -1443,7 +1463,7 @@ static int launch(const SgParams& p, cudaStream_t st) {
       note_launch(ROC_SG_LAUNCH_STAT_FIXUP, RED, 1, 32, 1, grid);
     }
   } else if constexpr (R.fix != SG_FIX_NONE) {
-    if ((rc = launch_fixups<VEC, L, NCH, R.fix == SG_FIX_OWN ? RED : SG_RED_SUM>(p, st)) != ROC_OK) return rc;
+    if ((rc = launch_fixups<VEC, L, NCH, R.fix == SG_FIX_OWN ? R.red : SG_RED_SUM>(p, st)) != ROC_OK) return rc;
   }
   if constexpr (R.headsFix) {
     SgParams p2 = p;
@@ -1721,12 +1741,13 @@ struct SgEdge {
 // on float4 rows when every leading dimension and pointer allows them.  `arg` holds the min / max indices
 // (written by the forward, gathered by the backward); the sum passes none.  EDOT's column blocks add their partial
 // dot products to dw in block order: the first overwrites it (or adds, with ed.accumulate), the later ones add.
-// `in` holds fp32 rows, bf16 ones (raw bits) for BSUM; its leading dimension is in elements either way.
+// `in` holds fp32 rows, bf16 ones (raw bits) for BSUM and the bf16 forms; its leading dimension is in elements either
+// way.
 template <int RED>
 static int run_planned(roc_sg_plan* pl, int H, const void* in, int64_t ldIn, float* out, int64_t ldOut,
                        const roc_vid_t* arg, int64_t ldArg, int epilogue, roc_vid_t selfBase, cudaStream_t st,
                        const SgEdge& ed = SgEdge()) {
-  constexpr SgCarry CARRY = SG_REDS[RED].carry;
+  constexpr SgCarry CARRY = sg_red(RED).carry;
   const bool vec = float4_rows({in, out, arg, ed.g}, {ldIn, ldOut, ldArg, ed.ldG});
   const int blockCols = vec ? 4 * sg_max_q(4, RED) : sg_max_q(1, RED);
   int rc = CARRY == SG_CARRY_NONE ? ROC_OK : grow_carries(pl, std::min(H, blockCols), st);
@@ -1736,7 +1757,7 @@ static int run_planned(roc_sg_plan* pl, int H, const void* in, int64_t ldIn, flo
   if (rc != ROC_OK) return rc;
   for (int c0 = 0; c0 < H; c0 += blockCols) {
     SgParams p = plan_params(pl);
-    p.in = static_cast<const char*>(in) + (size_t)c0 * (RED == SG_RED_BSUM ? 2 : 4);
+    p.in = static_cast<const char*>(in) + (size_t)c0 * (sg_bf16_in(RED) ? 2 : 4);
     p.out = out ? out + c0 : nullptr; p.epi = epilogue; p.selfBase = selfBase;
     if (arg) p.arg = const_cast<roc_vid_t*>(arg) + c0;
     p.ldIn = (size_t)ldIn; p.ldOut = (size_t)ldOut; p.ldArg = (size_t)ldArg;
@@ -1750,6 +1771,10 @@ static int run_planned(roc_sg_plan* pl, int H, const void* in, int64_t ldIn, flo
   }
   return ROC_OK;
 }
+
+// The input rule of every bf16 feature input `in` (a NULL one is left to the call's own checks): 16-byte aligned, with
+// a leading dimension that is a multiple of 8 elements, so that it takes float4 rows exactly when its fp32 twin does.
+static bool bf16_rows_bad(const void* in, int64_t ldIn) { return in && ((ldIn % 8) || !aligned16(in)); }
 
 extern "C" int roc_sg_forward_planned(const roc_sg_plan* plc, int H, const float* in, int64_t ldIn,
                                       float* out, int64_t ldOut, int epilogue, roc_stream_t stream) {
@@ -1791,17 +1816,29 @@ extern "C" int roc_sg_plan_rows_sorted(const roc_sg_plan* pl, int* sorted, roc_s
   return ROC_OK;
 }
 
-extern "C" int roc_sg_minmax_forward_planned(const roc_sg_plan* plc, int aggr, int H, const float* in, int64_t ldIn,
-                                             float* out, int64_t ldOut, roc_vid_t* arg, int64_t ldArg,
-                                             roc_stream_t stream) {
+template <int BF>
+static int minmax_forward(const roc_sg_plan* plc, int aggr, int H, const void* in, int64_t ldIn, float* out,
+                          int64_t ldOut, roc_vid_t* arg, int64_t ldArg, roc_stream_t stream) {
   roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
   clear_launches();
   if (!pl || (aggr != ROC_SG_AGGR_MAX && aggr != ROC_SG_AGGR_MIN) || H <= 0 || !in || !out || !arg || ldIn < H ||
-      ldOut < H || ldArg < H)
+      ldOut < H || ldArg < H || (BF && bf16_rows_bad(in, ldIn)))
     return ROC_ERR_INVALID;
   cudaStream_t st = as_stream(stream);
-  return aggr == ROC_SG_AGGR_MAX ? run_planned<SG_RED_MAX>(pl, H, in, ldIn, out, ldOut, arg, ldArg, 0, 0, st)
-                                 : run_planned<SG_RED_MIN>(pl, H, in, ldIn, out, ldOut, arg, ldArg, 0, 0, st);
+  return aggr == ROC_SG_AGGR_MAX ? run_planned<SG_RED_MAX | BF>(pl, H, in, ldIn, out, ldOut, arg, ldArg, 0, 0, st)
+                                 : run_planned<SG_RED_MIN | BF>(pl, H, in, ldIn, out, ldOut, arg, ldArg, 0, 0, st);
+}
+
+extern "C" int roc_sg_minmax_forward_planned(const roc_sg_plan* plc, int aggr, int H, const float* in, int64_t ldIn,
+                                             float* out, int64_t ldOut, roc_vid_t* arg, int64_t ldArg,
+                                             roc_stream_t stream) {
+  return minmax_forward<0>(plc, aggr, H, in, ldIn, out, ldOut, arg, ldArg, stream);
+}
+
+extern "C" int roc_sg_minmax_forward_planned_bf16(const roc_sg_plan* plc, int aggr, int H, const uint16_t* in,
+                                                  int64_t ldIn, float* out, int64_t ldOut, roc_vid_t* arg,
+                                                  int64_t ldArg, roc_stream_t stream) {
+  return minmax_forward<SG_RED_BF16>(plc, aggr, H, in, ldIn, out, ldOut, arg, ldArg, stream);
 }
 
 extern "C" int roc_sg_minmax_backward_planned(const roc_sg_plan* plc, int H, roc_vid_t selfBase, const float* outGrad,
@@ -1844,8 +1881,10 @@ static SgParams attn_params(const roc_sg_plan* pl, int heads, int H, float slope
 // ids [0, n) and B1 (d s_dst) over `pl`, B2 (inGrad, d s_src) over `plB2`.  With plB2 = pl, B2 is the gather over the
 // same CSR (quirk Q1); over the transposed plan its row j gathers the destinations i of j's out-edges, where the same
 // formula, a(i<-j) G[i] against the record of i, is the true adjoint.
+// BF = SG_RED_BF16: `in` holds bf16 rows, gathered by B1 and read as each row's own row by B2.
+template <int BF>
 static int attn_backward_passes(roc_sg_plan* pl, roc_sg_plan* plB2, uint32_t n, int heads, int H, float slope,
-                                roc_vid_t selfBase, uint32_t fs, bool vec, const float* in, int64_t ldIn,
+                                roc_vid_t selfBase, uint32_t fs, bool vec, const void* in, int64_t ldIn,
                                 const float* score, int64_t ldS, const float* out, int64_t ldOut, const float* stats,
                                 int64_t ldStats, const float* outGrad, int64_t ldG, float* inGrad, int64_t ldInG,
                                 float* scoreGrad, int64_t ldSG, cudaStream_t st) {
@@ -1864,7 +1903,7 @@ static int attn_backward_passes(roc_sg_plan* pl, roc_sg_plan* plB2, uint32_t n, 
   b1.in = in; b1.ldIn = (size_t)ldIn; b1.xrow = outGrad; b1.ldX = (size_t)ldG;
   b1.out = nullptr; b1.out2 = scoreGrad; b1.ldOut2 = (size_t)ldSG;
   t_units(b1, vw, H);
-  rc = vec ? dispatch<4, SG_RED_ADST>(b1, st) : dispatch<1, SG_RED_ADST>(b1, st);
+  rc = vec ? dispatch<4, SG_RED_ADST | BF>(b1, st) : dispatch<1, SG_RED_ADST | BF>(b1, st);
   if (rc != ROC_OK) return rc;
   // B2: inGrad and d s_src, gathering G[j] and the record of j against X[i]
   SgParams b2 = attn_params(plB2, heads, H, slope, selfBase, score, ldS, stats, ldStats, fs);
@@ -1872,17 +1911,17 @@ static int attn_backward_passes(roc_sg_plan* pl, roc_sg_plan* plB2, uint32_t n, 
   b2.in = outGrad; b2.ldIn = (size_t)ldG; b2.xrow = in; b2.ldX = (size_t)ldIn;
   b2.out = inGrad; b2.ldOut = (size_t)ldInG; b2.out2 = scoreGrad + heads; b2.ldOut2 = (size_t)ldSG;
   t_units(b2, vw, H);
-  return vec ? dispatch<4, SG_RED_ASRC>(b2, st) : dispatch<1, SG_RED_ASRC>(b2, st);
+  return vec ? dispatch<4, SG_RED_ASRC | BF>(b2, st) : dispatch<1, SG_RED_ASRC | BF>(b2, st);
 }
 
-extern "C" int roc_sg_attn_forward_planned(const roc_sg_plan* plc, int heads, int H, float slope, roc_vid_t selfBase,
-                                           const float* in, int64_t ldIn, const float* score, int64_t ldS,
-                                           float* out, int64_t ldOut, float* stats, int64_t ldStats,
-                                           roc_stream_t stream) {
+template <int BF>
+static int attn_forward(const roc_sg_plan* plc, int heads, int H, float slope, roc_vid_t selfBase, const void* in,
+                        int64_t ldIn, const float* score, int64_t ldS, float* out, int64_t ldOut, float* stats,
+                        int64_t ldStats, roc_stream_t stream) {
   roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
   clear_launches();
   if (!pl || !in || !score || !out || !stats || heads <= 0 || H <= 0 || ldIn < H || ldOut < H ||
-      ldS < 2 * (int64_t)heads || ldStats < 2 * (int64_t)heads)
+      ldS < 2 * (int64_t)heads || ldStats < 2 * (int64_t)heads || (BF && bf16_rows_bad(in, ldIn)))
     return ROC_ERR_INVALID;
   const bool vec = float4_rows({in, out}, {ldIn, ldOut});
   cudaStream_t st = as_stream(stream);
@@ -1898,19 +1937,34 @@ extern "C" int roc_sg_attn_forward_planned(const roc_sg_plan* plc, int heads, in
   SgParams b = attn_params(pl, heads, H, slope, selfBase, score, ldS, stats, ldStats, fs);
   b.in = in; b.ldIn = (size_t)ldIn; b.out = out; b.ldOut = (size_t)ldOut;
   t_units(b, vec ? 4 : 1, H);
-  return vec ? dispatch<4, SG_RED_ATTN>(b, st) : dispatch<1, SG_RED_ATTN>(b, st);
+  return vec ? dispatch<4, SG_RED_ATTN | BF>(b, st) : dispatch<1, SG_RED_ATTN | BF>(b, st);
 }
 
-extern "C" int roc_sg_attn_backward_planned(const roc_sg_plan* plc, int heads, int H, float slope, roc_vid_t selfBase,
-                                            const float* in, int64_t ldIn, const float* score, int64_t ldS,
-                                            const float* out, int64_t ldOut, const float* stats, int64_t ldStats,
-                                            const float* outGrad, int64_t ldG, float* inGrad, int64_t ldInG,
-                                            float* scoreGrad, int64_t ldSG, roc_stream_t stream) {
+extern "C" int roc_sg_attn_forward_planned(const roc_sg_plan* plc, int heads, int H, float slope, roc_vid_t selfBase,
+                                           const float* in, int64_t ldIn, const float* score, int64_t ldS,
+                                           float* out, int64_t ldOut, float* stats, int64_t ldStats,
+                                           roc_stream_t stream) {
+  return attn_forward<0>(plc, heads, H, slope, selfBase, in, ldIn, score, ldS, out, ldOut, stats, ldStats, stream);
+}
+
+extern "C" int roc_sg_attn_forward_planned_bf16(const roc_sg_plan* plc, int heads, int H, float slope,
+                                                roc_vid_t selfBase, const uint16_t* in, int64_t ldIn,
+                                                const float* score, int64_t ldS, float* out, int64_t ldOut,
+                                                float* stats, int64_t ldStats, roc_stream_t stream) {
+  return attn_forward<SG_RED_BF16>(plc, heads, H, slope, selfBase, in, ldIn, score, ldS, out, ldOut, stats, ldStats,
+                                   stream);
+}
+
+template <int BF>
+static int attn_backward(const roc_sg_plan* plc, int heads, int H, float slope, roc_vid_t selfBase, const void* in,
+                         int64_t ldIn, const float* score, int64_t ldS, const float* out, int64_t ldOut,
+                         const float* stats, int64_t ldStats, const float* outGrad, int64_t ldG, float* inGrad,
+                         int64_t ldInG, float* scoreGrad, int64_t ldSG, roc_stream_t stream) {
   roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
   clear_launches();
   if (!pl || !in || !score || !out || !stats || !outGrad || !inGrad || !scoreGrad || heads <= 0 || H <= 0 ||
       ldIn < H || ldOut < H || ldG < H || ldInG < H || ldS < 2 * (int64_t)heads || ldStats < 2 * (int64_t)heads ||
-      ldSG < 2 * (int64_t)heads)
+      ldSG < 2 * (int64_t)heads || (BF && bf16_rows_bad(in, ldIn)))
     return ROC_ERR_INVALID;
   const bool vec = float4_rows({in, out, outGrad, inGrad}, {ldIn, ldOut, ldG, ldInG});
   cudaStream_t st = as_stream(stream);
@@ -1920,20 +1974,39 @@ extern "C" int roc_sg_attn_backward_planned(const roc_sg_plan* plc, int heads, i
   if ((rc = find_id_end(pl, st)) != ROC_OK) return rc;
   const uint64_t n64 = std::max<uint64_t>(pl->idEnd, (uint64_t)selfBase + pl->nloc);
   if (n64 >= 0xFFFFFFF0ull) return ROC_ERR_UNSUPPORTED;
-  return attn_backward_passes(pl, pl, (uint32_t)n64, heads, H, slope, selfBase, fs, vec, in, ldIn, score, ldS, out,
-                              ldOut, stats, ldStats, outGrad, ldG, inGrad, ldInG, scoreGrad, ldSG, st);
+  return attn_backward_passes<BF>(pl, pl, (uint32_t)n64, heads, H, slope, selfBase, fs, vec, in, ldIn, score, ldS, out,
+                                  ldOut, stats, ldStats, outGrad, ldG, inGrad, ldInG, scoreGrad, ldSG, st);
 }
 
-extern "C" int roc_sg_attn_backward_exact(const roc_sg_plan* plc, roc_sg_transpose* tr, int heads, int H, float slope,
-                                          const float* in, int64_t ldIn, const float* score, int64_t ldS,
-                                          const float* out, int64_t ldOut, const float* stats, int64_t ldStats,
-                                          const float* outGrad, int64_t ldG, float* inGrad, int64_t ldInG,
-                                          float* scoreGrad, int64_t ldSG, roc_stream_t stream) {
+extern "C" int roc_sg_attn_backward_planned(const roc_sg_plan* plc, int heads, int H, float slope, roc_vid_t selfBase,
+                                            const float* in, int64_t ldIn, const float* score, int64_t ldS,
+                                            const float* out, int64_t ldOut, const float* stats, int64_t ldStats,
+                                            const float* outGrad, int64_t ldG, float* inGrad, int64_t ldInG,
+                                            float* scoreGrad, int64_t ldSG, roc_stream_t stream) {
+  return attn_backward<0>(plc, heads, H, slope, selfBase, in, ldIn, score, ldS, out, ldOut, stats, ldStats, outGrad,
+                          ldG, inGrad, ldInG, scoreGrad, ldSG, stream);
+}
+
+extern "C" int roc_sg_attn_backward_planned_bf16(const roc_sg_plan* plc, int heads, int H, float slope,
+                                                 roc_vid_t selfBase, const uint16_t* in, int64_t ldIn,
+                                                 const float* score, int64_t ldS, const float* out, int64_t ldOut,
+                                                 const float* stats, int64_t ldStats, const float* outGrad,
+                                                 int64_t ldG, float* inGrad, int64_t ldInG, float* scoreGrad,
+                                                 int64_t ldSG, roc_stream_t stream) {
+  return attn_backward<SG_RED_BF16>(plc, heads, H, slope, selfBase, in, ldIn, score, ldS, out, ldOut, stats, ldStats,
+                                    outGrad, ldG, inGrad, ldInG, scoreGrad, ldSG, stream);
+}
+
+template <int BF>
+static int attn_backward_exact(const roc_sg_plan* plc, roc_sg_transpose* tr, int heads, int H, float slope,
+                               const void* in, int64_t ldIn, const float* score, int64_t ldS, const float* out,
+                               int64_t ldOut, const float* stats, int64_t ldStats, const float* outGrad, int64_t ldG,
+                               float* inGrad, int64_t ldInG, float* scoreGrad, int64_t ldSG, roc_stream_t stream) {
   roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
   clear_launches();
   if (!pl || !tr || !in || !score || !out || !stats || !outGrad || !inGrad || !scoreGrad || heads <= 0 || H <= 0 ||
       ldIn < H || ldOut < H || ldG < H || ldInG < H || ldS < 2 * (int64_t)heads || ldStats < 2 * (int64_t)heads ||
-      ldSG < 2 * (int64_t)heads || pl->nloc != tr->N || pl->E != tr->E)
+      ldSG < 2 * (int64_t)heads || pl->nloc != tr->N || pl->E != tr->E || (BF && bf16_rows_bad(in, ldIn)))
     return ROC_ERR_INVALID;
   const bool vec = float4_rows({in, out, outGrad, inGrad}, {ldIn, ldOut, ldG, ldInG});
   cudaStream_t st = as_stream(stream);
@@ -1942,28 +2015,71 @@ extern "C" int roc_sg_attn_backward_exact(const roc_sg_plan* plc, roc_sg_transpo
   if (rc == ROC_OK) rc = attn_setup(tr->planT, heads, H, slope, vec, st, &fs);
   if (rc != ROC_OK) return rc;
   // a whole graph: every id is below N, so the records cover [0, N) with no id scan
-  return attn_backward_passes(pl, tr->planT, tr->N, heads, H, slope, 0, fs, vec, in, ldIn, score, ldS, out, ldOut,
-                              stats, ldStats, outGrad, ldG, inGrad, ldInG, scoreGrad, ldSG, st);
+  return attn_backward_passes<BF>(pl, tr->planT, tr->N, heads, H, slope, 0, fs, vec, in, ldIn, score, ldS, out, ldOut,
+                                  stats, ldStats, outGrad, ldG, inGrad, ldInG, scoreGrad, ldSG, st);
+}
+
+extern "C" int roc_sg_attn_backward_exact(const roc_sg_plan* plc, roc_sg_transpose* tr, int heads, int H, float slope,
+                                          const float* in, int64_t ldIn, const float* score, int64_t ldS,
+                                          const float* out, int64_t ldOut, const float* stats, int64_t ldStats,
+                                          const float* outGrad, int64_t ldG, float* inGrad, int64_t ldInG,
+                                          float* scoreGrad, int64_t ldSG, roc_stream_t stream) {
+  return attn_backward_exact<0>(plc, tr, heads, H, slope, in, ldIn, score, ldS, out, ldOut, stats, ldStats, outGrad,
+                                ldG, inGrad, ldInG, scoreGrad, ldSG, stream);
+}
+
+extern "C" int roc_sg_attn_backward_exact_bf16(const roc_sg_plan* plc, roc_sg_transpose* tr, int heads, int H,
+                                               float slope, const uint16_t* in, int64_t ldIn, const float* score,
+                                               int64_t ldS, const float* out, int64_t ldOut, const float* stats,
+                                               int64_t ldStats, const float* outGrad, int64_t ldG, float* inGrad,
+                                               int64_t ldInG, float* scoreGrad, int64_t ldSG, roc_stream_t stream) {
+  return attn_backward_exact<SG_RED_BF16>(plc, tr, heads, H, slope, in, ldIn, score, ldS, out, ldOut, stats, ldStats,
+                                          outGrad, ldG, inGrad, ldInG, scoreGrad, ldSG, stream);
+}
+
+template <int BF>
+static int weighted_forward(const roc_sg_plan* plc, int H, const void* in, int64_t ldIn, const float* w, float* out,
+                            int64_t ldOut, roc_stream_t stream) {
+  roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  clear_launches();
+  if (!pl || H <= 0 || !in || !w || !out || ldIn < H || ldOut < H || (BF && bf16_rows_bad(in, ldIn)))
+    return ROC_ERR_INVALID;
+  SgEdge ed;
+  ed.w = w;
+  return run_planned<SG_RED_WSUM | BF>(pl, H, in, ldIn, out, ldOut, nullptr, 0, 0, 0, as_stream(stream), ed);
 }
 
 extern "C" int roc_sg_weighted_forward_planned(const roc_sg_plan* plc, int H, const float* in, int64_t ldIn,
                                                const float* w, float* out, int64_t ldOut, roc_stream_t stream) {
+  return weighted_forward<0>(plc, H, in, ldIn, w, out, ldOut, stream);
+}
+
+extern "C" int roc_sg_weighted_forward_planned_bf16(const roc_sg_plan* plc, int H, const uint16_t* in, int64_t ldIn,
+                                                    const float* w, float* out, int64_t ldOut, roc_stream_t stream) {
+  return weighted_forward<SG_RED_BF16>(plc, H, in, ldIn, w, out, ldOut, stream);
+}
+
+template <int BF>
+static int edge_dot(const roc_sg_plan* plc, int H, const float* outGrad, int64_t ldG, const void* in, int64_t ldIn,
+                    float* dw, int accumulate, roc_stream_t stream) {
   roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
   clear_launches();
-  if (!pl || H <= 0 || !in || !w || !out || ldIn < H || ldOut < H) return ROC_ERR_INVALID;
+  if (!pl || H <= 0 || !outGrad || !in || !dw || ldG < H || ldIn < H || (BF && bf16_rows_bad(in, ldIn)))
+    return ROC_ERR_INVALID;
   SgEdge ed;
-  ed.w = w;
-  return run_planned<SG_RED_WSUM>(pl, H, in, ldIn, out, ldOut, nullptr, 0, 0, 0, as_stream(stream), ed);
+  ed.g = outGrad; ed.ldG = ldG; ed.dw = dw; ed.accumulate = accumulate != 0;
+  return run_planned<SG_RED_EDOT | BF>(pl, H, in, ldIn, nullptr, 0, nullptr, 0, 0, 0, as_stream(stream), ed);
 }
 
 extern "C" int roc_sg_edge_dot_planned(const roc_sg_plan* plc, int H, const float* outGrad, int64_t ldG,
                                        const float* in, int64_t ldIn, float* dw, int accumulate, roc_stream_t stream) {
-  roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
-  clear_launches();
-  if (!pl || H <= 0 || !outGrad || !in || !dw || ldG < H || ldIn < H) return ROC_ERR_INVALID;
-  SgEdge ed;
-  ed.g = outGrad; ed.ldG = ldG; ed.dw = dw; ed.accumulate = accumulate != 0;
-  return run_planned<SG_RED_EDOT>(pl, H, in, ldIn, nullptr, 0, nullptr, 0, 0, 0, as_stream(stream), ed);
+  return edge_dot<0>(plc, H, outGrad, ldG, in, ldIn, dw, accumulate, stream);
+}
+
+extern "C" int roc_sg_edge_dot_planned_bf16(const roc_sg_plan* plc, int H, const float* outGrad, int64_t ldG,
+                                            const uint16_t* in, int64_t ldIn, float* dw, int accumulate,
+                                            roc_stream_t stream) {
+  return edge_dot<SG_RED_BF16>(plc, H, outGrad, ldG, in, ldIn, dw, accumulate, stream);
 }
 
 extern "C" void roc_sg_transpose_destroy(roc_sg_transpose* tr) {

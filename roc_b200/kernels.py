@@ -103,6 +103,16 @@ class SgPlan:
                                                 _ptr(arg), _ld(arg), _stream()), "roc_sg_minmax_forward_planned")
         return out, arg
 
+    def minmax_forward_bf16(self, x, aggr, out=None, arg=None):
+        """roc_sg_minmax_forward_planned_bf16: minmax_forward() over bf16 rows (16-byte aligned, ld a multiple of 8, as bf16_padded makes them)."""
+        assert x.dtype == torch.bfloat16
+        out = self._rows(x) if out is None else out
+        arg = self._rows(x, dtype=torch.int32) if arg is None else arg
+        check(lib.roc_sg_minmax_forward_planned_bf16(self.handle, int(aggr), x.shape[1], _ptr(x), _ld(x), _ptr(out),
+                                                     _ld(out), _ptr(arg), _ld(arg), _stream()),
+              "roc_sg_minmax_forward_planned_bf16")
+        return out, arg
+
     def minmax_backward(self, gy, arg, self_base=0, out=None):
         """Gradient of minmax_forward's input: out[u] = sum over row u's edges e (v = col[e]) of gy[v] where
         arg[v] == self_base + u.  gy and arg are indexed like the forward's input."""
@@ -127,6 +137,17 @@ class SgPlan:
                                               _ld(stats), _stream()), "roc_sg_attn_forward_planned")
         return out, stats
 
+    def attn_forward_bf16(self, x, scores, heads=1, slope=0.2, self_base=0, out=None, stats=None):
+        """roc_sg_attn_forward_planned_bf16: attn_forward() over bf16 feature rows (16-byte aligned, ld a multiple of 8, as bf16_padded makes them)."""
+        assert x.dtype == torch.bfloat16
+        out = self._rows(x) if out is None else out
+        stats = torch.empty((self.nloc, 2 * heads), device=x.device) if stats is None else stats
+        check(lib.roc_sg_attn_forward_planned_bf16(self.handle, int(heads), x.shape[1], float(slope), int(self_base),
+                                                   _ptr(x), _ld(x), _ptr(scores), _ld(scores), _ptr(out), _ld(out),
+                                                   _ptr(stats), _ld(stats), _stream()),
+              "roc_sg_attn_forward_planned_bf16")
+        return out, stats
+
     def attn_backward(self, x, scores, out, stats, gy, heads=1, slope=0.2, self_base=0, in_grad=None,
                       score_grad=None):
         """Its backward -> (in_grad [Nloc][H], score_grad [Nloc][2*heads] = d s_dst | d s_src).  x, scores, out, stats
@@ -143,6 +164,19 @@ class SgPlan:
               "roc_sg_attn_backward_planned")
         return in_grad, score_grad
 
+    def attn_backward_bf16(self, x, scores, out, stats, gy, heads=1, slope=0.2, self_base=0, in_grad=None,
+                           score_grad=None):
+        """roc_sg_attn_backward_planned_bf16: attn_backward() with bf16 feature rows x (16-byte aligned, ld a multiple of 8, as bf16_padded makes them)."""
+        assert x.dtype == torch.bfloat16
+        in_grad = self._rows(x) if in_grad is None else in_grad
+        score_grad = torch.empty((self.nloc, 2 * heads), device=x.device) if score_grad is None else score_grad
+        check(lib.roc_sg_attn_backward_planned_bf16(self.handle, int(heads), x.shape[1], float(slope), int(self_base),
+                                                    _ptr(x), _ld(x), _ptr(scores), _ld(scores), _ptr(out), _ld(out),
+                                                    _ptr(stats), _ld(stats), _ptr(gy), _ld(gy), _ptr(in_grad),
+                                                    _ld(in_grad), _ptr(score_grad), _ld(score_grad), _stream()),
+              "roc_sg_attn_backward_planned_bf16")
+        return in_grad, score_grad
+
     def weighted_forward(self, x, w, out=None):
         """Edge-weighted sum: out[r] = sum over row r's edges e of w[e - col_left] * x[col[e]]; w is a flat fp32 array in
         the plan's edge order, x is indexed like forward's input."""
@@ -153,6 +187,14 @@ class SgPlan:
                                                   _stream()), "roc_sg_weighted_forward_planned")
         return out
 
+    def weighted_forward_bf16(self, x, w, out=None):
+        """roc_sg_weighted_forward_planned_bf16: weighted_forward() over bf16 rows (16-byte aligned, ld a multiple of 8, as bf16_padded makes them)."""
+        assert x.dtype == torch.bfloat16
+        out = self._rows(x) if out is None else out
+        check(lib.roc_sg_weighted_forward_planned_bf16(self.handle, x.shape[1], _ptr(x), _ld(x), _ptr(w), _ptr(out),
+                                                       _ld(out), _stream()), "roc_sg_weighted_forward_planned_bf16")
+        return out
+
     def edge_dot(self, gy, x, dw=None, accumulate=False):
         """Gradient of weighted_forward's weights: dw[e - col_left] (+)= gy[r] . x[col[e]] for every edge e of row r;
         gy has the plan's rows, x is indexed like the forward's input."""
@@ -160,6 +202,14 @@ class SgPlan:
             dw = torch.empty(max(self.num_edges(), 1), device=gy.device)
         check(lib.roc_sg_edge_dot_planned(self.handle, gy.shape[1], _ptr(gy), _ld(gy), _ptr(x), _ld(x), _ptr(dw),
                                           int(bool(accumulate)), _stream()), "roc_sg_edge_dot_planned")
+        return dw
+
+    def edge_dot_bf16(self, gy, x, dw=None, accumulate=False):
+        """roc_sg_edge_dot_planned_bf16: edge_dot() with bf16 rows x (16-byte aligned, ld a multiple of 8, as bf16_padded makes them)."""
+        assert x.dtype == torch.bfloat16
+        dw = torch.empty(max(self.num_edges(), 1), device=gy.device) if dw is None else dw
+        check(lib.roc_sg_edge_dot_planned_bf16(self.handle, gy.shape[1], _ptr(gy), _ld(gy), _ptr(x), _ld(x), _ptr(dw),
+                                               int(bool(accumulate)), _stream()), "roc_sg_edge_dot_planned_bf16")
         return dw
 
     def num_edges(self):
@@ -247,6 +297,18 @@ class SgTranspose:
                                              _ld(score_grad), _stream()), "roc_sg_attn_backward_exact")
         return in_grad, score_grad
 
+    def attn_backward_bf16(self, plan, x, scores, out, stats, gy, heads=1, slope=0.2, in_grad=None, score_grad=None):
+        """roc_sg_attn_backward_exact_bf16: attn_backward() with bf16 feature rows x (16-byte aligned, ld a multiple of 8, as bf16_padded makes them)."""
+        assert x.dtype == torch.bfloat16
+        in_grad = self._rows(x) if in_grad is None else in_grad
+        score_grad = torch.empty((self.n, 2 * heads), device=x.device) if score_grad is None else score_grad
+        check(lib.roc_sg_attn_backward_exact_bf16(plan.handle, self.handle, int(heads), x.shape[1], float(slope),
+                                                  _ptr(x), _ld(x), _ptr(scores), _ld(scores), _ptr(out), _ld(out),
+                                                  _ptr(stats), _ld(stats), _ptr(gy), _ld(gy), _ptr(in_grad),
+                                                  _ld(in_grad), _ptr(score_grad), _ld(score_grad), _stream()),
+              "roc_sg_attn_backward_exact_bf16")
+        return in_grad, score_grad
+
     def info(self):
         """Copies of the transposed CSR: {"row_end": int64 [N], "col": int32 [E], "perm": int32 [E]} (the uint32 /
         uint64 bits in signed storage) on the device."""
@@ -328,6 +390,25 @@ def activation_bwd(y, dy, mode, dx=None):
         dx = torch.empty_like(y)
     check(lib.roc_activation_bwd(y.shape[0], y.shape[1], mode, _ptr(y), _ld(y), _ptr(dy), _ld(dy), _ptr(dx), _ld(dx),
                                  int(acc), _stream()))
+    return dx
+
+
+def activation_fwd_y_bf16(x, mode=_lib.AC_MODE_RELU, out=None):
+    """roc_activation_fwd_y_bf16: relu of fp32 x stored as bf16 (bf16_padded rows unless `out` is given)."""
+    if out is None:
+        out = bf16_padded(x.shape[0], x.shape[1], x.device)
+    check(lib.roc_activation_fwd_y_bf16(x.shape[0], x.shape[1], int(mode), _ptr(x), _ld(x), _ptr(out), _ld(out),
+                                        _stream()), "roc_activation_fwd_y_bf16")
+    return out
+
+
+def activation_bwd_y_bf16(y, dy, mode=_lib.AC_MODE_RELU, dx=None):
+    """roc_activation_bwd_y_bf16: activation_bwd() with the relu mask read from a bf16 y."""
+    acc = dx is not None
+    if dx is None:
+        dx = torch.empty_like(dy)
+    check(lib.roc_activation_bwd_y_bf16(y.shape[0], y.shape[1], int(mode), _ptr(y), _ld(y), _ptr(dy), _ld(dy),
+                                        _ptr(dx), _ld(dx), int(acc), _stream()), "roc_activation_bwd_y_bf16")
     return dx
 
 

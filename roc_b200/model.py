@@ -165,9 +165,12 @@ class Model:
 
     def set_bf16_aggregation(self, on=True):
         """Store in bf16 each tensor that a Linear without activation writes (its output, or the indegree_norm fused
-        into it) and that one sum scatter_gather alone reads: the Linear rounds as it stores, the scatter_gather
-        gathers half-width rows and accumulates in fp32.  Gradients and every other tensor stay fp32; tensor_dtype()
-        shows which tensors init() chose.  Call before init().  One partition only."""
+        into it) and that one sum scatter_gather alone reads; and each tensor that a Linear without activation or an
+        unfused relu writes, that a max / min, weighted or attention aggregation reads as its features, and that
+        nothing else reads but those and Linears taking it as X without a fused dropout.  The producer rounds as it
+        stores (a relu's backward masks by the stored value), the aggregations read half-width rows and compute in
+        fp32.  Gradients and every other tensor stay fp32; tensor_dtype() shows which tensors init() chose.  Call
+        before init().  One partition only."""
         check(lib.roc_host_set_bf16_aggregation(self.h, int(bool(on))))
 
     def init(self):
@@ -331,7 +334,7 @@ def build_gcn(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exact_bac
     build_sage_mean, build_sage_pool and build_gat.  features="bfloat16" keeps the input features in bf16
     (Model.create_node_tensor); the same keyword on every builder.  aggregation="bfloat16" stores the fused
     linear -> indegree_norm output each scatter_gather reads in bf16 (Model.set_bf16_aggregation); the same keyword
-    on build_sage_mean."""
+    on every builder."""
     L = len(layers)
     x = _input_tensor(model, layers[0], features)
     label = model.create_node_tensor(layers[-1])
@@ -401,7 +404,7 @@ def build_sage_mean(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exa
 
 
 def build_sage_pool(model, layers, dropout_rate, aggr=_lib.AGGR_MAX, lr=0.01, weight_decay=0.05, exact_backward=False,
-                    features="float32"):
+                    features="float32", aggregation="float32"):
     """GraphSAGE with the pooling aggregator (Hamilton et al., 2017) composed from the reference's ops plus the max
     (or min) ScatterGather.  The reference's Linear has no bias, so neither has this.  Per layer:
 
@@ -411,7 +414,8 @@ def build_sage_pool(model, layers, dropout_rate, aggr=_lib.AGGR_MAX, lr=0.01, we
         t  = add(linear(nb, d_i), linear(d, d_i))      # neighbour weight + root / self weight
         t  = relu(t)                                   # all but the last layer
 
-    Single partition; init refuses a graph with a duplicate edge in a row.  Returns the handles, with `pools`
+    Single partition; init refuses a graph with a duplicate edge in a row.  aggregation="bfloat16" stores p, the relu
+    output the scatter_gather reads, in bf16 (Model.set_bf16_aggregation).  Returns the handles, with `pools`
     (the scatter_gather outputs, for get_aggr_index) and `pool_ins` (their inputs)."""
     L = len(layers)
     x = _input_tensor(model, layers[0], features)
@@ -433,13 +437,14 @@ def build_sage_pool(model, layers, dropout_rate, aggr=_lib.AGGR_MAX, lr=0.01, we
     model.adam(lr, weight_decay)
     if exact_backward:
         model.set_exact_backward(True)
+    _aggregation(model, aggregation)
     model.init()
     return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs, "pools": pools,
             "pool_ins": pool_ins}
 
 
 def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01, weight_decay=0.05,
-              exact_backward=False, features="float32"):
+              exact_backward=False, features="float32", aggregation="float32"):
     """GAT (Velickovic et al., 2018) built from the reference's ops plus attention_gather.  `heads` (an int, or one
     value per hidden layer) applies to the hidden layers; the last layer has one head.  layers[i] is the width of
     layer i's output, heads_i * F_i.  Per layer:
@@ -452,8 +457,9 @@ def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01,
 
     Where this differs from the paper: there is no bias (the reference's Linear has none); ReLU replaces ELU (the
     engine has no ELU); with heads > 1 each head's scores are a dense projection of all heads' features, where the
-    paper uses a per-head block.  With one head it is GAT exactly.  Single partition.  Returns the handles, with
-    `attn` (the attention_gather outputs), `attn_ins` (their feature inputs) and `scores`."""
+    paper uses a per-head block.  With one head it is GAT exactly.  Single partition.  aggregation="bfloat16" stores
+    wh, which the attention_gather and the score linear read, in bf16 (Model.set_bf16_aggregation).  Returns the
+    handles, with `attn` (the attention_gather outputs), `attn_ins` (their feature inputs) and `scores`."""
     L = len(layers)
     hs = list(heads) if isinstance(heads, (list, tuple)) else [int(heads)] * (L - 2)
     assert len(hs) == L - 2, "one head count per hidden layer"
@@ -478,19 +484,21 @@ def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01,
     model.adam(lr, weight_decay)
     if exact_backward:
         model.set_exact_backward(True)
+    _aggregation(model, aggregation)
     model.init()
     return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs, "attn": attn,
             "attn_ins": attn_ins, "scores": scores}
 
 
 def build_gcn_weighted(model, layers, dropout_rate, edge_weights, edge_grad=False, lr=0.01, weight_decay=0.05,
-                       features="float32"):
+                       features="float32", aggregation="float32"):
     """GCN with edge weights (e.g. datasets.gcn_edge_weights, which folds in the symmetric normalisation).  Per layer
 
         t = relu(scatter_gather(linear(dropout(t), layers[i]), weights=e))     # no relu on the last layer
 
     with one edge tensor e shared by every layer.  edge_weights: one fp32 value per edge in CSR order, loaded after
     init().  edge_grad: compute e's gradient in backward (the sum of the layers' contributions).  Single partition.
+    aggregation="bfloat16" stores each linear output the scatter_gather reads in bf16 (Model.set_bf16_aggregation).
     Returns the handles, with `edges` and the aggregations' inputs `sg_ins` and outputs `sg_outs`."""
     L = len(layers)
     x = _input_tensor(model, layers[0], features)
@@ -509,6 +517,7 @@ def build_gcn_weighted(model, layers, dropout_rate, edge_weights, edge_grad=Fals
     model.softmax_cross_entropy(t, label, mask)
     model.adam(lr, weight_decay)
     model.set_edge_grad(e, edge_grad)
+    _aggregation(model, aggregation)
     model.init()
     model.set_tensor(e, np.asarray(edge_weights, dtype=np.float32))
     return {"input": x, "label": label, "mask": mask, "logits": t, "edges": e, "sg_ins": sg_ins, "sg_outs": sg_outs}

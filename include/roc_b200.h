@@ -76,6 +76,15 @@ typedef struct {
   int trainAll, testAll, valAll, trainCorrect, testCorrect, valCorrect;
 } roc_perf_metrics;
 
+/* Metrics of the multi-label sigmoid cross-entropy (roc_sigmoid_xent_bwd), each field indexed by split:
+ * [0] train, [1] val, [2] test (the ROC_MASK_* value of the row).  loss: the sum of the per-element loss over the
+ * split's rows and classes; rows: the split's rows; exact: rows whose C predictions all equal their labels;
+ * tp / fp / fn: true positives, false positives, false negatives over the split's rows and classes. */
+typedef struct {
+  double loss[3];
+  uint64_t rows[3], exact[3], tp[3], fp[3], fn[3];
+} roc_multilabel_metrics;
+
 const char* roc_version(void);
 /* Number of usable CUDA devices (0 if none); never fails. */
 int roc_device_count(void);
@@ -540,6 +549,30 @@ int roc_softmax_xent_bwd_norm(int64_t rows, int C, const float* logits, int64_t 
                               const int32_t* mask, float* grad, int64_t ldG,
                               const roc_eid_t* rowEnd, roc_eid_t colLeft,
                               roc_perf_metrics* perf, roc_stream_t stream);
+
+/* Multi-label sigmoid cross-entropy: loss, gradient and metrics in one pass over logits Z[rows][C] (row pitch ldZ)
+ * with hard labels Y[rows][C] in {0, 1} and the row mask (ROC_MASK_*).
+ *  - Labels are bit-packed: each row holds W = ceil(C / 32) words, bit (c % 32) of word c / 32 is label c, and the
+ *    row pitch is ldB words.
+ *  - Per element the loss is  l = max(z, 0) - z*y + log1p(exp(-|z|))  (torch's binary_cross_entropy_with_logits in its
+ *    stable form), computed in fp32.
+ *  - grad[r][c] = sigmoid(z) - y on rows whose mask is ROC_MASK_TRAIN and 0 on every other row (no averaging, the
+ *    softmax head's convention).  Exactly columns [0, C) of every row are written.
+ *  - A class is predicted positive iff z > 0 (so z = 0 and NaN are negative).
+ *  - With a non-NULL rowEnd the gradient is divided by sqrtf(in-degree) as roc_softmax_xent_bwd_norm does (the
+ *    backward of the InDegreeNorm that produced the logits; rowEnd is rowLeft-relative): bit-identical to the call
+ *    with rowEnd = NULL followed by roc_indegree_norm on the gradient.
+ *  - `metrics` (device, may be NULL) is ACCUMULATED into: zero it first.  Rows with mask ROC_MASK_NONE (or any value
+ *    outside 0..2) count nowhere.  The loss is summed in fp32 over each run of up to 4 consecutive elements of a row,
+ *    then in fp64 into per-block partials that one block adds in block order, so the same call on the same device
+ *    gives the same bits; the counts are exact.  Calls that
+ *    pass `metrics` share one per-device scratch for the partials: do not run two of them at once on different
+ *    streams of one device.
+ * ROC_ERR_INVALID: a NULL logits / labelBits / mask / grad, rows < 0, C < 1, ldZ or ldG < C, ldB < W. */
+int roc_sigmoid_xent_bwd(int64_t rows, int C, const float* logits, int64_t ldZ, const uint32_t* labelBits,
+                         int64_t ldB, const int32_t* mask, float* grad, int64_t ldG,
+                         const roc_eid_t* rowEnd /* NULL: no norm */, roc_eid_t colLeft,
+                         roc_multilabel_metrics* metrics /* may be NULL */, roc_stream_t stream);
 
 /* --------------------------------------------------------------- Linear --- */
 

@@ -207,6 +207,10 @@ public:
    * previous step's value is never kept.  Call it before init() when the op's input needs no gradient of its own. */
   void set_edge_grad(const Tensor& edges, bool on);
   void softmax_cross_entropy(const Tensor& logits, const Tensor& labels, const Tensor& mask);
+  /* Multi-label sigmoid cross-entropy (roc_sigmoid_xent_bwd): labels set by set_multilabels, one 0/1 label per class.
+   * Like the softmax it does nothing in the training forward, and in infer mode its forward runs the kernel for the
+   * metrics only.  Single partition only (exit(1) otherwise). */
+  void sigmoid_cross_entropy(const Tensor& logits, const Tensor& labels, const Tensor& mask);
   Tensor indegree_norm(const Tensor& _input);
   Tensor linear(const Tensor& _input, int outDim, ActiMode activation, Initializer* initializer = NULL);
   Tensor relu(const Tensor& _input);
@@ -243,7 +247,13 @@ public:
   void get_tensor_bf16(const Tensor& t, uint16_t* host) const;
   /* labels as class indices (what load_labels parses, load_task.cu:118-123) */
   void set_labels(const Tensor& label, const int* host_class_idx);
-  roc_perf_metrics last_metrics(void) const;   /* PerfMetrics of the latest softmax pass */
+  /* multi-labels for sigmoid_cross_entropy, bit-packed: ceil(H / 32) words per row (bit c % 32 of word c / 32 is
+   * label c), rows dense.  Only these words travel; the tensor's fp32 data is not used. */
+  void set_multilabels(const Tensor& label, const uint32_t* host_packed_bits);
+  /* PerfMetrics of the latest loss pass (after a sigmoid cross-entropy: its loss[0], rows and exact matches) */
+  roc_perf_metrics last_metrics(void) const;
+  /* the multi-label metrics of the latest sigmoid cross-entropy pass; false before one has run */
+  bool last_multilabel_metrics(roc_multilabel_metrics* out) const;
   void set_fusion(bool on) { fuse = on; }
   /* Opt-in exact backward (off by default) for the sum (and so AGGR_AVG), max / min and attention aggregations on
    * directed graphs: their input gradients run over the graph's transpose (roc_sg_transpose_sum_backward,
@@ -344,7 +354,7 @@ public:
   virtual void backward(const Model& model);
   int reluOut;      /* a relu fused into the forward: its output region, whose grad the backward reads and whose
                        values' mask it applies (-1: none; the backward reads its own output's grad) */
-  bool bwdFused;    /* backward done in another op's epilogue (a Linear's dX or the softmax) */
+  bool bwdFused;    /* backward done in another op's epilogue (a Linear's dX or the loss) */
 };
 
 class Linear : public GnnOp {  /* gnn.h:263-285, linear.cc */
@@ -402,6 +412,17 @@ public:
 class SoftmaxCrossEntropy : public GnnOp {  /* gnn.h:346-363, softmax.cc */
 public:
   SoftmaxCrossEntropy(const Model& model, const Tensor& logits, const Tensor& labels, const Tensor& mask);
+  virtual void init(const Model& model);
+  virtual void forward(const Model& model);
+  virtual void backward(const Model& model);
+public:
+  int epoch_num;
+  int gradOut;      /* >= 0: write the logits' grad / sqrt(deg) into this region's grad (fused norm backward) */
+};
+
+class SigmoidCrossEntropy : public GnnOp {  /* not in the reference: Model::sigmoid_cross_entropy */
+public:
+  SigmoidCrossEntropy(const Model& model, const Tensor& logits, const Tensor& labels, const Tensor& mask);
   virtual void init(const Model& model);
   virtual void forward(const Model& model);
   virtual void backward(const Model& model);

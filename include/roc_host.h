@@ -57,6 +57,9 @@ int roc_host_relu(roc_host* h, int t);
 int roc_host_sigmoid(roc_host* h, int t);
 int roc_host_add(roc_host* h, int a, int b);
 int roc_host_softmax_cross_entropy(roc_host* h, int logits, int labels, int mask);
+/* Model::sigmoid_cross_entropy: the multi-label loss of roc_sigmoid_xent_bwd; labels set by roc_host_set_multilabels.
+ * One partition only. */
+int roc_host_sigmoid_cross_entropy(roc_host* h, int logits, int labels, int mask);
 /* AdamOptimizer(&model, lr) + set_weight_decay; call after all linear() calls. */
 int roc_host_adam(roc_host* h, double lr, double weight_decay);
 int roc_host_set_lr(roc_host* h, double lr);
@@ -78,6 +81,9 @@ int roc_host_get_tensor(roc_host* h, int t, void* host, int grad);
 int roc_host_set_tensor_bf16(roc_host* h, int t, const uint16_t* host);   /* raw bf16 bits, rows x hidden */
 int roc_host_get_tensor_bf16(roc_host* h, int t, uint16_t* host);
 int roc_host_set_labels(roc_host* h, int t, const int32_t* host_class_idx);
+/* multi-labels of a [rows][C] label tensor, bit-packed as roc_sigmoid_xent_bwd takes them: ceil(C / 32) words per
+ * row, dense (Model::set_multilabels) */
+int roc_host_set_multilabels(roc_host* h, int t, const uint32_t* host_packed_bits);
 /* the source ids a max / min scatter_gather output t was taken from, [rows][hidden] u32 (Model::get_aggr_index) */
 int roc_host_get_aggr_index(roc_host* h, int t, uint32_t* host);
 int roc_host_tensor_shape(roc_host* h, int t, int64_t out[3]);   /* rows, hidden, ld */
@@ -108,10 +114,11 @@ int roc_host_set_parameter(roc_host* h, int p, const float* host);
 #define ROC_HOST_OP_ADD 9
 #define ROC_HOST_OP_DROPOUT 10
 #define ROC_HOST_OP_SOFTMAX_CROSS_ENTROPY 11
+#define ROC_HOST_OP_SIGMOID_CROSS_ENTROPY 12
 struct roc_host_op_info {   /* a struct tag only: roc_host_op_info is also the function's name */
   int kind;          /* ROC_HOST_OP_* */
   int fusedInto;     /* >= 0: the layer whose kernel does this op's forward */
-  int bwdFused;      /* norm: its backward is done by a Linear's dX epilogue or by the softmax */
+  int bwdFused;      /* norm: its backward is done by a Linear's dX epilogue or by the loss */
   int epilogue;      /* sum ScatterGather: ROC_SG_EPI_* of the forward store */
   int bwdEpilogue;   /*   ... and of the backward store */
   int fwdOut;        /*   the tensor the forward writes (-1: its own output); also a Linear's */
@@ -121,7 +128,8 @@ struct roc_host_op_info {   /* a struct tag only: roc_host_op_info is also the f
   int dxOut;         /*   the tensor whose gradient dX goes to (-1: its input's) */
   int dxReluOf;      /*   the tensor whose relu mask the dX epilogue applies (-1: none) */
   int dxNorm;        /*   the dX epilogue divides by sqrt(in-degree) */
-  int gradOut;       /* softmax: the tensor whose gradient it writes, divided by sqrt(in-degree) (-1: the logits') */
+  int gradOut;       /* softmax or sigmoid cross-entropy: the tensor whose gradient it writes, divided by
+                        sqrt(in-degree) (-1: the logits') */
 };
 int roc_host_num_ops(roc_host* h);
 int roc_host_op_info(roc_host* h, int layer, struct roc_host_op_info* out);
@@ -135,7 +143,11 @@ int roc_host_backward(roc_host* h);
 int roc_host_update(roc_host* h);
 /* one full training epoch: zero_gradients; forward; backward; update */
 int roc_host_train_epoch(roc_host* h);
+/* PerfMetrics of the last loss pass.  After a sigmoid cross-entropy: trainLoss = (float)loss[0], *All = rows,
+ * *Correct = exact (subset accuracy) of its roc_multilabel_metrics. */
 int roc_host_metrics(roc_host* h, roc_perf_metrics* out);
+/* The roc_multilabel_metrics of the last sigmoid cross-entropy pass; ROC_ERR_INVALID before that loss has run. */
+int roc_host_multilabel_metrics(roc_host* h, roc_multilabel_metrics* out);
 /* Per-launch device time of the ScatterGather kernels (CUDA events on the host's
  * stream around each roc_sg_forward_planned): enable, run steps, read {H, ms}. */
 int roc_host_profile_sg(roc_host* h, int on);

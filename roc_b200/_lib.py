@@ -77,9 +77,18 @@ class PerfMetrics(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+class MultilabelMetrics(C.Structure):
+    """roc_multilabel_metrics (include/roc_b200.h): each field indexed [0] train, [1] val, [2] test."""
+    _fields_ = [("loss", C.c_double * 3), ("rows", C.c_uint64 * 3), ("exact", C.c_uint64 * 3),
+                ("tp", C.c_uint64 * 3), ("fp", C.c_uint64 * 3), ("fn", C.c_uint64 * 3)]
+
+    def as_dict(self):
+        return {k: list(getattr(self, k)) for k, _ in self._fields_}
+
+
 HOST_OPS = ("linear", "indegree_norm", "scatter_gather", "scatter_gather_max", "scatter_gather_min",
             "scatter_gather_weighted", "attention_gather", "relu", "sigmoid", "add", "dropout",
-            "softmax_cross_entropy")                       # ROC_HOST_OP_* by value
+            "softmax_cross_entropy", "sigmoid_cross_entropy")   # ROC_HOST_OP_* by value
 
 
 class HostOpInfo(C.Structure):
@@ -176,6 +185,7 @@ PROTOTYPES = {
     "roc_softmax_xent_bwd": (i32, [i64, i32, vp, i64, vp, i64, vp, vp, i64, vp, vp]),
     "roc_softmax_xent_bwd_idx": (i32, [i64, i32, vp, i64, vp, vp, vp, i64, vp, vp]),
     "roc_softmax_xent_bwd_norm": (i32, [i64, i32, vp, i64, vp, i64, vp, vp, vp, i64, vp, u64, vp, vp]),
+    "roc_sigmoid_xent_bwd": (i32, [i64, i32, vp, i64, vp, i64, vp, vp, i64, vp, u64, vp, vp]),
     "roc_linear_bwd_fused": (i32, [vp, vp]),
     "roc_linear_fwd": (i32, [i64, i32, i32, vp, i64, vp, vp, i64, i32, i32, vp, u64, vp]),
     "roc_linear_bwd_workspace_bytes": (sz, [i64, i32, i32]),
@@ -221,6 +231,7 @@ PROTOTYPES = {
     "roc_host_sigmoid": (i32, [vp, i32]),
     "roc_host_add": (i32, [vp, i32, i32]),
     "roc_host_softmax_cross_entropy": (i32, [vp, i32, i32, i32]),
+    "roc_host_sigmoid_cross_entropy": (i32, [vp, i32, i32, i32]),
     "roc_host_adam": (i32, [vp, f64, f64]),
     "roc_host_set_lr": (i32, [vp, f64]),
     "roc_host_get_lr": (f64, [vp]),
@@ -237,6 +248,7 @@ PROTOTYPES = {
     "roc_host_set_tensor_bf16": (i32, [vp, i32, vp]),
     "roc_host_get_tensor_bf16": (i32, [vp, i32, vp]),
     "roc_host_set_labels": (i32, [vp, i32, vp]),
+    "roc_host_set_multilabels": (i32, [vp, i32, vp]),
     "roc_host_tensor_shape": (i32, [vp, i32, vp]),
     "roc_host_tensor_ptr": (vp, [vp, i32, i32]),
     "roc_host_tensor_dtype": (i32, [vp, i32]),
@@ -254,6 +266,7 @@ PROTOTYPES = {
     "roc_host_update": (i32, [vp]),
     "roc_host_train_epoch": (i32, [vp]),
     "roc_host_metrics": (i32, [vp, vp]),
+    "roc_host_multilabel_metrics": (i32, [vp, C.POINTER(MultilabelMetrics)]),
     "roc_host_profile_sg": (i32, [vp, i32]),
     "roc_host_profile_sg_read": (i32, [vp, i32, vp, vp]),
 }

@@ -466,6 +466,182 @@ static void launch_softmax(int64_t rows, int C, const float* logits, int64_t ldZ
   }
 }
 
+// ------------------------------------------ multi-label sigmoid + loss + grad ---
+// Nothing reduces across a row but the exact-match flag, so the kernel streams: a row is LR lanes wide (the smallest
+// power of two covering its VEC-wide chunks, at most 32, so a warp takes 32 / LR rows when C is small) and lane lr
+// takes chunks lr, lr + LR, ...  A chunk of 4 columns never straddles a label word, so each chunk reads one word.
+// Per element: one expf shared by the loss and the sigmoid; the loss of a chunk's (up to 4) elements is summed in fp32,
+// the predictions and labels compared as bit masks.  Metrics: per-thread fp64 loss and u32 counts per split
+// (in shared memory, one column per thread), a fixed-order block reduce into the block's slot of g_mlPartial, and the block that finishes last adds the slots in
+// block order into *metrics (no float atomics: the loss has the same bits run to run).
+constexpr int ML_T = 256;
+constexpr int ML_MAX_BLOCKS = 4096;
+constexpr int ML_FIELDS = 18;   // roc_multilabel_metrics: 3 doubles (loss), then 15 u64 (rows, exact, tp, fp, fn)
+__device__ roc_multilabel_metrics g_mlPartial[ML_MAX_BLOCKS];
+__device__ unsigned int g_mlTicket;
+
+template <int VEC, int LR>
+__global__ void __launch_bounds__(ML_T, 4)
+k_sigmoid_xent(int64_t rows, int C, const float* __restrict__ z, int64_t ldz, const uint32_t* __restrict__ bits,
+               int64_t ldb, const int32_t* __restrict__ mask, float* __restrict__ g, int64_t ldg,
+               const uint64_t* __restrict__ rowEnd, uint64_t colLeft, roc_multilabel_metrics* metrics) {
+  const int lr = threadIdx.x % LR;
+  const unsigned gmask = (LR == 32) ? 0xffffffffu : (((1u << LR) - 1u) << (((threadIdx.x & 31) / LR) * LR));
+  const int rowsPerBlock = ML_T / LR;
+  const int Q = (C + VEC - 1) / VEC;
+  // this thread's running metrics, kept in shared memory (registers go to the stream): loss and the counts
+  // rows, exact, tp, fp, fn of each split
+  __shared__ double sLossT[3][ML_T];
+  __shared__ uint32_t sCntT[15][ML_T];
+  const int tid = threadIdx.x;
+  if (metrics) {
+#pragma unroll
+    for (int f = 0; f < 3; f++) sLossT[f][tid] = 0.0;
+#pragma unroll
+    for (int f = 0; f < 15; f++) sCntT[f][tid] = 0u;
+  }
+  for (int64_t r = blockIdx.x * (int64_t)rowsPerBlock + threadIdx.x / LR; r < rows;
+       r += (int64_t)gridDim.x * rowsPerBlock) {
+    const int mk = __ldg(mask + r);
+    const bool train = (mk == ROC_MASK_TRAIN);
+    const bool counted = (unsigned)mk < 3u;
+    RowDiv rd = rowdiv_make(1.0f);
+    if (rowEnd) {
+      const uint64_t st = (r == 0) ? colLeft : rowEnd[r - 1];
+      rd = rowdiv_make(sqrtf((float)(uint32_t)(rowEnd[r] - st)));
+    }
+    const float* zr = z + r * ldz;
+    float* gr = g + r * ldg;
+    const uint32_t* br = bits + r * ldb;
+    double rowLoss = 0.0;
+    uint32_t tp = 0, fp = 0, fn = 0;
+    bool exact = true;
+    for (int q = lr; q < Q; q += LR) {
+      const int c0 = q * VEC;
+      const int nv = min(VEC, C - c0);
+      float v[VEC];
+      if (VEC == 4) *reinterpret_cast<float4*>(v) = ld_stream4(reinterpret_cast<const float4*>(zr + c0));
+      else v[0] = zr[c0];
+      const uint32_t word = __ldg(br + (c0 >> 5)) >> (c0 & 31);
+      const uint32_t valid = (1u << nv) - 1u;
+      const uint32_t ybits = word & valid;
+      uint32_t pbits = 0;
+      float chunkLoss = 0.0f;
+      float gv[VEC];
+#pragma unroll
+      for (int k = 0; k < VEC; k++) {
+        const float x = v[k];
+        const bool y = (ybits >> k) & 1u;
+        const float e = expf(-fabsf(x));
+        const float rinv = __frcp_rn(1.0f + e);
+        const float s = (x >= 0.0f) ? rinv : e * rinv;   // sigmoid(x), from the one exp
+        gv[k] = (train && k < nv) ? s - (y ? 1.0f : 0.0f) : 0.0f;
+        // max(z, 0) - z*y is max(-z, 0) when y = 1 and max(z, 0) when y = 0: no cancellation
+        if (counted && k < nv) chunkLoss += relu_nanprop(y ? -x : x) + log1pf(e);
+        pbits |= (x > 0.0f ? 1u : 0u) << k;
+      }
+      if (counted) {
+        pbits &= valid;
+        rowLoss += (double)chunkLoss;
+        tp += __popc(pbits & ybits); fp += __popc(pbits & ~ybits); fn += __popc(~pbits & ybits);
+        exact = exact && (pbits == ybits);
+      }
+      if (VEC == 4) {
+        if (rowEnd) rowdiv4(*reinterpret_cast<float(*)[4]>(gv), rd);   // fused InDegreeNorm backward (== gv / sqrtf(deg))
+        if (nv == 4) st_stream4(reinterpret_cast<float4*>(gr + c0), *reinterpret_cast<float4*>(gv));
+        else
+          for (int k = 0; k < nv; k++) gr[c0 + k] = gv[k];
+      } else {
+        gr[c0] = rowEnd ? rowdiv(gv[0], rd) : gv[0];
+      }
+    }
+    if (metrics && counted) {   // uniform across the row's lanes
+      int ex = exact ? 1 : 0;
+#pragma unroll
+      for (int o = LR / 2; o > 0; o >>= 1) ex &= __shfl_xor_sync(gmask, ex, o, LR);
+      sLossT[mk][tid] += rowLoss;
+      if (lr == 0) { sCntT[mk][tid] += 1u; sCntT[3 + mk][tid] += (uint32_t)ex; }
+      sCntT[6 + mk][tid] += tp; sCntT[9 + mk][tid] += fp; sCntT[12 + mk][tid] += fn;
+    }
+  }
+  if (!metrics) return;
+  // block reduce: warp trees, then the warps in order (the same order every run)
+  __shared__ double sLoss[ML_T / 32][3];
+  __shared__ unsigned long long sCnt[ML_T / 32][15];
+  __shared__ bool sLast;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int f = 0; f < 3; f++) {
+    double a = sLossT[f][tid];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+    if (lane == 0) sLoss[warp][f] = a;
+  }
+#pragma unroll
+  for (int f = 0; f < 15; f++) {
+    unsigned long long a = sCntT[f][tid];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+    if (lane == 0) sCnt[warp][f] = a;
+  }
+  __syncthreads();
+  double* slotL = g_mlPartial[blockIdx.x].loss;
+  unsigned long long* slotC = reinterpret_cast<unsigned long long*>(g_mlPartial[blockIdx.x].rows);
+  if (threadIdx.x < ML_FIELDS) {
+    const int f = threadIdx.x;
+    if (f < 3) {
+      double a = 0.0;
+      for (int w = 0; w < ML_T / 32; w++) a += sLoss[w][f];
+      slotL[f] = a;
+    } else {
+      unsigned long long a = 0;
+      for (int w = 0; w < ML_T / 32; w++) a += sCnt[w][f - 3];
+      slotC[f - 3] = a;
+    }
+    __threadfence();
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) sLast = (atomicAdd(&g_mlTicket, 1u) == gridDim.x - 1);
+  __syncthreads();
+  if (!sLast) return;
+  // the last block: every slot is visible (each writer fenced before taking its ticket); add them in block order
+  if (threadIdx.x < ML_FIELDS) {
+    const int f = threadIdx.x;
+    if (f < 3) {
+      double a = 0.0;
+      for (unsigned b = 0; b < gridDim.x; b++) a += __ldcg(&g_mlPartial[b].loss[f]);
+      metrics->loss[f] += a;
+    } else {
+      unsigned long long a = 0;
+      for (unsigned b = 0; b < gridDim.x; b++)
+        a += __ldcg(reinterpret_cast<const unsigned long long*>(g_mlPartial[b].rows) + (f - 3));
+      reinterpret_cast<unsigned long long*>(metrics->rows)[f - 3] += a;
+    }
+  }
+  if (threadIdx.x == 0) g_mlTicket = 0;   // ready for the next call on this device (stream order)
+}
+
+template <int VEC>
+static void launch_sigmoid_xent(int64_t rows, int C, const float* z, int64_t ldz, const uint32_t* bits, int64_t ldb,
+                                const int32_t* mask, float* g, int64_t ldg, const uint64_t* rowEnd, uint64_t colLeft,
+                                roc_multilabel_metrics* metrics, cudaStream_t st) {
+  const int Q = (C + VEC - 1) / VEC;
+  const int LR = Q <= 1 ? 1 : Q <= 2 ? 2 : Q <= 4 ? 4 : Q <= 8 ? 8 : Q <= 16 ? 16 : 32;
+  const unsigned need = ew_grid(rows * LR, ML_T);
+  const unsigned grid = need < (unsigned)ML_MAX_BLOCKS ? need : (unsigned)ML_MAX_BLOCKS;
+#define ROC_ML_LAUNCH(L) \
+  k_sigmoid_xent<VEC, L><<<grid, ML_T, 0, st>>>(rows, C, z, ldz, bits, ldb, mask, g, ldg, rowEnd, colLeft, metrics)
+  switch (LR) {
+    case 1: ROC_ML_LAUNCH(1); break;
+    case 2: ROC_ML_LAUNCH(2); break;
+    case 4: ROC_ML_LAUNCH(4); break;
+    case 8: ROC_ML_LAUNCH(8); break;
+    case 16: ROC_ML_LAUNCH(16); break;
+    default: ROC_ML_LAUNCH(32); break;
+  }
+#undef ROC_ML_LAUNCH
+}
+
 // ------------------------------------------------------------------ adam -----
 __global__ void __launch_bounds__(EW_T)
 k_adam(int64_t count, float alpha_t, float beta1, float beta2, float wd, float eps,
@@ -763,6 +939,22 @@ extern "C" int roc_softmax_xent_bwd_norm(int64_t rows, int C, const float* logit
   if (rows == 0) return ROC_OK;
   if (labels) launch_softmax<true>(rows, C, logits, ldZ, labels, ldL, nullptr, mask, grad, ldG, perf, rowEnd, colLeft, as_stream(stream));
   else launch_softmax<false>(rows, C, logits, ldZ, nullptr, 0, labelIdx, mask, grad, ldG, perf, rowEnd, colLeft, as_stream(stream));
+  ROC_LAUNCH_CHECK();
+  return ROC_OK;
+}
+
+extern "C" int roc_sigmoid_xent_bwd(int64_t rows, int C, const float* logits, int64_t ldZ, const uint32_t* labelBits,
+                                    int64_t ldB, const int32_t* mask, float* grad, int64_t ldG, const roc_eid_t* rowEnd,
+                                    roc_eid_t colLeft, roc_multilabel_metrics* metrics, roc_stream_t stream) {
+  if (!logits || !labelBits || !mask || !grad || rows < 0 || C < 1 || ldZ < C || ldG < C) return ROC_ERR_INVALID;
+  if (ldB < (C + 31) / 32) return ROC_ERR_INVALID;
+  if (rows == 0) return ROC_OK;
+  cudaStream_t st = as_stream(stream);
+  // float4 rows when both pitches and bases allow (ld % 4 == 0 leaves room for the last chunk's pad columns)
+  if (vec_ok(4, {ldZ, ldG}, {logits, grad}))
+    launch_sigmoid_xent<4>(rows, C, logits, ldZ, labelBits, ldB, mask, grad, ldG, rowEnd, colLeft, metrics, st);
+  else
+    launch_sigmoid_xent<1>(rows, C, logits, ldZ, labelBits, ldB, mask, grad, ldG, rowEnd, colLeft, metrics, st);
   ROC_LAUNCH_CHECK();
   return ROC_OK;
 }

@@ -111,6 +111,10 @@ int roc_host_softmax_cross_entropy(roc_host* h, int logits, int labels, int mask
   h->m().softmax_cross_entropy(h->at(logits), h->at(labels), h->at(mask));
   return 0;
 }
+int roc_host_sigmoid_cross_entropy(roc_host* h, int logits, int labels, int mask) {
+  h->m().sigmoid_cross_entropy(h->at(logits), h->at(labels), h->at(mask));
+  return 0;
+}
 
 int roc_host_adam(roc_host* h, double lr, double weight_decay) {
   h->adam = new AdamOptimizer(&h->m(), lr);
@@ -134,6 +138,10 @@ int roc_host_get_tensor(roc_host* h, int t, void* host, int grad) { h->m().get_t
 int roc_host_set_tensor_bf16(roc_host* h, int t, const uint16_t* host) { h->m().set_tensor_bf16(h->at(t), host); return 0; }
 int roc_host_get_tensor_bf16(roc_host* h, int t, uint16_t* host) { h->m().get_tensor_bf16(h->at(t), host); return 0; }
 int roc_host_set_labels(roc_host* h, int t, const int32_t* cls) { h->m().set_labels(h->at(t), cls); return 0; }
+int roc_host_set_multilabels(roc_host* h, int t, const uint32_t* bits) {
+  h->m().set_multilabels(h->at(t), bits);
+  return 0;
+}
 
 int roc_host_tensor_shape(roc_host* h, int t, int64_t out[3]) {
   TensorImpl& x = h->rt->impl->t(h->at(t).region);
@@ -208,6 +216,8 @@ int roc_host_op_info(roc_host* h, int layer, struct roc_host_op_info* out) {
     r.bwdFused = n->bwdFused ? 1 : 0;
   } else if (const SoftmaxCrossEntropy* s = dynamic_cast<const SoftmaxCrossEntropy*>(op)) {
     r.gradOut = handle(s->gradOut);
+  } else if (const SigmoidCrossEntropy* b = dynamic_cast<const SigmoidCrossEntropy*>(op)) {
+    r.gradOut = handle(b->gradOut);
   }
   *out = r;
   return 0;
@@ -249,5 +259,9 @@ int roc_host_profile_sg_read(roc_host* h, int maxEntries, int* H, float* ms) {
   return n;
 }
 int roc_host_metrics(roc_host* h, roc_perf_metrics* out) { *out = h->m().last_metrics(); return 0; }
+int roc_host_multilabel_metrics(roc_host* h, roc_multilabel_metrics* out) {
+  if (!out) return ROC_ERR_INVALID;
+  return h->m().last_multilabel_metrics(out) ? 0 : ROC_ERR_INVALID;
+}
 
 }  // extern "C"

@@ -45,6 +45,7 @@ struct TensorImpl {
   float* data = nullptr;  // lazily allocated (node tensors)
   float* grad = nullptr;
   int32_t* labelIdx = nullptr;   // compact labels when loaded through load_labels / set_labels
+  uint32_t* labelBits = nullptr; // bit-packed multi-labels (set_multilabels): ceil(H / 32) words per row
   // peer-write halo exchange: this tensor's buffers on the other partitions' GPUs (CUDA IPC mappings, index = part)
   std::vector<float*> peerData, peerGrad;
   bool freshData = false, freshGrad = false;   // the producer already pushed this step's boundary rows
@@ -101,6 +102,9 @@ struct RuntimeImpl {
   roc_sg_transpose* sgTranspose = nullptr;                // the graph's transpose: exact backward, weighted ops
   roc_perf_metrics* d_perf = nullptr;
   roc_perf_metrics h_perf{};
+  roc_multilabel_metrics* d_multilabel = nullptr;   // what the sigmoid cross-entropy accumulates
+  bool multilabelRan = false;   // d_multilabel holds a sigmoid cross-entropy's metrics
+  int lossKind = -1;   // ROC_HOST_OP_* of the loss that ran last (-1: none yet); last_metrics reads its metrics
   uint32_t trainStep = 0;
   // optional per-launch timing of the ScatterGather kernels (bench.py's roofline leg)
   struct SgTiming { int H; cudaEvent_t a, b; };
@@ -140,7 +144,7 @@ inline int64_t round_up8(int64_t x) { return (x + 7) / 8 * 8; }
 
 // an op's ROC_HOST_OP_* kind (roc_host_op_info), and each kind's name in refusals and the per-op trace / profile
 int op_kind(const GnnOp* op);
-extern const char* const opKindNames[ROC_HOST_OP_SOFTMAX_CROSS_ENTROPY + 1];
+extern const char* const opKindNames[ROC_HOST_OP_SIGMOID_CROSS_ENTROPY + 1];
 
 }  // namespace host
 }  // namespace roc

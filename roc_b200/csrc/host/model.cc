@@ -177,6 +177,11 @@ void Model::get_aggr_index(const Tensor& out, uint32_t* host) const {
 void Model::softmax_cross_entropy(const Tensor& logits, const Tensor& labels, const Tensor& mask) {
   layers.push_back(new SoftmaxCrossEntropy(*this, logits, labels, mask));
 }
+void Model::sigmoid_cross_entropy(const Tensor& logits, const Tensor& labels, const Tensor& mask) {
+  if (ctx->numParts > 1)
+    ROC_FATAL("sigmoid_cross_entropy: runs on one partition only (numParts > 1 is not supported)");
+  layers.push_back(new SigmoidCrossEntropy(*this, logits, labels, mask));
+}
 Tensor Model::indegree_norm(const Tensor& _input) {
   GnnOp* op = new InDegreeNorm(*this, _input);
   layers.push_back(op);
@@ -202,9 +207,10 @@ Tensor Model::sigmoid(const Tensor& _input) {
 void Model::train_mode(void) { mode = MD_MODE_TRAIN; }
 void Model::infer_mode(void) { mode = MD_MODE_INFER; }
 
-const char* const roc::host::opKindNames[ROC_HOST_OP_SOFTMAX_CROSS_ENTROPY + 1] = {
+const char* const roc::host::opKindNames[ROC_HOST_OP_SIGMOID_CROSS_ENTROPY + 1] = {
     "linear", "indegree_norm", "scatter_gather", "scatter_gather(max)", "scatter_gather(min)",
-    "scatter_gather(weighted)", "attention_gather", "relu", "sigmoid", "add", "dropout", "softmax_cross_entropy"};
+    "scatter_gather(weighted)", "attention_gather", "relu", "sigmoid", "add", "dropout", "softmax_cross_entropy",
+    "sigmoid_cross_entropy"};
 int roc::host::op_kind(const GnnOp* op) {
   if (const ScatterGather* sg = dynamic_cast<const ScatterGather*>(op))
     return sg->aggr == AGGR_MAX   ? ROC_HOST_OP_SCATTER_GATHER_MAX
@@ -218,6 +224,7 @@ int roc::host::op_kind(const GnnOp* op) {
          : dynamic_cast<const AttentionGather*>(op)       ? ROC_HOST_OP_ATTENTION_GATHER
          : dynamic_cast<const Dropout*>(op)               ? ROC_HOST_OP_DROPOUT
          : dynamic_cast<const SoftmaxCrossEntropy*>(op)   ? ROC_HOST_OP_SOFTMAX_CROSS_ENTROPY
+         : dynamic_cast<const SigmoidCrossEntropy*>(op)   ? ROC_HOST_OP_SIGMOID_CROSS_ENTROPY
                                                           : ROC_HOST_OP_ADD;
 }
 
@@ -460,16 +467,19 @@ static void fuse_dropout_into_linear(const std::vector<GnnOp*>& layers, Wiring& 
 // ---- backward-only fusions into epilogues
 static void fuse_backward_epilogues(RuntimeImpl* rt, const std::vector<GnnOp*>& layers, Wiring& w) {
   for (size_t l = 0; l < layers.size(); l++) {
-    // (a) ... -> indegree_norm -> softmax_cross_entropy: the softmax kernel divides the logits'
-    //     gradient by sqrt(deg) and writes it where the norm's input gradient lives
-    if (SoftmaxCrossEntropy* sce = as<SoftmaxCrossEntropy>(layers[l])) {
-      const int rz = sce->inputs[0].region;
+    // (a) ... -> indegree_norm -> softmax_cross_entropy or sigmoid_cross_entropy: the loss kernel divides the
+    //     logits' gradient by sqrt(deg) and writes it where the norm's input gradient lives
+    int* lossGradOut = nullptr;
+    if (SoftmaxCrossEntropy* sce = as<SoftmaxCrossEntropy>(layers[l])) lossGradOut = &sce->gradOut;
+    else if (SigmoidCrossEntropy* bce = as<SigmoidCrossEntropy>(layers[l])) lossGradOut = &bce->gradOut;
+    if (lossGradOut) {
+      const int rz = layers[l]->inputs[0].region;
       if (!w.producer.count(rz) || w.consumers[rz] != 1) continue;
       InDegreeNorm* n = as<InDegreeNorm>(layers[w.producer[rz]]);
       if (!n || n->bwdFused || n->reluOut >= 0) continue;
       if (n->fusedInto >= 0 && as<Linear>(layers[(size_t)n->fusedInto])) continue;   // handled by the SG epilogue
       if (!rt->t(n->inputs[0].region).requiresGrad) continue;
-      sce->gradOut = n->inputs[0].region;
+      *lossGradOut = n->inputs[0].region;
       n->bwdFused = true;
       continue;
     }
@@ -698,11 +708,40 @@ void Model::set_labels(const Tensor& label, const int* host_class_idx) {
   ROC_CHECK(cudaStreamSynchronize(rt->stream));
 }
 
+void Model::set_multilabels(const Tensor& label, const uint32_t* host_packed_bits) {
+  RuntimeImpl* rt = ctx;
+  TensorImpl& x = rt->t(label.region);
+  const size_t words = (size_t)x.rows * (size_t)((x.H + 31) / 32);
+  if (!x.labelBits) x.labelBits = (uint32_t*)rt->dmalloc((words ? words : 1) * sizeof(uint32_t));
+  ROC_CHECK(cudaMemcpyAsync(x.labelBits, host_packed_bits, words * sizeof(uint32_t), cudaMemcpyHostToDevice, rt->stream));
+  ROC_CHECK(cudaStreamSynchronize(rt->stream));
+}
+
 roc_perf_metrics Model::last_metrics(void) const {
   RuntimeImpl* rt = ctx;
+  roc_multilabel_metrics ml;
+  if (rt->lossKind == ROC_HOST_OP_SIGMOID_CROSS_ENTROPY && last_multilabel_metrics(&ml)) {
+    // the multi-label head's PerfMetrics: its train loss, its rows, and its exact matches (subset accuracy)
+    rt->h_perf.trainLoss = (float)ml.loss[0];
+    rt->h_perf.trainAll = (int)ml.rows[ROC_MASK_TRAIN];
+    rt->h_perf.valAll = (int)ml.rows[ROC_MASK_VAL];
+    rt->h_perf.testAll = (int)ml.rows[ROC_MASK_TEST];
+    rt->h_perf.trainCorrect = (int)ml.exact[ROC_MASK_TRAIN];
+    rt->h_perf.valCorrect = (int)ml.exact[ROC_MASK_VAL];
+    rt->h_perf.testCorrect = (int)ml.exact[ROC_MASK_TEST];
+    return rt->h_perf;
+  }
   ROC_CHECK(cudaMemcpyAsync(&rt->h_perf, rt->d_perf, sizeof(roc_perf_metrics), cudaMemcpyDeviceToHost, rt->stream));
   ROC_CHECK(cudaStreamSynchronize(rt->stream));
   return rt->h_perf;
+}
+
+bool Model::last_multilabel_metrics(roc_multilabel_metrics* out) const {
+  RuntimeImpl* rt = ctx;
+  if (!rt->multilabelRan) return false;
+  ROC_CHECK(cudaMemcpyAsync(out, rt->d_multilabel, sizeof(roc_multilabel_metrics), cudaMemcpyDeviceToHost, rt->stream));
+  ROC_CHECK(cudaStreamSynchronize(rt->stream));
+  return true;
 }
 
 // ---- dataset loaders: load_task.cu:25-199 (formats in SURVEY Appendix C) ----
@@ -1419,6 +1458,30 @@ void Dropout::backward(const Model& model) {
                             rt->grad(inputs[0].region), rt->t(inputs[0].region).ld, rt->stream));
 }
 
+// The [INFER] line of softmax_kernel.cu:141-152 (printed once per partition, quirk Q20), to stderr AND stdout, as the
+// reference does (scripts scrape either).  With the multi-label metrics a second line gives each split's micro-F1.
+static void print_infer(int epoch, const roc_perf_metrics& p, const roc_multilabel_metrics* ml) {
+  FILE* sinks[2] = {stderr, stdout};
+  for (FILE* f : sinks) {
+    fprintf(f,
+            "\t[INFER][%d] train_loss: %.4lf  train_accuracy: %.2lf%%(%d/%d)  val_accuracy: %.2lf%%(%d/%d)  "
+            "test_accuracy: %.2lf%%(%d/%d)\n",
+            epoch, p.trainLoss, p.trainCorrect * 100.0f / p.trainAll, p.trainCorrect, p.trainAll,
+            p.valCorrect * 100.0f / p.valAll, p.valCorrect, p.valAll, p.testCorrect * 100.0f / p.testAll,
+            p.testCorrect, p.testAll);
+    if (ml) {
+      double f1[3];
+      for (int s = 0; s < 3; s++) {
+        const double d = 2.0 * (double)ml->tp[s] + (double)ml->fp[s] + (double)ml->fn[s];
+        f1[s] = d > 0 ? 2.0 * (double)ml->tp[s] / d : NAN;
+      }
+      fprintf(f, "\t[INFER][%d] train_micro_f1: %.4lf  val_micro_f1: %.4lf  test_micro_f1: %.4lf\n", epoch, f1[0],
+              f1[1], f1[2]);
+    }
+  }
+  fflush(stdout);
+}
+
 // ---------------------------------------------------- SoftmaxCrossEntropy ---
 SoftmaxCrossEntropy::SoftmaxCrossEntropy(const Model&, const Tensor& _logit, const Tensor& _label, const Tensor& _mask)
     : GnnOp(_logit, _label, _mask), epoch_num(0), gradOut(-1) {
@@ -1444,6 +1507,10 @@ void SoftmaxCrossEntropy::backward(const Model& model) {
   ROC_ASSERT(inputs[2].region >= 0);   // softmax_kernel.cu:157-160: masks are required
   const int C = (int)inputs[0].dims[0];
   TensorImpl& lab = rt->t(inputs[1].region);
+  if (lab.labelBits)
+    ROC_FATAL("softmax_cross_entropy: the label tensor holds multi-labels (set_multilabels); the softmax takes one "
+              "class per row (set_labels / set_tensor)");
+  rt->lossKind = ROC_HOST_OP_SOFTMAX_CROSS_ENTROPY;
   ROC_CHECK(cudaMemsetAsync(rt->d_perf, 0, sizeof(roc_perf_metrics), rt->stream));
   const int32_t* mask = reinterpret_cast<const int32_t*>(rt->data(inputs[2].region));
   if (gradOut >= 0) {
@@ -1473,19 +1540,46 @@ void SoftmaxCrossEntropy::backward(const Model& model) {
                                    rt->data(inputs[1].region), lab.ld, mask, rt->grad(inputs[0].region),
                                    rt->t(inputs[0].region).ld, rt->d_perf, rt->stream));
   }
+  if (mode == MD_MODE_INFER && model.printMetrics) print_infer(epoch_num, model.last_metrics(), nullptr);
+}
+
+// ---------------------------------------------------- SigmoidCrossEntropy ---
+SigmoidCrossEntropy::SigmoidCrossEntropy(const Model&, const Tensor& _logit, const Tensor& _label, const Tensor& _mask)
+    : GnnOp(_logit, _label, _mask), epoch_num(0), gradOut(-1) {
+  ROC_ASSERT(_logit.numDim == 2);
+  ROC_ASSERT(_label.numDim == 2);
+  if (_label.dims[0] != _logit.dims[0])
+    ROC_FATAL("sigmoid_cross_entropy: the label tensor's width (classes) differs from the logits'");
+  ROC_ASSERT(_label.dims[1] == _logit.dims[1]);
+  numOutputs = 0;
+}
+void SigmoidCrossEntropy::init(const Model&) {}
+void SigmoidCrossEntropy::forward(const Model& model) {
+  mode = model.mode;
+  if (model.mode == MD_MODE_INFER) backward(model);   // as the softmax: nothing in training, metrics in inference
+}
+void SigmoidCrossEntropy::backward(const Model& model) {
+  RuntimeImpl* rt = model.ctx;
+  mode = model.mode;
+  if (mode == MD_MODE_TRAIN) epoch_num++;
+  ROC_ASSERT(inputs[2].region >= 0);   // masks are required
+  const int C = (int)inputs[0].dims[0];
+  const TensorImpl& lab = rt->t(inputs[1].region);
+  if (!lab.labelBits)
+    ROC_FATAL("sigmoid_cross_entropy: the label tensor has no multi-labels (set them with set_multilabels)");
+  rt->lossKind = ROC_HOST_OP_SIGMOID_CROSS_ENTROPY;
+  ROC_CHECK(cudaMemsetAsync(rt->d_multilabel, 0, sizeof(roc_multilabel_metrics), rt->stream));
+  // one partition: the fused norm backward divides by the in-degree of the whole CSR (rowEnd from colLeft)
+  const int rg = gradOut >= 0 ? gradOut : inputs[0].region;
+  ROC_CHECK(roc_sigmoid_xent_bwd(model.local_rows(), C, rt->data(inputs[0].region), rt->t(inputs[0].region).ld,
+                                 lab.labelBits, (C + 31) / 32, reinterpret_cast<const int32_t*>(rt->data(inputs[2].region)),
+                                 rt->grad(rg), rt->t(rg).ld, gradOut >= 0 ? model.myGraph.d_rowEnd : NULL,
+                                 model.myGraph.colLeft, rt->d_multilabel, rt->stream));
+  rt->multilabelRan = true;
   if (mode == MD_MODE_INFER && model.printMetrics) {
-    roc_perf_metrics p = model.last_metrics();
-    // softmax_kernel.cu:141-152 (printed once per partition, quirk Q20)
-    // to stderr AND stdout, as the reference does (scripts scrape either)
-    FILE* sinks[2] = {stderr, stdout};
-    for (FILE* f : sinks)
-      fprintf(f,
-              "\t[INFER][%d] train_loss: %.4lf  train_accuracy: %.2lf%%(%d/%d)  val_accuracy: %.2lf%%(%d/%d)  "
-              "test_accuracy: %.2lf%%(%d/%d)\n",
-              epoch_num, p.trainLoss, p.trainCorrect * 100.0f / p.trainAll, p.trainCorrect, p.trainAll,
-              p.valCorrect * 100.0f / p.valAll, p.valCorrect, p.valAll, p.testCorrect * 100.0f / p.testAll,
-              p.testCorrect, p.testAll);
-    fflush(stdout);
+    roc_multilabel_metrics ml;
+    model.last_multilabel_metrics(&ml);
+    print_infer(epoch_num, model.last_metrics(), &ml);
   }
 }
 

@@ -400,6 +400,8 @@ Runtime::Runtime(int device, int myPart, int numParts) {
   }
   impl->d_perf = (roc_perf_metrics*)impl->dmalloc(sizeof(roc_perf_metrics));
   ROC_CHECK(cudaMemsetAsync(impl->d_perf, 0, sizeof(roc_perf_metrics), impl->stream));
+  impl->d_multilabel = (roc_multilabel_metrics*)impl->dmalloc(sizeof(roc_multilabel_metrics));
+  ROC_CHECK(cudaMemsetAsync(impl->d_multilabel, 0, sizeof(roc_multilabel_metrics), impl->stream));
 }
 
 Runtime::~Runtime() {

@@ -93,6 +93,25 @@ def node_data(n, in_dim, num_classes, seed=1, device="cpu"):
     return feats, labels, mask
 
 
+def multilabel_node_data(n, in_dim, num_labels, seed=1, device="cpu", positive_rate=0.1):
+    """Multi-label node data a model can learn: features ~ U(-1,1) fp32; labels y = (x @ R + noise > tau) as uint8
+    [n][num_labels] 0/1, with R and the noise drawn from the seed and tau the (1 - positive_rate) quantile of all
+    scores, so that about positive_rate of the labels are positive; mask 66% Train / 10% Val / 24% Test as node_data."""
+    g = torch.Generator(device=device)
+    g.manual_seed(seed + 11)
+    feats = torch.rand((n, in_dim), generator=g, device=device, dtype=torch.float32) * 2.0 - 1.0
+    r = torch.randn((in_dim, num_labels), generator=g, device=device, dtype=torch.float64) / np.sqrt(in_dim)
+    noise = torch.randn((n, num_labels), generator=g, device=device, dtype=torch.float64) * 0.1
+    score = feats.double() @ r + noise
+    tau = torch.quantile(score.flatten()[: 1 << 24], 1.0 - positive_rate)
+    labels = (score > tau).to(torch.uint8)
+    u = torch.rand(n, generator=g, device=device)
+    mask = torch.full((n,), 2, dtype=torch.int32, device=device)   # MASK_TEST
+    mask[u < 0.76] = 1                                              # MASK_VAL
+    mask[u < 0.66] = 0                                              # MASK_TRAIN
+    return feats, labels, mask
+
+
 def onehot(labels, num_classes):
     labels = np.asarray(labels)
     out = np.zeros((labels.shape[0], num_classes), dtype=np.float32)

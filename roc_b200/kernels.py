@@ -600,6 +600,24 @@ def softmax_xent_bwd_norm(logits, labels, mask, row_end, col_left=0, compact=Fal
     return (g, _perf_dict(perf)) if with_perf else g
 
 
+def sigmoid_xent_bwd(logits, labels_bits, mask, row_end=None, col_left=0, with_metrics=False, out=None):
+    """roc_sigmoid_xent_bwd: the multi-label sigmoid cross-entropy's gradient (sigmoid(z) - y on train rows, 0 on the
+    rest), divided by sqrt(deg) when row_end is given (the logits' InDegreeNorm backward).  labels_bits: int32 or
+    uint32-valued [N][W >= ceil(C / 32)] bit-packed labels (model.pack_multilabels).  Returns the gradient, or
+    (gradient, metrics dict as _lib.MultilabelMetrics.as_dict()) with with_metrics=True.  out: the gradient's
+    [N][C] (ld-padded ok) buffer."""
+    g = torch.empty_like(logits) if out is None else out
+    metrics = torch.zeros(18, dtype=torch.float64, device=logits.device) if with_metrics else None
+    check(lib.roc_sigmoid_xent_bwd(logits.shape[0], logits.shape[1], _ptr(logits), _ld(logits), _ptr(labels_bits),
+                                   _ld(labels_bits), _ptr(mask), _ptr(g), _ld(g), _ptr(row_end), col_left,
+                                   _ptr(metrics), _stream()), "roc_sigmoid_xent_bwd")
+    if not with_metrics:
+        return g
+    raw = metrics.cpu().numpy()
+    m = _lib.MultilabelMetrics.from_buffer_copy(raw.tobytes())
+    return g, m.as_dict()
+
+
 def linear_bwd(x, w, y, dy, dw, dx=None, activation=0, accumulate_dx=False):
     ws_bytes = lib.roc_linear_bwd_workspace_bytes(x.shape[0], x.shape[1], w.shape[0])
     ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=x.device)

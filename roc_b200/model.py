@@ -143,6 +143,11 @@ class Model:
     def softmax_cross_entropy(self, logits, labels, mask):
         check(lib.roc_host_softmax_cross_entropy(self.h, logits, labels, mask))
 
+    def sigmoid_cross_entropy(self, logits, labels, mask):
+        """Multi-label loss: per class, binary cross-entropy on the logit (labels from set_multilabels).  Gradient
+        sigmoid(z) - y on train rows; metrics in multilabel_metrics().  One partition only."""
+        check(lib.roc_host_sigmoid_cross_entropy(self.h, logits, labels, mask))
+
     def adam(self, lr=0.01, weight_decay=0.05):
         check(lib.roc_host_adam(self.h, lr, weight_decay))
 
@@ -244,6 +249,15 @@ class Model:
         a = np.ascontiguousarray(class_idx, dtype=np.int32)
         check(lib.roc_host_set_labels(self.h, t, a.ctypes.data))
 
+    def set_multilabels(self, t, labels):
+        """labels: a [rows][C] 0/1 or bool array for the label tensor t (C = its width), packed here
+        (pack_multilabels) for sigmoid_cross_entropy."""
+        rows, hidden, _ = self.tensor_shape(t)
+        labels = np.asarray(labels)
+        assert labels.shape == (rows, hidden), (labels.shape, rows, hidden)
+        bits = pack_multilabels(labels)
+        check(lib.roc_host_set_multilabels(self.h, t, bits.ctypes.data))
+
     def num_parameters(self):
         return lib.roc_host_num_parameters(self.h)
 
@@ -310,6 +324,33 @@ class Model:
         check(lib.roc_host_metrics(self.h, C.byref(pm)))
         return pm.as_dict()
 
+    def multilabel_metrics(self):
+        """The last sigmoid_cross_entropy pass's metrics: loss, rows, exact, tp, fp, fn (each [train, val, test]) and
+        micro_f1 = 2tp / (2tp + fp + fn) per split (NaN where that denominator is 0)."""
+        mm = _lib.MultilabelMetrics()
+        check(lib.roc_host_multilabel_metrics(self.h, C.byref(mm)), "roc_host_multilabel_metrics")
+        d = mm.as_dict()
+        d["micro_f1"] = [_micro_f1(tp, fp, fn) for tp, fp, fn in zip(d["tp"], d["fp"], d["fn"])]
+        return d
+
+
+def _micro_f1(tp, fp, fn):
+    den = 2 * tp + fp + fn
+    return 2.0 * tp / den if den else float("nan")
+
+
+def pack_multilabels(labels):
+    """[rows][C] 0/1 or bool labels -> uint32 [rows][ceil(C / 32)]: bit c % 32 of word c // 32 is label c (the layout
+    of roc_sigmoid_xent_bwd and Model.set_multilabels)."""
+    y = np.asarray(labels)
+    assert y.ndim == 2, "labels must be [rows][C]"
+    rows, c = y.shape
+    w = (c + 31) // 32
+    padded = np.zeros((rows, w * 32), dtype=np.uint8)
+    padded[:, :c] = y != 0
+    bytes_ = np.packbits(padded.reshape(rows, w * 4, 8), axis=2, bitorder="little").reshape(rows, w * 4)
+    return np.ascontiguousarray(bytes_).view("<u4").astype(np.uint32).reshape(rows, w)
+
 
 def _input_tensor(model, hidden, features):
     """the builders' input features: fp32, or bf16 with features="bfloat16" (the plain call for fp32, so that any object
@@ -327,14 +368,26 @@ def _aggregation(model, aggregation):
         model.set_bf16_aggregation(True)
 
 
+def _loss(model, loss, logits, label, mask):
+    """The builders' head: loss="softmax" (the default) is softmax_cross_entropy with one class per row (set_labels);
+    "sigmoid" is the multi-label sigmoid_cross_entropy (set_multilabels)."""
+    if loss == "softmax":
+        model.softmax_cross_entropy(logits, label, mask)
+    elif loss == "sigmoid":
+        model.sigmoid_cross_entropy(logits, label, mask)
+    else:
+        raise ValueError("loss must be \"softmax\" or \"sigmoid\"")
+
+
 def build_gcn(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exact_backward=False, features="float32",
-              aggregation="float32"):
+              aggregation="float32", loss="softmax"):
     """The model script of gnn.cc:65-98 for `-layers a-b-...-c`.  Returns the handles.  exact_backward: train on the
     exact gradient over the graph's transpose (Model.set_exact_backward), for directed graphs; the same keyword on
     build_sage_mean, build_sage_pool and build_gat.  features="bfloat16" keeps the input features in bf16
     (Model.create_node_tensor); the same keyword on every builder.  aggregation="bfloat16" stores the fused
     linear -> indegree_norm output each scatter_gather reads in bf16 (Model.set_bf16_aggregation); the same keyword
-    on every builder."""
+    on every builder.  loss="sigmoid" ends the model in the multi-label sigmoid_cross_entropy instead of the softmax
+    (labels then go in with Model.set_multilabels); the same keyword on every builder."""
     L = len(layers)
     x = _input_tensor(model, layers[0], features)
     label = model.create_node_tensor(layers[-1])
@@ -354,7 +407,7 @@ def build_gcn(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exact_bac
         if L > 3:   # residual branch, gnn.cc:86-90
             skip = model.linear(skip, layers[i], _lib.AC_MODE_NONE)
             t = model.add(t, skip)
-    model.softmax_cross_entropy(t, label, mask)
+    _loss(model, loss, t, label, mask)
     model.adam(lr, weight_decay)
     if exact_backward:
         model.set_exact_backward(True)
@@ -364,7 +417,7 @@ def build_gcn(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exact_bac
 
 
 def build_sage_mean(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exact_backward=False,
-                    features="float32", aggregation="float32"):
+                    features="float32", aggregation="float32", loss="softmax"):
     """GraphSAGE with the mean aggregator (BASELINE.json configs[2]) composed from the reference's own ops
     (gnn.h:165-179; AGGR_AVG is declared at gnn.h:75-80 but the reference's ScatterGather only sums):
 
@@ -394,7 +447,7 @@ def build_sage_mean(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exa
         if i != L - 1:
             t = model.relu(t)
             relu_outs.append(t)
-    model.softmax_cross_entropy(t, label, mask)
+    _loss(model, loss, t, label, mask)
     model.adam(lr, weight_decay)
     if exact_backward:
         model.set_exact_backward(True)
@@ -404,7 +457,7 @@ def build_sage_mean(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exa
 
 
 def build_sage_pool(model, layers, dropout_rate, aggr=_lib.AGGR_MAX, lr=0.01, weight_decay=0.05, exact_backward=False,
-                    features="float32", aggregation="float32"):
+                    features="float32", aggregation="float32", loss="softmax"):
     """GraphSAGE with the pooling aggregator (Hamilton et al., 2017) composed from the reference's ops plus the max
     (or min) ScatterGather.  The reference's Linear has no bias, so neither has this.  Per layer:
 
@@ -433,7 +486,7 @@ def build_sage_pool(model, layers, dropout_rate, aggr=_lib.AGGR_MAX, lr=0.01, we
         if i != L - 1:
             t = model.relu(t)
             relu_outs.append(t)
-    model.softmax_cross_entropy(t, label, mask)
+    _loss(model, loss, t, label, mask)
     model.adam(lr, weight_decay)
     if exact_backward:
         model.set_exact_backward(True)
@@ -444,7 +497,7 @@ def build_sage_pool(model, layers, dropout_rate, aggr=_lib.AGGR_MAX, lr=0.01, we
 
 
 def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01, weight_decay=0.05,
-              exact_backward=False, features="float32", aggregation="float32"):
+              exact_backward=False, features="float32", aggregation="float32", loss="softmax"):
     """GAT (Velickovic et al., 2018) built from the reference's ops plus attention_gather.  `heads` (an int, or one
     value per hidden layer) applies to the hidden layers; the last layer has one head.  layers[i] is the width of
     layer i's output, heads_i * F_i.  Per layer:
@@ -480,7 +533,7 @@ def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01,
         if i != L - 1:
             t = model.relu(t)
             relu_outs.append(t)
-    model.softmax_cross_entropy(t, label, mask)
+    _loss(model, loss, t, label, mask)
     model.adam(lr, weight_decay)
     if exact_backward:
         model.set_exact_backward(True)
@@ -491,7 +544,7 @@ def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01,
 
 
 def build_gcn_weighted(model, layers, dropout_rate, edge_weights, edge_grad=False, lr=0.01, weight_decay=0.05,
-                       features="float32", aggregation="float32"):
+                       features="float32", aggregation="float32", loss="softmax"):
     """GCN with edge weights (e.g. datasets.gcn_edge_weights, which folds in the symmetric normalisation).  Per layer
 
         t = relu(scatter_gather(linear(dropout(t), layers[i]), weights=e))     # no relu on the last layer
@@ -514,7 +567,7 @@ def build_gcn_weighted(model, layers, dropout_rate, edge_weights, edge_grad=Fals
         sg_outs.append(t)
         if i != L - 1:
             t = model.relu(t)
-    model.softmax_cross_entropy(t, label, mask)
+    _loss(model, loss, t, label, mask)
     model.adam(lr, weight_decay)
     model.set_edge_grad(e, edge_grad)
     _aggregation(model, aggregation)

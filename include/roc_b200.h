@@ -574,6 +574,45 @@ int roc_sigmoid_xent_bwd(int64_t rows, int C, const float* logits, int64_t ldZ, 
                          const roc_eid_t* rowEnd /* NULL: no norm */, roc_eid_t colLeft,
                          roc_multilabel_metrics* metrics /* may be NULL */, roc_stream_t stream);
 
+/* ------------------------------------------------------- batch normalisation --- */
+
+/* Batch normalisation over the rows of X[rows][H] (torch.nn.BatchNorm1d over every row), one forward and one
+ * backward entry.  X, Y, dY and dX rows are read and written as 16-byte groups: their pitches must be multiples of 4
+ * and their bases 16-byte aligned (ROC_ERR_INVALID otherwise).  Columns [H, ld) of a row may be loaded but are never
+ * written, and their values reach no result.
+ *  - Statistics: per column, the mean and the biased variance (divide by rows) from one pass that sums (x - K) and
+ *    (x - K)^2 in fp64 with K = X[0][c], so the variance stays accurate when |mean| >> std.  Rows are summed in fixed
+ *    blocks whose size depends on (rows, H) only, each block's fp64 partial is added in block order, so the same call
+ *    gives the same bits on any device.
+ *  - training != 0: a = gamma * invstd and b = beta - mean * a, invstd = 1 / sqrt(var + eps), computed in fp64 and
+ *    stored in fp32 in saveA / saveB; saveMean / saveInvStd (fp64) keep mean and invstd for the backward.  The running
+ *    statistics (fp32, may both be NULL) become  runMean = (1 - momentum) runMean + momentum mean  and
+ *    runVar = (1 - momentum) runVar + momentum var rows / (rows - 1), computed in fp64.  Needs rows >= 2.
+ *  - training == 0: a and b from runMean / runVar instead (both required), into the workspace; nothing else is
+ *    written but Y.
+ *  - Y = fma(X, a, b) per column, then relu (x > 0 ? x : 0, NaN kept) when relu != 0.
+ * The workspace holds the coefficients and the fp64 partials: roc_batchnorm_workspace_bytes(rows, H), 16-byte aligned.
+ * ROC_ERR_INVALID: a NULL x / gamma / beta / y / workspace, rows < 0, H <= 0, ldX or ldY < H, eps < 0, momentum
+ * outside [0, 1], only one running statistic, a missing save pointer or rows < 2 in training, no running statistics in
+ * inference, a short workspace. */
+size_t roc_batchnorm_workspace_bytes(int64_t rows, int H);
+int roc_batchnorm_fwd(int64_t rows, int H, const float* x, int64_t ldX, const float* gamma, const float* beta,
+                      double eps, double momentum, float* runMean, float* runVar, int training, int relu,
+                      float* y, int64_t ldY, float* saveA, float* saveB, double* saveMean, double* saveInvStd,
+                      void* workspace, size_t workspaceBytes, roc_stream_t stream);
+/* The backward of a training roc_batchnorm_fwd on the same x, gamma and saved values.  With g' = dY, or with relu != 0
+ * dY masked by fma(x, saveA, saveB) > 0 (the forward's own relu test, so no Y is read):
+ *   dBeta = sum_rows g',  dGamma = invstd * sum_rows g' (x - mean)        (fp64 sums as the forward's, stored fp32)
+ *   dX (+)= A g' + B x + C  with  A = gamma invstd,  B = -A invstd dGamma / rows,  C = -A dBeta / rows - B mean
+ * (fp64 coefficients stored in fp32, two fp32 FMAs per element), which is gamma invstd (g' - dBeta / rows -
+ * xhat dGamma / rows).  accumulate selects += over =; dX == NULL computes dGamma and dBeta only.  dGamma and dBeta are
+ * overwritten.  ROC_ERR_INVALID as for the forward, and for rows < 2, a NULL dY / gamma / saved statistics / dGamma /
+ * dBeta, or relu without saveA / saveB. */
+int roc_batchnorm_bwd(int64_t rows, int H, const float* x, int64_t ldX, const float* dY, int64_t ldDY, int relu,
+                      const float* gamma, const float* saveA, const float* saveB, const double* saveMean,
+                      const double* saveInvStd, float* dGamma, float* dBeta, float* dX, int64_t ldDX, int accumulate,
+                      void* workspace, size_t workspaceBytes, roc_stream_t stream);
+
 /* --------------------------------------------------------------- Linear --- */
 
 /* Replaces cublasSgemm in Linear::forward_task, linear_kernel.cu:76-80 (+ the

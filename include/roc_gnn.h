@@ -215,6 +215,12 @@ public:
   Tensor linear(const Tensor& _input, int outDim, ActiMode activation, Initializer* initializer = NULL);
   Tensor relu(const Tensor& _input);
   Tensor sigmoid(const Tensor& _input);
+  /* Batch normalisation over every local row (torch.nn.BatchNorm1d; roc_batchnorm_fwd / roc_batchnorm_bwd).  Appends
+   * two parameters, gamma (filled with 1) then beta (0), each a weight tensor of dims {H, 1}; creating them draws no
+   * random numbers.  A training forward normalises by the batch statistics and updates the running mean (start 0) and
+   * variance (start 1); an infer-mode forward uses the running statistics and updates nothing.  init() refuses a
+   * partition of fewer than 2 rows.  Single partition only (exit(1) otherwise). */
+  Tensor batch_norm(const Tensor& input, float momentum = 0.1f, float eps = 1e-5f);
   /* DT = DATATYPE (fp32), int (masks), or __nv_bfloat16 (<cuda_bf16.h>): a leaf feature matrix stored in bf16, rounded
    * to nearest even, rows of round_up(H, 8) elements.  It never has a gradient and is never an op's output; linear and
    * dropout read it (bit-identical to the same model on an fp32 input holding the widened values), and init() refuses
@@ -274,6 +280,9 @@ public:
   void set_bf16_aggregation(bool on);
   /* the source ids a max / min scatter_gather chose (its `arg`), [rows_local][H] u32; `out` is its output tensor */
   void get_aggr_index(const Tensor& out, uint32_t* host) const;
+  /* the running mean and variance (fp32, H values each) of the batch_norm whose output is `out` */
+  void get_batch_norm_stats(const Tensor& out, float* mean, float* var) const;
+  void set_batch_norm_stats(const Tensor& out, const float* mean, const float* var);
   int64_t local_rows(void) const { return (int64_t)myGraph.rowRight - myGraph.rowLeft + 1; }
 
 public:
@@ -407,6 +416,24 @@ public:
   float rate;
   int seed;
   int opIndex;      /* position in the model: distinguishes the Philox streams of the layers */
+};
+
+class BatchNorm : public GnnOp {  /* not in the reference: Model::batch_norm */
+public:
+  BatchNorm(const Model& model, const Tensor& input, float momentum, float eps);
+  virtual void init(const Model& model);
+  virtual void forward(const Model& model);
+  virtual void backward(const Model& model);
+public:
+  float momentum, eps;
+  Tensor gamma, beta;   /* parameters, dims {H, 1} */
+  int fwdOut;           /* a relu fused into the forward (Model::init): its output region, which the forward writes and
+                           whose gradient the backward reads (-1: none) */
+  /* Runtime arena, H values each: running statistics; a, b of the last training forward; its mean and invstd */
+  float *runMean, *runVar, *saveA, *saveB;
+  double *saveMean, *saveInvStd;
+  void* workspace;      /* roc_batchnorm_workspace_bytes */
+  size_t workspaceBytes;
 };
 
 class SoftmaxCrossEntropy : public GnnOp {  /* gnn.h:346-363, softmax.cc */

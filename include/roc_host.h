@@ -56,6 +56,11 @@ int roc_host_set_edge_grad(roc_host* h, int edges, int on);
 int roc_host_relu(roc_host* h, int t);
 int roc_host_sigmoid(roc_host* h, int t);
 int roc_host_add(roc_host* h, int a, int b);
+/* Model::batch_norm(t, momentum, eps): appends two parameters (gamma, beta).  One partition only. */
+int roc_host_batch_norm(roc_host* h, int t, float momentum, float eps);
+/* the running mean and variance (H floats each) of the batch_norm whose output is t (Model::get / set_batch_norm_stats) */
+int roc_host_get_batch_norm_stats(roc_host* h, int t, float* mean, float* var);
+int roc_host_set_batch_norm_stats(roc_host* h, int t, const float* mean, const float* var);
 int roc_host_softmax_cross_entropy(roc_host* h, int logits, int labels, int mask);
 /* Model::sigmoid_cross_entropy: the multi-label loss of roc_sigmoid_xent_bwd; labels set by roc_host_set_multilabels.
  * One partition only. */
@@ -115,13 +120,15 @@ int roc_host_set_parameter(roc_host* h, int p, const float* host);
 #define ROC_HOST_OP_DROPOUT 10
 #define ROC_HOST_OP_SOFTMAX_CROSS_ENTROPY 11
 #define ROC_HOST_OP_SIGMOID_CROSS_ENTROPY 12
+#define ROC_HOST_OP_BATCH_NORM 13
 struct roc_host_op_info {   /* a struct tag only: roc_host_op_info is also the function's name */
   int kind;          /* ROC_HOST_OP_* */
   int fusedInto;     /* >= 0: the layer whose kernel does this op's forward */
   int bwdFused;      /* norm: its backward is done by a Linear's dX epilogue or by the loss */
   int epilogue;      /* sum ScatterGather: ROC_SG_EPI_* of the forward store */
   int bwdEpilogue;   /*   ... and of the backward store */
-  int fwdOut;        /*   the tensor the forward writes (-1: its own output); also a Linear's */
+  int fwdOut;        /*   the tensor the forward writes (-1: its own output); also a Linear's and a batch_norm's (the
+                        output of the relu fused into it) */
   int bwdOut;        /*   the tensor whose gradient the backward writes (-1: its input's) */
   int flags;         /* Linear: ROC_LINEAR_* of the forward */
   int dropOp;        /*   >= 0: the Dropout layer applied while X is loaded */

@@ -88,7 +88,7 @@ class MultilabelMetrics(C.Structure):
 
 HOST_OPS = ("linear", "indegree_norm", "scatter_gather", "scatter_gather_max", "scatter_gather_min",
             "scatter_gather_weighted", "attention_gather", "relu", "sigmoid", "add", "dropout",
-            "softmax_cross_entropy", "sigmoid_cross_entropy")   # ROC_HOST_OP_* by value
+            "softmax_cross_entropy", "sigmoid_cross_entropy", "batch_norm")   # ROC_HOST_OP_* by value
 
 
 class HostOpInfo(C.Structure):
@@ -186,6 +186,10 @@ PROTOTYPES = {
     "roc_softmax_xent_bwd_idx": (i32, [i64, i32, vp, i64, vp, vp, vp, i64, vp, vp]),
     "roc_softmax_xent_bwd_norm": (i32, [i64, i32, vp, i64, vp, i64, vp, vp, vp, i64, vp, u64, vp, vp]),
     "roc_sigmoid_xent_bwd": (i32, [i64, i32, vp, i64, vp, i64, vp, vp, i64, vp, u64, vp, vp]),
+    "roc_batchnorm_workspace_bytes": (sz, [i64, i32]),
+    "roc_batchnorm_fwd": (i32, [i64, i32, vp, i64, vp, vp, f64, f64, vp, vp, i32, i32, vp, i64, vp, vp, vp, vp, vp, sz,
+                                vp]),
+    "roc_batchnorm_bwd": (i32, [i64, i32, vp, i64, vp, i64, i32, vp, vp, vp, vp, vp, vp, vp, vp, i64, i32, vp, sz, vp]),
     "roc_linear_bwd_fused": (i32, [vp, vp]),
     "roc_linear_fwd": (i32, [i64, i32, i32, vp, i64, vp, vp, i64, i32, i32, vp, u64, vp]),
     "roc_linear_bwd_workspace_bytes": (sz, [i64, i32, i32]),
@@ -230,6 +234,9 @@ PROTOTYPES = {
     "roc_host_relu": (i32, [vp, i32]),
     "roc_host_sigmoid": (i32, [vp, i32]),
     "roc_host_add": (i32, [vp, i32, i32]),
+    "roc_host_batch_norm": (i32, [vp, i32, f32, f32]),
+    "roc_host_get_batch_norm_stats": (i32, [vp, i32, vp, vp]),
+    "roc_host_set_batch_norm_stats": (i32, [vp, i32, vp, vp]),
     "roc_host_softmax_cross_entropy": (i32, [vp, i32, i32, i32]),
     "roc_host_sigmoid_cross_entropy": (i32, [vp, i32, i32, i32]),
     "roc_host_adam": (i32, [vp, f64, f64]),

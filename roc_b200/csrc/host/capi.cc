@@ -107,6 +107,17 @@ int roc_host_get_aggr_index(roc_host* h, int t, uint32_t* host) { h->m().get_agg
 int roc_host_relu(roc_host* h, int t) { return h->push(h->m().relu(h->at(t))); }
 int roc_host_sigmoid(roc_host* h, int t) { return h->push(h->m().sigmoid(h->at(t))); }
 int roc_host_add(roc_host* h, int a, int b) { return h->push(h->m().add(h->at(a), h->at(b))); }
+int roc_host_batch_norm(roc_host* h, int t, float momentum, float eps) {
+  return h->push(h->m().batch_norm(h->at(t), momentum, eps));
+}
+int roc_host_get_batch_norm_stats(roc_host* h, int t, float* mean, float* var) {
+  h->m().get_batch_norm_stats(h->at(t), mean, var);
+  return 0;
+}
+int roc_host_set_batch_norm_stats(roc_host* h, int t, const float* mean, const float* var) {
+  h->m().set_batch_norm_stats(h->at(t), mean, var);
+  return 0;
+}
 int roc_host_softmax_cross_entropy(roc_host* h, int logits, int labels, int mask) {
   h->m().softmax_cross_entropy(h->at(logits), h->at(labels), h->at(mask));
   return 0;
@@ -218,6 +229,8 @@ int roc_host_op_info(roc_host* h, int layer, struct roc_host_op_info* out) {
     r.gradOut = handle(s->gradOut);
   } else if (const SigmoidCrossEntropy* b = dynamic_cast<const SigmoidCrossEntropy*>(op)) {
     r.gradOut = handle(b->gradOut);
+  } else if (const BatchNorm* bn = dynamic_cast<const BatchNorm*>(op)) {
+    r.fwdOut = handle(bn->fwdOut);
   }
   *out = r;
   return 0;

@@ -174,6 +174,27 @@ void Model::get_aggr_index(const Tensor& out, uint32_t* host) const {
   }
   ROC_FATAL("get_aggr_index: no scatter_gather produces this tensor");
 }
+static BatchNorm* batch_norm_of(const std::vector<GnnOp*>& layers, const Tensor& out, const char* what) {
+  for (GnnOp* op : layers) {
+    BatchNorm* bn = dynamic_cast<BatchNorm*>(op);
+    if (bn && bn->outputs[0].region == out.region) return bn;
+  }
+  ROC_FATAL((std::string(what) + ": no batch_norm produces this tensor").c_str());
+}
+void Model::get_batch_norm_stats(const Tensor& out, float* mean, float* var) const {
+  const BatchNorm* bn = batch_norm_of(layers, out, "get_batch_norm_stats");
+  const size_t bytes = (size_t)bn->outputs[0].dims[0] * sizeof(float);
+  ROC_CHECK(cudaMemcpyAsync(mean, bn->runMean, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+  ROC_CHECK(cudaMemcpyAsync(var, bn->runVar, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+  ROC_CHECK(cudaStreamSynchronize(ctx->stream));
+}
+void Model::set_batch_norm_stats(const Tensor& out, const float* mean, const float* var) {
+  BatchNorm* bn = batch_norm_of(layers, out, "set_batch_norm_stats");
+  const size_t bytes = (size_t)bn->outputs[0].dims[0] * sizeof(float);
+  ROC_CHECK(cudaMemcpyAsync(bn->runMean, mean, bytes, cudaMemcpyHostToDevice, ctx->stream));
+  ROC_CHECK(cudaMemcpyAsync(bn->runVar, var, bytes, cudaMemcpyHostToDevice, ctx->stream));
+  ROC_CHECK(cudaStreamSynchronize(ctx->stream));
+}
 void Model::softmax_cross_entropy(const Tensor& logits, const Tensor& labels, const Tensor& mask) {
   layers.push_back(new SoftmaxCrossEntropy(*this, logits, labels, mask));
 }
@@ -203,14 +224,23 @@ Tensor Model::sigmoid(const Tensor& _input) {
   layers.push_back(op);
   return op->outputs[0];
 }
+Tensor Model::batch_norm(const Tensor& input, float momentum, float eps) {
+  if (ctx->numParts > 1)
+    ROC_FATAL("batch_norm: runs on one partition only (numParts > 1 is not supported)");
+  BatchNorm* op = new BatchNorm(*this, input, momentum, eps);
+  layers.push_back(op);
+  parameters.push_back(op->gamma);
+  parameters.push_back(op->beta);
+  return op->outputs[0];
+}
 
 void Model::train_mode(void) { mode = MD_MODE_TRAIN; }
 void Model::infer_mode(void) { mode = MD_MODE_INFER; }
 
-const char* const roc::host::opKindNames[ROC_HOST_OP_SIGMOID_CROSS_ENTROPY + 1] = {
+const char* const roc::host::opKindNames[ROC_HOST_OP_BATCH_NORM + 1] = {
     "linear", "indegree_norm", "scatter_gather", "scatter_gather(max)", "scatter_gather(min)",
     "scatter_gather(weighted)", "attention_gather", "relu", "sigmoid", "add", "dropout", "softmax_cross_entropy",
-    "sigmoid_cross_entropy"};
+    "sigmoid_cross_entropy", "batch_norm"};
 int roc::host::op_kind(const GnnOp* op) {
   if (const ScatterGather* sg = dynamic_cast<const ScatterGather*>(op))
     return sg->aggr == AGGR_MAX   ? ROC_HOST_OP_SCATTER_GATHER_MAX
@@ -225,6 +255,7 @@ int roc::host::op_kind(const GnnOp* op) {
          : dynamic_cast<const Dropout*>(op)               ? ROC_HOST_OP_DROPOUT
          : dynamic_cast<const SoftmaxCrossEntropy*>(op)   ? ROC_HOST_OP_SOFTMAX_CROSS_ENTROPY
          : dynamic_cast<const SigmoidCrossEntropy*>(op)   ? ROC_HOST_OP_SIGMOID_CROSS_ENTROPY
+         : dynamic_cast<const BatchNorm*>(op)             ? ROC_HOST_OP_BATCH_NORM
                                                           : ROC_HOST_OP_ADD;
 }
 
@@ -281,7 +312,7 @@ static void mark_gradients(const Model& m) {
     bool any = false;
     for (int j = 0; j < op->numInputs; j++)
       if (op->inputs[j].region >= 0) any = any || rt->t(op->inputs[j].region).requiresGrad;
-    if (as<Linear>(op)) any = true;
+    if (as<Linear>(op) || as<BatchNorm>(op)) any = true;   // their own parameters
     for (int j = 0; j < op->numOutputs; j++) {
       rt->t(op->outputs[j].region).requiresGrad = any;
       rt->t(op->outputs[j].region).produced = true;
@@ -450,6 +481,23 @@ static void fuse_gcn_block(const std::vector<GnnOp*>& layers, Wiring& w) {
   }
 }
 
+// ---- fusion of  batch_norm -> relu: the BN output feeds only the relu.  The BN forward writes the relu's output, and
+//      its backward reads that output's gradient and masks it by fma(x, a, b) > 0 from its saved affine map.
+//      The other peepholes never cross a BN.  In GCN, SG -> indegree_norm still fuses, and the relu after the BN is
+//      this pass's.  The backward fusion (b) needs an indegree_norm under the relu, so it does not match here.
+static void fuse_batch_norm_relu(const std::vector<GnnOp*>& layers, Wiring& w) {
+  for (size_t l = 0; l < layers.size(); l++) {
+    BatchNorm* bn = as<BatchNorm>(layers[l]);
+    if (!bn || bn->fwdOut >= 0) continue;
+    const int ro = bn->outputs[0].region;
+    if (w.consumers[ro] != 1) continue;
+    Activation* act = as<Activation>(layers[w.consumerOp[ro]]);
+    if (!act || act->actiMode != AC_MODE_RELU || act->fusedInto >= 0) continue;
+    bn->fwdOut = act->outputs[0].region;
+    act->fusedInto = (int)l;
+  }
+}
+
 // ---- fusion of  dropout -> linear  (gnn.cc:79-81, 86-88): the dropout output feeds only the linear
 static void fuse_dropout_into_linear(const std::vector<GnnOp*>& layers, Wiring& w) {
   for (size_t l = 0; l < layers.size(); l++) {
@@ -556,6 +604,7 @@ bool Model::init(const Config&) {
   Wiring w = wire(layers);   // the passes below change no op's inputs or outputs
   if (fuse) {
     fuse_gcn_block(layers, w);
+    fuse_batch_norm_relu(layers, w);
     fuse_dropout_into_linear(layers, w);
     fuse_backward_epilogues(ctx, layers, w);
   }
@@ -1395,6 +1444,52 @@ void Activation::backward(const Model& model) {
   else
     ROC_CHECK(roc_activation_bwd(rows, H, (int)actiMode, rt->data(y), rt->t(y).ld, rt->grad(y), rt->t(y).ld,
                                  rt->grad(x), rt->t(x).ld, acc, rt->stream));
+}
+
+// -------------------------------------------------------------- BatchNorm ---
+BatchNorm::BatchNorm(const Model& model, const Tensor& _input, float _momentum, float _eps)
+    : GnnOp(_input), momentum(_momentum), eps(_eps), fwdOut(-1), workspace(nullptr), workspaceBytes(0) {
+  ROC_ASSERT(_input.type == Tensor::NODE_TENSOR && _input.numDim == 2 && _input.dims[1] == model.myGraph.numNodes);
+  if (!(_momentum >= 0.0f && _momentum <= 1.0f)) ROC_FATAL("batch_norm: the momentum must be in [0, 1]");
+  if (!(_eps >= 0.0f) || !std::isfinite(_eps)) ROC_FATAL("batch_norm: eps must be finite and >= 0");
+  RuntimeImpl* rt = model.ctx;
+  const int H = (int)_input.dims[0];
+  // constant fills only: the Linears' GlorotUniform draws do not move
+  ZerosInitializer zeros;
+  gamma = model.create_weight_tensor(H, 1, &zeros);
+  beta = model.create_weight_tensor(H, 1, &zeros);
+  ROC_CHECK(roc_fill(1, H, 1.0f, rt->data(gamma.region), H, rt->stream));
+  float* f = (float*)rt->dmalloc((size_t)4 * H * sizeof(float));
+  runMean = f; runVar = f + H; saveA = f + 2 * H; saveB = f + 3 * H;
+  ROC_CHECK(roc_fill(1, H, 0.0f, runMean, H, rt->stream));
+  ROC_CHECK(roc_fill(1, H, 1.0f, runVar, H, rt->stream));
+  saveMean = (double*)rt->dmalloc((size_t)2 * H * sizeof(double));
+  saveInvStd = saveMean + H;
+  numOutputs = 1;
+  outputs[0] = model.create_node_tensor<DATATYPE>(H);
+}
+void BatchNorm::init(const Model& model) {
+  const int64_t rows = model.local_rows();
+  if (rows < 2) ROC_FATAL("batch_norm: the partition has fewer than 2 rows (no batch variance)");
+  workspaceBytes = roc_batchnorm_workspace_bytes(rows, (int)inputs[0].dims[0]);
+  workspace = model.ctx->dmalloc(workspaceBytes);
+}
+void BatchNorm::forward(const Model& model) {
+  RuntimeImpl* rt = model.ctx;
+  const int x = inputs[0].region, y = fwdOut >= 0 ? fwdOut : outputs[0].region;
+  ROC_CHECK(roc_batchnorm_fwd(model.local_rows(), (int)inputs[0].dims[0], rt->data(x), rt->t(x).ld,
+                              rt->data(gamma.region), rt->data(beta.region), eps, momentum, runMean, runVar,
+                              model.mode == MD_MODE_TRAIN, fwdOut >= 0, rt->data(y), rt->t(y).ld, saveA, saveB, saveMean,
+                              saveInvStd, workspace, workspaceBytes, rt->stream));
+}
+void BatchNorm::backward(const Model& model) {
+  RuntimeImpl* rt = model.ctx;
+  const int x = inputs[0].region, y = fwdOut >= 0 ? fwdOut : outputs[0].region;
+  float* dX = rt->t(x).requiresGrad ? rt->grad(x) : nullptr;
+  ROC_CHECK(roc_batchnorm_bwd(model.local_rows(), (int)inputs[0].dims[0], rt->data(x), rt->t(x).ld, rt->grad(y),
+                              rt->t(y).ld, fwdOut >= 0, rt->data(gamma.region), saveA, saveB, saveMean, saveInvStd,
+                              rt->grad(gamma.region), rt->grad(beta.region), dX, rt->t(x).ld, resetInputGrads[0] ? 0 : 1,
+                              workspace, workspaceBytes, rt->stream));
 }
 
 // ---------------------------------------------------------------- Element ---

@@ -618,6 +618,53 @@ def sigmoid_xent_bwd(logits, labels_bits, mask, row_end=None, col_left=0, with_m
     return g, m.as_dict()
 
 
+class BatchNormState:
+    """What a training batchnorm_fwd keeps for batchnorm_bwd: a, b (fp32), mean, invstd (fp64), H values each; and the
+    workspace (roc_batchnorm_workspace_bytes)."""
+
+    def __init__(self, rows, h, device="cuda"):
+        self.a = torch.zeros(h, device=device)
+        self.b = torch.zeros(h, device=device)
+        self.mean = torch.zeros(h, device=device, dtype=torch.float64)
+        self.invstd = torch.zeros(h, device=device, dtype=torch.float64)
+        self.ws_bytes = lib.roc_batchnorm_workspace_bytes(rows, h)
+        self.ws = torch.empty(max(self.ws_bytes, 16), device=device, dtype=torch.uint8)
+
+
+def batchnorm_fwd(x, gamma, beta, run_mean, run_var, training=True, relu=False, eps=1e-5, momentum=0.1, state=None,
+                  out=None):
+    """roc_batchnorm_fwd on a [rows][H] tensor whose rows are padded to float4 (padded()): y = relu?(x a + b) per
+    column, with a, b from the batch statistics (training: run_mean / run_var updated in place, `state` filled) or from
+    the running statistics.  Returns (y, state)."""
+    rows, h = x.shape
+    if state is None:
+        state = BatchNormState(rows, h, x.device)
+    if out is None:
+        out = padded(rows, h, x.device)
+    check(lib.roc_batchnorm_fwd(rows, h, _ptr(x), _ld(x), _ptr(gamma), _ptr(beta), float(eps), float(momentum),
+                                _ptr(run_mean), _ptr(run_var), int(bool(training)), int(bool(relu)), _ptr(out),
+                                _ld(out), _ptr(state.a), _ptr(state.b), _ptr(state.mean), _ptr(state.invstd),
+                                _ptr(state.ws), state.ws_bytes, _stream()), "roc_batchnorm_fwd")
+    return out, state
+
+
+def batchnorm_bwd(x, dy, gamma, state, relu=False, dx=None, accumulate=False, need_dx=True):
+    """roc_batchnorm_bwd after a training batchnorm_fwd that filled `state`: returns (dx, dgamma, dbeta).  dx is
+    written into (or with accumulate=True added to) `dx` when given; need_dx=False skips it (dx is then None)."""
+    rows, h = x.shape
+    dgamma = torch.empty(h, device=x.device)
+    dbeta = torch.empty(h, device=x.device)
+    if need_dx and dx is None:
+        dx = padded(rows, h, x.device)
+    if not need_dx:
+        dx = None
+    check(lib.roc_batchnorm_bwd(rows, h, _ptr(x), _ld(x), _ptr(dy), _ld(dy), int(bool(relu)), _ptr(gamma),
+                                _ptr(state.a), _ptr(state.b), _ptr(state.mean), _ptr(state.invstd), _ptr(dgamma),
+                                _ptr(dbeta), _ptr(dx), _ld(dx) if dx is not None else 0, int(bool(accumulate)),
+                                _ptr(state.ws), state.ws_bytes, _stream()), "roc_batchnorm_bwd")
+    return dx, dgamma, dbeta
+
+
 def linear_bwd(x, w, y, dy, dw, dx=None, activation=0, accumulate_dx=False):
     ws_bytes = lib.roc_linear_bwd_workspace_bytes(x.shape[0], x.shape[1], w.shape[0])
     ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=x.device)

@@ -140,6 +140,26 @@ class Model:
     def add(self, a, b):
         return lib.roc_host_add(self.h, a, b)
 
+    def batch_norm(self, t, momentum=0.1, eps=1e-5):
+        """torch.nn.BatchNorm1d over every local row: appends two parameters, gamma (ones) then beta (zeros), each of
+        parameter_shape (H, 1).  A training forward uses the batch statistics and updates the running mean / variance
+        (start 0 / 1); infer mode uses the running statistics.  A relu that alone reads the output is fused into it.
+        One partition only; init() refuses fewer than 2 rows."""
+        return lib.roc_host_batch_norm(self.h, t, float(momentum), float(eps))
+
+    def batch_norm_stats(self, t):
+        """(running mean, running variance), fp32 [H] each, of the batch_norm whose output is t."""
+        h = self.tensor_shape(t)[1]
+        mean, var = np.empty(h, dtype=np.float32), np.empty(h, dtype=np.float32)
+        check(lib.roc_host_get_batch_norm_stats(self.h, t, mean.ctypes.data, var.ctypes.data))
+        return mean, var
+
+    def set_batch_norm_stats(self, t, mean, var):
+        h = self.tensor_shape(t)[1]
+        mean, var = np.ascontiguousarray(mean, dtype=np.float32), np.ascontiguousarray(var, dtype=np.float32)
+        assert mean.shape == (h,) and var.shape == (h,), (mean.shape, var.shape, h)
+        check(lib.roc_host_set_batch_norm_stats(self.h, t, mean.ctypes.data, var.ctypes.data))
+
     def softmax_cross_entropy(self, logits, labels, mask):
         check(lib.roc_host_softmax_cross_entropy(self.h, logits, labels, mask))
 
@@ -379,21 +399,39 @@ def _loss(model, loss, logits, label, mask):
         raise ValueError("loss must be \"softmax\" or \"sigmoid\"")
 
 
+def _check_norm(norm):
+    if norm not in (None, "batch"):
+        raise ValueError("norm must be None or \"batch\"")
+
+
+def _hidden_norm(model, norm, t, bns):
+    """norm="batch": batch_norm on a hidden layer's output, right before its relu; None leaves t as it is."""
+    if norm is None:
+        return t
+    t = model.batch_norm(t)
+    bns.append(t)
+    return t
+
+
 def build_gcn(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exact_backward=False, features="float32",
-              aggregation="float32", loss="softmax"):
+              aggregation="float32", loss="softmax", norm=None):
     """The model script of gnn.cc:65-98 for `-layers a-b-...-c`.  Returns the handles.  exact_backward: train on the
     exact gradient over the graph's transpose (Model.set_exact_backward), for directed graphs; the same keyword on
     build_sage_mean, build_sage_pool and build_gat.  features="bfloat16" keeps the input features in bf16
     (Model.create_node_tensor); the same keyword on every builder.  aggregation="bfloat16" stores the fused
     linear -> indegree_norm output each scatter_gather reads in bf16 (Model.set_bf16_aggregation); the same keyword
     on every builder.  loss="sigmoid" ends the model in the multi-label sigmoid_cross_entropy instead of the softmax
-    (labels then go in with Model.set_multilabels); the same keyword on every builder."""
+    (labels then go in with Model.set_multilabels); the same keyword on every builder.  norm="batch" puts a
+    batch_norm (Model.batch_norm) on every hidden layer's output right before its relu (here after the second
+    indegree_norm, and before the residual add), never on the last layer; the same keyword on every builder, which
+    then returns the batch_norm outputs as `bns`."""
+    _check_norm(norm)
     L = len(layers)
     x = _input_tensor(model, layers[0], features)
     label = model.create_node_tensor(layers[-1])
     mask = model.create_node_tensor(1, is_int=True)
     t = x
-    relu_outs = []
+    relu_outs, bns = [], []
     for i in range(1, L):
         t = model.dropout(t, dropout_rate)
         skip = t
@@ -402,7 +440,7 @@ def build_gcn(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exact_bac
         t = model.scatter_gather(t)
         t = model.indegree_norm(t)
         if i != L - 1:
-            t = model.relu(t)
+            t = model.relu(_hidden_norm(model, norm, t, bns))
             relu_outs.append(t)
         if L > 3:   # residual branch, gnn.cc:86-90
             skip = model.linear(skip, layers[i], _lib.AC_MODE_NONE)
@@ -413,11 +451,11 @@ def build_gcn(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exact_bac
         model.set_exact_backward(True)
     _aggregation(model, aggregation)
     model.init()
-    return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs}
+    return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs, "bns": bns}
 
 
 def build_sage_mean(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exact_backward=False,
-                    features="float32", aggregation="float32", loss="softmax"):
+                    features="float32", aggregation="float32", loss="softmax", norm=None):
     """GraphSAGE with the mean aggregator (BASELINE.json configs[2]) composed from the reference's own ops
     (gnn.h:165-179; AGGR_AVG is declared at gnn.h:75-80 but the reference's ScatterGather only sums):
 
@@ -429,13 +467,15 @@ def build_sage_mean(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exa
 
     x / sqrt(deg) / sqrt(deg) is the mean to within one fp32 rounding.  Same wiring as the reference's residual
     GCN layer (gnn.cc:79-90) with both norms after the aggregation.  aggregation="bfloat16" stores linear(D, d_i),
-    which only the scatter_gather reads, in bf16 (Model.set_bf16_aggregation)."""
+    which only the scatter_gather reads, in bf16 (Model.set_bf16_aggregation).  norm="batch": batch_norm on t before
+    each hidden relu (see build_gcn)."""
+    _check_norm(norm)
     L = len(layers)
     x = _input_tensor(model, layers[0], features)
     label = model.create_node_tensor(layers[-1])
     mask = model.create_node_tensor(1, is_int=True)
     t = x
-    relu_outs = []
+    relu_outs, bns = [], []
     for i in range(1, L):
         d = model.dropout(t, dropout_rate)
         nb = model.linear(d, layers[i], _lib.AC_MODE_NONE)
@@ -445,7 +485,7 @@ def build_sage_mean(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exa
         root = model.linear(d, layers[i], _lib.AC_MODE_NONE)
         t = model.add(nb, root)
         if i != L - 1:
-            t = model.relu(t)
+            t = model.relu(_hidden_norm(model, norm, t, bns))
             relu_outs.append(t)
     _loss(model, loss, t, label, mask)
     model.adam(lr, weight_decay)
@@ -453,11 +493,11 @@ def build_sage_mean(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exa
         model.set_exact_backward(True)
     _aggregation(model, aggregation)
     model.init()
-    return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs}
+    return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs, "bns": bns}
 
 
 def build_sage_pool(model, layers, dropout_rate, aggr=_lib.AGGR_MAX, lr=0.01, weight_decay=0.05, exact_backward=False,
-                    features="float32", aggregation="float32", loss="softmax"):
+                    features="float32", aggregation="float32", loss="softmax", norm=None):
     """GraphSAGE with the pooling aggregator (Hamilton et al., 2017) composed from the reference's ops plus the max
     (or min) ScatterGather.  The reference's Linear has no bias, so neither has this.  Per layer:
 
@@ -468,14 +508,16 @@ def build_sage_pool(model, layers, dropout_rate, aggr=_lib.AGGR_MAX, lr=0.01, we
         t  = relu(t)                                   # all but the last layer
 
     Single partition; init refuses a graph with a duplicate edge in a row.  aggregation="bfloat16" stores p, the relu
-    output the scatter_gather reads, in bf16 (Model.set_bf16_aggregation).  Returns the handles, with `pools`
-    (the scatter_gather outputs, for get_aggr_index) and `pool_ins` (their inputs)."""
+    output the scatter_gather reads, in bf16 (Model.set_bf16_aggregation).  norm="batch": batch_norm on t before each
+    hidden layer's last relu (see build_gcn; the pooling network's relu is not a hidden layer's output).  Returns the
+    handles, with `pools` (the scatter_gather outputs, for get_aggr_index) and `pool_ins` (their inputs)."""
+    _check_norm(norm)
     L = len(layers)
     x = _input_tensor(model, layers[0], features)
     label = model.create_node_tensor(layers[-1])
     mask = model.create_node_tensor(1, is_int=True)
     t = x
-    relu_outs, pools, pool_ins = [], [], []
+    relu_outs, pools, pool_ins, bns = [], [], [], []
     for i in range(1, L):
         d = model.dropout(t, dropout_rate)
         p = model.relu(model.linear(d, layers[i], _lib.AC_MODE_NONE))
@@ -484,7 +526,7 @@ def build_sage_pool(model, layers, dropout_rate, aggr=_lib.AGGR_MAX, lr=0.01, we
         pools.append(nb)
         t = model.add(model.linear(nb, layers[i], _lib.AC_MODE_NONE), model.linear(d, layers[i], _lib.AC_MODE_NONE))
         if i != L - 1:
-            t = model.relu(t)
+            t = model.relu(_hidden_norm(model, norm, t, bns))
             relu_outs.append(t)
     _loss(model, loss, t, label, mask)
     model.adam(lr, weight_decay)
@@ -493,11 +535,11 @@ def build_sage_pool(model, layers, dropout_rate, aggr=_lib.AGGR_MAX, lr=0.01, we
     _aggregation(model, aggregation)
     model.init()
     return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs, "pools": pools,
-            "pool_ins": pool_ins}
+            "pool_ins": pool_ins, "bns": bns}
 
 
 def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01, weight_decay=0.05,
-              exact_backward=False, features="float32", aggregation="float32", loss="softmax"):
+              exact_backward=False, features="float32", aggregation="float32", loss="softmax", norm=None):
     """GAT (Velickovic et al., 2018) built from the reference's ops plus attention_gather.  `heads` (an int, or one
     value per hidden layer) applies to the hidden layers; the last layer has one head.  layers[i] is the width of
     layer i's output, heads_i * F_i.  Per layer:
@@ -511,8 +553,10 @@ def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01,
     Where this differs from the paper: there is no bias (the reference's Linear has none); ReLU replaces ELU (the
     engine has no ELU); with heads > 1 each head's scores are a dense projection of all heads' features, where the
     paper uses a per-head block.  With one head it is GAT exactly.  Single partition.  aggregation="bfloat16" stores
-    wh, which the attention_gather and the score linear read, in bf16 (Model.set_bf16_aggregation).  Returns the
-    handles, with `attn` (the attention_gather outputs), `attn_ins` (their feature inputs) and `scores`."""
+    wh, which the attention_gather and the score linear read, in bf16 (Model.set_bf16_aggregation).  norm="batch":
+    batch_norm on t before each hidden relu (see build_gcn).  Returns the handles, with `attn` (the attention_gather
+    outputs), `attn_ins` (their feature inputs) and `scores`."""
+    _check_norm(norm)
     L = len(layers)
     hs = list(heads) if isinstance(heads, (list, tuple)) else [int(heads)] * (L - 2)
     assert len(hs) == L - 2, "one head count per hidden layer"
@@ -521,7 +565,7 @@ def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01,
     label = model.create_node_tensor(layers[-1])
     mask = model.create_node_tensor(1, is_int=True)
     t = x
-    relu_outs, attn, attn_ins, scores = [], [], [], []
+    relu_outs, attn, attn_ins, scores, bns = [], [], [], [], []
     for i in range(1, L):
         d = model.dropout(t, dropout_rate)
         wh = model.linear(d, layers[i], _lib.AC_MODE_NONE)
@@ -531,7 +575,7 @@ def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01,
         scores.append(sc)
         attn.append(t)
         if i != L - 1:
-            t = model.relu(t)
+            t = model.relu(_hidden_norm(model, norm, t, bns))
             relu_outs.append(t)
     _loss(model, loss, t, label, mask)
     model.adam(lr, weight_decay)
@@ -540,11 +584,11 @@ def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01,
     _aggregation(model, aggregation)
     model.init()
     return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs, "attn": attn,
-            "attn_ins": attn_ins, "scores": scores}
+            "attn_ins": attn_ins, "scores": scores, "bns": bns}
 
 
 def build_gcn_weighted(model, layers, dropout_rate, edge_weights, edge_grad=False, lr=0.01, weight_decay=0.05,
-                       features="float32", aggregation="float32", loss="softmax"):
+                       features="float32", aggregation="float32", loss="softmax", norm=None):
     """GCN with edge weights (e.g. datasets.gcn_edge_weights, which folds in the symmetric normalisation).  Per layer
 
         t = relu(scatter_gather(linear(dropout(t), layers[i]), weights=e))     # no relu on the last layer
@@ -552,25 +596,28 @@ def build_gcn_weighted(model, layers, dropout_rate, edge_weights, edge_grad=Fals
     with one edge tensor e shared by every layer.  edge_weights: one fp32 value per edge in CSR order, loaded after
     init().  edge_grad: compute e's gradient in backward (the sum of the layers' contributions).  Single partition.
     aggregation="bfloat16" stores each linear output the scatter_gather reads in bf16 (Model.set_bf16_aggregation).
-    Returns the handles, with `edges` and the aggregations' inputs `sg_ins` and outputs `sg_outs`."""
+    norm="batch": batch_norm on t before each hidden relu (see build_gcn).  Returns the handles, with `edges` and the
+    aggregations' inputs `sg_ins` and outputs `sg_outs`."""
+    _check_norm(norm)
     L = len(layers)
     x = _input_tensor(model, layers[0], features)
     label = model.create_node_tensor(layers[-1])
     mask = model.create_node_tensor(1, is_int=True)
     e = model.create_edge_tensor(1)
     t = x
-    sg_ins, sg_outs = [], []
+    sg_ins, sg_outs, bns = [], [], []
     for i in range(1, L):
         t = model.linear(model.dropout(t, dropout_rate), layers[i], _lib.AC_MODE_NONE)
         sg_ins.append(t)
         t = model.scatter_gather(t, weights=e)
         sg_outs.append(t)
         if i != L - 1:
-            t = model.relu(t)
+            t = model.relu(_hidden_norm(model, norm, t, bns))
     _loss(model, loss, t, label, mask)
     model.adam(lr, weight_decay)
     model.set_edge_grad(e, edge_grad)
     _aggregation(model, aggregation)
     model.init()
     model.set_tensor(e, np.asarray(edge_weights, dtype=np.float32))
-    return {"input": x, "label": label, "mask": mask, "logits": t, "edges": e, "sg_ins": sg_ins, "sg_outs": sg_outs}
+    return {"input": x, "label": label, "mask": mask, "logits": t, "edges": e, "sg_ins": sg_ins, "sg_outs": sg_outs,
+            "bns": bns}

@@ -52,6 +52,7 @@ typedef void*    roc_stream_t; /* cudaStream_t */
 #define ROC_AC_MODE_NONE    0
 #define ROC_AC_MODE_RELU    1
 #define ROC_AC_MODE_SIGMOID 2
+#define ROC_AC_MODE_ELU     3   /* not in the reference: ELU with alpha = 1 (roc_activation_* only) */
 
 /* MaskType, gnn.h:98-103 */
 #define ROC_MASK_TRAIN 0
@@ -468,7 +469,9 @@ int roc_indegree_norm(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft, 
 
 /* Replaces cudnnActivationForward/Backward, activation_kernel.cu:64-66, 128-132.
  * bwd: dX (+)= dY * f'(.) evaluated from the OUTPUT y; accumulate != 0 adds
- * into dX (the reference's beta = 1 on a loaded buffer, gnn.cc:704-713). */
+ * into dX (the reference's beta = 1 on a loaded buffer, gnn.cc:704-713).
+ * ROC_AC_MODE_ELU: y = x > 0 ? x : expm1f(x) (NaN propagates), and dX (+)= dY * (y > 0 ? 1 : y + 1), which is the
+ * derivative because y > 0 exactly when x > 0 (torch's elu_backward with is_result). */
 int roc_activation_fwd(int64_t rows, int H, int mode, const float* x, int64_t ldX,
                        float* y, int64_t ldY, roc_stream_t stream);
 int roc_activation_bwd(int64_t rows, int H, int mode, const float* y, int64_t ldY,
@@ -612,6 +615,38 @@ int roc_batchnorm_bwd(int64_t rows, int H, const float* x, int64_t ldX, const fl
                       const float* gamma, const float* saveA, const float* saveB, const double* saveMean,
                       const double* saveInvStd, float* dGamma, float* dBeta, float* dX, int64_t ldDX, int accumulate,
                       void* workspace, size_t workspaceBytes, roc_stream_t stream);
+
+/* ------------------------------------------------------- attention scores --- */
+
+/* The per-head GAT attention scores (Velickovic et al., 2018; PyG's GATConv): X is [rows][H] with H = heads * F, and
+ * column c belongs to head c / F.  A is [2 * heads][F], dense: row k is a_dst of head k and row heads + k its a_src.
+ * S is [rows][2 * heads] in the layout roc_sg_attn_* read:
+ *   S[v][k] = sum_f A[k][f] X[v][kF + f],   S[v][heads + k] = sum_f A[heads + k][f] X[v][kF + f]
+ * each summed in fp32 with one fma per product, f = 0 .. F - 1 in order.  Only columns [0, 2 * heads) of S and
+ * [0, H) of dX are written; columns [H, ldX) of X may be loaded but reach no result.
+ * bwd:
+ *   dX[v][kF + f] (+)= fma(dS[v][heads + k], A[heads + k][f], dS[v][k] * A[k][f])   (accumulate != 0: +=)
+ *   dA[k][f] = sum_v dS[v][k] X[v][kF + f],  dA[heads + k][f] = sum_v dS[v][heads + k] X[v][kF + f]
+ * dA is overwritten; its sums are taken in fp64 over row blocks whose size depends on (rows, H) only, the blocks'
+ * partials added in block order, then rounded once to fp32, so the same call gives the same bits every time.
+ * dX == NULL computes dA only.  The workspace holds the partials: roc_attn_scores_workspace_bytes(rows, H, heads),
+ * 16-byte aligned.  X rows are read as 16-byte vectors (bf16: 8-byte) when ldX is a multiple of 4 and X is so
+ * aligned, else element by element, with the same results.
+ * ROC_ERR_INVALID: a NULL X / A / S / dS / dA / workspace, rows < 0, H <= 0, heads <= 0, ldX < H, ldS or
+ * ldDS < 2 * heads, ldDX < H with a dX, a short or misaligned workspace.  ROC_ERR_UNSUPPORTED: H % heads != 0 or
+ * H > 1024.  The _bf16 forms take X as raw bf16 bits (see roc_f32_to_bf16) and give the bytes of the fp32 call on the
+ * widened rows. */
+size_t roc_attn_scores_workspace_bytes(int64_t rows, int H, int heads);
+int roc_attn_scores_fwd(int64_t rows, int H, int heads, const float* X, int64_t ldX, const float* A, float* S,
+                        int64_t ldS, roc_stream_t stream);
+int roc_attn_scores_bwd(int64_t rows, int H, int heads, const float* X, int64_t ldX, const float* A, const float* dS,
+                        int64_t ldDS, float* dX, int64_t ldDX, int accumulate, float* dA, void* workspace,
+                        size_t workspaceBytes, roc_stream_t stream);
+int roc_attn_scores_fwd_bf16(int64_t rows, int H, int heads, const uint16_t* X, int64_t ldX, const float* A, float* S,
+                             int64_t ldS, roc_stream_t stream);
+int roc_attn_scores_bwd_bf16(int64_t rows, int H, int heads, const uint16_t* X, int64_t ldX, const float* A,
+                             const float* dS, int64_t ldDS, float* dX, int64_t ldDX, int accumulate, float* dA,
+                             void* workspace, size_t workspaceBytes, roc_stream_t stream);
 
 /* --------------------------------------------------------------- Linear --- */
 

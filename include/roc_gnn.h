@@ -42,7 +42,7 @@ typedef float DATATYPE;  /* types.h:7 */
 #define FILE_HEADER_SIZE (sizeof(E_ID) + sizeof(V_ID)) /* gnn.h:33 */
 
 enum AggrType { AGGR_AVG, AGGR_MAX, AGGR_MIN, AGGR_SUM };            /* gnn.h:75-80 */
-enum ActiMode { AC_MODE_NONE, AC_MODE_RELU, AC_MODE_SIGMOID };         /* gnn.h:82-86 */
+enum ActiMode { AC_MODE_NONE, AC_MODE_RELU, AC_MODE_SIGMOID, AC_MODE_ELU };   /* gnn.h:82-86, + ELU */
 enum ElementType { EW_TYPE_ADD, EW_TYPE_MUL };                         /* gnn.h:88-91 */
 enum ModelMode { MD_MODE_TRAIN, MD_MODE_INFER };                       /* gnn.h:93-96 */
 enum MaskType { MASK_TRAIN, MASK_VAL, MASK_TEST, MASK_NONE };          /* gnn.h:98-103 */
@@ -195,6 +195,12 @@ public:
    * destination scores, the true gradient of the rest on a symmetric graph.  Never fused with neighbouring ops.
    * Single partition only (exit(1) otherwise). */
   Tensor attention_gather(const Tensor& input, const Tensor& scores, int heads, float negativeSlope = 0.2f);
+  /* The per-head GAT scores of `input` (H = heads * F columns; roc_attn_scores_fwd / _bwd): a [rows][2 * heads] output
+   * [s_dst | s_src], head k's scores the dot products of its own F columns with its a_dst and a_src.  Appends one
+   * parameter A, a weight tensor of dims {F, 2 * heads} (row k: a_dst of head k, row heads + k: its a_src), drawn by the
+   * GlorotUniform of a Linear F -> 2 * heads.  Reads a bf16 input only when set_bf16_aggregation made it so.  Exits
+   * when H % heads != 0 or H > 1024.  Single partition only (exit(1) otherwise). */
+  Tensor attention_scores(const Tensor& input, int heads);
   /* Edge-weighted aggregation (roc_sg_weighted_forward_planned): out[v] = sum over v's in-edges e of
    * edgeWeights[e] * input[src(e)].  edgeWeights is an edge tensor (create_edge_tensor).  Its backward is exact on any
    * graph: init() builds the graph's transpose once (roc_sg_transpose) the first time a model has such an op, and the
@@ -215,6 +221,10 @@ public:
   Tensor linear(const Tensor& _input, int outDim, ActiMode activation, Initializer* initializer = NULL);
   Tensor relu(const Tensor& _input);
   Tensor sigmoid(const Tensor& _input);
+  /* ELU with alpha = 1 (roc_activation_fwd with ROC_AC_MODE_ELU); never fused with another op.  A Linear cannot apply
+   * it (linear() exits on AC_MODE_ELU).  Row-local like relu, so not refused on more than one partition, but untested
+   * there. */
+  Tensor elu(const Tensor& _input);
   /* Batch normalisation over every local row (torch.nn.BatchNorm1d; roc_batchnorm_fwd / roc_batchnorm_bwd).  Appends
    * two parameters, gamma (filled with 1) then beta (0), each a weight tensor of dims {H, 1}; creating them draws no
    * random numbers.  A training forward normalises by the batch statistics and updates the running mean (start 0) and
@@ -272,7 +282,7 @@ public:
    *    into its epilogue) and one sum scatter_gather alone reads it; or
    *  - a Linear with AC_MODE_NONE or an unfused relu writes it, at least one max / min scatter_gather, weighted
    *    scatter_gather or attention_gather reads it as its feature input, and every other reader is one of those or a
-   *    Linear reading it as X with no fused dropout (GAT's score Linear).
+   *    Linear reading it as X with no fused dropout (GAT's score Linear) or an attention_scores.
    * Its producer rounds the fp32 result to nearest even as it stores it (a relu's gradient then takes its mask from the
    * stored bf16 value), the aggregations read the rows at half width and compute in fp32, and a Linear reads them as a
    * bf16 X.  The gradient of such a tensor is an ordinary fp32 tensor; every other tensor stays fp32.  Call it before
@@ -344,6 +354,18 @@ public:
   float* stats;      /* [Nloc][statsLd] m | 1/Z per head of the last forward (Runtime arena) */
   int64_t statsLd;
   float* scratch[2]; /* gradients of an input that accumulates (or needs none), written here first (Runtime arena) */
+};
+
+class AttentionScores : public GnnOp {  /* not in the reference: Model::attention_scores */
+public:
+  AttentionScores(const Model& model, const Tensor& input, int heads);
+  virtual void init(const Model& model);
+  virtual void forward(const Model& model);
+  virtual void backward(const Model& model);
+  int heads;
+  Tensor a;          /* parameter, dims {F, 2 * heads} */
+  void* workspace;   /* roc_attn_scores_workspace_bytes (Runtime arena) */
+  size_t workspaceBytes;
 };
 
 class WeightedScatterGather : public GnnOp {  /* not in the reference: Model::scatter_gather(input, edgeWeights) */

@@ -55,6 +55,10 @@ int roc_host_scatter_gather_weighted(roc_host* h, int t, int edges);
 int roc_host_set_edge_grad(roc_host* h, int edges, int on);
 int roc_host_relu(roc_host* h, int t);
 int roc_host_sigmoid(roc_host* h, int t);
+/* Model::elu(t) */
+int roc_host_elu(roc_host* h, int t);
+/* Model::attention_scores(t, heads): appends one parameter (A, 2 * heads rows of F).  One partition only. */
+int roc_host_attention_scores(roc_host* h, int t, int heads);
 int roc_host_add(roc_host* h, int a, int b);
 /* Model::batch_norm(t, momentum, eps): appends two parameters (gamma, beta).  One partition only. */
 int roc_host_batch_norm(roc_host* h, int t, float momentum, float eps);
@@ -121,6 +125,8 @@ int roc_host_set_parameter(roc_host* h, int p, const float* host);
 #define ROC_HOST_OP_SOFTMAX_CROSS_ENTROPY 11
 #define ROC_HOST_OP_SIGMOID_CROSS_ENTROPY 12
 #define ROC_HOST_OP_BATCH_NORM 13
+#define ROC_HOST_OP_ELU 14
+#define ROC_HOST_OP_ATTENTION_SCORES 15
 struct roc_host_op_info {   /* a struct tag only: roc_host_op_info is also the function's name */
   int kind;          /* ROC_HOST_OP_* */
   int fusedInto;     /* >= 0: the layer whose kernel does this op's forward */

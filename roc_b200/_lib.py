@@ -12,7 +12,7 @@ LIB_PATH = os.path.join(_HERE, "lib", "libroc_b200.so")
 
 ROC_OK = 0
 ROC_ERR_INVALID, ROC_ERR_UNSUPPORTED, ROC_ERR_NOMEM, ROC_ERR_NO_DEVICE, ROC_ERR_IO = -1, -2, -3, -4, -5
-AC_MODE_NONE, AC_MODE_RELU, AC_MODE_SIGMOID = 0, 1, 2
+AC_MODE_NONE, AC_MODE_RELU, AC_MODE_SIGMOID, AC_MODE_ELU = 0, 1, 2, 3
 MASK_TRAIN, MASK_VAL, MASK_TEST, MASK_NONE = 0, 1, 2, 3
 SG_EPI_NONE, SG_EPI_NORM, SG_EPI_RELU = 0, 1, 2
 AGGR_AVG, AGGR_MAX, AGGR_MIN, AGGR_SUM = 0, 1, 2, 3        # AggrType (gnn.h:75-80); ROC_SG_AGGR_MAX / _MIN = 1 / 2
@@ -88,7 +88,8 @@ class MultilabelMetrics(C.Structure):
 
 HOST_OPS = ("linear", "indegree_norm", "scatter_gather", "scatter_gather_max", "scatter_gather_min",
             "scatter_gather_weighted", "attention_gather", "relu", "sigmoid", "add", "dropout",
-            "softmax_cross_entropy", "sigmoid_cross_entropy", "batch_norm")   # ROC_HOST_OP_* by value
+            "softmax_cross_entropy", "sigmoid_cross_entropy", "batch_norm", "elu",
+            "attention_scores")   # ROC_HOST_OP_* by value
 
 
 class HostOpInfo(C.Structure):
@@ -190,6 +191,11 @@ PROTOTYPES = {
     "roc_batchnorm_fwd": (i32, [i64, i32, vp, i64, vp, vp, f64, f64, vp, vp, i32, i32, vp, i64, vp, vp, vp, vp, vp, sz,
                                 vp]),
     "roc_batchnorm_bwd": (i32, [i64, i32, vp, i64, vp, i64, i32, vp, vp, vp, vp, vp, vp, vp, vp, i64, i32, vp, sz, vp]),
+    "roc_attn_scores_workspace_bytes": (sz, [i64, i32, i32]),
+    "roc_attn_scores_fwd": (i32, [i64, i32, i32, vp, i64, vp, vp, i64, vp]),
+    "roc_attn_scores_fwd_bf16": (i32, [i64, i32, i32, vp, i64, vp, vp, i64, vp]),
+    "roc_attn_scores_bwd": (i32, [i64, i32, i32, vp, i64, vp, vp, i64, vp, i64, i32, vp, vp, sz, vp]),
+    "roc_attn_scores_bwd_bf16": (i32, [i64, i32, i32, vp, i64, vp, vp, i64, vp, i64, i32, vp, vp, sz, vp]),
     "roc_linear_bwd_fused": (i32, [vp, vp]),
     "roc_linear_fwd": (i32, [i64, i32, i32, vp, i64, vp, vp, i64, i32, i32, vp, u64, vp]),
     "roc_linear_bwd_workspace_bytes": (sz, [i64, i32, i32]),
@@ -234,6 +240,8 @@ PROTOTYPES = {
     "roc_host_relu": (i32, [vp, i32]),
     "roc_host_sigmoid": (i32, [vp, i32]),
     "roc_host_add": (i32, [vp, i32, i32]),
+    "roc_host_elu": (i32, [vp, i32]),
+    "roc_host_attention_scores": (i32, [vp, i32, i32]),
     "roc_host_batch_norm": (i32, [vp, i32, f32, f32]),
     "roc_host_get_batch_norm_stats": (i32, [vp, i32, vp, vp]),
     "roc_host_set_batch_norm_stats": (i32, [vp, i32, vp, vp]),

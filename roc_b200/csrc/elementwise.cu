@@ -77,7 +77,7 @@ k_norm(int64_t rows, int Wq, uint64_t colLeft, const uint64_t* __restrict__ rowE
 }
 
 // ---------------------------------------------------------- generic maps ----
-enum { OP_RELU_F, OP_SIGM_F, OP_RELU_B, OP_SIGM_B, OP_ADD_F, OP_COPY };
+enum { OP_RELU_F, OP_SIGM_F, OP_RELU_B, OP_SIGM_B, OP_ADD_F, OP_COPY, OP_ELU_F, OP_ELU_B };
 
 template <int OP, int VEC, bool ACC>
 __global__ void __launch_bounds__(EW_T)
@@ -105,6 +105,8 @@ k_map(int64_t rows, int Wq, const float* __restrict__ a, int64_t lda, const floa
       else if (OP == OP_SIGM_F) res = 1.0f / (1.0f + expf(-av[k]));
       else if (OP == OP_RELU_B) res = (av[k] > 0.f) ? bv[k] : 0.f;           // a = y, b = dy
       else if (OP == OP_SIGM_B) res = bv[k] * av[k] * (1.0f - av[k]);
+      else if (OP == OP_ELU_F) res = av[k] > 0.f ? av[k] : expm1f(av[k]);     // NaN: expm1f(NaN) = NaN
+      else if (OP == OP_ELU_B) res = bv[k] * (av[k] > 0.f ? 1.0f : av[k] + 1.0f);   // a = y, b = dy
       else if (OP == OP_ADD_F) res = av[k] + bv[k];
       else res = av[k];
       ov[k] = ACC ? ov[k] + res : res;
@@ -824,6 +826,7 @@ extern "C" int roc_activation_fwd(int64_t rows, int H, int mode, const float* x,
   cudaStream_t st = as_stream(stream);
   if (mode == ROC_AC_MODE_RELU) return launch_map<OP_RELU_F, false>(rows, H, x, ldX, nullptr, 0, y, ldY, st);
   if (mode == ROC_AC_MODE_SIGMOID) return launch_map<OP_SIGM_F, false>(rows, H, x, ldX, nullptr, 0, y, ldY, st);
+  if (mode == ROC_AC_MODE_ELU) return launch_map<OP_ELU_F, false>(rows, H, x, ldX, nullptr, 0, y, ldY, st);
   return ROC_ERR_UNSUPPORTED;
 }
 
@@ -838,6 +841,9 @@ extern "C" int roc_activation_bwd(int64_t rows, int H, int mode, const float* y,
   if (mode == ROC_AC_MODE_SIGMOID)
     return accumulate ? launch_map<OP_SIGM_B, true>(rows, H, y, ldY, dY, ldDY, dX, ldDX, st)
                       : launch_map<OP_SIGM_B, false>(rows, H, y, ldY, dY, ldDY, dX, ldDX, st);
+  if (mode == ROC_AC_MODE_ELU)
+    return accumulate ? launch_map<OP_ELU_B, true>(rows, H, y, ldY, dY, ldDY, dX, ldDX, st)
+                      : launch_map<OP_ELU_B, false>(rows, H, y, ldY, dY, ldDY, dX, ldDX, st);
   return ROC_ERR_UNSUPPORTED;
 }
 

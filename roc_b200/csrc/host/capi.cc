@@ -106,6 +106,10 @@ int roc_host_set_edge_grad(roc_host* h, int edges, int on) { h->m().set_edge_gra
 int roc_host_get_aggr_index(roc_host* h, int t, uint32_t* host) { h->m().get_aggr_index(h->at(t), host); return 0; }
 int roc_host_relu(roc_host* h, int t) { return h->push(h->m().relu(h->at(t))); }
 int roc_host_sigmoid(roc_host* h, int t) { return h->push(h->m().sigmoid(h->at(t))); }
+int roc_host_elu(roc_host* h, int t) { return h->push(h->m().elu(h->at(t))); }
+int roc_host_attention_scores(roc_host* h, int t, int heads) {
+  return h->push(h->m().attention_scores(h->at(t), heads));
+}
 int roc_host_add(roc_host* h, int a, int b) { return h->push(h->m().add(h->at(a), h->at(b))); }
 int roc_host_batch_norm(roc_host* h, int t, float momentum, float eps) {
   return h->push(h->m().batch_norm(h->at(t), momentum, eps));

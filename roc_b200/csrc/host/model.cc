@@ -139,6 +139,14 @@ Tensor Model::attention_gather(const Tensor& input, const Tensor& scores, int he
   layers.push_back(op);
   return op->outputs[0];
 }
+Tensor Model::attention_scores(const Tensor& input, int heads) {
+  if (ctx->numParts > 1)
+    ROC_FATAL("attention_scores: runs on one partition only (numParts > 1 is not supported)");
+  AttentionScores* op = new AttentionScores(*this, input, heads);
+  layers.push_back(op);
+  parameters.push_back(op->a);
+  return op->outputs[0];
+}
 Tensor Model::scatter_gather(const Tensor& input, const Tensor& edgeWeights) {
   if (ctx->numParts > 1)
     ROC_FATAL("scatter_gather: edge-weighted aggregation runs on one partition only (numParts > 1 is not supported)");
@@ -209,6 +217,7 @@ Tensor Model::indegree_norm(const Tensor& _input) {
   return op->outputs[0];
 }
 Tensor Model::linear(const Tensor& _input, int outDim, ActiMode activation, Initializer* initializer) {
+  if (activation == AC_MODE_ELU) ROC_FATAL("linear: a Linear cannot apply AC_MODE_ELU; call elu() on its output");
   Linear* op = new Linear(*this, _input, outDim, activation, initializer);
   layers.push_back(op);
   parameters.push_back(op->weight);   // linear.cc:30
@@ -221,6 +230,11 @@ Tensor Model::relu(const Tensor& _input) {
 }
 Tensor Model::sigmoid(const Tensor& _input) {
   GnnOp* op = new Activation(*this, _input, AC_MODE_SIGMOID);
+  layers.push_back(op);
+  return op->outputs[0];
+}
+Tensor Model::elu(const Tensor& _input) {
+  GnnOp* op = new Activation(*this, _input, AC_MODE_ELU);
   layers.push_back(op);
   return op->outputs[0];
 }
@@ -237,17 +251,19 @@ Tensor Model::batch_norm(const Tensor& input, float momentum, float eps) {
 void Model::train_mode(void) { mode = MD_MODE_TRAIN; }
 void Model::infer_mode(void) { mode = MD_MODE_INFER; }
 
-const char* const roc::host::opKindNames[ROC_HOST_OP_BATCH_NORM + 1] = {
+const char* const roc::host::opKindNames[ROC_HOST_OP_ATTENTION_SCORES + 1] = {
     "linear", "indegree_norm", "scatter_gather", "scatter_gather(max)", "scatter_gather(min)",
     "scatter_gather(weighted)", "attention_gather", "relu", "sigmoid", "add", "dropout", "softmax_cross_entropy",
-    "sigmoid_cross_entropy", "batch_norm"};
+    "sigmoid_cross_entropy", "batch_norm", "elu", "attention_scores"};
 int roc::host::op_kind(const GnnOp* op) {
   if (const ScatterGather* sg = dynamic_cast<const ScatterGather*>(op))
     return sg->aggr == AGGR_MAX   ? ROC_HOST_OP_SCATTER_GATHER_MAX
            : sg->aggr == AGGR_MIN ? ROC_HOST_OP_SCATTER_GATHER_MIN
                                   : ROC_HOST_OP_SCATTER_GATHER;
   if (const Activation* a = dynamic_cast<const Activation*>(op))
-    return a->actiMode == AC_MODE_RELU ? ROC_HOST_OP_RELU : ROC_HOST_OP_SIGMOID;
+    return a->actiMode == AC_MODE_RELU ? ROC_HOST_OP_RELU
+           : a->actiMode == AC_MODE_ELU ? ROC_HOST_OP_ELU
+                                        : ROC_HOST_OP_SIGMOID;
   return dynamic_cast<const Linear*>(op)                  ? ROC_HOST_OP_LINEAR
          : dynamic_cast<const InDegreeNorm*>(op)          ? ROC_HOST_OP_INDEGREE_NORM
          : dynamic_cast<const WeightedScatterGather*>(op) ? ROC_HOST_OP_SCATTER_GATHER_WEIGHTED
@@ -256,6 +272,7 @@ int roc::host::op_kind(const GnnOp* op) {
          : dynamic_cast<const SoftmaxCrossEntropy*>(op)   ? ROC_HOST_OP_SOFTMAX_CROSS_ENTROPY
          : dynamic_cast<const SigmoidCrossEntropy*>(op)   ? ROC_HOST_OP_SIGMOID_CROSS_ENTROPY
          : dynamic_cast<const BatchNorm*>(op)             ? ROC_HOST_OP_BATCH_NORM
+         : dynamic_cast<const AttentionScores*>(op)       ? ROC_HOST_OP_ATTENTION_SCORES
                                                           : ROC_HOST_OP_ADD;
 }
 
@@ -312,7 +329,7 @@ static void mark_gradients(const Model& m) {
     bool any = false;
     for (int j = 0; j < op->numInputs; j++)
       if (op->inputs[j].region >= 0) any = any || rt->t(op->inputs[j].region).requiresGrad;
-    if (as<Linear>(op) || as<BatchNorm>(op)) any = true;   // their own parameters
+    if (as<Linear>(op) || as<BatchNorm>(op) || as<AttentionScores>(op)) any = true;   // their own parameters
     for (int j = 0; j < op->numOutputs; j++) {
       rt->t(op->outputs[j].region).requiresGrad = any;
       rt->t(op->outputs[j].region).produced = true;
@@ -567,7 +584,8 @@ static void choose_bf16_aggregation(RuntimeImpl* rt, const std::vector<GnnOp*>& 
     make_bf16(rt, r);
   }
   // ... and what a Linear(NONE) or an unfused relu writes when a max / min, weighted or attention aggregation reads it
-  // as its feature input, and every other reader is one of those or a Linear reading it as X (no fused dropout)
+  // as its feature input, and every other reader is one of those, a Linear reading it as X (no fused dropout) or an
+  // attention_scores
   for (size_t l = 0; l < layers.size(); l++) {
     int r = -1;
     if (Linear* lin = as<Linear>(layers[l]))
@@ -583,7 +601,7 @@ static void choose_bf16_aggregation(RuntimeImpl* rt, const std::vector<GnnOp*>& 
         Linear* lin = as<Linear>(op);
         if (j == 0 && ((sg && sg->aggr != AGGR_SUM) || as<WeightedScatterGather>(op) || as<AttentionGather>(op)))
           aggregated = true;
-        else if (!(j == 0 && lin && lin->dropOp < 0))
+        else if (!(j == 0 && ((lin && lin->dropOp < 0) || as<AttentionScores>(op))))
           others = false;
       }
     if (aggregated && others) make_bf16(rt, r);
@@ -1181,6 +1199,48 @@ void AttentionGather::backward(const Model& model) {
   rt->sg_end();
   for (int i = 0; i < 2; i++)
     if (rt->t(inputs[i].region).requiresGrad && !resetInputGrads[i]) add_scratch(model, inputs[i].region, scratch[i]);
+}
+
+// ------------------------------------------------------- AttentionScores -----
+AttentionScores::AttentionScores(const Model& model, const Tensor& _input, int _heads)
+    : GnnOp(_input), heads(_heads), workspace(nullptr), workspaceBytes(0) {
+  ROC_ASSERT(_input.type == Tensor::NODE_TENSOR && _input.numDim == 2 && _input.dims[1] == model.myGraph.numNodes);
+  const int64_t H = (int64_t)_input.dims[0];
+  if (_heads <= 0 || H % _heads) ROC_FATAL("attention_scores: the input width must be heads * F with heads >= 1");
+  if (H > 1024) ROC_FATAL("attention_scores: the input width must be at most 1024");
+  a = model.create_weight_tensor((int)(H / _heads), 2 * _heads, NULL);   // a Linear F -> 2 * heads's GlorotUniform
+  numOutputs = 1;
+  outputs[0] = model.create_node_tensor<DATATYPE>(2 * _heads);
+}
+void AttentionScores::init(const Model& model) {
+  workspaceBytes = roc_attn_scores_workspace_bytes(model.local_rows(), (int)inputs[0].dims[0], heads);
+  workspace = model.ctx->dmalloc(std::max<size_t>(workspaceBytes, 16));
+}
+void AttentionScores::forward(const Model& model) {
+  RuntimeImpl* rt = model.ctx;
+  const int x = inputs[0].region, s = outputs[0].region, H = (int)inputs[0].dims[0];
+  if (rt->t(x).isBf16)   // set_bf16_aggregation: GAT's wh
+    ROC_CHECK(roc_attn_scores_fwd_bf16(model.local_rows(), H, heads, rt->data_bf16(x), rt->t(x).ld, rt->data(a.region),
+                                       rt->data(s), rt->t(s).ld, rt->stream));
+  else
+    ROC_CHECK(roc_attn_scores_fwd(model.local_rows(), H, heads, rt->data(x), rt->t(x).ld, rt->data(a.region),
+                                  rt->data(s), rt->t(s).ld, rt->stream));
+}
+// dA is overwritten; dX is written by the first op to run backward on the input (resetInputGrads) and added to in the
+// others (in GAT the attention_gather has written it)
+void AttentionScores::backward(const Model& model) {
+  RuntimeImpl* rt = model.ctx;
+  const int x = inputs[0].region, s = outputs[0].region, H = (int)inputs[0].dims[0];
+  float* dX = rt->t(x).requiresGrad ? rt->grad(x) : nullptr;
+  const int acc = resetInputGrads[0] ? 0 : 1;
+  if (rt->t(x).isBf16)
+    ROC_CHECK(roc_attn_scores_bwd_bf16(model.local_rows(), H, heads, rt->data_bf16(x), rt->t(x).ld, rt->data(a.region),
+                                       rt->grad(s), rt->t(s).ld, dX, rt->t(x).ld, acc, rt->grad(a.region), workspace,
+                                       workspaceBytes, rt->stream));
+  else
+    ROC_CHECK(roc_attn_scores_bwd(model.local_rows(), H, heads, rt->data(x), rt->t(x).ld, rt->data(a.region),
+                                  rt->grad(s), rt->t(s).ld, dX, rt->t(x).ld, acc, rt->grad(a.region), workspace,
+                                  workspaceBytes, rt->stream));
 }
 
 // ------------------------------------------------- WeightedScatterGather -----

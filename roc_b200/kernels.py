@@ -665,6 +665,64 @@ def batchnorm_bwd(x, dy, gamma, state, relu=False, dx=None, accumulate=False, ne
     return dx, dgamma, dbeta
 
 
+def _check_a(a, h, heads):
+    """the C ABI reads A as a dense [2 * heads][F] fp32 array"""
+    assert a.dtype == torch.float32 and a.is_contiguous() and tuple(a.shape) == (2 * int(heads), h // int(heads)), \
+        "a must be a contiguous fp32 [2 * heads][F] tensor"
+
+
+def attn_scores_fwd(x, a, heads, out=None):
+    """roc_attn_scores_fwd on fp32 x [rows][H] (H = heads * F) and a [2 * heads][F]: returns s [rows][2 * heads] =
+    [s_dst | s_src] (padded rows unless `out` is given)."""
+    rows, h = x.shape
+    _check_a(a, h, heads)
+    if out is None:
+        out = padded(rows, 2 * heads, x.device)
+    check(lib.roc_attn_scores_fwd(rows, h, int(heads), _ptr(x), _ld(x), _ptr(a), _ptr(out), _ld(out), _stream()),
+          "roc_attn_scores_fwd")
+    return out
+
+
+def attn_scores_fwd_bf16(x, a, heads, out=None):
+    """roc_attn_scores_fwd_bf16: attn_scores_fwd() on bf16 rows (the bytes of the fp32 call on x.float())."""
+    assert x.dtype == torch.bfloat16
+    rows, h = x.shape
+    _check_a(a, h, heads)
+    if out is None:
+        out = padded(rows, 2 * heads, x.device)
+    check(lib.roc_attn_scores_fwd_bf16(rows, h, int(heads), _ptr(x), _ld(x), _ptr(a), _ptr(out), _ld(out),
+                                       _stream()), "roc_attn_scores_fwd_bf16")
+    return out
+
+
+def _attn_scores_bwd(fn, x, a, ds, heads, dx, accumulate, need_dx):
+    rows, h = x.shape
+    _check_a(a, h, heads)
+    if need_dx and dx is None:
+        dx = padded(rows, h, x.device)
+    if not need_dx:
+        dx = None
+    da = torch.empty(a.shape, device=x.device)
+    ws_bytes = lib.roc_attn_scores_workspace_bytes(rows, h, int(heads))
+    ws = torch.empty(max(ws_bytes, 16), device=x.device, dtype=torch.uint8)
+    check(getattr(lib, fn)(rows, h, int(heads), _ptr(x), _ld(x), _ptr(a), _ptr(ds), _ld(ds), _ptr(dx),
+                           _ld(dx) if dx is not None else 0, int(bool(accumulate)), _ptr(da), _ptr(ws), ws_bytes,
+                           _stream()), fn)
+    return dx, da
+
+
+def attn_scores_bwd(x, a, ds, heads, dx=None, accumulate=False, need_dx=True):
+    """roc_attn_scores_bwd: returns (dx, da).  dx is written into (accumulate=True: added to) `dx` when given;
+    need_dx=False computes da only (dx is then None)."""
+    return _attn_scores_bwd("roc_attn_scores_bwd", x, a, ds, heads, dx, accumulate, need_dx)
+
+
+def attn_scores_bwd_bf16(x, a, ds, heads, dx=None, accumulate=False, need_dx=True):
+    """roc_attn_scores_bwd_bf16: attn_scores_bwd() on bf16 rows of x; dx stays fp32."""
+    assert x.dtype == torch.bfloat16
+    return _attn_scores_bwd("roc_attn_scores_bwd_bf16", x, a, ds, heads, dx, accumulate, need_dx)
+
+
 def linear_bwd(x, w, y, dy, dw, dx=None, activation=0, accumulate_dx=False):
     ws_bytes = lib.roc_linear_bwd_workspace_bytes(x.shape[0], x.shape[1], w.shape[0])
     ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=x.device)

@@ -131,8 +131,19 @@ class Model:
         LeakyReLU(s_dst[v] + s_src[u]); scores has 2 * heads columns [s_dst | s_src].  One partition only."""
         return lib.roc_host_attention_gather(self.h, t, scores, int(heads), float(negative_slope))
 
+    def attention_scores(self, t, heads=1):
+        """GAT's per-head scores of t (H = heads * F columns): [s_dst | s_src], 2 * heads columns, the scores attention_gather
+        takes.  Head k's scores are the dot products of its own F columns with its a_dst and a_src.  Appends one parameter
+        A of parameter_shape (F, 2 * heads), so get_parameter returns it as (2 * heads, F): rows 0 .. heads - 1 the a_dst,
+        the rest the a_src, drawn as a Linear F -> 2 * heads draws its W.  One partition only."""
+        return lib.roc_host_attention_scores(self.h, t, int(heads))
+
     def relu(self, t):
         return lib.roc_host_relu(self.h, t)
+
+    def elu(self, t):
+        """ELU with alpha = 1: x > 0 ? x : exp(x) - 1.  Never fused; linear() does not take it as an activation."""
+        return lib.roc_host_elu(self.h, t)
 
     def sigmoid(self, t):
         return lib.roc_host_sigmoid(self.h, t)
@@ -539,24 +550,34 @@ def build_sage_pool(model, layers, dropout_rate, aggr=_lib.AGGR_MAX, lr=0.01, we
 
 
 def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01, weight_decay=0.05,
-              exact_backward=False, features="float32", aggregation="float32", loss="softmax", norm=None):
+              exact_backward=False, features="float32", aggregation="float32", loss="softmax", norm=None,
+              scores="dense", activation="relu"):
     """GAT (Velickovic et al., 2018) built from the reference's ops plus attention_gather.  `heads` (an int, or one
     value per hidden layer) applies to the hidden layers; the last layer has one head.  layers[i] is the width of
     layer i's output, heads_i * F_i.  Per layer:
 
         d  = dropout(t)
         wh = linear(d, layers[i])                       # heads_i * F_i columns
-        sc = linear(wh, 2 * heads_i)                    # [s_dst | s_src] per head
+        sc = linear(wh, 2 * heads_i)                    # scores="dense": [s_dst | s_src] per head
+        sc = attention_scores(wh, heads_i)              # scores="per_head": the same, head k from its own F columns
         t  = attention_gather(wh, sc, heads_i, slope)   # per head, softmax over N(v) + v (self loops are in A)
-        t  = relu(t)                                    # all but the last layer
+        t  = relu(t)                                    # all but the last layer; activation="elu": elu(t)
 
-    Where this differs from the paper: there is no bias (the reference's Linear has none); ReLU replaces ELU (the
-    engine has no ELU); with heads > 1 each head's scores are a dense projection of all heads' features, where the
-    paper uses a per-head block.  With one head it is GAT exactly.  Single partition.  aggregation="bfloat16" stores
-    wh, which the attention_gather and the score linear read, in bf16 (Model.set_bf16_aggregation).  norm="batch":
-    batch_norm on t before each hidden relu (see build_gcn).  Returns the handles, with `attn` (the attention_gather
-    outputs), `attn_ins` (their feature inputs) and `scores`."""
+    scores="per_head" gives each head its own a_dst and a_src (Model.attention_scores), as the paper and PyG's GATConv
+    do; the default "dense" projects all heads' features for every head's scores, which is the same function only
+    with one head.  activation="elu" uses the paper's ELU in place of ReLU.  With both, the model is the paper's GAT
+    without bias, with any number of heads.
+
+    Where this differs from the paper: there is no bias (the reference's Linear has none; norm="batch" gives a
+    per-feature shift).  Single partition.  aggregation="bfloat16" stores wh, which the attention_gather and the score
+    op read, in bf16 (Model.set_bf16_aggregation).  norm="batch": batch_norm on t before each hidden activation (see
+    build_gcn).  Returns the handles, with `attn` (the attention_gather outputs), `attn_ins` (their feature inputs),
+    `scores` and `relu_outs` (the hidden activations' outputs, ELU or ReLU)."""
     _check_norm(norm)
+    if scores not in ("dense", "per_head"):
+        raise ValueError("scores must be \"dense\" or \"per_head\"")
+    if activation not in ("relu", "elu"):
+        raise ValueError("activation must be \"relu\" or \"elu\"")
     L = len(layers)
     hs = list(heads) if isinstance(heads, (list, tuple)) else [int(heads)] * (L - 2)
     assert len(hs) == L - 2, "one head count per hidden layer"
@@ -564,18 +585,22 @@ def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01,
     x = _input_tensor(model, layers[0], features)
     label = model.create_node_tensor(layers[-1])
     mask = model.create_node_tensor(1, is_int=True)
+    act = model.elu if activation == "elu" else model.relu
     t = x
-    relu_outs, attn, attn_ins, scores, bns = [], [], [], [], []
+    relu_outs, attn, attn_ins, score_outs, bns = [], [], [], [], []
     for i in range(1, L):
         d = model.dropout(t, dropout_rate)
         wh = model.linear(d, layers[i], _lib.AC_MODE_NONE)
-        sc = model.linear(wh, 2 * hs[i - 1], _lib.AC_MODE_NONE)
+        if scores == "per_head":
+            sc = model.attention_scores(wh, hs[i - 1])
+        else:
+            sc = model.linear(wh, 2 * hs[i - 1], _lib.AC_MODE_NONE)
         t = model.attention_gather(wh, sc, hs[i - 1], negative_slope)
         attn_ins.append(wh)
-        scores.append(sc)
+        score_outs.append(sc)
         attn.append(t)
         if i != L - 1:
-            t = model.relu(_hidden_norm(model, norm, t, bns))
+            t = act(_hidden_norm(model, norm, t, bns))
             relu_outs.append(t)
     _loss(model, loss, t, label, mask)
     model.adam(lr, weight_decay)
@@ -584,7 +609,7 @@ def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01,
     _aggregation(model, aggregation)
     model.init()
     return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs, "attn": attn,
-            "attn_ins": attn_ins, "scores": scores, "bns": bns}
+            "attn_ins": attn_ins, "scores": score_outs, "bns": bns}
 
 
 def build_gcn_weighted(model, layers, dropout_rate, edge_weights, edge_grad=False, lr=0.01, weight_decay=0.05,

@@ -241,6 +241,55 @@ int roc_sg_attn_backward_planned_bf16(const roc_sg_plan* plan, int heads, int H,
                                       const float* outGrad, int64_t ldG, float* inGrad, int64_t ldInG,
                                       float* scoreGrad, int64_t ldSG, roc_stream_t stream);
 
+/* Attention dropout (the paper's dropout of the normalised attention coefficients; PyG GATConv(dropout=), DGL
+ * GATConv(attn_drop=)).  y, m, Z, a and stats are as above: m and Z come from the undropped softmax.  For plan row r
+ * with id i = selfBase + r and each in-edge's source j = colSrc[e], with T16 = round(rate * 65536) as in
+ * roc_dropout_fwd:
+ *   keep(i<-j,k) = 16-bit lane k of Philox4x32-10(counter = {i, j, 0, step}, key = {seed lo, seed hi}) >= T16
+ * with the lanes numbered as in roc_dropout_fwd: one Philox block decides all heads of one (destination, source) pair.
+ * The mask is keyed by the pair, not by the edge's position, so any edge order computes it, and the duplicate edges of
+ * a multigraph share it.  With s = 1.0f / (1.0f - rate) (fp32, roc_dropout_fwd's scale) and M = keep ? s : 0:
+ *   a'(i<-j,k)   = keep(i<-j,k) ? a(i<-j,k) * s : 0
+ *   out[r][kF+f] = sum_e a'(i<-j,k) * in[j][kF+f]
+ * Backward, with D[i][k] = sum_f G[i][kF+f] O[i][kF+f] over the dropped output O:
+ *   dz(i<-j,k)   = a(i<-j,k) (M(i<-j,k) sum_f G[i][kF+f] X[j][kF+f] - D[i][k]) l
+ *   inGrad gathers a'(i<-j,k) G[i] where the calls above gather a(i<-j,k) G[i]; d s_dst and d s_src are the sums of
+ *   dz as there.
+ * The passes read the mask as one keep byte per edge (bit k = head k), made by roc_sg_attn_keep_mask:
+ *   keep     the forward plan's edge order, pairs (i <- j) with the row the destination        (the forward and B1)
+ *   keepRev  the same plan's order with the row the source: edge e of row r holds keep(j <- i)  (the planned B2)
+ *   keepT    the transposed plan's order (roc_sg_transpose_info's planT, selfBase 0), the row the source (exact B2)
+ * rate = 0, or NULL masks: the calls above, byte for byte.  ROC_ERR_INVALID also for a rate outside [0, 1) and, in a
+ * backward, for one NULL mask of two.  Everything else (shapes, errors, determinism, the launches but the main
+ * kernels' reduction numbers) is the call without dropout's. */
+int roc_sg_attn_forward_dropout_planned(const roc_sg_plan* plan, int heads, int H, float slope, roc_vid_t selfBase,
+                                        const float* in, int64_t ldIn, const float* score, int64_t ldS, float* out,
+                                        int64_t ldOut, float* stats, int64_t ldStats, const uint8_t* keep, float rate,
+                                        roc_stream_t stream);
+int roc_sg_attn_forward_dropout_planned_bf16(const roc_sg_plan* plan, int heads, int H, float slope,
+                                             roc_vid_t selfBase, const uint16_t* in, int64_t ldIn, const float* score,
+                                             int64_t ldS, float* out, int64_t ldOut, float* stats, int64_t ldStats,
+                                             const uint8_t* keep, float rate, roc_stream_t stream);
+int roc_sg_attn_backward_dropout_planned(const roc_sg_plan* plan, int heads, int H, float slope, roc_vid_t selfBase,
+                                         const float* in, int64_t ldIn, const float* score, int64_t ldS,
+                                         const float* out, int64_t ldOut, const float* stats, int64_t ldStats,
+                                         const float* outGrad, int64_t ldG, float* inGrad, int64_t ldInG,
+                                         float* scoreGrad, int64_t ldSG, const uint8_t* keep, const uint8_t* keepRev,
+                                         float rate, roc_stream_t stream);
+int roc_sg_attn_backward_dropout_planned_bf16(const roc_sg_plan* plan, int heads, int H, float slope,
+                                              roc_vid_t selfBase, const uint16_t* in, int64_t ldIn, const float* score,
+                                              int64_t ldS, const float* out, int64_t ldOut, const float* stats,
+                                              int64_t ldStats, const float* outGrad, int64_t ldG, float* inGrad,
+                                              int64_t ldInG, float* scoreGrad, int64_t ldSG, const uint8_t* keep,
+                                              const uint8_t* keepRev, float rate, roc_stream_t stream);
+/* The keep bytes of every edge of `plan` in its edge order: keep[e - colLeft] bit k = keep(i<-j,k) for all 8 lanes,
+ * with, for edge e of plan row r and c = colSrc[e], (i, j) = (selfBase + r, c) when rowIsSource == 0 (the forward
+ * order) and (c, selfBase + r) when rowIsSource == 1 (keepRev over the forward plan, keepT over the transposed plan
+ * with selfBase 0).  One Philox block per edge, E bytes written.  ROC_ERR_INVALID: a NULL plan, a NULL keep with
+ * edges, rowIsSource not 0 or 1, a rate outside [0, 1).  Launch: ROC_SG_LAUNCH_KEEP_MASK. */
+int roc_sg_attn_keep_mask(const roc_sg_plan* plan, roc_vid_t selfBase, int rowIsSource, float rate, uint64_t seed,
+                          uint32_t step, uint8_t* keep, roc_stream_t stream);
+
 /* Edge-weighted aggregation (GCN with edge weights, weighted graphs, edge saliency).  The reference declares edge
  * tensors (gnn.h:178) but never reads them; these semantics are this library's own.  For plan row r with id
  * i = selfBase + r and in-edges e in CSR order with sources j = colSrc[e], the edge's weight is w[e - colLeft]: a flat
@@ -341,6 +390,21 @@ int roc_sg_attn_backward_exact_bf16(const roc_sg_plan* plan, roc_sg_transpose* t
                                     const float* out, int64_t ldOut, const float* stats, int64_t ldStats,
                                     const float* outGrad, int64_t ldG, float* inGrad, int64_t ldInG, float* scoreGrad,
                                     int64_t ldSG, roc_stream_t stream);
+/* roc_sg_attn_backward_exact and its bf16 form with attention dropout (see roc_sg_attn_forward_dropout_planned): keep
+ * in the forward plan's edge order, keepT in the transposed plan's (roc_sg_attn_keep_mask over planT, selfBase 0,
+ * rowIsSource 1). */
+int roc_sg_attn_backward_dropout_exact(const roc_sg_plan* plan, roc_sg_transpose* transpose, int heads, int H,
+                                       float slope, const float* in, int64_t ldIn, const float* score, int64_t ldS,
+                                       const float* out, int64_t ldOut, const float* stats, int64_t ldStats,
+                                       const float* outGrad, int64_t ldG, float* inGrad, int64_t ldInG,
+                                       float* scoreGrad, int64_t ldSG, const uint8_t* keep, const uint8_t* keepT,
+                                       float rate, roc_stream_t stream);
+int roc_sg_attn_backward_dropout_exact_bf16(const roc_sg_plan* plan, roc_sg_transpose* transpose, int heads, int H,
+                                            float slope, const uint16_t* in, int64_t ldIn, const float* score,
+                                            int64_t ldS, const float* out, int64_t ldOut, const float* stats,
+                                            int64_t ldStats, const float* outGrad, int64_t ldG, float* inGrad,
+                                            int64_t ldInG, float* scoreGrad, int64_t ldSG, const uint8_t* keep,
+                                            const uint8_t* keepT, float rate, roc_stream_t stream);
 
 /* Plan-less form with exactly the reference kernel's argument list
  * (scattergather_kernel.cu:21-28, EdgeStruct.dst dropped), dense ld == H.
@@ -370,7 +434,10 @@ int roc_sg_backward(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft, in
  *          min backward, 12 the sum over bf16 rows (its main kernel and ring); 16 + r for the main kernel of
  *          reduction r over bf16 feature rows (17 max, 18 min, 21 attention forward, 22 d s_dst, 23 input gradient,
  *          24 weighted sum, 25 edge-weight gradient: the roc_sg_*_bf16 calls), whose fix-ups are reduction r's and
- *          report as there; -1 for the record and the permutation, which have none.  A sum fix-up finishing another
+ *          report as there; 32 + r for the main kernel of attention pass r (5, 6, 7, or 21, 22, 23 on bf16 feature
+ *          rows) with dropout (the roc_sg_attn_*_dropout_* calls at rate > 0: 37, 38, 39, 53, 54, 55), whose other
+ *          launches report as without dropout; -1 for the record, the permutation and the keep mask, which have
+ *          none.  A sum fix-up finishing another
  *          reduction's partials reports 0.
  *   vec    4 for float4 rows, else 1;  lanes, nch: the row shape (L lanes, chunks per lane);  grid: CTAs launched
  * count is the number of launches; the first ROC_SG_MAX_LAUNCHES are stored.  Every planned call clears the list first,
@@ -384,6 +451,7 @@ int roc_sg_backward(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft, in
 #define ROC_SG_LAUNCH_HEADS_FIXUP 6
 #define ROC_SG_LAUNCH_HEADS_BIG_FIXUP 7
 #define ROC_SG_LAUNCH_PERMUTE 8
+#define ROC_SG_LAUNCH_KEEP_MASK 9     /* roc_sg_attn_keep_mask (red -1) */
 #define ROC_SG_MAX_LAUNCHES 32
 typedef struct {
   int kind, red, vec, lanes, nch;

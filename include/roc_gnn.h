@@ -193,8 +193,12 @@ public:
    * head; the output has the input's width, each head's block of H / heads columns weighted by that head's
    * softmax over the row's in-edges.  Its backward is a gather over the same CSR (quirk Q1): exact for the
    * destination scores, the true gradient of the rest on a symmetric graph.  Never fused with neighbouring ops.
-   * Single partition only (exit(1) otherwise). */
-  Tensor attention_gather(const Tensor& input, const Tensor& scores, int heads, float negativeSlope = 0.2f);
+   * Single partition only (exit(1) otherwise).  dropout > 0: attention dropout at that rate in train mode
+   * (roc_sg_attn_forward_dropout_planned), each step's keep mask drawn from Philox with key (seed << 32) | the op's
+   * position and the model's train step, as Model::dropout draws its own; infer mode and dropout = 0 run the plain
+   * calls.  A rate outside [0, 1) exits. */
+  Tensor attention_gather(const Tensor& input, const Tensor& scores, int heads, float negativeSlope = 0.2f,
+                          float dropout = 0.0f, int seed = 0);
   /* The per-head GAT scores of `input` (H = heads * F columns; roc_attn_scores_fwd / _bwd): a [rows][2 * heads] output
    * [s_dst | s_src], head k's scores the dot products of its own F columns with its a_dst and a_src.  Appends one
    * parameter A, a weight tensor of dims {F, 2 * heads} (row k: a_dst of head k, row heads + k: its a_src), drawn by the
@@ -345,15 +349,25 @@ public:
 
 class AttentionGather : public GnnOp {  /* not in the reference: Model::attention_gather */
 public:
-  AttentionGather(const Model& model, const Tensor& input, const Tensor& scores, int heads, float slope);
+  AttentionGather(const Model& model, const Tensor& input, const Tensor& scores, int heads, float slope, float dropRate,
+                  int seed);
   virtual void init(const Model& model);
   virtual void forward(const Model& model);
   virtual void backward(const Model& model);
   int heads;
   float slope;
+  float dropRate;    /* attention dropout in train mode (0: none) */
+  int seed;
+  int opIndex;       /* position in the model: the Philox key is (seed << 32) | opIndex, as a Dropout's */
+  uint8_t* keep;     /* [E] keep bytes of the last training forward, in the plan's edge order (Runtime arena) */
+  uint8_t* keep2;    /* [E] the backward's input-gradient pass's: reverse pairs, or the transposed plan's order */
   float* stats;      /* [Nloc][statsLd] m | 1/Z per head of the last forward (Runtime arena) */
   int64_t statsLd;
   float* scratch[2]; /* gradients of an input that accumulates (or needs none), written here first (Runtime arena) */
+private:
+  float drop_rate(const Model& model) const;
+  uint64_t drop_key() const;
+  void keep_mask(const Model& model, const roc_sg_plan* plan, roc_vid_t selfBase, int rowIsSource, uint8_t*& buf);
 };
 
 class AttentionScores : public GnnOp {  /* not in the reference: Model::attention_scores */

@@ -47,6 +47,8 @@ int roc_host_scatter_gather(roc_host* h, int t);
 int roc_host_scatter_gather_aggr(roc_host* h, int t, int aggr);
 /* Model::attention_gather(t, scores, heads, slope); scores has 2 * heads columns */
 int roc_host_attention_gather(roc_host* h, int t, int scores, int heads, float slope);
+/* Model::attention_gather(t, scores, heads, slope, rate, seed): with attention dropout at `rate` in train mode */
+int roc_host_attention_gather_dropout(roc_host* h, int t, int scores, int heads, float slope, float rate, int seed);
 /* Model::create_edge_tensor<float>(hidden): rows = this partition's edge count */
 int roc_host_create_edge_tensor(roc_host* h, int hidden);
 /* Model::scatter_gather(t, edges): edge-weighted aggregation */

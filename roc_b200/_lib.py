@@ -51,9 +51,9 @@ class GemmInfo(C.Structure):
 
 SG_LAUNCH_MAIN, SG_LAUNCH_RING, SG_LAUNCH_FIXUP, SG_LAUNCH_BIG_FIXUP = 0, 1, 2, 3      # roc_sg_launch.kind
 SG_LAUNCH_STAT_FIXUP, SG_LAUNCH_RECORD, SG_LAUNCH_HEADS_FIXUP, SG_LAUNCH_HEADS_BIG_FIXUP = 4, 5, 6, 7
-SG_LAUNCH_PERMUTE = 8
+SG_LAUNCH_PERMUTE, SG_LAUNCH_KEEP_MASK = 8, 9
 SG_LAUNCH_KINDS = ("main", "ring", "fixup", "big_fixup", "stat_fixup", "record", "heads_fixup", "heads_big_fixup",
-                   "permute")
+                   "permute", "keep_mask")
 SG_MAX_LAUNCHES = 32
 
 
@@ -149,6 +149,15 @@ PROTOTYPES = {
     "roc_sg_edge_dot_planned": (i32, [vp, i32, vp, i64, vp, i64, vp, i32, vp]),
     "roc_sg_weighted_forward_planned_bf16": (i32, [vp, i32, vp, i64, vp, vp, i64, vp]),
     "roc_sg_edge_dot_planned_bf16": (i32, [vp, i32, vp, i64, vp, i64, vp, i32, vp]),
+    "roc_sg_attn_forward_dropout_planned": (i32, [vp, i32, i32, f32, u32, vp, i64, vp, i64, vp, i64, vp, i64, vp, f32,
+                                                  vp]),
+    "roc_sg_attn_forward_dropout_planned_bf16": (i32, [vp, i32, i32, f32, u32, vp, i64, vp, i64, vp, i64, vp, i64, vp,
+                                                       f32, vp]),
+    "roc_sg_attn_backward_dropout_planned": (i32, [vp, i32, i32, f32, u32, vp, i64, vp, i64, vp, i64, vp, i64, vp, i64,
+                                                   vp, i64, vp, i64, vp, vp, f32, vp]),
+    "roc_sg_attn_backward_dropout_planned_bf16": (i32, [vp, i32, i32, f32, u32, vp, i64, vp, i64, vp, i64, vp, i64, vp,
+                                                        i64, vp, i64, vp, i64, vp, vp, f32, vp]),
+    "roc_sg_attn_keep_mask": (i32, [vp, u32, i32, f32, u64, u32, vp, vp]),
     "roc_sg_transpose_create": (i32, [u32, vp, vp, vp, C.POINTER(vp)]),
     "roc_sg_transpose_info": (i32, [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]),
     "roc_sg_transpose_destroy": (None, [vp]),
@@ -159,6 +168,10 @@ PROTOTYPES = {
                                          vp, i64, vp]),
     "roc_sg_attn_backward_exact_bf16": (i32, [vp, vp, i32, i32, f32, vp, i64, vp, i64, vp, i64, vp, i64, vp, i64, vp,
                                               i64, vp, i64, vp]),
+    "roc_sg_attn_backward_dropout_exact": (i32, [vp, vp, i32, i32, f32, vp, i64, vp, i64, vp, i64, vp, i64, vp, i64,
+                                                 vp, i64, vp, i64, vp, vp, f32, vp]),
+    "roc_sg_attn_backward_dropout_exact_bf16": (i32, [vp, vp, i32, i32, f32, vp, i64, vp, i64, vp, i64, vp, i64, vp,
+                                                      i64, vp, i64, vp, i64, vp, vp, f32, vp]),
     "roc_sg_forward": (i32, [u32, u32, u64, i32, vp, vp, vp, vp, vp]),
     "roc_sg_backward": (i32, [u32, u32, u64, i32, vp, vp, vp, vp, vp]),
     "roc_sg_last_call_info": (i32, [C.POINTER(SgCallInfo)]),
@@ -233,6 +246,7 @@ PROTOTYPES = {
     "roc_host_scatter_gather": (i32, [vp, i32]),
     "roc_host_scatter_gather_aggr": (i32, [vp, i32, i32]),
     "roc_host_attention_gather": (i32, [vp, i32, i32, i32, f32]),
+    "roc_host_attention_gather_dropout": (i32, [vp, i32, i32, i32, f32, f32, i32]),
     "roc_host_get_aggr_index": (i32, [vp, i32, vp]),
     "roc_host_create_edge_tensor": (i32, [vp, i32]),
     "roc_host_scatter_gather_weighted": (i32, [vp, i32, i32]),

@@ -98,6 +98,9 @@ int roc_host_scatter_gather_aggr(roc_host* h, int t, int aggr) {
 int roc_host_attention_gather(roc_host* h, int t, int scores, int heads, float slope) {
   return h->push(h->m().attention_gather(h->at(t), h->at(scores), heads, slope));
 }
+int roc_host_attention_gather_dropout(roc_host* h, int t, int scores, int heads, float slope, float rate, int seed) {
+  return h->push(h->m().attention_gather(h->at(t), h->at(scores), heads, slope, rate, seed));
+}
 int roc_host_create_edge_tensor(roc_host* h, int hidden) { return h->push(h->m().create_edge_tensor<DATATYPE>(hidden)); }
 int roc_host_scatter_gather_weighted(roc_host* h, int t, int edges) {
   return h->push(h->m().scatter_gather(h->at(t), h->at(edges)));

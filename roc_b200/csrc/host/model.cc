@@ -132,10 +132,12 @@ Tensor Model::scatter_gather(const Tensor& _input, AggrType aggr) {
   ROC_FATAL("scatter_gather: unknown AggrType");
   return Tensor();
 }
-Tensor Model::attention_gather(const Tensor& input, const Tensor& scores, int heads, float negativeSlope) {
+Tensor Model::attention_gather(const Tensor& input, const Tensor& scores, int heads, float negativeSlope, float dropout,
+                               int seed) {
   if (ctx->numParts > 1)
     ROC_FATAL("attention_gather: runs on one partition only (numParts > 1 is not supported)");
-  GnnOp* op = new AttentionGather(*this, input, scores, heads, negativeSlope);
+  AttentionGather* op = new AttentionGather(*this, input, scores, heads, negativeSlope, dropout, seed);
+  op->opIndex = (int)layers.size();
   layers.push_back(op);
   return op->outputs[0];
 }
@@ -1126,8 +1128,10 @@ static void add_scratch(const Model& model, int region, const float* scratch) {
 }
 
 // ------------------------------------------------------- AttentionGather -----
-AttentionGather::AttentionGather(const Model& model, const Tensor& _input, const Tensor& _scores, int _heads, float _slope)
-    : GnnOp(_input, _scores), heads(_heads), slope(_slope), stats(nullptr), statsLd(0) {
+AttentionGather::AttentionGather(const Model& model, const Tensor& _input, const Tensor& _scores, int _heads, float _slope,
+                                 float _dropRate, int _seed)
+    : GnnOp(_input, _scores), heads(_heads), slope(_slope), dropRate(_dropRate), seed(_seed), opIndex(0),
+      keep(nullptr), keep2(nullptr), stats(nullptr), statsLd(0) {
   scratch[0] = scratch[1] = nullptr;
   ROC_ASSERT(_input.type == Tensor::NODE_TENSOR && _scores.type == Tensor::NODE_TENSOR);
   ROC_ASSERT(_input.numDim == 2 && _scores.numDim == 2);
@@ -1135,6 +1139,7 @@ AttentionGather::AttentionGather(const Model& model, const Tensor& _input, const
   if (_heads <= 0 || _scores.dims[0] != 2 * (E_ID)_heads)
     ROC_FATAL("attention_gather: the scores need 2 * heads columns ([s_dst | s_src] per head)");
   if (!(_slope >= 0.0f) || !std::isfinite(_slope)) ROC_FATAL("attention_gather: the negative slope must be finite and >= 0");
+  if (!(_dropRate >= 0.0f && _dropRate < 1.0f)) ROC_FATAL("attention_gather: the dropout rate must be in [0, 1)");
   // the layouts roc_sg_attn_* take on node tensors (rows padded to float4: the vector path)
   const int64_t H = (int64_t)_input.dims[0], F = H / _heads;
   if (_heads != 1 && _heads != 2 && _heads != 4 && _heads != 8)
@@ -1147,6 +1152,18 @@ AttentionGather::AttentionGather(const Model& model, const Tensor& _input, const
 }
 void AttentionGather::init(const Model&) {}
 
+// the attention dropout rate in the current mode (infer: none) and its Philox key
+float AttentionGather::drop_rate(const Model& model) const { return model.mode == MD_MODE_TRAIN ? dropRate : 0.0f; }
+uint64_t AttentionGather::drop_key() const { return ((uint64_t)(uint32_t)seed << 32) | (uint32_t)opIndex; }
+
+// one keep byte per edge of `plan`, in buffer `buf` (allocated on first use)
+void AttentionGather::keep_mask(const Model& model, const roc_sg_plan* plan, roc_vid_t selfBase, int rowIsSource,
+                                uint8_t*& buf) {
+  RuntimeImpl* rt = model.ctx;
+  if (!buf) buf = (uint8_t*)rt->dmalloc(std::max<size_t>((size_t)model.myGraph.numEdges, 16));
+  ROC_CHECK(roc_sg_attn_keep_mask(plan, selfBase, rowIsSource, dropRate, drop_key(), rt->trainStep, buf, rt->stream));
+}
+
 void AttentionGather::forward(const Model& model) {
   RuntimeImpl* rt = model.ctx;
   const int H = (int)inputs[0].dims[0];
@@ -1155,15 +1172,20 @@ void AttentionGather::forward(const Model& model) {
     stats = (float*)rt->dmalloc((size_t)std::max<int64_t>(model.local_rows(), 1) * (size_t)statsLd * sizeof(float));
   }
   const int x = inputs[0].region, sc = inputs[1].region, y = outputs[0].region;
+  const roc_sg_plan* plan = model.myGraph.plan;
+  const roc_vid_t self = model.myGraph.rowLeft;
+  const float rate = drop_rate(model);
+  if (rate > 0.0f) keep_mask(model, plan, self, 0, keep);
+  const uint8_t* k = rate > 0.0f ? keep : nullptr;
   rt->sg_begin(H);
   if (rt->t(x).isBf16)
-    ROC_CHECK(roc_sg_attn_forward_planned_bf16(model.myGraph.plan, heads, H, slope, model.myGraph.rowLeft,
-                                               rt->data_bf16(x), rt->t(x).ld, rt->data(sc), rt->t(sc).ld, rt->data(y),
-                                               rt->t(y).ld, stats, statsLd, rt->stream));
+    ROC_CHECK(roc_sg_attn_forward_dropout_planned_bf16(plan, heads, H, slope, self, rt->data_bf16(x), rt->t(x).ld,
+                                                       rt->data(sc), rt->t(sc).ld, rt->data(y), rt->t(y).ld, stats,
+                                                       statsLd, k, rate, rt->stream));
   else
-    ROC_CHECK(roc_sg_attn_forward_planned(model.myGraph.plan, heads, H, slope, model.myGraph.rowLeft, rt->data(x),
-                                          rt->t(x).ld, rt->data(sc), rt->t(sc).ld, rt->data(y), rt->t(y).ld, stats,
-                                          statsLd, rt->stream));
+    ROC_CHECK(roc_sg_attn_forward_dropout_planned(plan, heads, H, slope, self, rt->data(x), rt->t(x).ld, rt->data(sc),
+                                                  rt->t(sc).ld, rt->data(y), rt->t(y).ld, stats, statsLd, k, rate,
+                                                  rt->stream));
   rt->sg_end();
 }
 
@@ -1179,23 +1201,35 @@ void AttentionGather::backward(const Model& model) {
   const int ox = outputs[0].region, x = inputs[0].region, sc = inputs[1].region;
   const int64_t ldX = rt->t(x).ld, ldS = rt->t(sc).ld, ldO = rt->t(ox).ld;
   const bool xBf16 = rt->t(x).isBf16;
+  const roc_sg_plan* plan = model.myGraph.plan;
+  // the forward's mask, and the input-gradient pass's: the reverse pairs over the same plan, or the transposed plan's
+  const float rate = drop_rate(model);
+  if (rate > 0.0f) {
+    const roc_sg_plan* planT = nullptr;
+    if (model.exactBackward) ROC_CHECK(roc_sg_transpose_info(rt->sgTranspose, nullptr, nullptr, nullptr, &planT));
+    keep_mask(model, model.exactBackward ? planT : plan, model.exactBackward ? 0 : model.myGraph.rowLeft, 1, keep2);
+  }
+  const uint8_t* k1 = rate > 0.0f ? keep : nullptr;
+  const uint8_t* k2 = rate > 0.0f ? keep2 : nullptr;
   rt->sg_begin(H);
   if (model.exactBackward && xBf16)
-    ROC_CHECK(roc_sg_attn_backward_exact_bf16(model.myGraph.plan, rt->sgTranspose, heads, H, slope, rt->data_bf16(x),
-                                              ldX, rt->data(sc), ldS, rt->data(ox), ldO, stats, statsLd, rt->grad(ox),
-                                              ldO, dst[0], ldX, dst[1], ldS, rt->stream));
+    ROC_CHECK(roc_sg_attn_backward_dropout_exact_bf16(plan, rt->sgTranspose, heads, H, slope, rt->data_bf16(x), ldX,
+                                                      rt->data(sc), ldS, rt->data(ox), ldO, stats, statsLd,
+                                                      rt->grad(ox), ldO, dst[0], ldX, dst[1], ldS, k1, k2, rate,
+                                                      rt->stream));
   else if (model.exactBackward)
-    ROC_CHECK(roc_sg_attn_backward_exact(model.myGraph.plan, rt->sgTranspose, heads, H, slope, rt->data(x), ldX,
-                                         rt->data(sc), ldS, rt->data(ox), ldO, stats, statsLd, rt->grad(ox), ldO,
-                                         dst[0], ldX, dst[1], ldS, rt->stream));
+    ROC_CHECK(roc_sg_attn_backward_dropout_exact(plan, rt->sgTranspose, heads, H, slope, rt->data(x), ldX,
+                                                 rt->data(sc), ldS, rt->data(ox), ldO, stats, statsLd, rt->grad(ox),
+                                                 ldO, dst[0], ldX, dst[1], ldS, k1, k2, rate, rt->stream));
   else if (xBf16)
-    ROC_CHECK(roc_sg_attn_backward_planned_bf16(model.myGraph.plan, heads, H, slope, model.myGraph.rowLeft,
-                                                rt->data_bf16(x), ldX, rt->data(sc), ldS, rt->data(ox), ldO, stats,
-                                                statsLd, rt->grad(ox), ldO, dst[0], ldX, dst[1], ldS, rt->stream));
+    ROC_CHECK(roc_sg_attn_backward_dropout_planned_bf16(plan, heads, H, slope, model.myGraph.rowLeft,
+                                                        rt->data_bf16(x), ldX, rt->data(sc), ldS, rt->data(ox), ldO,
+                                                        stats, statsLd, rt->grad(ox), ldO, dst[0], ldX, dst[1], ldS,
+                                                        k1, k2, rate, rt->stream));
   else
-    ROC_CHECK(roc_sg_attn_backward_planned(model.myGraph.plan, heads, H, slope, model.myGraph.rowLeft, rt->data(x),
-                                           ldX, rt->data(sc), ldS, rt->data(ox), ldO, stats, statsLd, rt->grad(ox),
-                                           ldO, dst[0], ldX, dst[1], ldS, rt->stream));
+    ROC_CHECK(roc_sg_attn_backward_dropout_planned(plan, heads, H, slope, model.myGraph.rowLeft, rt->data(x), ldX,
+                                                   rt->data(sc), ldS, rt->data(ox), ldO, stats, statsLd, rt->grad(ox),
+                                                   ldO, dst[0], ldX, dst[1], ldS, k1, k2, rate, rt->stream));
   rt->sg_end();
   for (int i = 0; i < 2; i++)
     if (rt->t(inputs[i].region).requiresGrad && !resetInputGrads[i]) add_scratch(model, inputs[i].region, scratch[i]);

@@ -44,6 +44,9 @@
 //  * the max / min, weighted, edge-dot and attention calls over bf16 feature rows (roc_sg_*_bf16) are those
 //    reductions plus SG_RED_BF16: the same row of the table and the same fix-ups, with the feature rows loaded at half
 //    width and widened in registers as BSUM's are.  Their bytes per gathered row fall from 4H to 2H.
+//  * attention dropout (roc_sg_attn_*_dropout_*) is SG_RED_DROP on ATTN, ADST and ASRC: each pass loads one keep byte
+//    per edge beside its source id and weighs a dropped head's term by 0.  k_attn_keep writes those bytes from Philox,
+//    keyed by the (destination, source) pair, in any plan's edge order.
 //
 // Algorithmic bytes per launch (DESIGN.md): E*(4H+4) + Nloc*(4H+8); min / max forward E*(4H+4) + Nloc*(8H+8),
 // backward E*(8H+4) + Nloc*(4H+8); the sum over bf16 rows E*(2H+4) + Nloc*(4H+8); weighted forward E*(4H+8) + Nloc*(4H+8), edge dot E*(4H+8) + Nloc*4H; attention
@@ -259,6 +262,11 @@ enum { SG_RED_SUM = 0, SG_RED_MAX = ROC_SG_AGGR_MAX, SG_RED_MIN = ROC_SG_AGGR_MI
        SG_RED_ASTAT = 4, SG_RED_ATTN = 5, SG_RED_ADST = 6, SG_RED_ASRC = 7, SG_RED_WSUM = 8, SG_RED_EDOT = 9,
        SG_RED_TSUM = 10, SG_RED_TMASK = 11, SG_RED_BSUM = 12 };
 constexpr int SG_RED_BF16 = 16;
+// SG_RED_DROP added to ATTN, ADST or ASRC (with or without SG_RED_BF16) is that pass with attention dropout
+// (roc_sg_attn_*_dropout): it loads each edge's keep byte (p.keep) beside its source id, the way WSUM loads its weight,
+// and weighs a dropped head's term by 0 and a kept one's by p.keepScale; everything else, its row of SG_REDS included,
+// is the pass without dropout's.
+constexpr int SG_RED_DROP = 32;
 __host__ __device__ constexpr int sg_red_base(int RF) { return RF & (SG_RED_BF16 - 1); }
 // the rows gathered as `in` are bf16 (every bf16 form but ASRC's, which gathers fp32 gradients)
 __host__ __device__ constexpr bool sg_bf16_in(int RF) {
@@ -325,6 +333,8 @@ __device__ __forceinline__ float dot_t(const float4& a, const float4& b, int nv)
 __device__ __forceinline__ float dot_t(float a, float b, int nv) { return nv > 0 ? a * b : 0.f; }
 __device__ __forceinline__ float4 attn_scale(float a, const float4& v) { return make_float4(a * v.x, a * v.y, a * v.z, a * v.w); }
 __device__ __forceinline__ float attn_scale(float a, float v) { return a * v; }
+// attention dropout: x scaled by s where bit k of the edge's keep byte is set, else 0
+__device__ __forceinline__ float keep_mul(uint32_t kb, uint32_t k, float s, float x) { return ((kb >> k) & 1u) ? x * s : 0.f; }
 // Per-head sums of d[ch] (lane `lane` holds T-column lane + ch*L; a head is 2^ftShift consecutive T-columns): first
 // across the chunks of one head in the lane (a pairwise tree), then across the head's lanes (an xor butterfly, whose
 // two operands are added in either order to the same bits, so every lane of the head ends with identical sums).
@@ -369,11 +379,19 @@ struct SgParams {
   int epi;
   const uint32_t* desc; // [numChunks][8] chunk start records (k_chunk_desc)
   // min / max aggregation
-  void* arg;            // MAX / MIN: [nloc][ldArg] indices written; MASK: [*][ldArg] indices gathered like `in`
+  // The attention dropout passes (SG_RED_DROP) take the arg and dwAdd slots, which no attention pass uses, so that the
+  // struct keeps its size: the record kernel's arguments after it keep their offsets, and so its code.
+  union {
+    void* arg;          // MAX / MIN: [nloc][ldArg] indices written; MASK: [*][ldArg] indices gathered like `in`
+    const uint8_t* keep;  // attention dropout: [E] one keep byte per local edge (bit k keeps head k)
+  };
   void* carryArg;       // MAX / MIN: [numCarries][ldC] indices of the carry partials
   size_t ldArg;         // in units of T
   uint32_t selfBase;    // MASK, attention: id of local row 0 in the id space of col
-  int dwAdd;            // EDOT: add to dw instead of overwriting it
+  union {
+    int dwAdd;          // EDOT: add to dw instead of overwriting it
+    float keepScale;    // attention dropout: the scale of a kept weight
+  };
   // attention (units of float unless stated).  The edge-weighted passes use two of its slots (score, out2), so that
   // the struct, every kernel's parameter block, keeps its layout (a union there changed the attention kernels' code).
   const float* score;   // [*][ldS]  s_dst | s_src, indexed like `in`;  WSUM: [E] each local edge's weight
@@ -451,6 +469,8 @@ sg_chunk_kernel(const SgParams p) {
   constexpr bool MK = RED == SG_RED_MASK || RED == SG_RED_TMASK; // gathers an index row beside each gradient row
   constexpr bool BX = (RF & SG_RED_BF16) && RED == SG_RED_ASRC;  // its own row X[i] (xrow) is bf16
   constexpr bool BF = sg_bf16_in(RF);                            // gathers bf16 rows
+  constexpr bool DR = (RF & SG_RED_DROP) != 0;                   // attention dropout: loads each edge's keep byte
+  static_assert(!DR || RED == SG_RED_ATTN || RED == SG_RED_ADST || RED == SG_RED_ASRC, "dropout of an attention gather");
   constexpr uint32_t TB = BF ? 2 * VEC : sizeof(T);              // bytes of one T-column of `in`
   constexpr int WPB = SG_THREADS / L;
   constexpr uint32_t CH = SG_CH;
@@ -646,6 +666,7 @@ sg_chunk_kernel(const SgParams p) {
     const uint32_t cnt = min((uint32_t)U, ee - base);
     uint32_t srcs[U];
     float wv[WS ? U : 1];                      // WSUM: each edge's weight, loaded like its source id
+    uint32_t kb[DR ? U : 1];                   // attention dropout: each edge's keep byte, likewise
     if (cnt == (uint32_t)U) {
       const uint32_t* colp = col + base;       // full group: one address, immediate offsets
 #pragma unroll
@@ -654,12 +675,20 @@ sg_chunk_kernel(const SgParams p) {
 #pragma unroll
         for (int u = 0; u < U; u++) wv[u] = __ldg(p.score + base + u);
       }
+      if constexpr (DR) {
+#pragma unroll
+        for (int u = 0; u < U; u++) kb[u] = __ldg(p.keep + base + u);
+      }
     } else {
 #pragma unroll
       for (int u = 0; u < U; u++) srcs[u] = __ldg(col + min(base + (uint32_t)u, eLast));
       if constexpr (WS) {
 #pragma unroll
         for (int u = 0; u < U; u++) wv[u] = __ldg(p.score + min(base + (uint32_t)u, eLast));
+      }
+      if constexpr (DR) {
+#pragma unroll
+        for (int u = 0; u < U; u++) kb[u] = __ldg(p.keep + min(base + (uint32_t)u, eLast));
       }
     }
     // TMASK: bit u is set when edge base + u has the destination of the edge before it (for u = 0 the edge before the
@@ -723,10 +752,12 @@ sg_chunk_kernel(const SgParams p) {
 #pragma unroll
               for (int ch = 0; ch < NCH; ch++) {
                 const float a = attn_alpha(leaky(r0s[ch] + sv[u][ch], p.slope), r1s[ch], r2s[ch]);
-                V<VEC>::add(acc[ch], attn_scale(a, v[u][ch]));
+                // dropout: a' = keep ? a s : 0
+                V<VEC>::add(acc[ch], attn_scale(DR ? keep_mul(kb[u], kh[ch], p.keepScale, a) : a, v[u][ch]));
               }
             } else if constexpr (RED == SG_RED_ADST) {
-              // dz(i<-j) = a(i<-j) (G[i].X[j] - D[i]) l: v is X[j], xi is G[i], rrec is {s_dst, m, 1/Z, D} of i
+              // dz(i<-j) = a(i<-j) (G[i].X[j] - D[i]) l: v is X[j], xi is G[i], rrec is {s_dst, m, 1/Z, D} of i;
+              // dropout: a(i<-j) (M G[i].X[j] - D[i]) l, M = keep ? s : 0, with D over the dropped output
               float d[NCH];
 #pragma unroll
               for (int ch = 0; ch < NCH; ch++) d[ch] = dot_t(xi[ch], v[u][ch], nv[ch]);
@@ -735,10 +766,12 @@ sg_chunk_kernel(const SgParams p) {
               for (int ch = 0; ch < NCH; ch++) {
                 const float z = rrec[ch].x + sv[u][ch];
                 const float a = attn_alpha(leaky(z, p.slope), rrec[ch].y, rrec[ch].z);
-                accS[ch] += a * (d[ch] - rrec[ch].w) * (z > 0.f ? 1.f : p.slope);
+                const float md = DR ? keep_mul(kb[u], kh[ch], p.keepScale, d[ch]) : d[ch];
+                accS[ch] += a * (md - rrec[ch].w) * (z > 0.f ? 1.f : p.slope);
               }
             } else if constexpr (RED == SG_RED_ASRC) {
-              // a(j<-i) G[j] and dz(j<-i) = a(j<-i) (G[j].X[i] - D[j]) l: v is G[j], xi is X[i], rv the record of j
+              // a(j<-i) G[j] and dz(j<-i) = a(j<-i) (G[j].X[i] - D[j]) l: v is G[j], xi is X[i], rv the record of j;
+              // dropout: a'(j<-i) G[j] and a(j<-i) (M G[j].X[i] - D[j]) l, with the keep byte of the pair (j<-i)
               float d[NCH];
 #pragma unroll
               for (int ch = 0; ch < NCH; ch++) d[ch] = dot_t(v[u][ch], xi[ch], nv[ch]);
@@ -748,8 +781,9 @@ sg_chunk_kernel(const SgParams p) {
                 const float4 r = rv[u][ch];
                 const float z = r.x + r0s[ch];
                 const float a = attn_alpha(leaky(z, p.slope), r.y, r.z);
-                V<VEC>::add(acc[ch], attn_scale(a, v[u][ch]));
-                accS[ch] += a * (d[ch] - r.w) * (z > 0.f ? 1.f : p.slope);
+                V<VEC>::add(acc[ch], attn_scale(DR ? keep_mul(kb[u], kh[ch], p.keepScale, a) : a, v[u][ch]));
+                const float md = DR ? keep_mul(kb[u], kh[ch], p.keepScale, d[ch]) : d[ch];
+                accS[ch] += a * (md - r.w) * (z > 0.f ? 1.f : p.slope);
               }
             } else if constexpr (WS) {
 #pragma unroll
@@ -1590,6 +1624,26 @@ __global__ void k_permute(uint32_t E, const uint32_t* __restrict__ perm, const f
   if (t < E) wT[t] = __ldg(w + perm[t]);
 }
 
+// Attention dropout's keep bytes in a plan's edge order (roc_sg_attn_keep_mask): one thread and one Philox block per
+// edge.  The edge's row is the last row starting at or before it; only the rows from the one before chunk c's first
+// owned row up to chunk c + 1's first owned row can hold it, so the search touches a few adjacent rs entries.
+__global__ void k_attn_keep(uint32_t E, const uint32_t* __restrict__ rs, const uint32_t* __restrict__ firstRow,
+                            const uint32_t* __restrict__ col, uint32_t selfBase, int rowIsSource, uint32_t thresh16,
+                            uint32_t seedLo, uint32_t seedHi, uint32_t step, uint8_t* __restrict__ keep) {
+  const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= E) return;
+  const uint32_t c = e / (uint32_t)SG_CH;
+  uint32_t lo = __ldg(firstRow + c), hi = __ldg(firstRow + c + 1);
+  lo = lo ? lo - 1 : 0;           // rs[lo] <= e < rs[hi]
+  while (hi - lo > 1) {
+    const uint32_t mid = lo + ((hi - lo) >> 1);
+    if (__ldg(rs + mid) <= e) lo = mid; else hi = mid;
+  }
+  const uint32_t self = selfBase + lo, other = __ldg(col + e);
+  const uint32_t i = rowIsSource ? other : self, j = rowIsSource ? self : other;    // the pair (i <- j)
+  keep[e] = (uint8_t)dropout_keep8(((uint64_t)j << 32) | i, 0u, step, seedLo, seedHi, thresh16);
+}
+
 }  // namespace roc
 
 struct roc_sg_transpose {
@@ -1877,21 +1931,41 @@ static SgParams attn_params(const roc_sg_plan* pl, int heads, int H, float slope
   return p;
 }
 
+// The attention passes RF (with SG_RED_BF16 as the call's rows are) on float4 or scalar rows, with dropout
+// (SG_RED_DROP) when `drop`.
+template <int RF>
+static int dispatch_attn(const SgParams& p, bool vec, bool drop, cudaStream_t st) {
+  if (drop) return vec ? dispatch<4, RF | SG_RED_DROP>(p, st) : dispatch<1, RF | SG_RED_DROP>(p, st);
+  return vec ? dispatch<4, RF>(p, st) : dispatch<1, RF>(p, st);
+}
+
+// Attention dropout's arguments: ROC_ERR_INVALID for a rate outside [0, 1); *drop when there is a mask and rate > 0
+// (rate 0 or no mask: the calls without dropout).  The scale is roc_dropout_fwd's.
+static int attn_drop_args(const void* keep, float rate, bool* drop, float* scale) {
+  if (!(rate >= 0.f && rate < 1.f)) return ROC_ERR_INVALID;
+  *drop = keep != nullptr && rate > 0.f;
+  *scale = 1.0f / (1.0f - rate);
+  return ROC_OK;
+}
+
 // The attention backward's passes once its arguments are checked and both plans' carries grown: the node records of
 // ids [0, n) and B1 (d s_dst) over `pl`, B2 (inGrad, d s_src) over `plB2`.  With plB2 = pl, B2 is the gather over the
 // same CSR (quirk Q1); over the transposed plan its row j gathers the destinations i of j's out-edges, where the same
 // formula, a(i<-j) G[i] against the record of i, is the true adjoint.
-// BF = SG_RED_BF16: `in` holds bf16 rows, gathered by B1 and read as each row's own row by B2.
+// BF = SG_RED_BF16: `in` holds bf16 rows, gathered by B1 and read as each row's own row by B2.  With `drop`, B1 reads
+// the keep bytes `keep` in pl's edge order and B2 `keep2` in plB2's, each byte the pair's that pass weighs.
 template <int BF>
 static int attn_backward_passes(roc_sg_plan* pl, roc_sg_plan* plB2, uint32_t n, int heads, int H, float slope,
                                 roc_vid_t selfBase, uint32_t fs, bool vec, const void* in, int64_t ldIn,
                                 const float* score, int64_t ldS, const float* out, int64_t ldOut, const float* stats,
                                 int64_t ldStats, const float* outGrad, int64_t ldG, float* inGrad, int64_t ldInG,
-                                float* scoreGrad, int64_t ldSG, cudaStream_t st) {
+                                float* scoreGrad, int64_t ldSG, bool drop, const uint8_t* keep, const uint8_t* keep2,
+                                float keepScale, cudaStream_t st) {
   int rc = grow(pl->attnRec, pl->attnRecBytes, (size_t)n * heads * sizeof(float4), st);
   if (rc != ROC_OK) return rc;
   const int vw = vec ? 4 : 1;
-  const SgParams p = attn_params(pl, heads, H, slope, selfBase, score, ldS, stats, ldStats, fs);
+  SgParams p = attn_params(pl, heads, H, slope, selfBase, score, ldS, stats, ldStats, fs);
+  p.keepScale = keepScale;
   // the node records {s_dst, m, 1/Z, D}, from G and O
   SgParams r = p;
   r.in = outGrad; r.ldIn = (size_t)ldG; r.xrow = out; r.ldX = (size_t)ldOut;
@@ -1901,34 +1975,38 @@ static int attn_backward_passes(roc_sg_plan* pl, roc_sg_plan* plB2, uint32_t n, 
   // B1: d s_dst, gathering X[j] and s_src[j] against G[i]
   SgParams b1 = p;
   b1.in = in; b1.ldIn = (size_t)ldIn; b1.xrow = outGrad; b1.ldX = (size_t)ldG;
-  b1.out = nullptr; b1.out2 = scoreGrad; b1.ldOut2 = (size_t)ldSG;
+  b1.out = nullptr; b1.out2 = scoreGrad; b1.ldOut2 = (size_t)ldSG; b1.keep = keep;
   t_units(b1, vw, H);
-  rc = vec ? dispatch<4, SG_RED_ADST | BF>(b1, st) : dispatch<1, SG_RED_ADST | BF>(b1, st);
+  rc = dispatch_attn<SG_RED_ADST | BF>(b1, vec, drop, st);
   if (rc != ROC_OK) return rc;
   // B2: inGrad and d s_src, gathering G[j] and the record of j against X[i]
   SgParams b2 = attn_params(plB2, heads, H, slope, selfBase, score, ldS, stats, ldStats, fs);
   b2.rec = pl->attnRec;
   b2.in = outGrad; b2.ldIn = (size_t)ldG; b2.xrow = in; b2.ldX = (size_t)ldIn;
   b2.out = inGrad; b2.ldOut = (size_t)ldInG; b2.out2 = scoreGrad + heads; b2.ldOut2 = (size_t)ldSG;
+  b2.keep = keep2; b2.keepScale = keepScale;
   t_units(b2, vw, H);
-  return vec ? dispatch<4, SG_RED_ASRC | BF>(b2, st) : dispatch<1, SG_RED_ASRC | BF>(b2, st);
+  return dispatch_attn<SG_RED_ASRC | BF>(b2, vec, drop, st);
 }
 
 template <int BF>
 static int attn_forward(const roc_sg_plan* plc, int heads, int H, float slope, roc_vid_t selfBase, const void* in,
                         int64_t ldIn, const float* score, int64_t ldS, float* out, int64_t ldOut, float* stats,
-                        int64_t ldStats, roc_stream_t stream) {
+                        int64_t ldStats, const uint8_t* keep, float rate, roc_stream_t stream) {
   roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
   clear_launches();
+  bool drop = false;
+  float keepScale = 1.f;
   if (!pl || !in || !score || !out || !stats || heads <= 0 || H <= 0 || ldIn < H || ldOut < H ||
-      ldS < 2 * (int64_t)heads || ldStats < 2 * (int64_t)heads || (BF && bf16_rows_bad(in, ldIn)))
+      ldS < 2 * (int64_t)heads || ldStats < 2 * (int64_t)heads || (BF && bf16_rows_bad(in, ldIn)) ||
+      attn_drop_args(keep, rate, &drop, &keepScale) != ROC_OK)
     return ROC_ERR_INVALID;
   const bool vec = float4_rows({in, out}, {ldIn, ldOut});
   cudaStream_t st = as_stream(stream);
   uint32_t fs = 0;
   int rc = attn_setup(pl, heads, H, slope, vec, st, &fs);
   if (rc != ROC_OK) return rc;
-  // pass 1: (m, 1/Z) per row and head from the scores alone, one float per head
+  // pass 1: (m, 1/Z) per row and head from the scores alone, one float per head (dropout does not change them)
   SgParams a = attn_params(pl, heads, H, slope, selfBase, score, ldS, stats, ldStats, 0);
   a.in = score + heads; a.ldIn = (size_t)ldS; a.out = stats; a.ldOut = (size_t)ldStats;
   t_units(a, 1, heads);
@@ -1936,15 +2014,17 @@ static int attn_forward(const roc_sg_plan* plc, int heads, int H, float slope, r
   // pass 2: the a-weighted sum of the feature rows
   SgParams b = attn_params(pl, heads, H, slope, selfBase, score, ldS, stats, ldStats, fs);
   b.in = in; b.ldIn = (size_t)ldIn; b.out = out; b.ldOut = (size_t)ldOut;
+  b.keep = keep; b.keepScale = keepScale;
   t_units(b, vec ? 4 : 1, H);
-  return vec ? dispatch<4, SG_RED_ATTN | BF>(b, st) : dispatch<1, SG_RED_ATTN | BF>(b, st);
+  return dispatch_attn<SG_RED_ATTN | BF>(b, vec, drop, st);
 }
 
 extern "C" int roc_sg_attn_forward_planned(const roc_sg_plan* plc, int heads, int H, float slope, roc_vid_t selfBase,
                                            const float* in, int64_t ldIn, const float* score, int64_t ldS,
                                            float* out, int64_t ldOut, float* stats, int64_t ldStats,
                                            roc_stream_t stream) {
-  return attn_forward<0>(plc, heads, H, slope, selfBase, in, ldIn, score, ldS, out, ldOut, stats, ldStats, stream);
+  return attn_forward<0>(plc, heads, H, slope, selfBase, in, ldIn, score, ldS, out, ldOut, stats, ldStats, nullptr,
+                         0.f, stream);
 }
 
 extern "C" int roc_sg_attn_forward_planned_bf16(const roc_sg_plan* plc, int heads, int H, float slope,
@@ -1952,19 +2032,47 @@ extern "C" int roc_sg_attn_forward_planned_bf16(const roc_sg_plan* plc, int head
                                                 const float* score, int64_t ldS, float* out, int64_t ldOut,
                                                 float* stats, int64_t ldStats, roc_stream_t stream) {
   return attn_forward<SG_RED_BF16>(plc, heads, H, slope, selfBase, in, ldIn, score, ldS, out, ldOut, stats, ldStats,
-                                   stream);
+                                   nullptr, 0.f, stream);
+}
+
+extern "C" int roc_sg_attn_forward_dropout_planned(const roc_sg_plan* plc, int heads, int H, float slope,
+                                                   roc_vid_t selfBase, const float* in, int64_t ldIn,
+                                                   const float* score, int64_t ldS, float* out, int64_t ldOut,
+                                                   float* stats, int64_t ldStats, const uint8_t* keep, float rate,
+                                                   roc_stream_t stream) {
+  return attn_forward<0>(plc, heads, H, slope, selfBase, in, ldIn, score, ldS, out, ldOut, stats, ldStats, keep, rate,
+                         stream);
+}
+
+extern "C" int roc_sg_attn_forward_dropout_planned_bf16(const roc_sg_plan* plc, int heads, int H, float slope,
+                                                        roc_vid_t selfBase, const uint16_t* in, int64_t ldIn,
+                                                        const float* score, int64_t ldS, float* out, int64_t ldOut,
+                                                        float* stats, int64_t ldStats, const uint8_t* keep, float rate,
+                                                        roc_stream_t stream) {
+  return attn_forward<SG_RED_BF16>(plc, heads, H, slope, selfBase, in, ldIn, score, ldS, out, ldOut, stats, ldStats,
+                                   keep, rate, stream);
+}
+
+// The backward's keep bytes: both or neither (ROC_ERR_INVALID otherwise), then attn_drop_args.
+static int attn_drop_args2(const uint8_t* keep, const uint8_t* keep2, float rate, bool* drop, float* scale) {
+  if ((keep == nullptr) != (keep2 == nullptr)) return ROC_ERR_INVALID;
+  return attn_drop_args(keep, rate, drop, scale);
 }
 
 template <int BF>
 static int attn_backward(const roc_sg_plan* plc, int heads, int H, float slope, roc_vid_t selfBase, const void* in,
                          int64_t ldIn, const float* score, int64_t ldS, const float* out, int64_t ldOut,
                          const float* stats, int64_t ldStats, const float* outGrad, int64_t ldG, float* inGrad,
-                         int64_t ldInG, float* scoreGrad, int64_t ldSG, roc_stream_t stream) {
+                         int64_t ldInG, float* scoreGrad, int64_t ldSG, const uint8_t* keep, const uint8_t* keepRev,
+                         float rate, roc_stream_t stream) {
   roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
   clear_launches();
+  bool drop = false;
+  float keepScale = 1.f;
   if (!pl || !in || !score || !out || !stats || !outGrad || !inGrad || !scoreGrad || heads <= 0 || H <= 0 ||
       ldIn < H || ldOut < H || ldG < H || ldInG < H || ldS < 2 * (int64_t)heads || ldStats < 2 * (int64_t)heads ||
-      ldSG < 2 * (int64_t)heads || (BF && bf16_rows_bad(in, ldIn)))
+      ldSG < 2 * (int64_t)heads || (BF && bf16_rows_bad(in, ldIn)) ||
+      attn_drop_args2(keep, keepRev, rate, &drop, &keepScale) != ROC_OK)
     return ROC_ERR_INVALID;
   const bool vec = float4_rows({in, out, outGrad, inGrad}, {ldIn, ldOut, ldG, ldInG});
   cudaStream_t st = as_stream(stream);
@@ -1975,7 +2083,8 @@ static int attn_backward(const roc_sg_plan* plc, int heads, int H, float slope, 
   const uint64_t n64 = std::max<uint64_t>(pl->idEnd, (uint64_t)selfBase + pl->nloc);
   if (n64 >= 0xFFFFFFF0ull) return ROC_ERR_UNSUPPORTED;
   return attn_backward_passes<BF>(pl, pl, (uint32_t)n64, heads, H, slope, selfBase, fs, vec, in, ldIn, score, ldS, out,
-                                  ldOut, stats, ldStats, outGrad, ldG, inGrad, ldInG, scoreGrad, ldSG, st);
+                                  ldOut, stats, ldStats, outGrad, ldG, inGrad, ldInG, scoreGrad, ldSG, drop, keep,
+                                  keepRev, keepScale, st);
 }
 
 extern "C" int roc_sg_attn_backward_planned(const roc_sg_plan* plc, int heads, int H, float slope, roc_vid_t selfBase,
@@ -1984,7 +2093,7 @@ extern "C" int roc_sg_attn_backward_planned(const roc_sg_plan* plc, int heads, i
                                             const float* outGrad, int64_t ldG, float* inGrad, int64_t ldInG,
                                             float* scoreGrad, int64_t ldSG, roc_stream_t stream) {
   return attn_backward<0>(plc, heads, H, slope, selfBase, in, ldIn, score, ldS, out, ldOut, stats, ldStats, outGrad,
-                          ldG, inGrad, ldInG, scoreGrad, ldSG, stream);
+                          ldG, inGrad, ldInG, scoreGrad, ldSG, nullptr, nullptr, 0.f, stream);
 }
 
 extern "C" int roc_sg_attn_backward_planned_bf16(const roc_sg_plan* plc, int heads, int H, float slope,
@@ -1994,19 +2103,46 @@ extern "C" int roc_sg_attn_backward_planned_bf16(const roc_sg_plan* plc, int hea
                                                  int64_t ldG, float* inGrad, int64_t ldInG, float* scoreGrad,
                                                  int64_t ldSG, roc_stream_t stream) {
   return attn_backward<SG_RED_BF16>(plc, heads, H, slope, selfBase, in, ldIn, score, ldS, out, ldOut, stats, ldStats,
-                                    outGrad, ldG, inGrad, ldInG, scoreGrad, ldSG, stream);
+                                    outGrad, ldG, inGrad, ldInG, scoreGrad, ldSG, nullptr, nullptr, 0.f, stream);
+}
+
+extern "C" int roc_sg_attn_backward_dropout_planned(const roc_sg_plan* plc, int heads, int H, float slope,
+                                                    roc_vid_t selfBase, const float* in, int64_t ldIn,
+                                                    const float* score, int64_t ldS, const float* out, int64_t ldOut,
+                                                    const float* stats, int64_t ldStats, const float* outGrad,
+                                                    int64_t ldG, float* inGrad, int64_t ldInG, float* scoreGrad,
+                                                    int64_t ldSG, const uint8_t* keep, const uint8_t* keepRev,
+                                                    float rate, roc_stream_t stream) {
+  return attn_backward<0>(plc, heads, H, slope, selfBase, in, ldIn, score, ldS, out, ldOut, stats, ldStats, outGrad,
+                          ldG, inGrad, ldInG, scoreGrad, ldSG, keep, keepRev, rate, stream);
+}
+
+extern "C" int roc_sg_attn_backward_dropout_planned_bf16(const roc_sg_plan* plc, int heads, int H, float slope,
+                                                         roc_vid_t selfBase, const uint16_t* in, int64_t ldIn,
+                                                         const float* score, int64_t ldS, const float* out,
+                                                         int64_t ldOut, const float* stats, int64_t ldStats,
+                                                         const float* outGrad, int64_t ldG, float* inGrad,
+                                                         int64_t ldInG, float* scoreGrad, int64_t ldSG,
+                                                         const uint8_t* keep, const uint8_t* keepRev, float rate,
+                                                         roc_stream_t stream) {
+  return attn_backward<SG_RED_BF16>(plc, heads, H, slope, selfBase, in, ldIn, score, ldS, out, ldOut, stats, ldStats,
+                                    outGrad, ldG, inGrad, ldInG, scoreGrad, ldSG, keep, keepRev, rate, stream);
 }
 
 template <int BF>
 static int attn_backward_exact(const roc_sg_plan* plc, roc_sg_transpose* tr, int heads, int H, float slope,
                                const void* in, int64_t ldIn, const float* score, int64_t ldS, const float* out,
                                int64_t ldOut, const float* stats, int64_t ldStats, const float* outGrad, int64_t ldG,
-                               float* inGrad, int64_t ldInG, float* scoreGrad, int64_t ldSG, roc_stream_t stream) {
+                               float* inGrad, int64_t ldInG, float* scoreGrad, int64_t ldSG, const uint8_t* keep,
+                               const uint8_t* keepT, float rate, roc_stream_t stream) {
   roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
   clear_launches();
+  bool drop = false;
+  float keepScale = 1.f;
   if (!pl || !tr || !in || !score || !out || !stats || !outGrad || !inGrad || !scoreGrad || heads <= 0 || H <= 0 ||
       ldIn < H || ldOut < H || ldG < H || ldInG < H || ldS < 2 * (int64_t)heads || ldStats < 2 * (int64_t)heads ||
-      ldSG < 2 * (int64_t)heads || pl->nloc != tr->N || pl->E != tr->E || (BF && bf16_rows_bad(in, ldIn)))
+      ldSG < 2 * (int64_t)heads || pl->nloc != tr->N || pl->E != tr->E || (BF && bf16_rows_bad(in, ldIn)) ||
+      attn_drop_args2(keep, keepT, rate, &drop, &keepScale) != ROC_OK)
     return ROC_ERR_INVALID;
   const bool vec = float4_rows({in, out, outGrad, inGrad}, {ldIn, ldOut, ldG, ldInG});
   cudaStream_t st = as_stream(stream);
@@ -2016,7 +2152,8 @@ static int attn_backward_exact(const roc_sg_plan* plc, roc_sg_transpose* tr, int
   if (rc != ROC_OK) return rc;
   // a whole graph: every id is below N, so the records cover [0, N) with no id scan
   return attn_backward_passes<BF>(pl, tr->planT, tr->N, heads, H, slope, 0, fs, vec, in, ldIn, score, ldS, out, ldOut,
-                                  stats, ldStats, outGrad, ldG, inGrad, ldInG, scoreGrad, ldSG, st);
+                                  stats, ldStats, outGrad, ldG, inGrad, ldInG, scoreGrad, ldSG, drop, keep, keepT,
+                                  keepScale, st);
 }
 
 extern "C" int roc_sg_attn_backward_exact(const roc_sg_plan* plc, roc_sg_transpose* tr, int heads, int H, float slope,
@@ -2025,7 +2162,7 @@ extern "C" int roc_sg_attn_backward_exact(const roc_sg_plan* plc, roc_sg_transpo
                                           const float* outGrad, int64_t ldG, float* inGrad, int64_t ldInG,
                                           float* scoreGrad, int64_t ldSG, roc_stream_t stream) {
   return attn_backward_exact<0>(plc, tr, heads, H, slope, in, ldIn, score, ldS, out, ldOut, stats, ldStats, outGrad,
-                                ldG, inGrad, ldInG, scoreGrad, ldSG, stream);
+                                ldG, inGrad, ldInG, scoreGrad, ldSG, nullptr, nullptr, 0.f, stream);
 }
 
 extern "C" int roc_sg_attn_backward_exact_bf16(const roc_sg_plan* plc, roc_sg_transpose* tr, int heads, int H,
@@ -2034,7 +2171,44 @@ extern "C" int roc_sg_attn_backward_exact_bf16(const roc_sg_plan* plc, roc_sg_tr
                                                int64_t ldStats, const float* outGrad, int64_t ldG, float* inGrad,
                                                int64_t ldInG, float* scoreGrad, int64_t ldSG, roc_stream_t stream) {
   return attn_backward_exact<SG_RED_BF16>(plc, tr, heads, H, slope, in, ldIn, score, ldS, out, ldOut, stats, ldStats,
-                                          outGrad, ldG, inGrad, ldInG, scoreGrad, ldSG, stream);
+                                          outGrad, ldG, inGrad, ldInG, scoreGrad, ldSG, nullptr, nullptr, 0.f, stream);
+}
+
+extern "C" int roc_sg_attn_backward_dropout_exact(const roc_sg_plan* plc, roc_sg_transpose* tr, int heads, int H,
+                                                  float slope, const float* in, int64_t ldIn, const float* score,
+                                                  int64_t ldS, const float* out, int64_t ldOut, const float* stats,
+                                                  int64_t ldStats, const float* outGrad, int64_t ldG, float* inGrad,
+                                                  int64_t ldInG, float* scoreGrad, int64_t ldSG, const uint8_t* keep,
+                                                  const uint8_t* keepT, float rate, roc_stream_t stream) {
+  return attn_backward_exact<0>(plc, tr, heads, H, slope, in, ldIn, score, ldS, out, ldOut, stats, ldStats, outGrad,
+                                ldG, inGrad, ldInG, scoreGrad, ldSG, keep, keepT, rate, stream);
+}
+
+extern "C" int roc_sg_attn_backward_dropout_exact_bf16(const roc_sg_plan* plc, roc_sg_transpose* tr, int heads, int H,
+                                                       float slope, const uint16_t* in, int64_t ldIn,
+                                                       const float* score, int64_t ldS, const float* out,
+                                                       int64_t ldOut, const float* stats, int64_t ldStats,
+                                                       const float* outGrad, int64_t ldG, float* inGrad,
+                                                       int64_t ldInG, float* scoreGrad, int64_t ldSG,
+                                                       const uint8_t* keep, const uint8_t* keepT, float rate,
+                                                       roc_stream_t stream) {
+  return attn_backward_exact<SG_RED_BF16>(plc, tr, heads, H, slope, in, ldIn, score, ldS, out, ldOut, stats, ldStats,
+                                          outGrad, ldG, inGrad, ldInG, scoreGrad, ldSG, keep, keepT, rate, stream);
+}
+
+extern "C" int roc_sg_attn_keep_mask(const roc_sg_plan* plc, roc_vid_t selfBase, int rowIsSource, float rate,
+                                     uint64_t seed, uint32_t step, uint8_t* keep, roc_stream_t stream) {
+  clear_launches();
+  if (!plc || (plc->E && !keep) || (rowIsSource != 0 && rowIsSource != 1) || !(rate >= 0.f && rate < 1.f))
+    return ROC_ERR_INVALID;
+  if (plc->E == 0) return ROC_OK;
+  const uint32_t grid = (plc->E + 255) / 256;
+  k_attn_keep<<<grid, 256, 0, as_stream(stream)>>>(plc->E, plc->rs, plc->firstRow, plc->col, selfBase, rowIsSource,
+                                                   dropout_thresh16(rate), (uint32_t)seed, (uint32_t)(seed >> 32),
+                                                   step, keep);
+  ROC_LAUNCH_CHECK();
+  note_launch(ROC_SG_LAUNCH_KEEP_MASK, -1, 1, 1, 1, grid);
+  return ROC_OK;
 }
 
 template <int BF>

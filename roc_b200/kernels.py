@@ -177,6 +177,40 @@ class SgPlan:
               "roc_sg_attn_backward_planned_bf16")
         return in_grad, score_grad
 
+    def attn_keep_mask(self, rate, seed, step, self_base=0, row_is_source=False, out=None):
+        """roc_sg_attn_keep_mask: attention dropout's keep bytes of the plan's edges in its edge order, a uint8 [E]
+        tensor (bit k keeps head k).  row_is_source=False: the pairs (self_base + r <- col[e]), the forward's and the
+        d s_dst pass's; True: the reverse pairs (col[e] <- self_base + r), the planned input-gradient pass's."""
+        if out is None:
+            out = torch.empty(max(self.num_edges(), 1), dtype=torch.uint8, device="cuda")
+        check(lib.roc_sg_attn_keep_mask(self.handle, int(self_base), int(bool(row_is_source)), float(rate), int(seed),
+                                        int(step), _ptr(out), _stream()), "roc_sg_attn_keep_mask")
+        return out
+
+    def attn_forward_dropout(self, x, scores, keep, rate, heads=1, slope=0.2, self_base=0, out=None, stats=None):
+        """roc_sg_attn_forward_dropout_planned (its _bf16 form for a bf16 x): attn_forward() with attention dropout,
+        keep from attn_keep_mask(row_is_source=False); keep=None or rate=0 is attn_forward()."""
+        out = self._rows(x) if out is None else out
+        stats = torch.empty((self.nloc, 2 * heads), device=x.device) if stats is None else stats
+        name = "roc_sg_attn_forward_dropout_planned" + ("_bf16" if x.dtype == torch.bfloat16 else "")
+        check(getattr(lib, name)(self.handle, int(heads), x.shape[1], float(slope), int(self_base), _ptr(x), _ld(x),
+                                 _ptr(scores), _ld(scores), _ptr(out), _ld(out), _ptr(stats), _ld(stats), _ptr(keep),
+                                 float(rate), _stream()), name)
+        return out, stats
+
+    def attn_backward_dropout(self, x, scores, out, stats, gy, keep, keep_rev, rate, heads=1, slope=0.2, self_base=0,
+                              in_grad=None, score_grad=None):
+        """roc_sg_attn_backward_dropout_planned (its _bf16 form for a bf16 x): attn_backward() with attention dropout;
+        keep as the forward's, keep_rev from attn_keep_mask(row_is_source=True), out the dropped forward output."""
+        in_grad = self._rows(x) if in_grad is None else in_grad
+        score_grad = torch.empty((self.nloc, 2 * heads), device=x.device) if score_grad is None else score_grad
+        name = "roc_sg_attn_backward_dropout_planned" + ("_bf16" if x.dtype == torch.bfloat16 else "")
+        check(getattr(lib, name)(self.handle, int(heads), x.shape[1], float(slope), int(self_base), _ptr(x), _ld(x),
+                                 _ptr(scores), _ld(scores), _ptr(out), _ld(out), _ptr(stats), _ld(stats), _ptr(gy),
+                                 _ld(gy), _ptr(in_grad), _ld(in_grad), _ptr(score_grad), _ld(score_grad), _ptr(keep),
+                                 _ptr(keep_rev), float(rate), _stream()), name)
+        return in_grad, score_grad
+
     def weighted_forward(self, x, w, out=None):
         """Edge-weighted sum: out[r] = sum over row r's edges e of w[e - col_left] * x[col[e]]; w is a flat fp32 array in
         the plan's edge order, x is indexed like forward's input."""
@@ -307,6 +341,30 @@ class SgTranspose:
                                                   _ptr(stats), _ld(stats), _ptr(gy), _ld(gy), _ptr(in_grad),
                                                   _ld(in_grad), _ptr(score_grad), _ld(score_grad), _stream()),
               "roc_sg_attn_backward_exact_bf16")
+        return in_grad, score_grad
+
+    def attn_keep_mask(self, rate, seed, step, out=None):
+        """roc_sg_attn_keep_mask over the transposed plan (selfBase 0, the row the source): the keep bytes the exact
+        backward's input-gradient pass reads, a uint8 [E] tensor in the transposed edge order."""
+        plan_t = C.c_void_p()
+        check(lib.roc_sg_transpose_info(self.handle, None, None, None, C.byref(plan_t)), "roc_sg_transpose_info")
+        if out is None:
+            out = torch.empty(max(self.num_edges, 1), dtype=torch.uint8, device="cuda")
+        check(lib.roc_sg_attn_keep_mask(plan_t, 0, 1, float(rate), int(seed), int(step), _ptr(out), _stream()),
+              "roc_sg_attn_keep_mask")
+        return out
+
+    def attn_backward_dropout(self, plan, x, scores, out, stats, gy, keep, keep_t, rate, heads=1, slope=0.2,
+                              in_grad=None, score_grad=None):
+        """roc_sg_attn_backward_dropout_exact (its _bf16 form for a bf16 x): attn_backward() with attention dropout;
+        keep from plan.attn_keep_mask(), keep_t from attn_keep_mask()."""
+        in_grad = self._rows(x) if in_grad is None else in_grad
+        score_grad = torch.empty((self.n, 2 * heads), device=x.device) if score_grad is None else score_grad
+        name = "roc_sg_attn_backward_dropout_exact" + ("_bf16" if x.dtype == torch.bfloat16 else "")
+        check(getattr(lib, name)(plan.handle, self.handle, int(heads), x.shape[1], float(slope), _ptr(x), _ld(x),
+                                 _ptr(scores), _ld(scores), _ptr(out), _ld(out), _ptr(stats), _ld(stats), _ptr(gy),
+                                 _ld(gy), _ptr(in_grad), _ld(in_grad), _ptr(score_grad), _ld(score_grad), _ptr(keep),
+                                 _ptr(keep_t), float(rate), _stream()), name)
         return in_grad, score_grad
 
     def info(self):

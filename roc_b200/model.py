@@ -126,10 +126,17 @@ class Model:
             return lib.roc_host_scatter_gather(self.h, t)
         return lib.roc_host_scatter_gather_aggr(self.h, t, int(aggr))
 
-    def attention_gather(self, t, scores, heads=1, negative_slope=0.2):
+    def attention_gather(self, t, scores, heads=1, negative_slope=0.2, dropout=0.0, seed=0):
         """GAT aggregation of t (H = heads * F columns) weighted by a per-head softmax over each row's in-edges of
-        LeakyReLU(s_dst[v] + s_src[u]); scores has 2 * heads columns [s_dst | s_src].  One partition only."""
-        return lib.roc_host_attention_gather(self.h, t, scores, int(heads), float(negative_slope))
+        LeakyReLU(s_dst[v] + s_src[u]); scores has 2 * heads columns [s_dst | s_src].  One partition only.
+        dropout: attention dropout in train mode, each head's weight of each (destination, source) pair kept with
+        probability 1 - dropout and scaled by 1 / (1 - dropout), drawn anew every step from `seed` (include/roc_b200.h,
+        roc_sg_attn_forward_dropout_planned).  A rate outside [0, 1) raises ValueError."""
+        _check_rate(dropout, "dropout")
+        if dropout == 0:
+            return lib.roc_host_attention_gather(self.h, t, scores, int(heads), float(negative_slope))
+        return lib.roc_host_attention_gather_dropout(self.h, t, scores, int(heads), float(negative_slope),
+                                                     float(dropout), int(seed))
 
     def attention_scores(self, t, heads=1):
         """GAT's per-head scores of t (H = heads * F columns): [s_dst | s_src], 2 * heads columns, the scores attention_gather
@@ -415,6 +422,11 @@ def _check_norm(norm):
         raise ValueError("norm must be None or \"batch\"")
 
 
+def _check_rate(rate, name):
+    if not 0.0 <= float(rate) < 1.0:
+        raise ValueError("%s must be in [0, 1)" % name)
+
+
 def _hidden_norm(model, norm, t, bns):
     """norm="batch": batch_norm on a hidden layer's output, right before its relu; None leaves t as it is."""
     if norm is None:
@@ -551,7 +563,7 @@ def build_sage_pool(model, layers, dropout_rate, aggr=_lib.AGGR_MAX, lr=0.01, we
 
 def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01, weight_decay=0.05,
               exact_backward=False, features="float32", aggregation="float32", loss="softmax", norm=None,
-              scores="dense", activation="relu"):
+              scores="dense", activation="relu", attn_dropout=0.0):
     """GAT (Velickovic et al., 2018) built from the reference's ops plus attention_gather.  `heads` (an int, or one
     value per hidden layer) applies to the hidden layers; the last layer has one head.  layers[i] is the width of
     layer i's output, heads_i * F_i.  Per layer:
@@ -560,12 +572,15 @@ def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01,
         wh = linear(d, layers[i])                       # heads_i * F_i columns
         sc = linear(wh, 2 * heads_i)                    # scores="dense": [s_dst | s_src] per head
         sc = attention_scores(wh, heads_i)              # scores="per_head": the same, head k from its own F columns
-        t  = attention_gather(wh, sc, heads_i, slope)   # per head, softmax over N(v) + v (self loops are in A)
+        t  = attention_gather(wh, sc, heads_i, slope)   # per head, softmax over N(v) + v (self loops are in A),
+                                                        # attn_dropout > 0: with that attention dropout
         t  = relu(t)                                    # all but the last layer; activation="elu": elu(t)
 
     scores="per_head" gives each head its own a_dst and a_src (Model.attention_scores), as the paper and PyG's GATConv
     do; the default "dense" projects all heads' features for every head's scores, which is the same function only
-    with one head.  activation="elu" uses the paper's ELU in place of ReLU.  With both, the model is the paper's GAT
+    with one head.  activation="elu" uses the paper's ELU in place of ReLU.  attn_dropout: dropout of the normalised
+    attention coefficients at that rate on every layer (Model.attention_gather's dropout; the paper uses 0.6 beside
+    dropout_rate = 0.6).  With scores="per_head", activation="elu" and attn_dropout, the model is the paper's GAT
     without bias, with any number of heads.
 
     Where this differs from the paper: there is no bias (the reference's Linear has none; norm="batch" gives a
@@ -578,6 +593,7 @@ def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01,
         raise ValueError("scores must be \"dense\" or \"per_head\"")
     if activation not in ("relu", "elu"):
         raise ValueError("activation must be \"relu\" or \"elu\"")
+    _check_rate(attn_dropout, "attn_dropout")
     L = len(layers)
     hs = list(heads) if isinstance(heads, (list, tuple)) else [int(heads)] * (L - 2)
     assert len(hs) == L - 2, "one head count per hidden layer"
@@ -595,7 +611,10 @@ def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01,
             sc = model.attention_scores(wh, hs[i - 1])
         else:
             sc = model.linear(wh, 2 * hs[i - 1], _lib.AC_MODE_NONE)
-        t = model.attention_gather(wh, sc, hs[i - 1], negative_slope)
+        if attn_dropout:
+            t = model.attention_gather(wh, sc, hs[i - 1], negative_slope, attn_dropout)
+        else:
+            t = model.attention_gather(wh, sc, hs[i - 1], negative_slope)
         attn_ins.append(wh)
         score_outs.append(sc)
         attn.append(t)

@@ -66,6 +66,8 @@ typedef void*    roc_stream_t; /* cudaStream_t */
 #define ROC_SG_EPI_NONE 0
 #define ROC_SG_EPI_NORM 1
 #define ROC_SG_EPI_RELU 2
+/* roc_sg_forward_teleport_planned only: the indegree_norm after the teleport (the next hop's) */
+#define ROC_SG_EPI_NORM_OUT 4
 
 /* aggregation of roc_sg_minmax_forward_planned (the values of AGGR_MAX / AGGR_MIN, gnn.h:75-80) */
 #define ROC_SG_AGGR_MAX 1
@@ -161,6 +163,21 @@ int roc_sg_forward_planned(const roc_sg_plan* plan, int H, const float* in,
  * that call's.  Its launches report reduction 12 (the sum over bf16 rows) in roc_sg_last_call_info. */
 int roc_sg_forward_planned_bf16(const roc_sg_plan* plan, int H, const uint16_t* in, int64_t ldIn, float* out,
                                 int64_t ldOut, int epilogue, roc_stream_t stream);
+/* The sum with a teleport (initial residual) fused into its store, the hop of APPNP and GCNII:
+ *   out[v][h] = post( fmaf(alpha, pre( sum_{e in in(v)} in[colSrc[e]][h] ), beta * t[v][h]) ),  h < H
+ * with beta * t rounded to fp32 first, pre the divide by sqrtf(in-degree) of ROC_SG_EPI_NORM and post the same divide
+ * of ROC_SG_EPI_NORM_OUT (the next hop's indegree_norm).  t has one row per plan row (like out), any pitch ldT >= H.
+ * The bytes of out[v][0..H) are those of roc_sg_forward_planned(epilogue & ROC_SG_EPI_NORM) into a buffer laid out like
+ * out, then roc_scaled_add_fwd(alpha, that, beta, t), then (NORM_OUT) roc_indegree_norm, also on rows of degree 0 and
+ * NaN where that chain gives NaN: the same plan, row shapes, column blocks, add order and fix-ups as the sum.  The pad
+ * floats of a float4 row of `out` (past H, up to the next multiple of 4) are written with unspecified values: the
+ * teleport of the sum's pad with t = 0.  Every width runs on the
+ * register kernel (no ring form).  ROC_ERR_INVALID: a NULL pointer, out == t, a leading dimension < H, non-finite
+ * alpha or beta, or an epilogue with any bit but NORM and NORM_OUT (RELU included).  Its launches report reduction 13
+ * in roc_sg_last_call_info. */
+int roc_sg_forward_teleport_planned(const roc_sg_plan* plan, int H, const float* in, int64_t ldIn, float alpha,
+                                    const float* t, int64_t ldT, float beta, float* out, int64_t ldOut, int epilogue,
+                                    roc_stream_t stream);
 
 /* Max / min aggregation (GraphSAGE-pool).  The reference declares AGGR_MAX / AGGR_MIN but never implements them;
  * these semantics are this library's own.  For a row v with in-edges e in CSR order:
@@ -431,7 +448,8 @@ int roc_sg_backward(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft, in
  *          stats, 5 the attention forward, 6 its d s_dst gather, 7 its input-gradient gather, 8 the weighted sum
  *          (forward and backward), 9 the edge-weight gradient, 10 the exact sum backward with NORM (the sum whose
  *          epilogue divides by the original graph's in-degree; its main kernel, ring and fix-ups), 11 the exact max /
- *          min backward, 12 the sum over bf16 rows (its main kernel and ring); 16 + r for the main kernel of
+ *          min backward, 12 the sum over bf16 rows (its main kernel and ring), 13 the teleport sum
+ *          (roc_sg_forward_teleport_planned: its main kernel and fix-ups); 16 + r for the main kernel of
  *          reduction r over bf16 feature rows (17 max, 18 min, 21 attention forward, 22 d s_dst, 23 input gradient,
  *          24 weighted sum, 25 edge-weight gradient: the roc_sg_*_bf16 calls), whose fix-ups are reduction r's and
  *          report as there; 32 + r for the main kernel of attention pass r (5, 6, 7, or 21, 22, 23 on bf16 feature
@@ -562,6 +580,15 @@ int roc_add_fwd(int64_t rows, int H, const float* a, int64_t ldA, const float* b
 int roc_add_bwd(int64_t rows, int H, const float* dY, int64_t ldDY, float* dA,
                 int64_t ldDA, int accA, float* dB, int64_t ldDB, int accB,
                 roc_stream_t stream);
+/* Scaled add (APPNP / GCNII's initial residual; not in the reference): y = fmaf(alpha, a, beta * b), the product
+ * beta * b rounded to fp32 first.  At alpha = beta = 1 it gives roc_add_fwd's bits.  Backward: dA = alpha * dY, or
+ * fmaf(alpha, dY, dA) with accA; dB likewise with beta; a NULL dA or dB is skipped.  16-byte streaming accesses when H,
+ * the leading dimensions and the pointers allow.  ROC_ERR_INVALID: a NULL a, b, y or dY, a leading dimension < H,
+ * non-finite alpha or beta, or dA == dB. */
+int roc_scaled_add_fwd(int64_t rows, int H, float alpha, const float* a, int64_t ldA, float beta, const float* b,
+                       int64_t ldB, float* y, int64_t ldY, roc_stream_t stream);
+int roc_scaled_add_bwd(int64_t rows, int H, const float* dY, int64_t ldDY, float alpha, float* dA, int64_t ldDA,
+                       int accA, float beta, float* dB, int64_t ldDB, int accB, roc_stream_t stream);
 
 /* Replaces cudnnDropoutForward/Backward, dropout_kernel.cu:98-99, 149-150.
  * y = keep ? x / (1 - rate) : 0.  cuDNN's generator is not reproducible, so the

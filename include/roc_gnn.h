@@ -229,6 +229,11 @@ public:
    * it (linear() exits on AC_MODE_ELU).  Row-local like relu, so not refused on more than one partition, but untested
    * there. */
   Tensor elu(const Tensor& _input);
+  /* Scaled add (roc_scaled_add_fwd / _bwd): fmaf(alpha, a, beta * b), the initial residual of APPNP and GCNII.  Exits
+   * on unequal shapes, a non-finite alpha or beta, or a == b.  With fusion on and one partition, init() fuses it into
+   * the store of a sum scatter_gather whose indegree_norm feeds only it, as its first input (fuse_teleport in model.cc).
+   * Row-local like elu, so not refused on more than one partition, but untested there. */
+  Tensor scaled_add(const Tensor& a, const Tensor& b, float alpha, float beta);
   /* Batch normalisation over every local row (torch.nn.BatchNorm1d; roc_batchnorm_fwd / roc_batchnorm_bwd).  Appends
    * two parameters, gamma (filled with 1) then beta (0), each a weight tensor of dims {H, 1}; creating them draws no
    * random numbers.  A training forward normalises by the batch statistics and updates the running mean (start 0) and
@@ -345,6 +350,8 @@ public:
   int epilogue;      /* ROC_SG_EPI_* the forward store applies (set by Model::init fusion) */
   int bwdEpilogue;   /* same for the backward launch */
   int fwdOut, bwdOut;/* region the fused forward / backward writes (-1: own output / input grad) */
+  int teleT;         /* >= 0: a scaled_add fused into the store (roc_sg_forward_teleport_planned) reads this region as t */
+  float teleAlpha, teleBeta;   /*   ... with these coefficients */
 };
 
 class AttentionGather : public GnnOp {  /* not in the reference: Model::attention_gather */
@@ -400,6 +407,8 @@ public:
   int reluOut;      /* a relu fused into the forward: its output region, whose grad the backward reads and whose
                        values' mask it applies (-1: none; the backward reads its own output's grad) */
   bool bwdFused;    /* backward done in another op's epilogue (a Linear's dX or the loss) */
+  bool sharesWithScaledAdd;   /* a scaled_add also reads the input: the backward may add to its gradient (init) */
+  float* scratch;   /* the input gradient when another op already wrote it (added afterwards; Runtime arena) */
 };
 
 class Linear : public GnnOp {  /* gnn.h:263-285, linear.cc */
@@ -442,6 +451,16 @@ public:
   ElementType elementType;
 };
 
+class ScaledAdd : public GnnOp {  /* not in the reference: Model::scaled_add */
+public:
+  ScaledAdd(const Model& model, const Tensor& a, const Tensor& b, float alpha, float beta);
+  void init(const Model& model);
+  void forward(const Model& model);
+  void backward(const Model& model);
+public:
+  float alpha, beta;
+};
+
 class Dropout : public GnnOp {  /* gnn.h:321-344, dropout.cc */
 public:
   Dropout(const Model& model, const Tensor& input, float rate, int seed);
@@ -452,6 +471,8 @@ public:
   float rate;
   int seed;
   int opIndex;      /* position in the model: distinguishes the Philox streams of the layers */
+  bool sharesWithScaledAdd;   /* a scaled_add also reads the input: the backward may add to its gradient (init) */
+  float* scratch;   /* the input gradient when another op already wrote it (added afterwards; Runtime arena) */
 };
 
 class BatchNorm : public GnnOp {  /* not in the reference: Model::batch_norm */

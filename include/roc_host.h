@@ -62,6 +62,8 @@ int roc_host_elu(roc_host* h, int t);
 /* Model::attention_scores(t, heads): appends one parameter (A, 2 * heads rows of F).  One partition only. */
 int roc_host_attention_scores(roc_host* h, int t, int heads);
 int roc_host_add(roc_host* h, int a, int b);
+/* Model::scaled_add(a, b, alpha, beta): fmaf(alpha, a, beta * b) */
+int roc_host_scaled_add(roc_host* h, int a, int b, float alpha, float beta);
 /* Model::batch_norm(t, momentum, eps): appends two parameters (gamma, beta).  One partition only. */
 int roc_host_batch_norm(roc_host* h, int t, float momentum, float eps);
 /* the running mean and variance (H floats each) of the batch_norm whose output is t (Model::get / set_batch_norm_stats) */
@@ -129,11 +131,13 @@ int roc_host_set_parameter(roc_host* h, int p, const float* host);
 #define ROC_HOST_OP_BATCH_NORM 13
 #define ROC_HOST_OP_ELU 14
 #define ROC_HOST_OP_ATTENTION_SCORES 15
+#define ROC_HOST_OP_SCALED_ADD 16
 struct roc_host_op_info {   /* a struct tag only: roc_host_op_info is also the function's name */
   int kind;          /* ROC_HOST_OP_* */
   int fusedInto;     /* >= 0: the layer whose kernel does this op's forward */
   int bwdFused;      /* norm: its backward is done by a Linear's dX epilogue or by the loss */
-  int epilogue;      /* sum ScatterGather: ROC_SG_EPI_* of the forward store */
+  int epilogue;      /* sum ScatterGather: ROC_SG_EPI_* of the forward store (with a scaled_add fused into it: NORM and
+                        NORM_OUT of roc_sg_forward_teleport_planned) */
   int bwdEpilogue;   /*   ... and of the backward store */
   int fwdOut;        /*   the tensor the forward writes (-1: its own output); also a Linear's and a batch_norm's (the
                         output of the relu fused into it) */

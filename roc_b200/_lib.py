@@ -15,11 +15,13 @@ ROC_ERR_INVALID, ROC_ERR_UNSUPPORTED, ROC_ERR_NOMEM, ROC_ERR_NO_DEVICE, ROC_ERR_
 AC_MODE_NONE, AC_MODE_RELU, AC_MODE_SIGMOID, AC_MODE_ELU = 0, 1, 2, 3
 MASK_TRAIN, MASK_VAL, MASK_TEST, MASK_NONE = 0, 1, 2, 3
 SG_EPI_NONE, SG_EPI_NORM, SG_EPI_RELU = 0, 1, 2
+SG_EPI_NORM_OUT = 4                                        # roc_sg_forward_teleport_planned: the next hop's norm
 AGGR_AVG, AGGR_MAX, AGGR_MIN, AGGR_SUM = 0, 1, 2, 3        # AggrType (gnn.h:75-80); ROC_SG_AGGR_MAX / _MIN = 1 / 2
 SG_NOARG = 0xFFFFFFFF                                      # arg of a row with no in-edge
 LINEAR_NORM_EPILOGUE = 1
 LINEAR_Y_BF16 = 2                                          # Y holds bf16 bits
 SG_RED_BSUM = 12                                           # roc_sg_launch.red of the sum over bf16 rows
+SG_RED_TELE = 13                                           # roc_sg_launch.red of the teleport sum
 SG_RED_BF16 = 16                                           # + r: roc_sg_launch.red of reduction r's bf16 form
 HOST_DTYPES = ("float32", "bfloat16", "int32")             # ROC_HOST_DTYPE_* by value
 LINEAR_BWD_ONLY_DX, LINEAR_BWD_ONLY_DW = 1, 2
@@ -89,7 +91,7 @@ class MultilabelMetrics(C.Structure):
 HOST_OPS = ("linear", "indegree_norm", "scatter_gather", "scatter_gather_max", "scatter_gather_min",
             "scatter_gather_weighted", "attention_gather", "relu", "sigmoid", "add", "dropout",
             "softmax_cross_entropy", "sigmoid_cross_entropy", "batch_norm", "elu",
-            "attention_scores")   # ROC_HOST_OP_* by value
+            "attention_scores", "scaled_add")   # ROC_HOST_OP_* by value
 
 
 class HostOpInfo(C.Structure):
@@ -136,6 +138,7 @@ PROTOTYPES = {
     "roc_sg_plan_rows_sorted": (i32, [vp, C.POINTER(i32), vp]),
     "roc_sg_forward_planned": (i32, [vp, i32, vp, i64, vp, i64, i32, vp]),
     "roc_sg_forward_planned_bf16": (i32, [vp, i32, vp, i64, vp, i64, i32, vp]),
+    "roc_sg_forward_teleport_planned": (i32, [vp, i32, vp, i64, f32, vp, i64, f32, vp, i64, i32, vp]),
     "roc_sg_minmax_forward_planned": (i32, [vp, i32, i32, vp, i64, vp, i64, vp, i64, vp]),
     "roc_sg_minmax_forward_planned_bf16": (i32, [vp, i32, i32, vp, i64, vp, i64, vp, i64, vp]),
     "roc_sg_minmax_backward_planned": (i32, [vp, i32, u32, vp, i64, vp, i64, vp, i64, vp]),
@@ -192,6 +195,8 @@ PROTOTYPES = {
     "roc_activation_bwd_y_bf16": (i32, [i64, i32, i32, vp, i64, vp, i64, vp, i64, i32, vp]),
     "roc_add_fwd": (i32, [i64, i32, vp, i64, vp, i64, vp, i64, vp]),
     "roc_add_bwd": (i32, [i64, i32, vp, i64, vp, i64, i32, vp, i64, i32, vp]),
+    "roc_scaled_add_fwd": (i32, [i64, i32, f32, vp, i64, f32, vp, i64, vp, i64, vp]),
+    "roc_scaled_add_bwd": (i32, [i64, i32, vp, i64, f32, vp, i64, i32, f32, vp, i64, i32, vp]),
     "roc_dropout_fwd": (i32, [i64, i32, i64, f32, u64, u32, vp, i64, vp, i64, vp]),
     "roc_dropout_bwd": (i32, [i64, i32, i64, f32, u64, u32, vp, i64, vp, i64, vp]),
     "roc_dropout_mask": (i32, [i64, i32, i64, f32, u64, u32, vp, i64, vp]),
@@ -254,6 +259,7 @@ PROTOTYPES = {
     "roc_host_relu": (i32, [vp, i32]),
     "roc_host_sigmoid": (i32, [vp, i32]),
     "roc_host_add": (i32, [vp, i32, i32]),
+    "roc_host_scaled_add": (i32, [vp, i32, i32, f32, f32]),
     "roc_host_elu": (i32, [vp, i32]),
     "roc_host_attention_scores": (i32, [vp, i32, i32]),
     "roc_host_batch_norm": (i32, [vp, i32, f32, f32]),

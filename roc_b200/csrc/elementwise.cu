@@ -7,6 +7,7 @@
 // All are grid-stride kernels over [rows][H] windows of [rows][ld] tensors,
 // 16-byte vectorised when H, ld and the base pointers allow, launched with a
 // grid that is a multiple of the SM count (132 on H100).
+#include <cmath>
 #include <initializer_list>
 #include "common.cuh"
 
@@ -132,6 +133,64 @@ k_add_bwd(int64_t rows, int Wq, const float* __restrict__ dy, int64_t ldy, float
       float g = dy[r * ldy + c + k];
       if (da) da[r * lda + c + k] = accA ? da[r * lda + c + k] + g : g;
       if (db) db[r * ldb + c + k] = accB ? db[r * ldb + c + k] + g : g;
+    }
+  }
+}
+
+// ----------------------------------------------------------- scaled add -----
+// y = fmaf(alpha, a, beta * b), the product beta * b rounded to fp32 first (the teleport store of
+// roc_sg_forward_teleport_planned computes the same expression).  Streaming loads and stores: every byte is touched once.
+template <int VEC>
+__global__ void __launch_bounds__(EW_T)
+k_scaled_add(int64_t rows, int Wq, float alpha, const float* __restrict__ a, int64_t lda, float beta,
+             const float* __restrict__ b, int64_t ldb, float* __restrict__ y, int64_t ldy) {
+  const int64_t total = rows * (int64_t)Wq;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total;
+       i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = i / Wq;
+    const int c = (int)(i - r * Wq) * VEC;
+    if (VEC == 4) {
+      const float4 av = __ldcs(reinterpret_cast<const float4*>(a + r * lda + c));
+      const float4 bv = __ldcs(reinterpret_cast<const float4*>(b + r * ldb + c));
+      __stcs(reinterpret_cast<float4*>(y + r * ldy + c),
+             make_float4(fmaf(alpha, av.x, __fmul_rn(beta, bv.x)), fmaf(alpha, av.y, __fmul_rn(beta, bv.y)),
+                         fmaf(alpha, av.z, __fmul_rn(beta, bv.z)), fmaf(alpha, av.w, __fmul_rn(beta, bv.w))));
+    } else {
+      __stcs(y + r * ldy + c, fmaf(alpha, __ldcs(a + r * lda + c), __fmul_rn(beta, __ldcs(b + r * ldb + c))));
+    }
+  }
+}
+
+// its backward: dA (+)= alpha * dY, dB (+)= beta * dY in one pass over dY; a NULL output is skipped.  Accumulation is
+// fmaf(coef, dY, d).
+__device__ __forceinline__ float sa_grad(float coef, float g, float d, int acc) { return acc ? fmaf(coef, g, d) : coef * g; }
+template <int VEC>
+__global__ void __launch_bounds__(EW_T)
+k_scaled_add_bwd(int64_t rows, int Wq, const float* __restrict__ dy, int64_t ldy, float alpha, float* __restrict__ da,
+                 int64_t lda, int accA, float beta, float* __restrict__ db, int64_t ldb, int accB) {
+  const int64_t total = rows * (int64_t)Wq;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total;
+       i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = i / Wq;
+    const int c = (int)(i - r * Wq) * VEC;
+    if (VEC == 4) {
+      const float4 g = __ldcs(reinterpret_cast<const float4*>(dy + r * ldy + c));
+      if (da) {
+        float4* p = reinterpret_cast<float4*>(da + r * lda + c);
+        const float4 o = accA ? *p : make_float4(0.f, 0.f, 0.f, 0.f);
+        __stcs(p, make_float4(sa_grad(alpha, g.x, o.x, accA), sa_grad(alpha, g.y, o.y, accA),
+                              sa_grad(alpha, g.z, o.z, accA), sa_grad(alpha, g.w, o.w, accA)));
+      }
+      if (db) {
+        float4* p = reinterpret_cast<float4*>(db + r * ldb + c);
+        const float4 o = accB ? *p : make_float4(0.f, 0.f, 0.f, 0.f);
+        __stcs(p, make_float4(sa_grad(beta, g.x, o.x, accB), sa_grad(beta, g.y, o.y, accB),
+                              sa_grad(beta, g.z, o.z, accB), sa_grad(beta, g.w, o.w, accB)));
+      }
+    } else {
+      const float g = __ldcs(dy + r * ldy + c);
+      if (da) da[r * lda + c] = sa_grad(alpha, g, accA ? da[r * lda + c] : 0.f, accA);
+      if (db) db[r * ldb + c] = sa_grad(beta, g, accB ? db[r * ldb + c] : 0.f, accB);
     }
   }
 }
@@ -827,6 +886,39 @@ extern "C" int roc_add_bwd(int64_t rows, int H, const float* dY, int64_t ldDY, f
   if (!dY || rows < 0 || H <= 0 || ldDY < H) return ROC_ERR_INVALID;
   if (rows == 0 || (!dA && !dB)) return ROC_OK;
   k_add_bwd<1><<<ew_grid(rows * H, EW_T), EW_T, 0, as_stream(stream)>>>(rows, H, dY, ldDY, dA, ldDA, accA, dB, ldDB, accB);
+  ROC_LAUNCH_CHECK();
+  return ROC_OK;
+}
+
+extern "C" int roc_scaled_add_fwd(int64_t rows, int H, float alpha, const float* a, int64_t ldA, float beta,
+                                  const float* b, int64_t ldB, float* y, int64_t ldY, roc_stream_t stream) {
+  if (!a || !b || !y || rows < 0 || H <= 0 || ldA < H || ldB < H || ldY < H || !std::isfinite(alpha) ||
+      !std::isfinite(beta))
+    return ROC_ERR_INVALID;
+  if (rows == 0) return ROC_OK;
+  cudaStream_t st = as_stream(stream);
+  if (vec_ok(H, {ldA, ldB, ldY}, {a, b, y}))
+    k_scaled_add<4><<<ew_grid(rows * (H / 4), EW_T), EW_T, 0, st>>>(rows, H / 4, alpha, a, ldA, beta, b, ldB, y, ldY);
+  else
+    k_scaled_add<1><<<ew_grid(rows * H, EW_T), EW_T, 0, st>>>(rows, H, alpha, a, ldA, beta, b, ldB, y, ldY);
+  ROC_LAUNCH_CHECK();
+  return ROC_OK;
+}
+
+extern "C" int roc_scaled_add_bwd(int64_t rows, int H, const float* dY, int64_t ldDY, float alpha, float* dA,
+                                  int64_t ldDA, int accA, float beta, float* dB, int64_t ldDB, int accB,
+                                  roc_stream_t stream) {
+  if (!dY || rows < 0 || H <= 0 || ldDY < H || (dA && ldDA < H) || (dB && ldDB < H) || (dA && dA == dB) ||
+      !std::isfinite(alpha) || !std::isfinite(beta))
+    return ROC_ERR_INVALID;
+  if (rows == 0 || (!dA && !dB)) return ROC_OK;
+  cudaStream_t st = as_stream(stream);
+  if (vec_ok(H, {ldDY, dA ? ldDA : 4, dB ? ldDB : 4}, {dY, dA, dB}))
+    k_scaled_add_bwd<4><<<ew_grid(rows * (H / 4), EW_T), EW_T, 0, st>>>(rows, H / 4, dY, ldDY, alpha, dA, ldDA, accA,
+                                                                       beta, dB, ldDB, accB);
+  else
+    k_scaled_add_bwd<1><<<ew_grid(rows * H, EW_T), EW_T, 0, st>>>(rows, H, dY, ldDY, alpha, dA, ldDA, accA, beta, dB,
+                                                                 ldDB, accB);
   ROC_LAUNCH_CHECK();
   return ROC_OK;
 }

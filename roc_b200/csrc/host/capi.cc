@@ -114,6 +114,9 @@ int roc_host_attention_scores(roc_host* h, int t, int heads) {
   return h->push(h->m().attention_scores(h->at(t), heads));
 }
 int roc_host_add(roc_host* h, int a, int b) { return h->push(h->m().add(h->at(a), h->at(b))); }
+int roc_host_scaled_add(roc_host* h, int a, int b, float alpha, float beta) {
+  return h->push(h->m().scaled_add(h->at(a), h->at(b), alpha, beta));
+}
 int roc_host_batch_norm(roc_host* h, int t, float momentum, float eps) {
   return h->push(h->m().batch_norm(h->at(t), momentum, eps));
 }

@@ -144,7 +144,7 @@ inline int64_t round_up8(int64_t x) { return (x + 7) / 8 * 8; }
 
 // an op's ROC_HOST_OP_* kind (roc_host_op_info), and each kind's name in refusals and the per-op trace / profile
 int op_kind(const GnnOp* op);
-extern const char* const opKindNames[ROC_HOST_OP_ATTENTION_SCORES + 1];
+extern const char* const opKindNames[ROC_HOST_OP_SCALED_ADD + 1];
 
 }  // namespace host
 }  // namespace roc

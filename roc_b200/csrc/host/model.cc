@@ -105,6 +105,16 @@ Tensor Model::add(const Tensor& a, const Tensor& b) {
   layers.push_back(op);
   return op->outputs[0];
 }
+Tensor Model::scaled_add(const Tensor& a, const Tensor& b, float alpha, float beta) {
+  if (!std::isfinite(alpha) || !std::isfinite(beta)) ROC_FATAL("scaled_add: alpha and beta must be finite");
+  if (a.region == b.region) ROC_FATAL("scaled_add: a and b must be different tensors");
+  if (a.numDim != b.numDim) ROC_FATAL("scaled_add: a and b must have the same shape");
+  for (int i = 0; i < a.numDim; i++)
+    if (a.dims[i] != b.dims[i]) ROC_FATAL("scaled_add: a and b must have the same shape");
+  GnnOp* op = new ScaledAdd(*this, a, b, alpha, beta);
+  layers.push_back(op);
+  return op->outputs[0];
+}
 Tensor Model::dropout(const Tensor& _input, float rate, int seed) {
   Dropout* op = new Dropout(*this, _input, rate, seed);
   op->opIndex = (int)layers.size();
@@ -253,10 +263,10 @@ Tensor Model::batch_norm(const Tensor& input, float momentum, float eps) {
 void Model::train_mode(void) { mode = MD_MODE_TRAIN; }
 void Model::infer_mode(void) { mode = MD_MODE_INFER; }
 
-const char* const roc::host::opKindNames[ROC_HOST_OP_ATTENTION_SCORES + 1] = {
+const char* const roc::host::opKindNames[ROC_HOST_OP_SCALED_ADD + 1] = {
     "linear", "indegree_norm", "scatter_gather", "scatter_gather(max)", "scatter_gather(min)",
     "scatter_gather(weighted)", "attention_gather", "relu", "sigmoid", "add", "dropout", "softmax_cross_entropy",
-    "sigmoid_cross_entropy", "batch_norm", "elu", "attention_scores"};
+    "sigmoid_cross_entropy", "batch_norm", "elu", "attention_scores", "scaled_add"};
 int roc::host::op_kind(const GnnOp* op) {
   if (const ScatterGather* sg = dynamic_cast<const ScatterGather*>(op))
     return sg->aggr == AGGR_MAX   ? ROC_HOST_OP_SCATTER_GATHER_MAX
@@ -275,6 +285,7 @@ int roc::host::op_kind(const GnnOp* op) {
          : dynamic_cast<const SigmoidCrossEntropy*>(op)   ? ROC_HOST_OP_SIGMOID_CROSS_ENTROPY
          : dynamic_cast<const BatchNorm*>(op)             ? ROC_HOST_OP_BATCH_NORM
          : dynamic_cast<const AttentionScores*>(op)       ? ROC_HOST_OP_ATTENTION_SCORES
+         : dynamic_cast<const ScaledAdd*>(op)             ? ROC_HOST_OP_SCALED_ADD
                                                           : ROC_HOST_OP_ADD;
 }
 
@@ -500,6 +511,55 @@ static void fuse_gcn_block(const std::vector<GnnOp*>& layers, Wiring& w) {
   }
 }
 
+// which indegree_norm and dropout ops read a tensor a scaled_add also reads: their backward adds to an input gradient
+// another op already wrote, where any other wiring is refused (quirk Q7)
+static void mark_scaled_add_readers(const std::vector<GnnOp*>& layers) {
+  std::set<int> read;
+  for (GnnOp* op : layers)
+    if (as<ScaledAdd>(op))
+      for (int j = 0; j < op->numInputs; j++) read.insert(op->inputs[j].region);
+  for (GnnOp* op : layers) {
+    if (InDegreeNorm* n = as<InDegreeNorm>(op)) n->sharesWithScaledAdd = read.count(n->inputs[0].region) > 0;
+    if (Dropout* d = as<Dropout>(op)) d->sharesWithScaledAdd = read.count(d->inputs[0].region) > 0;
+  }
+}
+
+// ---- fusion of  sum scatter_gather -> indegree_norm -> scaled_add(., t) [-> indegree_norm]  (APPNP / GCNII's hop):
+//      on a scatter_gather whose store fuse_gcn_block fused with its indegree_norm (no relu), that norm's output feeding
+//      only a scaled_add as its first input.  The scatter_gather's store applies the teleport
+//      (roc_sg_forward_teleport_planned), reading t = the scaled_add's second input, and writes the scaled_add's output;
+//      when that output feeds only an unfused indegree_norm (the next hop's), the store also divides by sqrt(deg)
+//      (ROC_SG_EPI_NORM_OUT) and writes that norm's output.  Forward only: the scaled_add's and both norms' backward
+//      kernels still run.  t must exist when the scatter_gather runs: produced before it, or a leaf.  It runs after
+//      choose_bf16_aggregation (which none of its decisions changes): a scatter_gather whose input that pass made bf16
+//      has no teleport kernel, and is left unfused.
+static void fuse_teleport(const Model& m, Wiring& w) {
+  const std::vector<GnnOp*>& layers = m.layers;
+  for (size_t l = 0; l < layers.size(); l++) {
+    ScatterGather* sg = as_sum_sg(layers[l]);
+    if (!sg || sg->epilogue != ROC_SG_EPI_NORM || sg->fwdOut < 0 || sg->teleT >= 0) continue;
+    if (m.ctx->t(sg->inputs[0].region).isBf16) continue;
+    const int rn = sg->fwdOut;
+    if (w.consumers[rn] != 1) continue;
+    ScaledAdd* sa = as<ScaledAdd>(layers[w.consumerOp[rn]]);
+    if (!sa || sa->fusedInto >= 0 || sa->inputs[0].region != rn) continue;
+    const int rt = sa->inputs[1].region;
+    if (w.producer.count(rt) && w.producer[rt] >= (int)l) continue;
+    sg->teleT = rt;
+    sg->teleAlpha = sa->alpha;
+    sg->teleBeta = sa->beta;
+    sg->fwdOut = sa->outputs[0].region;
+    sa->fusedInto = (int)l;
+    const int ry = sa->outputs[0].region;
+    if (w.consumers[ry] != 1) continue;
+    InDegreeNorm* n = as<InDegreeNorm>(layers[w.consumerOp[ry]]);
+    if (!n || n->fusedInto >= 0) continue;
+    sg->epilogue |= ROC_SG_EPI_NORM_OUT;
+    sg->fwdOut = n->outputs[0].region;
+    n->fusedInto = (int)l;   // forward only; its backward kernel still runs
+  }
+}
+
 // ---- fusion of  batch_norm -> relu: the BN output feeds only the relu.  The BN forward writes the relu's output, and
 //      its backward reads that output's gradient and masks it by fma(x, a, b) > 0 from its saved affine map.
 //      The other peepholes never cross a BN.  In GCN, SG -> indegree_norm still fuses, and the relu after the BN is
@@ -622,6 +682,7 @@ bool Model::init(const Config&) {
   build_transpose(*this);
   set_up_halo(ctx, myGraph, layers, maxSg);
   Wiring w = wire(layers);   // the passes below change no op's inputs or outputs
+  mark_scaled_add_readers(layers);
   if (fuse) {
     fuse_gcn_block(layers, w);
     fuse_batch_norm_relu(layers, w);
@@ -629,6 +690,7 @@ bool Model::init(const Config&) {
     fuse_backward_epilogues(ctx, layers, w);
   }
   if (bf16Aggregation) choose_bf16_aggregation(ctx, layers, w);
+  if (fuse && ctx->numParts == 1) fuse_teleport(*this, w);   // after the bf16 choice, which it reads
   for (size_t l = 0; l < layers.size(); l++) layers[l]->init(*this);
   ctx->opNames.clear();
   for (size_t l = 0; l < layers.size(); l++)
@@ -983,7 +1045,8 @@ struct PushPipe {
 
 // -------------------------------------------------------- ScatterGather -----
 ScatterGather::ScatterGather(const Model& model, const Tensor& _input, AggrType _aggr)
-    : GnnOp(_input), aggr(_aggr), arg(nullptr), argLd(0), epilogue(0), bwdEpilogue(0), fwdOut(-1), bwdOut(-1) {
+    : GnnOp(_input), aggr(_aggr), arg(nullptr), argLd(0), epilogue(0), bwdEpilogue(0), fwdOut(-1), bwdOut(-1), teleT(-1),
+      teleAlpha(1.0f), teleBeta(1.0f) {
   // scattergather.cc:33-37
   ROC_ASSERT(inputs[0].type == Tensor::NODE_TENSOR);
   ROC_ASSERT(inputs[0].numDim == 2);
@@ -1067,7 +1130,11 @@ void ScatterGather::forward(const Model& model) {
   rt->sg_end();
   float* dst = rt->data(outRegion);
   rt->sg_begin(H);
-  if (xBf16)
+  if (teleT >= 0)   // a fused scaled_add (fuse_teleport: one partition, fp32 input)
+    ROC_CHECK(roc_sg_forward_teleport_planned(model.myGraph.plan, H, src, ldIn, teleAlpha, rt->data(teleT),
+                                              rt->t(teleT).ld, teleBeta, dst, rt->t(outRegion).ld, epilogue,
+                                              rt->stream));
+  else if (xBf16)
     ROC_CHECK(roc_sg_forward_planned_bf16(model.myGraph.plan, H, rt->data_bf16(inputs[0].region), ldIn, dst,
                                           rt->t(outRegion).ld, epilogue, rt->stream));
   else
@@ -1332,7 +1399,7 @@ void WeightedScatterGather::backward(const Model& model) {
 
 // --------------------------------------------------------- InDegreeNorm -----
 InDegreeNorm::InDegreeNorm(const Model& model, const Tensor& _input)
-    : GnnOp(_input), reluOut(-1), bwdFused(false) {
+    : GnnOp(_input), reluOut(-1), bwdFused(false), sharesWithScaledAdd(false), scratch(nullptr) {
   ROC_ASSERT(inputs[0].type == Tensor::NODE_TENSOR);   // graphnorm.cc:33-35
   ROC_ASSERT(inputs[0].numDim == 2);
   ROC_ASSERT(inputs[0].dims[1] == model.myGraph.numNodes);
@@ -1350,19 +1417,23 @@ void InDegreeNorm::forward(const Model& model) {
                               rt->t(outputs[0].region).ld, NULL, rt->stream));
 }
 
+// The kernel overwrites the input gradient, so an input whose gradient another op's backward already wrote is refused
+// (graphnorm_kernel.cu:133, quirk Q7), unless a scaled_add also reads it (sharesWithScaledAdd: APPNP's MLP output,
+// which every hop's scaled_add reads): that one gets its part in scratch, added afterwards.
 void InDegreeNorm::backward(const Model& model) {
   RuntimeImpl* rt = model.ctx;
-  ROC_ASSERT(resetInputGrads[0]);   // graphnorm_kernel.cu:133
+  ROC_ASSERT(resetInputGrads[0] || sharesWithScaledAdd);   // graphnorm_kernel.cu:133
   if (!rt->t(inputs[0].region).requiresGrad) return;
   // fused into the linear's epilogue forward => the SG backward epilogue already
   // produced d(linear out); nothing to do here
-  if (fusedInto >= 0 && dynamic_cast<Linear*>(model.layers[(size_t)fusedInto])) return;
-  if (bwdFused) return;   // a Linear's dX epilogue / the softmax already wrote this gradient
+  if (fusedInto >= 0 && dynamic_cast<Linear*>(model.layers[(size_t)fusedInto])) { ROC_ASSERT(resetInputGrads[0]); return; }
+  if (bwdFused) { ROC_ASSERT(resetInputGrads[0]); return; }   // a Linear's dX epilogue / the softmax already wrote this gradient
   const Graph& g = model.myGraph;
-  const int src = reluOut >= 0 ? reluOut : outputs[0].region;
+  const int src = reluOut >= 0 ? reluOut : outputs[0].region, in = inputs[0].region;
+  float* dst = grad_or_scratch(model, in, resetInputGrads[0], scratch);
   ROC_CHECK(roc_indegree_norm(g.rowLeft, g.rowRight, g.colLeft, (int)inputs[0].dims[0], g.d_rowEnd, rt->grad(src),
-                              rt->t(src).ld, rt->grad(inputs[0].region), rt->t(inputs[0].region).ld,
-                              reluOut >= 0 ? rt->data(reluOut) : NULL, rt->stream));
+                              rt->t(src).ld, dst, rt->t(in).ld, reluOut >= 0 ? rt->data(reluOut) : NULL, rt->stream));
+  if (!resetInputGrads[0]) add_scratch(model, in, scratch);
 }
 
 // ----------------------------------------------------------------- Linear ---
@@ -1612,9 +1683,33 @@ void Element::backward(const Model& model) {
                         rt->t(inputs[1].region).ld, resetInputGrads[1] ? 0 : 1, rt->stream));
 }
 
+// -------------------------------------------------------------- ScaledAdd ---
+ScaledAdd::ScaledAdd(const Model& model, const Tensor& a, const Tensor& b, float _alpha, float _beta)
+    : GnnOp(a, b), alpha(_alpha), beta(_beta) {
+  numOutputs = 1;
+  outputs[0] = model.create_node_tensor<DATATYPE>((int)a.dims[0]);
+}
+void ScaledAdd::init(const Model&) {}
+void ScaledAdd::forward(const Model& model) {
+  if (fusedInto >= 0) return;   // applied by the scatter_gather's store
+  RuntimeImpl* rt = model.ctx;
+  const int a = inputs[0].region, b = inputs[1].region, y = outputs[0].region;
+  ROC_CHECK(roc_scaled_add_fwd(model.local_rows(), (int)inputs[0].dims[0], alpha, rt->data(a), rt->t(a).ld, beta,
+                               rt->data(b), rt->t(b).ld, rt->data(y), rt->t(y).ld, rt->stream));
+}
+void ScaledAdd::backward(const Model& model) {
+  RuntimeImpl* rt = model.ctx;
+  const int a = inputs[0].region, b = inputs[1].region, y = outputs[0].region;
+  float* dA = rt->t(a).requiresGrad ? rt->grad(a) : NULL;
+  float* dB = rt->t(b).requiresGrad ? rt->grad(b) : NULL;
+  ROC_CHECK(roc_scaled_add_bwd(model.local_rows(), (int)inputs[0].dims[0], rt->grad(y), rt->t(y).ld, alpha, dA,
+                               rt->t(a).ld, resetInputGrads[0] ? 0 : 1, beta, dB, rt->t(b).ld,
+                               resetInputGrads[1] ? 0 : 1, rt->stream));
+}
+
 // ---------------------------------------------------------------- Dropout ---
 Dropout::Dropout(const Model& model, const Tensor& _input, float _rate, int _seed)
-    : GnnOp(_input), rate(_rate), seed(_seed), opIndex(0) {
+    : GnnOp(_input), rate(_rate), seed(_seed), opIndex(0), sharesWithScaledAdd(false), scratch(nullptr) {
   ROC_ASSERT(_input.numDim == 2);
   ROC_ASSERT(_input.type == Tensor::NODE_TENSOR);
   numOutputs = 1;
@@ -1639,12 +1734,17 @@ void Dropout::forward(const Model& model) {
 void Dropout::backward(const Model& model) {
   RuntimeImpl* rt = model.ctx;
   if (!rt->t(inputs[0].region).requiresGrad) return;   // leaf input (Q8)
-  ROC_ASSERT(resetInputGrads[0]);   // dropout_kernel.cu:119
+  ROC_ASSERT(resetInputGrads[0] || (sharesWithScaledAdd && fusedInto < 0));   // dropout_kernel.cu:119
   if (fusedInto >= 0) return;       // the consuming Linear's dX epilogue already wrote this gradient
+  // the kernel overwrites the input gradient; one another op already wrote (only where a scaled_add also reads the
+  // input: GCNII's x0) gets its part in scratch, added afterwards
+  const int in = inputs[0].region;
+  float* dst = grad_or_scratch(model, in, resetInputGrads[0], scratch);
   const DropDraw d = drop_draw(model, *this);
   ROC_CHECK(roc_dropout_bwd(model.local_rows(), (int)inputs[0].dims[0], model.myGraph.rowLeft, d.rate, d.key,
-                            rt->trainStep, rt->grad(outputs[0].region), rt->t(outputs[0].region).ld,
-                            rt->grad(inputs[0].region), rt->t(inputs[0].region).ld, rt->stream));
+                            rt->trainStep, rt->grad(outputs[0].region), rt->t(outputs[0].region).ld, dst,
+                            rt->t(in).ld, rt->stream));
+  if (!resetInputGrads[0]) add_scratch(model, in, scratch);
 }
 
 // The [INFER] line of softmax_kernel.cu:141-152 (printed once per partition, quirk Q20), to stderr AND stdout, as the

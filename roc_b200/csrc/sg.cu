@@ -47,6 +47,9 @@
 //  * attention dropout (roc_sg_attn_*_dropout_*) is SG_RED_DROP on ATTN, ADST and ASRC: each pass loads one keep byte
 //    per edge beside its source id and weighs a dropped head's term by 0.  k_attn_keep writes those bytes from Philox,
 //    keyed by the (destination, source) pair, in any plan's edge order.
+//  * the teleport sum (roc_sg_forward_teleport_planned, APPNP / GCNII's hop) is TELE: SUM's row of the table, column
+//    blocks and sum fix-ups, with a row store (tele_store) that also reads the row of t and applies
+//    post(fmaf(alpha, pre(sum), beta * t)) wherever a row is finally stored.  It runs every width on sg_chunk_kernel.
 //
 // Algorithmic bytes per launch (DESIGN.md): E*(4H+4) + Nloc*(4H+8); min / max forward E*(4H+4) + Nloc*(8H+8),
 // backward E*(8H+4) + Nloc*(4H+8); the sum over bf16 rows E*(2H+4) + Nloc*(4H+8); weighted forward E*(4H+8) + Nloc*(4H+8), edge dot E*(4H+8) + Nloc*4H; attention
@@ -258,9 +261,11 @@ __device__ __forceinline__ typename V<VEC>::T ld_bf16(const char* p) {
 // SG_RED_BF16 added to MAX, MIN, ATTN, ADST, ASRC, WSUM or EDOT is that reduction's bf16 form (the roc_sg_*_bf16
 // calls): the feature rows X it reads (gathered, or ASRC's own row i) are bf16, loaded and widened as BSUM's are, and
 // everything else is the fp32 reduction's, its row of SG_REDS included.
+// TELE is the sum whose row store is the teleport of roc_sg_forward_teleport_planned (tele_store): it adds what SUM adds
+// in SUM's order, and only what a finished row stores differs.
 enum { SG_RED_SUM = 0, SG_RED_MAX = ROC_SG_AGGR_MAX, SG_RED_MIN = ROC_SG_AGGR_MIN, SG_RED_MASK = 3,
        SG_RED_ASTAT = 4, SG_RED_ATTN = 5, SG_RED_ADST = 6, SG_RED_ASRC = 7, SG_RED_WSUM = 8, SG_RED_EDOT = 9,
-       SG_RED_TSUM = 10, SG_RED_TMASK = 11, SG_RED_BSUM = 12 };
+       SG_RED_TSUM = 10, SG_RED_TMASK = 11, SG_RED_BSUM = 12, SG_RED_TELE = 13 };
 constexpr int SG_RED_BF16 = 16;
 // SG_RED_DROP added to ATTN, ADST or ASRC (with or without SG_RED_BF16) is that pass with attention dropout
 // (roc_sg_attn_*_dropout): it loads each edge's keep byte (p.keep) beside its source id, the way WSUM loads its weight,
@@ -391,6 +396,7 @@ struct SgParams {
   union {
     int dwAdd;          // EDOT: add to dw instead of overwriting it
     float keepScale;    // attention dropout: the scale of a kept weight
+    float teleBeta;     // TELE: beta, the coefficient of t
   };
   // attention (units of float unless stated).  The edge-weighted passes use two of its slots (score, out2), so that
   // the struct, every kernel's parameter block, keeps its layout (a union there changed the attention kernels' code).
@@ -398,7 +404,8 @@ struct SgParams {
   const float* stats;   // ATTN: [nloc][ldStats] m | 1/Z of the local rows
   const float4* rec;    // ADST / ASRC: [*][heads] {s_dst, m, 1/Z, D}, indexed like `in`
   const void* xrow;     // ADST, EDOT: G, ASRC: X, the local row's own row (units of T, ldX); EDOT: indexed by plan
-                        // row, else like `in`.  TSUM: the original graph's rowEnd (u64), for in_degree
+                        // row, else like `in`.  TSUM: the original graph's rowEnd (u64), for in_degree.  TELE: t, fp32
+                        // rows indexed by plan row with leading dimension ldS (in floats), and alpha in `slope`
   float* out2;          // ASTAT: unused; ADST / ASRC: heads-wide output [nloc][ldOut2];  EDOT: [E] dw of each local edge
   float* carry2;        // [numCarries][SG_LDC2] heads-wide partials (ASTAT: m | Z)
   size_t ldS, ldStats, ldX, ldOut2;
@@ -448,6 +455,35 @@ template <int RED>
 __device__ __forceinline__ uint32_t norm_deg(const SgParams& p, uint32_t r, uint32_t len) {
   if constexpr (RED == SG_RED_TSUM) return in_degree(p, r);
   else return len;
+}
+
+// TELE's row store: out[v] = post(fmaf(alpha, pre(acc), beta * t[v])), pre and post the divide by sqrtf(deg) of
+// ROC_SG_EPI_NORM and ROC_SG_EPI_NORM_OUT, each in epi_store's row-uniform form (== the IEEE divide).  That is, float
+// for float, roc_sg_forward_planned (NORM or NONE), then roc_scaled_add_fwd (beta * t rounded first), then
+// roc_indegree_norm.  t is read one float at a time, so that any pitch and alignment of t takes the row form `in` and
+// `out` chose; the pad floats of a partial last float4 take t = 0.  Column c (in T-columns) of plan row `row`.
+__device__ __forceinline__ float tele_axpby(float a, float x, float b, float t) { return fmaf(a, x, __fmul_rn(b, t)); }
+__device__ __forceinline__ float4 tele_axpby(float a, const float4& x, float b, const float4& t) {
+  return make_float4(tele_axpby(a, x.x, b, t.x), tele_axpby(a, x.y, b, t.y), tele_axpby(a, x.z, b, t.z),
+                     tele_axpby(a, x.w, b, t.w));
+}
+template <int VEC>
+__device__ __forceinline__ void tele_store(const SgParams& p, typename V<VEC>::T v, typename V<VEC>::T* dst, uint32_t row,
+                                           uint32_t c, uint32_t deg) {
+  const float* tr = static_cast<const float*>(p.xrow) + (uint64_t)row * p.ldS + (uint64_t)c * VEC;
+  typename V<VEC>::T t;
+  if constexpr (VEC == 4) {
+    const int nv = min(4, (int)p.H - 4 * (int)c);
+    t = make_float4(__ldg(tr), nv > 1 ? __ldg(tr + 1) : 0.f, nv > 2 ? __ldg(tr + 2) : 0.f, nv > 3 ? __ldg(tr + 3) : 0.f);
+  } else {
+    t = __ldg(tr);
+  }
+  const bool pre = (p.epi & ROC_SG_EPI_NORM) != 0, post = (p.epi & ROC_SG_EPI_NORM_OUT) != 0;
+  const RowDiv rd = rowdiv_make((pre || post) ? sqrtf((float)deg) : 1.f);
+  if (pre) v = V<VEC>::rdiv(v, rd);
+  v = tele_axpby(p.slope, v, p.teleBeta, t);
+  if (post) v = V<VEC>::rdiv(v, rd);
+  V<VEC>::st(dst, v);
 }
 
 // ------------------------------------------------------------- main kernel ---
@@ -614,6 +650,18 @@ sg_chunk_kernel(const SgParams p) {
         accS[ch] = 0.f;
       }
       if constexpr (RED == SG_RED_ADST) return;
+    }
+    if constexpr (RED == SG_RED_TELE) {
+      // a complete row takes the teleport whatever p.epi is; a cut row's parts store raw partials for the fix-ups
+#pragma unroll
+      for (int ch = 0; ch < NCH; ch++) {
+        if (act[ch]) {
+          if (kind == 1) tele_store<VEC>(p, acc[ch], dst + ch * L, cur, (uint32_t)(lane + ch * L), curT - curS);
+          else V<VEC>::st(dst + ch * L, acc[ch]);
+        }
+        acc[ch] = V<VEC>::zero();
+      }
+      return;
     }
     const int epi = (kind == 1) ? p.epi : 0;
 #pragma unroll
@@ -808,7 +856,8 @@ sg_chunk_kernel(const SgParams p) {
             } else {
 #pragma unroll
               for (int ch = 0; ch < NCH; ch++) {
-                if constexpr (RED == SG_RED_SUM || RED == SG_RED_TSUM || RED == SG_RED_BSUM) V<VEC>::add(acc[ch], v[u][ch]);
+                if constexpr (RED == SG_RED_SUM || RED == SG_RED_TSUM || RED == SG_RED_BSUM || RED == SG_RED_TELE)
+                  V<VEC>::add(acc[ch], v[u][ch]);
                 else if constexpr (RED == SG_RED_MASK) mask_add(acc[ch], v[u][ch], av[u][ch], p.selfBase + cur);
                 else mm_add<RED>(acc[ch], aidx[ch], v[u][ch], srcs[u]);
               }
@@ -1102,7 +1151,7 @@ sg_chunk_kernel_t(const SgParams p) {
 // U carries are loaded per batch.  The carries are taken in chunk order whatever U is, so U never changes a result;
 // MAX / MIN take fewer per batch where their index carries would otherwise spill.
 __host__ __device__ constexpr int sg_fixup_u(int L, int NCH, int RED) {
-  return (RED == SG_RED_SUM || RED == SG_RED_TSUM) ? (NCH == 1 ? (L == 4 ? 4 : 8) : 8 / NCH) : (NCH <= 2 ? 4 : 1);
+  return (RED == SG_RED_SUM || RED == SG_RED_TSUM || RED == SG_RED_TELE) ? (NCH == 1 ? (L == 4 ? 4 : 8) : 8 / NCH) : (NCH <= 2 ? 4 : 1);
 }
 
 // One worker per heavy row.
@@ -1165,6 +1214,7 @@ sg_fixup_kernel(const SgParams p) {
   for (int ch = 0; ch < NCH; ch++) {
     if (act[ch]) {
       if constexpr (MM) { V<VEC>::st(dst + lane + ch * L, acc[ch]); adst[lane + ch * L] = ai[ch]; }
+      else if constexpr (RED == SG_RED_TELE) tele_store<VEC>(p, acc[ch], dst + lane + ch * L, R, (uint32_t)(lane + ch * L), t - s);
       else epi_store<VEC>(acc[ch], dst + lane + ch * L, norm_deg<RED>(p, R, t - s), p.epi);
     }
   }
@@ -1252,7 +1302,8 @@ sg_fixup_big_kernel(const SgParams p) {
         adst[lane + ch * L] = ia;
       } else {
         for (int gg = 0; gg < WPB; gg++) V<VEC>::add(a, sp[(gg * NCH + ch) * L + lane]);
-        epi_store<VEC>(a, dst + lane + ch * L, norm_deg<RED>(p, R, t - s), p.epi);
+        if constexpr (RED == SG_RED_TELE) tele_store<VEC>(p, a, dst + lane + ch * L, R, (uint32_t)(lane + ch * L), t - s);
+        else epi_store<VEC>(a, dst + lane + ch * L, norm_deg<RED>(p, R, t - s), p.epi);
       }
     }
   }
@@ -1384,7 +1435,11 @@ struct SgRed {
 // SM.  TSUM and TMASK take the shapes of SUM and MASK, but TMASK, which also holds each group's repeated-destination
 // bits, runs three CTAs per SM at one chunk per lane.  BSUM is SUM's row with bf16 loads (ring MODE bit 8): the same
 // column blocks, shapes and sum fix-ups, so that its results are SUM's bits on the widened rows.  The other bf16 forms
-// (SG_RED_BF16) have no row of their own: they take their reduction's, fix-ups included, for the same reason.
+// (SG_RED_BF16) have no row of their own: they take their reduction's, fix-ups included, for the same reason.  TELE is
+// SUM's row without the ring (its row store needs the row of t, which the ring kernel does not load), with its own
+// fix-ups (the sum's, storing through tele_store): the same column blocks, row shapes and carry order, hence SUM's sums.
+// Its row store holds a row of t and the coefficients while a group's gathered rows are live, so it runs three CTAs
+// per SM at one chunk per lane and one gather in flight at four, where SUM's occupancy and U would spill.
 constexpr SgRed SG_REDS[] = {
     // red           maxQ4 maxQ1 ring fix           heads  carry           u4  u             minb
     {SG_RED_SUM,     256,  256,  0,   SG_FIX_SUM,   false, SG_CARRY_FLOAT, 4, {8, 4, 2, 1}, {4, 3, 3, 2}},
@@ -1399,11 +1454,12 @@ constexpr SgRed SG_REDS[] = {
     {SG_RED_EDOT,    128,  256,  -1,  SG_FIX_NONE,  false, SG_CARRY_NONE,  4, {4, 2, 1, 1}, {4, 3, 2, 1}},
     {SG_RED_TSUM,    256,  256,  4,   SG_FIX_OWN,   false, SG_CARRY_FLOAT, 4, {8, 4, 2, 1}, {4, 3, 3, 2}},
     {SG_RED_TMASK,   128,  256,  -1,  SG_FIX_SUM,   false, SG_CARRY_FLOAT, 4, {4, 2, 1, 1}, {3, 3, 3, 2}},
-    {SG_RED_BSUM,    256,  256,  8,   SG_FIX_SUM,   false, SG_CARRY_FLOAT, 4, {8, 4, 2, 1}, {4, 3, 3, 2}}};
+    {SG_RED_BSUM,    256,  256,  8,   SG_FIX_SUM,   false, SG_CARRY_FLOAT, 4, {8, 4, 2, 1}, {4, 3, 3, 2}},
+    {SG_RED_TELE,    256,  256,  -1,  SG_FIX_OWN,   false, SG_CARRY_FLOAT, 4, {8, 4, 1, 1}, {3, 3, 3, 2}}};
 constexpr bool sg_reds_in_order() {
   for (int i = 0; i < (int)(sizeof(SG_REDS) / sizeof(SG_REDS[0])); i++)
     if (SG_REDS[i].red != i) return false;
-  return sizeof(SG_REDS) / sizeof(SG_REDS[0]) == SG_RED_BSUM + 1;
+  return sizeof(SG_REDS) / sizeof(SG_REDS[0]) == SG_RED_TELE + 1;
 }
 static_assert(sg_reds_in_order(), "SG_REDS has one row per SG_RED_* value, in order");
 
@@ -1781,7 +1837,7 @@ static void t_units(SgParams& p, int vw, int cols) {
 }
 
 // The operands of run_planned only some reductions take: WSUM's weights, EDOT's G rows (indexed by plan row) and its
-// output, TSUM's row ends of the original graph.
+// output, TSUM's row ends of the original graph, TELE's t (indexed by plan row) and coefficients.
 struct SgEdge {
   const float* w = nullptr;
   const float* g = nullptr;
@@ -1789,6 +1845,9 @@ struct SgEdge {
   float* dw = nullptr;
   bool accumulate = false;
   const roc_eid_t* rowEnd = nullptr;
+  const float* t = nullptr;
+  int64_t ldT = 0;
+  float alpha = 1.f, beta = 1.f;
 };
 
 // Reduction RED over the columns [0, H) of every row, in column blocks of the widest row one launch takes (SG_REDS),
@@ -1818,6 +1877,7 @@ static int run_planned(roc_sg_plan* pl, int H, const void* in, int64_t ldIn, flo
     p.score = ed.w; p.out2 = ed.dw; p.dwAdd = (ed.accumulate || c0 > 0) ? 1 : 0;
     if (ed.g) { p.xrow = ed.g + c0; p.ldX = (size_t)ed.ldG; }
     if (ed.rowEnd) p.xrow = ed.rowEnd;
+    if (ed.t) { p.xrow = ed.t + c0; p.ldS = (size_t)ed.ldT; p.slope = ed.alpha; p.teleBeta = ed.beta; }
     p.H = (uint32_t)std::min(H - c0, blockCols);
     t_units(p, vec ? 4 : 1, std::min(H - c0, blockCols));
     rc = vec ? dispatch<4, RED>(p, st) : dispatch<1, RED>(p, st);
@@ -1847,6 +1907,19 @@ extern "C" int roc_sg_forward_planned_bf16(const roc_sg_plan* plc, int H, const 
   clear_launches();
   if (!pl || H <= 0 || !in || !out || ldIn < H || ldOut < H || (ldIn % 8) || !aligned16(in)) return ROC_ERR_INVALID;
   return run_planned<SG_RED_BSUM>(pl, H, in, ldIn, out, ldOut, nullptr, 0, epilogue, 0, as_stream(stream));
+}
+
+extern "C" int roc_sg_forward_teleport_planned(const roc_sg_plan* plc, int H, const float* in, int64_t ldIn,
+                                               float alpha, const float* t, int64_t ldT, float beta, float* out,
+                                               int64_t ldOut, int epilogue, roc_stream_t stream) {
+  roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  clear_launches();
+  if (!pl || H <= 0 || !in || !t || !out || out == t || ldIn < H || ldT < H || ldOut < H ||
+      (epilogue & ~(ROC_SG_EPI_NORM | ROC_SG_EPI_NORM_OUT)) || !std::isfinite(alpha) || !std::isfinite(beta))
+    return ROC_ERR_INVALID;
+  SgEdge ed;
+  ed.t = t; ed.ldT = ldT; ed.alpha = alpha; ed.beta = beta;
+  return run_planned<SG_RED_TELE>(pl, H, in, ldIn, out, ldOut, nullptr, 0, epilogue, 0, as_stream(stream), ed);
 }
 
 extern "C" int roc_sg_plan_rows_sorted(const roc_sg_plan* pl, int* sorted, roc_stream_t stream) {

@@ -84,6 +84,17 @@ class SgPlan:
                                               int(epilogue), _stream()), "roc_sg_forward_planned_bf16")
         return out
 
+    def teleport_forward(self, x, t, alpha, beta, epilogue=0, out=None):
+        """roc_sg_forward_teleport_planned: post(fmaf(alpha, pre(sum of x over each row's in-edges), beta * t)), pre /
+        post the divide by sqrt(in-degree) of SG_EPI_NORM / SG_EPI_NORM_OUT in `epilogue`.  t has one row per plan row,
+        any pitch."""
+        if out is None:
+            out = self._rows(x)
+        check(lib.roc_sg_forward_teleport_planned(self.handle, x.shape[1], _ptr(x), _ld(x), float(alpha), _ptr(t),
+                                                  _ld(t), float(beta), _ptr(out), _ld(out), int(epilogue), _stream()),
+              "roc_sg_forward_teleport_planned")
+        return out
+
     def rows_sorted(self):
         """True if every row's sources are strictly increasing (no duplicate edges)."""
         ok = C.c_int()
@@ -479,6 +490,22 @@ def add_fwd(a, b):
 def add_bwd(dy, da, acc_a, db, acc_b):
     check(lib.roc_add_bwd(dy.shape[0], dy.shape[1], _ptr(dy), _ld(dy), _ptr(da), _ld(da) if da is not None else 0,
                           int(acc_a), _ptr(db), _ld(db) if db is not None else 0, int(acc_b), _stream()))
+
+
+def scaled_add_fwd(a, b, alpha, beta, out=None):
+    """roc_scaled_add_fwd: fmaf(alpha, a, beta * b), beta * b rounded first."""
+    if out is None:
+        out = torch.empty_like(a) if a.is_contiguous() else padded(a.shape[0], a.shape[1], a.device)
+    check(lib.roc_scaled_add_fwd(a.shape[0], a.shape[1], float(alpha), _ptr(a), _ld(a), float(beta), _ptr(b), _ld(b),
+                                 _ptr(out), _ld(out), _stream()), "roc_scaled_add_fwd")
+    return out
+
+
+def scaled_add_bwd(dy, alpha, da, acc_a, beta, db, acc_b):
+    """roc_scaled_add_bwd: da (+)= alpha * dy, db (+)= beta * dy (accumulating with fmaf); da or db may be None."""
+    check(lib.roc_scaled_add_bwd(dy.shape[0], dy.shape[1], _ptr(dy), _ld(dy), float(alpha), _ptr(da),
+                                 _ld(da) if da is not None else 0, int(acc_a), float(beta), _ptr(db),
+                                 _ld(db) if db is not None else 0, int(acc_b), _stream()), "roc_scaled_add_bwd")
 
 
 def dropout_fwd(x, first_row, rate, seed, step, out=None):

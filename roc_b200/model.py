@@ -12,6 +12,7 @@ script in gnn.cc:65-111:
     m.train_mode(); m.zero_gradients(); m.forward(); m.backward(); m.update()
 """
 import ctypes as C
+import math
 
 import numpy as np
 
@@ -157,6 +158,15 @@ class Model:
 
     def add(self, a, b):
         return lib.roc_host_add(self.h, a, b)
+
+    def scaled_add(self, a, b, alpha, beta):
+        """fmaf(alpha, a, beta * b) with alpha and beta rounded to fp32 (Model::scaled_add), the initial residual of
+        APPNP and GCNII; a and b are different tensors of one shape.  A non-finite coefficient raises ValueError.  With
+        fusion on, init() folds it into the store of a sum scatter_gather whose indegree_norm feeds only it (as a)."""
+        for name, v in (("alpha", alpha), ("beta", beta)):
+            if not (math.isfinite(float(v)) and abs(float(v)) <= float(np.finfo(np.float32).max)):
+                raise ValueError("%s must be finite in fp32" % name)
+        return lib.roc_host_scaled_add(self.h, a, b, float(alpha), float(beta))
 
     def batch_norm(self, t, momentum=0.1, eps=1e-5):
         """torch.nn.BatchNorm1d over every local row: appends two parameters, gamma (ones) then beta (zeros), each of
@@ -665,3 +675,112 @@ def build_gcn_weighted(model, layers, dropout_rate, edge_weights, edge_grad=Fals
     model.set_tensor(e, np.asarray(edge_weights, dtype=np.float32))
     return {"input": x, "label": label, "mask": mask, "logits": t, "edges": e, "sg_ins": sg_ins, "sg_outs": sg_outs,
             "bns": bns}
+
+
+def _check_count(v, name):
+    if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < 1:
+        raise ValueError("%s must be an integer >= 1" % name)
+
+
+def _check_alpha(alpha):
+    if not (isinstance(alpha, (int, float, np.floating)) and 0.0 <= float(alpha) <= 1.0):
+        raise ValueError("alpha must be in [0, 1]")
+
+
+def fp32(x):
+    """x (computed in double) rounded once to fp32, as the builders pass their coefficients to scaled_add."""
+    return float(np.float32(x))
+
+
+def build_appnp(model, layers, dropout_rate, K=10, alpha=0.1, lr=0.01, weight_decay=0.05, exact_backward=False,
+                features="float32", loss="softmax"):
+    """APPNP (Klicpera et al., 2019), PyG's APPNP after an MLP:
+
+        h = MLP(x)                     # per layer: dropout -> linear -> relu, no relu on the last layer
+        z = h
+        z = scaled_add(indegree_norm(scatter_gather(indegree_norm(z))), h, 1 - alpha, alpha)     # K times
+        loss(z)
+
+    i.e. z' = (1 - alpha) D^-1/2 A D^-1/2 z + alpha h with the self loops already in A.  The coefficients are computed
+    in double and rounded to fp32 once (fp32()).  With fusion on, each hop's scaled_add is fused into its
+    scatter_gather's store, and so is the next hop's first indegree_norm (Model.init).  No edge dropout, one partition
+    for the fusion.  Bad K or alpha raises ValueError.  Returns the handles, with `h` (the MLP output), `hops` (each
+    hop's z) and `coefficients` (the fp32 pair (1 - alpha, alpha)).  With fusion on, a hop's z before the last is never
+    written (its scatter_gather stores the next hop's normalised z instead), so only the last, the logits, can be read
+    after a forward; set_fusion(False) writes every hop's z."""
+    _check_count(K, "K")
+    _check_alpha(alpha)
+    _check_rate(dropout_rate, "dropout_rate")
+    c = (fp32(1.0 - float(alpha)), fp32(float(alpha)))
+    L = len(layers)
+    x = _input_tensor(model, layers[0], features)
+    label = model.create_node_tensor(layers[-1])
+    mask = model.create_node_tensor(1, is_int=True)
+    t = x
+    for i in range(1, L):
+        t = model.linear(model.dropout(t, dropout_rate), layers[i], _lib.AC_MODE_NONE)
+        if i != L - 1:
+            t = model.relu(t)
+    h = z = t
+    hops = []
+    for _ in range(int(K)):
+        z = model.indegree_norm(model.scatter_gather(model.indegree_norm(z)))
+        z = model.scaled_add(z, h, c[0], c[1])
+        hops.append(z)
+    _loss(model, loss, z, label, mask)
+    model.adam(lr, weight_decay)
+    if exact_backward:
+        model.set_exact_backward(True)
+    model.init()
+    return {"input": x, "label": label, "mask": mask, "logits": z, "h": h, "hops": hops, "coefficients": c}
+
+
+def gcnii_beta(theta, layer):
+    """GCNII's identity-mapping strength of layer `layer` (1-based): log(theta / layer + 1), in double."""
+    return math.log(float(theta) / layer + 1.0)
+
+
+def build_gcnii(model, layers, dropout_rate, depth, alpha=0.1, theta=0.5, lr=0.01, weight_decay=0.05,
+                exact_backward=False, features="float32", loss="softmax"):
+    """GCNII (Chen et al., 2020), PyG's gcn2_cora example with shared weights; layers = [in, hidden, out]:
+
+        x0 = relu(linear(dropout(x), hidden))
+        h  = x0
+        for l in 1 .. depth:
+            p = scaled_add(indegree_norm(scatter_gather(indegree_norm(dropout(h)))), x0, 1 - alpha, alpha)
+            h = relu(scaled_add(p, linear(p, hidden), 1 - beta_l, beta_l))       # beta_l = log(theta / l + 1)
+        logits = linear(dropout(h), out)
+
+    The coefficients are computed in double and rounded to fp32 once (fp32(), gcnii_beta()).  With fusion on, each
+    hop's first scaled_add is fused into its scatter_gather's store.  One weight decay for every weight (PyG's example
+    uses two).  Bad layers, depth, alpha or theta raise ValueError.  Returns the handles, with `x0`, `hops` (each
+    layer's p), `relu_outs` (each layer's h) and `coefficients` (the fp32 (1 - alpha, alpha) and, per layer, the fp32
+    (1 - beta_l, beta_l))."""
+    if len(layers) != 3:
+        raise ValueError("layers must be [in, hidden, out]")
+    _check_count(depth, "depth")
+    _check_alpha(alpha)
+    if not (isinstance(theta, (int, float, np.floating)) and math.isfinite(float(theta)) and float(theta) > 0.0):
+        raise ValueError("theta must be finite and > 0")
+    _check_rate(dropout_rate, "dropout_rate")
+    ca = (fp32(1.0 - float(alpha)), fp32(float(alpha)))
+    cb = [(fp32(1.0 - gcnii_beta(theta, l)), fp32(gcnii_beta(theta, l))) for l in range(1, int(depth) + 1)]
+    x = _input_tensor(model, layers[0], features)
+    label = model.create_node_tensor(layers[-1])
+    mask = model.create_node_tensor(1, is_int=True)
+    x0 = h = model.relu(model.linear(model.dropout(x, dropout_rate), layers[1], _lib.AC_MODE_NONE))
+    hops, relu_outs = [], []
+    for l in range(int(depth)):
+        z = model.indegree_norm(model.scatter_gather(model.indegree_norm(model.dropout(h, dropout_rate))))
+        p = model.scaled_add(z, x0, ca[0], ca[1])
+        hops.append(p)
+        h = model.relu(model.scaled_add(p, model.linear(p, layers[1], _lib.AC_MODE_NONE), cb[l][0], cb[l][1]))
+        relu_outs.append(h)
+    t = model.linear(model.dropout(h, dropout_rate), layers[2], _lib.AC_MODE_NONE)
+    _loss(model, loss, t, label, mask)
+    model.adam(lr, weight_decay)
+    if exact_backward:
+        model.set_exact_backward(True)
+    model.init()
+    return {"input": x, "label": label, "mask": mask, "logits": t, "x0": x0, "hops": hops, "relu_outs": relu_outs,
+            "coefficients": {"alpha": ca, "beta": cb}}

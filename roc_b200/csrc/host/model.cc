@@ -577,11 +577,13 @@ static void fuse_batch_norm_relu(const std::vector<GnnOp*>& layers, Wiring& w) {
   }
 }
 
-// ---- fusion of  dropout -> linear  (gnn.cc:79-81, 86-88): the dropout output feeds only the linear
+// ---- fusion of  dropout -> linear  (gnn.cc:79-81, 86-88): the dropout output feeds only the linear.  Not when a
+//      scaled_add also reads the dropout's input: the Linear's dX epilogue overwrites that gradient, where the dropout
+//      alone adds its part to what the scaled_add wrote.
 static void fuse_dropout_into_linear(const std::vector<GnnOp*>& layers, Wiring& w) {
   for (size_t l = 0; l < layers.size(); l++) {
     Dropout* d = as<Dropout>(layers[l]);
-    if (!d || d->fusedInto >= 0) continue;
+    if (!d || d->fusedInto >= 0 || d->sharesWithScaledAdd) continue;
     const int ro = d->outputs[0].region;
     if (w.consumers[ro] != 1) continue;
     Linear* lin = as<Linear>(layers[w.consumerOp[ro]]);
@@ -595,7 +597,8 @@ static void fuse_dropout_into_linear(const std::vector<GnnOp*>& layers, Wiring& 
 static void fuse_backward_epilogues(RuntimeImpl* rt, const std::vector<GnnOp*>& layers, Wiring& w) {
   for (size_t l = 0; l < layers.size(); l++) {
     // (a) ... -> indegree_norm -> softmax_cross_entropy or sigmoid_cross_entropy: the loss kernel divides the
-    //     logits' gradient by sqrt(deg) and writes it where the norm's input gradient lives
+    //     logits' gradient by sqrt(deg) and writes it where the norm's input gradient lives (not when a scaled_add
+    //     also reads that input: the norm's own backward adds to it instead)
     int* lossGradOut = nullptr;
     if (SoftmaxCrossEntropy* sce = as<SoftmaxCrossEntropy>(layers[l])) lossGradOut = &sce->gradOut;
     else if (SigmoidCrossEntropy* bce = as<SigmoidCrossEntropy>(layers[l])) lossGradOut = &bce->gradOut;
@@ -603,7 +606,7 @@ static void fuse_backward_epilogues(RuntimeImpl* rt, const std::vector<GnnOp*>& 
       const int rz = layers[l]->inputs[0].region;
       if (!w.producer.count(rz) || w.consumers[rz] != 1) continue;
       InDegreeNorm* n = as<InDegreeNorm>(layers[w.producer[rz]]);
-      if (!n || n->bwdFused || n->reluOut >= 0) continue;
+      if (!n || n->bwdFused || n->reluOut >= 0 || n->sharesWithScaledAdd) continue;
       if (n->fusedInto >= 0 && as<Linear>(layers[(size_t)n->fusedInto])) continue;   // handled by the SG epilogue
       if (!rt->t(n->inputs[0].region).requiresGrad) continue;
       *lossGradOut = n->inputs[0].region;

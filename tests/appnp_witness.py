@@ -1,26 +1,16 @@
 """APPNP and GCNII (roc_b200.model.build_appnp / build_gcnii) as recorded op graphs, and a torch fp64 autograd
 interpreter of them: no code shared with the product.
 
-Rec is test_batchnorm_cpu.Rec (opgraph.Recorder with bf16 features and the sigmoid loss) plus scaled_add, whose node
-has attrs alpha / beta: the fp32 coefficients the product was given, as doubles.  witness() runs the ops the two
-builders use (linear, dropout, indegree_norm, scatter_gather, relu, scaled_add and the two losses) from edge lists."""
+The graphs are recorded by opgraph.Recorder; a scaled_add node has attrs alpha / beta, the fp32 coefficients the
+product was given, as doubles.  witness() runs the ops the two builders use (linear, dropout, indegree_norm,
+scatter_gather, relu, scaled_add and the two losses) from edge lists."""
 import numpy as np
 import torch
 
 from oracle import oracle
 from opgraph import _relu_with_mask
 from roc_b200 import _lib
-from test_batchnorm_cpu import Rec as BnRec
 from witness_gat import edge_lists, train_loss
-
-
-class Rec(BnRec):
-    def scaled_add(self, a, b, alpha, beta):
-        return self._node("scaled_add", [a, b], self._call("scaled_add", a, b, alpha, beta),
-                          alpha=float(np.float32(alpha)), beta=float(np.float32(beta)))
-
-    def set_bf16_aggregation(self, on=True):
-        self._call("set_bf16_aggregation", on)
 
 
 def bce_train_loss(x, labels, mask):

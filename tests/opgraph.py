@@ -1,27 +1,34 @@
 """An op-graph recorder over roc_b200.model.Model and an fp64 interpreter of what it recorded.
 
-Recorder(model) offers the Model's builder methods with the same signatures.  Each call goes to the product, and the
-recorder appends one IR node per layer the product creates (scatter_gather(t, AGGR_AVG) appends three: the sum and two
-norms), numbered by layer index as Model::layers is.  A node is a dict:
+Recorder(model) offers every builder method of the Model with the same signatures.  Each call goes to the product,
+and the recorder appends one IR node per layer the product creates (scatter_gather(t, AGGR_AVG) appends three: the sum
+and two norms), numbered by layer index as Model::layers is.  A node is a dict:
 
-    kind    "linear", "indegree_norm", "scatter_gather", "scatter_gather_max", "scatter_gather_min",
-            "scatter_gather_weighted", "attention_gather", "relu", "sigmoid", "add", "dropout" or
-            "softmax_cross_entropy" (roc_b200._lib.HOST_OPS)
+    kind    one of roc_b200._lib.HOST_OPS: "linear", "indegree_norm", "scatter_gather", "scatter_gather_max",
+            "scatter_gather_min", "scatter_gather_weighted", "attention_gather", "attention_scores", "relu", "elu",
+            "sigmoid", "add", "scaled_add", "dropout", "batch_norm", "softmax_cross_entropy" or "sigmoid_cross_entropy"
     ins     input tensor ids (tensor handles; the inner tensors of AGGR_AVG get ids of their own, from INNER on)
-    out     output tensor id (None for the loss)
+    out     output tensor id (None for a loss)
     layer   the layer index
-    attrs   out_dim, activation, param (linear); rate, seed, key (dropout); heads, slope (attention); edges (weighted)
+    attrs   out_dim, activation, param (linear); rate, seed, key (dropout); heads, slope, dropout, seed, key
+            (attention_gather); heads, param (attention_scores); edges (weighted); alpha, beta (scaled_add, the fp32
+            coefficients as doubles); gamma, beta (parameter indices), momentum, eps (batch_norm)
+
+A dropout's and an attention_gather's Philox key is (seed << 32) | layer, as Model::dropout computes it.  The
+recorder also keeps the bf16 leaves (create_node_tensor(dtype="bfloat16")) and whether set_bf16_aggregation is on.
 
 witness() runs the recorded graph in torch fp64 with autograd over edge lists (index_add): no code shared with the
 product.  The op semantics are the ones include/roc_b200.h and include/roc_gnn.h state."""
 import numpy as np
 import torch
 
+import attn_dropout_oracle as ado
 from oracle import oracle
 from roc_b200 import _lib
 from witness_gat import attend, edge_lists, train_loss
 
 INNER = 1 << 20      # ids of tensors the caller holds no handle for
+LOSSES = ("softmax_cross_entropy", "sigmoid_cross_entropy")
 
 
 class Recorder:
@@ -33,9 +40,11 @@ class Recorder:
         self.nodes = []
         self.width = {}           # tensor id -> hidden width
         self.leaves = []          # float node tensors the script created, in order
+        self.bf16 = set()         # the leaves held in bf16
         self.edges = []           # edge tensors
         self.edge_grad = {}       # edge tensor -> set_edge_grad's last value
         self.exact = False
+        self.bf16_aggregation = False
         self.params = 0
         self._inner = INNER
 
@@ -53,11 +62,15 @@ class Recorder:
         return out
 
     # ---- builders (roc_b200.model.Model)
-    def create_node_tensor(self, hidden, is_int=False):
-        t = self._call("create_node_tensor", hidden, is_int)
+    def create_node_tensor(self, hidden, is_int=False, dtype="float32"):
+        bf16 = dtype in ("bfloat16", "bf16")
+        t = self._call("create_node_tensor", hidden, is_int, dtype) if bf16 else \
+            self._call("create_node_tensor", hidden, is_int)
         self.width[t] = hidden
         if not is_int:
             self.leaves.append(t)
+        if bf16:
+            self.bf16.add(t)
         return t
 
     def create_edge_tensor(self, hidden=1):
@@ -74,11 +87,17 @@ class Recorder:
         self._call("set_exact_backward", on)
         self.exact = bool(on)
 
+    def set_bf16_aggregation(self, on=True):
+        self._call("set_bf16_aggregation", on)
+        self.bf16_aggregation = bool(on)
+
+    def _key(self, seed):
+        # Model::dropout / Model::attention_gather: opIndex = the layer index; the Philox key is (seed << 32) | opIndex
+        return ((seed & 0xFFFFFFFF) << 32) | len(self.nodes)
+
     def dropout(self, t, rate, seed=0):
-        layer = len(self.nodes)
-        # Model::dropout: opIndex = the layer index; the Philox key is (seed << 32) | opIndex
-        return self._node("dropout", [t], self._call("dropout", t, rate, seed), rate=float(rate), seed=seed,
-                          key=((seed & 0xFFFFFFFF) << 32) | layer)
+        key = self._key(seed)
+        return self._node("dropout", [t], self._call("dropout", t, rate, seed), rate=float(rate), seed=seed, key=key)
 
     def linear(self, t, out_dim, activation=_lib.AC_MODE_NONE):
         self.params += 1
@@ -102,12 +121,24 @@ class Recorder:
                 _lib.AGGR_MIN: "scatter_gather_min"}[aggr]
         return self._node(kind, [t], out, aggr=aggr)
 
-    def attention_gather(self, t, scores, heads=1, negative_slope=0.2):
-        return self._node("attention_gather", [t, scores], self._call("attention_gather", t, scores, heads, negative_slope),
-                          width=self.width[t], heads=int(heads), slope=float(np.float32(negative_slope)))
+    def attention_gather(self, t, scores, heads=1, negative_slope=0.2, dropout=0.0, seed=0):
+        key = self._key(seed)
+        # the rate-0 call takes the four arguments Model.attention_gather has always taken
+        args = (t, scores, heads, negative_slope) + ((dropout, seed) if dropout or seed else ())
+        return self._node("attention_gather", [t, scores], self._call("attention_gather", *args), width=self.width[t],
+                          heads=int(heads), slope=float(np.float32(negative_slope)), dropout=float(dropout),
+                          seed=seed, key=key)
+
+    def attention_scores(self, t, heads=1):
+        self.params += 1
+        return self._node("attention_scores", [t], self._call("attention_scores", t, heads), width=2 * int(heads),
+                          heads=int(heads), param=self.params - 1)
 
     def relu(self, t):
         return self._node("relu", [t], self._call("relu", t))
+
+    def elu(self, t):
+        return self._node("elu", [t], self._call("elu", t))
 
     def sigmoid(self, t):
         return self._node("sigmoid", [t], self._call("sigmoid", t))
@@ -115,9 +146,22 @@ class Recorder:
     def add(self, a, b):
         return self._node("add", [a, b], self._call("add", a, b))
 
+    def scaled_add(self, a, b, alpha, beta):
+        return self._node("scaled_add", [a, b], self._call("scaled_add", a, b, alpha, beta),
+                          alpha=float(np.float32(alpha)), beta=float(np.float32(beta)))
+
+    def batch_norm(self, t, momentum=0.1, eps=1e-5):
+        self.params += 2
+        return self._node("batch_norm", [t], self._call("batch_norm", t, momentum, eps), gamma=self.params - 2,
+                          beta=self.params - 1, momentum=float(momentum), eps=float(np.float32(eps)))
+
     def softmax_cross_entropy(self, logits, labels, mask):
         self._call("softmax_cross_entropy", logits, labels, mask)
         return self._node("softmax_cross_entropy", [logits, labels, mask], None)
+
+    def sigmoid_cross_entropy(self, logits, labels, mask):
+        self._call("sigmoid_cross_entropy", logits, labels, mask)
+        return self._node("sigmoid_cross_entropy", [logits, labels, mask], None)
 
     def init(self):
         if self.m is not None:
@@ -136,9 +180,17 @@ class Recorder:
 
     # ---- what the IR implies
     def loss_node(self):
-        losses = [n for n in self.nodes if n["kind"] == "softmax_cross_entropy"]
+        losses = [n for n in self.nodes if n["kind"] in LOSSES]
         assert len(losses) == 1, "one loss"
         return losses[0]
+
+
+def bce_train_loss(logits, labels, mask):
+    """The sigmoid loss in fp64: binary cross-entropy summed over the train rows and every class.
+    labels: [N][C] 0/1."""
+    train = torch.from_numpy(np.asarray(mask) == _lib.MASK_TRAIN)
+    y = torch.from_numpy(np.asarray(labels, dtype=np.float64))
+    return torch.nn.functional.binary_cross_entropy_with_logits(logits[train], y[train], reduction="sum")
 
 
 def _relu_with_mask(pre, product_mask, what):
@@ -178,30 +230,39 @@ def _extreme_sources(row_end, col, x, is_max, product_args, what):
     return out
 
 
-def witness(ir, graph, feats, labels, mask, weights, edge_values=None, step=1, relu_masks=None, aggr_args=None):
+def witness(ir, graph, feats, labels, mask, weights, edge_values=None, step=1, relu_masks=None, aggr_args=None,
+            training=True, run_stats=None, rounded=None):
     """The recorded graph (a Recorder) in torch fp64 with autograd, for one training step.
 
-    graph: (row_end, col).  feats: {leaf id: [N][H] array} (one array: the first leaf).  labels: [N] class indices.
-    mask: [N] MASK_*.  weights: W_mem[o][i] per parameter.  edge_values: {edge tensor: [E] weights}.  step: the
-    product's train-step counter during this step's forward (Model::forward increments it before the first op, so the
-    first step is 1).  relu_masks / aggr_args: {layer: the product's relu output > 0 / get_aggr_index}, taken where
-    fp32 and fp64 tie.
+    graph: (row_end, col).  feats: {leaf id: [N][H] array} (one array: the first leaf); a bf16 leaf is read as its
+    bf16 rounding.  labels: [N] class indices (softmax loss) or [N][C] 0/1 (sigmoid loss).  mask: [N] MASK_*.
+    weights: W_mem[o][i] per parameter (a batch_norm's gamma / beta as (1, H)).  edge_values: {edge tensor: [E]
+    weights}.  step: the product's train-step counter during this step's forward (Model::forward increments it before
+    the first op, so the first step is 1).  relu_masks / aggr_args: {layer: the product's relu output > 0 /
+    get_aggr_index}, taken where fp32 and fp64 tie.  rounded: {tensor: the product's values of a tensor it stores in
+    bf16 (set_bf16_aggregation)}, each checked to be a rounding of the fp64 value and taken in the forward with the
+    gradient passed straight through.
 
-    Returns dict(logits, dW (zeros for a Linear off the loss's path), edge_grad {edge tensor: dL/dw}, pre {layer: the
-    ReLU pre-activation})."""
+    training=False is the infer-mode model: dropout and attention dropout are copies, batch_norm uses
+    run_stats {bn output: (running mean, running variance)}, and nothing is differentiated.
+
+    Returns dict(logits, dW (zeros for a parameter off the loss's path), edge_grad {edge tensor: dL/dw}, pre {layer: the
+    ReLU pre-activation}, stats {bn output: its batch (mean, biased variance)})."""
     row_end, col = np.asarray(graph[0]), np.asarray(graph[1])
     n = row_end.shape[0]
     dst, src = edge_lists(row_end, col)
     deg = np.diff(np.concatenate([[0], row_end.astype(np.int64)]))
     dinv = torch.from_numpy(1.0 / np.sqrt(deg.astype(np.float64))).unsqueeze(1)
-    relu_masks, aggr_args = relu_masks or {}, aggr_args or {}
+    relu_masks, aggr_args, rounded = relu_masks or {}, aggr_args or {}, rounded or {}
     if not isinstance(feats, dict):
         feats = {ir.leaves[0]: feats}
-    ws = [torch.from_numpy(np.asarray(w, dtype=np.float64)).requires_grad_(True) for w in weights]
-    ew = {e: torch.from_numpy(np.asarray(v, dtype=np.float64)).requires_grad_(True)
+    ws = [torch.from_numpy(np.asarray(w, dtype=np.float64)).requires_grad_(training) for w in weights]
+    ew = {e: torch.from_numpy(np.asarray(v, dtype=np.float64)).requires_grad_(training)
           for e, v in (edge_values or {}).items()}
     val = {t: torch.from_numpy(np.asarray(a, dtype=np.float64)) for t, a in feats.items()}
-    pre, loss = {}, None
+    for t in ir.bf16 & set(val):                 # the fp32 rows as the product stores them: rounded to nearest even
+        val[t] = val[t].float().bfloat16().double()
+    pre, stats, loss, logits = {}, {}, None, None
     for node in ir.nodes:
         k, a, ins, what = node["kind"], node["attrs"], node["ins"], "layer %d (%s)" % (node["layer"], node["kind"])
         x = val[ins[0]] if ins[0] in val else None
@@ -221,31 +282,59 @@ def witness(ir, graph, feats, labels, mask, weights, edge_values=None, step=1, r
         elif k == "scatter_gather_weighted":
             y = torch.zeros((n, x.shape[1]), dtype=torch.float64).index_add(0, dst, ew[a["edges"]][:, None] * x[src])
         elif k == "attention_gather":
-            y = attend(x, val[ins[1]], dst, src, n, a["heads"], a["slope"])
+            drop = None
+            if training and a.get("dropout", 0.0) > 0:
+                drop = ado.multipliers(ado.edge_keep(row_end, col, a["dropout"], a["key"], step), a["heads"],
+                                       a["dropout"])
+            y = attend(x, val[ins[1]], dst, src, n, a["heads"], a["slope"], drop)
+        elif k == "attention_scores":
+            hd, w = a["heads"], ws[a["param"]]
+            xv = x.reshape(n, hd, -1)
+            y = torch.cat([(xv * w[:hd]).sum(2), (xv * w[hd:]).sum(2)], 1)
         elif k == "relu":
             pre[node["layer"]] = x.detach().numpy()
             y = _relu_with_mask(x, relu_masks.get(node["layer"]), what)
+        elif k == "elu":
+            y = torch.nn.functional.elu(x)
         elif k == "sigmoid":
             y = torch.sigmoid(x)
         elif k == "add":
             y = x + val[ins[1]]
+        elif k == "scaled_add":
+            y = a["alpha"] * x + a["beta"] * val[ins[1]]
+        elif k == "batch_norm":
+            gam, bet = ws[a["gamma"]][0], ws[a["beta"]][0]
+            if training:
+                mean = x.detach().mean(0)
+                stats[node["out"]] = (mean.numpy(), ((x.detach() - mean) ** 2).mean(0).numpy())
+                y = torch.nn.functional.batch_norm(x, None, None, gam, bet, training=True, eps=a["eps"])
+            else:
+                rm, rv = (torch.from_numpy(np.asarray(v, dtype=np.float64)) for v in run_stats[node["out"]])
+                y = torch.nn.functional.batch_norm(x, rm, rv, gam, bet, training=False, eps=a["eps"])
         elif k == "dropout":
-            if a["rate"] > 0:
+            if a["rate"] > 0 and training:
                 keep = oracle.dropout_mask(0, n, x.shape[1], a["rate"], a["key"], step)
                 scale = float(np.float32(1.0) / (np.float32(1.0) - np.float32(a["rate"])))
                 y = x * torch.from_numpy(keep.astype(np.float64) * scale)
             else:
                 y = x
-        elif k == "softmax_cross_entropy":
-            loss = train_loss(x, np.asarray(labels), np.asarray(mask))
+        elif k in LOSSES:
             logits = x
+            if training:
+                f = train_loss if k == "softmax_cross_entropy" else bce_train_loss
+                loss = f(x, np.asarray(labels), np.asarray(mask))
             continue
         else:
             raise AssertionError("unknown op " + k)
+        if node["out"] in rounded:
+            r, p = torch.from_numpy(np.asarray(rounded[node["out"]], dtype=np.float64)), y.detach()
+            assert ((r - p).abs() <= 2.0 ** -8 * 1.001 * p.abs() + 1e-5 * p.abs().max()).all(), \
+                "%s: the product's bf16 value is not a rounding of the fp64 one" % what
+            y = y + (r - p)
         val[node["out"]] = y
-    if loss.requires_grad:               # else no parameter reaches the loss
+    if loss is not None and loss.requires_grad:      # else no parameter reaches the loss
         loss.backward()
     return dict(logits=logits.detach().numpy(),
                 dW=[w.grad.numpy() if w.grad is not None else np.zeros(w.shape) for w in ws],
                 edge_grad={e: (t.grad.numpy() if t.grad is not None else np.zeros(t.shape)) for e, t in ew.items()},
-                pre=pre)
+                pre=pre, stats=stats)

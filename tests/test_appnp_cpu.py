@@ -11,7 +11,8 @@ import numpy as np
 import pytest
 import torch
 
-from appnp_witness import Rec, witness
+from appnp_witness import witness
+from opgraph import Recorder
 from roc_b200 import _lib
 from roc_b200.model import Model, build_appnp, build_gcnii, fp32, gcnii_beta
 
@@ -19,13 +20,13 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def appnp_ir(K=3, alpha=0.1, layers=(24, 16, 12), **kw):
-    ir = Rec(None)
+    ir = Recorder(None)
     h = build_appnp(ir, list(layers), 0.0, K=K, alpha=alpha, **kw)
     return ir, h
 
 
 def gcnii_ir(depth=4, alpha=0.1, theta=0.5, layers=(24, 16, 12), rate=0.0, **kw):
-    ir = Rec(None)
+    ir = Recorder(None)
     h = build_gcnii(ir, list(layers), rate, depth, alpha=alpha, theta=theta, **kw)
     return ir, h
 
@@ -82,16 +83,16 @@ def test_builders_keep_the_other_options():
     assert ir.nodes[-1]["kind"] == "sigmoid_cross_entropy"
     for build in (build_appnp, build_gcnii):
         with pytest.raises(TypeError):
-            build(Rec(None), [8, 4, 2], 0.0, 2, norm="batch")
+            build(Recorder(None), [8, 4, 2], 0.0, 2, norm="batch")
         with pytest.raises(TypeError):
-            build(Rec(None), [8, 4, 2], 0.0, 2, aggregation="bfloat16")
+            build(Recorder(None), [8, 4, 2], 0.0, 2, aggregation="bfloat16")
 
 
 @pytest.mark.parametrize("bad", [dict(K=0), dict(K=-3), dict(K=2.0), dict(K=True), dict(alpha=-0.01),
                                  dict(alpha=1.01), dict(alpha=float("nan")), dict(alpha="0.1")])
 def test_appnp_value_errors(bad):
     with pytest.raises(ValueError):
-        build_appnp(Rec(None), [8, 4], 0.0, **bad)
+        build_appnp(Recorder(None), [8, 4], 0.0, **bad)
 
 
 @pytest.mark.parametrize("bad", [dict(depth=0), dict(depth=1.5), dict(alpha=2.0), dict(theta=0.0), dict(theta=-1.0),
@@ -102,7 +103,7 @@ def test_gcnii_value_errors(bad):
     kw.update(bad)
     layers = kw.pop("layers", [8, 4, 2])
     with pytest.raises(ValueError):
-        build_gcnii(Rec(None), layers, 0.0, **kw)
+        build_gcnii(Recorder(None), layers, 0.0, **kw)
 
 
 def test_scaled_add_refuses_bad_coefficients_before_the_product():

@@ -5,10 +5,10 @@ the sigmoid loss.  bf16 aggregation picks no tensor in either model."""
 import numpy as np
 import pytest
 
-from appnp_witness import Rec, bce_train_loss, witness
+from appnp_witness import bce_train_loss, witness
+from opgraph import Recorder
 from roc_b200 import _lib, bf16, datasets
 from roc_b200.model import Host, Model, build_appnp, build_gcnii
-import test_opgraph_gpu as opgraph_cases
 from test_batchnorm_gpu import close, directed_graph, sym_graph
 from witness_gat import train_loss
 
@@ -47,7 +47,7 @@ def train(name, graph, fuse, steps=3, loss="softmax", bf16_aggregation=False, **
     m.set_fusion(fuse)
     if bf16_aggregation:
         m.set_bf16_aggregation(True)
-    ir = Rec(m)
+    ir = Recorder(m)
     h = MODELS[name](ir, loss=loss, **kw)
     if loss == "sigmoid":
         feats, labels, mask = (t.numpy() for t in datasets.multilabel_node_data(n, 24, 12, seed=5))
@@ -121,8 +121,6 @@ def test_model_matches_the_witness(name):
     check_witness(fused)
     check_identical(fused, unfused)
     check_fusion(name, fused, unfused)
-    # witness-checked at test_opgraph_gpu.py's bars: its coverage ledger counts scaled_add as reached
-    opgraph_cases.note_widths(fused["ir"])
 
 
 @pytest.mark.parametrize("name", list(BUILDERS))

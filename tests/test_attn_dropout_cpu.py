@@ -1,9 +1,7 @@
 """Attention dropout without a GPU: the numpy restatement of the keep mask (attn_dropout_oracle) pinned to the
 oracle's Philox on sampled pairs, its keep fraction, the fp64 attention oracle with a mask against torch autograd of
 the same masked function, build_gat(attn_dropout=)'s wiring on a recorder with no product behind it, and the refusals
-of a rate outside [0, 1).
-
-The recorder (DropRec) lives here so that tests/test_attn_dropout_gpu.py can import it."""
+of a rate outside [0, 1)."""
 import math
 
 import numpy as np
@@ -12,21 +10,9 @@ import torch
 
 import attn_dropout_oracle as ado
 import attn_oracle as ao
+from opgraph import Recorder
 from oracle import oracle
 from roc_b200.model import Model, build_gat
-from test_gat_heads_cpu import Rec
-
-
-class DropRec(Rec):
-    """test_gat_heads_cpu.Rec whose attention_gather also records the dropout rate, the seed and the Philox key
-    (seed << 32) | layer index."""
-
-    def attention_gather(self, t, scores, heads=1, negative_slope=0.2, dropout=0.0, seed=0):
-        layer = len(self.nodes)
-        args = (t, scores, heads, negative_slope) + ((dropout, seed) if dropout or seed else ())
-        return self._node("attention_gather", [t, scores], self._call("attention_gather", *args), width=self.width[t],
-                          heads=int(heads), slope=float(np.float32(negative_slope)), dropout=float(dropout),
-                          key=((seed & 0xFFFFFFFF) << 32) | layer)
 
 
 # ----------------------------------------------------------------------------------------------------- the mask ---
@@ -133,7 +119,7 @@ def test_oracle_with_a_mask_matches_autograd(heads, f):
 # --------------------------------------------------------------------------------------------- the Python API ---
 def test_build_gat_wiring_with_attn_dropout():
     layers = [24, 16, 32, 12]
-    plain, ir = DropRec(None), DropRec(None)
+    plain, ir = Recorder(None), Recorder(None)
     build_gat(plain, layers, 0.6, heads=[2, 8], scores="per_head", activation="elu")
     h = build_gat(ir, layers, 0.6, heads=[2, 8], scores="per_head", activation="elu", attn_dropout=0.6)
     gathers = [n for n in ir.nodes if n["kind"] == "attention_gather"]
@@ -151,7 +137,7 @@ def test_build_gat_defaults_call_attention_gather_as_before():
     only those builds the same model."""
     calls = []
 
-    class Plain(Rec):
+    class Plain(Recorder):
         def attention_gather(self, t, scores, heads=1, negative_slope=0.2):
             calls.append((heads, negative_slope))
             return super().attention_gather(t, scores, heads, negative_slope)
@@ -164,7 +150,7 @@ def test_build_gat_defaults_call_attention_gather_as_before():
 @pytest.mark.parametrize("rate", [-0.1, 1.0, 1.5, float("nan")])
 def test_rates_outside_the_unit_interval_are_refused(rate):
     with pytest.raises(ValueError):
-        build_gat(DropRec(None), [24, 16, 12], 0.5, heads=2, attn_dropout=rate)
+        build_gat(Recorder(None), [24, 16, 12], 0.5, heads=2, attn_dropout=rate)
     m = Model.__new__(Model)          # refused before the product is touched
     with pytest.raises(ValueError):
         m.attention_gather(0, 1, 2, 0.2, dropout=rate)

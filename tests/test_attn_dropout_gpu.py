@@ -20,13 +20,12 @@ import torch
 import attn_dropout_oracle as ado
 import attn_oracle as ao
 from conftest import ROOT
-from opgraph import _relu_with_mask
+from opgraph import Recorder, _relu_with_mask
 from roc_b200 import _lib, datasets
 from roc_b200 import kernels as K
 from roc_b200.model import Host, Model, build_gat
 from sg_matrix import (SLOPE, Guarded, close_terms, dev_in, exact, graphs, guarded, no_new_nan, same_bits,
                        valid_heads, wgraphs, xgraphs)
-from test_attn_dropout_cpu import DropRec
 from test_gat_heads_gpu import _bce_train_loss, close, directed_graph, sym_graph
 from witness_gat import edge_lists, train_loss
 
@@ -337,7 +336,7 @@ def train(graph, steps=3, fuse=True, infer=False, **kw):
     host.graph_from_arrays(row_end, col)
     m = Model(host, seed=1)
     m.set_fusion(fuse)
-    ir = DropRec(m)
+    ir = Recorder(m)
     h = build_gat(ir, LAYERS, 0.5, heads=HEADS, **kw)
     feats, labels, mask = (t.numpy() for t in datasets.node_data(n, LAYERS[0], LAYERS[-1], seed=5))
     m.set_labels(h["label"], labels)

@@ -2,35 +2,13 @@
 the refusal of an unknown norm, and the fp64 reference the GPU tests check against (bn_forward / bn_backward) against
 torch.nn.functional.batch_norm's forward and autograd in fp64.
 
-The recorder (Rec) and the reference live here so that tests/test_batchnorm_gpu.py can import them."""
+The reference lives here so that tests/test_batchnorm_gpu.py can import it."""
 import numpy as np
 import pytest
 import torch
 
 from opgraph import Recorder
 from roc_b200.model import build_gat, build_gcn, build_gcn_weighted, build_sage_mean, build_sage_pool
-
-
-class Rec(Recorder):
-    """opgraph.Recorder with the builders' bf16 feature tensors, the sigmoid loss and batch_norm: a batch_norm node has
-    attrs gamma / beta (parameter indices, gamma first), momentum and eps."""
-
-    def create_node_tensor(self, hidden, is_int=False, dtype="float32"):
-        if dtype == "float32":
-            return super().create_node_tensor(hidden, is_int)
-        t = self._call("create_node_tensor", hidden, False, dtype)
-        self.width[t] = hidden
-        self.leaves.append(t)
-        return t
-
-    def sigmoid_cross_entropy(self, logits, labels, mask):
-        self._call("sigmoid_cross_entropy", logits, labels, mask)
-        return self._node("sigmoid_cross_entropy", [logits, labels, mask], None)
-
-    def batch_norm(self, t, momentum=0.1, eps=1e-5):
-        self.params += 2
-        return self._node("batch_norm", [t], self._call("batch_norm", t, momentum, eps), gamma=self.params - 2,
-                          beta=self.params - 1, momentum=float(momentum), eps=float(np.float32(eps)))
 
 
 # ---------------------------------------------------------------------------------------- the fp64 reference ---
@@ -133,7 +111,7 @@ def _consumers(ir, t):
 
 @pytest.mark.parametrize("name", list(BUILDERS))
 def test_builder_puts_batch_norm_before_every_hidden_relu(name):
-    plain, ir = Rec(None), Rec(None)
+    plain, ir = Recorder(None), Recorder(None)
     BUILDERS[name](plain)
     h = BUILDERS[name](ir, norm="batch")
     bns = [n for n in ir.nodes if n["kind"] == "batch_norm"]
@@ -166,4 +144,4 @@ def test_builder_puts_batch_norm_before_every_hidden_relu(name):
 @pytest.mark.parametrize("bad", ["layer", "Batch", "", 1])
 def test_builder_refuses_an_unknown_norm(name, bad):
     with pytest.raises(ValueError):
-        BUILDERS[name](Rec(None), norm=bad)
+        BUILDERS[name](Recorder(None), norm=bad)

@@ -13,12 +13,11 @@ import torch
 
 from conftest import ROOT
 from oracle import oracle
-from opgraph import _extreme_sources, _relu_with_mask
+from opgraph import Recorder, _extreme_sources, _relu_with_mask
 from roc_b200 import _lib, datasets
 from roc_b200 import kernels as K
 from roc_b200.model import Host, Model
-import test_opgraph_gpu as opgraph_cases
-from test_batchnorm_cpu import BUILDERS, Rec, bn_backward, bn_forward
+from test_batchnorm_cpu import BUILDERS, bn_backward, bn_forward
 from witness_gat import attend, edge_lists, train_loss
 
 pytestmark = pytest.mark.gpu
@@ -256,7 +255,7 @@ def train(name, graph, fuse, steps=3, norm="batch", loss="softmax", **kw):
     host.graph_from_arrays(row_end, col)
     m = Model(host, seed=1)
     m.set_fusion(fuse)
-    ir = Rec(m)
+    ir = Recorder(m)
     ir.edge_w = np.random.RandomState(2).uniform(0.05, 0.6, size=col.shape[0]).astype(np.float32)
     if name == "gcn_weighted":
         kw = dict(kw, edge_weights=ir.edge_w)
@@ -357,9 +356,6 @@ def test_builder_with_batch_norm_matches_the_witness(name):
     check_witness(fused)
     check_identical(fused, unfused)
     check_fusion(fused, unfused)
-    # these graphs are witness-checked at test_opgraph_gpu.py's bars: its coverage ledger counts their op kinds
-    # (batch_norm among them) as reached
-    opgraph_cases.note_widths(fused["ir"])
     assert [i["kind"] for i in fused["info"]] == [nd["kind"] for nd in fused["ir"].nodes]
     # BN draws no random numbers: the Linears start where they start without it
     plain = train(name, g, True, steps=1, norm=None)

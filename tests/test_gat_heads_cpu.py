@@ -2,7 +2,7 @@
 scores_bwd_ref, elu_ref / elu_bwd_ref) against torch; build_gat's wiring for every scores x activation on a recorder
 with no product behind it; the refusal of unknown values; and a register / spill check of every new kernel.
 
-The recorder (Rec) and the references live here so that tests/test_gat_heads_gpu.py can import them."""
+The references live here so that tests/test_gat_heads_gpu.py can import them."""
 import os
 import re
 import shutil
@@ -12,20 +12,8 @@ import pytest
 import torch
 
 from conftest import ROOT
+from opgraph import Recorder
 from roc_b200.model import build_gat
-from test_batchnorm_cpu import Rec as BnRec
-
-
-class Rec(BnRec):
-    """test_batchnorm_cpu.Rec with attention_scores (attrs heads, param: the index of its A) and elu."""
-
-    def attention_scores(self, t, heads=1):
-        self.params += 1
-        return self._node("attention_scores", [t], self._call("attention_scores", t, heads), width=2 * int(heads),
-                          heads=int(heads), param=self.params - 1)
-
-    def elu(self, t):
-        return self._node("elu", [t], self._call("elu", t))
 
 
 # ---------------------------------------------------------------------------------------- the fp64 references ---
@@ -105,7 +93,7 @@ def test_elu_reference_matches_torch():
 @pytest.mark.parametrize("heads", [1, 4, [2, 8]])
 def test_build_gat_wiring(scores, activation, heads):
     layers = [24, 16, 32, 12] if isinstance(heads, list) else [24, 16, 12]
-    plain, ir = Rec(None), Rec(None)
+    plain, ir = Recorder(None), Recorder(None)
     build_gat(plain, layers, 0.5, heads=heads)
     h = build_gat(ir, layers, 0.5, heads=heads, scores=scores, activation=activation)
     hs = (heads if isinstance(heads, list) else [heads] * (len(layers) - 2)) + [1]
@@ -136,7 +124,7 @@ def test_build_gat_wiring(scores, activation, heads):
 
 
 def test_build_gat_with_batch_norm_puts_it_before_the_elu():
-    ir = Rec(None)
+    ir = Recorder(None)
     h = build_gat(ir, [24, 16, 12], 0.5, heads=2, scores="per_head", activation="elu", norm="batch")
     producer = {n["out"]: n for n in ir.nodes}
     (e,) = [n for n in ir.nodes if n["kind"] == "elu"]
@@ -147,7 +135,7 @@ def test_build_gat_with_batch_norm_puts_it_before_the_elu():
                                 dict(activation="gelu"), dict(activation=None)])
 def test_build_gat_refuses_unknown_values(kw):
     with pytest.raises(ValueError):
-        build_gat(Rec(None), [24, 16, 12], 0.5, heads=2, **kw)
+        build_gat(Recorder(None), [24, 16, 12], 0.5, heads=2, **kw)
 
 
 # -------------------------------------------------------------------------------------------------- the kernels ---

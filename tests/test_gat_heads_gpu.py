@@ -26,13 +26,12 @@ import pytest
 import torch
 
 from conftest import ROOT
-from opgraph import _relu_with_mask
+from opgraph import Recorder, _relu_with_mask
 from oracle import oracle
 from roc_b200 import _lib, datasets
 from roc_b200 import kernels as K
 from roc_b200.model import Host, Model, build_gat
-import test_opgraph_gpu as opgraph_cases
-from test_gat_heads_cpu import Rec, elu_bwd_ref, elu_ref, scores_bwd_ref, scores_ref
+from test_gat_heads_cpu import elu_bwd_ref, elu_ref, scores_bwd_ref, scores_ref
 from witness_gat import attend, edge_lists, train_loss
 
 pytestmark = pytest.mark.gpu
@@ -316,7 +315,7 @@ def train(config, graph, fuse, steps=3, loss="softmax", **kw):
     host.graph_from_arrays(row_end, col)
     m = Model(host, seed=1)
     m.set_fusion(fuse)
-    ir = Rec(m)
+    ir = Recorder(m)
     h = build_gat(ir, layers, 0.5, heads=heads, loss=loss, **kw)
     if loss == "sigmoid":
         feats, labels, mask = (t.numpy() for t in datasets.multilabel_node_data(n, layers[0], layers[-1], seed=5))
@@ -388,8 +387,6 @@ def test_paper_gat_matches_the_witness(config):
     fused, unfused = train(config, g, True, **PAPER), train(config, g, False, **PAPER)
     check_witness(fused)
     check_identical(fused, unfused)
-    # witness-checked at test_opgraph_gpu.py's bars: its coverage ledger counts these op kinds as reached
-    opgraph_cases.note_widths(fused["ir"])
     # the ELU is never fused, and each A has the shape (2 * heads, F)
     ir = fused["ir"]
     for nd in ir.nodes:
@@ -404,7 +401,6 @@ def test_paper_gat_matches_the_witness(config):
 def test_each_option_alone_matches_the_witness(kw):
     run = train("heads4", sym_graph(), True, **kw)
     check_witness(run)
-    opgraph_cases.note_widths(run["ir"])
 
 
 def test_per_head_scores_equal_the_dense_linear_at_one_head():
@@ -456,7 +452,6 @@ def test_paper_gat_with_batch_norm():
     fused, unfused = train("heads2_8", g, True, norm="batch", **PAPER), train("heads2_8", g, False, norm="batch", **PAPER)
     check_witness(fused)
     check_identical(fused, unfused)
-    opgraph_cases.note_widths(fused["ir"])
 
 
 REFUSALS = {

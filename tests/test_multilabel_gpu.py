@@ -1,14 +1,12 @@
 """The multi-label sigmoid cross-entropy on the GPU: roc_sigmoid_xent_bwd against the fp64 oracle of
 tests/multilabel_oracle.py over a matrix of widths, row counts, pitches, masks and logits; the fused norm variant
 against the plain call followed by roc_indegree_norm, bit for bit; the five model builders with loss="sigmoid" over
-three Adam steps against the fp64 autograd interpreter of tests/opgraph.py (its loss node read as the sigmoid loss),
-fused and unfused; the head with the other
+three Adam steps against the fp64 autograd interpreter of tests/opgraph.py, fused and unfused; the head with the other
 model options; inference metrics; a learning sanity check; and the refusals."""
 import ctypes as C
 import os
 import subprocess
 import sys
-import types
 
 import numpy as np
 import pytest
@@ -16,9 +14,7 @@ import torch
 
 from conftest import ROOT
 from multilabel_oracle import micro_f1, sigmoid_xent
-import opgraph
-import test_opgraph_gpu as opgraph_cases
-from opgraph import Recorder
+from opgraph import Recorder, witness
 from roc_b200 import _lib, datasets
 from roc_b200 import kernels as K
 from roc_b200.model import (Host, Model, build_gat, build_gcn, build_gcn_weighted, build_sage_mean, build_sage_pool,
@@ -146,44 +142,6 @@ def test_kernel_at_production_rows():
 
 
 # ------------------------------------------------------------------------------------------------- the models ---
-class Rec(Recorder):
-    """Recorder that also takes the builders' bf16 feature tensors (the witness reads them widened)."""
-
-    def create_node_tensor(self, hidden, is_int=False, dtype="float32"):
-        if dtype == "float32":
-            return super().create_node_tensor(hidden, is_int)
-        t = self.m.create_node_tensor(hidden, dtype=dtype)
-        self.width[t] = hidden
-        self.leaves.append(t)
-        return t
-
-    def sigmoid_cross_entropy(self, logits, labels, mask):
-        self._call("sigmoid_cross_entropy", logits, labels, mask)
-        return self._node("sigmoid_cross_entropy", [logits, labels, mask], None)
-
-
-def _bce_train_loss(x, labels, mask):
-    """The sigmoid head's loss in fp64: the sum of binary_cross_entropy_with_logits over the train rows and all
-    classes, whose gradient is the product's sigmoid(z) - y on those rows (no averaging).  labels: [N][C] 0/1."""
-    train = torch.from_numpy(np.asarray(mask) == _lib.MASK_TRAIN)
-    y = torch.from_numpy(np.asarray(labels, dtype=np.float64))
-    return torch.nn.functional.binary_cross_entropy_with_logits(x[train], y[train], reduction="sum")
-
-
-def sigmoid_witness(ir, *args, **kw):
-    """opgraph.witness for a graph that ends in the sigmoid loss.  witness interprets its one loss node through the
-    module's train_loss; here the node is shown to it under the loss kind it knows, and train_loss is _bce_train_loss
-    for the duration of the call.  Every other node is interpreted as for any op graph."""
-    nodes = [dict(n, kind="softmax_cross_entropy") if n["kind"] == "sigmoid_cross_entropy" else n for n in ir.nodes]
-    shadow = types.SimpleNamespace(nodes=nodes, leaves=ir.leaves)
-    saved = opgraph.train_loss
-    opgraph.train_loss = _bce_train_loss
-    try:
-        return opgraph.witness(shadow, *args, **kw)
-    finally:
-        opgraph.train_loss = saved
-
-
 def sym_graph():
     re_, col = datasets.rmat_graph(9, 2500, seed=3)
     return re_.numpy().astype(np.uint64), col.numpy().astype(np.uint32)
@@ -212,7 +170,7 @@ def train(name, graph, fuse, steps=3, **kw):
     host.graph_from_arrays(row_end, col)
     m = Model(host, seed=1)
     m.set_fusion(fuse)
-    ir = Rec(m)
+    ir = Recorder(m)
     ir.edge_w = np.random.RandomState(2).uniform(0.05, 0.6, size=col.shape[0]).astype(np.float32)
     h = BUILDERS[name](ir, **kw)
     feats, labels, mask = datasets.multilabel_node_data(n, 24, 12, seed=5)
@@ -256,7 +214,7 @@ def check_witness(run, feats=None):
     ir = run["ir"]
     edges = {e: ir.edge_w for e in ir.edges}
     for k, st in enumerate(run["steps"]):
-        wt = sigmoid_witness(ir, run["graph"], run["feats"] if feats is None else feats, run["labels"], run["mask"],
+        wt = witness(ir, run["graph"], run["feats"] if feats is None else feats, run["labels"], run["mask"],
                              st["w0"], edge_values=edges, step=k + 1, relu_masks=st["relu"], aggr_args=st["args"])
         close("step %d logits" % k, st["logits"], wt["logits"])
         for p, (a, b) in enumerate(zip(st["dw"], wt["dW"])):
@@ -300,9 +258,6 @@ def test_builder_with_sigmoid_loss_matches_the_witness(name):
     check_schedules_identical(fused, unfused)
     check_infer(fused)
     ir = fused["ir"]
-    # these graphs are witness-checked at test_opgraph_gpu.py's bars: its coverage ledger counts their op kinds
-    # (the sigmoid loss among them) as reached
-    opgraph_cases.note_widths(ir)
     assert ir.nodes[-1]["kind"] == "sigmoid_cross_entropy"
     assert [i["kind"] for i in unfused["info"]][-1] == "sigmoid_cross_entropy"
     if name == "gcn":

@@ -3,12 +3,21 @@ against the fp32 oracle's GCN with dropout.  The IR comes from the model builder
 Recorder with no product behind it, so it also pins the recorder's layer numbering (the dropout keys)."""
 import numpy as np
 import pytest
+import torch
 
+import appnp_witness
+import attn_dropout_oracle as ado
 from conftest import rel_close
 from oracle import oracle
 from opgraph import Recorder, witness
 from roc_b200 import _lib, datasets
-from roc_b200.model import build_gat, build_gcn, build_gcn_weighted, build_sage_mean, build_sage_pool
+from roc_b200.model import (build_appnp, build_gat, build_gcn, build_gcn_weighted, build_gcnii, build_sage_mean,
+                            build_sage_pool)
+from test_attn_dropout_cpu import _sym_graph
+from test_attn_dropout_gpu import witness as attn_dropout_witness
+from test_batchnorm_cpu import BUILDERS as BN_BUILDERS
+from test_batchnorm_gpu import _bce_train_loss, bn_witness
+from test_gat_heads_gpu import witness as gat_heads_witness
 from witness import torch_witness
 from witness_exact import gcn_sage_witness
 from witness_gat import gat_witness
@@ -174,3 +183,150 @@ def test_gcn_with_dropout_matches_the_oracle(layers):
     a = witness(ir, (row_end, col), feats, labels, mask, ws, step=1)["logits"]
     b = witness(ir, (row_end, col), feats, labels, mask, ws, step=2)["logits"]
     assert np.abs(a - b).max() > 1e-3
+
+
+# --------------------------------------------- the ops added since: each feature's own reference, on its builders ---
+def draw(ir, seed=4):
+    """A value for every parameter, in the shapes the product gives them: a Linear's W (out, in), an
+    attention_scores' A (2 * heads, F), a batch_norm's gamma and beta (1, H) (gamma near 1)."""
+    rng = np.random.RandomState(seed)
+    ws = [None] * ir.params
+    for nd in ir.nodes:
+        a = nd["attrs"]
+        if nd["kind"] == "linear":
+            i, o = ir.width[nd["ins"][0]], a["out_dim"]
+            s = np.sqrt(6.0 / (i + o))
+            ws[a["param"]] = rng.uniform(-s, s, size=(o, i))
+        elif nd["kind"] == "attention_scores":
+            hd = a["heads"]
+            ws[a["param"]] = rng.uniform(-0.5, 0.5, size=(2 * hd, ir.width[nd["ins"][0]] // hd))
+        elif nd["kind"] == "batch_norm":
+            h = ir.width[nd["out"]]
+            ws[a["gamma"]] = rng.uniform(0.5, 1.5, size=(1, h))
+            ws[a["beta"]] = rng.uniform(-0.3, 0.3, size=(1, h))
+    return [w.astype(np.float32) for w in ws]
+
+
+def bn_case(name, loss="softmax", features="float32"):
+    """A builder of test_batchnorm_cpu.BUILDERS with norm="batch" on a recorder, and inputs for it (12 classes)."""
+    n = 120
+    re_t, col_t = datasets.uniform_graph(n, 400, seed=2)
+    row_end, col = re_t.numpy().astype(np.uint64), col_t.numpy().astype(np.uint32)
+    data = datasets.multilabel_node_data if loss == "sigmoid" else datasets.node_data
+    feats, labels, mask = (t.numpy() for t in data(n, 24, 12, seed=2))
+    w = np.random.RandomState(1).uniform(0.05, 0.6, size=col.shape[0]).astype(np.float32)
+    ir = Recorder()
+    kw = dict(edge_weights=w) if name == "gcn_weighted" else {}
+    h = BN_BUILDERS[name](ir, norm="batch", loss=loss, features=features, **kw)
+    return ir, h, (row_end, col), feats, labels, mask, {e: w for e in ir.edges}
+
+
+@pytest.mark.parametrize("name", ["gcn", "gcn4", "sage_mean", "sage_pool", "gat", "gcn_weighted"])
+def test_batch_norm_matches_bn_witness(name):
+    """Train (batch statistics, dropout at step 2) and infer (running statistics, dropout a copy)."""
+    ir, h, graph, feats, labels, mask, ev = bn_case(name)
+    ws = draw(ir)
+    got = witness(ir, graph, feats, labels, mask, ws, edge_values=ev, step=2)
+    want = bn_witness(ir, graph, feats, labels, mask, ws, None, edge_values=ev, step=2)
+    check(ir, got, want["logits"], want["dW"], what="bn_witness")
+    assert sorted(got["stats"]) == sorted(h["bns"]) == sorted(want["stats"])
+    for t, (mean, var) in want["stats"].items():
+        close12(got["stats"][t][0], mean.numpy(), "batch mean")
+        close12(got["stats"][t][1], var.numpy(), "batch var")
+    rng = np.random.RandomState(3)
+    run = {t: (rng.uniform(-1, 1, ir.width[t]), rng.uniform(0.5, 2, ir.width[t])) for t in h["bns"]}
+    got = witness(ir, graph, feats, labels, mask, ws, edge_values=ev, training=False, run_stats=run)
+    want = bn_witness(ir, graph, feats, labels, mask, ws, run, training=False, edge_values=ev)
+    close12(got["logits"], want["logits"], "infer logits")
+    assert not any(np.any(d) for d in got["dW"]), "infer mode differentiates nothing"
+
+
+def test_sigmoid_loss_and_bf16_features_match_bn_witness():
+    ir, h, graph, feats, labels, mask, ev = bn_case("gcn", loss="sigmoid", features="bfloat16")
+    assert ir.loss_node()["kind"] == "sigmoid_cross_entropy" and ir.bf16 == {h["input"]}
+    ws = draw(ir)
+    got = witness(ir, graph, feats, labels, mask, ws, step=1)
+    rounded = torch.from_numpy(feats).bfloat16().double().numpy()
+    assert np.abs(rounded - feats).max() > 0                       # the rounding is visible
+    want = bn_witness(ir, graph, rounded, labels, mask, ws, None, loss_fn=_bce_train_loss)
+    check(ir, got, want["logits"], want["dW"], what="bn_witness, sigmoid loss")
+
+
+@pytest.mark.parametrize("name", ["appnp", "gcnii"])
+def test_appnp_and_gcnii_match_appnp_witness(name):
+    row_end, col, feats, labels, mask = case((24, 16, 12))
+    ir = Recorder()
+    if name == "appnp":
+        build_appnp(ir, [24, 16, 12], 0.5, K=4, alpha=0.1)
+    else:
+        build_gcnii(ir, [24, 16, 12], 0.5, 3, alpha=0.1, theta=0.5)
+    assert any(nd["kind"] == "scaled_add" for nd in ir.nodes)
+    ws = draw(ir)
+    for step in (1, 3):
+        got = witness(ir, (row_end, col), feats, labels, mask, ws, step=step)
+        want = appnp_witness.witness(ir, (row_end, col), feats, labels, mask, ws, step=step)
+        check(ir, got, want["logits"], want["dW"], what="appnp_witness step %d" % step)
+    got = witness(ir, (row_end, col), feats, labels, mask, ws, training=False)
+    want = appnp_witness.witness(ir, (row_end, col), feats, labels, mask, ws, training=False)
+    close12(got["logits"], want["logits"], "infer logits")
+
+
+@pytest.mark.parametrize("norm", [None, "batch"])
+def test_paper_gat_matches_the_gat_heads_witness(norm):
+    """Per-head attention_scores, ELU, dropout 0.5 (and a batch_norm before each ELU)."""
+    row_end, col, feats, labels, mask = case((24, 16, 32, 12))
+    ir = Recorder()
+    build_gat(ir, [24, 16, 32, 12], 0.5, heads=[2, 8], scores="per_head", activation="elu", norm=norm)
+    assert {"attention_scores", "elu"} <= {nd["kind"] for nd in ir.nodes}
+    ws = draw(ir)
+    got = witness(ir, (row_end, col), feats, labels, mask, ws, step=2)
+    logits, dw = gat_heads_witness(ir, (row_end, col), feats, labels, mask, ws, step=2)
+    check(ir, got, logits, dw, what="test_gat_heads_gpu.witness")
+
+
+def test_paper_gat_with_attention_dropout_matches_its_witness():
+    row_end, col, feats, labels, mask = case((24, 16, 32, 12))
+    ir = Recorder()
+    build_gat(ir, [24, 16, 32, 12], 0.5, heads=[2, 8], scores="per_head", activation="elu", attn_dropout=0.6)
+    ws = draw(ir)
+    for step in (1, 2):
+        got = witness(ir, (row_end, col), feats, labels, mask, ws, step=step)
+        logits, dw = attn_dropout_witness(ir, (row_end, col), feats, labels, mask, ws, step, None)
+        check(ir, got, logits, dw, what="test_attn_dropout_gpu.witness step %d" % step)
+    # infer mode: no attention dropout, no dropout
+    plain = Recorder()
+    build_gat(plain, [24, 16, 32, 12], 0.0, heads=[2, 8], scores="per_head", activation="elu")
+    a = witness(ir, (row_end, col), feats, labels, mask, ws, training=False)["logits"]
+    close12(a, witness(plain, (row_end, col), feats, labels, mask, ws)["logits"], "infer = the undropped model")
+
+
+@pytest.mark.parametrize("heads,f", [(1, 5), (2, 4), (8, 4)])
+def test_attention_dropout_matches_attn_dropout_oracle(heads, f):
+    """attention_gather(wh, sc, dropout=0.6, seed=5) read straight into the loss: its forward is
+    attn_dropout_oracle.forward with the step's key (seed << 32) | layer, and the gradients its two Linears see
+    are attn_dropout_oracle.backward's."""
+    n, rate, step = 60, 0.6, 3
+    row_end, col = _sym_graph(n, 150, heads)
+    ir = Recorder()
+    x0 = ir.create_node_tensor(7)
+    wh, sc = ir.linear(x0, heads * f), ir.linear(x0, 2 * heads)
+    out = ir.attention_gather(wh, sc, heads=heads, dropout=rate, seed=5)
+    ir.softmax_cross_entropy(out, ir.create_node_tensor(heads * f), ir.create_node_tensor(1, is_int=True))
+    assert ir.nodes[2]["attrs"]["key"] == (5 << 32) | 2
+    rng = np.random.RandomState(heads)
+    x = rng.uniform(-1, 1, size=(n, 7))
+    ws = [rng.uniform(-1, 1, size=(heads * f, 7)), rng.uniform(-1, 1, size=(2 * heads, 7))]
+    labels, mask = rng.randint(0, heads * f, size=n), rng.randint(0, 3, size=n)
+    got = witness(ir, (row_end, col), x, labels, mask, ws, step=step)
+    key = (5 << 32) | 2
+    m1 = ado.multipliers(ado.edge_keep(row_end, col, rate, key, step), heads, rate)
+    m2 = ado.multipliers(ado.edge_keep(row_end, col, rate, key, step, row_is_source=True), heads, rate)
+    xw, s, slope = x @ ws[0].T, x @ ws[1].T, float(np.float32(0.2))
+    o, stats = ado.forward(row_end, col, xw, s, heads, slope, m1)
+    close12(got["logits"], o, "forward")
+    p = np.exp(o - o.max(1, keepdims=True))
+    p /= p.sum(1, keepdims=True)
+    gy = np.where((mask == _lib.MASK_TRAIN)[:, None], p - np.eye(heads * f)[labels], 0.0)
+    ig, sg = ado.backward(row_end, col, xw, s, o, stats, gy, heads, slope, m1, m2)
+    np.testing.assert_allclose(got["dW"][0], ig.T @ x, rtol=1e-10, atol=1e-12)
+    np.testing.assert_allclose(got["dW"][1], sg.T @ x, rtol=1e-10, atol=1e-12)

@@ -1,16 +1,24 @@
 """Model op graphs, fused and unfused, against the fp64 interpreter of tests/opgraph.py over three Adam steps.
 
 Model::init decides which tensors need a gradient, who overwrites a gradient and who adds to it (resetInputGrads,
-set in reverse layer order by Model::backward), and five peephole fusions that reroute where a gradient is written
-and switch other ops' forward or backward off.  This file builds op graphs through a Recorder and checks, per case:
+set in reverse layer order by Model::backward), and the peephole fusions that reroute where a gradient is written
+and switch other ops' forward or backward off (the GCN block, batch_norm -> relu, dropout -> linear, the backward
+epilogues, the teleport of a scaled_add into a sum scatter_gather).  This file builds op graphs over every op kind
+through a Recorder and checks, per case:
 
 - the fusion report (Model.op_info) of both schedules: the hand-listed cases state it exactly, the unfused schedule
   has none;
 - against the witness at each step's weights: the logits at the parity bar, every dW and every edge gradient at
   rtol 2e-4 with atol_scale 2e-5 (the bars of test_exact_model_gpu.py);
-- between the schedules, bit for bit: logits, dW, edge gradients and the weights after each update;
-- after training, an infer-mode forward: equal metrics in both schedules (except trainLoss, an atomic sum), and the
-  *All counts equal to the mask's counts.
+- the batch_norm running statistics after training against the fp64 recurrence over the witness's batch statistics
+  (from 0 / 1, var scaled by N / (N - 1)), at the dW bars;
+- after training, an infer-mode forward: its logits against witness(training=False) at the final weights and running
+  statistics, at the parity bar; equal metrics in both schedules (except trainLoss, an atomic sum), and the *All
+  counts equal to the mask's counts;
+- between the schedules, bit for bit: logits, dW, edge gradients, the weights after each update, the running
+  statistics and the infer logits.  With set_bf16_aggregation the two schedules may store different tensors in bf16
+  (a Linear's fused norm output against its own output), so there each is held to the witness with its own bf16
+  values, and bit for bit only where both chose the same tensors.
 
 Wirings that break Q7 (below) run in a subprocess: both schedules must exit non-zero at the first backward() with
 the same assertion.
@@ -19,24 +27,36 @@ The rules every generated graph obeys, derived from model.cc:
 - Q7 as implemented.  ScatterGather::backward and InDegreeNorm::backward assert resetInputGrads[0] before they check
   requiresGrad, so each must be the last-created consumer of its input, even when that input is a leaf.
   Dropout::backward checks requiresGrad first: the rule binds a dropout only when its input needs a gradient.  Every
-  other op adds into a gradient another op already wrote.
+  other op (batch_norm, elu, attention_scores and scaled_add among them) adds into a gradient another op already
+  wrote.
+- Q7 amended (mark_scaled_add_readers): a norm or dropout whose input a scaled_add also reads need not be its
+  input's last reader; it adds its part through scratch.  The generator builds that shape in both creation orders.
+- bf16 leaves: only linear and dropout read them.  set_bf16_aggregation: the witness takes the values of the tensors
+  tensor_dtype reports as bf16, with the gradient passed straight through.
+- batch_norm on any fp32 tensor, sometimes read by a relu alone (the BN-relu fusion); elu on any fp32 tensor.
+- attention scores from linear(t, 2 * heads) or attention_scores(t, heads); attention dropout at rate 0 or 0.6.
+- scaled_add of two different same-width tensors, coefficients (1, 1), (0.9, 0.1), (1.5, -0.5) or (0, 1).
+- The teleport hop norm(sg(norm(t))) -> scaled_add(., t0) [-> norm], t0 a leaf or a tensor produced before the sum
+  scatter_gather (the fusion applies), or produced after it (refused).
 - Q1: without set_exact_backward, the sum, max / min and attention backwards gather over the forward CSR, the true
   adjoint only on a symmetric graph; so only exact-mode cases run on the directed multigraph.
 - Max / min without the exact mode need strictly increasing sources per row (the symmetric graphs have them).
 - attention_gather: scores of 2 * heads columns; heads 1, 2, 4 or 8; with heads > 1 the width is heads * F with F a
   power of two >= 4; width <= 512.
-- One loss."""
+- One loss, softmax or sigmoid (labels from datasets.node_data / datasets.multilabel_node_data)."""
+import atexit
 import itertools
 import os
 import subprocess
 import sys
+import tempfile
 import time
 
 import numpy as np
 import pytest
 
 from conftest import ROOT
-from opgraph import Recorder, witness
+from opgraph import INNER, Recorder, witness
 from roc_b200 import _lib, datasets
 from roc_b200.model import Host, Model
 
@@ -106,14 +126,38 @@ def note_fusions(fz, ir):
         if kind == "linear" and d.get("flags"):
             SEEN.add("fusion:linear_norm_sg")
         if kind == "scatter_gather" and "epilogue" in d:
-            SEEN.add("fusion:sg_norm" if d["epilogue"] == _lib.SG_EPI_NORM else "fusion:sg_norm_relu")
+            epi = d["epilogue"]
+            SEEN.add("fusion:sg_norm_relu" if epi & _lib.SG_EPI_RELU else "fusion:sg_norm")
+            if epi & _lib.SG_EPI_NORM_OUT:
+                SEEN.add("fusion:teleport_norm_out")
+        if kind == "scaled_add" and d.get("fusedInto", -1) >= 0:
+            SEEN.add("fusion:teleport")
+        if kind == "batch_norm" and d.get("fwdOut", -1) >= 0:
+            SEEN.add("fusion:batch_norm_relu")
         if kind == "linear" and d.get("dropOp", -1) >= 0:
             SEEN.add("fusion:dropout_linear")
-        if kind == "softmax_cross_entropy":
+        if kind in ("softmax_cross_entropy", "sigmoid_cross_entropy"):
             SEEN.add("fusion:norm_softmax")
         if kind == "linear" and d.get("dxNorm"):
             SEEN.add("fusion:norm_relu_linear" if ir.nodes[layer - 1]["kind"] == "relu" else
                      "fusion:norm_relu_dropout_linear")
+
+
+def note_features(ir, dtypes):
+    """What a case exercised beyond op kinds: attention dropout, the sigmoid loss, bf16 tensors, and a norm or dropout
+    that a later scaled_add shares its input with (the amended Q7)."""
+    if any(nd["kind"] == "attention_gather" and nd["attrs"]["dropout"] > 0 for nd in ir.nodes):
+        SEEN.add("attn_dropout")
+    if ir.loss_node()["kind"] == "sigmoid_cross_entropy":
+        SEEN.add("loss:sigmoid")
+    if ir.bf16:
+        SEEN.add("bf16:features")
+    if any(d == "bfloat16" and t not in ir.bf16 for t, d in dtypes.items()):
+        SEEN.add("bf16:aggregation")
+    for nd in ir.nodes:
+        if nd["kind"] in ("indegree_norm", "dropout") and any(
+                r["kind"] == "scaled_add" and r["layer"] > nd["layer"] and nd["ins"][0] in r["ins"] for r in ir.nodes):
+            SEEN.add("scaled_add_shared_reader")
 
 
 def note_widths(ir):
@@ -158,8 +202,9 @@ def family(name, got, want, rtol, atol_scale):
 
 def run(build, gkind, fuse, steps=3, feats_seed=5):
     """Build with `build(ir)` (it makes the graph and the loss, returns its handles), train `steps` Adam steps and
-    run one infer forward.  Per step: weights before it, logits, dW, edge gradients, weights after it, the relu masks
-    and max / min choices; then the infer metrics and the fusion report."""
+    run one infer forward.  Per step: weights before it, logits, dW, edge gradients, weights after it, the relu masks,
+    max / min choices and bf16 values; then the running statistics, the infer logits (with their masks, choices and
+    bf16 values), the infer metrics and the fusion report."""
     row_end, col = graph(gkind)
     n = row_end.shape[0]
     host = Host(0, 0, 1)
@@ -176,9 +221,14 @@ def run(build, gkind, fuse, steps=3, feats_seed=5):
     feats = {t: rng.uniform(-1, 1, size=(n, ir.width[t])).astype(np.float32) for t in ir.leaves if t != label_t}
     for t, a in feats.items():
         m.set_tensor(t, a)
-    _, labels, mask = datasets.node_data(n, 1, ir.width[logits_t], seed=feats_seed)
-    labels, mask = labels.numpy(), mask.numpy()
-    m.set_labels(label_t, labels)
+    if loss["kind"] == "sigmoid_cross_entropy":
+        _, labels, mask = datasets.multilabel_node_data(n, 1, ir.width[logits_t], seed=feats_seed)
+        labels, mask = labels.numpy(), mask.numpy()
+        m.set_multilabels(label_t, labels)
+    else:
+        _, labels, mask = datasets.node_data(n, 1, ir.width[logits_t], seed=feats_seed)
+        labels, mask = labels.numpy(), mask.numpy()
+        m.set_labels(label_t, labels)
     m.set_tensor(mask_t, mask.astype(np.int32))
     ev = {}
     for e in ir.edges:
@@ -187,20 +237,28 @@ def run(build, gkind, fuse, steps=3, feats_seed=5):
     relu_of = {nd["layer"]: nd["out"] for nd in ir.nodes
                if nd["kind"] == "relu" or (nd["kind"] == "linear" and nd["attrs"]["activation"] == RELU)}
     minmax = {nd["layer"]: nd["out"] for nd in ir.nodes if nd["kind"] in ("scatter_gather_max", "scatter_gather_min")}
-    out = dict(steps=[], ir=ir, h=h, feats=feats, labels=labels, mask=mask, edges=ev, info=m.op_info())
+    dtypes = {t: m.tensor_dtype(t) for t in ir.width if t < INNER}
+    half = [t for t, d in dtypes.items() if d == "bfloat16" and t not in ir.bf16]
+
+    def observe():
+        return dict(logits=m.get_tensor(logits_t), relu={l: m.get_tensor(t) > 0 for l, t in relu_of.items()},
+                    args={l: m.get_aggr_index(t) for l, t in minmax.items()},
+                    rounded={t: m.get_tensor(t) for t in half})
+
+    out = dict(steps=[], ir=ir, h=h, feats=feats, labels=labels, mask=mask, edges=ev, info=m.op_info(), dtypes=dtypes)
     for _ in range(steps):
         w0 = [m.get_parameter(p) for p in range(m.num_parameters())]
         m.train_mode(); m.zero_gradients(); m.forward()
-        st = dict(w0=w0, logits=m.get_tensor(logits_t),
-                  relu={l: m.get_tensor(t) > 0 for l, t in relu_of.items()},
-                  args={l: m.get_aggr_index(t) for l, t in minmax.items()})
+        st = dict(w0=w0, **observe())
         m.backward()
         st["dw"] = [m.get_parameter(p, "grad") for p in range(m.num_parameters())]
         st["de"] = {e: m.get_tensor(e, grad=True)[:, 0].copy() for e in ir.edges if ir.edge_grad[e]}
         m.update()
         st["w1"] = [m.get_parameter(p) for p in range(m.num_parameters())]
         out["steps"].append(st)
+    out["run_stats"] = {nd["out"]: m.batch_norm_stats(nd["out"]) for nd in ir.nodes if nd["kind"] == "batch_norm"}
     m.infer_mode(); m.forward()
+    out["infer"] = observe()
     out["metrics"] = m.metrics()
     host.close()
     return out
@@ -211,39 +269,65 @@ def check_case(build, gkind="sym", expect=None):
     fused, unfused = run(build, gkind, True), run(build, gkind, False)
     ir = fused["ir"]
     row_end, col = graph(gkind)
+    n = row_end.shape[0]
     fz = fusions(fused["info"])
     assert fusions(unfused["info"]) == {}, "the unfused schedule fused something"
     if expect is not None:
         assert fz == expect(fused["h"]), fz
     note_fusions(fz, ir)
     note_widths(ir)
+    note_features(ir, fused["dtypes"])
+    bn_momentum = {nd["out"]: nd["attrs"]["momentum"] for nd in ir.nodes if nd["kind"] == "batch_norm"}
     for r in (fused, unfused):
+        name = "fused" if r is fused else "unfused"
+        rec = {t: (np.zeros(ir.width[t]), np.ones(ir.width[t])) for t in bn_momentum}
         for step, st in enumerate(r["steps"]):
-            what = "%s step %d" % ("fused" if r is fused else "unfused", step)
+            what = "%s step %d" % (name, step)
             wit = witness(ir, (row_end, col), r["feats"], r["labels"], r["mask"], st["w0"], r["edges"], step=step + 1,
-                          relu_masks=st["relu"], aggr_args=st["args"])
+                          relu_masks=st["relu"], aggr_args=st["args"], rounded=st["rounded"])
             assert family("logits", st["logits"], wit["logits"], 1e-4, 1e-5) <= 1, what + " logits vs fp64"
             for p, (a, b) in enumerate(zip(st["dw"], wit["dW"])):
                 assert family("dW", a, b, 2e-4, 2e-5) <= 1, what + " dW[%d] vs fp64" % p
             for e, g in st["de"].items():
                 assert family("edge gradient", g, wit["edge_grad"][e], 2e-4, 2e-5) <= 1, what + " edge gradient"
-    for step, (a, b) in enumerate(zip(fused["steps"], unfused["steps"])):
-        assert np.array_equal(a["logits"], b["logits"]), "step %d: logits differ between the schedules" % step
-        for p in range(len(a["dw"])):
-            assert np.array_equal(a["dw"][p], b["dw"][p]), "step %d: dW[%d] differs between the schedules" % (step, p)
-            assert np.array_equal(a["w1"][p], b["w1"][p]), "step %d: W[%d] differs between the schedules" % (step, p)
-        for e in a["de"]:
-            assert np.array_equal(a["de"][e], b["de"][e]), "step %d: edge gradient differs" % step
-    fm, um = dict(fused["metrics"]), dict(unfused["metrics"])
-    fm.pop("trainLoss"), um.pop("trainLoss")
-    assert fm == um, (fm, um)
+            for t, (mean, var) in wit["stats"].items():
+                mo, (rm, rv) = bn_momentum[t], rec[t]
+                rec[t] = ((1 - mo) * rm + mo * mean, (1 - mo) * rv + mo * var * n / (n - 1))
+        for t, (rm, rv) in rec.items():
+            assert family("running stats", r["run_stats"][t][0], rm, 2e-4, 2e-5) <= 1, name + " running mean"
+            assert family("running stats", r["run_stats"][t][1], rv, 2e-4, 2e-5) <= 1, name + " running var"
+        inf = r["infer"]
+        wit = witness(ir, (row_end, col), r["feats"], r["labels"], r["mask"], r["steps"][-1]["w1"], r["edges"],
+                      relu_masks=inf["relu"], aggr_args=inf["args"], rounded=inf["rounded"], training=False,
+                      run_stats=r["run_stats"])
+        assert family("infer logits", inf["logits"], wit["logits"], 1e-4, 1e-5) <= 1, name + " infer logits vs fp64"
+    same = lambda a, b: np.array_equal(np.asarray(a).view(np.int32), np.asarray(b).view(np.int32))
+    if fused["dtypes"] == unfused["dtypes"]:
+        for step, (a, b) in enumerate(zip(fused["steps"], unfused["steps"])):
+            assert same(a["logits"], b["logits"]), "step %d: logits differ between the schedules" % step
+            for p in range(len(a["dw"])):
+                assert same(a["dw"][p], b["dw"][p]), "step %d: dW[%d] differs between the schedules" % (step, p)
+                assert same(a["w1"][p], b["w1"][p]), "step %d: W[%d] differs between the schedules" % (step, p)
+            for e in a["de"]:
+                assert same(a["de"][e], b["de"][e]), "step %d: edge gradient differs" % step
+        for t in fused["run_stats"]:
+            for a, b in zip(fused["run_stats"][t], unfused["run_stats"][t]):
+                assert same(a, b), "running statistics differ between the schedules"
+        assert same(fused["infer"]["logits"], unfused["infer"]["logits"]), "infer logits differ between the schedules"
+        fm, um = dict(fused["metrics"]), dict(unfused["metrics"])
+        fm.pop("trainLoss"), um.pop("trainLoss")
+        assert fm == um, (fm, um)
+    else:
+        assert ir.bf16_aggregation, "the schedules store different tensors in bf16 without set_bf16_aggregation"
+    fm = fused["metrics"]
     mask = fused["mask"]
     assert (fm["trainAll"], fm["valAll"], fm["testAll"]) == tuple(int((mask == k).sum()) for k in (0, 1, 2)), fm
     return fz
 
 
-def loss(ir, t):
-    ir.softmax_cross_entropy(t, ir.create_node_tensor(ir.width[t]), ir.create_node_tensor(1, is_int=True))
+def loss(ir, t, sigmoid=False):
+    f = ir.sigmoid_cross_entropy if sigmoid else ir.softmax_cross_entropy
+    f(t, ir.create_node_tensor(ir.width[t]), ir.create_node_tensor(1, is_int=True))
 
 
 # ------------------------------------------------------------------------------------------ (a) hand-listed cases ---
@@ -300,7 +384,52 @@ def expect_fused_chain(h, sg_layer, relu=True):
     return e
 
 
+def batch_norm_relu(ir):
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 16); b = ir.batch_norm(t); r = ir.relu(b)
+    loss(ir, ir.linear(r, 5))
+    return dict(b=b, r=r)
+
+
+def teleport(ir, norm_out=False, t0="before", second=False, sa_twice=False):
+    """linear -> norm -> sg -> norm -> scaled_add(., t0, 0.9, 0.1) [-> norm] -> linear: t0 a Linear made before the
+    scatter_gather (or after it); second: the norm output is the scaled_add's second input; sa_twice: a relu also
+    reads the scaled_add's output."""
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 16)
+    u = ir.linear(x, 16) if t0 == "before" else None
+    n1 = ir.indegree_norm(t); s = ir.scatter_gather(n1); n2 = ir.indegree_norm(s)
+    if u is None:
+        u = ir.linear(x, 16)
+    y = ir.scaled_add(u, n2, 0.9, 0.1) if second else ir.scaled_add(n2, u, 0.9, 0.1)
+    r = ir.relu(y) if sa_twice else None                # before the norm, which must be y's last reader
+    z = ir.indegree_norm(y) if norm_out else y
+    out = ir.linear(z, 5)
+    if sa_twice:
+        out = ir.add(out, ir.linear(r, 5))
+    loss(ir, out)
+    return dict(t=t, n1=n1, n2=n2, y=y, z=z)
+
+
+def expect_teleport(h, fused=True, norm_out=False, sg=3):
+    """the GCN block's two fusions on the layers teleport() makes, the teleport on top when `fused`"""
+    e = {0: dict(flags=_lib.LINEAR_NORM_EPILOGUE, fwdOut=h["n1"]), sg - 1: dict(fusedInto=0),
+         sg: dict(bwdEpilogue=_lib.SG_EPI_NORM, bwdOut=h["t"], epilogue=_lib.SG_EPI_NORM, fwdOut=h["n2"]),
+         sg + 1: dict(fusedInto=sg)}
+    if fused:
+        e[sg]["fwdOut"] = h["y"]
+        e[sg + 2] = dict(fusedInto=sg)
+    if norm_out:
+        e[sg]["epilogue"] |= _lib.SG_EPI_NORM_OUT
+        e[sg]["fwdOut"] = h["z"]
+        e[sg + 3] = dict(fusedInto=sg)
+    return e
+
+
 HAND = {
+    "batch_norm_relu": (batch_norm_relu, lambda h: {1: dict(fwdOut=h["r"]), 2: dict(fusedInto=1)}),
+    "teleport": (teleport, expect_teleport),
+    "teleport_norm_out": (lambda ir: teleport(ir, norm_out=True), lambda h: expect_teleport(h, norm_out=True)),
     # each fusion alone, in its minimal pattern
     "lin_norm_sg": (lin_norm_sg, lambda h: {0: dict(flags=_lib.LINEAR_NORM_EPILOGUE, fwdOut=h["n"]), 1: dict(fusedInto=0),
                                             2: dict(bwdEpilogue=_lib.SG_EPI_NORM, bwdOut=h["t"])}),
@@ -416,7 +545,51 @@ def nm_competing_norm(ir):
     return dict(t=t, n1=n1, n2=n2)
 
 
+def nm_bn(readers):
+    def build(ir):
+        x = ir.create_node_tensor(12)
+        b = ir.batch_norm(ir.linear(x, 16))
+        outs = [getattr(ir, k)(b) for k in readers]
+        loss(ir, ir.linear(outs[0] if len(outs) == 1 else ir.add(*outs), 5))
+    return build
+
+
+def nm_teleport_bf16(ir):
+    """set_bf16_aggregation stores the fused linear -> norm output the sum scatter_gather reads in bf16: no teleport
+    kernel reads it, so the hop stays unfused"""
+    ir.set_bf16_aggregation(True)
+    return teleport(ir)
+
+
+def nm_dropout_shared_linear(ir):
+    """y = linear(dropout(h)); scaled_add(y, h): the dropout adds to what the scaled_add wrote, so it must not be
+    fused into the Linear, whose dX epilogue overwrites"""
+    x = ir.create_node_tensor(12)
+    h = ir.linear(x, 16)
+    y = ir.linear(ir.dropout(h, 0.5, seed=1), 16)
+    loss(ir, ir.linear(ir.scaled_add(y, h, 0.9, 0.1), 5))
+
+
+def nm_norm_shared_loss(ir):
+    """norm(h) feeds the loss and a scaled_add made after the loss reads h: the norm's backward adds to what the
+    scaled_add wrote, so the loss must not take it over"""
+    x = ir.create_node_tensor(12)
+    h = ir.linear(x, 5); u = ir.linear(x, 5)
+    loss(ir, ir.indegree_norm(h))
+    ir.scaled_add(h, u, 1.0, 1.0)
+
+
 NEAR = {
+    "bn_out_read_twice": (nm_bn(("relu", "sigmoid")), lambda h: {}),
+    "bn_then_elu": (nm_bn(("elu",)), lambda h: {}),
+    "bn_then_sigmoid": (nm_bn(("sigmoid",)), lambda h: {}),
+    "teleport_sg_input_bf16": (nm_teleport_bf16, lambda h: expect_teleport(h, fused=False)),
+    "teleport_t0_after_sg": (lambda ir: teleport(ir, t0="after"), lambda h: expect_teleport(h, fused=False, sg=2)),
+    "teleport_norm_second_input": (lambda ir: teleport(ir, second=True), lambda h: expect_teleport(h, fused=False)),
+    "scaled_add_out_read_twice": (lambda ir: teleport(ir, norm_out=True, sa_twice=True),
+                                  lambda h: expect_teleport(h)),
+    "dropout_shared_with_scaled_add_into_linear": (nm_dropout_shared_linear, lambda h: {}),
+    "norm_shared_with_scaled_add_into_loss": (nm_norm_shared_loss, lambda h: {}),
     "linear_out_read_twice": (nm_linear_out_twice, lambda h: {}),
     "norm1_out_read_twice": (nm_norm1_out_twice, lambda h: {}),
     "sg_out_read_twice": (nm_sg_out_twice, lambda h: {}),
@@ -495,7 +668,28 @@ def dead_branch(ir):
     loss(ir, y)
 
 
+def scores_and_gather_t(ir):
+    x = ir.create_node_tensor(12)
+    wh = ir.linear(x, 16)
+    loss(ir, ir.linear(ir.attention_gather(wh, ir.attention_scores(wh, heads=4), heads=4, dropout=0.6, seed=1), 5))
+
+
+def scaled_add_t_relu_t(ir):
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 16)
+    loss(ir, ir.linear(ir.scaled_add(t, ir.relu(t), 0.9, 0.1), 5))
+
+
+def elu_and_bn_t(ir):
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 16)
+    loss(ir, ir.linear(ir.add(ir.elu(t), ir.batch_norm(t)), 5))
+
+
 SHARED = {
+    "attention_scores_and_gather_t": (scores_and_gather_t, lambda h: {}),
+    "scaled_add_t_relu_t": (scaled_add_t_relu_t, lambda h: {}),
+    "elu_and_batch_norm_t": (elu_and_bn_t, lambda h: {}),
     "add_t_t": (add_t_t, lambda h: {}),
     "attention_t_t_H2": (attention_t_t, lambda h: {}),
     "linear_relu_and_sigmoid": (linear_relu_sigmoid, lambda h: {}),
@@ -571,17 +765,25 @@ SMALL, RING_U, RING_T = (3, 5, 7, 12, 16), (72, 100, 128), (132, 160, 256)
 CLASSES = (5, 32, 33, 64, 65, 128, 129)
 
 
+SEEDS = 64
+COEFFS = ((1.0, 1.0), (0.9, 0.1), (1.5, -0.5), (0.0, 1.0))
+
+
 def random_graph(seed):
     """A seeded DAG over every op, obeying the rules in the module docstring.  Tensors a ScatterGather, a norm or a
-    dropout (whose input needs a gradient) have read are closed: nothing reads them again.  Every tensor nothing
-    reads at the end goes through a Linear into one sum that feeds the loss, except, now and then, a dead one."""
+    dropout (whose input needs a gradient) have read are closed: nothing reads them again, except the scaled_add a
+    "shared" step makes.  Every tensor nothing reads at the end goes through a Linear into one sum that feeds the
+    loss, except, now and then, a dead one."""
     exact = seed % 6 == 5
     gkind = "directed" if exact else ("hub" if seed % 8 == 3 else "sym")
+    half_x, half_aggr, sigmoid = seed % 5 == 2, seed % 7 == 4, seed % 3 == 1
 
     def build(ir):                       # called once per schedule: the same graph each time
         rng = np.random.RandomState(seed)
         if exact:
             ir.set_exact_backward(True)
+        if half_aggr:
+            ir.set_bf16_aggregation(True)
         open_, grad, closed = [], {}, set()
         edges = []
 
@@ -595,13 +797,23 @@ def random_graph(seed):
             grad[t] = g
             return t
 
-        x = ir.create_node_tensor(int(rng.choice((7, 12, 16, 33))))
+        def partner(t):
+            """an open fp32 tensor of t's width other than t, or None"""
+            same = [u for u in open_ if ir.width[u] == ir.width[t] and u != t and u not in ir.bf16]
+            return same[rng.randint(len(same))] if same else None
+
+        def coeffs():
+            return COEFFS[rng.randint(len(COEFFS))]
+
+        x = ir.create_node_tensor(int(rng.choice((7, 12, 16, 33))), dtype="bfloat16" if half_x else "float32")
         new(x, False)
-        for _ in range(rng.randint(3, 9)):
+        for _ in range(rng.randint(3, 10)):
             t = open_[rng.randint(len(open_))]
             w = ir.width[t]
             k = rng.choice(["linear", "linear", "norm", "sg", "sg_mm", "sg_w", "attn", "relu", "sigmoid", "add",
-                            "dropout"])
+                            "dropout", "batch_norm", "elu", "scaled_add", "shared", "teleport"])
+            if t in ir.bf16 and k not in ("linear", "dropout"):
+                k = "linear"
             if k == "linear":
                 pick = rng.randint(4)
                 o = int(rng.choice(SMALL + (136, 7) if pick == 0 else RING_U if pick == 1 else RING_T if pick == 2
@@ -626,17 +838,61 @@ def random_graph(seed):
                                                                                (w // h) & (w // h - 1) == 0)]))
                 if w > 512:
                     continue
-                sc = ir.linear(t, 2 * heads)
-                new(ir.attention_gather(t, sc, heads=heads), True)
-            elif k in ("relu", "sigmoid"):
+                sc = ir.attention_scores(t, heads) if rng.rand() < 0.5 else ir.linear(t, 2 * heads)
+                rate = 0.6 if rng.rand() < 0.4 else 0.0
+                new(ir.attention_gather(t, sc, heads=heads, dropout=rate, seed=int(rng.randint(4))), True)
+            elif k in ("relu", "sigmoid", "elu"):
                 new(getattr(ir, k)(t), grad[t])
+            elif k == "batch_norm":
+                b = ir.batch_norm(t)
+                if rng.rand() < 0.4:
+                    new(ir.relu(b), True)                     # read by a relu alone: the BN-relu fusion
+                else:
+                    new(b, True)
             elif k == "add":
-                same = [u for u in open_ if ir.width[u] == w]
+                same = [u for u in open_ if ir.width[u] == w and u not in ir.bf16]
                 u = same[rng.randint(len(same))]
                 new(ir.add(t, u), grad[t] or grad[u])
-            else:
+            elif k == "scaled_add":
+                u = partner(t)
+                if u is None:
+                    continue
+                a, b = (t, u) if rng.rand() < 0.5 else (u, t)
+                new(ir.scaled_add(a, b, *coeffs()), grad[t] or grad[u])
+            elif k == "shared":
+                # a norm or dropout and a scaled_add reading t, in either creation order; t is then closed
+                u = partner(t)
+                if u is None:
+                    continue
+                norm = rng.rand() < 0.5
+                rate = float(rng.choice([0.0, 0.5]))
+                first = rng.rand() < 0.5
+                if first:
+                    sa = ir.scaled_add(t, u, *coeffs())
+                r = ir.indegree_norm(t) if norm else ir.dropout(t, rate, seed=int(rng.randint(4)))
+                if not first:
+                    sa = ir.scaled_add(t, u, *coeffs())
+                take(t, True)
+                new(r, grad[t])
+                new(sa, grad[t] or grad[u])
+            elif k == "dropout":
                 take(t, grad[t])
                 new(ir.dropout(t, float(rng.choice([0.0, 0.5])), seed=int(rng.randint(4))), grad[t])
+            else:
+                # the teleport hop: t0 a leaf, an earlier tensor (t itself: APPNP's shape), or one made after the SG
+                take(t, True)
+                n1 = ir.indegree_norm(t)
+                s = ir.scatter_gather(n1)
+                n2 = ir.indegree_norm(s)
+                where = rng.randint(3)
+                if where == 1:
+                    t0, g0 = t, grad[t]
+                elif where == 2 and open_:
+                    t0, g0 = new(ir.linear(open_[rng.randint(len(open_))], w), True), True
+                else:
+                    t0, g0 = ir.create_node_tensor(w), False
+                y = ir.scaled_add(n2, t0, *coeffs())
+                new(ir.indegree_norm(y) if rng.rand() < 0.5 else y, grad[t] or g0)
         C = int(rng.choice(CLASSES))
         sinks = [t for t in open_ if t != x or len(open_) == 1]
         if len(sinks) > 1 and rng.rand() < 0.25:
@@ -647,13 +903,13 @@ def random_graph(seed):
             z = y if z is None else ir.add(z, y)
         if rng.rand() < 0.3:
             z = ir.indegree_norm(z)
-        loss(ir, z)
+        loss(ir, z, sigmoid=sigmoid)
         for e in edges:
             ir.set_edge_grad(e, bool(rng.rand() < 0.7))
     return build, gkind
 
 
-@pytest.mark.parametrize("seed", range(48))
+@pytest.mark.parametrize("seed", range(SEEDS))
 def test_random_graph(seed):
     build, gkind = random_graph(seed)
     check_case(build, gkind=gkind)
@@ -699,7 +955,16 @@ def rf_norm_softmax(ir):
     ir.relu(t)
 
 
-REFUSE = {"sg_not_last": rf_sg(False), "sg_on_leaf_not_last": rf_sg(True), "norm_not_last": rf_norm(False),
+def rf_norm_shared_with_add(ir):
+    """A plain add reads the norm's input after it: only a scaled_add makes that wiring legal."""
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 16)
+    n = ir.indegree_norm(t)
+    loss(ir, ir.linear(ir.add(n, t), 5))
+
+
+REFUSE = {"norm_shared_with_add_not_last": rf_norm_shared_with_add, "sg_not_last": rf_sg(False),
+          "sg_on_leaf_not_last": rf_sg(True), "norm_not_last": rf_norm(False),
           "norm_on_leaf_not_last": rf_norm(True), "dropout_not_last": rf_dropout(False),
           "dropout_into_linear_not_last": rf_dropout(True), "norm_into_softmax_not_last": rf_norm_softmax}
 
@@ -729,12 +994,43 @@ def refusal_prog(name, fuse):
     print("backward done", flush=True)
 
 
+RUNS = {}                  # (refusal case, fuse) -> (its process, its stdout and stderr files)
+
+
+def start_refusals():
+    """Every refusal case in both schedules, each in its own process (the abort ends it), all started together on
+    first use: each process spends most of its time starting Python, torch and the CUDA context."""
+    if RUNS:
+        return
+    for name in REFUSE:
+        for fuse in (True, False):
+            prog = "\n".join(["import sys; sys.path.insert(0, %r); sys.path.insert(0, %r)" %
+                              (ROOT, os.path.join(ROOT, "tests")),
+                              "from test_opgraph_gpu import refusal_prog",
+                              "refusal_prog(%r, %r)" % (name, fuse)])
+            out, err = tempfile.TemporaryFile("w+"), tempfile.TemporaryFile("w+")
+            RUNS[(name, fuse)] = (subprocess.Popen([sys.executable, "-c", prog], stdout=out, stderr=err, text=True,
+                                                   cwd=ROOT, env=dict(os.environ)), out, err)
+
+
+@atexit.register
+def _stop_refusals():
+    for proc, _, _ in RUNS.values():
+        if proc.poll() is None:
+            proc.kill()
+            proc.wait()
+
+
 def run_refusal(name, fuse):
-    prog = "\n".join(["import sys; sys.path.insert(0, %r); sys.path.insert(0, %r)" % (ROOT, os.path.join(ROOT, "tests")),
-                      "from test_opgraph_gpu import refusal_prog",
-                      "refusal_prog(%r, %r)" % (name, fuse)])
-    return subprocess.run([sys.executable, "-c", prog], capture_output=True, text=True, timeout=300, cwd=ROOT,
-                          env=dict(os.environ))
+    start_refusals()
+    proc, out, err = RUNS[(name, fuse)]
+    try:
+        proc.wait(timeout=300)
+    except subprocess.TimeoutExpired:
+        proc.kill()
+        proc.wait()
+    out.seek(0), err.seek(0)
+    return subprocess.CompletedProcess(proc.args, proc.returncode, out.read(), err.read())
 
 
 @pytest.mark.parametrize("name", list(REFUSE))
@@ -756,7 +1052,9 @@ def test_opgraph_covered():
     """Every op kind, fusion, near-miss and width class was reached (run the whole file: this test comes last)."""
     want = {"op:" + k for k in _lib.HOST_OPS} | {"op:linear_relu", "op:linear_none"}
     want |= {"fusion:" + f for f in ("linear_norm_sg", "sg_norm", "sg_norm_relu", "dropout_linear", "norm_softmax",
-                                     "norm_relu_linear", "norm_relu_dropout_linear")}
+                                     "norm_relu_linear", "norm_relu_dropout_linear", "batch_norm_relu", "teleport",
+                                     "teleport_norm_out")}
+    want |= {"attn_dropout", "loss:sigmoid", "bf16:features", "bf16:aggregation", "scaled_add_shared_reader"}
     want |= {"near:" + n for n in NEAR} | {"shared:" + s for s in SHARED} | {"exact:" + e for e in EXACT}
     want |= {"refusal:" + r for r in REFUSE} | {"random", "graph:hub"}
     want |= {"width:" + w for w in ("linear_in_not_float4", "linear_out_over_128", "sg_H_not_float4", "sg_65_128",

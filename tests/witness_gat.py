@@ -4,8 +4,9 @@ import numpy as np
 import torch
 
 
-def attend(wh, sc, dst, src, n, heads, slope):
-    """Per head, the softmax over each row's in-edges of LeakyReLU(sc_dst[v] + sc_src[u]) applied to wh[u]."""
+def attend(wh, sc, dst, src, n, heads, slope, drop=None):
+    """Per head, the softmax over each row's in-edges of LeakyReLU(sc_dst[v] + sc_src[u]) applied to wh[u].  drop:
+    [E][heads] multipliers of the softmax weights (attention dropout), or None."""
     z = sc[dst, :heads] + sc[src, heads:]
     y = torch.where(z > 0, z, slope * z)
     # the row max only shifts the exponent; the softmax, and so its gradient, does not depend on it
@@ -14,6 +15,8 @@ def attend(wh, sc, dst, src, n, heads, slope):
     ex = torch.exp(y - m[dst])
     den = torch.zeros((n, heads), dtype=torch.float64).index_add(0, dst, ex)
     a = ex / den[dst]
+    if drop is not None:
+        a = a * torch.from_numpy(np.asarray(drop, dtype=np.float64))
     f = wh.shape[1] // heads
     msg = (a.unsqueeze(2) * wh[src].reshape(-1, heads, f)).reshape(-1, wh.shape[1])
     return torch.zeros((n, wh.shape[1]), dtype=torch.float64).index_add(0, dst, msg)

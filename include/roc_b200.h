@@ -663,7 +663,9 @@ int roc_softmax_xent_bwd_norm(int64_t rows, int C, const float* logits, int64_t 
  *  - `metrics` (device, may be NULL) is ACCUMULATED into: zero it first.  Rows with mask ROC_MASK_NONE (or any value
  *    outside 0..2) count nowhere.  The loss is summed in fp32 over each run of up to 4 consecutive elements of a row,
  *    then in fp64 into per-block partials that one block adds in block order, so the same call on the same device
- *    gives the same bits; the counts are exact.  Calls that
+ *    with the same SM budget gives the same bits; the counts are exact.  The loss's bits may differ between SM
+ *    counts: each thread sums the rows it visits, and which rows those are depends on the grid, which is sized from
+ *    the SMs the calling thread may use (roc_set_sm_reserve).  The gradient's bits never depend on it.  Calls that
  *    pass `metrics` share one per-device scratch for the partials: do not run two of them at once on different
  *    streams of one device.
  * ROC_ERR_INVALID: a NULL logits / labelBits / mask / grad, rows < 0, C < 1, ldZ or ldG < C, ldB < W. */

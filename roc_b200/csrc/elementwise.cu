@@ -506,6 +506,8 @@ static void launch_softmax(int64_t rows, int C, const float* logits, int64_t ldZ
 constexpr int ML_T = 256;
 constexpr int ML_MAX_BLOCKS = 4096;
 constexpr int ML_FIELDS = 18;   // roc_multilabel_metrics: 3 doubles (loss), then 15 u64 (rows, exact, tp, fp, fn)
+// One set of slots and one ticket per device: two calls with metrics must not overlap (the header states it; the host
+// issues the loss once per step on one stream).
 __device__ roc_multilabel_metrics g_mlPartial[ML_MAX_BLOCKS];
 __device__ unsigned int g_mlTicket;
 

@@ -307,6 +307,31 @@ int roc_sg_attn_backward_dropout_planned_bf16(const roc_sg_plan* plan, int heads
 int roc_sg_attn_keep_mask(const roc_sg_plan* plan, roc_vid_t selfBase, int rowIsSource, float rate, uint64_t seed,
                           uint32_t step, uint8_t* keep, roc_stream_t stream);
 
+/* Edge dropout of the sum (the APPNP paper's dropout of the propagation matrix, PyG APPNP(dropout=); DropEdge, Rong et
+ * al. 2020, applied to GCN).  keep(i<-j) is bit 0 of the byte roc_sg_attn_keep_mask writes for the pair (i <- j): lane 0
+ * of Philox4x32-10 with counter {i, j, 0, step} and key {seed lo, seed hi}, against T16 = round(rate * 65536), the same
+ * generator as attention dropout, so duplicate edges of a multigraph share one decision.  With s = 1.0f / (1.0f - rate)
+ * (fp32, roc_dropout_fwd's scale):
+ *   out[v][h] = epilogue( sum over the kept in-edges e of v, in the sum's per-row order, acc = fmaf(s, in[j][h], acc) )
+ * accumulated from +0; a dropped edge contributes nothing and its source row is not loaded, and a row whose edges are
+ * all dropped gets epilogue(0).  The degrees the epilogues divide by stay the full graph's: this is dropout on the
+ * normalised adjacency entries (PyG APPNP's form), not DropEdge's renormalisation on the sampled graph.  On finite
+ * inputs the bytes equal roc_sg_weighted_forward_planned with w[e] = keep ? s : 0 (the sum's column blocks and order)
+ * followed by the unfused kernels the epilogue replaces (roc_indegree_norm for NORM, then relu for RELU).  keep holds
+ * one byte per edge of the plan, in its edge order (roc_sg_attn_keep_mask with rowIsSource 0 over the forward plan).
+ * rate = 0 or keep = NULL: roc_sg_forward_planned itself, byte for byte and launch for launch.  ROC_ERR_INVALID: as
+ * roc_sg_forward_planned, and a rate outside [0, 1).  Every width runs on the register kernel (no ring form); its main
+ * launches report reduction 32 in roc_sg_last_call_info, its fix-ups as the sum's. */
+int roc_sg_forward_dropout_planned(const roc_sg_plan* plan, int H, const float* in, int64_t ldIn, float* out,
+                                   int64_t ldOut, int epilogue, const uint8_t* keep, float rate, roc_stream_t stream);
+/* roc_sg_forward_teleport_planned over the dropped sum: post(fmaf(alpha, pre(dropped sum), beta * t)), bytes equal to
+ * roc_sg_forward_dropout_planned (epilogue & NORM) followed by the chain roc_sg_forward_teleport_planned documents.
+ * rate = 0 or keep = NULL: roc_sg_forward_teleport_planned itself.  ROC_ERR_INVALID: as that call, and a rate outside
+ * [0, 1).  Main launches report reduction 45, the fix-ups 13. */
+int roc_sg_forward_teleport_dropout_planned(const roc_sg_plan* plan, int H, const float* in, int64_t ldIn, float alpha,
+                                            const float* t, int64_t ldT, float beta, float* out, int64_t ldOut,
+                                            int epilogue, const uint8_t* keep, float rate, roc_stream_t stream);
+
 /* Edge-weighted aggregation (GCN with edge weights, weighted graphs, edge saliency).  The reference declares edge
  * tensors (gnn.h:178) but never reads them; these semantics are this library's own.  For plan row r with id
  * i = selfBase + r and in-edges e in CSR order with sources j = colSrc[e], the edge's weight is w[e - colLeft]: a flat
@@ -381,6 +406,18 @@ int roc_sg_weighted_backward_planned(roc_sg_transpose* transpose, int H, const f
  * ROC_ERR_INVALID), in the form that gives roc_indegree_norm's bits; RELU as in the forward. */
 int roc_sg_transpose_sum_backward(roc_sg_transpose* transpose, int H, const float* outGrad, int64_t ldG, float* inGrad,
                                   int64_t ldIn, int epilogue, const roc_eid_t* rowEnd, roc_stream_t stream);
+/* The exact backward of roc_sg_forward_dropout_planned: roc_sg_transpose_sum_backward over the kept edges only,
+ *   inGrad[j][h] = epi( sum over the kept edges e with colSrc[e] = j: acc = fmaf(s, outGrad[dst(e)][h], acc) )
+ * keep in the transposed plan's edge order (roc_sg_attn_keep_mask over roc_sg_transpose_info's planT, selfBase 0,
+ * rowIsSource 1), so transposed edge j -> i carries keep(i <- j).  NORM divides by the original graph's in-degree, as
+ * there.  Bytes equal roc_sg_weighted_backward_planned with w[e] = keep ? s : 0 followed by the unfused epilogue.
+ * rate = 0 or keep = NULL: roc_sg_transpose_sum_backward itself.  ROC_ERR_INVALID: as that call, and a rate outside
+ * [0, 1).  Main launches report reduction 42 with NORM (fix-ups 10), else 32 (fix-ups 0).  The backward over the same
+ * CSR (quirk Q1) is roc_sg_forward_dropout_planned over the output gradient with the reverse-pair bytes (rowIsSource 1
+ * over the forward plan), so that row u's edge to w carries keep(w <- u): exact on a symmetric graph. */
+int roc_sg_transpose_sum_backward_dropout(roc_sg_transpose* transpose, int H, const float* outGrad, int64_t ldG,
+                                          float* inGrad, int64_t ldIn, int epilogue, const roc_eid_t* rowEnd,
+                                          const uint8_t* keep, float rate, roc_stream_t stream);
 /* Max / min (counterpart roc_sg_minmax_backward_planned with selfBase 0), for arg from roc_sg_minmax_forward_planned:
  *   inGrad[j][h] = sum over the DISTINCT destinations i of j's out-edges of (arg[i][h] == j ? outGrad[i][h] : 0)
  * A duplicate edge j -> i lies next to its twin in transposed row j; an entry whose destination equals the previous
@@ -454,7 +491,9 @@ int roc_sg_backward(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft, in
  *          24 weighted sum, 25 edge-weight gradient: the roc_sg_*_bf16 calls), whose fix-ups are reduction r's and
  *          report as there; 32 + r for the main kernel of attention pass r (5, 6, 7, or 21, 22, 23 on bf16 feature
  *          rows) with dropout (the roc_sg_attn_*_dropout_* calls at rate > 0: 37, 38, 39, 53, 54, 55), whose other
- *          launches report as without dropout; -1 for the record, the permutation and the keep mask, which have
+ *          launches report as without dropout; likewise 32, 42 and 45 for the sum, the exact sum backward with NORM
+ *          and the teleport sum with edge dropout (roc_sg_forward_dropout_planned,
+ *          roc_sg_transpose_sum_backward_dropout, roc_sg_forward_teleport_dropout_planned at rate > 0); -1 for the record, the permutation and the keep mask, which have
  *          none.  A sum fix-up finishing another
  *          reduction's partials reports 0.
  *   vec    4 for float4 rows, else 1;  lanes, nch: the row shape (L lanes, chunks per lane);  grid: CTAs launched

@@ -189,6 +189,18 @@ public:
    * held the extreme.  That is the true gradient only on a symmetric graph without duplicate edges: init() refuses
    * a graph whose rows do not have strictly increasing sources.  Single partition only (exit(1) otherwise). */
   Tensor scatter_gather(const Tensor& _input, AggrType aggr);
+  /* Edge dropout (not in gnn.h): the sum aggregation with each in-edge dropped at rate `dropout` in train mode and a
+   * kept one scaled by 1 / (1 - dropout) (roc_sg_forward_dropout_planned), the APPNP paper's dropout of the propagation
+   * matrix and PyG APPNP(dropout=).  keep(i<-j) is drawn per step from Philox keyed by the pair (i <- j) with key
+   * (seed << 32) | the op's position and the model's train step, as Model::dropout draws its own, so every such op
+   * draws its own mask each step.  Degrees stay the full graph's (the epilogue fusions with indegree_norm and the
+   * teleport fusion apply as to the plain sum): dropout on the normalised adjacency entries, not DropEdge's
+   * renormalisation on the sampled graph.  The backward is the dropped sum over the output gradient with the reverse
+   * pairs' decisions (quirk Q1: exact on a symmetric graph), or with set_exact_backward the dropped transposed sum
+   * (roc_sg_transpose_sum_backward_dropout).  Infer mode and dropout = 0 run the plain sum.  The input stays fp32 under
+   * set_bf16_aggregation.  Exits for an aggregator other than AGGR_SUM with dropout > 0, a rate outside [0, 1), or more
+   * than one partition. */
+  Tensor scatter_gather(const Tensor& _input, AggrType aggr, float dropout, int seed = 0);
   /* Attention aggregation (GAT; roc_sg_attn_forward_planned): `scores` has 2 * heads columns, [s_dst | s_src] per
    * head; the output has the input's width, each head's block of H / heads columns weighted by that head's
    * softmax over the row's in-edges.  Its backward is a gather over the same CSR (quirk Q1): exact for the
@@ -352,6 +364,12 @@ public:
   int fwdOut, bwdOut;/* region the fused forward / backward writes (-1: own output / input grad) */
   int teleT;         /* >= 0: a scaled_add fused into the store (roc_sg_forward_teleport_planned) reads this region as t */
   float teleAlpha, teleBeta;   /*   ... with these coefficients */
+  float dropRate;    /* edge dropout of the sum in train mode (0: none; Model::scatter_gather(input, aggr, dropout, seed)) */
+  int seed;
+  int opIndex;       /* position in the model: the Philox key is (seed << 32) | opIndex, as a Dropout's */
+private:
+  float drop_rate(const Model& model) const;
+  const uint8_t* keep_mask(const Model& model, const roc_sg_plan* plan, roc_vid_t selfBase, int rowIsSource) const;
 };
 
 class AttentionGather : public GnnOp {  /* not in the reference: Model::attention_gather */

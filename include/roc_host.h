@@ -45,6 +45,8 @@ int roc_host_indegree_norm(roc_host* h, int t);
 int roc_host_scatter_gather(roc_host* h, int t);
 /* Model::scatter_gather(t, aggr); aggr = AggrType (0 AVG, 1 MAX, 2 MIN, 3 SUM) */
 int roc_host_scatter_gather_aggr(roc_host* h, int t, int aggr);
+/* Model::scatter_gather(t, AGGR_SUM, rate, seed): the sum with edge dropout at `rate` in train mode */
+int roc_host_scatter_gather_dropout(roc_host* h, int t, float rate, int seed);
 /* Model::attention_gather(t, scores, heads, slope); scores has 2 * heads columns */
 int roc_host_attention_gather(roc_host* h, int t, int scores, int heads, float slope);
 /* Model::attention_gather(t, scores, heads, slope, rate, seed): with attention dropout at `rate` in train mode */

@@ -23,6 +23,7 @@ LINEAR_Y_BF16 = 2                                          # Y holds bf16 bits
 SG_RED_BSUM = 12                                           # roc_sg_launch.red of the sum over bf16 rows
 SG_RED_TELE = 13                                           # roc_sg_launch.red of the teleport sum
 SG_RED_BF16 = 16                                           # + r: roc_sg_launch.red of reduction r's bf16 form
+SG_RED_DROP = 32                                           # + r: the main kernel of reduction r with (edge) dropout
 HOST_DTYPES = ("float32", "bfloat16", "int32")             # ROC_HOST_DTYPE_* by value
 LINEAR_BWD_ONLY_DX, LINEAR_BWD_ONLY_DW = 1, 2
 GEMM_FWD, GEMM_DW, GEMM_DX = 0, 1, 2                       # `which` of roc_last_gemm_path / roc_last_gemm_info
@@ -139,6 +140,8 @@ PROTOTYPES = {
     "roc_sg_forward_planned": (i32, [vp, i32, vp, i64, vp, i64, i32, vp]),
     "roc_sg_forward_planned_bf16": (i32, [vp, i32, vp, i64, vp, i64, i32, vp]),
     "roc_sg_forward_teleport_planned": (i32, [vp, i32, vp, i64, f32, vp, i64, f32, vp, i64, i32, vp]),
+    "roc_sg_forward_dropout_planned": (i32, [vp, i32, vp, i64, vp, i64, i32, vp, f32, vp]),
+    "roc_sg_forward_teleport_dropout_planned": (i32, [vp, i32, vp, i64, f32, vp, i64, f32, vp, i64, i32, vp, f32, vp]),
     "roc_sg_minmax_forward_planned": (i32, [vp, i32, i32, vp, i64, vp, i64, vp, i64, vp]),
     "roc_sg_minmax_forward_planned_bf16": (i32, [vp, i32, i32, vp, i64, vp, i64, vp, i64, vp]),
     "roc_sg_minmax_backward_planned": (i32, [vp, i32, u32, vp, i64, vp, i64, vp, i64, vp]),
@@ -166,6 +169,7 @@ PROTOTYPES = {
     "roc_sg_transpose_destroy": (None, [vp]),
     "roc_sg_weighted_backward_planned": (i32, [vp, i32, vp, i64, vp, vp, i64, vp]),
     "roc_sg_transpose_sum_backward": (i32, [vp, i32, vp, i64, vp, i64, i32, vp, vp]),
+    "roc_sg_transpose_sum_backward_dropout": (i32, [vp, i32, vp, i64, vp, i64, i32, vp, vp, f32, vp]),
     "roc_sg_transpose_minmax_backward": (i32, [vp, i32, vp, i64, vp, i64, vp, i64, vp]),
     "roc_sg_attn_backward_exact": (i32, [vp, vp, i32, i32, f32, vp, i64, vp, i64, vp, i64, vp, i64, vp, i64, vp, i64,
                                          vp, i64, vp]),
@@ -252,6 +256,7 @@ PROTOTYPES = {
     "roc_host_scatter_gather_aggr": (i32, [vp, i32, i32]),
     "roc_host_attention_gather": (i32, [vp, i32, i32, i32, f32]),
     "roc_host_attention_gather_dropout": (i32, [vp, i32, i32, i32, f32, f32, i32]),
+    "roc_host_scatter_gather_dropout": (i32, [vp, i32, f32, i32]),
     "roc_host_get_aggr_index": (i32, [vp, i32, vp]),
     "roc_host_create_edge_tensor": (i32, [vp, i32]),
     "roc_host_scatter_gather_weighted": (i32, [vp, i32, i32]),

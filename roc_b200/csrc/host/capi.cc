@@ -95,6 +95,9 @@ int roc_host_scatter_gather_aggr(roc_host* h, int t, int aggr) {
   if (aggr < AGGR_AVG || aggr > AGGR_SUM) ROC_FATAL("roc_host_scatter_gather_aggr: bad AggrType");
   return h->push(h->m().scatter_gather(h->at(t), (AggrType)aggr));
 }
+int roc_host_scatter_gather_dropout(roc_host* h, int t, float rate, int seed) {
+  return h->push(h->m().scatter_gather(h->at(t), AGGR_SUM, rate, seed));
+}
 int roc_host_attention_gather(roc_host* h, int t, int scores, int heads, float slope) {
   return h->push(h->m().attention_gather(h->at(t), h->at(scores), heads, slope));
 }

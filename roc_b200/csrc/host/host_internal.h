@@ -100,6 +100,7 @@ struct RuntimeImpl {
   void* staging = nullptr; size_t stagingBytes = 0;       // H2D staging for dense host rows -> padded rows
   float* flatGrad = nullptr; size_t flatGradCount = 0;    // all dW, one all-reduce
   roc_sg_transpose* sgTranspose = nullptr;                // the graph's transpose: exact backward, weighted ops
+  uint8_t* sgKeep = nullptr;                              // [E] edge dropout's keep bytes, refilled by each dropped sum
   roc_perf_metrics* d_perf = nullptr;
   roc_perf_metrics h_perf{};
   roc_multilabel_metrics* d_multilabel = nullptr;   // what the sigmoid cross-entropy accumulates

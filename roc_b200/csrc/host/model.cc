@@ -142,6 +142,19 @@ Tensor Model::scatter_gather(const Tensor& _input, AggrType aggr) {
   ROC_FATAL("scatter_gather: unknown AggrType");
   return Tensor();
 }
+Tensor Model::scatter_gather(const Tensor& _input, AggrType aggr, float dropout, int seed) {
+  if (!(dropout >= 0.0f && dropout < 1.0f)) ROC_FATAL("scatter_gather: the edge dropout rate must be in [0, 1)");
+  if (dropout == 0.0f) return scatter_gather(_input, aggr);
+  if (aggr != AGGR_SUM) ROC_FATAL("scatter_gather: edge dropout goes with the sum aggregation only");
+  if (ctx->numParts > 1)
+    ROC_FATAL("scatter_gather: edge dropout runs on one partition only (numParts > 1 is not supported)");
+  ScatterGather* op = new ScatterGather(*this, _input);
+  op->dropRate = dropout;
+  op->seed = seed;
+  op->opIndex = (int)layers.size();
+  layers.push_back(op);
+  return op->outputs[0];
+}
 Tensor Model::attention_gather(const Tensor& input, const Tensor& scores, int heads, float negativeSlope, float dropout,
                                int seed) {
   if (ctx->numParts > 1)
@@ -645,7 +658,9 @@ static void choose_bf16_aggregation(RuntimeImpl* rt, const std::vector<GnnOp*>& 
     Linear* lin = as<Linear>(layers[l]);
     if (!lin || lin->activation != AC_MODE_NONE) continue;
     const int r = lin->fwdOut >= 0 ? lin->fwdOut : lin->outputs[0].region;
-    if (w.consumers[r] != 1 || !as_sum_sg(layers[w.consumerOp[r]])) continue;
+    // a sum with edge dropout has no bf16 form: it reads fp32
+    ScatterGather* sg = w.consumers[r] == 1 ? as_sum_sg(layers[w.consumerOp[r]]) : nullptr;
+    if (!sg || sg->dropRate > 0.0f) continue;
     make_bf16(rt, r);
   }
   // ... and what a Linear(NONE) or an unfused relu writes when a max / min, weighted or attention aggregation reads it
@@ -1049,7 +1064,7 @@ struct PushPipe {
 // -------------------------------------------------------- ScatterGather -----
 ScatterGather::ScatterGather(const Model& model, const Tensor& _input, AggrType _aggr)
     : GnnOp(_input), aggr(_aggr), arg(nullptr), argLd(0), epilogue(0), bwdEpilogue(0), fwdOut(-1), bwdOut(-1), teleT(-1),
-      teleAlpha(1.0f), teleBeta(1.0f) {
+      teleAlpha(1.0f), teleBeta(1.0f), dropRate(0.0f), seed(0), opIndex(0) {
   // scattergather.cc:33-37
   ROC_ASSERT(inputs[0].type == Tensor::NODE_TENSOR);
   ROC_ASSERT(inputs[0].numDim == 2);
@@ -1132,11 +1147,16 @@ void ScatterGather::forward(const Model& model) {
       xBf16 ? nullptr : gathered(model, rt->data(inputs[0].region), ldIn, H, &rt->t(inputs[0].region), false);
   rt->sg_end();
   float* dst = rt->data(outRegion);
+  const float rate = drop_rate(model);
+  const uint8_t* keep = rate > 0.0f ? keep_mask(model, model.myGraph.plan, model.myGraph.rowLeft, 0) : nullptr;
   rt->sg_begin(H);
   if (teleT >= 0)   // a fused scaled_add (fuse_teleport: one partition, fp32 input)
-    ROC_CHECK(roc_sg_forward_teleport_planned(model.myGraph.plan, H, src, ldIn, teleAlpha, rt->data(teleT),
-                                              rt->t(teleT).ld, teleBeta, dst, rt->t(outRegion).ld, epilogue,
-                                              rt->stream));
+    ROC_CHECK(roc_sg_forward_teleport_dropout_planned(model.myGraph.plan, H, src, ldIn, teleAlpha, rt->data(teleT),
+                                                      rt->t(teleT).ld, teleBeta, dst, rt->t(outRegion).ld, epilogue,
+                                                      keep, rate, rt->stream));
+  else if (rate > 0.0f)   // edge dropout: one partition, fp32 input
+    ROC_CHECK(roc_sg_forward_dropout_planned(model.myGraph.plan, H, src, ldIn, dst, rt->t(outRegion).ld, epilogue, keep,
+                                             rate, rt->stream));
   else if (xBf16)
     ROC_CHECK(roc_sg_forward_planned_bf16(model.myGraph.plan, H, rt->data_bf16(inputs[0].region), ldIn, dst,
                                           rt->t(outRegion).ld, epilogue, rt->stream));
@@ -1172,13 +1192,39 @@ void ScatterGather::backward(const Model& model) {
   const float* src = gathered(model, rt->grad(outputs[0].region), ld, H, &rt->t(outputs[0].region), true);
   rt->sg_end();
   float* dst = rt->grad(dstRegion);
+  // edge dropout: the keep bytes of the pairs this pass weighs, (w <- u) for row u's edge to w, in the order of the
+  // plan it runs over (the same CSR's reverse pairs, or the transposed plan's)
+  const float rate = drop_rate(model);
+  const uint8_t* keep = nullptr;
+  if (rate > 0.0f) {
+    const roc_sg_plan* planT = nullptr;
+    if (model.exactBackward) ROC_CHECK(roc_sg_transpose_info(rt->sgTranspose, nullptr, nullptr, nullptr, &planT));
+    keep = keep_mask(model, model.exactBackward ? planT : model.myGraph.plan,
+                     model.exactBackward ? 0 : model.myGraph.rowLeft, 1);
+  }
   rt->sg_begin(H);
   if (model.exactBackward)
-    ROC_CHECK(roc_sg_transpose_sum_backward(rt->sgTranspose, H, src, ld, dst, rt->t(dstRegion).ld, bwdEpilogue,
-                                            model.myGraph.d_rowEnd, rt->stream));
+    ROC_CHECK(roc_sg_transpose_sum_backward_dropout(rt->sgTranspose, H, src, ld, dst, rt->t(dstRegion).ld, bwdEpilogue,
+                                                    model.myGraph.d_rowEnd, keep, rate, rt->stream));
   else
-    ROC_CHECK(roc_sg_forward_planned(model.myGraph.plan, H, src, ld, dst, rt->t(dstRegion).ld, bwdEpilogue, rt->stream));
+    ROC_CHECK(roc_sg_forward_dropout_planned(model.myGraph.plan, H, src, ld, dst, rt->t(dstRegion).ld, bwdEpilogue, keep,
+                                             rate, rt->stream));
   rt->sg_end();
+}
+
+// edge dropout's rate in the current mode (infer: none)
+float ScatterGather::drop_rate(const Model& model) const { return model.mode == MD_MODE_TRAIN ? dropRate : 0.0f; }
+
+// The keep bytes of every edge of `plan` for this op's key and the current step, in the runtime's one E-byte buffer
+// (allocated on first use): each dropped sum fills it right before the kernel that reads it, so the ops and the
+// forward / backward passes share it.
+const uint8_t* ScatterGather::keep_mask(const Model& model, const roc_sg_plan* plan, roc_vid_t selfBase,
+                                        int rowIsSource) const {
+  RuntimeImpl* rt = model.ctx;
+  if (!rt->sgKeep) rt->sgKeep = (uint8_t*)rt->dmalloc(std::max<size_t>((size_t)model.myGraph.numEdges, 16));
+  const uint64_t key = ((uint64_t)(uint32_t)seed << 32) | (uint32_t)opIndex;
+  ROC_CHECK(roc_sg_attn_keep_mask(plan, selfBase, rowIsSource, dropRate, key, rt->trainStep, rt->sgKeep, rt->stream));
+  return rt->sgKeep;
 }
 
 // An op whose kernel overwrites an input gradient writes it into the gradient itself when `direct`, else into

@@ -50,6 +50,10 @@
 //  * the teleport sum (roc_sg_forward_teleport_planned, APPNP / GCNII's hop) is TELE: SUM's row of the table, column
 //    blocks and sum fix-ups, with a row store (tele_store) that also reads the row of t and applies
 //    post(fmaf(alpha, pre(sum), beta * t)) wherever a row is finally stored.  It runs every width on sg_chunk_kernel.
+//  * edge dropout (roc_sg_forward_dropout_planned, roc_sg_forward_teleport_dropout_planned,
+//    roc_sg_transpose_sum_backward_dropout) is SG_RED_DROP on SUM, TELE and TSUM: the keep bytes attention dropout
+//    uses, bit 0 per edge, loaded beside the source ids; a dropped edge's row is not gathered, a kept one is added as
+//    fmaf(s, x, acc).  Every width runs on sg_chunk_kernel, with the sum's column blocks and fix-ups.
 //
 // Algorithmic bytes per launch (DESIGN.md): E*(4H+4) + Nloc*(4H+8); min / max forward E*(4H+4) + Nloc*(8H+8),
 // backward E*(8H+4) + Nloc*(4H+8); the sum over bf16 rows E*(2H+4) + Nloc*(4H+8); weighted forward E*(4H+8) + Nloc*(4H+8), edge dot E*(4H+8) + Nloc*4H; attention
@@ -271,6 +275,11 @@ constexpr int SG_RED_BF16 = 16;
 // (roc_sg_attn_*_dropout): it loads each edge's keep byte (p.keep) beside its source id, the way WSUM loads its weight,
 // and weighs a dropped head's term by 0 and a kept one's by p.keepScale; everything else, its row of SG_REDS included,
 // is the pass without dropout's.
+// SG_RED_DROP added to SUM, TSUM or TELE is that sum with edge dropout (roc_sg_forward_dropout_planned,
+// roc_sg_transpose_sum_backward_dropout, roc_sg_forward_teleport_dropout_planned): it loads each edge's keep byte the
+// same way, gathers the source row only where bit 0 is set and adds it as fmaf(p.dropScale, x, acc); a dropped edge's
+// row is never loaded.  Its column blocks, row shapes, fix-ups and row store are the sum's, but every width runs on
+// sg_chunk_kernel (no ring form).
 constexpr int SG_RED_DROP = 32;
 __host__ __device__ constexpr int sg_red_base(int RF) { return RF & (SG_RED_BF16 - 1); }
 // the rows gathered as `in` are bf16 (every bf16 form but ASRC's, which gathers fp32 gradients)
@@ -409,7 +418,12 @@ struct SgParams {
   float* out2;          // ASTAT: unused; ADST / ASRC: heads-wide output [nloc][ldOut2];  EDOT: [E] dw of each local edge
   float* carry2;        // [numCarries][SG_LDC2] heads-wide partials (ASTAT: m | Z)
   size_t ldS, ldStats, ldX, ldOut2;
-  uint32_t heads, ftShift, H;   // ftShift: log2 of the T-columns per head (31 for one head); EDOT: H floats per row
+  uint32_t heads;
+  union {
+    uint32_t ftShift;   // log2 of the T-columns per head (31 for one head)
+    float dropScale;    // edge dropout (SG_RED_DROP on SUM, TSUM, TELE): the scale of a kept row
+  };
+  uint32_t H;           // EDOT, TELE: H floats per row
   float slope;
 };
 constexpr int SG_LDC2 = 16;     // 2 * the most heads
@@ -505,8 +519,11 @@ sg_chunk_kernel(const SgParams p) {
   constexpr bool MK = RED == SG_RED_MASK || RED == SG_RED_TMASK; // gathers an index row beside each gradient row
   constexpr bool BX = (RF & SG_RED_BF16) && RED == SG_RED_ASRC;  // its own row X[i] (xrow) is bf16
   constexpr bool BF = sg_bf16_in(RF);                            // gathers bf16 rows
-  constexpr bool DR = (RF & SG_RED_DROP) != 0;                   // attention dropout: loads each edge's keep byte
-  static_assert(!DR || RED == SG_RED_ATTN || RED == SG_RED_ADST || RED == SG_RED_ASRC, "dropout of an attention gather");
+  constexpr bool DR = (RF & SG_RED_DROP) != 0;                   // attention or edge dropout: loads each edge's keep byte
+  constexpr bool DS = DR && (RED == SG_RED_SUM || RED == SG_RED_TSUM || RED == SG_RED_TELE);   // edge dropout of a sum
+  static_assert(!DR || DS || RED == SG_RED_ATTN || RED == SG_RED_ADST || RED == SG_RED_ASRC,
+                "dropout of an attention gather or a sum");
+  static_assert(!DR || !(RF & SG_RED_BF16) || !DS, "no edge dropout over bf16 rows");
   constexpr uint32_t TB = BF ? 2 * VEC : sizeof(T);              // bytes of one T-column of `in`
   constexpr int WPB = SG_THREADS / L;
   constexpr uint32_t CH = SG_CH;
@@ -761,6 +778,8 @@ sg_chunk_kernel(const SgParams p) {
 #pragma unroll
       for (int ch = 0; ch < NCH; ch++) {
         if constexpr (BF) v[u][ch] = ld_bf16<VEC>(inl[ch] + off);
+        else if constexpr (DS)   // edge dropout: a dropped edge's row is not loaded, and adds fmaf(s, 0, acc) == acc
+          v[u][ch] = (kb[u] & 1u) ? V<VEC>::ld(reinterpret_cast<const T*>(inl[ch] + off)) : V<VEC>::zero();
         else v[u][ch] = V<VEC>::ld(reinterpret_cast<const T*>(inl[ch] + off));
       }
       if constexpr (MK) {
@@ -856,7 +875,8 @@ sg_chunk_kernel(const SgParams p) {
             } else {
 #pragma unroll
               for (int ch = 0; ch < NCH; ch++) {
-                if constexpr (RED == SG_RED_SUM || RED == SG_RED_TSUM || RED == SG_RED_BSUM || RED == SG_RED_TELE)
+                if constexpr (DS) V<VEC>::fma(acc[ch], p.dropScale, v[u][ch]);
+                else if constexpr (RED == SG_RED_SUM || RED == SG_RED_TSUM || RED == SG_RED_BSUM || RED == SG_RED_TELE)
                   V<VEC>::add(acc[ch], v[u][ch]);
                 else if constexpr (RED == SG_RED_MASK) mask_add(acc[ch], v[u][ch], av[u][ch], p.selfBase + cur);
                 else mm_add<RED>(acc[ch], aidx[ch], v[u][ch], srcs[u]);
@@ -1468,7 +1488,12 @@ constexpr const SgRed& sg_red(int RF) { return SG_REDS[sg_red_base(RF)]; }
 constexpr int sg_max_q(int VEC, int RED) { return VEC == 4 ? sg_red(RED).maxQ4 : sg_red(RED).maxQ1; }
 constexpr int sg_nch_index(int NCH) { return NCH == 1 ? 0 : NCH == 2 ? 1 : NCH == 4 ? 2 : 3; }
 constexpr int sg_chunk_u(int RED, int L, int NCH) { return L == 4 ? sg_red(RED).u4 : sg_red(RED).u[sg_nch_index(NCH)]; }
-constexpr int sg_chunk_minb(int RED, int NCH) { return sg_red(RED).minb[sg_nch_index(NCH)]; }
+// The dropped sums (SG_RED_DROP on SUM, TSUM and TELE) take their sum's row, holding U keep bytes beside the gathered
+// rows.  On float4 rows at eight chunks per lane that pushes TELE's, whose store also holds a row of t, past two CTAs'
+// registers: it runs one CTA per SM there rather than spill.
+constexpr int sg_chunk_minb(int VEC, int RED, int NCH) {
+  return (VEC == 4 && RED == (SG_RED_TELE | SG_RED_DROP) && NCH == 8) ? 1 : sg_red(RED).minb[sg_nch_index(NCH)];
+}
 
 // sg_chunk_kernel_t's two shapes, the measured defaults (DESIGN.md §3.1), four workers per CTA: rows of 65..128 floats
 // (one float4 per lane) with lane-held ids and two stages of two four-row units per worker; rows of 129..256 floats
@@ -1535,11 +1560,11 @@ static int launch(const SgParams& p, cudaStream_t st) {
   constexpr int WPB = SG_THREADS / L;
   int rc = ROC_OK;
   if (p.numChunks) {
-    if constexpr (VEC == 4 && R.ring >= 0 && L == 32 && NCH <= 2) {
+    if constexpr (VEC == 4 && R.ring >= 0 && !(RED & SG_RED_DROP) && L == 32 && NCH <= 2) {
       if ((rc = launch_ring<NCH, RED>(p, st)) != ROC_OK) return rc;
     } else {
       const uint32_t grid = (p.numChunks + WPB - 1) / WPB;
-      sg_chunk_kernel<VEC, L, NCH, sg_chunk_u(RED, L, NCH), sg_chunk_minb(RED, NCH), RED><<<grid, SG_THREADS, 0, st>>>(p);
+      sg_chunk_kernel<VEC, L, NCH, sg_chunk_u(RED, L, NCH), sg_chunk_minb(VEC, RED, NCH), RED><<<grid, SG_THREADS, 0, st>>>(p);
       ROC_LAUNCH_CHECK();
       note_launch(ROC_SG_LAUNCH_MAIN, RED, VEC, L, NCH, grid);
     }
@@ -1848,6 +1873,8 @@ struct SgEdge {
   const float* t = nullptr;
   int64_t ldT = 0;
   float alpha = 1.f, beta = 1.f;
+  const uint8_t* keep = nullptr;   // edge dropout (SG_RED_DROP): one keep byte per edge of the plan, and a kept row's scale
+  float dropScale = 1.f;
 };
 
 // Reduction RED over the columns [0, H) of every row, in column blocks of the widest row one launch takes (SG_REDS),
@@ -1878,6 +1905,7 @@ static int run_planned(roc_sg_plan* pl, int H, const void* in, int64_t ldIn, flo
     if (ed.g) { p.xrow = ed.g + c0; p.ldX = (size_t)ed.ldG; }
     if (ed.rowEnd) p.xrow = ed.rowEnd;
     if (ed.t) { p.xrow = ed.t + c0; p.ldS = (size_t)ed.ldT; p.slope = ed.alpha; p.teleBeta = ed.beta; }
+    if (ed.keep) { p.keep = ed.keep; p.dropScale = ed.dropScale; }
     p.H = (uint32_t)std::min(H - c0, blockCols);
     t_units(p, vec ? 4 : 1, std::min(H - c0, blockCols));
     rc = vec ? dispatch<4, RED>(p, st) : dispatch<1, RED>(p, st);
@@ -2012,8 +2040,8 @@ static int dispatch_attn(const SgParams& p, bool vec, bool drop, cudaStream_t st
   return vec ? dispatch<4, RF>(p, st) : dispatch<1, RF>(p, st);
 }
 
-// Attention dropout's arguments: ROC_ERR_INVALID for a rate outside [0, 1); *drop when there is a mask and rate > 0
-// (rate 0 or no mask: the calls without dropout).  The scale is roc_dropout_fwd's.
+// Attention and edge dropout's arguments: ROC_ERR_INVALID for a rate outside [0, 1); *drop when there is a mask and
+// rate > 0 (rate 0 or no mask: the calls without dropout).  The scale is roc_dropout_fwd's.
 static int attn_drop_args(const void* keep, float rate, bool* drop, float* scale) {
   if (!(rate >= 0.f && rate < 1.f)) return ROC_ERR_INVALID;
   *drop = keep != nullptr && rate > 0.f;
@@ -2430,6 +2458,63 @@ extern "C" int roc_sg_transpose_sum_backward(roc_sg_transpose* tr, int H, const 
   SgEdge ed;
   ed.rowEnd = rowEnd;
   return run_planned<SG_RED_TSUM>(tr->planT, H, outGrad, ldG, inGrad, ldIn, nullptr, 0, epilogue, 0, st, ed);
+}
+
+// ------------------------------------------------------------ edge dropout ---
+// The sums above with edge dropout (SG_RED_DROP): each checks its arguments as its plain call does, plus the rate
+// (attn_drop_args: rate 0 or no mask runs the plain call itself).
+extern "C" int roc_sg_forward_dropout_planned(const roc_sg_plan* plc, int H, const float* in, int64_t ldIn, float* out,
+                                              int64_t ldOut, int epilogue, const uint8_t* keep, float rate,
+                                              roc_stream_t stream) {
+  roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  clear_launches();
+  bool drop = false;
+  SgEdge ed;
+  if (attn_drop_args(keep, rate, &drop, &ed.dropScale) != ROC_OK) return ROC_ERR_INVALID;
+  if (!drop) return roc_sg_forward_planned(plc, H, in, ldIn, out, ldOut, epilogue, stream);
+  if (!pl || H <= 0 || !in || !out || ldIn < H || ldOut < H) return ROC_ERR_INVALID;
+  ed.keep = keep;
+  return run_planned<SG_RED_SUM | SG_RED_DROP>(pl, H, in, ldIn, out, ldOut, nullptr, 0, epilogue, 0, as_stream(stream),
+                                               ed);
+}
+
+extern "C" int roc_sg_forward_teleport_dropout_planned(const roc_sg_plan* plc, int H, const float* in, int64_t ldIn,
+                                                       float alpha, const float* t, int64_t ldT, float beta, float* out,
+                                                       int64_t ldOut, int epilogue, const uint8_t* keep, float rate,
+                                                       roc_stream_t stream) {
+  roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  clear_launches();
+  bool drop = false;
+  SgEdge ed;
+  if (attn_drop_args(keep, rate, &drop, &ed.dropScale) != ROC_OK) return ROC_ERR_INVALID;
+  if (!drop)
+    return roc_sg_forward_teleport_planned(plc, H, in, ldIn, alpha, t, ldT, beta, out, ldOut, epilogue, stream);
+  if (!pl || H <= 0 || !in || !t || !out || out == t || ldIn < H || ldT < H || ldOut < H ||
+      (epilogue & ~(ROC_SG_EPI_NORM | ROC_SG_EPI_NORM_OUT)) || !std::isfinite(alpha) || !std::isfinite(beta))
+    return ROC_ERR_INVALID;
+  ed.t = t; ed.ldT = ldT; ed.alpha = alpha; ed.beta = beta; ed.keep = keep;
+  return run_planned<SG_RED_TELE | SG_RED_DROP>(pl, H, in, ldIn, out, ldOut, nullptr, 0, epilogue, 0,
+                                                as_stream(stream), ed);
+}
+
+extern "C" int roc_sg_transpose_sum_backward_dropout(roc_sg_transpose* tr, int H, const float* outGrad, int64_t ldG,
+                                                     float* inGrad, int64_t ldIn, int epilogue, const roc_eid_t* rowEnd,
+                                                     const uint8_t* keep, float rate, roc_stream_t stream) {
+  clear_launches();
+  bool drop = false;
+  SgEdge ed;
+  if (attn_drop_args(keep, rate, &drop, &ed.dropScale) != ROC_OK) return ROC_ERR_INVALID;
+  if (!drop) return roc_sg_transpose_sum_backward(tr, H, outGrad, ldG, inGrad, ldIn, epilogue, rowEnd, stream);
+  if (!tr || H <= 0 || !outGrad || !inGrad || ldG < H || ldIn < H || ((epilogue & ROC_SG_EPI_NORM) && !rowEnd))
+    return ROC_ERR_INVALID;
+  cudaStream_t st = as_stream(stream);
+  ed.keep = keep;
+  if (!(epilogue & ROC_SG_EPI_NORM))
+    return run_planned<SG_RED_SUM | SG_RED_DROP>(tr->planT, H, outGrad, ldG, inGrad, ldIn, nullptr, 0, epilogue, 0, st,
+                                                 ed);
+  ed.rowEnd = rowEnd;
+  return run_planned<SG_RED_TSUM | SG_RED_DROP>(tr->planT, H, outGrad, ldG, inGrad, ldIn, nullptr, 0, epilogue, 0, st,
+                                                ed);
 }
 
 extern "C" int roc_sg_transpose_minmax_backward(roc_sg_transpose* tr, int H, const float* outGrad, int64_t ldG,

@@ -95,6 +95,26 @@ class SgPlan:
               "roc_sg_forward_teleport_planned")
         return out
 
+    def forward_dropout(self, x, keep, rate, out=None, epilogue=0):
+        """roc_sg_forward_dropout_planned: forward() with edge dropout, each kept edge's row added as fmaf(s, x, acc),
+        s = 1 / (1 - rate) in fp32, and a dropped edge's row never read.  keep: bit 0 of attn_keep_mask()'s bytes
+        (row_is_source=False for the forward, True for the backward over the same CSR); keep=None or rate=0 is
+        forward()."""
+        out = self._rows(x) if out is None else out
+        check(lib.roc_sg_forward_dropout_planned(self.handle, x.shape[1], _ptr(x), _ld(x), _ptr(out), _ld(out),
+                                                 int(epilogue), _ptr(keep), float(rate), _stream()),
+              "roc_sg_forward_dropout_planned")
+        return out
+
+    def teleport_forward_dropout(self, x, t, alpha, beta, keep, rate, epilogue=0, out=None):
+        """roc_sg_forward_teleport_dropout_planned: teleport_forward() over forward_dropout()'s sum."""
+        out = self._rows(x) if out is None else out
+        check(lib.roc_sg_forward_teleport_dropout_planned(self.handle, x.shape[1], _ptr(x), _ld(x), float(alpha),
+                                                          _ptr(t), _ld(t), float(beta), _ptr(out), _ld(out),
+                                                          int(epilogue), _ptr(keep), float(rate), _stream()),
+              "roc_sg_forward_teleport_dropout_planned")
+        return out
+
     def rows_sorted(self):
         """True if every row's sources are strictly increasing (no duplicate edges)."""
         ok = C.c_int()
@@ -316,6 +336,16 @@ class SgTranspose:
             out = self._rows(gy)
         check(lib.roc_sg_transpose_sum_backward(self.handle, h, _ptr(gy), _ld(gy), _ptr(out), _ld(out), int(epilogue),
                                                 _ptr(row_end), _stream()), "roc_sg_transpose_sum_backward")
+        return out
+
+    def sum_backward_dropout(self, gy, keep, rate, epilogue=0, row_end=None, out=None):
+        """roc_sg_transpose_sum_backward_dropout: sum_backward() over the kept edges, each added as fmaf(s, gy, acc);
+        keep in the transposed plan's edge order (attn_keep_mask()).  keep=None or rate=0 is sum_backward()."""
+        out = self._rows(gy) if out is None else out
+        check(lib.roc_sg_transpose_sum_backward_dropout(self.handle, gy.shape[1], _ptr(gy), _ld(gy), _ptr(out),
+                                                        _ld(out), int(epilogue), _ptr(row_end), _ptr(keep),
+                                                        float(rate), _stream()),
+              "roc_sg_transpose_sum_backward_dropout")
         return out
 
     def minmax_backward(self, gy, arg, out=None):

@@ -116,10 +116,20 @@ class Model:
         that read it.  Call before init() when the weighted op's input has no gradient of its own."""
         check(lib.roc_host_set_edge_grad(self.h, edges, int(bool(on))))
 
-    def scatter_gather(self, t, aggr=_lib.AGGR_SUM, weights=None):
+    def scatter_gather(self, t, aggr=_lib.AGGR_SUM, weights=None, dropout=0.0, seed=0):
         """aggr: AGGR_SUM (the reference's op), AGGR_AVG (sum -> indegree_norm -> indegree_norm), AGGR_MAX / AGGR_MIN
         (per feature over the in-neighbours; one partition only).  weights: an edge tensor (create_edge_tensor) for
-        the edge-weighted sum over each row's in-edges, whose backward is exact on any graph (one partition only)."""
+        the edge-weighted sum over each row's in-edges, whose backward is exact on any graph (one partition only).
+        dropout: edge dropout of the sum in train mode (one partition only): each in-edge kept with probability
+        1 - dropout and scaled by 1 / (1 - dropout), the mask drawn anew every step from `seed` and the op's position
+        (include/roc_b200.h, roc_sg_forward_dropout_planned).  Degrees stay the full graph's: dropout on the normalised
+        adjacency entries as in PyG's APPNP, not DropEdge's renormalisation.  A rate outside [0, 1), or dropout with
+        weights or another aggregator than AGGR_SUM, raises ValueError."""
+        _check_rate(dropout, "dropout")
+        if dropout != 0 and (weights is not None or aggr != _lib.AGGR_SUM):
+            raise ValueError("edge dropout goes with the unweighted sum aggregation only")
+        if dropout != 0:
+            return lib.roc_host_scatter_gather_dropout(self.h, t, float(dropout), int(seed))
         if weights is not None:
             assert aggr == _lib.AGGR_SUM, "edge weights go with the sum"
             return lib.roc_host_scatter_gather_weighted(self.h, t, weights)
@@ -437,6 +447,13 @@ def _check_rate(rate, name):
         raise ValueError("%s must be in [0, 1)" % name)
 
 
+def _sum_gather(model, t, edge_dropout):
+    """The sum scatter_gather of a builder, with edge dropout when edge_dropout > 0 (else the plain call)."""
+    if edge_dropout:
+        return model.scatter_gather(t, dropout=float(edge_dropout))
+    return model.scatter_gather(t)
+
+
 def _hidden_norm(model, norm, t, bns):
     """norm="batch": batch_norm on a hidden layer's output, right before its relu; None leaves t as it is."""
     if norm is None:
@@ -447,7 +464,7 @@ def _hidden_norm(model, norm, t, bns):
 
 
 def build_gcn(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exact_backward=False, features="float32",
-              aggregation="float32", loss="softmax", norm=None):
+              aggregation="float32", loss="softmax", norm=None, edge_dropout=0.0):
     """The model script of gnn.cc:65-98 for `-layers a-b-...-c`.  Returns the handles.  exact_backward: train on the
     exact gradient over the graph's transpose (Model.set_exact_backward), for directed graphs; the same keyword on
     build_sage_mean, build_sage_pool and build_gat.  features="bfloat16" keeps the input features in bf16
@@ -457,8 +474,12 @@ def build_gcn(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exact_bac
     (labels then go in with Model.set_multilabels); the same keyword on every builder.  norm="batch" puts a
     batch_norm (Model.batch_norm) on every hidden layer's output right before its relu (here after the second
     indegree_norm, and before the residual add), never on the last layer; the same keyword on every builder, which
-    then returns the batch_norm outputs as `bns`."""
+    then returns the batch_norm outputs as `bns`.  edge_dropout > 0 drops each layer's in-edges at that rate in
+    train mode (Model.scatter_gather(dropout=)), a fresh mask per layer and step, with the degrees of the full graph
+    (DropEdge's regulariser on the normalised adjacency, without its renormalisation); a rate outside [0, 1) raises
+    ValueError, and 0 builds the model without it."""
     _check_norm(norm)
+    _check_rate(edge_dropout, "edge_dropout")
     L = len(layers)
     x = _input_tensor(model, layers[0], features)
     label = model.create_node_tensor(layers[-1])
@@ -470,7 +491,7 @@ def build_gcn(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exact_bac
         skip = t
         t = model.linear(t, layers[i], _lib.AC_MODE_NONE)
         t = model.indegree_norm(t)
-        t = model.scatter_gather(t)
+        t = _sum_gather(model, t, edge_dropout)
         t = model.indegree_norm(t)
         if i != L - 1:
             t = model.relu(_hidden_norm(model, norm, t, bns))
@@ -693,7 +714,7 @@ def fp32(x):
 
 
 def build_appnp(model, layers, dropout_rate, K=10, alpha=0.1, lr=0.01, weight_decay=0.05, exact_backward=False,
-                features="float32", loss="softmax"):
+                features="float32", loss="softmax", edge_dropout=0.0):
     """APPNP (Klicpera et al., 2019), PyG's APPNP after an MLP:
 
         h = MLP(x)                     # per layer: dropout -> linear -> relu, no relu on the last layer
@@ -703,14 +724,18 @@ def build_appnp(model, layers, dropout_rate, K=10, alpha=0.1, lr=0.01, weight_de
 
     i.e. z' = (1 - alpha) D^-1/2 A D^-1/2 z + alpha h with the self loops already in A.  The coefficients are computed
     in double and rounded to fp32 once (fp32()).  With fusion on, each hop's scaled_add is fused into its
-    scatter_gather's store, and so is the next hop's first indegree_norm (Model.init).  No edge dropout, one partition
-    for the fusion.  Bad K or alpha raises ValueError.  Returns the handles, with `h` (the MLP output), `hops` (each
+    scatter_gather's store, and so is the next hop's first indegree_norm (Model.init); one partition for the fusion.
+    edge_dropout > 0 is the paper's (and PyG APPNP(dropout=)'s) dropout of the propagation matrix: every hop's
+    scatter_gather drops its in-edges at that rate in train mode (Model.scatter_gather(dropout=)), each hop and step
+    drawing its own mask, with the degrees of the full graph; the fusions still apply.  0 builds the model without it.
+    Bad K, alpha or edge_dropout raises ValueError.  Returns the handles, with `h` (the MLP output), `hops` (each
     hop's z) and `coefficients` (the fp32 pair (1 - alpha, alpha)).  With fusion on, a hop's z before the last is never
     written (its scatter_gather stores the next hop's normalised z instead), so only the last, the logits, can be read
     after a forward; set_fusion(False) writes every hop's z."""
     _check_count(K, "K")
     _check_alpha(alpha)
     _check_rate(dropout_rate, "dropout_rate")
+    _check_rate(edge_dropout, "edge_dropout")
     c = (fp32(1.0 - float(alpha)), fp32(float(alpha)))
     L = len(layers)
     x = _input_tensor(model, layers[0], features)
@@ -724,7 +749,7 @@ def build_appnp(model, layers, dropout_rate, K=10, alpha=0.1, lr=0.01, weight_de
     h = z = t
     hops = []
     for _ in range(int(K)):
-        z = model.indegree_norm(model.scatter_gather(model.indegree_norm(z)))
+        z = model.indegree_norm(_sum_gather(model, model.indegree_norm(z), edge_dropout))
         z = model.scaled_add(z, h, c[0], c[1])
         hops.append(z)
     _loss(model, loss, z, label, mask)

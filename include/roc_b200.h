@@ -307,6 +307,53 @@ int roc_sg_attn_backward_dropout_planned_bf16(const roc_sg_plan* plan, int heads
 int roc_sg_attn_keep_mask(const roc_sg_plan* plan, roc_vid_t selfBase, int rowIsSource, float rate, uint64_t seed,
                           uint32_t step, uint8_t* keep, roc_stream_t stream);
 
+/* Dynamic attention (GATv2: Brody et al., "How Attentive are Graph Attention Networks?", PyG GATv2Conv without bias,
+ * edge features or head averaging).  xl holds the source (value) rows and xr the target rows, H = heads * F columns,
+ * 1 <= H <= 256, heads <= 8; `a` holds the attention vector of each head, a[k][f] at a[f * heads + k] (F x heads
+ * floats: the memory of a Model parameter of parameter_shape (heads, F)).  The plan covers a whole graph: every id in
+ * colSrc is one of its rows, which index xl, xr and every other row operand.  For row v, each in-edge e from u =
+ * colSrc[e] (self loops are in the graph, duplicate edges count once each), head k and l(z) = LeakyReLU(z) (z > 0 ? z :
+ * slope * z; l'(z) = z > 0 ? 1 : slope, as torch):
+ *   z[v,u][c]  = xl[u][c] + xr[v][c]
+ *   e[v,u,k]   = sum_f a[k][f] * l(z[v,u][kF+f])
+ *   m[v][k]    = max_u e,  Z[v][k] = sum_u exp(e - m),  p[v,u,k] = exp(e - m) / Z
+ *   out[v][kF+f] = sum_u p[v,u,k] * xl[u][kF+f]           (accumulated as fmaf(p, xl, acc) from +0 in CSR order)
+ * stats[v] = m | 1/Z per head, as roc_sg_attn_forward_planned's (0 | 0 for a row of degree 0, whose out is 0).
+ * e is computed by one device function whose summation order depends on (H, heads) only: lane l of a warp holds
+ * columns l + 32 j; a head's terms are added in column order within each lane, then across the warp by an xor
+ * butterfly.  The forward and both backward passes therefore see the same bits for every e.
+ * Backward, from outGrad = gy and the forward's out and stats, with c[v][k] = gy[v]_k . out[v]_k (the record pass) and
+ * d[v,u,k] = p (gy[v]_k . xl[u]_k - c[v][k]):
+ *   dxr[v][c] = sum_u d[v,u,k] * a[k][f] * l'(z)          (the destination pass, over the plan)
+ *   R[v][c]   = sum_u d[v,u,k] * l(z)                     (the same pass; N x H floats of workspace of the call)
+ *   dxl[u][c] = sum over u's out-edges (v <- u) of p gy[v][c] + d a[k][f] l'(z)   (the source pass)
+ *   da[k][f]  = sum_v R[v][kF+f], in a's layout: fp64 sums over blocks of 512 rows, then the blocks in order
+ * roc_sg_attn_v2_backward_planned runs the source pass over the same CSR, reading row u's in-edges as its out-edges:
+ * exact on a symmetric graph, as roc_sg_attn_backward_planned.  roc_sg_attn_v2_backward_exact runs it over the
+ * transposed plan: exact on any graph, multigraphs included.  When xl and xr are one tensor, its gradient is dxl + dxr.
+ * No per-edge buffer: every pass recomputes e from the rows.  No atomics: every output is the same bits run to run and
+ * whatever the grid or the SMs available.  Every call overwrites its outputs; dxl and dxr are distinct buffers.
+ * ROC_ERR_INVALID: a NULL pointer, heads <= 0, H <= 0, a leading dimension < H (stats < 2 * heads), a bad slope, dxl ==
+ * dxr, and for the exact call a transpose of another graph.  ROC_ERR_UNSUPPORTED: H % heads != 0, H > 256, heads > 8,
+ * or a plan whose colSrc names an id outside its rows.  The first call on a plan finds its largest id (one
+ * synchronisation of the stream).  Launches (roc_sg_last_call_info): the main kernel reports reduction 64 (stats), 65
+ * (weighted sum), 66 (destination pass) and 67 (source pass), with lanes 32 and nch = ceil(H / 32); the stats fix-up
+ * and the sum's fix-ups of cut rows follow their pass (the destination pass: dxr's, then R's); the backward starts with
+ * a ROC_SG_LAUNCH_RECORD and ends with two ROC_SG_LAUNCH_COLSUM launches (da). */
+int roc_sg_attn_v2_forward_planned(const roc_sg_plan* plan, int heads, int H, float slope, const float* xl,
+                                   int64_t ldXl, const float* xr, int64_t ldXr, const float* a, float* out,
+                                   int64_t ldOut, float* stats, int64_t ldStats, roc_stream_t stream);
+int roc_sg_attn_v2_backward_planned(const roc_sg_plan* plan, int heads, int H, float slope, const float* xl,
+                                    int64_t ldXl, const float* xr, int64_t ldXr, const float* a, const float* out,
+                                    int64_t ldOut, const float* stats, int64_t ldStats, const float* outGrad,
+                                    int64_t ldG, float* dxl, int64_t ldDxl, float* dxr, int64_t ldDxr, float* da,
+                                    roc_stream_t stream);
+int roc_sg_attn_v2_backward_exact(const roc_sg_plan* plan, struct roc_sg_transpose* tr, int heads, int H, float slope,
+                                  const float* xl, int64_t ldXl, const float* xr, int64_t ldXr, const float* a,
+                                  const float* out, int64_t ldOut, const float* stats, int64_t ldStats,
+                                  const float* outGrad, int64_t ldG, float* dxl, int64_t ldDxl, float* dxr,
+                                  int64_t ldDxr, float* da, roc_stream_t stream);
+
 /* Edge dropout of the sum (the APPNP paper's dropout of the propagation matrix, PyG APPNP(dropout=); DropEdge, Rong et
  * al. 2020, applied to GCN).  keep(i<-j) is bit 0 of the byte roc_sg_attn_keep_mask writes for the pair (i <- j): lane 0
  * of Philox4x32-10 with counter {i, j, 0, step} and key {seed lo, seed hi}, against T16 = round(rate * 65536), the same
@@ -479,8 +526,9 @@ int roc_sg_backward(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft, in
  * to one list.  Each entry:
  *   kind   ROC_SG_LAUNCH_*: the main kernel, its cp.async.bulk ring form (float4 sums of 17..64 T-columns), the
  *          fix-up of rows with at most 32 carries (one worker each), of rows with more (one CTA each), the attention
- *          stats fix-up, the attention backward's per-node record, the fix-ups of its heads-wide partials, and the
- *          weighted backward's weight permutation (first in its list)
+ *          stats fix-up, the attention backward's per-node record, the fix-ups of its heads-wide partials, the
+ *          weighted backward's weight permutation (first in its list), the keep mask, and the dynamic attention
+ *          backward's column sums of da
  *   red    the reduction the kernel is instantiated for: 0 sum, 1 max, 2 min, 3 the min / max backward, 4 attention
  *          stats, 5 the attention forward, 6 its d s_dst gather, 7 its input-gradient gather, 8 the weighted sum
  *          (forward and backward), 9 the edge-weight gradient, 10 the exact sum backward with NORM (the sum whose
@@ -493,8 +541,9 @@ int roc_sg_backward(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft, in
  *          rows) with dropout (the roc_sg_attn_*_dropout_* calls at rate > 0: 37, 38, 39, 53, 54, 55), whose other
  *          launches report as without dropout; likewise 32, 42 and 45 for the sum, the exact sum backward with NORM
  *          and the teleport sum with edge dropout (roc_sg_forward_dropout_planned,
- *          roc_sg_transpose_sum_backward_dropout, roc_sg_forward_teleport_dropout_planned at rate > 0); -1 for the record, the permutation and the keep mask, which have
- *          none.  A sum fix-up finishing another
+ *          roc_sg_transpose_sum_backward_dropout, roc_sg_forward_teleport_dropout_planned at rate > 0); 64, 65, 66 and 67 for
+ *          the dynamic attention passes (roc_sg_attn_v2_*); -1 for the records, the permutation, the keep mask and
+ *          the column sums, which have none.  A sum fix-up finishing another
  *          reduction's partials reports 0.
  *   vec    4 for float4 rows, else 1;  lanes, nch: the row shape (L lanes, chunks per lane);  grid: CTAs launched
  * count is the number of launches; the first ROC_SG_MAX_LAUNCHES are stored.  Every planned call clears the list first,
@@ -509,6 +558,7 @@ int roc_sg_backward(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft, in
 #define ROC_SG_LAUNCH_HEADS_BIG_FIXUP 7
 #define ROC_SG_LAUNCH_PERMUTE 8
 #define ROC_SG_LAUNCH_KEEP_MASK 9     /* roc_sg_attn_keep_mask (red -1) */
+#define ROC_SG_LAUNCH_COLSUM 10       /* roc_sg_attn_v2_backward_*: da's fp64 column sums (red -1) */
 #define ROC_SG_MAX_LAUNCHES 32
 typedef struct {
   int kind, red, vec, lanes, nch;

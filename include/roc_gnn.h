@@ -211,6 +211,16 @@ public:
    * calls.  A rate outside [0, 1) exits. */
   Tensor attention_gather(const Tensor& input, const Tensor& scores, int heads, float negativeSlope = 0.2f,
                           float dropout = 0.0f, int seed = 0);
+  /* GATv2's dynamic attention (roc_sg_attn_v2_forward_planned): per destination v and head k over v's in-edges u,
+   *   e[v,u,k] = sum_f a[k][f] * LeakyReLU(xl[u][kF+f] + xr[v][kF+f]),  p = softmax_u(e),
+   *   out[v][kF:(k+1)F] = sum_u p[v,u,k] * xl[u][kF:(k+1)F]
+   * xl (the values) and xr (the targets) have H = heads * F columns, H <= 256, heads <= 8; they may be one tensor
+   * (PyG's share_weights), whose gradient then takes both parts.  Appends one parameter `a` of parameter_shape
+   * (heads, F), drawn by GlorotUniform (uniform in +-sqrt(6 / (heads + F)), PyG's glorot of GATv2Conv.att).  A mode of
+   * attention_gather: op_info reports it as one.  Its backward runs over the same CSR (exact on a symmetric graph), or
+   * over the transpose with set_exact_backward.  Never fused; set_bf16_aggregation leaves both inputs fp32.  Exits on
+   * different widths, H % heads != 0, H > 256, heads > 8, bf16 inputs, a bad slope, or more than one partition. */
+  Tensor dynamic_attention_gather(const Tensor& xl, const Tensor& xr, int heads, float negativeSlope = 0.2f);
   /* The per-head GAT scores of `input` (H = heads * F columns; roc_attn_scores_fwd / _bwd): a [rows][2 * heads] output
    * [s_dst | s_src], head k's scores the dot products of its own F columns with its a_dst and a_src.  Appends one
    * parameter A, a weight tensor of dims {F, 2 * heads} (row k: a_dst of head k, row heads + k: its a_src), drawn by the
@@ -376,6 +386,8 @@ class AttentionGather : public GnnOp {  /* not in the reference: Model::attentio
 public:
   AttentionGather(const Model& model, const Tensor& input, const Tensor& scores, int heads, float slope, float dropRate,
                   int seed);
+  /* the dynamic (GATv2) mode: inputs xl, xr (Model::dynamic_attention_gather) */
+  AttentionGather(const Model& model, const Tensor& xl, const Tensor& xr, int heads, float slope);
   virtual void init(const Model& model);
   virtual void forward(const Model& model);
   virtual void backward(const Model& model);
@@ -389,10 +401,13 @@ public:
   float* stats;      /* [Nloc][statsLd] m | 1/Z per head of the last forward (Runtime arena) */
   int64_t statsLd;
   float* scratch[2]; /* gradients of an input that accumulates (or needs none), written here first (Runtime arena) */
+  bool dynamic;      /* GATv2's dynamic attention: inputs[0] = xl, inputs[1] = xr, parameter a */
+  Tensor a;          /* dynamic: parameter, dims {heads, F} (memory a[k][f] at f * heads + k) */
 private:
   float drop_rate(const Model& model) const;
   uint64_t drop_key() const;
   void keep_mask(const Model& model, const roc_sg_plan* plan, roc_vid_t selfBase, int rowIsSource, uint8_t*& buf);
+  void dynamic_backward(const Model& model);
 };
 
 class AttentionScores : public GnnOp {  /* not in the reference: Model::attention_scores */

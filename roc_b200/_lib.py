@@ -56,7 +56,7 @@ SG_LAUNCH_MAIN, SG_LAUNCH_RING, SG_LAUNCH_FIXUP, SG_LAUNCH_BIG_FIXUP = 0, 1, 2, 
 SG_LAUNCH_STAT_FIXUP, SG_LAUNCH_RECORD, SG_LAUNCH_HEADS_FIXUP, SG_LAUNCH_HEADS_BIG_FIXUP = 4, 5, 6, 7
 SG_LAUNCH_PERMUTE, SG_LAUNCH_KEEP_MASK = 8, 9
 SG_LAUNCH_KINDS = ("main", "ring", "fixup", "big_fixup", "stat_fixup", "record", "heads_fixup", "heads_big_fixup",
-                   "permute", "keep_mask")
+                   "permute", "keep_mask", "colsum")
 SG_MAX_LAUNCHES = 32
 
 
@@ -164,6 +164,11 @@ PROTOTYPES = {
     "roc_sg_attn_backward_dropout_planned_bf16": (i32, [vp, i32, i32, f32, u32, vp, i64, vp, i64, vp, i64, vp, i64, vp,
                                                         i64, vp, i64, vp, i64, vp, vp, f32, vp]),
     "roc_sg_attn_keep_mask": (i32, [vp, u32, i32, f32, u64, u32, vp, vp]),
+    "roc_sg_attn_v2_forward_planned": (i32, [vp, i32, i32, f32, vp, i64, vp, i64, vp, vp, i64, vp, i64, vp]),
+    "roc_sg_attn_v2_backward_planned": (i32, [vp, i32, i32, f32, vp, i64, vp, i64, vp, vp, i64, vp, i64, vp, i64, vp,
+                                              i64, vp, i64, vp, vp]),
+    "roc_sg_attn_v2_backward_exact": (i32, [vp, vp, i32, i32, f32, vp, i64, vp, i64, vp, vp, i64, vp, i64, vp, i64,
+                                            vp, i64, vp, i64, vp, vp]),
     "roc_sg_transpose_create": (i32, [u32, vp, vp, vp, C.POINTER(vp)]),
     "roc_sg_transpose_info": (i32, [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]),
     "roc_sg_transpose_destroy": (None, [vp]),
@@ -255,6 +260,7 @@ PROTOTYPES = {
     "roc_host_scatter_gather": (i32, [vp, i32]),
     "roc_host_scatter_gather_aggr": (i32, [vp, i32, i32]),
     "roc_host_attention_gather": (i32, [vp, i32, i32, i32, f32]),
+    "roc_host_dynamic_attention_gather": (i32, [vp, i32, i32, i32, f32]),
     "roc_host_attention_gather_dropout": (i32, [vp, i32, i32, i32, f32, f32, i32]),
     "roc_host_scatter_gather_dropout": (i32, [vp, i32, f32, i32]),
     "roc_host_get_aggr_index": (i32, [vp, i32, vp]),

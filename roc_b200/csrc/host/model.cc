@@ -164,6 +164,15 @@ Tensor Model::attention_gather(const Tensor& input, const Tensor& scores, int he
   layers.push_back(op);
   return op->outputs[0];
 }
+Tensor Model::dynamic_attention_gather(const Tensor& xl, const Tensor& xr, int heads, float negativeSlope) {
+  if (ctx->numParts > 1)
+    ROC_FATAL("dynamic_attention_gather: runs on one partition only (numParts > 1 is not supported)");
+  AttentionGather* op = new AttentionGather(*this, xl, xr, heads, negativeSlope);
+  op->opIndex = (int)layers.size();
+  layers.push_back(op);
+  parameters.push_back(op->a);
+  return op->outputs[0];
+}
 Tensor Model::attention_scores(const Tensor& input, int heads) {
   if (ctx->numParts > 1)
     ROC_FATAL("attention_scores: runs on one partition only (numParts > 1 is not supported)");
@@ -355,7 +364,9 @@ static void mark_gradients(const Model& m) {
     bool any = false;
     for (int j = 0; j < op->numInputs; j++)
       if (op->inputs[j].region >= 0) any = any || rt->t(op->inputs[j].region).requiresGrad;
-    if (as<Linear>(op) || as<BatchNorm>(op) || as<AttentionScores>(op)) any = true;   // their own parameters
+    const AttentionGather* ag = as<AttentionGather>(op);
+    if (as<Linear>(op) || as<BatchNorm>(op) || as<AttentionScores>(op) || (ag && ag->dynamic))
+      any = true;   // their own parameters
     for (int j = 0; j < op->numOutputs; j++) {
       rt->t(op->outputs[j].region).requiresGrad = any;
       rt->t(op->outputs[j].region).produced = true;
@@ -679,7 +690,8 @@ static void choose_bf16_aggregation(RuntimeImpl* rt, const std::vector<GnnOp*>& 
         if (op->inputs[j].region != r) continue;
         ScatterGather* sg = as<ScatterGather>(op);
         Linear* lin = as<Linear>(op);
-        if (j == 0 && ((sg && sg->aggr != AGGR_SUM) || as<WeightedScatterGather>(op) || as<AttentionGather>(op)))
+        AttentionGather* ag = as<AttentionGather>(op);   // a dynamic one has no bf16 form: it reads fp32
+        if (j == 0 && ((sg && sg->aggr != AGGR_SUM) || as<WeightedScatterGather>(op) || (ag && !ag->dynamic)))
           aggregated = true;
         else if (!(j == 0 && ((lin && lin->dropOp < 0) || as<AttentionScores>(op))))
           others = false;
@@ -1247,7 +1259,7 @@ static void add_scratch(const Model& model, int region, const float* scratch) {
 AttentionGather::AttentionGather(const Model& model, const Tensor& _input, const Tensor& _scores, int _heads, float _slope,
                                  float _dropRate, int _seed)
     : GnnOp(_input, _scores), heads(_heads), slope(_slope), dropRate(_dropRate), seed(_seed), opIndex(0),
-      keep(nullptr), keep2(nullptr), stats(nullptr), statsLd(0) {
+      keep(nullptr), keep2(nullptr), stats(nullptr), statsLd(0), dynamic(false) {
   scratch[0] = scratch[1] = nullptr;
   ROC_ASSERT(_input.type == Tensor::NODE_TENSOR && _scores.type == Tensor::NODE_TENSOR);
   ROC_ASSERT(_input.numDim == 2 && _scores.numDim == 2);
@@ -1266,7 +1278,32 @@ AttentionGather::AttentionGather(const Model& model, const Tensor& _input, const
   numOutputs = 1;
   outputs[0] = model.create_node_tensor<DATATYPE>((int)_input.dims[0]);
 }
-void AttentionGather::init(const Model&) {}
+// The dynamic mode: xl and xr are the op's two inputs, one region twice when they are one tensor (the second then adds
+// its gradient through scratch, as any input another op already wrote).
+AttentionGather::AttentionGather(const Model& model, const Tensor& xl, const Tensor& xr, int _heads, float _slope)
+    : GnnOp(xl, xr), heads(_heads), slope(_slope), dropRate(0.0f), seed(0), opIndex(0), keep(nullptr), keep2(nullptr),
+      stats(nullptr), statsLd(0), dynamic(true) {
+  scratch[0] = scratch[1] = nullptr;
+  ROC_ASSERT(xl.type == Tensor::NODE_TENSOR && xr.type == Tensor::NODE_TENSOR);
+  ROC_ASSERT(xl.numDim == 2 && xr.numDim == 2);
+  ROC_ASSERT(xl.dims[1] == model.myGraph.numNodes && xr.dims[1] == model.myGraph.numNodes);
+  const int64_t H = (int64_t)xl.dims[0];
+  if (xr.dims[0] != xl.dims[0]) ROC_FATAL("dynamic_attention_gather: xl and xr must have the same width");
+  if (_heads <= 0 || _heads > 8 || H % _heads)
+    ROC_FATAL("dynamic_attention_gather: the width must be heads * F with 1 <= heads <= 8");
+  if (H > 256) ROC_FATAL("dynamic_attention_gather: the width must be at most 256");
+  if (!(_slope >= 0.0f) || !std::isfinite(_slope))
+    ROC_FATAL("dynamic_attention_gather: the negative slope must be finite and >= 0");
+  if (model.ctx->t(xl.region).isBf16 || model.ctx->t(xr.region).isBf16)
+    ROC_FATAL("dynamic_attention_gather: xl and xr must be fp32 (there is no bf16 form)");
+  a = model.create_weight_tensor(_heads, (int)(H / _heads), NULL);   // GlorotUniform: +-sqrt(6 / (heads + F))
+  numOutputs = 1;
+  outputs[0] = model.create_node_tensor<DATATYPE>((int)H);
+}
+void AttentionGather::init(const Model& model) {
+  if (dynamic && (model.ctx->t(inputs[0].region).isBf16 || model.ctx->t(inputs[1].region).isBf16))
+    ROC_FATAL("dynamic_attention_gather: xl and xr must be fp32 (there is no bf16 form)");
+}
 
 // the attention dropout rate in the current mode (infer: none) and its Philox key
 float AttentionGather::drop_rate(const Model& model) const { return model.mode == MD_MODE_TRAIN ? dropRate : 0.0f; }
@@ -1286,6 +1323,15 @@ void AttentionGather::forward(const Model& model) {
   if (!stats) {
     statsLd = round_up4(2 * heads);
     stats = (float*)rt->dmalloc((size_t)std::max<int64_t>(model.local_rows(), 1) * (size_t)statsLd * sizeof(float));
+  }
+  if (dynamic) {
+    const int xl = inputs[0].region, xr = inputs[1].region, y = outputs[0].region;
+    rt->sg_begin(H);
+    ROC_CHECK(roc_sg_attn_v2_forward_planned(model.myGraph.plan, heads, H, slope, rt->data(xl), rt->t(xl).ld,
+                                             rt->data(xr), rt->t(xr).ld, rt->data(a.region), rt->data(y), rt->t(y).ld,
+                                             stats, statsLd, rt->stream));
+    rt->sg_end();
+    return;
   }
   const int x = inputs[0].region, sc = inputs[1].region, y = outputs[0].region;
   const roc_sg_plan* plan = model.myGraph.plan;
@@ -1307,6 +1353,10 @@ void AttentionGather::forward(const Model& model) {
 
 void AttentionGather::backward(const Model& model) {
   RuntimeImpl* rt = model.ctx;
+  if (dynamic) {
+    dynamic_backward(model);
+    return;
+  }
   if (!rt->t(inputs[0].region).requiresGrad && !rt->t(inputs[1].region).requiresGrad) return;
   const int H = (int)inputs[0].dims[0];
   // The kernel overwrites both gradients.  An input whose gradient another op already wrote (the features feed the
@@ -1346,6 +1396,31 @@ void AttentionGather::backward(const Model& model) {
     ROC_CHECK(roc_sg_attn_backward_dropout_planned(plan, heads, H, slope, model.myGraph.rowLeft, rt->data(x), ldX,
                                                    rt->data(sc), ldS, rt->data(ox), ldO, stats, statsLd, rt->grad(ox),
                                                    ldO, dst[0], ldX, dst[1], ldS, k1, k2, rate, rt->stream));
+  rt->sg_end();
+  for (int i = 0; i < 2; i++)
+    if (rt->t(inputs[i].region).requiresGrad && !resetInputGrads[i]) add_scratch(model, inputs[i].region, scratch[i]);
+}
+
+// dxl, dxr and da (overwritten) from the same CSR, or over the transpose with the exact backward.  The kernels overwrite
+// both input gradients; an input whose gradient another op already wrote (or xr when it is xl) takes its part through
+// scratch, added afterwards.
+void AttentionGather::dynamic_backward(const Model& model) {
+  RuntimeImpl* rt = model.ctx;
+  const int H = (int)inputs[0].dims[0];
+  const int xl = inputs[0].region, xr = inputs[1].region, y = outputs[0].region;
+  float* dst[2];
+  for (int i = 0; i < 2; i++)
+    dst[i] = grad_or_scratch(model, inputs[i].region, rt->t(inputs[i].region).requiresGrad && resetInputGrads[i], scratch[i]);
+  const int64_t ld0 = rt->t(xl).ld, ld1 = rt->t(xr).ld, ldY = rt->t(y).ld;
+  rt->sg_begin(H);
+  if (model.exactBackward)
+    ROC_CHECK(roc_sg_attn_v2_backward_exact(model.myGraph.plan, rt->sgTranspose, heads, H, slope, rt->data(xl), ld0,
+                                            rt->data(xr), ld1, rt->data(a.region), rt->data(y), ldY, stats, statsLd,
+                                            rt->grad(y), ldY, dst[0], ld0, dst[1], ld1, rt->grad(a.region), rt->stream));
+  else
+    ROC_CHECK(roc_sg_attn_v2_backward_planned(model.myGraph.plan, heads, H, slope, rt->data(xl), ld0, rt->data(xr), ld1,
+                                              rt->data(a.region), rt->data(y), ldY, stats, statsLd, rt->grad(y), ldY,
+                                              dst[0], ld0, dst[1], ld1, rt->grad(a.region), rt->stream));
   rt->sg_end();
   for (int i = 0; i < 2; i++)
     if (rt->t(inputs[i].region).requiresGrad && !resetInputGrads[i]) add_scratch(model, inputs[i].region, scratch[i]);

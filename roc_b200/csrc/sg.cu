@@ -54,6 +54,8 @@
 //    roc_sg_transpose_sum_backward_dropout) is SG_RED_DROP on SUM, TELE and TSUM: the keep bytes attention dropout
 //    uses, bit 0 per edge, loaded beside the source ids; a dropped edge's row is not gathered, a kept one is added as
 //    fmaf(s, x, acc).  Every width runs on sg_chunk_kernel, with the sum's column blocks and fix-ups.
+//  * dynamic attention (roc_sg_attn_v2_*, GATv2) runs on its own kernel, sg_v2_kernel (end of file): one warp per
+//    chunk of the same plan, finished by the attention stats fix-up and the sum's fix-ups.
 //
 // Algorithmic bytes per launch (DESIGN.md): E*(4H+4) + Nloc*(4H+8); min / max forward E*(4H+4) + Nloc*(8H+8),
 // backward E*(8H+4) + Nloc*(4H+8); the sum over bf16 rows E*(2H+4) + Nloc*(4H+8); weighted forward E*(4H+8) + Nloc*(4H+8), edge dot E*(4H+8) + Nloc*4H; attention
@@ -2549,4 +2551,524 @@ extern "C" int roc_sg_last_call_info(roc_sg_call_info* info) {
   if (!info) return ROC_ERR_INVALID;
   *info = t_call;
   return ROC_OK;
+}
+
+// ------------------------------------------------- dynamic attention (GATv2) ---
+// roc_sg_attn_v2_*: GATv2's logit e(v<-u, k) = sum_f a[k][f] LeakyReLU(xl[u][kF+f] + xr[v][kF+f]) needs both endpoint
+// rows of every edge, so every pass recomputes it from the rows.  The passes run on their own kernel, sg_v2_kernel, over
+// the plan's chunks, chunk records and carry slots, and are finished by the attention stats fix-up and the sum's
+// fix-ups, as ASTAT and ATTN are.  One worker is a whole warp: lane l holds columns l + 32 j, j < J = ceil(H / 32), of
+// every row, scalar, so a head's F columns may start anywhere.  A per-head sum (v2_head_sums) adds the lane's columns of
+// the head in column order, then runs an xor butterfly over the warp; both depend on (H, heads) only, and every lane
+// ends with the same bits.  e is computed by v2_logits alone, with the products and sums rounded one by one, so the
+// forward and both backward passes see the same bits for every e (and the backward passes the same d).
+namespace roc {
+
+enum { SG_V2_STAT = 0, SG_V2_SUM = 1, SG_V2_DST = 2, SG_V2_SRC = 3 };
+constexpr int SG_RED_V2 = 64;                 // the `red` sg_last_call_info reports for pass P is SG_RED_V2 + P
+constexpr int SG_V2_HEADS = SG_LDC2 / 2;      // the most heads (the stats carries hold m | Z of each)
+constexpr uint32_t SG_V2_RB = 512;            // rows per block of da's fp64 column sums
+
+struct V2Params {
+  const uint32_t* rs;
+  const uint32_t* col;
+  const uint32_t* desc;
+  uint32_t E, numChunks, H, heads;
+  float slope;
+  const float* a;                 // [F][heads]: a[k][f] at f * heads + k
+  const float* g;  size_t ldG;    // gathered rows (by col id): STAT, SUM, DST xl; SRC xr; the record kernel: gy
+  const float* g2; size_t ldG2;   // SRC: gy, gathered beside xr
+  const float* o;  size_t ldO;    // the row's own row (by plan row): STAT, SUM, DST xr; SRC xl; the record kernel: y
+  const float* o2; size_t ldO2;   // DST: gy of the row
+  const float* stats; size_t ldStats;   // SUM, the record kernel: m | 1/Z per head
+  float4* rec;                    // DST, SRC: {m, 1/Z, c, 0} per (id, head)
+  float* out;  size_t ldOut;      // STAT: m | 1/Z (a cut row's owner: m | Z); SUM: y; DST: dxr; SRC: dxl
+  float* out2; size_t ldOut2;     // DST: R
+  float* carry; size_t ldC;       // H-wide partials (DST: out's at [0, H), out2's at [H, 2H))
+  float* carry2;                  // STAT: [numCarries][SG_LDC2] m | Z
+};
+
+// s[k] = sum over the warp of t over the columns of head k (hj: the head of each of the lane's columns, -1 for none)
+template <int J>
+__device__ __forceinline__ void v2_head_sums(const float (&t)[J], const int (&hj)[J], uint32_t heads,
+                                             float (&s)[SG_V2_HEADS]) {
+#pragma unroll
+  for (int k = 0; k < SG_V2_HEADS; k++) {
+    float x = 0.f;
+    if ((uint32_t)k < heads) {
+#pragma unroll
+      for (int j = 0; j < J; j++) x = __fadd_rn(x, hj[j] == k ? t[j] : 0.f);
+#pragma unroll
+      for (int o = 16; o >= 1; o >>= 1) x = __fadd_rn(x, __shfl_xor_sync(0xffffffffu, x, o));
+    }
+    s[k] = x;
+  }
+}
+// s[h] without indexing a register array at run time
+__device__ __forceinline__ float v2_pick(const float (&s)[SG_V2_HEADS], int h) {
+  float r = s[0];
+#pragma unroll
+  for (int k = 1; k < SG_V2_HEADS; k++) r = h == k ? s[k] : r;
+  return r;
+}
+// The one computation of e: z = xl + xr per column, e[k] the head sums of a * LeakyReLU(z).
+template <int J>
+__device__ __forceinline__ void v2_logits(const float (&xl)[J], const float (&xr)[J], const float (&a)[J],
+                                          const int (&hj)[J], uint32_t heads, float slope, float (&z)[J],
+                                          float (&e)[SG_V2_HEADS]) {
+  float t[J];
+#pragma unroll
+  for (int j = 0; j < J; j++) {
+    z[j] = __fadd_rn(xl[j], xr[j]);
+    t[j] = __fmul_rn(a[j], leaky(z[j], slope));
+  }
+  v2_head_sums<J>(t, hj, heads, e);
+}
+// g[k] = gy_k . x_k, the backward's dot products (the record's c and each edge's gy[v] . xl[u])
+template <int J>
+__device__ __forceinline__ void v2_dots(const float (&gy)[J], const float (&x)[J], const int (&hj)[J], uint32_t heads,
+                                        float (&g)[SG_V2_HEADS]) {
+  float t[J];
+#pragma unroll
+  for (int j = 0; j < J; j++) t[j] = __fmul_rn(gy[j], x[j]);
+  v2_head_sums<J>(t, hj, heads, g);
+}
+template <int J>
+__device__ __forceinline__ void v2_load_row(const float* row, int lane, const bool (&vj)[J], float (&x)[J]) {
+#pragma unroll
+  for (int j = 0; j < J; j++) x[j] = vj[j] ? __ldg(row + lane + 32 * j) : 0.f;
+}
+
+// One warp per chunk of the plan, the schedule of sg_chunk_kernel (a row cut at chunk boundaries: its owner stores a raw
+// partial, every later chunk a carry).  Per edge (row v's edge from u in the forward plan):
+//   STAT  online (m, Z) of e per head;                    SUM  y[v] += p xl[u], p = exp(e - m) / Z;
+//   DST   d = p (gy[v] . xl[u] - c[v]) per head, dxr[v] += d a LeakyReLU'(z), R[v] += d LeakyReLU(z);
+//   SRC   (row u, gathering v) dxl[u] += p gy[v] + d a LeakyReLU'(z).
+// __launch_bounds__(SG_THREADS, 1) asks for at least one resident CTA per SM, which lets ptxas use up to 255 registers
+// per thread: with no minimum it held J = 3 sums and J = 5 destination passes to fewer registers and gave them a stack
+// frame.  It does not fix the occupancy, which follows each instantiation's registers (about four CTAs per SM for the
+// J = 1 stats pass, one for the J = 8 destination pass).
+template <int J, int PASS>
+__global__ void __launch_bounds__(SG_THREADS, 1)
+sg_v2_kernel(const V2Params p) {
+  constexpr bool SRC = PASS == SG_V2_SRC, DST = PASS == SG_V2_DST;
+  constexpr int U = SRC ? (J <= 2 ? 2 : 1) : (J <= 2 ? 4 : J <= 4 ? 2 : 1);   // edges in flight
+  constexpr int WPB = SG_THREADS / 32;
+  constexpr uint32_t CH = SG_CH;
+  const int lane = threadIdx.x % 32;
+  const uint32_t w = blockIdx.x * WPB + threadIdx.x / 32;
+  if (w >= p.numChunks) return;
+  // the chunk record (k_chunk_desc), read field by field: held as two uint4 it took a stack frame at some J
+  const uint32_t* dsc = p.desc + 8 * (size_t)w;
+  const uint32_t flags = __ldg(dsc + 6);
+  if (flags & 2u) return;
+  const uint32_t ce = min(w * CH + CH, p.E);
+  uint32_t cur = __ldg(dsc + 2), curS = __ldg(dsc + 3), curT = __ldg(dsc + 4);
+  const uint32_t e0 = __ldg(dsc), ee = __ldg(dsc + 1), r1 = __ldg(dsc + 5), carrySlot = __ldg(dsc + 7);
+  int kind = (flags & 1u) ? 0 : ((curT - curS > CH) ? 2 : 1);   // 0 carry-in part, 1 complete row, 2 cut row's owner
+  uint32_t segEnd = (kind == 1) ? curT : min(curT, ce);
+
+  const uint32_t heads = p.heads, F = p.H / heads;
+  int hj[J];
+  bool vj[J];
+  float a[J];
+#pragma unroll
+  for (int j = 0; j < J; j++) {
+    const uint32_t c = (uint32_t)(lane + 32 * j);
+    vj[j] = c < p.H;
+    hj[j] = vj[j] ? (int)(c / F) : -1;
+    a[j] = vj[j] ? __ldg(p.a + (c % F) * heads + c / F) : 0.f;
+  }
+  float xo[J], yo[DST ? J : 1];                 // the row's own row (and DST: its gy)
+  float sm[SG_V2_HEADS], sz[SG_V2_HEADS], sc[SG_V2_HEADS];   // STAT: running m, Z; SUM, DST: m, 1/Z (DST: c)
+  float acc[J], acc2[DST ? J : 1];
+#pragma unroll
+  for (int k = 0; k < SG_V2_HEADS; k++) { sm[k] = PASS == SG_V2_STAT ? -INFINITY : 0.f; sz[k] = 0.f; sc[k] = 0.f; }
+#pragma unroll
+  for (int j = 0; j < J; j++) { acc[j] = 0.f; if constexpr (DST) acc2[j] = 0.f; }
+
+  auto row_state = [&]() {
+    v2_load_row<J>(p.o + (uint64_t)cur * p.ldO, lane, vj, xo);
+    if constexpr (DST) v2_load_row<J>(p.o2 + (uint64_t)cur * p.ldO2, lane, vj, yo);
+    if constexpr (PASS == SG_V2_SUM) {
+#pragma unroll
+      for (int k = 0; k < SG_V2_HEADS; k++)
+        if ((uint32_t)k < heads) {
+          sm[k] = __ldg(p.stats + (uint64_t)cur * p.ldStats + k);
+          sz[k] = __ldg(p.stats + (uint64_t)cur * p.ldStats + heads + k);
+        }
+    }
+    if constexpr (DST) {
+#pragma unroll
+      for (int k = 0; k < SG_V2_HEADS; k++)
+        if ((uint32_t)k < heads) {
+          const float4 r = __ldg(p.rec + (uint64_t)cur * heads + k);
+          sm[k] = r.x; sz[k] = r.y; sc[k] = r.z;
+        }
+    }
+  };
+  row_state();
+
+  auto flush = [&]() {
+    if constexpr (PASS == SG_V2_STAT) {
+      // as ASTAT's store: a complete row stores m and 1/Z (0 and 0 with no edge), a cut row's parts their raw (m, Z)
+      float* sdst = (kind == 0) ? p.carry2 + (uint64_t)carrySlot * SG_LDC2 : p.out + (uint64_t)cur * p.ldOut;
+      if ((uint32_t)lane < heads) {
+        const float m = v2_pick(sm, lane), z = v2_pick(sz, lane);
+        const bool done = kind == 1;
+        sdst[lane] = (done && !(z > 0.f)) ? 0.f : m;
+        sdst[heads + lane] = !done ? z : (z > 0.f ? 1.f / z : 0.f);
+      }
+#pragma unroll
+      for (int k = 0; k < SG_V2_HEADS; k++) { sm[k] = -INFINITY; sz[k] = 0.f; }
+    } else {
+      float* d1 = (kind == 0) ? p.carry + (uint64_t)carrySlot * p.ldC : p.out + (uint64_t)cur * p.ldOut;
+      float* d2 = (kind == 0) ? d1 + p.H : p.out2 + (uint64_t)cur * p.ldOut2;
+      (void)d2;
+#pragma unroll
+      for (int j = 0; j < J; j++) {
+        if (vj[j]) {
+          d1[lane + 32 * j] = acc[j];
+          if constexpr (DST) d2[lane + 32 * j] = acc2[j];
+        }
+        acc[j] = 0.f;
+        if constexpr (DST) acc2[j] = 0.f;
+      }
+    }
+  };
+  auto advance = [&]() {
+    cur += 1; curS = curT; curT = p.rs[cur + 1];
+    const bool heavy = curT - curS > CH;
+    segEnd = heavy ? min(curT, ce) : curT;
+    kind = heavy ? 2 : 1;
+    row_state();
+  };
+
+  const uint32_t eLast = ee - 1u;
+#pragma unroll 1
+  for (uint32_t base = e0; base < ee; base += U) {
+    const uint32_t cnt = min((uint32_t)U, ee - base);
+    uint32_t srcs[U];
+#pragma unroll
+    for (int u = 0; u < U; u++) srcs[u] = __ldg(p.col + min(base + (uint32_t)u, eLast));
+    float gv[U][J], gv2[SRC ? U : 1][SRC ? J : 1];
+    float4 gr[SRC ? U : 1];
+#pragma unroll
+    for (int u = 0; u < U; u++) {
+      v2_load_row<J>(p.g + (uint64_t)srcs[u] * p.ldG, lane, vj, gv[u]);
+      if constexpr (SRC) {
+        v2_load_row<J>(p.g2 + (uint64_t)srcs[u] * p.ldG2, lane, vj, gv2[u]);
+        gr[u] = __ldg(p.rec + (uint64_t)srcs[u] * heads + min((uint32_t)lane, heads - 1u));
+      }
+    }
+    uint32_t pos = 0;
+    for (;;) {
+      const uint32_t lim = min(cnt, segEnd - base);
+#pragma unroll
+      for (int u = 0; u < U; u++) {
+        if ((uint32_t)u >= pos && (uint32_t)u < lim) {
+          float z[J], e[SG_V2_HEADS];
+          if constexpr (SRC) v2_logits<J>(xo, gv[u], a, hj, heads, p.slope, z, e);
+          else v2_logits<J>(gv[u], xo, a, hj, heads, p.slope, z, e);
+          if constexpr (PASS == SG_V2_STAT) {
+#pragma unroll
+            for (int k = 0; k < SG_V2_HEADS; k++)
+              if ((uint32_t)k < heads) {
+                if (e[k] > sm[k]) { sz[k] = sz[k] * expf(sm[k] - e[k]) + 1.f; sm[k] = e[k]; }
+                else sz[k] += expf(e[k] - sm[k]);
+              }
+          } else if constexpr (PASS == SG_V2_SUM) {
+            float pk[SG_V2_HEADS];
+#pragma unroll
+            for (int k = 0; k < SG_V2_HEADS; k++) pk[k] = attn_alpha(e[k], sm[k], sz[k]);
+#pragma unroll
+            for (int j = 0; j < J; j++) acc[j] = fmaf(v2_pick(pk, hj[j]), gv[u][j], acc[j]);
+          } else {
+            // DST: v's own m, 1/Z, c and gy; SRC: those of the gathered v, its record's heads spread over the lanes
+            float m[SG_V2_HEADS], iz[SG_V2_HEADS], c[SG_V2_HEADS], g[SG_V2_HEADS];
+            if constexpr (SRC) {
+#pragma unroll
+              for (int k = 0; k < SG_V2_HEADS; k++) {
+                m[k] = __shfl_sync(0xffffffffu, gr[u].x, k);
+                iz[k] = __shfl_sync(0xffffffffu, gr[u].y, k);
+                c[k] = __shfl_sync(0xffffffffu, gr[u].z, k);
+              }
+              v2_dots<J>(gv2[u], xo, hj, heads, g);
+            } else {
+#pragma unroll
+              for (int k = 0; k < SG_V2_HEADS; k++) { m[k] = sm[k]; iz[k] = sz[k]; c[k] = sc[k]; }
+              v2_dots<J>(yo, gv[u], hj, heads, g);
+            }
+            float pk[SG_V2_HEADS], dk[SG_V2_HEADS];
+#pragma unroll
+            for (int k = 0; k < SG_V2_HEADS; k++) {
+              pk[k] = attn_alpha(e[k], m[k], iz[k]);
+              dk[k] = __fmul_rn(pk[k], __fsub_rn(g[k], c[k]));
+            }
+#pragma unroll
+            for (int j = 0; j < J; j++) {
+              const float d = v2_pick(dk, hj[j]);
+              const float da = __fmul_rn(a[j], z[j] > 0.f ? 1.f : p.slope);
+              if constexpr (SRC) {
+                acc[j] = fmaf(v2_pick(pk, hj[j]), gv2[u][j], acc[j]);
+                acc[j] = fmaf(d, da, acc[j]);
+              } else {
+                acc[j] = fmaf(d, da, acc[j]);
+                acc2[j] = fmaf(d, leaky(z[j], p.slope), acc2[j]);
+              }
+            }
+          }
+        }
+      }
+      pos = lim;
+      if (pos >= cnt) break;
+      flush();
+      advance();
+    }
+  }
+  flush();
+  while (cur + 1 < r1) { advance(); flush(); }   // trailing zero-degree rows
+}
+
+// The backward's record {m, 1/Z, c, 0} of nodes [0, n), c[k] = gy[v]_k . y[v]_k: one warp per node (g = gy, o = y).
+template <int J>
+__global__ void __launch_bounds__(SG_THREADS)
+sg_v2_rec_kernel(const V2Params p, uint32_t n) {
+  const int lane = threadIdx.x % 32;
+  const uint32_t v = blockIdx.x * (SG_THREADS / 32) + threadIdx.x / 32;
+  if (v >= n) return;
+  const uint32_t F = p.H / p.heads;
+  int hj[J];
+  bool vj[J];
+#pragma unroll
+  for (int j = 0; j < J; j++) {
+    const uint32_t c = (uint32_t)(lane + 32 * j);
+    vj[j] = c < p.H;
+    hj[j] = vj[j] ? (int)(c / F) : -1;
+  }
+  float gy[J], y[J], c[SG_V2_HEADS];
+  v2_load_row<J>(p.g + (uint64_t)v * p.ldG, lane, vj, gy);
+  v2_load_row<J>(p.o + (uint64_t)v * p.ldO, lane, vj, y);
+  v2_dots<J>(gy, y, hj, p.heads, c);
+  if ((uint32_t)lane < p.heads)
+    p.rec[(uint64_t)v * p.heads + lane] = make_float4(p.stats[(uint64_t)v * p.ldStats + lane],
+                                                      p.stats[(uint64_t)v * p.ldStats + p.heads + lane], v2_pick(c, lane), 0.f);
+}
+
+// da, the column sums of R [n][H] (ld ldR), in the layout of a: fp64 sums over blocks of SG_V2_RB rows, one thread per
+// column, then the blocks' sums added in block order.  The blocks depend on (n, H) only.
+__global__ void __launch_bounds__(SG_THREADS)
+sg_v2_colsum_part(uint32_t n, uint32_t H, const float* __restrict__ R, size_t ldR, double* __restrict__ part) {
+  const uint32_t c = threadIdx.x, r0 = blockIdx.x * SG_V2_RB, r1 = min(n, r0 + SG_V2_RB);
+  if (c >= H) return;
+  double s = 0.0;
+  for (uint32_t r = r0; r < r1; r++) s += (double)__ldg(R + (uint64_t)r * ldR + c);
+  part[(uint64_t)blockIdx.x * H + c] = s;
+}
+__global__ void __launch_bounds__(SG_THREADS)
+sg_v2_colsum_final(uint32_t nb, uint32_t H, uint32_t heads, const double* __restrict__ part, float* __restrict__ da) {
+  const uint32_t c = threadIdx.x;
+  if (c >= H) return;
+  double s = 0.0;
+  for (uint32_t b = 0; b < nb; b++) s += part[(uint64_t)b * H + c];
+  const uint32_t F = H / heads;
+  da[(c % F) * heads + c / F] = (float)s;
+}
+
+// J = ceil(H / 32) as a std::integral_constant
+template <class Fn>
+static int v2_with_j(uint32_t H, Fn&& f) {
+  switch ((H + 31) / 32) {
+    case 1: return f(std::integral_constant<int, 1>{});
+    case 2: return f(std::integral_constant<int, 2>{});
+    case 3: return f(std::integral_constant<int, 3>{});
+    case 4: return f(std::integral_constant<int, 4>{});
+    case 5: return f(std::integral_constant<int, 5>{});
+    case 6: return f(std::integral_constant<int, 6>{});
+    case 7: return f(std::integral_constant<int, 7>{});
+    case 8: return f(std::integral_constant<int, 8>{});
+    default: return ROC_ERR_UNSUPPORTED;
+  }
+}
+
+static V2Params v2_params(const roc_sg_plan* pl, int heads, int H, float slope, const float* a) {
+  V2Params p;
+  memset(&p, 0, sizeof(p));
+  p.rs = pl->rs; p.col = pl->col; p.desc = pl->desc; p.E = pl->E; p.numChunks = pl->numChunks;
+  p.H = (uint32_t)H; p.heads = (uint32_t)heads; p.slope = slope; p.a = a;
+  p.carry = pl->carry; p.ldC = pl->carryLd; p.carry2 = pl->carry2;
+  return p;
+}
+
+// The sum's fix-ups of the H-wide partials `carryOff` floats into pl's carry slots, into out.
+static int v2_fixups(const roc_sg_plan* pl, int H, float* out, int64_t ldOut, size_t carryOff, cudaStream_t st) {
+  SgParams sp = plan_params(pl);
+  sp.out = out; sp.ldOut = (size_t)ldOut; sp.carry = pl->carry + carryOff; sp.ldC = pl->carryLd; sp.Q = (uint32_t)H;
+  return with_shape<256>((uint32_t)H, [&](auto L, auto NCH) { return launch_fixups<1, L, NCH, SG_RED_SUM>(sp, st); });
+}
+
+// One pass of sg_v2_kernel over pl, then its fix-ups: the stats fix-up (STAT), or the sum's over out (and DST: out2).
+template <int PASS>
+static int v2_pass(const roc_sg_plan* pl, const V2Params& p, cudaStream_t st) {
+  int rc = v2_with_j(p.H, [&](auto J) {
+    if (p.numChunks) {
+      constexpr int WPB = SG_THREADS / 32;
+      const uint32_t grid = (p.numChunks + WPB - 1) / WPB;
+      sg_v2_kernel<J, PASS><<<grid, SG_THREADS, 0, st>>>(p);
+      ROC_LAUNCH_CHECK();
+      note_launch(ROC_SG_LAUNCH_MAIN, SG_RED_V2 + PASS, 1, 32, J, grid);
+    }
+    return ROC_OK;
+  });
+  if (rc != ROC_OK) return rc;
+  if constexpr (PASS == SG_V2_STAT) {
+    const uint32_t rows = pl->numHeavy + pl->numBig;
+    if (rows) {
+      SgParams sp = plan_params(pl);
+      sp.carry2 = pl->carry2; sp.out = p.out; sp.ldOut = p.ldOut; sp.heads = p.heads;
+      const uint32_t grid = (rows + SG_THREADS / 32 - 1) / (SG_THREADS / 32);
+      sg_attn_stat_fixup<<<grid, SG_THREADS, 0, st>>>(sp);
+      ROC_LAUNCH_CHECK();
+      note_launch(ROC_SG_LAUNCH_STAT_FIXUP, SG_RED_V2 + PASS, 1, 32, 1, grid);
+    }
+    return ROC_OK;
+  } else {
+    rc = v2_fixups(pl, (int)p.H, p.out, (int64_t)p.ldOut, 0, st);
+    if (rc == ROC_OK && PASS == SG_V2_DST) rc = v2_fixups(pl, (int)p.H, p.out2, (int64_t)p.ldOut2, p.H, st);
+    return rc;
+  }
+}
+
+// The checks every dynamic attention call shares once its pointers and leading dimensions are checked: a bad slope is
+// ROC_ERR_INVALID; H % heads, H > 256, heads > SG_V2_HEADS and a plan whose ids are not all its own rows (a graph slice)
+// are ROC_ERR_UNSUPPORTED.  Then the carries: `cols` floats per slot, and the stats slots.
+static int v2_setup(roc_sg_plan* pl, int heads, int H, float slope, int cols, cudaStream_t st) {
+  if (!(slope >= 0.f) || !std::isfinite(slope)) return ROC_ERR_INVALID;
+  if (H > 256 || H % heads || heads > SG_V2_HEADS) return ROC_ERR_UNSUPPORTED;
+  int rc = find_id_end(pl, st);
+  if (rc != ROC_OK) return rc;
+  if (pl->idEnd > pl->nloc) return ROC_ERR_UNSUPPORTED;
+  rc = grow_carries(pl, cols, st);
+  if (rc == ROC_OK) rc = grow(pl->carry2, pl->carry2Bytes, (size_t)pl->numCarries * SG_LDC2 * sizeof(float), st);
+  return rc;
+}
+
+// da from R [n][H]: the blocks' fp64 column sums, then their sum in block order (da = 0 with no rows).
+static int v2_colsum(uint32_t n, uint32_t nb, int H, int heads, const float* R, double* part, float* da,
+                     cudaStream_t st) {
+  if (!nb) {
+    ROC_CUDA(cudaMemsetAsync(da, 0, (size_t)H * sizeof(float), st));
+    return ROC_OK;
+  }
+  sg_v2_colsum_part<<<nb, SG_THREADS, 0, st>>>(n, (uint32_t)H, R, (size_t)H, part);
+  ROC_LAUNCH_CHECK();
+  note_launch(ROC_SG_LAUNCH_COLSUM, -1, 1, SG_THREADS, 1, nb);
+  sg_v2_colsum_final<<<1, SG_THREADS, 0, st>>>(nb, (uint32_t)H, (uint32_t)heads, part, da);
+  ROC_LAUNCH_CHECK();
+  note_launch(ROC_SG_LAUNCH_COLSUM, -1, 1, SG_THREADS, 1, 1);
+  return ROC_OK;
+}
+
+// The backward once its arguments are checked: the records over pl's rows, the destination pass over pl, the source
+// pass over plB (pl itself, or the transposed plan), and da from R, a workspace of this call.
+static int v2_backward(roc_sg_plan* pl, roc_sg_plan* plB, int heads, int H, float slope, const float* xl, int64_t ldXl,
+                       const float* xr, int64_t ldXr, const float* a, const float* out, int64_t ldOut,
+                       const float* stats, int64_t ldStats, const float* outGrad, int64_t ldG, float* dxl,
+                       int64_t ldDxl, float* dxr, int64_t ldDxr, float* da, cudaStream_t st) {
+  int rc = v2_setup(pl, heads, H, slope, 2 * H, st);
+  if (rc == ROC_OK && plB != pl) rc = v2_setup(plB, heads, H, slope, H, st);
+  if (rc != ROC_OK) return rc;
+  const uint32_t n = pl->nloc;
+  if ((rc = grow(pl->attnRec, pl->attnRecBytes, (size_t)n * heads * sizeof(float4), st)) != ROC_OK) return rc;
+  const uint32_t nb = (n + SG_V2_RB - 1) / SG_V2_RB;
+  const size_t rBytes = ((size_t)n * H * sizeof(float) + 15) / 16 * 16;
+  char* ws = nullptr;
+  ROC_CUDA(cudaMallocAsync((void**)&ws, rBytes + (size_t)std::max(nb, 1u) * H * sizeof(double), st));
+  float* R = reinterpret_cast<float*>(ws);
+  double* part = reinterpret_cast<double*>(ws + rBytes);
+  // the records {m, 1/Z, c}
+  V2Params r = v2_params(pl, heads, H, slope, a);
+  r.g = outGrad; r.ldG = (size_t)ldG; r.o = out; r.ldO = (size_t)ldOut; r.stats = stats; r.ldStats = (size_t)ldStats;
+  r.rec = pl->attnRec;
+  rc = v2_with_j((uint32_t)H, [&](auto J) {
+    if (n) {
+      const uint32_t grid = (n + SG_THREADS / 32 - 1) / (SG_THREADS / 32);
+      sg_v2_rec_kernel<J><<<grid, SG_THREADS, 0, st>>>(r, n);
+      ROC_LAUNCH_CHECK();
+      note_launch(ROC_SG_LAUNCH_RECORD, -1, 1, 32, J, grid);
+    }
+    return ROC_OK;
+  });
+  // destination pass: dxr and R
+  if (rc == ROC_OK) {
+    V2Params d = v2_params(pl, heads, H, slope, a);
+    d.g = xl; d.ldG = (size_t)ldXl; d.o = xr; d.ldO = (size_t)ldXr; d.o2 = outGrad; d.ldO2 = (size_t)ldG;
+    d.rec = pl->attnRec; d.out = dxr; d.ldOut = (size_t)ldDxr; d.out2 = R; d.ldOut2 = (size_t)H;
+    rc = v2_pass<SG_V2_DST>(pl, d, st);
+  }
+  // source pass: dxl
+  if (rc == ROC_OK) {
+    V2Params s = v2_params(plB, heads, H, slope, a);
+    s.g = xr; s.ldG = (size_t)ldXr; s.g2 = outGrad; s.ldG2 = (size_t)ldG; s.o = xl; s.ldO = (size_t)ldXl;
+    s.rec = pl->attnRec; s.out = dxl; s.ldOut = (size_t)ldDxl;
+    rc = v2_pass<SG_V2_SRC>(plB, s, st);
+  }
+  if (rc == ROC_OK) rc = v2_colsum(n, nb, H, heads, R, part, da, st);
+  // every path after the allocation ends here, so the workspace is always returned
+  const cudaError_t e = cudaFreeAsync(ws, st);
+  if (rc == ROC_OK && e != cudaSuccess) rc = (int)e;
+  return rc;
+}
+
+}  // namespace roc
+
+extern "C" int roc_sg_attn_v2_forward_planned(const roc_sg_plan* plc, int heads, int H, float slope, const float* xl,
+                                              int64_t ldXl, const float* xr, int64_t ldXr, const float* a, float* out,
+                                              int64_t ldOut, float* stats, int64_t ldStats, roc_stream_t stream) {
+  roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  clear_launches();
+  if (!pl || !xl || !xr || !a || !out || !stats || heads <= 0 || H <= 0 || ldXl < H || ldXr < H || ldOut < H ||
+      ldStats < 2 * (int64_t)heads)
+    return ROC_ERR_INVALID;
+  cudaStream_t st = as_stream(stream);
+  int rc = v2_setup(pl, heads, H, slope, H, st);
+  if (rc != ROC_OK) return rc;
+  // pass 1: m and 1/Z per row and head
+  V2Params s = v2_params(pl, heads, H, slope, a);
+  s.g = xl; s.ldG = (size_t)ldXl; s.o = xr; s.ldO = (size_t)ldXr; s.out = stats; s.ldOut = (size_t)ldStats;
+  if ((rc = v2_pass<SG_V2_STAT>(pl, s, st)) != ROC_OK) return rc;
+  // pass 2: the p-weighted sum of the xl rows
+  V2Params b = v2_params(pl, heads, H, slope, a);
+  b.g = xl; b.ldG = (size_t)ldXl; b.o = xr; b.ldO = (size_t)ldXr; b.stats = stats; b.ldStats = (size_t)ldStats;
+  b.out = out; b.ldOut = (size_t)ldOut;
+  return v2_pass<SG_V2_SUM>(pl, b, st);
+}
+
+extern "C" int roc_sg_attn_v2_backward_planned(const roc_sg_plan* plc, int heads, int H, float slope, const float* xl,
+                                               int64_t ldXl, const float* xr, int64_t ldXr, const float* a,
+                                               const float* out, int64_t ldOut, const float* stats, int64_t ldStats,
+                                               const float* outGrad, int64_t ldG, float* dxl, int64_t ldDxl,
+                                               float* dxr, int64_t ldDxr, float* da, roc_stream_t stream) {
+  roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  clear_launches();
+  if (!pl || !xl || !xr || !a || !out || !stats || !outGrad || !dxl || !dxr || !da || dxl == dxr || heads <= 0 ||
+      H <= 0 || ldXl < H || ldXr < H || ldOut < H || ldG < H || ldDxl < H || ldDxr < H || ldStats < 2 * (int64_t)heads)
+    return ROC_ERR_INVALID;
+  return v2_backward(pl, pl, heads, H, slope, xl, ldXl, xr, ldXr, a, out, ldOut, stats, ldStats, outGrad, ldG, dxl,
+                     ldDxl, dxr, ldDxr, da, as_stream(stream));
+}
+
+extern "C" int roc_sg_attn_v2_backward_exact(const roc_sg_plan* plc, roc_sg_transpose* tr, int heads, int H,
+                                             float slope, const float* xl, int64_t ldXl, const float* xr, int64_t ldXr,
+                                             const float* a, const float* out, int64_t ldOut, const float* stats,
+                                             int64_t ldStats, const float* outGrad, int64_t ldG, float* dxl,
+                                             int64_t ldDxl, float* dxr, int64_t ldDxr, float* da, roc_stream_t stream) {
+  roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  clear_launches();
+  if (!pl || !tr || !xl || !xr || !a || !out || !stats || !outGrad || !dxl || !dxr || !da || dxl == dxr ||
+      heads <= 0 || H <= 0 || ldXl < H || ldXr < H || ldOut < H || ldG < H || ldDxl < H || ldDxr < H ||
+      ldStats < 2 * (int64_t)heads || pl->nloc != tr->N || pl->E != tr->E)
+    return ROC_ERR_INVALID;
+  return v2_backward(pl, tr->planT, heads, H, slope, xl, ldXl, xr, ldXr, a, out, ldOut, stats, ldStats, outGrad, ldG,
+                     dxl, ldDxl, dxr, ldDxr, da, as_stream(stream));
 }

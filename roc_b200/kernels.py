@@ -35,6 +35,12 @@ def padded(rows, h, device="cuda", dtype=torch.float32, fill=None):
     return v
 
 
+def _v2_a(a):
+    """GATv2's attention vectors [heads][F] in the kernels' layout: a[k][f] at f * heads + k (a Model parameter's)."""
+    assert a.dim() == 2 and a.dtype == torch.float32
+    return a.t().contiguous()
+
+
 class SgPlan:
     """roc_sg_plan for one partition's CSR (rowEnd u64 END offsets, colSrc u32)."""
 
@@ -207,6 +213,29 @@ class SgPlan:
                                                     _ld(in_grad), _ptr(score_grad), _ld(score_grad), _stream()),
               "roc_sg_attn_backward_planned_bf16")
         return in_grad, score_grad
+
+    def attn_v2_forward(self, xl, xr, a, heads=1, slope=0.2, out=None, stats=None):
+        """GATv2's dynamic attention (roc_sg_attn_v2_forward_planned) -> (out [Nloc][H], stats [Nloc][2*heads] =
+        m | 1/Z per head).  xl, xr: [Nloc][H] fp32 rows (the plan covers a whole graph); a: [heads][F] fp32."""
+        out = self._rows(xl) if out is None else out
+        stats = torch.empty((self.nloc, 2 * heads), device=xl.device) if stats is None else stats
+        check(lib.roc_sg_attn_v2_forward_planned(self.handle, int(heads), xl.shape[1], float(slope), _ptr(xl), _ld(xl),
+                                                 _ptr(xr), _ld(xr), _ptr(_v2_a(a)), _ptr(out), _ld(out),
+                                                 _ptr(stats), _ld(stats), _stream()), "roc_sg_attn_v2_forward_planned")
+        return out, stats
+
+    def attn_v2_backward(self, xl, xr, a, out, stats, gy, heads=1, slope=0.2, dxl=None, dxr=None):
+        """Its backward over the same CSR (exact on a symmetric graph) -> (dxl, dxr, da [heads][F]).  When xl and xr
+        are one tensor its gradient is dxl + dxr."""
+        dxl = self._rows(xl) if dxl is None else dxl
+        dxr = self._rows(xr) if dxr is None else dxr
+        da = torch.empty((a.shape[1], a.shape[0]), device=xl.device)
+        check(lib.roc_sg_attn_v2_backward_planned(self.handle, int(heads), xl.shape[1], float(slope), _ptr(xl),
+                                                  _ld(xl), _ptr(xr), _ld(xr), _ptr(_v2_a(a)), _ptr(out), _ld(out),
+                                                  _ptr(stats), _ld(stats), _ptr(gy), _ld(gy), _ptr(dxl), _ld(dxl),
+                                                  _ptr(dxr), _ld(dxr), _ptr(da), _stream()),
+              "roc_sg_attn_v2_backward_planned")
+        return dxl, dxr, da.t()
 
     def attn_keep_mask(self, rate, seed, step, self_base=0, row_is_source=False, out=None):
         """roc_sg_attn_keep_mask: attention dropout's keep bytes of the plan's edges in its edge order, a uint8 [E]
@@ -383,6 +412,19 @@ class SgTranspose:
                                                   _ld(in_grad), _ptr(score_grad), _ld(score_grad), _stream()),
               "roc_sg_attn_backward_exact_bf16")
         return in_grad, score_grad
+
+    def attn_v2_backward(self, plan, xl, xr, a, out, stats, gy, heads=1, slope=0.2, dxl=None, dxr=None):
+        """roc_sg_attn_v2_backward_exact: SgPlan.attn_v2_backward with the source pass over this transpose, exact on
+        any graph.  plan is the forward's plan of the same graph."""
+        dxl = plan._rows(xl) if dxl is None else dxl
+        dxr = plan._rows(xr) if dxr is None else dxr
+        da = torch.empty((a.shape[1], a.shape[0]), device=xl.device)
+        check(lib.roc_sg_attn_v2_backward_exact(plan.handle, self.handle, int(heads), xl.shape[1], float(slope),
+                                                _ptr(xl), _ld(xl), _ptr(xr), _ld(xr), _ptr(_v2_a(a)), _ptr(out),
+                                                _ld(out), _ptr(stats), _ld(stats), _ptr(gy), _ld(gy), _ptr(dxl),
+                                                _ld(dxl), _ptr(dxr), _ld(dxr), _ptr(da), _stream()),
+              "roc_sg_attn_v2_backward_exact")
+        return dxl, dxr, da.t()
 
     def attn_keep_mask(self, rate, seed, step, out=None):
         """roc_sg_attn_keep_mask over the transposed plan (selfBase 0, the row the source): the keep bytes the exact

@@ -149,6 +149,15 @@ class Model:
         return lib.roc_host_attention_gather_dropout(self.h, t, scores, int(heads), float(negative_slope),
                                                      float(dropout), int(seed))
 
+    def dynamic_attention_gather(self, xl, xr, heads=1, negative_slope=0.2):
+        """GATv2's dynamic attention (Brody et al., PyG GATv2Conv without bias): per destination v and head k over v's
+        in-edges u, e = sum_f a[k][f] LeakyReLU(xl[u][kF+f] + xr[v][kF+f]), p = softmax_u(e), and
+        out[v][kF:(k+1)F] = sum_u p xl[u][kF:(k+1)F].  xl and xr have H = heads * F columns (H <= 256, heads <= 8) and
+        may be one tensor (PyG's share_weights).  Appends one parameter a of parameter_shape (heads, F), so get_parameter
+        returns it as (F, heads), drawn uniform in +-sqrt(6 / (heads + F)) as PyG's glorot draws GATv2Conv.att.  A mode
+        of attention_gather: op_info reports it as one.  One partition only."""
+        return lib.roc_host_dynamic_attention_gather(self.h, xl, xr, int(heads), float(negative_slope))
+
     def attention_scores(self, t, heads=1):
         """GAT's per-head scores of t (H = heads * F columns): [s_dst | s_src], 2 * heads columns, the scores attention_gather
         takes.  Head k's scores are the dot products of its own F columns with its a_dst and a_src.  Appends one parameter
@@ -660,6 +669,59 @@ def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01,
     model.init()
     return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs, "attn": attn,
             "attn_ins": attn_ins, "scores": score_outs, "bns": bns}
+
+
+def build_gatv2(model, layers, dropout_rate, heads=1, negative_slope=0.2, share_weights=False, lr=0.01,
+                weight_decay=0.05, exact_backward=False, features="float32", loss="softmax", norm=None,
+                activation="relu"):
+    """GATv2 (Brody et al., "How Attentive are Graph Attention Networks?"; PyG GATv2Conv without bias) built on
+    dynamic_attention_gather.  `heads` (an int, or one value per hidden layer) applies to the hidden layers; the last
+    layer has one head.  layers[i] is the width of layer i's output, heads_i * F_i.  Per layer:
+
+        d  = dropout(t)
+        xl = linear(d, layers[i])                          # the source / value rows
+        xr = linear(d, layers[i])                          # the target rows; share_weights: xr = xl
+        t  = dynamic_attention_gather(xl, xr, heads_i, slope)
+        t  = relu(t)                                       # all but the last layer; activation="elu": elu(t)
+
+    norm="batch": batch_norm on t before each hidden activation (see build_gcn).  exact_backward: the attention's
+    source pass over the transposed graph (Model.set_exact_backward), exact on directed graphs and multigraphs.
+    Single partition; the attention reads fp32 rows (features="bfloat16" stores only the input features in bf16).
+    Returns the handles, with `attn` (the attention outputs), `attn_ins` (their (xl, xr) pairs) and `relu_outs`."""
+    _check_norm(norm)
+    if activation not in ("relu", "elu"):
+        raise ValueError("activation must be \"relu\" or \"elu\"")
+    L = len(layers)
+    hs = list(heads) if isinstance(heads, (list, tuple)) else [heads] * (L - 2)
+    if len(hs) != L - 2 or any(isinstance(h, bool) or not isinstance(h, (int, np.integer)) or not 1 <= h <= 8
+                               for h in hs):
+        raise ValueError("heads must be an integer in [1, 8], or one per hidden layer")
+    if any(layers[i] % hs[i - 1] for i in range(1, L - 1)):
+        raise ValueError("each hidden width must be a multiple of its heads")
+    hs = [int(h) for h in hs] + [1]
+    x = _input_tensor(model, layers[0], features)
+    label = model.create_node_tensor(layers[-1])
+    mask = model.create_node_tensor(1, is_int=True)
+    act = model.elu if activation == "elu" else model.relu
+    t = x
+    relu_outs, attn, attn_ins, bns = [], [], [], []
+    for i in range(1, L):
+        d = model.dropout(t, dropout_rate)
+        xl = model.linear(d, layers[i], _lib.AC_MODE_NONE)
+        xr = xl if share_weights else model.linear(d, layers[i], _lib.AC_MODE_NONE)
+        t = model.dynamic_attention_gather(xl, xr, hs[i - 1], negative_slope)
+        attn_ins.append((xl, xr))
+        attn.append(t)
+        if i != L - 1:
+            t = act(_hidden_norm(model, norm, t, bns))
+            relu_outs.append(t)
+    _loss(model, loss, t, label, mask)
+    model.adam(lr, weight_decay)
+    if exact_backward:
+        model.set_exact_backward(True)
+    model.init()
+    return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs, "attn": attn,
+            "attn_ins": attn_ins, "bns": bns}
 
 
 def build_gcn_weighted(model, layers, dropout_rate, edge_weights, edge_grad=False, lr=0.01, weight_decay=0.05,

@@ -354,6 +354,46 @@ int roc_sg_attn_v2_backward_exact(const roc_sg_plan* plan, struct roc_sg_transpo
                                   const float* outGrad, int64_t ldG, float* dxl, int64_t ldDxl, float* dxr,
                                   int64_t ldDxr, float* da, roc_stream_t stream);
 
+/* Softmax aggregation with one temperature t (PyG SoftmaxAggregation(t, learn=True), GENConv's default aggregator;
+ * DeeperGCN, Li et al. 2020).  For row v, column f and the in-edges u = colSrc[e] of v (duplicates counted):
+ *   z_u = t * x[u][f],  m = max_u z_u,  Z = sum_u exp(z_u - m),  p_u = exp(z_u - m) / Z,  y[v][f] = sum_u p_u x[u][f]
+ * (y = 0 for a row with no in-edge).  Every column is its own softmax; t = 0 gives the mean, a large t approaches the
+ * max and a negative t leans towards the min.  t is one float in device memory (so that a learned t never needs a
+ * host synchronisation).  The plan covers a whole graph: every id in colSrc is one of its rows, which index x, y,
+ * stats and every gradient.  Any H >= 1; rows wider than 256 columns run in column blocks of 256.
+ * Forward: one pass with an online softmax per column (running m, s = sum exp(z - m), w = sum exp(z - m) x, added as
+ * s = fmaf(s, c, 1), w = fmaf(w, c, x) when z raises m, else s += e, w = fmaf(e, x, w)); a row cut at chunk
+ * boundaries is merged in chunk order by rescale-and-add, y = w / s.  stats (may be NULL, e.g. in inference): when
+ * given, [Nloc][ldStats >= 2H] rows of m | 1/Z per column (0 | 0 for a row with no in-edge), which the backward reads.
+ * Backward, with g = gy[v] and e = exp(t x[u] - m_v), never split into exp(t x) exp(-m):
+ *   dx[u][f] = sum over v with u in N(v) of g p_vu (1 + t (x[u][f] - y[v][f]))
+ *   dt       = sum_v sum_f g sum_u p_vu (x[u][f] - y[v][f])^2
+ * A record pass packs {m | g / Z | y} per destination (3 min(H, 256) floats per node); a source pass per row u gathers
+ * each in-edge's record, accumulates dx and, when dt is wanted, R[u][f] = sum_v (g / Z) e (x - y)^2 (N x H floats).
+ * Both live in a workspace of the plan, grown on demand and kept (freed with the plan); an inference forward on a plan
+ * with cut rows keeps their (m, s) there (2 min(H, 256) floats per node).  dt is R's sum in fp64 over blocks of 512 rows, added in block order, written (not added) as one
+ * fp32.  dt NULL: R and dt are skipped.  roc_sg_softmax_backward_planned runs the source pass over the same CSR,
+ * reading row u's in-edges as its out-edges: exact on a symmetric graph.  roc_sg_softmax_backward_exact runs it over
+ * the transposed plan: exact on any graph, multigraphs included.  No per-edge buffer and no atomics: every output is
+ * the same bits run to run and whatever the grid or the SMs available.  expf throughout, in a fixed order.
+ * ROC_ERR_INVALID: a NULL pointer (dt and the forward's stats may be NULL), H <= 0, a leading dimension < H (stats
+ * < 2H), y == x, dx aliasing x, y, stats, gy or t, dt == t, and for the exact call a transpose of another graph.
+ * ROC_ERR_UNSUPPORTED: a plan whose colSrc names an id outside its rows.  The first call on a plan finds its largest id
+ * (one synchronisation of the stream).  Launches (roc_sg_last_call_info), per column block: the forward's main kernel
+ * reports reduction 72, then its own fix-ups of cut rows (ROC_SG_LAUNCH_FIXUP, ROC_SG_LAUNCH_BIG_FIXUP, reduction 72);
+ * the backward's ROC_SG_LAUNCH_RECORD, then the source pass, reduction 73 (without dt) or 74 (with dt), then the
+ * sum's fix-ups of dx and, with dt, of R; with dt the backward ends with two ROC_SG_LAUNCH_COLSUM launches.  Every
+ * pass runs lanes 32 and nch = ceil(Hb / 32) for the block's Hb columns. */
+int roc_sg_softmax_forward_planned(const roc_sg_plan* plan, int H, const float* t, const float* x, int64_t ldX,
+                                   float* y, int64_t ldY, float* stats, int64_t ldStats, roc_stream_t stream);
+int roc_sg_softmax_backward_planned(const roc_sg_plan* plan, int H, const float* t, const float* x, int64_t ldX,
+                                    const float* y, int64_t ldY, const float* stats, int64_t ldStats, const float* gy,
+                                    int64_t ldG, float* dx, int64_t ldDx, float* dt, roc_stream_t stream);
+int roc_sg_softmax_backward_exact(const roc_sg_plan* plan, struct roc_sg_transpose* tr, int H, const float* t,
+                                  const float* x, int64_t ldX, const float* y, int64_t ldY, const float* stats,
+                                  int64_t ldStats, const float* gy, int64_t ldG, float* dx, int64_t ldDx, float* dt,
+                                  roc_stream_t stream);
+
 /* Edge dropout of the sum (the APPNP paper's dropout of the propagation matrix, PyG APPNP(dropout=); DropEdge, Rong et
  * al. 2020, applied to GCN).  keep(i<-j) is bit 0 of the byte roc_sg_attn_keep_mask writes for the pair (i <- j): lane 0
  * of Philox4x32-10 with counter {i, j, 0, step} and key {seed lo, seed hi}, against T16 = round(rate * 65536), the same
@@ -528,7 +568,7 @@ int roc_sg_backward(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft, in
  *          fix-up of rows with at most 32 carries (one worker each), of rows with more (one CTA each), the attention
  *          stats fix-up, the attention backward's per-node record, the fix-ups of its heads-wide partials, the
  *          weighted backward's weight permutation (first in its list), the keep mask, and the dynamic attention
- *          backward's column sums of da
+ *          backward's column sums of da (and the softmax backward's sums of dt)
  *   red    the reduction the kernel is instantiated for: 0 sum, 1 max, 2 min, 3 the min / max backward, 4 attention
  *          stats, 5 the attention forward, 6 its d s_dst gather, 7 its input-gradient gather, 8 the weighted sum
  *          (forward and backward), 9 the edge-weight gradient, 10 the exact sum backward with NORM (the sum whose
@@ -542,7 +582,8 @@ int roc_sg_backward(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft, in
  *          launches report as without dropout; likewise 32, 42 and 45 for the sum, the exact sum backward with NORM
  *          and the teleport sum with edge dropout (roc_sg_forward_dropout_planned,
  *          roc_sg_transpose_sum_backward_dropout, roc_sg_forward_teleport_dropout_planned at rate > 0); 64, 65, 66 and 67 for
- *          the dynamic attention passes (roc_sg_attn_v2_*); -1 for the records, the permutation, the keep mask and
+ *          the dynamic attention passes (roc_sg_attn_v2_*); 72, 73 and 74 for the softmax aggregation's forward and
+ *          source passes (roc_sg_softmax_*: its forward fix-ups report 72); -1 for the records, the permutation, the keep mask and
  *          the column sums, which have none.  A sum fix-up finishing another
  *          reduction's partials reports 0.
  *   vec    4 for float4 rows, else 1;  lanes, nch: the row shape (L lanes, chunks per lane);  grid: CTAs launched
@@ -558,7 +599,8 @@ int roc_sg_backward(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft, in
 #define ROC_SG_LAUNCH_HEADS_BIG_FIXUP 7
 #define ROC_SG_LAUNCH_PERMUTE 8
 #define ROC_SG_LAUNCH_KEEP_MASK 9     /* roc_sg_attn_keep_mask (red -1) */
-#define ROC_SG_LAUNCH_COLSUM 10       /* roc_sg_attn_v2_backward_*: da's fp64 column sums (red -1) */
+#define ROC_SG_LAUNCH_COLSUM 10       /* roc_sg_attn_v2_backward_*: da's fp64 column sums; roc_sg_softmax_backward_*:
+                                         dt's fp64 sums (red -1) */
 #define ROC_SG_MAX_LAUNCHES 32
 typedef struct {
   int kind, red, vec, lanes, nch;

@@ -221,6 +221,16 @@ public:
    * over the transpose with set_exact_backward.  Never fused; set_bf16_aggregation leaves both inputs fp32.  Exits on
    * different widths, H % heads != 0, H > 256, heads > 8, bf16 inputs, a bad slope, or more than one partition. */
   Tensor dynamic_attention_gather(const Tensor& xl, const Tensor& xr, int heads, float negativeSlope = 0.2f);
+  /* Softmax aggregation with one temperature t (roc_sg_softmax_forward_planned; PyG SoftmaxAggregation, GENConv's
+   * default aggregator): per destination v and column f over v's in-edges u, p = softmax_u(t * x[u][f]) and
+   * out[v][f] = sum_u p * x[u][f] (0 for a row with no in-edge).  t = 0 is the mean, a large t approaches the max.
+   * learnTemperature: t is a parameter of parameter_shape (1, 1), appended here and filled with `temperature` (no
+   * random draw, so the Linears' GlorotUniform draws do not move), trained by Adam with the model's weight decay;
+   * otherwise t is a constant and the backward skips dt.  A mode of attention_gather: op_info reports it as one.  Its
+   * backward runs over the same CSR (exact on a symmetric graph), or over the transpose with set_exact_backward; it adds
+   * into its input's gradient when another op wrote it first.  Never fused; set_bf16_aggregation leaves its input fp32.
+   * Exits on a temperature that is not finite, a bf16 input (at init()), or more than one partition. */
+  Tensor softmax_gather(const Tensor& x, float temperature = 1.0f, bool learnTemperature = false);
   /* The per-head GAT scores of `input` (H = heads * F columns; roc_attn_scores_fwd / _bwd): a [rows][2 * heads] output
    * [s_dst | s_src], head k's scores the dot products of its own F columns with its a_dst and a_src.  Appends one
    * parameter A, a weight tensor of dims {F, 2 * heads} (row k: a_dst of head k, row heads + k: its a_src), drawn by the
@@ -388,6 +398,8 @@ public:
                   int seed);
   /* the dynamic (GATv2) mode: inputs xl, xr (Model::dynamic_attention_gather) */
   AttentionGather(const Model& model, const Tensor& xl, const Tensor& xr, int heads, float slope);
+  /* the softmax aggregation mode: input x (Model::softmax_gather) */
+  AttentionGather(const Model& model, const Tensor& x, float temperature, bool learnTemperature);
   virtual void init(const Model& model);
   virtual void forward(const Model& model);
   virtual void backward(const Model& model);
@@ -403,11 +415,16 @@ public:
   float* scratch[2]; /* gradients of an input that accumulates (or needs none), written here first (Runtime arena) */
   bool dynamic;      /* GATv2's dynamic attention: inputs[0] = xl, inputs[1] = xr, parameter a */
   Tensor a;          /* dynamic: parameter, dims {heads, F} (memory a[k][f] at f * heads + k) */
+  bool softmax;      /* the softmax aggregation: inputs[0] = x, stats [Nloc][statsLd] m | 1/Z per column */
+  bool learnTemperature;   /* softmax: t is the parameter `temperature` */
+  Tensor temperature;      /* softmax with learnTemperature: parameter, dims {1, 1} */
+  float* tConst;     /* softmax without it: t in one device float (Runtime arena) */
 private:
   float drop_rate(const Model& model) const;
   uint64_t drop_key() const;
   void keep_mask(const Model& model, const roc_sg_plan* plan, roc_vid_t selfBase, int rowIsSource, uint8_t*& buf);
   void dynamic_backward(const Model& model);
+  void softmax_backward(const Model& model);
 };
 
 class AttentionScores : public GnnOp {  /* not in the reference: Model::attention_scores */

@@ -53,6 +53,8 @@ int roc_host_attention_gather(roc_host* h, int t, int scores, int heads, float s
 int roc_host_attention_gather_dropout(roc_host* h, int t, int scores, int heads, float slope, float rate, int seed);
 /* Model::dynamic_attention_gather(xl, xr, heads, slope): GATv2's attention; xl and xr may be one tensor */
 int roc_host_dynamic_attention_gather(roc_host* h, int xl, int xr, int heads, float slope);
+/* Model::softmax_gather(t, temperature, learnTemperature): softmax aggregation with one temperature */
+int roc_host_softmax_gather(roc_host* h, int t, float temperature, int learnTemperature);
 /* Model::create_edge_tensor<float>(hidden): rows = this partition's edge count */
 int roc_host_create_edge_tensor(roc_host* h, int hidden);
 /* Model::scatter_gather(t, edges): edge-weighted aggregation */

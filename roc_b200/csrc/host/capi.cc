@@ -107,6 +107,9 @@ int roc_host_attention_gather_dropout(roc_host* h, int t, int scores, int heads,
 int roc_host_dynamic_attention_gather(roc_host* h, int xl, int xr, int heads, float slope) {
   return h->push(h->m().dynamic_attention_gather(h->at(xl), h->at(xr), heads, slope));
 }
+int roc_host_softmax_gather(roc_host* h, int t, float temperature, int learnTemperature) {
+  return h->push(h->m().softmax_gather(h->at(t), temperature, learnTemperature != 0));
+}
 int roc_host_create_edge_tensor(roc_host* h, int hidden) { return h->push(h->m().create_edge_tensor<DATATYPE>(hidden)); }
 int roc_host_scatter_gather_weighted(roc_host* h, int t, int edges) {
   return h->push(h->m().scatter_gather(h->at(t), h->at(edges)));

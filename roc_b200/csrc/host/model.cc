@@ -173,6 +173,15 @@ Tensor Model::dynamic_attention_gather(const Tensor& xl, const Tensor& xr, int h
   parameters.push_back(op->a);
   return op->outputs[0];
 }
+Tensor Model::softmax_gather(const Tensor& x, float temperature, bool learnTemperature) {
+  if (ctx->numParts > 1)
+    ROC_FATAL("softmax_gather: runs on one partition only (numParts > 1 is not supported)");
+  AttentionGather* op = new AttentionGather(*this, x, temperature, learnTemperature);
+  op->opIndex = (int)layers.size();
+  layers.push_back(op);
+  if (learnTemperature) parameters.push_back(op->temperature);
+  return op->outputs[0];
+}
 Tensor Model::attention_scores(const Tensor& input, int heads) {
   if (ctx->numParts > 1)
     ROC_FATAL("attention_scores: runs on one partition only (numParts > 1 is not supported)");
@@ -365,7 +374,7 @@ static void mark_gradients(const Model& m) {
     for (int j = 0; j < op->numInputs; j++)
       if (op->inputs[j].region >= 0) any = any || rt->t(op->inputs[j].region).requiresGrad;
     const AttentionGather* ag = as<AttentionGather>(op);
-    if (as<Linear>(op) || as<BatchNorm>(op) || as<AttentionScores>(op) || (ag && ag->dynamic))
+    if (as<Linear>(op) || as<BatchNorm>(op) || as<AttentionScores>(op) || (ag && (ag->dynamic || ag->learnTemperature)))
       any = true;   // their own parameters
     for (int j = 0; j < op->numOutputs; j++) {
       rt->t(op->outputs[j].region).requiresGrad = any;
@@ -690,8 +699,9 @@ static void choose_bf16_aggregation(RuntimeImpl* rt, const std::vector<GnnOp*>& 
         if (op->inputs[j].region != r) continue;
         ScatterGather* sg = as<ScatterGather>(op);
         Linear* lin = as<Linear>(op);
-        AttentionGather* ag = as<AttentionGather>(op);   // a dynamic one has no bf16 form: it reads fp32
-        if (j == 0 && ((sg && sg->aggr != AGGR_SUM) || as<WeightedScatterGather>(op) || (ag && !ag->dynamic)))
+        AttentionGather* ag = as<AttentionGather>(op);   // dynamic and softmax ones have no bf16 form: they read fp32
+        if (j == 0 && ((sg && sg->aggr != AGGR_SUM) || as<WeightedScatterGather>(op) ||
+                       (ag && !ag->dynamic && !ag->softmax)))
           aggregated = true;
         else if (!(j == 0 && ((lin && lin->dropOp < 0) || as<AttentionScores>(op))))
           others = false;
@@ -1259,7 +1269,8 @@ static void add_scratch(const Model& model, int region, const float* scratch) {
 AttentionGather::AttentionGather(const Model& model, const Tensor& _input, const Tensor& _scores, int _heads, float _slope,
                                  float _dropRate, int _seed)
     : GnnOp(_input, _scores), heads(_heads), slope(_slope), dropRate(_dropRate), seed(_seed), opIndex(0),
-      keep(nullptr), keep2(nullptr), stats(nullptr), statsLd(0), dynamic(false) {
+      keep(nullptr), keep2(nullptr), stats(nullptr), statsLd(0), dynamic(false), softmax(false),
+      learnTemperature(false), tConst(nullptr) {
   scratch[0] = scratch[1] = nullptr;
   ROC_ASSERT(_input.type == Tensor::NODE_TENSOR && _scores.type == Tensor::NODE_TENSOR);
   ROC_ASSERT(_input.numDim == 2 && _scores.numDim == 2);
@@ -1282,7 +1293,7 @@ AttentionGather::AttentionGather(const Model& model, const Tensor& _input, const
 // its gradient through scratch, as any input another op already wrote).
 AttentionGather::AttentionGather(const Model& model, const Tensor& xl, const Tensor& xr, int _heads, float _slope)
     : GnnOp(xl, xr), heads(_heads), slope(_slope), dropRate(0.0f), seed(0), opIndex(0), keep(nullptr), keep2(nullptr),
-      stats(nullptr), statsLd(0), dynamic(true) {
+      stats(nullptr), statsLd(0), dynamic(true), softmax(false), learnTemperature(false), tConst(nullptr) {
   scratch[0] = scratch[1] = nullptr;
   ROC_ASSERT(xl.type == Tensor::NODE_TENSOR && xr.type == Tensor::NODE_TENSOR);
   ROC_ASSERT(xl.numDim == 2 && xr.numDim == 2);
@@ -1300,9 +1311,33 @@ AttentionGather::AttentionGather(const Model& model, const Tensor& xl, const Ten
   numOutputs = 1;
   outputs[0] = model.create_node_tensor<DATATYPE>((int)H);
 }
+// The softmax aggregation mode: one input x, and t as a (1, 1) parameter or a constant device float, both filled
+// without a random draw.
+AttentionGather::AttentionGather(const Model& model, const Tensor& x, float _temperature, bool _learn)
+    : GnnOp(x), heads(1), slope(0.0f), dropRate(0.0f), seed(0), opIndex(0), keep(nullptr), keep2(nullptr),
+      stats(nullptr), statsLd(0), dynamic(false), softmax(true), learnTemperature(_learn), tConst(nullptr) {
+  scratch[0] = scratch[1] = nullptr;
+  ROC_ASSERT(x.type == Tensor::NODE_TENSOR && x.numDim == 2 && x.dims[1] == model.myGraph.numNodes);
+  if (!std::isfinite(_temperature)) ROC_FATAL("softmax_gather: the temperature must be finite");
+  if (model.ctx->t(x.region).isBf16) ROC_FATAL("softmax_gather: x must be fp32 (there is no bf16 form)");
+  RuntimeImpl* rt = model.ctx;
+  float* t;
+  if (_learn) {
+    ZerosInitializer zeros;
+    temperature = model.create_weight_tensor(1, 1, &zeros);
+    t = rt->data(temperature.region);
+  } else {
+    t = tConst = (float*)rt->dmalloc(sizeof(float));
+  }
+  ROC_CHECK(roc_fill(1, 1, _temperature, t, 1, rt->stream));
+  numOutputs = 1;
+  outputs[0] = model.create_node_tensor<DATATYPE>((int)x.dims[0]);
+}
 void AttentionGather::init(const Model& model) {
   if (dynamic && (model.ctx->t(inputs[0].region).isBf16 || model.ctx->t(inputs[1].region).isBf16))
     ROC_FATAL("dynamic_attention_gather: xl and xr must be fp32 (there is no bf16 form)");
+  if (softmax && model.ctx->t(inputs[0].region).isBf16)
+    ROC_FATAL("softmax_gather: x must be fp32 (there is no bf16 form)");
 }
 
 // the attention dropout rate in the current mode (infer: none) and its Philox key
@@ -1320,6 +1355,21 @@ void AttentionGather::keep_mask(const Model& model, const roc_sg_plan* plan, roc
 void AttentionGather::forward(const Model& model) {
   RuntimeImpl* rt = model.ctx;
   const int H = (int)inputs[0].dims[0];
+  if (softmax) {
+    // a training forward keeps m | 1/Z per column for the backward; an inference forward writes none
+    const bool train = model.mode == MD_MODE_TRAIN;
+    if (train && !stats) {
+      statsLd = round_up4(2 * H);
+      stats = (float*)rt->dmalloc((size_t)std::max<int64_t>(model.local_rows(), 1) * (size_t)statsLd * sizeof(float));
+    }
+    const int x = inputs[0].region, y = outputs[0].region;
+    const float* t = learnTemperature ? rt->data(temperature.region) : tConst;
+    rt->sg_begin(H);
+    ROC_CHECK(roc_sg_softmax_forward_planned(model.myGraph.plan, H, t, rt->data(x), rt->t(x).ld, rt->data(y),
+                                             rt->t(y).ld, train ? stats : nullptr, statsLd, rt->stream));
+    rt->sg_end();
+    return;
+  }
   if (!stats) {
     statsLd = round_up4(2 * heads);
     stats = (float*)rt->dmalloc((size_t)std::max<int64_t>(model.local_rows(), 1) * (size_t)statsLd * sizeof(float));
@@ -1355,6 +1405,10 @@ void AttentionGather::backward(const Model& model) {
   RuntimeImpl* rt = model.ctx;
   if (dynamic) {
     dynamic_backward(model);
+    return;
+  }
+  if (softmax) {
+    softmax_backward(model);
     return;
   }
   if (!rt->t(inputs[0].region).requiresGrad && !rt->t(inputs[1].region).requiresGrad) return;
@@ -1424,6 +1478,30 @@ void AttentionGather::dynamic_backward(const Model& model) {
   rt->sg_end();
   for (int i = 0; i < 2; i++)
     if (rt->t(inputs[i].region).requiresGrad && !resetInputGrads[i]) add_scratch(model, inputs[i].region, scratch[i]);
+}
+
+// dx (and, with a learned t, dt into t's gradient) from the same CSR, or over the transpose with the exact backward.  The
+// kernels overwrite dx: when another op wrote x's gradient first (or x needs none) it goes through scratch, added
+// afterwards only in the first case.
+void AttentionGather::softmax_backward(const Model& model) {
+  RuntimeImpl* rt = model.ctx;
+  const int x = inputs[0].region, y = outputs[0].region;
+  const bool wantDx = rt->t(x).requiresGrad;
+  if (!wantDx && !learnTemperature) return;
+  const int H = (int)inputs[0].dims[0];
+  float* dx = grad_or_scratch(model, x, wantDx && resetInputGrads[0], scratch[0]);
+  const float* t = learnTemperature ? rt->data(temperature.region) : tConst;
+  float* dt = learnTemperature ? rt->grad(temperature.region) : nullptr;
+  const int64_t ldX = rt->t(x).ld, ldY = rt->t(y).ld;
+  rt->sg_begin(H);
+  if (model.exactBackward)
+    ROC_CHECK(roc_sg_softmax_backward_exact(model.myGraph.plan, rt->sgTranspose, H, t, rt->data(x), ldX, rt->data(y),
+                                            ldY, stats, statsLd, rt->grad(y), ldY, dx, ldX, dt, rt->stream));
+  else
+    ROC_CHECK(roc_sg_softmax_backward_planned(model.myGraph.plan, H, t, rt->data(x), ldX, rt->data(y), ldY, stats,
+                                              statsLd, rt->grad(y), ldY, dx, ldX, dt, rt->stream));
+  rt->sg_end();
+  if (wantDx && !resetInputGrads[0]) add_scratch(model, x, scratch[0]);
 }
 
 // ------------------------------------------------------- AttentionScores -----

@@ -56,6 +56,9 @@
 //    fmaf(s, x, acc).  Every width runs on sg_chunk_kernel, with the sum's column blocks and fix-ups.
 //  * dynamic attention (roc_sg_attn_v2_*, GATv2) runs on its own kernel, sg_v2_kernel (end of file): one warp per
 //    chunk of the same plan, finished by the attention stats fix-up and the sum's fix-ups.
+//  * softmax aggregation (roc_sg_softmax_*, PyG's SoftmaxAggregation) runs on its own kernel, sg_smx_kernel (end of
+//    file), with the schedule of sg_v2_kernel: a one-pass online softmax per column forward, finished by its own
+//    rescale-and-add fix-ups (sg_smx_fixup), and a record pass and a source pass backward, finished by the sum's.
 //
 // Algorithmic bytes per launch (DESIGN.md): E*(4H+4) + Nloc*(4H+8); min / max forward E*(4H+4) + Nloc*(8H+8),
 // backward E*(8H+4) + Nloc*(4H+8); the sum over bf16 rows E*(2H+4) + Nloc*(4H+8); weighted forward E*(4H+8) + Nloc*(4H+8), edge dot E*(4H+8) + Nloc*4H; attention
@@ -95,6 +98,9 @@ struct roc_sg_plan {
   size_t carry2Bytes = 0;
   float4* attnRec = nullptr;      // attention backward: {s_dst, m, 1/Z, D} per (node id, head)
   size_t attnRecBytes = 0;
+  char* smxWs = nullptr;          // softmax aggregation: the backward's records, R and dt's block sums; the inference
+  size_t smxWsBytes = 0;          // forward's (m, s) of cut rows
+
   uint64_t idEnd = 0;             // 1 + the largest id in col (found by the first attention backward)
   bool idEndKnown = false;
   uint32_t* desc = nullptr;       // [numChunks][8] per-chunk start state of a worker (k_chunk_desc)
@@ -1817,7 +1823,7 @@ done:
 extern "C" void roc_sg_plan_destroy(roc_sg_plan* pl) {
   if (!pl) return;
   cudaFree(pl->rs); cudaFree(pl->firstRow); cudaFree(pl->carryIdx); cudaFree(pl->heavyRows); cudaFree(pl->bigRows); cudaFree(pl->carry); cudaFree(pl->desc);
-  cudaFree(pl->carryArg); cudaFree(pl->carry2); cudaFree(pl->attnRec);
+  cudaFree(pl->carryArg); cudaFree(pl->carry2); cudaFree(pl->attnRec); cudaFree(pl->smxWs);
   delete pl;
 }
 
@@ -3071,4 +3077,478 @@ extern "C" int roc_sg_attn_v2_backward_exact(const roc_sg_plan* plc, roc_sg_tran
     return ROC_ERR_INVALID;
   return v2_backward(pl, tr->planT, heads, H, slope, xl, ldXl, xr, ldXr, a, out, ldOut, stats, ldStats, outGrad, ldG,
                      dxl, ldDxl, dxr, ldDxr, da, as_stream(stream));
+}
+
+// ------------------------------------------------------ softmax aggregation ---
+// roc_sg_softmax_*: PyG's SoftmaxAggregation with one temperature t.  Per destination v and column f over v's in-edges
+// u: z = t x[u][f], p = softmax_u(z), y[v][f] = sum_u p x[u][f].  Every column is its own softmax, so a lane owns its
+// columns outright: one warp per chunk of the plan, lane l holding columns l + 32 j (j < J = ceil(Hb / 32)) of a column
+// block of Hb <= 256 columns, scalar, as sg_v2_kernel.  The forward is one pass with an online softmax per column,
+// (m, s, w) = (max z, sum exp(z - m), sum exp(z - m) x); a cut row's parts are merged by sg_smx_fixup in chunk order.
+// The backward is a record pass per destination and a source pass per row, whose cut rows are plain sums finished by
+// the sum's fix-ups; dt is the fp64 sum of the source pass's R.  t is read from device memory (a learned t is updated
+// there by Adam).  expf throughout, never exp(t x) exp(-m): each factor can overflow where the product cannot.
+namespace roc {
+
+enum { SG_SMX_FWD = 0, SG_SMX_SRC = 1, SG_SMX_SRC_DT = 2 };
+constexpr int SG_RED_SMX = 72;                // the `red` sg_last_call_info reports for pass P is SG_RED_SMX + P
+constexpr int SG_SMX_COLS = 256;              // columns per block (J <= 8)
+constexpr uint32_t SG_SMX_RB = 512;           // rows per block of dt's fp64 sums
+
+struct SmxParams {
+  const uint32_t* rs;
+  const uint32_t* col;
+  const uint32_t* desc;
+  const uint32_t* carryIdx;
+  const uint32_t* heavyRows;
+  const uint32_t* bigRows;
+  uint32_t E, numChunks, numHeavy, numBig, H;   // H: the block's columns
+  const float* t;
+  const float* g;  size_t ldG;    // gathered rows: FWD x; SRC the records {m | r | y} (3H floats per id)
+  const float* o;  size_t ldO;    // SRC: x of the row itself
+  float* out;  size_t ldOut;      // FWD: y; SRC: dx
+  float* m;    float* z; size_t ldMZ;   // FWD: m and 1/Z of a complete row (when `stats`); a cut row's owner: raw m, s
+  float* out2; size_t ldOut2;     // SRC_DT: R
+  float* carry; size_t ldC;       // FWD: [m | s | w]; SRC: [dx | R]
+  int stats;                      // FWD: complete rows store m and 1/Z
+};
+
+// Two (m, s, w) partials of one column merged, the first one earlier in chunk order.  s = 0: no edge (w = 0), which
+// leaves the other partial as it is.  Selects rather than branches, so that the unrolled merges of a row stay in
+// registers.
+__device__ __forceinline__ void smx_merge(float& m, float& s, float& w, float m2, float s2, float w2) {
+  const bool h1 = s > 0.f, h2 = s2 > 0.f;
+  const float M = h2 ? (h1 ? fmaxf(m, m2) : m2) : m;
+  const float a = h1 ? expf(m - M) : 0.f, b = h2 ? expf(m2 - M) : 0.f;
+  s = fmaf(s, a, __fmul_rn(s2, b));
+  w = fmaf(w, a, __fmul_rn(w2, b));
+  m = M;
+}
+
+// A finished column: y = w / s, m and 1/Z (0, 0 and 0 for a row with no edge).
+__device__ __forceinline__ void smx_store(float m, float s, float w, float* y, float* mo, float* zo, bool stats) {
+  const bool any = s > 0.f;
+  *y = any ? __fdiv_rn(w, s) : 0.f;
+  if (stats) { *mo = any ? m : 0.f; *zo = any ? __frcp_rn(s) : 0.f; }
+}
+
+// One warp per chunk of the plan, the schedule of sg_v2_kernel.  Per edge (row v's edge from u):
+//   FWD  online (m, s, w) of z = t x[u] per column;
+//   SRC  (row u, gathering v's record {m, r = gy / Z, y}) e = exp(t x[u] - m), q = r e, d = x[u] - y[v]:
+//        dx[u] += q (1 + t d); SRC_DT also R[u] += q d d.
+template <int J, int PASS>
+__global__ void __launch_bounds__(SG_THREADS, 2)
+sg_smx_kernel(const SmxParams p) {
+  constexpr bool SRC = PASS != SG_SMX_FWD, DT = PASS == SG_SMX_SRC_DT;
+  constexpr int U = SRC ? (J <= 2 ? 4 : J <= 4 ? 2 : 1) : (J <= 2 ? 8 : J <= 4 ? 4 : 2);   // edges in flight
+  constexpr int NG = SRC ? 3 : 1;                 // floats gathered per column and edge
+  constexpr int WPB = SG_THREADS / 32;
+  constexpr uint32_t CH = SG_CH;
+  const int lane = threadIdx.x % 32;
+  const uint32_t w = blockIdx.x * WPB + threadIdx.x / 32;
+  if (w >= p.numChunks) return;
+  const uint32_t* dsc = p.desc + 8 * (size_t)w;
+  const uint32_t flags = __ldg(dsc + 6);
+  if (flags & 2u) return;
+  const uint32_t ce = min(w * CH + CH, p.E);
+  uint32_t cur = __ldg(dsc + 2), curS = __ldg(dsc + 3), curT = __ldg(dsc + 4);
+  const uint32_t e0 = __ldg(dsc), ee = __ldg(dsc + 1), r1 = __ldg(dsc + 5), carrySlot = __ldg(dsc + 7);
+  int kind = (flags & 1u) ? 0 : ((curT - curS > CH) ? 2 : 1);   // 0 carry-in part, 1 complete row, 2 cut row's owner
+  uint32_t segEnd = (kind == 1) ? curT : min(curT, ce);
+
+  const float t = __ldg(p.t);
+  const uint32_t H = p.H;
+  bool vj[J];
+#pragma unroll
+  for (int j = 0; j < J; j++) vj[j] = (uint32_t)(lane + 32 * j) < H;
+  float xo[SRC ? J : 1], zo[SRC ? J : 1];         // SRC: the row's own x and t x
+  float sm[SRC ? 1 : J], ss[SRC ? 1 : J];         // FWD: running m, s (acc: w)
+  float acc[J], acc2[DT ? J : 1];
+#pragma unroll
+  for (int j = 0; j < J; j++) {
+    acc[j] = 0.f;
+    if constexpr (DT) acc2[j] = 0.f;
+    if constexpr (!SRC) { sm[j] = -INFINITY; ss[j] = 0.f; }
+  }
+  auto row_state = [&]() {
+    if constexpr (SRC) {
+#pragma unroll
+      for (int j = 0; j < J; j++) {
+        xo[j] = vj[j] ? __ldg(p.o + (uint64_t)cur * p.ldO + lane + 32 * j) : 0.f;
+        zo[j] = __fmul_rn(t, xo[j]);
+      }
+    }
+  };
+  row_state();
+
+  auto flush = [&]() {
+    if constexpr (!SRC) {
+      if (kind == 0) {
+        float* c = p.carry + (uint64_t)carrySlot * p.ldC;
+#pragma unroll
+        for (int j = 0; j < J; j++)
+          if (vj[j]) { c[lane + 32 * j] = sm[j]; c[H + lane + 32 * j] = ss[j]; c[2 * H + lane + 32 * j] = acc[j]; }
+      } else {
+        float* y = p.out + (uint64_t)cur * p.ldOut;
+        float* mo = p.m + (uint64_t)cur * p.ldMZ;
+        float* zr = p.z + (uint64_t)cur * p.ldMZ;
+#pragma unroll
+        for (int j = 0; j < J; j++) {
+          if (!vj[j]) continue;
+          const int c = lane + 32 * j;
+          if (kind == 2) { y[c] = acc[j]; mo[c] = sm[j]; zr[c] = ss[j]; }   // the raw partial, for sg_smx_fixup
+          else smx_store(sm[j], ss[j], acc[j], y + c, mo + c, zr + c, p.stats != 0);
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < J; j++) { sm[j] = -INFINITY; ss[j] = 0.f; acc[j] = 0.f; }
+    } else {
+      float* d1 = (kind == 0) ? p.carry + (uint64_t)carrySlot * p.ldC : p.out + (uint64_t)cur * p.ldOut;
+      float* d2 = (kind == 0) ? d1 + H : p.out2 + (uint64_t)cur * p.ldOut2;
+      (void)d2;
+#pragma unroll
+      for (int j = 0; j < J; j++) {
+        if (vj[j]) {
+          d1[lane + 32 * j] = acc[j];
+          if constexpr (DT) d2[lane + 32 * j] = acc2[j];
+        }
+        acc[j] = 0.f;
+        if constexpr (DT) acc2[j] = 0.f;
+      }
+    }
+  };
+  auto advance = [&]() {
+    cur += 1; curS = curT; curT = p.rs[cur + 1];
+    const bool heavy = curT - curS > CH;
+    segEnd = heavy ? min(curT, ce) : curT;
+    kind = heavy ? 2 : 1;
+    row_state();
+  };
+
+  const uint32_t eLast = ee - 1u;
+#pragma unroll 1
+  for (uint32_t base = e0; base < ee; base += U) {
+    const uint32_t cnt = min((uint32_t)U, ee - base);
+    float gv[U][NG][J];
+#pragma unroll
+    for (int u = 0; u < U; u++) {
+      const float* row = p.g + (uint64_t)__ldg(p.col + min(base + (uint32_t)u, eLast)) * p.ldG;
+#pragma unroll
+      for (int k = 0; k < NG; k++)
+#pragma unroll
+        for (int j = 0; j < J; j++) gv[u][k][j] = vj[j] ? __ldg(row + k * H + lane + 32 * j) : 0.f;
+    }
+    uint32_t pos = 0;
+    for (;;) {
+      const uint32_t lim = min(cnt, segEnd - base);
+#pragma unroll
+      for (int u = 0; u < U; u++) {
+        if ((uint32_t)u >= pos && (uint32_t)u < lim) {
+#pragma unroll
+          for (int j = 0; j < J; j++) {
+            if constexpr (!SRC) {
+              const float x = gv[u][0][j], z = __fmul_rn(t, x);
+              if (z > sm[j]) {
+                const float c = expf(sm[j] - z);
+                ss[j] = fmaf(ss[j], c, 1.f); acc[j] = fmaf(acc[j], c, x); sm[j] = z;
+              } else {
+                const float e = expf(z - sm[j]);
+                ss[j] = __fadd_rn(ss[j], e); acc[j] = fmaf(e, x, acc[j]);
+              }
+            } else {
+              const float q = __fmul_rn(gv[u][1][j], expf(__fsub_rn(zo[j], gv[u][0][j])));
+              const float d = __fsub_rn(xo[j], gv[u][2][j]);
+              acc[j] = fmaf(q, fmaf(t, d, 1.f), acc[j]);
+              if constexpr (DT) acc2[j] = fmaf(__fmul_rn(q, d), d, acc2[j]);
+            }
+          }
+        }
+      }
+      pos = lim;
+      if (pos >= cnt) break;
+      flush();
+      advance();
+    }
+  }
+  flush();
+  while (cur + 1 < r1) { advance(); flush(); }   // trailing zero-degree rows
+}
+
+// Finishes the forward's cut rows: the owner's raw partial (y: w, m, z: s), then the carries in chunk order, stored as
+// y, m and 1/Z.  Heavy rows (at most 32 carries): one warp each.  BIG rows: one CTA each, whose warps merge contiguous
+// blocks of the carries, then warp 0 the owner's partial and the blocks' in block order.  The grouping depends on the
+// plan only, so the result is reproducible.
+template <int J, bool BIG>
+__global__ void __launch_bounds__(SG_THREADS)
+sg_smx_fixup(const SmxParams p) {
+  constexpr uint32_t CH = SG_CH;
+  constexpr int WPB = SG_THREADS / 32;
+  const int lane = threadIdx.x % 32, g = threadIdx.x / 32;
+  const uint32_t w = BIG ? blockIdx.x : blockIdx.x * WPB + g;
+  if (w >= (BIG ? p.numBig : p.numHeavy)) return;
+  const uint32_t R = BIG ? p.bigRows[w] : p.heavyRows[w];
+  const uint32_t s = p.rs[R], t = p.rs[R + 1];
+  const uint32_t c0 = s / CH, n = (t - 1) / CH - c0;
+  const float* cb = p.carry + (uint64_t)p.carryIdx[c0 + 1] * p.ldC;
+  const uint32_t H = p.H;
+  uint32_t k0 = 0, k1 = n;
+  if constexpr (BIG) { const uint32_t per = (n + WPB - 1) / WPB; k0 = min(n, g * per); k1 = min(n, k0 + per); }
+  float m[J], z[J], a[J];
+#pragma unroll
+  for (int j = 0; j < J; j++) { m[j] = -INFINITY; z[j] = 0.f; a[j] = 0.f; }
+  if (!BIG) {   // a heavy row starts from its owner's partial
+#pragma unroll
+    for (int j = 0; j < J; j++) {
+      const uint32_t c = lane + 32 * j;
+      if (c < H) { m[j] = p.m[(uint64_t)R * p.ldMZ + c]; z[j] = p.z[(uint64_t)R * p.ldMZ + c]; a[j] = p.out[(uint64_t)R * p.ldOut + c]; }
+    }
+  }
+  for (uint32_t k = k0; k < k1; k++) {
+    const float* ck = cb + (uint64_t)k * p.ldC;
+#pragma unroll
+    for (int j = 0; j < J; j++) {
+      const uint32_t c = lane + 32 * j;
+      if (c < H) smx_merge(m[j], z[j], a[j], ck[c], ck[H + c], ck[2 * H + c]);
+    }
+  }
+  float* y = p.out + (uint64_t)R * p.ldOut;
+  float* mo = p.m + (uint64_t)R * p.ldMZ;
+  float* zo = p.z + (uint64_t)R * p.ldMZ;
+  if constexpr (BIG) {
+    __shared__ float part[WPB][3][32 * J];
+#pragma unroll
+    for (int j = 0; j < J; j++) { part[g][0][lane + 32 * j] = m[j]; part[g][1][lane + 32 * j] = z[j]; part[g][2][lane + 32 * j] = a[j]; }
+    __syncthreads();
+    if (g != 0) return;
+#pragma unroll
+    for (int j = 0; j < J; j++) {
+      const uint32_t c = lane + 32 * j;
+      if (c >= H) continue;
+      float mm = mo[c], zz = zo[c], aa = y[c];
+      for (int gg = 0; gg < WPB; gg++) smx_merge(mm, zz, aa, part[gg][0][c], part[gg][1][c], part[gg][2][c]);
+      smx_store(mm, zz, aa, y + c, mo + c, zo + c, true);
+    }
+  } else {
+#pragma unroll
+    for (int j = 0; j < J; j++) {
+      const uint32_t c = lane + 32 * j;
+      if (c < H) smx_store(m[j], z[j], a[j], y + c, mo + c, zo + c, true);
+    }
+  }
+}
+
+// The backward's records of ids [0, n) over one column block, one warp per id: {m | r | y}, 3H floats, with
+// r = gy / Z = gy * (1/Z); a row with no in-edge records m = +inf, so that exp(t x - m) = 0 for any finite t x.
+template <int J>
+__global__ void __launch_bounds__(SG_THREADS)
+sg_smx_rec_kernel(uint32_t n, uint32_t H, const float* __restrict__ M, const float* __restrict__ IZ, size_t ldS,
+                  const float* __restrict__ gy, size_t ldG, const float* __restrict__ y, size_t ldY,
+                  float* __restrict__ rec) {
+  const int lane = threadIdx.x % 32;
+  const uint32_t v = blockIdx.x * (SG_THREADS / 32) + threadIdx.x / 32;
+  if (v >= n) return;
+  float* r = rec + (uint64_t)v * 3 * H;
+#pragma unroll
+  for (int j = 0; j < J; j++) {
+    const uint32_t c = lane + 32 * j;
+    if (c >= H) continue;
+    const float iz = __ldg(IZ + (uint64_t)v * ldS + c);
+    r[c] = iz > 0.f ? __ldg(M + (uint64_t)v * ldS + c) : INFINITY;
+    r[H + c] = __fmul_rn(__ldg(gy + (uint64_t)v * ldG + c), iz);
+    r[2 * H + c] = __ldg(y + (uint64_t)v * ldY + c);
+  }
+}
+
+// dt = the sum of R [n][H] (packed): fp64 sums over blocks of SG_SMX_RB rows (each thread its columns, then the CTA's
+// threads in a fixed tree), then the blocks' sums added in block order.  The blocks depend on (n, H) only.
+__global__ void __launch_bounds__(SG_THREADS)
+sg_smx_dt_part(uint32_t n, uint32_t H, const float* __restrict__ R, double* __restrict__ part) {
+  __shared__ double sh[SG_THREADS];
+  const uint32_t r0 = blockIdx.x * SG_SMX_RB, r1 = min(n, r0 + SG_SMX_RB);
+  double s = 0.0;
+  for (uint32_t r = r0; r < r1; r++)
+    for (uint32_t c = threadIdx.x; c < H; c += SG_THREADS) s += (double)__ldg(R + (uint64_t)r * H + c);
+  sh[threadIdx.x] = s;
+  __syncthreads();
+  for (int k = SG_THREADS / 2; k > 0; k >>= 1) {
+    if ((int)threadIdx.x < k) sh[threadIdx.x] += sh[threadIdx.x + k];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) part[blockIdx.x] = sh[0];
+}
+__global__ void sg_smx_dt_final(uint32_t nb, const double* __restrict__ part, float* __restrict__ dt) {
+  const int lane = threadIdx.x;
+  double s = 0.0;
+  for (uint32_t b0 = 0; b0 < nb; b0 += 32) {
+    const double v = b0 + lane < nb ? part[b0 + lane] : 0.0;
+    for (int k = 0; k < 32 && b0 + k < nb; k++) s += __shfl_sync(0xffffffffu, v, k);
+  }
+  if (lane == 0) *dt = (float)s;
+}
+
+static SmxParams smx_params(const roc_sg_plan* pl, const float* t, int Hb) {
+  SmxParams p;
+  memset(&p, 0, sizeof(p));
+  p.rs = pl->rs; p.col = pl->col; p.desc = pl->desc; p.carryIdx = pl->carryIdx; p.heavyRows = pl->heavyRows;
+  p.bigRows = pl->bigRows; p.E = pl->E; p.numChunks = pl->numChunks; p.numHeavy = pl->numHeavy; p.numBig = pl->numBig;
+  p.H = (uint32_t)Hb; p.t = t; p.carry = pl->carry; p.ldC = pl->carryLd;
+  return p;
+}
+
+// One pass of sg_smx_kernel over pl, then its fix-ups: sg_smx_fixup (FWD), or the sum's over dx (and SRC_DT: R).
+template <int PASS>
+static int smx_pass(const roc_sg_plan* pl, const SmxParams& p, cudaStream_t st) {
+  return v2_with_j(p.H, [&](auto J) {
+    constexpr int WPB = SG_THREADS / 32;
+    if (p.numChunks) {
+      const uint32_t grid = (p.numChunks + WPB - 1) / WPB;
+      sg_smx_kernel<J, PASS><<<grid, SG_THREADS, 0, st>>>(p);
+      ROC_LAUNCH_CHECK();
+      note_launch(ROC_SG_LAUNCH_MAIN, SG_RED_SMX + PASS, 1, 32, J, grid);
+    }
+    if constexpr (PASS == SG_SMX_FWD) {
+      if (p.numHeavy) {
+        const uint32_t grid = (p.numHeavy + WPB - 1) / WPB;
+        sg_smx_fixup<J, false><<<grid, SG_THREADS, 0, st>>>(p);
+        ROC_LAUNCH_CHECK();
+        note_launch(ROC_SG_LAUNCH_FIXUP, SG_RED_SMX + PASS, 1, 32, J, grid);
+      }
+      if (p.numBig) {
+        sg_smx_fixup<J, true><<<p.numBig, SG_THREADS, 0, st>>>(p);
+        ROC_LAUNCH_CHECK();
+        note_launch(ROC_SG_LAUNCH_BIG_FIXUP, SG_RED_SMX + PASS, 1, 32, J, p.numBig);
+      }
+      return ROC_OK;
+    } else {
+      int rc = v2_fixups(pl, (int)p.H, p.out, (int64_t)p.ldOut, 0, st);
+      if (rc == ROC_OK && PASS == SG_SMX_SRC_DT) rc = v2_fixups(pl, (int)p.H, p.out2, (int64_t)p.ldOut2, p.H, st);
+      return rc;
+    }
+  });
+}
+
+// A plan whose ids are not all its own rows (a graph slice) is ROC_ERR_UNSUPPORTED; then the carries, `cols` floats.
+static int smx_setup(roc_sg_plan* pl, int cols, cudaStream_t st) {
+  int rc = find_id_end(pl, st);
+  if (rc != ROC_OK) return rc;
+  if (pl->idEnd > pl->nloc) return ROC_ERR_UNSUPPORTED;
+  return grow_carries(pl, cols, st);
+}
+
+static int smx_forward(roc_sg_plan* pl, int H, const float* t, const float* x, int64_t ldX, float* y, int64_t ldY,
+                       float* stats, int64_t ldStats, cudaStream_t st) {
+  const int bc = std::min(H, SG_SMX_COLS);
+  int rc = smx_setup(pl, 3 * bc, st);
+  if (rc != ROC_OK) return rc;
+  // without stats, a cut row's owner keeps its raw (m, s) in the plan's workspace
+  float* ws = nullptr;
+  if (!stats && pl->numHeavy + pl->numBig) {
+    if ((rc = grow(pl->smxWs, pl->smxWsBytes, (size_t)pl->nloc * 2 * bc * sizeof(float), st)) != ROC_OK) return rc;
+    ws = reinterpret_cast<float*>(pl->smxWs);
+  }
+  for (int c0 = 0; c0 < H && rc == ROC_OK; c0 += SG_SMX_COLS) {
+    const int Hb = std::min(H - c0, SG_SMX_COLS);
+    SmxParams p = smx_params(pl, t, Hb);
+    p.g = x + c0; p.ldG = (size_t)ldX; p.out = y + c0; p.ldOut = (size_t)ldY;
+    if (stats) { p.m = stats + c0; p.z = stats + H + c0; p.ldMZ = (size_t)ldStats; p.stats = 1; }
+    else { p.m = ws; p.z = ws + bc; p.ldMZ = 2 * (size_t)bc; }
+    rc = smx_pass<SG_SMX_FWD>(pl, p, st);
+  }
+  return rc;
+}
+
+// The backward once its arguments are checked: per column block the records over pl's rows and the source pass over
+// plB (pl itself, or the transposed plan); then dt from R.  The records, R and dt's block sums live in pl's workspace,
+// grown on demand (grow) and kept, so that a training step does not allocate and map gigabytes per call.
+static int smx_backward(roc_sg_plan* pl, roc_sg_plan* plB, int H, const float* t, const float* x, int64_t ldX,
+                        const float* y, int64_t ldY, const float* stats, int64_t ldStats, const float* gy, int64_t ldG,
+                        float* dx, int64_t ldDx, float* dt, cudaStream_t st) {
+  const int bc = std::min(H, SG_SMX_COLS);
+  int rc = find_id_end(pl, st);
+  if (rc == ROC_OK && pl->idEnd > pl->nloc) rc = ROC_ERR_UNSUPPORTED;
+  if (rc == ROC_OK) rc = smx_setup(plB, (dt ? 2 : 1) * bc, st);
+  if (rc != ROC_OK) return rc;
+  const uint32_t n = pl->nloc, nb = (n + SG_SMX_RB - 1) / SG_SMX_RB;
+  const size_t recBytes = ((size_t)n * 3 * bc * sizeof(float) + 15) / 16 * 16;
+  const size_t rBytes = dt ? ((size_t)n * H * sizeof(float) + 15) / 16 * 16 : 0;
+  rc = grow(pl->smxWs, pl->smxWsBytes, recBytes + rBytes + (dt ? (size_t)std::max(nb, 1u) * sizeof(double) : 0), st);
+  if (rc != ROC_OK) return rc;
+  char* ws = pl->smxWs;
+  float* rec = reinterpret_cast<float*>(ws);
+  float* R = dt ? reinterpret_cast<float*>(ws + recBytes) : nullptr;
+  double* part = dt ? reinterpret_cast<double*>(ws + recBytes + rBytes) : nullptr;
+  for (int c0 = 0; c0 < H && rc == ROC_OK; c0 += SG_SMX_COLS) {
+    const int Hb = std::min(H - c0, SG_SMX_COLS);
+    rc = v2_with_j((uint32_t)Hb, [&](auto J) {
+      if (n) {
+        const uint32_t grid = (n + SG_THREADS / 32 - 1) / (SG_THREADS / 32);
+        sg_smx_rec_kernel<J><<<grid, SG_THREADS, 0, st>>>(n, (uint32_t)Hb, stats + c0, stats + H + c0, (size_t)ldStats,
+                                                          gy + c0, (size_t)ldG, y + c0, (size_t)ldY, rec);
+        ROC_LAUNCH_CHECK();
+        note_launch(ROC_SG_LAUNCH_RECORD, -1, 1, 32, J, grid);
+      }
+      return ROC_OK;
+    });
+    if (rc != ROC_OK) break;
+    SmxParams p = smx_params(plB, t, Hb);
+    p.g = rec; p.ldG = 3 * (size_t)Hb; p.o = x + c0; p.ldO = (size_t)ldX; p.out = dx + c0; p.ldOut = (size_t)ldDx;
+    if (dt) { p.out2 = R + c0; p.ldOut2 = (size_t)H; rc = smx_pass<SG_SMX_SRC_DT>(plB, p, st); }
+    else rc = smx_pass<SG_SMX_SRC>(plB, p, st);
+  }
+  if (rc == ROC_OK && dt) {
+    if (!nb) {
+      const cudaError_t e = cudaMemsetAsync(dt, 0, sizeof(float), st);
+      if (e != cudaSuccess) rc = (int)e;
+    } else {
+      sg_smx_dt_part<<<nb, SG_THREADS, 0, st>>>(n, (uint32_t)H, R, part);
+      ROC_LAUNCH_CHECK();
+      note_launch(ROC_SG_LAUNCH_COLSUM, -1, 1, SG_THREADS, 1, nb);
+      sg_smx_dt_final<<<1, 32, 0, st>>>(nb, part, dt);
+      ROC_LAUNCH_CHECK();
+      note_launch(ROC_SG_LAUNCH_COLSUM, -1, 1, 32, 1, 1);
+    }
+  }
+  return rc;
+}
+
+// dx may alias none of the inputs, nor dt t.
+static bool smx_backward_args_bad(int H, const float* t, const float* x, int64_t ldX, const float* y, int64_t ldY,
+                                  const float* stats, int64_t ldStats, const float* gy, int64_t ldG, const float* dx,
+                                  int64_t ldDx, const float* dt) {
+  return !t || !x || !y || !stats || !gy || !dx || H <= 0 || ldX < H || ldY < H || ldStats < 2 * (int64_t)H ||
+         ldG < H || ldDx < H || dx == x || dx == y || dx == stats || dx == gy || dx == t || (dt && dt == t);
+}
+
+}  // namespace roc
+
+extern "C" int roc_sg_softmax_forward_planned(const roc_sg_plan* plc, int H, const float* t, const float* x,
+                                              int64_t ldX, float* y, int64_t ldY, float* stats, int64_t ldStats,
+                                              roc_stream_t stream) {
+  roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  clear_launches();
+  if (!pl || !t || !x || !y || H <= 0 || ldX < H || ldY < H || y == x || (stats && ldStats < 2 * (int64_t)H))
+    return ROC_ERR_INVALID;
+  return smx_forward(pl, H, t, x, ldX, y, ldY, stats, ldStats, as_stream(stream));
+}
+
+extern "C" int roc_sg_softmax_backward_planned(const roc_sg_plan* plc, int H, const float* t, const float* x,
+                                               int64_t ldX, const float* y, int64_t ldY, const float* stats,
+                                               int64_t ldStats, const float* gy, int64_t ldG, float* dx, int64_t ldDx,
+                                               float* dt, roc_stream_t stream) {
+  roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  clear_launches();
+  if (!pl || smx_backward_args_bad(H, t, x, ldX, y, ldY, stats, ldStats, gy, ldG, dx, ldDx, dt)) return ROC_ERR_INVALID;
+  return smx_backward(pl, pl, H, t, x, ldX, y, ldY, stats, ldStats, gy, ldG, dx, ldDx, dt, as_stream(stream));
+}
+
+extern "C" int roc_sg_softmax_backward_exact(const roc_sg_plan* plc, roc_sg_transpose* tr, int H, const float* t,
+                                             const float* x, int64_t ldX, const float* y, int64_t ldY,
+                                             const float* stats, int64_t ldStats, const float* gy, int64_t ldG,
+                                             float* dx, int64_t ldDx, float* dt, roc_stream_t stream) {
+  roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  clear_launches();
+  if (!pl || !tr || smx_backward_args_bad(H, t, x, ldX, y, ldY, stats, ldStats, gy, ldG, dx, ldDx, dt) ||
+      pl->nloc != tr->N || pl->E != tr->E)
+    return ROC_ERR_INVALID;
+  return smx_backward(pl, tr->planT, H, t, x, ldX, y, ldY, stats, ldStats, gy, ldG, dx, ldDx, dt, as_stream(stream));
 }

@@ -41,6 +41,15 @@ def _v2_a(a):
     return a.t().contiguous()
 
 
+def _smx_t(t, device):
+    """The softmax aggregation's temperature as one fp32 float in device memory: a float, or a 1-element fp32 tensor on
+    the device, used as is (a learned t is read where Adam updates it)."""
+    if isinstance(t, torch.Tensor):
+        assert t.numel() == 1 and t.dtype == torch.float32 and t.is_cuda
+        return t
+    return torch.full((1,), float(t), device=device, dtype=torch.float32)
+
+
 class SgPlan:
     """roc_sg_plan for one partition's CSR (rowEnd u64 END offsets, colSrc u32)."""
 
@@ -237,6 +246,30 @@ class SgPlan:
               "roc_sg_attn_v2_backward_planned")
         return dxl, dxr, da.t()
 
+    def softmax_forward(self, x, t, out=None, stats=None, keep_stats=True):
+        """Softmax aggregation with temperature t (roc_sg_softmax_forward_planned) -> (out [Nloc][H], stats
+        [Nloc][2H] = m | 1/Z per column, or None with keep_stats=False, the inference form).  x: [Nloc][H] fp32 rows
+        (the plan covers a whole graph); t: a float or a 1-element fp32 device tensor."""
+        out = self._rows(x) if out is None else out
+        if stats is None and keep_stats:
+            stats = torch.empty((self.nloc, 2 * x.shape[1]), device=x.device)
+        tt = _smx_t(t, x.device)
+        check(lib.roc_sg_softmax_forward_planned(self.handle, x.shape[1], _ptr(tt), _ptr(x), _ld(x), _ptr(out),
+                                                 _ld(out), _ptr(stats), _ld(stats) if stats is not None else 0,
+                                                 _stream()), "roc_sg_softmax_forward_planned")
+        return out, stats
+
+    def softmax_backward(self, x, t, out, stats, gy, dx=None, want_dt=True):
+        """Its backward over the same CSR (exact on a symmetric graph) -> (dx, dt as a 1-element tensor, or None with
+        want_dt=False)."""
+        dx = self._rows(x) if dx is None else dx
+        dt = torch.empty((1,), device=x.device) if want_dt else None
+        tt = _smx_t(t, x.device)
+        check(lib.roc_sg_softmax_backward_planned(self.handle, x.shape[1], _ptr(tt), _ptr(x), _ld(x), _ptr(out),
+                                                  _ld(out), _ptr(stats), _ld(stats), _ptr(gy), _ld(gy), _ptr(dx),
+                                                  _ld(dx), _ptr(dt), _stream()), "roc_sg_softmax_backward_planned")
+        return dx, dt
+
     def attn_keep_mask(self, rate, seed, step, self_base=0, row_is_source=False, out=None):
         """roc_sg_attn_keep_mask: attention dropout's keep bytes of the plan's edges in its edge order, a uint8 [E]
         tensor (bit k keeps head k).  row_is_source=False: the pairs (self_base + r <- col[e]), the forward's and the
@@ -425,6 +458,18 @@ class SgTranspose:
                                                 _ld(dxl), _ptr(dxr), _ld(dxr), _ptr(da), _stream()),
               "roc_sg_attn_v2_backward_exact")
         return dxl, dxr, da.t()
+
+    def softmax_backward(self, plan, x, t, out, stats, gy, dx=None, want_dt=True):
+        """roc_sg_softmax_backward_exact: SgPlan.softmax_backward with the source pass over this transpose, exact on
+        any graph.  plan is the forward's plan of the same graph."""
+        dx = plan._rows(x) if dx is None else dx
+        dt = torch.empty((1,), device=x.device) if want_dt else None
+        tt = _smx_t(t, x.device)
+        check(lib.roc_sg_softmax_backward_exact(plan.handle, self.handle, x.shape[1], _ptr(tt), _ptr(x), _ld(x),
+                                                _ptr(out), _ld(out), _ptr(stats), _ld(stats), _ptr(gy), _ld(gy),
+                                                _ptr(dx), _ld(dx), _ptr(dt), _stream()),
+              "roc_sg_softmax_backward_exact")
+        return dx, dt
 
     def attn_keep_mask(self, rate, seed, step, out=None):
         """roc_sg_attn_keep_mask over the transposed plan (selfBase 0, the row the source): the keep bytes the exact

@@ -158,6 +158,18 @@ class Model:
         of attention_gather: op_info reports it as one.  One partition only."""
         return lib.roc_host_dynamic_attention_gather(self.h, xl, xr, int(heads), float(negative_slope))
 
+    def softmax_gather(self, t, temperature=1.0, learn_temperature=False):
+        """Softmax aggregation with one temperature t (PyG SoftmaxAggregation(t, learn=learn_temperature), GENConv's
+        default aggregator): per destination v and column f over v's in-edges u, p = softmax_u(t * x[u][f]) and
+        out[v][f] = sum_u p * x[u][f] (0 for a row with no in-edge).  t = 0 is the mean, a large t approaches the max and
+        a negative t leans towards the min.  learn_temperature: t is a parameter of parameter_shape (1, 1), appended
+        here and set to `temperature` without a random draw, trained by Adam with the model's weight decay; otherwise a
+        constant.  A mode of attention_gather: op_info reports it as one.  fp32 input only (init() refuses a bf16 one);
+        one partition only.  A temperature that is not finite raises ValueError."""
+        if not math.isfinite(float(temperature)):
+            raise ValueError("temperature must be finite")
+        return lib.roc_host_softmax_gather(self.h, t, float(temperature), int(bool(learn_temperature)))
+
     def attention_scores(self, t, heads=1):
         """GAT's per-head scores of t (H = heads * F columns): [s_dst | s_src], 2 * heads columns, the scores attention_gather
         takes.  Head k's scores are the dot products of its own F columns with its a_dst and a_src.  Appends one parameter
@@ -722,6 +734,72 @@ def build_gatv2(model, layers, dropout_rate, heads=1, negative_slope=0.2, share_
     model.init()
     return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs, "attn": attn,
             "attn_ins": attn_ins, "bns": bns}
+
+
+def build_deepergcn(model, layers, dropout_rate, depth, temperature=1.0, learn_temperature=True, norm="batch",
+                    expansion=2, lr=0.01, weight_decay=0.05, exact_backward=False, features="float32", loss="softmax"):
+    """DeeperGCN (Li et al., "DeeperGCN: All You Need to Train Deeper GCNs", 2020) as PyG's
+    examples/ogbn_proteins_deepgcn.py builds it: DeepGCNLayer(block="res+") over GENConv(aggr="softmax", learn_t=True),
+    without edge features.  layers = [in, hidden, out]:
+
+        x = linear(x, hidden)                                   # node encoder
+        x = genconv_1(x)                                        # layer 1: the conv alone
+        for l in 2 .. depth:
+            h = dropout(relu(norm(x)))                          # res+: norm, relu, dropout, conv, then the residual
+            x = add(x, genconv_l(h))
+        logits = linear(dropout(relu(norm(x))), out)
+
+        genconv_l(h):  a = softmax_gather(relu(h), temperature, learn_temperature)
+                       s = add(a, h)
+                       z = relu(norm(linear(s, expansion * hidden)))
+                       return linear(z, hidden)
+
+    norm="batch" is batch_norm (the relu after it is fused into it); None leaves it out.  It differs from PyG's model in
+    three ways: there is no bias (the Linear has none); norm is batch norm or none (PyG's example uses LayerNorm, which
+    the engine lacks); and GENConv's eps = 1e-7 added to each message is left out (the softmax weights sum to 1, so its
+    only effect is to add eps to each aggregated value of a row that has an in-edge).  Each layer learns its own t when
+    learn_temperature, else every t is the constant `temperature`.  exact_backward: the aggregation's backward over the
+    transposed graph (Model.set_exact_backward), exact on directed graphs and multigraphs.  Single partition; the
+    aggregation reads fp32 rows (features="bfloat16" stores only the input features in bf16).  Bad layers, depth,
+    expansion, rates, norm or temperature raise ValueError.  Returns the handles, with `aggs` (the softmax_gather
+    outputs), `temperatures` (each layer's t parameter index, or None) and `bns` (the batch_norm outputs)."""
+    if len(layers) != 3 or any(isinstance(w, bool) or not isinstance(w, (int, np.integer)) or w < 1 for w in layers):
+        raise ValueError("layers must be [in, hidden, out], three positive integers")
+    if isinstance(depth, bool) or not isinstance(depth, (int, np.integer)) or depth < 1:
+        raise ValueError("depth must be an integer >= 1")
+    if isinstance(expansion, bool) or not isinstance(expansion, (int, np.integer)) or expansion < 1:
+        raise ValueError("expansion must be an integer >= 1")
+    _check_rate(dropout_rate, "dropout_rate")
+    _check_norm(norm)
+    if not math.isfinite(float(temperature)):
+        raise ValueError("temperature must be finite")
+    hidden = int(layers[1])
+    x = _input_tensor(model, layers[0], features)
+    label = model.create_node_tensor(layers[-1])
+    mask = model.create_node_tensor(1, is_int=True)
+    aggs, temps, bns = [], [], []
+
+    def norm_relu(t):
+        return model.relu(_hidden_norm(model, norm, t, bns))
+
+    def genconv(h):
+        a = model.softmax_gather(model.relu(h), float(temperature), bool(learn_temperature))
+        aggs.append(a)
+        temps.append(model.num_parameters() - 1 if learn_temperature else None)
+        z = norm_relu(model.linear(model.add(a, h), int(expansion) * hidden, _lib.AC_MODE_NONE))
+        return model.linear(z, hidden, _lib.AC_MODE_NONE)
+
+    t = genconv(model.linear(x, hidden, _lib.AC_MODE_NONE))
+    for _ in range(2, int(depth) + 1):
+        t = model.add(t, genconv(model.dropout(norm_relu(t), dropout_rate)))
+    logits = model.linear(model.dropout(norm_relu(t), dropout_rate), layers[-1], _lib.AC_MODE_NONE)
+    _loss(model, loss, logits, label, mask)
+    model.adam(lr, weight_decay)
+    if exact_backward:
+        model.set_exact_backward(True)
+    model.init()
+    return {"input": x, "label": label, "mask": mask, "logits": logits, "aggs": aggs, "temperatures": temps,
+            "bns": bns}
 
 
 def build_gcn_weighted(model, layers, dropout_rate, edge_weights, edge_grad=False, lr=0.01, weight_decay=0.05,

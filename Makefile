@@ -10,7 +10,7 @@ NVFLAGS := $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Iinclude -Iroc_b20
 CXXFLAGS := -O2 -std=c++17 -fPIC -Iinclude -Iroc_b200/csrc -Iroc_b200/csrc/host -I$(CUDA)/include -Wall -Wno-unused-function
 
 BUILD := build
-CU_SRCS := sg elementwise linear_simt linear linear_tc linear_tc_dw halo batchnorm attn_scores
+CU_SRCS := sg elementwise linear_simt linear linear_tc linear_tc_dw halo batchnorm layernorm attn_scores
 HOST_SRCS := runtime graph model capi
 CU_OBJS := $(CU_SRCS:%=$(BUILD)/%.o)
 HOST_OBJS := $(HOST_SRCS:%=$(BUILD)/host_%.o)

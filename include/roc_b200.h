@@ -844,6 +844,40 @@ int roc_batchnorm_bwd(int64_t rows, int H, const float* x, int64_t ldX, const fl
                       const double* saveInvStd, float* dGamma, float* dBeta, float* dX, int64_t ldDX, int accumulate,
                       void* workspace, size_t workspaceBytes, roc_stream_t stream);
 
+/* ------------------------------------------------------- layer normalisation --- */
+
+/* Layer normalisation over the columns of each row of X[rows][H] (torch.nn.LayerNorm(H, eps) with its affine gamma,
+ * beta), one forward and one backward entry.  Per row, in fp32:
+ *   mu = mean_c x[c],  var = mean_c (x[c] - mu)^2  (the biased variance about the mean, never E[x^2] - E[x]^2),
+ *   rstd = 1 / sqrt(var + eps),  xhat = (x - mu) rstd,  y = xhat gamma[c] + beta[c]  (one fma),
+ * then relu (x > 0 ? x : 0, NaN kept) when relu != 0.  The sums are fp32 in a fixed order (each row's own elements in
+ * column order within a lane, then an xor butterfly across the lanes of the row) and the divisions and the square
+ * root are correctly rounded, so a row's results depend on that row alone and are the same bits on any device and at
+ * any SM budget.  The same forward serves training and inference: nothing is kept per row and there are no running
+ * statistics.  An H = 1 row gives y = beta.  X, Y, dY and dX rows are read and written as 16-byte groups: their
+ * pitches must be multiples of 4 and their bases 16-byte aligned (ROC_ERR_INVALID otherwise).  Columns [H, ld) may be
+ * loaded but are never written, and their values reach no result.  rows = 0 writes nothing.
+ * ROC_ERR_INVALID: a NULL x / gamma / beta / y, rows < 0, H <= 0, ldX or ldY < H, a misaligned base or pitch, eps
+ * negative or not finite. */
+int roc_layernorm_fwd(int64_t rows, int H, const float* x, int64_t ldX, const float* gamma, const float* beta,
+                      float eps, int relu, float* y, int64_t ldY, roc_stream_t stream);
+/* The fp64 gamma / beta partials of roc_layernorm_bwd: double2 [ceil(rows / 1024)][H] (at least one block). */
+size_t roc_layernorm_workspace_bytes(int64_t rows, int H);
+/* The backward of roc_layernorm_fwd on the same x, gamma, beta and eps.  It recomputes each row's mu, rstd and xhat
+ * from x, bit for bit the forward's.  With g' = dY, or with relu != 0 dY masked by the forward's own pre-relu value
+ * xhat gamma + beta > 0 (so no Y is read):
+ *   gh = g' gamma,  dX (+)= rstd (gh - mean_c gh - xhat mean_c(gh xhat))       (fp32; accumulate selects += over =)
+ *   dGamma = sum_rows g' xhat,  dBeta = sum_rows g'
+ * The column sums are fp64 over fixed blocks of 1024 rows, the blocks added in block order and rounded once to fp32,
+ * so they are the same bits on any device.  dGamma and dBeta are overwritten; rows = 0 writes zeros there.  dX == NULL
+ * computes dGamma and dBeta only.  An H = 1 row gives dX = 0.  A NaN in a row reaches that row's y and dx, and dGamma
+ * through its xhat; dBeta only through dY.  One pass over x and dY (and dX when accumulating), no atomics.
+ * ROC_ERR_INVALID: as for the forward, and for a NULL dY / dGamma / dBeta / workspace, ldDY or ldDX < H, a
+ * misaligned dY / dX / workspace, or workspaceBytes < roc_layernorm_workspace_bytes(rows, H). */
+int roc_layernorm_bwd(int64_t rows, int H, const float* x, int64_t ldX, const float* dY, int64_t ldDY, int relu,
+                      const float* gamma, const float* beta, float eps, float* dGamma, float* dBeta, float* dX,
+                      int64_t ldDX, int accumulate, void* workspace, size_t workspaceBytes, roc_stream_t stream);
+
 /* ------------------------------------------------------- attention scores --- */
 
 /* The per-head GAT attention scores (Velickovic et al., 2018; PyG's GATConv): X is [rows][H] with H = heads * F, and

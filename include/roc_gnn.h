@@ -272,6 +272,13 @@ public:
    * variance (start 1); an infer-mode forward uses the running statistics and updates nothing.  init() refuses a
    * partition of fewer than 2 rows.  Single partition only (exit(1) otherwise). */
   Tensor batch_norm(const Tensor& input, float momentum = 0.1f, float eps = 1e-5f);
+  /* Layer normalisation over the columns of each local row (torch.nn.LayerNorm(H, eps); roc_layernorm_fwd /
+   * roc_layernorm_bwd).  Appends two parameters, gamma (filled with 1) then beta (0), each a weight tensor of dims
+   * {H, 1}, trained by the optimizer as batch_norm's are; creating them draws no random numbers.  The same forward runs
+   * in train and infer mode (no running statistics), and any row count is accepted.  op_info reports it as a
+   * batch_norm, the normalisation kind, and a relu that alone reads its output is fused into it as into a batch_norm.
+   * Exits on a negative or non-finite eps.  Single partition only (exit(1) otherwise). */
+  Tensor layer_norm(const Tensor& input, float eps = 1e-5f);
   /* DT = DATATYPE (fp32), int (masks), or __nv_bfloat16 (<cuda_bf16.h>): a leaf feature matrix stored in bf16, rounded
    * to nearest even, rows of round_up(H, 8) elements.  It never has a gradient and is never an op's output; linear and
    * dropout read it (bit-identical to the same model on an fp32 input holding the widened values), and init() refuses
@@ -540,6 +547,20 @@ public:
   float *runMean, *runVar, *saveA, *saveB;
   double *saveMean, *saveInvStd;
   void* workspace;      /* roc_batchnorm_workspace_bytes */
+  size_t workspaceBytes;
+};
+
+class LayerNorm : public GnnOp {  /* not in the reference: Model::layer_norm */
+public:
+  LayerNorm(const Model& model, const Tensor& input, float eps);
+  virtual void init(const Model& model);
+  virtual void forward(const Model& model);
+  virtual void backward(const Model& model);
+public:
+  float eps;
+  Tensor gamma, beta;   /* parameters, dims {H, 1} */
+  int fwdOut;           /* a relu fused into the forward, as BatchNorm::fwdOut (-1: none) */
+  void* workspace;      /* roc_layernorm_workspace_bytes */
   size_t workspaceBytes;
 };
 

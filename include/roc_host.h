@@ -75,6 +75,9 @@ int roc_host_batch_norm(roc_host* h, int t, float momentum, float eps);
 /* the running mean and variance (H floats each) of the batch_norm whose output is t (Model::get / set_batch_norm_stats) */
 int roc_host_get_batch_norm_stats(roc_host* h, int t, float* mean, float* var);
 int roc_host_set_batch_norm_stats(roc_host* h, int t, const float* mean, const float* var);
+/* Model::layer_norm(t, eps): appends two parameters (gamma, beta).  One partition only.  op_info reports it as
+ * ROC_HOST_OP_BATCH_NORM. */
+int roc_host_layer_norm(roc_host* h, int t, float eps);
 int roc_host_softmax_cross_entropy(roc_host* h, int logits, int labels, int mask);
 /* Model::sigmoid_cross_entropy: the multi-label loss of roc_sigmoid_xent_bwd; labels set by roc_host_set_multilabels.
  * One partition only. */
@@ -134,7 +137,7 @@ int roc_host_set_parameter(roc_host* h, int p, const float* host);
 #define ROC_HOST_OP_DROPOUT 10
 #define ROC_HOST_OP_SOFTMAX_CROSS_ENTROPY 11
 #define ROC_HOST_OP_SIGMOID_CROSS_ENTROPY 12
-#define ROC_HOST_OP_BATCH_NORM 13
+#define ROC_HOST_OP_BATCH_NORM 13            /* the normalisations: batch_norm and layer_norm */
 #define ROC_HOST_OP_ELU 14
 #define ROC_HOST_OP_ATTENTION_SCORES 15
 #define ROC_HOST_OP_SCALED_ADD 16
@@ -145,8 +148,8 @@ struct roc_host_op_info {   /* a struct tag only: roc_host_op_info is also the f
   int epilogue;      /* sum ScatterGather: ROC_SG_EPI_* of the forward store (with a scaled_add fused into it: NORM and
                         NORM_OUT of roc_sg_forward_teleport_planned) */
   int bwdEpilogue;   /*   ... and of the backward store */
-  int fwdOut;        /*   the tensor the forward writes (-1: its own output); also a Linear's and a batch_norm's (the
-                        output of the relu fused into it) */
+  int fwdOut;        /*   the tensor the forward writes (-1: its own output); also a Linear's and a batch_norm's or a
+                        layer_norm's (the output of the relu fused into it) */
   int bwdOut;        /*   the tensor whose gradient the backward writes (-1: its input's) */
   int flags;         /* Linear: ROC_LINEAR_* of the forward */
   int dropOp;        /*   >= 0: the Dropout layer applied while X is loaded */

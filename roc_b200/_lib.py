@@ -221,6 +221,9 @@ PROTOTYPES = {
     "roc_batchnorm_fwd": (i32, [i64, i32, vp, i64, vp, vp, f64, f64, vp, vp, i32, i32, vp, i64, vp, vp, vp, vp, vp, sz,
                                 vp]),
     "roc_batchnorm_bwd": (i32, [i64, i32, vp, i64, vp, i64, i32, vp, vp, vp, vp, vp, vp, vp, vp, i64, i32, vp, sz, vp]),
+    "roc_layernorm_fwd": (i32, [i64, i32, vp, i64, vp, vp, f32, i32, vp, i64, vp]),
+    "roc_layernorm_workspace_bytes": (sz, [i64, i32]),
+    "roc_layernorm_bwd": (i32, [i64, i32, vp, i64, vp, i64, i32, vp, vp, f32, vp, vp, vp, i64, i32, vp, sz, vp]),
     "roc_attn_scores_workspace_bytes": (sz, [i64, i32, i32]),
     "roc_attn_scores_fwd": (i32, [i64, i32, i32, vp, i64, vp, vp, i64, vp]),
     "roc_attn_scores_fwd_bf16": (i32, [i64, i32, i32, vp, i64, vp, vp, i64, vp]),
@@ -280,6 +283,7 @@ PROTOTYPES = {
     "roc_host_batch_norm": (i32, [vp, i32, f32, f32]),
     "roc_host_get_batch_norm_stats": (i32, [vp, i32, vp, vp]),
     "roc_host_set_batch_norm_stats": (i32, [vp, i32, vp, vp]),
+    "roc_host_layer_norm": (i32, [vp, i32, f32]),
     "roc_host_softmax_cross_entropy": (i32, [vp, i32, i32, i32]),
     "roc_host_sigmoid_cross_entropy": (i32, [vp, i32, i32, i32]),
     "roc_host_adam": (i32, [vp, f64, f64]),

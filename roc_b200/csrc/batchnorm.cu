@@ -14,7 +14,6 @@ constexpr int BN_T = 256;               // threads per CTA (at most)
 constexpr int BN_MAX_TX = 64;           // column groups per CTA: 256 columns
 constexpr int BN_ROWS_PER_LANE = 128;   // rows a thread sums in one reduction block
 constexpr int BN_UNROLL = 4;            // rows in flight per thread
-constexpr int BN_FIN_T = 128;           // finalize: threads per column
 
 struct BnShape {
   int H4, TX, TY, colBlocks;
@@ -33,25 +32,6 @@ BnShape bn_shape(int64_t rows, int H) {
 // workspace: 3 coefficient rows of round_up4(H) floats (the backward's A, B, C; inference's a, b), then the
 // reduction partials, double2 [rowBlocks][H]
 size_t bn_coef_bytes(int H) { return ((size_t)3 * ((H + 3) / 4 * 4) * sizeof(float) + 255) / 256 * 256; }
-
-__device__ __forceinline__ float4 fma4(const float4& x, const float (&a)[4], const float (&b)[4]) {
-  return make_float4(__fmaf_rn(x.x, a[0], b[0]), __fmaf_rn(x.y, a[1], b[1]), __fmaf_rn(x.z, a[2], b[2]),
-                     __fmaf_rn(x.w, a[3], b[3]));
-}
-__device__ __forceinline__ float lane(const float4& v, int k) { return k == 0 ? v.x : k == 1 ? v.y : k == 2 ? v.z : v.w; }
-// stores columns [4 * c4, min(4 * c4 + 4, H)) of one row: one 16-byte store for a whole group, else per element
-__device__ __forceinline__ void store_group(float* row, int c4, int H, const float4& v) {
-  if (4 * c4 + 4 <= H) {
-    st_stream4(reinterpret_cast<float4*>(row + 4 * c4), v);
-  } else {
-    for (int k = 0; 4 * c4 + k < H; k++) row[4 * c4 + k] = lane(v, k);
-  }
-}
-// the per-column coefficients of this thread's group; 0 beyond H
-__device__ __forceinline__ void load_coef(const float* __restrict__ p, int c4, int H, float (&v)[4]) {
-#pragma unroll
-  for (int k = 0; k < 4; k++) v[k] = (4 * c4 + k < H) ? p[4 * c4 + k] : 0.0f;
-}
 
 // One reduction block of rows per blockIdx.x, one group of TX column groups per blockIdx.y.
 //  forward:  s = sum (x - K), q = sum (x - K)^2 with K = x[0][c]
@@ -128,27 +108,6 @@ k_bn_reduce(int64_t rows, int H, int64_t blockRows, const float* __restrict__ x,
 #pragma unroll
   for (int k = 0; k < 4; k++)
     if (4 * c4 + k < H) partial[(int64_t)blockIdx.x * H + 4 * c4 + k] = make_double2(s[k], q[k]);
-}
-
-// sum of column blockIdx.x's partials over the row blocks: thread t takes blocks t, t + BN_FIN_T, ... in order, then a
-// fixed tree; the result is in thread 0
-__device__ __forceinline__ double2 bn_column_sum(const double2* __restrict__ partial, int64_t rowBlocks, int H, int c) {
-  __shared__ double2 red[BN_FIN_T];
-  double2 acc = make_double2(0.0, 0.0);
-  for (int64_t i = threadIdx.x; i < rowBlocks; i += BN_FIN_T) {
-    const double2 p = partial[i * H + c];
-    acc.x += p.x; acc.y += p.y;
-  }
-  red[threadIdx.x] = acc;
-  __syncthreads();
-  for (int w = BN_FIN_T / 2; w > 0; w >>= 1) {
-    if ((int)threadIdx.x < w) {
-      red[threadIdx.x].x += red[threadIdx.x + w].x;
-      red[threadIdx.x].y += red[threadIdx.x + w].y;
-    }
-    __syncthreads();
-  }
-  return red[0];
 }
 
 // training forward: batch statistics of column blockIdx.x, running statistics, and the affine map a, b

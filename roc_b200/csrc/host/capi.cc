@@ -129,6 +129,7 @@ int roc_host_scaled_add(roc_host* h, int a, int b, float alpha, float beta) {
 int roc_host_batch_norm(roc_host* h, int t, float momentum, float eps) {
   return h->push(h->m().batch_norm(h->at(t), momentum, eps));
 }
+int roc_host_layer_norm(roc_host* h, int t, float eps) { return h->push(h->m().layer_norm(h->at(t), eps)); }
 int roc_host_get_batch_norm_stats(roc_host* h, int t, float* mean, float* var) {
   h->m().get_batch_norm_stats(h->at(t), mean, var);
   return 0;
@@ -250,6 +251,8 @@ int roc_host_op_info(roc_host* h, int layer, struct roc_host_op_info* out) {
     r.gradOut = handle(b->gradOut);
   } else if (const BatchNorm* bn = dynamic_cast<const BatchNorm*>(op)) {
     r.fwdOut = handle(bn->fwdOut);
+  } else if (const LayerNorm* ln = dynamic_cast<const LayerNorm*>(op)) {
+    r.fwdOut = handle(ln->fwdOut);
   }
   *out = r;
   return 0;

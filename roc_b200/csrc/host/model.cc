@@ -290,6 +290,15 @@ Tensor Model::batch_norm(const Tensor& input, float momentum, float eps) {
   parameters.push_back(op->beta);
   return op->outputs[0];
 }
+Tensor Model::layer_norm(const Tensor& input, float eps) {
+  if (ctx->numParts > 1)
+    ROC_FATAL("layer_norm: runs on one partition only (numParts > 1 is not supported)");
+  LayerNorm* op = new LayerNorm(*this, input, eps);
+  layers.push_back(op);
+  parameters.push_back(op->gamma);
+  parameters.push_back(op->beta);
+  return op->outputs[0];
+}
 
 void Model::train_mode(void) { mode = MD_MODE_TRAIN; }
 void Model::infer_mode(void) { mode = MD_MODE_INFER; }
@@ -315,6 +324,7 @@ int roc::host::op_kind(const GnnOp* op) {
          : dynamic_cast<const SoftmaxCrossEntropy*>(op)   ? ROC_HOST_OP_SOFTMAX_CROSS_ENTROPY
          : dynamic_cast<const SigmoidCrossEntropy*>(op)   ? ROC_HOST_OP_SIGMOID_CROSS_ENTROPY
          : dynamic_cast<const BatchNorm*>(op)             ? ROC_HOST_OP_BATCH_NORM
+         : dynamic_cast<const LayerNorm*>(op)             ? ROC_HOST_OP_BATCH_NORM   // the normalisation kind
          : dynamic_cast<const AttentionScores*>(op)       ? ROC_HOST_OP_ATTENTION_SCORES
          : dynamic_cast<const ScaledAdd*>(op)             ? ROC_HOST_OP_SCALED_ADD
                                                           : ROC_HOST_OP_ADD;
@@ -374,7 +384,8 @@ static void mark_gradients(const Model& m) {
     for (int j = 0; j < op->numInputs; j++)
       if (op->inputs[j].region >= 0) any = any || rt->t(op->inputs[j].region).requiresGrad;
     const AttentionGather* ag = as<AttentionGather>(op);
-    if (as<Linear>(op) || as<BatchNorm>(op) || as<AttentionScores>(op) || (ag && (ag->dynamic || ag->learnTemperature)))
+    if (as<Linear>(op) || as<BatchNorm>(op) || as<LayerNorm>(op) || as<AttentionScores>(op) ||
+        (ag && (ag->dynamic || ag->learnTemperature)))
       any = true;   // their own parameters
     for (int j = 0; j < op->numOutputs; j++) {
       rt->t(op->outputs[j].region).requiresGrad = any;
@@ -593,19 +604,23 @@ static void fuse_teleport(const Model& m, Wiring& w) {
   }
 }
 
-// ---- fusion of  batch_norm -> relu: the BN output feeds only the relu.  The BN forward writes the relu's output, and
-//      its backward reads that output's gradient and masks it by fma(x, a, b) > 0 from its saved affine map.
-//      The other peepholes never cross a BN.  In GCN, SG -> indegree_norm still fuses, and the relu after the BN is
-//      this pass's.  The backward fusion (b) needs an indegree_norm under the relu, so it does not match here.
+// ---- fusion of  batch_norm -> relu  and  layer_norm -> relu: the norm's output feeds only the relu.  The norm's
+//      forward writes the relu's output, and its backward reads that output's gradient and masks it by the forward's
+//      own pre-relu test (batch norm: fma(x, a, b) > 0 from its saved affine map; layer norm: xhat gamma + beta > 0,
+//      recomputed from x).  The other peepholes never cross a norm.  In GCN, SG -> indegree_norm still fuses, and the
+//      relu after the norm is this pass's.  The backward fusion (b) needs an indegree_norm under the relu, so it does
+//      not match here.
 static void fuse_batch_norm_relu(const std::vector<GnnOp*>& layers, Wiring& w) {
   for (size_t l = 0; l < layers.size(); l++) {
-    BatchNorm* bn = as<BatchNorm>(layers[l]);
-    if (!bn || bn->fwdOut >= 0) continue;
-    const int ro = bn->outputs[0].region;
+    int* fwdOut = nullptr;
+    if (BatchNorm* bn = as<BatchNorm>(layers[l])) fwdOut = &bn->fwdOut;
+    else if (LayerNorm* ln = as<LayerNorm>(layers[l])) fwdOut = &ln->fwdOut;
+    if (!fwdOut || *fwdOut >= 0) continue;
+    const int ro = layers[l]->outputs[0].region;
     if (w.consumers[ro] != 1) continue;
     Activation* act = as<Activation>(layers[w.consumerOp[ro]]);
     if (!act || act->actiMode != AC_MODE_RELU || act->fusedInto >= 0) continue;
-    bn->fwdOut = act->outputs[0].region;
+    *fwdOut = act->outputs[0].region;
     act->fusedInto = (int)l;
   }
 }
@@ -1857,6 +1872,42 @@ void BatchNorm::backward(const Model& model) {
                               rt->t(y).ld, fwdOut >= 0, rt->data(gamma.region), saveA, saveB, saveMean, saveInvStd,
                               rt->grad(gamma.region), rt->grad(beta.region), dX, rt->t(x).ld, resetInputGrads[0] ? 0 : 1,
                               workspace, workspaceBytes, rt->stream));
+}
+
+// -------------------------------------------------------------- LayerNorm ---
+LayerNorm::LayerNorm(const Model& model, const Tensor& _input, float _eps)
+    : GnnOp(_input), eps(_eps), fwdOut(-1), workspace(nullptr), workspaceBytes(0) {
+  ROC_ASSERT(_input.type == Tensor::NODE_TENSOR && _input.numDim == 2 && _input.dims[1] == model.myGraph.numNodes);
+  if (!(_eps >= 0.0f) || !std::isfinite(_eps)) ROC_FATAL("layer_norm: eps must be finite and >= 0");
+  RuntimeImpl* rt = model.ctx;
+  const int H = (int)_input.dims[0];
+  // constant fills only: the Linears' GlorotUniform draws do not move
+  ZerosInitializer zeros;
+  gamma = model.create_weight_tensor(H, 1, &zeros);
+  beta = model.create_weight_tensor(H, 1, &zeros);
+  ROC_CHECK(roc_fill(1, H, 1.0f, rt->data(gamma.region), H, rt->stream));
+  numOutputs = 1;
+  outputs[0] = model.create_node_tensor<DATATYPE>(H);
+}
+void LayerNorm::init(const Model& model) {
+  workspaceBytes = roc_layernorm_workspace_bytes(model.local_rows(), (int)inputs[0].dims[0]);
+  workspace = model.ctx->dmalloc(workspaceBytes);
+}
+void LayerNorm::forward(const Model& model) {
+  RuntimeImpl* rt = model.ctx;
+  const int x = inputs[0].region, y = fwdOut >= 0 ? fwdOut : outputs[0].region;
+  ROC_CHECK(roc_layernorm_fwd(model.local_rows(), (int)inputs[0].dims[0], rt->data(x), rt->t(x).ld,
+                              rt->data(gamma.region), rt->data(beta.region), eps, fwdOut >= 0, rt->data(y),
+                              rt->t(y).ld, rt->stream));
+}
+void LayerNorm::backward(const Model& model) {
+  RuntimeImpl* rt = model.ctx;
+  const int x = inputs[0].region, y = fwdOut >= 0 ? fwdOut : outputs[0].region;
+  float* dX = rt->t(x).requiresGrad ? rt->grad(x) : nullptr;
+  ROC_CHECK(roc_layernorm_bwd(model.local_rows(), (int)inputs[0].dims[0], rt->data(x), rt->t(x).ld, rt->grad(y),
+                              rt->t(y).ld, fwdOut >= 0, rt->data(gamma.region), rt->data(beta.region), eps,
+                              rt->grad(gamma.region), rt->grad(beta.region), dX, rt->t(x).ld,
+                              resetInputGrads[0] ? 0 : 1, workspace, workspaceBytes, rt->stream));
 }
 
 // ---------------------------------------------------------------- Element ---

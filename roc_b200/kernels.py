@@ -867,6 +867,35 @@ def batchnorm_bwd(x, dy, gamma, state, relu=False, dx=None, accumulate=False, ne
     return dx, dgamma, dbeta
 
 
+def layernorm_fwd(x, gamma, beta, relu=False, eps=1e-5, out=None):
+    """roc_layernorm_fwd on a [rows][H] tensor whose rows are padded to float4 (padded()): per row,
+    y = relu?((x - mean) / sqrt(var + eps) * gamma + beta).  Returns y (padded rows unless `out` is given)."""
+    rows, h = x.shape
+    if out is None:
+        out = padded(rows, h, x.device)
+    check(lib.roc_layernorm_fwd(rows, h, _ptr(x), _ld(x), _ptr(gamma), _ptr(beta), float(eps), int(bool(relu)),
+                                _ptr(out), _ld(out), _stream()), "roc_layernorm_fwd")
+    return out
+
+
+def layernorm_bwd(x, dy, gamma, beta, relu=False, eps=1e-5, dx=None, accumulate=False, need_dx=True):
+    """roc_layernorm_bwd on the inputs of a layernorm_fwd: returns (dx, dgamma, dbeta).  dx is written into (or with
+    accumulate=True added to) `dx` when given; need_dx=False skips it (dx is then None)."""
+    rows, h = x.shape
+    dgamma = torch.empty(h, device=x.device)
+    dbeta = torch.empty(h, device=x.device)
+    if need_dx and dx is None:
+        dx = padded(rows, h, x.device)
+    if not need_dx:
+        dx = None
+    ws_bytes = lib.roc_layernorm_workspace_bytes(rows, h)
+    ws = torch.empty(max(ws_bytes, 16), device=x.device, dtype=torch.uint8)
+    check(lib.roc_layernorm_bwd(rows, h, _ptr(x), _ld(x), _ptr(dy), _ld(dy), int(bool(relu)), _ptr(gamma), _ptr(beta),
+                                float(eps), _ptr(dgamma), _ptr(dbeta), _ptr(dx), _ld(dx) if dx is not None else 0,
+                                int(bool(accumulate)), _ptr(ws), ws_bytes, _stream()), "roc_layernorm_bwd")
+    return dx, dgamma, dbeta
+
+
 def _check_a(a, h, heads):
     """the C ABI reads A as a dense [2 * heads][F] fp32 array"""
     assert a.dtype == torch.float32 and a.is_contiguous() and tuple(a.shape) == (2 * int(heads), h // int(heads)), \

@@ -206,6 +206,15 @@ class Model:
         One partition only; init() refuses fewer than 2 rows."""
         return lib.roc_host_batch_norm(self.h, t, float(momentum), float(eps))
 
+    def layer_norm(self, t, eps=1e-5):
+        """torch.nn.LayerNorm(H, eps) over the columns of each local row: appends two parameters, gamma (ones) then
+        beta (zeros), each of parameter_shape (H, 1).  The same forward in train and infer mode (no running
+        statistics).  A relu that alone reads the output is fused into it.  op_info reports it as a batch_norm, the
+        normalisation kind.  A negative or non-finite eps raises ValueError.  One partition only."""
+        if not (math.isfinite(float(eps)) and float(eps) >= 0.0 and abs(float(eps)) <= float(np.finfo(np.float32).max)):
+            raise ValueError("eps must be finite and >= 0")
+        return lib.roc_host_layer_norm(self.h, t, float(eps))
+
     def batch_norm_stats(self, t):
         """(running mean, running variance), fp32 [H] each, of the batch_norm whose output is t."""
         h = self.tensor_shape(t)[1]
@@ -459,8 +468,8 @@ def _loss(model, loss, logits, label, mask):
 
 
 def _check_norm(norm):
-    if norm not in (None, "batch"):
-        raise ValueError("norm must be None or \"batch\"")
+    if norm not in (None, "batch", "layer_norm"):
+        raise ValueError("norm must be None, \"batch\" or \"layer_norm\"")
 
 
 def _check_rate(rate, name):
@@ -476,10 +485,11 @@ def _sum_gather(model, t, edge_dropout):
 
 
 def _hidden_norm(model, norm, t, bns):
-    """norm="batch": batch_norm on a hidden layer's output, right before its relu; None leaves t as it is."""
+    """norm="batch": batch_norm on a hidden layer's output, right before its relu; norm="layer_norm": layer_norm in
+    the same place; None leaves t as it is."""
     if norm is None:
         return t
-    t = model.batch_norm(t)
+    t = model.layer_norm(t) if norm == "layer_norm" else model.batch_norm(t)
     bns.append(t)
     return t
 
@@ -494,8 +504,9 @@ def build_gcn(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exact_bac
     on every builder.  loss="sigmoid" ends the model in the multi-label sigmoid_cross_entropy instead of the softmax
     (labels then go in with Model.set_multilabels); the same keyword on every builder.  norm="batch" puts a
     batch_norm (Model.batch_norm) on every hidden layer's output right before its relu (here after the second
-    indegree_norm, and before the residual add), never on the last layer; the same keyword on every builder, which
-    then returns the batch_norm outputs as `bns`.  edge_dropout > 0 drops each layer's in-edges at that rate in
+    indegree_norm, and before the residual add), never on the last layer; norm="layer_norm" puts a layer_norm
+    (Model.layer_norm, torch.nn.LayerNorm over each row's features) in the same place.  The same keyword on every
+    builder, which then returns the norm outputs as `bns`.  edge_dropout > 0 drops each layer's in-edges at that rate in
     train mode (Model.scatter_gather(dropout=)), a fresh mask per layer and step, with the degrees of the full graph
     (DropEdge's regulariser on the normalised adjacency, without its renormalisation); a rate outside [0, 1) raises
     ValueError, and 0 builds the model without it."""
@@ -542,7 +553,7 @@ def build_sage_mean(model, layers, dropout_rate, lr=0.01, weight_decay=0.05, exa
 
     x / sqrt(deg) / sqrt(deg) is the mean to within one fp32 rounding.  Same wiring as the reference's residual
     GCN layer (gnn.cc:79-90) with both norms after the aggregation.  aggregation="bfloat16" stores linear(D, d_i),
-    which only the scatter_gather reads, in bf16 (Model.set_bf16_aggregation).  norm="batch": batch_norm on t before
+    which only the scatter_gather reads, in bf16 (Model.set_bf16_aggregation).  norm="batch" / "layer_norm": batch_norm / layer_norm on t before
     each hidden relu (see build_gcn)."""
     _check_norm(norm)
     L = len(layers)
@@ -583,7 +594,7 @@ def build_sage_pool(model, layers, dropout_rate, aggr=_lib.AGGR_MAX, lr=0.01, we
         t  = relu(t)                                   # all but the last layer
 
     Single partition; init refuses a graph with a duplicate edge in a row.  aggregation="bfloat16" stores p, the relu
-    output the scatter_gather reads, in bf16 (Model.set_bf16_aggregation).  norm="batch": batch_norm on t before each
+    output the scatter_gather reads, in bf16 (Model.set_bf16_aggregation).  norm="batch" / "layer_norm": batch_norm / layer_norm on t before each
     hidden layer's last relu (see build_gcn; the pooling network's relu is not a hidden layer's output).  Returns the
     handles, with `pools` (the scatter_gather outputs, for get_aggr_index) and `pool_ins` (their inputs)."""
     _check_norm(norm)
@@ -637,7 +648,7 @@ def build_gat(model, layers, dropout_rate, heads=1, negative_slope=0.2, lr=0.01,
 
     Where this differs from the paper: there is no bias (the reference's Linear has none; norm="batch" gives a
     per-feature shift).  Single partition.  aggregation="bfloat16" stores wh, which the attention_gather and the score
-    op read, in bf16 (Model.set_bf16_aggregation).  norm="batch": batch_norm on t before each hidden activation (see
+    op read, in bf16 (Model.set_bf16_aggregation).  norm="batch" / "layer_norm": batch_norm / layer_norm on t before each hidden activation (see
     build_gcn).  Returns the handles, with `attn` (the attention_gather outputs), `attn_ins` (their feature inputs),
     `scores` and `relu_outs` (the hidden activations' outputs, ELU or ReLU)."""
     _check_norm(norm)
@@ -696,7 +707,7 @@ def build_gatv2(model, layers, dropout_rate, heads=1, negative_slope=0.2, share_
         t  = dynamic_attention_gather(xl, xr, heads_i, slope)
         t  = relu(t)                                       # all but the last layer; activation="elu": elu(t)
 
-    norm="batch": batch_norm on t before each hidden activation (see build_gcn).  exact_backward: the attention's
+    norm="batch" / "layer_norm": batch_norm / layer_norm on t before each hidden activation (see build_gcn).  exact_backward: the attention's
     source pass over the transposed graph (Model.set_exact_backward), exact on directed graphs and multigraphs.
     Single partition; the attention reads fp32 rows (features="bfloat16" stores only the input features in bf16).
     Returns the handles, with `attn` (the attention outputs), `attn_ins` (their (xl, xr) pairs) and `relu_outs`."""
@@ -754,15 +765,15 @@ def build_deepergcn(model, layers, dropout_rate, depth, temperature=1.0, learn_t
                        z = relu(norm(linear(s, expansion * hidden)))
                        return linear(z, hidden)
 
-    norm="batch" is batch_norm (the relu after it is fused into it); None leaves it out.  It differs from PyG's model in
-    three ways: there is no bias (the Linear has none); norm is batch norm or none (PyG's example uses LayerNorm, which
-    the engine lacks); and GENConv's eps = 1e-7 added to each message is left out (the softmax weights sum to 1, so its
-    only effect is to add eps to each aggregated value of a row that has an in-edge).  Each layer learns its own t when
+    norm="layer_norm" is layer_norm, as PyG's example uses; norm="batch" is batch_norm; either fuses the relu after it;
+    None leaves it out.  With norm="layer_norm" the model is PyG's except in two ways: there is no bias (the Linear has
+    none), and GENConv's eps = 1e-7 added to each message is left out (the softmax weights sum to 1, so its only effect
+    is to add eps to each aggregated value of a row that has an in-edge).  Each layer learns its own t when
     learn_temperature, else every t is the constant `temperature`.  exact_backward: the aggregation's backward over the
     transposed graph (Model.set_exact_backward), exact on directed graphs and multigraphs.  Single partition; the
     aggregation reads fp32 rows (features="bfloat16" stores only the input features in bf16).  Bad layers, depth,
     expansion, rates, norm or temperature raise ValueError.  Returns the handles, with `aggs` (the softmax_gather
-    outputs), `temperatures` (each layer's t parameter index, or None) and `bns` (the batch_norm outputs)."""
+    outputs), `temperatures` (each layer's t parameter index, or None) and `bns` (the norm outputs)."""
     if len(layers) != 3 or any(isinstance(w, bool) or not isinstance(w, (int, np.integer)) or w < 1 for w in layers):
         raise ValueError("layers must be [in, hidden, out], three positive integers")
     if isinstance(depth, bool) or not isinstance(depth, (int, np.integer)) or depth < 1:
@@ -811,7 +822,7 @@ def build_gcn_weighted(model, layers, dropout_rate, edge_weights, edge_grad=Fals
     with one edge tensor e shared by every layer.  edge_weights: one fp32 value per edge in CSR order, loaded after
     init().  edge_grad: compute e's gradient in backward (the sum of the layers' contributions).  Single partition.
     aggregation="bfloat16" stores each linear output the scatter_gather reads in bf16 (Model.set_bf16_aggregation).
-    norm="batch": batch_norm on t before each hidden relu (see build_gcn).  Returns the handles, with `edges` and the
+    norm="batch" / "layer_norm": batch_norm / layer_norm on t before each hidden relu (see build_gcn).  Returns the handles, with `edges` and the
     aggregations' inputs `sg_ins` and outputs `sg_outs`."""
     _check_norm(norm)
     L = len(layers)

@@ -354,6 +354,54 @@ int roc_sg_attn_v2_backward_exact(const roc_sg_plan* plan, struct roc_sg_transpo
                                   const float* outGrad, int64_t ldG, float* dxl, int64_t ldDxl, float* dxr,
                                   int64_t ldDxr, float* da, roc_stream_t stream);
 
+/* Dot-product attention (the graph transformer layer: PyG TransformerConv without edge features, beta or lin_skip;
+ * UniMP, Shi et al. 2021).  q holds the target rows, k the keys and v the values, each H = heads * F columns,
+ * 1 <= H <= 256, heads <= 8; a head may start anywhere in a float4 group.  The plan covers a whole graph: every id in
+ * colSrc is one of its rows, which index q, k, v and every other row operand.  For row v, each in-edge from u =
+ * colSrc[e] (duplicate edges count once each, self loops as in the graph) and head k:
+ *   s[v,u,k]   = scale * (q[v]_k . k[u]_k)
+ *   m[v][k]    = max_u s,  Z[v][k] = sum_u exp(s - m),  p[v,u,k] = exp(s - m) / Z
+ *   out[v]_k   = sum_u p[v,u,k] * v[u]_k
+ * The dot is summed in a fixed order that depends on (H, heads) only: lane l of a warp holds columns l + 32 j; where F
+ * divides 32 a head's columns are reduced over their own F lanes by an xor butterfly, otherwise the lane's columns of
+ * the head are added in column order and then reduced over the warp.  The forward and both backward passes see the
+ * same bits for every s.  The forward is one pass with an online softmax (every exponent expf of a difference, so a
+ * logit of any finite size cannot overflow); scale is a float, neither 0 nor non-finite (PyG's 1 / sqrt(F) is the
+ * caller's).  stats[v] = m | 1/Z per head, as roc_sg_attn_v2_forward_planned's (0 | 0 for a row of degree 0, whose
+ * out is 0); stats may be NULL, an inference forward that writes none.
+ * Backward, from outGrad = gy and the forward's out and stats, with c[v][k] = gy[v]_k . out[v]_k (the record pass) and
+ * d[v,u,k] = p (gy[v]_k . v[u]_k - c[v][k]):
+ *   dq[v]_k = scale * sum_u d * k[u]_k                          (the destination pass, over the plan)
+ *   dk[u]_k = scale * sum over u's out-edges v of d * q[v]_k     (the source pass)
+ *   dv[u]_k = sum over u's out-edges v of p * gy[v]_k            (the same source pass)
+ * roc_sg_attn_dot_backward_planned runs the source pass over the same CSR, reading row u's in-edges as its out-edges:
+ * exact on a symmetric graph, as roc_sg_attn_backward_planned.  roc_sg_attn_dot_backward_exact runs it over the
+ * transposed plan: exact on any graph, multigraphs included.  q, k and v may be the same memory, or column blocks of one
+ * packed [q | k | v] buffer (ld 3H); when they are one tensor its gradient is the sum of dq, dk and dv.  No per-edge
+ * buffer and no atomics: every output is the same bits run to run and whatever the grid or the SMs available.  Every
+ * call overwrites its outputs; dq, dk and dv are distinct buffers.
+ * ROC_ERR_INVALID: a NULL pointer (stats in the backward), heads <= 0, H <= 0, a leading dimension < H (stats < 2 *
+ * heads), a scale of 0 or not finite, an output that is another output or an input, and for the exact call a
+ * transpose of another graph.  ROC_ERR_UNSUPPORTED: H % heads != 0, H > 256, heads > 8, or a plan whose colSrc names
+ * an id outside its rows.  The first call on a plan finds its largest id (one synchronisation of the stream); an
+ * inference forward over a plan with cut rows grows a workspace the plan keeps.  Launches (roc_sg_last_call_info):
+ * the main kernel reports reduction 80 (forward), 81 (destination pass) and 82 (source pass), with lanes 32 and nch =
+ * ceil(H / 32); the forward's own fix-ups of cut rows follow it and report 80; the sum's fix-ups follow the backward
+ * passes (the source pass: dk's, then dv's); the backward starts with a ROC_SG_LAUNCH_RECORD. */
+int roc_sg_attn_dot_forward_planned(const roc_sg_plan* plan, int heads, int H, float scale, const float* q,
+                                    int64_t ldQ, const float* k, int64_t ldK, const float* v, int64_t ldV, float* out,
+                                    int64_t ldOut, float* stats, int64_t ldStats, roc_stream_t stream);
+int roc_sg_attn_dot_backward_planned(const roc_sg_plan* plan, int heads, int H, float scale, const float* q,
+                                     int64_t ldQ, const float* k, int64_t ldK, const float* v, int64_t ldV,
+                                     const float* out, int64_t ldOut, const float* stats, int64_t ldStats,
+                                     const float* outGrad, int64_t ldG, float* dq, int64_t ldDq, float* dk,
+                                     int64_t ldDk, float* dv, int64_t ldDv, roc_stream_t stream);
+int roc_sg_attn_dot_backward_exact(const roc_sg_plan* plan, struct roc_sg_transpose* tr, int heads, int H, float scale,
+                                   const float* q, int64_t ldQ, const float* k, int64_t ldK, const float* v,
+                                   int64_t ldV, const float* out, int64_t ldOut, const float* stats, int64_t ldStats,
+                                   const float* outGrad, int64_t ldG, float* dq, int64_t ldDq, float* dk, int64_t ldDk,
+                                   float* dv, int64_t ldDv, roc_stream_t stream);
+
 /* Softmax aggregation with one temperature t (PyG SoftmaxAggregation(t, learn=True), GENConv's default aggregator;
  * DeeperGCN, Li et al. 2020).  For row v, column f and the in-edges u = colSrc[e] of v (duplicates counted):
  *   z_u = t * x[u][f],  m = max_u z_u,  Z = sum_u exp(z_u - m),  p_u = exp(z_u - m) / Z,  y[v][f] = sum_u p_u x[u][f]
@@ -583,7 +631,9 @@ int roc_sg_backward(roc_vid_t rowLeft, roc_vid_t rowRight, roc_eid_t colLeft, in
  *          and the teleport sum with edge dropout (roc_sg_forward_dropout_planned,
  *          roc_sg_transpose_sum_backward_dropout, roc_sg_forward_teleport_dropout_planned at rate > 0); 64, 65, 66 and 67 for
  *          the dynamic attention passes (roc_sg_attn_v2_*); 72, 73 and 74 for the softmax aggregation's forward and
- *          source passes (roc_sg_softmax_*: its forward fix-ups report 72); -1 for the records, the permutation, the keep mask and
+ *          source passes (roc_sg_softmax_*: its forward fix-ups report 72); 80, 81 and 82 for the dot-product
+ *          attention's forward, destination and source passes (roc_sg_attn_dot_*: its forward fix-ups report 80);
+ *          -1 for the records, the permutation, the keep mask and
  *          the column sums, which have none.  A sum fix-up finishing another
  *          reduction's partials reports 0.
  *   vec    4 for float4 rows, else 1;  lanes, nch: the row shape (L lanes, chunks per lane);  grid: CTAs launched

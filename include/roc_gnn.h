@@ -231,6 +231,17 @@ public:
    * into its input's gradient when another op wrote it first.  Never fused; set_bf16_aggregation leaves its input fp32.
    * Exits on a temperature that is not finite, a bf16 input (at init()), or more than one partition. */
   Tensor softmax_gather(const Tensor& x, float temperature = 1.0f, bool learnTemperature = false);
+  /* Dot-product attention (roc_sg_attn_dot_forward_planned; the graph transformer layer, PyG TransformerConv's
+   * attention): per destination v and head k over v's in-edges u, s = scale * q[v]_k . k[u]_k, p = softmax_u(s) and
+   * out[v]_k = sum_u p * v[u]_k (0 for a row with no in-edge).  q, k and v have H = heads * F columns, H <= 256,
+   * heads <= 8, and any of them may be the same tensor (its gradient then takes every part).  scale is neither 0 nor
+   * non-finite (PyG's 1 / sqrt(F) is the caller's: Model.dot_attention_gather computes it).  No parameter.  A mode of
+   * attention_gather: op_info reports it as one.  Training forwards keep m | 1/Z per head; inference forwards write
+   * none.  Its backward runs over the same CSR (exact on a symmetric graph), or over the transpose with
+   * set_exact_backward; it adds into an input's gradient when another op wrote it first.  Never fused;
+   * set_bf16_aggregation leaves q, k and v fp32.  Exits on unequal widths, H % heads != 0, H > 256, heads > 8, a bad
+   * scale, bf16 inputs, or more than one partition. */
+  Tensor dot_attention_gather(const Tensor& q, const Tensor& k, const Tensor& v, int heads, float scale);
   /* The per-head GAT scores of `input` (H = heads * F columns; roc_attn_scores_fwd / _bwd): a [rows][2 * heads] output
    * [s_dst | s_src], head k's scores the dot products of its own F columns with its a_dst and a_src.  Appends one
    * parameter A, a weight tensor of dims {F, 2 * heads} (row k: a_dst of head k, row heads + k: its a_src), drawn by the
@@ -407,6 +418,8 @@ public:
   AttentionGather(const Model& model, const Tensor& xl, const Tensor& xr, int heads, float slope);
   /* the softmax aggregation mode: input x (Model::softmax_gather) */
   AttentionGather(const Model& model, const Tensor& x, float temperature, bool learnTemperature);
+  /* the dot-product mode: inputs q, k, v (Model::dot_attention_gather) */
+  AttentionGather(const Model& model, const Tensor& q, const Tensor& k, const Tensor& v, int heads, float scale);
   virtual void init(const Model& model);
   virtual void forward(const Model& model);
   virtual void backward(const Model& model);
@@ -419,19 +432,22 @@ public:
   uint8_t* keep2;    /* [E] the backward's input-gradient pass's: reverse pairs, or the transposed plan's order */
   float* stats;      /* [Nloc][statsLd] m | 1/Z per head of the last forward (Runtime arena) */
   int64_t statsLd;
-  float* scratch[2]; /* gradients of an input that accumulates (or needs none), written here first (Runtime arena) */
+  float* scratch[3]; /* gradients of an input that accumulates (or needs none), written here first (Runtime arena) */
   bool dynamic;      /* GATv2's dynamic attention: inputs[0] = xl, inputs[1] = xr, parameter a */
   Tensor a;          /* dynamic: parameter, dims {heads, F} (memory a[k][f] at f * heads + k) */
   bool softmax;      /* the softmax aggregation: inputs[0] = x, stats [Nloc][statsLd] m | 1/Z per column */
   bool learnTemperature;   /* softmax: t is the parameter `temperature` */
   Tensor temperature;      /* softmax with learnTemperature: parameter, dims {1, 1} */
   float* tConst;     /* softmax without it: t in one device float (Runtime arena) */
+  bool dot;          /* dot-product attention: inputs[0] = q, inputs[1] = k, inputs[2] = v */
+  float scale;       /* dot: the logits' scale */
 private:
   float drop_rate(const Model& model) const;
   uint64_t drop_key() const;
   void keep_mask(const Model& model, const roc_sg_plan* plan, roc_vid_t selfBase, int rowIsSource, uint8_t*& buf);
   void dynamic_backward(const Model& model);
   void softmax_backward(const Model& model);
+  void dot_backward(const Model& model);
 };
 
 class AttentionScores : public GnnOp {  /* not in the reference: Model::attention_scores */

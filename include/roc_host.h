@@ -55,6 +55,8 @@ int roc_host_attention_gather_dropout(roc_host* h, int t, int scores, int heads,
 int roc_host_dynamic_attention_gather(roc_host* h, int xl, int xr, int heads, float slope);
 /* Model::softmax_gather(t, temperature, learnTemperature): softmax aggregation with one temperature */
 int roc_host_softmax_gather(roc_host* h, int t, float temperature, int learnTemperature);
+/* Model::dot_attention_gather(q, k, v, heads, scale): dot-product attention; q, k and v may be one tensor */
+int roc_host_dot_attention_gather(roc_host* h, int q, int k, int v, int heads, float scale);
 /* Model::create_edge_tensor<float>(hidden): rows = this partition's edge count */
 int roc_host_create_edge_tensor(roc_host* h, int hidden);
 /* Model::scatter_gather(t, edges): edge-weighted aggregation */

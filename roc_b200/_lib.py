@@ -169,6 +169,11 @@ PROTOTYPES = {
                                               i64, vp, i64, vp, vp]),
     "roc_sg_attn_v2_backward_exact": (i32, [vp, vp, i32, i32, f32, vp, i64, vp, i64, vp, vp, i64, vp, i64, vp, i64,
                                             vp, i64, vp, i64, vp, vp]),
+    "roc_sg_attn_dot_forward_planned": (i32, [vp, i32, i32, f32, vp, i64, vp, i64, vp, i64, vp, i64, vp, i64, vp]),
+    "roc_sg_attn_dot_backward_planned": (i32, [vp, i32, i32, f32, vp, i64, vp, i64, vp, i64, vp, i64, vp, i64, vp, i64,
+                                               vp, i64, vp, i64, vp, i64, vp]),
+    "roc_sg_attn_dot_backward_exact": (i32, [vp, vp, i32, i32, f32, vp, i64, vp, i64, vp, i64, vp, i64, vp, i64, vp,
+                                             i64, vp, i64, vp, i64, vp, i64, vp]),
     "roc_sg_softmax_forward_planned": (i32, [vp, i32, vp, vp, i64, vp, i64, vp, i64, vp]),
     "roc_sg_softmax_backward_planned": (i32, [vp, i32, vp, vp, i64, vp, i64, vp, i64, vp, i64, vp, i64, vp, vp]),
     "roc_sg_softmax_backward_exact": (i32, [vp, vp, i32, vp, vp, i64, vp, i64, vp, i64, vp, i64, vp, i64, vp, vp]),
@@ -268,6 +273,7 @@ PROTOTYPES = {
     "roc_host_attention_gather": (i32, [vp, i32, i32, i32, f32]),
     "roc_host_dynamic_attention_gather": (i32, [vp, i32, i32, i32, f32]),
     "roc_host_softmax_gather": (i32, [vp, i32, f32, i32]),
+    "roc_host_dot_attention_gather": (i32, [vp, i32, i32, i32, i32, f32]),
     "roc_host_attention_gather_dropout": (i32, [vp, i32, i32, i32, f32, f32, i32]),
     "roc_host_scatter_gather_dropout": (i32, [vp, i32, f32, i32]),
     "roc_host_get_aggr_index": (i32, [vp, i32, vp]),

@@ -110,6 +110,9 @@ int roc_host_dynamic_attention_gather(roc_host* h, int xl, int xr, int heads, fl
 int roc_host_softmax_gather(roc_host* h, int t, float temperature, int learnTemperature) {
   return h->push(h->m().softmax_gather(h->at(t), temperature, learnTemperature != 0));
 }
+int roc_host_dot_attention_gather(roc_host* h, int q, int k, int v, int heads, float scale) {
+  return h->push(h->m().dot_attention_gather(h->at(q), h->at(k), h->at(v), heads, scale));
+}
 int roc_host_create_edge_tensor(roc_host* h, int hidden) { return h->push(h->m().create_edge_tensor<DATATYPE>(hidden)); }
 int roc_host_scatter_gather_weighted(roc_host* h, int t, int edges) {
   return h->push(h->m().scatter_gather(h->at(t), h->at(edges)));

@@ -182,6 +182,14 @@ Tensor Model::softmax_gather(const Tensor& x, float temperature, bool learnTempe
   if (learnTemperature) parameters.push_back(op->temperature);
   return op->outputs[0];
 }
+Tensor Model::dot_attention_gather(const Tensor& q, const Tensor& k, const Tensor& v, int heads, float scale) {
+  if (ctx->numParts > 1)
+    ROC_FATAL("dot_attention_gather: runs on one partition only (numParts > 1 is not supported)");
+  AttentionGather* op = new AttentionGather(*this, q, k, v, heads, scale);
+  op->opIndex = (int)layers.size();
+  layers.push_back(op);
+  return op->outputs[0];
+}
 Tensor Model::attention_scores(const Tensor& input, int heads) {
   if (ctx->numParts > 1)
     ROC_FATAL("attention_scores: runs on one partition only (numParts > 1 is not supported)");
@@ -714,9 +722,9 @@ static void choose_bf16_aggregation(RuntimeImpl* rt, const std::vector<GnnOp*>& 
         if (op->inputs[j].region != r) continue;
         ScatterGather* sg = as<ScatterGather>(op);
         Linear* lin = as<Linear>(op);
-        AttentionGather* ag = as<AttentionGather>(op);   // dynamic and softmax ones have no bf16 form: they read fp32
+        AttentionGather* ag = as<AttentionGather>(op);   // dynamic, softmax and dot ones have no bf16 form: they read fp32
         if (j == 0 && ((sg && sg->aggr != AGGR_SUM) || as<WeightedScatterGather>(op) ||
-                       (ag && !ag->dynamic && !ag->softmax)))
+                       (ag && !ag->dynamic && !ag->softmax && !ag->dot)))
           aggregated = true;
         else if (!(j == 0 && ((lin && lin->dropOp < 0) || as<AttentionScores>(op))))
           others = false;
@@ -1285,8 +1293,8 @@ AttentionGather::AttentionGather(const Model& model, const Tensor& _input, const
                                  float _dropRate, int _seed)
     : GnnOp(_input, _scores), heads(_heads), slope(_slope), dropRate(_dropRate), seed(_seed), opIndex(0),
       keep(nullptr), keep2(nullptr), stats(nullptr), statsLd(0), dynamic(false), softmax(false),
-      learnTemperature(false), tConst(nullptr) {
-  scratch[0] = scratch[1] = nullptr;
+      learnTemperature(false), tConst(nullptr), dot(false), scale(0.0f) {
+  scratch[0] = scratch[1] = scratch[2] = nullptr;
   ROC_ASSERT(_input.type == Tensor::NODE_TENSOR && _scores.type == Tensor::NODE_TENSOR);
   ROC_ASSERT(_input.numDim == 2 && _scores.numDim == 2);
   ROC_ASSERT(_input.dims[1] == model.myGraph.numNodes && _scores.dims[1] == model.myGraph.numNodes);
@@ -1308,8 +1316,9 @@ AttentionGather::AttentionGather(const Model& model, const Tensor& _input, const
 // its gradient through scratch, as any input another op already wrote).
 AttentionGather::AttentionGather(const Model& model, const Tensor& xl, const Tensor& xr, int _heads, float _slope)
     : GnnOp(xl, xr), heads(_heads), slope(_slope), dropRate(0.0f), seed(0), opIndex(0), keep(nullptr), keep2(nullptr),
-      stats(nullptr), statsLd(0), dynamic(true), softmax(false), learnTemperature(false), tConst(nullptr) {
-  scratch[0] = scratch[1] = nullptr;
+      stats(nullptr), statsLd(0), dynamic(true), softmax(false), learnTemperature(false), tConst(nullptr),
+      dot(false), scale(0.0f) {
+  scratch[0] = scratch[1] = scratch[2] = nullptr;
   ROC_ASSERT(xl.type == Tensor::NODE_TENSOR && xr.type == Tensor::NODE_TENSOR);
   ROC_ASSERT(xl.numDim == 2 && xr.numDim == 2);
   ROC_ASSERT(xl.dims[1] == model.myGraph.numNodes && xr.dims[1] == model.myGraph.numNodes);
@@ -1330,8 +1339,9 @@ AttentionGather::AttentionGather(const Model& model, const Tensor& xl, const Ten
 // without a random draw.
 AttentionGather::AttentionGather(const Model& model, const Tensor& x, float _temperature, bool _learn)
     : GnnOp(x), heads(1), slope(0.0f), dropRate(0.0f), seed(0), opIndex(0), keep(nullptr), keep2(nullptr),
-      stats(nullptr), statsLd(0), dynamic(false), softmax(true), learnTemperature(_learn), tConst(nullptr) {
-  scratch[0] = scratch[1] = nullptr;
+      stats(nullptr), statsLd(0), dynamic(false), softmax(true), learnTemperature(_learn), tConst(nullptr),
+      dot(false), scale(0.0f) {
+  scratch[0] = scratch[1] = scratch[2] = nullptr;
   ROC_ASSERT(x.type == Tensor::NODE_TENSOR && x.numDim == 2 && x.dims[1] == model.myGraph.numNodes);
   if (!std::isfinite(_temperature)) ROC_FATAL("softmax_gather: the temperature must be finite");
   if (model.ctx->t(x.region).isBf16) ROC_FATAL("softmax_gather: x must be fp32 (there is no bf16 form)");
@@ -1348,11 +1358,38 @@ AttentionGather::AttentionGather(const Model& model, const Tensor& x, float _tem
   numOutputs = 1;
   outputs[0] = model.create_node_tensor<DATATYPE>((int)x.dims[0]);
 }
+// The dot-product mode: q, k and v are the op's three inputs, one region more than once when they are one tensor (a
+// later one then adds its gradient through scratch, as any input another op already wrote).  No parameter.
+AttentionGather::AttentionGather(const Model& model, const Tensor& q, const Tensor& k, const Tensor& v, int _heads,
+                                 float _scale)
+    : GnnOp(q, k, v), heads(_heads), slope(0.0f), dropRate(0.0f), seed(0), opIndex(0), keep(nullptr), keep2(nullptr),
+      stats(nullptr), statsLd(0), dynamic(false), softmax(false), learnTemperature(false), tConst(nullptr), dot(true),
+      scale(_scale) {
+  scratch[0] = scratch[1] = scratch[2] = nullptr;
+  for (const Tensor* t : {&q, &k, &v}) {
+    ROC_ASSERT(t->type == Tensor::NODE_TENSOR && t->numDim == 2 && t->dims[1] == model.myGraph.numNodes);
+    if (model.ctx->t(t->region).isBf16)
+      ROC_FATAL("dot_attention_gather: q, k and v must be fp32 (there is no bf16 form)");
+  }
+  const int64_t H = (int64_t)q.dims[0];
+  if (k.dims[0] != q.dims[0] || v.dims[0] != q.dims[0])
+    ROC_FATAL("dot_attention_gather: q, k and v must have the same width");
+  if (_heads <= 0 || _heads > 8 || H % _heads)
+    ROC_FATAL("dot_attention_gather: the width must be heads * F with 1 <= heads <= 8");
+  if (H > 256) ROC_FATAL("dot_attention_gather: the width must be at most 256");
+  if (_scale == 0.0f || !std::isfinite(_scale)) ROC_FATAL("dot_attention_gather: the scale must be finite and not 0");
+  numOutputs = 1;
+  outputs[0] = model.create_node_tensor<DATATYPE>((int)H);
+}
 void AttentionGather::init(const Model& model) {
   if (dynamic && (model.ctx->t(inputs[0].region).isBf16 || model.ctx->t(inputs[1].region).isBf16))
     ROC_FATAL("dynamic_attention_gather: xl and xr must be fp32 (there is no bf16 form)");
   if (softmax && model.ctx->t(inputs[0].region).isBf16)
     ROC_FATAL("softmax_gather: x must be fp32 (there is no bf16 form)");
+  if (dot)
+    for (int i = 0; i < 3; i++)
+      if (model.ctx->t(inputs[i].region).isBf16)
+        ROC_FATAL("dot_attention_gather: q, k and v must be fp32 (there is no bf16 form)");
 }
 
 // the attention dropout rate in the current mode (infer: none) and its Philox key
@@ -1382,6 +1419,21 @@ void AttentionGather::forward(const Model& model) {
     rt->sg_begin(H);
     ROC_CHECK(roc_sg_softmax_forward_planned(model.myGraph.plan, H, t, rt->data(x), rt->t(x).ld, rt->data(y),
                                              rt->t(y).ld, train ? stats : nullptr, statsLd, rt->stream));
+    rt->sg_end();
+    return;
+  }
+  if (dot) {
+    // a training forward keeps m | 1/Z per head for the backward; an inference forward writes none
+    const bool train = model.mode == MD_MODE_TRAIN;
+    if (train && !stats) {
+      statsLd = round_up4(2 * heads);
+      stats = (float*)rt->dmalloc((size_t)std::max<int64_t>(model.local_rows(), 1) * (size_t)statsLd * sizeof(float));
+    }
+    const int q = inputs[0].region, k = inputs[1].region, v = inputs[2].region, y = outputs[0].region;
+    rt->sg_begin(H);
+    ROC_CHECK(roc_sg_attn_dot_forward_planned(model.myGraph.plan, heads, H, scale, rt->data(q), rt->t(q).ld,
+                                              rt->data(k), rt->t(k).ld, rt->data(v), rt->t(v).ld, rt->data(y),
+                                              rt->t(y).ld, train ? stats : nullptr, statsLd, rt->stream));
     rt->sg_end();
     return;
   }
@@ -1424,6 +1476,10 @@ void AttentionGather::backward(const Model& model) {
   }
   if (softmax) {
     softmax_backward(model);
+    return;
+  }
+  if (dot) {
+    dot_backward(model);
     return;
   }
   if (!rt->t(inputs[0].region).requiresGrad && !rt->t(inputs[1].region).requiresGrad) return;
@@ -1517,6 +1573,34 @@ void AttentionGather::softmax_backward(const Model& model) {
                                               statsLd, rt->grad(y), ldY, dx, ldX, dt, rt->stream));
   rt->sg_end();
   if (wantDx && !resetInputGrads[0]) add_scratch(model, x, scratch[0]);
+}
+
+// dq, dk and dv from the same CSR, or over the transpose with the exact backward.  The kernels overwrite all three: an
+// input whose gradient another op already wrote (or a repeat of an earlier input) takes its part through scratch,
+// added afterwards; so does one that needs no gradient.
+void AttentionGather::dot_backward(const Model& model) {
+  RuntimeImpl* rt = model.ctx;
+  bool any = false;
+  for (int i = 0; i < 3; i++) any = any || rt->t(inputs[i].region).requiresGrad;
+  if (!any) return;
+  const int H = (int)inputs[0].dims[0];
+  const int q = inputs[0].region, k = inputs[1].region, v = inputs[2].region, y = outputs[0].region;
+  float* dst[3];
+  for (int i = 0; i < 3; i++)
+    dst[i] = grad_or_scratch(model, inputs[i].region, rt->t(inputs[i].region).requiresGrad && resetInputGrads[i], scratch[i]);
+  const int64_t ldQ = rt->t(q).ld, ldK = rt->t(k).ld, ldV = rt->t(v).ld, ldY = rt->t(y).ld;
+  rt->sg_begin(H);
+  if (model.exactBackward)
+    ROC_CHECK(roc_sg_attn_dot_backward_exact(model.myGraph.plan, rt->sgTranspose, heads, H, scale, rt->data(q), ldQ,
+                                             rt->data(k), ldK, rt->data(v), ldV, rt->data(y), ldY, stats, statsLd,
+                                             rt->grad(y), ldY, dst[0], ldQ, dst[1], ldK, dst[2], ldV, rt->stream));
+  else
+    ROC_CHECK(roc_sg_attn_dot_backward_planned(model.myGraph.plan, heads, H, scale, rt->data(q), ldQ, rt->data(k), ldK,
+                                               rt->data(v), ldV, rt->data(y), ldY, stats, statsLd, rt->grad(y), ldY,
+                                               dst[0], ldQ, dst[1], ldK, dst[2], ldV, rt->stream));
+  rt->sg_end();
+  for (int i = 0; i < 3; i++)
+    if (rt->t(inputs[i].region).requiresGrad && !resetInputGrads[i]) add_scratch(model, inputs[i].region, scratch[i]);
 }
 
 // ------------------------------------------------------- AttentionScores -----

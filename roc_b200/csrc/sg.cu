@@ -59,6 +59,9 @@
 //  * softmax aggregation (roc_sg_softmax_*, PyG's SoftmaxAggregation) runs on its own kernel, sg_smx_kernel (end of
 //    file), with the schedule of sg_v2_kernel: a one-pass online softmax per column forward, finished by its own
 //    rescale-and-add fix-ups (sg_smx_fixup), and a record pass and a source pass backward, finished by the sum's.
+//  * dot-product attention (roc_sg_attn_dot_*, the graph transformer's) runs on its own kernel, sg_dot_kernel (end of
+//    file), with the same schedule: a one-pass online softmax per head forward, finished by sg_dot_fixup, and
+//    GATv2's record pass, a destination pass and a source pass backward, finished by the sum's fix-ups.
 //
 // Algorithmic bytes per launch (DESIGN.md): E*(4H+4) + Nloc*(4H+8); min / max forward E*(4H+4) + Nloc*(8H+8),
 // backward E*(8H+4) + Nloc*(4H+8); the sum over bf16 rows E*(2H+4) + Nloc*(4H+8); weighted forward E*(4H+8) + Nloc*(4H+8), edge dot E*(4H+8) + Nloc*4H; attention
@@ -3551,4 +3554,508 @@ extern "C" int roc_sg_softmax_backward_exact(const roc_sg_plan* plc, roc_sg_tran
       pl->nloc != tr->N || pl->E != tr->E)
     return ROC_ERR_INVALID;
   return smx_backward(pl, tr->planT, H, t, x, ldX, y, ldY, stats, ldStats, gy, ldG, dx, ldDx, dt, as_stream(stream));
+}
+
+// ------------------------------------------------ dot-product attention ---
+// roc_sg_attn_dot_*: the graph transformer's attention (PyG TransformerConv, UniMP): s(v<-u, k) = scale q[v]_k . k[u]_k
+// and out[v]_k = sum_u softmax_u(s) v[u]_k.  The passes run on their own kernel, sg_dot_kernel, over the plan's chunks,
+// chunk records and carry slots, one warp per chunk with lane l holding columns l + 32 j (j < J = ceil(H / 32)),
+// scalar, as sg_v2_kernel.  Unlike sg_v2_kernel, every per-head quantity is held per column, replicated over the head's
+// columns, so that the row walk needs no shuffle and no per-head select:
+//  * dot_head_sums reduces a group's U edges' products together, before the row walk.  Where F divides 32 a head's
+//    columns sit at one lane each within an aligned group of F lanes, and each is reduced over those lanes alone
+//    (log2 F xor levels); otherwise each head is summed over the lane's columns in column order, then over the warp by
+//    an xor butterfly.  The order depends on (H, heads) only and every lane of a head ends with the same bits, so the
+//    forward and both backward passes see the same s.
+//  * the forward is one pass with an online softmax per head, kept per column as (m, s, w) = (max s, sum exp(s - m),
+//    sum exp(s - m) v): the softmax aggregation's scheme, whose merge (smx_merge) and store (smx_store) it reuses.
+//    A cut row's owner stores w and its per-head (m, s); the carries hold [m | s | w] per column; sg_dot_fixup merges
+//    them in chunk order.
+//  * the backward is the record pass of GATv2 (sg_v2_rec_kernel: {m, 1/Z, c} per head), a destination pass (dq) and a
+//    source pass (dk, dv), finished by the sum's fix-ups.
+namespace roc {
+
+enum { SG_DOT_FWD = 0, SG_DOT_DST = 1, SG_DOT_SRC = 2 };
+constexpr int SG_RED_DOT = 80;                // the `red` sg_last_call_info reports for pass P is SG_RED_DOT + P
+
+struct DotParams {
+  const uint32_t* rs;
+  const uint32_t* col;
+  const uint32_t* desc;
+  const uint32_t* carryIdx;
+  const uint32_t* heavyRows;
+  const uint32_t* bigRows;
+  uint32_t E, numChunks, numHeavy, numBig, H, heads;
+  float scale;
+  const float* g;  size_t ldG;    // gathered rows (by col id): FWD, DST k; SRC q
+  const float* g2; size_t ldG2;   // FWD, DST v; SRC gy
+  const float* o;  size_t ldO;    // the row's own row: FWD, DST q; SRC k
+  const float* o2; size_t ldO2;   // DST gy; SRC v
+  const float4* rec;              // DST, SRC: {m, 1/Z, c, 0} per (id, head)
+  float* out;  size_t ldOut;      // FWD y (a cut row's owner: w); DST dq; SRC dk
+  float* out2; size_t ldOut2;     // SRC dv
+  float* stats; size_t ldStats;   // FWD: m | 1/Z per head of finished rows (nullptr: none)
+  float* raw;  size_t ldRaw;      // FWD: a cut row's owner's raw m | s per head (stats, or a workspace)
+  float* carry; size_t ldC;       // FWD [m | s | w]; DST dq; SRC [dk | dv]
+};
+
+// r[n][j] = the sum over the warp of t[n] over the columns of head hj[j] (the fixed order described above); N rows of
+// products reduced together, each xor level issued for all of them at once.
+template <int N, int J>
+__device__ __forceinline__ void dot_head_sums(const float (&t)[N][J], const int (&hj)[J], uint32_t heads, uint32_t F,
+                                              float (&r)[N][J]) {
+  if (32u % F == 0u) {
+#pragma unroll
+    for (int n = 0; n < N; n++)
+#pragma unroll
+      for (int j = 0; j < J; j++) r[n][j] = t[n][j];
+#pragma unroll
+    for (int o = 16; o >= 1; o >>= 1)
+      if ((uint32_t)o < F) {
+#pragma unroll
+        for (int n = 0; n < N; n++)
+#pragma unroll
+          for (int j = 0; j < J; j++) r[n][j] = __fadd_rn(r[n][j], __shfl_xor_sync(0xffffffffu, r[n][j], o));
+      }
+  } else {
+#pragma unroll
+    for (int n = 0; n < N; n++)
+#pragma unroll
+      for (int j = 0; j < J; j++) r[n][j] = 0.f;
+#pragma unroll
+    for (int k = 0; k < SG_V2_HEADS; k++) {
+      if ((uint32_t)k < heads) {
+        float x[N];
+#pragma unroll
+        for (int n = 0; n < N; n++) {
+          x[n] = 0.f;
+#pragma unroll
+          for (int j = 0; j < J; j++) x[n] = __fadd_rn(x[n], hj[j] == k ? t[n][j] : 0.f);
+        }
+#pragma unroll
+        for (int o = 16; o >= 1; o >>= 1)
+#pragma unroll
+          for (int n = 0; n < N; n++) x[n] = __fadd_rn(x[n], __shfl_xor_sync(0xffffffffu, x[n], o));
+#pragma unroll
+        for (int n = 0; n < N; n++)
+#pragma unroll
+          for (int j = 0; j < J; j++) r[n][j] = hj[j] == k ? x[n] : r[n][j];
+      }
+    }
+  }
+}
+
+// One warp per chunk of the plan, the schedule of sg_v2_kernel.  Per edge (row v's edge from u in the forward plan),
+// with s = scale q[v] . k[u] per head:
+//   FWD  online (m, s, w) per column of s and v[u];
+//   DST  p = exp(s - m) / Z, d = p (gy[v] . v[u] - c[v]), dq[v] += scale d k[u];
+//   SRC  (row u, gathering v and v's record) dk[u] += scale d q[v], dv[u] += p gy[v].
+// The dot products of a group of U edges are taken together with the current row's own row, before the walk over the
+// rows the group spans; a row that starts inside the group takes them again for the whole group.  The per-edge branch
+// of the walk holds no shuffle.  __launch_bounds__(SG_THREADS, 1) as sg_v2_kernel: it lets ptxas use up to 255
+// registers, so that no instantiation needs local memory.
+template <int J, int PASS>
+__global__ void __launch_bounds__(SG_THREADS, 1)
+sg_dot_kernel(const DotParams p) {
+  constexpr bool FWD = PASS == SG_DOT_FWD, DST = PASS == SG_DOT_DST, SRC = PASS == SG_DOT_SRC;
+  constexpr int ND = FWD ? 1 : 2;               // dot products per edge and head
+  constexpr int U = FWD ? (J <= 2 ? 8 : J <= 4 ? 4 : 2) : (J <= 2 ? 4 : J <= 4 ? 2 : 1);   // edges in flight
+  constexpr int WPB = SG_THREADS / 32;
+  constexpr uint32_t CH = SG_CH;
+  const int lane = threadIdx.x % 32;
+  const uint32_t w = blockIdx.x * WPB + threadIdx.x / 32;
+  if (w >= p.numChunks) return;
+  const uint32_t* dsc = p.desc + 8 * (size_t)w;
+  const uint32_t flags = __ldg(dsc + 6);
+  if (flags & 2u) return;
+  const uint32_t ce = min(w * CH + CH, p.E);
+  uint32_t cur = __ldg(dsc + 2), curS = __ldg(dsc + 3), curT = __ldg(dsc + 4);
+  const uint32_t e0 = __ldg(dsc), ee = __ldg(dsc + 1), r1 = __ldg(dsc + 5), carrySlot = __ldg(dsc + 7);
+  int kind = (flags & 1u) ? 0 : ((curT - curS > CH) ? 2 : 1);   // 0 carry-in part, 1 complete row, 2 cut row's owner
+  uint32_t segEnd = (kind == 1) ? curT : min(curT, ce);
+
+  const uint32_t H = p.H, heads = p.heads, F = H / heads;
+  const float scale = p.scale;
+  int hj[J];
+  bool vj[J], lead[J];          // lead: the head's first column, which stores its per-head values
+#pragma unroll
+  for (int j = 0; j < J; j++) {
+    const uint32_t c = (uint32_t)(lane + 32 * j);
+    vj[j] = c < H;
+    hj[j] = vj[j] ? (int)(c / F) : -1;
+    lead[j] = vj[j] && c % F == 0u;
+  }
+  float xo[J], yo[FWD ? 1 : J];               // the row's own rows: FWD q; DST q, gy; SRC k, v
+  float rm[DST ? J : 1], ri[DST ? J : 1], rc[DST ? J : 1];   // DST: the row's m, 1/Z and c per column
+  float sm[FWD ? J : 1], ss[FWD ? J : 1];     // FWD: running m, s (acc: w)
+  float acc[J], acc2[SRC ? J : 1];
+#pragma unroll
+  for (int j = 0; j < J; j++) {
+    acc[j] = 0.f;
+    if constexpr (SRC) acc2[j] = 0.f;
+    if constexpr (FWD) { sm[j] = -INFINITY; ss[j] = 0.f; }
+  }
+
+  auto row_state = [&]() {
+    v2_load_row<J>(p.o + (uint64_t)cur * p.ldO, lane, vj, xo);
+    if constexpr (!FWD) v2_load_row<J>(p.o2 + (uint64_t)cur * p.ldO2, lane, vj, yo);
+    if constexpr (DST) {
+#pragma unroll
+      for (int j = 0; j < J; j++) {
+        const float4 r = vj[j] ? __ldg(p.rec + (uint64_t)cur * heads + hj[j]) : make_float4(0.f, 0.f, 0.f, 0.f);
+        rm[j] = r.x; ri[j] = r.y; rc[j] = r.z;
+      }
+    }
+  };
+  row_state();
+
+  auto flush = [&]() {
+    if constexpr (FWD) {
+      if (kind == 0) {
+        float* c = p.carry + (uint64_t)carrySlot * p.ldC;
+#pragma unroll
+        for (int j = 0; j < J; j++)
+          if (vj[j]) { c[lane + 32 * j] = sm[j]; c[H + lane + 32 * j] = ss[j]; c[2 * H + lane + 32 * j] = acc[j]; }
+      } else {
+        float* y = p.out + (uint64_t)cur * p.ldOut;
+#pragma unroll
+        for (int j = 0; j < J; j++) {
+          if (!vj[j]) continue;
+          const uint32_t c = lane + 32 * j, h = (uint32_t)hj[j];
+          if (kind == 2) {    // the raw partial, for sg_dot_fixup
+            y[c] = acc[j];
+            if (lead[j]) { p.raw[(uint64_t)cur * p.ldRaw + h] = sm[j]; p.raw[(uint64_t)cur * p.ldRaw + heads + h] = ss[j]; }
+          } else {
+            float* st = p.stats + (uint64_t)cur * p.ldStats;
+            smx_store(sm[j], ss[j], acc[j], y + c, st + h, st + heads + h, p.stats && lead[j]);
+          }
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < J; j++) { sm[j] = -INFINITY; ss[j] = 0.f; acc[j] = 0.f; }
+    } else {
+      float* d1 = (kind == 0) ? p.carry + (uint64_t)carrySlot * p.ldC : p.out + (uint64_t)cur * p.ldOut;
+      float* d2 = (kind == 0) ? d1 + H : p.out2 + (uint64_t)cur * p.ldOut2;
+      (void)d2;
+#pragma unroll
+      for (int j = 0; j < J; j++) {
+        if (vj[j]) {
+          d1[lane + 32 * j] = acc[j];
+          if constexpr (SRC) d2[lane + 32 * j] = acc2[j];
+        }
+        acc[j] = 0.f;
+        if constexpr (SRC) acc2[j] = 0.f;
+      }
+    }
+  };
+  auto advance = [&]() {
+    cur += 1; curS = curT; curT = p.rs[cur + 1];
+    const bool heavy = curT - curS > CH;
+    segEnd = heavy ? min(curT, ce) : curT;
+    kind = heavy ? 2 : 1;
+    row_state();
+  };
+
+  const uint32_t eLast = ee - 1u;
+#pragma unroll 1
+  for (uint32_t base = e0; base < ee; base += U) {
+    const uint32_t cnt = min((uint32_t)U, ee - base);
+    float ga[U][J], gb[U][J];        // FWD, DST: k[u], v[u]; SRC: q[v], gy[v]
+    float4 gr[SRC ? U : 1][SRC ? J : 1];
+#pragma unroll
+    for (int u = 0; u < U; u++) {
+      const uint32_t id = __ldg(p.col + min(base + (uint32_t)u, eLast));
+      v2_load_row<J>(p.g + (uint64_t)id * p.ldG, lane, vj, ga[u]);
+      v2_load_row<J>(p.g2 + (uint64_t)id * p.ldG2, lane, vj, gb[u]);
+      if constexpr (SRC) {
+#pragma unroll
+        for (int j = 0; j < J; j++)
+          gr[u][j] = vj[j] ? __ldg(p.rec + (uint64_t)id * heads + hj[j]) : make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+    }
+    uint32_t pos = 0;
+    for (;;) {
+      const uint32_t lim = min(cnt, segEnd - base);
+      if (lim > pos) {
+        // the group's dot products with this row: q . k (and gy . v) per edge and head, all U edges together
+        float t[ND * U][J], d[ND * U][J];
+#pragma unroll
+        for (int u = 0; u < U; u++)
+#pragma unroll
+          for (int j = 0; j < J; j++) {
+            t[ND * u][j] = __fmul_rn(xo[j], ga[u][j]);
+            if constexpr (DST) t[ND * u + 1][j] = __fmul_rn(yo[j], gb[u][j]);
+            if constexpr (SRC) t[ND * u + 1][j] = __fmul_rn(gb[u][j], yo[j]);
+          }
+        dot_head_sums<ND * U, J>(t, hj, heads, F, d);
+#pragma unroll
+        for (int u = 0; u < U; u++) {
+          if ((uint32_t)u >= pos && (uint32_t)u < lim) {
+#pragma unroll
+            for (int j = 0; j < J; j++) {
+              const float e = __fmul_rn(scale, d[ND * u][j]);
+              if constexpr (FWD) {
+                const float x = gb[u][j];
+                if (e > sm[j]) {
+                  const float c = expf(sm[j] - e);
+                  ss[j] = fmaf(ss[j], c, 1.f); acc[j] = fmaf(acc[j], c, x); sm[j] = e;
+                } else {
+                  const float q = expf(e - sm[j]);
+                  ss[j] = __fadd_rn(ss[j], q); acc[j] = fmaf(q, x, acc[j]);
+                }
+              } else {
+                const float m = SRC ? gr[u][j].x : rm[j], iz = SRC ? gr[u][j].y : ri[j];
+                const float c = SRC ? gr[u][j].z : rc[j];
+                const float pk = attn_alpha(e, m, iz);
+                const float ds = __fmul_rn(scale, __fmul_rn(pk, __fsub_rn(d[ND * u + 1][j], c)));
+                acc[j] = fmaf(ds, ga[u][j], acc[j]);
+                if constexpr (SRC) acc2[j] = fmaf(pk, gb[u][j], acc2[j]);
+              }
+            }
+          }
+        }
+      }
+      pos = lim;
+      if (pos >= cnt) break;
+      flush();
+      advance();
+    }
+  }
+  flush();
+  while (cur + 1 < r1) { advance(); flush(); }   // trailing zero-degree rows
+}
+
+// Finishes the forward's cut rows, as sg_smx_fixup with the owner's (m, s) per head: the owner's raw partial (y: w,
+// raw: m | s per head), then the carries in chunk order, stored as y and, with stats, m | 1/Z per head.  Heavy rows (at
+// most 32 carries): one warp each.  BIG rows: one CTA each, whose warps merge contiguous blocks of the carries, then
+// warp 0 the owner's partial and the blocks' in block order.  The grouping depends on the plan only.
+template <int J, bool BIG>
+__global__ void __launch_bounds__(SG_THREADS, 1)
+sg_dot_fixup(const DotParams p) {
+  constexpr uint32_t CH = SG_CH;
+  constexpr int WPB = SG_THREADS / 32;
+  const int lane = threadIdx.x % 32, g = threadIdx.x / 32;
+  const uint32_t w = BIG ? blockIdx.x : blockIdx.x * WPB + g;
+  if (w >= (BIG ? p.numBig : p.numHeavy)) return;
+  const uint32_t R = BIG ? p.bigRows[w] : p.heavyRows[w];
+  const uint32_t s = p.rs[R], t = p.rs[R + 1];
+  const uint32_t c0 = s / CH, n = (t - 1) / CH - c0;
+  const float* cb = p.carry + (uint64_t)p.carryIdx[c0 + 1] * p.ldC;
+  const uint32_t H = p.H, heads = p.heads, F = H / heads;
+  float* y = p.out + (uint64_t)R * p.ldOut;
+  const float* raw = p.raw + (uint64_t)R * p.ldRaw;
+  uint32_t hc[J];               // the head of each of the lane's columns
+  bool vj[J];
+#pragma unroll
+  for (int j = 0; j < J; j++) { vj[j] = (uint32_t)(lane + 32 * j) < H; hc[j] = vj[j] ? (lane + 32 * j) / F : 0u; }
+  uint32_t k0 = 0, k1 = n;
+  if constexpr (BIG) { const uint32_t per = (n + WPB - 1) / WPB; k0 = min(n, g * per); k1 = min(n, k0 + per); }
+  float m[J], z[J], a[J];
+#pragma unroll
+  for (int j = 0; j < J; j++) { m[j] = -INFINITY; z[j] = 0.f; a[j] = 0.f; }
+  if (!BIG) {   // a heavy row starts from its owner's partial
+#pragma unroll
+    for (int j = 0; j < J; j++)
+      if (vj[j]) { m[j] = raw[hc[j]]; z[j] = raw[heads + hc[j]]; a[j] = y[lane + 32 * j]; }
+  }
+  for (uint32_t k = k0; k < k1; k++) {
+    const float* ck = cb + (uint64_t)k * p.ldC;
+#pragma unroll
+    for (int j = 0; j < J; j++) {
+      const uint32_t c = lane + 32 * j;
+      if (vj[j]) smx_merge(m[j], z[j], a[j], ck[c], ck[H + c], ck[2 * H + c]);
+    }
+  }
+  if constexpr (BIG) {
+    __shared__ float part[WPB][3][32 * J];
+#pragma unroll
+    for (int j = 0; j < J; j++) { part[g][0][lane + 32 * j] = m[j]; part[g][1][lane + 32 * j] = z[j]; part[g][2][lane + 32 * j] = a[j]; }
+    __syncthreads();
+    if (g != 0) return;
+#pragma unroll
+    for (int j = 0; j < J; j++) {
+      const uint32_t c = lane + 32 * j;
+      if (vj[j]) {
+        m[j] = raw[hc[j]]; z[j] = raw[heads + hc[j]]; a[j] = y[c];
+#pragma unroll
+        for (int gg = 0; gg < WPB; gg++) smx_merge(m[j], z[j], a[j], part[gg][0][c], part[gg][1][c], part[gg][2][c]);
+      }
+    }
+  }
+  __syncwarp();   // every lane of a head has read the owner's (m, s) before its first column overwrites them
+  float* st = p.stats ? p.stats + (uint64_t)R * p.ldStats : nullptr;
+#pragma unroll
+  for (int j = 0; j < J; j++) {
+    const uint32_t c = lane + 32 * j;
+    if (vj[j]) smx_store(m[j], z[j], a[j], y + c, st + hc[j], st + heads + hc[j], st && c % F == 0u);
+  }
+}
+
+static DotParams dot_params(const roc_sg_plan* pl, int heads, int H, float scale) {
+  DotParams p;
+  memset(&p, 0, sizeof(p));
+  p.rs = pl->rs; p.col = pl->col; p.desc = pl->desc; p.carryIdx = pl->carryIdx; p.heavyRows = pl->heavyRows;
+  p.bigRows = pl->bigRows; p.E = pl->E; p.numChunks = pl->numChunks; p.numHeavy = pl->numHeavy; p.numBig = pl->numBig;
+  p.H = (uint32_t)H; p.heads = (uint32_t)heads; p.scale = scale; p.carry = pl->carry; p.ldC = pl->carryLd;
+  return p;
+}
+
+// One pass of sg_dot_kernel over pl, then its fix-ups: sg_dot_fixup (FWD), or the sum's over out (and SRC: out2).
+template <int PASS>
+static int dot_pass(const roc_sg_plan* pl, const DotParams& p, cudaStream_t st) {
+  return v2_with_j(p.H, [&](auto J) {
+    constexpr int WPB = SG_THREADS / 32;
+    if (p.numChunks) {
+      const uint32_t grid = (p.numChunks + WPB - 1) / WPB;
+      sg_dot_kernel<J, PASS><<<grid, SG_THREADS, 0, st>>>(p);
+      ROC_LAUNCH_CHECK();
+      note_launch(ROC_SG_LAUNCH_MAIN, SG_RED_DOT + PASS, 1, 32, J, grid);
+    }
+    if constexpr (PASS == SG_DOT_FWD) {
+      if (p.numHeavy) {
+        const uint32_t grid = (p.numHeavy + WPB - 1) / WPB;
+        sg_dot_fixup<J, false><<<grid, SG_THREADS, 0, st>>>(p);
+        ROC_LAUNCH_CHECK();
+        note_launch(ROC_SG_LAUNCH_FIXUP, SG_RED_DOT + PASS, 1, 32, J, grid);
+      }
+      if (p.numBig) {
+        sg_dot_fixup<J, true><<<p.numBig, SG_THREADS, 0, st>>>(p);
+        ROC_LAUNCH_CHECK();
+        note_launch(ROC_SG_LAUNCH_BIG_FIXUP, SG_RED_DOT + PASS, 1, 32, J, p.numBig);
+      }
+      return ROC_OK;
+    } else {
+      int rc = v2_fixups(pl, (int)p.H, p.out, (int64_t)p.ldOut, 0, st);
+      if (rc == ROC_OK && PASS == SG_DOT_SRC) rc = v2_fixups(pl, (int)p.H, p.out2, (int64_t)p.ldOut2, p.H, st);
+      return rc;
+    }
+  });
+}
+
+// The checks every dot-product attention call shares once its pointers and leading dimensions are checked: a scale of
+// 0 or not finite is ROC_ERR_INVALID; H % heads, H > 256, heads > SG_V2_HEADS and a plan whose ids are not all its own
+// rows (a graph slice) are ROC_ERR_UNSUPPORTED.  Then the carries, `cols` floats per slot.
+static int dot_setup(roc_sg_plan* pl, int heads, int H, float scale, int cols, cudaStream_t st) {
+  if (scale == 0.f || !std::isfinite(scale)) return ROC_ERR_INVALID;
+  if (H > 256 || H % heads || heads > SG_V2_HEADS) return ROC_ERR_UNSUPPORTED;
+  int rc = find_id_end(pl, st);
+  if (rc != ROC_OK) return rc;
+  if (pl->idEnd > pl->nloc) return ROC_ERR_UNSUPPORTED;
+  return grow_carries(pl, cols, st);
+}
+
+static int dot_forward(roc_sg_plan* pl, int heads, int H, float scale, const float* q, int64_t ldQ, const float* k,
+                       int64_t ldK, const float* v, int64_t ldV, float* out, int64_t ldOut, float* stats,
+                       int64_t ldStats, cudaStream_t st) {
+  int rc = dot_setup(pl, heads, H, scale, 3 * H, st);
+  if (rc != ROC_OK) return rc;
+  DotParams p = dot_params(pl, heads, H, scale);
+  p.g = k; p.ldG = (size_t)ldK; p.g2 = v; p.ldG2 = (size_t)ldV; p.o = q; p.ldO = (size_t)ldQ;
+  p.out = out; p.ldOut = (size_t)ldOut;
+  if (stats) {
+    p.stats = p.raw = stats; p.ldStats = p.ldRaw = (size_t)ldStats;
+  } else if (pl->numHeavy + pl->numBig) {
+    // without stats, a cut row's owner keeps its raw (m, s) in the plan's workspace (the softmax aggregation's)
+    if ((rc = grow(pl->smxWs, pl->smxWsBytes, (size_t)pl->nloc * 2 * heads * sizeof(float), st)) != ROC_OK) return rc;
+    p.raw = reinterpret_cast<float*>(pl->smxWs); p.ldRaw = 2 * (size_t)heads;
+  }
+  return dot_pass<SG_DOT_FWD>(pl, p, st);
+}
+
+// The backward once its arguments are checked: the records over pl's rows (the GATv2 record kernel), the destination
+// pass over pl, and the source pass over plB (pl itself, or the transposed plan).
+static int dot_backward(roc_sg_plan* pl, roc_sg_plan* plB, int heads, int H, float scale, const float* q, int64_t ldQ,
+                        const float* k, int64_t ldK, const float* v, int64_t ldV, const float* out, int64_t ldOut,
+                        const float* stats, int64_t ldStats, const float* gy, int64_t ldG, float* dq, int64_t ldDq,
+                        float* dk, int64_t ldDk, float* dv, int64_t ldDv, cudaStream_t st) {
+  int rc = dot_setup(pl, heads, H, scale, plB == pl ? 2 * H : H, st);
+  if (rc == ROC_OK && plB != pl) rc = dot_setup(plB, heads, H, scale, 2 * H, st);
+  if (rc != ROC_OK) return rc;
+  const uint32_t n = pl->nloc;
+  if ((rc = grow(pl->attnRec, pl->attnRecBytes, (size_t)n * heads * sizeof(float4), st)) != ROC_OK) return rc;
+  V2Params r = v2_params(pl, heads, H, 0.f, nullptr);
+  r.g = gy; r.ldG = (size_t)ldG; r.o = out; r.ldO = (size_t)ldOut; r.stats = stats; r.ldStats = (size_t)ldStats;
+  r.rec = pl->attnRec;
+  rc = v2_with_j((uint32_t)H, [&](auto J) {
+    if (n) {
+      const uint32_t grid = (n + SG_THREADS / 32 - 1) / (SG_THREADS / 32);
+      sg_v2_rec_kernel<J><<<grid, SG_THREADS, 0, st>>>(r, n);
+      ROC_LAUNCH_CHECK();
+      note_launch(ROC_SG_LAUNCH_RECORD, -1, 1, 32, J, grid);
+    }
+    return ROC_OK;
+  });
+  if (rc == ROC_OK) {   // destination pass: dq
+    DotParams d = dot_params(pl, heads, H, scale);
+    d.g = k; d.ldG = (size_t)ldK; d.g2 = v; d.ldG2 = (size_t)ldV; d.o = q; d.ldO = (size_t)ldQ;
+    d.o2 = gy; d.ldO2 = (size_t)ldG; d.rec = pl->attnRec; d.out = dq; d.ldOut = (size_t)ldDq;
+    rc = dot_pass<SG_DOT_DST>(pl, d, st);
+  }
+  if (rc == ROC_OK) {   // source pass: dk and dv
+    DotParams s = dot_params(plB, heads, H, scale);
+    s.g = q; s.ldG = (size_t)ldQ; s.g2 = gy; s.ldG2 = (size_t)ldG; s.o = k; s.ldO = (size_t)ldK;
+    s.o2 = v; s.ldO2 = (size_t)ldV; s.rec = pl->attnRec; s.out = dk; s.ldOut = (size_t)ldDk;
+    s.out2 = dv; s.ldOut2 = (size_t)ldDv;
+    rc = dot_pass<SG_DOT_SRC>(plB, s, st);
+  }
+  return rc;
+}
+
+// NULL pointers, bad leading dimensions, and outputs that alias each other or an input.
+static bool dot_backward_args_bad(int heads, int H, const float* q, int64_t ldQ, const float* k, int64_t ldK,
+                                  const float* v, int64_t ldV, const float* out, int64_t ldOut, const float* stats,
+                                  int64_t ldStats, const float* gy, int64_t ldG, const float* dq, int64_t ldDq,
+                                  const float* dk, int64_t ldDk, const float* dv, int64_t ldDv) {
+  if (!q || !k || !v || !out || !stats || !gy || !dq || !dk || !dv || heads <= 0 || H <= 0 || ldQ < H || ldK < H ||
+      ldV < H || ldOut < H || ldG < H || ldDq < H || ldDk < H || ldDv < H || ldStats < 2 * (int64_t)heads)
+    return true;
+  if (dq == dk || dq == dv || dk == dv) return true;
+  for (const float* o : {dq, dk, dv})
+    if (o == q || o == k || o == v || o == out || o == stats || o == gy) return true;
+  return false;
+}
+
+}  // namespace roc
+
+extern "C" int roc_sg_attn_dot_forward_planned(const roc_sg_plan* plc, int heads, int H, float scale, const float* q,
+                                               int64_t ldQ, const float* k, int64_t ldK, const float* v, int64_t ldV,
+                                               float* out, int64_t ldOut, float* stats, int64_t ldStats,
+                                               roc_stream_t stream) {
+  roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  clear_launches();
+  if (!pl || !q || !k || !v || !out || heads <= 0 || H <= 0 || ldQ < H || ldK < H || ldV < H || ldOut < H ||
+      (stats && ldStats < 2 * (int64_t)heads) || out == q || out == k || out == v ||
+      (stats && (stats == out || stats == q || stats == k || stats == v)))
+    return ROC_ERR_INVALID;
+  return dot_forward(pl, heads, H, scale, q, ldQ, k, ldK, v, ldV, out, ldOut, stats, ldStats, as_stream(stream));
+}
+
+extern "C" int roc_sg_attn_dot_backward_planned(const roc_sg_plan* plc, int heads, int H, float scale, const float* q,
+                                                int64_t ldQ, const float* k, int64_t ldK, const float* v, int64_t ldV,
+                                                const float* out, int64_t ldOut, const float* stats, int64_t ldStats,
+                                                const float* outGrad, int64_t ldG, float* dq, int64_t ldDq, float* dk,
+                                                int64_t ldDk, float* dv, int64_t ldDv, roc_stream_t stream) {
+  roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  clear_launches();
+  if (!pl || dot_backward_args_bad(heads, H, q, ldQ, k, ldK, v, ldV, out, ldOut, stats, ldStats, outGrad, ldG, dq, ldDq,
+                                   dk, ldDk, dv, ldDv))
+    return ROC_ERR_INVALID;
+  return dot_backward(pl, pl, heads, H, scale, q, ldQ, k, ldK, v, ldV, out, ldOut, stats, ldStats, outGrad, ldG, dq,
+                      ldDq, dk, ldDk, dv, ldDv, as_stream(stream));
+}
+
+extern "C" int roc_sg_attn_dot_backward_exact(const roc_sg_plan* plc, roc_sg_transpose* tr, int heads, int H,
+                                              float scale, const float* q, int64_t ldQ, const float* k, int64_t ldK,
+                                              const float* v, int64_t ldV, const float* out, int64_t ldOut,
+                                              const float* stats, int64_t ldStats, const float* outGrad, int64_t ldG,
+                                              float* dq, int64_t ldDq, float* dk, int64_t ldDk, float* dv,
+                                              int64_t ldDv, roc_stream_t stream) {
+  roc_sg_plan* pl = const_cast<roc_sg_plan*>(plc);
+  clear_launches();
+  if (!pl || !tr || dot_backward_args_bad(heads, H, q, ldQ, k, ldK, v, ldV, out, ldOut, stats, ldStats, outGrad, ldG,
+                                          dq, ldDq, dk, ldDk, dv, ldDv) ||
+      pl->nloc != tr->N || pl->E != tr->E)
+    return ROC_ERR_INVALID;
+  return dot_backward(pl, tr->planT, heads, H, scale, q, ldQ, k, ldK, v, ldV, out, ldOut, stats, ldStats, outGrad, ldG,
+                      dq, ldDq, dk, ldDk, dv, ldDv, as_stream(stream));
 }

@@ -5,7 +5,9 @@ function passes raw device pointers + the current CUDA stream to the C ABI.
 2-D tensors may be row-padded views (stride(0) = ld >= shape[1], stride(1) = 1).
 """
 import ctypes as C
+import math
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -48,6 +50,14 @@ def _smx_t(t, device):
         assert t.numel() == 1 and t.dtype == torch.float32 and t.is_cuda
         return t
     return torch.full((1,), float(t), device=device, dtype=torch.float32)
+
+
+def _dot_scale(q, heads, scale):
+    """The dot-product attention's scale: as given, or 1 / sqrt(F), F = H / heads, computed in double and rounded to
+    fp32 once."""
+    if scale is None:
+        return float(np.float32(1.0 / math.sqrt(q.shape[1] // int(heads))))
+    return float(scale)
 
 
 class SgPlan:
@@ -245,6 +255,32 @@ class SgPlan:
                                                   _ptr(dxr), _ld(dxr), _ptr(da), _stream()),
               "roc_sg_attn_v2_backward_planned")
         return dxl, dxr, da.t()
+
+    def attn_dot_forward(self, q, k, v, heads=1, scale=None, out=None, stats=None, keep_stats=True):
+        """Dot-product attention (roc_sg_attn_dot_forward_planned) -> (out [Nloc][H], stats [Nloc][2*heads] = m | 1/Z
+        per head, or None with keep_stats=False, the inference form).  q, k, v: [Nloc][H] fp32 rows (the plan covers a
+        whole graph; they may be one tensor or column blocks of one buffer); scale: None for 1 / sqrt(F)."""
+        out = self._rows(q) if out is None else out
+        if stats is None and keep_stats:
+            stats = torch.empty((self.nloc, 2 * heads), device=q.device)
+        check(lib.roc_sg_attn_dot_forward_planned(self.handle, int(heads), q.shape[1], _dot_scale(q, heads, scale),
+                                                  _ptr(q), _ld(q), _ptr(k), _ld(k), _ptr(v), _ld(v), _ptr(out),
+                                                  _ld(out), _ptr(stats), _ld(stats) if stats is not None else 0,
+                                                  _stream()), "roc_sg_attn_dot_forward_planned")
+        return out, stats
+
+    def attn_dot_backward(self, q, k, v, out, stats, gy, heads=1, scale=None, dq=None, dk=None, dv=None):
+        """Its backward over the same CSR (exact on a symmetric graph) -> (dq, dk, dv).  When q, k and v are one
+        tensor its gradient is dq + dk + dv."""
+        dq = self._rows(q) if dq is None else dq
+        dk = self._rows(k) if dk is None else dk
+        dv = self._rows(v) if dv is None else dv
+        check(lib.roc_sg_attn_dot_backward_planned(self.handle, int(heads), q.shape[1], _dot_scale(q, heads, scale),
+                                                   _ptr(q), _ld(q), _ptr(k), _ld(k), _ptr(v), _ld(v), _ptr(out),
+                                                   _ld(out), _ptr(stats), _ld(stats), _ptr(gy), _ld(gy), _ptr(dq),
+                                                   _ld(dq), _ptr(dk), _ld(dk), _ptr(dv), _ld(dv), _stream()),
+              "roc_sg_attn_dot_backward_planned")
+        return dq, dk, dv
 
     def softmax_forward(self, x, t, out=None, stats=None, keep_stats=True):
         """Softmax aggregation with temperature t (roc_sg_softmax_forward_planned) -> (out [Nloc][H], stats
@@ -458,6 +494,19 @@ class SgTranspose:
                                                 _ld(dxl), _ptr(dxr), _ld(dxr), _ptr(da), _stream()),
               "roc_sg_attn_v2_backward_exact")
         return dxl, dxr, da.t()
+
+    def attn_dot_backward(self, plan, q, k, v, out, stats, gy, heads=1, scale=None, dq=None, dk=None, dv=None):
+        """roc_sg_attn_dot_backward_exact: SgPlan.attn_dot_backward with the source pass over this transpose, exact on
+        any graph.  plan is the forward's plan of the same graph."""
+        dq = plan._rows(q) if dq is None else dq
+        dk = plan._rows(k) if dk is None else dk
+        dv = plan._rows(v) if dv is None else dv
+        check(lib.roc_sg_attn_dot_backward_exact(plan.handle, self.handle, int(heads), q.shape[1],
+                                                 _dot_scale(q, heads, scale), _ptr(q), _ld(q), _ptr(k), _ld(k), _ptr(v),
+                                                 _ld(v), _ptr(out), _ld(out), _ptr(stats), _ld(stats), _ptr(gy),
+                                                 _ld(gy), _ptr(dq), _ld(dq), _ptr(dk), _ld(dk), _ptr(dv), _ld(dv),
+                                                 _stream()), "roc_sg_attn_dot_backward_exact")
+        return dq, dk, dv
 
     def softmax_backward(self, plan, x, t, out, stats, gy, dx=None, want_dt=True):
         """roc_sg_softmax_backward_exact: SgPlan.softmax_backward with the source pass over this transpose, exact on

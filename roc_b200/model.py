@@ -170,6 +170,22 @@ class Model:
             raise ValueError("temperature must be finite")
         return lib.roc_host_softmax_gather(self.h, t, float(temperature), int(bool(learn_temperature)))
 
+    def dot_attention_gather(self, q, k, v, heads=1, scale=None):
+        """Dot-product attention, the graph transformer layer's (PyG TransformerConv's attention; UniMP, Shi et al.
+        2021): per destination v and head k over v's in-edges u, s = scale * q[v]_k . k[u]_k, p = softmax_u(s) and
+        out[v]_k = sum_u p * v[u]_k (0 for a row with no in-edge).  q, k and v have H = heads * F columns (H <= 256,
+        heads <= 8), and any of them may be the same tensor, whose gradient then takes every part.  scale=None is
+        1 / sqrt(F), computed in double and rounded once to fp32.  No parameter.  A mode of attention_gather: op_info
+        reports it as one.  fp32 inputs only; one partition only.  heads outside [1, 8] and a scale that is 0 or not
+        finite in fp32 raise ValueError."""
+        if isinstance(heads, bool) or not isinstance(heads, (int, np.integer)) or not 1 <= heads <= 8:
+            raise ValueError("heads must be an integer in [1, 8]")
+        if scale is None:
+            scale = fp32(1.0 / math.sqrt(max(self.tensor_shape(q)[1] // int(heads), 1)))
+        if not math.isfinite(fp32(scale)) or fp32(scale) == 0.0:
+            raise ValueError("scale must be finite and not 0 in fp32")
+        return lib.roc_host_dot_attention_gather(self.h, q, k, v, int(heads), fp32(scale))
+
     def attention_scores(self, t, heads=1):
         """GAT's per-head scores of t (H = heads * F columns): [s_dst | s_src], 2 * heads columns, the scores attention_gather
         takes.  Head k's scores are the dot products of its own F columns with its a_dst and a_src.  Appends one parameter
@@ -735,6 +751,64 @@ def build_gatv2(model, layers, dropout_rate, heads=1, negative_slope=0.2, share_
         t = model.dynamic_attention_gather(xl, xr, hs[i - 1], negative_slope)
         attn_ins.append((xl, xr))
         attn.append(t)
+        if i != L - 1:
+            t = act(_hidden_norm(model, norm, t, bns))
+            relu_outs.append(t)
+    _loss(model, loss, t, label, mask)
+    model.adam(lr, weight_decay)
+    if exact_backward:
+        model.set_exact_backward(True)
+    model.init()
+    return {"input": x, "label": label, "mask": mask, "logits": t, "relu_outs": relu_outs, "attn": attn,
+            "attn_ins": attn_ins, "bns": bns}
+
+
+def build_graph_transformer(model, layers, dropout_rate, heads=1, root_weight=True, lr=0.01, weight_decay=0.05,
+                            exact_backward=False, features="float32", loss="softmax", norm=None, activation="relu"):
+    """The graph transformer (UniMP, Shi et al., "Masked Label Prediction", 2021; PyG TransformerConv without bias,
+    edge features, beta or attention dropout) built on dot_attention_gather and stacked as build_gat stacks GAT.
+    `heads` (an int, or one value per hidden layer) applies to the hidden layers; the last layer has one head.
+    layers[i] is the width of layer i's output, heads_i * F_i.  Per layer:
+
+        d       = dropout(t)
+        q, k, v = linear(d, layers[i]) x 3                  # PyG's lin_query, lin_key, lin_value
+        t       = dot_attention_gather(q, k, v, heads_i)    # scale 1 / sqrt(F_i)
+        t       = add(t, linear(d, layers[i]))              # root_weight: PyG's lin_skip
+        t       = act(norm(t))                              # all but the last layer
+
+    activation: "relu" or "elu".  norm="batch" / "layer_norm": batch_norm / layer_norm before each hidden activation
+    (see build_gcn).  exact_backward: the attention's source pass over the transposed graph
+    (Model.set_exact_backward), exact on directed graphs and multigraphs.  Single partition; the attention reads fp32
+    rows (features="bfloat16" stores only the input features in bf16).  Bad heads, widths, norm or activation raise
+    ValueError.  Returns the handles, with `attn` (the attention outputs), `attn_ins` (their (q, k, v) triples),
+    `relu_outs` (the hidden activations' outputs) and `bns`."""
+    _check_norm(norm)
+    if activation not in ("relu", "elu"):
+        raise ValueError("activation must be \"relu\" or \"elu\"")
+    L = len(layers)
+    hs = list(heads) if isinstance(heads, (list, tuple)) else [heads] * (L - 2)
+    if len(hs) != L - 2 or any(isinstance(h, bool) or not isinstance(h, (int, np.integer)) or not 1 <= h <= 8
+                               for h in hs):
+        raise ValueError("heads must be an integer in [1, 8], or one per hidden layer")
+    if any(layers[i] % hs[i - 1] for i in range(1, L - 1)):
+        raise ValueError("each hidden width must be a multiple of its heads")
+    if any(w > 256 for w in layers[1:]):
+        raise ValueError("the attention widths must be at most 256")
+    hs = [int(h) for h in hs] + [1]
+    x = _input_tensor(model, layers[0], features)
+    label = model.create_node_tensor(layers[-1])
+    mask = model.create_node_tensor(1, is_int=True)
+    act = model.elu if activation == "elu" else model.relu
+    t = x
+    relu_outs, attn, attn_ins, bns = [], [], [], []
+    for i in range(1, L):
+        d = model.dropout(t, dropout_rate)
+        q, k, v = (model.linear(d, layers[i], _lib.AC_MODE_NONE) for _ in range(3))
+        t = model.dot_attention_gather(q, k, v, hs[i - 1], fp32(1.0 / math.sqrt(layers[i] // hs[i - 1])))
+        attn_ins.append((q, k, v))
+        attn.append(t)
+        if root_weight:
+            t = model.add(t, model.linear(d, layers[i], _lib.AC_MODE_NONE))
         if i != L - 1:
             t = act(_hidden_norm(model, norm, t, bns))
             relu_outs.append(t)

@@ -1,6 +1,6 @@
 """Edge dropout of the sum ScatterGather (include/roc_b200.h, roc_sg_forward_dropout_planned) restated: the keep bit
-of every edge, a recorder of model scripts that take Model.scatter_gather(dropout=), and a torch fp64 autograd
-interpreter of the GCN and APPNP graphs such scripts build.  No code shared with the product.
+of every edge, and a torch fp64 autograd interpreter of the GCN and APPNP graphs that model scripts with
+Model.scatter_gather(dropout=) build, as opgraph.Recorder records them.  No code shared with the product.
 
 keep(i<-j) is bit 0 of attention dropout's keep byte of the pair (attn_dropout_oracle.keep_bytes); a kept edge's row
 is weighted by s = 1.0f / (1.0f - rate) (fp32), a dropped one's by 0, and the degrees are the full graph's."""
@@ -8,8 +8,8 @@ import numpy as np
 import torch
 
 import attn_dropout_oracle as ado
+import opgraph          # a module import: opgraph imports this module too
 from oracle import oracle
-from opgraph import Recorder, _relu_with_mask
 from roc_b200 import _lib
 from witness_gat import edge_lists, train_loss
 
@@ -28,22 +28,6 @@ def edge_keep(row_end, col, rate, key, step, col_left=0, self_base=0, row_is_sou
 def edge_weights(keep, rate):
     """fp32 [E]: keep ? s : 0, the weights under which the weighted sum is the dropped sum"""
     return np.where(keep, np.float32(drop_scale(rate)), np.float32(0.0)).astype(np.float32)
-
-
-class EdgeRecorder(Recorder):
-    """opgraph.Recorder plus the dropout= / seed= keywords of Model.scatter_gather: a dropped sum is recorded as a
-    scatter_gather node with attrs dropout, seed and key = (seed << 32) | its layer index."""
-
-    def scatter_gather(self, t, aggr=_lib.AGGR_SUM, weights=None, dropout=0.0, seed=0):
-        if not dropout:
-            return super().scatter_gather(t, aggr, weights)
-        key = self._key(seed)
-        if self.m is not None:
-            out = self.m.scatter_gather(t, aggr, weights, dropout, seed)
-        else:
-            self._next += 1
-            out = self._next - 1
-        return self._node("scatter_gather", [t], out, aggr=aggr, dropout=float(dropout), seed=seed, key=key)
 
 
 def witness(ir, graph, feats, labels, mask, weights, step=1, relu_masks=None, training=True):
@@ -67,7 +51,7 @@ def witness(ir, graph, feats, labels, mask, weights, step=1, relu_masks=None, tr
         if k == "linear":
             y = x @ ws[a["param"]].T
             if a["activation"] == _lib.AC_MODE_RELU:
-                y = _relu_with_mask(y, relu_masks.get(node["layer"]), what)
+                y = opgraph._relu_with_mask(y, relu_masks.get(node["layer"]), what)
         elif k == "indegree_norm":
             y = x * dinv
         elif k == "scatter_gather":
@@ -78,7 +62,7 @@ def witness(ir, graph, feats, labels, mask, weights, step=1, relu_masks=None, tr
                 rows = rows * torch.from_numpy(keep.astype(np.float64) * drop_scale(a["dropout"])).unsqueeze(1)
             y = torch.zeros((n, x.shape[1]), dtype=torch.float64).index_add(0, dst, rows)
         elif k == "relu":
-            y = _relu_with_mask(x, relu_masks.get(node["layer"]), what)
+            y = opgraph._relu_with_mask(x, relu_masks.get(node["layer"]), what)
         elif k == "add":
             y = x + val[ins[1]]
         elif k == "scaled_add":

@@ -6,25 +6,38 @@ and two norms), numbered by layer index as Model::layers is.  A node is a dict:
 
     kind    one of roc_b200._lib.HOST_OPS: "linear", "indegree_norm", "scatter_gather", "scatter_gather_max",
             "scatter_gather_min", "scatter_gather_weighted", "attention_gather", "attention_scores", "relu", "elu",
-            "sigmoid", "add", "scaled_add", "dropout", "batch_norm", "softmax_cross_entropy" or "sigmoid_cross_entropy"
+            "sigmoid", "add", "scaled_add", "dropout", "batch_norm", "softmax_cross_entropy" or "sigmoid_cross_entropy";
+            or "layer_norm", which op_info reports as "batch_norm" (the normalisation kind)
     ins     input tensor ids (tensor handles; the inner tensors of AGGR_AVG get ids of their own, from INNER on)
     out     output tensor id (None for a loss)
     layer   the layer index
-    attrs   out_dim, activation, param (linear); rate, seed, key (dropout); heads, slope, dropout, seed, key
-            (attention_gather); heads, param (attention_scores); edges (weighted); alpha, beta (scaled_add, the fp32
-            coefficients as doubles); gamma, beta (parameter indices), momentum, eps (batch_norm)
+    attrs   out_dim, activation, param (linear); rate, seed, key (dropout); aggr, and dropout, seed, key for a sum with
+            edge dropout (scatter_gather); mode (attention_gather: "gat", "dynamic", "softmax" or "dot"), then per mode
+            heads, slope, dropout, seed, key (gat: ins [t, scores]); heads, slope, param (dynamic: ins [xl, xr], the
+            parameter a); temperature, learn, param (softmax: ins [x], param the learned t or None); heads, scale
+            (dot: ins [q, k, v]); heads, param (attention_scores); edges (weighted); alpha, beta (scaled_add, the fp32
+            coefficients as doubles); gamma, beta (parameter indices), momentum, eps (batch_norm); gamma, beta, eps
+            (layer_norm).  Every fp32 attribute (slope, temperature, scale, eps) is held as the fp32 value, as a double.
 
-A dropout's and an attention_gather's Philox key is (seed << 32) | layer, as Model::dropout computes it.  The
-recorder also keeps the bf16 leaves (create_node_tensor(dtype="bfloat16")) and whether set_bf16_aggregation is on.
+A dropout's, an attention_gather's and a dropped sum's Philox key is (seed << 32) | layer, as Model::dropout computes
+it.  Parameters are numbered in the product's order: a Linear's W, attention_scores' A, a dynamic gather's a, a
+learned temperature, a norm's gamma then beta.  The recorder also keeps the bf16 leaves
+(create_node_tensor(dtype="bfloat16")) and whether set_bf16_aggregation is on.
 
 witness() runs the recorded graph in torch fp64 with autograd over edge lists (index_add): no code shared with the
-product.  The op semantics are the ones include/roc_b200.h and include/roc_gnn.h state."""
+product.  The op semantics are the ones include/roc_b200.h and include/roc_gnn.h state; the newer aggregations take
+their per-edge math from the feature witnesses (gatv2_witness, softmax_aggr_witness, transformer_witness and
+edge_dropout_witness's keep bits), which are test code too."""
 import numpy as np
 import torch
 
 import attn_dropout_oracle as ado
+import edge_dropout_witness as edw
+from gatv2_witness import dynamic_attend
 from oracle import oracle
 from roc_b200 import _lib
+from softmax_aggr_witness import softmax_aggr
+from transformer_witness import dot_attend
 from witness_gat import attend, edge_lists, train_loss
 
 INNER = 1 << 20      # ids of tensors the caller holds no handle for
@@ -107,7 +120,11 @@ class Recorder:
     def indegree_norm(self, t):
         return self._node("indegree_norm", [t], self._call("indegree_norm", t))
 
-    def scatter_gather(self, t, aggr=_lib.AGGR_SUM, weights=None):
+    def scatter_gather(self, t, aggr=_lib.AGGR_SUM, weights=None, dropout=0.0, seed=0):
+        if dropout:                        # Model::scatter_gather with edge dropout: one sum, keyed by its layer
+            key = self._key(seed)
+            return self._node("scatter_gather", [t], self._call("scatter_gather", t, aggr, weights, dropout, seed),
+                              aggr=aggr, dropout=float(dropout), seed=seed, key=key)
         out = self._call("scatter_gather", t, aggr, weights)
         if weights is not None:
             return self._node("scatter_gather_weighted", [t, weights], out, edges=weights)
@@ -126,8 +143,27 @@ class Recorder:
         # the rate-0 call takes the four arguments Model.attention_gather has always taken
         args = (t, scores, heads, negative_slope) + ((dropout, seed) if dropout or seed else ())
         return self._node("attention_gather", [t, scores], self._call("attention_gather", *args), width=self.width[t],
-                          heads=int(heads), slope=float(np.float32(negative_slope)), dropout=float(dropout),
-                          seed=seed, key=key)
+                          mode="gat", heads=int(heads), slope=float(np.float32(negative_slope)),
+                          dropout=float(dropout), seed=seed, key=key)
+
+    def dynamic_attention_gather(self, xl, xr, heads=1, negative_slope=0.2):
+        self.params += 1
+        return self._node("attention_gather", [xl, xr],
+                          self._call("dynamic_attention_gather", xl, xr, heads, negative_slope), mode="dynamic",
+                          heads=int(heads), slope=float(np.float32(negative_slope)), param=self.params - 1)
+
+    def softmax_gather(self, t, temperature=1.0, learn_temperature=False):
+        if learn_temperature:
+            self.params += 1
+        return self._node("attention_gather", [t], self._call("softmax_gather", t, temperature, learn_temperature),
+                          mode="softmax", temperature=float(np.float32(temperature)), learn=bool(learn_temperature),
+                          param=self.params - 1 if learn_temperature else None)
+
+    def dot_attention_gather(self, q, k, v, heads=1, scale=None):
+        if scale is None:                  # Model.dot_attention_gather's default, from this recorder's widths
+            scale = float(np.float32(1.0 / np.sqrt(max(self.width[q] // int(heads), 1))))
+        return self._node("attention_gather", [q, k, v], self._call("dot_attention_gather", q, k, v, heads, scale),
+                          mode="dot", heads=int(heads), scale=float(np.float32(scale)))
 
     def attention_scores(self, t, heads=1):
         self.params += 1
@@ -155,6 +191,11 @@ class Recorder:
         return self._node("batch_norm", [t], self._call("batch_norm", t, momentum, eps), gamma=self.params - 2,
                           beta=self.params - 1, momentum=float(momentum), eps=float(np.float32(eps)))
 
+    def layer_norm(self, t, eps=1e-5):
+        self.params += 2
+        return self._node("layer_norm", [t], self._call("layer_norm", t, eps), gamma=self.params - 2,
+                          beta=self.params - 1, eps=float(np.float32(eps)))
+
     def softmax_cross_entropy(self, logits, labels, mask):
         self._call("softmax_cross_entropy", logits, labels, mask)
         return self._node("softmax_cross_entropy", [logits, labels, mask], None)
@@ -168,15 +209,21 @@ class Recorder:
             self.m.init()
             self.check_against_product()
 
+    def num_parameters(self):
+        return self.params if self.m is None else self.m.num_parameters()
+
     def __getattr__(self, name):          # adam, set_fusion, set_tensor, forward, ...: straight to the product
         if self.m is None:                # a hand-written IR: nothing to run
             return lambda *args, **kw: None
         return getattr(self.m, name)
 
     def check_against_product(self):
-        """The product's layer list matches the recorded one, kind by kind."""
+        """The product's layer list matches the recorded one, kind by kind (a layer_norm reports as batch_norm, the
+        normalisation kind)."""
         got = [i["kind"] for i in self.m.op_info()]
-        assert got == [n["kind"] for n in self.nodes], (got, [n["kind"] for n in self.nodes])
+        want = ["batch_norm" if n["kind"] == "layer_norm" else n["kind"] for n in self.nodes]
+        assert got == want, (got, want)
+        assert self.m.num_parameters() == self.params, (self.m.num_parameters(), self.params)
 
     # ---- what the IR implies
     def loss_node(self):
@@ -243,7 +290,7 @@ def witness(ir, graph, feats, labels, mask, weights, edge_values=None, step=1, r
     bf16 (set_bf16_aggregation)}, each checked to be a rounding of the fp64 value and taken in the forward with the
     gradient passed straight through.
 
-    training=False is the infer-mode model: dropout and attention dropout are copies, batch_norm uses
+    training=False is the infer-mode model: dropout, attention dropout and edge dropout are copies, batch_norm uses
     run_stats {bn output: (running mean, running variance)}, and nothing is differentiated.
 
     Returns dict(logits, dW (zeros for a parameter off the loss's path), edge_grad {edge tensor: dL/dw}, pre {layer: the
@@ -274,13 +321,24 @@ def witness(ir, graph, feats, labels, mask, weights, edge_values=None, step=1, r
         elif k == "indegree_norm":
             y = x * dinv
         elif k == "scatter_gather":
-            y = torch.zeros((n, x.shape[1]), dtype=torch.float64).index_add(0, dst, x[src])
+            rows = x[src]
+            if training and a.get("dropout", 0.0) > 0:
+                keep = edw.edge_keep(row_end, col, a["dropout"], a["key"], step)
+                rows = rows * torch.from_numpy(keep.astype(np.float64) * edw.drop_scale(a["dropout"])).unsqueeze(1)
+            y = torch.zeros((n, x.shape[1]), dtype=torch.float64).index_add(0, dst, rows)
         elif k in ("scatter_gather_max", "scatter_gather_min"):
             s = _extreme_sources(row_end, col, x.detach().numpy(), k.endswith("max"), aggr_args.get(node["layer"]),
                                  what)
             y = x.gather(0, torch.from_numpy(s))
         elif k == "scatter_gather_weighted":
             y = torch.zeros((n, x.shape[1]), dtype=torch.float64).index_add(0, dst, ew[a["edges"]][:, None] * x[src])
+        elif k == "attention_gather" and a["mode"] == "dynamic":
+            y = dynamic_attend(x, val[ins[1]], ws[a["param"]].T, dst, src, n, a["heads"], a["slope"])[0]
+        elif k == "attention_gather" and a["mode"] == "softmax":
+            t = ws[a["param"]][0, 0] if a["learn"] else torch.tensor(a["temperature"], dtype=torch.float64)
+            y = softmax_aggr(x, t, dst, src, n)[0]
+        elif k == "attention_gather" and a["mode"] == "dot":
+            y = dot_attend(x, val[ins[1]], val[ins[2]], dst, src, n, a["heads"], a["scale"])[0]
         elif k == "attention_gather":
             drop = None
             if training and a.get("dropout", 0.0) > 0:
@@ -311,6 +369,8 @@ def witness(ir, graph, feats, labels, mask, weights, edge_values=None, step=1, r
             else:
                 rm, rv = (torch.from_numpy(np.asarray(v, dtype=np.float64)) for v in run_stats[node["out"]])
                 y = torch.nn.functional.batch_norm(x, rm, rv, gam, bet, training=False, eps=a["eps"])
+        elif k == "layer_norm":
+            y = torch.nn.functional.layer_norm(x, (x.shape[1],), ws[a["gamma"]][0], ws[a["beta"]][0], a["eps"])
         elif k == "dropout":
             if a["rate"] > 0 and training:
                 keep = oracle.dropout_mask(0, n, x.shape[1], a["rate"], a["key"], step)

@@ -11,7 +11,7 @@ import numpy as np
 import pytest
 import torch
 
-from edge_dropout_witness import EdgeRecorder, drop_scale, edge_keep, witness
+from edge_dropout_witness import drop_scale, edge_keep, witness
 from opgraph import Recorder
 from roc_b200 import _lib
 from roc_b200.model import Model, build_appnp, build_gcn, fp32
@@ -38,9 +38,9 @@ def test_scatter_gather_refuses_before_the_product(kw):
 @pytest.mark.parametrize("rate", [1.0, -0.5, float("nan"), 2.0])
 def test_builders_refuse_bad_edge_dropout(rate):
     with pytest.raises(ValueError):
-        build_appnp(EdgeRecorder(None), [8, 4], 0.0, K=2, edge_dropout=rate)
+        build_appnp(Recorder(None), [8, 4], 0.0, K=2, edge_dropout=rate)
     with pytest.raises(ValueError):
-        build_gcn(EdgeRecorder(None), [8, 6, 4], 0.0, edge_dropout=rate)
+        build_gcn(Recorder(None), [8, 6, 4], 0.0, edge_dropout=rate)
 
 
 def test_host_entry_points_are_declared():
@@ -57,7 +57,7 @@ def _graph(ir):
 
 def test_default_builders_are_unchanged():
     for build, args, kw in ((build_appnp, ([12, 8, 4], 0.5), dict(K=3)), (build_gcn, ([12, 8, 4], 0.5), {})):
-        a, b = Recorder(None), EdgeRecorder(None)
+        a, b = Recorder(None), Recorder(None)
         build(a, *args, **kw)
         build(b, *args, edge_dropout=0.0, **kw)
         assert _graph(a) == _graph(b)
@@ -65,7 +65,7 @@ def test_default_builders_are_unchanged():
 
 
 def test_every_hop_and_layer_draws_its_own_mask():
-    ir = EdgeRecorder(None)
+    ir = Recorder(None)
     h = build_appnp(ir, [12, 8, 4], 0.5, K=4, edge_dropout=0.3)
     sgs = [n for n in ir.nodes if n["kind"] == "scatter_gather"]
     assert len(sgs) == 4 and all(n["attrs"]["dropout"] == 0.3 for n in sgs)
@@ -75,7 +75,7 @@ def test_every_hop_and_layer_draws_its_own_mask():
     build_appnp(plain, [12, 8, 4], 0.5, K=4)
     assert [n["kind"] for n in ir.nodes] == [n["kind"] for n in plain.nodes]
     assert h["coefficients"] == (fp32(0.9), fp32(0.1))
-    ir = EdgeRecorder(None)
+    ir = Recorder(None)
     build_gcn(ir, [12, 8, 6, 4], 0.5, edge_dropout=0.5)
     sgs = [n for n in ir.nodes if n["kind"] == "scatter_gather"]
     assert len(sgs) == 3 and len({n["attrs"]["key"] for n in sgs}) == 3
@@ -129,7 +129,7 @@ def _pyg_propagate(row_end, col, z, edge_mask, rate):
 def test_witness_is_pyg_appnp(rate):
     row_end, col = small_graph()
     n, K, step = row_end.shape[0], 10, 2
-    ir = EdgeRecorder(None)
+    ir = Recorder(None)
     build_appnp(ir, [12, 9, 5], 0.0, K=K, alpha=0.1, edge_dropout=rate)
     rng = np.random.RandomState(1)
     x = rng.standard_normal((n, 12))
@@ -157,7 +157,7 @@ def test_witness_is_pyg_appnp(rate):
 def test_witness_is_pyg_gcn():
     row_end, col = small_graph(seed=5)
     n, rate, step = row_end.shape[0], 0.5, 3
-    ir = EdgeRecorder(None)
+    ir = Recorder(None)
     build_gcn(ir, [12, 10, 4], 0.0, edge_dropout=rate)
     rng = np.random.RandomState(2)
     x = rng.standard_normal((n, 12))

@@ -13,7 +13,8 @@ import pytest
 import torch
 
 import sg_matrix as M
-from edge_dropout_witness import EdgeRecorder, drop_scale, edge_keep, witness
+from edge_dropout_witness import drop_scale, edge_keep, witness
+from opgraph import Recorder
 from roc_b200 import _lib, datasets
 from roc_b200 import kernels as K
 from roc_b200.model import Host, Model, build_appnp, build_gcn
@@ -273,7 +274,7 @@ def train(name, graph, fuse, steps=3, edge_dropout=0.5, infer=False, **kw):
     host.graph_from_arrays(row_end, col)
     m = Model(host, seed=1)
     m.set_fusion(fuse)
-    ir = EdgeRecorder(m)
+    ir = Recorder(m)
     h = BUILDERS[name](ir, edge_dropout=edge_dropout, **kw)
     feats, labels, mask = (t.numpy() for t in datasets.node_data(n, 24, 12, seed=5))
     m.set_labels(h["label"], labels)
@@ -391,7 +392,7 @@ def test_masks_differ_between_hops_and_steps():
     """each hop draws its own mask every step: the witness's masks of the recorded APPNP are all distinct, and they
     are what the product used (the model matches the witness above)"""
     re_, col = sym_graph()
-    ir = EdgeRecorder(None)
+    ir = Recorder(None)
     build_appnp(ir, [24, 16, 12], 0.5, K=10, edge_dropout=0.5)
     keys = [nd["attrs"]["key"] for nd in ir.nodes if nd["kind"] == "scatter_gather"]
     masks = {(k, s): edge_keep(re_, col, 0.5, k, s).tobytes() for k in keys for s in (1, 2, 3)}

@@ -62,35 +62,6 @@ def test_witness_matches_the_row_formulas(h, relu, shift):
 
 
 # ------------------------------------------------------------------------------------------ builders' wiring ---
-class LnRecorder(Recorder):
-    """Recorder with Model.layer_norm (node kind "layer_norm": gamma, beta parameter indices and eps) and the builders'
-    other extensions (softmax_gather as the attention_gather it reports as, dynamic_attention_gather)."""
-
-    def layer_norm(self, t, eps=1e-5):
-        self.params += 2
-        return self._node("layer_norm", [t], self._call("layer_norm", t, eps), gamma=self.params - 2,
-                          beta=self.params - 1, eps=float(np.float32(eps)))
-
-    def softmax_gather(self, t, temperature=1.0, learn_temperature=False):
-        if learn_temperature:
-            self.params += 1
-        return self._node("attention_gather", [t], self._call("softmax_gather", t, temperature, learn_temperature),
-                          softmax=True)
-
-    def dynamic_attention_gather(self, xl, xr, heads=1, negative_slope=0.2):
-        self.params += 1
-        return self._node("attention_gather", [xl, xr], self._call("dynamic_attention_gather", xl, xr, heads,
-                                                                   negative_slope), dynamic=True)
-
-    def num_parameters(self):
-        return self.params
-
-    def check_against_product(self):
-        """the product reports a layer_norm as the normalisation kind, batch_norm"""
-        got = [i["kind"] for i in self.m.op_info()]
-        assert got == [("batch_norm" if n["kind"] == "layer_norm" else n["kind"]) for n in self.nodes], got
-
-
 BUILDERS = {
     "gcn": lambda ir, **kw: build_gcn(ir, [24, 16, 12], 0.5, **kw),
     "gcn4": lambda ir, **kw: build_gcn(ir, [24, 16, 16, 12], 0.5, **kw),
@@ -107,7 +78,7 @@ BUILDERS = {
 
 @pytest.mark.parametrize("name", list(BUILDERS))
 def test_layer_norm_sits_where_batch_norm_does(name):
-    bn, ln = LnRecorder(None), LnRecorder(None)
+    bn, ln = Recorder(None), Recorder(None)
     hb = BUILDERS[name](bn, norm="batch")
     hl = BUILDERS[name](ln, norm="layer_norm")
     assert [n["kind"] for n in ln.nodes] == [("layer_norm" if n["kind"] == "batch_norm" else n["kind"])
@@ -124,7 +95,7 @@ def test_layer_norm_sits_where_batch_norm_does(name):
 @pytest.mark.parametrize("name", list(BUILDERS))
 def test_defaults_are_unchanged(name):
     """no builder puts a layer_norm in unless asked"""
-    ir = LnRecorder(None)
+    ir = Recorder(None)
     BUILDERS[name](ir)
     assert all(n["kind"] != "layer_norm" for n in ir.nodes)
 
@@ -133,7 +104,7 @@ def test_defaults_are_unchanged(name):
 @pytest.mark.parametrize("bad", ["layer", "LayerNorm", "layernorm", "Layer_norm"])
 def test_other_spellings_are_refused(name, bad):
     with pytest.raises(ValueError):
-        BUILDERS[name](LnRecorder(None), norm=bad)
+        BUILDERS[name](Recorder(None), norm=bad)
 
 
 @pytest.mark.parametrize("eps", [-1e-5, float("nan"), float("inf"), -float("inf"), 1e39])

@@ -13,10 +13,10 @@ import pytest
 import torch
 
 from layernorm_witness import LN_EPS, deepergcn_witness, graph_witness, kernel_witness
+from opgraph import Recorder
 from roc_b200 import _lib, datasets
 from roc_b200 import kernels as K
 from roc_b200.model import Host, Model, build_deepergcn, build_gat, build_gcn, build_sage_mean
-from test_layernorm_cpu import LnRecorder
 from witness_gat import train_loss
 
 pytestmark = pytest.mark.gpu
@@ -343,7 +343,7 @@ def train(build, graph, fuse=True, steps=3, loss="softmax", **kw):
     host.graph_from_arrays(row_end, col)
     m = Model(host, seed=1)
     m.set_fusion(fuse)
-    ir = LnRecorder(m)
+    ir = Recorder(m)
     h = build(ir, norm="layer_norm", dropout_rate=0.0, loss=loss, **kw) if build is build_dgcn else \
         build(ir, norm="layer_norm", **kw)
     gen = datasets.multilabel_node_data if loss == "sigmoid" else datasets.node_data
@@ -459,7 +459,7 @@ def test_infer_logits_are_the_train_forward_bits():
     host = Host(0, 0, 1)
     host.graph_from_arrays(*g)
     m = Model(host, seed=1)
-    h = MODELS["gcn"](LnRecorder(m), norm="layer_norm")
+    h = MODELS["gcn"](Recorder(m), norm="layer_norm")
     m.set_labels(h["label"], run["labels"])
     m.set_tensor(h["input"], run["feats"])
     m.set_tensor(h["mask"], run["mask"].astype(np.int32))

@@ -7,12 +7,17 @@ import torch
 
 import appnp_witness
 import attn_dropout_oracle as ado
+import edge_dropout_witness
+import gatv2_witness
+import layernorm_witness
+import softmax_aggr_witness
+import transformer_witness
 from conftest import rel_close
 from oracle import oracle
 from opgraph import Recorder, witness
 from roc_b200 import _lib, datasets
-from roc_b200.model import (build_appnp, build_gat, build_gcn, build_gcn_weighted, build_gcnii, build_sage_mean,
-                            build_sage_pool)
+from roc_b200.model import (build_appnp, build_deepergcn, build_gat, build_gatv2, build_gcn, build_gcn_weighted,
+                            build_gcnii, build_graph_transformer, build_sage_mean, build_sage_pool)
 from test_attn_dropout_cpu import _sym_graph
 from test_attn_dropout_gpu import witness as attn_dropout_witness
 from test_batchnorm_cpu import BUILDERS as BN_BUILDERS
@@ -187,8 +192,9 @@ def test_gcn_with_dropout_matches_the_oracle(layers):
 
 # --------------------------------------------- the ops added since: each feature's own reference, on its builders ---
 def draw(ir, seed=4):
-    """A value for every parameter, in the shapes the product gives them: a Linear's W (out, in), an
-    attention_scores' A (2 * heads, F), a batch_norm's gamma and beta (1, H) (gamma near 1)."""
+    """A value for every parameter, in the shapes get_parameter gives them: a Linear's W (out, in), an
+    attention_scores' A (2 * heads, F), a dynamic gather's a (F, heads), a learned temperature (1, 1), a batch_norm's
+    or layer_norm's gamma and beta (1, H) (gamma near 1)."""
     rng = np.random.RandomState(seed)
     ws = [None] * ir.params
     for nd in ir.nodes:
@@ -200,7 +206,12 @@ def draw(ir, seed=4):
         elif nd["kind"] == "attention_scores":
             hd = a["heads"]
             ws[a["param"]] = rng.uniform(-0.5, 0.5, size=(2 * hd, ir.width[nd["ins"][0]] // hd))
-        elif nd["kind"] == "batch_norm":
+        elif nd["kind"] == "attention_gather" and a["mode"] == "dynamic":
+            hd = a["heads"]
+            ws[a["param"]] = rng.uniform(-0.5, 0.5, size=(ir.width[nd["ins"][0]] // hd, hd))
+        elif nd["kind"] == "attention_gather" and a["mode"] == "softmax" and a["learn"]:
+            ws[a["param"]] = rng.uniform(0.5, 2.0, size=(1, 1))
+        elif nd["kind"] in ("batch_norm", "layer_norm"):
             h = ir.width[nd["out"]]
             ws[a["gamma"]] = rng.uniform(0.5, 1.5, size=(1, h))
             ws[a["beta"]] = rng.uniform(-0.3, 0.3, size=(1, h))
@@ -330,3 +341,105 @@ def test_attention_dropout_matches_attn_dropout_oracle(heads, f):
     ig, sg = ado.backward(row_end, col, xw, s, o, stats, gy, heads, slope, m1, m2)
     np.testing.assert_allclose(got["dW"][0], ig.T @ x, rtol=1e-10, atol=1e-12)
     np.testing.assert_allclose(got["dW"][1], sg.T @ x, rtol=1e-10, atol=1e-12)
+
+
+# ------------------------- edge dropout, GATv2, softmax aggregation, layer norm, dot attention: their own witnesses ---
+@pytest.mark.parametrize("share_weights", [False, True])
+def test_gatv2_matches_gatv2_witness(share_weights):
+    row_end, col, feats, labels, mask = case((24, 16, 12))
+    ir = Recorder()
+    h = build_gatv2(ir, [24, 16, 12], 0.0, heads=2, share_weights=share_weights)
+    assert [n["attrs"]["mode"] for n in ir.nodes if n["kind"] == "attention_gather"] == ["dynamic", "dynamic"]
+    assert all(xl == xr for xl, xr in h["attn_ins"]) == share_weights
+    ws = draw(ir)
+    got = witness(ir, (row_end, col), feats, labels, mask, ws)
+    # the interpreter takes the product's fp32 slope; a is (F, heads) as get_parameter returns it
+    logits, dw = gatv2_witness.model_witness(row_end, col, feats, labels, mask, (24, 16, 12), ws, [2],
+                                             share_weights=share_weights, slope=float(np.float32(0.2)))
+    check(ir, got, logits, dw, what="gatv2_witness")
+
+
+@pytest.mark.parametrize("norm", ["batch", "layer_norm"])
+@pytest.mark.parametrize("learn", [True, False])
+def test_deepergcn_matches_its_witnesses(learn, norm):
+    """softmax_aggr_witness.model_witness for batch norm, layernorm_witness.deepergcn_witness for layer norm; a
+    constant temperature of -0.5 leans towards the min."""
+    row_end, col, feats, labels, mask = case((24, 16, 12))
+    ir = Recorder()
+    temperature = 1.0 if learn else -0.5
+    h = build_deepergcn(ir, [24, 16, 12], 0.0, 3, temperature=temperature, learn_temperature=learn, norm=norm)
+    modes = [n["attrs"] for n in ir.nodes if n["kind"] == "attention_gather"]
+    assert [a["mode"] for a in modes] == ["softmax"] * 3 and [a["param"] for a in modes] == h["temperatures"]
+    ws = draw(ir)
+    got = witness(ir, (row_end, col), feats, labels, mask, ws)
+    if norm == "batch":
+        logits, dw = softmax_aggr_witness.model_witness(row_end, col, feats, labels, mask, (24, 16, 12), ws, 3,
+                                                        learn_temperature=learn, temperature=temperature)
+    else:
+        logits, dw = layernorm_witness.deepergcn_witness(row_end, col, feats, labels, mask, (24, 16, 12), ws, 3,
+                                                         learn_temperature=learn, temperature=temperature)
+    check(ir, got, logits, dw, what="deepergcn witness")
+
+
+@pytest.mark.parametrize("root_weight", [True, False])
+def test_graph_transformer_matches_transformer_witness(root_weight):
+    row_end, col, feats, labels, mask = case((24, 16, 12))
+    ir = Recorder()
+    build_graph_transformer(ir, [24, 16, 12], 0.0, heads=2, root_weight=root_weight, norm="layer_norm")
+    ws = draw(ir)
+    got = witness(ir, (row_end, col), feats, labels, mask, ws)
+    logits, dw = transformer_witness.model_witness(row_end, col, feats, labels, mask, (24, 16, 12), ws, [2],
+                                                   root_weight=root_weight, norm="layer_norm")
+    check(ir, got, logits, dw, what="transformer_witness")
+
+
+def test_dot_attention_default_scale_comes_from_the_widths():
+    """No product behind the recorder: the default scale is fp32(1 / sqrt(F)) from the recorder's own widths."""
+    ir = Recorder()
+    q = ir.create_node_tensor(24)
+    ir.dot_attention_gather(q, q, q, heads=8)
+    ir.dot_attention_gather(q, q, q, heads=2, scale=0.3)
+    assert [n["attrs"]["scale"] for n in ir.nodes] == [transformer_witness.dot_scale(3), float(np.float32(0.3))]
+
+
+@pytest.mark.parametrize("name", ["gcn", "gcn_residual", "appnp"])
+def test_edge_dropout_matches_edge_dropout_witness(name):
+    """Three steps of keep masks: the keys (seed << 32) | layer and the step counter pin the recorder's layer
+    numbering; infer mode drops nothing."""
+    layers = (24, 16, 16, 12) if name == "gcn_residual" else (24, 16, 12)
+    row_end, col, feats, labels, mask = case(layers)
+    ir = Recorder()
+    if name == "appnp":
+        build_appnp(ir, list(layers), 0.0, K=3, edge_dropout=0.5)
+    else:
+        build_gcn(ir, list(layers), 0.0, edge_dropout=0.5)
+    sgs = [n for n in ir.nodes if n["kind"] == "scatter_gather"]
+    assert sgs and all(n["attrs"]["key"] == n["layer"] and n["attrs"]["dropout"] == 0.5 for n in sgs)
+    ws = draw(ir)
+    for step in (1, 2, 3):
+        got = witness(ir, (row_end, col), feats, labels, mask, ws, step=step)
+        want = edge_dropout_witness.witness(ir, (row_end, col), feats, labels, mask, ws, step=step)
+        check(ir, got, want["logits"], want["dW"], what="edge_dropout_witness step %d" % step)
+    got = witness(ir, (row_end, col), feats, labels, mask, ws, training=False)
+    want = edge_dropout_witness.witness(ir, (row_end, col), feats, labels, mask, ws, training=False)
+    close12(got["logits"], want["logits"], "infer logits")
+    a = witness(ir, (row_end, col), feats, labels, mask, ws, step=1)["logits"]
+    assert np.abs(a - got["logits"]).max() > 1e-3, "edge dropout changed nothing"
+
+
+LN_BUILDERS = {"gcn4": lambda ir: build_gcn(ir, [24, 16, 16, 12], 0.0, norm="layer_norm"),
+               "sage_mean": lambda ir: build_sage_mean(ir, [24, 16, 16, 12], 0.0, norm="layer_norm"),
+               "gat": lambda ir: build_gat(ir, [24, 16, 12], 0.0, heads=2, norm="layer_norm")}
+
+
+@pytest.mark.parametrize("name", list(LN_BUILDERS))
+def test_layer_norm_matches_layernorm_witness(name):
+    row_end, col, feats, labels, mask = case((24, 16, 12))
+    ir = Recorder()
+    h = LN_BUILDERS[name](ir)
+    assert h["bns"] and [n["out"] for n in ir.nodes if n["kind"] == "layer_norm"] == h["bns"]
+    ws = draw(ir)
+    got = witness(ir, (row_end, col), feats, labels, mask, ws)
+    want = layernorm_witness.graph_witness(ir, (row_end, col), feats, labels, mask, ws)
+    check(ir, got, want["logits"], want["dW"], what="layernorm_witness")
+    assert not got["stats"], "a layer norm keeps no batch statistics"

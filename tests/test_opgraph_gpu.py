@@ -2,14 +2,17 @@
 
 Model::init decides which tensors need a gradient, who overwrites a gradient and who adds to it (resetInputGrads,
 set in reverse layer order by Model::backward), and the peephole fusions that reroute where a gradient is written
-and switch other ops' forward or backward off (the GCN block, batch_norm -> relu, dropout -> linear, the backward
-epilogues, the teleport of a scaled_add into a sum scatter_gather).  This file builds op graphs over every op kind
-through a Recorder and checks, per case:
+and switch other ops' forward or backward off (the GCN block, batch_norm or layer_norm -> relu, dropout -> linear,
+the backward epilogues, the teleport of a scaled_add into a sum scatter_gather, with or without edge dropout).  This
+file builds op graphs over every op kind and every attention_gather mode (GAT, GATv2's dynamic attention, the softmax
+aggregation, dot-product attention) through a Recorder and checks, per case:
 
 - the fusion report (Model.op_info) of both schedules: the hand-listed cases state it exactly, the unfused schedule
   has none;
 - against the witness at each step's weights: the logits at the parity bar, every dW and every edge gradient at
-  rtol 2e-4 with atol_scale 2e-5 (the bars of test_exact_model_gpu.py);
+  rtol 2e-4 with atol_scale 2e-5 (the bars of test_exact_model_gpu.py); a learned temperature's gradient (family dt)
+  and a GATv2 a's (family da), sums over every edge and column that cancel, at rtol 1e-3 with atol_scale 1e-4 (the
+  bars of test_softmax_aggr_gpu.py and test_gatv2_gpu.py);
 - the batch_norm running statistics after training against the fp64 recurrence over the witness's batch statistics
   (from 0 / 1, var scaled by N / (N - 1)), at the dW bars;
 - after training, an infer-mode forward: its logits against witness(training=False) at the final weights and running
@@ -43,6 +46,17 @@ The rules every generated graph obeys, derived from model.cc:
 - Max / min without the exact mode need strictly increasing sources per row (the symmetric graphs have them).
 - attention_gather: scores of 2 * heads columns; heads 1, 2, 4 or 8; with heads > 1 the width is heads * F with F a
   power of two >= 4; width <= 512.
+- dynamic_attention_gather and dot_attention_gather: width <= 256, heads <= 8 and heads divides the width; xr (of q,
+  k and v, any) another open tensor of the same width or the first input itself.  Their backward, and
+  softmax_gather's, writes an input gradient another op already wrote (or a repeated input's) through scratch and adds
+  it, so they close nothing.  A dynamic gather's output and a learned temperature's gather's need a gradient even over
+  leaves (their own parameter); a dot gather's only when an input does.
+- softmax_gather: temperature 0, 1, -0.5 or 3, learned or constant.
+- layer_norm on any fp32 tensor, sometimes read by a relu alone (the norm-relu fusion).
+- Edge dropout at rate 0.1 or 0.5 on a sum scatter_gather (plain or a teleport hop's), which closes its input as
+  every ScatterGather does (Q7).
+- None of the five reads a bf16 tensor: only linear and dropout read a bf16 leaf, and set_bf16_aggregation keeps the
+  inputs of a dropped sum and of the dynamic, softmax and dot gathers in fp32.
 - One loss, softmax or sigmoid (labels from datasets.node_data / datasets.multilabel_node_data)."""
 import atexit
 import itertools
@@ -130,10 +144,15 @@ def note_fusions(fz, ir):
             SEEN.add("fusion:sg_norm_relu" if epi & _lib.SG_EPI_RELU else "fusion:sg_norm")
             if epi & _lib.SG_EPI_NORM_OUT:
                 SEEN.add("fusion:teleport_norm_out")
+        if kind == "scatter_gather" and ir.nodes[layer]["attrs"].get("dropout", 0.0) > 0 and \
+                ("epilogue" in d or "bwdEpilogue" in d):
+            SEEN.add("fusion:gcn_block_edge_dropout")
         if kind == "scaled_add" and d.get("fusedInto", -1) >= 0:
             SEEN.add("fusion:teleport")
-        if kind == "batch_norm" and d.get("fwdOut", -1) >= 0:
-            SEEN.add("fusion:batch_norm_relu")
+            if ir.nodes[d["fusedInto"]]["attrs"].get("dropout", 0.0) > 0:
+                SEEN.add("fusion:teleport_edge_dropout")
+        if kind in ("batch_norm", "layer_norm") and d.get("fwdOut", -1) >= 0:
+            SEEN.add("fusion:%s_relu" % kind)
         if kind == "linear" and d.get("dropOp", -1) >= 0:
             SEEN.add("fusion:dropout_linear")
         if kind in ("softmax_cross_entropy", "sigmoid_cross_entropy"):
@@ -143,11 +162,33 @@ def note_fusions(fz, ir):
                      "fusion:norm_relu_dropout_linear")
 
 
-def note_features(ir, dtypes):
-    """What a case exercised beyond op kinds: attention dropout, the sigmoid loss, bf16 tensors, and a norm or dropout
-    that a later scaled_add shares its input with (the amended Q7)."""
-    if any(nd["kind"] == "attention_gather" and nd["attrs"]["dropout"] > 0 for nd in ir.nodes):
+def note_features(ir, dtypes, gkind):
+    """What a case exercised beyond op kinds: attention dropout, edge dropout, each attention_gather mode, learned and
+    constant temperatures, inputs of a gather that are one tensor, a new gather's input another op also reads (before
+    or after it), the infer-mode softmax and dot forwards on the hub graph's cut rows, the sigmoid loss, bf16 tensors,
+    and a norm or dropout that a later scaled_add shares its input with (the amended Q7)."""
+    if any(nd["kind"] == "attention_gather" and nd["attrs"].get("dropout", 0.0) > 0 for nd in ir.nodes):
         SEEN.add("attn_dropout")
+    if any(nd["kind"] == "scatter_gather" and nd["attrs"].get("dropout", 0.0) > 0 for nd in ir.nodes):
+        SEEN.add("edge_dropout")
+    for nd in ir.nodes:
+        if nd["kind"] != "attention_gather":
+            continue
+        a, ins = nd["attrs"], nd["ins"]
+        SEEN.add("mode:" + a["mode"])
+        if a["mode"] == "softmax":
+            SEEN.add("temperature:learned" if a["learn"] else "temperature:constant")
+        if a["mode"] in ("softmax", "dot") and gkind == "hub":
+            SEEN.add("cut_rows_infer:" + a["mode"])
+        if a["mode"] == "dynamic" and ins[0] == ins[1]:
+            SEEN.add("alias:xl_is_xr")
+        if a["mode"] == "dot" and len(set(ins)) < 3:
+            SEEN.add("alias:" + {(True, True): "q_is_k_is_v", (True, False): "q_is_k", (False, True): "k_is_v",
+                                 (False, False): "q_is_v"}[(ins[0] == ins[1], ins[1] == ins[2])])
+        if a["mode"] != "gat":
+            for r in ir.nodes:
+                if r is not nd and set(r["ins"]) & set(ins):
+                    SEEN.add("gather_input_also_read_" + ("before" if r["layer"] < nd["layer"] else "after"))
     if ir.loss_node()["kind"] == "sigmoid_cross_entropy":
         SEEN.add("loss:sigmoid")
     if ir.bf16:
@@ -265,7 +306,8 @@ def run(build, gkind, fuse, steps=3, feats_seed=5):
 
 
 def check_case(build, gkind="sym", expect=None):
-    """Both schedules against the witness and each other; `expect(h)`: the fused schedule's fusion report."""
+    """Both schedules against the witness and each other; `expect(h)`: the fused schedule's fusion report.  Returns
+    the fused schedule's run."""
     fused, unfused = run(build, gkind, True), run(build, gkind, False)
     ir = fused["ir"]
     row_end, col = graph(gkind)
@@ -276,8 +318,12 @@ def check_case(build, gkind="sym", expect=None):
         assert fz == expect(fused["h"]), fz
     note_fusions(fz, ir)
     note_widths(ir)
-    note_features(ir, fused["dtypes"])
+    note_features(ir, fused["dtypes"], gkind)
     bn_momentum = {nd["out"]: nd["attrs"]["momentum"] for nd in ir.nodes if nd["kind"] == "batch_norm"}
+    # a learned temperature's and a GATv2 a's gradient sum over every edge and column, sums that cancel: the bars of
+    # test_softmax_aggr_gpu.py and test_gatv2_gpu.py, as families of their own
+    sums = {nd["attrs"]["param"]: "dt" if nd["attrs"]["mode"] == "softmax" else "da" for nd in ir.nodes
+            if nd["kind"] == "attention_gather" and nd["attrs"].get("param") is not None}
     for r in (fused, unfused):
         name = "fused" if r is fused else "unfused"
         rec = {t: (np.zeros(ir.width[t]), np.ones(ir.width[t])) for t in bn_momentum}
@@ -287,7 +333,9 @@ def check_case(build, gkind="sym", expect=None):
                           relu_masks=st["relu"], aggr_args=st["args"], rounded=st["rounded"])
             assert family("logits", st["logits"], wit["logits"], 1e-4, 1e-5) <= 1, what + " logits vs fp64"
             for p, (a, b) in enumerate(zip(st["dw"], wit["dW"])):
-                assert family("dW", a, b, 2e-4, 2e-5) <= 1, what + " dW[%d] vs fp64" % p
+                fam = sums.get(p, "dW")
+                bar = (1e-3, 1e-4) if p in sums else (2e-4, 2e-5)
+                assert family(fam, a, b, *bar) <= 1, what + " %s[%d] vs fp64" % (fam, p)
             for e, g in st["de"].items():
                 assert family("edge gradient", g, wit["edge_grad"][e], 2e-4, 2e-5) <= 1, what + " edge gradient"
             for t, (mean, var) in wit["stats"].items():
@@ -322,7 +370,7 @@ def check_case(build, gkind="sym", expect=None):
     fm = fused["metrics"]
     mask = fused["mask"]
     assert (fm["trainAll"], fm["valAll"], fm["testAll"]) == tuple(int((mask == k).sum()) for k in (0, 1, 2)), fm
-    return fz
+    return fused
 
 
 def loss(ir, t, sigmoid=False):
@@ -391,14 +439,14 @@ def batch_norm_relu(ir):
     return dict(b=b, r=r)
 
 
-def teleport(ir, norm_out=False, t0="before", second=False, sa_twice=False):
+def teleport(ir, norm_out=False, t0="before", second=False, sa_twice=False, drop=0.0):
     """linear -> norm -> sg -> norm -> scaled_add(., t0, 0.9, 0.1) [-> norm] -> linear: t0 a Linear made before the
     scatter_gather (or after it); second: the norm output is the scaled_add's second input; sa_twice: a relu also
-    reads the scaled_add's output."""
+    reads the scaled_add's output; drop: the sum's edge dropout rate."""
     x = ir.create_node_tensor(12)
     t = ir.linear(x, 16)
     u = ir.linear(x, 16) if t0 == "before" else None
-    n1 = ir.indegree_norm(t); s = ir.scatter_gather(n1); n2 = ir.indegree_norm(s)
+    n1 = ir.indegree_norm(t); s = ir.scatter_gather(n1, dropout=drop, seed=2); n2 = ir.indegree_norm(s)
     if u is None:
         u = ir.linear(x, 16)
     y = ir.scaled_add(u, n2, 0.9, 0.1) if second else ir.scaled_add(n2, u, 0.9, 0.1)
@@ -426,8 +474,34 @@ def expect_teleport(h, fused=True, norm_out=False, sg=3):
     return e
 
 
+def layer_norm_relu(ir):
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 16); b = ir.layer_norm(t); r = ir.relu(b)
+    loss(ir, ir.linear(r, 5))
+    return dict(b=b, r=r)
+
+
+def gcn_block_edge_dropout(ir):
+    """linear -> norm -> sg(dropout) -> norm -> relu -> linear: every GCN-block fusion around a dropped sum"""
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 16); n1 = ir.indegree_norm(t); s = ir.scatter_gather(n1, dropout=0.5, seed=3)
+    n2 = ir.indegree_norm(s); r = ir.relu(n2)
+    loss(ir, ir.linear(r, 5))
+    return dict(t=t, n1=n1, s=s, r=r)
+
+
 HAND = {
     "batch_norm_relu": (batch_norm_relu, lambda h: {1: dict(fwdOut=h["r"]), 2: dict(fusedInto=1)}),
+    "layer_norm_relu": (layer_norm_relu, lambda h: {1: dict(fwdOut=h["r"]), 2: dict(fusedInto=1)}),
+    # the dropped sum's forward takes the norm (and relu) epilogue, its backward the norm epilogue into d(linear out)
+    "gcn_block_edge_dropout": (gcn_block_edge_dropout, lambda h: {
+        0: dict(flags=_lib.LINEAR_NORM_EPILOGUE, fwdOut=h["n1"]), 1: dict(fusedInto=0),
+        2: dict(bwdEpilogue=_lib.SG_EPI_NORM, bwdOut=h["t"], epilogue=_lib.SG_EPI_NORM | _lib.SG_EPI_RELU,
+                fwdOut=h["r"]),
+        3: dict(fusedInto=2, bwdFused=1), 4: dict(fusedInto=2), 5: dict(dxReluOf=h["r"], dxNorm=1, dxOut=h["s"])}),
+    "teleport_edge_dropout": (lambda ir: teleport(ir, drop=0.5), expect_teleport),
+    "teleport_norm_out_edge_dropout": (lambda ir: teleport(ir, norm_out=True, drop=0.1),
+                                       lambda h: expect_teleport(h, norm_out=True)),
     "teleport": (teleport, expect_teleport),
     "teleport_norm_out": (lambda ir: teleport(ir, norm_out=True), lambda h: expect_teleport(h, norm_out=True)),
     # each fusion alone, in its minimal pattern
@@ -545,13 +619,24 @@ def nm_competing_norm(ir):
     return dict(t=t, n1=n1, n2=n2)
 
 
-def nm_bn(readers):
+def nm_bn(readers, norm="batch_norm"):
     def build(ir):
         x = ir.create_node_tensor(12)
-        b = ir.batch_norm(ir.linear(x, 16))
+        b = getattr(ir, norm)(ir.linear(x, 16))
         outs = [getattr(ir, k)(b) for k in readers]
         loss(ir, ir.linear(outs[0] if len(outs) == 1 else ir.add(*outs), 5))
     return build
+
+
+def nm_dropped_sum_bf16(ir):
+    """set_bf16_aggregation: a Linear read by a plain sum alone goes bf16; one read by a dropped sum alone stays fp32
+    (edge dropout has no bf16 form)"""
+    ir.set_bf16_aggregation(True)
+    x = ir.create_node_tensor(12)
+    a = ir.linear(x, 16); b = ir.linear(x, 16)
+    s = ir.add(ir.scatter_gather(a, dropout=0.5, seed=1), ir.scatter_gather(b))
+    loss(ir, ir.linear(s, 5))
+    return dict(fp32=a, bf16=b)
 
 
 def nm_teleport_bf16(ir):
@@ -583,6 +668,8 @@ NEAR = {
     "bn_out_read_twice": (nm_bn(("relu", "sigmoid")), lambda h: {}),
     "bn_then_elu": (nm_bn(("elu",)), lambda h: {}),
     "bn_then_sigmoid": (nm_bn(("sigmoid",)), lambda h: {}),
+    "layer_norm_out_read_twice": (nm_bn(("relu", "sigmoid"), norm="layer_norm"), lambda h: {}),
+    "dropped_sum_input_stays_fp32": (nm_dropped_sum_bf16, lambda h: {}),
     "teleport_sg_input_bf16": (nm_teleport_bf16, lambda h: expect_teleport(h, fused=False)),
     "teleport_t0_after_sg": (lambda ir: teleport(ir, t0="after"), lambda h: expect_teleport(h, fused=False, sg=2)),
     "teleport_norm_second_input": (lambda ir: teleport(ir, second=True), lambda h: expect_teleport(h, fused=False)),
@@ -686,7 +773,56 @@ def elu_and_bn_t(ir):
     loss(ir, ir.linear(ir.add(ir.elu(t), ir.batch_norm(t)), 5))
 
 
+def gather(kind, ir, t, u=None, v=None):
+    """one of the new gathers over (t, u, v) (the ones its mode reads)"""
+    if kind == "dynamic":
+        return ir.dynamic_attention_gather(t, u, heads=4)
+    if kind == "softmax":
+        return ir.softmax_gather(t, 3.0, learn_temperature=False)
+    return ir.dot_attention_gather(t, u, v, heads=2)
+
+
+def aliased(kind, names):
+    """the gather's inputs drawn from three Linears by name: "ttt" is q = k = v = t"""
+    def build(ir):
+        x = ir.create_node_tensor(12)
+        lin = {c: ir.linear(x, 16) for c in sorted(set(names))}
+        loss(ir, ir.linear(gather(kind, ir, *(lin[c] for c in names)), 5))
+    return build
+
+
+def gather_input_also_read(kind, before):
+    """a relu reads the gather's first input t, created before or after the gather: its backward writes t's gradient
+    first or last"""
+    def build(ir):
+        x = ir.create_node_tensor(12)
+        t, u, v = ir.linear(x, 16), ir.linear(x, 16), ir.linear(x, 16)
+        r = ir.relu(t) if before else None
+        g = gather(kind, ir, t, u, v)
+        if r is None:
+            r = ir.relu(t)
+        loss(ir, ir.linear(ir.add(g, r), 5))
+    return build
+
+
+def over_leaves(kind):
+    """the gather reads leaves only: the dynamic one's a and the learned temperature still give its output a gradient;
+    the dot one has none, its backward runs nothing"""
+    def build(ir):
+        x, y, z = (ir.create_node_tensor(16) for _ in range(3))
+        g = ir.softmax_gather(x, 1.0, learn_temperature=True) if kind == "softmax" else gather(kind, ir, x, y, z)
+        loss(ir, ir.linear(g, 5))
+    return build
+
+
 SHARED = {
+    "dynamic_xl_is_xr": (aliased("dynamic", "tt"), lambda h: {}),
+    "dot_q_is_k_is_v": (aliased("dot", "ttt"), lambda h: {}),
+    "dot_q_is_k": (aliased("dot", "ttu"), lambda h: {}),
+    "dot_k_is_v": (aliased("dot", "tuu"), lambda h: {}),
+    "softmax_learned_over_a_leaf": (over_leaves("softmax"), lambda h: {}),
+    "dynamic_over_leaves": (over_leaves("dynamic"), lambda h: {}),
+    "dot_over_leaves": (over_leaves("dot"), lambda h: {}),
     "attention_scores_and_gather_t": (scores_and_gather_t, lambda h: {}),
     "scaled_add_t_relu_t": (scaled_add_t_relu_t, lambda h: {}),
     "elu_and_batch_norm_t": (elu_and_bn_t, lambda h: {}),
@@ -700,6 +836,10 @@ SHARED = {
 }
 for _o in itertools.permutations(("relu", "sigmoid", "linear")):
     SHARED["three_readers_" + "_".join(_o)] = (three_readers(_o), lambda h: {})
+for _k in ("dynamic", "softmax", "dot"):
+    for _b in (True, False):
+        SHARED["%s_input_also_read_%s" % (_k, "before" if _b else "after")] = (gather_input_also_read(_k, _b),
+                                                                              lambda h: {})
 
 
 def exact_gcn(ir):
@@ -730,8 +870,45 @@ def exact_attention_weighted(ir):
     loss(ir, ir.linear(b, 5))
 
 
+def exact_gather(kind):
+    def build(ir):
+        ir.set_exact_backward(True)
+        x = ir.create_node_tensor(12)
+        t, u, v = ir.linear(x, 16), ir.linear(x, 16), ir.linear(x, 16)
+        g = ir.softmax_gather(ir.relu(t), 1.0, learn_temperature=True) if kind == "softmax" else \
+            gather(kind, ir, t, u, v)
+        loss(ir, ir.linear(ir.relu(g), 5))
+    return build
+
+
+def exact_edge_dropout(ir):
+    """two GCN layers on dropped sums: the backward's keep bits are the transposed plan's"""
+    ir.set_exact_backward(True)
+    x = ir.create_node_tensor(12)
+    t = ir.linear(x, 16); s = ir.scatter_gather(ir.indegree_norm(t), dropout=0.5, seed=1)
+    r = ir.relu(ir.indegree_norm(s))
+    t2 = ir.linear(r, 5)
+    loss(ir, ir.indegree_norm(ir.scatter_gather(ir.indegree_norm(t2), dropout=0.1, seed=1)))
+
+
 EXACT = {"gcn_dropout": exact_gcn, "pool_max": exact_pool(_lib.AGGR_MAX), "pool_min": exact_pool(_lib.AGGR_MIN),
-         "attention_avg_weighted": exact_attention_weighted}
+         "attention_avg_weighted": exact_attention_weighted, "dynamic": exact_gather("dynamic"),
+         "softmax_learned": exact_gather("softmax"), "dot": exact_gather("dot"), "edge_dropout": exact_edge_dropout}
+
+
+def cut_rows(kind):
+    """a softmax or dot gather on the hub graph: the infer forward keeps no stats, and each cut row's raw (m, s) go
+    through the plan's shared workspace"""
+    def build(ir):
+        x = ir.create_node_tensor(12)
+        t, u, v = ir.linear(x, 16), ir.linear(x, 16), ir.linear(x, 16)
+        g = ir.softmax_gather(t, 1.0, learn_temperature=True) if kind == "softmax" else \
+            ir.dot_attention_gather(t, u, v, heads=4)
+        loss(ir, ir.linear(g, 5))
+    return build
+
+
+CUT = {"softmax": cut_rows("softmax"), "dot": cut_rows("dot")}
 
 
 @pytest.mark.parametrize("name", list(HAND))
@@ -743,7 +920,9 @@ def test_each_fusion_alone(name):
 @pytest.mark.parametrize("name", list(NEAR))
 def test_fusion_near_miss(name):
     build, expect = NEAR[name]
-    check_case(build, expect=expect)
+    r = check_case(build, expect=expect)
+    if name == "dropped_sum_input_stays_fp32":
+        assert (r["dtypes"][r["h"]["fp32"]], r["dtypes"][r["h"]["bf16"]]) == ("float32", "bfloat16"), r["dtypes"]
     near(name)
 
 
@@ -760,6 +939,11 @@ def test_exact_mode_on_a_directed_multigraph(name):
     SEEN.add("exact:" + name)
 
 
+@pytest.mark.parametrize("name", list(CUT))
+def test_softmax_and_dot_on_cut_rows(name):
+    check_case(CUT[name], gkind="hub")
+
+
 # ------------------------------------------------------------------------------------------ (b) random graphs ---
 SMALL, RING_U, RING_T = (3, 5, 7, 12, 16), (72, 100, 128), (132, 160, 256)
 CLASSES = (5, 32, 33, 64, 65, 128, 129)
@@ -767,6 +951,8 @@ CLASSES = (5, 32, 33, 64, 65, 128, 129)
 
 SEEDS = 64
 COEFFS = ((1.0, 1.0), (0.9, 0.1), (1.5, -0.5), (0.0, 1.0))
+TEMPERATURES = (0.0, 1.0, -0.5, 3.0)
+EDGE_DROPOUT = (0.1, 0.5)
 
 
 def random_graph(seed):
@@ -805,13 +991,17 @@ def random_graph(seed):
         def coeffs():
             return COEFFS[rng.randint(len(COEFFS))]
 
+        def drop_rate():
+            return EDGE_DROPOUT[rng.randint(len(EDGE_DROPOUT))]
+
         x = ir.create_node_tensor(int(rng.choice((7, 12, 16, 33))), dtype="bfloat16" if half_x else "float32")
         new(x, False)
         for _ in range(rng.randint(3, 10)):
             t = open_[rng.randint(len(open_))]
             w = ir.width[t]
             k = rng.choice(["linear", "linear", "norm", "sg", "sg_mm", "sg_w", "attn", "relu", "sigmoid", "add",
-                            "dropout", "batch_norm", "elu", "scaled_add", "shared", "teleport"])
+                            "dropout", "batch_norm", "elu", "scaled_add", "shared", "teleport", "dynamic", "softmax",
+                            "dot", "layer_norm"])
             if t in ir.bf16 and k not in ("linear", "dropout"):
                 k = "linear"
             if k == "linear":
@@ -824,7 +1014,13 @@ def random_graph(seed):
                 new(ir.indegree_norm(t), grad[t])
             elif k == "sg":
                 take(t, True)
-                new(ir.scatter_gather(t, _lib.AGGR_AVG if rng.rand() < 0.25 else _lib.AGGR_SUM), grad[t])
+                pick = rng.rand()
+                if pick < 0.25:
+                    new(ir.scatter_gather(t, _lib.AGGR_AVG), grad[t])
+                elif pick < 0.5:
+                    new(ir.scatter_gather(t, dropout=drop_rate(), seed=int(rng.randint(4))), grad[t])
+                else:
+                    new(ir.scatter_gather(t), grad[t])
             elif k == "sg_mm":
                 take(t, True)
                 new(ir.scatter_gather(t, _lib.AGGR_MAX if rng.rand() < 0.5 else _lib.AGGR_MIN), grad[t])
@@ -841,6 +1037,25 @@ def random_graph(seed):
                 sc = ir.attention_scores(t, heads) if rng.rand() < 0.5 else ir.linear(t, 2 * heads)
                 rate = 0.6 if rng.rand() < 0.4 else 0.0
                 new(ir.attention_gather(t, sc, heads=heads, dropout=rate, seed=int(rng.randint(4))), True)
+            elif k in ("dynamic", "dot"):
+                heads = [h for h in range(1, 9) if w % h == 0]
+                if w > 256:
+                    continue
+                heads = heads[rng.randint(len(heads))]
+                ins = [t] + [t if u is None or rng.rand() < 0.3 else u for u in
+                             (partner(t) for _ in range(1 if k == "dynamic" else 2))]
+                if k == "dot" and rng.rand() < 0.5:
+                    ins = [ins[j] for j in rng.permutation(3)]
+                if k == "dynamic":
+                    new(ir.dynamic_attention_gather(*ins, heads=heads), True)
+                else:
+                    new(ir.dot_attention_gather(*ins, heads=heads), any(grad[u] for u in ins))
+            elif k == "softmax":
+                learn = rng.rand() < 0.5
+                new(ir.softmax_gather(t, TEMPERATURES[rng.randint(len(TEMPERATURES))], learn), grad[t] or learn)
+            elif k == "layer_norm":
+                b = ir.layer_norm(t)
+                new(ir.relu(b) if rng.rand() < 0.4 else b, True)   # read by a relu alone: the norm-relu fusion
             elif k in ("relu", "sigmoid", "elu"):
                 new(getattr(ir, k)(t), grad[t])
             elif k == "batch_norm":
@@ -882,7 +1097,7 @@ def random_graph(seed):
                 # the teleport hop: t0 a leaf, an earlier tensor (t itself: APPNP's shape), or one made after the SG
                 take(t, True)
                 n1 = ir.indegree_norm(t)
-                s = ir.scatter_gather(n1)
+                s = ir.scatter_gather(n1, dropout=drop_rate() if rng.rand() < 0.3 else 0.0, seed=int(rng.randint(4)))
                 n2 = ir.indegree_norm(s)
                 where = rng.randint(3)
                 if where == 1:
@@ -1050,11 +1265,17 @@ def test_q7_refusal_is_the_same_in_both_schedules(name):
 # ------------------------------------------------------------------------------------------------ (f) coverage ---
 def test_opgraph_covered():
     """Every op kind, fusion, near-miss and width class was reached (run the whole file: this test comes last)."""
-    want = {"op:" + k for k in _lib.HOST_OPS} | {"op:linear_relu", "op:linear_none"}
+    want = {"op:" + k for k in _lib.HOST_OPS} | {"op:linear_relu", "op:linear_none", "op:layer_norm"}
     want |= {"fusion:" + f for f in ("linear_norm_sg", "sg_norm", "sg_norm_relu", "dropout_linear", "norm_softmax",
                                      "norm_relu_linear", "norm_relu_dropout_linear", "batch_norm_relu", "teleport",
-                                     "teleport_norm_out")}
-    want |= {"attn_dropout", "loss:sigmoid", "bf16:features", "bf16:aggregation", "scaled_add_shared_reader"}
+                                     "teleport_norm_out", "layer_norm_relu", "gcn_block_edge_dropout",
+                                     "teleport_edge_dropout")}
+    want |= {"attn_dropout", "edge_dropout", "loss:sigmoid", "bf16:features", "bf16:aggregation",
+             "scaled_add_shared_reader"}
+    want |= {"mode:" + m for m in ("gat", "dynamic", "softmax", "dot")}
+    want |= {"temperature:learned", "temperature:constant", "cut_rows_infer:softmax", "cut_rows_infer:dot"}
+    want |= {"alias:" + a for a in ("xl_is_xr", "q_is_k_is_v", "q_is_k", "k_is_v")}
+    want |= {"gather_input_also_read_before", "gather_input_also_read_after"}
     want |= {"near:" + n for n in NEAR} | {"shared:" + s for s in SHARED} | {"exact:" + e for e in EXACT}
     want |= {"refusal:" + r for r in REFUSE} | {"random", "graph:hub"}
     want |= {"width:" + w for w in ("linear_in_not_float4", "linear_out_over_128", "sg_H_not_float4", "sg_65_128",
